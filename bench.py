@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- audio samples/sec of the VITS2 inference path (BASELINE.json metric) on N B200s.
+"""bench.py -- audio samples/sec of the VITS2 inference path (BASELINE.json metric) on N H100s.
 
 One "step" = one pass of the hot path (SynthesizerTrn.infer) over one batch: BASELINE.json configs[1], a single
 128-phoneme utterance (tokens = randint(0,62,(128,), seed 0), sid 2, scales [0.8, 1.0, 0.8], fp32), synthetic seeded
@@ -17,6 +17,8 @@ utterance path; the packed weights are broadcast once from rank 0 over NCCL at i
   extra    : N = 1 only -- BASELINE configs[2] (64 utterances in one call) with its own roofline, configs[4] (2000-phoneme
              streaming: time to first chunk / total) and the fp32-exact mode (precision 0) of the headline workload.
   --impl reference : the CPU path (oracle restatement of the reference's PyTorch graph) on the host cores.
+  --dump-outputs DIR : after the timed steps, the waveform and frame count of the last timed step as DIR/wav.npy (float32,
+             [1, samples]) and DIR/y_lengths.npy (float64); the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -59,7 +61,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    # NVIDIA data sheet, H100 SXM at 700 W (dense bf16); not a measured rate
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="data-sheet")
 
 
 class ClockSampler(threading.Thread):
@@ -154,23 +157,9 @@ def pin_to_gpu_numa(index):
     return None
 
 
-def ncu_traffic(family):
-    """dram read+write bytes per launch of the dominant kernel from this round's committed `ncu --set full` capture
-    (profiles/r2_conv_tc_traffic.json, made by the command in profiles/README.md), or None."""
-    for name in ("r2_conv_tc_traffic.json", "r1_conv_tc_traffic.json"):
-        path = os.path.join(ROOT, "profiles", name)
-        if family == "tc" and os.path.exists(path):
-            try:
-                with open(path) as f:
-                    return float(json.load(f)["dram_bytes_per_launch_mean"]), "profiles/" + name
-            except Exception:
-                pass
-    return None, None
-
-
 def pick_threads(cfg, w, cores):
     """PyTorch's intra-op pool is at its best well below the core count on these tiny convs (128 threads ran 300x
-    slower than 8 on the B200 host): probe a short utterance at a few thread counts and keep the fastest, so that
+    slower than 8 on a many-core host): probe a short utterance at a few thread counts and keep the fastest, so that
     the CPU arm is the reference at ITS best, not a strawman."""
     import torch
     from oracle import vits_oracle as vo
@@ -405,8 +394,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--cpu-steps", type=int, default=5)
-    ap.add_argument("--precision", type=int, default=1, help="0: fp32 FFMA everywhere; 1: flow+decoder on tcgen05 (split-bf16 x3); 2: encoder too; 3: encoder on tcgen05 with the exact 3-way split")
+    ap.add_argument("--precision", type=int, default=1, help="0: fp32 FFMA everywhere; 1: flow+decoder on wgmma (split-bf16 x3); 2: encoder too; 3: encoder on wgmma with the exact 3-way split")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary configs (configs[2], configs[4], fp32-exact mode)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     from vosk_tts_b200 import config as C
@@ -486,7 +476,7 @@ def main():
     d_eps_z = torch.as_tensor(wl["eps_z"][:, :, :Ty], device=dev).contiguous()
     d_wav = torch.zeros(1, (Ty + 64) * hop, device=dev)
     eng.synthesize_dev(d_wav.data_ptr(), (Ty + 64) * hop, d_eps_z.data_ptr(), Ty)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
     estream = torch.cuda.ExternalStream(eng.stream(), device=dev)
 
     def step_dev():
@@ -518,6 +508,10 @@ def main():
         step_ms.append(e0.elapsed_time(e1))
     barrier()
     launches = eng.kernel_launches() - launches0
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "wav.npy"), d_wav[:, : Ty * hop].cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "y_lengths.npy"), np.array([Ty], np.float64))
     total_ms = float(sum(step_ms))
     # roofline pass: same steps with every conv launch bracketed by CUDA events on the engine stream (eager launches,
     # so this pass is slower than the timed one; only per-kernel durations are taken from it)
@@ -617,11 +611,10 @@ def main():
         dom = "tc" if fam["tc"][0] > fam["ffma"][0] else "ffma"
         d_ms, d_fl, d_n = fam[dom]
         ach = d_fl / (d_ms / 1e3) / 1e12 if d_ms > 0 else 0.0
-        kname = {"tc": "conv_tc_kernel<64, cluster split-K> (tcgen05 + TMA conv1d-as-GEMM, split-bf16 x3, fp32 accumulate in TMEM, DSMEM reduce-scatter)",
+        kname = {"tc": "conv_tc_kernel<64, cluster split-K> (wgmma + TMA conv1d-as-GEMM, split-bf16 x3, fp32 accumulate in registers, DSMEM reduce-scatter)",
                  "ffma": "conv_kernel<G> (fp32 FFMA conv1d-as-GEMM, cluster split-K)"}[dom]
         other = "ffma" if dom == "tc" else "tc"
         o_ms, o_fl, o_n = fam[other]
-        traffic, traffic_src = ncu_traffic(dom)
         # CPU baseline beside it (bounded sample), N=1 only
         cpu = None
         extra = None
@@ -660,7 +653,7 @@ def main():
                     extra["value_fp32_exact"] = {"error": repr(ex)}
         line = {"metric": METRIC, "value": value, "unit": "samples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": "fp32" if args.precision == 0 else "fp32 (flow/decoder convs + attention: bf16 hi+lo split x3 MMAs on tcgen05, fp32 accumulate; rest fp32 FFMA)",
+                "dtype": "fp32" if args.precision == 0 else "fp32 (flow/decoder convs + attention: bf16 hi+lo split x3 MMAs on wgmma, fp32 accumulate; rest fp32 FFMA)",
                 "data": "synthetic", "config": conf,
                 "engine": {"precision_mode": args.precision, "cuda_graphs": "per length bucket", "speculative_second_phase": eng.speculation_stats(),
                            "ranks_pinned_to_gpu_numa_cores": pinned},
@@ -683,10 +676,10 @@ def main():
                 "gpu_launches": int(launches),
                 "roofline": {"kernel": kname, "bound": "tensor", "achieved": ach,
                              "peak": pk["bf16_sustained"], "unit": "TFLOP/s", "frac": ach / pk["bf16_sustained"],
-                             "peak_source": pk["src"] + " cuBLAS bf16 (sustained). achieved = algorithmic FLOPs (2*Cin*k*Cout per output "
+                             "peak_source": pk["src"] + " bf16 rate. achieved = algorithmic FLOPs (2*Cin*k*Cout per output "
                              "position) / summed CUDA-event durations of the launches in the profiled pass; the split-bf16 kernel "
                              "issues 3 MMAs per algorithmic MAC, so its ceiling on this scale is peak/3",
-                             "traffic": traffic, "traffic_source": traffic_src, "launches_per_step": d_n / max(args.steps, 1),
+                             "launches_per_step": d_n / max(args.steps, 1),
                              "share_of_step": d_ms / prof_total_ms if prof_total_ms else None,
                              "flops_per_step": d_fl / max(args.steps, 1),
                              "other_family": {"kernel": other, "ms_per_step": o_ms / max(args.steps, 1),

@@ -1,5 +1,5 @@
 /*
- * vtts.h -- C ABI of the B200-native VITS2 inference engine (libvtts.so).
+ * vtts.h -- C ABI of the H100-native VITS2 inference engine (libvtts.so).
  *
  * Drop-in boundary: the single call the reference makes into its inference runtime,
  *
@@ -60,8 +60,8 @@ typedef struct vtts_config {
   int32_t upsample_kernel_sizes[8];
   int32_t upsample_initial_channel;
   int32_t subbands, istft_n_fft, istft_hop;
-  int32_t precision;               /* 0 = fp32 FFMA everywhere; 1 = split-bf16 tcgen05 for the flow + decoder (dense convs and
-                                      attention); 2 = text encoder on tcgen05 as well */
+  int32_t precision;               /* 0 = fp32 FFMA everywhere; 1 = split-bf16 wgmma for the flow + decoder (dense convs and
+                                      attention); 2 = text encoder on wgmma as well */
   int32_t flow_n_heads;            /* heads of the flow's pre_transformer: the reference hard-codes 2 (models.py:355) */
 } vtts_config;
 
@@ -154,7 +154,7 @@ int vtts_host_timings(vtts_handle h, double* us, int n);
  * number of launches and the algorithmic FLOPs (2*Cin*k*Cout per output position) since vtts_profile(h,1). */
 int vtts_profile(vtts_handle h, int enable);
 int vtts_profile_read(vtts_handle h, double* conv_ms, uint64_t* conv_launches, double* conv_flops);
-/* Same counters for the tcgen05 conv kernel (precision mode 1). */
+/* Same counters for the tensor-core conv kernel (precision mode 1). */
 int vtts_profile_read_tc(vtts_handle h, double* ms, uint64_t* launches, double* flops);
 
 /* In-graph timeline for tuning: enable=1 arms it, enable=0 disarms, enable=2 reads up to max_pairs (source line,
@@ -168,7 +168,7 @@ int vtts_debug_flags(vtts_handle h, int flags);
 int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floats, size_t* n_out);
 /* Unit-test hook for the relative-position attention kernels (attentions.py:165-196): one launch of layer "enc.<i>" or
  * "flow.<f>.tr" on a host fp32 qkv tensor [T][3H] of one utterance; out receives fp32 [T][H].  use_tc = 1 selects the
- * tcgen05 kernel (attn_tc.cuh), 0 the fp32 FFMA kernels.  iters > 0: *ms_out = average device time of `iters` more launches. */
+ * wgmma kernel (attn_tc.cuh), 0 the fp32 FFMA kernels.  iters > 0: *ms_out = average device time of `iters` more launches. */
 int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host, int T, int use_tc, float* out_host, int iters,
                          float* ms_out);
 

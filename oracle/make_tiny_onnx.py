@@ -8,7 +8,6 @@ deployment path end to end: model.onnx -> initializers -> packed weights -> engi
 
 Run in the build container:  python oracle/make_tiny_onnx.py
 """
-import copy
 import os
 import sys
 
@@ -18,21 +17,13 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import ref_harness as rh  # noqa: E402
 from vosk_tts_b200 import config as C, synthetic  # noqa: E402
+from golden_ref import tiny_training_json  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 N_VOCAB = 40
-
-
-def tiny_training_json():
-    j = copy.deepcopy(rh.load_ref_config())
-    m = j["model"]
-    m.update(inter_channels=64, hidden_channels=64, filter_channels=128, n_heads=2, n_layers=3, kernel_size=3,
-             resblock_kernel_sizes=[3, 5], resblock_dilation_sizes=[[1, 3, 5], [1, 3, 5]], upsample_rates=[4, 4],
-             upsample_initial_channel=64, upsample_kernel_sizes=[16, 16], gin_channels=32)
-    j["data"]["n_speakers"] = 4
-    return j
 
 
 def main():

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE (not collected): per-row error map of the tcgen05 attention against the torch reference."""
+"""TEST INFRASTRUCTURE (not collected): per-row error map of the tensor-core attention against the torch reference."""
 import os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

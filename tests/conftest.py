@@ -13,7 +13,7 @@ GOLDEN_CASES = ["t17_sid2", "t128_sid2", "t50_slow", "t33_nonoise", "ragged3", "
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -42,8 +42,9 @@ def packed(folded, cfg):
 
 @pytest.fixture(scope="session", params=[0, 1, 2, 3], ids=["fp32-ffma", "tcgen05-flow-decoder", "tcgen05-all", "tcgen05-all-exact-encoder"])
 def engine(request, packed, cfg):
-    """precision 0: fp32 FFMA kernels everywhere; 1: flow + decoder convs (and batched attention) on tcgen05 (split-bf16, 3 MMAs
-    per K16 slice); 2: text encoder too; 3: text encoder on tcgen05 with the exact 3-way split (6 MMAs per K16 slice)."""
+    """precision 0: fp32 FFMA kernels everywhere; 1: flow + decoder convs (and batched attention) on wgmma (split-bf16, 3 MMAs
+    per K16 slice); 2: text encoder too; 3: text encoder on wgmma with the exact 3-way split (6 MMAs per K16 slice).
+    (The ids keep the names the tensor-core modes were first given; they select precision modes, not an instruction set.)"""
     import torch
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")

@@ -68,24 +68,15 @@ def test_missing_model_is_an_error_not_a_download():
         Model(model_name="vosk-model-tts-ru-0.9-multi")
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/vosk_tts/g2p.py"), reason="reference tree absent")
 def test_g2p_matches_reference_converter():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("ref_g2p", "/root/reference/vosk_tts/g2p.py")
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
-    import itertools
-    words = ["прив+ет", "абстр+акция", "+ёлка", "подъ+езд", "семь+я", "чащ+а", "й+од", "объявл+ение", "в+ьюга", "съ+ёмка",
-             "по-р+усски", "+я", "мышь", "компь+ютер", "ш+ёлк", "Гог+оль"]
-    letters = "абвгдеёжзийклмнопрстуфхцчшщъыьэюя"
-    rng = np.random.RandomState(0)
-    for _ in range(300):
-        n = rng.randint(1, 9)
-        w = "".join(letters[i] for i in rng.randint(0, len(letters), n))
-        p = rng.randint(0, n)
-        words.append(w[:p] + "+" + w[p:])
+    """against what the reference converter (vosk_tts/g2p.py) returned for the same words (oracle/make_golden_ref.py)"""
+    import golden_ref as GR
+    with open(os.path.join(GR.GOLDEN, "g2p_reference.json"), encoding="utf-8") as f:
+        ref = json.load(f)
+    words = GR.g2p_words()
+    assert sorted(ref) == sorted(set(words))
     for w in words:
-        assert g2p.convert(w) == ref.convert(w), w
+        assert g2p.convert(w) == ref[w], w
 
 
 class _StubEngine:

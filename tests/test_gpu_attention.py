@@ -1,7 +1,7 @@
 """GPU (-m gpu): the relative-position attention kernels in isolation against a plain PyTorch reference of the same
 op (attentions.py:165-196 restated on q, k, v directly; float64 so that both kernels' errors are visible).
 
-  tensor-core kernel (csrc/attn_tc.cuh: tcgen05 QK^T / PV with split-bf16 operands, P in TMEM, online softmax)
+  tensor-core kernel (csrc/attn_tc.cuh: wgmma QK^T / PV with split-bf16 operands, P in registers, online softmax)
   fp32 FFMA kernels (csrc/kernels.cuh attn_kernel / attn_split_kernel)
 
 Tolerances: fp32 FFMA <= 2e-5, tensor-core <= 2e-4 max-abs on outputs of magnitude ~1 (the split-bf16 operands carry

@@ -401,7 +401,7 @@ def test_bucketed_graphs_serve_unseen_utterances(engine, cfg):
                               "ffma-attention-in-the-flow", "tc-persistent-tile-loop-tall", "tc-persistent-tile-loop-per-tap-tiles",
                               "tc-persistent-weight-multicast-pairs", "tc-persistent-coalesced-epilogue-128-wide", "tc-coalesced-epilogue"])
 def test_alternative_kernel_configurations_match_golden(packed, cfg, env):
-    """The tuning switches select different tilings / launch modes of the same kernels (128-wide tcgen05 tiles are what
+    """The tuning switches select different tilings / launch modes of the same kernels (128-wide tensor-core tiles are what
     batched calls use automatically); each must still reproduce the reference fixture."""
     import os
     from vosk_tts_b200.engine import Engine

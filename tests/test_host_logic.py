@@ -106,10 +106,8 @@ def test_convt_polyphase_equals_conv_transpose(u, K):
 
 
 def test_config_mapping_from_reference_json():
-    path = "/root/reference/training/vits2/configs/mb_istft_vits2_multi.json"
-    if not os.path.exists(path):
-        pytest.skip("reference tree absent")
-    assert C.from_training_json(path) == C.DEFAULT_CONFIG
+    """the reference's training configuration of the default architecture (stored under tests/golden/)"""
+    assert C.from_training_json(os.path.join(os.path.dirname(__file__), "golden", "mb_istft_vits2_multi.json")) == C.DEFAULT_CONFIG
     assert C.hop_total(C.DEFAULT_CONFIG) == 256
 
 

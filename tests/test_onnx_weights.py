@@ -1,32 +1,32 @@
 """Weights and configuration straight from a ``model.onnx`` written by the reference's own export path
-(training/vits2/onnx_export.py:60-104, run here on the seeded reference model; build container only)."""
+(training/vits2/onnx_export.py:60-104).  The graph is the committed tests/golden/tiny_model.onnx: the reference model of
+golden_ref.tiny_training_json() built from the seeded checkpoint 77 and exported by oracle/make_tiny_onnx.py."""
 import os
 import time
 
 import numpy as np
 import pytest
 
-from oracle import ref_harness as rh
+import golden_ref as GR
 from vosk_tts_b200 import config as C, onnx_weights as ow, synthetic, weights
 
-needs_ref = pytest.mark.skipif(not rh.available(), reason="needs the reference tree to export model.onnx")
+TINY_SEED = 77
 
 
 @pytest.fixture(scope="module")
-def onnx_path(tmp_path_factory):
-    if not rh.available():
-        pytest.skip("needs the reference tree")
-    sd = synthetic.make_random_checkpoint(C.DEFAULT_CONFIG, 1234)
-    net = rh.build_reference_model(sd)
-    path = tmp_path_factory.mktemp("onnx") / "model.onnx"
-    rh.export_reference_onnx(path, net)
-    return str(path)
+def onnx_path():
+    return os.path.join(GR.GOLDEN, "tiny_model.onnx")
 
 
-@needs_ref
-def test_state_dict_from_onnx_matches_folded_checkpoint(onnx_path):
+@pytest.fixture(scope="module")
+def onnx_cfg():
+    """the configuration the graph was exported with"""
+    return C.from_training_json(GR.tiny_training_json(), n_vocab=GR.N_VOCAB)
+
+
+def test_state_dict_from_onnx_matches_folded_checkpoint(onnx_path, onnx_cfg):
     sd = ow.state_dict_from_onnx(onnx_path)
-    ref = weights.fold_weight_norm(synthetic.make_random_checkpoint(C.DEFAULT_CONFIG, 1234))
+    ref = weights.fold_weight_norm(synthetic.make_random_checkpoint(onnx_cfg, TINY_SEED))
     unused = {k for k in ref if k.startswith("dp.flows.1.")}          # the flow the reverse pass drops (models.py:94-96)
     for k, v in ref.items():
         v = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
@@ -38,23 +38,21 @@ def test_state_dict_from_onnx_matches_folded_checkpoint(onnx_path):
         assert float(np.abs(sd[k] - v).max()) <= 1e-7, k               # 1-ulp differences of the weight-norm fold
     assert set(sd) <= set(ref)
     # the three anonymous constants: Linear weight (transposed), -logs of the ElementwiseAffine, the iSTFT basis
-    assert sd["enc_p.encoder.spk_emb_linear.weight"].shape == (192, 256)
+    assert sd["enc_p.encoder.spk_emb_linear.weight"].shape == (onnx_cfg["hidden_channels"], onnx_cfg["gin_channels"])
     assert sd["dp.flows.0.logs"].shape == (2, 1)
 
 
-@needs_ref
-def test_config_from_onnx_recovers_the_training_configuration(onnx_path):
+def test_config_from_onnx_recovers_the_training_configuration(onnx_path, onnx_cfg):
     cfg = ow.config_from_onnx(onnx_path)
-    assert cfg == C.DEFAULT_CONFIG
+    assert cfg == onnx_cfg
 
 
-@needs_ref
-def test_packed_blob_from_onnx_has_the_same_layout(onnx_path):
+def test_packed_blob_from_onnx_has_the_same_layout(onnx_path, onnx_cfg):
     sd = ow.state_dict_from_onnx(onnx_path)
     cfg = ow.config_from_onnx(onnx_path)
-    ref = weights.fold_weight_norm(synthetic.make_random_checkpoint(C.DEFAULT_CONFIG, 1234))
+    ref = weights.fold_weight_norm(synthetic.make_random_checkpoint(onnx_cfg, TINY_SEED))
     b1, m1 = weights.pack(sd, cfg)
-    b2, m2 = weights.pack(ref, C.DEFAULT_CONFIG)
+    b2, m2 = weights.pack(ref, onnx_cfg)
     assert m1 == m2 and b1.shape == b2.shape
 
 

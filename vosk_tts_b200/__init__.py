@@ -1,1 +1,1 @@
-"""B200-native VITS2 inference engine behind the vosk_tts Model/Synth API (hot path only)."""
+"""H100-native VITS2 inference engine behind the vosk_tts Model/Synth API (hot path only)."""

@@ -1,4 +1,4 @@
-"""Builds libvtts.so (the C-ABI library, include/vtts.h) in-tree with nvcc for sm_100a."""
+"""Builds libvtts.so (the C-ABI library, include/vtts.h) in-tree with nvcc for sm_90a (H100)."""
 import os
 import subprocess
 import sys
@@ -7,10 +7,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvtts.so")
 SOURCES = ["engine.cu"]
-DEPS = ["engine.cu", "kernels.cuh", "conv_tc.cuh", "attn_tc.cuh", "wn_tc.cuh", "mas.cuh", os.path.join("..", "..", "include", "vtts.h")]
+DEPS = ["engine.cu", "kernels.cuh", "conv_tc.cuh", "attn_tc.cuh", "wgmma.cuh", "mas.cuh", os.path.join("..", "..", "include", "vtts.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-shared",
 ]
 

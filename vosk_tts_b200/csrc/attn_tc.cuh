@@ -1,40 +1,40 @@
-// attn_tc.cuh -- windowed relative-position multi-head self-attention (attentions.py:165-196) on the 5th-generation
-// tensor cores (tcgen05 + TMEM + TMA), sm_100a only.  One CTA = 128 query rows of one head of one utterance.
+// attn_tc.cuh -- windowed relative-position multi-head self-attention (attentions.py:165-196) on the Hopper tensor cores
+// (wgmma + TMA + mbarrier), sm_90a.  One CTA = 128 query rows of one head of one utterance.
 //
-//   S  = Q K^T            128 x 64 key tile, fp32 in TMEM                       (attentions.py:172, scores)
+//   S  = Q K^T            128 x 64 key tile, fp32 in registers                  (attentions.py:172, scores)
 //   Sr = Q Ek^T           128 x 16 (9 relative offsets, zero padded), once      (:173-177, rel_logits before the skew)
 //   s_ij = (S_ij + [|j-i|<=W] Sr_i[j-i+W]) / sqrt(dk);  keys >= len masked      (:178,183: -1e4 fill == exp -> 0 in fp32)
 //   P  = exp(s - m)       online softmax, running max refreshed lazily          (:190 softmax)
-//   O += P V + Pband Ev   128 x dk, fp32 in TMEM                                (:192-196, output + relative values)
+//   O += P V + Pband Ev   128 x dk, fp32 in registers                           (:192-196, output + relative values)
 //   out = O / l
 //
 // Operand format = the split-bf16 planes of the tensor-core convs: x = hi + lo to ~2^-18, three MMAs per K16 slice
 // (lo*hi + hi*lo + hi*hi).  Q, K: K-major 128B-swizzled TMA tiles of the qkv planes (channels-last, so a head is a
 // channel range and no transposition is needed).  V is consumed as an MN-major B operand straight from the same
-// channels-last tiles.  P never leaves the SM: the softmax warps write it back into TMEM as packed bf16 (hi and lo
-// planes, tcgen05.st) and the P V MMAs take their A operand from TMEM.  The relative-position terms ride on the same
-// tensor-core path: Q Ek^T is one extra N=16 MMA group per CTA, and P_band Ev one extra K=16 MMA per diagonal key tile.
+// channels-last tiles.  P never leaves the registers: the S accumulator fragment of a K16 slice of keys is exactly the
+// A-operand fragment of the P V MMA, so P is split into bf16 hi/lo pairs in place.  The relative-position terms ride on
+// the same tensor-core path: Q Ek^T is one extra N=16 MMA group per CTA, and P_band Ev one extra K=16 MMA per diagonal
+// key tile (its A fragment is gathered from a small per-row band scratch in shared memory).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-// warps 2..5 = softmax (one query row per thread, no shuffles), O rescaling and the epilogue.
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups of 64 query rows each (MMAs, softmax with the row
+// statistics reduced over the 4 lanes that share a row, O rescaling and the epilogue); warp 8 = TMA producer.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace vtts {
 
-constexpr int ATC_BM = 128;        // query rows per CTA (UMMA M)
+constexpr int ATC_BM = 128;        // query rows per CTA
 constexpr int ATC_KT = 64;         // keys per tile
 constexpr int ATC_NS = 2;          // K/V ring depth
-constexpr int ATC_THREADS = 192;
+constexpr int ATC_CWG = 2;         // consumer warpgroups
+constexpr int ATC_THREADS = ATC_CWG * 128 + 32;
 constexpr int ATC_RELP = 16;       // relative-offset slots (2W+1 <= 16)
 constexpr int ATC_RS = 13;         // floats per row of the per-row band scratch in shared memory
 constexpr float ATC_LAZY = 6.0f;   // the running max is refreshed only when a tile exceeds it by more than this (natural log units)
-
-// TMEM columns (fp32 cells): S double buffer, P double buffer (bf16 pairs: hi 32 cols + lo 32 cols), O, Sr, Pband (hi 8 + lo 8) x 2
-constexpr int ATC_COL_S = 0, ATC_COL_P = 128, ATC_COL_O = 256, ATC_COL_SR = 384, ATC_COL_PB = 400, ATC_TMEM_COLS = 512;
 
 struct AttnTcParams {
   CUtensorMap q_hi, q_lo;      // qkv planes [rows][ld], box 64 channels x 128 rows
@@ -58,49 +58,17 @@ constexpr int atc_smem_bytes(int dk) {
          + 1024 /*alignment slack*/ + 256 /*barriers*/;
 }
 
-__device__ __forceinline__ uint32_t umma_idesc_bf16_ex(int n, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(b_mn_major & 1) << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(ATC_BM >> 4) << 24);
-}
-// D[tmem] (+)= A[tmem] * B[smem descriptor]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float lds_f32(uint32_t saddr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr));
   return v;
 }
 __device__ __forceinline__ void sts_f32(uint32_t saddr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory"); }
-__device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) {
-  return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+
+template <int N>
+__device__ __forceinline__ void atc_pv(float* d, const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (N == 64) wgmma_rs_n64(d, a, db);
+  else wgmma_rs_n32(d, a, db);
 }
 
 template <int DK>
@@ -115,7 +83,7 @@ attn_tc_kernel(const __grid_constant__ AttnTcParams ap, const int* __restrict__ 
   const int b = blockIdx.z, head = blockIdx.y;
   const int q0 = blockIdx.x * ATC_BM;
   // lens/offs are final before the graph that contains this kernel starts (host copies or the previous phase): an idle
-  // CTA leaves before it allocates anything
+  // CTA leaves before it initialises anything
   const int len = lens[b];
   if (q0 >= len) return;
   const long base = offs[b];
@@ -133,37 +101,22 @@ attn_tc_kernel(const __grid_constant__ AttnTcParams ap, const int* __restrict__ 
   uint64_t* q_full = bars;              // Q tile + relative tables landed
   uint64_t* kv_full = bars + 1;         // [NS]
   uint64_t* kv_empty = kv_full + ATC_NS;
-  uint64_t* s_full = kv_empty + ATC_NS; // [2] S tile complete in TMEM
-  uint64_t* p_full = s_full + 2;        // [2] P tile written by all 128 softmax threads
-  uint64_t* pv_done = p_full + 2;       // the P V MMAs of a tile have retired
-  uint64_t* sr_full = pv_done + 1;      // Sr complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sr_full + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nt = (len + ATC_KT - 1) / ATC_KT;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == ATC_CWG * 4 && lane == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < ATC_NS; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&p_full[s], 128); }
-    mbar_init(pv_done, 1);
-    mbar_init(sr_full, 1);
+    for (int s = 0; s < ATC_NS; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], ATC_CWG); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&ap.q_hi)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&ap.q_lo)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&ap.kv_hi)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&ap.kv_lo)) : "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)ATC_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == ATC_CWG * 4) {
     // ------------------------------------------------------------------ TMA producer
     if (lane == 0) {
       // the relative-position tables are constants: requested before the dependency wait
@@ -198,279 +151,233 @@ attn_tc_kernel(const __grid_constant__ AttnTcParams ap, const int* __restrict__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one thread)
-    if (lane == 0) {
-      PDL_WAIT();
-      const uint32_t id_s = umma_idesc_bf16_ex(ATC_KT, 0), id_r = umma_idesc_bf16_ex(ATC_RELP, 0);
-      // S[buf] = Q K(t)^T : three MMAs per K16 slice
-      auto issue_qk = [&](int t) {
-        const int st = t % ATC_NS;
-        mbar_wait(&kv_full[st], (t / ATC_NS) & 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + ATC_COL_S + (t & 1) * ATC_KT;
-        const uint32_t kb = smem_u32(sKV + st * STAGE_BYTES);
-        uint32_t acc = 0;
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          const uint64_t qh = umma_desc_sw128(smem_u32(sQ + c * Q_TILE)), ql = umma_desc_sw128(smem_u32(sQ + (NC + c) * Q_TILE));
-          const uint64_t kh = umma_desc_sw128(kb + c * KV_TILE), kl = umma_desc_sw128(kb + (NC + c) * KV_TILE);
-          const int nk = (c == NC - 1 ? LASTW : 64) / 16;
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            if (kk < nk) {
-              const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-              umma_bf16(d, ql + adv, kh + adv, id_s, acc);
-              umma_bf16(d, qh + adv, kl + adv, id_s, 1u);
-              umma_bf16(d, qh + adv, kh + adv, id_s, 1u);
-              acc = 1u;
-            }
-          }
-        }
-        umma_commit(&s_full[t & 1]);
-      };
-      mbar_wait(q_full, 0);
-      timeline_stamp_t(-32);
-      tc_fence_after();
-      {   // Sr = Q Ek^T (N = 16)
-        const uint32_t d = tmem_base + ATC_COL_SR;
-        uint32_t acc = 0;
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          const uint64_t qh = umma_desc_sw128(smem_u32(sQ + c * Q_TILE)), ql = umma_desc_sw128(smem_u32(sQ + (NC + c) * Q_TILE));
-          const uint64_t eh = umma_desc_sw128(smem_u32(sRK + c * R_TILE)), el = umma_desc_sw128(smem_u32(sRK + (NC + c) * R_TILE));
-          const int nk = (c == NC - 1 ? LASTW : 64) / 16;
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            if (kk < nk) {
-              const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-              umma_bf16(d, ql + adv, eh + adv, id_r, acc);
-              umma_bf16(d, qh + adv, el + adv, id_r, 1u);
-              umma_bf16(d, qh + adv, eh + adv, id_r, 1u);
-              acc = 1u;
-            }
-          }
-        }
-        umma_commit(sr_full);
-      }
-      issue_qk(0);
-      for (int t = 0; t < nt; ++t) {
-        if (t + 1 < nt) issue_qk(t + 1);            // overlaps the softmax of tile t
-        mbar_wait(&p_full[t & 1], (t >> 1) & 1);
-        tc_fence_after();
-        const int st = t % ATC_NS;
-        const uint32_t vb = smem_u32(sKV + st * STAGE_BYTES + 2 * NC * KV_TILE);
-        const uint32_t pa = tmem_base + ATC_COL_P + (t & 1) * 64;       // hi: +0..31, lo: +32..63 (packed bf16 pairs)
-        const int k0 = t * ATC_KT;
-        const bool band = (k0 + ATC_KT - 1 + W >= q0) && (k0 - W <= q0 + ATC_BM - 1);
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          const int n = (c == NC - 1) ? LASTW : 64;
-          const uint32_t id_v = umma_idesc_bf16_ex(n, 1);
-          const uint32_t d = tmem_base + ATC_COL_O + c * 64;
-          const uint64_t vh = umma_desc_sw128(vb + c * KV_TILE), vl = umma_desc_sw128(vb + (NC + c) * KV_TILE);
-#pragma unroll
-          for (int kk = 0; kk < ATC_KT / 16; ++kk) {
-            const uint64_t adv = (uint64_t)((kk * 16 * 128) >> 4);      // 16 keys = 16 rows of 128 bytes
-            umma_bf16_ts(d, pa + 32 + kk * 8, vh + adv, id_v, (t | kk) ? 1u : 0u);
-            umma_bf16_ts(d, pa + kk * 8, vl + adv, id_v, 1u);
-            umma_bf16_ts(d, pa + kk * 8, vh + adv, id_v, 1u);
-          }
-          if (band) {      // + P_band Ev (K = 16 relative offsets)
-            const uint32_t pb = tmem_base + ATC_COL_PB + (t & 1) * 16;   // hi 8 cols, lo 8 cols
-            const uint64_t eh = umma_desc_sw128(smem_u32(sRV + c * R_TILE)), el = umma_desc_sw128(smem_u32(sRV + (NC + c) * R_TILE));
-            umma_bf16_ts(d, pb + 8, eh, id_v, 1u);
-            umma_bf16_ts(d, pb, el, id_v, 1u);
-            umma_bf16_ts(d, pb, eh, id_v, 1u);
-          }
-        }
-        umma_commit(&kv_empty[st]);
-        umma_commit(pv_done);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax / correction / epilogue: one row per thread
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;                // row of the query tile == TMEM lane
-    const int qi = q0 + row;
-    const uint32_t lane_sel = (uint32_t)(quad * 32) << 16;
-    const float scale = 1.0f / sqrtf((float)DK);
-    const float L2E = 1.4426950408889634f;
-    const uint32_t mySr = smem_u32(sSr + row * ATC_RS);     // (explicit shared-space accesses: generic LD/ST otherwise)
-    const uint32_t myPb = smem_u32(sPb + row * ATC_RS);
-    PDL_WAIT();
-    {   // relative-key logits of this row -> shared memory (indexed by a run-time offset below)
-      mbar_wait(sr_full, 0);
-      tc_fence_after();
-      uint32_t r[16];
-      tmem_ld_x16(tmem_base + lane_sel + ATC_COL_SR, r);
-      tmem_wait_ld();
-#pragma unroll
-      for (int m = 0; m < ATC_RS; ++m) sts_f32(mySr + 4 * m, __uint_as_float(r[m]) * scale);
-    }
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int t = 0; t < nt; ++t) {
-      const int bsel = t & 1;
-      const int k0 = t * ATC_KT;
-      mbar_wait(&s_full[bsel], (t >> 1) & 1);
-      if (threadIdx.x == 64) timeline_stamp_t(-40 - t);
-      tc_fence_after();
-      float s[ATC_KT];
-      {
-        uint32_t r0[16], r1[16], r2[16], r3[16];           // all four loads in flight, one wait
-        const uint32_t sa = tmem_base + lane_sel + ATC_COL_S + bsel * ATC_KT;
-        tmem_ld_x16(sa, r0); tmem_ld_x16(sa + 16, r1); tmem_ld_x16(sa + 32, r2); tmem_ld_x16(sa + 48, r3);
-        tmem_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          s[i] = __uint_as_float(r0[i]) * scale; s[16 + i] = __uint_as_float(r1[i]) * scale;
-          s[32 + i] = __uint_as_float(r2[i]) * scale; s[48 + i] = __uint_as_float(r3[i]) * scale;
-        }
-      }
-      // does the +-W band of any row of this CTA / of this warp cross the key tile?
-      const bool band_cta = (k0 + ATC_KT - 1 + W >= q0) && (k0 - W <= q0 + ATC_BM - 1);
-      const int w_lo = q0 + quad * 32, w_hi = w_lo + 31;
-      const bool band_warp = (k0 + ATC_KT - 1 + W >= w_lo) && (k0 - W <= w_hi);
-      const int moff = k0 - qi + W;                  // relative slot of key column c is c + moff
-      if (band_warp) {
-#pragma unroll
-        for (int c = 0; c < ATC_KT; ++c) {
-          const int m = c + moff;
-          if ((unsigned)m < (unsigned)nrel) s[c] += lds_f32(mySr + 4 * m);
-        }
-      }
-      const int kvalid = len - k0;                   // columns >= kvalid are beyond the utterance
-      float mx = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < ATC_KT; ++c) {
-        if (c >= kvalid) s[c] = -INFINITY;
-        mx = fmaxf(mx, s[c]);
-      }
-      // lazily refreshed running max: O and l are rescaled only when the tile max exceeds it by more than ATC_LAZY
-      float alpha = 1.f;
-      bool need = false;
-      if (t == 0) {
-        m_run = mx;
-      } else if (mx > m_run + ATC_LAZY) {
-        alpha = exp2f((m_run - mx) * L2E);
-        m_run = mx;
-        need = true;
-      }
-      // pv_done completes one phase per key tile and a parity wait can only tell the current phase from the one before it:
-      // every thread therefore observes EVERY phase, in order -- here when O has to be rescaled, otherwise just before this
-      // tile's P is handed over (by then the P V MMAs of tile t-1 have normally retired, so the wait costs nothing)
-      bool pv_seen = (t == 0);
-      if (__any_sync(0xffffffffu, need)) {           // warp-uniform: tcgen05.ld/st are warp collectives
-        mbar_wait(pv_done, (t - 1) & 1);             // the P V MMAs of tile t-1 have retired: O is quiescent
-        pv_seen = true;
-        tc_fence_after();
-        l_run *= alpha;
-#pragma unroll
-        for (int n0 = 0; n0 < DK; n0 += 16) {
-          uint32_t r[16];
-          tmem_ld_x16(tmem_base + lane_sel + ATC_COL_O + n0, r);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-          tmem_st_x16(tmem_base + lane_sel + ATC_COL_O + n0, r);
-        }
-      }
-      const float mneg = -m_run * L2E;
-      float lsum = 0.f;
-      if (band_cta) {
-#pragma unroll
-        for (int m = 0; m < ATC_RS; ++m) sts_f32(myPb + 4 * m, 0.f);
-      }
-      {
-        uint32_t ph[ATC_KT / 2], pl[ATC_KT / 2];
-#pragma unroll
-        for (int c = 0; c < ATC_KT; c += 2) {
-          const float p0 = exp2f(fmaf(s[c], L2E, mneg)), p1 = exp2f(fmaf(s[c + 1], L2E, mneg));
-          lsum += p0 + p1;
-          if (band_warp) {
-            const int m0 = c + moff, m1 = c + 1 + moff;
-            if ((unsigned)m0 < (unsigned)nrel) sts_f32(myPb + 4 * m0, p0);
-            if ((unsigned)m1 < (unsigned)nrel) sts_f32(myPb + 4 * m1, p1);
-          }
-          split_bf16_pair(p0, p1, ph[c >> 1], pl[c >> 1]);
-        }
-        l_run += lsum;
-        const uint32_t pa = tmem_base + lane_sel + ATC_COL_P + bsel * 64;
-#pragma unroll
-        for (int n0 = 0; n0 < ATC_KT / 2; n0 += 16) {
-          uint32_t r[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) r[i] = ph[n0 + i];
-          tmem_st_x16(pa + n0, r);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) r[i] = pl[n0 + i];
-          tmem_st_x16(pa + 32 + n0, r);
-        }
-      }
-      if (band_cta) {
-        uint32_t bh[8], bl[8];
-#pragma unroll
-        for (int m = 0; m < 16; m += 2) {
-          const float p0 = m < ATC_RS ? lds_f32(myPb + 4 * m) : 0.f, p1 = m + 1 < ATC_RS ? lds_f32(myPb + 4 * (m + 1)) : 0.f;
-          split_bf16_pair(p0, p1, bh[m >> 1], bl[m >> 1]);
-        }
-        const uint32_t pb = tmem_base + lane_sel + ATC_COL_PB + bsel * 16;
-        tmem_st_x8(pb, bh);
-        tmem_st_x8(pb + 8, bl);
-      }
-      if (!pv_seen) mbar_wait(pv_done, (t - 1) & 1);
-      tmem_wait_st();
-      tc_fence_before();
-      mbar_arrive(&p_full[bsel]);
-      if (threadIdx.x == 64) timeline_stamp_t(-60 - t);
-    }
-    // ---- epilogue: O / l -> fp32 rows and/or split-bf16 planes
-    mbar_wait(pv_done, (nt - 1) & 1);
-    if (threadIdx.x == 64) timeline_stamp_t(-36);
-    tc_fence_after();
-    const float inv = 1.f / l_run;
-    const bool rowok = qi < len;
-    const long orow = base + qi;
-#pragma unroll
-    for (int n0 = 0; n0 < DK; n0 += 32) {
-      uint32_t ra[16], rb[16];
-      tmem_ld_x16(tmem_base + lane_sel + ATC_COL_O + n0, ra);
-      tmem_ld_x16(tmem_base + lane_sel + ATC_COL_O + n0 + 16, rb);
-      tmem_wait_ld();
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-      const uint32_t (&r)[16] = hh ? rb : ra;
-      const int nb = n0 + 16 * hh;
-      if (rowok) {
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]) * inv;
-        if (ap.out) {
-          float* o = ap.out + orow * (long)ap.ldo + head * DK + nb;
-#pragma unroll
-          for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(o + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-        }
-        if (ap.p_hi) {
-          __align__(16) __nv_bfloat16 hb[16], lb[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) split_bf16(v[i], hb[i], lb[i]);
-          __nv_bfloat16* ph = ap.p_hi + orow * (long)ap.ldp + head * DK + nb;
-          __nv_bfloat16* pl = ap.p_lo + orow * (long)ap.ldp + head * DK + nb;
-          *reinterpret_cast<uint4*>(ph) = *reinterpret_cast<const uint4*>(hb);
-          *reinterpret_cast<uint4*>(ph + 8) = *reinterpret_cast<const uint4*>(hb + 8);
-          *reinterpret_cast<uint4*>(pl) = *reinterpret_cast<const uint4*>(lb);
-          *reinterpret_cast<uint4*>(pl + 8) = *reinterpret_cast<const uint4*>(lb + 8);
-        }
-      }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 64) timeline_stamp_t(-37);
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)ATC_TMEM_COLS) : "memory");
+  // -------------------------------------------------------------------- consumers: 64 query rows per warpgroup
+  const int wg = warp >> 2;
+  const int g = lane >> 2, q4 = lane & 3;
+  const int wrow0 = wg * 64 + (warp & 3) * 16;             // first tile row of this warp
+  int row[2], qi[2];
+  uint32_t mySr[2], myPb[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    row[h] = wrow0 + g + 8 * h;
+    qi[h] = q0 + row[h];
+    mySr[h] = smem_u32(sSr + row[h] * ATC_RS);              // (explicit shared-space accesses: generic LD/ST otherwise)
+    myPb[h] = smem_u32(sPb + row[h] * ATC_RS);
+  }
+  const bool leader = (threadIdx.x & 127) == 0;
+  const float scale = 1.0f / sqrtf((float)DK);
+  const float L2E = 1.4426950408889634f;
+  const uint32_t qoff = (uint32_t)(wg * 64 * 128);         // this warpgroup's 64 rows of the Q tile
+  PDL_WAIT();
+  mbar_wait(q_full, 0);
+  timeline_stamp_t(-32);
+  {   // Sr = Q Ek^T (N = 16) -> relative-key logits of this thread's rows in shared memory (indexed by a run-time offset below)
+    float sr[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) sr[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+      const uint64_t qh = gmma_desc_sw128(smem_u32(sQ + c * Q_TILE) + qoff), ql = gmma_desc_sw128(smem_u32(sQ + (NC + c) * Q_TILE) + qoff);
+      const uint64_t eh = gmma_desc_sw128(smem_u32(sRK + c * R_TILE)), el = gmma_desc_sw128(smem_u32(sRK + (NC + c) * R_TILE));
+      const int nk = (c == NC - 1 ? LASTW : 64) / 16;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        if (kk < nk) {
+          const uint64_t adv = (uint64_t)((kk * 32) >> 4);
+          wgmma_ss_n16(sr, ql + adv, eh + adv);
+          wgmma_ss_n16(sr, qh + adv, el + adv);
+          wgmma_ss_n16(sr, qh + adv, eh + adv);
+        }
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_touch<8>(sr);
+#pragma unroll
+    for (int jn = 0; jn < 2; ++jn)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = jn * 8 + 2 * q4 + e;
+          if (m < ATC_RS) sts_f32(mySr[h] + 4 * m, sr[4 * jn + 2 * h + e] * scale);
+        }
+    __syncwarp();
+  }
+  float o[NC][32];
+#pragma unroll
+  for (int c = 0; c < NC; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: this thread's share of the row sum
+  for (int t = 0; t < nt; ++t) {
+    const int st = t % ATC_NS;
+    const int k0 = t * ATC_KT;
+    mbar_wait(&kv_full[st], (t / ATC_NS) & 1);
+    if (threadIdx.x == 0) timeline_stamp_t(-40 - t);
+    const uint32_t kb = smem_u32(sKV + st * STAGE_BYTES);
+    float s[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+      const uint64_t qh = gmma_desc_sw128(smem_u32(sQ + c * Q_TILE) + qoff), ql = gmma_desc_sw128(smem_u32(sQ + (NC + c) * Q_TILE) + qoff);
+      const uint64_t kh = gmma_desc_sw128(kb + c * KV_TILE), kl = gmma_desc_sw128(kb + (NC + c) * KV_TILE);
+      const int nk = (c == NC - 1 ? LASTW : 64) / 16;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        if (kk < nk) {
+          const uint64_t adv = (uint64_t)((kk * 32) >> 4);
+          wgmma_ss_n64(s, ql + adv, kh + adv);
+          wgmma_ss_n64(s, qh + adv, kl + adv);
+          wgmma_ss_n64(s, qh + adv, kh + adv);
+        }
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_touch<32>(s);
+    // does the +-W band of any row of this warpgroup cross the key tile?  (warpgroup-uniform: the band MMA is collective)
+    const int g_lo = q0 + wg * 64, g_hi = g_lo + 63;
+    const bool band = (k0 + ATC_KT - 1 + W >= g_lo) && (k0 - W <= g_hi);
+    const int kvalid = len - k0;                   // columns >= kvalid are beyond the utterance
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jn = 0; jn < 8; ++jn)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = jn * 8 + 2 * q4 + e;
+          float v = s[4 * jn + 2 * h + e] * scale;
+          if (band) {
+            const int m = c + k0 - qi[h] + W;      // relative slot of key column c
+            if ((unsigned)m < (unsigned)nrel) v += lds_f32(mySr[h] + 4 * m);
+          }
+          if (c >= kvalid) v = -INFINITY;
+          s[4 * jn + 2 * h + e] = v;
+          mx[h] = fmaxf(mx[h], v);
+        }
+    float mneg[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      // lazily refreshed running max: O and l are rescaled only when the tile max exceeds it by more than ATC_LAZY
+      if (t == 0) {
+        m_run[h] = mx[h];
+      } else if (mx[h] > m_run[h] + ATC_LAZY) {
+        const float alpha = exp2f((m_run[h] - mx[h]) * L2E);
+        m_run[h] = mx[h];
+        l_run[h] *= alpha;
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+#pragma unroll
+          for (int jn = 0; jn < 8; ++jn) { o[c][4 * jn + 2 * h] *= alpha; o[c][4 * jn + 2 * h + 1] *= alpha; }
+      }
+      mneg[h] = -m_run[h] * L2E;
+    }
+    if (band) {
+      __syncwarp();                                 // the previous tile's band fragment has been read
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        for (int m = q4; m < ATC_RS; m += 4) sts_f32(myPb[h] + 4 * m, 0.f);
+      __syncwarp();
+    }
+#pragma unroll
+    for (int jn = 0; jn < 8; ++jn)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float p = exp2f(fmaf(s[4 * jn + 2 * h + e], L2E, mneg[h]));
+          l_run[h] += p;
+          s[4 * jn + 2 * h + e] = p;
+          if (band) {
+            const int m = jn * 8 + 2 * q4 + e + k0 - qi[h] + W;
+            if ((unsigned)m < (unsigned)nrel) sts_f32(myPb[h] + 4 * m, p);
+          }
+        }
+    // P as the A operand of the P V MMAs: the S fragment of keys [16 kk, 16 kk + 16) is the A fragment of K16 slice kk
+    uint32_t ph[4][4], pl[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) split_bf16_pair(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1], ph[kk][r], pl[kk][r]);
+    uint32_t bh[4], bl[4];
+    if (band) {
+      __syncwarp();
+      float pv[4][2];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 2 * q4 + e + ((r & 2) ? 8 : 0);
+          pv[r][e] = m < ATC_RS ? lds_f32(myPb[r & 1] + 4 * m) : 0.f;
+        }
+#pragma unroll
+      for (int r = 0; r < 4; ++r) split_bf16_pair(pv[r][0], pv[r][1], bh[r], bl[r]);
+    }
+    const uint32_t vb = kb + 2 * NC * KV_TILE;
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+      constexpr int NL = LASTW;
+      const uint64_t vh = gmma_desc_sw128(vb + c * KV_TILE), vl = gmma_desc_sw128(vb + (NC + c) * KV_TILE);
+      auto pv_mma = [&](const uint32_t (&a)[4], uint64_t db) {
+        if (c == NC - 1) atc_pv<NL>(o[c], a, db);
+        else atc_pv<64>(o[c], a, db);
+      };
+#pragma unroll
+      for (int kk = 0; kk < ATC_KT / 16; ++kk) {
+        const uint64_t adv = (uint64_t)((kk * 16 * 128) >> 4);      // 16 keys = 16 rows of 128 bytes
+        pv_mma(pl[kk], vh + adv);
+        pv_mma(ph[kk], vl + adv);
+        pv_mma(ph[kk], vh + adv);
+      }
+      if (band) {      // + P_band Ev (K = 16 relative offsets)
+        const uint64_t eh = gmma_desc_sw128(smem_u32(sRV + c * R_TILE)), el = gmma_desc_sw128(smem_u32(sRV + (NC + c) * R_TILE));
+        pv_mma(bl, eh);
+        pv_mma(bh, el);
+        pv_mma(bh, eh);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < NC; ++c) wgmma_touch<32>(o[c]);
+    if (leader) mbar_arrive(&kv_empty[st]);
+    if (threadIdx.x == 0) timeline_stamp_t(-60 - t);
+  }
+  // ---- epilogue: O / l -> fp32 rows and/or split-bf16 planes
+  if (threadIdx.x == 0) timeline_stamp_t(-36);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    if (qi[h] >= len) continue;
+    const long orow = base + qi[h];
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int jn = 0; jn < 8; ++jn) {
+        if (c == NC - 1 && jn * 8 >= LASTW) continue;
+        const int ch = head * DK + c * 64 + jn * 8 + 2 * q4;
+        const float v0 = o[c][4 * jn + 2 * h] * inv, v1 = o[c][4 * jn + 2 * h + 1] * inv;
+        if (ap.out) *reinterpret_cast<float2*>(ap.out + orow * (long)ap.ldo + ch) = make_float2(v0, v1);
+        if (ap.p_hi) {
+          uint32_t hi, lo;
+          split_bf16_pair(v0, v1, hi, lo);
+          *reinterpret_cast<uint32_t*>(ap.p_hi + orow * (long)ap.ldp + ch) = hi;
+          *reinterpret_cast<uint32_t*>(ap.p_lo + orow * (long)ap.ldp + ch) = lo;
+        }
+      }
   }
 }
 

@@ -1,28 +1,29 @@
-// conv_tc.cuh -- dense conv1d-as-GEMM on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// conv_tc.cuh -- dense conv1d-as-GEMM on the Hopper tensor cores (wgmma + TMA + mbarrier rings), sm_90a.
 //
-//   D[t, co] (fp32, TMEM) = sum_{tap j} sum_{ci} A_j[t, ci] * W_j[co, ci]
+//   D[t, co] (fp32, registers) = sum_{tap j} sum_{ci} A_j[t, ci] * W_j[co, ci]
 //     A_j = rows (t0 + j*dil - pad .. +128) x 64 channels of the producer's *split-bf16 planes* (hi + lo = fp32
 //           value to ~2^-17), K-major, fetched by TMA with the 128-byte swizzle straight from the channels-last
 //           activation buffer (im2col-free: a tap shift is just a different TMA row coordinate; rows outside the
 //           utterance are zero through TMA out-of-bounds fill or the zeroed gap rows between packed utterances),
 //     W_j = 64..128 output channels x 64 input channels of the packed bf16 hi/lo weights of tap j.
 //   Three bf16 MMAs per K16 slice (hi*hi + lo*hi + hi*lo, fp32 accumulate) give fp32-class accuracy (~1e-5 rel)
-//   at 1/3 of the bf16 tensor rate -- about 10x the FFMA pipe -- which keeps the waveform inside the 1e-3 budget
+//   at 1/3 of the bf16 tensor rate -- several times the FFMA pipe -- which keeps the waveform inside the 1e-3 budget
 //   where single-pass bf16 (4.9e-3) or TF32 (6e-4 at 0.2 amplitude) do not (SURVEY.md section 7 "Hard parts").
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-// warps 2..5 = epilogue (tcgen05.ld -> bias/cond/activation/residual -> fp32 rows and/or split-bf16 planes for the
-// next conv).  A 4-stage mbarrier ring decouples TMA from the tensor pipe.
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups, each issuing wgmma for 64 of the tile's 128 rows with
+// the accumulator in registers and then running the epilogue on it (bias/cond/activation/residual -> fp32 rows and/or
+// split-bf16 planes for the next conv); warp 8 = TMA producer.  Multi-stage mbarrier rings decouple TMA from the tensor pipe.
 #pragma once
 #include <type_traits>
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace vtts {
 
-constexpr int TC_BM = 128;        // time rows per CTA (UMMA M)
+constexpr int TC_BM = 128;        // time rows per CTA (two warpgroups of 64)
 constexpr int TC_BK = 64;         // input channels per stage (one 128-byte swizzle atom of bf16)
 // ring depths per weight-tile width (BN): the 64-wide kernel has room for deeper rings than the 128-wide one
 #ifndef VTTS_TC_AST64
@@ -39,7 +40,8 @@ constexpr int TC_BK = 64;         // input channels per stage (one 128-byte swiz
 #endif
 template <int BN> constexpr int tc_ast() { return BN == 64 ? VTTS_TC_AST64 : VTTS_TC_AST128; }   // activation-tile ring depth
 template <int BN> constexpr int tc_wst() { return BN == 64 ? VTTS_TC_WST64 : VTTS_TC_WST128; }   // weight-tile ring depth
-constexpr int TC_THREADS = 192;
+constexpr int TC_CWG = 2;                      // consumer warpgroups
+constexpr int TC_THREADS = TC_CWG * 128 + 32;  // + the producer warp
 constexpr int TC_MAXP = 4;
 
 enum : int { TCE_RELU = 1, TCE_GATE = 2 };
@@ -71,7 +73,7 @@ struct TcBatchScalars {
   int n;
   int rmul;
   int tall;     // 1: one activation tile of 128 + (k-1)*dil rows per channel chunk, taps address it through row-shifted
-                //    UMMA descriptors; 0: a fresh 128-row tile per (chunk, tap)
+                //    wgmma descriptors; 0: a fresh 128-row tile per (chunk, tap)
   int a_bytes;  // bytes of one activation plane tile in shared memory (multiple of 1024)
   int baseoff;  // experiment: fill the descriptor base-offset field for row-shifted tiles
   int cn;       // CTAs of a cluster along the channel-tile axis that share (TMA-multicast) one activation tile; 1 = off
@@ -80,14 +82,13 @@ struct TcBatchScalars {
                 //   3 = (hi, mid, lo), six MMAs (hl + lh + mm + mh + hm + hh): products exact to the last fp32 bit
   int ast, wst; // ring depths (activation / weight tiles) for this launch
   int dbgskip;  // tuning experiments (timing only, wrong results): 1 = no epilogue stores, 2 = no MMAs issued, 4 = no residual loads
-  int coal;     // 1: launches without split-K finish their tiles through the shared-memory transposition (coalesced rows)
   int wmc;      // persistent launches: 2 = CTA pairs (cluster (2,1,1)) walk adjacent row tiles and share every weight tile: each CTA
                 //   fetches half of it and TMA-multicasts it into both (halves the L2 reads of the dominant operand); 1 = off
   int persist;  // 1: 1-D grid of resident CTAs walking the (gx, gy, gz) tile space (machine-filling launches)
   int gx, gy, gz;
   int split;    // cluster split-K: `split` CTAs (cluster dims (1,1,split)) each run a contiguous range of the k-steps of one
                 //    output tile, exchange partial accumulators through distributed shared memory and each finish
-                //    64/split of the tile's columns (reduce-scatter; fixed summation order => deterministic).  1 = off
+                //    BN/split of the tile's columns (reduce-scatter; fixed summation order => deterministic).  1 = off
   unsigned long long* dbg;   // optional: %globaltimer stamps of CTA (0,0,0) for tuning (tools/microbench.py)
 };
 template <class PT, int MP = TC_MAXP>
@@ -95,8 +96,7 @@ struct TcBatchT : TcBatchScalars {
   PT p[MP];
 };
 using TcBatch = TcBatchT<TcProblem>;          // what the host fills
-// Parameter of the two-plane one-tile kernels: no third-plane maps (3.7 KB -> 2.65 KB of kernel parameters: conv_tc 744 -> 723 us
-// over the 68 launches of an utterance, in-graph A/B).
+// Parameter of the two-plane kernels: no third-plane maps (3.7 KB -> 2.65 KB of kernel parameters per launch).
 template <int MP>
 inline TcBatchT<TcProblemBase, MP> tc_lite(const TcBatch& tb) {
   TcBatchT<TcProblemBase, MP> l;
@@ -126,641 +126,127 @@ __device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-// tcgen05.commit that arrives on the mbarrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask)
-               : "memory");
-}
 __device__ __forceinline__ uint32_t cluster_rank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// K-major, 128-byte-swizzled operand tile whose rows are 128 bytes apart (8-row groups 1024 bytes apart)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, int use_base_offset = 0) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address, 16-byte units, bits [0,14)
-  if (use_base_offset) d |= (uint64_t)((saddr >> 7) & 7) << 49;   // base offset field (experiment, see DESIGN.md)
-  d |= (uint64_t)1 << 16;                           // leading byte offset (ignored for swizzled K-major), bits [16,30)
-  d |= (uint64_t)(1024 >> 4) << 32;                 // stride byte offset between 8-row groups, bits [32,46)
-  d |= (uint64_t)1 << 46;                           // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                           // layout type: SWIZZLE_128B
-  return d;
+// arrive on the mbarrier at this offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
+  uint32_t ra;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(rank));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
 }
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32, both operands K-major, M = 128
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- epilogue pieces shared by the plain and the split-K paths: EN accumulator columns starting at absolute column `cofs`
-template <int EN>
-__device__ __forceinline__ void tc_load_res(const TcProblemBase& P, float (&rr)[EN], int cofs, long orow, bool rowok) {
-  const bool gate = (P.epi & TCE_GATE) != 0;
-  const int ocb = gate ? (cofs >> 1) : cofs;
-  const int nvalid = gate ? min(EN / 2, (P.Cout >> 1) - ocb) : min(EN, P.Cout - cofs);
-  if (P.res && rowok && nvalid > 0) {
-    const float* rp = P.res + orow * (long)P.ldr + P.roff + ocb;
-#pragma unroll
-    for (int i = 0; i < EN; i += 4) {
-      if (i + 4 <= nvalid) {
-        const float4 q4 = *reinterpret_cast<const float4*>(rp + i);
-        rr[i] = q4.x; rr[i + 1] = q4.y; rr[i + 2] = q4.z; rr[i + 3] = q4.w;
-      } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) rr[i + e] = (i + e < nvalid) ? rp[i + e] : 0.f;
-      }
-    }
+// a ring slot shared by `n` CTAs of the cluster (multicast) is released in every one of them
+__device__ __forceinline__ void tc_release(uint64_t* bar, int n) {
+  if (n > 1) {
+    for (int r = 0; r < n; ++r) mbar_arrive_remote(bar, (uint32_t)r);
   } else {
-#pragma unroll
-    for (int i = 0; i < EN; ++i) rr[i] = 0.f;
+    mbar_arrive(bar);
   }
 }
-// v = accumulator + bias of EN columns; applies gate / relu / alpha / residual and stores fp32 rows and split-bf16 planes
-template <int EN>
-__device__ __forceinline__ void tc_finish_cols(const TcProblemBase& P, float (&v)[EN], const float (&rr)[EN], int cofs, long orow) {
+
+// ---- epilogue of one accumulator pair: columns (c, c+1) of output row `orow`; v0/v1 are the accumulator (or the split-K sum)
+__device__ __forceinline__ float tc_bias(const TcProblemBase& P, int b, int c) {
+  float bv = P.bias[c];
+  if (P.cond) bv += P.cond[(long)b * P.cond_ld + c];
+  return bv;
+}
+__device__ __forceinline__ void tc_epi_pair(const TcProblemBase& P, int b, long orow, int c, float v0, float v1, int dbgskip) {
   const bool gate = (P.epi & TCE_GATE) != 0;
+  float u[2];
+  int oc, nout;
+  if (gate) {                                   // channel pair (2i, 2i+1) makes output channel i
+    oc = c >> 1;
+    if (oc >= (P.Cout >> 1)) return;
+    nout = 1;
+    const float a = v0 + tc_bias(P, b, c), s = v1 + tc_bias(P, b, c + 1);
+    u[0] = tanhf(a) * (1.f / (1.f + expf(-s)));
+    u[1] = 0.f;
+  } else {
+    oc = c;
+    if (oc >= P.Cout) return;
+    nout = min(2, P.Cout - oc);
+    u[0] = v0 + tc_bias(P, b, c);
+    u[1] = nout > 1 ? v1 + tc_bias(P, b, c + 1) : 0.f;
+  }
   const bool relu = (P.epi & TCE_RELU) != 0;
-  const int ocb = gate ? (cofs >> 1) : cofs;           // first output channel of this pass
-  const int nvalid = gate ? min(EN / 2, (P.Cout >> 1) - ocb) : min(EN, P.Cout - cofs);
-  if (gate) {
 #pragma unroll
-    for (int i = 0; i < EN / 2; ++i) v[i] = tanhf(v[2 * i]) * (1.f / (1.f + expf(-v[2 * i + 1])));
+  for (int e = 0; e < 2; ++e) {
+    float q = u[e];
+    if (relu) q = fmaxf(q, 0.f);
+    u[e] = q * P.alpha;
   }
-#pragma unroll
-  for (int i = 0; i < EN; ++i) {
-    float u = v[i];
-    if (relu) u = fmaxf(u, 0.f);
-    v[i] = u * P.alpha + rr[i];
-  }
-  if (P.y) {
-    float* yr = P.y + orow * (long)P.ldy + P.yoff + ocb;
-    const bool al = ((P.ldy | P.yoff) & 3) == 0;
-#pragma unroll
-    for (int i = 0; i < EN; i += 4) {
-      if (al && i + 4 <= nvalid) {
-        *reinterpret_cast<float4*>(yr + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          if (i + e < nvalid) yr[i + e] = v[i + e];
-      }
+  if (P.res && !(dbgskip & 4)) {
+    const float* rp = P.res + orow * (long)P.ldr + P.roff + oc;
+    if (nout == 2 && ((P.ldr | P.roff | oc) & 1) == 0) {
+      const float2 q2 = *reinterpret_cast<const float2*>(rp);
+      u[0] += q2.x; u[1] += q2.y;
+    } else {
+      for (int e = 0; e < nout; ++e) u[e] += rp[e];
     }
+  }
+  if (dbgskip & 1) return;
+  if (P.y) {
+    float* yr = P.y + orow * (long)P.ldy + P.yoff + oc;
+    if (nout == 2 && ((P.ldy | P.yoff | oc) & 1) == 0) *reinterpret_cast<float2*>(yr) = make_float2(u[0], u[1]);
+    else for (int e = 0; e < nout; ++e) yr[e] = u[e];
   }
   if (P.p_hi) {
-    __nv_bfloat16* ph = P.p_hi + orow * (long)P.ldp + P.poff + ocb;
-    __nv_bfloat16* pl = P.p_lo + orow * (long)P.ldp + P.poff + ocb;
-    const bool al = ((P.ldp | P.poff) & 7) == 0;
+    const long po = orow * (long)P.ldp + P.poff + oc;
+    __align__(4) __nv_bfloat16 hb[2], mb[2], lb[2];
 #pragma unroll
-    for (int i = 0; i < EN; i += 8) {
-      __align__(16) __nv_bfloat16 hb[8], lb[8], mb[8];
-      if (P.p_mid) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          float u = v[i + e];
-          u = u > 0.f ? u : u * P.pl_slope;
-          split_bf16_3(u, hb[e], mb[e], lb[e]);
-        }
-        __nv_bfloat16* pm = P.p_mid + orow * (long)P.ldp + P.poff + ocb;
-        if (al && i + 8 <= nvalid) {
-          *reinterpret_cast<uint4*>(pm + i) = *reinterpret_cast<const uint4*>(mb);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            if (i + e < nvalid) pm[i + e] = mb[e];
-        }
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          float u = v[i + e];
-          u = u > 0.f ? u : u * P.pl_slope;
-          split_bf16(u, hb[e], lb[e]);
-        }
-      }
-      if (al && i + 8 <= nvalid) {
-        *reinterpret_cast<uint4*>(ph + i) = *reinterpret_cast<const uint4*>(hb);
-        *reinterpret_cast<uint4*>(pl + i) = *reinterpret_cast<const uint4*>(lb);
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; ++e)
-          if (i + e < nvalid) { ph[i + e] = hb[e]; pl[i + e] = lb[e]; }
-      }
-    }
-  }
-}
-
-// Coalesced finish of one epilogue pass (S == 1).  A TMEM lane is a tile row, so after tcgen05.ld a thread owns 64 columns of
-// ONE row: stores straight from that layout make every warp instruction touch 32 different rows (32 L1 wavefronts for
-// 512 bytes; ncu on the batched decoder launches: the LSU, not the tensor pipe or HBM, bounded the tile).  The warp
-// therefore parks its 32 x 64 block in shared memory (16-byte chunks XOR-swizzled by row, conflict-free both ways) and
-// reads it back with 16 lanes per row: a warp instruction then covers two rows x 256 contiguous bytes, the residual
-// is loaded and the fp32 rows / bf16 planes are stored as full lines.  `stg` = this warp's [32][64] floats.
-template <bool GATE>
-__device__ __forceinline__ void tc_finish_rows(const TcProblemBase& P, const float* stg, const float* bias_t, int cofs, int trow0, int L,
-                                               long out_base, int lane, const float4 (&rq)[16], bool r_pre) {
-  constexpr int NO = GATE ? 2 : 4;                    // outputs per thread (a gate pair (2i, 2i+1) makes one channel)
-  const int half = lane >> 4, cj = lane & 15;
-  const int c = cofs + cj * 4;
-  const int oc = GATE ? (c >> 1) : c;
-  const int nvalid = min(NO, (GATE ? (P.Cout >> 1) : P.Cout) - oc);
-  if (nvalid <= 0) return;
-  const float4 b4 = *reinterpret_cast<const float4*>(bias_t + cj * 4);
-  const bool relu = (P.epi & TCE_RELU) != 0;
-  const bool full = nvalid == NO;
-  const bool y_vec = full && ((P.ldy | P.yoff) & (NO - 1)) == 0;
-  const bool r_vec = full && ((P.ldr | P.roff) & (NO - 1)) == 0;
-  const bool p_vec = full && ((P.ldp | P.poff) & (NO - 1)) == 0;
-#pragma unroll
-  for (int it = 0; it < 16; ++it) {
-    const int r = it * 2 + half;
-    const int t = trow0 + r;
-    if (t >= L) break;
-    const long orow = out_base + (long)t * P.out_mul + P.out_add;
-    float4 a = *reinterpret_cast<const float4*>(stg + r * 64 + ((cj ^ (r & 7)) << 2));
-    a.x += b4.x; a.y += b4.y; a.z += b4.z; a.w += b4.w;
-    float u[4];
-    if (GATE) {
-      u[0] = tanhf(a.x) * (1.f / (1.f + expf(-a.y)));
-      u[1] = tanhf(a.z) * (1.f / (1.f + expf(-a.w)));
-      u[2] = u[3] = 0.f;
-    } else {
-      u[0] = a.x; u[1] = a.y; u[2] = a.z; u[3] = a.w;
-    }
-#pragma unroll
-    for (int e = 0; e < NO; ++e) {
+    for (int e = 0; e < 2; ++e) {
       float q = u[e];
-      if (relu) q = fmaxf(q, 0.f);
-      u[e] = q * P.alpha;
+      q = q > 0.f ? q : q * P.pl_slope;
+      if (P.p_mid) split_bf16_3(q, hb[e], mb[e], lb[e]);
+      else split_bf16(q, hb[e], lb[e]);
     }
-    if (r_pre) {
-      u[0] += rq[it].x; u[1] += rq[it].y; u[2] += rq[it].z; u[3] += rq[it].w;
-    } else if (P.res) {
-      const float* rp = P.res + orow * (long)P.ldr + P.roff + oc;
-      if (r_vec) {
-        if (GATE) { const float2 q2 = *reinterpret_cast<const float2*>(rp); u[0] += q2.x; u[1] += q2.y; }
-        else { const float4 q4 = *reinterpret_cast<const float4*>(rp); u[0] += q4.x; u[1] += q4.y; u[2] += q4.z; u[3] += q4.w; }
-      } else {
-#pragma unroll
-        for (int e = 0; e < NO; ++e) if (e < nvalid) u[e] += rp[e];
-      }
-    }
-    if (P.y) {
-      float* yr = P.y + orow * (long)P.ldy + P.yoff + oc;
-      if (y_vec) {
-        if (GATE) *reinterpret_cast<float2*>(yr) = make_float2(u[0], u[1]);
-        else *reinterpret_cast<float4*>(yr) = make_float4(u[0], u[1], u[2], u[3]);
-      } else {
-#pragma unroll
-        for (int e = 0; e < NO; ++e) if (e < nvalid) yr[e] = u[e];
-      }
-    }
-    if (P.p_hi) {
-      const long po = orow * (long)P.ldp + P.poff + oc;
-      __align__(8) __nv_bfloat16 hb[4], lb[4], mb[4];
-#pragma unroll
-      for (int e = 0; e < NO; ++e) {
-        float q = u[e];
-        q = q > 0.f ? q : q * P.pl_slope;
-        if (P.p_mid) split_bf16_3(q, hb[e], mb[e], lb[e]);
-        else split_bf16(q, hb[e], lb[e]);
-      }
-      if (p_vec) {
-        if (GATE) {
-          *reinterpret_cast<uint32_t*>(P.p_hi + po) = *reinterpret_cast<const uint32_t*>(hb);
-          *reinterpret_cast<uint32_t*>(P.p_lo + po) = *reinterpret_cast<const uint32_t*>(lb);
-          if (P.p_mid) *reinterpret_cast<uint32_t*>(P.p_mid + po) = *reinterpret_cast<const uint32_t*>(mb);
-        } else {
-          *reinterpret_cast<uint2*>(P.p_hi + po) = *reinterpret_cast<const uint2*>(hb);
-          *reinterpret_cast<uint2*>(P.p_lo + po) = *reinterpret_cast<const uint2*>(lb);
-          if (P.p_mid) *reinterpret_cast<uint2*>(P.p_mid + po) = *reinterpret_cast<const uint2*>(mb);
-        }
-      } else {
-#pragma unroll
-        for (int e = 0; e < NO; ++e)
-          if (e < nvalid) {
-            P.p_hi[po + e] = hb[e]; P.p_lo[po + e] = lb[e];
-            if (P.p_mid) P.p_mid[po + e] = mb[e];
-          }
+    if (nout == 2 && ((P.ldp | P.poff | oc) & 1) == 0) {
+      *reinterpret_cast<uint32_t*>(P.p_hi + po) = *reinterpret_cast<const uint32_t*>(hb);
+      *reinterpret_cast<uint32_t*>(P.p_lo + po) = *reinterpret_cast<const uint32_t*>(lb);
+      if (P.p_mid) *reinterpret_cast<uint32_t*>(P.p_mid + po) = *reinterpret_cast<const uint32_t*>(mb);
+    } else {
+      for (int e = 0; e < nout; ++e) {
+        P.p_hi[po + e] = hb[e]; P.p_lo[po + e] = lb[e];
+        if (P.p_mid) P.p_mid[po + e] = mb[e];
       }
     }
   }
-}
-
-// residual of the 16 (row, 4-column) units tc_finish_rows<false> handles in this thread, requested in one go (the loads
-// are in flight while the mainloop of the tile still runs).  Returns false when the vector path does not apply.
-__device__ __forceinline__ bool tc_prefetch_res_rows(const TcProblemBase& P, float4 (&rq)[16], int cofs, int trow0, int L, long out_base, int lane) {
-  if (!P.res || (P.epi & TCE_GATE) || ((P.ldr | P.roff) & 3) != 0) return false;
-  const int half = lane >> 4, cj = lane & 15;
-  const int c = cofs + cj * 4;
-  const bool colok = c + 4 <= P.Cout;
-#pragma unroll
-  for (int it = 0; it < 16; ++it) {
-    const int t = trow0 + it * 2 + half;
-    float4 q4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (colok && t < L) {
-      const long orow = out_base + (long)t * P.out_mul + P.out_add;
-      q4 = *reinterpret_cast<const float4*>(P.res + orow * (long)P.ldr + P.roff + c);
-    }
-    rq[it] = q4;
-  }
-  return true;
-}
-
-// Split-K tail of one epilogue thread (= one tile row).  The tile's BN columns are cut into SS slices of W = BN/SS;
-// slice q is finished by CTA q.  tc_split_send pushes the slices contained in one 64-column accumulator pass into the
-// owners' staging buffers [src CTA][row][W] (this CTA's own slice included, so no register array is indexed dynamically);
-// after the cluster barrier tc_split_finish adds the SS partials of its slice in rank order and runs the epilogue on them.
-template <int SS, int BN>
-__device__ __forceinline__ void tc_split_send(const float (&acc)[64], int half, float* stage, int sp, int row) {
-  constexpr int W = BN / SS;
-  constexpr int PER = 64 / W;              // slices inside one 64-column pass
-  const uint32_t mine = smem_u32(stage + ((size_t)sp * TC_BM + row) * W);
-#pragma unroll
-  for (int qq = 0; qq < PER; ++qq) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(mine), "r"(half * PER + qq));
-#pragma unroll
-    for (int i = 0; i < W; i += 4)
-      asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(ra + i * 4), "f"(acc[qq * W + i]), "f"(acc[qq * W + i + 1]),
-                   "f"(acc[qq * W + i + 2]), "f"(acc[qq * W + i + 3])
-                   : "memory");
-  }
-}
-template <int SS, int BN>
-__device__ __forceinline__ void tc_split_finish(const TcProblemBase& P, const float* stage, const float* bias_s, int sp, int row, int co0,
-                                                long orow, bool rowok) {
-  constexpr int W = BN / SS;
-  float rr[W];
-  tc_load_res<W>(P, rr, co0 + sp * W, orow, rowok);
-  cluster_sync_all();                      // (2) all partials have landed; nobody writes into a CTA after this point
-  float v[W];
-#pragma unroll
-  for (int i = 0; i < W; ++i) v[i] = 0.f;
-#pragma unroll
-  for (int src = 0; src < SS; ++src) {
-    const float4* sp4 = reinterpret_cast<const float4*>(stage + ((size_t)src * TC_BM + row) * W);
-#pragma unroll
-    for (int i = 0; i < W; i += 4) {
-      const float4 q4 = sp4[i >> 2];
-      v[i] += q4.x; v[i + 1] += q4.y; v[i + 2] += q4.z; v[i + 3] += q4.w;
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < W; ++i) v[i] += bias_s[sp * W + i];
-  if (rowok && co0 + sp * W < P.Cout) tc_finish_cols<W>(P, v, rr, co0 + sp * W, orow);
-}
-template <int SS, int BN, typename LoadAcc>
-__device__ __forceinline__ void tc_split_tail(const TcProblemBase& P, LoadAcc&& load_acc, float* stage, const float* bias_s, int sp, int row,
-                                              int co0, long orow, bool rowok) {
-  float v[64];
-  load_acc(0, v);
-  cluster_sync_all();                      // (1) every CTA of the cluster is done with its operand rings
-  tc_split_send<SS, BN>(v, 0, stage, sp, row);
-  if constexpr (BN == 128) {
-    load_acc(1, v);
-    tc_split_send<SS, BN>(v, 1, stage, sp, row);
-  }
-  tc_split_finish<SS, BN>(P, stage, bias_s, sp, row, co0, orow, rowok);
 }
 
 template <int BN>
-constexpr int tc_smem_bytes(int a_bytes, int np = 2, int ast = tc_ast<BN>(), int wst = tc_wst<BN>(), int stage_bytes = 0) {
-  return ast * np * a_bytes + wst * np * BN * TC_BK * 2 + 1024 /*alignment slack*/ + 256 /*barriers*/ + 2 * BN * 4 /*bias, two tiles in flight*/ +
-         stage_bytes /*epilogue transposition buffer of the S == 1 launches*/;
+constexpr int tc_smem_bytes(int a_bytes, int np = 2, int ast = tc_ast<BN>(), int wst = tc_wst<BN>()) {
+  return ast * np * a_bytes + wst * np * BN * TC_BK * 2 + 1024 /*alignment slack*/ + 256 /*barriers*/;
 }
-constexpr int TC_STAGE_BYTES = 4 * 32 * 64 * 4;   // four epilogue warps x [32 rows][64 columns] fp32
 constexpr int TC_MAXST = 4;   // barrier slots per ring
-
-// ---------------------------------------------------------------------------------------------------------------------
-// conv_tc_kernel<BN, SPLIT>: ONE tile per CTA, grid (row tiles, channel tiles, utterances x problems x split).  This is the
-// kernel of the latency-bound single-utterance launches (cluster split-K, or a single wave without split).  It is kept
-// separate from the persistent kernel below on purpose: folding both into one body cost 1.3-3 us on every one of the 68
-// launches of an utterance (in-graph timeline A/B of the two builds, r2: conv_tc 918 -> 1006 us, step +6.9 %) -- a longer
-// prologue in front of the first TMA request and a larger image for a chain in which every launch starts cold.
-// ---------------------------------------------------------------------------------------------------------------------
-// DYN = false: two operand planes and the default ring depths as compile-time constants (the single-utterance launches of the
-// bench default; the run-time depths / plane count of DYN = true -- exact 3-way split, tall tiles -- cost ~0.4 us per launch
-// on this chain: r1 vs r2 timeline A/B, conv_tc 729 -> 756 us over 68 launches).
-template <int BN, bool SPLIT, bool DYN, int MP = TC_MAXP>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-conv_tc_kernel(const __grid_constant__ TcBatchT<std::conditional_t<DYN, TcProblem, TcProblemBase>, MP> tb, const int* __restrict__ lens,
-               const int* __restrict__ offs) {
-  constexpr int B_BYTES = BN * TC_BK * 2;
-  const int TC_AST = DYN ? tb.ast : tc_ast<BN>(), TC_WST = DYN ? tb.wst : tc_wst<BN>(), NP = DYN ? tb.np : 2;
-  PDL_LAUNCH();
-  if (threadIdx.x == 0) TC_STAMP(0);
-  // cluster split-K ways; blockIdx.z = (b * n + problem) * S + rank.  The non-split instantiation carries none of the
-  // exchange code (measured: 6 % faster on machine-filling launches)
-  const int S = SPLIT ? tb.split : 1;
-  const int zi = blockIdx.z / S, sp = blockIdx.z - zi * S;
-  const int pi = zi % tb.n;
-  const int b = zi / tb.n;
-  const auto& P = tb.p[pi];
-  const int co0 = blockIdx.y * BN;
-  if (co0 >= P.Cout) return;
-  const int t0 = blockIdx.x * TC_BM;
-  const int A_BYTES = tb.a_bytes;
-  const bool tall = tb.tall != 0;
-
-  extern __shared__ uint8_t tc_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smem_w = smem + TC_AST * NP * A_BYTES;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem_w + TC_WST * NP * B_BYTES);
-  uint64_t* a_empty = a_full + TC_MAXST;
-  uint64_t* w_full = a_empty + TC_MAXST;
-  uint64_t* w_empty = w_full + TC_MAXST;
-  uint64_t* tmem_full = w_empty + TC_MAXST;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);          // [BN]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nsteps_all = (P.Cin / TC_BK) * P.k;
-  const int s_beg = (int)((long)nsteps_all * sp / S), s_end = (int)((long)nsteps_all * (sp + 1) / S);   // this CTA's k-steps
-  const int a_per = tall ? P.k : 1;                    // k-steps sharing one activation tile (tall => S == 1)
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < TC_AST; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], (uint32_t)tb.cn); }
-    for (int s = 0; s < TC_WST; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 1); }
-    mbar_init(tmem_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&P.a_hi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&P.a_lo)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&P.w_hi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&P.w_lo)) : "memory");
-    if constexpr (DYN) {
-      if (NP == 3) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&P.a_mid)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&P.w_mid)) : "memory");
-      }
-    }
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int cn = tb.cn;
-  const uint32_t crank = cn > 1 ? cluster_rank() : 0u;
-  const uint16_t cmask = (uint16_t)((1u << cn) - 1u);
-  if (cn > 1) cluster_sync_all();        // every peer's mbarriers exist before anybody multicasts into / arrives on them
-  // Weights are immutable: the first ring of weight tiles is requested before waiting for the producer of the activations.
-  // (lens/offs are final before any graph that reads them starts -- host copies or the previous phase's graph -- so the
-  //  peek below only decides whether prefetching is worth it: idle CTAs of ragged batches must not fetch and then drain
-  //  128 KB of weights; the authoritative read stays after the wait)
-  const bool peek_active = t0 < lens[b] * tb.rmul + P.in_extra;
-  const int w_pre = (tb.wpre && peek_active) ? min(TC_WST, s_end - s_beg) : 0;
-  // (ring slots, use parities and the (chunk, tap) pair of a k-step are carried as counters: the ring depths are launch
-  //  parameters, and run-time divisions in the single producer / issuer threads cost ~8 % on machine-filling launches)
-  auto issue_w = [&](int c, int j, int wst) {
-    uint8_t* wb = smem_w + wst * NP * B_BYTES;
-    mbar_expect_tx(&w_full[wst], NP * B_BYTES);
-    tma_load_2d(wb, &P.w_hi, c * TC_BK, j * P.Cout + co0, &w_full[wst]);
-    tma_load_2d(wb + B_BYTES, &P.w_lo, c * TC_BK, j * P.Cout + co0, &w_full[wst]);
-    if constexpr (DYN) { if (NP == 3) tma_load_2d(wb + 2 * B_BYTES, &P.w_mid, c * TC_BK, j * P.Cout + co0, &w_full[wst]); }
-  };
-  if (warp == 0 && lane == 0) {
-    int c = s_beg / P.k, j = s_beg - c * P.k;
-    for (int i = 0; i < w_pre; ++i) {          // w_pre <= TC_WST: slot == i
-      issue_w(c, j, i);
-      if (++j == P.k) { j = 0; ++c; }
-    }
-  }
-  // everything above touched only this CTA's resources and constants; from here on the producer kernel's results are needed
-  PDL_WAIT();
-  const int L = lens[b] * tb.rmul + P.in_extra;
-  const bool active = t0 < L;            // an idle CTA still has to release its TMEM columns below
-  const long in_base = (long)offs[b] * tb.rmul + (long)b * P.in_extra;
-  const long out_base = (long)offs[b] * tb.rmul * P.out_mul + (long)b * P.out_seq_extra;
-  if (threadIdx.x == 0) TC_STAMP(1);
-
-  if (!active) {
-    // nothing to compute; the prefetched weight tiles must have landed before this CTA's shared memory is released
-    if (warp == 0 && lane == 0)
-      for (int i = 0; i < w_pre; ++i) mbar_wait(&w_full[i], 0);
-  } else if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      const uint32_t a_tx = (uint32_t)NP * (uint32_t)(tall ? (TC_BM + (P.k - 1) * P.dil) : TC_BM) * 128u;   // bytes TMA delivers per set of planes
-      int c = s_beg / P.k, j = s_beg - c * P.k;
-      int ast = 0, a_use = 0, a_cnt = 0, wst = 0, w_use = 0;    // ring slot / times the ring wrapped / steps since the last A tile
-      for (int s = s_beg; s < s_end; ++s) {
-        const int ls = s - s_beg;                              // ring positions count this CTA's own steps
-        if (a_cnt == 0) {
-          const int use = a_use;
-          if (use > 0) mbar_wait(&a_empty[ast], (use - 1) & 1);
-          uint8_t* ab = smem + ast * NP * A_BYTES;
-          mbar_expect_tx(&a_full[ast], a_tx);
-          const int row = (int)in_base + t0 - P.pad + (tall ? 0 : j * P.dil);
-          if (cn > 1) {
-            // this CTA fetches rows [crank, crank+1) * 128/cn of the tile and multicasts them to all cn CTAs
-            const int slice = TC_BM / cn;
-            const int soff = (int)crank * slice;
-            tma_load_2d_mc(ab + soff * 128, &P.a_hi, c * TC_BK, row + soff, &a_full[ast], cmask);
-            tma_load_2d_mc(ab + A_BYTES + soff * 128, &P.a_lo, c * TC_BK, row + soff, &a_full[ast], cmask);
-          } else {
-            tma_load_2d(ab, &P.a_hi, c * TC_BK, row, &a_full[ast]);
-            tma_load_2d(ab + A_BYTES, &P.a_lo, c * TC_BK, row, &a_full[ast]);
-            if constexpr (DYN) { if (NP == 3) tma_load_2d(ab + 2 * A_BYTES, &P.a_mid, c * TC_BK, row, &a_full[ast]); }
-          }
-          if (++ast == TC_AST) { ast = 0; ++a_use; }
-        }
-        if (++a_cnt == a_per) a_cnt = 0;
-        if (ls >= w_pre) {                                     // (the first ring was requested before PDL_WAIT)
-          if (w_use > 0) mbar_wait(&w_empty[wst], (w_use - 1) & 1);
-          issue_w(c, j, wst);
-        }
-        if (++wst == TC_WST) { wst = 0; ++w_use; }
-        if (++j == P.k) { j = 0; ++c; }
-        if (ls == 0) TC_STAMP(2);
-      }
-      TC_STAMP(3);
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one thread)
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(BN);
-      int c = s_beg / P.k, j = s_beg - c * P.k;
-      int ast = 0, a_use = 0, a_cnt = 0, wst = 0, w_use = 0;
-      for (int s = s_beg; s < s_end; ++s) {
-        const int ls = s - s_beg;
-        if (a_cnt == 0) mbar_wait(&a_full[ast], a_use & 1);
-        mbar_wait(&w_full[wst], w_use & 1);
-        if (ls == 0) TC_STAMP(4);
-        tc_fence_after();
-        const uint32_t abase = smem_u32(smem + ast * NP * A_BYTES) + (tall ? (uint32_t)(j * P.dil) * 128u : 0u);
-        const uint32_t wbase = smem_u32(smem_w + wst * NP * B_BYTES);
-        const uint64_t ahi = umma_desc_sw128(abase, tb.baseoff), alo = umma_desc_sw128(abase + A_BYTES, tb.baseoff);
-        const uint64_t bhi = umma_desc_sw128(wbase), blo = umma_desc_sw128(wbase + B_BYTES);
-        if (NP == 3) {
-          // exact 3-way split: the six products that reach the last bit of an fp32 product, smallest first
-          const uint64_t ami = umma_desc_sw128(abase + 2 * A_BYTES), bmi = umma_desc_sw128(wbase + 2 * B_BYTES);
-#pragma unroll
-          for (int kk = 0; kk < TC_BK / 16; ++kk) {
-            const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-            umma_bf16(tmem_base, ahi + adv, blo + adv, idesc, (ls | kk) ? 1u : 0u);
-            umma_bf16(tmem_base, alo + adv, bhi + adv, idesc, 1u);
-            umma_bf16(tmem_base, ami + adv, bmi + adv, idesc, 1u);
-            umma_bf16(tmem_base, ami + adv, bhi + adv, idesc, 1u);
-            umma_bf16(tmem_base, ahi + adv, bmi + adv, idesc, 1u);
-            umma_bf16(tmem_base, ahi + adv, bhi + adv, idesc, 1u);
-          }
-        } else {
-#pragma unroll
-          for (int kk = 0; kk < TC_BK / 16; ++kk) {
-            const uint64_t adv = (uint64_t)((kk * 32) >> 4);     // 16 bf16 = 32 bytes along K inside the swizzle atom
-            umma_bf16(tmem_base, alo + adv, bhi + adv, idesc, (ls | kk) ? 1u : 0u);
-            umma_bf16(tmem_base, ahi + adv, blo + adv, idesc, 1u);
-            umma_bf16(tmem_base, ahi + adv, bhi + adv, idesc, 1u);
-          }
-        }
-        umma_commit(&w_empty[wst]);                            // frees the weight stage when these MMAs retire
-        if (++wst == TC_WST) { wst = 0; ++w_use; }
-        if (++a_cnt == a_per) {                                // ... and the activation tile after its last tap
-          if (cn > 1) umma_commit_mc(&a_empty[ast], cmask);    //     (in every CTA that multicasts into it)
-          else umma_commit(&a_empty[ast]);
-          a_cnt = 0;
-          if (++ast == TC_AST) { ast = 0; ++a_use; }
-        }
-        if (++j == P.k) { j = 0; ++c; }
-      }
-      umma_commit(tmem_full);                 // accumulator complete
-      TC_STAMP(5);
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue: 4 warps, one TMEM lane quadrant each
-    // Everything that does not depend on the accumulator is fetched while the mainloop runs: bias (+ per-utterance
-    // conditioning) into shared memory, the residual row into registers.
-    const int quad = warp & 3;
-    const int et = threadIdx.x - 64;                       // 0..127
-    if (et < BN) {
-      const int cc = co0 + et;
-      float bv = 0.f;
-      if (cc < P.Cout) {
-        bv = P.bias[cc];
-        if (P.cond) bv += P.cond[(long)b * P.cond_ld + cc];
-      }
-      bias_s[et] = bv;
-    }
-    const int t = t0 + quad * 32 + lane;
-    const bool rowok = t < L;
-    const long orow = out_base + (long)t * P.out_mul + P.out_add;
-    constexpr int EN = 64;                                 // columns handled per epilogue pass
-    float rr[EN];
-    if (S == 1) tc_load_res<EN>(P, rr, co0, orow, rowok);
-    asm volatile("bar.sync 1, 128;" ::: "memory");          // bias_s visible to the 4 epilogue warps
-    mbar_wait(tmem_full, 0);
-    if (threadIdx.x == 64) TC_STAMP(6);
-    tc_fence_after();
-    auto load_acc = [&](int eh, float (&v)[EN]) {           // 64 accumulator columns of this thread's TMEM lane
-      uint32_t rg[EN];
-#pragma unroll
-      for (int n0 = 0; n0 < EN; n0 += 16) {
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(eh * EN + n0);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(rg[n0 + 0]), "=r"(rg[n0 + 1]), "=r"(rg[n0 + 2]), "=r"(rg[n0 + 3]), "=r"(rg[n0 + 4]), "=r"(rg[n0 + 5]),
-              "=r"(rg[n0 + 6]), "=r"(rg[n0 + 7]), "=r"(rg[n0 + 8]), "=r"(rg[n0 + 9]), "=r"(rg[n0 + 10]), "=r"(rg[n0 + 11]),
-              "=r"(rg[n0 + 12]), "=r"(rg[n0 + 13]), "=r"(rg[n0 + 14]), "=r"(rg[n0 + 15])
-            : "r"(taddr));
-      }
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int i = 0; i < EN; ++i) v[i] = __uint_as_float(rg[i]);
-    };
-    if (S == 1) {
-#pragma unroll 1
-      for (int eh = 0; eh < BN / EN; ++eh) {
-        const int co0e = co0 + eh * EN;
-        if (co0e >= P.Cout) break;
-        if (eh > 0) tc_load_res<EN>(P, rr, co0e, orow, rowok);
-        float v[EN];
-        load_acc(eh, v);
-#pragma unroll
-        for (int i = 0; i < EN; ++i) v[i] += bias_s[eh * EN + i];
-        if (rowok) tc_finish_cols<EN>(P, v, rr, co0e, orow);
-      }
-    } else if constexpr (SPLIT) {
-      float* stage = reinterpret_cast<float*>(smem);       // [S][128][BN/S] fp32 (32 or 64 KB), aliases the activation ring
-      const int row = quad * 32 + lane;
-      if (S == 2) tc_split_tail<2, BN>(P, load_acc, stage, bias_s, sp, row, co0, orow, rowok);
-      else if (S == 4) tc_split_tail<4, BN>(P, load_acc, stage, bias_s, sp, row, co0, orow, rowok);
-      else tc_split_tail<8, BN>(P, load_acc, stage, bias_s, sp, row, co0, orow, rowok);
-    }
-  }
-  if (S > 1 && active && warp < 2) {       // the producer and MMA warps take part in the two split-K cluster barriers
-    __syncwarp();
-    cluster_sync_all();
-    cluster_sync_all();
-  }
-  if (threadIdx.x == 64) TC_STAMP(7);
-  tc_fence_before();
-  __syncthreads();
-  if (cn > 1) cluster_sync_all();        // no peer may still multicast into, or arrive on, this CTA's shared memory
-  if (threadIdx.x == 0) TC_STAMP(8);
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-  }
-}
-
 
 // One output tile of a launch: 128 rows x BN channels of problem `P` in utterance `b`.
 struct TcTile {
   int pi;           // problem index (the problem is always addressed as tb.p[pi]: a pointer into the __grid_constant__ parameter
-                    //  turns every field access into a generic load instead of an indexed constant-bank read -- measured +7 % on
-                    //  the 68-launch single-utterance chain)
+                    //  turns every field access into a generic load instead of an indexed constant-bank read)
   int b, co0, t0, sp;
   int t0u;          // first row of the scheduling unit (== t0, or the pair's first tile with weight multicast)
   bool valid;       // the problem has this channel tile (grouped problems may differ in Cout)
 };
 
-// Launch shapes.  (1) one tile per CTA, grid (row tiles, channel tiles, utterances x problems x split): the latency-bound
-// single-utterance launches, with cluster split-K.  (2) tb.persist: a 1-D grid of one CTA per SM walks the same tile space
-// with a stride of gridDim.x; the accumulator is double-buffered in TMEM (2 x BN columns), the operand rings and their
-// parities run on across tiles, so tile i's epilogue (TMEM -> registers -> global) overlaps tile i+1's TMA + MMA mainloop
-// and the per-CTA prologue (barrier init, TMEM allocation, descriptor prefetch, pipeline fill) is paid once per SM
-// instead of once per tile.
-template <int BN>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict__ lens, const int* __restrict__ offs) {
-  constexpr bool SPLIT = false;          // (this kernel carries no split-K exchange; the S > 1 branches below fold away)
+// ---------------------------------------------------------------------------------------------------------------------
+// The kernel body.  Launch shapes: (1) one tile per CTA, grid (row tiles, channel tiles, utterances x problems x split):
+// the latency-bound single-utterance launches, with cluster split-K.  (2) tb.persist: a 1-D grid of one CTA per SM walks
+// the same tile space with a stride of gridDim.x; the operand rings and their parities run on across tiles, so the
+// producer fetches tile i+1's operands while the consumers run tile i's epilogue, and the per-CTA prologue (barrier
+// init, descriptor prefetch, pipeline fill) is paid once per SM instead of once per tile.
+// ---------------------------------------------------------------------------------------------------------------------
+template <int BN, class PT, int MP>
+__device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const int* __restrict__ lens, const int* __restrict__ offs) {
+  constexpr bool HAS_MID = std::is_same<PT, TcProblem>::value;
   constexpr int B_BYTES = BN * TC_BK * 2;
-  const int TC_AST = tb.ast, TC_WST = tb.wst, NP = tb.np;
+  constexpr int NACC = BN / 2;                 // accumulator registers per consumer thread (m64nBN fragment)
+  const int TC_AST = tb.ast, TC_WST = tb.wst, NP = HAS_MID ? tb.np : 2;
   PDL_LAUNCH();
   if (threadIdx.x == 0) TC_STAMP(0);
-  // cluster split-K ways; z = (b * n + problem) * S + rank.  The non-split instantiation carries none of the
-  // exchange code (measured: 6 % faster on machine-filling launches)
-  const int S = SPLIT ? tb.split : 1;
-  const bool persist = !SPLIT && tb.persist != 0;
+  const int S = tb.split;
+  const bool persist = tb.persist != 0;
   const int A_BYTES = tb.a_bytes;
   const bool tall = tb.tall != 0;
   const int wmc = persist ? tb.wmc : 1;                    // CTAs sharing each weight tile (scheduling unit = wmc adjacent row tiles)
@@ -770,8 +256,7 @@ conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict
   const int tstride = persist ? (int)gridDim.x / wmc : 1;
   const int tile0 = persist ? (int)blockIdx.x / wmc : 0;
   auto decode = [&](int tile) {
-    int bx, by, bz;
-    int bxu;
+    int bx, by, bz, bxu;
     if (persist) {
       bxu = tile % gxu;
       const int r = tile / gxu;
@@ -801,51 +286,41 @@ conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict
   uint64_t* a_empty = a_full + TC_MAXST;
   uint64_t* w_full = a_empty + TC_MAXST;
   uint64_t* w_empty = w_full + TC_MAXST;
-  uint64_t* acc_full = w_empty + TC_MAXST;          // [2] accumulator buffer complete (tcgen05.commit)
-  uint64_t* acc_empty = acc_full + 2;               // [2] accumulator buffer drained by the 4 epilogue warps
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* bias_s = reinterpret_cast<float*>(tmem_slot + 4);          // [2][BN]
-  float* stage_t = bias_s + 2 * BN;                                 // [4][32][64] (launches without split-K only)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool producer = warp == TC_CWG * 4;
   const TcTile first = decode(tile0);
-  const uint32_t tmem_cols = persist ? 2u * BN : (uint32_t)BN;
+  const int cn = tb.cn;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < TC_AST; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], (uint32_t)tb.cn); }
-    for (int s = 0; s < TC_WST; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], (uint32_t)wmc); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+  if (producer && lane == 0) {
+    // every consumer warpgroup of every CTA reading a slot releases it
+    for (int s = 0; s < TC_AST; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], (uint32_t)(cn * TC_CWG)); }
+    for (int s = 0; s < TC_WST; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], (uint32_t)(wmc * TC_CWG)); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     for (int q = 0; q < (persist ? tb.n : 1); ++q) {
-      const TcProblem& Q = tb.p[persist ? q : first.pi];
+      const PT& Q = tb.p[persist ? q : first.pi];
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.a_hi)) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.a_lo)) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.w_hi)) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.w_lo)) : "memory");
-      if (NP == 3) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.a_mid)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.w_mid)) : "memory");
+      if constexpr (HAS_MID) {
+        if (NP == 3) {
+          asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.a_mid)) : "memory");
+          asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&Q.w_mid)) : "memory");
+        }
       }
     }
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int cn = tb.cn;
   const uint32_t crank = cn > 1 ? cluster_rank() : 0u;
   const uint16_t cmask = (uint16_t)((1u << cn) - 1u);
   if (cn > 1 || wmc > 1) cluster_sync_all();   // every peer's mbarriers exist before anybody multicasts into / arrives on them
   // Weights are immutable: the first ring of weight tiles is requested before waiting for the producer of the activations.
   // (lens/offs are final before any graph that reads them starts -- host copies or the previous phase's graph -- so the
   //  peek below only decides whether prefetching is worth it: idle CTAs of ragged batches must not fetch and then drain
-  //  128 KB of weights; the authoritative read stays after the wait)
+  //  weights; the authoritative read stays after the wait)
   int w_pre = 0;
-  auto issue_w = [&](const TcProblem& P, int co0, int c, int j, int wst) {
+  auto issue_w = [&](const PT& P, int co0, int c, int j, int wst) {
     uint8_t* wb = smem_w + wst * NP * B_BYTES;
     mbar_expect_tx(&w_full[wst], NP * B_BYTES);
     if (wmc > 1) {
@@ -858,15 +333,15 @@ conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict
     }
     tma_load_2d(wb, &P.w_hi, c * TC_BK, j * P.Cout + co0, &w_full[wst]);
     tma_load_2d(wb + B_BYTES, &P.w_lo, c * TC_BK, j * P.Cout + co0, &w_full[wst]);
-    if (NP == 3) tma_load_2d(wb + 2 * B_BYTES, &P.w_mid, c * TC_BK, j * P.Cout + co0, &w_full[wst]);
+    if constexpr (HAS_MID) { if (NP == 3) tma_load_2d(wb + 2 * B_BYTES, &P.w_mid, c * TC_BK, j * P.Cout + co0, &w_full[wst]); }
   };
   if (!persist && first.valid) {
-    const TcProblem& P = tb.p[first.pi];
+    const PT& P = tb.p[first.pi];
     const int nsteps_all = (P.Cin / TC_BK) * P.k;
     const int s_beg = (int)((long)nsteps_all * first.sp / S), s_end = (int)((long)nsteps_all * (first.sp + 1) / S);
     const bool peek_active = first.t0 < lens[first.b] * tb.rmul + P.in_extra;
     w_pre = (tb.wpre && peek_active) ? min(TC_WST, s_end - s_beg) : 0;
-    if (warp == 0 && lane == 0) {
+    if (producer && lane == 0) {
       int c = s_beg / P.k, j = s_beg - c * P.k;
       for (int i = 0; i < w_pre; ++i) {          // w_pre <= TC_WST: slot == i
         issue_w(P, first.co0, c, j, i);
@@ -879,16 +354,16 @@ conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict
   if (threadIdx.x == 0) TC_STAMP(1);
   bool any_active = false;               // (split-K: the single tile of this CTA is active)
 
-  if (warp == 0) {
+  if (producer) {
     // ------------------------------------------------------------------ TMA producer (one thread)
     // (ring slots, use parities and the (chunk, tap) pair of a k-step are carried as counters: the ring depths are launch
-    //  parameters, and run-time divisions in the single producer / issuer threads cost ~8 % on machine-filling launches)
+    //  parameters, and run-time divisions in the single producer thread are on the critical path of every step)
     if (lane == 0) {
       int ast = 0, a_use = 0, wst = 0, w_use = 0;    // ring slot / times the ring wrapped: run on across tiles
       for (int tile = tile0; tile < ntiles; tile += tstride) {
         const TcTile T = persist ? decode(tile) : first;
         if (!T.valid) continue;
-        const TcProblem& P = tb.p[T.pi];
+        const PT& P = tb.p[T.pi];
         const int L = lens[T.b] * tb.rmul + P.in_extra;
         if (T.t0u >= L) {
           // nothing to compute; prefetched weight tiles must have landed before this CTA's shared memory is released
@@ -919,7 +394,7 @@ conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict
             } else {
               tma_load_2d(ab, &P.a_hi, c * TC_BK, row, &a_full[ast]);
               tma_load_2d(ab + A_BYTES, &P.a_lo, c * TC_BK, row, &a_full[ast]);
-              if (NP == 3) tma_load_2d(ab + 2 * A_BYTES, &P.a_mid, c * TC_BK, row, &a_full[ast]);
+              if constexpr (HAS_MID) { if (NP == 3) tma_load_2d(ab + 2 * A_BYTES, &P.a_mid, c * TC_BK, row, &a_full[ast]); }
             }
             if (++ast == TC_AST) { ast = 0; ++a_use; }
           }
@@ -937,197 +412,170 @@ conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict
       }
     }
     any_active = __shfl_sync(0xffffffffu, (int)any_active, 0) != 0;
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one thread)
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(BN);
-      int ast = 0, a_use = 0, wst = 0, w_use = 0, lt = 0;
-      for (int tile = tile0; tile < ntiles; tile += tstride) {
-        const TcTile T = persist ? decode(tile) : first;
-        if (!T.valid) continue;
-        const TcProblem& P = tb.p[T.pi];
-        const int L = lens[T.b] * tb.rmul + P.in_extra;
-        if (T.t0u >= L) continue;
-        any_active = true;
-        const int nsteps_all = (P.Cin / TC_BK) * P.k;
-        const int s_beg = (int)((long)nsteps_all * T.sp / S), s_end = (int)((long)nsteps_all * (T.sp + 1) / S);
-        const int a_per = tall ? P.k : 1;
-        const int buf = lt & 1;
-        const uint32_t tmem_acc = tmem_base + (uint32_t)(buf * BN);
-        if (lt >= 2) {                                          // the epilogue has drained this buffer's previous tile
-          mbar_wait(&acc_empty[buf], ((lt >> 1) - 1) & 1);
-          tc_fence_after();
-        }
-        int c = s_beg / P.k, j = s_beg - c * P.k;
-        int a_cnt = 0;
-        for (int s = s_beg; s < s_end; ++s) {
-          const int ls = s - s_beg;
-          if (a_cnt == 0) mbar_wait(&a_full[ast], a_use & 1);
-          mbar_wait(&w_full[wst], w_use & 1);
-          if (ls == 0) TC_STAMP(4);
-          tc_fence_after();
-          const uint32_t abase = smem_u32(smem + ast * NP * A_BYTES) + (tall ? (uint32_t)(j * P.dil) * 128u : 0u);
-          const uint32_t wbase = smem_u32(smem_w + wst * NP * B_BYTES);
-          const uint64_t ahi = umma_desc_sw128(abase, tb.baseoff), alo = umma_desc_sw128(abase + A_BYTES, tb.baseoff);
-          const uint64_t bhi = umma_desc_sw128(wbase), blo = umma_desc_sw128(wbase + B_BYTES);
-          if (tb.dbgskip & 2) {
-          } else if (NP == 3) {
-            // exact 3-way split: the six products that reach the last bit of an fp32 product, smallest first
-            const uint64_t ami = umma_desc_sw128(abase + 2 * A_BYTES), bmi = umma_desc_sw128(wbase + 2 * B_BYTES);
-#pragma unroll
-            for (int kk = 0; kk < TC_BK / 16; ++kk) {
-              const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-              umma_bf16(tmem_acc, ahi + adv, blo + adv, idesc, (ls | kk) ? 1u : 0u);
-              umma_bf16(tmem_acc, alo + adv, bhi + adv, idesc, 1u);
-              umma_bf16(tmem_acc, ami + adv, bmi + adv, idesc, 1u);
-              umma_bf16(tmem_acc, ami + adv, bhi + adv, idesc, 1u);
-              umma_bf16(tmem_acc, ahi + adv, bmi + adv, idesc, 1u);
-              umma_bf16(tmem_acc, ahi + adv, bhi + adv, idesc, 1u);
-            }
-          } else {
-#pragma unroll
-            for (int kk = 0; kk < TC_BK / 16; ++kk) {
-              const uint64_t adv = (uint64_t)((kk * 32) >> 4);     // 16 bf16 = 32 bytes along K inside the swizzle atom
-              umma_bf16(tmem_acc, alo + adv, bhi + adv, idesc, (ls | kk) ? 1u : 0u);
-              umma_bf16(tmem_acc, ahi + adv, blo + adv, idesc, 1u);
-              umma_bf16(tmem_acc, ahi + adv, bhi + adv, idesc, 1u);
-            }
-          }
-          if (wmc > 1) umma_commit_mc(&w_empty[wst], (uint16_t)3);   // frees the weight stage (in both CTAs of a pair) when these MMAs retire
-          else umma_commit(&w_empty[wst]);
-          if (++wst == TC_WST) { wst = 0; ++w_use; }
-          if (++a_cnt == a_per) {                                // ... and the activation tile after its last tap
-            if (cn > 1) umma_commit_mc(&a_empty[ast], cmask);    //     (in every CTA that multicasts into it)
-            else umma_commit(&a_empty[ast]);
-            a_cnt = 0;
-            if (++ast == TC_AST) { ast = 0; ++a_use; }
-          }
-          if (++j == P.k) { j = 0; ++c; }
-        }
-        umma_commit(&acc_full[buf]);            // accumulator complete
-        ++lt;
-        TC_STAMP(5);
-      }
-    }
-    any_active = __shfl_sync(0xffffffffu, (int)any_active, 0) != 0;
   } else {
-    // ------------------------------------------------------------------ epilogue: 4 warps, one TMEM lane quadrant each
-    // Everything that does not depend on the accumulator is fetched while the mainloop runs: bias (+ per-utterance
-    // conditioning) into shared memory, the residual row into registers.
-    const int quad = warp & 3;
-    const int et = threadIdx.x - 64;                       // 0..127
-    int lt = 0;
+    // ------------------------------------------------------------------ consumers: wgmma mainloop + epilogue
+    const int wg = warp >> 2;                              // rows [64 wg, 64 wg + 64) of the tile
+    const int g = lane >> 2, q4 = lane & 3;
+    const int rbase = wg * 64 + (warp & 3) * 16 + g;       // this thread's rows: rbase, rbase + 8
+    const bool leader = (threadIdx.x & 127) == 0;
+    int ast = 0, a_use = 0, wst = 0, w_use = 0;
     for (int tile = tile0; tile < ntiles; tile += tstride) {
       const TcTile T = persist ? decode(tile) : first;
       if (!T.valid) continue;
-      const TcProblem& P = tb.p[T.pi];
+      const PT& P = tb.p[T.pi];
       const int L = lens[T.b] * tb.rmul + P.in_extra;
       if (T.t0u >= L) continue;                              // (with weight multicast a CTA whose own tile lies behind the end of the
-                                                             //  utterance still runs the mainloop and this handshake; it stores nothing)
-      const int b = T.b, co0 = T.co0, sp = T.sp;
-      const int buf = lt & 1;
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(buf * BN);
-      float* bias_t = bias_s + buf * BN;
+                                                             //  utterance still runs the mainloop; it stores nothing)
+      any_active = true;
+      const int nsteps_all = (P.Cin / TC_BK) * P.k;
+      const int s_beg = (int)((long)nsteps_all * T.sp / S), s_end = (int)((long)nsteps_all * (T.sp + 1) / S);
+      const int a_per = tall ? P.k : 1;
+      float acc[NACC];
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+      int j = s_beg % P.k;
+      int a_cnt = 0;
+      // the slots of the previous k-step are released once its MMAs have retired (one wgmma group stays in flight)
+      int prev_w = -1, prev_a = -1;
+      for (int s = s_beg; s < s_end; ++s) {
+        const int ls = s - s_beg;
+        if (a_cnt == 0) mbar_wait(&a_full[ast], a_use & 1);
+        mbar_wait(&w_full[wst], w_use & 1);
+        if (ls == 0 && threadIdx.x == 0) TC_STAMP(4);
+        const uint32_t abase = smem_u32(smem + ast * NP * A_BYTES) + (uint32_t)(wg * 64 * 128) + (tall ? (uint32_t)(j * P.dil) * 128u : 0u);
+        const uint32_t wbase = smem_u32(smem_w + wst * NP * B_BYTES);
+        const uint64_t ahi = gmma_desc_sw128(abase, tb.baseoff), alo = gmma_desc_sw128(abase + A_BYTES, tb.baseoff);
+        const uint64_t bhi = gmma_desc_sw128(wbase), blo = gmma_desc_sw128(wbase + B_BYTES);
+        auto mma = [&](uint64_t da, uint64_t db) {
+          if constexpr (BN == 128) wgmma_ss_n128(acc, da, db);
+          else wgmma_ss_n64(acc, da, db);
+        };
+        wgmma_fence();
+        if (tb.dbgskip & 2) {
+        } else if (NP == 3) {
+          // exact 3-way split: the six products that reach the last bit of an fp32 product, smallest first
+          const uint64_t ami = gmma_desc_sw128(abase + 2 * A_BYTES, tb.baseoff), bmi = gmma_desc_sw128(wbase + 2 * B_BYTES);
+#pragma unroll
+          for (int kk = 0; kk < TC_BK / 16; ++kk) {
+            const uint64_t adv = (uint64_t)((kk * 32) >> 4);
+            mma(ahi + adv, blo + adv);
+            mma(alo + adv, bhi + adv);
+            mma(ami + adv, bmi + adv);
+            mma(ami + adv, bhi + adv);
+            mma(ahi + adv, bmi + adv);
+            mma(ahi + adv, bhi + adv);
+          }
+        } else {
+#pragma unroll
+          for (int kk = 0; kk < TC_BK / 16; ++kk) {
+            const uint64_t adv = (uint64_t)((kk * 32) >> 4);     // 16 bf16 = 32 bytes along K inside the swizzle atom
+            mma(alo + adv, bhi + adv);
+            mma(ahi + adv, blo + adv);
+            mma(ahi + adv, bhi + adv);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        wgmma_touch<NACC>(acc);
+        if (leader) {
+          if (prev_w >= 0) tc_release(&w_empty[prev_w], wmc);
+          if (prev_a >= 0) tc_release(&a_empty[prev_a], cn);
+        }
+        prev_w = wst;
+        prev_a = -1;
+        if (++wst == TC_WST) { wst = 0; ++w_use; }
+        if (++a_cnt == a_per) {                                // the activation tile is released after its last tap
+          prev_a = ast;
+          a_cnt = 0;
+          if (++ast == TC_AST) { ast = 0; ++a_use; }
+        }
+        if (++j == P.k) j = 0;
+      }
+      wgmma_wait<0>();
+      wgmma_touch<NACC>(acc);
+      if (leader) {
+        if (prev_w >= 0) tc_release(&w_empty[prev_w], wmc);
+        if (prev_a >= 0) tc_release(&a_empty[prev_a], cn);
+      }
+      if (threadIdx.x == 0) TC_STAMP(5);
+      // ---- epilogue
+      const int b = T.b, co0 = T.co0;
       const long out_base = (long)offs[b] * tb.rmul * P.out_mul + (long)b * P.out_seq_extra;
-      if (et < BN) {
-        const int cc = co0 + et;
-        float bv = 0.f;
-        if (cc < P.Cout) {
-          bv = P.bias[cc];
-          if (P.cond) bv += P.cond[(long)b * P.cond_ld + cc];
-        }
-        bias_t[et] = bv;
+      long orow[2];
+      bool rowok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = T.t0 + rbase + 8 * h;
+        rowok[h] = t < L;
+        orow[h] = out_base + (long)t * P.out_mul + P.out_add;
       }
-      const int t = T.t0 + quad * 32 + lane;
-      const bool rowok = t < L;
-      const long orow = out_base + (long)t * P.out_mul + P.out_add;
-      constexpr int EN = 64;                                 // columns handled per epilogue pass
-      const bool coal = S == 1 && tb.coal != 0;
-      const int trow0 = T.t0 + quad * 32;
-      float rr[EN];                                          // residual, fetched while the mainloop runs: a row's 64 columns, or
-      float4 (&rq)[16] = *reinterpret_cast<float4 (*)[16]>(rr);   // (coalesced epilogue) 16 (row, 4-column) units
-      bool r_pre = false;
       if (S == 1) {
-        if (coal) r_pre = tc_prefetch_res_rows(P, rq, co0, trow0, L, out_base, lane);
-        else tc_load_res<EN>(P, rr, co0, orow, rowok && !(tb.dbgskip & 4));
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");          // bias visible to the 4 epilogue warps (two tiles may be in flight:
-                                                              //  bias_s is double-buffered, tile i+2 is written after tile i+1's barrier)
-      mbar_wait(&acc_full[buf], (lt >> 1) & 1);
-      if (threadIdx.x == 64) TC_STAMP(6);
-      tc_fence_after();
-      auto load_acc = [&](int eh, float (&v)[EN]) {           // 64 accumulator columns of this thread's TMEM lane
-        uint32_t rg[EN];
 #pragma unroll
-        for (int n0 = 0; n0 < EN; n0 += 16) {
-          const uint32_t taddr = tmem_acc + ((uint32_t)(quad * 32) << 16) + (uint32_t)(eh * EN + n0);
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-              : "=r"(rg[n0 + 0]), "=r"(rg[n0 + 1]), "=r"(rg[n0 + 2]), "=r"(rg[n0 + 3]), "=r"(rg[n0 + 4]), "=r"(rg[n0 + 5]),
-                "=r"(rg[n0 + 6]), "=r"(rg[n0 + 7]), "=r"(rg[n0 + 8]), "=r"(rg[n0 + 9]), "=r"(rg[n0 + 10]), "=r"(rg[n0 + 11]),
-                "=r"(rg[n0 + 12]), "=r"(rg[n0 + 13]), "=r"(rg[n0 + 14]), "=r"(rg[n0 + 15])
-              : "r"(taddr));
+        for (int jn = 0; jn < BN / 8; ++jn) {
+          const int c = co0 + jn * 8 + 2 * q4;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (rowok[h]) tc_epi_pair(P, b, orow[h], c, acc[4 * jn + 2 * h], acc[4 * jn + 2 * h + 1], tb.dbgskip);
         }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      } else {
+        // split-K reduce-scatter: CTA q of the cluster finishes columns [q W, q W + W) of the tile.  Every CTA sends each
+        // partial pair to the owner's staging buffer [src CTA][row][W]; the owner adds the S partials in rank order.
+        const int W = BN / S, sp = T.sp;
+        float* stage = reinterpret_cast<float*>(smem);       // [S][128][W] fp32 (BN/2 KB), aliases the operand rings
+        cluster_sync_all();                                  // (1) every CTA of the cluster is done with its operand rings
 #pragma unroll
-        for (int i = 0; i < EN; ++i) v[i] = __uint_as_float(rg[i]);
-      };
-      if (S == 1) {
-        const int npass = min(BN / EN, (P.Cout - co0 + EN - 1) / EN);
-        float* stg = stage_t + quad * (32 * 64);
-        const bool gate = (P.epi & TCE_GATE) != 0;
-#pragma unroll 1
-        for (int eh = 0; eh < npass; ++eh) {
-          const int co0e = co0 + eh * EN;
-          if (eh > 0) {
-            if (coal) r_pre = tc_prefetch_res_rows(P, rq, co0e, trow0, L, out_base, lane);
-            else tc_load_res<EN>(P, rr, co0e, orow, rowok && !(tb.dbgskip & 4));
-          }
-          float v[EN];
-          load_acc(eh, v);
-          if (persist && eh == npass - 1) {                    // accumulator buffer drained: the MMA warp may refill it
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-          }
-          if (coal) {
+        for (int jn = 0; jn < BN / 8; ++jn) {
+          const int cc = jn * 8 + 2 * q4;
+          const int qo = cc / W;
 #pragma unroll
-            for (int jq = 0; jq < EN / 4; ++jq)
-              *reinterpret_cast<float4*>(stg + lane * 64 + ((jq ^ (lane & 7)) << 2)) = make_float4(v[4 * jq], v[4 * jq + 1], v[4 * jq + 2], v[4 * jq + 3]);
-            __syncwarp();
-            if (gate) tc_finish_rows<true>(P, stg, bias_t + eh * EN, co0e, trow0, L, out_base, lane, rq, false);
-            else tc_finish_rows<false>(P, stg, bias_t + eh * EN, co0e, trow0, L, out_base, lane, rq, r_pre);
-            __syncwarp();                                      // the next pass (or tile) overwrites the block
-          } else {
-#pragma unroll
-            for (int i = 0; i < EN; ++i) v[i] += bias_t[eh * EN + i];
-            if (rowok && !(tb.dbgskip & 1)) tc_finish_cols<EN>(P, v, rr, co0e, orow);
+          for (int h = 0; h < 2; ++h) {
+            uint32_t ra;
+            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(stage + ((size_t)sp * TC_BM + rbase + 8 * h) * W + (cc - qo * W))), "r"(qo));
+            asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(ra), "f"(acc[4 * jn + 2 * h]), "f"(acc[4 * jn + 2 * h + 1]) : "memory");
           }
         }
-      } else if constexpr (SPLIT) {
-        float* stage = reinterpret_cast<float*>(smem);       // [S][128][BN/S] fp32 (32 or 64 KB), aliases the activation ring
-        const int row = quad * 32 + lane;
-        if (S == 2) tc_split_tail<2, BN>(P, load_acc, stage, bias_t, sp, row, co0, orow, rowok);
-        else if (S == 4) tc_split_tail<4, BN>(P, load_acc, stage, bias_t, sp, row, co0, orow, rowok);
-        else tc_split_tail<8, BN>(P, load_acc, stage, bias_t, sp, row, co0, orow, rowok);
+        cluster_sync_all();                                  // (2) all partials have landed; nobody writes into a CTA after this point
+#pragma unroll
+        for (int jn = 0; jn < BN / 8; ++jn) {
+          const int cc = jn * 8 + 2 * q4;
+          if (cc / W != sp) continue;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float v0 = 0.f, v1 = 0.f;
+            for (int src = 0; src < S; ++src) {
+              const float2 p2 = *reinterpret_cast<const float2*>(stage + ((size_t)src * TC_BM + rbase + 8 * h) * W + (cc - sp * W));
+              v0 += p2.x; v1 += p2.y;
+            }
+            if (rowok[h]) tc_epi_pair(P, b, orow[h], co0 + cc, v0, v1, tb.dbgskip);
+          }
+        }
       }
-      ++lt;
     }
   }
-  if (S > 1 && any_active && warp < 2) {   // the producer and MMA warps take part in the two split-K cluster barriers
+  if (S > 1 && any_active && producer) {   // the producer warp takes part in the two split-K cluster barriers
     __syncwarp();
     cluster_sync_all();
     cluster_sync_all();
   }
-  if (threadIdx.x == 64) TC_STAMP(7);
-  tc_fence_before();
+  if (threadIdx.x == 0) TC_STAMP(7);
   __syncthreads();
   if (cn > 1 || wmc > 1) cluster_sync_all();   // no peer may still multicast into, or arrive on, this CTA's shared memory
   if (threadIdx.x == 0) TC_STAMP(8);
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
-  }
+}
+
+// Single-wave launches (cluster split-K, or one tile per CTA).  DYN = false: two operand planes, the launch descriptor without
+// the third-plane tensor maps (the default single-utterance launches).
+template <int BN, bool DYN, int MP = TC_MAXP>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+conv_tc_kernel(const __grid_constant__ TcBatchT<std::conditional_t<DYN, TcProblem, TcProblemBase>, MP> tb, const int* __restrict__ lens,
+               const int* __restrict__ offs) {
+  conv_tc_body<BN>(tb, lens, offs);
+}
+// More than one wave of tiles: persistent grid (tb.persist), or one tile per CTA.
+template <int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict__ lens, const int* __restrict__ offs) {
+  conv_tc_body<BN>(tb, lens, offs);
 }
 
 // ------------------------------------------------------------------------------------------------

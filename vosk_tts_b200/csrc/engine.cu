@@ -2,7 +2,7 @@
 //
 // Replaces the one call `self.model.onnx.run(None, args)` (vosk_tts/synth.py:123-126), i.e. the trace
 // of SynthesizerTrn.infer (training/vits2/models.py:1679-1704).  The launch sequence below follows that
-// function stage by stage; every kernel is in kernels.cuh (fp32 FFMA) or conv_tc.cuh (tcgen05).
+// function stage by stage; every kernel is in kernels.cuh (fp32 FFMA) or conv_tc.cuh (wgmma).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -26,7 +26,6 @@
 #include "conv_tc.cuh"
 #include "mas.cuh"
 #include "attn_tc.cuh"
-#include "wn_tc.cuh"
 
 using namespace vtts;
 
@@ -79,7 +78,7 @@ struct EncLayerW {
   const float* relk = nullptr;
   const float* relv = nullptr;
   int heads = 1;
-  // split-bf16 [16][128] tiles of the relative-position tables for the tcgen05 attention (null: FFMA attention only)
+  // split-bf16 [16][128] tiles of the relative-position tables for the wgmma attention (null: FFMA attention only)
   const __nv_bfloat16 *rk_hi = nullptr, *rk_lo = nullptr, *rv_hi = nullptr, *rv_lo = nullptr;
 };
 struct DdsW {
@@ -168,9 +167,9 @@ struct vtts_engine {
   std::vector<UpW> ups;
   std::vector<RbW> rbs;
   int hop = 0, up_total = 1;
-  bool tc = false;                      // precision mode 1: tcgen05 path for the decoder convs
+  bool tc = false;                      // precision mode 1: wgmma path for the decoder convs
   TcW tc_pre, tc_post, tc_encproj;
-  bool enc_on_tc = false;               // precision modes 2 / 3: the text encoder's convs on tcgen05 as well
+  bool enc_on_tc = false;               // precision modes 2 / 3: the text encoder's convs on wgmma as well
   bool enc_three = false;               // mode 3: with the exact 3-way operand split
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -306,12 +305,12 @@ struct vtts_engine {
   uint64_t ws_gen = 0, graph_clock = 0, graph_replays = 0;
   bool capture_on_first = true;
   bool capturing = false, use_graphs = true, last_graphed = false, use_pdl = true;    // programmatic dependent launch (VTTS_PDL=0 turns it off)
-  int conv_max_s = 8, conv_target = 120, conv_max_g = 4, conv_big_g = 1, tc_tall = 0, tc_baseoff = 0, tc_bn = 0, attn_rows = 0, tc_mc = 0, tc_split = 0, conv_min_g = 1, tc_min_steps = 2, conv_auto_g = 4, attn_split = 1, tc_persist = 1, tc_persist_min = 1, n_sm = 148, tc_coal = 0, tc_dbgskip = 0, tc_wmc = 0;
+  int conv_max_s = 8, conv_target = 120, conv_max_g = 4, conv_big_g = 1, tc_tall = 0, tc_baseoff = 0, tc_bn = 0, attn_rows = 0, tc_mc = 0, tc_split = 0, conv_min_g = 1, tc_min_steps = 2, conv_auto_g = 4, attn_split = 1, tc_persist = 1, tc_persist_min = 1, n_sm = 132, tc_dbgskip = 0, tc_wmc = 0;
   int tc_cluster_cap[2][3] = {{0, 0, 0}, {0, 0, 0}};   // co-resident clusters of 2/4/8 conv_tc CTAs, [BN 64/128][log2(S)-1]   // multicast measured slower (see DESIGN.md 4.2)   // tuning knobs (env VTTS_CONV_MAXS / _TARGET / _MAXG)
   cudaEvent_t ev[8] = {};
   cudaStream_t side[3] = {};               // branch streams of the decoder's independent resblock chains (forked / joined with events)
   cudaEvent_t ev_fork = nullptr, ev_join[3] = {};
-  int attn_tc_mode = 1;                    // tcgen05 attention where the qkv conv runs on tensor cores: 0 never, 1 when throughput bound, 2 always
+  int attn_tc_mode = 1;                    // wgmma attention where the qkv conv runs on tensor cores: 0 never, 1 when throughput bound, 2 always
   int mrf_heavy_first = 1;
   int mrf_branch = 0;                      // VTTS_MRF_BRANCH=1: one stream per resblock chain (measured slower: 1.74 vs 1.62 ms)
   float stage_ms[8] = {};
@@ -434,7 +433,7 @@ struct vtts_engine {
   std::vector<std::string> looked_up;          // tensors the engine bound, in first-use order
   Buf<PrefRange> d_pref;                       // L2 prefetch list for this precision mode
   int n_pref = 0, n_pref_phase1 = 0;
-  bool use_prefetch = false;                   // measured: no gain on B200 (weights are not the latency bottleneck)
+  bool use_prefetch = false;                   // measured: no gain (weights are not the latency bottleneck)
   void build_prefetch_list();
   const float* vec(const std::string& name, size_t n) {
     Tensor t = tensor(name);
@@ -445,7 +444,7 @@ struct vtts_engine {
     }
     return t.p;
   }
-  // need_w = false: the conv runs on tcgen05 from its split-bf16 copy in this precision mode; the fp32 copy is bound only if
+  // need_w = false: the conv runs on wgmma from its split-bf16 copy in this precision mode; the fp32 copy is bound only if
   // the blob happens to carry it (weights.pack(precision=...) leaves it out of the one-time weight broadcast)
   ConvW conv(const std::string& name, int Cin, int Cout, int k, bool need_w = true) {
     ConvW c;
@@ -529,19 +528,7 @@ struct vtts_engine {
   void launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
   // plane buffers of the frame-resolution stages: allocated (and their tails zeroed by ONE zero_tails launch) before the
   // first kernel of the phase
-  struct FlowPl { Planes ph, pao, ph1, pff, pwx, pwx2, pacts, pskip, pqkv; } flp;
-  // One cluster kernel per WN layer (wn_tc.cuh).  Correct (all goldens), but measured SLOWER than the two launches it
-  // replaces: 36 vs 22 us per layer at batch 1 (1.94 vs 1.69 ms per utterance) -- without split-K the 15 k-steps of the gated
-  // conv run serially in each CTA (8.7 us), the gate for 48 channels per thread costs 4.3 us, the DSMEM all-gather of the
-  // 96 KB acts tile 4.1 us plus two cluster barriers, and the second epilogue 10.8 us (profiles/r2_timeline_wn_fused_nopdl.txt).
-  // Kept behind VTTS_WN_FUSED=1.
-  int wn_fused = 0;
-  bool wn_fused_ok() const {
-    const int H = cfg.hidden_channels;
-    return wn_fused && (H == 64 || H == 128 || H == 192) && cfg.flow_kernel_size % 2 == 1;
-  }
-  void launch_wn_fused(const FlowW& W, int f, int i, const Planes& xin, const Planes& xout, float* x, float* skip, const Planes& pskip,
-                       int dil, const int* fl, const int* fo);
+  struct FlowPl { Planes ph, pao, ph1, pff, pwx, pacts, pskip, pqkv; } flp;
   struct DecPl { Planes pz, cur; std::vector<Planes> px, nxt; std::vector<std::vector<Planes>> pj, pt; } dcp;
   void alloc_flow_planes();
   void alloc_decoder_planes();
@@ -588,7 +575,7 @@ ConvP mk(const ConvW& W, const float* x, int ldx, int xoff, float* y, int ldy, i
 }  // namespace
 
 // Which bound tensors does a call actually read in this precision mode?  (fp32 `.w` copies of convs that run on
-// tcgen05 are skipped, and so are the bf16 `.th/.tl` copies of convs that stay on the FFMA pipe.)
+// wgmma are skipped, and so are the bf16 `.th/.tl` copies of convs that stay on the FFMA pipe.)
 void vtts_engine::build_prefetch_list() {
   auto on_tc = [&](const std::string& nm) {
     if (nm.rfind("enc.", 0) == 0) return cfg.precision >= 2;
@@ -679,7 +666,7 @@ void vtts_engine::bind_weights() {
   for (int f = 0; f < nf; ++f) {
     FlowW F;
     const std::string p = "flow." + std::to_string(f);
-    const bool fw = !(c.precision >= 1 && H % TC_BK == 0);       // fp32 copies needed? (no: the whole flow but its pre conv is on tcgen05)
+    const bool fw = !(c.precision >= 1 && H % TC_BK == 0);       // fp32 copies needed? (no: the whole flow but its pre conv is on wgmma)
     F.pre = conv(p + ".pre", I / 2, H, 1);
     if (c.use_transformer_flows) F.tr = enc_layer(p + ".tr", H, H, c.flow_kernel_size, fheads, fw);
     for (int i = 0; i < nl; ++i) {
@@ -789,7 +776,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
       if (q.Cout < 128) wide = false;
       for (int b = 0; b < nB; ++b) ctas128 += (long)((hl[b] * rmul + q.in_extra + TC_BM - 1) / TC_BM) * ((q.Cout + 127) / 128);
     }
-    if (wide && ctas128 >= 2 * 148) BN = 128;
+    if (wide && ctas128 >= 2 * n_sm) BN = 128;
     if (tc_bn == 64 || tc_bn == 128) BN = tc_bn;
   }
   REQUIRE(!ps.empty() && (int)ps.size() <= TC_MAXP, VTTS_ERR_INVALID, "bad grouped tensor-core conv");
@@ -816,8 +803,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   if (np3) tall = false;
   if (tall) {
     const int ab = (maxNR * 128 + 1023) / 1024 * 1024;
-    const int need = BN == 128 ? tc_smem_bytes<128>(ab, 2, 2, tc_coal ? 3 : tc_wst<128>(), tc_coal ? TC_STAGE_BYTES : 0)
-                               : tc_smem_bytes<64>(ab, 2, 2, tc_wst<64>(), tc_coal ? TC_STAGE_BYTES : 0);
+    const int need = BN == 128 ? tc_smem_bytes<128>(ab, 2, 2, tc_wst<128>()) : tc_smem_bytes<64>(ab, 2, 2, tc_wst<64>());
     if (need > 227 * 1024) tall = false;
   }
   if (!tall) maxNR = TC_BM;
@@ -874,18 +860,14 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   if (np == 3) { tall = false; cn = 1; }
   tb.np = np;
   tb.ast = (np == 3 || tall) ? 2 : (BN == 128 ? tc_ast<128>() : tc_ast<64>());
-  // launches without split-K finish their tiles through a 32 KB transposition buffer (coalesced epilogue, conv_tc.cuh); with
-  // 128-wide channel tiles it takes the place of the fourth weight stage
   long tiles_all = 0;                        // the launch's tile space (one wave or less: the one-tile-per-CTA kernel)
   {
     int mc = 0, ml = 0;
     for (const TcSpec& q : ps) { mc = std::max(mc, q.Cout); ml = std::max(ml, maxLen * rmul + q.in_extra); }
     tiles_all = (long)((ml + TC_BM - 1) / TC_BM) * ((mc + BN - 1) / BN) * nB * (long)ps.size() * split;
   }
-  const bool one_wave = tiles_all <= 148 && !(tc_persist == 2 && split == 1 && cn == 1);
-  tb.coal = (split == 1 && !one_wave && tc_coal) ? 1 : 0;
-  const int stage_bytes = tb.coal ? TC_STAGE_BYTES : 0;
-  tb.wst = np == 3 ? (BN == 128 ? 2 : 3) : (BN == 128 ? (tb.coal ? 3 : tc_wst<128>()) : tc_wst<64>());
+  const bool one_wave = tiles_all <= n_sm && !(tc_persist == 2 && split == 1 && cn == 1);
+  tb.wst = np == 3 ? (BN == 128 ? 2 : 3) : (BN == 128 ? tc_wst<128>() : tc_wst<64>());
   tb.split = split;
   tb.cn = cn;
   tb.tall = tall ? 1 : 0;
@@ -951,7 +933,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     cudaLaunchConfig_t lc;
     memset(&lc, 0, sizeof(lc));
     lc.gridDim = grid; lc.blockDim = dim3(TC_THREADS); lc.stream = stream;
-    lc.dynamicSmemBytes = BN == 128 ? tc_smem_bytes<128>(tb.a_bytes, tb.np, tb.ast, tb.wst, stage_bytes) : tc_smem_bytes<64>(tb.a_bytes, tb.np, tb.ast, tb.wst, stage_bytes);
+    lc.dynamicSmemBytes = BN == 128 ? tc_smem_bytes<128>(tb.a_bytes, tb.np, tb.ast, tb.wst) : tc_smem_bytes<64>(tb.a_bytes, tb.np, tb.ast, tb.wst);
     REQUIRE(lc.dynamicSmemBytes <= 227 * 1024, VTTS_ERR_INVALID, "tensor-core conv: shared-memory budget exceeded");
     cudaLaunchAttribute at[2];
     int na = 0;
@@ -971,14 +953,14 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     if (split > 1 || tb.wpre) {
       const bool dyn = tb.np != 2 || tb.ast != (BN == 128 ? tc_ast<128>() : tc_ast<64>()) || tb.wst != (BN == 128 ? tc_wst<128>() : tc_wst<64>());
       if (dyn) {
-        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, true, true>, tb, lens, offs));
-        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, true, true>, tb, lens, offs));
+        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, true>, tb, lens, offs));
+        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, true>, tb, lens, offs));
       } else {                    // the default launches carry the descriptor without the third-plane tensor maps
         // (a one-slot descriptor for the single-conv launches was tried as well: alternating between two kernel images on the
         //  chain cost more than the 2 KB of parameters saved -- conv_tc 723 -> 765 us in-graph)
         const auto tl = tc_lite<TC_MAXP>(tb);
-        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, true, false, TC_MAXP>, tl, lens, offs));
-        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, true, false, TC_MAXP>, tl, lens, offs));
+        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, false, TC_MAXP>, tl, lens, offs));
+        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, false, TC_MAXP>, tl, lens, offs));
       }
     } else {                      // more than one wave of tiles: the persistent kernel (also runs them one per CTA when tb.persist == 0)
       if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_persist_kernel<128>, tb, lens, offs));
@@ -1000,7 +982,7 @@ bool vtts_engine::attn_tc_ok(const EncLayerW& L, int Hc) const {
 }
 // Which attention kernel for this launch?  The tensor-core kernel wins as soon as the launch is throughput bound (batches,
 // long utterances: 8.8x at 4765 frames, 2.8x on the flow of a 64-utterance batch).  A single short utterance is latency
-// bound -- a 128-row tcgen05 tile walks its 2-4 key tiles serially while the split-KV FFMA kernel spreads 4 query rows x 4
+// bound -- a 128-row wgmma tile walks its 2-4 key tiles serially while the split-KV FFMA kernel spreads 4 query rows x 4
 // key segments over 16 warps of ~80 CTAs -- and keeps the FFMA kernel (measured at 162 frames: 6 vs 19 us per launch in the
 // graph).  VTTS_ATTN_TC = 0 never / 1 this rule / 2 always.
 bool vtts_engine::attn_use_tc(const EncLayerW& L, int Hc, const int* lens, int maxLen) const {
@@ -1010,7 +992,7 @@ bool vtts_engine::attn_use_tc(const EncLayerW& L, int Hc, const int* lens, int m
   long ctas = 0;
   for (int b = 0; b < B; ++b) ctas += (long)((hl[b] + ATS_ROWS - 1) / ATS_ROWS) * L.heads;
   const int mt = (maxLen + AT_KT - 1) / AT_KT;
-  const bool split_kv_fits = attn_split && (attn_rows == 0 || attn_rows == 1) && mt <= ATS_MAXT && ctas <= 148;
+  const bool split_kv_fits = attn_split && (attn_rows == 0 || attn_rows == 1) && mt <= ATS_MAXT && ctas <= n_sm;
   return !split_kv_fits;
 }
 
@@ -1053,13 +1035,13 @@ void vtts_engine::launch_attn(const float* qkv, float* ao, const EncLayerW& L, i
   const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
   long rows = 0;
   for (int b = 0; b < B; ++b) rows += hl[b];
-  const int R = (attn_rows == 1 || attn_rows == 4) ? attn_rows : (rows * n_heads >= 8L * 2 * 148 * 4 ? 4 : 1);
+  const int R = (attn_rows == 1 || attn_rows == 4) ? attn_rows : (rows * n_heads >= 8L * 2 * n_sm * 4 ? 4 : 1);
   // single short utterances: split-KV variant (all K/V tiles resident, 4 warps per query row) when it fits one wave
   {
     long ctas = 0;
     for (int b = 0; b < B; ++b) ctas += (long)((hl[b] + ATS_ROWS - 1) / ATS_ROWS) * n_heads;
     const int mt = (maxLen + AT_KT - 1) / AT_KT;
-    if (attn_split && R == 1 && mt <= ATS_MAXT && ctas <= 148 && dk % 32 == 0 && dk <= 128) {
+    if (attn_split && R == 1 && mt <= ATS_MAXT && ctas <= n_sm && dk % 32 == 0 && dk <= 128) {
       dim3 grid((maxLen + ATS_ROWS - 1) / ATS_ROWS, n_heads, B);
       const size_t smem = (size_t)attn_split_smem_floats(dk, nrel, mt) * sizeof(float);
 #define ATTN_SPLIT(D) klaunch(attn_split_kernel<D>, grid, dim3(ATS_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, mt, lens, offs, ph, plo, pmi)
@@ -1095,67 +1077,8 @@ void vtts_engine::alloc_flow_planes() {
   flp.pff = planes(slot++, F, 1, H); flp.pwx = planes(slot++, F, 1, H); flp.pacts = planes(slot++, F, 1, H);
   flp.pskip = planes(slot++, F, 1, H);
   flp.pqkv = planes(slot++, F, 1, 3 * H);
-  flp.pwx2 = planes(slot++, F, 1, H);
 }
 
-// One WaveNet layer as a single cluster kernel (wn_tc.cuh): reads the planes `xin`, writes the updated hidden state to
-// x (fp32, in place) and to the OTHER plane set `xout` (neighbouring row tiles still read `xin` for their conv halos).
-void vtts_engine::launch_wn_fused(const FlowW& W, int f, int i, const Planes& xin, const Planes& xout, float* x, float* skip,
-                                  const Planes& pskip, int dil, const int* fl, const int* fo) {
-  const vtts_config& c = cfg;
-  const int H = c.hidden_channels, nl = c.flow_wn_layers, fk = c.flow_kernel_size;
-  const bool last = (i == nl - 1);
-  const int BN1 = 2 * H / WN_NCL, BN2 = (last ? H : 2 * H) / WN_NCL;
-  WnParams wp;
-  memset(&wp, 0, sizeof(wp));
-  wp.a_hi = make_map(xin.hi, H, xin.rows, 128);
-  wp.a_lo = make_map(xin.lo, H, xin.rows, 128);
-  wp.win_hi = make_map(W.t_in[i].hi, H, (long)fk * 2 * H, BN1);
-  wp.win_lo = make_map(W.t_in[i].lo, H, (long)fk * 2 * H, BN1);
-  if (!last) {
-    wp.wrx_hi = make_map(W.t_rsx[i].hi, H, H, BN2);
-    wp.wrx_lo = make_map(W.t_rsx[i].lo, H, H, BN2);
-    wp.bias_rx = W.rsx[i].b;
-  }
-  wp.wrs_hi = make_map(W.t_rss[i].hi, H, H, BN2);
-  wp.wrs_lo = make_map(W.t_rss[i].lo, H, H, BN2);
-  wp.bias_rs = W.rss[i].b;
-  wp.bias_in = W.in[i].b;
-  if (has_g) { wp.cond = d_condv.p + r_flow + (f * nl + i) * 2 * H; wp.cond_ld = condR; }
-  wp.x = x; wp.xp_hi = xout.hi; wp.xp_lo = xout.lo;
-  wp.skip = skip;
-  if (last) { wp.sp_hi = pskip.hi; wp.sp_lo = pskip.lo; }
-  wp.k = fk; wp.dil = dil; wp.pad = dil * (fk - 1) / 2;
-  wp.first = (i == 0) ? 1 : 0;
-  dim3 grid((maxFrm + 127) / 128, WN_NCL, B);
-  cudaLaunchConfig_t lc;
-  memset(&lc, 0, sizeof(lc));
-  lc.gridDim = grid; lc.blockDim = dim3(WN_THREADS); lc.stream = stream;
-  cudaLaunchAttribute at[2];
-  int na = 0;
-  at[na].id = cudaLaunchAttributeClusterDimension;
-  at[na].val.clusterDim.x = 1; at[na].val.clusterDim.y = WN_NCL; at[na].val.clusterDim.z = 1;
-  ++na;
-  if (use_pdl) {
-    at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  lc.attrs = at; lc.numAttrs = na;
-#define WN_LAUNCH(HH)                                                                                                   \
-  do {                                                                                                                  \
-    lc.dynamicSmemBytes = wn_smem_bytes<HH>();                                                                          \
-    if (last) CK(cudaLaunchKernelEx(&lc, wn_layer_tc_kernel<HH, true>, wp, fl, fo));                                    \
-    else CK(cudaLaunchKernelEx(&lc, wn_layer_tc_kernel<HH, false>, wp, fl, fo));                                        \
-  } while (0)
-  if (H == 192) WN_LAUNCH(192); else if (H == 128) WN_LAUNCH(128); else WN_LAUNCH(64);
-#undef WN_LAUNCH
-  CK(cudaGetLastError());
-  if (profiling) {   // counted with the tcgen05 conv family (algorithmic FLOPs of both GEMMs)
-    for (int b = 0; b < B; ++b) tc_prof_flops += 2.0 * h_frm_len[b] * ((double)2 * H * H * fk + (double)(last ? H : 2 * H) * H);
-  }
-  ++launches;
-}
 void vtts_engine::alloc_decoder_planes() {
   const vtts_config& c = cfg;
   const long F = Tfrm;
@@ -1190,7 +1113,6 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz) 
   float* fqkv = ensure(d_fqkv, (size_t)F * 3 * H);
   float* fao = ensure(d_fao, (size_t)F * H);
   Planes ph = flp.ph, pao = flp.pao, ph1 = flp.ph1, pff = flp.pff, pwx = flp.pwx, pacts = flp.pacts, pskip = flp.pskip, pqkv = flp.pqkv;
-  const bool fused = wn_fused_ok();
   dim3 lg((maxFrm + 3) / 4, B);
   for (int f = nf - 1; f >= 0; --f) {
     const FlowW& W = flow[f];
@@ -1205,7 +1127,7 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz) 
     float* wn_x = h;
     if (c.use_transformer_flows) {
       if (attn_use_tc(W.tr, H, fl, maxFrm)) {
-        // q, k, v leave the qkv conv as split-bf16 planes only; attention runs on tcgen05 (attn_tc.cuh)
+        // q, k, v leave the qkv conv as split-bf16 planes only; attention runs on wgmma (attn_tc.cuh)
         { TcSpec q; q.in = ph; q.w = W.t_qkv; q.bias = W.tr.qkv.b; q.Cin = H; q.Cout = 3 * H; q.out = pqkv; q.pl_slope = 1.f;
           launch_tc({q}, 1, fl, fo, maxFrm, B); }
         launch_attn_tc(pqkv, nullptr, &pao, W.tr, H, fl, fo, maxFrm);
@@ -1231,12 +1153,7 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz) 
       wn_x = wx;
     }
     int dil = 1;
-    for (int i = 0; i < nl && fused; ++i) {
-      // layer i reads the hidden state's planes from one buffer and writes the updated ones to the other
-      launch_wn_fused(W, f, i, (i % 2 == 0) ? pwx : flp.pwx2, (i % 2 == 0) ? flp.pwx2 : pwx, wn_x, skip, pskip, dil, fl, fo);
-      dil *= c.flow_dilation_rate;
-    }
-    for (int i = 0; i < nl && !fused; ++i) {
+    for (int i = 0; i < nl; ++i) {
       { TcSpec q; q.in = pwx; q.w = W.t_in[i]; q.bias = W.in[i].b; q.Cin = H; q.Cout = 2 * H; q.k = fk; q.dil = dil;
         q.pad = dil * (fk - 1) / 2; q.epi = TCE_GATE; q.out = pacts; q.pl_slope = 1.f;
         if (has_g) { q.cond = d_condv.p + r_flow + (f * nl + i) * 2 * H; q.cond_ld = condR; }
@@ -1333,7 +1250,7 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     // contend and the step gets slower (1.74 vs 1.62 ms).
     long group_tiles = 0;
     for (int b = 0; b < B; ++b) group_tiles += (long)nk * ((v_frm_len[b] * rm + TC_BM - 1) / TC_BM) * ((ch + 63) / 64);
-    const bool branch = mrf_branch && !profiling && nk > 1 && nk - 1 <= 3 && group_tiles <= 148;
+    const bool branch = mrf_branch && !profiling && nk > 1 && nk - 1 <= 3 && group_tiles <= n_sm;
     if (branch) {
       struct Restore { cudaStream_t& s; cudaStream_t v; ~Restore() { s = v; } } restore{stream, stream};
       cudaStream_t main_stream = stream;
@@ -1420,7 +1337,7 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
   // with 2 / 4 groups), no cluster.  Few tiles (batch 1): the k-steps of a tile are
   // spread over a cluster of S CTAs until the launch fills ~1 wave of SMs; ranks that still have long k-loops then get
   // 2-4 thread groups each (a lone warp per scheduler issues an FFMA only every other cycle).
-  int G = base0 >= 2 * 148 ? conv_big_g : conv_min_g;
+  int G = base0 >= 2 * n_sm ? conv_big_g : conv_min_g;
   for (const ConvP& q : ps)
     while (G > 1 && q.Cin % (CV_CK * G) != 0) G >>= 1;
   auto min_steps = [&](int g) {
@@ -1435,7 +1352,7 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
     const size_t pipe = (size_t)2 * CV_CK * g * xw + (size_t)CV_NS * CV_CK * g * CV_TC;
     return (std::max(pipe, (size_t)(g - 1) * 32 * CV_THREADS) + 3) / 4 * 4 + (size_t)32 * CV_THREADS;
   };
-  if (conv_auto_g && base0 < 2 * 148)
+  if (conv_auto_g && base0 < 2 * n_sm)
     while (G * 2 <= conv_max_g && min_steps(G * 2) / S >= conv_auto_g && smem_floats(G * 2) * sizeof(float) <= (size_t)CONV_SMEM_MAX) G *= 2;
   REQUIRE(smem_floats(G) * sizeof(float) <= (size_t)CONV_SMEM_MAX, VTTS_ERR_INVALID, "conv tile does not fit in shared memory");
   cb.S = S;
@@ -1629,7 +1546,7 @@ void vtts_engine::phase1(const int* ids_packed_host, const int64_t* d_ids64, int
       encoder_layer(enc[i], x, xb, qkv, ao, y, ffh, H, Fc, c.kernel_size, tl, to, maxTok, va, condR, nullptr);
       continue;
     }
-    // precision mode 2: same layer with the four convs on tcgen05 (attentions.py:57-63)
+    // precision mode 2: same layer with the four convs on wgmma (attentions.py:57-63)
     const EncLayerW& L = enc[i];
     const int ks = c.kernel_size;
     dim3 lg((maxTok + 3) / 4, B);
@@ -2349,10 +2266,10 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
       h->encode_tiled = reinterpret_cast<vtts_engine::EncodeFn>(fn);
       CK(cudaFuncSetAttribute(conv_tc_persist_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       CK(cudaFuncSetAttribute(conv_tc_persist_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      CK(cudaFuncSetAttribute(conv_tc_kernel<64, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      CK(cudaFuncSetAttribute(conv_tc_kernel<128, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      CK(cudaFuncSetAttribute(conv_tc_kernel<64, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      CK(cudaFuncSetAttribute(conv_tc_kernel<128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      CK(cudaFuncSetAttribute(conv_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      CK(cudaFuncSetAttribute(conv_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      CK(cudaFuncSetAttribute(conv_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      CK(cudaFuncSetAttribute(conv_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       for (int wi = 0; wi < 2; ++wi)
         for (int si = 0; si < 3; ++si) {
           const int S = 2 << si;
@@ -2365,7 +2282,7 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
           at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = S;
           lc.attrs = at; lc.numAttrs = 1;
           int nc = 0;
-          cudaError_t e = wi ? cudaOccupancyMaxActiveClusters(&nc, conv_tc_kernel<128, true, false>, &lc) : cudaOccupancyMaxActiveClusters(&nc, conv_tc_kernel<64, true, false>, &lc);
+          cudaError_t e = wi ? cudaOccupancyMaxActiveClusters(&nc, conv_tc_kernel<128, false>, &lc) : cudaOccupancyMaxActiveClusters(&nc, conv_tc_kernel<64, false>, &lc);
           if (e != cudaSuccess) { nc = 0; cudaGetLastError(); }
           h->tc_cluster_cap[wi][si] = nc;
         }
@@ -2402,11 +2319,9 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     if (const char* e = getenv("VTTS_TC_PERSIST")) h->tc_persist = atoi(e);                 // 0: one tile per CTA also on machine-filling launches; 2: persistent grid on every launch without split-K (tests)
     if (const char* e = getenv("VTTS_TC_DBGSKIP")) h->tc_dbgskip = atoi(e);                 // timing experiments only (wrong results)
     if (const char* e = getenv("VTTS_TC_WMC")) h->tc_wmc = atoi(e);                         // 1: weight-tile multicast between CTA pairs of persistent launches (measured neutral, off)
-    if (const char* e = getenv("VTTS_TC_COAL")) h->tc_coal = atoi(e);                       // 1: coalesced (transposed) epilogue on launches without split-K
     if (const char* e = getenv("VTTS_TC_PERSIST_MIN")) h->tc_persist_min = std::max(1, atoi(e));   // tiles per SM from which the persistent grid is used
     if (const char* e = getenv("VTTS_MRF_BRANCH")) h->mrf_branch = atoi(e);
     if (const char* e = getenv("VTTS_MRF_HEAVY_FIRST")) h->mrf_heavy_first = atoi(e);
-    if (const char* e = getenv("VTTS_WN_FUSED")) h->wn_fused = atoi(e);
     if (const char* e = getenv("VTTS_ATTN_SPLIT")) h->attn_split = atoi(e);       // 0: never use the split-KV attention
     if (const char* e = getenv("VTTS_CONV_AUTOG")) h->conv_auto_g = std::max(0, atoi(e));   // k-steps per rank needed to add thread groups; 0 = never
     if (const char* e = getenv("VTTS_CONV_MING")) h->conv_min_g = std::max(1, std::min(4, atoi(e)));      // 0 auto, 1 off, 2/4/8 cap
@@ -2424,12 +2339,6 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     h->build_prefetch_list();
     CK(cudaMemsetAsync(h->ensure(h->d_done_ctr, 4), 0, 4 * sizeof(int), h->stream));     // ticket counter of duration_kernel (self-resetting)
     CK(cudaFuncSetAttribute(dds_layer_kernel<DDS_TT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    CK(cudaFuncSetAttribute(wn_layer_tc_kernel<192, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wn_smem_bytes<192>()));
-    CK(cudaFuncSetAttribute(wn_layer_tc_kernel<192, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wn_smem_bytes<192>()));
-    CK(cudaFuncSetAttribute(wn_layer_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wn_smem_bytes<128>()));
-    CK(cudaFuncSetAttribute(wn_layer_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wn_smem_bytes<128>()));
-    CK(cudaFuncSetAttribute(wn_layer_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wn_smem_bytes<64>()));
-    CK(cudaFuncSetAttribute(wn_layer_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wn_smem_bytes<64>()));
     CK(cudaFuncSetAttribute(attn_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc_smem_bytes(32)));
     CK(cudaFuncSetAttribute(attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc_smem_bytes(64)));
     CK(cudaFuncSetAttribute(attn_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc_smem_bytes(96)));
@@ -2839,7 +2748,7 @@ int vtts_profile_read_tc(vtts_handle h, double* ms, uint64_t* launches, double* 
 }
 
 // Micro-benchmark of one conv kernel in isolation (back-to-back launches, CUDA events on the engine stream):
-//   what = "tc:<Cin>:<Cout>:<k>:<dil>:<rows>"   tcgen05 kernel (precision mode 1 engines only)
+//   what = "tc:<Cin>:<Cout>:<k>:<dil>:<rows>"   wgmma kernel (precision mode 1 engines only)
 //          "ffma:<Cin>:<Cout>:<k>:<dil>:<rows>" fp32 FFMA kernel
 // Returns the average milliseconds per launch, or a negative status.  Used by bench.py for the roofline of the
 // dominant kernel timed alone, and by tools/ for tuning.

@@ -1,4 +1,4 @@
-// kernels.cuh -- hand-written sm_100a kernels of the VITS2 inference path (fp32 FFMA family).
+// kernels.cuh -- hand-written sm_90a kernels of the VITS2 inference path (fp32 FFMA family).
 //
 // Activation layout: channels-last, packed utterances.  A tensor that the reference holds as
 // [B, C, T] (training/vits2/models.py) lives here as rows[off[b] + t][C]; `len[b]`/`off[b]` are
@@ -15,7 +15,7 @@
 namespace vtts {
 
 // Programmatic dependent launch (PDL): every kernel of the engine is launched with programmatic stream serialisation,
-// so kernel N+1 may start (and run its prologue: barrier init, TMEM allocation, weight prefetch) while kernel N drains.
+// so kernel N+1 may start (and run its prologue: barrier init, weight prefetch) while kernel N drains.
 // PDL_WAIT() blocks until the predecessor grid has completed and its writes are visible; nothing that a predecessor
 // produces (activations, lens/offs) may be touched, and nothing may be written, before it.  Both are no-ops when the
 // kernel was launched without the attribute.
@@ -47,7 +47,7 @@ __device__ __forceinline__ void timeline_stamp_t(int line) {
 #define PDL_LAUNCH() timeline_stamp(__LINE__)
 #define PDL_WAIT() asm volatile("griddepcontrol.wait;\n\tgriddepcontrol.launch_dependents;" ::: "memory")
 
-// ---- mbarrier / bulk-async-copy wrappers (shared by the tcgen05 conv and the DDS kernel)
+// ---- mbarrier / bulk-async-copy wrappers (shared by the tensor-core conv and the DDS kernel)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -189,7 +189,7 @@ __device__ __forceinline__ float ld_dsmem(const float* local_smem_ptr, int rank)
 //  * S CTAs of a thread-block cluster split the k-steps (s = rank, rank+S, ...) and reduce their partial
 //    tiles through distributed shared memory in a fixed order (deterministic), each CTA finishing 1/S of
 //    the tile.  At batch 1 a conv has only a handful of output tiles; the cluster dimension is what lets
-//    it spread over the 148 SMs.
+//    it spread over the SMs.
 //  * inside a group each thread accumulates 4 rows (tx + 16m) x 8 channels (shared-memory operand delivery is
 //    128 B/clk/SM of *delivered* data, so wider register tiles than the 2x16 variant tried first are needed).
 // Weight tiles run through an NS-deep cp.async ring (one __syncthreads per step); the input tile of the

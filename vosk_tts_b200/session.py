@@ -23,7 +23,7 @@ class VitsSession:
         reserve: optional (max_tokens, max_frames[, batch]) -- size the workspace for such requests now (Engine.reserve)."""
         self.cfg = cfg or _config.DEFAULT_CONFIG
         if precision > 0 and not _weights.tc_supported(self.cfg):
-            logging.warning("model widths are not multiples of 64: the tcgen05 conv path is unavailable, using the fp32 kernels")
+            logging.warning("model widths are not multiples of 64: the tensor-core conv path is unavailable, using the fp32 kernels")
             precision = 0
         if packed is None:
             folded = _weights.fold_weight_norm(state_dict)

@@ -110,7 +110,7 @@ class _Packer:
         self.pos += a.size
 
     def conv(self, name, w, b=None, co_perm=None, ci_perm=None, need_w=True):
-        """w: [Co, Ci, k] (Conv1d layout).  need_w=False: only the bias is packed (the conv runs on tcgen05 from its .th/.tl copy)."""
+        """w: [Co, Ci, k] (Conv1d layout).  need_w=False: only the bias is packed (the conv runs on tensor-core from its .th/.tl copy)."""
         w = np.asarray(w, np.float32)
         if co_perm is not None:
             w = w[co_perm]
@@ -129,7 +129,7 @@ class _Packer:
         self.add(name + ".b", bp)
 
     def conv_tc(self, name, w, co_perm=None, ci_perm=None):
-        """Split-bf16 copy of a conv weight for the tcgen05 path: <name>.th / <name>.tl = [k][Cout][Cin] bf16
+        """Split-bf16 copy of a conv weight for the tensor-core path: <name>.th / <name>.tl = [k][Cout][Cin] bf16
         (K-major rows for TMA), hi = rne_bf16(w), lo = rne_bf16(w - hi); two bf16 per fp32 blob slot."""
         w = np.asarray(w, np.float32)
         if co_perm is not None:
@@ -181,7 +181,7 @@ def convt_phases(u, K):
 
 
 def tc_supported(cfg):
-    """The tcgen05 conv path packs 64-channel K chunks: every conv it takes over must have Cin % 64 == 0."""
+    """The tensor-core conv path packs 64-channel K chunks: every conv it takes over must have Cin % 64 == 0."""
     n_ups = len(cfg["upsample_rates"])
     return (cfg["decoder"] in ("mb_istft", "ms_istft", "istft") and str(cfg["resblock"]) == "1" and cfg["hidden_channels"] % 64 == 0 and
             cfg["filter_channels"] % 64 == 0 and cfg["inter_channels"] % 64 == 0 and
@@ -190,14 +190,14 @@ def tc_supported(cfg):
 
 def pack(w, cfg, tc=True, precision=None):
     """w: folded state dict (reference names); returns (blob float32[n], manifest str).
-    tc=True also packs split-bf16 copies of the convs for the tcgen05 path (precision modes 1 / 2).
+    tc=True also packs split-bf16 copies of the convs for the tensor-core path (precision modes 1 / 2).
     precision: None packs everything (a blob any engine mode can be created from); 0 / 1 / 2 leave out the tensors that
     mode never reads (mode 0: no split-bf16 copies at all; mode 1: none for the text encoder) -- what travels in the
     one-time NCCL weight broadcast of a multi-GPU job."""
     tc = tc and tc_supported(cfg) and precision != 0
     enc_tc = tc and precision in (None, 2)
     enc_tc3 = tc and precision in (None, 3)    # exact 3-way split copies of the text encoder's convs (mode 3)
-    fw = not (tc and precision in (1, 2, 3))   # fp32 copies of the flow / decoder convs (the tcgen05 modes read only .th/.tl + bias)
+    fw = not (tc and precision in (1, 2, 3))   # fp32 copies of the flow / decoder convs (the tensor-core modes read only .th/.tl + bias)
     ew = not (tc and precision in (2, 3))      # ... of the text encoder's convs
     g = lambda k: w[k].detach().cpu().numpy() if hasattr(w[k], "detach") else np.asarray(w[k])
     H, I, G = cfg["hidden_channels"], cfg["inter_channels"], cfg["gin_channels"]
@@ -229,7 +229,7 @@ def pack(w, cfg, tc=True, precision=None):
         P.add(dst + ".relk", g(a + ".emb_rel_k")[0])
         P.add(dst + ".relv", g(a + ".emb_rel_v")[0])
         if with_tc:
-            # the same tables as split-bf16 [16 offsets][128 channels] tiles (zero padded) for the tcgen05 attention:
+            # the same tables as split-bf16 [16 offsets][128 channels] tiles (zero padded) for the tensor-core attention:
             # Ek is a K-major B operand of Q Ek^T, Ev an MN-major B operand of P_band Ev (csrc/attn_tc.cuh)
             for nm, src_t in ((".rk", g(a + ".emb_rel_k")[0]), (".rv", g(a + ".emb_rel_v")[0])):
                 nrel, dk = src_t.shape
