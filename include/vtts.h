@@ -63,6 +63,12 @@ typedef struct vtts_config {
   int32_t precision;               /* 0 = fp32 FFMA everywhere; 1 = split-bf16 wgmma for the flow + decoder (dense convs and
                                       attention); 2 = text encoder on wgmma as well */
   int32_t flow_n_heads;            /* heads of the flow's pre_transformer: the reference hard-codes 2 (models.py:355) */
+  /* Voice conversion (vtts_convert): input features of the posterior encoder enc_q (models.py:1616, mel_processing.py).
+   * Only read when the blob carries enc_q (weights.pack(..., posterior=True)). */
+  int32_t spec_channels;           /* enc_q input channels: n_mel_channels (mel) or filter_length/2+1 (linear spectrogram) */
+  int32_t use_mel_posterior_encoder;
+  int32_t filter_length, hop_length, win_length, n_mel_channels;
+  float mel_fmin, mel_fmax;        /* (the mel filter bank itself is packed into the blob) */
 } vtts_config;
 
 /* Replaces onnxruntime.InferenceSession(model.onnx) (vosk_tts/model.py:46).
@@ -163,7 +169,9 @@ int vtts_timeline(vtts_handle h, int enable, unsigned long long* out, size_t max
 
 /* Test hooks: flags bit0 keeps a copy of z_p (models.py:1700); vtts_debug_read copies a named workspace
  * tensor of the last call ("x", "stats", "dx", "za", "zb", "condv", "z_p", "z", "d0", "stage<i>", "post") to
- * host memory in the engine's channels-last packed layout. */
+ * host memory in the engine's channels-last packed layout.  After a conversion: "vc_spec" (enc_q input rows: the log-mel or
+ * linear spectrogram, spec_channels rounded up to 16 columns), "vc_z" (posterior sample) and "vc_z_p" (flow forward output;
+ * both kept when bit0 is set), "vc_z_hat" (flow reverse output). */
 int vtts_debug_flags(vtts_handle h, int flags);
 int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floats, size_t* n_out);
 /* Unit-test hook for the relative-position attention kernels (attentions.py:165-196): one launch of layer "enc.<i>" or
@@ -171,6 +179,30 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
  * wgmma kernel (attn_tc.cuh), 0 the fp32 FFMA kernels.  iters > 0: *ms_out = average device time of `iters` more launches. */
 int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host, int T, int use_tc, float* out_host, int iters,
                          float* ms_out);
+
+/* Voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718): re-voices recordings of speaker sid_src as
+ * speaker sid_tgt of the same multi-speaker model.  One call = spectrogram front end, posterior encoder enc_q (g_src),
+ * flow forward (g_src), flow reverse (g_tgt), decoder (g_tgt); no host synchronisation inside (the frame counts follow
+ * from the input lengths: frames = (len + 2*pad - filter_length) / hop_length + 1, pad = (filter_length - hop_length) / 2,
+ * i.e. len / 256 for the reference configuration).
+ *   wav          float [B, wav_ld] in [-1, 1], clip b = wav[b*wav_ld .. + wav_lengths[b]); every clip is padded and framed
+ *                on its own samples; needs wav_lengths[b] > pad (385 samples for the reference configuration)
+ *   noise_scale  scales the posterior's eps (the reference uses 1); 0 gives z = m
+ *   noise_q      float [B, inter_channels, q_ld] replaces torch.randn_like at models.py:841 (columns < frames[b] read), or
+ *                NULL -> Philox(seed)
+ *   out_wav      out float [B, out_ld]: clip b gets hop * out_frames[b] samples
+ *   out_frames   out int64 [B]
+ * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: the blob has no enc_q, n_speakers <= 1, a speaker id out of range,
+ * a clip too short for the reflect padding, or an odd flow_n_flows (the Flip folding of the packed flow is only valid for
+ * both directions with an even count).  VTTS_ERR_CAPACITY: out_ld < hop * max(frames). */
+int vtts_convert(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const int64_t* sid_src,
+                 const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed, float* out_wav,
+                 int64_t out_ld, int64_t* out_frames);
+/* Same without the front end: spec float [B, spec_channels, spec_ld] is the reference's `y` (log-mel or linear magnitude
+ * spectrogram), spec_lengths[b] frames valid (1 <= spec_lengths[b] <= spec_ld). */
+int vtts_convert_spec(vtts_handle h, const float* spec, const int64_t* spec_lengths, int B, int64_t spec_ld, const int64_t* sid_src,
+                      const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed, float* out_wav,
+                      int64_t out_ld, int64_t* out_frames);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

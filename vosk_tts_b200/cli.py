@@ -20,6 +20,8 @@ def main(argv=None):
     p.add_argument("--output", "-o", default="out.wav", type=str, help="optional output filename path")
     p.add_argument("--log-level", default="INFO", help="logging level")
     p.add_argument("--device", type=int, default=0, help="CUDA device index (extension)")
+    p.add_argument("--convert-from", type=str, help="voice conversion (extension): re-voice this mono WAV as --speaker")
+    p.add_argument("--source-speaker", type=int, help="speaker id of the --convert-from recording")
     args = p.parse_args(argv)
     logging.getLogger().setLevel(args.log_level.upper())
     if args.list_models:
@@ -27,6 +29,12 @@ def main(argv=None):
         return 0
     if args.list_languages:
         list_languages()
+        return 0
+    if args.convert_from:
+        if args.source_speaker is None or args.speaker is None:
+            p.error("--convert-from needs --source-speaker and --speaker (the target)")
+        model = Model(args.model, args.model_name, args.lang, device=args.device, voice_conversion=True)
+        Synth(model).convert(args.convert_from, args.output, args.source_speaker, args.speaker)
         return 0
     if not args.input:
         logging.info("Please specify input text or file")

@@ -46,6 +46,15 @@ DEFAULT_CONFIG = {
     "gen_istft_n_fft": 16,
     "gen_istft_hop_size": 4,
     "sampling_rate": 22050,
+    # input features of the posterior encoder enc_q (voice conversion only; json "data" block :2-15, models.py:1616)
+    "use_mel_posterior_encoder": True,
+    "filter_length": 1024,
+    "hop_length": 256,
+    "win_length": 1024,
+    "n_mel_channels": 80,
+    "mel_fmin": 0.0,
+    "mel_fmax": None,                # None: sampling_rate / 2 (librosa.filters.mel)
+    "spec_channels": 80,             # n_mel_channels (mel) or filter_length // 2 + 1 (linear spectrogram)
 }
 
 
@@ -87,6 +96,14 @@ def from_training_json(path_or_dict, n_vocab=62):
     elif out["transformer_flow_type"] == "mono_layer_post_residual":
         raise ValueError("use_transformer_flows=false with transformer_flow_type 'mono_layer_post_residual' (the reference "
                          "default) adds MonoTransformerFlowLayers to the flow (models.py:716-734): not supported")
+    # posterior encoder input (voice conversion): the model block decides, as in onnx_export.py:38-45 / train.py:77, which
+    # overwrite the data block's flag with it
+    d = cfg["data"]
+    out["use_mel_posterior_encoder"] = m.get("use_mel_posterior_encoder", False) is True
+    for k in ("filter_length", "hop_length", "win_length", "n_mel_channels", "mel_fmin", "mel_fmax"):
+        if k in d:
+            out[k] = d[k]
+    out["spec_channels"] = out["n_mel_channels"] if out["use_mel_posterior_encoder"] else out["filter_length"] // 2 + 1
     # same precedence as SynthesizerTrn.__init__ (models.py:1585-1606)
     if m.get("mb_istft_vits", False):
         out["decoder"] = "mb_istft"

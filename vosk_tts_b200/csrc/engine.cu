@@ -26,6 +26,7 @@
 #include "conv_tc.cuh"
 #include "mas.cuh"
 #include "attn_tc.cuh"
+#include "vc.cuh"
 
 using namespace vtts;
 
@@ -533,7 +534,7 @@ struct vtts_engine {
   void alloc_flow_planes();
   void alloc_decoder_planes();
   void decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready);
-  void flow_tc(float* z, const int* fl, const int* fo, bool emit_pz);
+  void flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, const float* cond, int cond_ld, bool forward);
   void launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen, Planes* pl);
   void bind_weights();
   void launch_conv(const std::vector<ConvP>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
@@ -558,6 +559,33 @@ struct vtts_engine {
   void decode(float* z, const int* fl, const int* fo, bool planes_ready = false, bool pz_ready = false);
   bool have_latent = false;
   Buf<int> d_chunk;                              // [len, off, off_end] of the chunk being decoded
+
+  // WN stack (modules.py:148-176) shared by the flow's coupling layers and the posterior encoder: `x` (and, on the tensor
+  // cores, its planes px) is updated in place, `skip` receives the summed skip halves (planes pskip from the last layer);
+  // layer i adds the cond rows cond + i*2H (row stride cond_ld) before the gate, none when cond is null.
+  void wn_ffma(const std::vector<ConvW>& in, const std::vector<ConvW>& rsx, const std::vector<ConvW>& rss, int nl, int fk,
+               int dil_rate, float* x, float* acts, float* skip, const float* cond, int cond_ld, const int* fl, const int* fo);
+  void wn_tc(const std::vector<TcW>& t_in, const std::vector<ConvW>& in, const std::vector<TcW>& t_rsx, const std::vector<ConvW>& rsx,
+             const std::vector<TcW>& t_rss, const std::vector<ConvW>& rss, int nl, int fk, int dil_rate, float* x, float* skip, const Planes& px,
+             const Planes& pacts, const Planes& pskip, const float* cond, int cond_ld, const int* fl, const int* fo);
+  // The flow on the fp32 pipe; forward = models.py:750-753 (layers in order, x1 <- x1 + m), else the reverse of infer.
+  void flow_ffma(float* z, const int* fl, const int* fo, const float* cond, int cond_ld, bool forward);
+
+  // ---- voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718)
+  bool has_encq = false, q_tc = false;
+  static constexpr int Q_LAYERS = 16, Q_KERNEL = 5;        // PosteriorEncoder(spec_channels, I, H, 5, 1, 16, gin) (models.py:1616)
+  ConvW q_pre, q_proj;
+  std::vector<ConvW> q_in, q_rsx, q_rss;
+  std::vector<TcW> qt_in, qt_rsx, qt_rss;
+  TcW qt_proj;
+  const float *q_cond_w = nullptr, *q_cond_b = nullptr, *stft_basis = nullptr, *mel_fb = nullptr;
+  int q_R = 0, spec_pad = 0, vc_pad = 0, vc_wld = 0;
+  Buf<int> d_vint;                                 // [clip_len B][sid 2B]
+  Buf<float> d_vprm, d_vin, d_vlin, d_vfeat, d_vstats, d_vcsrc, d_vnoise, d_vz_dbg, d_vzp_dbg;
+  Buf<char> h_pin_vc;
+  struct VcPin { int *frm_len, *frm_off, *clip_len, *sid; float *prm, *in, *eps; };
+  VcPin vc_layout(bool from_spec, bool eps);
+  void convert_enqueue(bool from_spec, bool eps);
 };
 
 namespace {
@@ -747,6 +775,43 @@ void vtts_engine::bind_weights() {
   } else {
     dec_post = conv("dec.post", ch, 1, 7);
     hop = up_total;
+  }
+  // ---- posterior encoder enc_q + front end (only in blobs packed with posterior=True)
+  has_encq = tensors.count("encq.pre.b") > 0;
+  if (has_encq) {
+    REQUIRE(c.spec_channels > 0 && c.filter_length > 0 && c.hop_length > 0 && c.filter_length % ST_TN == 0 &&
+                c.filter_length > c.hop_length && (c.filter_length - c.hop_length) % 2 == 0,
+            VTTS_ERR_INVALID, "bad spectrogram configuration (filter_length must be a multiple of 64, above hop_length)");
+    REQUIRE(c.win_length == c.filter_length, VTTS_ERR_INVALID, "win_length != filter_length is not supported by the spectrogram front end");
+    REQUIRE(c.use_mel_posterior_encoder ? c.spec_channels == c.n_mel_channels : c.spec_channels == c.filter_length / 2 + 1,
+            VTTS_ERR_INVALID, "spec_channels does not match the posterior encoder's input (n_mel_channels / filter_length/2+1)");
+    const bool qfw = !(c.precision >= 1 && H % TC_BK == 0);
+    spec_pad = (c.spec_channels + CV_CK - 1) / CV_CK * CV_CK;     // enc_q.pre runs on the FFMA conv: input zero-padded to 16 channels
+    vc_pad = (c.filter_length - c.hop_length) / 2;
+    q_pre = conv("encq.pre", spec_pad, H, 1);
+    q_in.clear(); q_rsx.clear(); q_rss.clear(); qt_in.clear(); qt_rsx.clear(); qt_rss.clear();
+    for (int i = 0; i < Q_LAYERS; ++i) {
+      q_in.push_back(conv("encq.in" + std::to_string(i), H, 2 * H, Q_KERNEL, qfw));
+      if (i < Q_LAYERS - 1) q_rsx.push_back(conv("encq.rsx" + std::to_string(i), H, H, 1, qfw));
+      q_rss.push_back(conv("encq.rss" + std::to_string(i), H, H, 1, qfw));
+    }
+    q_proj = conv("encq.proj", H, 2 * I, 1, qfw);
+    q_tc = tc && !qfw;
+    if (q_tc) {
+      for (int i = 0; i < Q_LAYERS; ++i) {
+        qt_in.push_back(tcw("encq.in" + std::to_string(i), H, 2 * H, Q_KERNEL));
+        if (i < Q_LAYERS - 1) qt_rsx.push_back(tcw("encq.rsx" + std::to_string(i), H, H, 1));
+        qt_rss.push_back(tcw("encq.rss" + std::to_string(i), H, H, 1));
+      }
+      qt_proj = tcw("encq.proj", H, 2 * I, 1);
+    }
+    if (has_g) {
+      q_R = Q_LAYERS * 2 * H;
+      q_cond_w = vec("encq.cond.w", (size_t)q_R * G);
+      q_cond_b = vec("encq.cond.b", q_R);
+    }
+    stft_basis = vec("vc.stft", (size_t)c.filter_length * c.filter_length);
+    mel_fb = c.use_mel_posterior_encoder ? vec("vc.mel", (size_t)c.n_mel_channels * (c.filter_length / 2 + 1)) : nullptr;
   }
 }
 
@@ -1100,7 +1165,10 @@ void vtts_engine::alloc_decoder_planes() {
 
 // emit_pz: the post convs of the last two coupling layers also write the split-bf16 planes of their half of z for the
 // decoder's conv_pre (dcp.pz), which saves the separate fp32 -> planes pass
-void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz) {
+// forward: the flow's forward direction (models.py:750-753, x1 <- x1 + m, layers in order) for voice conversion; the
+// Flip folding of the packed weights is valid for it when flow_n_flows is even.  cond: the [B][cond_ld] rows of the stacked
+// conditioning matrix of the speaker the flow runs for (null: unconditioned).
+void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, const float* cond, int cond_ld, bool forward) {
   const vtts_config& c = cfg;
   const int H = c.hidden_channels, I = c.inter_channels, half = I / 2;
   const long F = Tfrm;
@@ -1114,7 +1182,8 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz) 
   float* fao = ensure(d_fao, (size_t)F * H);
   Planes ph = flp.ph, pao = flp.pao, ph1 = flp.ph1, pff = flp.pff, pwx = flp.pwx, pacts = flp.pacts, pskip = flp.pskip, pqkv = flp.pqkv;
   dim3 lg((maxFrm + 3) / 4, B);
-  for (int f = nf - 1; f >= 0; --f) {
+  for (int s = 0; s < nf; ++s) {
+    const int f = forward ? s : nf - 1 - s;
     const FlowW& W = flow[f];
     const bool flipped = ((nf - f) % 2) == 1;
     const int x0off = flipped ? half : 0, x1off = flipped ? 0 : half;
@@ -1152,28 +1221,37 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz) 
       ++launches;
       wn_x = wx;
     }
-    int dil = 1;
-    for (int i = 0; i < nl; ++i) {
-      { TcSpec q; q.in = pwx; q.w = W.t_in[i]; q.bias = W.in[i].b; q.Cin = H; q.Cout = 2 * H; q.k = fk; q.dil = dil;
-        q.pad = dil * (fk - 1) / 2; q.epi = TCE_GATE; q.out = pacts; q.pl_slope = 1.f;
-        if (has_g) { q.cond = d_condv.p + r_flow + (f * nl + i) * 2 * H; q.cond_ld = condR; }
-        launch_tc({q}, 1, fl, fo, maxFrm, B); }
-      TcSpec qs; qs.in = pacts; qs.w = W.t_rss[i]; qs.bias = W.rss[i].b; qs.Cin = H; qs.Cout = H; qs.y = skip; qs.ldy = H;
-      if (i > 0) { qs.res = skip; qs.ldr = H; }
-      if (i < nl - 1) {
-        TcSpec qx; qx.in = pacts; qx.w = W.t_rsx[i]; qx.bias = W.rsx[i].b; qx.Cin = H; qx.Cout = H; qx.y = wn_x; qx.ldy = H;
-        qx.res = wn_x; qx.ldr = H; qx.out = pwx; qx.pl_slope = 1.f;
-        launch_tc({qx, qs}, 1, fl, fo, maxFrm, B);
-      } else {
-        qs.out = pskip; qs.pl_slope = 1.f;
-        launch_tc({qs}, 1, fl, fo, maxFrm, B);
-      }
-      dil *= c.flow_dilation_rate;
-    }
-    { TcSpec q; q.in = pskip; q.w = W.t_post; q.bias = W.post.b; q.Cin = H; q.Cout = half; q.alpha = -1.f;
+    wn_tc(W.t_in, W.in, W.t_rsx, W.rsx, W.t_rss, W.rss, nl, fk, c.flow_dilation_rate, wn_x, skip, pwx, pacts, pskip,
+          cond ? cond + r_flow + f * nl * 2 * H : nullptr, cond_ld, fl, fo);
+    { TcSpec q; q.in = pskip; q.w = W.t_post; q.bias = W.post.b; q.Cin = H; q.Cout = half; q.alpha = forward ? 1.f : -1.f;
       q.y = z; q.ldy = I; q.yoff = x1off; q.res = z; q.ldr = I; q.roff = x1off;
       if (emit_pz && f <= 1) { q.out = dcp.pz; q.poff = x1off; q.pl_slope = 1.f; }     // this half of z is final now
       launch_tc({q}, 1, fl, fo, maxFrm, B); }
+  }
+}
+
+void vtts_engine::wn_tc(const std::vector<TcW>& t_in, const std::vector<ConvW>& in, const std::vector<TcW>& t_rsx,
+                        const std::vector<ConvW>& rsx, const std::vector<TcW>& t_rss, const std::vector<ConvW>& rss, int nl, int fk,
+                        int dil_rate, float* x, float* skip, const Planes& px, const Planes& pacts, const Planes& pskip, const float* cond,
+                        int cond_ld, const int* fl, const int* fo) {
+  const int H = cfg.hidden_channels;
+  int dil = 1;
+  for (int i = 0; i < nl; ++i) {
+    { TcSpec q; q.in = px; q.w = t_in[i]; q.bias = in[i].b; q.Cin = H; q.Cout = 2 * H; q.k = fk; q.dil = dil;
+      q.pad = dil * (fk - 1) / 2; q.epi = TCE_GATE; q.out = pacts; q.pl_slope = 1.f;
+      if (cond) { q.cond = cond + i * 2 * H; q.cond_ld = cond_ld; }
+      launch_tc({q}, 1, fl, fo, maxFrm, B); }
+    TcSpec qs; qs.in = pacts; qs.w = t_rss[i]; qs.bias = rss[i].b; qs.Cin = H; qs.Cout = H; qs.y = skip; qs.ldy = H;
+    if (i > 0) { qs.res = skip; qs.ldr = H; }
+    if (i < nl - 1) {
+      TcSpec qx; qx.in = pacts; qx.w = t_rsx[i]; qx.bias = rsx[i].b; qx.Cin = H; qx.Cout = H; qx.y = x; qx.ldy = H;
+      qx.res = x; qx.ldr = H; qx.out = px; qx.pl_slope = 1.f;
+      launch_tc({qx, qs}, 1, fl, fo, maxFrm, B);
+    } else {
+      qs.out = pskip; qs.pl_slope = 1.f;
+      launch_tc({qs}, 1, fl, fo, maxFrm, B);
+    }
+    dil *= dil_rate;
   }
 }
 
@@ -1780,8 +1858,37 @@ void vtts_engine::phase2(const float* noise_z, int z_ld, bool noise_on_device, b
     if (dec_now) alloc_decoder_planes();
     flush_tails(fl, fo);
   }
-  if (flow_on_tc) flow_tc(z, fl, fo, emit_pz);
-  for (int f = nf - 1; f >= 0 && !flow_on_tc; --f) {
+  (void)h; (void)h1; (void)wx; (void)acts; (void)skip; (void)fy; (void)fqkv; (void)fao; (void)ffh2; (void)nl; (void)fk; (void)half;
+  const float* cond = has_g ? d_condv.p : nullptr;
+  if (flow_on_tc) flow_tc(z, fl, fo, emit_pz, cond, condR, /*forward=*/false);
+  else flow_ffma(z, fl, fo, cond, condR, /*forward=*/false);
+  if (!capturing) CK(cudaEventRecord(ev[5], stream));
+
+  if (!run_decoder) return;
+  decode(z, fl, fo, /*planes_ready=*/dec_now, /*pz_ready=*/emit_pz);
+}
+
+// Flow on the fp32 pipe (models.py:750-757).  Flip (modules.py:272-279) is folded into the packed pre/post weights: for a
+// "flipped" layer x0 lives in physical channels [half, 2*half), x1 in [0, half).  forward / cond: see flow_tc.
+void vtts_engine::flow_ffma(float* z, const int* fl, const int* fo, const float* cond, int cond_ld, bool forward) {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, I = c.inter_channels, half = I / 2;
+  const size_t F = (size_t)Tfrm;
+  float* h = ensure(d_h, F * H);
+  float* h1 = ensure(d_h1, F * H);
+  float* wx = ensure(d_wx, F * H);
+  float* acts = ensure(d_acts, F * H);
+  float* skip = ensure(d_skip, F * H);
+  float* fy = ensure(d_fy, F * H);
+  float* fqkv = nullptr; float* fao = nullptr; float* ffh2 = nullptr;
+  if (c.use_transformer_flows) {
+    fqkv = ensure(d_fqkv, F * 3 * H);
+    fao = ensure(d_fao, F * H);
+    ffh2 = ensure(d_ffh2, F * H);
+  }
+  const int nf = c.flow_n_flows, nl = c.flow_wn_layers, fk = c.flow_kernel_size;
+  for (int s = 0; s < nf; ++s) {
+    const int f = forward ? s : nf - 1 - s;
     const FlowW& W = flow[f];
     const bool flipped = ((nf - f) % 2) == 1;
     const int x0off = flipped ? half : 0, x1off = flipped ? 0 : half;
@@ -1811,37 +1918,40 @@ void vtts_engine::phase2(const float* noise_z, int z_ld, bool noise_on_device, b
       wn_in = wx;
     }
     // WN (modules.py:148-176).  The hidden state is updated in place in `wn_in`.
-    int dil = 1;
-    for (int i = 0; i < nl; ++i) {
-      {
-        ConvP p = mk(W.in[i], wn_in, H, 0, acts, H, 0, dil, dil * (fk - 1) / 2);
-        p.epi = EPI_GATE;
-        if (has_g) { p.cond = d_condv.p + r_flow + (f * nl + i) * 2 * H; p.cond_ld = condR; }
-        launch_conv({p}, 1, fl, fo, maxFrm, B);
-      }
-      ConvP ps = mk(W.rss[i], acts, H, 0, skip, H, 0, 1, 0);
-      if (i > 0) { ps.res = skip; ps.ldr = H; ps.roff = 0; }
-      if (i < nl - 1) {
-        ConvP px = mk(W.rsx[i], acts, H, 0, wn_in, H, 0, 1, 0);
-        px.res = wn_in; px.ldr = H; px.roff = 0;
-        launch_conv({px, ps}, 1, fl, fo, maxFrm, B);
-      } else {
-        launch_conv({ps}, 1, fl, fo, maxFrm, B);
-      }
-      dil *= c.flow_dilation_rate;
-    }
+    wn_ffma(W.in, W.rsx, W.rss, nl, fk, c.flow_dilation_rate, wn_in, acts, skip, cond ? cond + r_flow + f * nl * 2 * H : nullptr, cond_ld,
+            fl, fo);
     {
-      // x1 <- (x1 - post(h)) (mean_only; models.py:381-391)
+      // x1 <- x1 - post(h) (reverse) / x1 + post(h) (forward) (mean_only; models.py:381-391)
       ConvP p = mk(W.post, skip, H, 0, z, I, x1off, 1, 0);
-      p.alpha = -1.f;
+      p.alpha = forward ? 1.f : -1.f;
       p.res = z; p.ldr = I; p.roff = x1off;
       launch_conv({p}, 1, fl, fo, maxFrm, B);
     }
   }
-  if (!capturing) CK(cudaEventRecord(ev[5], stream));
+}
 
-  if (!run_decoder) return;
-  decode(z, fl, fo, /*planes_ready=*/dec_now, /*pz_ready=*/emit_pz);
+void vtts_engine::wn_ffma(const std::vector<ConvW>& in, const std::vector<ConvW>& rsx, const std::vector<ConvW>& rss, int nl, int fk,
+                          int dil_rate, float* x, float* acts, float* skip, const float* cond, int cond_ld, const int* fl, const int* fo) {
+  const int H = cfg.hidden_channels;
+  int dil = 1;
+  for (int i = 0; i < nl; ++i) {
+    {
+      ConvP p = mk(in[i], x, H, 0, acts, H, 0, dil, dil * (fk - 1) / 2);
+      p.epi = EPI_GATE;
+      if (cond) { p.cond = cond + i * 2 * H; p.cond_ld = cond_ld; }
+      launch_conv({p}, 1, fl, fo, maxFrm, B);
+    }
+    ConvP ps = mk(rss[i], acts, H, 0, skip, H, 0, 1, 0);
+    if (i > 0) { ps.res = skip; ps.ldr = H; ps.roff = 0; }
+    if (i < nl - 1) {
+      ConvP px = mk(rsx[i], acts, H, 0, x, H, 0, 1, 0);
+      px.res = x; px.ldr = H; px.roff = 0;
+      launch_conv({px, ps}, 1, fl, fo, maxFrm, B);
+    } else {
+      launch_conv({ps}, 1, fl, fo, maxFrm, B);
+    }
+    dil *= dil_rate;
+  }
 }
 
 // Decoder over the utterance rows described by (fl, fo) -- the whole batch, or one halo-extended chunk of a single
@@ -1957,6 +2067,127 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     launch_conv({p}, rm, fl, fo, maxFrm, B);
   }
   if (!capturing) CK(cudaEventRecord(ev[6], stream));
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Voice conversion (models.py:1710-1718): spectrogram front end, enc_q with g_src, flow forward with g_src, flow reverse
+// with g_tgt, decoder.  The frame counts follow from the input lengths, so the whole call is ONE graphed phase.
+// ---------------------------------------------------------------------------------------------------
+// Pinned staging of one call (fixed layout for a given batch / length bucket, so a captured graph re-reads it on replay):
+// ints [frm_len B][frm_off B+1][clip_len B][sid_src B][sid_tgt B], prm[16], input (wav [B][vc_wld] or spec
+// [B][spec_channels][maxFrm]), eps [B][inter][maxFrm].
+vtts_engine::VcPin vtts_engine::vc_layout(bool from_spec, bool eps) {
+  const vtts_config& c = cfg;
+  const size_t nin = from_spec ? (size_t)B * c.spec_channels * maxFrm : (size_t)B * vc_wld;
+  const size_t ints = (size_t)(5 * B + 1) * sizeof(int);
+  const size_t head = (ints + 63) / 64 * 64;
+  const size_t bytes = head + 16 * sizeof(float) + nin * sizeof(float) + (eps ? (size_t)B * c.inter_channels * maxFrm * sizeof(float) : 0) + 64;
+  char* pin = ensure_pinned(h_pin_vc, bytes);
+  VcPin pp;
+  pp.frm_len = reinterpret_cast<int*>(pin);
+  pp.frm_off = pp.frm_len + B;
+  pp.clip_len = pp.frm_off + B + 1;
+  pp.sid = pp.clip_len + B;
+  pp.prm = reinterpret_cast<float*>(pin + head);
+  pp.in = pp.prm + 16;
+  pp.eps = pp.in + nin;
+  return pp;
+}
+
+void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, I = c.inter_channels;
+  const size_t F = (size_t)Tfrm;
+  if (!capturing) CK(cudaEventRecord(ev[4], stream));
+  VcPin pp = vc_layout(from_spec, eps);
+  int* fl = ensure(d_frm_len, B);
+  int* fo = ensure(d_frm_off, B + 1);
+  int* vi = ensure(d_vint, 3 * B);                       // [clip_len B][sid_src B][sid_tgt B]
+  float* prm = ensure(d_vprm, 16);
+  const size_t nin = from_spec ? (size_t)B * c.spec_channels * maxFrm : (size_t)B * vc_wld;
+  float* vin = ensure(d_vin, nin);
+  CK(cudaMemcpyAsync(fl, pp.frm_len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(fo, pp.frm_off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(vi, pp.clip_len, 3 * B * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(prm, pp.prm, 16 * sizeof(float), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(vin, pp.in, nin * sizeof(float), cudaMemcpyHostToDevice, stream));
+  float* noise = nullptr;
+  if (eps) {
+    noise = ensure(d_vnoise, (size_t)B * I * maxFrm);
+    CK(cudaMemcpyAsync(noise, pp.eps, (size_t)B * I * maxFrm * sizeof(float), cudaMemcpyHostToDevice, stream));
+  }
+  // ---- g_src / g_tgt (models.py:1712-1713) and every cond row of both, one launch: src -> d_vcsrc [B][condR + q_R]
+  //      (the TTS rows, then enc_q's), tgt -> d_condv [B][condR] (where the reverse flow and the decoder read them)
+  const int qld = condR + q_R;
+  float* csrc = ensure(d_vcsrc, (size_t)B * qld);
+  float* ctgt = ensure(d_condv, (size_t)B * condR);
+  klaunch(cond_vc_kernel, dim3((qld + 7) / 8, 2 * B), dim3(256), (size_t)(c.gin_channels * sizeof(float)), emb_g, (const int*)(vi + B),
+          cond_w, cond_b, condR, q_cond_w, q_cond_b, q_R, csrc, ctgt, c.gin_channels, B, c.n_speakers);
+  CK(cudaGetLastError());
+  ++launches;
+  // ---- enc_q input rows [F][spec_pad]
+  float* feat = ensure(d_vfeat, F * spec_pad);
+  if (from_spec) {
+    klaunch(spec_pack_kernel, dim3(maxFrm, B), dim3(128), (size_t)0, (const float*)vin, c.spec_channels, maxFrm, (const int*)fl,
+            (const int*)fo, feat, spec_pad);
+    CK(cudaGetLastError());
+    ++launches;
+  } else {
+    const int nbins = c.filter_length / 2 + 1;
+    const bool mel = c.use_mel_posterior_encoder != 0;
+    float* lin = mel ? ensure(d_vlin, F * nbins) : feat;
+    dim3 g((maxFrm + ST_TM - 1) / ST_TM, c.filter_length / ST_TN, B);
+    klaunch(stft_mag_kernel, g, dim3(ST_THREADS), (size_t)0, (const float*)vin, (long)vc_wld, (const int*)vi, stft_basis, c.filter_length,
+            c.hop_length, vc_pad, (const int*)fl, (const int*)fo, lin, mel ? nbins : spec_pad);
+    CK(cudaGetLastError());
+    ++launches;
+    if (mel) {
+      klaunch(mel_log_kernel, dim3((maxFrm + MEL_ROWS - 1) / MEL_ROWS, B), dim3(MEL_THREADS), (size_t)MEL_ROWS * nbins * sizeof(float),
+              (const float*)lin, nbins, mel_fb, nbins, c.n_mel_channels, (const int*)fl, (const int*)fo, feat, spec_pad);
+      CK(cudaGetLastError());
+      ++launches;
+    }
+  }
+  // ---- posterior encoder (models.py:836-842): pre -> 16-layer WN (g_src) -> proj -> sample
+  float* h = ensure(d_h, F * H);
+  float* acts = ensure(d_acts, F * H);
+  float* skip = ensure(d_skip, F * H);
+  float* stats = ensure(d_vstats, F * 2 * I);
+  float* z = ensure(d_z, F * I);
+  const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
+  if (flow_on_tc || q_tc) {
+    begin_planes();
+    alloc_flow_planes();                     // (enc_q uses the flow's WN planes before the flow runs)
+    flush_tails(fl, fo);
+  }
+  {
+    ConvP p = mk(q_pre, feat, spec_pad, 0, h, H, 0, 1, 0);
+    if (q_tc) { p.p_hi = flp.pwx.hi; p.p_lo = flp.pwx.lo; p.ldp = H; p.pl_slope = 1.f; }
+    launch_conv({p}, 1, fl, fo, maxFrm, B);
+  }
+  const float* qcond = csrc + condR;
+  if (q_tc) {
+    wn_tc(qt_in, q_in, qt_rsx, q_rsx, qt_rss, q_rss, Q_LAYERS, Q_KERNEL, 1, h, skip, flp.pwx, flp.pacts, flp.pskip, qcond, qld, fl, fo);
+    TcSpec q; q.in = flp.pskip; q.w = qt_proj; q.bias = q_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
+    launch_tc({q}, 1, fl, fo, maxFrm, B);
+  } else {
+    wn_ffma(q_in, q_rsx, q_rss, Q_LAYERS, Q_KERNEL, 1, h, acts, skip, qcond, qld, fl, fo);
+    launch_conv({mk(q_proj, skip, H, 0, stats, 2 * I, 0, 1, 0)}, 1, fl, fo, maxFrm, B);
+  }
+  klaunch(posterior_sample_kernel, dim3(maxFrm, B), dim3(64), (size_t)0, (const float*)stats, I, (const float*)noise, maxFrm,
+          (const float*)prm, (const int*)fl, (const int*)fo, z);
+  CK(cudaGetLastError());
+  ++launches;
+  if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vz_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  // ---- z_p = flow(z, g_src); z_hat = flow^-1(z_p, g_tgt)   (models.py:1715-1716)
+  if (flow_on_tc) flow_tc(z, fl, fo, false, csrc, qld, /*forward=*/true);
+  else flow_ffma(z, fl, fo, csrc, qld, /*forward=*/true);
+  if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vzp_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  if (flow_on_tc) flow_tc(z, fl, fo, false, ctgt, condR, /*forward=*/false);
+  else flow_ffma(z, fl, fo, ctgt, condR, /*forward=*/false);
+  if (!capturing) CK(cudaEventRecord(ev[5], stream));
+  // ---- o_hat = dec(z_hat * y_mask, g=g_tgt)   (models.py:1717)
+  decode(z, fl, fo);
 }
 
 // ===================================================================================================
@@ -2230,6 +2461,81 @@ static void impl_infer_dev(vtts_handle h, const int64_t* d_ids, const int64_t* l
   impl_synthesize_dev(h, d_noise_z, z_ld, d_wav, wav_ld);
 }
 
+// Voice conversion through host buffers (vtts_convert / vtts_convert_spec).
+static void impl_convert(vtts_handle h, bool from_spec, const float* in, const int64_t* lengths, int B, int64_t ld,
+                         const int64_t* sid_src, const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld,
+                         uint64_t seed, float* out_wav, int64_t out_ld, int64_t* out_frames) {
+  const vtts_config& c = h->cfg;
+  REQUIRE(c.flow_n_flows % 2 == 0, VTTS_ERR_INVALID, "voice conversion needs an even flow_n_flows (the Flip folding of the packed "
+          "flow holds for both directions only then)");
+  REQUIRE(h->has_encq, VTTS_ERR_INVALID, "the weight blob has no posterior encoder (enc_q): voice conversion needs a model packed "
+          "with posterior=True from a training checkpoint (model.onnx does not contain enc_q)");
+  REQUIRE(h->has_g && c.n_speakers > 1, VTTS_ERR_INVALID, "voice conversion needs a multi-speaker model (n_speakers > 1)");
+  REQUIRE(B >= 1 && B <= 16384 && ld >= 1, VTTS_ERR_INVALID, "bad batch size / row pitch");
+  std::vector<int> frames(B);
+  for (int b = 0; b < B; ++b) {
+    const int64_t L = lengths[b];
+    if (from_spec) {
+      REQUIRE(L >= 1 && L <= ld, VTTS_ERR_INVALID, "spec_lengths must be in [1, spec_ld]");
+      frames[b] = (int)L;
+    } else {
+      REQUIRE(L <= ld, VTTS_ERR_INVALID, "wav_lengths must not exceed wav_ld");
+      REQUIRE(L > h->vc_pad, VTTS_ERR_INVALID, "clip too short: the reflect padding of the spectrogram needs more than " +
+              std::to_string(h->vc_pad) + " samples");
+      REQUIRE(L < (1LL << 30), VTTS_ERR_INVALID, "clip too long");
+      frames[b] = (int)((L + 2 * h->vc_pad - c.filter_length) / c.hop_length + 1);
+    }
+    REQUIRE(sid_src[b] >= 0 && sid_src[b] < c.n_speakers && sid_tgt[b] >= 0 && sid_tgt[b] < c.n_speakers, VTTS_ERR_INVALID,
+            "speaker id out of range [0, n_speakers)");
+  }
+  h->B = B;
+  h->h_frm_len = frames;
+  h->h_frm_off.assign(B + 1, 0);
+  int off = 0;
+  for (int b = 0; b < B; ++b) { h->h_frm_off[b] = off; off += frames[b] + (b + 1 < B ? SEQ_GAP : 0); }
+  h->h_frm_off[B] = off;
+  h->set_frame_shape();
+  h->have_durations = false;
+  h->have_latent = false;
+  REQUIRE((int64_t)h->real_maxFrm * h->hop <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than hop * max(frames)");
+  REQUIRE(!noise_q || q_ld >= h->real_maxFrm, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
+  h->vc_wld = (h->maxFrm + 2) * c.hop_length + c.filter_length;
+  const int maxF = h->maxFrm, I = c.inter_channels, C = c.spec_channels;
+  vtts_engine::VcPin pp = h->vc_layout(from_spec, noise_q != nullptr);
+  memcpy(pp.frm_len, frames.data(), B * sizeof(int));
+  memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
+  for (int b = 0; b < B; ++b) {
+    pp.clip_len[b] = (int)lengths[b];
+    pp.sid[b] = (int)sid_src[b];
+    pp.sid[B + b] = (int)sid_tgt[b];
+    if (from_spec) {
+      for (int ch = 0; ch < C; ++ch)
+        memcpy(pp.in + ((size_t)b * C + ch) * maxF, in + ((size_t)b * C + ch) * ld, (size_t)frames[b] * sizeof(float));
+    } else {
+      memcpy(pp.in + (size_t)b * h->vc_wld, in + (size_t)b * ld, (size_t)lengths[b] * sizeof(float));
+    }
+    if (noise_q)
+      for (int ch = 0; ch < I; ++ch)
+        memcpy(pp.eps + ((size_t)b * I + ch) * maxF, noise_q + ((size_t)b * I + ch) * q_ld, (size_t)frames[b] * sizeof(float));
+  }
+  for (int i = 0; i < 16; ++i) pp.prm[i] = 0.f;
+  pp.prm[0] = noise_scale;
+  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
+  memcpy(&pp.prm[4], &lo, 4);
+  memcpy(&pp.prm[5], &hi, 4);
+  h->run_graphed({0x55, B, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
+                 [&] { h->convert_enqueue(from_spec, noise_q != nullptr); });
+  const size_t nw = (size_t)h->real_Tfrm * h->hop;
+  float* pw = reinterpret_cast<float*>(h->ensure_pinned((size_t)h->Tfrm * h->hop * sizeof(float) + 64));
+  CK(cudaMemcpyAsync(pw, h->d_wav.p, nw * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaEventRecord(h->ev[7], h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; ++b) {
+    memcpy(out_wav + (size_t)b * out_ld, pw + (size_t)h->h_frm_off[b] * h->hop, (size_t)frames[b] * h->hop * sizeof(float));
+    out_frames[b] = frames[b];
+  }
+}
+
 static void impl_synthesize_dev(vtts_handle h, const float* d_noise_z, int z_ld, float* d_wav, int64_t wav_ld) {
   REQUIRE(h->have_durations, VTTS_ERR_STATE, "vtts_synthesize_dev called without vtts_durations_dev");
   REQUIRE((int64_t)h->real_maxFrm * h->hop <= wav_ld, VTTS_ERR_CAPACITY, "wav_ld is smaller than hop * max(y_lengths)");
@@ -2374,10 +2680,13 @@ void vtts_destroy(vtts_handle h) {
                       &h->d_h29, &h->d_za, &h->d_zb, &h->d_eps_dp, &h->d_z, &h->d_h, &h->d_h1, &h->d_wx, &h->d_acts, &h->d_skip, &h->d_fqkv,
                       &h->d_fao, &h->d_fy, &h->d_ffh2, &h->d_eps_z, &h->d_d0, &h->d_post, &h->d_wav};
   for (auto* b : fb) fr(b->p);
+  Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg};
+  for (auto* b : vb) fr(b->p);
+  fr(h->d_vint.p);
   for (auto& b : h->d_stage) fr(b.p);
   for (auto& v : h->d_xj) for (auto& b : v) fr(b.p);
   for (auto& v : h->d_tmp) for (auto& b : v) fr(b.p);
-  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z}) if (hb->p) cudaFreeHost(hb->p);
+  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc}) if (hb->p) cudaFreeHost(hb->p);
   for (auto& kv : h->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   fr(h->d_prm.p);
   fr(h->d_pref.p);
@@ -2551,6 +2860,22 @@ int vtts_infer_dev(vtts_handle h, const int64_t* d_ids, const int64_t* lengths_h
   return rc;
 }
 
+int vtts_convert(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const int64_t* sid_src,
+                 const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed, float* out_wav,
+                 int64_t out_ld, int64_t* out_frames) {
+  if (!wav || !wav_lengths || !sid_src || !sid_tgt || !out_wav || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_convert(h, false, wav, wav_lengths, B, wav_ld, sid_src, sid_tgt, noise_scale, noise_q, q_ld, seed, out_wav,
+                                       out_ld, out_frames); });
+}
+
+int vtts_convert_spec(vtts_handle h, const float* spec, const int64_t* spec_lengths, int B, int64_t spec_ld, const int64_t* sid_src,
+                      const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed, float* out_wav,
+                      int64_t out_ld, int64_t* out_frames) {
+  if (!spec || !spec_lengths || !sid_src || !sid_tgt || !out_wav || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_convert(h, true, spec, spec_lengths, B, spec_ld, sid_src, sid_tgt, noise_scale, noise_q, q_ld, seed,
+                                       out_wav, out_ld, out_frames); });
+}
+
 int vtts_hop(vtts_handle h) { return h ? h->hop : 0; }
 
 int vtts_stage_timings(vtts_handle h, float* ms, int n) {
@@ -2654,6 +2979,10 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "z_p") { src = h->d_zp_dbg.p; n = F * c.inter_channels; }
     else if (nm == "z") { src = h->d_z.p; n = F * c.inter_channels; }
     else if (nm == "d0") { src = h->d_d0.p; n = F * c.upsample_initial_channel; }
+    else if (nm == "vc_spec") { src = h->d_vfeat.p; n = F * h->spec_pad; }
+    else if (nm == "vc_z") { src = h->d_vz_dbg.p; n = F * c.inter_channels; }
+    else if (nm == "vc_z_p") { src = h->d_vzp_dbg.p; n = F * c.inter_channels; }
+    else if (nm == "vc_z_hat") { src = h->d_z.p; n = F * c.inter_channels; }
     else if (nm == "post") { src = h->d_post.p; n = (F * h->up_total + h->B) * c.subbands * (c.istft_n_fft + 2); }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);

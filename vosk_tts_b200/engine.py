@@ -6,6 +6,7 @@ import os
 import numpy as np
 
 from . import build as _build
+from . import config as _config
 
 _LIB = None
 
@@ -35,6 +36,9 @@ class VttsConfig(C.Structure):
         ("upsample_initial_channel", C.c_int32),
         ("subbands", C.c_int32), ("istft_n_fft", C.c_int32), ("istft_hop", C.c_int32),
         ("precision", C.c_int32), ("flow_n_heads", C.c_int32),
+        ("spec_channels", C.c_int32), ("use_mel_posterior_encoder", C.c_int32),
+        ("filter_length", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32), ("n_mel_channels", C.c_int32),
+        ("mel_fmin", C.c_float), ("mel_fmax", C.c_float),
     ]
 
 
@@ -44,7 +48,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_profile", "vtts_profile_read", "vtts_set_graphs", "vtts_graph_replays",
            "vtts_profile_read_tc", "vtts_timeline", "vtts_infer", "vtts_infer_dev",
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
-           "vtts_maximum_path", "vtts_maximum_path_dev"]
+           "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec"]
 
 
 class _Missing:
@@ -148,6 +152,10 @@ def load_library(build_if_missing=True):
     lib.vtts_maximum_path.restype = i32
     lib.vtts_maximum_path_dev.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
     lib.vtts_maximum_path_dev.restype = i32
+    for nm in ("vtts_convert", "vtts_convert_spec"):
+        fn = getattr(lib, nm)
+        fn.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, C.c_float, vp, i32, C.c_uint64, vp, C.c_int64, vp]
+        fn.restype = i32
     _LIB = lib
     return lib
 
@@ -182,6 +190,14 @@ def make_c_config(cfg, precision=0):
     c.istft_hop = int(cfg["gen_istft_hop_size"])
     c.precision = int(precision)
     c.flow_n_heads = int(cfg.get("flow_n_heads", 2))
+    d = _config.DEFAULT_CONFIG
+    c.use_mel_posterior_encoder = int(bool(cfg.get("use_mel_posterior_encoder", d["use_mel_posterior_encoder"])))
+    for k in ("filter_length", "hop_length", "win_length", "n_mel_channels"):
+        setattr(c, k, int(cfg.get(k, d[k])))
+    c.spec_channels = int(cfg.get("spec_channels", c.n_mel_channels if c.use_mel_posterior_encoder else c.filter_length // 2 + 1))
+    c.mel_fmin = float(cfg.get("mel_fmin", 0.0) or 0.0)
+    fmax = cfg.get("mel_fmax")
+    c.mel_fmax = float(cfg.get("sampling_rate", 22050)) / 2 if fmax is None else float(fmax)
     return c
 
 
@@ -364,6 +380,65 @@ class Engine:
         ez = np.zeros((B, int(self.cfg["inter_channels"]), F), np.float32)
         self.synthesize(yl, ez)
         self.infer(ids, lens, sid, (0.667, ls, 0.8), None, None, seed=1, frames_hint=F + 64)
+        return F
+
+    # ---- voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718)
+    def _convert(self, from_wav, x, lengths, ld, sid_src, sid_tgt, noise_scale, noise, seed):
+        B = x.shape[0]
+        lengths = np.ascontiguousarray(lengths, dtype=np.int64).reshape(B)
+        src = np.ascontiguousarray(np.broadcast_to(np.asarray(sid_src, np.int64), (B,)))
+        tgt = np.ascontiguousarray(np.broadcast_to(np.asarray(sid_tgt, np.int64), (B,)))
+        q_ld = 0
+        if noise is not None:
+            noise = np.ascontiguousarray(noise, dtype=np.float32)
+            if noise.ndim != 3 or noise.shape[0] != B or noise.shape[1] != int(self.cfg["inter_channels"]):
+                raise ValueError("noise must be float32 [B, inter_channels, >= frames]")
+            q_ld = noise.shape[2]
+        frames = np.zeros(B, np.int64)
+        cap = self.convert_frames(lengths) if from_wav else lengths
+        fn = self.lib.vtts_convert if from_wav else self.lib.vtts_convert_spec
+        out = np.zeros((B, max(1, int(np.max(cap))) * self.hop), np.float32)
+        self._check(fn(self.h, _ptr(x), _ptr(lengths), B, ld, _ptr(src), _ptr(tgt), float(noise_scale), _ptr(noise), q_ld,
+                       int(seed), _ptr(out), out.shape[1], _ptr(frames)))
+        return out[:, : int(frames.max()) * self.hop], frames
+
+    def convert_frames(self, wav_lengths):
+        """Frames of the spectrogram of clips of `wav_lengths` samples (center=False after reflect padding by
+        (filter_length - hop_length) / 2 on both sides, mel_processing.py:67-71): len // 256 for the reference configuration."""
+        c = self.cfg
+        n_fft, hop = int(c.get("filter_length", 1024)), int(c.get("hop_length", 256))
+        pad = (n_fft - hop) // 2
+        L = np.asarray(wav_lengths, np.int64)
+        return np.maximum((L + 2 * pad - n_fft) // hop + 1, 0)
+
+    def convert(self, wav, sid_src, sid_tgt, lengths=None, noise_scale=1.0, noise=None, seed=0):
+        """Re-voices clips of speaker `sid_src` as speaker `sid_tgt` (vtts_convert).  wav: float32 [B, L] (or [L]) in [-1, 1],
+        `lengths` the valid samples per row (default: all).  Returns (float32 [B, hop * max(frames)], frames [B]); row b holds
+        hop * frames[b] samples.  noise: optional eps [B, inter_channels, >= frames] of the posterior sample."""
+        wav = np.ascontiguousarray(wav, dtype=np.float32)
+        if wav.ndim == 1:
+            wav = wav[None, :]
+        lengths = np.full(wav.shape[0], wav.shape[1], np.int64) if lengths is None else lengths
+        return self._convert(True, wav, lengths, wav.shape[1], sid_src, sid_tgt, noise_scale, noise, seed)
+
+    def convert_spec(self, spec, sid_src, sid_tgt, lengths=None, noise_scale=1.0, noise=None, seed=0):
+        """Same from the posterior encoder's input features (the reference's `y`): float32 [B, spec_channels, T]."""
+        spec = np.ascontiguousarray(spec, dtype=np.float32)
+        if spec.ndim == 2:
+            spec = spec[None]
+        lengths = np.full(spec.shape[0], spec.shape[2], np.int64) if lengths is None else lengths
+        return self._convert(False, spec, lengths, spec.shape[2], sid_src, sid_tgt, noise_scale, noise, seed)
+
+    def reserve_convert(self, max_frames=1024, batch=1):
+        """Workspace reservation for conversions of up to `batch` clips x `max_frames` frames (see reserve): one conversion
+        from a waveform and one from a spectrogram of that size, so later calls within these bounds move no buffer."""
+        hop = int(self.cfg.get("hop_length", 256))
+        B, F = int(batch), int(max_frames)
+        wav = np.zeros((B, F * hop), np.float32)
+        n = int(self.cfg["n_speakers"])
+        self.convert(wav, 0, min(1, n - 1), noise_scale=0.0)
+        spec = np.zeros((B, int(self.cfg.get("spec_channels", 80)), F), np.float32)
+        self.convert_spec(spec, 0, min(1, n - 1), noise_scale=0.0)
         return F
 
     # ---- streaming (one utterance): flow once, then vocode chunk by chunk

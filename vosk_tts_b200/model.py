@@ -55,7 +55,9 @@ def _reserve_from_env():
 
 
 class Model:
-    def __init__(self, model_path=None, model_name=None, lang=None, device=0, precision=1, session=None):
+    def __init__(self, model_path=None, model_name=None, lang=None, device=0, precision=1, session=None, voice_conversion=False):
+        """voice_conversion: also load the posterior encoder (Synth.convert_audio); needs the training checkpoint (G_*.pth)
+        -- model.onnx is a trace of SynthesizerTrn.infer and holds no enc_q."""
         if model_path is None:
             model_path = self.get_model_path(model_name, lang)
         model_path = Path(model_path)
@@ -71,7 +73,10 @@ class Model:
         cks = sorted(glob.glob(str(model_path / "G_*.pth")), key=lambda p: int(re.sub(r"\D", "", os.path.basename(p)) or 0))
         if (model_path / "model.pth").exists():
             cks.append(str(model_path / "model.pth"))
-        if (model_path / "model.onnx").exists():
+        if (model_path / "model.onnx").exists() and not (voice_conversion and cks):
+            if voice_conversion:
+                raise ValueError("voice conversion needs the training checkpoint (G_*.pth / model.pth) and its training json: "
+                                 "%s holds model.onnx, a trace of SynthesizerTrn.infer without the posterior encoder enc_q" % model_path)
             # the deployed layout (vosk_tts/model.py:46): everything comes out of the graph.  Preferred over a checkpoint
             # lying next to it: model.onnx is what the reference itself would load, and it is not a pickle
             from . import onnx_weights as _onnx
@@ -91,7 +96,8 @@ class Model:
         if not cks:
             raise FileNotFoundError("no weights in %s: expected model.onnx (deployed layout) or G_*.pth / model.pth" % model_path)
         folded = _weights.load_checkpoint(cks[-1])
-        self.onnx = VitsSession(state_dict=folded, cfg=cfg, device=device, precision=precision, reserve=_reserve_from_env())
+        self.onnx = VitsSession(state_dict=folded, cfg=cfg, device=device, precision=precision, reserve=_reserve_from_env(),
+                                voice_conversion=voice_conversion)
 
     def get_model_path(self, model_name, lang):
         for directory in MODEL_DIRS:

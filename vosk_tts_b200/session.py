@@ -17,17 +17,18 @@ from .engine import Engine
 
 
 class VitsSession:
-    def __init__(self, state_dict=None, cfg=None, device=0, seed=0, packed=None, precision=0, reserve=None):
+    def __init__(self, state_dict=None, cfg=None, device=0, seed=0, packed=None, precision=0, reserve=None, voice_conversion=False):
         """state_dict: reference checkpoint `['model']` dict (weight_g/weight_v allowed) or already folded.
         packed: optional (blob, manifest) to skip packing (e.g. received through an NCCL broadcast).
-        reserve: optional (max_tokens, max_frames[, batch]) -- size the workspace for such requests now (Engine.reserve)."""
+        reserve: optional (max_tokens, max_frames[, batch]) -- size the workspace for such requests now (Engine.reserve).
+        voice_conversion: also pack the posterior encoder enc_q (training checkpoints only) so that `convert` works."""
         self.cfg = cfg or _config.DEFAULT_CONFIG
         if precision > 0 and not _weights.tc_supported(self.cfg):
             logging.warning("model widths are not multiples of 64: the tensor-core conv path is unavailable, using the fp32 kernels")
             precision = 0
         if packed is None:
             folded = _weights.fold_weight_norm(state_dict)
-            packed = _weights.pack(folded, self.cfg)
+            packed = _weights.pack(folded, self.cfg, posterior=voice_conversion)
         self.engine = Engine(self.cfg, packed[0], packed[1], device=device, precision=precision)
         self._lock = threading.Lock()
         self._seed = int(seed)
@@ -107,6 +108,20 @@ class VitsSession:
                 stream.close()
             self.last_wav_lengths = np.array([total], np.int64)
             self.last_y_lengths = self.last_wav_lengths // self.engine.hop
+
+    def convert(self, wav, src, tgt, noise=None, noise_scale=1.0):
+        """Voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718; extension, no onnxruntime equivalent):
+        float32 samples [L] in [-1, 1] of speaker `src` -> float32 [hop * frames] of speaker `tgt`, frames = L // 256 for the
+        reference configuration.  noise: optional eps [1, inter_channels, >= frames] of the posterior sample; otherwise
+        Philox with a per-call seed.  noise_scale = 1 is the reference."""
+        wav = np.ascontiguousarray(wav, dtype=np.float32).reshape(-1)
+        with self._lock:
+            self._calls += 1
+            seed = (self._seed * 0x9E3779B97F4A7C15 + self._calls) & 0xFFFFFFFFFFFFFFFF
+            out, frames = self.engine.convert(wav, int(src), int(tgt), noise_scale=noise_scale, noise=noise, seed=seed)
+            self.last_y_lengths = frames
+            self.last_wav_lengths = frames * self.engine.hop
+        return out[0, : int(frames[0]) * self.engine.hop]
 
     def close(self):
         self.engine.close()

@@ -102,6 +102,56 @@ class Synth:
         dur = n / 22050
         logging.info("Real-time factor: %0.2f (infer=%0.2f sec, audio=%0.2f sec)" % (infer_sec / dur if dur > 0 else 0.0, infer_sec, dur))
 
+    def _sample_rate(self):
+        cfg = getattr(self.model.onnx, "cfg", None)
+        if isinstance(cfg, dict) and "sampling_rate" in cfg:
+            return int(cfg["sampling_rate"])
+        return int(self.model.config.get("audio", {}).get("sample_rate", self.model.config.get("data", {}).get("sampling_rate", 22050)))
+
+    def convert_audio(self, audio, src_speaker, tgt_speaker, noise_scale=None, scale=None):
+        """Voice conversion (extension): re-voices `audio` of speaker `src_speaker` as `tgt_speaker` of the same model
+        (SynthesizerTrn.voice_conversion, models.py:1710-1718).  audio: int16 samples (divided by 32768, data_utils.py:77) or
+        float in [-1, 1], at the model's sample rate.  Returns int16 [256 * (len // 256)] for the reference configuration."""
+        audio = np.asarray(audio)
+        if audio.ndim != 1:
+            raise ValueError("convert_audio takes one mono clip ([n] samples)")
+        if audio.dtype == np.int16:
+            wav = audio.astype(np.float32) / 32768.0
+        elif np.issubdtype(audio.dtype, np.floating):
+            wav = audio.astype(np.float32)
+            if wav.size and float(np.abs(wav).max()) > 1.0:
+                raise ValueError("float audio must lie in [-1, 1]")
+        else:
+            raise ValueError("audio must be int16 or float samples, not %s" % audio.dtype)
+        if src_speaker is None or tgt_speaker is None:
+            raise ValueError("voice conversion needs both a source and a target speaker id")
+        inf = self.model.config.get("inference", {})
+        noise_scale = 1.0 if noise_scale is None else noise_scale      # the reference samples the posterior at scale 1 (:841)
+        scale = inf.get("scale", 1.0) if scale is None else scale
+        t0 = time.perf_counter()
+        out = self.model.onnx.convert(wav, int(src_speaker), int(tgt_speaker), noise_scale=noise_scale) * scale
+        out = self.audio_float_to_int16(out)
+        sec = time.perf_counter() - t0
+        dur = out.shape[-1] / self._sample_rate()
+        logging.info("Real-time factor: %0.2f (convert=%0.2f sec, audio=%0.2f sec)" % (sec / dur if dur > 0 else 0.0, sec, dur))
+        return out
+
+    def convert(self, iname, oname, src_speaker, tgt_speaker, noise_scale=None, scale=None):
+        """Reads a mono 16-bit WAV at the model's sample rate (no resampling), writes the converted clip as one."""
+        sr = self._sample_rate()
+        with wave.open(iname, "rb") as f:
+            if f.getnchannels() != 1 or f.getsampwidth() != 2:
+                raise ValueError("%s: expected a mono 16-bit WAV" % iname)
+            if f.getframerate() != sr:
+                raise ValueError("%s is sampled at %d Hz, the model at %d Hz: resample it first" % (iname, f.getframerate(), sr))
+            audio = np.frombuffer(f.readframes(f.getnframes()), dtype="<i2").astype(np.int16)
+        out = self.convert_audio(audio, src_speaker, tgt_speaker, noise_scale, scale)
+        with wave.open(oname, "w") as f:
+            f.setnchannels(1)
+            f.setsampwidth(2)
+            f.setframerate(sr)
+            f.writeframes(out.tobytes())
+
     def synth(self, text, oname, speaker_id=0, noise_level=None, speech_rate=None, duration_noise_level=None, scale=None):
         audio = self.synth_audio(text, speaker_id, noise_level, speech_rate, duration_noise_level, scale)
         with wave.open(oname, "w") as f:

@@ -22,8 +22,9 @@ import zlib
 import torch
 
 
-def _spec(cfg):
-    """Ordered list of (name, shape, kind, scale) for every tensor ``infer`` touches."""
+def _spec(cfg, posterior=False):
+    """Ordered list of (name, shape, kind, scale) for every tensor ``infer`` touches (posterior=True: and the posterior
+    encoder ``enc_q`` that ``voice_conversion`` uses, models.py:1616, 813-842)."""
     H = cfg["hidden_channels"]
     I = cfg["inter_channels"]
     Fc = cfg["filter_channels"]
@@ -143,6 +144,17 @@ def _spec(cfg):
         conv("dec.conv_post", cfg["gen_istft_n_fft"] + 2, ch, 7, wn=True, bias=False, gain=0.25)
     else:
         conv("dec.conv_post", 1, ch, 7, wn=False, bias=False, gain=0.5)     # plain Conv1d (models.py:868)
+
+    # --- posterior encoder (models.py:813-842): pre 1x1, 16-layer WN (kernel 5, weight-normed), proj 1x1
+    if posterior:
+        nq = 16
+        conv("enc_q.pre", H, cfg.get("spec_channels", 80), 1, gain=0.5)
+        for i in range(nq):
+            conv("enc_q.enc.in_layers.%d" % i, 2 * H, H, 5, wn=True, gain=1.0)
+            conv("enc_q.enc.res_skip_layers.%d" % i, 2 * H if i < nq - 1 else H, H, 1, wn=True, gain=0.5)
+        if G > 0:
+            conv("enc_q.enc.cond_layer", 2 * H * nq, G, 1, wn=True, gain=0.5)
+        conv("enc_q.proj", 2 * I, H, 1, gain=0.1)
     return out
 
 
@@ -152,10 +164,11 @@ def _gen(name, seed):
     return g
 
 
-def make_random_checkpoint(cfg, seed=1234):
-    """state_dict (CPU fp32) in checkpoint layout; deterministic for (cfg, seed)."""
+def make_random_checkpoint(cfg, seed=1234, posterior=False):
+    """state_dict (CPU fp32) in checkpoint layout; deterministic for (cfg, seed).  posterior=True adds the ``enc_q.*``
+    tensors (every tensor is seeded by its name, so the others come out the same either way)."""
     sd = {}
-    spec = _spec(cfg)
+    spec = _spec(cfg, posterior)
     for name, shape, kind, arg in spec:
         if kind == "wn_g":
             continue
@@ -185,5 +198,5 @@ def make_random_checkpoint(cfg, seed=1234):
     return sd
 
 
-def param_names(cfg):
-    return [s[0] for s in _spec(cfg)]
+def param_names(cfg, posterior=False):
+    return [s[0] for s in _spec(cfg, posterior)]

@@ -65,6 +65,50 @@ def istft_inverse_basis(n_fft, hop):
     return (inv * hann[None, :]).astype(np.float32)                # [2*cutoff, n_fft]
 
 
+def _hz_to_mel_slaney(f):
+    f = np.asarray(f, np.float64)
+    f_sp, min_log_hz = 200.0 / 3, 1000.0
+    min_log_mel, logstep = min_log_hz / f_sp, np.log(6.4) / 27.0
+    return np.where(f >= min_log_hz, min_log_mel + np.log(np.maximum(f, min_log_hz) / min_log_hz) / logstep, f / f_sp)
+
+
+def _mel_to_hz_slaney(m):
+    m = np.asarray(m, np.float64)
+    f_sp, min_log_hz = 200.0 / 3, 1000.0
+    min_log_mel, logstep = min_log_hz / f_sp, np.log(6.4) / 27.0
+    return np.where(m >= min_log_mel, min_log_hz * np.exp(logstep * (m - min_log_mel)), f_sp * m)
+
+
+def mel_basis(sr, n_fft, n_mels, fmin=0.0, fmax=None):
+    """librosa.filters.mel(sr=, n_fft=, n_mels=, fmin=, fmax=) with its defaults (Slaney mel scale, Slaney area
+    normalisation), as mel_processing.py:85-86 calls it: float32 [n_mels, n_fft // 2 + 1], computed in float64."""
+    fmax = sr / 2.0 if fmax is None else float(fmax)
+    fftfreqs = np.fft.rfftfreq(n_fft, 1.0 / sr)
+    mel_f = _mel_to_hz_slaney(np.linspace(_hz_to_mel_slaney(fmin), _hz_to_mel_slaney(fmax), n_mels + 2))
+    fdiff = np.diff(mel_f)
+    ramps = np.subtract.outer(mel_f, fftfreqs)
+    lower = -ramps[:n_mels] / fdiff[:n_mels, None]
+    upper = ramps[2:] / fdiff[1:, None]
+    weights = np.maximum(0.0, np.minimum(lower, upper))
+    weights *= (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
+    return weights.astype(np.float32)
+
+
+def stft_basis(n_fft):
+    """Windowed DFT basis of the spectrogram front end (csrc/vc.cuh stft_mag_kernel): float32 [n_fft samples][n_fft columns],
+    columns (2k, 2k+1) = hann[n] * (cos, -sin)(2 pi k n / n_fft) of bin k < n_fft/2, except that column 1 (the sine of bin 0,
+    identically zero) holds the cosine of the Nyquist bin.  Periodic Hann window of n_fft (torch.hann_window)."""
+    n = np.arange(n_fft)
+    hann = 0.5 - 0.5 * np.cos(2.0 * np.pi * n / n_fft)
+    k = np.arange(n_fft // 2)
+    ang = 2.0 * np.pi * ((np.outer(n, k) % n_fft) / n_fft)
+    basis = np.zeros((n_fft, n_fft), np.float64)
+    basis[:, 0::2] = np.cos(ang)
+    basis[:, 1::2] = -np.sin(ang)
+    basis[:, 1] = np.where(n % 2 == 0, 1.0, -1.0)
+    return (basis * hann[:, None]).astype(np.float32)
+
+
 def pqmf_synthesis_filter(subbands=4, taps=62, cutoff_ratio=0.15, beta=9.0):
     """PQMF.__init__ (training/vits2/pqmf.py:15-43,63-89): fp32 [subbands, taps+1]."""
     n = np.arange(taps + 1)
@@ -188,8 +232,10 @@ def tc_supported(cfg):
             (cfg["upsample_initial_channel"] >> n_ups) % 64 == 0)
 
 
-def pack(w, cfg, tc=True, precision=None):
+def pack(w, cfg, tc=True, precision=None, posterior=False):
     """w: folded state dict (reference names); returns (blob float32[n], manifest str).
+    posterior=True also packs the posterior encoder enc_q and the spectrogram front end (voice conversion, vtts_convert),
+    after every other tensor: the rest of the blob and its manifest stay what they are without it.
     tc=True also packs split-bf16 copies of the convs for the tensor-core path (precision modes 1 / 2).
     precision: None packs everything (a blob any engine mode can be created from); 0 / 1 / 2 leave out the tensors that
     mode never reads (mode 0: no split-bf16 copies at all; mode 1: none for the text encoder) -- what travels in the
@@ -382,4 +428,50 @@ def pack(w, cfg, tc=True, precision=None):
         P.add("dec.pqmf", bank)
     else:
         P.conv("dec.post", g("dec.conv_post.weight"), None)
+
+    # ---- posterior encoder enc_q (models.py:813-842) + spectrogram front end, for voice conversion
+    if posterior:
+        if "enc_q.pre.weight" not in w:
+            raise ValueError("the state dict has no enc_q (posterior encoder): voice conversion needs a training checkpoint "
+                             "(G_*.pth); model.onnx holds only what SynthesizerTrn.infer uses")
+        if cfg["flow_n_flows"] % 2:
+            raise ValueError("voice conversion needs an even flow_n_flows (the Flip folding of the packed flow holds for both "
+                             "directions only then)")
+        sc = cfg.get("spec_channels", 80)
+        pre = g("enc_q.pre.weight")
+        if pre.shape[1] != sc:
+            raise ValueError("enc_q.pre has %d input channels, the config says spec_channels=%d" % (pre.shape[1], sc))
+        # enc_q.pre runs on the FFMA conv, which takes input channels in multiples of 16: zero-padded (513 -> 528 for a
+        # linear spectrogram; the front end writes zeros into the pad columns)
+        P.conv("encq.pre", np.pad(pre, ((0, 0), (0, (-sc) % 16), (0, 0))), g("enc_q.pre.bias"))
+        il = np.arange(2 * H).reshape(2, H).T.reshape(-1)
+        nq = 16
+        for i in range(nq):
+            src = "enc_q.enc.in_layers.%d" % i
+            P.conv("encq.in%d" % i, g(src + ".weight"), g(src + ".bias"), co_perm=il, need_w=fw)
+            if tc:
+                P.conv_tc("encq.in%d" % i, g(src + ".weight"), co_perm=il)
+            rw, rb = g("enc_q.enc.res_skip_layers.%d.weight" % i), g("enc_q.enc.res_skip_layers.%d.bias" % i)
+            if i < nq - 1:
+                P.conv("encq.rsx%d" % i, rw[:H], rb[:H], need_w=fw)
+                P.conv("encq.rss%d" % i, rw[H:], rb[H:], need_w=fw)
+                if tc:
+                    P.conv_tc("encq.rsx%d" % i, rw[:H])
+                    P.conv_tc("encq.rss%d" % i, rw[H:])
+            else:
+                P.conv("encq.rss%d" % i, rw, rb, need_w=fw)
+                if tc:
+                    P.conv_tc("encq.rss%d" % i, rw)
+        P.conv("encq.proj", g("enc_q.proj.weight"), g("enc_q.proj.bias"), need_w=fw)
+        if tc:
+            P.conv_tc("encq.proj", g("enc_q.proj.weight"))
+        if has_g:
+            cw, cb = g("enc_q.enc.cond_layer.weight")[:, :, 0], g("enc_q.enc.cond_layer.bias")
+            P.add("encq.cond.w", np.concatenate([cw[i * 2 * H:(i + 1) * 2 * H][il] for i in range(nq)], 0))
+            P.add("encq.cond.b", np.concatenate([cb[i * 2 * H:(i + 1) * 2 * H][il] for i in range(nq)], 0))
+        n_fft = cfg.get("filter_length", 1024)
+        P.add("vc.stft", stft_basis(n_fft))
+        if cfg.get("use_mel_posterior_encoder", True):
+            P.add("vc.mel", mel_basis(cfg.get("sampling_rate", 22050), n_fft, cfg.get("n_mel_channels", 80),
+                                      cfg.get("mel_fmin", 0.0), cfg.get("mel_fmax")))
     return P.finish()
