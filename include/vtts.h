@@ -180,6 +180,59 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
 int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host, int T, int use_tc, float* out_host, int iters,
                          float* ms_out);
 
+/* Unit-test hook for the dense conv kernels: ONE grouped launch of the tensor-core conv (conv_tc.cuh) or of the fp32 FFMA
+ * conv (kernels.cuh conv_kernel) through the engine's own launch code, on host tensors.
+ *   B, lens, rmul    utterance b has lens[b] * rmul input rows; utterances are packed as the engine packs them
+ *                    (SEQ_GAP = 8 rows between utterances, scaled by rmul, plus in_extra / out_seq_extra per utterance)
+ *   problems         1..4 problems of the launch (vtts_conv_problem)
+ *   x, x_n           tensor cores: x_planes (2 or 3) bf16 planes [x_n rows][Cin] back to back (hi, lo or hi, mid, lo), shared
+ *                    by every problem; copied into the engine's plane pool, whose rows behind each utterance are then
+ *                    zeroed as at the start of a phase.  FFMA: x_n fp32 values, problem-specific ldx / xoff.
+ *   y, y_n           in/out fp32 buffer every problem with y_on writes to (its prior contents are uploaded, so rows a
+ *                    kernel must not touch keep what the caller wrote, and res == 2 reads it as the residual)
+ *   res, res_n       fp32 residual buffer of the problems with res == 1
+ *   p_out, p_n       in/out split-bf16 output planes, p_planes (2 or 3) planes of p_n elements back to back (hi, lo or
+ *                    hi, mid, lo), written by the problems with planes_on as split(lrelu(out, pl_slope))
+ *   ov               launch-shape overrides for this call only (VTTS_CONV_KEEP: the engine's setting), or NULL
+ *   report           out: the launch that ran
+ * Malformed specs (channel counts the kernel cannot take, more than 4 problems, mixed plane counts, halos the packed layout
+ * or the FFMA tile cannot hold, buffers too small for the rows a problem writes or reads) return VTTS_ERR_INVALID before
+ * anything is launched.  Tensor cores need a precision >= 1 engine. */
+#define VTTS_CONV_KEEP (-1000000)
+typedef struct vtts_conv_problem {
+  int Cin, Cout, k, dil, pad;
+  int out_mul, out_add;         /* output row of input position t: t * out_mul + out_add (polyphase ConvTranspose1d) */
+  int in_extra, out_seq_extra;  /* extra logical input rows / extra output rows per utterance */
+  int epi;                      /* 1 ReLU, 2 gate (tanh(even) * sigmoid(odd) channel pairs), 4 tanh (FFMA only) */
+  float alpha, pl_slope;        /* out = act(conv + bias + cond) * alpha + res; planes of lrelu(out, pl_slope) */
+  const uint16_t *w_hi, *w_mid, *w_lo;  /* tensor cores: bf16 [k][Cout][Cin] (w_mid for 3-plane launches only) */
+  const float* w;               /* FFMA: [k][Cin][ldw], ldw = (Cout + 3) / 4 * 4 */
+  const float* bias;            /* [Cout] (FFMA: [ldw]) */
+  const float* cond;            /* optional [B][cond_ld], added to the bias of utterance b */
+  int cond_ld;
+  int y_on, ldy, yoff;
+  int res, ldr, roff;           /* 0 none, 1 the res buffer, 2 the y buffer itself (in place) */
+  int planes_on, ldp, poff;     /* poff: tensor cores only */
+  int ldx, xoff, reflect, pro;  /* FFMA input: row pitch / column offset, ReflectionPad1d((1,0)) row map, 1 = leaky-ReLU prologue */
+  float slope;
+} vtts_conv_problem;
+typedef struct vtts_conv_overrides {
+  int tc_bn, tc_split, tc_tall, tc_mc, tc_persist, tc_wmc, tc_min_steps, conv_max_s, conv_min_g, conv_max_g, conv_big_g;
+} vtts_conv_overrides;
+typedef struct vtts_conv_report {
+  int use_tc;
+  int bn, split, tall, cn, wmc, persist, np, ast, wst;
+  int image;                    /* 0 conv_tc_kernel<BN, false>, 1 conv_tc_kernel<BN, true>, 2 conv_tc_persist_kernel<BN> */
+  int S, G;                     /* FFMA: cluster split-K and thread groups */
+  int grid_x, grid_y, grid_z;
+} vtts_conv_report;
+int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul, int n_problems, const vtts_conv_problem* problems,
+                    const void* x, size_t x_n, int x_planes, float* y, size_t y_n, const float* res, size_t res_n, uint16_t* p_out,
+                    size_t p_n, int p_planes, const vtts_conv_overrides* ov, vtts_conv_report* report);
+/* Launch-shape log of the dense conv launches: mode 1 clears and starts it, 0 stops it, 2 copies up to max_n entries (one
+ * per launch the host enqueued since it was started; graph replays enqueue none) and sets *n_out. */
+int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_n, int* n_out);
+
 /* Voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718): re-voices recordings of speaker sid_src as
  * speaker sid_tgt of the same multi-speaker model.  One call = spectrogram front end, posterior encoder enc_q (g_src),
  * flow forward (g_src), flow reverse (g_tgt), decoder (g_tgt); no host synchronisation inside (the frame counts follow

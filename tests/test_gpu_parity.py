@@ -393,16 +393,18 @@ def test_bucketed_graphs_serve_unseen_utterances(engine, cfg):
                                  {"VTTS_CONV_AUTOG": "0"}, {"VTTS_MRF_BRANCH": "1"}, {"VTTS_BUCKETS": "0"}, {"VTTS_ATTN_TC": "0"},
                                  {"VTTS_TC_PERSIST": "2", "VTTS_TC_SPLIT": "1"}, {"VTTS_TC_PERSIST": "2", "VTTS_TC_SPLIT": "1", "VTTS_TC_TALL": "-1"},
                                  {"VTTS_TC_PERSIST": "2", "VTTS_TC_SPLIT": "1", "VTTS_TC_WMC": "1"},
-                                 {"VTTS_TC_PERSIST": "2", "VTTS_TC_SPLIT": "1", "VTTS_TC_COAL": "1", "VTTS_TC_BN": "128"}, {"VTTS_TC_SPLIT": "1", "VTTS_TC_COAL": "1"}],
+                                 {"VTTS_TC_PERSIST": "2", "VTTS_TC_SPLIT": "1", "VTTS_TC_BN": "128"}, {"VTTS_TC_SPLIT": "1", "VTTS_TC_MULTICAST": "2"}],
                          ids=["tc-128-wide-tiles", "tc-tall-activation-tiles", "no-programmatic-dependent-launch", "ffma-no-cluster-4-groups",
                               "attention-4-rows-per-warp", "tc-tma-multicast-cluster", "tc-no-split-k", "tc-split-k-pairs",
                               "tc-split-k-8-ways", "tc-128-wide-split-k-8-ways", "tc-64-wide-only", "attention-without-split-kv",
                               "ffma-single-thread-group", "mrf-chains-on-separate-streams", "exact-sizes-no-length-buckets",
                               "ffma-attention-in-the-flow", "tc-persistent-tile-loop-tall", "tc-persistent-tile-loop-per-tap-tiles",
-                              "tc-persistent-weight-multicast-pairs", "tc-persistent-coalesced-epilogue-128-wide", "tc-coalesced-epilogue"])
-def test_alternative_kernel_configurations_match_golden(packed, cfg, env):
+                              "tc-persistent-weight-multicast-pairs", "tc-persistent-tile-loop-128-wide", "tc-tma-multicast-pairs-no-split-k"])
+def test_alternative_kernel_configurations_match_golden(packed, cfg, env, default_conv_shapes):
     """The tuning switches select different tilings / launch modes of the same kernels (128-wide tensor-core tiles are what
-    batched calls use automatically); each must still reproduce the reference fixture."""
+    batched calls use automatically); each must still reproduce the reference fixture.  A switch of the dense conv launches
+    (VTTS_TC_* / VTTS_CONV_*) must also change the launch of at least one conv of these utterances -- otherwise the case
+    would silently re-run the default configuration."""
     import os
     from vosk_tts_b200.engine import Engine
     old = {k: os.environ.get(k) for k in env}
@@ -415,6 +417,16 @@ def test_alternative_kernel_configurations_match_golden(packed, cfg, env):
                 os.environ.pop(k, None)
             else:
                 os.environ[k] = v
+    shapes = _golden_pair_conv_shapes(e)
+    if any(k.startswith(("VTTS_TC_", "VTTS_CONV_")) for k in env):
+        assert shapes != default_conv_shapes, "the switch changed no conv launch"
+    e.close()
+
+
+def _golden_pair_conv_shapes(e):
+    """Runs t128_sid2 and t17_sid2 (eager, capture, replay) against their fixtures; returns the conv launch shapes in launch
+    order (an ordered list: the same shape may be right for one conv and a change for another)."""
+    e.conv_log(1)
     for name in ("t128_sid2", "t17_sid2"):
         g = load_golden(name)
         c = _case(g, 0)
@@ -424,7 +436,18 @@ def test_alternative_kernel_configurations_match_golden(packed, cfg, env):
             assert np.array_equal(dur[0], c["w_ceil"])
             wav = e.synthesize(ylen, c["eps_z"][None])
             assert np.abs(wav[0, : c["Ty"] * 256] - c["wav"]).max() < WAV_TIGHT
+    shapes = [tuple(sorted(r.items())) for r in e.conv_log(2)]
+    e.conv_log(0)
+    return shapes
+
+
+@pytest.fixture(scope="module")
+def default_conv_shapes(packed, cfg):
+    from vosk_tts_b200.engine import Engine
+    e = Engine(cfg, packed[0], packed[1], device=0, precision=1)
+    shapes = _golden_pair_conv_shapes(e)
     e.close()
+    return shapes
 
 
 def test_reserved_workspace_keeps_bucket_graphs_valid(packed, cfg):

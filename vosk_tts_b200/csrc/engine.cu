@@ -307,6 +307,14 @@ struct vtts_engine {
   bool capture_on_first = true;
   bool capturing = false, use_graphs = true, last_graphed = false, use_pdl = true;    // programmatic dependent launch (VTTS_PDL=0 turns it off)
   int conv_max_s = 8, conv_target = 120, conv_max_g = 4, conv_big_g = 1, tc_tall = 0, tc_baseoff = 0, tc_bn = 0, attn_rows = 0, tc_mc = 0, tc_split = 0, conv_min_g = 1, tc_min_steps = 2, conv_auto_g = 4, attn_split = 1, tc_persist = 1, tc_persist_min = 1, n_sm = 132, tc_dbgskip = 0, tc_wmc = 0;
+  // shape of the last dense conv launch (vtts_debug_conv) and, while log_conv is set, of every one (vtts_debug_conv_log)
+  vtts_conv_report last_conv{};
+  bool log_conv = false;
+  std::vector<vtts_conv_report> conv_log;
+  void note_conv(const vtts_conv_report& r) {
+    last_conv = r;
+    if (log_conv) conv_log.push_back(r);
+  }
   int tc_cluster_cap[2][3] = {{0, 0, 0}, {0, 0, 0}};   // co-resident clusters of 2/4/8 conv_tc CTAs, [BN 64/128][log2(S)-1]   // multicast measured slower (see DESIGN.md 4.2)   // tuning knobs (env VTTS_CONV_MAXS / _TARGET / _MAXG)
   cudaEvent_t ev[8] = {};
   cudaStream_t side[3] = {};               // branch streams of the decoder's independent resblock chains (forked / joined with events)
@@ -982,6 +990,15 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     grid = dim3((unsigned)n_sm, 1, 1);
   }
   REQUIRE(tb.persist || wmc == 1, VTTS_ERR_INVALID, "tensor-core conv: weight multicast planned for a launch that is not persistent");
+  const bool single_wave_image = split > 1 || tb.wpre;
+  const bool dyn_image = tb.np != 2 || tb.ast != (BN == 128 ? tc_ast<128>() : tc_ast<64>()) || tb.wst != (BN == 128 ? tc_wst<128>() : tc_wst<64>());
+  {
+    vtts_conv_report r{};
+    r.use_tc = 1; r.bn = BN; r.split = split; r.tall = tb.tall; r.cn = cn; r.wmc = tb.wmc; r.persist = tb.persist; r.np = tb.np;
+    r.ast = tb.ast; r.wst = tb.wst; r.image = single_wave_image ? (dyn_image ? 1 : 0) : 2;
+    r.grid_x = (int)grid.x; r.grid_y = (int)grid.y; r.grid_z = (int)grid.z;
+    note_conv(r);
+  }
   if (profiling) {
     if (tc_prof_used + 2 > tc_prof_ev.size()) {
       tc_prof_ev.resize(tc_prof_used + 2);
@@ -1015,9 +1032,8 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     lc.attrs = at; lc.numAttrs = na;
     // single-wave launches all use the split-capable instantiation (also with split == 1): alternating between two kernel
     // images costs instruction-cache misses on every launch of a latency-bound chain
-    if (split > 1 || tb.wpre) {
-      const bool dyn = tb.np != 2 || tb.ast != (BN == 128 ? tc_ast<128>() : tc_ast<64>()) || tb.wst != (BN == 128 ? tc_wst<128>() : tc_wst<64>());
-      if (dyn) {
+    if (single_wave_image) {
+      if (dyn_image) {
         if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, true>, tb, lens, offs));
         else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, true>, tb, lens, offs));
       } else {                    // the default launches carry the descriptor without the third-plane tensor maps
@@ -1443,6 +1459,12 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
   const std::vector<int>& hl = hl_true;      // (profiling FLOP count below)
   dim3 grid(((maxL + CV_TT - 1) / CV_TT) * S, (maxCout + CV_TC - 1) / CV_TC, nB * cb.n);
   if (grid.x == 0) return;
+  {
+    vtts_conv_report r{};
+    r.S = S; r.G = G;
+    r.grid_x = (int)grid.x; r.grid_y = (int)grid.y; r.grid_z = (int)grid.z;
+    note_conv(r);
+  }
   if (profiling) {
     if (prof_used + 2 > prof_ev.size()) {
       prof_ev.resize(prof_used + 2);
@@ -3057,6 +3079,220 @@ int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host
     }
     cudaFree(dl); cudaFree(dq); cudaFree(dout);
     h->B = B0; h->h_frm_len = fl0; h->h_tok_len = tl0; h->maxFrm = mf0; h->v_frm_len = vf0; h->v_tok_len = vt0;
+  });
+}
+
+// Unit-test hook of the dense conv kernels (include/vtts.h): one grouped launch through launch_tc / launch_conv on host tensors.
+int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul, int n_problems, const vtts_conv_problem* problems,
+                    const void* x, size_t x_n, int x_planes, float* y, size_t y_n, const float* res, size_t res_n, uint16_t* p_out,
+                    size_t p_n, int p_planes, const vtts_conv_overrides* ov, vtts_conv_report* report) {
+  return guarded(h, [&] {
+    REQUIRE(lens && problems && x && B >= 1 && rmul >= 1, VTTS_ERR_INVALID, "debug_conv: missing lengths, problems or input");
+    REQUIRE(n_problems >= 1 && n_problems <= TC_MAXP && n_problems <= CV_MAXP, VTTS_ERR_INVALID, "debug_conv: 1..4 problems per launch");
+    REQUIRE(!use_tc || h->encode_tiled, VTTS_ERR_INVALID, "debug_conv: the tensor-core conv needs a precision >= 1 engine");
+    std::vector<long> off(B + 1, 0);
+    int maxLen = 0;
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(lens[b] >= 1, VTTS_ERR_INVALID, "debug_conv: lengths must be >= 1");
+      off[b + 1] = off[b] + lens[b] + (b + 1 < B ? SEQ_GAP : 0);
+      maxLen = std::max(maxLen, lens[b]);
+    }
+    const long gap = (long)SEQ_GAP * rmul;
+    const vtts_conv_problem& P0 = problems[0];
+    if (use_tc) {
+      REQUIRE(x_planes == 2 || x_planes == 3, VTTS_ERR_INVALID, "debug_conv: the tensor-core input has 2 or 3 planes");
+    }
+    bool any_planes = false;
+    for (int i = 0; i < n_problems; ++i) {
+      const vtts_conv_problem& q = problems[i];
+      REQUIRE(q.Cin > 0 && q.Cout > 0 && q.k >= 1 && q.dil >= 1 && q.pad >= 0 && q.out_mul >= 1 && q.out_add >= 0 && q.in_extra >= 0 &&
+                  q.out_seq_extra >= 0 && q.bias,
+              VTTS_ERR_INVALID, "debug_conv: bad problem geometry or missing bias");
+      REQUIRE((q.epi & ~(use_tc ? (TCE_RELU | TCE_GATE) : (EPI_RELU | EPI_GATE | EPI_TANH))) == 0, VTTS_ERR_INVALID, "debug_conv: unknown epilogue");
+      REQUIRE(!(q.epi & EPI_GATE) || q.Cout % 2 == 0, VTTS_ERR_INVALID, "debug_conv: the gate needs an even Cout");
+      REQUIRE(!q.cond || q.cond_ld >= q.Cout, VTTS_ERR_INVALID, "debug_conv: cond_ld < Cout");
+      REQUIRE(q.res >= 0 && q.res <= 2 && (q.res != 1 || res) && (q.res != 2 || q.y_on), VTTS_ERR_INVALID, "debug_conv: bad residual");
+      REQUIRE(q.y_on || q.planes_on, VTTS_ERR_INVALID, "debug_conv: a problem must write y or planes");
+      if (q.planes_on) {
+        REQUIRE(p_out && (p_planes == 2 || p_planes == 3) && q.ldp > 0 && q.poff >= 0, VTTS_ERR_INVALID, "debug_conv: bad output planes");
+        any_planes = true;
+      }
+      if (q.y_on) REQUIRE(y && q.ldy > 0 && q.yoff >= 0, VTTS_ERR_INVALID, "debug_conv: bad y");
+      if (use_tc) {
+        REQUIRE(q.Cin % TC_BK == 0 && q.Cin == P0.Cin && q.in_extra == P0.in_extra, VTTS_ERR_INVALID,
+                "debug_conv: tensor-core problems share one input of Cin (a multiple of 64) channels and in_extra rows");
+        REQUIRE(q.w_hi && q.w_lo && (x_planes == 3) == (q.w_mid != nullptr), VTTS_ERR_INVALID,
+                "debug_conv: mixed plane counts (every problem's weights must have as many planes as the input)");
+        REQUIRE(!q.reflect && !q.pro && q.ldx == 0 && q.xoff == 0, VTTS_ERR_INVALID, "debug_conv: reflect / prologue / ldx are FFMA-only");
+        REQUIRE(!q.planes_on || q.ldp >= q.poff + ((q.epi & TCE_GATE) ? q.Cout / 2 : q.Cout), VTTS_ERR_INVALID, "debug_conv: ldp too small");
+      } else {
+        REQUIRE(q.Cin % CV_CK == 0, VTTS_ERR_INVALID, "debug_conv: FFMA input channels must be a multiple of 16");
+        REQUIRE(q.w && q.y_on && q.poff == 0 && q.pro >= 0 && q.pro <= 1, VTTS_ERR_INVALID, "debug_conv: the FFMA conv writes y, takes w and no poff");
+        REQUIRE(q.ldx % 4 == 0 && q.xoff % 4 == 0 && q.ldx >= q.xoff + q.Cin, VTTS_ERR_INVALID, "debug_conv: FFMA input rows are read as float4");
+        REQUIRE(CV_TT + (q.k - 1) * q.dil <= 32 * CV_XR, VTTS_ERR_INVALID, "debug_conv: halo larger than the FFMA tile");
+        REQUIRE(!q.reflect || (q.in_extra == 1 && q.pad == 0), VTTS_ERR_INVALID, "debug_conv: reflect maps ReflectionPad1d((1,0)) (in_extra 1, pad 0)");
+      }
+    }
+    // rows written per utterance must fit the buffers; inputs must cover every utterance's rows
+    auto check_rows = [&](size_t n, int ld, int col0, int ncol, const vtts_conv_problem& q, const char* what) {
+      for (int b = 0; b < B; ++b) {
+        const long L = (long)lens[b] * rmul + q.in_extra;
+        const long last = off[b] * rmul * q.out_mul + (long)b * q.out_seq_extra + (L - 1) * q.out_mul + q.out_add;
+        REQUIRE((size_t)(last * ld + col0 + ncol) <= n, VTTS_ERR_INVALID, std::string("debug_conv: ") + what + " buffer too small");
+      }
+    };
+    for (int i = 0; i < n_problems; ++i) {
+      const vtts_conv_problem& q = problems[i];
+      const int ncol = (q.epi & EPI_GATE) ? q.Cout / 2 : q.Cout;
+      if (q.y_on) check_rows(y_n, q.ldy, q.yoff, ncol, q, "y");
+      if (q.res == 1) check_rows(res_n, q.ldr, q.roff, ncol, q, "res");
+      if (q.res == 2) check_rows(y_n, q.ldr, q.roff, ncol, q, "residual (y)");
+      if (q.planes_on) check_rows(p_n, q.ldp, q.poff, ncol, q, "planes");
+      if (!use_tc) {
+        for (int b = 0; b < B; ++b) {
+          const long Lp = (long)lens[b] * rmul;
+          REQUIRE(!q.reflect || Lp >= 2, VTTS_ERR_INVALID, "debug_conv: reflect needs >= 2 input rows per utterance");
+          const long lastrow = off[b] * rmul + (q.reflect ? Lp - 1 : Lp + q.in_extra - 1);
+          REQUIRE((size_t)(lastrow * q.ldx + q.xoff + q.Cin) <= x_n, VTTS_ERR_INVALID, "debug_conv: x buffer too small");
+        }
+      }
+    }
+    // tensor cores: the input planes as a phase holds them (rows behind each utterance read as zero through the zeroed tails,
+    // TMA's out-of-bounds fill in front of the first and behind the last row) -- the halo must stay inside that
+    const int extra = P0.in_extra;
+    const long end_last = (off[B - 1] + lens[B - 1]) * rmul + (long)B * extra;
+    const long units = use_tc ? std::max<long>(off[B], ((long)x_n - (long)B * extra + rmul - 1) / rmul) : 0;
+    const long rows_cap = units * rmul + (long)B * extra;
+    if (use_tc) {
+      REQUIRE((long)x_n >= end_last, VTTS_ERR_INVALID, "debug_conv: x planes have fewer rows than the packed utterances");
+      const long inner = gap <= 2 * ZT_ROWS ? gap : ZT_ROWS;          // zeroed rows between two utterances (zero_tails_kernel)
+      for (int i = 0; i < n_problems; ++i) {
+        const vtts_conv_problem& q = problems[i];
+        const long left = q.pad, right = (long)(q.k - 1) * q.dil - q.pad;
+        REQUIRE(B == 1 || (left <= inner && right <= inner), VTTS_ERR_INVALID, "debug_conv: conv halo wider than the zeroed gap between utterances");
+        REQUIRE(right <= ZT_ROWS || rows_cap <= end_last + ZT_ROWS, VTTS_ERR_INVALID, "debug_conv: conv halo reaches rows behind the zeroed tail");
+      }
+    }
+    // ---- per-call engine state the launch code reads, restored on every exit
+    struct Saved {
+      vtts_engine* h;
+      int B, maxFrm, knobs[11];
+      std::vector<int> fl, fo, vf;
+      int* kp[11];
+      explicit Saved(vtts_engine* e) : h(e), B(e->B), maxFrm(e->maxFrm), fl(e->h_frm_len), fo(e->h_frm_off), vf(e->v_frm_len),
+          kp{&e->tc_bn, &e->tc_split, &e->tc_tall, &e->tc_mc, &e->tc_persist, &e->tc_wmc, &e->tc_min_steps, &e->conv_max_s,
+             &e->conv_min_g, &e->conv_max_g, &e->conv_big_g} {
+        for (int i = 0; i < 11; ++i) knobs[i] = *kp[i];
+      }
+      ~Saved() {
+        h->B = B; h->maxFrm = maxFrm; h->h_frm_len = fl; h->h_frm_off = fo; h->v_frm_len = vf;
+        for (int i = 0; i < 11; ++i) *kp[i] = knobs[i];
+      }
+    } saved(h);
+    if (ov) {
+      const int v[11] = {ov->tc_bn, ov->tc_split, ov->tc_tall, ov->tc_mc, ov->tc_persist, ov->tc_wmc, ov->tc_min_steps, ov->conv_max_s,
+                         ov->conv_min_g, ov->conv_max_g, ov->conv_big_g};
+      for (int i = 0; i < 11; ++i) if (v[i] != VTTS_CONV_KEEP) *saved.kp[i] = v[i];
+    }
+    h->B = B; h->maxFrm = maxLen;
+    h->h_frm_len.assign(lens, lens + B);
+    h->h_frm_off.assign(off.begin(), off.end());
+    h->v_frm_len = h->h_frm_len;                  // the heuristics see this call's lengths
+    // ---- device copies (freed on every exit)
+    struct DevBufs {
+      std::vector<void*> p;
+      ~DevBufs() { for (void* q : p) cudaFree(q); }
+      void* up(const void* src, size_t bytes, cudaStream_t s) {
+        void* d = nullptr;
+        CK(cudaMalloc(&d, std::max<size_t>(bytes, 16)));
+        p.push_back(d);
+        if (src) CK(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, s));
+        return d;
+      }
+    } dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    std::vector<int> lo(2 * B + 1);
+    for (int b = 0; b < B; ++b) lo[b] = lens[b];
+    for (int b = 0; b <= B; ++b) lo[B + b] = (int)off[b];
+    int* dl = static_cast<int*>(dev.up(lo.data(), lo.size() * sizeof(int), st));
+    const int* dlens = dl;
+    const int* doffs = dl + B;
+    float* dy = y ? static_cast<float*>(dev.up(y, y_n * sizeof(float), st)) : nullptr;
+    const float* dres = res ? static_cast<const float*>(dev.up(res, res_n * sizeof(float), st)) : nullptr;
+    __nv_bfloat16* dp = any_planes ? static_cast<__nv_bfloat16*>(dev.up(p_out, (size_t)p_planes * p_n * 2, st)) : nullptr;
+    __nv_bfloat16 *dp_hi = dp, *dp_mid = (dp && p_planes == 3) ? dp + p_n : nullptr, *dp_lo = dp ? dp + (p_planes - 1) * p_n : nullptr;
+    auto cond_of = [&](const vtts_conv_problem& q) {
+      return q.cond ? static_cast<const float*>(dev.up(q.cond, (size_t)B * q.cond_ld * sizeof(float), st)) : nullptr;
+    };
+    if (use_tc) {
+      const int Cin = P0.Cin;
+      h->begin_planes();
+      Planes in = h->planes(57, units, rmul, Cin, extra, x_planes == 3);
+      const uint16_t* xs = static_cast<const uint16_t*>(x);
+      __nv_bfloat16* dst[3] = {in.hi, x_planes == 3 ? in.mid : in.lo, in.lo};
+      for (int pl = 0; pl < x_planes; ++pl)
+        CK(cudaMemcpyAsync(dst[pl], xs + (size_t)pl * x_n * Cin, x_n * Cin * 2, cudaMemcpyHostToDevice, st));
+      h->flush_tails(dlens, doffs);
+      std::vector<TcSpec> ps;
+      for (int i = 0; i < n_problems; ++i) {
+        const vtts_conv_problem& q = problems[i];
+        const size_t wn = (size_t)q.k * q.Cout * q.Cin;
+        TcSpec s;
+        s.in = in;
+        s.w.hi = static_cast<const __nv_bfloat16*>(dev.up(q.w_hi, wn * 2, st));
+        s.w.lo = static_cast<const __nv_bfloat16*>(dev.up(q.w_lo, wn * 2, st));
+        if (q.w_mid) s.w.mid = static_cast<const __nv_bfloat16*>(dev.up(q.w_mid, wn * 2, st));
+        s.bias = static_cast<const float*>(dev.up(q.bias, (size_t)q.Cout * sizeof(float), st));
+        s.Cin = q.Cin; s.Cout = q.Cout; s.k = q.k; s.dil = q.dil; s.pad = q.pad;
+        s.y = q.y_on ? dy : nullptr; s.ldy = q.ldy; s.yoff = q.yoff;
+        s.res = q.res == 1 ? dres : (q.res == 2 ? dy : nullptr); s.ldr = q.ldr; s.roff = q.roff;
+        if (q.planes_on) { s.out.hi = dp_hi; s.out.lo = dp_lo; s.out.mid = dp_mid; s.out.C = q.ldp; }
+        s.pl_slope = q.pl_slope; s.poff = q.poff;
+        s.out_mul = q.out_mul; s.out_add = q.out_add; s.in_extra = q.in_extra; s.out_seq_extra = q.out_seq_extra;
+        s.epi = q.epi; s.alpha = q.alpha;
+        s.cond = cond_of(q); s.cond_ld = q.cond_ld;
+        ps.push_back(s);
+      }
+      h->launch_tc(ps, rmul, dlens, doffs, maxLen, B);
+    } else {
+      const float* dx = static_cast<const float*>(dev.up(x, x_n * sizeof(float), st));
+      std::vector<ConvP> ps;
+      for (int i = 0; i < n_problems; ++i) {
+        const vtts_conv_problem& q = problems[i];
+        ConvW W;
+        W.Cin = q.Cin; W.Cout = q.Cout; W.k = q.k; W.ldw = (q.Cout + 3) / 4 * 4;
+        W.w = static_cast<const float*>(dev.up(q.w, (size_t)q.k * q.Cin * W.ldw * sizeof(float), st));
+        W.b = static_cast<const float*>(dev.up(q.bias, (size_t)W.ldw * sizeof(float), st));
+        ConvP p = mk(W, dx, q.ldx, q.xoff, dy, q.ldy, q.yoff, q.dil, q.pad);
+        p.cond = cond_of(q); p.cond_ld = q.cond_ld;
+        p.res = q.res == 1 ? dres : (q.res == 2 ? dy : nullptr); p.ldr = q.ldr; p.roff = q.roff;
+        p.in_extra = q.in_extra; p.reflect = q.reflect; p.out_mul = q.out_mul; p.out_add = q.out_add; p.out_seq_extra = q.out_seq_extra;
+        p.pro = q.pro; p.slope = q.slope; p.epi = q.epi; p.alpha = q.alpha;
+        if (q.planes_on) { p.p_hi = dp_hi; p.p_lo = dp_lo; p.p_mid = dp_mid; p.ldp = q.ldp; }
+        p.pl_slope = q.pl_slope;
+        ps.push_back(p);
+      }
+      h->launch_conv(ps, rmul, dlens, doffs, maxLen, B);
+    }
+    CK(cudaStreamSynchronize(st));
+    if (y) CK(cudaMemcpy(y, dy, y_n * sizeof(float), cudaMemcpyDeviceToHost));
+    if (dp) CK(cudaMemcpy(p_out, dp, (size_t)p_planes * p_n * 2, cudaMemcpyDeviceToHost));
+    if (report) *report = h->last_conv;
+  });
+}
+
+int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_n, int* n_out) {
+  return guarded(h, [&] {
+    REQUIRE(mode >= 0 && mode <= 2, VTTS_ERR_INVALID, "debug_conv_log: mode 0, 1 or 2");
+    if (mode == 1) { h->conv_log.clear(); h->log_conv = true; }
+    else if (mode == 0) h->log_conv = false;
+    else {
+      REQUIRE(out && n_out && max_n >= 0, VTTS_ERR_INVALID, "debug_conv_log: missing output");
+      const int n = std::min<int>(max_n, (int)h->conv_log.size());
+      std::copy(h->conv_log.begin(), h->conv_log.begin() + n, out);
+      *n_out = n;
+    }
   });
 }
 

@@ -48,7 +48,36 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_profile", "vtts_profile_read", "vtts_set_graphs", "vtts_graph_replays",
            "vtts_profile_read_tc", "vtts_timeline", "vtts_infer", "vtts_infer_dev",
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
-           "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec"]
+           "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
+           "vtts_debug_conv_log"]
+
+CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
+
+
+class ConvProblem(C.Structure):
+    """vtts_conv_problem (include/vtts.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("Cin", "Cout", "k", "dil", "pad", "out_mul", "out_add", "in_extra", "out_seq_extra",
+                                         "epi")] + \
+        [("alpha", C.c_float), ("pl_slope", C.c_float), ("w_hi", C.c_void_p), ("w_mid", C.c_void_p), ("w_lo", C.c_void_p),
+         ("w", C.c_void_p), ("bias", C.c_void_p), ("cond", C.c_void_p), ("cond_ld", C.c_int32)] + \
+        [(n, C.c_int32) for n in ("y_on", "ldy", "yoff", "res", "ldr", "roff", "planes_on", "ldp", "poff", "ldx", "xoff",
+                                  "reflect", "pro")] + [("slope", C.c_float)]
+
+
+CONV_OVERRIDES = ("tc_bn", "tc_split", "tc_tall", "tc_mc", "tc_persist", "tc_wmc", "tc_min_steps", "conv_max_s", "conv_min_g",
+                  "conv_max_g", "conv_big_g")
+
+
+class ConvOverrides(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in CONV_OVERRIDES]
+
+
+class ConvReport(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("use_tc", "bn", "split", "tall", "cn", "wmc", "persist", "np", "ast", "wst", "image",
+                                         "S", "G", "grid_x", "grid_y", "grid_z")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
 class _Missing:
@@ -144,6 +173,11 @@ def load_library(build_if_missing=True):
     lib.vtts_profile_read_tc.restype = i32
     lib.vtts_debug_attention.argtypes = [vp, C.c_char_p, vp, i32, i32, vp, i32, fp]
     lib.vtts_debug_attention.restype = i32
+    lib.vtts_debug_conv.argtypes = [vp, i32, i32, vp, i32, i32, C.POINTER(ConvProblem), vp, C.c_size_t, i32, vp, C.c_size_t, vp,
+                                    C.c_size_t, vp, C.c_size_t, i32, C.POINTER(ConvOverrides), C.POINTER(ConvReport)]
+    lib.vtts_debug_conv.restype = i32
+    lib.vtts_debug_conv_log.argtypes = [vp, i32, C.POINTER(ConvReport), i32, C.POINTER(C.c_int)]
+    lib.vtts_debug_conv_log.restype = i32
     lib.vtts_speculation_stats.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.vtts_speculation_stats.restype = i32
     lib.vtts_host_timings.argtypes = [vp, C.POINTER(C.c_double), i32]
@@ -538,6 +572,66 @@ class Engine:
         ms = C.c_float(0.0)
         self._check(self.lib.vtts_debug_attention(self.h, layer.encode(), _ptr(qkv), T, int(use_tc), _ptr(out), int(iters), C.byref(ms)))
         return out, (float(ms.value) if iters > 0 else None)
+
+    def debug_conv(self, use_tc, lens, rmul, problems, x, y=None, res=None, planes=None, overrides=None):
+        """One grouped launch of the tensor-core (use_tc) or FFMA conv kernel on host tensors (vtts_debug_conv).
+        problems: list of dicts with the vtts_conv_problem fields; array fields (w_hi / w_mid / w_lo uint16 [k][Cout][Cin],
+        w float32 [k][Cin][ldw], bias, cond) are numpy arrays.  x: tensor cores uint16 [np][rows][Cin] planes, FFMA float32
+        (any shape, flat layout).  y / res: float32 buffers (y is in/out), planes: uint16 [2 or 3][n] (in/out).
+        overrides: dict of CONV_OVERRIDES names.  Returns (y, planes, launch report dict)."""
+        keep = []
+
+        def arr(a, dt):
+            a = np.ascontiguousarray(a, dtype=dt)
+            keep.append(a)
+            return a
+
+        ps = (ConvProblem * len(problems))()
+        for i, q in enumerate(problems):
+            p = ps[i]
+            p.out_mul, p.alpha, p.pl_slope = 1, 1.0, 1.0
+            for key, v in q.items():
+                if key in ("w_hi", "w_mid", "w_lo"):
+                    setattr(p, key, None if v is None else arr(v, np.uint16).ctypes.data)
+                elif key in ("w", "bias", "cond"):
+                    setattr(p, key, None if v is None else arr(v, np.float32).ctypes.data)
+                else:
+                    setattr(p, key, v)
+        if use_tc:
+            x = arr(x, np.uint16)
+            x_planes, x_n = x.shape[0], x.shape[1]
+        else:
+            x = arr(x, np.float32)
+            x_planes, x_n = 0, x.size
+        y = None if y is None else np.ascontiguousarray(y, dtype=np.float32).copy()
+        res = None if res is None else arr(res, np.float32)
+        planes = None if planes is None else np.ascontiguousarray(planes, dtype=np.uint16).copy()
+        ov = None
+        if overrides:
+            ov = ConvOverrides(*[CONV_KEEP] * len(CONV_OVERRIDES))
+            for key, v in overrides.items():
+                if key not in CONV_OVERRIDES:
+                    raise ValueError("unknown conv launch override %r" % key)
+                setattr(ov, key, int(v))
+        rep = ConvReport()
+        lens = arr(lens, np.int32)
+        self._check(self.lib.vtts_debug_conv(
+            self.h, int(bool(use_tc)), lens.size, _ptr(lens), int(rmul), len(problems), ps, _ptr(x), x_n, x_planes,
+            _ptr(y), 0 if y is None else y.size, _ptr(res), 0 if res is None else res.size,
+            _ptr(planes), 0 if planes is None else planes.shape[1], 0 if planes is None else planes.shape[0],
+            None if ov is None else C.byref(ov), C.byref(rep)))
+        return y, planes, rep.as_dict()
+
+    def conv_log(self, mode):
+        """Launch-shape log of the dense conv launches (vtts_debug_conv_log): 1 clears and starts it, 0 stops it, 2 returns the
+        list of report dicts recorded since it was started."""
+        if mode != 2:
+            self._check(self.lib.vtts_debug_conv_log(self.h, int(mode), None, 0, None))
+            return None
+        out = (ConvReport * 65536)()
+        n = C.c_int(0)
+        self._check(self.lib.vtts_debug_conv_log(self.h, 2, out, len(out), C.byref(n)))
+        return [out[i].as_dict() for i in range(n.value)]
 
     def debug_flags(self, flags):
         self._check(self.lib.vtts_debug_flags(self.h, int(flags)))

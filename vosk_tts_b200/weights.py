@@ -135,6 +135,37 @@ def from_bf16_bits(b):
     return (b.astype(np.uint32) << 16).view(np.float32)
 
 
+def conv_ffma_layout(w, b=None):
+    """Conv1d weight [Co, Ci, k] (+ bias [Co]) in the FFMA conv's layout: w [k][Ci][ldw], bias [ldw], ldw = Co rounded up to 4."""
+    w = np.asarray(w, np.float32)
+    co, ci, k = w.shape
+    ldw = (co + 3) // 4 * 4
+    wp = np.zeros((k, ci, ldw), np.float32)
+    wp[:, :, :co] = np.transpose(w, (2, 1, 0))
+    bp = np.zeros(ldw, np.float32)
+    if b is not None:
+        bp[:co] = np.asarray(b, np.float32)
+    return wp, bp
+
+
+def conv_tc_planes(w):
+    """Conv1d weight [Co, Ci, k] -> split-bf16 bit planes (hi, lo), each uint16 [k][Co][Ci] (K-major rows for TMA):
+    hi = rne_bf16(w), lo = rne_bf16(w - hi)."""
+    wt = np.ascontiguousarray(np.transpose(np.asarray(w, np.float32), (2, 0, 1)))
+    hi = to_bf16_bits(wt)
+    return hi, to_bf16_bits(wt - from_bf16_bits(hi))
+
+
+def conv_tc3_planes(w):
+    """Exact 3-way split (hi, mid, lo) of a conv weight [Co, Ci, k], each uint16 [k][Co][Ci]: hi + mid + lo == w to the last
+    fp32 bit."""
+    wt = np.ascontiguousarray(np.transpose(np.asarray(w, np.float32), (2, 0, 1)))
+    hi = to_bf16_bits(wt)
+    r1 = wt - from_bf16_bits(hi)
+    mid = to_bf16_bits(r1)
+    return hi, mid, to_bf16_bits(r1 - from_bf16_bits(mid))
+
+
 class _Packer:
     ALIGN = 64  # floats
 
@@ -161,13 +192,7 @@ class _Packer:
             b = None if b is None else np.asarray(b, np.float32)[co_perm]
         if ci_perm is not None:
             w = w[:, ci_perm]
-        co, ci, k = w.shape
-        ldw = (co + 3) // 4 * 4
-        wp = np.zeros((k, ci, ldw), np.float32)
-        wp[:, :, :co] = np.transpose(w, (2, 1, 0))
-        bp = np.zeros(ldw, np.float32)
-        if b is not None:
-            bp[:co] = np.asarray(b, np.float32)
+        wp, bp = conv_ffma_layout(w, b)
         if need_w:
             self.add(name + ".w", wp)
         self.add(name + ".b", bp)
@@ -180,10 +205,8 @@ class _Packer:
             w = w[co_perm]
         if ci_perm is not None:
             w = w[:, ci_perm]
-        wt = np.ascontiguousarray(np.transpose(w, (2, 0, 1)))          # [k][Cout][Cin]
-        hi = to_bf16_bits(wt)
-        lo = to_bf16_bits(wt - from_bf16_bits(hi))
-        assert wt.size % 2 == 0
+        hi, lo = conv_tc_planes(w)
+        assert hi.size % 2 == 0
         self.add(name + ".th", hi.reshape(-1).view(np.float32))
         self.add(name + ".tl", lo.reshape(-1).view(np.float32))
 
@@ -194,11 +217,7 @@ class _Packer:
             w = w[co_perm]
         if ci_perm is not None:
             w = w[:, ci_perm]
-        wt = np.ascontiguousarray(np.transpose(w, (2, 0, 1)))          # [k][Cout][Cin]
-        hi = to_bf16_bits(wt)
-        r1 = wt - from_bf16_bits(hi)
-        mid = to_bf16_bits(r1)
-        lo = to_bf16_bits(r1 - from_bf16_bits(mid))
+        hi, mid, lo = conv_tc3_planes(w)
         self.add(name + ".t3h", hi.reshape(-1).view(np.float32))
         self.add(name + ".t3m", mid.reshape(-1).view(np.float32))
         self.add(name + ".t3l", lo.reshape(-1).view(np.float32))
