@@ -174,11 +174,41 @@ int vtts_timeline(vtts_handle h, int enable, unsigned long long* out, size_t max
  * both kept when bit0 is set), "vc_z_hat" (flow reverse output). */
 int vtts_debug_flags(vtts_handle h, int flags);
 int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floats, size_t* n_out);
-/* Unit-test hook for the relative-position attention kernels (attentions.py:165-196): one launch of layer "enc.<i>" or
- * "flow.<f>.tr" on a host fp32 qkv tensor [T][3H] of one utterance; out receives fp32 [T][H].  use_tc = 1 selects the
- * wgmma kernel (attn_tc.cuh), 0 the fp32 FFMA kernels.  iters > 0: *ms_out = average device time of `iters` more launches. */
-int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host, int T, int use_tc, float* out_host, int iters,
-                         float* ms_out);
+/* Unit-test hook for the relative-position attention kernels (attentions.py:165-196): ONE attention launch of layer
+ * "enc.<i>" or "flow.<f>.tr" through the engine's own launch code, on host tensors.
+ *   B, lens          utterances, packed as the engine packs them: utterance b starts at row offs[b], SEQ_GAP (8) rows between
+ *                    consecutive utterances
+ *   launch_lens      per-utterance lengths >= lens the launch is sized for (the bucket lengths of a captured graph: grid,
+ *                    maxLen and the kernel heuristics see them, the kernels read lens), or NULL = lens
+ *   qkv              fp32 [rows][3H], every row: gap rows and rows behind the last utterance hold whatever the caller put there.
+ *                    The tensor-core kernel reads the split-bf16 planes of all rows, taken from the engine's plane pool and
+ *                    cleared behind each utterance by the production zero_tails pass, as a phase does
+ *   kernel           VTTS_ATTN_AUTO (the engine's choice), _TC (attn_tc_kernel), _SPLIT (attn_split_kernel), _R1 / _R4
+ *                    (attn_kernel with 1 / 4 query rows per warp), _FFMA (the engine's choice among the FFMA kernels)
+ *   out              fp32 [rows][H] (in/out: rows outside the utterances are left as they are), or NULL
+ *   planes           uint16 [p_planes][rows * H] (in/out) split-bf16 planes of the output (hi, lo) or (hi, mid, lo), or NULL;
+ *                    the tensor-core kernel writes 2 planes only.  At least one of out / planes.
+ *   iters > 0        *ms_out = average device time of `iters` more launches
+ *   report           out: the launch that ran
+ * A kernel the layer cannot run (tensor cores without the split-bf16 relative tables or with 2W+1 > 13, split-KV where the
+ * key tiles do not fit shared memory or the CTAs one wave) and malformed arguments return VTTS_ERR_INVALID before any launch.
+ * The engine's kernel selection settings are restored on every exit. */
+#define VTTS_ATTN_AUTO 0
+#define VTTS_ATTN_TC 1
+#define VTTS_ATTN_SPLIT 2
+#define VTTS_ATTN_R1 3
+#define VTTS_ATTN_R4 4
+#define VTTS_ATTN_FFMA 5
+typedef struct vtts_attn_report {
+  int kernel;                   /* VTTS_ATTN_TC / _SPLIT / _R1 / _R4 */
+  int dk;                       /* head width: the kernel's template */
+  int R;                        /* query rows per warp (FFMA kernels) */
+  int grid_x, grid_y, grid_z;
+  int smem;                     /* dynamic shared memory bytes */
+} vtts_attn_report;
+int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* lens, const int* launch_lens, const float* qkv,
+                         size_t rows, int kernel, float* out, uint16_t* planes, int p_planes, int iters, float* ms_out,
+                         vtts_attn_report* report);
 
 /* Unit-test hook for the dense conv kernels: ONE grouped launch of the tensor-core conv (conv_tc.cuh) or of the fp32 FFMA
  * conv (kernels.cuh conv_kernel) through the engine's own launch code, on host tensors.

@@ -309,6 +309,7 @@ struct vtts_engine {
   int conv_max_s = 8, conv_target = 120, conv_max_g = 4, conv_big_g = 1, tc_tall = 0, tc_baseoff = 0, tc_bn = 0, attn_rows = 0, tc_mc = 0, tc_split = 0, conv_min_g = 1, tc_min_steps = 2, conv_auto_g = 4, attn_split = 1, tc_persist = 1, tc_persist_min = 1, n_sm = 132, tc_dbgskip = 0, tc_wmc = 0;
   // shape of the last dense conv launch (vtts_debug_conv) and, while log_conv is set, of every one (vtts_debug_conv_log)
   vtts_conv_report last_conv{};
+  vtts_attn_report last_attn{};               // the last attention launch (vtts_debug_attention)
   bool log_conv = false;
   std::vector<vtts_conv_report> conv_log;
   void note_conv(const vtts_conv_report& r) {
@@ -533,6 +534,7 @@ struct vtts_engine {
   CUtensorMap make_map(const void* base, int C, long rows, int box_rows);
   bool attn_tc_ok(const EncLayerW& L, int Hc) const;
   bool attn_use_tc(const EncLayerW& L, int Hc, const int* lens, int maxLen) const;
+  bool attn_split_fits(const EncLayerW& L, int Hc, const int* lens, int maxLen) const;
   void launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen);
   void launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
   // plane buffers of the frame-resolution stages: allocated (and their tails zeroed by ONE zero_tails launch) before the
@@ -1069,12 +1071,20 @@ bool vtts_engine::attn_tc_ok(const EncLayerW& L, int Hc) const {
 bool vtts_engine::attn_use_tc(const EncLayerW& L, int Hc, const int* lens, int maxLen) const {
   if (!attn_tc_ok(L, Hc)) return false;
   if (attn_tc_mode >= 2) return true;
+  return !((attn_rows == 0 || attn_rows == 1) && attn_split_fits(L, Hc, lens, maxLen));
+}
+
+// Can the split-KV FFMA kernel take this launch?  All key tiles of the longest utterance must be resident in shared memory
+// (at most ATS_MAXT tiles, and at most ATS_SMEM_MAX bytes: dk 128 at W 4 overflows from 7 tiles, i.e. 193 positions), and
+// the CTAs must fit one wave.
+bool vtts_engine::attn_split_fits(const EncLayerW& L, int Hc, const int* lens, int maxLen) const {
+  const int dk = Hc / L.heads, nrel = 2 * cfg.window_size + 1;
   const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
   long ctas = 0;
   for (int b = 0; b < B; ++b) ctas += (long)((hl[b] + ATS_ROWS - 1) / ATS_ROWS) * L.heads;
   const int mt = (maxLen + AT_KT - 1) / AT_KT;
-  const bool split_kv_fits = attn_split && (attn_rows == 0 || attn_rows == 1) && mt <= ATS_MAXT && ctas <= n_sm;
-  return !split_kv_fits;
+  return attn_split && mt <= ATS_MAXT && ctas <= n_sm && dk % 32 == 0 && dk <= 128 &&
+         (long)attn_split_smem_floats(dk, nrel, mt) * (long)sizeof(float) <= ATS_SMEM_MAX;
 }
 
 void vtts_engine::launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen) {
@@ -1096,6 +1106,7 @@ void vtts_engine::launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const
   ap.koff = Hc; ap.voff = 2 * Hc;
   dim3 grid((maxLen + ATC_BM - 1) / ATC_BM, L.heads, B);
   if (grid.x == 0) return;
+  last_attn = vtts_attn_report{VTTS_ATTN_TC, dk, 0, (int)grid.x, (int)grid.y, (int)grid.z, atc_smem_bytes(dk)};
   switch (dk / 32) {
     case 1: klaunch(attn_tc_kernel<32>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(32), ap, lens, offs); break;
     case 2: klaunch(attn_tc_kernel<64>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(64), ap, lens, offs); break;
@@ -1119,12 +1130,11 @@ void vtts_engine::launch_attn(const float* qkv, float* ao, const EncLayerW& L, i
   const int R = (attn_rows == 1 || attn_rows == 4) ? attn_rows : (rows * n_heads >= 8L * 2 * n_sm * 4 ? 4 : 1);
   // single short utterances: split-KV variant (all K/V tiles resident, 4 warps per query row) when it fits one wave
   {
-    long ctas = 0;
-    for (int b = 0; b < B; ++b) ctas += (long)((hl[b] + ATS_ROWS - 1) / ATS_ROWS) * n_heads;
     const int mt = (maxLen + AT_KT - 1) / AT_KT;
-    if (attn_split && R == 1 && mt <= ATS_MAXT && ctas <= n_sm && dk % 32 == 0 && dk <= 128) {
+    if (R == 1 && attn_split_fits(L, Hc, lens, maxLen)) {
       dim3 grid((maxLen + ATS_ROWS - 1) / ATS_ROWS, n_heads, B);
       const size_t smem = (size_t)attn_split_smem_floats(dk, nrel, mt) * sizeof(float);
+      last_attn = vtts_attn_report{VTTS_ATTN_SPLIT, dk, 1, (int)grid.x, (int)grid.y, (int)grid.z, (int)smem};
 #define ATTN_SPLIT(D) klaunch(attn_split_kernel<D>, grid, dim3(ATS_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, mt, lens, offs, ph, plo, pmi)
       switch (dk / 32) { case 1: ATTN_SPLIT(1); break; case 2: ATTN_SPLIT(2); break; case 3: ATTN_SPLIT(3); break; default: ATTN_SPLIT(4); break; }
 #undef ATTN_SPLIT
@@ -1136,6 +1146,7 @@ void vtts_engine::launch_attn(const float* qkv, float* ao, const EncLayerW& L, i
   const int QT = 8 * R;
   dim3 grid((maxLen + QT - 1) / QT, n_heads, B);
   const size_t smem = (size_t)attn_smem_floats(dk, nrel, R) * sizeof(float);
+  last_attn = vtts_attn_report{R == 4 ? VTTS_ATTN_R4 : VTTS_ATTN_R1, dk, R, (int)grid.x, (int)grid.y, (int)grid.z, (int)smem};
 #define ATTN_CASE(D, RR) klaunch(attn_kernel<D, RR>, grid, dim3(AT_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, lens, offs, ph, plo, pmi)
   if (R == 4) {
     switch (dk / 32) { case 1: ATTN_CASE(1, 4); break; case 2: ATTN_CASE(2, 4); break; case 3: ATTN_CASE(3, 4); break; default: ATTN_CASE(4, 4); break; }
@@ -2671,10 +2682,10 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     CK(cudaFuncSetAttribute(attn_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc_smem_bytes(64)));
     CK(cudaFuncSetAttribute(attn_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc_smem_bytes(96)));
     CK(cudaFuncSetAttribute(attn_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc_smem_bytes(128)));
-    CK(cudaFuncSetAttribute(attn_split_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CK(cudaFuncSetAttribute(attn_split_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CK(cudaFuncSetAttribute(attn_split_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    CK(cudaFuncSetAttribute(attn_split_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CK(cudaFuncSetAttribute(attn_split_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATS_SMEM_MAX));
+    CK(cudaFuncSetAttribute(attn_split_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATS_SMEM_MAX));
+    CK(cudaFuncSetAttribute(attn_split_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATS_SMEM_MAX));
+    CK(cudaFuncSetAttribute(attn_split_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATS_SMEM_MAX));
     CK(cudaFuncSetAttribute(attn_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     CK(cudaFuncSetAttribute(attn_kernel<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     CK(cudaFuncSetAttribute(attn_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -3021,13 +3032,28 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
   });
 }
 
-// Unit-test hook: runs ONE attention launch of the named encoder layer ("enc.<i>" or "flow.<f>.tr") on a caller-supplied
-// fp32 qkv tensor [T][3H] of a single utterance and returns the fp32 output [T][H].  use_tc = 1: attn_tc_kernel on the
-// split-bf16 planes of the input (needs a precision >= 1 engine); 0: the fp32 FFMA kernels.  iters > 0 also times the launch.
-int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host, int T, int use_tc, float* out_host, int iters,
-                         float* ms_out) {
-  if (!layer || !qkv_host || !out_host || T < 1) return VTTS_ERR_INVALID;
+// Host copies of a debug hook's arguments on the device (freed on every exit).
+struct DebugBufs {
+  std::vector<void*> p;
+  ~DebugBufs() { for (void* q : p) cudaFree(q); }
+  void* up(const void* src, size_t bytes, cudaStream_t s) {
+    void* d = nullptr;
+    CK(cudaMalloc(&d, std::max<size_t>(bytes, 16)));
+    p.push_back(d);
+    if (src) CK(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, s));
+    return d;
+  }
+};
+
+// Unit-test hook of the attention kernels (include/vtts.h): one launch through launch_attn_tc / launch_attn on host tensors.
+int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* lens, const int* launch_lens, const float* qkv,
+                         size_t rows, int kernel, float* out, uint16_t* planes, int p_planes, int iters, float* ms_out,
+                         vtts_attn_report* report) {
   return guarded(h, [&] {
+    REQUIRE(layer && lens && qkv && B >= 1, VTTS_ERR_INVALID, "debug_attention: missing layer, lengths or input");
+    REQUIRE(out || planes, VTTS_ERR_INVALID, "debug_attention: neither fp32 output nor output planes requested");
+    REQUIRE(!planes || p_planes == 2 || p_planes == 3, VTTS_ERR_INVALID, "debug_attention: the output has 2 or 3 planes");
+    REQUIRE(kernel >= VTTS_ATTN_AUTO && kernel <= VTTS_ATTN_FFMA, VTTS_ERR_INVALID, "debug_attention: unknown kernel selection");
     const std::string nm(layer);
     const EncLayerW* L = nullptr;
     if (nm.rfind("enc.", 0) == 0) {
@@ -3041,44 +3067,100 @@ int vtts_debug_attention(vtts_handle h, const char* layer, const float* qkv_host
     }
     REQUIRE(L != nullptr, VTTS_ERR_INVALID, "layer must be enc.<i> or flow.<f>.tr");
     const int H = h->cfg.hidden_channels;
-    REQUIRE(!use_tc || h->attn_tc_ok(*L, H), VTTS_ERR_INVALID, "tensor-core attention is not available for this layer / precision mode");
-    const int B0 = h->B; const std::vector<int> fl0 = h->h_frm_len, tl0 = h->h_tok_len, vf0 = h->v_frm_len, vt0 = h->v_tok_len; const int mf0 = h->maxFrm;
-    h->B = 1; h->h_frm_len.assign(1, T); h->h_tok_len.assign(1, T); h->maxFrm = T; h->v_frm_len = h->h_frm_len; h->v_tok_len = h->h_tok_len;
-    int* dl = nullptr; float *dq = nullptr, *dout = nullptr;
-    CK(cudaMalloc(&dl, 16));
-    const int hl[3] = {T, 0, T};
-    CK(cudaMemcpy(dl, hl, 12, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&dq, (size_t)T * 3 * H * 4)); CK(cudaMalloc(&dout, (size_t)T * H * 4));
-    CK(cudaMemcpy(dq, qkv_host, (size_t)T * 3 * H * 4, cudaMemcpyHostToDevice));
-    CK(cudaMemset(dout, 0, (size_t)T * H * 4));
+    std::vector<int> ll(B);
+    std::vector<long> off(B + 1, 0);
+    int maxLen = 0;
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(lens[b] >= 1, VTTS_ERR_INVALID, "debug_attention: lengths must be >= 1");
+      ll[b] = launch_lens ? launch_lens[b] : lens[b];
+      REQUIRE(ll[b] >= lens[b], VTTS_ERR_INVALID, "debug_attention: launch lengths must be >= the lengths");
+      off[b + 1] = off[b] + lens[b] + (b + 1 < B ? SEQ_GAP : 0);
+      maxLen = std::max(maxLen, ll[b]);
+    }
+    REQUIRE((long)rows >= off[B], VTTS_ERR_INVALID, "debug_attention: qkv has fewer rows than the packed utterances");
+    // ---- per-call engine state the launch code reads, restored on every exit
+    struct Saved {
+      vtts_engine* h;
+      int B, maxFrm, maxTok, tc_mode, split, arows;
+      std::vector<int> fl, tl, vf, vt;
+      explicit Saved(vtts_engine* e) : h(e), B(e->B), maxFrm(e->maxFrm), maxTok(e->maxTok), tc_mode(e->attn_tc_mode),
+          split(e->attn_split), arows(e->attn_rows), fl(e->h_frm_len), tl(e->h_tok_len), vf(e->v_frm_len), vt(e->v_tok_len) {}
+      ~Saved() {
+        h->B = B; h->maxFrm = maxFrm; h->maxTok = maxTok; h->attn_tc_mode = tc_mode; h->attn_split = split; h->attn_rows = arows;
+        h->h_frm_len = fl; h->h_tok_len = tl; h->v_frm_len = vf; h->v_tok_len = vt;
+      }
+    } saved(h);
+    h->B = B; h->maxFrm = maxLen; h->maxTok = maxLen;
+    h->h_frm_len.assign(lens, lens + B); h->h_tok_len = h->h_frm_len;
+    h->v_frm_len = ll; h->v_tok_len = ll;           // the heuristics see the launch lengths
+    // ---- kernel selection (refused before anything is launched)
+    bool use_tc = false;
+    switch (kernel) {
+      case VTTS_ATTN_AUTO: use_tc = h->attn_use_tc(*L, H, nullptr, maxLen); break;
+      case VTTS_ATTN_TC:
+        h->attn_tc_mode = 2;
+        REQUIRE(h->attn_tc_ok(*L, H), VTTS_ERR_INVALID, "debug_attention: tensor-core attention is not available for this layer (relative tables / window)");
+        use_tc = true;
+        break;
+      case VTTS_ATTN_SPLIT:
+        h->attn_split = 1; h->attn_rows = 1;
+        REQUIRE(h->attn_split_fits(*L, H, nullptr, maxLen), VTTS_ERR_INVALID, "debug_attention: the split-KV kernel does not fit this launch");
+        break;
+      case VTTS_ATTN_R1: h->attn_split = 0; h->attn_rows = 1; break;
+      case VTTS_ATTN_R4: h->attn_split = 0; h->attn_rows = 4; break;
+      default: break;                               // VTTS_ATTN_FFMA: launch_attn's own choice
+    }
+    REQUIRE(!(use_tc && planes && p_planes != 2), VTTS_ERR_INVALID, "debug_attention: the tensor-core kernel writes 2 output planes");
+    // ---- device copies
+    DebugBufs dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    std::vector<int> lo(2 * B + 3);
+    for (int b = 0; b < B; ++b) lo[b] = lens[b];
+    for (int b = 0; b <= B; ++b) lo[B + b] = (int)off[b];
+    lo[2 * B + 1] = (int)rows; lo[2 * B + 2] = 0;   // all rows as one span (input split)
+    int* dl = static_cast<int*>(dev.up(lo.data(), lo.size() * sizeof(int), st));
+    const int* dlens = dl;
+    const int* doffs = dl + B;
+    const float* dq = static_cast<const float*>(dev.up(qkv, rows * 3 * H * sizeof(float), st));
+    float* dout = static_cast<float*>(dev.up(out, rows * H * sizeof(float), st));   // (the FFMA kernels always write fp32)
+    const size_t pn = rows * H;
+    Planes po;
+    if (planes) {
+      __nv_bfloat16* dp = static_cast<__nv_bfloat16*>(dev.up(planes, (size_t)p_planes * pn * 2, st));
+      po.hi = dp; po.mid = p_planes == 3 ? dp + pn : nullptr; po.lo = dp + (p_planes - 1) * pn; po.C = H; po.rows = (long)rows;
+    }
     Planes pq;
     if (use_tc) {
+      // split every row on the device, then the production zero_tails pass: gap rows and rows behind each utterance hold the
+      // caller's data until that pass clears them, as in a phase
       h->begin_planes();
-      pq = h->planes(58, T, 1, 3 * H);
-      h->flush_tails(dl, dl + 1);
-      h->klaunch(split_planes_kernel, dim3((T + EW_ROWS - 1) / EW_ROWS, 1), dim3(EW_THREADS), (size_t)0, (const float*)dq, 3 * H, pq.hi, pq.lo, 3 * H, 3 * H, 1.f, 0, 1, (const int*)dl, (const int*)(dl + 1));
+      pq = h->planes(58, (long)rows, 1, 3 * H);
+      h->klaunch(split_planes_kernel, dim3((unsigned)((rows + EW_ROWS - 1) / EW_ROWS), 1), dim3(EW_THREADS), (size_t)0, dq, 3 * H, pq.hi,
+                 pq.lo, 3 * H, 3 * H, 1.f, 0, 1, (const int*)(dl + 2 * B + 1), (const int*)(dl + 2 * B + 2));
+      h->flush_tails(dlens, doffs);
     }
     auto once = [&] {
-      if (use_tc) h->launch_attn_tc(pq, dout, nullptr, *L, H, dl, dl + 1, T);
-      else h->launch_attn(dq, dout, *L, H, dl, dl + 1, T, nullptr);
+      if (use_tc) h->launch_attn_tc(pq, out ? dout : nullptr, planes ? &po : nullptr, *L, H, dlens, doffs, maxLen);
+      else h->launch_attn(dq, dout, *L, H, dlens, doffs, maxLen, planes ? &po : nullptr);
     };
     once();
-    CK(cudaStreamSynchronize(h->stream));
-    CK(cudaMemcpy(out_host, dout, (size_t)T * H * 4, cudaMemcpyDeviceToHost));
+    CK(cudaStreamSynchronize(st));
+    if (out) CK(cudaMemcpy(out, dout, rows * H * sizeof(float), cudaMemcpyDeviceToHost));
+    if (planes) CK(cudaMemcpy(planes, po.hi, (size_t)p_planes * pn * 2, cudaMemcpyDeviceToHost));
+    if (report) *report = h->last_attn;
     if (iters > 0 && ms_out) {
       cudaEvent_t e0, e1;
       CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-      CK(cudaEventRecord(e0, h->stream));
+      CK(cudaEventRecord(e0, st));
       for (int i = 0; i < iters; ++i) once();
-      CK(cudaEventRecord(e1, h->stream));
-      CK(cudaStreamSynchronize(h->stream));
+      CK(cudaEventRecord(e1, st));
+      CK(cudaStreamSynchronize(st));
       float ms = 0.f;
       CK(cudaEventElapsedTime(&ms, e0, e1));
       *ms_out = ms / iters;
       cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
-    cudaFree(dl); cudaFree(dq); cudaFree(dout);
-    h->B = B0; h->h_frm_len = fl0; h->h_tok_len = tl0; h->maxFrm = mf0; h->v_frm_len = vf0; h->v_tok_len = vt0;
   });
 }
 
@@ -3199,17 +3281,7 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
     h->h_frm_off.assign(off.begin(), off.end());
     h->v_frm_len = h->h_frm_len;                  // the heuristics see this call's lengths
     // ---- device copies (freed on every exit)
-    struct DevBufs {
-      std::vector<void*> p;
-      ~DevBufs() { for (void* q : p) cudaFree(q); }
-      void* up(const void* src, size_t bytes, cudaStream_t s) {
-        void* d = nullptr;
-        CK(cudaMalloc(&d, std::max<size_t>(bytes, 16)));
-        p.push_back(d);
-        if (src) CK(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, s));
-        return d;
-      }
-    } dev;
+    DebugBufs dev;
     cudaStream_t st = h->stream;
     CK(cudaStreamSynchronize(st));
     std::vector<int> lo(2 * B + 1);

@@ -820,6 +820,7 @@ attn_kernel(const float* __restrict__ qkv, int ld, float* __restrict__ out, int 
 // partial (max, sum, accumulator) states of a row are merged in segment order at the end.
 // ------------------------------------------------------------------------------------------------
 constexpr int ATS_ROWS = 4, ATS_SEG = 4, ATS_MAXT = 8, ATS_WARPS = ATS_ROWS * ATS_SEG, ATS_THREADS = 32 * ATS_WARPS;
+constexpr int ATS_SMEM_MAX = 227 * 1024;          // dynamic shared memory the split-KV kernel is allowed (sm_90 maximum)
 constexpr int attn_split_smem_floats(int dk, int nrel, int ntiles) {
   return 2 * ntiles * AT_KT * (dk + 4) + ATS_ROWS * (dk + 4) + 2 * nrel * (dk + 4) + ATS_ROWS * nrel + ATS_WARPS * AT_KT + ATS_WARPS * (4 + dk);
 }

@@ -80,6 +80,19 @@ class ConvReport(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+ATTN_KERNELS = {"auto": 0, "tc": 1, "split": 2, "r1": 3, "r4": 4, "ffma": 5}    # VTTS_ATTN_*
+
+
+class AttnReport(C.Structure):
+    """vtts_attn_report: the attention launch that ran."""
+    _fields_ = [(n, C.c_int32) for n in ("kernel", "dk", "R", "grid_x", "grid_y", "grid_z", "smem")]
+
+    def as_dict(self):
+        d = {n: int(getattr(self, n)) for n, _ in self._fields_}
+        d["kernel"] = {v: k for k, v in ATTN_KERNELS.items()}.get(d["kernel"], d["kernel"])
+        return d
+
+
 class _Missing:
     """Stand-in for an entry point an alternative build (VTTS_LIB) does not export: accepts the argtypes / restype
     assignments of load_library and raises when called."""
@@ -171,7 +184,8 @@ def load_library(build_if_missing=True):
     lib.vtts_profile_read.restype = i32
     lib.vtts_profile_read_tc.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
     lib.vtts_profile_read_tc.restype = i32
-    lib.vtts_debug_attention.argtypes = [vp, C.c_char_p, vp, i32, i32, vp, i32, fp]
+    lib.vtts_debug_attention.argtypes = [vp, C.c_char_p, i32, vp, vp, vp, C.c_size_t, i32, vp, vp, i32, i32, fp,
+                                         C.POINTER(AttnReport)]
     lib.vtts_debug_attention.restype = i32
     lib.vtts_debug_conv.argtypes = [vp, i32, i32, vp, i32, i32, C.POINTER(ConvProblem), vp, C.c_size_t, i32, vp, C.c_size_t, vp,
                                     C.c_size_t, vp, C.c_size_t, i32, C.POINTER(ConvOverrides), C.POINTER(ConvReport)]
@@ -564,14 +578,36 @@ class Engine:
         out.update(tc_ms=ms.value, tc_launches=int(n.value), tc_flops=fl.value)
         return out
 
-    def debug_attention(self, layer, qkv, use_tc, iters=0):
-        """One attention launch of `layer` ("enc.<i>" / "flow.<f>.tr") on qkv float32 [T, 3H]; returns (out [T, H], ms or None)."""
+    def debug_attention(self, layer, qkv, lens=None, kernel="auto", launch_lens=None, out=True, planes=None, iters=0):
+        """One attention launch of `layer` ("enc.<i>" / "flow.<f>.tr") through the engine's launch code (vtts_debug_attention).
+        qkv: float32 [rows, 3H], every row of the packed batch (utterance b at row cr.offsets(lens)[b], 8 rows between
+        utterances).  lens: lengths (default: one utterance of all rows); launch_lens: lengths >= lens the launch is sized for.
+        kernel: "auto", "tc", "split", "r1", "r4" or "ffma" (the engine's choice among the FFMA kernels).
+        out: True (zero-filled), an initial float32 [rows, H] (rows outside the utterances keep it) or False for none.
+        planes: None, 2 / 3 (zero-filled) or an initial uint16 [p, rows * H].
+        Returns (out [rows, H] or None, planes or None, launch report dict, ms or None)."""
         qkv = np.ascontiguousarray(qkv, dtype=np.float32)
-        T, H = qkv.shape[0], qkv.shape[1] // 3
-        out = np.zeros((T, H), np.float32)
+        rows, H = qkv.shape[0], qkv.shape[1] // 3
+        lens = np.ascontiguousarray([rows] if lens is None else lens, dtype=np.int32)
+        ll = None if launch_lens is None else np.ascontiguousarray(launch_lens, dtype=np.int32)
+        if out is True:
+            out = np.zeros((rows, H), np.float32)
+        elif out is not None and out is not False:
+            out = np.ascontiguousarray(out, dtype=np.float32).reshape(rows, H).copy()
+        else:
+            out = None
+        if isinstance(planes, int):
+            planes = np.zeros((planes, rows * H), np.uint16)
+        elif planes is not None:
+            planes = np.ascontiguousarray(planes, dtype=np.uint16).copy()
+        if kernel not in ATTN_KERNELS:
+            raise ValueError("unknown attention kernel %r" % (kernel,))
         ms = C.c_float(0.0)
-        self._check(self.lib.vtts_debug_attention(self.h, layer.encode(), _ptr(qkv), T, int(use_tc), _ptr(out), int(iters), C.byref(ms)))
-        return out, (float(ms.value) if iters > 0 else None)
+        rep = AttnReport()
+        self._check(self.lib.vtts_debug_attention(
+            self.h, layer.encode(), lens.size, _ptr(lens), _ptr(ll), _ptr(qkv), rows, ATTN_KERNELS[kernel], _ptr(out),
+            _ptr(planes), 0 if planes is None else planes.shape[0], int(iters), C.byref(ms), C.byref(rep)))
+        return out, planes, rep.as_dict(), (float(ms.value) if iters > 0 else None)
 
     def debug_conv(self, use_tc, lens, rmul, problems, x, y=None, res=None, planes=None, overrides=None):
         """One grouped launch of the tensor-core (use_tc) or FFMA conv kernel on host tensors (vtts_debug_conv).

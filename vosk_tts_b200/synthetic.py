@@ -50,10 +50,10 @@ def _spec(cfg, posterior=False):
         out.append((name + ".gamma", (c,), "gamma", 0.1))
         out.append((name + ".beta", (c,), "normal", 0.1))
 
-    def encoder(prefix, hidden, filt, n_layers, ks):
+    def encoder(prefix, hidden, filt, n_layers, ks, heads):
         for i in range(n_layers):
             a = "%s.attn_layers.%d" % (prefix, i)
-            dk = hidden // nh
+            dk = hidden // heads
             out.append((a + ".emb_rel_k", (1, 2 * W + 1, dk), "normal", dk ** -0.5))
             out.append((a + ".emb_rel_v", (1, 2 * W + 1, dk), "normal", dk ** -0.5))
             for nm in ("conv_q", "conv_k", "conv_v", "conv_o"):
@@ -75,7 +75,7 @@ def _spec(cfg, posterior=False):
     if cfg["n_speakers"] > 1:
         out.append(("emb_g.weight", (cfg["n_speakers"], G), "normal", 1.0))
     out.append(("enc_p.emb.weight", (cfg["n_vocab"], H), "normal", H ** -0.5))
-    encoder("enc_p.encoder", H, Fc, cfg["n_layers"], k)
+    encoder("enc_p.encoder", H, Fc, cfg["n_layers"], k, nh)
     if cfg["use_spk_conditioned_encoder"] and G > 0:
         out.append(("enc_p.encoder.spk_emb_linear.weight", (H, G), "normal", 0.5 / math.sqrt(G)))
         out.append(("enc_p.encoder.spk_emb_linear.bias", (H,), "normal", 0.05))
@@ -104,7 +104,7 @@ def _spec(cfg, posterior=False):
         p = "flow.flows.%d" % (2 * f)
         conv(p + ".pre", H, I // 2, 1)
         if cfg["use_transformer_flows"]:
-            encoder(p + ".pre_transformer", H, H, 1, fk)
+            encoder(p + ".pre_transformer", H, H, 1, fk, cfg.get("flow_n_heads", 2))   # (2 heads hard-coded, models.py:355)
         for i in range(cfg["flow_wn_layers"]):
             conv("%s.enc.in_layers.%d" % (p, i), 2 * H, H, fk, wn=True, gain=1.0)
             rs = 2 * H if i < cfg["flow_wn_layers"] - 1 else H
