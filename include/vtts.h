@@ -255,6 +255,9 @@ typedef struct vtts_conv_report {
   int image;                    /* 0 conv_tc_kernel<BN, false>, 1 conv_tc_kernel<BN, true>, 2 conv_tc_persist_kernel<BN> */
   int S, G;                     /* FFMA: cluster split-K and thread groups */
   int grid_x, grid_y, grid_z;
+  int psplit[4];                /* tensor cores: split-K of each problem's tiles (dividing `split`, the cluster size; 0 past the
+                                   last problem).  Problems with psplit < split share a cluster between split / psplit tiles,
+                                   and the grid is then (1, 1, clusters * split) */
 } vtts_conv_report;
 int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul, int n_problems, const vtts_conv_problem* problems,
                     const void* x, size_t x_n, int x_planes, float* y, size_t y_n, const float* res, size_t res_n, uint16_t* p_out,
@@ -262,6 +265,13 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
 /* Launch-shape log of the dense conv launches: mode 1 clears and starts it, 0 stops it, 2 copies up to max_n entries (one
  * per launch the host enqueued since it was started; graph replays enqueue none) and sets *n_out. */
 int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_n, int* n_out);
+/* The split-K plan the engine makes for one grouped tensor-core conv launch, computed on the host alone (no device, no
+ * engine).  Problems p < n (1..4): cin[p] (a multiple of 64), cout[p], k[p], in_extra[p]; B utterances of lens[b] <= max_len
+ * rows / rmul; bn 64 / 128 pins the tile width (0: either); max_split caps the cluster size (8: none); min_steps = k-steps
+ * per split CTA at least; n_sm and cluster_cap (co-resident clusters of 2/4/8 CTAs at BN 64, then at BN 128) describe the
+ * device.  plan (out, 6 ints): BN, cluster size, and the split of each problem (0 past the last). */
+int vtts_tc_split_plan(int n, const int* cin, const int* cout, const int* k, const int* in_extra, int B, const int* lens,
+                       int rmul, int max_len, int bn, int max_split, int min_steps, int n_sm, const int* cluster_cap, int* plan);
 
 /* Voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718): re-voices recordings of speaker sid_src as
  * speaker sid_tgt of the same multi-speaker model.  One call = spectrogram front end, posterior encoder enc_q (g_src),

@@ -64,6 +64,8 @@ struct TcProblemBase {
   int in_extra, out_seq_extra;
   int epi;
   float alpha, pl_slope;
+  int split;                  // split-K of this problem's tiles (divides TcBatchScalars::split, the cluster size)
+  int cl0;                    // mixed-split launches: index of the problem's first cluster
 };
 struct TcProblem : TcProblemBase {
   CUtensorMap a_mid, w_mid;   // third planes of the exact 3-way split (np == 3)
@@ -89,6 +91,10 @@ struct TcBatchScalars {
   int split;    // cluster split-K: `split` CTAs (cluster dims (1,1,split)) each run a contiguous range of the k-steps of one
                 //    output tile, exchange partial accumulators through distributed shared memory and each finish
                 //    BN/split of the tile's columns (reduce-scatter; fixed summation order => deterministic).  1 = off
+  int mixed;    // 1: the problems' splits differ (TcProblemBase::split).  Grid (1, 1, clusters * split), the clusters of one
+                //    problem after another; a cluster of problem p covers split / p.split consecutive output tiles (row tile
+                //    fastest, then channel tile, then utterance), each reduced over p.split adjacent ranks
+  int nb;       // utterances of the launch
   unsigned long long* dbg;   // optional: %globaltimer stamps of CTA (0,0,0) for tuning (tools/microbench.py)
 };
 template <class PT, int MP = TC_MAXP>
@@ -226,7 +232,8 @@ struct TcTile {
   int pi;           // problem index (the problem is always addressed as tb.p[pi]: a pointer into the __grid_constant__ parameter
                     //  turns every field access into a generic load instead of an indexed constant-bank read)
   int b, co0, t0, sp;
-  int t0u;          // first row of the scheduling unit (== t0, or the pair's first tile with weight multicast)
+  int s;            // CTAs reducing this tile (split-K), sp = this CTA's rank among them
+  int t0u;         // first row of the scheduling unit (== t0, or the pair's first tile with weight multicast)
   bool valid;       // the problem has this channel tile (grouped problems may differ in Cout)
 };
 
@@ -237,7 +244,9 @@ struct TcTile {
 // producer fetches tile i+1's operands while the consumers run tile i's epilogue, and the per-CTA prologue (barrier
 // init, descriptor prefetch, pipeline fill) is paid once per SM instead of once per tile.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int BN, class PT, int MP>
+// MIXED: the single-wave image, which also runs mixed-split launches (tb.mixed); the persistent image never does (mixed
+// splits imply split-K, and split-K launches are single-wave), so it is compiled without that code.
+template <int BN, bool MIXED, class PT, int MP>
 __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const int* __restrict__ lens, const int* __restrict__ offs) {
   constexpr bool HAS_MID = std::is_same<PT, TcProblem>::value;
   constexpr int B_BYTES = BN * TC_BK * 2;
@@ -255,7 +264,27 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
   const int ntiles = persist ? gxu * tb.gy * tb.gz : 1;
   const int tstride = persist ? (int)gridDim.x / wmc : 1;
   const int tile0 = persist ? (int)blockIdx.x / wmc : 0;
+  // mixed-split launches: output tile `g` of this CTA's cluster, or the CTA's own tile (g < 0: g = rank / p.split)
+  auto decode_mixed = [&](int g) {
+    const int ci = (int)blockIdx.z / S, rank = (int)blockIdx.z - ci * S;
+    int pi = 0;
+    while (pi + 1 < tb.n && ci >= tb.p[pi + 1].cl0) ++pi;
+    const int s = tb.p[pi].split, gyp = (tb.p[pi].Cout + BN - 1) / BN;
+    if (g < 0) g = rank / s;
+    const int tile = (ci - tb.p[pi].cl0) * (S / s) + g;
+    TcTile t;
+    t.pi = pi;
+    t.s = s;
+    t.sp = rank % s;
+    t.t0 = (tile % tb.gx) * TC_BM;
+    t.t0u = t.t0;
+    t.co0 = ((tile / tb.gx) % gyp) * BN;
+    t.b = tile / (tb.gx * gyp);
+    t.valid = t.b < tb.nb;
+    return t;
+  };
   auto decode = [&](int tile) {
+    if constexpr (MIXED) { if (tb.mixed) return decode_mixed(-1); }
     int bx, by, bz, bxu;
     if (persist) {
       bxu = tile % gxu;
@@ -270,6 +299,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
     TcTile t;
     t.t0u = bxu * wmc * TC_BM;
     const int zi = bz / S;
+    t.s = S;
     t.sp = bz - zi * S;
     t.pi = zi % tb.n;
     t.b = zi / tb.n;
@@ -338,7 +368,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
   if (!persist && first.valid) {
     const PT& P = tb.p[first.pi];
     const int nsteps_all = (P.Cin / TC_BK) * P.k;
-    const int s_beg = (int)((long)nsteps_all * first.sp / S), s_end = (int)((long)nsteps_all * (first.sp + 1) / S);
+    const int s_beg = (int)((long)nsteps_all * first.sp / first.s), s_end = (int)((long)nsteps_all * (first.sp + 1) / first.s);
     const bool peek_active = first.t0 < lens[first.b] * tb.rmul + P.in_extra;
     w_pre = (tb.wpre && peek_active) ? min(TC_WST, s_end - s_beg) : 0;
     if (producer && lane == 0) {
@@ -373,7 +403,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
         any_active = true;
         const long in_base = (long)offs[T.b] * tb.rmul + (long)T.b * P.in_extra;
         const int nsteps_all = (P.Cin / TC_BK) * P.k;
-        const int s_beg = (int)((long)nsteps_all * T.sp / S), s_end = (int)((long)nsteps_all * (T.sp + 1) / S);   // this CTA's k-steps
+        const int s_beg = (int)((long)nsteps_all * T.sp / T.s), s_end = (int)((long)nsteps_all * (T.sp + 1) / T.s);   // this CTA's k-steps
         const int a_per = tall ? P.k : 1;                    // k-steps sharing one activation tile (tall => S == 1)
         const uint32_t a_tx = (uint32_t)NP * (uint32_t)(tall ? (TC_BM + (P.k - 1) * P.dil) : TC_BM) * 128u;   // bytes TMA delivers per set of planes
         int c = s_beg / P.k, j = s_beg - c * P.k;
@@ -428,7 +458,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
                                                              //  utterance still runs the mainloop; it stores nothing)
       any_active = true;
       const int nsteps_all = (P.Cin / TC_BK) * P.k;
-      const int s_beg = (int)((long)nsteps_all * T.sp / S), s_end = (int)((long)nsteps_all * (T.sp + 1) / S);
+      const int s_beg = (int)((long)nsteps_all * T.sp / T.s), s_end = (int)((long)nsteps_all * (T.sp + 1) / T.s);
       const int a_per = tall ? P.k : 1;
       float acc[NACC];
 #pragma unroll
@@ -509,7 +539,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
         rowok[h] = t < L;
         orow[h] = out_base + (long)t * P.out_mul + P.out_add;
       }
-      if (S == 1) {
+      if (T.s == 1) {
 #pragma unroll
         for (int jn = 0; jn < BN / 8; ++jn) {
           const int c = co0 + jn * 8 + 2 * q4;
@@ -518,10 +548,10 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
             if (rowok[h]) tc_epi_pair(P, b, orow[h], c, acc[4 * jn + 2 * h], acc[4 * jn + 2 * h + 1], tb.dbgskip);
         }
       } else {
-        // split-K reduce-scatter: CTA q of the cluster finishes columns [q W, q W + W) of the tile.  Every CTA sends each
-        // partial pair to the owner's staging buffer [src CTA][row][W]; the owner adds the S partials in rank order.
-        const int W = BN / S, sp = T.sp;
-        float* stage = reinterpret_cast<float*>(smem);       // [S][128][W] fp32 (BN/2 KB), aliases the operand rings
+        // split-K reduce-scatter among the T.s ranks g0 .. g0 + T.s - 1 of the tile: rank g0 + q finishes columns [q W, q W + W).
+        // Every CTA sends each partial pair to the owner's staging buffer [src][row][W]; the owner adds the partials in rank order.
+        const int W = BN / T.s, sp = T.sp, g0 = MIXED ? (int)blockIdx.z % S - sp : 0;
+        float* stage = reinterpret_cast<float*>(smem);       // [T.s][128][W] fp32 (BN/2 KB), aliases the operand rings
         cluster_sync_all();                                  // (1) every CTA of the cluster is done with its operand rings
 #pragma unroll
         for (int jn = 0; jn < BN / 8; ++jn) {
@@ -530,7 +560,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             uint32_t ra;
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(stage + ((size_t)sp * TC_BM + rbase + 8 * h) * W + (cc - qo * W))), "r"(qo));
+            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(stage + ((size_t)sp * TC_BM + rbase + 8 * h) * W + (cc - qo * W))), "r"(g0 + qo));
             asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(ra), "f"(acc[4 * jn + 2 * h]), "f"(acc[4 * jn + 2 * h + 1]) : "memory");
           }
         }
@@ -542,7 +572,7 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             float v0 = 0.f, v1 = 0.f;
-            for (int src = 0; src < S; ++src) {
+            for (int src = 0; src < T.s; ++src) {
               const float2 p2 = *reinterpret_cast<const float2*>(stage + ((size_t)src * TC_BM + rbase + 8 * h) * W + (cc - sp * W));
               v0 += p2.x; v1 += p2.y;
             }
@@ -552,10 +582,20 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
       }
     }
   }
-  if (S > 1 && any_active && producer) {   // the producer warp takes part in the two split-K cluster barriers
-    __syncwarp();
-    cluster_sync_all();
-    cluster_sync_all();
+  if (first.s > 1) {
+    // every CTA of a cluster with an active tile takes part in the two split-K cluster barriers: the producer warp always,
+    // the consumers here when their own tile is idle (mixed-split clusters cover several tiles, not all of them active)
+    bool cl_active = any_active;
+    if (MIXED && tb.mixed)
+      for (int g = 0; g < S / first.s; ++g) {
+        const TcTile u = decode_mixed(g);
+        if (u.valid && u.t0 < lens[u.b] * tb.rmul + tb.p[u.pi].in_extra) cl_active = true;
+      }
+    if (cl_active && (producer || !any_active)) {
+      __syncwarp();
+      cluster_sync_all();
+      cluster_sync_all();
+    }
   }
   if (threadIdx.x == 0) TC_STAMP(7);
   __syncthreads();
@@ -569,13 +609,13 @@ template <int BN, bool DYN, int MP = TC_MAXP>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ TcBatchT<std::conditional_t<DYN, TcProblem, TcProblemBase>, MP> tb, const int* __restrict__ lens,
                const int* __restrict__ offs) {
-  conv_tc_body<BN>(tb, lens, offs);
+  conv_tc_body<BN, true>(tb, lens, offs);
 }
 // More than one wave of tiles: persistent grid (tb.persist), or one tile per CTA.
 template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc_persist_kernel(const __grid_constant__ TcBatch tb, const int* __restrict__ lens, const int* __restrict__ offs) {
-  conv_tc_body<BN>(tb, lens, offs);
+  conv_tc_body<BN, false>(tb, lens, offs);
 }
 
 // ------------------------------------------------------------------------------------------------

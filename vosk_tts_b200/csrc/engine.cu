@@ -838,6 +838,84 @@ CUtensorMap vtts_engine::make_map(const void* base, int C, long rows, int box_ro
   return m;
 }
 
+// Split-K plan of a grouped single-wave tensor-core conv launch: the tile width, the cluster size `split` (1, 2, 4 or 8) and
+// a split psplit[p] dividing it per problem; a cluster of problem p covers split / psplit[p] tiles.  Every CTA of the launch
+// runs at once, so the launch lasts as long as its longest k-loop, max_p ceil(steps_p / psplit[p]), weighted by what one
+// k-step moves into shared memory (48 KB at 64-wide tiles, 64 KB at 128-wide: 3 : 4); the per-CTA prologue and epilogue
+// are the same for every CTA and drop out.  Constraints: every cluster with an active tile co-resident (cluster_cap),
+// at least min_steps k-steps per split CTA.  Equal costs go to fewer CTAs.  With one problem (or equal k-loops) this is
+// the widest co-resident split, and 128-wide tiles exactly when they allow a wider split than 64-wide ones.
+struct TcSplitIn {
+  int n, nb, gx;                 // problems, utterances, row tiles of the grid
+  int bn;                        // 64 / 128 pinned, 0: either
+  int max_split, min_steps, n_sm;
+  int cluster_cap[2][3];         // co-resident clusters of 2/4/8 CTAs at BN 64 / 128
+  int steps[TC_MAXP], cout[TC_MAXP], in_extra[TC_MAXP];
+  const int* lens;               // [nb] utterance lengths; problem p has lens[b] * rmul + in_extra[p] rows
+  int rmul;
+  int rt(int p, int b) const { return (lens[b] * rmul + in_extra[p] + TC_BM - 1) / TC_BM; }   // active row tiles
+};
+struct TcSplitPlan {
+  int bn, split, psplit[TC_MAXP];
+};
+static TcSplitPlan tc_split_plan(const TcSplitIn& in) {
+  TcSplitPlan best{in.bn ? in.bn : 64, 1, {1, 1, 1, 1}};
+  long best_cost = -1, best_ctas = 0;
+  bool wide = true;
+  for (int p = 0; p < in.n; ++p) wide = wide && in.cout[p] >= 128;
+  for (int wi = 0; wi < 2; ++wi) {
+    const int bn = wi ? 128 : 64;
+    if (in.bn ? in.bn != bn : (wi && !wide)) continue;
+    // clusters[p][l]: clusters of problem p with an active tile when 2^l consecutive tiles share one
+    long clusters[TC_MAXP][4] = {};
+    long active = 0;
+    for (int p = 0; p < in.n; ++p) {
+      const int gyp = (in.cout[p] + bn - 1) / bn;
+      for (int b = 0; b < in.nb; ++b) clusters[p][0] += (long)in.rt(p, b) * gyp;
+      active += clusters[p][0];
+    }
+    const bool small = active <= in.n_sm;            // (no cluster split fits beside a machine-filling launch)
+    for (int p = 0; p < in.n && small; ++p) {
+      const int gyp = (in.cout[p] + bn - 1) / bn;
+      for (int l = 1; l < 4; ++l) {
+        long c = 0, last = -1;
+        for (int b = 0; b < in.nb; ++b)
+          for (int by = 0; by < gyp; ++by)
+            for (int bx = 0, rt = in.rt(p, b); bx < rt; ++bx) {
+              const long t = ((long)b * gyp + by) * in.gx + bx;
+              if ((t >> l) != last) { ++c; last = t >> l; }
+            }
+        clusters[p][l] = c;
+      }
+    }
+    for (int ls = 0; (1 << ls) <= std::min(8, in.max_split) && (ls == 0 || small); ++ls) {
+      const int sc = 1 << ls;
+      // every assignment psplit[p] = 2^e[p] (e <= ls) with at least one problem at the full cluster
+      int ncomb = 1;
+      for (int p = 0; p < in.n; ++p) ncomb *= ls + 1;
+      for (int ci = 0; ci < ncomb; ++ci) {
+        long ncl = 0, crit = 0;
+        bool full = false, ok = true;
+        for (int q = 0, r = ci; q < in.n; ++q, r /= ls + 1) {
+          const int e = r % (ls + 1), s = 1 << e;
+          ok = ok && (e == 0 || in.steps[q] >= in.min_steps * s);
+          full = full || e == ls;
+          ncl += clusters[q][ls - e];
+          crit = std::max(crit, (long)((in.steps[q] + s - 1) / s));
+        }
+        if (!ok || !full || (sc > 1 && ncl > in.cluster_cap[wi][ls - 1])) continue;
+        const long cost = crit * (wi ? 4 : 3), ctas = ncl * sc;
+        if (best_cost < 0 || cost < best_cost || (cost == best_cost && ctas < best_ctas)) {
+          best_cost = cost; best_ctas = ctas;
+          best.bn = bn; best.split = sc;
+          for (int q = 0, r = ci; q < TC_MAXP; ++q, r /= ls + 1) best.psplit[q] = q < in.n ? 1 << (r % (ls + 1)) : 1;
+        }
+      }
+    }
+  }
+  return best;
+}
+
 // Grouped tensor-core conv launch (conv_tc.cuh).  One CTA = 128 rows x 64 output channels of one problem.
 void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB) {
   // 128-wide channel tiles halve the activation traffic and run the MMA at its smem-operand optimum, but halve the CTA
@@ -858,6 +936,37 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   TcBatch& tb = tc_batch;   // per-engine scratch (2.6 KB: kept off the stack frame of every caller)
   memset(&tb, 0, sizeof(tb));
   int maxCout = 0, maxL = 0, maxNR = TC_BM;
+  // Cluster split-K for launches whose tiles leave most SMs idle (single utterances): clusters of `split` CTAs, problem
+  // p's tiles each reduced over psplit[p] of them (tc_split_plan).  Decided before the persistent path: a group with more
+  // 64-wide tiles than SMs may still fit one wave of split-K clusters at 128-wide tiles (the decoder's second MRF stage:
+  // 144 tiles at BN 64, 72 at BN 128).
+  int split = 1;
+  int psplit[TC_MAXP] = {1, 1, 1, 1};
+  int gx = 0;                                // row tiles of the grid
+  for (const TcSpec& q : ps) gx = std::max(gx, (maxLen * rmul + q.in_extra + TC_BM - 1) / TC_BM);
+  if (tc_tall <= 0 && tc_split != 1 && (tc_bn == 64 || tc_bn == 128 || BN == 64)) {
+    const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
+    TcSplitIn in;
+    in.n = (int)ps.size(); in.nb = nB; in.gx = gx;
+    in.bn = (tc_bn == 64 || tc_bn == 128) ? tc_bn : 0;
+    in.max_split = tc_split > 1 ? tc_split : 8;
+    in.min_steps = tc_min_steps;
+    in.n_sm = n_sm;
+    memcpy(in.cluster_cap, tc_cluster_cap, sizeof(in.cluster_cap));
+    in.lens = hl.data(); in.rmul = rmul;
+    for (int p = 0; p < in.n; ++p) {
+      in.steps[p] = ps[p].Cin / TC_BK * ps[p].k;
+      in.cout[p] = ps[p].Cout;
+      in.in_extra[p] = ps[p].in_extra;
+    }
+    const TcSplitPlan pl = tc_split_plan(in);
+    BN = pl.bn;
+    split = pl.split;
+    for (int p = 0; p < in.n; ++p) psplit[p] = pl.psplit[p];
+  }
+  bool mixed = false;                        // (single-wave image only: split > 1)
+  for (size_t p = 0; p < ps.size(); ++p) mixed |= psplit[p] != split;
+  if (!mixed) for (int& s : psplit) s = split;
   // "Tall" activation tiles (one TMA box of 128 + (k-1)*dil rows per channel chunk, the taps read it through row-shifted
   // descriptors) cut the L2 -> shared-memory traffic of a k-step from A + W to A/k + W.  On machine-filling launches the
   // mainloop is bound by exactly that traffic (64 KB per k-step and SM at 128-wide tiles against 768 tensor-pipe cycles),
@@ -869,7 +978,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     grid_tiles += (long)((maxLen * rmul + q.in_extra + TC_BM - 1) / TC_BM) * ((q.Cout + BN - 1) / BN) * nB;
   }
   const bool big = tc_persist == 2 || (tc_persist && grid_tiles > (long)tc_persist_min * n_sm);   // (2: forced, for tests)
-  bool tall = tc_tall > 0 || (tc_tall == 0 && big);
+  bool tall = split == 1 && (tc_tall > 0 || (tc_tall == 0 && big));
   for (const TcSpec& q : ps) {
     const int nr = TC_BM + (q.k - 1) * q.dil;
     if (nr > 192) tall = false;              // shared-memory budget of the activation ring (and TMA box <= 256)
@@ -895,36 +1004,6 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     if (same) cn = (ny % 4 == 0) ? 4 : (ny % 2 == 0 ? 2 : 1);
     if (tc_mc == 2 && same && ny % 2 == 0) cn = 2;          // VTTS_TC_MULTICAST=2: pairs only
   }
-  // Cluster split-K for launches that leave most SMs idle (single utterances): S CTAs share the k-steps of one tile.
-  // The widest split whose clusters are all co-resident wins; 128-wide channel tiles are taken when they allow a
-  // wider split than 64-wide ones (same k-steps per CTA-step, half the CTAs per tile row).
-  int split = 1;
-  if (!tall && tc_split != 1) {
-    const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
-    long active[2] = {0, 0};
-    int minsteps = 1 << 30;
-    bool wide = true;
-    for (const TcSpec& q : ps) {
-      minsteps = std::min(minsteps, q.Cin / TC_BK * q.k);
-      if (q.Cout < 128) wide = false;
-      for (int b = 0; b < nB; ++b) {
-        const long rt = (hl[b] * rmul + q.in_extra + TC_BM - 1) / TC_BM;
-        active[0] += rt * ((q.Cout + 63) / 64);
-        active[1] += rt * ((q.Cout + 127) / 128);
-      }
-    }
-    const int cap = tc_split > 1 ? tc_split : 8;
-    auto best = [&](int wi) {
-      for (int S = 8, si = 2; S >= 2; S >>= 1, --si)
-        if (S <= cap && minsteps >= tc_min_steps * S && active[wi] * S <= (long)tc_cluster_cap[wi][si] * S) return S;
-      return 1;
-    };
-    if (tc_bn == 64 || tc_bn == 128) split = best(tc_bn == 128);
-    else if (BN == 64) {
-      const int s64 = best(0), s128 = wide ? best(1) : 1;
-      if (s128 > s64) { BN = 128; split = s128; } else split = s64;
-    }
-  }
   if (split > 1) cn = 1;
   int np = 0;
   for (const TcSpec& q : ps) {
@@ -935,11 +1014,19 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   if (np == 3) { tall = false; cn = 1; }
   tb.np = np;
   tb.ast = (np == 3 || tall) ? 2 : (BN == 128 ? tc_ast<128>() : tc_ast<64>());
-  long tiles_all = 0;                        // the launch's tile space (one wave or less: the one-tile-per-CTA kernel)
-  {
-    int mc = 0, ml = 0;
-    for (const TcSpec& q : ps) { mc = std::max(mc, q.Cout); ml = std::max(ml, maxLen * rmul + q.in_extra); }
-    tiles_all = (long)((ml + TC_BM - 1) / TC_BM) * ((mc + BN - 1) / BN) * nB * (long)ps.size() * split;
+  long tiles_all = 0;                        // the launch's CTAs (one wave or less: the one-tile-per-CTA kernel)
+  int ncl = 0;                               // mixed splits: clusters of the grid
+  if (mixed) {
+    for (size_t p = 0; p < ps.size(); ++p) {
+      tb.p[p].cl0 = ncl;
+      const int m = split / psplit[p];
+      ncl += (int)(((long)gx * ((ps[p].Cout + BN - 1) / BN) * nB + m - 1) / m);
+    }
+    tiles_all = (long)ncl * split;
+  } else {
+    int mc = 0;
+    for (const TcSpec& q : ps) mc = std::max(mc, q.Cout);
+    tiles_all = (long)gx * ((mc + BN - 1) / BN) * nB * (long)ps.size() * split;
   }
   const bool one_wave = tiles_all <= n_sm && !(tc_persist == 2 && split == 1 && cn == 1);
   tb.wst = np == 3 ? (BN == 128 ? 2 : 3) : (BN == 128 ? tc_wst<128>() : tc_wst<64>());
@@ -972,6 +1059,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     P.Cin = q.Cin; P.Cout = q.Cout; P.k = q.k; P.dil = q.dil; P.pad = q.pad;
     P.out_mul = q.out_mul; P.out_add = q.out_add; P.in_extra = q.in_extra; P.out_seq_extra = q.out_seq_extra;
     P.alpha = q.alpha; P.pl_slope = q.pl_slope;
+    P.split = psplit[i];
     REQUIRE(q.in.C == q.Cin, VTTS_ERR_INVALID, "plane width must equal the conv input channels");
     maxCout = std::max(maxCout, q.Cout);
     maxL = std::max(maxL, maxLen * rmul + q.in_extra);
@@ -979,11 +1067,14 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   tb.n = (int)ps.size();
   tb.rmul = rmul;
   tb.dbg = tc_dbg;
+  tb.nb = nB;
   dim3 grid((maxL + TC_BM - 1) / TC_BM, (maxCout + BN - 1) / BN, nB * tb.n * split);
   if (grid.x == 0) return;
   tb.wpre = one_wave ? 1 : 0;
   // machine-filling launches: one resident CTA per SM walks the tile space (conv_tc.cuh)
   tb.gx = (int)grid.x; tb.gy = (int)grid.y; tb.gz = (int)grid.z;
+  tb.mixed = mixed ? 1 : 0;
+  if (mixed) grid = dim3(1, 1, (unsigned)tiles_all);
   tb.persist = 0;
   tb.wmc = 1;
   if (split == 1 && cn == 1 && !tb.wpre && (tc_persist == 2 || (tc_persist && (long)grid.x * grid.y * grid.z > (long)tc_persist_min * n_sm))) {
@@ -999,6 +1090,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     r.use_tc = 1; r.bn = BN; r.split = split; r.tall = tb.tall; r.cn = cn; r.wmc = tb.wmc; r.persist = tb.persist; r.np = tb.np;
     r.ast = tb.ast; r.wst = tb.wst; r.image = single_wave_image ? (dyn_image ? 1 : 0) : 2;
     r.grid_x = (int)grid.x; r.grid_y = (int)grid.y; r.grid_z = (int)grid.z;
+    for (size_t p = 0; p < ps.size(); ++p) r.psplit[p] = psplit[p];
     note_conv(r);
   }
   if (profiling) {
@@ -1380,8 +1472,9 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     } else {
       for (int d = 0; d < nd; ++d) {
         std::vector<TcSpec> p1(nk), p2(nk);
-        // CTAs are dispatched in blockIdx.z order = problem order: the resblock with the longest k-loop (largest kernel
-        // size) goes first, so that a second wave holds the short ones
+        // Launches of more than one wave (long utterances, batches) walk the tiles in problem order: the resblock with the
+        // longest k-loop (largest kernel size) goes first, so that the last tiles are short ones.  Single-wave launches give
+        // each resblock its own split instead (tc_split_plan), where the order does not matter.
         for (int j = 0; j < nk; ++j) rb_pair(j, d, p1[mrf_heavy_first ? nk - 1 - j : j], p2[mrf_heavy_first ? nk - 1 - j : j]);
         launch_tc(p1, rm, fl, fo, maxFrm, B);
         launch_tc(p2, rm, fl, fo, maxFrm, B);
@@ -3366,6 +3459,32 @@ int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_
       *n_out = n;
     }
   });
+}
+
+// Host-only restatement of launch_tc's split-K plan (tc_split_plan) for tests: no device, no engine.
+int vtts_tc_split_plan(int n, const int* cin, const int* cout, const int* k, const int* in_extra, int B, const int* lens,
+                       int rmul, int max_len, int bn, int max_split, int min_steps, int n_sm, const int* cluster_cap, int* plan) {
+  if (n < 1 || n > TC_MAXP || B < 1 || rmul < 1 || max_len < 0 || !cin || !cout || !k || !in_extra || !lens || !cluster_cap || !plan)
+    return VTTS_ERR_INVALID;
+  if ((bn != 0 && bn != 64 && bn != 128) || max_split < 1 || min_steps < 1 || n_sm < 1) return VTTS_ERR_INVALID;
+  TcSplitIn in;
+  in.n = n; in.nb = B; in.gx = 0;
+  in.bn = bn; in.max_split = max_split; in.min_steps = min_steps; in.n_sm = n_sm;
+  memcpy(in.cluster_cap, cluster_cap, sizeof(in.cluster_cap));
+  in.lens = lens; in.rmul = rmul;
+  for (int p = 0; p < n; ++p) {
+    if (cin[p] < TC_BK || cin[p] % TC_BK || k[p] < 1 || cout[p] < 1 || in_extra[p] < 0) return VTTS_ERR_INVALID;
+    in.steps[p] = cin[p] / TC_BK * k[p];
+    in.cout[p] = cout[p];
+    in.in_extra[p] = in_extra[p];
+    in.gx = std::max(in.gx, (max_len * rmul + in_extra[p] + TC_BM - 1) / TC_BM);
+  }
+  for (int b = 0; b < B; ++b)
+    if (lens[b] < 0 || lens[b] > max_len) return VTTS_ERR_INVALID;
+  const TcSplitPlan pl = tc_split_plan(in);
+  plan[0] = pl.bn; plan[1] = pl.split;
+  for (int p = 0; p < TC_MAXP; ++p) plan[2 + p] = p < n ? pl.psplit[p] : 0;
+  return VTTS_OK;
 }
 
 int vtts_profile_read_tc(vtts_handle h, double* ms, uint64_t* launches, double* flops) {

@@ -49,7 +49,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_profile_read_tc", "vtts_timeline", "vtts_infer", "vtts_infer_dev",
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
-           "vtts_debug_conv_log"]
+           "vtts_debug_conv_log", "vtts_tc_split_plan"]
 
 CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
 
@@ -74,10 +74,13 @@ class ConvOverrides(C.Structure):
 
 class ConvReport(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("use_tc", "bn", "split", "tall", "cn", "wmc", "persist", "np", "ast", "wst", "image",
-                                         "S", "G", "grid_x", "grid_y", "grid_z")]
+                                         "S", "G", "grid_x", "grid_y", "grid_z")] + [("psplit", C.c_int32 * 4)]
 
     def as_dict(self):
-        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+        """psplit is a list of the per-problem splits (as many as the launch had problems)."""
+        d = {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "psplit"}
+        d["psplit"] = [int(s) for s in self.psplit if s]
+        return d
 
 
 ATTN_KERNELS = {"auto": 0, "tc": 1, "split": 2, "r1": 3, "r4": 4, "ffma": 5}    # VTTS_ATTN_*
@@ -192,6 +195,8 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_conv.restype = i32
     lib.vtts_debug_conv_log.argtypes = [vp, i32, C.POINTER(ConvReport), i32, C.POINTER(C.c_int)]
     lib.vtts_debug_conv_log.restype = i32
+    lib.vtts_tc_split_plan.argtypes = [i32, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp]
+    lib.vtts_tc_split_plan.restype = i32
     lib.vtts_speculation_stats.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.vtts_speculation_stats.restype = i32
     lib.vtts_host_timings.argtypes = [vp, C.POINTER(C.c_double), i32]
@@ -206,6 +211,23 @@ def load_library(build_if_missing=True):
         fn.restype = i32
     _LIB = lib
     return lib
+
+
+def tc_split_plan(problems, lens, rmul, n_sm, cluster_cap, max_len=None, bn=0, max_split=8, min_steps=2):
+    """The engine's split-K plan of one grouped tensor-core conv launch (vtts_tc_split_plan), on the host alone.
+    problems: list of dicts with Cin, Cout, k and optionally in_extra; cluster_cap: co-resident clusters of 2/4/8 CTAs at
+    BN 64, then at BN 128 (6 ints).  Returns (BN, cluster size, [split of each problem])."""
+    lib = load_library()
+    ints = lambda v: np.ascontiguousarray(v, dtype=np.int32)
+    cin, cout, k = (ints([q[n] for q in problems]) for n in ("Cin", "Cout", "k"))
+    extra, lens, cap = ints([q.get("in_extra", 0) for q in problems]), ints(lens), ints(cluster_cap)
+    plan = np.zeros(6, np.int32)
+    st = lib.vtts_tc_split_plan(len(problems), _ptr(cin), _ptr(cout), _ptr(k), _ptr(extra), lens.size, _ptr(lens), int(rmul),
+                                int(lens.max() if max_len is None else max_len), int(bn), int(max_split), int(min_steps),
+                                int(n_sm), _ptr(cap), _ptr(plan))
+    if st != 0:
+        raise VttsError(st, "vtts_tc_split_plan: invalid arguments")
+    return int(plan[0]), int(plan[1]), [int(s) for s in plan[2:2 + len(problems)]]
 
 
 def make_c_config(cfg, precision=0):
