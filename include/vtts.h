@@ -297,6 +297,29 @@ int vtts_convert_spec(vtts_handle h, const float* spec, const int64_t* spec_leng
                       const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed, float* out_wav,
                       int64_t out_ld, int64_t* out_frames);
 
+/* Forced alignment: the text-to-frame alignment at the head of SynthesizerTrn.forward (models.py:1632-1660).  One call =
+ * text encoder enc_p on the ids (speaker sid), spectrogram front end, enc_q and the forward flow on the recording (g = the
+ * same speaker; none for a single-speaker model, n_speakers <= 1, where sid may be NULL), the Gaussian log-likelihood
+ * neg_cent of every frame under every token's prior, and Monotonic Alignment Search; no host synchronisation inside.  The
+ * noise-scaled MAS of models.py:1653-1655 (a training regulariser) is never added.
+ *   ids          int64 [B, t_max], id_lengths[b] tokens valid (1 <= t_x <= min(t_max, 2048, frames[b]))
+ *   wav ... seed as vtts_convert: noise_scale 1 is the reference's forward, 0 aligns the posterior mean
+ *   durations    out int32 [B, t_max]: frames of each token (the reference's w = attn.sum(2)), 0 past id_lengths[b]
+ *   token_of_frame  out int32 [B, tof_ld] or NULL: the token each frame is aligned to, -1 past out_frames[b]
+ *   score        out float [B] or NULL: log-likelihood of the best path (sum of neg_cent along it, fp32)
+ *   out_frames   out int64 [B]
+ * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: the blob has no enc_q (model.onnx never has it: pack with
+ * posterior=True), an odd flow_n_flows, a phoneme id out of [0, n_vocab), a speaker id out of range for a multi-speaker
+ * model, a clip too short for the reflect padding, t_x < 1, t_x > frames (no monotonic path exists) or t_x > 2048.
+ * VTTS_ERR_CAPACITY: tof_ld < max(frames) or q_ld < max(frames). */
+int vtts_align(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid, const float* wav,
+               const int64_t* wav_lengths, int B, int64_t wav_ld, float noise_scale, const float* noise_q, int q_ld, uint64_t seed,
+               int32_t* durations, int32_t* token_of_frame, int64_t tof_ld, float* score, int64_t* out_frames);
+/* Same from the posterior encoder's input features: spec float [B, spec_channels, spec_ld], spec_lengths[b] frames valid. */
+int vtts_align_spec(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid, const float* spec,
+                    const int64_t* spec_lengths, int B, int64_t spec_ld, float noise_scale, const float* noise_q, int q_ld, uint64_t seed,
+                    int32_t* durations, int32_t* token_of_frame, int64_t tof_ld, float* score, int64_t* out_frames);
+
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are
  * read with vtts_last_error(NULL) on the calling thread.

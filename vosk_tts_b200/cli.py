@@ -1,5 +1,6 @@
 """`vosk-tts` command line (flags of vosk_tts/cli.py:12-43) on top of the CUDA engine."""
 import argparse
+import json
 import logging
 import sys
 
@@ -22,6 +23,8 @@ def main(argv=None):
     p.add_argument("--device", type=int, default=0, help="CUDA device index (extension)")
     p.add_argument("--convert-from", type=str, help="voice conversion (extension): re-voice this mono WAV as --speaker")
     p.add_argument("--source-speaker", type=int, help="speaker id of the --convert-from recording")
+    p.add_argument("--align", type=str, metavar="WAV",
+                   help="forced alignment (extension): print the phoneme segments of --input in this mono WAV as JSON")
     args = p.parse_args(argv)
     logging.getLogger().setLevel(args.log_level.upper())
     if args.list_models:
@@ -35,6 +38,12 @@ def main(argv=None):
             p.error("--convert-from needs --source-speaker and --speaker (the target)")
         model = Model(args.model, args.model_name, args.lang, device=args.device, voice_conversion=True)
         Synth(model).convert(args.convert_from, args.output, args.source_speaker, args.speaker)
+        return 0
+    if args.align:
+        if not args.input:
+            p.error("--align needs --input (the transcript of the recording)")
+        model = Model(args.model, args.model_name, args.lang, device=args.device, voice_conversion=True)
+        print(json.dumps(Synth(model).align(args.align, args.input, speaker_id=args.speaker)))
         return 0
     if not args.input:
         logging.info("Please specify input text or file")

@@ -557,6 +557,9 @@ struct vtts_engine {
   P1Pin p1_layout(int t_max, bool eps);
   void stage1(const int* ids_packed_host, const int* sid_host, int t_max, const float* noise_dp_host);
   void finish1();
+  Planes enc_px;                               // the text encoder's output planes (precision modes 2 / 3), read by prior_stats
+  void text_encoder(const float* cond, int cond_ld);
+  void prior_stats();
   void phase1(const int* ids_packed_host, const int64_t* d_ids64, int t_max, const int64_t* d_sid64, const int* sid_host,
               const float* noise_dp, bool noise_on_device);
   void phase2(const float* noise_z, int z_ld, bool noise_on_device, bool run_decoder = true);
@@ -595,7 +598,15 @@ struct vtts_engine {
   Buf<char> h_pin_vc;
   struct VcPin { int *frm_len, *frm_off, *clip_len, *sid; float *prm, *in, *eps; };
   VcPin vc_layout(bool from_spec, bool eps);
+  float* vc_upload(bool from_spec, bool eps);
+  float* cond_src(bool tgt);
+  void posterior_side(bool from_spec, const float* noise, const float* csrc);
   void convert_enqueue(bool from_spec, bool eps);
+
+  // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
+  Buf<float> d_ncent, d_ncent_dbg, d_ascore;       // neg_cent [B][maxFrm][maxTok] (MAS accumulates in place), scores [B]
+  Buf<int> d_adur, d_atof;                         // durations (token rows), token of every frame (frame rows)
+  void align_enqueue(bool from_spec, bool eps);
 };
 
 namespace {
@@ -1671,7 +1682,7 @@ void vtts_engine::dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, c
 void vtts_engine::phase1(const int* ids_packed_host, const int64_t* d_ids64, int t_max, const int64_t* d_sid64,
                          const int* sid_host, const float* noise_dp, bool noise_on_device) {
   const vtts_config& c = cfg;
-  const int H = c.hidden_channels, I = c.inter_channels, D = c.dp_filter_channels, Fc = c.filter_channels;
+  const int H = c.hidden_channels, D = c.dp_filter_channels;
   const size_t T = (size_t)Ttok;
   if (!capturing) CK(cudaEventRecord(ev[0], stream));
   // ---- inputs (host data was staged into h_pin_in by stage1(); only device work is enqueued here)
@@ -1719,63 +1730,8 @@ void vtts_engine::phase1(const int* ids_packed_host, const int64_t* d_ids64, int
     CK(cudaGetLastError());
     ++launches;
   }
-  const float* spk_vec = (has_g && r_spk >= 0) ? condv + r_spk : nullptr;
-
-  // ---- text encoder (models.py:317-326)
-  float* x = ensure(d_x, T * H);
-  float* xb = ensure(d_xb, T * H);
-  float* qkv = ensure(d_qkv, T * 3 * H);
-  float* ao = ensure(d_ao, T * H);
-  float* y = ensure(d_y, T * H);
-  float* ffh = ensure(d_ffh, T * Fc);
-  float* stats = ensure(d_stats, T * 2 * I);
-  Planes px, px1, pao, pff, pqkv;
-  if (enc_on_tc) {
-    begin_planes();
-    px = planes(60, (long)T, 1, H, 0, enc_three); px1 = planes(61, (long)T, 1, H, 0, enc_three);
-    pao = planes(62, (long)T, 1, H, 0, enc_three); pff = planes(63, (long)T, 1, Fc, 0, enc_three);
-    pqkv = planes(59, (long)T, 1, 3 * H);
-    flush_tails(tl, to);
-  }
-  {
-    dim3 g(maxTok, B);
-    klaunch(embed_kernel, dim3(g), dim3(64), (size_t)(0), ids, enc_emb, x, tl, to, H, sqrtf((float)H), c.n_vocab,
-            (spk_vec && c.cond_layer_idx == 0) ? spk_vec : (const float*)nullptr, condR, px.hi, px.lo, px.mid);
-    CK(cudaGetLastError());
-    ++launches;
-  }
-  for (int i = 0; i < c.n_layers; ++i) {
-    const float* va = (spk_vec && c.cond_layer_idx == i + 1) ? spk_vec : nullptr;
-    if (!enc_on_tc) {
-      encoder_layer(enc[i], x, xb, qkv, ao, y, ffh, H, Fc, c.kernel_size, tl, to, maxTok, va, condR, nullptr);
-      continue;
-    }
-    // precision mode 2: same layer with the four convs on wgmma (attentions.py:57-63)
-    const EncLayerW& L = enc[i];
-    const int ks = c.kernel_size;
-    dim3 lg((maxTok + 3) / 4, B);
-    if (attn_use_tc(L, H, tl, maxTok)) {
-      { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.out = pqkv; q.pl_slope = 1.f;
-        launch_tc({q}, 1, tl, to, maxTok, B); }
-      launch_attn_tc(pqkv, nullptr, &pao, L, H, tl, to, maxTok);
-    } else {
-      { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.y = qkv; q.ldy = 3 * H;
-        launch_tc({q}, 1, tl, to, maxTok, B); }
-      launch_attn(qkv, ao, L, H, tl, to, maxTok, &pao);
-    }
-    { TcSpec q; q.in = pao; q.w = L.t_o; q.bias = L.o.b; q.Cin = H; q.Cout = H; q.y = y; q.ldy = H;
-      launch_tc({q}, 1, tl, to, maxTok, B); }
-    klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, x, y, L.ln1.g, L.ln1.b, (const float*)nullptr, (const float*)nullptr, 0, xb, tl, to, H, px1.hi, px1.lo, px1.mid);
-    ++launches;
-    { TcSpec q; q.in = px1; q.w = L.t_ffn1; q.bias = L.ffn1.b; q.Cin = H; q.Cout = Fc; q.k = ks; q.pad = (ks - 1) / 2;
-      q.epi = TCE_RELU; q.out = pff; q.pl_slope = 1.f;
-      launch_tc({q}, 1, tl, to, maxTok, B); }
-    { TcSpec q; q.in = pff; q.w = L.t_ffn2; q.bias = L.ffn2.b; q.Cin = Fc; q.Cout = H; q.k = ks; q.pad = (ks - 1) / 2;
-      q.y = y; q.ldy = H;
-      launch_tc({q}, 1, tl, to, maxTok, B); }
-    klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, xb, y, L.ln2.g, L.ln2.b, (const float*)nullptr, va, condR, x, tl, to, H, px.hi, px.lo, px.mid);
-    ++launches;
-  }
+  text_encoder(condv, condR);
+  float* x = d_x.p;
   // (the prior projection enc_p.proj, models.py:323, is only needed by phase 2: it is enqueued at the end of this phase so
   //  that it runs while the host picks up the utterance lengths)
   if (!capturing) CK(cudaEventRecord(ev[2], stream));
@@ -1840,11 +1796,90 @@ void vtts_engine::phase1(const int* ids_packed_host, const int64_t* d_ids64, int
     CK(cudaMemcpyAsync(p_len + B, fo, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
   }
   // prior statistics m_p, logs_p (models.py:323-325): overlaps the host's round trip between the two phases
+  prior_stats();
+}
+
+// TextEncoder up to its projection (models.py:317-322): embedding, the n_layers relative-attention layers in the precision
+// mode's variant -> d_x (and, on the tensor cores, its planes enc_px).  cond: [B][cond_ld] conditioning rows of the speaker
+// (the spk_emb_linear rows at r_spk are read), null for an unconditioned model.  Token shape and d_tok_len / d_tok_off / d_ids
+// must be set.  Used by phase 1 (TTS) and by the alignment.
+void vtts_engine::text_encoder(const float* cond, int cond_ld) {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, Fc = c.filter_channels;
+  const size_t T = (size_t)Ttok;
+  const int* tl = d_tok_len.p;
+  const int* to = d_tok_off.p;
+  const int* ids = d_ids.p;
+  const float* spk_vec = (cond && r_spk >= 0) ? cond + r_spk : nullptr;
+
+  // ---- text encoder (models.py:317-326)
+  float* x = ensure(d_x, T * H);
+  float* xb = ensure(d_xb, T * H);
+  float* qkv = ensure(d_qkv, T * 3 * H);
+  float* ao = ensure(d_ao, T * H);
+  float* y = ensure(d_y, T * H);
+  float* ffh = ensure(d_ffh, T * Fc);
+  Planes& px = enc_px;
+  Planes px1, pao, pff, pqkv;
   if (enc_on_tc) {
-    TcSpec q; q.in = px; q.w = tc_encproj; q.bias = enc_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
+    begin_planes();
+    px = planes(60, (long)T, 1, H, 0, enc_three); px1 = planes(61, (long)T, 1, H, 0, enc_three);
+    pao = planes(62, (long)T, 1, H, 0, enc_three); pff = planes(63, (long)T, 1, Fc, 0, enc_three);
+    pqkv = planes(59, (long)T, 1, 3 * H);
+    flush_tails(tl, to);
+  }
+  {
+    dim3 g(maxTok, B);
+    klaunch(embed_kernel, dim3(g), dim3(64), (size_t)(0), ids, enc_emb, x, tl, to, H, sqrtf((float)H), c.n_vocab,
+            (spk_vec && c.cond_layer_idx == 0) ? spk_vec : (const float*)nullptr, cond_ld, px.hi, px.lo, px.mid);
+    CK(cudaGetLastError());
+    ++launches;
+  }
+  for (int i = 0; i < c.n_layers; ++i) {
+    const float* va = (spk_vec && c.cond_layer_idx == i + 1) ? spk_vec : nullptr;
+    if (!enc_on_tc) {
+      encoder_layer(enc[i], x, xb, qkv, ao, y, ffh, H, Fc, c.kernel_size, tl, to, maxTok, va, cond_ld, nullptr);
+      continue;
+    }
+    // precision mode 2: same layer with the four convs on wgmma (attentions.py:57-63)
+    const EncLayerW& L = enc[i];
+    const int ks = c.kernel_size;
+    dim3 lg((maxTok + 3) / 4, B);
+    if (attn_use_tc(L, H, tl, maxTok)) {
+      { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.out = pqkv; q.pl_slope = 1.f;
+        launch_tc({q}, 1, tl, to, maxTok, B); }
+      launch_attn_tc(pqkv, nullptr, &pao, L, H, tl, to, maxTok);
+    } else {
+      { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.y = qkv; q.ldy = 3 * H;
+        launch_tc({q}, 1, tl, to, maxTok, B); }
+      launch_attn(qkv, ao, L, H, tl, to, maxTok, &pao);
+    }
+    { TcSpec q; q.in = pao; q.w = L.t_o; q.bias = L.o.b; q.Cin = H; q.Cout = H; q.y = y; q.ldy = H;
+      launch_tc({q}, 1, tl, to, maxTok, B); }
+    klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, x, y, L.ln1.g, L.ln1.b, (const float*)nullptr, (const float*)nullptr, 0, xb, tl, to, H, px1.hi, px1.lo, px1.mid);
+    ++launches;
+    { TcSpec q; q.in = px1; q.w = L.t_ffn1; q.bias = L.ffn1.b; q.Cin = H; q.Cout = Fc; q.k = ks; q.pad = (ks - 1) / 2;
+      q.epi = TCE_RELU; q.out = pff; q.pl_slope = 1.f;
+      launch_tc({q}, 1, tl, to, maxTok, B); }
+    { TcSpec q; q.in = pff; q.w = L.t_ffn2; q.bias = L.ffn2.b; q.Cin = Fc; q.Cout = H; q.k = ks; q.pad = (ks - 1) / 2;
+      q.y = y; q.ldy = H;
+      launch_tc({q}, 1, tl, to, maxTok, B); }
+    klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, xb, y, L.ln2.g, L.ln2.b, (const float*)nullptr, va, cond_ld, x, tl, to, H, px.hi, px.lo, px.mid);
+    ++launches;
+  }
+}
+
+// Prior statistics m_p, logs_p (models.py:323-325): enc_p.proj of text_encoder's output -> d_stats [Ttok][2I].
+void vtts_engine::prior_stats() {
+  const int H = cfg.hidden_channels, I = cfg.inter_channels;
+  const int* tl = d_tok_len.p;
+  const int* to = d_tok_off.p;
+  float* stats = ensure(d_stats, (size_t)Ttok * 2 * I);
+  if (enc_on_tc) {
+    TcSpec q; q.in = enc_px; q.w = tc_encproj; q.bias = enc_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
     launch_tc({q}, 1, tl, to, maxTok, B);
   } else {
-    launch_conv({mk(enc_proj, x, H, 0, stats, 2 * I, 0, 1, 0)}, 1, tl, to, maxTok, B);
+    launch_conv({mk(enc_proj, d_x.p, H, 0, stats, 2 * I, 0, 1, 0)}, 1, tl, to, maxTok, B);
   }
 }
 
@@ -2220,11 +2255,11 @@ vtts_engine::VcPin vtts_engine::vc_layout(bool from_spec, bool eps) {
   return pp;
 }
 
-void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
+// Inputs of a call on the posterior side, from the pinned staging (vc_layout) to the device: frame lengths / offsets, clip
+// lengths and speaker ids, the per-call scalars, the waveform or spectrogram, and the posterior eps (returned; null: Philox).
+float* vtts_engine::vc_upload(bool from_spec, bool eps) {
   const vtts_config& c = cfg;
-  const int H = c.hidden_channels, I = c.inter_channels;
-  const size_t F = (size_t)Tfrm;
-  if (!capturing) CK(cudaEventRecord(ev[4], stream));
+  const int I = c.inter_channels;
   VcPin pp = vc_layout(from_spec, eps);
   int* fl = ensure(d_frm_len, B);
   int* fo = ensure(d_frm_off, B + 1);
@@ -2242,20 +2277,38 @@ void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
     noise = ensure(d_vnoise, (size_t)B * I * maxFrm);
     CK(cudaMemcpyAsync(noise, pp.eps, (size_t)B * I * maxFrm * sizeof(float), cudaMemcpyHostToDevice, stream));
   }
-  // ---- g_src / g_tgt (models.py:1712-1713) and every cond row of both, one launch: src -> d_vcsrc [B][condR + q_R]
-  //      (the TTS rows, then enc_q's), tgt -> d_condv [B][condR] (where the reverse flow and the decoder read them)
+  return noise;
+}
+
+// Conditioning rows of g_src (rows [0, condR) of the stacked TTS matrix, then enc_q's q_R rows) -> d_vcsrc [B][condR + q_R];
+// with `tgt` also g_tgt's TTS rows -> d_condv [B][condR], in the same launch (cond_vc_kernel, sid from d_vint).
+float* vtts_engine::cond_src(bool tgt) {
   const int qld = condR + q_R;
   float* csrc = ensure(d_vcsrc, (size_t)B * qld);
-  float* ctgt = ensure(d_condv, (size_t)B * condR);
-  klaunch(cond_vc_kernel, dim3((qld + 7) / 8, 2 * B), dim3(256), (size_t)(c.gin_channels * sizeof(float)), emb_g, (const int*)(vi + B),
-          cond_w, cond_b, condR, q_cond_w, q_cond_b, q_R, csrc, ctgt, c.gin_channels, B, c.n_speakers);
+  float* ctgt = tgt ? ensure(d_condv, (size_t)B * condR) : nullptr;
+  klaunch(cond_vc_kernel, dim3((qld + 7) / 8, tgt ? 2 * B : B), dim3(256), (size_t)(cfg.gin_channels * sizeof(float)), emb_g,
+          (const int*)(d_vint.p + B), cond_w, cond_b, condR, q_cond_w, q_cond_b, q_R, csrc, ctgt, cfg.gin_channels, B, cfg.n_speakers);
   CK(cudaGetLastError());
   ++launches;
+  return csrc;
+}
+
+// Front end, posterior encoder and forward flow (models.py:836-842, 750-753): the uploaded waveform / spectrogram -> z
+// (vc_z) -> z_p = flow(z, g_src) in d_z.  csrc: g_src's rows [B][condR + q_R] (cond_src), null for an unconditioned model.
+// Opens the phase's plane collection (the flow's WN planes, also used by enc_q) for the frame shape.
+void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc) {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, I = c.inter_channels;
+  const size_t F = (size_t)Tfrm;
+  const int qld = condR + q_R;
+  const int* fl = d_frm_len.p;
+  const int* fo = d_frm_off.p;
+  const int* vi = d_vint.p;
+  const float* vin = d_vin.p;
   // ---- enc_q input rows [F][spec_pad]
   float* feat = ensure(d_vfeat, F * spec_pad);
   if (from_spec) {
-    klaunch(spec_pack_kernel, dim3(maxFrm, B), dim3(128), (size_t)0, (const float*)vin, c.spec_channels, maxFrm, (const int*)fl,
-            (const int*)fo, feat, spec_pad);
+    klaunch(spec_pack_kernel, dim3(maxFrm, B), dim3(128), (size_t)0, vin, c.spec_channels, maxFrm, fl, fo, feat, spec_pad);
     CK(cudaGetLastError());
     ++launches;
   } else {
@@ -2263,13 +2316,13 @@ void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
     const bool mel = c.use_mel_posterior_encoder != 0;
     float* lin = mel ? ensure(d_vlin, F * nbins) : feat;
     dim3 g((maxFrm + ST_TM - 1) / ST_TM, c.filter_length / ST_TN, B);
-    klaunch(stft_mag_kernel, g, dim3(ST_THREADS), (size_t)0, (const float*)vin, (long)vc_wld, (const int*)vi, stft_basis, c.filter_length,
-            c.hop_length, vc_pad, (const int*)fl, (const int*)fo, lin, mel ? nbins : spec_pad);
+    klaunch(stft_mag_kernel, g, dim3(ST_THREADS), (size_t)0, vin, (long)vc_wld, vi, stft_basis, c.filter_length,
+            c.hop_length, vc_pad, fl, fo, lin, mel ? nbins : spec_pad);
     CK(cudaGetLastError());
     ++launches;
     if (mel) {
       klaunch(mel_log_kernel, dim3((maxFrm + MEL_ROWS - 1) / MEL_ROWS, B), dim3(MEL_THREADS), (size_t)MEL_ROWS * nbins * sizeof(float),
-              (const float*)lin, nbins, mel_fb, nbins, c.n_mel_channels, (const int*)fl, (const int*)fo, feat, spec_pad);
+              (const float*)lin, nbins, mel_fb, nbins, c.n_mel_channels, fl, fo, feat, spec_pad);
       CK(cudaGetLastError());
       ++launches;
     }
@@ -2291,7 +2344,7 @@ void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
     if (q_tc) { p.p_hi = flp.pwx.hi; p.p_lo = flp.pwx.lo; p.ldp = H; p.pl_slope = 1.f; }
     launch_conv({p}, 1, fl, fo, maxFrm, B);
   }
-  const float* qcond = csrc + condR;
+  const float* qcond = csrc ? csrc + condR : nullptr;
   if (q_tc) {
     wn_tc(qt_in, q_in, qt_rsx, q_rsx, qt_rss, q_rss, Q_LAYERS, Q_KERNEL, 1, h, skip, flp.pwx, flp.pacts, flp.pskip, qcond, qld, fl, fo);
     TcSpec q; q.in = flp.pskip; q.w = qt_proj; q.bias = q_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
@@ -2300,20 +2353,88 @@ void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
     wn_ffma(q_in, q_rsx, q_rss, Q_LAYERS, Q_KERNEL, 1, h, acts, skip, qcond, qld, fl, fo);
     launch_conv({mk(q_proj, skip, H, 0, stats, 2 * I, 0, 1, 0)}, 1, fl, fo, maxFrm, B);
   }
-  klaunch(posterior_sample_kernel, dim3(maxFrm, B), dim3(64), (size_t)0, (const float*)stats, I, (const float*)noise, maxFrm,
-          (const float*)prm, (const int*)fl, (const int*)fo, z);
+  klaunch(posterior_sample_kernel, dim3(maxFrm, B), dim3(64), (size_t)0, (const float*)stats, I, noise, maxFrm,
+          (const float*)d_vprm.p, fl, fo, z);
   CK(cudaGetLastError());
   ++launches;
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vz_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  // ---- z_p = flow(z, g_src); z_hat = flow^-1(z_p, g_tgt)   (models.py:1715-1716)
+  // ---- z_p = flow(z, g_src)   (models.py:1715, 1640)
   if (flow_on_tc) flow_tc(z, fl, fo, false, csrc, qld, /*forward=*/true);
   else flow_ffma(z, fl, fo, csrc, qld, /*forward=*/true);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vzp_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+}
+
+void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
+  if (!capturing) CK(cudaEventRecord(ev[4], stream));
+  const float* noise = vc_upload(from_spec, eps);
+  // ---- g_src / g_tgt (models.py:1712-1713) and every cond row of both, one launch: src -> d_vcsrc [B][condR + q_R]
+  //      (the TTS rows, then enc_q's), tgt -> d_condv [B][condR] (where the reverse flow and the decoder read them)
+  const float* csrc = cond_src(/*tgt=*/true);
+  const float* ctgt = d_condv.p;
+  posterior_side(from_spec, noise, csrc);
+  // ---- z_hat = flow^-1(z_p, g_tgt)   (models.py:1716)
+  const int* fl = d_frm_len.p;
+  const int* fo = d_frm_off.p;
+  float* z = d_z.p;
+  const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
   if (flow_on_tc) flow_tc(z, fl, fo, false, ctgt, condR, /*forward=*/false);
   else flow_ffma(z, fl, fo, ctgt, condR, /*forward=*/false);
   if (!capturing) CK(cudaEventRecord(ev[5], stream));
   // ---- o_hat = dec(z_hat * y_mask, g=g_tgt)   (models.py:1717)
   decode(z, fl, fo);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Forced alignment: the text-to-frame alignment at the head of SynthesizerTrn.forward (models.py:1632-1660) -- enc_p on the
+// ids, enc_q + forward flow on the recording (g_src; none for a single-speaker model), neg_cent, MAS -- as ONE graphed phase.
+// Token lengths come from the input and frame lengths from the clip lengths, so nothing waits for the host.  The
+// noise-scaled MAS of :1653-1655 is a training regulariser (off in the shipped configuration) and is never added here.
+// ---------------------------------------------------------------------------------------------------
+void vtts_engine::align_enqueue(bool from_spec, bool eps) {
+  const int I = cfg.inter_channels;
+  if (!capturing) CK(cudaEventRecord(ev[0], stream));
+  const float* noise = vc_upload(from_spec, eps);
+  int* tl = ensure(d_tok_len, B);
+  int* to = ensure(d_tok_off, B + 1);
+  int* ids = ensure(d_ids, Ttok);
+  {
+    P1Pin pp = p1_layout(0, false);                    // (staged by the host: lengths, offsets, packed ids)
+    CK(cudaMemcpyAsync(tl, pp.len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
+    CK(cudaMemcpyAsync(to, pp.off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
+    CK(cudaMemcpyAsync(ids, pp.ids, (size_t)Ttok * sizeof(int), cudaMemcpyHostToDevice, stream));
+  }
+  const int* fl = d_frm_len.p;
+  const int* fo = d_frm_off.p;
+  const float* csrc = has_g ? cond_src(/*tgt=*/false) : nullptr;
+  // ---- m_p, logs_p = enc_p(x, g)   (models.py:1632-1633)
+  text_encoder(csrc, condR + q_R);
+  prior_stats();
+  if (!capturing) CK(cudaEventRecord(ev[2], stream));
+  // ---- z_p = flow(enc_q(y, g), g)   (models.py:1639-1640)
+  posterior_side(from_spec, noise, csrc);
+  if (!capturing) CK(cudaEventRecord(ev[4], stream));
+  // ---- neg_cent [B][T_y][T_x] over the frame and token buckets (models.py:1645-1651), then MAS (:1656-1660)
+  const int Ty = maxFrm, Tx = maxTok;
+  float* nc = ensure(d_ncent, (size_t)B * Ty * Tx);
+  if (debug_flags & 1) CK(cudaMemsetAsync(nc, 0xFF, (size_t)B * Ty * Tx * sizeof(float), stream));   // NaN outside the utterances
+  klaunch(neg_cent_kernel, dim3((Tx + NC_T - 1) / NC_T, (Ty + NC_T - 1) / NC_T, B), dim3(NC_THREADS), (size_t)0, (const float*)d_z.p,
+          (const float*)d_stats.p, I, fl, fo, (const int*)tl, (const int*)to, nc, Ty, Tx);
+  CK(cudaGetLastError());
+  ++launches;
+  if (debug_flags & 1) {       // [B][max t_y][max t_x] (debug runs are eager: the real shape is known here)
+    float* dbg = ensure(d_ncent_dbg, (size_t)B * real_maxFrm * real_maxTok);
+    for (int b = 0; b < B; ++b)
+      CK(cudaMemcpy2DAsync(dbg + (size_t)b * real_maxFrm * real_maxTok, (size_t)real_maxTok * sizeof(float), nc + (size_t)b * Ty * Tx,
+                           (size_t)Tx * sizeof(float), (size_t)real_maxTok * sizeof(float), real_maxFrm, cudaMemcpyDeviceToDevice, stream));
+  }
+  int* dur = ensure(d_adur, Ttok);
+  int* tof = ensure(d_atof, Tfrm);
+  float* score = ensure(d_ascore, B);
+  klaunch(mas_kernel, dim3(B), dim3(MAS_THREADS), (size_t)2 * Tx * sizeof(float), nc, (int*)nullptr, fl, (const int*)tl, Ty, Tx, tof, fo,
+          dur, (const int*)to, score);
+  CK(cudaGetLastError());
+  ++launches;
+  if (!capturing) CK(cudaEventRecord(ev[5], stream));
 }
 
 // ===================================================================================================
@@ -2587,16 +2708,9 @@ static void impl_infer_dev(vtts_handle h, const int64_t* d_ids, const int64_t* l
   impl_synthesize_dev(h, d_noise_z, z_ld, d_wav, wav_ld);
 }
 
-// Voice conversion through host buffers (vtts_convert / vtts_convert_spec).
-static void impl_convert(vtts_handle h, bool from_spec, const float* in, const int64_t* lengths, int B, int64_t ld,
-                         const int64_t* sid_src, const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld,
-                         uint64_t seed, float* out_wav, int64_t out_ld, int64_t* out_frames) {
+// Frame shape of a call on recordings (vtts_convert*, vtts_align*): frames per clip from the sample / spectrogram lengths.
+static std::vector<int> clip_frames(vtts_handle h, bool from_spec, const int64_t* lengths, int B, int64_t ld) {
   const vtts_config& c = h->cfg;
-  REQUIRE(c.flow_n_flows % 2 == 0, VTTS_ERR_INVALID, "voice conversion needs an even flow_n_flows (the Flip folding of the packed "
-          "flow holds for both directions only then)");
-  REQUIRE(h->has_encq, VTTS_ERR_INVALID, "the weight blob has no posterior encoder (enc_q): voice conversion needs a model packed "
-          "with posterior=True from a training checkpoint (model.onnx does not contain enc_q)");
-  REQUIRE(h->has_g && c.n_speakers > 1, VTTS_ERR_INVALID, "voice conversion needs a multi-speaker model (n_speakers > 1)");
   REQUIRE(B >= 1 && B <= 16384 && ld >= 1, VTTS_ERR_INVALID, "bad batch size / row pitch");
   std::vector<int> frames(B);
   for (int b = 0; b < B; ++b) {
@@ -2611,20 +2725,21 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
       REQUIRE(L < (1LL << 30), VTTS_ERR_INVALID, "clip too long");
       frames[b] = (int)((L + 2 * h->vc_pad - c.filter_length) / c.hop_length + 1);
     }
-    REQUIRE(sid_src[b] >= 0 && sid_src[b] < c.n_speakers && sid_tgt[b] >= 0 && sid_tgt[b] < c.n_speakers, VTTS_ERR_INVALID,
-            "speaker id out of range [0, n_speakers)");
   }
-  h->B = B;
+  return frames;
+}
+
+// Sets the frame shape and stages the recordings, speaker ids (sid_tgt may be null), noise and scalars in vc_layout.
+static void stage_clips(vtts_handle h, bool from_spec, const float* in, const int64_t* lengths, int64_t ld, const std::vector<int>& frames,
+                        const int64_t* sid_src, const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed) {
+  const vtts_config& c = h->cfg;
+  const int B = h->B;
   h->h_frm_len = frames;
   h->h_frm_off.assign(B + 1, 0);
   int off = 0;
   for (int b = 0; b < B; ++b) { h->h_frm_off[b] = off; off += frames[b] + (b + 1 < B ? SEQ_GAP : 0); }
   h->h_frm_off[B] = off;
   h->set_frame_shape();
-  h->have_durations = false;
-  h->have_latent = false;
-  REQUIRE((int64_t)h->real_maxFrm * h->hop <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than hop * max(frames)");
-  REQUIRE(!noise_q || q_ld >= h->real_maxFrm, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
   h->vc_wld = (h->maxFrm + 2) * c.hop_length + c.filter_length;
   const int maxF = h->maxFrm, I = c.inter_channels, C = c.spec_channels;
   vtts_engine::VcPin pp = h->vc_layout(from_spec, noise_q != nullptr);
@@ -2632,8 +2747,8 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
   memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
   for (int b = 0; b < B; ++b) {
     pp.clip_len[b] = (int)lengths[b];
-    pp.sid[b] = (int)sid_src[b];
-    pp.sid[B + b] = (int)sid_tgt[b];
+    pp.sid[b] = sid_src ? (int)sid_src[b] : 0;
+    pp.sid[B + b] = sid_tgt ? (int)sid_tgt[b] : 0;
     if (from_spec) {
       for (int ch = 0; ch < C; ++ch)
         memcpy(pp.in + ((size_t)b * C + ch) * maxF, in + ((size_t)b * C + ch) * ld, (size_t)frames[b] * sizeof(float));
@@ -2649,6 +2764,29 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
   const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
   memcpy(&pp.prm[4], &lo, 4);
   memcpy(&pp.prm[5], &hi, 4);
+}
+
+// Voice conversion through host buffers (vtts_convert / vtts_convert_spec).
+static void impl_convert(vtts_handle h, bool from_spec, const float* in, const int64_t* lengths, int B, int64_t ld,
+                         const int64_t* sid_src, const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld,
+                         uint64_t seed, float* out_wav, int64_t out_ld, int64_t* out_frames) {
+  const vtts_config& c = h->cfg;
+  REQUIRE(c.flow_n_flows % 2 == 0, VTTS_ERR_INVALID, "voice conversion needs an even flow_n_flows (the Flip folding of the packed "
+          "flow holds for both directions only then)");
+  REQUIRE(h->has_encq, VTTS_ERR_INVALID, "the weight blob has no posterior encoder (enc_q): voice conversion needs a model packed "
+          "with posterior=True from a training checkpoint (model.onnx does not contain enc_q)");
+  REQUIRE(h->has_g && c.n_speakers > 1, VTTS_ERR_INVALID, "voice conversion needs a multi-speaker model (n_speakers > 1)");
+  const std::vector<int> frames = clip_frames(h, from_spec, lengths, B, ld);
+  for (int b = 0; b < B; ++b)
+    REQUIRE(sid_src[b] >= 0 && sid_src[b] < c.n_speakers && sid_tgt[b] >= 0 && sid_tgt[b] < c.n_speakers, VTTS_ERR_INVALID,
+            "speaker id out of range [0, n_speakers)");
+  h->B = B;
+  h->have_durations = false;
+  h->have_latent = false;
+  const int real_max = *std::max_element(frames.begin(), frames.end());
+  REQUIRE((int64_t)real_max * h->hop <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than hop * max(frames)");
+  REQUIRE(!noise_q || q_ld >= real_max, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
+  stage_clips(h, from_spec, in, lengths, ld, frames, sid_src, sid_tgt, noise_scale, noise_q, q_ld, seed);
   h->run_graphed({0x55, B, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
                  [&] { h->convert_enqueue(from_spec, noise_q != nullptr); });
   const size_t nw = (size_t)h->real_Tfrm * h->hop;
@@ -2659,6 +2797,68 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
   for (int b = 0; b < B; ++b) {
     memcpy(out_wav + (size_t)b * out_ld, pw + (size_t)h->h_frm_off[b] * h->hop, (size_t)frames[b] * h->hop * sizeof(float));
     out_frames[b] = frames[b];
+  }
+}
+
+// Forced alignment through host buffers (vtts_align / vtts_align_spec).
+static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid,
+                       const float* in, const int64_t* lengths, int B, int64_t ld, float noise_scale, const float* noise_q, int q_ld,
+                       uint64_t seed, int32_t* durations, int32_t* token_of_frame, int64_t tof_ld, float* score, int64_t* out_frames) {
+  const vtts_config& c = h->cfg;
+  REQUIRE(c.flow_n_flows % 2 == 0, VTTS_ERR_INVALID, "alignment needs an even flow_n_flows (the Flip folding of the packed flow holds "
+          "for the forward direction only then)");
+  REQUIRE(h->has_encq, VTTS_ERR_INVALID, "the weight blob has no posterior encoder (enc_q): alignment needs a model packed with "
+          "pack(posterior=True) / Model(voice_conversion=True) from a training checkpoint (model.onnx does not contain enc_q)");
+  REQUIRE(t_max >= 1, VTTS_ERR_INVALID, "bad t_max");
+  const std::vector<int> frames = clip_frames(h, from_spec, lengths, B, ld);
+  constexpr int TX_MAX = MAS_THREADS * MAS_MAXPT;
+  for (int b = 0; b < B; ++b) {
+    const int64_t tx = id_lengths[b];
+    REQUIRE(tx >= 1, VTTS_ERR_INVALID, "id_lengths must be at least 1: an utterance without tokens has no alignment");
+    REQUIRE(tx <= t_max, VTTS_ERR_INVALID, "id_lengths must not exceed t_max");
+    REQUIRE(tx <= TX_MAX, VTTS_ERR_INVALID, "more than " + std::to_string(TX_MAX) + " tokens in one utterance: above the alignment's limit");
+    REQUIRE(tx <= frames[b], VTTS_ERR_INVALID, "more tokens (" + std::to_string(tx) + ") than frames (" + std::to_string(frames[b]) +
+            ") in utterance " + std::to_string(b) + ": no monotonic alignment exists");
+    for (int64_t t = 0; t < tx; ++t) {
+      const int64_t id = ids[(size_t)b * t_max + t];
+      REQUIRE(id >= 0 && id < c.n_vocab, VTTS_ERR_INVALID, "phoneme id out of range [0, n_vocab)");
+    }
+    REQUIRE(!h->has_g || (sid && sid[b] >= 0 && sid[b] < c.n_speakers), VTTS_ERR_INVALID, "speaker id out of range [0, n_speakers)");
+  }
+  const int real_max = *std::max_element(frames.begin(), frames.end());
+  REQUIRE(!token_of_frame || tof_ld >= real_max, VTTS_ERR_CAPACITY, "tof_ld is smaller than max(frames)");
+  REQUIRE(!noise_q || q_ld >= real_max, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
+  setup_lengths(h, id_lengths, B, t_max);
+  stage_clips(h, from_spec, in, lengths, ld, frames, h->has_g ? sid : nullptr, nullptr, noise_scale, noise_q, q_ld, seed);
+  {
+    vtts_engine::P1Pin pp = h->p1_layout(t_max, false);
+    memcpy(pp.len, h->h_tok_len.data(), B * sizeof(int));
+    memcpy(pp.off, h->h_tok_off.data(), (B + 1) * sizeof(int));
+    memset(pp.ids, 0, (size_t)h->Ttok * sizeof(int));
+    for (int b = 0; b < B; ++b)
+      for (int t = 0; t < h->h_tok_len[b]; ++t) pp.ids[h->h_tok_off[b] + t] = (int)ids[(size_t)b * t_max + t];
+  }
+  h->run_graphed({0x66, B, h->maxTok, h->Ttok, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
+                 [&] { h->align_enqueue(from_spec, noise_q != nullptr); });
+  const size_t nt = (size_t)h->real_Ttok, nf = (size_t)h->real_Tfrm;
+  int* pin = reinterpret_cast<int*>(h->ensure_pinned((nt + nf + (size_t)B) * sizeof(int) + 64));
+  CK(cudaMemcpyAsync(pin, h->d_adur.p, nt * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(pin + nt, h->d_atof.p, nf * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(pin + nt + nf, h->d_ascore.p, (size_t)B * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaEventRecord(h->ev[7], h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; ++b) {
+    const int tx = h->h_tok_len[b], ty = frames[b];
+    int32_t* d = durations + (size_t)b * t_max;
+    memcpy(d, pin + h->h_tok_off[b], (size_t)tx * sizeof(int));
+    std::fill(d + tx, d + t_max, 0);
+    if (token_of_frame) {
+      int32_t* f = token_of_frame + (size_t)b * tof_ld;
+      memcpy(f, pin + nt + h->h_frm_off[b], (size_t)ty * sizeof(int));
+      std::fill(f + ty, f + tof_ld, -1);
+    }
+    if (score) memcpy(score + b, pin + nt + nf + b, sizeof(float));
+    out_frames[b] = ty;
   }
 }
 
@@ -2839,7 +3039,7 @@ static int mas_launch(float* d_value, const int* d_ty, const int* d_tx, int B, i
   const size_t smem = (size_t)2 * Tx * sizeof(float);
   cudaError_t e = cudaMemsetAsync(d_path, 0, (size_t)B * Ty * Tx * sizeof(int), st);
   if (e == cudaSuccess) {
-    mas_kernel<<<B, MAS_THREADS, smem, st>>>(d_value, d_path, d_ty, d_tx, Ty, Tx);
+    mas_kernel<<<B, MAS_THREADS, smem, st>>>(d_value, d_path, d_ty, d_tx, Ty, Tx, nullptr, nullptr, nullptr, nullptr, nullptr);
     e = cudaGetLastError();
   }
   if (e != cudaSuccess) { g_free_err = std::string("vtts_maximum_path: ") + cudaGetErrorString(e); return VTTS_ERR_CUDA; }
@@ -3002,6 +3202,22 @@ int vtts_convert_spec(vtts_handle h, const float* spec, const int64_t* spec_leng
                                        out_wav, out_ld, out_frames); });
 }
 
+int vtts_align(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid, const float* wav,
+               const int64_t* wav_lengths, int B, int64_t wav_ld, float noise_scale, const float* noise_q, int q_ld, uint64_t seed,
+               int32_t* durations, int32_t* token_of_frame, int64_t tof_ld, float* score, int64_t* out_frames) {
+  if (!ids || !id_lengths || !wav || !wav_lengths || !durations || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_align(h, false, ids, id_lengths, t_max, sid, wav, wav_lengths, B, wav_ld, noise_scale, noise_q, q_ld, seed,
+                                     durations, token_of_frame, tof_ld, score, out_frames); });
+}
+
+int vtts_align_spec(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid, const float* spec,
+                    const int64_t* spec_lengths, int B, int64_t spec_ld, float noise_scale, const float* noise_q, int q_ld, uint64_t seed,
+                    int32_t* durations, int32_t* token_of_frame, int64_t tof_ld, float* score, int64_t* out_frames) {
+  if (!ids || !id_lengths || !spec || !spec_lengths || !durations || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_align(h, true, ids, id_lengths, t_max, sid, spec, spec_lengths, B, spec_ld, noise_scale, noise_q, q_ld,
+                                     seed, durations, token_of_frame, tof_ld, score, out_frames); });
+}
+
 int vtts_hop(vtts_handle h) { return h ? h->hop : 0; }
 
 int vtts_stage_timings(vtts_handle h, float* ms, int n) {
@@ -3109,6 +3325,7 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "vc_z") { src = h->d_vz_dbg.p; n = F * c.inter_channels; }
     else if (nm == "vc_z_p") { src = h->d_vzp_dbg.p; n = F * c.inter_channels; }
     else if (nm == "vc_z_hat") { src = h->d_z.p; n = F * c.inter_channels; }
+    else if (nm == "align_neg_cent") { src = h->d_ncent_dbg.p; n = (size_t)h->B * h->real_maxFrm * h->real_maxTok; }
     else if (nm == "post") { src = h->d_post.p; n = (F * h->up_total + h->B) * c.subbands * (c.istft_n_fft + 2); }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);

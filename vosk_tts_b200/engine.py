@@ -49,7 +49,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_profile_read_tc", "vtts_timeline", "vtts_infer", "vtts_infer_dev",
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
-           "vtts_debug_conv_log", "vtts_tc_split_plan"]
+           "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec"]
 
 CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
 
@@ -208,6 +208,10 @@ def load_library(build_if_missing=True):
     for nm in ("vtts_convert", "vtts_convert_spec"):
         fn = getattr(lib, nm)
         fn.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, C.c_float, vp, i32, C.c_uint64, vp, C.c_int64, vp]
+        fn.restype = i32
+    for nm in ("vtts_align", "vtts_align_spec"):
+        fn = getattr(lib, nm)
+        fn.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, C.c_int64, C.c_float, vp, i32, C.c_uint64, vp, vp, C.c_int64, vp, vp]
         fn.restype = i32
     _LIB = lib
     return lib
@@ -509,6 +513,68 @@ class Engine:
         self.convert(wav, 0, min(1, n - 1), noise_scale=0.0)
         spec = np.zeros((B, int(self.cfg.get("spec_channels", 80)), F), np.float32)
         self.convert_spec(spec, 0, min(1, n - 1), noise_scale=0.0)
+        return F
+
+    # ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
+    def _align(self, from_wav, ids, lengths, sid, x, x_lengths, noise_scale, noise, seed):
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        if ids.ndim == 1:
+            ids = ids[None, :]
+        B, t_max = ids.shape
+        if x.shape[0] != B:
+            raise ValueError("ids and recordings must have the same batch size")
+        lengths = np.ascontiguousarray(np.broadcast_to(np.asarray(lengths, np.int64), (B,)))
+        sid = np.ascontiguousarray(np.broadcast_to(np.asarray(0 if sid is None else sid, np.int64), (B,)))
+        ld = x.shape[-1]
+        x_lengths = np.full(B, ld, np.int64) if x_lengths is None else \
+            np.ascontiguousarray(np.broadcast_to(np.asarray(x_lengths, np.int64), (B,)))
+        q_ld = 0
+        if noise is not None:
+            noise = np.ascontiguousarray(noise, dtype=np.float32)
+            if noise.ndim != 3 or noise.shape[0] != B or noise.shape[1] != int(self.cfg["inter_channels"]):
+                raise ValueError("noise must be float32 [B, inter_channels, >= frames]")
+            q_ld = noise.shape[2]
+        cap = self.convert_frames(x_lengths) if from_wav else x_lengths
+        max_f = max(1, int(np.max(cap)))
+        dur = np.zeros((B, t_max), np.int32)
+        tof = np.full((B, max_f), -1, np.int32)
+        score = np.zeros(B, np.float32)
+        frames = np.zeros(B, np.int64)
+        fn = self.lib.vtts_align if from_wav else self.lib.vtts_align_spec
+        self._check(fn(self.h, _ptr(ids), _ptr(lengths), t_max, _ptr(sid), _ptr(x), _ptr(x_lengths), B, ld, float(noise_scale),
+                       _ptr(noise), q_ld, int(seed), _ptr(dur), _ptr(tof), max_f, _ptr(score), _ptr(frames)))
+        return dur, frames, tof[:, : int(frames.max())], score
+
+    def align(self, ids, lengths, sid, wav, wav_lengths=None, noise_scale=1.0, noise=None, seed=0):
+        """Forced alignment (vtts_align): phoneme ids int64 [B, t_max] (`lengths` valid per row) of speaker `sid` against
+        recordings float32 [B, L] in [-1, 1] (`wav_lengths` valid samples per row, default all).  Returns (durations int32
+        [B, t_max] -- frames per token, 0 past lengths[b]; frames int64 [B]; token_of_frame int32 [B, max frames], -1 past
+        frames[b]; score float32 [B], the best path's log-likelihood).  noise: optional eps [B, inter_channels, >= frames] of
+        the posterior sample, else Philox(seed); noise_scale 1 is the reference's forward, 0 the posterior mean."""
+        wav = np.ascontiguousarray(wav, dtype=np.float32)
+        if wav.ndim == 1:
+            wav = wav[None, :]
+        return self._align(True, ids, lengths, sid, wav, wav_lengths, noise_scale, noise, seed)
+
+    def align_spec(self, ids, lengths, sid, spec, spec_lengths=None, noise_scale=1.0, noise=None, seed=0):
+        """Same from the posterior encoder's input features (the reference's `y`): float32 [B, spec_channels, T]."""
+        spec = np.ascontiguousarray(spec, dtype=np.float32)
+        if spec.ndim == 2:
+            spec = spec[None]
+        return self._align(False, ids, lengths, sid, spec, spec_lengths, noise_scale, noise, seed)
+
+    def reserve_align(self, max_tokens=256, max_frames=1024, batch=1):
+        """Workspace reservation for alignments of up to `batch` utterances x `max_tokens` tokens x `max_frames` frames (see
+        reserve): one alignment from a waveform and one from a spectrogram of that size, so that later calls within these
+        bounds move no buffer (a move invalidates every captured CUDA graph)."""
+        hop = int(self.cfg.get("hop_length", 256))
+        B, T, F = int(batch), int(max_tokens), int(max_frames)
+        if not 1 <= T <= F:
+            raise ValueError("reserve_align needs 1 <= max_tokens <= max_frames")
+        ids = (np.arange(B * T, dtype=np.int64).reshape(B, T) * 7 + 1) % int(self.cfg["n_vocab"])
+        self.align(ids, T, 0, np.zeros((B, F * hop), np.float32), noise_scale=0.0)
+        spec = np.zeros((B, int(self.cfg.get("spec_channels", 80)), F), np.float32)
+        self.align_spec(ids, T, 0, spec, noise_scale=0.0)
         return F
 
     # ---- streaming (one utterance): flow once, then vocode chunk by chunk

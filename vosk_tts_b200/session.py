@@ -123,5 +123,20 @@ class VitsSession:
             self.last_wav_lengths = frames * self.engine.hop
         return out[0, : int(frames[0]) * self.engine.hop]
 
+    def align(self, ids, wav, sid=0, noise=None, noise_scale=1.0):
+        """Forced alignment of one utterance (the alignment of SynthesizerTrn.forward, models.py:1632-1660; extension):
+        phoneme ids [T] against float32 samples [L] in [-1, 1] of speaker `sid`.  Returns (durations int32 [T], token_of_frame
+        int32 [frames], score) -- frames of every token, the token of every frame, the best path's log-likelihood.  noise:
+        optional eps [1, inter_channels, >= frames] of the posterior sample, otherwise Philox with a per-call seed."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64).reshape(1, -1)
+        wav = np.ascontiguousarray(wav, dtype=np.float32).reshape(-1)
+        with self._lock:
+            self._calls += 1
+            seed = (self._seed * 0x9E3779B97F4A7C15 + self._calls) & 0xFFFFFFFFFFFFFFFF
+            dur, frames, tof, score = self.engine.align(ids, ids.shape[1], sid, wav, noise_scale=noise_scale, noise=noise, seed=seed)
+            self.last_y_lengths = frames
+            self.last_wav_lengths = frames * self.engine.hop
+        return dur[0], tof[0, : int(frames[0])], float(score[0])
+
     def close(self):
         self.engine.close()

@@ -26,6 +26,11 @@ class Synth:
         return audio_norm.astype("int16")
 
     def g2p_noembed(self, text):
+        return self._g2p(text)[1]
+
+    def _g2p(self, text):
+        """(phonemes, ids, spans): spans[i] = (first, end) of phoneme i's ids in `ids`; the blank between phonemes i - 1
+        and i is the id at spans[i][0] - 1."""
         phonemes = ["^"]
         for word in re.split(_PUNCT, text.lower()):
             if word == "":
@@ -38,15 +43,17 @@ class Synth:
                 phonemes.extend(convert(word).split())
         phonemes.append("$")
         id_map = self.model.config["phoneme_id_map"]
-        ids = []
+        ids, spans = [], []
         for i, p in enumerate(phonemes):            # intersperse the blank id 0 (synth.py:244-251)
             if i:
                 ids.append(0)
             v = id_map[p]
+            first = len(ids)
             ids.extend(v if isinstance(v, list) else [v])
+            spans.append((first, len(ids)))
         logging.info(f"Text: {text}")
         logging.info(f"Phonemes: {phonemes}")
-        return ids
+        return phonemes, ids, spans
 
     def synth_audio(self, text, speaker_id=0, noise_level=None, speech_rate=None, duration_noise_level=None, scale=None):
         inf = self.model.config.get("inference", {})
@@ -112,17 +119,7 @@ class Synth:
         """Voice conversion (extension): re-voices `audio` of speaker `src_speaker` as `tgt_speaker` of the same model
         (SynthesizerTrn.voice_conversion, models.py:1710-1718).  audio: int16 samples (divided by 32768, data_utils.py:77) or
         float in [-1, 1], at the model's sample rate.  Returns int16 [256 * (len // 256)] for the reference configuration."""
-        audio = np.asarray(audio)
-        if audio.ndim != 1:
-            raise ValueError("convert_audio takes one mono clip ([n] samples)")
-        if audio.dtype == np.int16:
-            wav = audio.astype(np.float32) / 32768.0
-        elif np.issubdtype(audio.dtype, np.floating):
-            wav = audio.astype(np.float32)
-            if wav.size and float(np.abs(wav).max()) > 1.0:
-                raise ValueError("float audio must lie in [-1, 1]")
-        else:
-            raise ValueError("audio must be int16 or float samples, not %s" % audio.dtype)
+        wav = self._float_audio(audio, "convert_audio")
         if src_speaker is None or tgt_speaker is None:
             raise ValueError("voice conversion needs both a source and a target speaker id")
         inf = self.model.config.get("inference", {})
@@ -136,21 +133,75 @@ class Synth:
         logging.info("Real-time factor: %0.2f (convert=%0.2f sec, audio=%0.2f sec)" % (sec / dur if dur > 0 else 0.0, sec, dur))
         return out
 
-    def convert(self, iname, oname, src_speaker, tgt_speaker, noise_scale=None, scale=None):
-        """Reads a mono 16-bit WAV at the model's sample rate (no resampling), writes the converted clip as one."""
+    def _read_wav(self, iname):
+        """A mono 16-bit WAV at the model's sample rate (no resampling) -> int16 samples."""
         sr = self._sample_rate()
         with wave.open(iname, "rb") as f:
             if f.getnchannels() != 1 or f.getsampwidth() != 2:
                 raise ValueError("%s: expected a mono 16-bit WAV" % iname)
             if f.getframerate() != sr:
                 raise ValueError("%s is sampled at %d Hz, the model at %d Hz: resample it first" % (iname, f.getframerate(), sr))
-            audio = np.frombuffer(f.readframes(f.getnframes()), dtype="<i2").astype(np.int16)
+            return np.frombuffer(f.readframes(f.getnframes()), dtype="<i2").astype(np.int16)
+
+    @staticmethod
+    def _float_audio(audio, what):
+        audio = np.asarray(audio)
+        if audio.ndim != 1:
+            raise ValueError("%s takes one mono clip ([n] samples)" % what)
+        if audio.dtype == np.int16:
+            return audio.astype(np.float32) / 32768.0          # data_utils.py:77
+        if np.issubdtype(audio.dtype, np.floating):
+            wav = audio.astype(np.float32)
+            if wav.size and float(np.abs(wav).max()) > 1.0:
+                raise ValueError("float audio must lie in [-1, 1]")
+            return wav
+        raise ValueError("audio must be int16 or float samples, not %s" % audio.dtype)
+
+    def convert(self, iname, oname, src_speaker, tgt_speaker, noise_scale=None, scale=None):
+        """Reads a mono 16-bit WAV at the model's sample rate (no resampling), writes the converted clip as one."""
+        sr = self._sample_rate()
+        audio = self._read_wav(iname)
         out = self.convert_audio(audio, src_speaker, tgt_speaker, noise_scale, scale)
         with wave.open(oname, "w") as f:
             f.setnchannels(1)
             f.setsampwidth(2)
             f.setframerate(sr)
             f.writeframes(out.tobytes())
+
+    def align_audio(self, text, audio, speaker_id=0, noise_scale=None):
+        """Forced alignment (extension): the phonemes of `text` (the g2p of synth_audio) against `audio` of speaker
+        `speaker_id`, by the model's own monotonic alignment search (SynthesizerTrn.forward, models.py:1632-1660).  audio as
+        in convert_audio.  Returns one dict per g2p phoneme, "^", "$" and punctuation included -- {"phoneme", "start", "end"}
+        in seconds (frames * hop / sample rate) -- with each interspersed blank as its own entry with phoneme None; the
+        frames of a phoneme that maps to several ids are merged, and the entries tile [0, frames * hop / sample rate).
+        The best path's log-likelihood (higher: the audio fits the text better) is kept in `last_score`."""
+        if self.model.tokenizer is not None or str(self.model.config.get("model_type", "")).startswith("multistream"):
+            raise ValueError("model_type %r is not a VITS2 graph: not supported by this engine" % self.model.config.get("model_type"))
+        wav = self._float_audio(audio, "align_audio")
+        phonemes, ids, spans = self._g2p(re.sub("—", "-", text.strip()))
+        noise_scale = 1.0 if noise_scale is None else noise_scale      # the reference samples the posterior at scale 1 (:841)
+        t0 = time.perf_counter()
+        dur, _, score = self.model.onnx.align(np.array(ids, np.int64), wav, 0 if speaker_id is None else int(speaker_id),
+                                              noise_scale=noise_scale)
+        sec = time.perf_counter() - t0
+        cum = np.concatenate([[0], np.cumsum(np.asarray(dur[: len(ids)], np.int64))])
+        step = self._hop() / float(self._sample_rate())
+        entries = []
+        for i, (p, (a, e)) in enumerate(zip(phonemes, spans)):
+            if i:
+                entries.append({"phoneme": None, "start": float(cum[a - 1] * step), "end": float(cum[a] * step)})
+            entries.append({"phoneme": p, "start": float(cum[a] * step), "end": float(cum[e] * step)})
+        self.last_score = float(score)
+        logging.info("Alignment: %d phonemes, %d frames, score %.1f (%.2f sec)" % (len(phonemes), int(cum[-1]), score, sec))
+        return entries
+
+    def align(self, wav_path, text, speaker_id=0, noise_scale=None):
+        """align_audio of a mono 16-bit WAV at the model's sample rate (no resampling)."""
+        return self.align_audio(text, self._read_wav(wav_path), speaker_id, noise_scale)
+
+    def _hop(self):
+        cfg = getattr(self.model.onnx, "cfg", None)
+        return int(cfg.get("hop_length", 256)) if isinstance(cfg, dict) else 256
 
     def synth(self, text, oname, speaker_id=0, noise_level=None, speech_rate=None, duration_noise_level=None, scale=None):
         audio = self.synth_audio(text, speaker_id, noise_level, speech_rate, duration_noise_level, scale)
