@@ -69,7 +69,14 @@ typedef struct vtts_config {
   int32_t use_mel_posterior_encoder;
   int32_t filter_length, hop_length, win_length, n_mel_channels;
   float mel_fmin, mel_fmax;        /* (the mel filter bank itself is packed into the blob) */
+  /* Model family of the blob: 0 = VITS2 SynthesizerTrn (every entry point above and below except the QuickVC ones),
+   * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding*.  The entry points of one family
+   * return VTTS_ERR_INVALID on an engine of the other. */
+  int32_t model_family;
 } vtts_config;
+
+#define VTTS_FAMILY_VITS2 0
+#define VTTS_FAMILY_QUICKVC 1
 
 /* Replaces onnxruntime.InferenceSession(model.onnx) (vosk_tts/model.py:46).
  * `blob` holds the packed fp32 tensors produced by vosk_tts_b200.weights.pack(); `manifest` is a
@@ -171,7 +178,10 @@ int vtts_timeline(vtts_handle h, int enable, unsigned long long* out, size_t max
  * tensor of the last call ("x", "stats", "dx", "za", "zb", "condv", "z_p", "z", "d0", "stage<i>", "post") to
  * host memory in the engine's channels-last packed layout.  After a conversion: "vc_spec" (enc_q input rows: the log-mel or
  * linear spectrogram, spec_channels rounded up to 16 columns), "vc_z" (posterior sample) and "vc_z_p" (flow forward output;
- * both kept when bit0 is set), "vc_z_hat" (flow reverse output). */
+ * both kept when bit0 is set), "vc_z_hat" (flow reverse output).  After a speaker embedding (QuickVC): "vc_spec" (log-mel
+ * rows), "spk_x<l>" (projected LSTM inputs of layer l, [rows][1024]: frame rows for l = 0, slice rows for l = 1, 2),
+ * "spk_h<l>" (hidden states of layer l, slice rows [rows][256]: the slices in clip order, each occupying as many rows as it
+ * has frames, 8 rows between consecutive slices) and "spk_g". */
 int vtts_debug_flags(vtts_handle h, int flags);
 int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floats, size_t* n_out);
 /* Unit-test hook for the relative-position attention kernels (attentions.py:165-196): ONE attention launch of layer
@@ -319,6 +329,22 @@ int vtts_align(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int
 int vtts_align_spec(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid, const float* spec,
                     const int64_t* spec_lengths, int B, int64_t spec_ld, float noise_scale, const float* noise_q, int q_ld, uint64_t seed,
                     int32_t* durations, int32_t* token_of_frame, int64_t tof_ld, float* score, int64_t* out_frames);
+
+/* QuickVC speaker embedding (SpeakerEncoder.embed_utterance, vc/models.py:728-767, as SynthesizerTrn.infer calls it on the
+ * target's mel_spectrogram_torch): the g a conversion is conditioned on, from a recording of any speaker.  A clip of T <= 128
+ * mel frames is one sequence of T frames; a longer one is cut into 128-frame slices starting at 0, 64, ... < T - 128, plus
+ * its last 128 frames; the 3-layer LSTM runs over every slice, each slice's final hidden state goes through linear, ReLU
+ * and L2 normalisation, and g is the mean over the clip's slices.  One call, no host synchronisation inside.
+ *   wav          float [B, wav_ld] in [-1, 1] at the model's sampling rate (16 kHz), clip b = wav[b*wav_ld .. +
+ *                wav_lengths[b]); each clip is framed on its own samples (frames = (len + 2*pad - filter_length) / hop_length
+ *                + 1, pad = (filter_length - hop_length) / 2), and needs wav_lengths[b] > pad (480 samples at the published
+ *                configuration)
+ *   g_out        out float [B, gin_channels]
+ * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: not a QuickVC engine, a clip too short for the reflect padding. */
+int vtts_speaker_embedding(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, float* g_out);
+/* Same from log-mel rows: mel float [B, n_mel_channels, mel_ld] (the reference's mel_spectrogram_torch output),
+ * mel_lengths[b] frames valid (1 <= mel_lengths[b] <= mel_ld). */
+int vtts_speaker_embedding_mel(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* g_out);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

@@ -117,6 +117,42 @@ def from_training_json(path_or_dict, n_vocab=62):
     return out
 
 
+def from_quickvc_json(path_or_dict):
+    """Map a QuickVC config (vc/configs/quickvc.json) onto the engine config, model_family "quickvc".
+
+    What the engine serves of it is the speaker encoder SpeakerEncoder (vc/models.py:728-767) with the target's mel front end
+    (mel_spectrogram_torch, vc/convert.py:60-69).  Hard-coded in the reference, not in the json: the LSTM has 3 layers with
+    hidden = gin_channels = 256 over n_mel_channels inputs (models.py:842, SpeakerEncoder defaults :729); the content units are 768
+    wide (models.py:825, while the json's ssl_dim says 1024).  Only the published ms_istft_vits decoder is accepted."""
+    cfg = path_or_dict
+    if not isinstance(cfg, dict):
+        with open(path_or_dict) as f:
+            cfg = json.load(f)
+    m, d = cfg["model"], cfg["data"]
+    if m.get("mb_istft_vits", False) or m.get("istft_vits", False) or not m.get("ms_istft_vits", False):
+        raise ValueError("only the published QuickVC decoder (ms_istft_vits=true, Multistream_iSTFT_Generator) is supported; "
+                         "mb_istft_vits / istft_vits are not")
+    if int(m.get("gin_channels", 0)) != 256:
+        raise ValueError("gin_channels must be 256: the speaker encoder's LSTM hidden size and embedding (models.py:842)")
+    out = copy.deepcopy(DEFAULT_CONFIG)
+    out["model_family"] = "quickvc"
+    out["n_speakers"] = 0
+    out["decoder"] = "ms_istft"
+    out["unit_channels"] = 768
+    for k in ("gin_channels", "inter_channels", "hidden_channels", "filter_channels", "resblock", "resblock_kernel_sizes",
+              "resblock_dilation_sizes", "upsample_rates", "upsample_initial_channel", "upsample_kernel_sizes", "subbands",
+              "gen_istft_n_fft", "gen_istft_hop_size"):
+        if k in m:
+            out[k] = m[k]
+    for k in ("sampling_rate", "filter_length", "hop_length", "win_length", "n_mel_channels", "mel_fmin", "mel_fmax"):
+        if k in d:
+            out[k] = d[k]
+    out["use_mel_posterior_encoder"] = True
+    out["spec_channels"] = out["n_mel_channels"]
+    out["spk_layers"] = 3
+    return out
+
+
 def hop_total(cfg):
     """Output samples per latent frame (256 for the reference config)."""
     up = 1

@@ -27,6 +27,7 @@
 #include "mas.cuh"
 #include "attn_tc.cuh"
 #include "vc.cuh"
+#include "spk.cuh"
 
 using namespace vtts;
 
@@ -600,8 +601,19 @@ struct vtts_engine {
   VcPin vc_layout(bool from_spec, bool eps);
   float* vc_upload(bool from_spec, bool eps);
   float* cond_src(bool tgt);
+  float* front_end(bool from_spec);
   void posterior_side(bool from_spec, const float* noise, const float* csrc);
   void convert_enqueue(bool from_spec, bool eps);
+
+  // ---- QuickVC speaker encoder (SpeakerEncoder.embed_utterance, vc/models.py:728-767; spk.cuh)
+  ConvW spk_ih[3];                                 // W_ih x + b_ih + b_hh of each layer, a 1x1 conv
+  const float *spk_hh[3] = {}, *spk_lin_w = nullptr, *spk_lin_b = nullptr;
+  int spk_nseq = 0, spk_rows = 0;
+  int spk_clusters[4] = {};                        // co-resident clusters of lstm_rec_kernel<1 / 2 / 4 / 8>
+  Buf<int> d_sseq;                                 // [xrow nseq][len nseq][off nseq + 1][last nseq][seq_of_clip B + 1]
+  Buf<float> d_sx[3], d_sh[3], d_sg;
+  void bind_quickvc();
+  void spk_enqueue(bool from_mel, const std::vector<int>& seq, int max_len);
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
   Buf<float> d_ncent, d_ncent_dbg, d_ascore;       // neg_cent [B][maxFrm][maxTok] (MAS accumulates in place), scores [B]
@@ -2296,16 +2308,15 @@ float* vtts_engine::cond_src(bool tgt) {
 // Front end, posterior encoder and forward flow (models.py:836-842, 750-753): the uploaded waveform / spectrogram -> z
 // (vc_z) -> z_p = flow(z, g_src) in d_z.  csrc: g_src's rows [B][condR + q_R] (cond_src), null for an unconditioned model.
 // Opens the phase's plane collection (the flow's WN planes, also used by enc_q) for the frame shape.
-void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc) {
+// Spectrogram front end of the uploaded waveforms (vc_upload) -> feature rows [Tfrm][spec_pad] (d_vfeat): the magnitude
+// spectrogram, or its log-mel when the model reads mel; caller-supplied features are only repacked.
+float* vtts_engine::front_end(bool from_spec) {
   const vtts_config& c = cfg;
-  const int H = c.hidden_channels, I = c.inter_channels;
   const size_t F = (size_t)Tfrm;
-  const int qld = condR + q_R;
   const int* fl = d_frm_len.p;
   const int* fo = d_frm_off.p;
   const int* vi = d_vint.p;
   const float* vin = d_vin.p;
-  // ---- enc_q input rows [F][spec_pad]
   float* feat = ensure(d_vfeat, F * spec_pad);
   if (from_spec) {
     klaunch(spec_pack_kernel, dim3(maxFrm, B), dim3(128), (size_t)0, vin, c.spec_channels, maxFrm, fl, fo, feat, spec_pad);
@@ -2327,6 +2338,18 @@ void vtts_engine::posterior_side(bool from_spec, const float* noise, const float
       ++launches;
     }
   }
+  return feat;
+}
+
+void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc) {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, I = c.inter_channels;
+  const size_t F = (size_t)Tfrm;
+  const int qld = condR + q_R;
+  const int* fl = d_frm_len.p;
+  const int* fo = d_frm_off.p;
+  // ---- enc_q input rows [F][spec_pad]
+  float* feat = front_end(from_spec);
   // ---- posterior encoder (models.py:836-842): pre -> 16-layer WN (g_src) -> proj -> sample
   float* h = ensure(d_h, F * H);
   float* acts = ensure(d_acts, F * H);
@@ -2437,6 +2460,94 @@ void vtts_engine::align_enqueue(bool from_spec, bool eps) {
   if (!capturing) CK(cudaEventRecord(ev[5], stream));
 }
 
+// ---------------------------------------------------------------------------------------------------
+// QuickVC speaker encoder (SpeakerEncoder.embed_utterance, vc/models.py:728-767).  A QuickVC blob (weights.pack_quickvc) holds
+// the encoder and the mel front end; none of the VITS2 tensors.
+// ---------------------------------------------------------------------------------------------------
+void vtts_engine::bind_quickvc() {
+  const vtts_config& c = cfg;
+  REQUIRE(c.gin_channels == SPK_H, VTTS_ERR_INVALID, "the speaker encoder needs gin_channels == 256 (its LSTM hidden size)");
+  REQUIRE(c.n_mel_channels % CV_CK == 0 && c.spec_channels == c.n_mel_channels && c.use_mel_posterior_encoder, VTTS_ERR_INVALID,
+          "the speaker encoder reads n_mel_channels (a multiple of 16) log-mel rows");
+  REQUIRE(c.filter_length > 0 && c.hop_length > 0 && c.filter_length % ST_TN == 0 && c.filter_length > c.hop_length &&
+              (c.filter_length - c.hop_length) % 2 == 0 && c.win_length == c.filter_length,
+          VTTS_ERR_INVALID, "bad spectrogram configuration (filter_length must be a multiple of 64, above hop_length, == win_length)");
+  spec_pad = c.n_mel_channels;
+  vc_pad = (c.filter_length - c.hop_length) / 2;
+  for (int l = 0; l < 3; ++l) {
+    const std::string p = "spk.l" + std::to_string(l);
+    spk_ih[l] = conv(p + ".ih", l == 0 ? c.n_mel_channels : SPK_H, SPK_GATES, 1);
+    spk_hh[l] = vec(p + ".hh", (size_t)SPK_GATES * SPK_H);
+  }
+  spk_lin_w = vec("spk.lin.w", (size_t)SPK_H * SPK_H);
+  spk_lin_b = vec("spk.lin.b", SPK_H);
+  stft_basis = vec("vc.stft", (size_t)c.filter_length * c.filter_length);
+  mel_fb = vec("vc.mel", (size_t)c.n_mel_channels * (c.filter_length / 2 + 1));
+  // clusters that fit at once: a cluster must sit inside one GPC, so this can be fewer than n_sm / SPK_CTAS
+  auto fit = [&](auto kern, size_t smem, int& out) {
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaLaunchConfig_t lc;
+    memset(&lc, 0, sizeof(lc));
+    lc.gridDim = dim3(SPK_CTAS * 64); lc.blockDim = dim3(SPK_THREADS); lc.dynamicSmemBytes = smem;
+    int nc = 0;
+    if (cudaOccupancyMaxActiveClusters(&nc, kern, &lc) != cudaSuccess) { nc = 0; cudaGetLastError(); }
+    out = std::max(1, nc);
+  };
+  fit(lstm_rec_kernel<1>, spk_rec_smem<1>(), spk_clusters[0]);
+  fit(lstm_rec_kernel<2>, spk_rec_smem<2>(), spk_clusters[1]);
+  fit(lstm_rec_kernel<4>, spk_rec_smem<4>(), spk_clusters[2]);
+  fit(lstm_rec_kernel<8>, spk_rec_smem<8>(), spk_clusters[3]);
+}
+
+// Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
+// d_sseq (host copy); max_len: the longest slice.
+void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int max_len) {
+  const int ns = spk_nseq;
+  int* ds = ensure(d_sseq, seq.size());
+  CK(cudaMemcpyAsync(ds, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+  const int *xrow = ds, *slen = ds + ns, *soff = ds + 2 * ns, *last = ds + 3 * ns + 1, *of_clip = ds + 4 * ns + 1;
+  vc_upload(from_mel, false);
+  const float* feat = front_end(from_mel);
+  // Sequences per cluster: the fewest that keep every cluster co-resident; more sequences per cluster lengthen each step,
+  // more clusters than fit run in waves.
+  int NS = 1, li = 0;
+  while (NS < 8 && (ns + NS - 1) / NS > spk_clusters[li]) { NS *= 2; ++li; }
+  const int groups = (ns + NS - 1) / NS;
+  // The projections run with one fixed launch shape (no split-K across CTAs or thread groups), so every row is summed in the
+  // same order whatever the batch: a clip's g does not depend on the clips it is batched with.  Layers 1 and 2 launch over
+  // the slices, so the host-side lengths the launch heuristics read are the slices' for those launches.
+  struct Saved {
+    vtts_engine* e; int ms, ming, bigg, autog; std::vector<int> vf, hf;
+    explicit Saved(vtts_engine* h) : e(h), ms(h->conv_max_s), ming(h->conv_min_g), bigg(h->conv_big_g), autog(h->conv_auto_g),
+                                     vf(h->v_frm_len), hf(h->h_frm_len) {}
+    ~Saved() { e->conv_max_s = ms; e->conv_min_g = ming; e->conv_big_g = bigg; e->conv_auto_g = autog; e->v_frm_len = vf; e->h_frm_len = hf; }
+  } saved(this);
+  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
+  const std::vector<int> slen_h(seq.begin() + ns, seq.begin() + 2 * ns);
+  const float* x = feat;
+  for (int l = 0; l < 3; ++l) {
+    if (l == 1) { v_frm_len = slen_h; h_frm_len = slen_h; }
+    float* xp = ensure(d_sx[l], (size_t)(l == 0 ? Tfrm : spk_rows) * SPK_GATES);
+    float* hs = ensure(d_sh[l], (size_t)spk_rows * SPK_H);
+    if (l == 0) launch_conv({mk(spk_ih[0], x, spec_pad, 0, xp, SPK_GATES, 0, 1, 0)}, 1, d_frm_len.p, d_frm_off.p, maxFrm, B);
+    else launch_conv({mk(spk_ih[l], x, SPK_H, 0, xp, SPK_GATES, 0, 1, 0)}, 1, slen, soff, max_len, ns);
+    const int* xr = l == 0 ? xrow : soff;
+    const dim3 grid(groups * SPK_CTAS), blk(SPK_THREADS);
+    switch (NS) {
+      case 1: klaunch(lstm_rec_kernel<1>, grid, blk, spk_rec_smem<1>(), (const float*)xp, spk_hh[l], xr, slen, soff, ns, hs); break;
+      case 2: klaunch(lstm_rec_kernel<2>, grid, blk, spk_rec_smem<2>(), (const float*)xp, spk_hh[l], xr, slen, soff, ns, hs); break;
+      case 4: klaunch(lstm_rec_kernel<4>, grid, blk, spk_rec_smem<4>(), (const float*)xp, spk_hh[l], xr, slen, soff, ns, hs); break;
+      default: klaunch(lstm_rec_kernel<8>, grid, blk, spk_rec_smem<8>(), (const float*)xp, spk_hh[l], xr, slen, soff, ns, hs); break;
+    }
+    CK(cudaGetLastError());
+    ++launches;
+    x = hs;
+  }
+  klaunch(spk_embed_kernel, dim3(B), dim3(SPK_H), (size_t)0, x, last, of_clip, spk_lin_w, spk_lin_b, ensure(d_sg, (size_t)B * SPK_H));
+  CK(cudaGetLastError());
+  ++launches;
+}
+
 // ===================================================================================================
 // C ABI
 // ===================================================================================================
@@ -2444,10 +2555,18 @@ namespace {
 
 enum : int { G_ATOMIC = 0, G_BEGIN = 1, G_CONT = 2 };    // one-shot call | opens a two-phase section | continues / closes it
 
+constexpr int ANY_FAMILY = -1;
+
+// family: the model family the entry point serves (VTTS_FAMILY_*), or ANY_FAMILY.
 template <typename Fn>
-int guarded(vtts_handle h, Fn fn, int mode = G_ATOMIC) {
+int guarded(vtts_handle h, Fn fn, int mode = G_ATOMIC, int family = VTTS_FAMILY_VITS2) {
   if (!h) return VTTS_ERR_INVALID;
   std::unique_lock<std::mutex> lk(h->mu);
+  if (family != ANY_FAMILY && h->cfg.model_family != family) {
+    h->err = h->cfg.model_family == VTTS_FAMILY_QUICKVC ? "this entry point serves VITS2 models; the engine holds a QuickVC model"
+                                                        : "this entry point serves QuickVC models; the engine holds a VITS2 model";
+    return VTTS_ERR_INVALID;
+  }
   const std::thread::id me = std::this_thread::get_id();
   if (mode == G_CONT) {
     if (!h->two_phase || h->owner != me) {
@@ -2800,6 +2919,47 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
   }
 }
 
+// QuickVC speaker embedding through host buffers (vtts_speaker_embedding / _mel).
+static void impl_speaker_embedding(vtts_handle h, bool from_mel, const float* in, const int64_t* lengths, int B, int64_t ld, float* g_out) {
+  const std::vector<int> frames = clip_frames(h, from_mel, lengths, B, ld);
+  h->B = B;
+  stage_clips(h, from_mel, in, lengths, ld, frames, nullptr, nullptr, 0.f, nullptr, 0, 0);
+  // slices of embed_utterance (vc/models.py:739-760): T <= 128 frames -> the whole clip; else starts 0, 64, ... < T - 128
+  // and the last 128 frames.  Slice rows are packed in clip order with SEQ_GAP rows between slices.
+  std::vector<int> xrow, slen, soff, last, of_clip(1, 0);
+  int off = 0, max_len = 0;
+  for (int b = 0; b < B; ++b) {
+    const int T = frames[b];
+    std::vector<int> starts;
+    if (T <= SPK_SLICE) starts.push_back(0);
+    else {
+      for (int s = 0; s < T - SPK_SLICE; s += SPK_HOP) starts.push_back(s);
+      starts.push_back(T - SPK_SLICE);
+    }
+    for (int s : starts) {
+      const int L = std::min(T, SPK_SLICE);
+      xrow.push_back(h->h_frm_off[b] + s);
+      slen.push_back(L);
+      soff.push_back(off);
+      last.push_back(off + L - 1);
+      off += L + SEQ_GAP;
+      max_len = std::max(max_len, L);
+    }
+    of_clip.push_back((int)xrow.size());
+  }
+  const int ns = (int)xrow.size();
+  h->spk_nseq = ns;
+  h->spk_rows = off;
+  soff.push_back(off);
+  std::vector<int> seq;
+  for (auto* v : {&xrow, &slen, &soff, &last, &of_clip}) seq.insert(seq.end(), v->begin(), v->end());
+  h->spk_enqueue(from_mel, seq, max_len);
+  float* pg = reinterpret_cast<float*>(h->ensure_pinned((size_t)B * SPK_H * sizeof(float) + 64));
+  CK(cudaMemcpyAsync(pg, h->d_sg.p, (size_t)B * SPK_H * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  memcpy(g_out, pg, (size_t)B * SPK_H * sizeof(float));
+}
+
 // Forced alignment through host buffers (vtts_align / vtts_align_spec).
 static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid,
                        const float* in, const int64_t* lengths, int B, int64_t ld, float noise_scale, const float* noise_q, int q_ld,
@@ -2967,7 +3127,9 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     if (const char* e = getenv("VTTS_SPEC_MARGIN")) h->spec_margin = (float)atof(e);      // (< 1 forces mispredictions: tests)
     if (const char* e = getenv("VTTS_CAPTURE_FIRST")) h->capture_on_first = atoi(e) != 0;   // 0: capture a bucket's graph on its second call          // 0: never enqueue phase 2 before the lengths are known    // 0: size everything by the exact lengths
     if (const char* e = getenv("VTTS_PREFETCH")) h->use_prefetch = atoi(e) != 0;
-    h->bind_weights();
+    REQUIRE(cfg->model_family == VTTS_FAMILY_VITS2 || cfg->model_family == VTTS_FAMILY_QUICKVC, VTTS_ERR_INVALID, "unknown model family");
+    if (cfg->model_family == VTTS_FAMILY_QUICKVC) h->bind_quickvc();
+    else h->bind_weights();
     h->build_prefetch_list();
     CK(cudaMemsetAsync(h->ensure(h->d_done_ctr, 4), 0, 4 * sizeof(int), h->stream));     // ticket counter of duration_kernel (self-resetting)
     CK(cudaFuncSetAttribute(dds_layer_kernel<DDS_TT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
@@ -2991,7 +3153,7 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     CK(cudaFuncSetAttribute(conv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONV_SMEM_MAX));
     CK(cudaFuncSetAttribute(conv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONV_SMEM_MAX));
     CK(cudaStreamSynchronize(h->stream));
-  });
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 void vtts_destroy(vtts_handle h) {
@@ -3006,9 +3168,11 @@ void vtts_destroy(vtts_handle h) {
                       &h->d_h29, &h->d_za, &h->d_zb, &h->d_eps_dp, &h->d_z, &h->d_h, &h->d_h1, &h->d_wx, &h->d_acts, &h->d_skip, &h->d_fqkv,
                       &h->d_fao, &h->d_fy, &h->d_ffh2, &h->d_eps_z, &h->d_d0, &h->d_post, &h->d_wav};
   for (auto* b : fb) fr(b->p);
-  Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg};
+  Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg,
+                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg};
   for (auto* b : vb) fr(b->p);
   fr(h->d_vint.p);
+  fr(h->d_sseq.p);
   for (auto& b : h->d_stage) fr(b.p);
   for (auto& v : h->d_xj) for (auto& b : v) fr(b.p);
   for (auto& v : h->d_tmp) for (auto& b : v) fr(b.p);
@@ -3230,7 +3394,7 @@ uint64_t vtts_kernel_launches(vtts_handle h) { return h ? h->launches : 0; }
 void* vtts_stream(vtts_handle h) { return h ? (void*)h->stream : nullptr; }
 
 int vtts_set_graphs(vtts_handle h, int enable) {
-  return guarded(h, [&] { h->use_graphs = enable != 0; });
+  return guarded(h, [&] { h->use_graphs = enable != 0; }, G_ATOMIC, ANY_FAMILY);
 }
 
 uint64_t vtts_graph_replays(vtts_handle h) { return h ? h->graph_replays : 0; }
@@ -3257,7 +3421,7 @@ int vtts_profile(vtts_handle h, int enable) {
     h->tc_prof_used = 0;
     h->tc_prof_flops = 0.0;
     h->tc_prof_launches = 0;
-  });
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 int vtts_profile_read(vtts_handle h, double* conv_ms, uint64_t* conv_launches, double* conv_flops) {
@@ -3273,7 +3437,7 @@ int vtts_profile_read(vtts_handle h, double* conv_ms, uint64_t* conv_launches, d
     *conv_ms = ms;
     *conv_launches = h->prof_launches;
     *conv_flops = h->prof_flops;
-  });
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 // Timeline: enable -> every kernel's first CTA appends (source line, globaltimer) to a device buffer; read returns pairs.
@@ -3295,7 +3459,7 @@ int vtts_timeline(vtts_handle h, int enable, unsigned long long* out, size_t max
       memcpy(out, hbuf.data() + 1, n * 16);
       *n_out = n;
     }
-  });
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 int vtts_debug_flags(vtts_handle h, int flags) {
@@ -3327,6 +3491,10 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "vc_z_hat") { src = h->d_z.p; n = F * c.inter_channels; }
     else if (nm == "align_neg_cent") { src = h->d_ncent_dbg.p; n = (size_t)h->B * h->real_maxFrm * h->real_maxTok; }
     else if (nm == "post") { src = h->d_post.p; n = (F * h->up_total + h->B) * c.subbands * (c.istft_n_fft + 2); }
+    else if (nm == "spk_x0") { src = h->d_sx[0].p; n = F * SPK_GATES; }
+    else if (nm == "spk_x1" || nm == "spk_x2") { src = h->d_sx[nm[5] - '0'].p; n = (size_t)h->spk_rows * SPK_GATES; }
+    else if (nm == "spk_h0" || nm == "spk_h1" || nm == "spk_h2") { src = h->d_sh[nm[5] - '0'].p; n = (size_t)h->spk_rows * SPK_H; }
+    else if (nm == "spk_g") { src = h->d_sg.p; n = (size_t)h->B * SPK_H; }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);
       REQUIRE(i >= 0 && i < (int)h->d_stage.size(), VTTS_ERR_INVALID, "no such stage");
@@ -3339,7 +3507,17 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     CK(cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     *n_out = n;
-  });
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_speaker_embedding(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, float* g_out) {
+  if (!wav || !wav_lengths || !g_out) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_speaker_embedding(h, false, wav, wav_lengths, B, wav_ld, g_out); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_speaker_embedding_mel(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* g_out) {
+  if (!mel || !mel_lengths || !g_out) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_speaker_embedding(h, true, mel, mel_lengths, B, mel_ld, g_out); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
 }
 
 // Host copies of a debug hook's arguments on the device (freed on every exit).
@@ -3675,7 +3853,7 @@ int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_
       std::copy(h->conv_log.begin(), h->conv_log.begin() + n, out);
       *n_out = n;
     }
-  });
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 // Host-only restatement of launch_tc's split-K plan (tc_split_plan) for tests: no device, no engine.
@@ -3717,7 +3895,7 @@ int vtts_profile_read_tc(vtts_handle h, double* ms, uint64_t* launches, double* 
     *ms = t;
     *launches = h->tc_prof_launches;
     *flops = h->tc_prof_flops;
-  });
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 // Micro-benchmark of one conv kernel in isolation (back-to-back launches, CUDA events on the engine stream):

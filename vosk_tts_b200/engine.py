@@ -39,6 +39,7 @@ class VttsConfig(C.Structure):
         ("spec_channels", C.c_int32), ("use_mel_posterior_encoder", C.c_int32),
         ("filter_length", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32), ("n_mel_channels", C.c_int32),
         ("mel_fmin", C.c_float), ("mel_fmax", C.c_float),
+        ("model_family", C.c_int32),
     ]
 
 
@@ -49,7 +50,10 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_profile_read_tc", "vtts_timeline", "vtts_infer", "vtts_infer_dev",
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
-           "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec"]
+           "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
+           "vtts_speaker_embedding_mel"]
+
+MODEL_FAMILIES = {"vits2": 0, "quickvc": 1}    # vtts_config.model_family
 
 CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
 
@@ -213,6 +217,10 @@ def load_library(build_if_missing=True):
         fn = getattr(lib, nm)
         fn.argtypes = [vp, vp, vp, i32, vp, vp, vp, i32, C.c_int64, C.c_float, vp, i32, C.c_uint64, vp, vp, C.c_int64, vp, vp]
         fn.restype = i32
+    for nm in ("vtts_speaker_embedding", "vtts_speaker_embedding_mel"):
+        fn = getattr(lib, nm)
+        fn.argtypes = [vp, vp, vp, i32, C.c_int64, vp]
+        fn.restype = i32
     _LIB = lib
     return lib
 
@@ -272,6 +280,7 @@ def make_c_config(cfg, precision=0):
     c.mel_fmin = float(cfg.get("mel_fmin", 0.0) or 0.0)
     fmax = cfg.get("mel_fmax")
     c.mel_fmax = float(cfg.get("sampling_rate", 22050)) / 2 if fmax is None else float(fmax)
+    c.model_family = MODEL_FAMILIES[cfg.get("model_family", "vits2")]
     return c
 
 
@@ -514,6 +523,37 @@ class Engine:
         spec = np.zeros((B, int(self.cfg.get("spec_channels", 80)), F), np.float32)
         self.convert_spec(spec, 0, min(1, n - 1), noise_scale=0.0)
         return F
+
+    # ---- QuickVC speaker embedding (SpeakerEncoder.embed_utterance, vc/models.py:728-767)
+    def speaker_embedding(self, wav, lengths=None):
+        """The QuickVC target embedding g of each clip (vtts_speaker_embedding): wav float32 [B, L] (or [L]) in [-1, 1] at the
+        model's sampling rate, `lengths` the valid samples per row (default: all).  Returns float32 [B, gin_channels]."""
+        wav = np.ascontiguousarray(wav, dtype=np.float32)
+        if wav.ndim == 1:
+            wav = wav[None, :]
+        B = wav.shape[0]
+        lengths = np.ascontiguousarray(np.full(B, wav.shape[1]) if lengths is None else lengths, dtype=np.int64).reshape(B)
+        g = np.zeros((B, int(self.cfg["gin_channels"])), np.float32)
+        self._check(self.lib.vtts_speaker_embedding(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], _ptr(g)))
+        return g
+
+    def speaker_embedding_mel(self, mel, lengths=None):
+        """Same from log-mel rows (mel_spectrogram_torch's output): float32 [B, n_mel_channels, T] (or [n_mel_channels, T])."""
+        mel = np.ascontiguousarray(mel, dtype=np.float32)
+        if mel.ndim == 2:
+            mel = mel[None]
+        B = mel.shape[0]
+        lengths = np.ascontiguousarray(np.full(B, mel.shape[2]) if lengths is None else lengths, dtype=np.int64).reshape(B)
+        g = np.zeros((B, int(self.cfg["gin_channels"])), np.float32)
+        self._check(self.lib.vtts_speaker_embedding_mel(self.h, _ptr(mel), _ptr(lengths), B, mel.shape[2], _ptr(g)))
+        return g
+
+    def reserve_quickvc(self, max_frames=1024, batch=1):
+        """Workspace reservation for embeddings of up to `batch` clips x `max_frames` mel frames: one call of that size, so
+        later calls within these bounds move no buffer."""
+        hop = int(self.cfg["hop_length"])
+        self.speaker_embedding(np.zeros((int(batch), int(max_frames) * hop), np.float32))
+        return int(max_frames)
 
     # ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
     def _align(self, from_wav, ids, lengths, sid, x, x_lengths, noise_scale, noise, seed):

@@ -200,3 +200,17 @@ def make_random_checkpoint(cfg, seed=1234, posterior=False):
 
 def param_names(cfg, posterior=False):
     return [s[0] for s in _spec(cfg, posterior)]
+
+
+def make_random_speaker_encoder(cfg, seed=1234):
+    """The ``enc_spk.*`` tensors of a QuickVC checkpoint (SpeakerEncoder, vc/models.py:728-736: nn.LSTM(n_mel, G, 3) +
+    nn.Linear(G, G)), CPU fp32, deterministic for (cfg, seed).  Drawn like PyTorch's own initialisation, uniform in
+    +-1/sqrt(G), so that the gates operate in the range a trained encoder sees rather than saturating."""
+    G, n_mel = cfg["gin_channels"], cfg["n_mel_channels"]
+    a = 1.0 / math.sqrt(G)
+    shapes = []
+    for l in range(cfg.get("spk_layers", 3)):
+        shapes += [("enc_spk.lstm.weight_ih_l%d" % l, (4 * G, n_mel if l == 0 else G)), ("enc_spk.lstm.weight_hh_l%d" % l, (4 * G, G)),
+                   ("enc_spk.lstm.bias_ih_l%d" % l, (4 * G,)), ("enc_spk.lstm.bias_hh_l%d" % l, (4 * G,))]
+    shapes += [("enc_spk.linear.weight", (G, G)), ("enc_spk.linear.bias", (G,))]
+    return {name: ((torch.rand(shape, generator=_gen(name, seed)) * 2 - 1) * a).float().contiguous() for name, shape in shapes}

@@ -494,3 +494,35 @@ def pack(w, cfg, tc=True, precision=None, posterior=False):
             P.add("vc.mel", mel_basis(cfg.get("sampling_rate", 22050), n_fft, cfg.get("n_mel_channels", 80),
                                       cfg.get("mel_fmin", 0.0), cfg.get("mel_fmax")))
     return P.finish()
+
+
+SPK_CTAS = 8      # CTAs of one cluster of the LSTM recurrence kernel (csrc/spk.cuh)
+
+
+def spk_hh_layout(whh):
+    """W_hh [4G][G] (PyTorch gate order i, f, g, o) in the layout of csrc/spk.cuh lstm_rec_kernel: [rank][k][gate * U + unit],
+    U = G / SPK_CTAS, CTA `rank` owning hidden units [U rank, U rank + U) of every gate."""
+    whh = np.asarray(whh, np.float32)
+    G = whh.shape[1]
+    U = G // SPK_CTAS
+    w = whh.reshape(4, SPK_CTAS, U, G)                  # [gate][rank][unit][k]
+    return np.ascontiguousarray(np.transpose(w, (1, 3, 0, 2)))   # [rank][k][gate][unit]
+
+
+def pack_quickvc(w, cfg):
+    """QuickVC state dict (folded) -> (blob, manifest) of a model_family "quickvc" engine: the speaker encoder enc_spk and
+    the mel front end of the target (vc/convert.py:60-69).  Each LSTM layer's input projection is a 1x1 conv whose bias is
+    b_ih + b_hh folded; W_hh goes in the CTA-blocked layout of the recurrence kernel; the linear layer is stored transposed.
+    enc_q and the discriminators, which inference never reads, are left out."""
+    g = lambda k: w[k].detach().cpu().numpy() if hasattr(w[k], "detach") else np.asarray(w[k])
+    P = _Packer()
+    for l in range(cfg.get("spk_layers", 3)):
+        p = "enc_spk.lstm.%s_l%d"
+        P.conv("spk.l%d.ih" % l, g(p % ("weight_ih", l))[:, :, None], g(p % ("bias_ih", l)) + g(p % ("bias_hh", l)))
+        P.add("spk.l%d.hh" % l, spk_hh_layout(g(p % ("weight_hh", l))))
+    P.add("spk.lin.w", np.ascontiguousarray(g("enc_spk.linear.weight").T))
+    P.add("spk.lin.b", g("enc_spk.linear.bias"))
+    n_fft = cfg["filter_length"]
+    P.add("vc.stft", stft_basis(n_fft))
+    P.add("vc.mel", mel_basis(cfg["sampling_rate"], n_fft, cfg["n_mel_channels"], cfg["mel_fmin"], cfg["mel_fmax"]))
+    return P.finish()
