@@ -70,7 +70,7 @@ typedef struct vtts_config {
   int32_t filter_length, hop_length, win_length, n_mel_channels;
   float mel_fmin, mel_fmax;        /* (the mel filter bank itself is packed into the blob) */
   /* Model family of the blob: 0 = VITS2 SynthesizerTrn (every entry point above and below except the QuickVC ones),
-   * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding*.  The entry points of one family
+   * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding* and vtts_quickvc_convert.  The entry points of one family
    * return VTTS_ERR_INVALID on an engine of the other. */
   int32_t model_family;
 } vtts_config;
@@ -345,6 +345,26 @@ int vtts_speaker_embedding(vtts_handle h, const float* wav, const int64_t* wav_l
 /* Same from log-mel rows: mel float [B, n_mel_channels, mel_ld] (the reference's mel_spectrogram_torch output),
  * mel_lengths[b] frames valid (1 <= mel_lengths[b] <= mel_ld). */
 int vtts_speaker_embedding_mel(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* g_out);
+
+/* QuickVC conversion (SynthesizerTrn.infer, vc/models.py:862-872, as vc/convert.py:62-87 calls it) of content units into the
+ * voice of a target: z_p = enc_p(units) (PosteriorEncoder(768, I, H, 5, 1, 16), no g), z = flow(z_p, g, reverse=True),
+ * o = dec(z, g) (Multistream_iSTFT_Generator: x = conv_pre(z) + cond(g), the inverse STFT divided by the window envelope as
+ * torch.istft does).  Each clip is converted as if alone.  One call, no host synchronisation inside.
+ *   units        float [B, units_ld, 768], frame-major (ContentVec's last_hidden_state, vc/encode.py's [T, 768] .npy rows);
+ *                clip b = its first unit_lengths[b] frames, 1 <= unit_lengths[b] <= units_ld
+ *   g            float [B, gin_channels]: the target's speaker embedding (vtts_speaker_embedding; a target is enrolled once
+ *                and reused across sources)
+ *   noise_scale  scales enc_p's sample: 1 is the reference (z_p = m + eps * exp(logs)), 0 gives z_p = m
+ *   noise        float [B, inter_channels, noise_ld] standing in for torch.randn_like (vc/models.py:270), or NULL for Philox(seed)
+ *   out_wav      out float [B, out_ld]: clip b gets hop * unit_lengths[b] samples (320 per 20 ms unit at the published
+ *                configuration), zeros after them;  out_frames out int64 [B] = unit_lengths
+ * Host pointers, atomic on the handle.  Precision modes 2 and 3 run as mode 1 (they differ only in the VITS2 text encoder).
+ * VTTS_ERR_INVALID: not a QuickVC engine, a blob without the conversion tensors (speaker encoder only), B < 1, a length outside
+ * [1, units_ld], g NULL.  VTTS_ERR_CAPACITY: out_ld < hop * max(unit_lengths), noise_ld < max(unit_lengths).
+ * After a call, vtts_debug_read "vc_z" (bit0 of vtts_debug_flags set) is z_p and "vc_z_hat" is z, frame rows [rows][inter]. */
+int vtts_quickvc_convert(vtts_handle h, const float* units, const int64_t* unit_lengths, int B, int64_t units_ld,
+                         const float* g, float noise_scale, const float* noise, int noise_ld, uint64_t seed,
+                         float* out_wav, int64_t out_ld, int64_t* out_frames);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

@@ -120,10 +120,13 @@ def from_training_json(path_or_dict, n_vocab=62):
 def from_quickvc_json(path_or_dict):
     """Map a QuickVC config (vc/configs/quickvc.json) onto the engine config, model_family "quickvc".
 
-    What the engine serves of it is the speaker encoder SpeakerEncoder (vc/models.py:728-767) with the target's mel front end
-    (mel_spectrogram_torch, vc/convert.py:60-69).  Hard-coded in the reference, not in the json: the LSTM has 3 layers with
-    hidden = gin_channels = 256 over n_mel_channels inputs (models.py:842, SpeakerEncoder defaults :729); the content units are 768
-    wide (models.py:825, while the json's ssl_dim says 1024).  Only the published ms_istft_vits decoder is accepted."""
+    What the engine serves of it is SynthesizerTrn.infer (vc/models.py:862-872): the speaker encoder SpeakerEncoder
+    (:728-767) with the target's mel front end (mel_spectrogram_torch, vc/convert.py:60-69), the content encoder enc_p, the
+    reverse flow and the Multistream_iSTFT_Generator decoder.  Hard-coded in the reference, not in the json: the LSTM has 3
+    layers with hidden = gin_channels = 256 over n_mel_channels inputs (models.py:842, SpeakerEncoder defaults :729); the
+    content units are 768 wide (models.py:825, while the json's ssl_dim says 1024); enc_p is PosteriorEncoder(768, I, H, 5, 1, 16)
+    without g; the flow is ResidualCouplingBlock(I, H, 5, 1, 4, gin) with 4 mean-only coupling layers (:840).  Only the published
+    ms_istft_vits decoder with two upsampling stages is accepted (convt_pad)."""
     cfg = path_or_dict
     if not isinstance(cfg, dict):
         with open(path_or_dict) as f:
@@ -150,7 +153,28 @@ def from_quickvc_json(path_or_dict):
     out["use_mel_posterior_encoder"] = True
     out["spec_channels"] = out["n_mel_channels"]
     out["spk_layers"] = 3
+    out["use_transformer_flows"] = False
+    out.update(flow_kernel_size=5, flow_dilation_rate=1, flow_wn_layers=4, flow_n_flows=4)
+    if len(out["upsample_rates"]) != 2 or len(out["upsample_kernel_sizes"]) != 2:
+        raise ValueError("the QuickVC decoder needs exactly two upsampling stages: its ConvTranspose1d output_padding = 1 - i "
+                         "(vc/models.py:428-430) is negative past the second")
+    for i in range(2):
+        convt_pad(out, i)
     return out
+
+
+def convt_pad(cfg, i):
+    """(padding, output_padding) of the decoder's upsampling ConvTranspose1d of stage i: (K-u)//2 and 0 in VITS2
+    (training/vits2/models.py, every generator), (K-u+1-i)//2 and 1-i in QuickVC (vc/models.py:428-430).  The engine lays out
+    u*T output rows per stage, so the stage must emit exactly that many: K - u + output_padding == 2 * padding."""
+    u, K = cfg["upsample_rates"][i], cfg["upsample_kernel_sizes"][i]
+    if cfg.get("model_family", "vits2") == "quickvc":
+        p, op = (K - u + 1 - i) // 2, 1 - i
+        if K - u + op != 2 * p:
+            raise ValueError("upsampling stage %d (rate %d, kernel %d) would emit %d frames per input frame plus %d, not exactly %d"
+                             % (i, u, K, u, K - u + op - 2 * p, u))
+        return p, op
+    return (K - u) // 2, 0
 
 
 def hop_total(cfg):

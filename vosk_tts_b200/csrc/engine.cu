@@ -160,6 +160,7 @@ struct vtts_engine {
   bool has_g = false;
   const float *emb_g = nullptr, *cond_w = nullptr, *cond_b = nullptr, *enc_emb = nullptr, *dp_ea = nullptr;
   const float *istft_basis = nullptr, *pqmf = nullptr;
+  const float* istft_w2 = nullptr;      // squared window: the tail divides by the window envelope (torch.istft; QuickVC)
   int condR = 0, r_spk = -1, r_dp = 0, r_flow = 0, r_dec = -1;
   std::vector<EncLayerW> enc;
   ConvW enc_proj, dp_pre, dp_proj, dec_pre, dec_post;
@@ -548,6 +549,8 @@ struct vtts_engine {
   void flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, const float* cond, int cond_ld, bool forward);
   void launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen, Planes* pl);
   void bind_weights();
+  void bind_flow_decoder();
+  void bind_wn_encoder(const std::string& p, int cin);
   void launch_conv(const std::vector<ConvP>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
   void encoder_layer(const EncLayerW& L, float*& x, float*& xb, float* qkv, float* ao, float* y, float* ffh, int Hc, int Fc,
                      int ks, const int* lens, const int* offs, int maxLen, const float* vec_after, int vec_ld,
@@ -588,6 +591,7 @@ struct vtts_engine {
   // ---- voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718)
   bool has_encq = false, q_tc = false;
   static constexpr int Q_LAYERS = 16, Q_KERNEL = 5;        // PosteriorEncoder(spec_channels, I, H, 5, 1, 16, gin) (models.py:1616)
+  static constexpr int QV_UNITS = 768;                     // QuickVC's enc_p = PosteriorEncoder(768, I, H, 5, 1, 16) (vc/models.py:825)
   ConvW q_pre, q_proj;
   std::vector<ConvW> q_in, q_rsx, q_rss;
   std::vector<TcW> qt_in, qt_rsx, qt_rss;
@@ -602,6 +606,7 @@ struct vtts_engine {
   float* vc_upload(bool from_spec, bool eps);
   float* cond_src(bool tgt);
   float* front_end(bool from_spec);
+  void posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld);
   void posterior_side(bool from_spec, const float* noise, const float* csrc);
   void convert_enqueue(bool from_spec, bool eps);
 
@@ -614,6 +619,15 @@ struct vtts_engine {
   Buf<float> d_sx[3], d_sh[3], d_sg;
   void bind_quickvc();
   void spk_enqueue(bool from_mel, const std::vector<int>& seq, int max_len);
+
+  // ---- QuickVC conversion (SynthesizerTrn.infer, vc/models.py:862-872): enc_p is bound into the q_* members (the same
+  //      16-layer k=5 WN as enc_q, which a QuickVC engine does not hold), the flow and the decoder as in a VITS2 engine
+  bool has_encp = false;
+  Buf<float> d_units, d_qg;                        // content-unit rows [Tfrm][unit channels], g [B][gin]
+  Buf<char> h_pin_qv;
+  struct QvPin { int *frm_len, *frm_off, *ident; float *prm, *units, *g, *eps; };
+  QvPin qv_layout(bool eps);
+  void quickvc_enqueue(bool eps);
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
   Buf<float> d_ncent, d_ncent_dbg, d_ascore;       // neg_cent [B][maxFrm][maxTok] (MAS accumulates in place), scores [B]
@@ -723,6 +737,60 @@ void vtts_engine::bind_weights() {
     cf.push_back(f);
   }
   dp_ea = vec("dp.ea", 4);
+  bind_flow_decoder();
+  // ---- posterior encoder enc_q + front end (only in blobs packed with posterior=True)
+  has_encq = tensors.count("encq.pre.b") > 0;
+  if (has_encq) {
+    REQUIRE(c.spec_channels > 0 && c.filter_length > 0 && c.hop_length > 0 && c.filter_length % ST_TN == 0 &&
+                c.filter_length > c.hop_length && (c.filter_length - c.hop_length) % 2 == 0,
+            VTTS_ERR_INVALID, "bad spectrogram configuration (filter_length must be a multiple of 64, above hop_length)");
+    REQUIRE(c.win_length == c.filter_length, VTTS_ERR_INVALID, "win_length != filter_length is not supported by the spectrogram front end");
+    REQUIRE(c.use_mel_posterior_encoder ? c.spec_channels == c.n_mel_channels : c.spec_channels == c.filter_length / 2 + 1,
+            VTTS_ERR_INVALID, "spec_channels does not match the posterior encoder's input (n_mel_channels / filter_length/2+1)");
+    spec_pad = (c.spec_channels + CV_CK - 1) / CV_CK * CV_CK;     // enc_q.pre runs on the FFMA conv: input zero-padded to 16 channels
+    vc_pad = (c.filter_length - c.hop_length) / 2;
+    bind_wn_encoder("encq", spec_pad);
+    if (has_g) {
+      q_R = Q_LAYERS * 2 * H;
+      q_cond_w = vec("encq.cond.w", (size_t)q_R * G);
+      q_cond_b = vec("encq.cond.b", q_R);
+    }
+    stft_basis = vec("vc.stft", (size_t)c.filter_length * c.filter_length);
+    mel_fb = c.use_mel_posterior_encoder ? vec("vc.mel", (size_t)c.n_mel_channels * (c.filter_length / 2 + 1)) : nullptr;
+  }
+}
+
+// A PosteriorEncoder's pre / 16-layer WN / proj (models.py:813-842) from the blob's <p>.* (weights._pack_wn_encoder) into the
+// q_* members: enc_q of a VITS2 engine, enc_p of a QuickVC one.
+void vtts_engine::bind_wn_encoder(const std::string& p, int cin) {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, I = c.inter_channels;
+  const bool qfw = !(c.precision >= 1 && H % TC_BK == 0);
+  q_pre = conv(p + ".pre", cin, H, 1);
+  q_in.clear(); q_rsx.clear(); q_rss.clear(); qt_in.clear(); qt_rsx.clear(); qt_rss.clear();
+  for (int i = 0; i < Q_LAYERS; ++i) {
+    q_in.push_back(conv(p + ".in" + std::to_string(i), H, 2 * H, Q_KERNEL, qfw));
+    if (i < Q_LAYERS - 1) q_rsx.push_back(conv(p + ".rsx" + std::to_string(i), H, H, 1, qfw));
+    q_rss.push_back(conv(p + ".rss" + std::to_string(i), H, H, 1, qfw));
+  }
+  q_proj = conv(p + ".proj", H, 2 * I, 1, qfw);
+  q_tc = tc && !qfw;
+  if (q_tc) {
+    for (int i = 0; i < Q_LAYERS; ++i) {
+      qt_in.push_back(tcw(p + ".in" + std::to_string(i), H, 2 * H, Q_KERNEL));
+      if (i < Q_LAYERS - 1) qt_rsx.push_back(tcw(p + ".rsx" + std::to_string(i), H, H, 1));
+      qt_rss.push_back(tcw(p + ".rss" + std::to_string(i), H, H, 1));
+    }
+    qt_proj = tcw(p + ".proj", H, 2 * I, 1);
+  }
+}
+
+// The reverse flow and the decoder (weights._pack_flow_decoder): shared by both model families.
+void vtts_engine::bind_flow_decoder() {
+  const vtts_config& c = cfg;
+  const int H = c.hidden_channels, I = c.inter_channels;
+  const int nl = c.flow_wn_layers, nf = c.flow_n_flows;
+  const int fheads = c.flow_n_heads > 0 ? c.flow_n_heads : 2;
   flow.clear();
   for (int f = 0; f < nf; ++f) {
     FlowW F;
@@ -765,7 +833,10 @@ void vtts_engine::bind_weights() {
   int ch = c.upsample_initial_channel;
   up_total = 1;
   for (int i = 0; i < c.n_upsamples; ++i) {
-    const int u = c.upsample_rates[i], K = c.upsample_kernel_sizes[i], p = (K - u) / 2;
+    // ConvTranspose1d padding: (K-u)/2 in VITS2 (training/vits2/models.py:857-858, 989-990), (K-u+1-i)/2 with output_padding 1-i in
+    // QuickVC (vc/models.py:428-430); both make exactly u*T output rows (config.convt_pad checks QuickVC's)
+    const int u = c.upsample_rates[i], K = c.upsample_kernel_sizes[i];
+    const int p = c.model_family == VTTS_FAMILY_QUICKVC ? (K - u + 1 - i) / 2 : (K - u) / 2;
     UpW U;
     for (int r = 0; r < u; ++r) {
       // polyphase split of ConvTranspose1d (see weights.convt_phases): taps per phase and left padding
@@ -808,43 +879,6 @@ void vtts_engine::bind_weights() {
   } else {
     dec_post = conv("dec.post", ch, 1, 7);
     hop = up_total;
-  }
-  // ---- posterior encoder enc_q + front end (only in blobs packed with posterior=True)
-  has_encq = tensors.count("encq.pre.b") > 0;
-  if (has_encq) {
-    REQUIRE(c.spec_channels > 0 && c.filter_length > 0 && c.hop_length > 0 && c.filter_length % ST_TN == 0 &&
-                c.filter_length > c.hop_length && (c.filter_length - c.hop_length) % 2 == 0,
-            VTTS_ERR_INVALID, "bad spectrogram configuration (filter_length must be a multiple of 64, above hop_length)");
-    REQUIRE(c.win_length == c.filter_length, VTTS_ERR_INVALID, "win_length != filter_length is not supported by the spectrogram front end");
-    REQUIRE(c.use_mel_posterior_encoder ? c.spec_channels == c.n_mel_channels : c.spec_channels == c.filter_length / 2 + 1,
-            VTTS_ERR_INVALID, "spec_channels does not match the posterior encoder's input (n_mel_channels / filter_length/2+1)");
-    const bool qfw = !(c.precision >= 1 && H % TC_BK == 0);
-    spec_pad = (c.spec_channels + CV_CK - 1) / CV_CK * CV_CK;     // enc_q.pre runs on the FFMA conv: input zero-padded to 16 channels
-    vc_pad = (c.filter_length - c.hop_length) / 2;
-    q_pre = conv("encq.pre", spec_pad, H, 1);
-    q_in.clear(); q_rsx.clear(); q_rss.clear(); qt_in.clear(); qt_rsx.clear(); qt_rss.clear();
-    for (int i = 0; i < Q_LAYERS; ++i) {
-      q_in.push_back(conv("encq.in" + std::to_string(i), H, 2 * H, Q_KERNEL, qfw));
-      if (i < Q_LAYERS - 1) q_rsx.push_back(conv("encq.rsx" + std::to_string(i), H, H, 1, qfw));
-      q_rss.push_back(conv("encq.rss" + std::to_string(i), H, H, 1, qfw));
-    }
-    q_proj = conv("encq.proj", H, 2 * I, 1, qfw);
-    q_tc = tc && !qfw;
-    if (q_tc) {
-      for (int i = 0; i < Q_LAYERS; ++i) {
-        qt_in.push_back(tcw("encq.in" + std::to_string(i), H, 2 * H, Q_KERNEL));
-        if (i < Q_LAYERS - 1) qt_rsx.push_back(tcw("encq.rsx" + std::to_string(i), H, H, 1));
-        qt_rss.push_back(tcw("encq.rss" + std::to_string(i), H, H, 1));
-      }
-      qt_proj = tcw("encq.proj", H, 2 * I, 1);
-    }
-    if (has_g) {
-      q_R = Q_LAYERS * 2 * H;
-      q_cond_w = vec("encq.cond.w", (size_t)q_R * G);
-      q_cond_b = vec("encq.cond.b", q_R);
-    }
-    stft_basis = vec("vc.stft", (size_t)c.filter_length * c.filter_length);
-    mel_fb = c.use_mel_posterior_encoder ? vec("vc.mel", (size_t)c.n_mel_channels * (c.filter_length / 2 + 1)) : nullptr;
   }
 }
 
@@ -1418,6 +1452,7 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     TcSpec q;
     q.in = pz; q.w = tc_pre; q.bias = dec_pre.b; q.Cin = I; q.Cout = ch; q.k = 7; q.dil = 1; q.pad = 3;
     q.out = cur; q.pl_slope = 0.1f;
+    if (r_dec >= 0) { q.cond = d_condv.p + r_dec; q.cond_ld = condR; }     // x = conv_pre(z) + cond(g) (QuickVC, vc/models.py:465)
     if (debug_flags & 1) { q.y = ensure(d_d0, (size_t)F * ch); q.ldy = ch; }
     launch_tc({q}, 1, fl, fo, maxFrm, B);
   }
@@ -1530,7 +1565,7 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
   dim3 g((M + TL_M - 1) / TL_M, B);
   const size_t smem = ((size_t)tl_rec_frames(63, c.subbands, c.istft_n_fft, c.istft_hop) * pc + (size_t)c.subbands * (TL_M + 2 * tl_halo(63, c.subbands))) * sizeof(float);
   REQUIRE(c.istft_hop == 4 && c.istft_n_fft == 16, VTTS_ERR_INVALID, "iSTFT tail kernel is sized for n_fft=16, hop=4");
-  klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1);
+  klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1, istft_w2);
   CK(cudaGetLastError());
   ++launches;
 }
@@ -2148,7 +2183,7 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
   float* cur = ensure(d_d0, F * ch);
   {
     ConvP p = mk(dec_pre, z, I, 0, cur, ch, 0, 1, 3);
-    if (has_g && r_dec >= 0) { p.cond = d_condv.p + r_dec; p.cond_ld = condR; }
+    if (r_dec >= 0) { p.cond = d_condv.p + r_dec; p.cond_ld = condR; }     // x = conv_pre(z) + cond(g)
     launch_conv({p}, 1, fl, fo, maxFrm, B);
   }
   int rm = 1;
@@ -2230,7 +2265,7 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     dim3 g((M + TL_M - 1) / TL_M, B);
     const size_t smem = ((size_t)tl_rec_frames(63, c.subbands, c.istft_n_fft, c.istft_hop) * pc + (size_t)c.subbands * (TL_M + 2 * tl_halo(63, c.subbands))) * sizeof(float);
     REQUIRE(c.istft_hop == 4 && c.istft_n_fft == 16, VTTS_ERR_INVALID, "iSTFT tail kernel is sized for n_fft=16, hop=4");
-    klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1);
+    klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1, istft_w2);
     CK(cudaGetLastError());
     ++launches;
   } else {
@@ -2341,16 +2376,15 @@ float* vtts_engine::front_end(bool from_spec) {
   return feat;
 }
 
-void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc) {
+// Posterior encoder over feature rows [Tfrm][feat_ld] (models.py:836-842; QuickVC's enc_p, vc/models.py:264-271): pre ->
+// 16-layer WN (cond rows qcond, row stride qld; null: none) -> proj -> stats (d_vstats) -> z = m + eps * exp(logs) in d_z.
+// Opens the phase's plane collection (the flow's WN planes, also used here) for the frame shape.
+void vtts_engine::posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld) {
   const vtts_config& c = cfg;
   const int H = c.hidden_channels, I = c.inter_channels;
   const size_t F = (size_t)Tfrm;
-  const int qld = condR + q_R;
   const int* fl = d_frm_len.p;
   const int* fo = d_frm_off.p;
-  // ---- enc_q input rows [F][spec_pad]
-  float* feat = front_end(from_spec);
-  // ---- posterior encoder (models.py:836-842): pre -> 16-layer WN (g_src) -> proj -> sample
   float* h = ensure(d_h, F * H);
   float* acts = ensure(d_acts, F * H);
   float* skip = ensure(d_skip, F * H);
@@ -2363,11 +2397,10 @@ void vtts_engine::posterior_side(bool from_spec, const float* noise, const float
     flush_tails(fl, fo);
   }
   {
-    ConvP p = mk(q_pre, feat, spec_pad, 0, h, H, 0, 1, 0);
+    ConvP p = mk(q_pre, feat, feat_ld, 0, h, H, 0, 1, 0);
     if (q_tc) { p.p_hi = flp.pwx.hi; p.p_lo = flp.pwx.lo; p.ldp = H; p.pl_slope = 1.f; }
     launch_conv({p}, 1, fl, fo, maxFrm, B);
   }
-  const float* qcond = csrc ? csrc + condR : nullptr;
   if (q_tc) {
     wn_tc(qt_in, q_in, qt_rsx, q_rsx, qt_rss, q_rss, Q_LAYERS, Q_KERNEL, 1, h, skip, flp.pwx, flp.pacts, flp.pskip, qcond, qld, fl, fo);
     TcSpec q; q.in = flp.pskip; q.w = qt_proj; q.bias = q_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
@@ -2381,7 +2414,21 @@ void vtts_engine::posterior_side(bool from_spec, const float* noise, const float
   CK(cudaGetLastError());
   ++launches;
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vz_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+}
+
+void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc) {
+  const int I = cfg.inter_channels;
+  const size_t F = (size_t)Tfrm;
+  const int qld = condR + q_R;
+  const int* fl = d_frm_len.p;
+  const int* fo = d_frm_off.p;
+  // ---- enc_q input rows [F][spec_pad]
+  float* feat = front_end(from_spec);
+  // ---- posterior encoder (models.py:836-842): pre -> 16-layer WN (g_src) -> proj -> sample
+  posterior_encode(feat, spec_pad, noise, csrc ? csrc + condR : nullptr, qld);
+  float* z = d_z.p;
   // ---- z_p = flow(z, g_src)   (models.py:1715, 1640)
+  const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
   if (flow_on_tc) flow_tc(z, fl, fo, false, csrc, qld, /*forward=*/true);
   else flow_ffma(z, fl, fo, csrc, qld, /*forward=*/true);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vzp_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -2497,6 +2544,22 @@ void vtts_engine::bind_quickvc() {
   fit(lstm_rec_kernel<2>, spk_rec_smem<2>(), spk_clusters[1]);
   fit(lstm_rec_kernel<4>, spk_rec_smem<4>(), spk_clusters[2]);
   fit(lstm_rec_kernel<8>, spk_rec_smem<8>(), spk_clusters[3]);
+  // ---- the conversion side, when the blob has it (weights.pack_quickvc of a whole checkpoint)
+  has_encp = tensors.count("encp.pre.b") > 0;
+  if (has_encp) {
+    REQUIRE(c.decoder_type == 0 && c.resblock_type == 1 && c.n_upsamples == 2 && !c.use_transformer_flows && c.flow_n_flows % 2 == 0 &&
+                c.hidden_channels % 32 == 0 && c.hidden_channels <= 256 && c.n_resblock_kernels <= CV_MAXP,
+            VTTS_ERR_INVALID, "unsupported QuickVC configuration (the published ms_istft_vits model: two upsampling stages, "
+            "ResBlock1, plain coupling flow with an even number of layers)");
+    r_flow = 0;
+    r_dec = c.flow_n_flows * c.flow_wn_layers * 2 * c.hidden_channels;
+    condR = r_dec + c.upsample_initial_channel;
+    cond_w = vec("cond.w", (size_t)condR * c.gin_channels);
+    cond_b = vec("cond.b", condR);
+    bind_flow_decoder();
+    bind_wn_encoder("encp", QV_UNITS);
+    istft_w2 = vec("dec.w2", (size_t)c.istft_n_fft);
+  }
 }
 
 // Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
@@ -2546,6 +2609,72 @@ void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int ma
   klaunch(spk_embed_kernel, dim3(B), dim3(SPK_H), (size_t)0, x, last, of_clip, spk_lin_w, spk_lin_b, ensure(d_sg, (size_t)B * SPK_H));
   CK(cudaGetLastError());
   ++launches;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// QuickVC conversion (SynthesizerTrn.infer, vc/models.py:862-872) from content units and g: cond rows of g, enc_p, the
+// reverse flow with g, the decoder with cond(g) and the torch.istft tail.  The frame counts are the unit counts, so the whole
+// call is ONE graphed phase.
+// ---------------------------------------------------------------------------------------------------
+// Pinned staging of one call (fixed layout for a given batch / length bucket): ints [frm_len B][frm_off B+1][identity B],
+// prm[16], unit rows [Tfrm][QV_UNITS] (clips packed as the engine's rows, SEQ_GAP zero rows between them), g [B][gin],
+// eps [B][inter][maxFrm].
+vtts_engine::QvPin vtts_engine::qv_layout(bool eps) {
+  const vtts_config& c = cfg;
+  const size_t ints = (size_t)(3 * B + 1) * sizeof(int);
+  const size_t head = (ints + 63) / 64 * 64;
+  const size_t nu = (size_t)Tfrm * QV_UNITS, ng = (size_t)B * c.gin_channels, ne = eps ? (size_t)B * c.inter_channels * maxFrm : 0;
+  char* pin = ensure_pinned(h_pin_qv, head + (16 + nu + ng + ne) * sizeof(float) + 64);
+  QvPin pp;
+  pp.frm_len = reinterpret_cast<int*>(pin);
+  pp.frm_off = pp.frm_len + B;
+  pp.ident = pp.frm_off + B + 1;
+  pp.prm = reinterpret_cast<float*>(pin + head);
+  pp.units = pp.prm + 16;
+  pp.g = pp.units + nu;
+  pp.eps = pp.g + ng;
+  return pp;
+}
+
+void vtts_engine::quickvc_enqueue(bool eps) {
+  const vtts_config& c = cfg;
+  const int I = c.inter_channels, G = c.gin_channels;
+  if (!capturing) CK(cudaEventRecord(ev[4], stream));
+  QvPin pp = qv_layout(eps);
+  int* fl = ensure(d_frm_len, B);
+  int* fo = ensure(d_frm_off, B + 1);
+  int* ident = ensure(d_vint, B);
+  float* prm = ensure(d_vprm, 16);
+  float* units = ensure(d_units, (size_t)Tfrm * QV_UNITS);
+  float* g = ensure(d_qg, (size_t)B * G);
+  CK(cudaMemcpyAsync(fl, pp.frm_len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(fo, pp.frm_off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(ident, pp.ident, B * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(prm, pp.prm, 16 * sizeof(float), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(units, pp.units, (size_t)Tfrm * QV_UNITS * sizeof(float), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(g, pp.g, (size_t)B * G * sizeof(float), cudaMemcpyHostToDevice, stream));
+  float* noise = nullptr;
+  if (eps) {
+    noise = ensure(d_vnoise, (size_t)B * I * maxFrm);
+    CK(cudaMemcpyAsync(noise, pp.eps, (size_t)B * I * maxFrm * sizeof(float), cudaMemcpyHostToDevice, stream));
+  }
+  // ---- g's cond rows [B][condR] (the flow's WN cond layers, then dec.cond) in d_condv: the uploaded g rows are the table
+  //      cond_vc_kernel reads, through the identity index
+  float* cond = ensure(d_condv, (size_t)B * condR);
+  klaunch(cond_vc_kernel, dim3((condR + 7) / 8, B), dim3(256), (size_t)(G * sizeof(float)), (const float*)g, (const int*)ident, cond_w,
+          cond_b, condR, (const float*)nullptr, (const float*)nullptr, 0, cond, (float*)nullptr, G, B, B);
+  CK(cudaGetLastError());
+  ++launches;
+  // ---- z_p, m_p, logs_p = enc_p(c)   (models.py:868)
+  posterior_encode(units, QV_UNITS, noise, nullptr, 0);
+  // ---- z = flow(z_p, g, reverse=True)   (models.py:869)
+  float* z = d_z.p;
+  const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
+  if (flow_on_tc) flow_tc(z, fl, fo, false, cond, condR, /*forward=*/false);
+  else flow_ffma(z, fl, fo, cond, condR, /*forward=*/false);
+  if (!capturing) CK(cudaEventRecord(ev[5], stream));
+  // ---- o = dec(z * c_mask, g)   (models.py:870)
+  decode(z, fl, fo);
 }
 
 // ===================================================================================================
@@ -3022,6 +3151,68 @@ static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const 
   }
 }
 
+// QuickVC conversion through host buffers (vtts_quickvc_convert).
+static void impl_quickvc_convert(vtts_handle h, const float* units, const int64_t* lengths, int B, int64_t units_ld, const float* g,
+                                 float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
+                                 int64_t* out_frames) {
+  const vtts_config& c = h->cfg;
+  REQUIRE(h->has_encp, VTTS_ERR_INVALID, "the weight blob holds only the speaker encoder: conversion needs a model packed by "
+          "weights.pack_quickvc from a whole QuickVC checkpoint (enc_p, flow, dec)");
+  REQUIRE(B >= 1 && B <= 16384, VTTS_ERR_INVALID, "bad batch size");
+  REQUIRE(units_ld >= 1 && units_ld < (1LL << 24), VTTS_ERR_INVALID, "bad units_ld");
+  REQUIRE(g != nullptr, VTTS_ERR_INVALID, "g (the target's speaker embedding, vtts_speaker_embedding) is required");
+  std::vector<int> frames(B);
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lengths[b] >= 1 && lengths[b] <= units_ld, VTTS_ERR_INVALID, "unit_lengths must be in [1, units_ld]");
+    frames[b] = (int)lengths[b];
+  }
+  const int real_max = *std::max_element(frames.begin(), frames.end());
+  REQUIRE((int64_t)real_max * h->hop <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than hop * max(unit_lengths)");
+  REQUIRE(!noise || noise_ld >= real_max, VTTS_ERR_CAPACITY, "noise has fewer columns than max(unit_lengths)");
+  h->B = B;
+  h->have_durations = false;
+  h->have_latent = false;
+  h->h_frm_len = frames;
+  h->h_frm_off.assign(B + 1, 0);
+  int off = 0;
+  for (int b = 0; b < B; ++b) { h->h_frm_off[b] = off; off += frames[b] + (b + 1 < B ? SEQ_GAP : 0); }
+  h->h_frm_off[B] = off;
+  h->set_frame_shape();
+  const int maxF = h->maxFrm, I = c.inter_channels, G = c.gin_channels;
+  vtts_engine::QvPin pp = h->qv_layout(noise != nullptr);
+  memcpy(pp.frm_len, frames.data(), B * sizeof(int));
+  memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
+  for (int b = 0; b < B; ++b) {
+    pp.ident[b] = b;
+    const int o = h->h_frm_off[b];
+    memcpy(pp.units + (size_t)o * vtts_engine::QV_UNITS, units + (size_t)b * units_ld * vtts_engine::QV_UNITS,
+           (size_t)frames[b] * vtts_engine::QV_UNITS * sizeof(float));
+    const int gap_end = b + 1 < B ? h->h_frm_off[b + 1] : h->Tfrm;       // rows behind the clip: the gap, or the bucket's tail
+    memset(pp.units + (size_t)(o + frames[b]) * vtts_engine::QV_UNITS, 0, (size_t)(gap_end - o - frames[b]) * vtts_engine::QV_UNITS * sizeof(float));
+    memcpy(pp.g + (size_t)b * G, g + (size_t)b * G, G * sizeof(float));
+    if (noise)
+      for (int ch = 0; ch < I; ++ch)
+        memcpy(pp.eps + ((size_t)b * I + ch) * maxF, noise + ((size_t)b * I + ch) * noise_ld, (size_t)frames[b] * sizeof(float));
+  }
+  for (int i = 0; i < 16; ++i) pp.prm[i] = 0.f;
+  pp.prm[0] = noise_scale;
+  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
+  memcpy(&pp.prm[4], &lo, 4);
+  memcpy(&pp.prm[5], &hi, 4);
+  h->run_graphed({0x77, B, h->maxFrm, h->Tfrm, noise ? 1 : 0}, [&] { h->quickvc_enqueue(noise != nullptr); });
+  const size_t nw = (size_t)h->real_Tfrm * h->hop;
+  float* pw = reinterpret_cast<float*>(h->ensure_pinned((size_t)h->Tfrm * h->hop * sizeof(float) + 64));
+  CK(cudaMemcpyAsync(pw, h->d_wav.p, nw * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaEventRecord(h->ev[7], h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; ++b) {
+    const size_t n = (size_t)frames[b] * h->hop;
+    memcpy(out_wav + (size_t)b * out_ld, pw + (size_t)h->h_frm_off[b] * h->hop, n * sizeof(float));
+    std::fill(out_wav + (size_t)b * out_ld + n, out_wav + (size_t)(b + 1) * out_ld, 0.f);
+    out_frames[b] = frames[b];
+  }
+}
+
 static void impl_synthesize_dev(vtts_handle h, const float* d_noise_z, int z_ld, float* d_wav, int64_t wav_ld) {
   REQUIRE(h->have_durations, VTTS_ERR_STATE, "vtts_synthesize_dev called without vtts_durations_dev");
   REQUIRE((int64_t)h->real_maxFrm * h->hop <= wav_ld, VTTS_ERR_CAPACITY, "wav_ld is smaller than hop * max(y_lengths)");
@@ -3169,14 +3360,14 @@ void vtts_destroy(vtts_handle h) {
                       &h->d_fao, &h->d_fy, &h->d_ffh2, &h->d_eps_z, &h->d_d0, &h->d_post, &h->d_wav};
   for (auto* b : fb) fr(b->p);
   Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg,
-                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg};
+                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg, &h->d_units, &h->d_qg};
   for (auto* b : vb) fr(b->p);
   fr(h->d_vint.p);
   fr(h->d_sseq.p);
   for (auto& b : h->d_stage) fr(b.p);
   for (auto& v : h->d_xj) for (auto& b : v) fr(b.p);
   for (auto& v : h->d_tmp) for (auto& b : v) fr(b.p);
-  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc}) if (hb->p) cudaFreeHost(hb->p);
+  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc, &h->h_pin_qv}) if (hb->p) cudaFreeHost(hb->p);
   for (auto& kv : h->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   fr(h->d_prm.p);
   fr(h->d_pref.p);
@@ -3518,6 +3709,14 @@ int vtts_speaker_embedding(vtts_handle h, const float* wav, const int64_t* wav_l
 int vtts_speaker_embedding_mel(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* g_out) {
   if (!mel || !mel_lengths || !g_out) return VTTS_ERR_INVALID;
   return guarded(h, [&] { impl_speaker_embedding(h, true, mel, mel_lengths, B, mel_ld, g_out); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_quickvc_convert(vtts_handle h, const float* units, const int64_t* unit_lengths, int B, int64_t units_ld, const float* g,
+                         float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
+                         int64_t* out_frames) {
+  if (!units || !unit_lengths || !out_wav || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_quickvc_convert(h, units, unit_lengths, B, units_ld, g, noise_scale, noise, noise_ld, seed, out_wav, out_ld,
+                                               out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
 }
 
 // Host copies of a debug hook's arguments on the device (freed on every exit).

@@ -1544,6 +1544,9 @@ __global__ void mrf_mean_kernel(const float* __restrict__ a, const float* __rest
 // (pqmf.py:105-116: zero-stuffing x subbands, 63-tap FIR).  One CTA produces TL_M subband samples
 // (= TL_M*subbands output samples) of one utterance.
 //   post rows: per utterance L1 = 16*Ty + 1 frames of `subbands*(n_fft+2)` channels.
+//   w2: null for OnnxSTFT.inverse (VITS2); else the squared window [nfft], and every sample is divided by the window
+//       envelope sum_f w2[pos] over the frames that cover it -- torch.istft, as QuickVC's TorchSTFT.inverse calls it
+//       (vc/stft.py:197-202).
 // ------------------------------------------------------------------------------------------------
 constexpr int TL_M = 64;        // subband samples per CTA (256 output samples): 4x more CTAs than the first version, 40 -> ~12 us at batch 1
 constexpr int TL_THREADS = 256;
@@ -1558,7 +1561,7 @@ __global__ void __launch_bounds__(TL_THREADS)
 istft_pqmf_kernel(const float* __restrict__ post, int ldp, const float* __restrict__ basis, const float* __restrict__ pqmf,
                   int subbands, int nfft, int hop, int taps, int up_total /* frames -> post rows multiplier */,
                   const int* __restrict__ frm_len, const int* __restrict__ frm_off, float* __restrict__ wav, long wav_ld,
-                  int packed_out) {
+                  int packed_out, const float* __restrict__ w2) {
   PDL_LAUNCH();
   PDL_WAIT();
   const int b = blockIdx.y;
@@ -1606,12 +1609,15 @@ istft_pqmf_kernel(const float* __restrict__ post, int ldp, const float* __restri
       fa = fa <= 0 ? 0 : (fa + hop - 1) / hop;
       int fb = u / hop;
       if (fb > L1 - 1) fb = L1 - 1;
+      float env = 0.f;
       for (int f = fa; f <= fb; ++f) {
         const float* rr = rec + ((f - f_lo) * subbands + k) * cps;
         const int pos = u - f * hop;
         for (int c = 0; c < cps; ++c) a = fmaf(rr[c], basis[c * nfft + pos], a);
+        if (w2) env += w2[pos];
       }
-      a *= scale;
+      if (w2) a *= scale / env;          // (env >= 1.25 on every kept sample: no division by a vanishing envelope)
+      else a *= scale;
     }
     ysub[k * yw + (m - ms)] = a;
   }

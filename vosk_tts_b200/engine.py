@@ -51,7 +51,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
-           "vtts_speaker_embedding_mel"]
+           "vtts_speaker_embedding_mel", "vtts_quickvc_convert"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1}    # vtts_config.model_family
 
@@ -221,6 +221,8 @@ def load_library(build_if_missing=True):
         fn = getattr(lib, nm)
         fn.argtypes = [vp, vp, vp, i32, C.c_int64, vp]
         fn.restype = i32
+    lib.vtts_quickvc_convert.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_float, vp, i32, C.c_uint64, vp, C.c_int64, vp]
+    lib.vtts_quickvc_convert.restype = i32
     _LIB = lib
     return lib
 
@@ -553,6 +555,44 @@ class Engine:
         later calls within these bounds move no buffer."""
         hop = int(self.cfg["hop_length"])
         self.speaker_embedding(np.zeros((int(batch), int(max_frames) * hop), np.float32))
+        return int(max_frames)
+
+    # ---- QuickVC conversion (SynthesizerTrn.infer, vc/models.py:862-872)
+    def quickvc_convert(self, units, g, lengths=None, noise_scale=1.0, noise=None, seed=0):
+        """Content units -> waveforms in the voice of g (vtts_quickvc_convert).  units: one clip [T, 768] (ContentVec's
+        last_hidden_state, vc/encode.py's .npy), a batch [B, T, 768] with `lengths`, or a list of ragged [T_b, 768] arrays;
+        g: [gin_channels] (one target for every clip) or [B, gin_channels] (speaker_embedding's output).  noise: None
+        (Philox from `seed`) or [B, inter_channels, >= max T] standing in for torch.randn_like.  Returns (wav float32
+        [B, hop * max T], zeros past each clip's end; frames int64 [B])."""
+        if isinstance(units, (list, tuple)):
+            clips = [np.asarray(u, np.float32) for u in units]
+            lengths = np.array([u.shape[0] for u in clips], np.int64)
+            batch = np.zeros((len(clips), int(lengths.max()), 768), np.float32)
+            for b, u in enumerate(clips):
+                batch[b, :u.shape[0]] = u
+            units = batch
+        units = np.ascontiguousarray(units, dtype=np.float32)
+        if units.ndim == 2:
+            units = units[None]
+        B, T = units.shape[0], units.shape[1]
+        lengths = np.ascontiguousarray(np.full(B, T) if lengths is None else lengths, dtype=np.int64).reshape(B)
+        G = int(self.cfg["gin_channels"])
+        g = np.ascontiguousarray(np.broadcast_to(np.asarray(g, np.float32).reshape(-1, G), (B, G)), dtype=np.float32)
+        ld = 0
+        if noise is not None:
+            noise = np.ascontiguousarray(noise, dtype=np.float32)
+            ld = noise.shape[2]
+        wav = np.zeros((B, max(1, int(lengths.max())) * self.hop), np.float32)
+        frames = np.zeros(B, np.int64)
+        self._check(self.lib.vtts_quickvc_convert(self.h, _ptr(units), _ptr(lengths), B, T, _ptr(g), float(noise_scale), _ptr(noise),
+                                                  ld, int(seed), _ptr(wav), wav.shape[1], _ptr(frames)))
+        return wav, frames
+
+    def reserve_quickvc_convert(self, max_frames=1024, batch=1):
+        """Workspace reservation for conversions of up to `batch` clips x `max_frames` content frames: one call of that size,
+        so later calls within these bounds move no buffer."""
+        self.quickvc_convert(np.zeros((int(batch), int(max_frames), 768), np.float32), np.zeros(int(self.cfg["gin_channels"]), np.float32),
+                             noise_scale=0.0)
         return int(max_frames)
 
     # ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)

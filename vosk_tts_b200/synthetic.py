@@ -22,6 +22,20 @@ import zlib
 import torch
 
 
+def _conv(out, name, co, ci, ks, wn=False, bias=True, gain=1.0, transposed=False):
+    """Appends the spec of one Conv1d / ConvTranspose1d (weight-normed: weight_g + weight_v) to `out`."""
+    shape = (ci, co, ks) if transposed else (co, ci, ks)
+    fan_in = ci * ks if not transposed else ci * ks / 4.0
+    std = gain / math.sqrt(fan_in)
+    if wn:
+        out.append((name + ".weight_g", (shape[0], 1, 1), "wn_g", name + ".weight_v"))
+        out.append((name + ".weight_v", shape, "normal", std))
+    else:
+        out.append((name + ".weight", shape, "normal", std))
+    if bias:
+        out.append((name + ".bias", (co,), "normal", 0.05))
+
+
 def _spec(cfg, posterior=False):
     """Ordered list of (name, shape, kind, scale) for every tensor ``infer`` touches (posterior=True: and the posterior
     encoder ``enc_q`` that ``voice_conversion`` uses, models.py:1616, 813-842)."""
@@ -34,17 +48,8 @@ def _spec(cfg, posterior=False):
     k = cfg["kernel_size"]
     out = []
 
-    def conv(name, co, ci, ks, wn=False, bias=True, gain=1.0, transposed=False):
-        shape = (ci, co, ks) if transposed else (co, ci, ks)
-        fan_in = ci * ks if not transposed else ci * ks / 4.0
-        std = gain / math.sqrt(fan_in)
-        if wn:
-            out.append((name + ".weight_g", (shape[0], 1, 1), "wn_g", name + ".weight_v"))
-            out.append((name + ".weight_v", shape, "normal", std))
-        else:
-            out.append((name + ".weight", shape, "normal", std))
-        if bias:
-            out.append((name + ".bias", (co,), "normal", 0.05))
+    def conv(*a, **kw):
+        _conv(out, *a, **kw)
 
     def ln(name, c):
         out.append((name + ".gamma", (c,), "gamma", 0.1))
@@ -167,8 +172,11 @@ def _gen(name, seed):
 def make_random_checkpoint(cfg, seed=1234, posterior=False):
     """state_dict (CPU fp32) in checkpoint layout; deterministic for (cfg, seed).  posterior=True adds the ``enc_q.*``
     tensors (every tensor is seeded by its name, so the others come out the same either way)."""
+    return _draw(_spec(cfg, posterior), seed)
+
+
+def _draw(spec, seed):
     sd = {}
-    spec = _spec(cfg, posterior)
     for name, shape, kind, arg in spec:
         if kind == "wn_g":
             continue
@@ -214,3 +222,58 @@ def make_random_speaker_encoder(cfg, seed=1234):
                    ("enc_spk.lstm.bias_ih_l%d" % l, (4 * G,)), ("enc_spk.lstm.bias_hh_l%d" % l, (4 * G,))]
     shapes += [("enc_spk.linear.weight", (G, G)), ("enc_spk.linear.bias", (G,))]
     return {name: ((torch.rand(shape, generator=_gen(name, seed)) * 2 - 1) * a).float().contiguous() for name, shape in shapes}
+
+
+def _spec_quickvc(cfg):
+    """(name, shape, kind, scale) of every tensor of the reference QuickVC SynthesizerTrn (vc/models.py:774-842) but the
+    speaker encoder: enc_p (PosteriorEncoder(768, I, H, 5, 1, 16), no g), enc_q (the same over the linear spectrogram, with
+    g), the flow (ResidualCouplingBlock(I, H, 5, 1, 4, gin): mean-only coupling layers at even indices, Flip between) and
+    the Multistream_iSTFT_Generator decoder (:416-501) with its cond Conv1d(256, 512, 1) and the updown_filter buffer."""
+    H, I, G = cfg["hidden_channels"], cfg["inter_channels"], cfg["gin_channels"]
+    out = []
+    conv = lambda *a, **kw: _conv(out, *a, **kw)
+    for p, cin, gin in (("enc_p", cfg["unit_channels"], 0), ("enc_q", cfg["filter_length"] // 2 + 1, G)):
+        conv(p + ".pre", H, cin, 1, gain=0.5 if p == "enc_q" else 1.0)
+        for i in range(16):
+            conv("%s.enc.in_layers.%d" % (p, i), 2 * H, H, 5, wn=True, gain=1.0)
+            conv("%s.enc.res_skip_layers.%d" % (p, i), 2 * H if i < 15 else H, H, 1, wn=True, gain=0.5)
+        if gin:
+            conv(p + ".enc.cond_layer", 2 * H * 16, gin, 1, wn=True, gain=0.5)
+        conv(p + ".proj", 2 * I, H, 1, gain=0.1)
+    for f in range(cfg["flow_n_flows"]):
+        p = "flow.flows.%d" % (2 * f)
+        conv(p + ".pre", H, I // 2, 1)
+        for i in range(cfg["flow_wn_layers"]):
+            conv("%s.enc.in_layers.%d" % (p, i), 2 * H, H, cfg["flow_kernel_size"], wn=True, gain=1.0)
+            conv("%s.enc.res_skip_layers.%d" % (p, i), 2 * H if i < cfg["flow_wn_layers"] - 1 else H, H, 1, wn=True, gain=0.7)
+        conv(p + ".enc.cond_layer", 2 * H * cfg["flow_wn_layers"], G, 1, wn=True, gain=0.5)
+        conv(p + ".post", I // 2, H, 1, gain=0.35)
+    C0 = cfg["upsample_initial_channel"]
+    conv("dec.conv_pre", C0, I, 7, wn=True, gain=1.0)
+    ch = C0
+    nk = len(cfg["resblock_kernel_sizes"])
+    for i, ku in enumerate(cfg["upsample_kernel_sizes"]):
+        conv("dec.ups.%d" % i, ch // 2, ch, ku, wn=True, gain=1.0, transposed=True)
+        ch //= 2
+        for j, rd in enumerate(cfg["resblock_dilation_sizes"]):
+            for d in range(len(rd)):
+                conv("dec.resblocks.%d.convs1.%d" % (i * nk + j, d), ch, ch, cfg["resblock_kernel_sizes"][j], wn=True, gain=0.55)
+                conv("dec.resblocks.%d.convs2.%d" % (i * nk + j, d), ch, ch, cfg["resblock_kernel_sizes"][j], wn=True, gain=0.55)
+    conv("dec.subband_conv_post", cfg["subbands"] * (cfg["gen_istft_n_fft"] + 2), ch, 7, wn=True, bias=True, gain=0.25)
+    conv("dec.multistream_conv_post", 1, cfg["subbands"], 63, wn=True, bias=False, gain=1.0)
+    conv("dec.cond", C0, G, 1, gain=0.5)
+    return out
+
+
+def make_random_quickvc(cfg, seed=1234):
+    """A whole QuickVC checkpoint state dict (CPU fp32) in the reference's names and shapes, weight-normed convs as
+    weight_g / weight_v: enc_p, enc_q (real checkpoints carry it; inference never reads it), the flow, the decoder with its
+    updown_filter buffer, and enc_spk exactly as make_random_speaker_encoder(cfg, seed) draws it."""
+    sd = _draw(_spec_quickvc(cfg), seed)
+    sb = cfg["subbands"]
+    updown = torch.zeros(sb, sb, sb)
+    for k in range(sb):
+        updown[k, k, 0] = 1.0
+    sd["dec.updown_filter"] = updown
+    sd.update(make_random_speaker_encoder(cfg, seed))
+    return sd

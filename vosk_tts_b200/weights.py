@@ -9,6 +9,8 @@ tensor out the way the CUDA kernels consume it.
 import numpy as np
 import torch
 
+from . import config as _config
+
 
 def fold_weight_norm(sd):
     """w = g * v / ||v||, the norm taken over all dims but 0 (torch.nn.utils.weight_norm dim=0;
@@ -228,11 +230,12 @@ class _Packer:
         return blob, manifest
 
 
-def convt_phases(u, K):
-    """Polyphase split of ConvTranspose1d(k=K, stride=u, padding=(K-u)//2): for phase r the taps
-    (in increasing input position) are kernel columns j_m, and `pad` inputs lie left of t.
+def convt_phases(u, K, p=None):
+    """Polyphase split of ConvTranspose1d(k=K, stride=u, padding=p) (default p = (K-u)//2; config.convt_pad gives each
+    stage's): for phase r the taps (in increasing input position) are kernel columns j_m, and `pad` inputs lie left of t.
     out[u*t + r] = sum_m x[t - pad + m] * W[:, :, j_m]."""
-    p = (K - u) // 2
+    if p is None:
+        p = (K - u) // 2
     phases = []
     for r in range(u):
         d_min = -((r + p) // u)            # ceil(-(r+p)/u)
@@ -249,6 +252,135 @@ def tc_supported(cfg):
     return (cfg["decoder"] in ("mb_istft", "ms_istft", "istft") and str(cfg["resblock"]) == "1" and cfg["hidden_channels"] % 64 == 0 and
             cfg["filter_channels"] % 64 == 0 and cfg["inter_channels"] % 64 == 0 and
             (cfg["upsample_initial_channel"] >> n_ups) % 64 == 0)
+
+
+def _pack_wn_encoder(P, g, dst, src, H, tc, fw):
+    """The 16-layer WN stack (kernel 5, no cond here) and proj of a PosteriorEncoder (models.py:813-842; QuickVC's enc_p and
+    enc_q, vc/models.py:242-271) under <dst>.in<i> / .rsx<i> / .rss<i> / .proj, gate channels interleaved; <dst>.pre and the
+    cond rows are packed by the caller."""
+    il = np.arange(2 * H).reshape(2, H).T.reshape(-1)
+    nq = 16
+    for i in range(nq):
+        lay = "%s.enc.in_layers.%d" % (src, i)
+        P.conv("%s.in%d" % (dst, i), g(lay + ".weight"), g(lay + ".bias"), co_perm=il, need_w=fw)
+        if tc:
+            P.conv_tc("%s.in%d" % (dst, i), g(lay + ".weight"), co_perm=il)
+        rw, rb = g("%s.enc.res_skip_layers.%d.weight" % (src, i)), g("%s.enc.res_skip_layers.%d.bias" % (src, i))
+        if i < nq - 1:
+            P.conv("%s.rsx%d" % (dst, i), rw[:H], rb[:H], need_w=fw)
+            P.conv("%s.rss%d" % (dst, i), rw[H:], rb[H:], need_w=fw)
+            if tc:
+                P.conv_tc("%s.rsx%d" % (dst, i), rw[:H])
+                P.conv_tc("%s.rss%d" % (dst, i), rw[H:])
+        else:
+            P.conv("%s.rss%d" % (dst, i), rw, rb, need_w=fw)
+            if tc:
+                P.conv_tc("%s.rss%d" % (dst, i), rw)
+    P.conv(dst + ".proj", g(src + ".proj.weight"), g(src + ".proj.bias"), need_w=fw)
+    if tc:
+        P.conv_tc(dst + ".proj", g(src + ".proj.weight"))
+
+
+def _flow_cond_rows(g, cfg, rows_w, rows_b):
+    """Appends the WN cond_layer rows of every coupling layer (flow.flows.<2f>.enc.cond_layer), layer by layer, with the
+    gate channels interleaved as the packed in_layers are: one block of the stacked conditioning matrix cond.w / cond.b."""
+    H, nl = cfg["hidden_channels"], cfg["flow_wn_layers"]
+    il = np.arange(2 * H).reshape(2, H).T.reshape(-1)     # gate interleave: [t0,s0,t1,s1,...]
+    for f in range(cfg["flow_n_flows"]):
+        cw = g("flow.flows.%d.enc.cond_layer.weight" % (2 * f))[:, :, 0]
+        cb = g("flow.flows.%d.enc.cond_layer.bias" % (2 * f))
+        for i in range(nl):
+            rows_w.append(cw[i * 2 * H:(i + 1) * 2 * H][il])
+            rows_b.append(cb[i * 2 * H:(i + 1) * 2 * H][il])
+
+
+def _pack_flow_decoder(P, g, w, cfg, tc, fw, enc_layer=None):
+    """The reverse flow (flow.*) and the decoder (dec.*) of a VITS2 or QuickVC state dict; enc_layer packs the flow's
+    pre_transformer (use_transformer_flows only)."""
+    H, I = cfg["hidden_channels"], cfg["inter_channels"]
+    # ---- flow (reverse); channel flips are folded into the pre/post weights (see csrc/engine.cu)
+    nf = cfg["flow_n_flows"]
+    half = I // 2
+    rev = np.arange(half)[::-1].copy()
+    for f in range(nf):
+        src = "flow.flows.%d" % (2 * f)
+        dst = "flow.%d" % f
+        flipped = ((nf - f) % 2) == 1
+        P.conv(dst + ".pre", g(src + ".pre.weight"), g(src + ".pre.bias"), ci_perm=rev if flipped else None)
+        if cfg["use_transformer_flows"]:
+            enc_layer(dst + ".tr", src + ".pre_transformer", 0, with_tc=tc, need_w=fw)
+        nl = cfg["flow_wn_layers"]
+        il = np.arange(2 * H).reshape(2, H).T.reshape(-1)
+        for i in range(nl):
+            P.conv("%s.in%d" % (dst, i), g("%s.enc.in_layers.%d.weight" % (src, i)),
+                   g("%s.enc.in_layers.%d.bias" % (src, i)), co_perm=il, need_w=fw)
+            rw, rb = g("%s.enc.res_skip_layers.%d.weight" % (src, i)), g("%s.enc.res_skip_layers.%d.bias" % (src, i))
+            if tc:
+                P.conv_tc("%s.in%d" % (dst, i), g("%s.enc.in_layers.%d.weight" % (src, i)), co_perm=il)
+            if i < nl - 1:
+                P.conv("%s.rsx%d" % (dst, i), rw[:H], rb[:H], need_w=fw)
+                P.conv("%s.rss%d" % (dst, i), rw[H:], rb[H:], need_w=fw)
+                if tc:
+                    P.conv_tc("%s.rsx%d" % (dst, i), rw[:H])
+                    P.conv_tc("%s.rss%d" % (dst, i), rw[H:])
+            else:
+                P.conv("%s.rss%d" % (dst, i), rw, rb, need_w=fw)
+                if tc:
+                    P.conv_tc("%s.rss%d" % (dst, i), rw)
+        P.conv(dst + ".post", g(src + ".post.weight"), g(src + ".post.bias"), co_perm=rev if flipped else None, need_w=fw)
+        if tc:
+            P.conv_tc(dst + ".post", g(src + ".post.weight"), co_perm=rev if flipped else None)
+
+    # ---- decoder
+    pre_w = g("dec.conv_pre.weight")
+    if nf % 2 == 1:   # odd number of flips leaves the latent channel-reversed: fold into conv_pre
+        pre_w = pre_w[:, ::-1].copy()
+    P.conv("dec.pre", pre_w, g("dec.conv_pre.bias"), need_w=fw)
+    if tc:
+        P.conv_tc("dec.pre", pre_w)
+    nk = len(cfg["resblock_kernel_sizes"])
+    for i, (u, ku) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+        wt = g("dec.ups.%d.weight" % i)                      # [Cin, Cout, K]
+        bt = g("dec.ups.%d.bias" % i)
+        for r, (pad, js) in enumerate(convt_phases(u, ku, _config.convt_pad(cfg, i)[0])):
+            wr = np.stack([wt[:, :, j] for j in js], axis=-1)   # [Cin, Cout, ntaps]
+            P.conv("dec.up%d.p%d" % (i, r), np.transpose(wr, (1, 0, 2)), bt, need_w=fw)
+            if tc:
+                P.conv_tc("dec.up%d.p%d" % (i, r), np.transpose(wr, (1, 0, 2)))
+        for j in range(nk):
+            n = i * nk + j
+            nd = len(cfg["resblock_dilation_sizes"][j])
+            for d in range(nd):
+                if cfg["resblock"] == "1":
+                    P.conv("dec.rb%d.c1.%d" % (n, d), g("dec.resblocks.%d.convs1.%d.weight" % (n, d)), g("dec.resblocks.%d.convs1.%d.bias" % (n, d)), need_w=fw)
+                    P.conv("dec.rb%d.c2.%d" % (n, d), g("dec.resblocks.%d.convs2.%d.weight" % (n, d)), g("dec.resblocks.%d.convs2.%d.bias" % (n, d)), need_w=fw)
+                    if tc:
+                        P.conv_tc("dec.rb%d.c1.%d" % (n, d), g("dec.resblocks.%d.convs1.%d.weight" % (n, d)))
+                        P.conv_tc("dec.rb%d.c2.%d" % (n, d), g("dec.resblocks.%d.convs2.%d.weight" % (n, d)))
+                else:
+                    P.conv("dec.rb%d.c.%d" % (n, d), g("dec.resblocks.%d.convs.%d.weight" % (n, d)), g("dec.resblocks.%d.convs.%d.bias" % (n, d)))
+    if cfg["decoder"] in ("mb_istft", "ms_istft", "istft"):
+        # All three end in conv_post -> exp / pi*sin -> inverse STFT -> zero-stuffing by `subbands` -> a 63-tap filter per band
+        # (zero padding 31).  Only the filter differs: the fixed PQMF synthesis bank (pqmf.py:63-89), the learned
+        # multistream_conv_post (models.py:1107), or -- one band, nothing after the iSTFT (models.py:962-965) -- a unit impulse.
+        post = "dec.conv_post" if cfg["decoder"] == "istft" else "dec.subband_conv_post"
+        post_b = g(post + ".bias") if (post + ".bias") in w else None          # only the multistream decoder has one (:1095)
+        P.conv("dec.post", g(post + ".weight"), post_b, need_w=fw)
+        if tc:
+            P.conv_tc("dec.post", g(post + ".weight"))
+        P.add("dec.istft", istft_inverse_basis(cfg["gen_istft_n_fft"], cfg["gen_istft_hop_size"]))
+        if cfg["decoder"] == "mb_istft":
+            bank = pqmf_synthesis_filter(cfg["subbands"])
+        elif cfg["decoder"] == "ms_istft":
+            bank = g("dec.multistream_conv_post.weight")[0]
+            assert bank.shape == (cfg["subbands"], 63), bank.shape
+        else:
+            bank = np.zeros((1, 63), np.float32)
+            bank[0, 31] = 1.0
+        P.add("dec.pqmf", bank)
+    else:
+        P.conv("dec.post", g("dec.conv_post.weight"), None)
+
 
 
 def pack(w, cfg, tc=True, precision=None, posterior=False):
@@ -329,14 +461,7 @@ def pack(w, cfg, tc=True, precision=None, posterior=False):
             rows_b.append(g("enc_p.encoder.spk_emb_linear.bias"))
         rows_w.append(g("dp.cond.weight")[:, :, 0])
         rows_b.append(g("dp.cond.bias"))
-        nl = cfg["flow_wn_layers"]
-        il = np.arange(2 * H).reshape(2, H).T.reshape(-1)     # gate interleave: [t0,s0,t1,s1,...]
-        for f in range(cfg["flow_n_flows"]):
-            cw = g("flow.flows.%d.enc.cond_layer.weight" % (2 * f))[:, :, 0]
-            cb = g("flow.flows.%d.enc.cond_layer.bias" % (2 * f))
-            for i in range(nl):
-                rows_w.append(cw[i * 2 * H:(i + 1) * 2 * H][il])
-                rows_b.append(cb[i * 2 * H:(i + 1) * 2 * H][il])
+        _flow_cond_rows(g, cfg, rows_w, rows_b)
         if cfg["decoder"] == "hifigan" and "dec.cond.weight" in w:
             rows_w.append(g("dec.cond.weight")[:, :, 0])       # Generator's speaker projection (models.py:869-875)
             rows_b.append(g("dec.cond.bias"))
@@ -365,88 +490,7 @@ def pack(w, cfg, tc=True, precision=None, posterior=False):
         P.conv("dp.cf%d.proj" % n, g(src + ".proj.weight"), g(src + ".proj.bias"))
     P.add("dp.ea", np.concatenate([g("dp.flows.0.m").reshape(-1), g("dp.flows.0.logs").reshape(-1)]))
 
-    # ---- flow (reverse); channel flips are folded into the pre/post weights (see csrc/engine.cu)
-    nf = cfg["flow_n_flows"]
-    half = I // 2
-    rev = np.arange(half)[::-1].copy()
-    for f in range(nf):
-        src = "flow.flows.%d" % (2 * f)
-        dst = "flow.%d" % f
-        flipped = ((nf - f) % 2) == 1
-        P.conv(dst + ".pre", g(src + ".pre.weight"), g(src + ".pre.bias"), ci_perm=rev if flipped else None)
-        if cfg["use_transformer_flows"]:
-            enc_layer(dst + ".tr", src + ".pre_transformer", 0, with_tc=tc, need_w=fw)
-        nl = cfg["flow_wn_layers"]
-        il = np.arange(2 * H).reshape(2, H).T.reshape(-1)
-        for i in range(nl):
-            P.conv("%s.in%d" % (dst, i), g("%s.enc.in_layers.%d.weight" % (src, i)),
-                   g("%s.enc.in_layers.%d.bias" % (src, i)), co_perm=il, need_w=fw)
-            rw, rb = g("%s.enc.res_skip_layers.%d.weight" % (src, i)), g("%s.enc.res_skip_layers.%d.bias" % (src, i))
-            if tc:
-                P.conv_tc("%s.in%d" % (dst, i), g("%s.enc.in_layers.%d.weight" % (src, i)), co_perm=il)
-            if i < nl - 1:
-                P.conv("%s.rsx%d" % (dst, i), rw[:H], rb[:H], need_w=fw)
-                P.conv("%s.rss%d" % (dst, i), rw[H:], rb[H:], need_w=fw)
-                if tc:
-                    P.conv_tc("%s.rsx%d" % (dst, i), rw[:H])
-                    P.conv_tc("%s.rss%d" % (dst, i), rw[H:])
-            else:
-                P.conv("%s.rss%d" % (dst, i), rw, rb, need_w=fw)
-                if tc:
-                    P.conv_tc("%s.rss%d" % (dst, i), rw)
-        P.conv(dst + ".post", g(src + ".post.weight"), g(src + ".post.bias"), co_perm=rev if flipped else None, need_w=fw)
-        if tc:
-            P.conv_tc(dst + ".post", g(src + ".post.weight"), co_perm=rev if flipped else None)
-
-    # ---- decoder
-    pre_w = g("dec.conv_pre.weight")
-    if nf % 2 == 1:   # odd number of flips leaves the latent channel-reversed: fold into conv_pre
-        pre_w = pre_w[:, ::-1].copy()
-    P.conv("dec.pre", pre_w, g("dec.conv_pre.bias"), need_w=fw)
-    if tc:
-        P.conv_tc("dec.pre", pre_w)
-    nk = len(cfg["resblock_kernel_sizes"])
-    for i, (u, ku) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
-        wt = g("dec.ups.%d.weight" % i)                      # [Cin, Cout, K]
-        bt = g("dec.ups.%d.bias" % i)
-        for r, (pad, js) in enumerate(convt_phases(u, ku)):
-            wr = np.stack([wt[:, :, j] for j in js], axis=-1)   # [Cin, Cout, ntaps]
-            P.conv("dec.up%d.p%d" % (i, r), np.transpose(wr, (1, 0, 2)), bt, need_w=fw)
-            if tc:
-                P.conv_tc("dec.up%d.p%d" % (i, r), np.transpose(wr, (1, 0, 2)))
-        for j in range(nk):
-            n = i * nk + j
-            nd = len(cfg["resblock_dilation_sizes"][j])
-            for d in range(nd):
-                if cfg["resblock"] == "1":
-                    P.conv("dec.rb%d.c1.%d" % (n, d), g("dec.resblocks.%d.convs1.%d.weight" % (n, d)), g("dec.resblocks.%d.convs1.%d.bias" % (n, d)), need_w=fw)
-                    P.conv("dec.rb%d.c2.%d" % (n, d), g("dec.resblocks.%d.convs2.%d.weight" % (n, d)), g("dec.resblocks.%d.convs2.%d.bias" % (n, d)), need_w=fw)
-                    if tc:
-                        P.conv_tc("dec.rb%d.c1.%d" % (n, d), g("dec.resblocks.%d.convs1.%d.weight" % (n, d)))
-                        P.conv_tc("dec.rb%d.c2.%d" % (n, d), g("dec.resblocks.%d.convs2.%d.weight" % (n, d)))
-                else:
-                    P.conv("dec.rb%d.c.%d" % (n, d), g("dec.resblocks.%d.convs.%d.weight" % (n, d)), g("dec.resblocks.%d.convs.%d.bias" % (n, d)))
-    if cfg["decoder"] in ("mb_istft", "ms_istft", "istft"):
-        # All three end in conv_post -> exp / pi*sin -> inverse STFT -> zero-stuffing by `subbands` -> a 63-tap filter per band
-        # (zero padding 31).  Only the filter differs: the fixed PQMF synthesis bank (pqmf.py:63-89), the learned
-        # multistream_conv_post (models.py:1107), or -- one band, nothing after the iSTFT (models.py:962-965) -- a unit impulse.
-        post = "dec.conv_post" if cfg["decoder"] == "istft" else "dec.subband_conv_post"
-        post_b = g(post + ".bias") if (post + ".bias") in w else None          # only the multistream decoder has one (:1095)
-        P.conv("dec.post", g(post + ".weight"), post_b, need_w=fw)
-        if tc:
-            P.conv_tc("dec.post", g(post + ".weight"))
-        P.add("dec.istft", istft_inverse_basis(cfg["gen_istft_n_fft"], cfg["gen_istft_hop_size"]))
-        if cfg["decoder"] == "mb_istft":
-            bank = pqmf_synthesis_filter(cfg["subbands"])
-        elif cfg["decoder"] == "ms_istft":
-            bank = g("dec.multistream_conv_post.weight")[0]
-            assert bank.shape == (cfg["subbands"], 63), bank.shape
-        else:
-            bank = np.zeros((1, 63), np.float32)
-            bank[0, 31] = 1.0
-        P.add("dec.pqmf", bank)
-    else:
-        P.conv("dec.post", g("dec.conv_post.weight"), None)
+    _pack_flow_decoder(P, g, w, cfg, tc, fw, enc_layer)
 
     # ---- posterior encoder enc_q (models.py:813-842) + spectrogram front end, for voice conversion
     if posterior:
@@ -463,27 +507,9 @@ def pack(w, cfg, tc=True, precision=None, posterior=False):
         # enc_q.pre runs on the FFMA conv, which takes input channels in multiples of 16: zero-padded (513 -> 528 for a
         # linear spectrogram; the front end writes zeros into the pad columns)
         P.conv("encq.pre", np.pad(pre, ((0, 0), (0, (-sc) % 16), (0, 0))), g("enc_q.pre.bias"))
+        _pack_wn_encoder(P, g, "encq", "enc_q", H, tc, fw)
         il = np.arange(2 * H).reshape(2, H).T.reshape(-1)
         nq = 16
-        for i in range(nq):
-            src = "enc_q.enc.in_layers.%d" % i
-            P.conv("encq.in%d" % i, g(src + ".weight"), g(src + ".bias"), co_perm=il, need_w=fw)
-            if tc:
-                P.conv_tc("encq.in%d" % i, g(src + ".weight"), co_perm=il)
-            rw, rb = g("enc_q.enc.res_skip_layers.%d.weight" % i), g("enc_q.enc.res_skip_layers.%d.bias" % i)
-            if i < nq - 1:
-                P.conv("encq.rsx%d" % i, rw[:H], rb[:H], need_w=fw)
-                P.conv("encq.rss%d" % i, rw[H:], rb[H:], need_w=fw)
-                if tc:
-                    P.conv_tc("encq.rsx%d" % i, rw[:H])
-                    P.conv_tc("encq.rss%d" % i, rw[H:])
-            else:
-                P.conv("encq.rss%d" % i, rw, rb, need_w=fw)
-                if tc:
-                    P.conv_tc("encq.rss%d" % i, rw)
-        P.conv("encq.proj", g("enc_q.proj.weight"), g("enc_q.proj.bias"), need_w=fw)
-        if tc:
-            P.conv_tc("encq.proj", g("enc_q.proj.weight"))
         if has_g:
             cw, cb = g("enc_q.enc.cond_layer.weight")[:, :, 0], g("enc_q.enc.cond_layer.bias")
             P.add("encq.cond.w", np.concatenate([cw[i * 2 * H:(i + 1) * 2 * H][il] for i in range(nq)], 0))
@@ -509,11 +535,24 @@ def spk_hh_layout(whh):
     return np.ascontiguousarray(np.transpose(w, (1, 3, 0, 2)))   # [rank][k][gate][unit]
 
 
-def pack_quickvc(w, cfg):
-    """QuickVC state dict (folded) -> (blob, manifest) of a model_family "quickvc" engine: the speaker encoder enc_spk and
-    the mel front end of the target (vc/convert.py:60-69).  Each LSTM layer's input projection is a 1x1 conv whose bias is
-    b_ih + b_hh folded; W_hh goes in the CTA-blocked layout of the recurrence kernel; the linear layer is stored transposed.
-    enc_q and the discriminators, which inference never reads, are left out."""
+def hann_squared(n_fft):
+    """Squared periodic Hann window of n_fft samples: the window envelope torch.istft divides by (vc/stft.py:197-202), summed
+    by the tail kernel over the frames that cover each sample."""
+    n = np.arange(n_fft)
+    return ((0.5 - 0.5 * np.cos(2.0 * np.pi * n / n_fft)) ** 2).astype(np.float32)
+
+
+def pack_quickvc(w, cfg, tc=True, precision=None):
+    """QuickVC state dict (folded) -> (blob, manifest) of a model_family "quickvc" engine.
+
+    First the speaker encoder enc_spk and the mel front end of the target (vc/convert.py:60-69): each LSTM layer's input
+    projection is a 1x1 conv whose bias is b_ih + b_hh folded; W_hh goes in the CTA-blocked layout of the recurrence kernel;
+    the linear layer is stored transposed.  Then, when the state dict has enc_p (a full checkpoint, not an encoder alone), the
+    conversion side of SynthesizerTrn.infer (vc/models.py:862-872), after every speaker-encoder tensor so that those keep
+    their offsets: encp.* (the content encoder, laid out as pack's encq.*, without cond), flow.* and dec.* as pack lays them
+    out, one stacked cond.w / cond.b (the flow's WN cond rows, then dec.cond, the decoder's Conv1d(256, 512, 1)), and
+    dec.w2, the squared Hann window of the decoder's inverse STFT.  tc / precision: as in pack (the speaker encoder is fp32
+    in every mode).  enc_q and the discriminators, which inference never reads, are left out."""
     g = lambda k: w[k].detach().cpu().numpy() if hasattr(w[k], "detach") else np.asarray(w[k])
     P = _Packer()
     for l in range(cfg.get("spk_layers", 3)):
@@ -525,4 +564,21 @@ def pack_quickvc(w, cfg):
     n_fft = cfg["filter_length"]
     P.add("vc.stft", stft_basis(n_fft))
     P.add("vc.mel", mel_basis(cfg["sampling_rate"], n_fft, cfg["n_mel_channels"], cfg["mel_fmin"], cfg["mel_fmax"]))
+    if "enc_p.pre.weight" in w:
+        tc = tc and tc_supported(cfg) and precision != 0
+        fw = not (tc and precision in (1, 2, 3))
+        H = cfg["hidden_channels"]
+        pre = g("enc_p.pre.weight")
+        if pre.shape[1] != cfg["unit_channels"] or pre.shape[1] % 16:
+            raise ValueError("enc_p.pre has %d input channels, expected %d content-unit channels" % (pre.shape[1], cfg["unit_channels"]))
+        P.conv("encp.pre", pre, g("enc_p.pre.bias"))
+        _pack_wn_encoder(P, g, "encp", "enc_p", H, tc, fw)
+        _pack_flow_decoder(P, g, w, cfg, tc, fw)
+        rows_w, rows_b = [], []
+        _flow_cond_rows(g, cfg, rows_w, rows_b)
+        rows_w.append(g("dec.cond.weight")[:, :, 0])
+        rows_b.append(g("dec.cond.bias"))
+        P.add("cond.w", np.concatenate(rows_w, 0))
+        P.add("cond.b", np.concatenate(rows_b, 0))
+        P.add("dec.w2", hann_squared(cfg["gen_istft_n_fft"]))
     return P.finish()
