@@ -73,6 +73,13 @@ typedef struct vtts_config {
    * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding* and vtts_quickvc_convert.  The entry points of one family
    * return VTTS_ERR_INVALID on an engine of the other. */
   int32_t model_family;
+  /* ContentVec (HubertModel of vc/contentvec.py, transformers' HubertConfig; QuickVC engines whose blob carries cv.*):
+   * vtts_content_units / vtts_quickvc_convert_wav.  cv_layers == 0: no ContentVec. */
+  int32_t cv_layers, cv_hidden, cv_heads, cv_ffn;          /* transformer: 12 post-LN layers, 768 wide, 12 heads, FFN 3072 */
+  int32_t cv_conv_dim, cv_n_conv;                          /* feature encoder: 7 convs of 512 channels */
+  int32_t cv_conv_kernel[8], cv_conv_stride[8];            /* (10,3,3,3,3,2,2) / (5,2,2,2,2,2,2) */
+  int32_t cv_pos_k, cv_pos_groups;                         /* positional conv: 128 taps, 16 groups */
+  float cv_ln_eps, cv_gn_eps;                              /* LayerNorm eps (layer_norm_eps), layer 0's GroupNorm eps */
 } vtts_config;
 
 #define VTTS_FAMILY_VITS2 0
@@ -365,6 +372,28 @@ int vtts_speaker_embedding_mel(vtts_handle h, const float* mel, const int64_t* m
 int vtts_quickvc_convert(vtts_handle h, const float* units, const int64_t* unit_lengths, int B, int64_t units_ld,
                          const float* g, float noise_scale, const float* noise, int noise_ld, uint64_t seed,
                          float* out_wav, int64_t out_ld, int64_t* out_frames);
+
+/* ContentVec content units (HubertModel(...)["last_hidden_state"], as vc/encode.py and vc/convert.py:82 compute them) of
+ * 16 kHz source recordings.  Each clip is processed as if alone (B = 1 in the reference).  Frames per clip: L0 = (len - K0) / s0
+ * + 1, then L_i = (L_{i-1} - k_i) / s_i + 1 (499 for 10 s; a clip needs at least 400 samples at the published shape).
+ *   wav        float [B, wav_ld] in [-1, 1], clip b = its first wav_lengths[b] samples (no normalisation, as convert.py)
+ *   units      out float [B, units_ld, cv_hidden], frame-major (vtts_quickvc_convert's input layout), zeros after each clip
+ *   out_frames out int64 [B]
+ * Host pointers, atomic on the handle; one graphed call keyed by batch and sample-length bucket.  Every stage runs on the fp32
+ * FFMA pipe in every precision mode.  VTTS_ERR_INVALID: not a QuickVC engine, a blob without cv.*, B < 1, a clip too short
+ * for one frame or longer than wav_ld.  VTTS_ERR_CAPACITY: units_ld below a clip's frame count.
+ * After a call with bit0 of vtts_debug_flags set, vtts_debug_read "cv_feat" is the feature encoder's output [rows][cv_conv_dim]
+ * and "cv_enc_in" the transformer's input (after the positional conv and its LayerNorm) [rows][cv_hidden]; clip 0 starts
+ * at row 0. */
+int vtts_content_units(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, float* units,
+                       int64_t units_ld, int64_t* out_frames);
+/* Source recordings -> waveforms in the voice of g: vtts_content_units, then vtts_quickvc_convert on its units, in ONE call
+ * (the last LayerNorm writes the rows enc_p reads).  Arguments as those two; noise [B, inter_channels, noise_ld] with
+ * noise_ld >= the largest frame count, out_ld >= hop * that count.  VTTS_ERR_INVALID also for a blob without the conversion
+ * tensors. */
+int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const float* g,
+                             float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
+                             int64_t* out_frames);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

@@ -185,3 +185,66 @@ def hop_total(cfg):
     if cfg["decoder"] in ISTFT_DECODERS:
         up *= cfg["gen_istft_hop_size"] * cfg["subbands"]
     return up
+
+
+# ContentVec (vc/contentvec.py: HubertModelWithFinalProj(HubertConfig(conv_bias=False, classifier_proj_size=256))): the defaults
+# of transformers' HubertConfig, which are hubert-base's.
+CONTENTVEC_DEFAULTS = {
+    "hidden_size": 768, "num_hidden_layers": 12, "num_attention_heads": 12, "intermediate_size": 3072, "hidden_act": "gelu",
+    "feat_extract_norm": "group", "feat_extract_activation": "gelu", "conv_dim": [512] * 7,
+    "conv_stride": [5, 2, 2, 2, 2, 2, 2], "conv_kernel": [10, 3, 3, 3, 3, 2, 2], "conv_bias": False,
+    "num_conv_pos_embeddings": 128, "num_conv_pos_embedding_groups": 16, "do_stable_layer_norm": False,
+    "feat_proj_layer_norm": True, "layer_norm_eps": 1e-5,
+}
+CV_GN_EPS = 1e-5          # HubertGroupNormConvLayer's nn.GroupNorm default
+
+
+def contentvec_config(path_or_dict=None):
+    """The engine's ContentVec shape (cv_* keys) from a Hugging Face HubertConfig config.json (None: the defaults).  Refuses, with
+    the reason, what the engine does not compute."""
+    cfg = dict(CONTENTVEC_DEFAULTS)
+    if path_or_dict is not None:
+        src = path_or_dict
+        if not isinstance(src, dict):
+            with open(path_or_dict) as f:
+                src = json.load(f)
+        cfg.update({k: src[k] for k in CONTENTVEC_DEFAULTS if k in src})
+    if cfg["feat_extract_norm"] != "group":
+        raise ValueError("feat_extract_norm %r: only 'group' (GroupNorm after the first conv) is supported" % cfg["feat_extract_norm"])
+    if cfg["do_stable_layer_norm"]:
+        raise ValueError("do_stable_layer_norm=true (pre-LN transformer) is not supported: ContentVec is post-LN")
+    if cfg["conv_bias"]:
+        raise ValueError("conv_bias=true is not supported: ContentVec's feature encoder has no conv bias")
+    if not cfg["feat_proj_layer_norm"]:
+        raise ValueError("feat_proj_layer_norm=false is not supported")
+    for k in ("hidden_act", "feat_extract_activation"):
+        if cfg[k] != "gelu":
+            raise ValueError("%s %r: only 'gelu' is supported" % (k, cfg[k]))
+    dims, ks, ss = list(cfg["conv_dim"]), list(cfg["conv_kernel"]), list(cfg["conv_stride"])
+    if not (2 <= len(dims) <= 8 and len(ks) == len(dims) == len(ss)) or len(set(dims)) != 1 or dims[0] % 16 or dims[0] > 1024:
+        raise ValueError("the feature encoder needs 2..8 convs of one width, a multiple of 16 up to 1024")
+    if any(s != 2 for s in ss[1:]):
+        raise ValueError("conv strides after the first must be 2 (got %s)" % ss[1:])
+    if not 1 <= ks[0] <= 16:
+        raise ValueError("the first conv's kernel must be 1..16")
+    H, nh = cfg["hidden_size"], cfg["num_attention_heads"]
+    if H % nh or (H // nh) % 32 or H // nh > 128 or H > 1024:
+        raise ValueError("head dim %s is not one the attention kernels take (a multiple of 32 up to 128)" % (H / nh))
+    pk, pg = cfg["num_conv_pos_embeddings"], cfg["num_conv_pos_embedding_groups"]
+    if pk % 2:
+        raise ValueError("num_conv_pos_embeddings must be even (got %d)" % pk)
+    if pk > 130 or H % pg or (H // pg) % 16:
+        raise ValueError("positional conv of %d taps in %d groups is not supported (up to 130 taps, groups a multiple of 16 wide)" % (pk, pg))
+    return {"cv_layers": cfg["num_hidden_layers"], "cv_hidden": H, "cv_heads": nh, "cv_ffn": cfg["intermediate_size"],
+            "cv_conv_dim": dims[0], "cv_conv_kernel": ks, "cv_conv_stride": ss, "cv_pos_k": pk, "cv_pos_groups": pg,
+            "cv_ln_eps": float(cfg["layer_norm_eps"]), "cv_gn_eps": CV_GN_EPS}
+
+
+def contentvec_frames(n_samples, cv=None):
+    """Frames ContentVec gives a clip of n_samples (0: too short): L0 = (n - k0) // s0 + 1, then L_i = (L_{i-1} - k_i) // s_i + 1."""
+    cv = cv or contentvec_config()
+    L = None
+    for k, s in zip(cv["cv_conv_kernel"], cv["cv_conv_stride"]):
+        n = n_samples if L is None else L
+        L = (n - k) // s + 1 if n >= k else 0
+    return max(L, 0)

@@ -28,6 +28,7 @@
 #include "attn_tc.cuh"
 #include "vc.cuh"
 #include "spk.cuh"
+#include "contentvec.cuh"
 
 using namespace vtts;
 
@@ -627,7 +628,26 @@ struct vtts_engine {
   Buf<char> h_pin_qv;
   struct QvPin { int *frm_len, *frm_off, *ident; float *prm, *units, *g, *eps; };
   QvPin qv_layout(bool eps);
-  void quickvc_enqueue(bool eps);
+  void quickvc_enqueue(bool eps, bool from_wav = false);
+
+  // ---- ContentVec (HubertModel of vc/contentvec.py; contentvec.cuh): waveform -> content-unit rows, fp32 FFMA in every mode
+  bool has_cv = false;
+  const float *cv_w0 = nullptr, *cv_gn_g = nullptr, *cv_gn_b = nullptr, *cv_fp_g = nullptr, *cv_fp_b = nullptr;
+  const float *cv_enc_g = nullptr, *cv_enc_b = nullptr, *cv_pos_w = nullptr, *cv_pos_b = nullptr;
+  ConvW cv_conv[8], cv_fp;                         // layers 1.. of the feature encoder: k taps of stride s as one 1x1 conv
+  TcW cv_tfp;
+  std::vector<EncLayerW> cv_enc;                   // relk / relv point at zeros: the attention's relative terms vanish
+  int cv_P = 1;                                    // product of the strides after layer 0
+  bool cv_tc = false;                              // precision modes >= 1: the transformer's GEMMs and attention on wgmma
+  // shape of the current call: maxS the sample bucket, tot0 the layer-0 rows (a multiple of cv_P), MC GroupNorm chunks per
+  // clip, maxL the longest clip of every level (from maxS), nint the int table [lens NL][offs NL][woff][sample mean, float bits] x B
+  struct CvPlan { int maxS = 0, tot0 = 0, MC = 0, nint = 0; std::vector<int> maxL; std::vector<int> h; } cvp;
+  Buf<int> d_cvi;
+  Buf<float> d_cvzero, d_cvwav, d_cvps, d_cvpq, d_cvl[2], d_cvx, d_cvx1, d_cvy, d_cvqkv, d_cvao, d_cvff, d_cvu, d_cvdbg;
+  Buf<char> h_pin_cv;
+  void bind_contentvec();
+  std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
+  void cv_enqueue(float* out, const int* out_offs);
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
   Buf<float> d_ncent, d_ncent_dbg, d_ascore;       // neg_cent [B][maxFrm][maxTok] (MAS accumulates in place), scores [B]
@@ -2560,6 +2580,278 @@ void vtts_engine::bind_quickvc() {
     bind_wn_encoder("encp", QV_UNITS);
     istft_w2 = vec("dec.w2", (size_t)c.istft_n_fft);
   }
+  bind_contentvec();
+}
+
+void vtts_engine::bind_contentvec() {
+  const vtts_config& c = cfg;
+  has_cv = c.cv_layers > 0 && tensors.count("cv.c0.w") > 0;
+  if (!has_cv) return;
+  const int NL = c.cv_n_conv, C = c.cv_conv_dim, H = c.cv_hidden, Fh = c.cv_ffn, G = c.cv_pos_groups;
+  REQUIRE(NL >= 2 && NL <= 8 && C % CV_CK == 0 && C <= 32 * CVL_MAXV && c.cv_conv_kernel[0] >= 1 && c.cv_conv_kernel[0] <= CVG_KMAX &&
+              c.cv_conv_stride[0] >= 1,
+          VTTS_ERR_INVALID, "unsupported ContentVec feature encoder (2..8 convs, width a multiple of 16 up to 1024, layer 0 up to 16 taps)");
+  cv_P = 1;
+  for (int i = 1; i < NL; ++i) {
+    REQUIRE(c.cv_conv_kernel[i] >= 1 && c.cv_conv_stride[i] >= 1, VTTS_ERR_INVALID, "bad ContentVec conv kernel / stride");
+    cv_P *= c.cv_conv_stride[i];
+  }
+  REQUIRE(cv_P <= 4096, VTTS_ERR_INVALID, "ContentVec strides too large");
+  REQUIRE(H % c.cv_heads == 0 && (H / c.cv_heads) % 32 == 0 && H / c.cv_heads <= 128 && H <= 32 * CVL_MAXV && Fh % CV_CK == 0,
+          VTTS_ERR_INVALID, "unsupported ContentVec transformer (head width a multiple of 32 up to 128, width up to 1024)");
+  REQUIRE(G >= 1 && H % G == 0 && (H / G) % CV_CK == 0 && c.cv_pos_k % 2 == 0 && CV_TT + c.cv_pos_k / 2 - 1 <= 32 * CV_XR, VTTS_ERR_INVALID,
+          "unsupported ContentVec positional conv (even kernel up to 130, group width a multiple of 16)");
+  const int K0 = c.cv_conv_kernel[0], kh = c.cv_pos_k / 2, Cg = H / G;
+  cv_w0 = vec("cv.c0.w", (size_t)C * K0);
+  cv_gn_g = vec("cv.gn.g", C);
+  cv_gn_b = vec("cv.gn.b", C);
+  for (int i = 1; i < NL; ++i) cv_conv[i] = conv("cv.c" + std::to_string(i), c.cv_conv_kernel[i] * C, C, 1);
+  cv_fp_g = vec("cv.fp.ln.g", C);
+  cv_fp_b = vec("cv.fp.ln.b", C);
+  cv_fp = conv("cv.fp", C, H, 1);
+  cv_pos_w = vec("cv.pos.w", (size_t)2 * G * kh * Cg * Cg);
+  cv_pos_b = vec("cv.pos.b", H);
+  cv_enc_g = vec("cv.enc.ln.g", H);
+  cv_enc_b = vec("cv.enc.ln.b", H);
+  // zeros: the bias of the positional conv's second half, the relative tables (fp32, and the [16][128] bf16 tiles of the
+  // tensor-core attention)
+  const size_t nz = std::max<size_t>({(size_t)H, (size_t)(2 * c.window_size + 1) * (H / c.cv_heads), (size_t)ATC_RELP * 128});
+  float* zero = ensure(d_cvzero, nz);
+  CK(cudaMemsetAsync(zero, 0, d_cvzero.cap * sizeof(float), stream));
+  cv_tc = c.precision >= 1 && c.precision <= 3;
+  if (cv_tc) {
+    REQUIRE(C % TC_BK == 0 && H % TC_BK == 0 && Fh % TC_BK == 0 && 2 * c.window_size + 1 <= ATC_RELP, VTTS_ERR_INVALID,
+            "ContentVec on the tensor cores needs widths in multiples of 64");
+    REQUIRE(tensors.count("cv.fp.th") > 0, VTTS_ERR_WEIGHTS, "the blob lacks ContentVec's tensor-core weights (packed with precision 0)");
+    cv_tfp = tcw("cv.fp", C, H, 1);
+  }
+  cv_enc.clear();
+  for (int l = 0; l < c.cv_layers; ++l) {
+    const std::string p = "cv.l" + std::to_string(l);
+    EncLayerW L;
+    L.heads = c.cv_heads;
+    L.qkv = conv(p + ".qkv", H, 3 * H, 1);
+    L.o = conv(p + ".o", H, H, 1);
+    L.ln1 = ln(p + ".ln1", H);
+    L.ffn1 = conv(p + ".ffn1", H, Fh, 1);
+    L.ffn2 = conv(p + ".ffn2", Fh, H, 1);
+    L.ln2 = ln(p + ".ln2", H);
+    L.relk = L.relv = zero;
+    if (cv_tc) {
+      L.t_qkv = tcw(p + ".qkv", H, 3 * H, 1);
+      L.t_o = tcw(p + ".o", H, H, 1);
+      L.t_ffn1 = tcw(p + ".ffn1", H, Fh, 1);
+      L.t_ffn2 = tcw(p + ".ffn2", Fh, H, 1);
+      const __nv_bfloat16* zb = reinterpret_cast<const __nv_bfloat16*>(zero);
+      L.rk_hi = L.rk_lo = L.rv_hi = L.rv_lo = zb;
+    }
+    cv_enc.push_back(L);
+  }
+}
+
+// Host side of a ContentVec call: every level's lengths and offsets follow from the sample counts, so nothing waits for the
+// device.  Clip b's layer-0 rows start at a multiple of cv_P (so every later level's offset is an exact division) and its
+// samples are staged at s0 times that row.  Returns each clip's frame count.
+std::vector<int> vtts_engine::cv_stage(const float* wav, const int64_t* lengths, int64_t ld) {
+  const vtts_config& c = cfg;
+  const int NL = c.cv_n_conv, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
+  auto levels = [&](int64_t n, int* L) {
+    L[0] = n >= K0 ? (int)((n - K0) / s0 + 1) : 0;
+    for (int i = 1; i < NL; ++i) L[i] = L[i - 1] >= c.cv_conv_kernel[i] ? (L[i - 1] - c.cv_conv_kernel[i]) / c.cv_conv_stride[i] + 1 : 0;
+  };
+  const int halo = (K0 + s0 - 1) / s0;               // rows of samples past the last frame's window
+  auto padded = [&](int L0) { return (L0 + halo + cv_P - 1) / cv_P * cv_P; };
+  int64_t mx = 0;
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lengths[b] >= 1 && lengths[b] <= ld, VTTS_ERR_INVALID, "wav_lengths must be in [1, wav_ld]");
+    int L[8];
+    levels(lengths[b], L);
+    REQUIRE(L[NL - 1] >= 1, VTTS_ERR_INVALID, "a clip is too short for one ContentVec frame (400 samples at the published shape)");
+    REQUIRE(lengths[b] <= (int64_t)1 << 30, VTTS_ERR_INVALID, "clip too long");
+    mx = std::max(mx, lengths[b]);
+  }
+  cvp.maxS = use_buckets ? (int)((mx + 7999) / 8000 * 8000) : (int)mx;
+  cvp.maxL.assign(NL, 0);
+  levels(cvp.maxS, cvp.maxL.data());
+  cvp.MC = (cvp.maxL[0] + CVG_CH - 1) / CVG_CH;
+  cvp.nint = (2 * NL + 2) * B;
+  std::vector<int>& h = cvp.h;
+  h.assign(cvp.nint, 0);
+  std::vector<int> frames(B);
+  int64_t total0 = 0;                                // layer-0 rows of the batch: every offset (and s0 times it) must fit an int
+  for (int b = 0; b < B; ++b) {
+    int L[8];
+    levels(lengths[b], L);
+    total0 += padded(L[0]);
+  }
+  REQUIRE((total0 + 65535) * s0 + K0 <= (int64_t)INT32_MAX, VTTS_ERR_INVALID, "the batch holds too many samples for one call");
+  int off0 = 0;
+  for (int b = 0; b < B; ++b) {
+    int L[8];
+    levels(lengths[b], L);
+    int div = 1;
+    for (int i = 0; i < NL; ++i) {
+      if (i) div *= c.cv_conv_stride[i];
+      h[i * B + b] = L[i];
+      h[(NL + i) * B + b] = off0 / div;
+    }
+    h[2 * NL * B + b] = off0 * s0;
+    frames[b] = L[NL - 1];
+    off0 += padded(L[0]);
+  }
+  cvp.tot0 = (B == 1 || !use_buckets) ? std::max(off0, use_buckets ? padded(cvp.maxL[0]) : 0) : (off0 + 65535) / 65536 * 65536;
+  const size_t head = ((size_t)cvp.nint * sizeof(int) + 63) / 64 * 64;
+  const size_t nsamp = (size_t)cvp.tot0 * s0 + K0;
+  char* pin = ensure_pinned(h_pin_cv, head + nsamp * sizeof(float) + 64);
+  memcpy(pin, h.data(), (size_t)(2 * NL + 1) * B * sizeof(int));
+  float* ps = reinterpret_cast<float*>(pin + head);
+  for (int b = 0; b < B; ++b) {
+    const int L0 = h[b];
+    const int64_t need = std::min<int64_t>(lengths[b], (int64_t)(L0 - 1) * s0 + K0);
+    const float* src = wav + (size_t)b * ld;
+    memcpy(ps + h[2 * NL * B + b], src, (size_t)need * sizeof(float));
+    double sum = 0.0;                                  // the clip's mean, in one fixed order (layer 0 runs centred on it)
+    for (int64_t i = 0; i < lengths[b]; ++i) sum += src[i];
+    const float mu = (float)(sum / (double)lengths[b]);
+    memcpy(pin + ((2 * NL + 1) * B + b) * sizeof(int), &mu, sizeof(float));
+  }
+  return frames;
+}
+
+// ContentVec of the staged clips (cv_stage): layer 0 + GroupNorm + GELU, layers 1.. (conv_kernel over the strided row view,
+// GELU epilogue), LayerNorm + projection, the grouped positional conv (two launches of half the taps each: the tile halo of
+// conv_kernel), LayerNorm(x + gelu(pos)), then the post-LN transformer layers.  The last LayerNorm writes frame t of clip b
+// to out row out_offs[b] + t (out_offs null: the frame level's own offsets).
+void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
+  const vtts_config& c = cfg;
+  const int NL = c.cv_n_conv, C = c.cv_conv_dim, H = c.cv_hidden, Fh = c.cv_ffn, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
+  // The tensor-core GEMMs run without split-K (every output summed by one CTA in one k order, whatever its launch shape) and
+  // attention on attn_tc_kernel whenever it takes the layer: a clip's units are then the same alone and in any batch.
+  struct Saved {
+    vtts_engine* e; std::vector<int> vf, hf; int split, atc;
+    explicit Saved(vtts_engine* h) : e(h), vf(h->v_frm_len), hf(h->h_frm_len), split(h->tc_split), atc(h->attn_tc_mode) {}
+    ~Saved() { e->v_frm_len = vf; e->h_frm_len = hf; e->tc_split = split; e->attn_tc_mode = atc; }
+  } saved(this);
+  if (cv_tc) {
+    tc_split = 1;
+    if (attn_tc_mode > 0) attn_tc_mode = 2;
+  }
+  const size_t head = ((size_t)cvp.nint * sizeof(int) + 63) / 64 * 64;
+  const size_t nsamp = (size_t)cvp.tot0 * s0 + K0;
+  int* di = ensure(d_cvi, cvp.nint);
+  float* dw = ensure(d_cvwav, nsamp);
+  CK(cudaMemcpyAsync(di, h_pin_cv.p, cvp.nint * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(dw, h_pin_cv.p + head, nsamp * sizeof(float), cudaMemcpyHostToDevice, stream));
+  auto Ls = [&](int l) -> const int* { return di + l * B; };
+  auto Os = [&](int l) -> const int* { return di + (NL + l) * B; };
+  const int* woff = di + 2 * NL * B;
+  const float* mu = reinterpret_cast<const float*>(di + (2 * NL + 1) * B);
+  const size_t np = (size_t)B * cvp.MC * C;
+  float* ps = ensure(d_cvps, np);
+  float* pq = ensure(d_cvpq, np);
+  float* lv[2] = {ensure(d_cvl[0], (size_t)cvp.tot0 * C), ensure(d_cvl[1], (size_t)cvp.tot0 / c.cv_conv_stride[1] * C)};
+  const dim3 gg(cvp.MC, B), gb(CVG_THREADS);
+  const size_t gsm = (size_t)((CVG_CH - 1) * s0 + K0) * sizeof(float);
+  klaunch(cv_gn_kernel<0>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
+  CK(cudaGetLastError());
+  klaunch(cv_gn_kernel<1>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
+  CK(cudaGetLastError());
+  klaunch(cv_gn_kernel<2>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
+  CK(cudaGetLastError());
+  launches += 3;
+  auto gelu = [&](float* y, int width, const int* lens, const int* offs, int maxLen, const Planes* pl) {
+    klaunch(cv_gelu_kernel, dim3(maxLen, B), dim3(256), (size_t)0, y, width, lens, offs, pl ? pl->hi : (__nv_bfloat16*)nullptr,
+            pl ? pl->lo : (__nv_bfloat16*)nullptr);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  float* x = lv[0];
+  for (int i = 1; i < NL; ++i) {
+    float* y = lv[i & 1];
+    v_frm_len.assign(B, cvp.maxL[i]);
+    h_frm_len = v_frm_len;
+    launch_conv({mk(cv_conv[i], x, c.cv_conv_stride[i] * C, 0, y, C, 0, 1, 0)}, 1, Ls(i), Os(i), cvp.maxL[i], B);
+    gelu(y, C, Ls(i), Os(i), cvp.maxL[i], nullptr);
+    x = y;
+  }
+  const int* Lf = Ls(NL - 1);
+  const int* Of = Os(NL - 1);
+  const int maxF = cvp.maxL[NL - 1];
+  const size_t Tf = (size_t)cvp.tot0 / cv_P;
+  float *X = ensure(d_cvx, Tf * H), *X1 = ensure(d_cvx1, Tf * H), *Y = ensure(d_cvy, Tf * H), *QKV = ensure(d_cvqkv, Tf * 3 * H);
+  float *AO = ensure(d_cvao, Tf * std::max(H, C)), *FF = ensure(d_cvff, Tf * Fh);
+  const dim3 lg((maxF + CVL_WARPS - 1) / CVL_WARPS, B), lb(32 * CVL_WARPS);
+  // precision modes >= 1: the projection and the transformer's qkv / out / FFN convs on conv_tc_kernel, attention on
+  // attn_tc_kernel; every producer of a GEMM operand also writes its split-bf16 planes.  All of
+  // them are 1x1, and the attention masks keys past a clip, so no plane row behind a clip is read (no tail zeroing).
+  Planes PX, P512, PQKV, PAO, PX1, PFF;
+  if (cv_tc) {
+    P512 = planes(50, (long)Tf, 1, C); PX = planes(51, (long)Tf, 1, H); PQKV = planes(52, (long)Tf, 1, 3 * H);
+    PAO = planes(53, (long)Tf, 1, H); PX1 = planes(54, (long)Tf, 1, H); PFF = planes(55, (long)Tf, 1, Fh);
+  }
+  auto ln = [&](const float* a, const float* yy, const float* g, const float* bt, float* o, const int* oo, int width, const Planes* pl) {
+    klaunch(cv_ln_kernel, lg, lb, (size_t)0, a, yy, g, bt, c.cv_ln_eps, o, Lf, Of, oo, width, pl ? pl->hi : (__nv_bfloat16*)nullptr,
+            pl ? pl->lo : (__nv_bfloat16*)nullptr);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  auto gemm = [&](const Planes& in, const TcW& w, const ConvW& cw, float* y, const float* res, const Planes* out, int epi) {
+    TcSpec s;
+    s.in = in; s.w = w; s.bias = cw.b; s.Cin = cw.Cin; s.Cout = cw.Cout;
+    s.y = y; s.ldy = cw.Cout; s.res = res; s.ldr = res ? cw.Cout : 0; s.epi = epi;
+    if (out) s.out = *out;
+    launch_tc({s}, 1, Lf, Of, maxF, B);
+  };
+  ln(x, nullptr, cv_fp_g, cv_fp_b, AO, Of, C, cv_tc ? &P512 : nullptr);
+  if (cv_tc) gemm(P512, cv_tfp, cv_fp, X, nullptr, nullptr, 0);
+  else launch_conv({mk(cv_fp, AO, C, 0, X, H, 0, 1, 0)}, 1, Lf, Of, maxF, B);
+  const int G = c.cv_pos_groups, Cg = H / G, kh = c.cv_pos_k / 2;
+  for (int half = 0; half < 2; ++half)
+    for (int g0 = 0; g0 < G; g0 += CV_MAXP) {
+      std::vector<ConvP> pp;
+      for (int g = g0; g < std::min(G, g0 + CV_MAXP); ++g) {
+        ConvW W;
+        W.w = cv_pos_w + (size_t)(half * G + g) * kh * Cg * Cg;
+        W.b = half ? d_cvzero.p : cv_pos_b + (size_t)g * Cg;
+        W.Cin = Cg; W.Cout = Cg; W.k = kh; W.ldw = Cg;
+        ConvP p = mk(W, X, H, g * Cg, Y, H, g * Cg, 1, half ? c.cv_pos_k / 2 - kh : c.cv_pos_k / 2);
+        if (half) { p.res = Y; p.ldr = H; p.roff = g * Cg; }
+        pp.push_back(p);
+      }
+      launch_conv(pp, 1, Lf, Of, maxF, B);
+    }
+  ln(X, Y, cv_enc_g, cv_enc_b, X1, Of, H, cv_tc ? &PX : nullptr);
+  if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_cvdbg, Tf * H), X1, Tf * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  float *xa = X1, *xb = X;
+  for (size_t l = 0; l < cv_enc.size() && cv_tc; ++l) {
+    const EncLayerW& Lw = cv_enc[l];
+    gemm(PX, Lw.t_qkv, Lw.qkv, QKV, nullptr, &PQKV, 0);
+    if (attn_use_tc(Lw, H, Lf, maxF)) launch_attn_tc(PQKV, AO, &PAO, Lw, H, Lf, Of, maxF);
+    else launch_attn(QKV, AO, Lw, H, Lf, Of, maxF, &PAO);
+    gemm(PAO, Lw.t_o, Lw.o, Y, xa, nullptr, 0);
+    ln(Y, nullptr, Lw.ln1.g, Lw.ln1.b, xb, Of, H, &PX1);
+    gemm(PX1, Lw.t_ffn1, Lw.ffn1, FF, nullptr, nullptr, 0);
+    gelu(FF, Fh, Lf, Of, maxF, &PFF);
+    gemm(PFF, Lw.t_ffn2, Lw.ffn2, Y, xb, nullptr, 0);
+    if (l + 1 == cv_enc.size()) ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, out, out_offs ? out_offs : Of, H, nullptr);
+    else ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, xa, Of, H, &PX);
+  }
+  for (size_t l = 0; l < cv_enc.size() && !cv_tc; ++l) {
+    const EncLayerW& Lw = cv_enc[l];
+    launch_conv({mk(Lw.qkv, xa, H, 0, QKV, 3 * H, 0, 1, 0)}, 1, Lf, Of, maxF, B);
+    launch_attn(QKV, AO, Lw, H, Lf, Of, maxF, nullptr);
+    ConvP po = mk(Lw.o, AO, H, 0, Y, H, 0, 1, 0);
+    po.res = xa; po.ldr = H;
+    launch_conv({po}, 1, Lf, Of, maxF, B);
+    ln(Y, nullptr, Lw.ln1.g, Lw.ln1.b, xb, Of, H, nullptr);
+    launch_conv({mk(Lw.ffn1, xb, H, 0, FF, Fh, 0, 1, 0)}, 1, Lf, Of, maxF, B);
+    gelu(FF, Fh, Lf, Of, maxF, nullptr);
+    ConvP p2 = mk(Lw.ffn2, FF, Fh, 0, Y, H, 0, 1, 0);
+    p2.res = xb; p2.ldr = H;
+    launch_conv({p2}, 1, Lf, Of, maxF, B);
+    if (l + 1 == cv_enc.size()) ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, out, out_offs ? out_offs : Of, H, nullptr);
+    else ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, xa, Of, H, nullptr);
+  }
 }
 
 // Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
@@ -2636,7 +2928,7 @@ vtts_engine::QvPin vtts_engine::qv_layout(bool eps) {
   return pp;
 }
 
-void vtts_engine::quickvc_enqueue(bool eps) {
+void vtts_engine::quickvc_enqueue(bool eps, bool from_wav) {
   const vtts_config& c = cfg;
   const int I = c.inter_channels, G = c.gin_channels;
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
@@ -2651,7 +2943,12 @@ void vtts_engine::quickvc_enqueue(bool eps) {
   CK(cudaMemcpyAsync(fo, pp.frm_off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(ident, pp.ident, B * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(prm, pp.prm, 16 * sizeof(float), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(units, pp.units, (size_t)Tfrm * QV_UNITS * sizeof(float), cudaMemcpyHostToDevice, stream));
+  if (from_wav) {      // ContentVec writes the unit rows; the gaps between clips and the bucket's tail stay zero
+    CK(cudaMemsetAsync(units, 0, (size_t)Tfrm * QV_UNITS * sizeof(float), stream));
+    cv_enqueue(units, fo);
+  } else {
+    CK(cudaMemcpyAsync(units, pp.units, (size_t)Tfrm * QV_UNITS * sizeof(float), cudaMemcpyHostToDevice, stream));
+  }
   CK(cudaMemcpyAsync(g, pp.g, (size_t)B * G * sizeof(float), cudaMemcpyHostToDevice, stream));
   float* noise = nullptr;
   if (eps) {
@@ -3152,19 +3449,57 @@ static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const 
 }
 
 // QuickVC conversion through host buffers (vtts_quickvc_convert).
-static void impl_quickvc_convert(vtts_handle h, const float* units, const int64_t* lengths, int B, int64_t units_ld, const float* g,
-                                 float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
-                                 int64_t* out_frames) {
+static void require_contentvec(vtts_handle h, int B) {
+  REQUIRE(h->has_cv, VTTS_ERR_INVALID, "the weight blob has no ContentVec (cv.*): pack it with weights.pack_quickvc(..., contentvec=...)");
+  REQUIRE(B >= 1 && B <= 16384, VTTS_ERR_INVALID, "bad batch size");
+}
+
+// ContentVec units through host buffers (vtts_content_units).
+static void impl_content_units(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t wav_ld, float* units,
+                               int64_t units_ld, int64_t* out_frames) {
+  require_contentvec(h, B);
+  REQUIRE(wav_ld >= 1, VTTS_ERR_INVALID, "bad wav_ld");
+  h->B = B;
+  const std::vector<int> frames = h->cv_stage(wav, lengths, wav_ld);
+  for (int b = 0; b < B; ++b) REQUIRE(frames[b] <= units_ld, VTTS_ERR_CAPACITY, "units_ld is smaller than a clip's frame count");
+  const int H = h->cfg.cv_hidden, NL = h->cfg.cv_n_conv;
+  const size_t Tf = (size_t)h->cvp.tot0 / h->cv_P;
+  h->run_graphed({0xC7, B, h->cvp.maxS, h->cvp.tot0}, [&] { h->cv_enqueue(h->ensure(h->d_cvu, Tf * H), nullptr); });
+  float* pu = reinterpret_cast<float*>(h->ensure_pinned(Tf * H * sizeof(float) + 64));
+  CK(cudaMemcpyAsync(pu, h->d_cvu.p, Tf * H * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; ++b) {
+    const size_t n = (size_t)frames[b] * H;
+    float* dst = units + (size_t)b * units_ld * H;
+    memcpy(dst, pu + (size_t)h->cvp.h[(NL + NL - 1) * B + b] * H, n * sizeof(float));
+    std::fill(dst + n, dst + (size_t)units_ld * H, 0.f);
+    out_frames[b] = frames[b];
+  }
+}
+
+// QuickVC conversion through host buffers: from content units (vtts_quickvc_convert, wav null) or from source waveforms through
+// ContentVec (vtts_quickvc_convert_wav, units null; in_ld is then wav_ld).
+static void impl_quickvc_convert(vtts_handle h, const float* units, const float* wav, const int64_t* lengths, int B, int64_t in_ld,
+                                 const float* g, float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav,
+                                 int64_t out_ld, int64_t* out_frames) {
   const vtts_config& c = h->cfg;
+  const int64_t units_ld = in_ld;
   REQUIRE(h->has_encp, VTTS_ERR_INVALID, "the weight blob holds only the speaker encoder: conversion needs a model packed by "
           "weights.pack_quickvc from a whole QuickVC checkpoint (enc_p, flow, dec)");
+  if (wav) require_contentvec(h, B);
   REQUIRE(B >= 1 && B <= 16384, VTTS_ERR_INVALID, "bad batch size");
-  REQUIRE(units_ld >= 1 && units_ld < (1LL << 24), VTTS_ERR_INVALID, "bad units_ld");
+  REQUIRE(in_ld >= 1 && (wav || units_ld < (1LL << 24)), VTTS_ERR_INVALID, wav ? "bad wav_ld" : "bad units_ld");
   REQUIRE(g != nullptr, VTTS_ERR_INVALID, "g (the target's speaker embedding, vtts_speaker_embedding) is required");
   std::vector<int> frames(B);
-  for (int b = 0; b < B; ++b) {
-    REQUIRE(lengths[b] >= 1 && lengths[b] <= units_ld, VTTS_ERR_INVALID, "unit_lengths must be in [1, units_ld]");
-    frames[b] = (int)lengths[b];
+  if (wav) {
+    REQUIRE(c.cv_hidden == vtts_engine::QV_UNITS, VTTS_ERR_INVALID, "ContentVec's width differs from enc_p's unit channels");
+    h->B = B;
+    frames = h->cv_stage(wav, lengths, in_ld);
+  } else {
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(lengths[b] >= 1 && lengths[b] <= units_ld, VTTS_ERR_INVALID, "unit_lengths must be in [1, units_ld]");
+      frames[b] = (int)lengths[b];
+    }
   }
   const int real_max = *std::max_element(frames.begin(), frames.end());
   REQUIRE((int64_t)real_max * h->hop <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than hop * max(unit_lengths)");
@@ -3185,10 +3520,12 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const int64_
   for (int b = 0; b < B; ++b) {
     pp.ident[b] = b;
     const int o = h->h_frm_off[b];
+    if (units) {
     memcpy(pp.units + (size_t)o * vtts_engine::QV_UNITS, units + (size_t)b * units_ld * vtts_engine::QV_UNITS,
            (size_t)frames[b] * vtts_engine::QV_UNITS * sizeof(float));
     const int gap_end = b + 1 < B ? h->h_frm_off[b + 1] : h->Tfrm;       // rows behind the clip: the gap, or the bucket's tail
     memset(pp.units + (size_t)(o + frames[b]) * vtts_engine::QV_UNITS, 0, (size_t)(gap_end - o - frames[b]) * vtts_engine::QV_UNITS * sizeof(float));
+    }
     memcpy(pp.g + (size_t)b * G, g + (size_t)b * G, G * sizeof(float));
     if (noise)
       for (int ch = 0; ch < I; ++ch)
@@ -3199,7 +3536,10 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const int64_
   const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
   memcpy(&pp.prm[4], &lo, 4);
   memcpy(&pp.prm[5], &hi, 4);
-  h->run_graphed({0x77, B, h->maxFrm, h->Tfrm, noise ? 1 : 0}, [&] { h->quickvc_enqueue(noise != nullptr); });
+  if (wav)
+    h->run_graphed({0x78, B, h->maxFrm, h->Tfrm, noise ? 1 : 0, h->cvp.maxS, h->cvp.tot0}, [&] { h->quickvc_enqueue(noise != nullptr, true); });
+  else
+    h->run_graphed({0x77, B, h->maxFrm, h->Tfrm, noise ? 1 : 0}, [&] { h->quickvc_enqueue(noise != nullptr); });
   const size_t nw = (size_t)h->real_Tfrm * h->hop;
   float* pw = reinterpret_cast<float*>(h->ensure_pinned((size_t)h->Tfrm * h->hop * sizeof(float) + 64));
   CK(cudaMemcpyAsync(pw, h->d_wav.p, nw * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
@@ -3360,14 +3700,17 @@ void vtts_destroy(vtts_handle h) {
                       &h->d_fao, &h->d_fy, &h->d_ffh2, &h->d_eps_z, &h->d_d0, &h->d_post, &h->d_wav};
   for (auto* b : fb) fr(b->p);
   Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg,
-                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg, &h->d_units, &h->d_qg};
+                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg, &h->d_units, &h->d_qg,
+                      &h->d_cvzero, &h->d_cvwav, &h->d_cvps, &h->d_cvpq, &h->d_cvl[0], &h->d_cvl[1], &h->d_cvx, &h->d_cvx1, &h->d_cvy,
+                      &h->d_cvqkv, &h->d_cvao, &h->d_cvff, &h->d_cvu, &h->d_cvdbg};
   for (auto* b : vb) fr(b->p);
   fr(h->d_vint.p);
   fr(h->d_sseq.p);
+  fr(h->d_cvi.p);
   for (auto& b : h->d_stage) fr(b.p);
   for (auto& v : h->d_xj) for (auto& b : v) fr(b.p);
   for (auto& v : h->d_tmp) for (auto& b : v) fr(b.p);
-  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc, &h->h_pin_qv}) if (hb->p) cudaFreeHost(hb->p);
+  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc, &h->h_pin_qv, &h->h_pin_cv}) if (hb->p) cudaFreeHost(hb->p);
   for (auto& kv : h->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   fr(h->d_prm.p);
   fr(h->d_pref.p);
@@ -3686,6 +4029,10 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "spk_x1" || nm == "spk_x2") { src = h->d_sx[nm[5] - '0'].p; n = (size_t)h->spk_rows * SPK_GATES; }
     else if (nm == "spk_h0" || nm == "spk_h1" || nm == "spk_h2") { src = h->d_sh[nm[5] - '0'].p; n = (size_t)h->spk_rows * SPK_H; }
     else if (nm == "spk_g") { src = h->d_sg.p; n = (size_t)h->B * SPK_H; }
+    else if (nm == "cv_feat") { src = h->d_cvl[(c.cv_n_conv - 1) & 1].p; n = (size_t)h->cvp.tot0 / h->cv_P * c.cv_conv_dim; }
+    else if (nm == "cv_gn_sum") { src = h->d_cvps.p; n = (size_t)h->B * h->cvp.MC * c.cv_conv_dim; }
+    else if (nm == "cv_gn_sq") { src = h->d_cvpq.p; n = (size_t)h->B * h->cvp.MC * c.cv_conv_dim; }
+    else if (nm == "cv_enc_in") { src = h->d_cvdbg.p; n = (size_t)h->cvp.tot0 / h->cv_P * c.cv_hidden; }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);
       REQUIRE(i >= 0 && i < (int)h->d_stage.size(), VTTS_ERR_INVALID, "no such stage");
@@ -3715,8 +4062,22 @@ int vtts_quickvc_convert(vtts_handle h, const float* units, const int64_t* unit_
                          float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
                          int64_t* out_frames) {
   if (!units || !unit_lengths || !out_wav || !out_frames) return VTTS_ERR_INVALID;
-  return guarded(h, [&] { impl_quickvc_convert(h, units, unit_lengths, B, units_ld, g, noise_scale, noise, noise_ld, seed, out_wav, out_ld,
-                                               out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+  return guarded(h, [&] { impl_quickvc_convert(h, units, nullptr, unit_lengths, B, units_ld, g, noise_scale, noise, noise_ld, seed, out_wav,
+                                               out_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_content_units(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, float* units,
+                       int64_t units_ld, int64_t* out_frames) {
+  if (!wav || !wav_lengths || !units || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_content_units(h, wav, wav_lengths, B, wav_ld, units, units_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const float* g,
+                             float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
+                             int64_t* out_frames) {
+  if (!wav || !wav_lengths || !out_wav || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_quickvc_convert(h, nullptr, wav, wav_lengths, B, wav_ld, g, noise_scale, noise, noise_ld, seed, out_wav,
+                                               out_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
 }
 
 // Host copies of a debug hook's arguments on the device (freed on every exit).

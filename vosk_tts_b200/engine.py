@@ -40,6 +40,9 @@ class VttsConfig(C.Structure):
         ("filter_length", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32), ("n_mel_channels", C.c_int32),
         ("mel_fmin", C.c_float), ("mel_fmax", C.c_float),
         ("model_family", C.c_int32),
+        ("cv_layers", C.c_int32), ("cv_hidden", C.c_int32), ("cv_heads", C.c_int32), ("cv_ffn", C.c_int32),
+        ("cv_conv_dim", C.c_int32), ("cv_n_conv", C.c_int32), ("cv_conv_kernel", C.c_int32 * 8), ("cv_conv_stride", C.c_int32 * 8),
+        ("cv_pos_k", C.c_int32), ("cv_pos_groups", C.c_int32), ("cv_ln_eps", C.c_float), ("cv_gn_eps", C.c_float),
     ]
 
 
@@ -51,7 +54,8 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_decoder_halo", "vtts_flow", "vtts_decode_chunk", "vtts_debug_attention", "vtts_speculation_stats", "vtts_host_timings",
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
-           "vtts_speaker_embedding_mel", "vtts_quickvc_convert"]
+           "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
+           "vtts_quickvc_convert_wav"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1}    # vtts_config.model_family
 
@@ -223,6 +227,10 @@ def load_library(build_if_missing=True):
         fn.restype = i32
     lib.vtts_quickvc_convert.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_float, vp, i32, C.c_uint64, vp, C.c_int64, vp]
     lib.vtts_quickvc_convert.restype = i32
+    lib.vtts_content_units.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64, vp]
+    lib.vtts_content_units.restype = i32
+    lib.vtts_quickvc_convert_wav.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_float, vp, i32, C.c_uint64, vp, C.c_int64, vp]
+    lib.vtts_quickvc_convert_wav.restype = i32
     _LIB = lib
     return lib
 
@@ -283,6 +291,14 @@ def make_c_config(cfg, precision=0):
     fmax = cfg.get("mel_fmax")
     c.mel_fmax = float(cfg.get("sampling_rate", 22050)) / 2 if fmax is None else float(fmax)
     c.model_family = MODEL_FAMILIES[cfg.get("model_family", "vits2")]
+    cv = cfg.get("contentvec")
+    if cv:
+        for k in ("cv_layers", "cv_hidden", "cv_heads", "cv_ffn", "cv_conv_dim", "cv_pos_k", "cv_pos_groups"):
+            setattr(c, k, int(cv[k]))
+        c.cv_n_conv = len(cv["cv_conv_kernel"])
+        for i, (k, s) in enumerate(zip(cv["cv_conv_kernel"], cv["cv_conv_stride"])):
+            c.cv_conv_kernel[i], c.cv_conv_stride[i] = int(k), int(s)
+        c.cv_ln_eps, c.cv_gn_eps = float(cv["cv_ln_eps"]), float(cv["cv_gn_eps"])
     return c
 
 
@@ -594,6 +610,58 @@ class Engine:
         self.quickvc_convert(np.zeros((int(batch), int(max_frames), 768), np.float32), np.zeros(int(self.cfg["gin_channels"]), np.float32),
                              noise_scale=0.0)
         return int(max_frames)
+
+    # ---- ContentVec (vc/contentvec.py) and conversion from source waveforms; cfg["contentvec"] is its shape
+    @staticmethod
+    def _clips(wav, lengths):
+        if isinstance(wav, (list, tuple)):
+            clips = [np.asarray(w, np.float32).reshape(-1) for w in wav]
+            lengths = np.array([w.size for w in clips], np.int64)
+            batch = np.zeros((len(clips), int(lengths.max())), np.float32)
+            for b, w in enumerate(clips):
+                batch[b, :w.size] = w
+            wav = batch
+        wav = np.ascontiguousarray(wav, dtype=np.float32)
+        if wav.ndim == 1:
+            wav = wav[None]
+        B = wav.shape[0]
+        lengths = np.ascontiguousarray(np.full(B, wav.shape[1]) if lengths is None else lengths, dtype=np.int64).reshape(B)
+        return wav, lengths
+
+    def content_units(self, wav, lengths=None):
+        """ContentVec units of 16 kHz sources (vtts_content_units): wav [L], [B, L] with `lengths`, or a list of ragged clips.
+        Returns (units float32 [B, max T, hidden], zeros past each clip's end; frames int64 [B])."""
+        wav, lengths = self._clips(wav, lengths)
+        B = wav.shape[0]
+        T = max(1, max(_config.contentvec_frames(int(n), self.cfg.get("contentvec")) for n in lengths))
+        units = np.zeros((B, T, int((self.cfg.get("contentvec") or _config.contentvec_config())["cv_hidden"])), np.float32)
+        frames = np.zeros(B, np.int64)
+        self._check(self.lib.vtts_content_units(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], _ptr(units), T, _ptr(frames)))
+        return units, frames
+
+    def quickvc_convert_wav(self, wav, g, lengths=None, noise_scale=1.0, noise=None, seed=0):
+        """Source waveforms -> waveforms in the voice of g in one call (vtts_quickvc_convert_wav): content_units, then
+        quickvc_convert, without the units leaving the GPU.  Arguments as those two.  Returns (wav [B, hop * max T], frames)."""
+        wav, lengths = self._clips(wav, lengths)
+        B = wav.shape[0]
+        T = max(1, max(_config.contentvec_frames(int(n), self.cfg.get("contentvec")) for n in lengths))
+        G = int(self.cfg["gin_channels"])
+        g = np.ascontiguousarray(np.broadcast_to(np.asarray(g, np.float32).reshape(-1, G), (B, G)), dtype=np.float32)
+        ld = 0
+        if noise is not None:
+            noise = np.ascontiguousarray(noise, dtype=np.float32)
+            ld = noise.shape[2]
+        out = np.zeros((B, T * self.hop), np.float32)
+        frames = np.zeros(B, np.int64)
+        self._check(self.lib.vtts_quickvc_convert_wav(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], _ptr(g), float(noise_scale),
+                                                      _ptr(noise), ld, int(seed), _ptr(out), out.shape[1], _ptr(frames)))
+        return out, frames
+
+    def reserve_contentvec(self, max_samples=160000, batch=1):
+        """Workspace reservation for ContentVec calls of up to `batch` clips x `max_samples` samples (layer 0's rows at 3200 Hz
+        are the large buffers): one call of that size, so later calls within these bounds move no buffer."""
+        self.content_units(np.zeros((int(batch), int(max_samples)), np.float32))
+        return int(max_samples)
 
     # ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
     def _align(self, from_wav, ids, lengths, sid, x, x_lengths, noise_scale, noise, seed):

@@ -277,3 +277,44 @@ def make_random_quickvc(cfg, seed=1234):
     sd["dec.updown_filter"] = updown
     sd.update(make_random_speaker_encoder(cfg, seed))
     return sd
+
+
+def make_random_contentvec(seed=1234, cv=None):
+    """A ContentVec state dict (HubertModelWithFinalProj of vc/contentvec.py, CPU fp32) in the reference's names and shapes for
+    the shape cv (config.contentvec_config; default hubert-base).  The positional conv is weight-normed as the published
+    checkpoint stores it (weight_g [1, 1, K] / weight_v, dim=2).  Biases and the LayerNorm / GroupNorm affines are non-trivial;
+    final_proj and masked_spec_embed, which inference never reads, are there as in a real checkpoint."""
+    from . import config as _config
+    cv = cv or _config.contentvec_config()
+    C, H, Fh, K, G = cv["cv_conv_dim"], cv["cv_hidden"], cv["cv_ffn"], cv["cv_pos_k"], cv["cv_pos_groups"]
+    out = []
+    ln = lambda name, c: out.extend([(name + ".weight", (c,), "gamma", 0.1), (name + ".bias", (c,), "normal", 0.1)])
+    fe = "feature_extractor.conv_layers.%d."
+    for i, k in enumerate(cv["cv_conv_kernel"]):
+        ci = 1 if i == 0 else C
+        out.append((fe % i + "conv.weight", (C, ci, k), "normal", (0.5 if i == 0 else 1.6) / math.sqrt(ci * k)))
+    ln(fe % 0 + "layer_norm", C)
+    ln("feature_projection.layer_norm", C)
+    _conv(out, "feature_projection.projection", H, C, 1)
+    ln("encoder.layer_norm", H)
+    for l in range(cv["cv_layers"]):
+        p = "encoder.layers.%d." % l
+        for n in ("q", "k", "v", "out"):
+            _conv(out, p + "attention.%s_proj" % n, H, H, 1, gain=1.5 if n in "qk" else 1.0)
+        ln(p + "layer_norm", H)
+        _conv(out, p + "feed_forward.intermediate_dense", Fh, H, 1)
+        _conv(out, p + "feed_forward.output_dense", H, Fh, 1)
+        ln(p + "final_layer_norm", H)
+    _conv(out, "final_proj", 256, H, 1)
+    out.append(("masked_spec_embed", (H,), "normal", 1.0))
+    sd = _draw(out, seed)
+    for name, shape in list(((n, s) for n, s, _, _ in out)):
+        if len(shape) == 3 and shape[2] == 1:
+            sd[name] = sd[name][:, :, 0].contiguous()          # the Linear layers: [out, in]
+    pos = "encoder.pos_conv_embed.conv."
+    v = torch.randn((H, H // G, K), generator=_gen(pos + "weight_v", seed)) / math.sqrt(H // G * K)
+    sd[pos + "weight_v"] = v.float().contiguous()
+    nrm = v.norm(dim=(0, 1), keepdim=True)
+    sd[pos + "weight_g"] = (nrm * (1.0 + 0.15 * torch.randn(nrm.shape, generator=_gen(pos + "weight_g", seed)))).float().contiguous()
+    sd[pos + "bias"] = (torch.randn((H,), generator=_gen(pos + "bias", seed)) * 0.05).float().contiguous()
+    return sd

@@ -542,7 +542,92 @@ def hann_squared(n_fft):
     return ((0.5 - 0.5 * np.cos(2.0 * np.pi * n / n_fft)) ** 2).astype(np.float32)
 
 
-def pack_quickvc(w, cfg, tc=True, precision=None):
+CV_POS = "encoder.pos_conv_embed.conv."
+
+
+def fold_contentvec_pos_conv(sd):
+    """The positional conv's weight-norm fold, w = g * v / ||v||, with HubertPositionalConvEmbedding's dim=2: one norm per tap,
+    taken over dims 0 and 1 (not fold_weight_norm's dim 0).  Takes weight_g / weight_v (the published checkpoint) or
+    parametrizations.weight.original0 / original1 (what transformers 5.x writes); returns the state dict with a plain
+    encoder.pos_conv_embed.conv.weight in their place."""
+    out = dict(sd)
+    for gk, vk in (("weight_g", "weight_v"), ("parametrizations.weight.original0", "parametrizations.weight.original1")):
+        if CV_POS + vk in sd:
+            g, v = (torch.as_tensor(np.asarray(sd[CV_POS + k]) if isinstance(sd[CV_POS + k], np.ndarray) else sd[CV_POS + k]).float()
+                    for k in (gk, vk))
+            out[CV_POS + "weight"] = torch._weight_norm(v, g.reshape(1, 1, -1), 2).contiguous()   # what the parametrization computes
+            del out[CV_POS + gk], out[CV_POS + vk]
+    if CV_POS + "weight" not in out:
+        raise ValueError("the state dict has no positional conv weight (%sweight_g/_v or parametrizations)" % CV_POS)
+    return out
+
+
+def load_contentvec(path, config_json=None):
+    """A Hugging Face ContentVec / HuBERT checkpoint: `path` a pytorch_model.bin (read with weights_only=True) or a directory
+    holding it and config.json.  Returns (folded state dict, cv config): config.contentvec_config of the config.json
+    (HubertConfig's defaults without one), the positional conv folded by fold_contentvec_pos_conv."""
+    import os
+    if os.path.isdir(path):
+        if config_json is None and os.path.exists(os.path.join(path, "config.json")):
+            config_json = os.path.join(path, "config.json")
+        path = os.path.join(path, "pytorch_model.bin")
+    cv = _config.contentvec_config(config_json)
+    sd = torch.load(path, map_location="cpu", weights_only=True)
+    sd = {k[len("hubert."):] if k.startswith("hubert.") else k: v for k, v in sd.items()}
+    return fold_contentvec_pos_conv(sd), cv
+
+
+def _pack_contentvec(P, sd, cv, tc):
+    """cv.* tensors of the engine's ContentVec (csrc/contentvec.cuh, engine.cu cv_enqueue).  Layers 1.. of the feature encoder
+    are 1x1 convs over k consecutive rows ([k*C] inputs, tap-major), the positional conv two halves of its taps per group.
+    tc: also the split-bf16 copies (.th / .tl) of the projection and the transformer's convs, which precision modes >= 1 run
+    on the tensor cores."""
+    g = lambda k: sd[k].detach().cpu().float().numpy() if hasattr(sd[k], "detach") else np.asarray(sd[k], np.float32)
+    C, H, nl = cv["cv_conv_dim"], cv["cv_hidden"], len(cv["cv_conv_kernel"])
+    fe = "feature_extractor.conv_layers.%d."
+    w0 = g(fe % 0 + "conv.weight")
+    if w0.shape != (C, 1, cv["cv_conv_kernel"][0]):
+        raise ValueError("%sconv.weight has shape %s" % (fe % 0, w0.shape))
+    P.add("cv.c0.w", w0[:, 0, :])
+    P.add("cv.gn.g", g(fe % 0 + "layer_norm.weight"))
+    P.add("cv.gn.b", g(fe % 0 + "layer_norm.bias"))
+    for i in range(1, nl):
+        w = g(fe % i + "conv.weight")                                   # [C, C, k]
+        k = w.shape[2]
+        P.conv("cv.c%d" % i, np.transpose(w, (0, 2, 1)).reshape(C, k * C)[:, :, None])
+    P.add("cv.fp.ln.g", g("feature_projection.layer_norm.weight"))
+    P.add("cv.fp.ln.b", g("feature_projection.layer_norm.bias"))
+    conv = lambda name, w, b: (P.conv(name, w, b), tc and P.conv_tc(name, w))
+    conv("cv.fp", g("feature_projection.projection.weight")[:, :, None], g("feature_projection.projection.bias"))
+    pw = g(CV_POS + "weight")                                          # [H, H/G, K]
+    G, K = cv["cv_pos_groups"], cv["cv_pos_k"]
+    Cg, kh = H // G, K // 2
+    if pw.shape != (H, Cg, K):
+        raise ValueError("positional conv weight has shape %s, expected %s" % (pw.shape, (H, Cg, K)))
+    halves = []
+    for half in range(2):
+        for gi in range(G):
+            blk = pw[gi * Cg:(gi + 1) * Cg, :, half * kh:(half + 1) * kh]   # [Cg out, Cg in, kh]
+            halves.append(np.transpose(blk, (2, 1, 0)))                    # [kh][Cg in][Cg out]
+    P.add("cv.pos.w", np.stack(halves))
+    P.add("cv.pos.b", g(CV_POS + "bias"))
+    P.add("cv.enc.ln.g", g("encoder.layer_norm.weight"))
+    P.add("cv.enc.ln.b", g("encoder.layer_norm.bias"))
+    for l in range(cv["cv_layers"]):
+        p = "encoder.layers.%d." % l
+        a = p + "attention.%s_proj."
+        qkv = np.concatenate([g(a % n + "weight") for n in "qkv"], 0)
+        conv("cv.l%d.qkv" % l, qkv[:, :, None], np.concatenate([g(a % n + "bias") for n in "qkv"]))
+        conv("cv.l%d.o" % l, g(a % "out" + "weight")[:, :, None], g(a % "out" + "bias"))
+        P.add("cv.l%d.ln1.g" % l, g(p + "layer_norm.weight"))
+        P.add("cv.l%d.ln1.b" % l, g(p + "layer_norm.bias"))
+        conv("cv.l%d.ffn1" % l, g(p + "feed_forward.intermediate_dense.weight")[:, :, None], g(p + "feed_forward.intermediate_dense.bias"))
+        conv("cv.l%d.ffn2" % l, g(p + "feed_forward.output_dense.weight")[:, :, None], g(p + "feed_forward.output_dense.bias"))
+        P.add("cv.l%d.ln2.g" % l, g(p + "final_layer_norm.weight"))
+        P.add("cv.l%d.ln2.b" % l, g(p + "final_layer_norm.bias"))
+
+
+def pack_quickvc(w, cfg, tc=True, precision=None, contentvec=None, cv=None):
     """QuickVC state dict (folded) -> (blob, manifest) of a model_family "quickvc" engine.
 
     First the speaker encoder enc_spk and the mel front end of the target (vc/convert.py:60-69): each LSTM layer's input
@@ -552,7 +637,10 @@ def pack_quickvc(w, cfg, tc=True, precision=None):
     their offsets: encp.* (the content encoder, laid out as pack's encq.*, without cond), flow.* and dec.* as pack lays them
     out, one stacked cond.w / cond.b (the flow's WN cond rows, then dec.cond, the decoder's Conv1d(256, 512, 1)), and
     dec.w2, the squared Hann window of the decoder's inverse STFT.  tc / precision: as in pack (the speaker encoder is fp32
-    in every mode).  enc_q and the discriminators, which inference never reads, are left out."""
+    in every mode).  enc_q and the discriminators, which inference never reads, are left out.  contentvec: a ContentVec state
+    dict (load_contentvec, or synthetic.make_random_contentvec) whose cv.* tensors go after everything else, with cv its
+    config.contentvec_config (default: hubert-base); without it the blob is what it was before.  Unless tc is off or precision
+    is 0, they include the split-bf16 copies of the convs that precision modes >= 1 run on the tensor cores."""
     g = lambda k: w[k].detach().cpu().numpy() if hasattr(w[k], "detach") else np.asarray(w[k])
     P = _Packer()
     for l in range(cfg.get("spk_layers", 3)):
@@ -581,4 +669,7 @@ def pack_quickvc(w, cfg, tc=True, precision=None):
         P.add("cond.w", np.concatenate(rows_w, 0))
         P.add("cond.b", np.concatenate(rows_b, 0))
         P.add("dec.w2", hann_squared(cfg["gen_istft_n_fft"]))
+    if contentvec is not None:
+        _pack_contentvec(P, fold_contentvec_pos_conv(contentvec) if CV_POS + "weight" not in contentvec else contentvec,
+                         cv or _config.contentvec_config(), tc and precision != 0)
     return P.finish()
