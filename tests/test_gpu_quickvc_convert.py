@@ -110,6 +110,8 @@ def test_noise(precision):
     e, _ = eng.quickvc_convert(u, g, seed=1)
     f, _ = eng.quickvc_convert(u, g, seed=2)
     assert np.array_equal(d, e) and not np.array_equal(d, f) and not np.array_equal(a, d)
+    with pytest.raises(ValueError, match="noise"):          # the engine reads inter_channels rows of every clip
+        eng.quickvc_convert(u, g, noise=np.zeros((1, 191, 37), np.float32))
 
 
 HALO = 32

@@ -224,6 +224,18 @@ struct vtts_engine {
     for (int i = 0; i < std::min(spec_n, 16); ++i) m = std::max(m, spec_hist[i]);
     spec_ratio = m;
   }
+  // Row offsets of items packed as the engine's rows (tokens or frames): item b starts at off[b], SEQ_GAP rows between
+  // items, off[n] the total.  frame_offsets_kernel is the device's copy of this rule.
+  static void pack_rows(const std::vector<int>& len, std::vector<int>& off) {
+    const size_t n = len.size();
+    off.assign(n + 1, 0);
+    for (size_t b = 0; b < n; ++b) off[b + 1] = off[b] + len[b] + (b + 1 < n ? SEQ_GAP : 0);
+  }
+  void pack_frames(const std::vector<int>& frames) {      // host-side frame shape of a call on recordings
+    h_frm_len = frames;
+    pack_rows(h_frm_len, h_frm_off);
+    set_frame_shape();
+  }
   void assume_frames(int frames) {      // host-side frame shape from a prediction (B == 1)
     h_frm_len.assign(1, frames);
     h_frm_off = {0, frames};
@@ -366,6 +378,11 @@ struct vtts_engine {
   // the *_dev entry points): entries are compared on the tuple itself, so there is no hash collision to replay a wrong
   // graph on.  The cache is bounded (LRU, checked on every insertion).
   static constexpr size_t GRAPH_CACHE_MAX = 48;
+  // phase tag, the first element of every key
+  enum GraphTag : long long {
+    TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
+    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7
+  };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
     last_graphed = false;
@@ -559,20 +576,32 @@ struct vtts_engine {
   void dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const int* lens, const int* offs, int maxLen,
                  const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
   struct P1Pin { int *len, *off, *sid, *ids; float *prm, *eps; };
-  P1Pin p1_layout(int t_max, bool eps);
-  void stage1(const int* ids_packed_host, const int* sid_host, int t_max, const float* noise_dp_host);
+  P1Pin p1_layout(bool eps);
+  P1Pin stage_tokens(const int64_t* ids, int t_max, bool eps);
+  void stage1(const P1Pin& pp, int t_max, const float* noise_dp_host);
   void finish1();
   Planes enc_px;                               // the text encoder's output planes (precision modes 2 / 3), read by prior_stats
   void text_encoder(const float* cond, int cond_ld);
   void prior_stats();
-  void phase1(const int* ids_packed_host, const int64_t* d_ids64, int t_max, const int64_t* d_sid64, const int* sid_host,
-              const float* noise_dp, bool noise_on_device);
+  void phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid64, const float* noise_dp, bool noise_on_device);
   void phase2(const float* noise_z, int z_ld, bool noise_on_device, bool run_decoder = true);
-  void stage_noise_z(const float* noise_z, int z_ld) {       // caller memory (maybe pageable) -> pinned [B][I][maxFrm]
+  // Per-call scalars prm[0..n): the call's scales (the noise scale, or TTS's three), zeros, the seed's 32-bit halves at [4..5]
+  static void put_scalars(float* prm, int n, const float* scales, int nscales, uint64_t seed) {
+    std::fill(prm, prm + n, 0.f);
+    std::copy(scales, scales + nscales, prm);
+    const uint32_t half[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
+    memcpy(prm + 4, half, sizeof(half));
+  }
+  // Caller noise rows [B][I][ld] (memory maybe pageable) -> pinned [B][I][maxFrm]: the first cols[b] columns of item b
+  void stage_noise(float* pin, const float* noise, int64_t ld, const std::vector<int>& cols) {
     const int I = cfg.inter_channels;
-    float* pin = reinterpret_cast<float*>(ensure_pinned(h_pin_z, (size_t)B * I * maxFrm * sizeof(float)));
-    const size_t ncopy = (size_t)std::min(z_ld, maxFrm);
-    for (long r = 0; r < (long)B * I; ++r) memcpy(pin + r * maxFrm, noise_z + r * (long)z_ld, ncopy * sizeof(float));
+    for (int b = 0; b < B; ++b)
+      for (int ch = 0; ch < I; ++ch)
+        memcpy(pin + ((size_t)b * I + ch) * maxFrm, noise + ((size_t)b * I + ch) * ld, (size_t)cols[b] * sizeof(float));
+  }
+  void stage_noise_z(const float* noise_z, int z_ld) {
+    float* pin = reinterpret_cast<float*>(ensure_pinned(h_pin_z, (size_t)B * cfg.inter_channels * maxFrm * sizeof(float)));
+    stage_noise(pin, noise_z, z_ld, std::vector<int>(B, std::min(z_ld, maxFrm)));
   }
   void decode(float* z, const int* fl, const int* fo, bool planes_ready = false, bool pz_ready = false);
   bool have_latent = false;
@@ -600,11 +629,15 @@ struct vtts_engine {
   const float *q_cond_w = nullptr, *q_cond_b = nullptr, *stft_basis = nullptr, *mel_fb = nullptr;
   int q_R = 0, spec_pad = 0, vc_pad = 0, vc_wld = 0;
   Buf<int> d_vint;                                 // [clip_len B][sid 2B]
-  Buf<float> d_vprm, d_vin, d_vlin, d_vfeat, d_vstats, d_vcsrc, d_vnoise, d_vz_dbg, d_vzp_dbg;
+  Buf<float> d_vprm, d_vin, d_vlin, d_vfeat, d_vstats, d_vcsrc, d_vnoise, d_vz_dbg, d_vzp_dbg, d_qg;
   Buf<char> h_pin_vc;
-  struct VcPin { int *frm_len, *frm_off, *clip_len, *sid; float *prm, *in, *eps; };
-  VcPin vc_layout(bool from_spec, bool eps);
-  float* vc_upload(bool from_spec, bool eps);
+  // what a call on recordings stages as its input: waveforms, spectrogram (or log-mel) rows, QuickVC's content-unit rows, or
+  // nothing (ContentVec writes the unit rows on the device); the last two also stage QuickVC's target voice g
+  enum ClipIn { IN_WAV, IN_SPEC, IN_UNITS, IN_NONE };
+  struct VcPin { int *frm_len, *frm_off, *clip_len, *sid; float *prm, *in, *g, *eps; };
+  size_t vc_in_floats(ClipIn in) const;
+  VcPin vc_layout(ClipIn in, bool eps);
+  float* vc_upload(ClipIn in, bool eps);
   float* cond_src(bool tgt);
   float* front_end(bool from_spec);
   void posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld);
@@ -624,10 +657,6 @@ struct vtts_engine {
   // ---- QuickVC conversion (SynthesizerTrn.infer, vc/models.py:862-872): enc_p is bound into the q_* members (the same
   //      16-layer k=5 WN as enc_q, which a QuickVC engine does not hold), the flow and the decoder as in a VITS2 engine
   bool has_encp = false;
-  Buf<float> d_units, d_qg;                        // content-unit rows [Tfrm][unit channels], g [B][gin]
-  Buf<char> h_pin_qv;
-  struct QvPin { int *frm_len, *frm_off, *ident; float *prm, *units, *g, *eps; };
-  QvPin qv_layout(bool eps);
   void quickvc_enqueue(bool eps, bool from_wav = false);
 
   // ---- ContentVec (HubertModel of vc/contentvec.py; contentvec.cuh): waveform -> content-unit rows, fp32 FFMA in every mode
@@ -648,6 +677,18 @@ struct vtts_engine {
   void bind_contentvec();
   std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
   void cv_enqueue(float* out, const int* out_offs);
+  // Restores, on scope exit, the host-side frame lengths and the launch knobs an enqueue overrides for its own launches.
+  struct SavedLaunch {
+    vtts_engine* e;
+    std::vector<int> vf, hf;
+    int split, atc, ms, ming, bigg, autog;
+    explicit SavedLaunch(vtts_engine* h) : e(h), vf(h->v_frm_len), hf(h->h_frm_len), split(h->tc_split), atc(h->attn_tc_mode),
+                                           ms(h->conv_max_s), ming(h->conv_min_g), bigg(h->conv_big_g), autog(h->conv_auto_g) {}
+    ~SavedLaunch() {
+      e->v_frm_len = vf; e->h_frm_len = hf; e->tc_split = split; e->attn_tc_mode = atc;
+      e->conv_max_s = ms; e->conv_min_g = ming; e->conv_big_g = bigg; e->conv_auto_g = autog;
+    }
+  };
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
   Buf<float> d_ncent, d_ncent_dbg, d_ascore;       // neg_cent [B][maxFrm][maxTok] (MAS accumulates in place), scores [B]
@@ -1746,24 +1787,24 @@ void vtts_engine::dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, c
 // ---------------------------------------------------------------------------------------------------
 // Phase 1: speaker vector, TextEncoder, StochasticDurationPredictor(reverse), durations.
 // ---------------------------------------------------------------------------------------------------
-void vtts_engine::phase1(const int* ids_packed_host, const int64_t* d_ids64, int t_max, const int64_t* d_sid64,
-                         const int* sid_host, const float* noise_dp, bool noise_on_device) {
+void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid64, const float* noise_dp, bool noise_on_device) {
   const vtts_config& c = cfg;
   const int H = c.hidden_channels, D = c.dp_filter_channels;
   const size_t T = (size_t)Ttok;
   if (!capturing) CK(cudaEventRecord(ev[0], stream));
-  // ---- inputs (host data was staged into h_pin_in by stage1(); only device work is enqueued here)
+  // ---- inputs (host data was staged into h_pin_in by stage_tokens() and stage1(); only device work is enqueued here;
+  //      d_ids64 null: the ids and speaker ids were staged by the host too)
   int* tl = ensure(d_tok_len, B);
   int* to = ensure(d_tok_off, B + 1);
   int* ids = ensure(d_ids, T);
   int* sid = ensure(d_sid, B);
   float* prm = ensure(d_prm, 8);
   {
-    P1Pin pp = p1_layout(t_max, noise_dp && !noise_on_device);
+    P1Pin pp = p1_layout(noise_dp && !noise_on_device);
     CK(cudaMemcpyAsync(tl, pp.len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
     CK(cudaMemcpyAsync(to, pp.off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
     CK(cudaMemcpyAsync(prm, pp.prm, 8 * sizeof(float), cudaMemcpyHostToDevice, stream));
-    if (ids_packed_host) {
+    if (!d_ids64) {
       CK(cudaMemcpyAsync(ids, pp.ids, T * sizeof(int), cudaMemcpyHostToDevice, stream));
       CK(cudaMemcpyAsync(sid, pp.sid, B * sizeof(int), cudaMemcpyHostToDevice, stream));
     } else {
@@ -1951,9 +1992,8 @@ void vtts_engine::prior_stats() {
 }
 
 // Host side of phase 1: stage the call's inputs in pinned memory (fixed layout, so a captured graph can re-read it).
-vtts_engine::P1Pin vtts_engine::p1_layout(int t_max, bool eps) {
+vtts_engine::P1Pin vtts_engine::p1_layout(bool eps) {
   const size_t T = (size_t)Ttok;
-  (void)t_max;
   const size_t bytes = (size_t)(3 * B + 1) * sizeof(int) + T * sizeof(int) + 8 * sizeof(float) +
                        (eps ? (size_t)B * 2 * maxTok * sizeof(float) : 0) + 64;
   char* pin = ensure_pinned(h_pin_in, bytes);
@@ -1967,18 +2007,29 @@ vtts_engine::P1Pin vtts_engine::p1_layout(int t_max, bool eps) {
   return pp;
 }
 
-void vtts_engine::stage1(const int* ids_packed_host, const int* sid_host, int t_max, const float* noise_dp_host) {
-  P1Pin pp = p1_layout(t_max, noise_dp_host != nullptr);
+// Token rows of a call (TTS phase 1, alignment): lengths and offsets of the token shape and, from host ids [B][t_max], the
+// packed ids (zero between and behind the utterances), each checked against n_vocab.  ids null: packed on the device.
+// eps: room for phase 1's staged noise (stage1).
+vtts_engine::P1Pin vtts_engine::stage_tokens(const int64_t* ids, int t_max, bool eps) {
+  P1Pin pp = p1_layout(eps);
   memcpy(pp.len, h_tok_len.data(), B * sizeof(int));
   memcpy(pp.off, h_tok_off.data(), (B + 1) * sizeof(int));
-  if (ids_packed_host) {
-    memcpy(pp.ids, ids_packed_host, (size_t)real_Ttok * sizeof(int));
-    memcpy(pp.sid, sid_host, B * sizeof(int));
+  if (ids) {
+    memset(pp.ids, 0, (size_t)Ttok * sizeof(int));
+    for (int b = 0; b < B; ++b)
+      for (int t = 0; t < h_tok_len[b]; ++t) {
+        const int64_t id = ids[(size_t)b * t_max + t];
+        REQUIRE(id >= 0 && id < cfg.n_vocab, VTTS_ERR_INVALID, "phoneme id out of range [0, n_vocab)");
+        pp.ids[h_tok_off[b] + t] = (int)id;
+      }
   }
-  pp.prm[0] = scales[0]; pp.prm[1] = scales[1]; pp.prm[2] = scales[2]; pp.prm[3] = 0.f;
-  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
-  memcpy(&pp.prm[4], &lo, 4);
-  memcpy(&pp.prm[5], &hi, 4);
+  return pp;
+}
+
+// The phase-1 rest of the staging (pp from stage_tokens): scales and seed, the poll sequence, the speculation's frame cap
+// and the duration predictor's noise.
+void vtts_engine::stage1(const P1Pin& pp, int t_max, const float* noise_dp_host) {
+  put_scalars(pp.prm, 8, scales, 3, seed);
   if (use_poll) {
     const size_t need = (size_t)(2 * B + 4);
     if (need > map_cap) {
@@ -1991,9 +2042,7 @@ void vtts_engine::stage1(const int* ids_packed_host, const int* sid_host, int t_
       ++ws_gen;
     }
     call_seq = (call_seq % 1000000) + 1;
-    memcpy(&pp.prm[6], &call_seq, 4);
-  } else {
-    pp.prm[6] = 0.f;
+    memcpy(&pp.prm[6], &call_seq, 4);       // (0 without polling)
   }
   memcpy(&pp.prm[7], &spec_cap, 4);        // frames the speculative second phase is sized for (0: none), see duration_kernel
   if (noise_dp_host) {        // [B][2][t_max] -> [B][2][maxTok]: the device layout depends on the length bucket only
@@ -2301,16 +2350,27 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
 // Voice conversion (models.py:1710-1718): spectrogram front end, enc_q with g_src, flow forward with g_src, flow reverse
 // with g_tgt, decoder.  The frame counts follow from the input lengths, so the whole call is ONE graphed phase.
 // ---------------------------------------------------------------------------------------------------
-// Pinned staging of one call (fixed layout for a given batch / length bucket, so a captured graph re-reads it on replay):
-// ints [frm_len B][frm_off B+1][clip_len B][sid_src B][sid_tgt B], prm[16], input (wav [B][vc_wld] or spec
-// [B][spec_channels][maxFrm]), eps [B][inter][maxFrm].
-vtts_engine::VcPin vtts_engine::vc_layout(bool from_spec, bool eps) {
+// Pinned staging of a call on recordings (voice conversion, alignment, speaker embedding, QuickVC conversion): ints
+// [frm_len B][frm_off B+1][clip_len B][sid_src B][sid_tgt B], prm[16], the input (wav [B][vc_wld], spec [B][C][maxFrm],
+// unit rows [Tfrm][QV_UNITS] packed as the engine's rows, or none), g [B][gin] (QuickVC conversion only), eps [B][inter][maxFrm].
+// A captured graph copies from these fixed pinned addresses on replay, so every offset here must follow from the graph key
+// alone (batch, length buckets, input kind, noise on / off): the callers key their graphs on all of them.
+size_t vtts_engine::vc_in_floats(ClipIn in) const {
+  switch (in) {
+    case IN_WAV: return (size_t)B * vc_wld;
+    case IN_SPEC: return (size_t)B * cfg.spec_channels * maxFrm;
+    case IN_UNITS: return (size_t)Tfrm * QV_UNITS;
+    default: return 0;
+  }
+}
+
+vtts_engine::VcPin vtts_engine::vc_layout(ClipIn in, bool eps) {
   const vtts_config& c = cfg;
-  const size_t nin = from_spec ? (size_t)B * c.spec_channels * maxFrm : (size_t)B * vc_wld;
+  const size_t nin = vc_in_floats(in), ng = in >= IN_UNITS ? (size_t)B * c.gin_channels : 0;
+  const size_t ne = eps ? (size_t)B * c.inter_channels * maxFrm : 0;
   const size_t ints = (size_t)(5 * B + 1) * sizeof(int);
   const size_t head = (ints + 63) / 64 * 64;
-  const size_t bytes = head + 16 * sizeof(float) + nin * sizeof(float) + (eps ? (size_t)B * c.inter_channels * maxFrm * sizeof(float) : 0) + 64;
-  char* pin = ensure_pinned(h_pin_vc, bytes);
+  char* pin = ensure_pinned(h_pin_vc, head + (16 + nin + ng + ne) * sizeof(float) + 64);
   VcPin pp;
   pp.frm_len = reinterpret_cast<int*>(pin);
   pp.frm_off = pp.frm_len + B;
@@ -2318,27 +2378,30 @@ vtts_engine::VcPin vtts_engine::vc_layout(bool from_spec, bool eps) {
   pp.sid = pp.clip_len + B;
   pp.prm = reinterpret_cast<float*>(pin + head);
   pp.in = pp.prm + 16;
-  pp.eps = pp.in + nin;
+  pp.g = pp.in + nin;
+  pp.eps = pp.g + ng;
   return pp;
 }
 
-// Inputs of a call on the posterior side, from the pinned staging (vc_layout) to the device: frame lengths / offsets, clip
-// lengths and speaker ids, the per-call scalars, the waveform or spectrogram, and the posterior eps (returned; null: Philox).
-float* vtts_engine::vc_upload(bool from_spec, bool eps) {
-  const vtts_config& c = cfg;
-  const int I = c.inter_channels;
-  VcPin pp = vc_layout(from_spec, eps);
+// Inputs of a call on recordings, from the pinned staging (vc_layout) to the device: frame lengths / offsets, clip lengths
+// and speaker ids (d_vint), the per-call scalars, the input (d_vin), g (d_qg), and the posterior eps (returned; null: Philox).
+float* vtts_engine::vc_upload(ClipIn in, bool eps) {
+  const int I = cfg.inter_channels;
+  VcPin pp = vc_layout(in, eps);
   int* fl = ensure(d_frm_len, B);
   int* fo = ensure(d_frm_off, B + 1);
   int* vi = ensure(d_vint, 3 * B);                       // [clip_len B][sid_src B][sid_tgt B]
   float* prm = ensure(d_vprm, 16);
-  const size_t nin = from_spec ? (size_t)B * c.spec_channels * maxFrm : (size_t)B * vc_wld;
-  float* vin = ensure(d_vin, nin);
   CK(cudaMemcpyAsync(fl, pp.frm_len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(fo, pp.frm_off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(vi, pp.clip_len, 3 * B * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(prm, pp.prm, 16 * sizeof(float), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(vin, pp.in, nin * sizeof(float), cudaMemcpyHostToDevice, stream));
+  if (const size_t nin = vc_in_floats(in))
+    CK(cudaMemcpyAsync(ensure(d_vin, nin), pp.in, nin * sizeof(float), cudaMemcpyHostToDevice, stream));
+  if (in >= IN_UNITS) {
+    const size_t ng = (size_t)B * cfg.gin_channels;
+    CK(cudaMemcpyAsync(ensure(d_qg, ng), pp.g, ng * sizeof(float), cudaMemcpyHostToDevice, stream));
+  }
   float* noise = nullptr;
   if (eps) {
     noise = ensure(d_vnoise, (size_t)B * I * maxFrm);
@@ -2456,7 +2519,7 @@ void vtts_engine::posterior_side(bool from_spec, const float* noise, const float
 
 void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
-  const float* noise = vc_upload(from_spec, eps);
+  const float* noise = vc_upload(from_spec ? IN_SPEC : IN_WAV, eps);
   // ---- g_src / g_tgt (models.py:1712-1713) and every cond row of both, one launch: src -> d_vcsrc [B][condR + q_R]
   //      (the TTS rows, then enc_q's), tgt -> d_condv [B][condR] (where the reverse flow and the decoder read them)
   const float* csrc = cond_src(/*tgt=*/true);
@@ -2483,12 +2546,12 @@ void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
 void vtts_engine::align_enqueue(bool from_spec, bool eps) {
   const int I = cfg.inter_channels;
   if (!capturing) CK(cudaEventRecord(ev[0], stream));
-  const float* noise = vc_upload(from_spec, eps);
+  const float* noise = vc_upload(from_spec ? IN_SPEC : IN_WAV, eps);
   int* tl = ensure(d_tok_len, B);
   int* to = ensure(d_tok_off, B + 1);
   int* ids = ensure(d_ids, Ttok);
   {
-    P1Pin pp = p1_layout(0, false);                    // (staged by the host: lengths, offsets, packed ids)
+    P1Pin pp = p1_layout(false);                    // (staged by the host: lengths, offsets, packed ids)
     CK(cudaMemcpyAsync(tl, pp.len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
     CK(cudaMemcpyAsync(to, pp.off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
     CK(cudaMemcpyAsync(ids, pp.ids, (size_t)Ttok * sizeof(int), cudaMemcpyHostToDevice, stream));
@@ -2727,11 +2790,7 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   const int NL = c.cv_n_conv, C = c.cv_conv_dim, H = c.cv_hidden, Fh = c.cv_ffn, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
   // The tensor-core GEMMs run without split-K (every output summed by one CTA in one k order, whatever its launch shape) and
   // attention on attn_tc_kernel whenever it takes the layer: a clip's units are then the same alone and in any batch.
-  struct Saved {
-    vtts_engine* e; std::vector<int> vf, hf; int split, atc;
-    explicit Saved(vtts_engine* h) : e(h), vf(h->v_frm_len), hf(h->h_frm_len), split(h->tc_split), atc(h->attn_tc_mode) {}
-    ~Saved() { e->v_frm_len = vf; e->h_frm_len = hf; e->tc_split = split; e->attn_tc_mode = atc; }
-  } saved(this);
+  SavedLaunch saved(this);
   if (cv_tc) {
     tc_split = 1;
     if (attn_tc_mode > 0) attn_tc_mode = 2;
@@ -2861,7 +2920,7 @@ void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int ma
   int* ds = ensure(d_sseq, seq.size());
   CK(cudaMemcpyAsync(ds, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
   const int *xrow = ds, *slen = ds + ns, *soff = ds + 2 * ns, *last = ds + 3 * ns + 1, *of_clip = ds + 4 * ns + 1;
-  vc_upload(from_mel, false);
+  vc_upload(from_mel ? IN_SPEC : IN_WAV, false);
   const float* feat = front_end(from_mel);
   // Sequences per cluster: the fewest that keep every cluster co-resident; more sequences per cluster lengthen each step,
   // more clusters than fit run in waves.
@@ -2871,12 +2930,7 @@ void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int ma
   // The projections run with one fixed launch shape (no split-K across CTAs or thread groups), so every row is summed in the
   // same order whatever the batch: a clip's g does not depend on the clips it is batched with.  Layers 1 and 2 launch over
   // the slices, so the host-side lengths the launch heuristics read are the slices' for those launches.
-  struct Saved {
-    vtts_engine* e; int ms, ming, bigg, autog; std::vector<int> vf, hf;
-    explicit Saved(vtts_engine* h) : e(h), ms(h->conv_max_s), ming(h->conv_min_g), bigg(h->conv_big_g), autog(h->conv_auto_g),
-                                     vf(h->v_frm_len), hf(h->h_frm_len) {}
-    ~Saved() { e->conv_max_s = ms; e->conv_min_g = ming; e->conv_big_g = bigg; e->conv_auto_g = autog; e->v_frm_len = vf; e->h_frm_len = hf; }
-  } saved(this);
+  SavedLaunch saved(this);
   conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
   const std::vector<int> slen_h(seq.begin() + ns, seq.begin() + 2 * ns);
   const float* x = feat;
@@ -2908,58 +2962,22 @@ void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int ma
 // reverse flow with g, the decoder with cond(g) and the torch.istft tail.  The frame counts are the unit counts, so the whole
 // call is ONE graphed phase.
 // ---------------------------------------------------------------------------------------------------
-// Pinned staging of one call (fixed layout for a given batch / length bucket): ints [frm_len B][frm_off B+1][identity B],
-// prm[16], unit rows [Tfrm][QV_UNITS] (clips packed as the engine's rows, SEQ_GAP zero rows between them), g [B][gin],
-// eps [B][inter][maxFrm].
-vtts_engine::QvPin vtts_engine::qv_layout(bool eps) {
-  const vtts_config& c = cfg;
-  const size_t ints = (size_t)(3 * B + 1) * sizeof(int);
-  const size_t head = (ints + 63) / 64 * 64;
-  const size_t nu = (size_t)Tfrm * QV_UNITS, ng = (size_t)B * c.gin_channels, ne = eps ? (size_t)B * c.inter_channels * maxFrm : 0;
-  char* pin = ensure_pinned(h_pin_qv, head + (16 + nu + ng + ne) * sizeof(float) + 64);
-  QvPin pp;
-  pp.frm_len = reinterpret_cast<int*>(pin);
-  pp.frm_off = pp.frm_len + B;
-  pp.ident = pp.frm_off + B + 1;
-  pp.prm = reinterpret_cast<float*>(pin + head);
-  pp.units = pp.prm + 16;
-  pp.g = pp.units + nu;
-  pp.eps = pp.g + ng;
-  return pp;
-}
-
 void vtts_engine::quickvc_enqueue(bool eps, bool from_wav) {
-  const vtts_config& c = cfg;
-  const int I = c.inter_channels, G = c.gin_channels;
+  const int G = cfg.gin_channels;
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
-  QvPin pp = qv_layout(eps);
-  int* fl = ensure(d_frm_len, B);
-  int* fo = ensure(d_frm_off, B + 1);
-  int* ident = ensure(d_vint, B);
-  float* prm = ensure(d_vprm, 16);
-  float* units = ensure(d_units, (size_t)Tfrm * QV_UNITS);
-  float* g = ensure(d_qg, (size_t)B * G);
-  CK(cudaMemcpyAsync(fl, pp.frm_len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(fo, pp.frm_off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(ident, pp.ident, B * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(prm, pp.prm, 16 * sizeof(float), cudaMemcpyHostToDevice, stream));
+  const float* noise = vc_upload(from_wav ? IN_NONE : IN_UNITS, eps);
+  const int* fl = d_frm_len.p;
+  const int* fo = d_frm_off.p;
+  float* units = ensure(d_vin, (size_t)Tfrm * QV_UNITS);       // unit rows, packed as the engine's rows
   if (from_wav) {      // ContentVec writes the unit rows; the gaps between clips and the bucket's tail stay zero
     CK(cudaMemsetAsync(units, 0, (size_t)Tfrm * QV_UNITS * sizeof(float), stream));
     cv_enqueue(units, fo);
-  } else {
-    CK(cudaMemcpyAsync(units, pp.units, (size_t)Tfrm * QV_UNITS * sizeof(float), cudaMemcpyHostToDevice, stream));
-  }
-  CK(cudaMemcpyAsync(g, pp.g, (size_t)B * G * sizeof(float), cudaMemcpyHostToDevice, stream));
-  float* noise = nullptr;
-  if (eps) {
-    noise = ensure(d_vnoise, (size_t)B * I * maxFrm);
-    CK(cudaMemcpyAsync(noise, pp.eps, (size_t)B * I * maxFrm * sizeof(float), cudaMemcpyHostToDevice, stream));
   }
   // ---- g's cond rows [B][condR] (the flow's WN cond layers, then dec.cond) in d_condv: the uploaded g rows are the table
-  //      cond_vc_kernel reads, through the identity index
+  //      cond_vc_kernel reads, through sid_src = b
   float* cond = ensure(d_condv, (size_t)B * condR);
-  klaunch(cond_vc_kernel, dim3((condR + 7) / 8, B), dim3(256), (size_t)(G * sizeof(float)), (const float*)g, (const int*)ident, cond_w,
-          cond_b, condR, (const float*)nullptr, (const float*)nullptr, 0, cond, (float*)nullptr, G, B, B);
+  klaunch(cond_vc_kernel, dim3((condR + 7) / 8, B), dim3(256), (size_t)(G * sizeof(float)), (const float*)d_qg.p,
+          (const int*)(d_vint.p + B), cond_w, cond_b, condR, (const float*)nullptr, (const float*)nullptr, 0, cond, (float*)nullptr, G, B, B);
   CK(cudaGetLastError());
   ++launches;
   // ---- z_p, m_p, logs_p = enc_p(c)   (models.py:868)
@@ -3042,21 +3060,29 @@ void collect_timings(vtts_handle h) {
   cudaEventElapsedTime(&t, h->ev[6], h->ev[7]); h->stage_ms[5] = t;
 }
 
+// Readback of a call's packed output rows: D2H of the first n values of src into pinned staging sized for `cap` values (the
+// bucket's, so that it does not grow with every new length), ev[7], a sync, then clip b's lens[b] rows of `width` values
+// from packed row offs[b] to out + b * out_ld.  The rest of each output row is left as it is.
+template <typename T>
+void read_clips(vtts_handle h, const T* src, size_t n, size_t cap, const int* offs, const std::vector<int>& lens, int width,
+                T* out, int64_t out_ld) {
+  T* pin = reinterpret_cast<T*>(h->ensure_pinned(cap * sizeof(T) + 64));
+  CK(cudaMemcpyAsync(pin, src, n * sizeof(T), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaEventRecord(h->ev[7], h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (size_t b = 0; b < lens.size(); ++b)
+    memcpy(out + b * out_ld, pin + (size_t)offs[b] * width, (size_t)lens[b] * width * sizeof(T));
+}
+
 void setup_lengths(vtts_handle h, const int64_t* lengths, int B, int t_max) {
   REQUIRE(B >= 1 && B <= 16384 && t_max >= 1, VTTS_ERR_INVALID, "bad batch size / t_max");
   h->B = B;
   h->h_tok_len.resize(B);
-  h->h_tok_off.resize(B + 1);
-  int off = 0, mx = 0;
   for (int b = 0; b < B; ++b) {
     REQUIRE(lengths[b] >= 1 && lengths[b] <= t_max, VTTS_ERR_INVALID, "input_lengths must be in [1, t_max]");
     h->h_tok_len[b] = (int)lengths[b];
-    h->h_tok_off[b] = off;
-    off += (int)lengths[b] + (b + 1 < B ? SEQ_GAP : 0);
-    mx = std::max(mx, (int)lengths[b]);
   }
-  h->h_tok_off[B] = off;
-  (void)mx;
+  vtts_engine::pack_rows(h->h_tok_len, h->h_tok_off);
   h->set_token_shape();
   h->have_durations = false;
   h->have_latent = false;
@@ -3073,18 +3099,14 @@ static void enqueue_phase1_host(vtts_handle h, const int64_t* ids, const int64_t
   memcpy(h->scales, scales, 3 * sizeof(float));
   h->seed = seed;
   h->spec_cap = (may_speculate && spec_ok(h, B)) ? vtts_engine::bucket_frm(h->spec_predict()) : 0;
-  std::vector<int> packed(h->Ttok), sid32(B);
+  const vtts_engine::P1Pin pp = h->stage_tokens(ids, t_max, noise_dp != nullptr);
   for (int b = 0; b < B; ++b) {
-    for (int t = 0; t < h->h_tok_len[b]; ++t) {
-      const int64_t id = ids[(size_t)b * t_max + t];
-      REQUIRE(id >= 0 && id < h->cfg.n_vocab, VTTS_ERR_INVALID, "phoneme id out of range [0, n_vocab)");
-      packed[h->h_tok_off[b] + t] = (int)id;
-    }
     REQUIRE(!h->has_g || (sid[b] >= 0 && sid[b] < h->cfg.n_speakers), VTTS_ERR_INVALID, "speaker id out of range [0, n_speakers)");
-    sid32[b] = (int)sid[b];
+    pp.sid[b] = (int)sid[b];
   }
-  h->stage1(packed.data(), sid32.data(), t_max, noise_dp);
-  h->run_graphed({0x11, B, h->maxTok, h->Ttok, noise_dp ? 1 : 0}, [&] { h->phase1(packed.data(), nullptr, t_max, nullptr, sid32.data(), noise_dp, false); });
+  h->stage1(pp, t_max, noise_dp);
+  h->run_graphed({vtts_engine::TAG_PHASE1, B, h->maxTok, h->Ttok, noise_dp ? 1 : 0},
+                 [&] { h->phase1(nullptr, t_max, nullptr, noise_dp, false); });
 }
 
 static void impl_durations(vtts_handle h, const int64_t* ids, const int64_t* lengths, const int64_t* sid, int B, int t_max,
@@ -3111,19 +3133,11 @@ static void impl_synthesize(vtts_handle h, const float* noise_z, int z_ld, float
   REQUIRE(!frame_token || idx_ld >= h->real_maxFrm, VTTS_ERR_CAPACITY, "frame_token has fewer columns than max(y_lengths)");
   if (noise_z) h->stage_noise_z(noise_z, z_ld);
   // graph key = the length BUCKETS (token rows, frame rows), not the lengths: kernels read the true lengths on the device
-  h->run_graphed({0x22, h->B, h->maxFrm, h->Tfrm, noise_z ? 1 : 0}, [&] { h->phase2(noise_z, z_ld, false); });
-  const size_t nw = (size_t)h->real_Tfrm * h->hop;
-  char* pin = h->ensure_pinned((size_t)h->Tfrm * h->hop * sizeof(float) + (size_t)h->Tfrm * sizeof(int) + 64);
-  float* pw = reinterpret_cast<float*>(pin);
-  int* pi = reinterpret_cast<int*>(pw + (size_t)h->Tfrm * h->hop);
-  CK(cudaMemcpyAsync(pw, h->d_wav.p, nw * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (frame_token) CK(cudaMemcpyAsync(pi, h->d_ftok.p, (size_t)h->real_Tfrm * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaEventRecord(h->ev[7], h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  for (int b = 0; b < h->B; ++b) {
-    memcpy(wav + (size_t)b * wav_ld, pw + (size_t)h->h_frm_off[b] * h->hop, (size_t)h->h_frm_len[b] * h->hop * sizeof(float));
-    if (frame_token) memcpy(frame_token + (size_t)b * idx_ld, pi + h->h_frm_off[b], (size_t)h->h_frm_len[b] * sizeof(int));
-  }
+  h->run_graphed({vtts_engine::TAG_PHASE2, h->B, h->maxFrm, h->Tfrm, noise_z ? 1 : 0}, [&] { h->phase2(noise_z, z_ld, false); });
+  if (frame_token)
+    read_clips(h, (const int*)h->d_ftok.p, h->real_Tfrm, h->Tfrm, h->h_frm_off.data(), h->h_frm_len, 1, frame_token, idx_ld);
+  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), h->h_frm_len,
+             h->hop, wav, wav_ld);
   collect_timings(h);
   h->have_durations = false;
 }
@@ -3134,10 +3148,11 @@ static void enqueue_phase1_dev(vtts_handle h, const int64_t* d_ids, const int64_
   memcpy(h->scales, scales, 3 * sizeof(float));
   h->seed = seed;
   h->spec_cap = (may_speculate && spec_ok(h, B)) ? vtts_engine::bucket_frm(h->spec_predict()) : 0;
-  h->stage1(nullptr, nullptr, t_max, nullptr);
+  h->stage1(h->stage_tokens(nullptr, t_max, false), t_max, nullptr);
   h->eps_dp_ld = t_max;      // device noise is read in the caller's [B][2][t_max] layout
-  h->run_graphed({0x33, B, h->maxTok, h->Ttok, t_max, (long long)(uintptr_t)d_ids, (long long)(uintptr_t)d_sid, (long long)(uintptr_t)d_noise_dp},
-                 [&] { h->phase1(nullptr, d_ids, t_max, d_sid, nullptr, d_noise_dp, true); });
+  h->run_graphed({vtts_engine::TAG_PHASE1_DEV, B, h->maxTok, h->Ttok, t_max, (long long)(uintptr_t)d_ids, (long long)(uintptr_t)d_sid,
+                  (long long)(uintptr_t)d_noise_dp},
+                 [&] { h->phase1(d_ids, t_max, d_sid, d_noise_dp, true); });
 }
 
 static void impl_durations_dev(vtts_handle h, const int64_t* d_ids, const int64_t* lengths_host, const int64_t* d_sid, int B, int t_max,
@@ -3168,7 +3183,7 @@ static void impl_infer(vtts_handle h, const int64_t* ids, const int64_t* lengths
     h->assume_frames(h->spec_cap);
     const int cap = h->maxFrm;
     if (noise_z) h->stage_noise_z(noise_z, z_ld);
-    h->run_graphed({0x22, h->B, h->maxFrm, h->Tfrm, noise_z ? 1 : 0}, [&] { h->phase2(noise_z, z_ld, false); });
+    h->run_graphed({vtts_engine::TAG_PHASE2, h->B, h->maxFrm, h->Tfrm, noise_z ? 1 : 0}, [&] { h->phase2(noise_z, z_ld, false); });
     // the true length is not known on the host yet: the bucket's worth of samples comes back
     const size_t ncap = (size_t)cap * h->hop;
     char* pin = h->ensure_pinned(ncap * sizeof(float) + (size_t)cap * sizeof(int) + 64);
@@ -3221,7 +3236,7 @@ static void impl_infer_dev(vtts_handle h, const int64_t* d_ids, const int64_t* l
   if (h->spec_cap > 0) {
     h->assume_frames(h->spec_cap);
     const int cap = h->maxFrm;
-    h->run_graphed({0x44, h->B, h->maxFrm, h->Tfrm, z_ld, (long long)(uintptr_t)d_noise_z}, [&] { h->phase2(d_noise_z, z_ld, true); });
+    h->run_graphed({vtts_engine::TAG_PHASE2_DEV, h->B, h->maxFrm, h->Tfrm, z_ld, (long long)(uintptr_t)d_noise_z}, [&] { h->phase2(d_noise_z, z_ld, true); });
     const size_t ncopy = (size_t)std::min<int64_t>((int64_t)cap * h->hop, wav_ld);
     CK(cudaMemcpyAsync(d_wav, h->d_wav.p, ncopy * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -3279,15 +3294,10 @@ static void stage_clips(vtts_handle h, bool from_spec, const float* in, const in
                         const int64_t* sid_src, const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed) {
   const vtts_config& c = h->cfg;
   const int B = h->B;
-  h->h_frm_len = frames;
-  h->h_frm_off.assign(B + 1, 0);
-  int off = 0;
-  for (int b = 0; b < B; ++b) { h->h_frm_off[b] = off; off += frames[b] + (b + 1 < B ? SEQ_GAP : 0); }
-  h->h_frm_off[B] = off;
-  h->set_frame_shape();
+  h->pack_frames(frames);
   h->vc_wld = (h->maxFrm + 2) * c.hop_length + c.filter_length;
-  const int maxF = h->maxFrm, I = c.inter_channels, C = c.spec_channels;
-  vtts_engine::VcPin pp = h->vc_layout(from_spec, noise_q != nullptr);
+  const int maxF = h->maxFrm, C = c.spec_channels;
+  const vtts_engine::VcPin pp = h->vc_layout(from_spec ? vtts_engine::IN_SPEC : vtts_engine::IN_WAV, noise_q != nullptr);
   memcpy(pp.frm_len, frames.data(), B * sizeof(int));
   memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
   for (int b = 0; b < B; ++b) {
@@ -3300,15 +3310,9 @@ static void stage_clips(vtts_handle h, bool from_spec, const float* in, const in
     } else {
       memcpy(pp.in + (size_t)b * h->vc_wld, in + (size_t)b * ld, (size_t)lengths[b] * sizeof(float));
     }
-    if (noise_q)
-      for (int ch = 0; ch < I; ++ch)
-        memcpy(pp.eps + ((size_t)b * I + ch) * maxF, noise_q + ((size_t)b * I + ch) * q_ld, (size_t)frames[b] * sizeof(float));
   }
-  for (int i = 0; i < 16; ++i) pp.prm[i] = 0.f;
-  pp.prm[0] = noise_scale;
-  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
-  memcpy(&pp.prm[4], &lo, 4);
-  memcpy(&pp.prm[5], &hi, 4);
+  if (noise_q) h->stage_noise(pp.eps, noise_q, q_ld, frames);
+  vtts_engine::put_scalars(pp.prm, 16, &noise_scale, 1, seed);
 }
 
 // Voice conversion through host buffers (vtts_convert / vtts_convert_spec).
@@ -3332,17 +3336,11 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
   REQUIRE((int64_t)real_max * h->hop <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than hop * max(frames)");
   REQUIRE(!noise_q || q_ld >= real_max, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
   stage_clips(h, from_spec, in, lengths, ld, frames, sid_src, sid_tgt, noise_scale, noise_q, q_ld, seed);
-  h->run_graphed({0x55, B, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
+  h->run_graphed({vtts_engine::TAG_CONVERT, B, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
                  [&] { h->convert_enqueue(from_spec, noise_q != nullptr); });
-  const size_t nw = (size_t)h->real_Tfrm * h->hop;
-  float* pw = reinterpret_cast<float*>(h->ensure_pinned((size_t)h->Tfrm * h->hop * sizeof(float) + 64));
-  CK(cudaMemcpyAsync(pw, h->d_wav.p, nw * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaEventRecord(h->ev[7], h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  for (int b = 0; b < B; ++b) {
-    memcpy(out_wav + (size_t)b * out_ld, pw + (size_t)h->h_frm_off[b] * h->hop, (size_t)frames[b] * h->hop * sizeof(float));
-    out_frames[b] = frames[b];
-  }
+  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames,
+             h->hop, out_wav, out_ld);
+  std::copy(frames.begin(), frames.end(), out_frames);
 }
 
 // QuickVC speaker embedding through host buffers (vtts_speaker_embedding / _mel).
@@ -3405,26 +3403,15 @@ static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const 
     REQUIRE(tx <= TX_MAX, VTTS_ERR_INVALID, "more than " + std::to_string(TX_MAX) + " tokens in one utterance: above the alignment's limit");
     REQUIRE(tx <= frames[b], VTTS_ERR_INVALID, "more tokens (" + std::to_string(tx) + ") than frames (" + std::to_string(frames[b]) +
             ") in utterance " + std::to_string(b) + ": no monotonic alignment exists");
-    for (int64_t t = 0; t < tx; ++t) {
-      const int64_t id = ids[(size_t)b * t_max + t];
-      REQUIRE(id >= 0 && id < c.n_vocab, VTTS_ERR_INVALID, "phoneme id out of range [0, n_vocab)");
-    }
     REQUIRE(!h->has_g || (sid && sid[b] >= 0 && sid[b] < c.n_speakers), VTTS_ERR_INVALID, "speaker id out of range [0, n_speakers)");
   }
   const int real_max = *std::max_element(frames.begin(), frames.end());
   REQUIRE(!token_of_frame || tof_ld >= real_max, VTTS_ERR_CAPACITY, "tof_ld is smaller than max(frames)");
   REQUIRE(!noise_q || q_ld >= real_max, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
   setup_lengths(h, id_lengths, B, t_max);
+  h->stage_tokens(ids, t_max, false);               // (the alignment does not advance phase 1's poll sequence)
   stage_clips(h, from_spec, in, lengths, ld, frames, h->has_g ? sid : nullptr, nullptr, noise_scale, noise_q, q_ld, seed);
-  {
-    vtts_engine::P1Pin pp = h->p1_layout(t_max, false);
-    memcpy(pp.len, h->h_tok_len.data(), B * sizeof(int));
-    memcpy(pp.off, h->h_tok_off.data(), (B + 1) * sizeof(int));
-    memset(pp.ids, 0, (size_t)h->Ttok * sizeof(int));
-    for (int b = 0; b < B; ++b)
-      for (int t = 0; t < h->h_tok_len[b]; ++t) pp.ids[h->h_tok_off[b] + t] = (int)ids[(size_t)b * t_max + t];
-  }
-  h->run_graphed({0x66, B, h->maxTok, h->Ttok, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
+  h->run_graphed({vtts_engine::TAG_ALIGN, B, h->maxTok, h->Ttok, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
                  [&] { h->align_enqueue(from_spec, noise_q != nullptr); });
   const size_t nt = (size_t)h->real_Ttok, nf = (size_t)h->real_Tfrm;
   int* pin = reinterpret_cast<int*>(h->ensure_pinned((nt + nf + (size_t)B) * sizeof(int) + 64));
@@ -3464,15 +3451,10 @@ static void impl_content_units(vtts_handle h, const float* wav, const int64_t* l
   for (int b = 0; b < B; ++b) REQUIRE(frames[b] <= units_ld, VTTS_ERR_CAPACITY, "units_ld is smaller than a clip's frame count");
   const int H = h->cfg.cv_hidden, NL = h->cfg.cv_n_conv;
   const size_t Tf = (size_t)h->cvp.tot0 / h->cv_P;
-  h->run_graphed({0xC7, B, h->cvp.maxS, h->cvp.tot0}, [&] { h->cv_enqueue(h->ensure(h->d_cvu, Tf * H), nullptr); });
-  float* pu = reinterpret_cast<float*>(h->ensure_pinned(Tf * H * sizeof(float) + 64));
-  CK(cudaMemcpyAsync(pu, h->d_cvu.p, Tf * H * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  h->run_graphed({vtts_engine::TAG_CONTENTVEC, B, h->cvp.maxS, h->cvp.tot0}, [&] { h->cv_enqueue(h->ensure(h->d_cvu, Tf * H), nullptr); });
+  read_clips(h, (const float*)h->d_cvu.p, Tf * H, Tf * H, h->cvp.h.data() + (NL + NL - 1) * B, frames, H, units, units_ld * H);
   for (int b = 0; b < B; ++b) {
-    const size_t n = (size_t)frames[b] * H;
-    float* dst = units + (size_t)b * units_ld * H;
-    memcpy(dst, pu + (size_t)h->cvp.h[(NL + NL - 1) * B + b] * H, n * sizeof(float));
-    std::fill(dst + n, dst + (size_t)units_ld * H, 0.f);
+    std::fill(units + ((size_t)b * units_ld + frames[b]) * H, units + (size_t)(b + 1) * units_ld * H, 0.f);
     out_frames[b] = frames[b];
   }
 }
@@ -3507,48 +3489,35 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const float*
   h->B = B;
   h->have_durations = false;
   h->have_latent = false;
-  h->h_frm_len = frames;
-  h->h_frm_off.assign(B + 1, 0);
-  int off = 0;
-  for (int b = 0; b < B; ++b) { h->h_frm_off[b] = off; off += frames[b] + (b + 1 < B ? SEQ_GAP : 0); }
-  h->h_frm_off[B] = off;
-  h->set_frame_shape();
-  const int maxF = h->maxFrm, I = c.inter_channels, G = c.gin_channels;
-  vtts_engine::QvPin pp = h->qv_layout(noise != nullptr);
+  h->pack_frames(frames);
+  constexpr int U = vtts_engine::QV_UNITS;
+  const int G = c.gin_channels;
+  const vtts_engine::VcPin pp = h->vc_layout(units ? vtts_engine::IN_UNITS : vtts_engine::IN_NONE, noise != nullptr);
   memcpy(pp.frm_len, frames.data(), B * sizeof(int));
   memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
   for (int b = 0; b < B; ++b) {
-    pp.ident[b] = b;
+    pp.clip_len[b] = frames[b];
+    pp.sid[b] = b;                                      // cond_vc_kernel's row of g
+    pp.sid[B + b] = 0;
     const int o = h->h_frm_off[b];
     if (units) {
-    memcpy(pp.units + (size_t)o * vtts_engine::QV_UNITS, units + (size_t)b * units_ld * vtts_engine::QV_UNITS,
-           (size_t)frames[b] * vtts_engine::QV_UNITS * sizeof(float));
-    const int gap_end = b + 1 < B ? h->h_frm_off[b + 1] : h->Tfrm;       // rows behind the clip: the gap, or the bucket's tail
-    memset(pp.units + (size_t)(o + frames[b]) * vtts_engine::QV_UNITS, 0, (size_t)(gap_end - o - frames[b]) * vtts_engine::QV_UNITS * sizeof(float));
+      memcpy(pp.in + (size_t)o * U, units + (size_t)b * units_ld * U, (size_t)frames[b] * U * sizeof(float));
+      const int gap_end = b + 1 < B ? h->h_frm_off[b + 1] : h->Tfrm;       // rows behind the clip: the gap, or the bucket's tail
+      memset(pp.in + (size_t)(o + frames[b]) * U, 0, (size_t)(gap_end - o - frames[b]) * U * sizeof(float));
     }
-    memcpy(pp.g + (size_t)b * G, g + (size_t)b * G, G * sizeof(float));
-    if (noise)
-      for (int ch = 0; ch < I; ++ch)
-        memcpy(pp.eps + ((size_t)b * I + ch) * maxF, noise + ((size_t)b * I + ch) * noise_ld, (size_t)frames[b] * sizeof(float));
   }
-  for (int i = 0; i < 16; ++i) pp.prm[i] = 0.f;
-  pp.prm[0] = noise_scale;
-  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
-  memcpy(&pp.prm[4], &lo, 4);
-  memcpy(&pp.prm[5], &hi, 4);
+  memcpy(pp.g, g, (size_t)B * G * sizeof(float));
+  if (noise) h->stage_noise(pp.eps, noise, noise_ld, frames);
+  vtts_engine::put_scalars(pp.prm, 16, &noise_scale, 1, seed);
   if (wav)
-    h->run_graphed({0x78, B, h->maxFrm, h->Tfrm, noise ? 1 : 0, h->cvp.maxS, h->cvp.tot0}, [&] { h->quickvc_enqueue(noise != nullptr, true); });
+    h->run_graphed({vtts_engine::TAG_QUICKVC_WAV, B, h->maxFrm, h->Tfrm, noise ? 1 : 0, h->cvp.maxS, h->cvp.tot0},
+                   [&] { h->quickvc_enqueue(noise != nullptr, true); });
   else
-    h->run_graphed({0x77, B, h->maxFrm, h->Tfrm, noise ? 1 : 0}, [&] { h->quickvc_enqueue(noise != nullptr); });
-  const size_t nw = (size_t)h->real_Tfrm * h->hop;
-  float* pw = reinterpret_cast<float*>(h->ensure_pinned((size_t)h->Tfrm * h->hop * sizeof(float) + 64));
-  CK(cudaMemcpyAsync(pw, h->d_wav.p, nw * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaEventRecord(h->ev[7], h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+    h->run_graphed({vtts_engine::TAG_QUICKVC, B, h->maxFrm, h->Tfrm, noise ? 1 : 0}, [&] { h->quickvc_enqueue(noise != nullptr); });
+  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames,
+             h->hop, out_wav, out_ld);
   for (int b = 0; b < B; ++b) {
-    const size_t n = (size_t)frames[b] * h->hop;
-    memcpy(out_wav + (size_t)b * out_ld, pw + (size_t)h->h_frm_off[b] * h->hop, n * sizeof(float));
-    std::fill(out_wav + (size_t)b * out_ld + n, out_wav + (size_t)(b + 1) * out_ld, 0.f);
+    std::fill(out_wav + (size_t)b * out_ld + (size_t)frames[b] * h->hop, out_wav + (size_t)(b + 1) * out_ld, 0.f);
     out_frames[b] = frames[b];
   }
 }
@@ -3557,7 +3526,7 @@ static void impl_synthesize_dev(vtts_handle h, const float* d_noise_z, int z_ld,
   REQUIRE(h->have_durations, VTTS_ERR_STATE, "vtts_synthesize_dev called without vtts_durations_dev");
   REQUIRE((int64_t)h->real_maxFrm * h->hop <= wav_ld, VTTS_ERR_CAPACITY, "wav_ld is smaller than hop * max(y_lengths)");
   REQUIRE(!d_noise_z || z_ld >= h->real_maxFrm, VTTS_ERR_CAPACITY, "noise_z has fewer columns than max(y_lengths)");
-  h->run_graphed({0x44, h->B, h->maxFrm, h->Tfrm, z_ld, (long long)(uintptr_t)d_noise_z}, [&] { h->phase2(d_noise_z, z_ld, true); });
+  h->run_graphed({vtts_engine::TAG_PHASE2_DEV, h->B, h->maxFrm, h->Tfrm, z_ld, (long long)(uintptr_t)d_noise_z}, [&] { h->phase2(d_noise_z, z_ld, true); });
   for (int b = 0; b < h->B; ++b)
     CK(cudaMemcpyAsync(d_wav + (size_t)b * wav_ld, h->d_wav.p + (size_t)h->h_frm_off[b] * h->hop,
                        (size_t)h->h_frm_len[b] * h->hop * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
@@ -3700,7 +3669,7 @@ void vtts_destroy(vtts_handle h) {
                       &h->d_fao, &h->d_fy, &h->d_ffh2, &h->d_eps_z, &h->d_d0, &h->d_post, &h->d_wav};
   for (auto* b : fb) fr(b->p);
   Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg,
-                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg, &h->d_units, &h->d_qg,
+                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg, &h->d_qg,
                       &h->d_cvzero, &h->d_cvwav, &h->d_cvps, &h->d_cvpq, &h->d_cvl[0], &h->d_cvl[1], &h->d_cvx, &h->d_cvx1, &h->d_cvy,
                       &h->d_cvqkv, &h->d_cvao, &h->d_cvff, &h->d_cvu, &h->d_cvdbg};
   for (auto* b : vb) fr(b->p);
@@ -3710,7 +3679,7 @@ void vtts_destroy(vtts_handle h) {
   for (auto& b : h->d_stage) fr(b.p);
   for (auto& v : h->d_xj) for (auto& b : v) fr(b.p);
   for (auto& v : h->d_tmp) for (auto& b : v) fr(b.p);
-  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc, &h->h_pin_qv, &h->h_pin_cv}) if (hb->p) cudaFreeHost(hb->p);
+  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc, &h->h_pin_cv}) if (hb->p) cudaFreeHost(hb->p);
   for (auto& kv : h->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
   fr(h->d_prm.p);
   fr(h->d_pref.p);

@@ -306,6 +306,44 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _batch(x, lengths, ndim, t_axis=-1, ragged=False):
+    """A batch of recordings or rows as the C ABI reads it: `x` with `ndim` axes, or one item without the batch axis, as
+    contiguous float32; `lengths` as int64 [B] (one value for every item; None: the full axis `t_axis`).  ragged: `x` may
+    also be a list of items of different lengths along their first axis, zero-padded to the longest (their lengths are
+    then the lengths)."""
+    if ragged and isinstance(x, (list, tuple)):
+        items = [np.asarray(u, np.float32) for u in x]
+        if ndim == 2:
+            items = [u.reshape(-1) for u in items]
+        lengths = np.array([u.shape[0] for u in items], np.int64)
+        x = np.zeros((len(items), int(lengths.max())) + items[0].shape[1:], np.float32)
+        for b, u in enumerate(items):
+            x[b, :u.shape[0]] = u
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    if x.ndim == ndim - 1:
+        x = x[None]
+    B = x.shape[0]
+    if lengths is None:
+        return x, np.full(B, x.shape[t_axis], np.int64)
+    return x, np.ascontiguousarray(np.broadcast_to(np.asarray(lengths, np.int64).reshape(-1), (B,)))
+
+
+def _noise(noise, B, channels):
+    """Caller noise standing in for a posterior sample's eps: (float32 [B, channels, >= 1], its row pitch), or (None, 0).
+    The engine reads every [b, channel] row, so any other shape is refused."""
+    if noise is None:
+        return None, 0
+    noise = np.ascontiguousarray(noise, dtype=np.float32)
+    if noise.ndim != 3 or noise.shape[0] != B or noise.shape[1] != channels or noise.shape[2] < 1:
+        raise ValueError("noise must be float32 [B, inter_channels, >= frames]")
+    return noise, noise.shape[2]
+
+
+def _per_item(v, B, width):
+    """One row [width] for every item, or one per item [B, width] -> contiguous float32 [B, width]."""
+    return np.ascontiguousarray(np.broadcast_to(np.asarray(v, np.float32).reshape(-1, width), (B, width)))
+
+
 class Engine:
     """One engine = one GPU.  `blob` may be a numpy float32 array (host) or an (int device_ptr, n_floats) tuple."""
 
@@ -486,15 +524,9 @@ class Engine:
     # ---- voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718)
     def _convert(self, from_wav, x, lengths, ld, sid_src, sid_tgt, noise_scale, noise, seed):
         B = x.shape[0]
-        lengths = np.ascontiguousarray(lengths, dtype=np.int64).reshape(B)
         src = np.ascontiguousarray(np.broadcast_to(np.asarray(sid_src, np.int64), (B,)))
         tgt = np.ascontiguousarray(np.broadcast_to(np.asarray(sid_tgt, np.int64), (B,)))
-        q_ld = 0
-        if noise is not None:
-            noise = np.ascontiguousarray(noise, dtype=np.float32)
-            if noise.ndim != 3 or noise.shape[0] != B or noise.shape[1] != int(self.cfg["inter_channels"]):
-                raise ValueError("noise must be float32 [B, inter_channels, >= frames]")
-            q_ld = noise.shape[2]
+        noise, q_ld = _noise(noise, B, int(self.cfg["inter_channels"]))
         frames = np.zeros(B, np.int64)
         cap = self.convert_frames(lengths) if from_wav else lengths
         fn = self.lib.vtts_convert if from_wav else self.lib.vtts_convert_spec
@@ -516,18 +548,12 @@ class Engine:
         """Re-voices clips of speaker `sid_src` as speaker `sid_tgt` (vtts_convert).  wav: float32 [B, L] (or [L]) in [-1, 1],
         `lengths` the valid samples per row (default: all).  Returns (float32 [B, hop * max(frames)], frames [B]); row b holds
         hop * frames[b] samples.  noise: optional eps [B, inter_channels, >= frames] of the posterior sample."""
-        wav = np.ascontiguousarray(wav, dtype=np.float32)
-        if wav.ndim == 1:
-            wav = wav[None, :]
-        lengths = np.full(wav.shape[0], wav.shape[1], np.int64) if lengths is None else lengths
+        wav, lengths = _batch(wav, lengths, 2)
         return self._convert(True, wav, lengths, wav.shape[1], sid_src, sid_tgt, noise_scale, noise, seed)
 
     def convert_spec(self, spec, sid_src, sid_tgt, lengths=None, noise_scale=1.0, noise=None, seed=0):
         """Same from the posterior encoder's input features (the reference's `y`): float32 [B, spec_channels, T]."""
-        spec = np.ascontiguousarray(spec, dtype=np.float32)
-        if spec.ndim == 2:
-            spec = spec[None]
-        lengths = np.full(spec.shape[0], spec.shape[2], np.int64) if lengths is None else lengths
+        spec, lengths = _batch(spec, lengths, 3)
         return self._convert(False, spec, lengths, spec.shape[2], sid_src, sid_tgt, noise_scale, noise, seed)
 
     def reserve_convert(self, max_frames=1024, batch=1):
@@ -546,22 +572,16 @@ class Engine:
     def speaker_embedding(self, wav, lengths=None):
         """The QuickVC target embedding g of each clip (vtts_speaker_embedding): wav float32 [B, L] (or [L]) in [-1, 1] at the
         model's sampling rate, `lengths` the valid samples per row (default: all).  Returns float32 [B, gin_channels]."""
-        wav = np.ascontiguousarray(wav, dtype=np.float32)
-        if wav.ndim == 1:
-            wav = wav[None, :]
+        wav, lengths = _batch(wav, lengths, 2)
         B = wav.shape[0]
-        lengths = np.ascontiguousarray(np.full(B, wav.shape[1]) if lengths is None else lengths, dtype=np.int64).reshape(B)
         g = np.zeros((B, int(self.cfg["gin_channels"])), np.float32)
         self._check(self.lib.vtts_speaker_embedding(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], _ptr(g)))
         return g
 
     def speaker_embedding_mel(self, mel, lengths=None):
         """Same from log-mel rows (mel_spectrogram_torch's output): float32 [B, n_mel_channels, T] (or [n_mel_channels, T])."""
-        mel = np.ascontiguousarray(mel, dtype=np.float32)
-        if mel.ndim == 2:
-            mel = mel[None]
+        mel, lengths = _batch(mel, lengths, 3)
         B = mel.shape[0]
-        lengths = np.ascontiguousarray(np.full(B, mel.shape[2]) if lengths is None else lengths, dtype=np.int64).reshape(B)
         g = np.zeros((B, int(self.cfg["gin_channels"])), np.float32)
         self._check(self.lib.vtts_speaker_embedding_mel(self.h, _ptr(mel), _ptr(lengths), B, mel.shape[2], _ptr(g)))
         return g
@@ -580,24 +600,10 @@ class Engine:
         g: [gin_channels] (one target for every clip) or [B, gin_channels] (speaker_embedding's output).  noise: None
         (Philox from `seed`) or [B, inter_channels, >= max T] standing in for torch.randn_like.  Returns (wav float32
         [B, hop * max T], zeros past each clip's end; frames int64 [B])."""
-        if isinstance(units, (list, tuple)):
-            clips = [np.asarray(u, np.float32) for u in units]
-            lengths = np.array([u.shape[0] for u in clips], np.int64)
-            batch = np.zeros((len(clips), int(lengths.max()), 768), np.float32)
-            for b, u in enumerate(clips):
-                batch[b, :u.shape[0]] = u
-            units = batch
-        units = np.ascontiguousarray(units, dtype=np.float32)
-        if units.ndim == 2:
-            units = units[None]
+        units, lengths = _batch(units, lengths, 3, t_axis=1, ragged=True)
         B, T = units.shape[0], units.shape[1]
-        lengths = np.ascontiguousarray(np.full(B, T) if lengths is None else lengths, dtype=np.int64).reshape(B)
-        G = int(self.cfg["gin_channels"])
-        g = np.ascontiguousarray(np.broadcast_to(np.asarray(g, np.float32).reshape(-1, G), (B, G)), dtype=np.float32)
-        ld = 0
-        if noise is not None:
-            noise = np.ascontiguousarray(noise, dtype=np.float32)
-            ld = noise.shape[2]
+        g = _per_item(g, B, int(self.cfg["gin_channels"]))
+        noise, ld = _noise(noise, B, int(self.cfg["inter_channels"]))
         wav = np.zeros((B, max(1, int(lengths.max())) * self.hop), np.float32)
         frames = np.zeros(B, np.int64)
         self._check(self.lib.vtts_quickvc_convert(self.h, _ptr(units), _ptr(lengths), B, T, _ptr(g), float(noise_scale), _ptr(noise),
@@ -612,26 +618,10 @@ class Engine:
         return int(max_frames)
 
     # ---- ContentVec (vc/contentvec.py) and conversion from source waveforms; cfg["contentvec"] is its shape
-    @staticmethod
-    def _clips(wav, lengths):
-        if isinstance(wav, (list, tuple)):
-            clips = [np.asarray(w, np.float32).reshape(-1) for w in wav]
-            lengths = np.array([w.size for w in clips], np.int64)
-            batch = np.zeros((len(clips), int(lengths.max())), np.float32)
-            for b, w in enumerate(clips):
-                batch[b, :w.size] = w
-            wav = batch
-        wav = np.ascontiguousarray(wav, dtype=np.float32)
-        if wav.ndim == 1:
-            wav = wav[None]
-        B = wav.shape[0]
-        lengths = np.ascontiguousarray(np.full(B, wav.shape[1]) if lengths is None else lengths, dtype=np.int64).reshape(B)
-        return wav, lengths
-
     def content_units(self, wav, lengths=None):
         """ContentVec units of 16 kHz sources (vtts_content_units): wav [L], [B, L] with `lengths`, or a list of ragged clips.
         Returns (units float32 [B, max T, hidden], zeros past each clip's end; frames int64 [B])."""
-        wav, lengths = self._clips(wav, lengths)
+        wav, lengths = _batch(wav, lengths, 2, ragged=True)
         B = wav.shape[0]
         T = max(1, max(_config.contentvec_frames(int(n), self.cfg.get("contentvec")) for n in lengths))
         units = np.zeros((B, T, int((self.cfg.get("contentvec") or _config.contentvec_config())["cv_hidden"])), np.float32)
@@ -642,15 +632,11 @@ class Engine:
     def quickvc_convert_wav(self, wav, g, lengths=None, noise_scale=1.0, noise=None, seed=0):
         """Source waveforms -> waveforms in the voice of g in one call (vtts_quickvc_convert_wav): content_units, then
         quickvc_convert, without the units leaving the GPU.  Arguments as those two.  Returns (wav [B, hop * max T], frames)."""
-        wav, lengths = self._clips(wav, lengths)
+        wav, lengths = _batch(wav, lengths, 2, ragged=True)
         B = wav.shape[0]
         T = max(1, max(_config.contentvec_frames(int(n), self.cfg.get("contentvec")) for n in lengths))
-        G = int(self.cfg["gin_channels"])
-        g = np.ascontiguousarray(np.broadcast_to(np.asarray(g, np.float32).reshape(-1, G), (B, G)), dtype=np.float32)
-        ld = 0
-        if noise is not None:
-            noise = np.ascontiguousarray(noise, dtype=np.float32)
-            ld = noise.shape[2]
+        g = _per_item(g, B, int(self.cfg["gin_channels"]))
+        noise, ld = _noise(noise, B, int(self.cfg["inter_channels"]))
         out = np.zeros((B, T * self.hop), np.float32)
         frames = np.zeros(B, np.int64)
         self._check(self.lib.vtts_quickvc_convert_wav(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], _ptr(g), float(noise_scale),
@@ -674,14 +660,7 @@ class Engine:
         lengths = np.ascontiguousarray(np.broadcast_to(np.asarray(lengths, np.int64), (B,)))
         sid = np.ascontiguousarray(np.broadcast_to(np.asarray(0 if sid is None else sid, np.int64), (B,)))
         ld = x.shape[-1]
-        x_lengths = np.full(B, ld, np.int64) if x_lengths is None else \
-            np.ascontiguousarray(np.broadcast_to(np.asarray(x_lengths, np.int64), (B,)))
-        q_ld = 0
-        if noise is not None:
-            noise = np.ascontiguousarray(noise, dtype=np.float32)
-            if noise.ndim != 3 or noise.shape[0] != B or noise.shape[1] != int(self.cfg["inter_channels"]):
-                raise ValueError("noise must be float32 [B, inter_channels, >= frames]")
-            q_ld = noise.shape[2]
+        noise, q_ld = _noise(noise, B, int(self.cfg["inter_channels"]))
         cap = self.convert_frames(x_lengths) if from_wav else x_lengths
         max_f = max(1, int(np.max(cap)))
         dur = np.zeros((B, t_max), np.int32)
@@ -699,16 +678,12 @@ class Engine:
         [B, t_max] -- frames per token, 0 past lengths[b]; frames int64 [B]; token_of_frame int32 [B, max frames], -1 past
         frames[b]; score float32 [B], the best path's log-likelihood).  noise: optional eps [B, inter_channels, >= frames] of
         the posterior sample, else Philox(seed); noise_scale 1 is the reference's forward, 0 the posterior mean."""
-        wav = np.ascontiguousarray(wav, dtype=np.float32)
-        if wav.ndim == 1:
-            wav = wav[None, :]
+        wav, wav_lengths = _batch(wav, wav_lengths, 2)
         return self._align(True, ids, lengths, sid, wav, wav_lengths, noise_scale, noise, seed)
 
     def align_spec(self, ids, lengths, sid, spec, spec_lengths=None, noise_scale=1.0, noise=None, seed=0):
         """Same from the posterior encoder's input features (the reference's `y`): float32 [B, spec_channels, T]."""
-        spec = np.ascontiguousarray(spec, dtype=np.float32)
-        if spec.ndim == 2:
-            spec = spec[None]
+        spec, spec_lengths = _batch(spec, spec_lengths, 3)
         return self._align(False, ids, lengths, sid, spec, spec_lengths, noise_scale, noise, seed)
 
     def reserve_align(self, max_tokens=256, max_frames=1024, batch=1):
