@@ -191,6 +191,10 @@ int vtts_timeline(vtts_handle h, int enable, unsigned long long* out, size_t max
  * has frames, 8 rows between consecutive slices) and "spk_g". */
 int vtts_debug_flags(vtts_handle h, int flags);
 int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floats, size_t* n_out);
+/* Bytes of device memory and of pinned host memory this process holds through the library right now, over every handle and
+ * the handle-free calls.  vtts_destroy gives back everything its handle allocated, so the pair returns to its value from
+ * before vtts_create. */
+int vtts_debug_live_bytes(uint64_t* device_bytes, uint64_t* pinned_bytes);
 /* Unit-test hook for the relative-position attention kernels (attentions.py:165-196): ONE attention launch of layer
  * "enc.<i>" or "flow.<f>.tr" through the engine's own launch code, on host tensors.
  *   B, lens          utterances, packed as the engine packs them: utterance b starts at row offs[b], SEQ_GAP (8) rows between

@@ -29,6 +29,7 @@
 #include "vc.cuh"
 #include "spk.cuh"
 #include "contentvec.cuh"
+#include "owned.cuh"
 
 using namespace vtts;
 
@@ -111,12 +112,6 @@ struct RbW {
   std::vector<TcW> t1, t2;
 };
 
-template <typename T>
-struct Buf {
-  T* p = nullptr;
-  size_t cap = 0;
-};
-
 struct Err {
   int code;
   std::string msg;
@@ -140,9 +135,10 @@ struct Err {
 }  // namespace
 
 struct vtts_engine {
+  // Members are destroyed in reverse order: the stream, declared first, goes last, and the graph execs go before the events.
+  Stream stream;
   vtts_config cfg{};
   int device = 0;
-  cudaStream_t stream = nullptr;
   std::mutex mu;
   // The two-phase API (vtts_durations -> vtts_synthesize / vtts_flow) keeps per-handle state between two calls.  A thread
   // that has run vtts_durations owns the handle until its vtts_synthesize / vtts_flow has succeeded (or failed for good);
@@ -153,7 +149,7 @@ struct vtts_engine {
   std::string err;
   uint64_t launches = 0;
 
-  float* d_blob = nullptr;
+  Buf<float> d_blob;
   size_t blob_floats = 0;
   std::unordered_map<std::string, Tensor> tensors;
 
@@ -184,7 +180,7 @@ struct vtts_engine {
   TcBatch tc_batch;                         // launch_tc's parameter block (calls on one handle are serialised by `mu`)
   double tc_prof_flops = 0.0;
   uint64_t tc_prof_launches = 0;
-  std::vector<cudaEvent_t> tc_prof_ev;
+  std::vector<Event> tc_prof_ev;
   size_t tc_prof_used = 0;
 
   // ---- per-call state
@@ -242,9 +238,9 @@ struct vtts_engine {
     set_frame_shape();
   }
   bool read_published_lengths() {       // what frame_offsets_kernel wrote into mapped host memory; false: not there (yet)
-    if (!h_map || h_map[0] != call_seq) return false;
-    h_frm_len.assign(h_map + 1, h_map + 1 + B);
-    h_frm_off.assign(h_map + 1 + B, h_map + 1 + 2 * B + 1);
+    if (!map.p || map.p[0] != call_seq) return false;
+    h_frm_len.assign(map.p + 1, map.p + 1 + B);
+    h_frm_off.assign(map.p + 1 + B, map.p + 1 + 2 * B + 1);
     return true;
   }
   int eps_dp_ld = 0;                 // row pitch of the duration-predictor noise the phase-1 kernels read
@@ -302,21 +298,23 @@ struct vtts_engine {
   std::vector<std::vector<Buf<float>>> d_xj, d_tmp;
   // per-launch profiling of the conv kernel family (bench.py roofline): event pairs around each launch
   bool profiling = false;
-  std::vector<cudaEvent_t> prof_ev;
+  std::vector<Event> prof_ev;
   size_t prof_used = 0;
   double prof_flops = 0.0;
   uint64_t prof_launches = 0;
+  Buf<unsigned long long> d_tl;                  // vtts_timeline's counter and (source line, ns) pairs
   Buf<float> d_zp_dbg;                           // copy of z_p kept when debug_flags & 1
   int debug_flags = 0;
-  Buf<char> h_pin, h_pin_in, h_pin_len, h_pin_z;  // pinned staging (host): outputs, phase-1 inputs, lengths, noise_z
+  PinnedBuf<char> h_pin, h_pin_in, h_pin_len, h_pin_z;  // pinned staging (host): outputs, phase-1 inputs, lengths, noise_z
   Buf<float> d_prm;                              // per-call scalars (see kernels.cuh prm_seed)
-  int* h_map = nullptr;                          // mapped pinned host memory: [0] sequence flag, lengths, offsets
-  int* d_map = nullptr;                          // its device alias
-  size_t map_cap = 0;
+  MappedBuf<int> map;                            // mapped pinned host memory: [0] sequence flag, lengths, offsets
   int call_seq = 0;
   bool use_poll = true;
+  Event ev[8];
+  Stream side[3];                          // branch streams of the decoder's independent resblock chains (forked / joined with events)
+  Event ev_fork, ev_join[3];
   // CUDA graphs: a call shape seen before is captured once and replayed (launch-bound at batch 1)
-  struct GraphEntry { cudaGraphExec_t exec = nullptr; uint64_t gen = 0; uint64_t used = 0; uint64_t nlaunch = 0; int seen = 0; };
+  struct GraphEntry { GraphExec exec; uint64_t gen = 0; uint64_t used = 0; uint64_t nlaunch = 0; int seen = 0; };
   std::map<std::vector<long long>, GraphEntry> graphs;
   uint64_t ws_gen = 0, graph_clock = 0, graph_replays = 0;
   bool capture_on_first = true;
@@ -332,9 +330,6 @@ struct vtts_engine {
     if (log_conv) conv_log.push_back(r);
   }
   int tc_cluster_cap[2][3] = {{0, 0, 0}, {0, 0, 0}};   // co-resident clusters of 2/4/8 conv_tc CTAs, [BN 64/128][log2(S)-1]   // multicast measured slower (see DESIGN.md 4.2)   // tuning knobs (env VTTS_CONV_MAXS / _TARGET / _MAXG)
-  cudaEvent_t ev[8] = {};
-  cudaStream_t side[3] = {};               // branch streams of the decoder's independent resblock chains (forked / joined with events)
-  cudaEvent_t ev_fork = nullptr, ev_join[3] = {};
   int attn_tc_mode = 1;                    // wgmma attention where the qkv conv runs on tensor cores: 0 never, 1 when throughput bound, 2 always
   int mrf_heavy_first = 1;
   int mrf_branch = 0;                      // VTTS_MRF_BRANCH=1: one stream per resblock chain (measured slower: 1.74 vs 1.62 ms)
@@ -342,34 +337,17 @@ struct vtts_engine {
   bool ev_valid = false;
 
   // -------------------------------------------------------------------------------------------
-  template <typename T>
-  T* ensure(Buf<T>& b, size_t n) {
+  template <typename T, Mem M>
+  T* ensure(Buf<T, M>& b, size_t n) {
     if (n > b.cap) {
-      REQUIRE(!capturing, VTTS_ERR_STATE, "workspace growth during graph capture");
-      if (b.p) CK(cudaFree(b.p));
-      size_t cap = n + n / 4 + 256;
-      CK(cudaMalloc(&b.p, cap * sizeof(T)));
-      b.cap = cap;
+      REQUIRE(!capturing, VTTS_ERR_STATE, M == Mem::Device ? "workspace growth during graph capture" : "staging growth during graph capture");
+      if (M == Mem::Pinned && b.p) CK(cudaStreamSynchronize(stream));   // copies staged through the old buffer may still be in flight
+      CK(b.grow(n));
       ++ws_gen;                                // captured graphs hold the old pointers
     }
     return b.p;
   }
-  char* ensure_pinned(Buf<char>& hb, size_t n) {
-    if (n > hb.cap) {
-      REQUIRE(!capturing, VTTS_ERR_STATE, "staging growth during graph capture");
-      if (hb.p) {
-        CK(cudaStreamSynchronize(stream));   // copies staged through the old buffer may still be in flight
-        CK(cudaFreeHost(hb.p));
-        hb.p = nullptr;
-      }
-      size_t cap = n + n / 4 + 4096;
-      CK(cudaMallocHost(&hb.p, cap));
-      hb.cap = cap;
-      ++ws_gen;
-    }
-    return hb.p;
-  }
-  char* ensure_pinned(size_t n) { return ensure_pinned(h_pin, n); }
+  char* ensure_pinned(size_t n) { return ensure(h_pin, n); }
 
   // Runs `enqueue` (which only enqueues work on `stream`) eagerly the first time a shape key is seen -- that run also
   // performs every workspace growth -- and right behind it records the same work into a CUDA graph (capture only, no second
@@ -393,13 +371,12 @@ struct vtts_engine {
       if (graphs.size() >= GRAPH_CACHE_MAX) {       // evict the least recently used entry before inserting
         auto old = graphs.begin();
         for (auto k = graphs.begin(); k != graphs.end(); ++k) if (k->second.used < old->second.used) old = k;
-        if (old->second.exec) cudaGraphExecDestroy(old->second.exec);
         graphs.erase(old);
       }
       it = graphs.emplace(key, GraphEntry{}).first;
     }
     GraphEntry& g = it->second;
-    if (g.exec && g.gen != ws_gen) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; g.seen = 0; }
+    if (g.exec && g.gen != ws_gen) { g.exec.reset(); g.seen = 0; }
     g.used = ++graph_clock;
     if (g.exec) {
       CK(cudaGraphLaunch(g.exec, stream));
@@ -414,24 +391,20 @@ struct vtts_engine {
       if (!capture_on_first) return;
     }
     const uint64_t gen0 = ws_gen, l0 = launches;      // ... then capture
-    cudaGraph_t graph = nullptr;
+    Graph graph;
     CK(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
     capturing = true;
     try {
       enqueue();
     } catch (...) {
       capturing = false;
-      cudaStreamEndCapture(stream, &graph);
-      if (graph) cudaGraphDestroy(graph);
+      cudaStreamEndCapture(stream, graph.out());
       throw;
     }
     capturing = false;
-    CK(cudaStreamEndCapture(stream, &graph));
-    cudaGraphExec_t exec = nullptr;
-    cudaError_t e = cudaGraphInstantiate(&exec, graph, 0);
-    cudaGraphDestroy(graph);
+    CK(cudaStreamEndCapture(stream, graph.out()));
+    cudaError_t e = cudaGraphInstantiate(g.exec.out(), graph, 0);
     if (e != cudaSuccess) throw Err{VTTS_ERR_CUDA, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e)};
-    g.exec = exec;
     g.gen = gen0;
     g.nlaunch = launches - l0;
     if (first) { launches = l0; return; }       // (the eager run above already did the work)
@@ -600,7 +573,7 @@ struct vtts_engine {
         memcpy(pin + ((size_t)b * I + ch) * maxFrm, noise + ((size_t)b * I + ch) * ld, (size_t)cols[b] * sizeof(float));
   }
   void stage_noise_z(const float* noise_z, int z_ld) {
-    float* pin = reinterpret_cast<float*>(ensure_pinned(h_pin_z, (size_t)B * cfg.inter_channels * maxFrm * sizeof(float)));
+    float* pin = reinterpret_cast<float*>(ensure(h_pin_z, (size_t)B * cfg.inter_channels * maxFrm * sizeof(float)));
     stage_noise(pin, noise_z, z_ld, std::vector<int>(B, std::min(z_ld, maxFrm)));
   }
   void decode(float* z, const int* fl, const int* fo, bool planes_ready = false, bool pz_ready = false);
@@ -630,7 +603,7 @@ struct vtts_engine {
   int q_R = 0, spec_pad = 0, vc_pad = 0, vc_wld = 0;
   Buf<int> d_vint;                                 // [clip_len B][sid 2B]
   Buf<float> d_vprm, d_vin, d_vlin, d_vfeat, d_vstats, d_vcsrc, d_vnoise, d_vz_dbg, d_vzp_dbg, d_qg;
-  Buf<char> h_pin_vc;
+  PinnedBuf<char> h_pin_vc;
   // what a call on recordings stages as its input: waveforms, spectrogram (or log-mel) rows, QuickVC's content-unit rows, or
   // nothing (ContentVec writes the unit rows on the device); the last two also stage QuickVC's target voice g
   enum ClipIn { IN_WAV, IN_SPEC, IN_UNITS, IN_NONE };
@@ -673,7 +646,7 @@ struct vtts_engine {
   struct CvPlan { int maxS = 0, tot0 = 0, MC = 0, nint = 0; std::vector<int> maxL; std::vector<int> h; } cvp;
   Buf<int> d_cvi;
   Buf<float> d_cvzero, d_cvwav, d_cvps, d_cvpq, d_cvl[2], d_cvx, d_cvx1, d_cvy, d_cvqkv, d_cvao, d_cvff, d_cvu, d_cvdbg;
-  Buf<char> h_pin_cv;
+  PinnedBuf<char> h_pin_cv;
   void bind_contentvec();
   std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
   void cv_enqueue(float* out, const int* out_offs);
@@ -1214,8 +1187,8 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   if (profiling) {
     if (tc_prof_used + 2 > tc_prof_ev.size()) {
       tc_prof_ev.resize(tc_prof_used + 2);
-      CK(cudaEventCreate(&tc_prof_ev[tc_prof_used]));
-      CK(cudaEventCreate(&tc_prof_ev[tc_prof_used + 1]));
+      CK(cudaEventCreate(tc_prof_ev[tc_prof_used].out()));
+      CK(cudaEventCreate(tc_prof_ev[tc_prof_used + 1].out()));
     }
     for (const TcSpec& q : ps)
       for (int b = 0; b < nB; ++b)
@@ -1568,26 +1541,25 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     for (int b = 0; b < B; ++b) group_tiles += (long)nk * ((v_frm_len[b] * rm + TC_BM - 1) / TC_BM) * ((ch + 63) / 64);
     const bool branch = mrf_branch && !profiling && nk > 1 && nk - 1 <= 3 && group_tiles <= n_sm;
     if (branch) {
-      struct Restore { cudaStream_t& s; cudaStream_t v; ~Restore() { s = v; } } restore{stream, stream};
-      cudaStream_t main_stream = stream;
-      CK(cudaEventRecord(ev_fork, main_stream));
-      for (int j = nk - 1; j >= 0; --j) {              // largest kernel size first
-        if (j > 0) {
-          CK(cudaStreamWaitEvent(side[j - 1], ev_fork, 0));
-          stream = side[j - 1];
-        } else {
-          stream = main_stream;
-        }
+      auto chain = [&](int j) {
         for (int d = 0; d < nd; ++d) {
           TcSpec a, b2;
           rb_pair(j, d, a, b2);
           launch_tc({a}, rm, fl, fo, maxFrm, B);
           launch_tc({b2}, rm, fl, fo, maxFrm, B);
         }
-        if (j > 0) CK(cudaEventRecord(ev_join[j - 1], stream));
+      };
+      CK(cudaEventRecord(ev_fork, stream));
+      for (int j = nk - 1; j > 0; --j) {              // largest kernel size first; chain 0 on the main stream
+        CK(cudaStreamWaitEvent(side[j - 1], ev_fork, 0));
+        // the launch code enqueues on `stream`: swap the two owners for this chain and back on every exit
+        struct Swap { Stream &a, &b; ~Swap() { std::swap(a, b); } } back{stream, side[j - 1]};
+        std::swap(stream, side[j - 1]);
+        chain(j);
+        CK(cudaEventRecord(ev_join[j - 1], stream));
       }
-      stream = main_stream;
-      for (int j = 1; j < nk; ++j) CK(cudaStreamWaitEvent(main_stream, ev_join[j - 1], 0));
+      chain(0);
+      for (int j = 1; j < nk; ++j) CK(cudaStreamWaitEvent(stream, ev_join[j - 1], 0));
     } else {
       for (int d = 0; d < nd; ++d) {
         std::vector<TcSpec> p1(nk), p2(nk);
@@ -1691,8 +1663,8 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
   if (profiling) {
     if (prof_used + 2 > prof_ev.size()) {
       prof_ev.resize(prof_used + 2);
-      CK(cudaEventCreate(&prof_ev[prof_used]));
-      CK(cudaEventCreate(&prof_ev[prof_used + 1]));
+      CK(cudaEventCreate(prof_ev[prof_used].out()));
+      CK(cudaEventCreate(prof_ev[prof_used + 1].out()));
     }
     for (const ConvP& q : ps)
       for (int b = 0; b < nB; ++b)
@@ -1894,12 +1866,12 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   unsigned int* dctr = reinterpret_cast<unsigned int*>(ensure(d_done_ctr, 4));
   int* fl_real = ensure(d_frm_len_real, B);
   klaunch(duration_kernel, dim3(B), dim3(256), (size_t)(0), zlast, dp_ea, 0, 2, prm, wceil, cum, fl, tl, to, fo, B,
-          (volatile int*)(use_poll ? d_map : nullptr), dctr, fl_real);
+          (volatile int*)(use_poll ? map.d : nullptr), dctr, fl_real);
   CK(cudaGetLastError());
   ++launches;
   if (!capturing) CK(cudaEventRecord(ev[3], stream));
   if (!use_poll) {
-    int* p_len = reinterpret_cast<int*>(ensure_pinned(h_pin_len, (size_t)(2 * B + 2) * sizeof(int)));
+    int* p_len = reinterpret_cast<int*>(ensure(h_pin_len, (size_t)(2 * B + 2) * sizeof(int)));
     CK(cudaMemcpyAsync(p_len, fl, B * sizeof(int), cudaMemcpyDeviceToHost, stream));
     CK(cudaMemcpyAsync(p_len + B, fo, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
   }
@@ -1996,7 +1968,7 @@ vtts_engine::P1Pin vtts_engine::p1_layout(bool eps) {
   const size_t T = (size_t)Ttok;
   const size_t bytes = (size_t)(3 * B + 1) * sizeof(int) + T * sizeof(int) + 8 * sizeof(float) +
                        (eps ? (size_t)B * 2 * maxTok * sizeof(float) : 0) + 64;
-  char* pin = ensure_pinned(h_pin_in, bytes);
+  char* pin = ensure(h_pin_in, bytes);
   P1Pin pp;
   pp.len = reinterpret_cast<int*>(pin);
   pp.off = pp.len + B;
@@ -2032,13 +2004,11 @@ void vtts_engine::stage1(const P1Pin& pp, int t_max, const float* noise_dp_host)
   put_scalars(pp.prm, 8, scales, 3, seed);
   if (use_poll) {
     const size_t need = (size_t)(2 * B + 4);
-    if (need > map_cap) {
+    if (need > map.cap) {
       REQUIRE(!capturing, VTTS_ERR_STATE, "mapped buffer growth during capture");
-      if (h_map) { CK(cudaStreamSynchronize(stream)); CK(cudaFreeHost(h_map)); h_map = nullptr; }
-      map_cap = need + 256;
-      CK(cudaHostAlloc(reinterpret_cast<void**>(&h_map), map_cap * sizeof(int), cudaHostAllocMapped));
-      CK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_map), h_map, 0));
-      h_map[0] = 0;
+      if (map.p) CK(cudaStreamSynchronize(stream));
+      CK(map.alloc(need + 256));
+      map.p[0] = 0;
       ++ws_gen;
     }
     call_seq = (call_seq % 1000000) + 1;
@@ -2055,7 +2025,7 @@ void vtts_engine::stage1(const P1Pin& pp, int t_max, const float* noise_dp_host)
 void vtts_engine::finish1() {
   if (use_poll) {
     // spin on the flag the last phase-1 kernel writes into mapped host memory (bounded; then fall back to a sync)
-    volatile int* flag = h_map;
+    volatile int* flag = map.p;
     bool seen = false;
     for (long spin = 0; spin < 40000000L; ++spin) {
       if (*flag == call_seq) { seen = true; break; }
@@ -2065,8 +2035,8 @@ void vtts_engine::finish1() {
       CK(cudaStreamSynchronize(stream));
       REQUIRE(*flag == call_seq, VTTS_ERR_CUDA, "phase 1 finished without publishing the utterance lengths");
     }
-    h_frm_len.assign(h_map + 1, h_map + 1 + B);
-    h_frm_off.assign(h_map + 1 + B, h_map + 1 + 2 * B + 1);
+    h_frm_len.assign(map.p + 1, map.p + 1 + B);
+    h_frm_off.assign(map.p + 1 + B, map.p + 1 + 2 * B + 1);
     set_frame_shape();
     have_durations = true;
     return;
@@ -2370,7 +2340,7 @@ vtts_engine::VcPin vtts_engine::vc_layout(ClipIn in, bool eps) {
   const size_t ne = eps ? (size_t)B * c.inter_channels * maxFrm : 0;
   const size_t ints = (size_t)(5 * B + 1) * sizeof(int);
   const size_t head = (ints + 63) / 64 * 64;
-  char* pin = ensure_pinned(h_pin_vc, head + (16 + nin + ng + ne) * sizeof(float) + 64);
+  char* pin = ensure(h_pin_vc, head + (16 + nin + ng + ne) * sizeof(float) + 64);
   VcPin pp;
   pp.frm_len = reinterpret_cast<int*>(pin);
   pp.frm_off = pp.frm_len + B;
@@ -2765,7 +2735,7 @@ std::vector<int> vtts_engine::cv_stage(const float* wav, const int64_t* lengths,
   cvp.tot0 = (B == 1 || !use_buckets) ? std::max(off0, use_buckets ? padded(cvp.maxL[0]) : 0) : (off0 + 65535) / 65536 * 65536;
   const size_t head = ((size_t)cvp.nint * sizeof(int) + 63) / 64 * 64;
   const size_t nsamp = (size_t)cvp.tot0 * s0 + K0;
-  char* pin = ensure_pinned(h_pin_cv, head + nsamp * sizeof(float) + 64);
+  char* pin = ensure(h_pin_cv, head + nsamp * sizeof(float) + 64);
   memcpy(pin, h.data(), (size_t)(2 * NL + 1) * B * sizeof(int));
   float* ps = reinterpret_cast<float*>(pin + head);
   for (int b = 0; b < B; ++b) {
@@ -3583,20 +3553,20 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
                 h->tc_cluster_cap[0][2], h->tc_cluster_cap[1][0], h->tc_cluster_cap[1][1], h->tc_cluster_cap[1][2]);
     }
     CK(cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device));
-    CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    for (auto& st : h->side) CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-    for (auto& e : h->ev_join) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    for (auto& e : h->ev) CK(cudaEventCreate(&e));
+    CK(cudaStreamCreateWithFlags(h->stream.out(), cudaStreamNonBlocking));
+    for (auto& st : h->side) CK(cudaStreamCreateWithFlags(st.out(), cudaStreamNonBlocking));
+    CK(cudaEventCreateWithFlags(h->ev_fork.out(), cudaEventDisableTiming));
+    for (auto& e : h->ev_join) CK(cudaEventCreateWithFlags(e.out(), cudaEventDisableTiming));
+    for (auto& e : h->ev) CK(cudaEventCreate(e.out()));
     h->blob_floats = blob_floats;
-    CK(cudaMalloc(&h->d_blob, blob_floats * sizeof(float)));
-    CK(cudaMemcpyAsync(h->d_blob, blob, blob_floats * sizeof(float), blob_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+    CK(h->d_blob.alloc(blob_floats));
+    CK(cudaMemcpyAsync(h->d_blob.p, blob, blob_floats * sizeof(float), blob_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
     std::istringstream is(manifest);
     std::string name;
     unsigned long long off, n;
     while (is >> name >> off >> n) {
       REQUIRE(off + n <= blob_floats, VTTS_ERR_WEIGHTS, "manifest entry exceeds the blob");
-      h->tensors[name] = Tensor{h->d_blob + off, (size_t)n};
+      h->tensors[name] = Tensor{h->d_blob.p + off, (size_t)n};
     }
     if (const char* e = getenv("VTTS_CONV_MAXS")) h->conv_max_s = std::max(1, atoi(e));
     if (const char* e = getenv("VTTS_CONV_TARGET")) h->conv_target = std::max(1, atoi(e));
@@ -3660,41 +3630,21 @@ void vtts_destroy(vtts_handle h) {
   if (!h) return;
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
-  auto fr = [](void* p) { if (p) cudaFree(p); };
-  fr(h->d_blob);
-  Buf<int>* ib[] = {&h->d_ids, &h->d_tok_len, &h->d_tok_off, &h->d_sid, &h->d_wceil, &h->d_cum, &h->d_frm_len, &h->d_frm_off, &h->d_ftok, &h->d_done_ctr, &h->d_frm_len_real};
-  for (auto* b : ib) fr(b->p);
-  Buf<float>* fb[] = {&h->d_condv, &h->d_x, &h->d_xb, &h->d_qkv, &h->d_ao, &h->d_y, &h->d_ffh, &h->d_stats, &h->d_dA, &h->d_dB, &h->d_dx,
-                      &h->d_h29, &h->d_za, &h->d_zb, &h->d_eps_dp, &h->d_z, &h->d_h, &h->d_h1, &h->d_wx, &h->d_acts, &h->d_skip, &h->d_fqkv,
-                      &h->d_fao, &h->d_fy, &h->d_ffh2, &h->d_eps_z, &h->d_d0, &h->d_post, &h->d_wav};
-  for (auto* b : fb) fr(b->p);
-  Buf<float>* vb[] = {&h->d_vprm, &h->d_vin, &h->d_vlin, &h->d_vfeat, &h->d_vstats, &h->d_vcsrc, &h->d_vnoise, &h->d_vz_dbg, &h->d_vzp_dbg,
-                      &h->d_sx[0], &h->d_sx[1], &h->d_sx[2], &h->d_sh[0], &h->d_sh[1], &h->d_sh[2], &h->d_sg, &h->d_qg,
-                      &h->d_cvzero, &h->d_cvwav, &h->d_cvps, &h->d_cvpq, &h->d_cvl[0], &h->d_cvl[1], &h->d_cvx, &h->d_cvx1, &h->d_cvy,
-                      &h->d_cvqkv, &h->d_cvao, &h->d_cvff, &h->d_cvu, &h->d_cvdbg};
-  for (auto* b : vb) fr(b->p);
-  fr(h->d_vint.p);
-  fr(h->d_sseq.p);
-  fr(h->d_cvi.p);
-  for (auto& b : h->d_stage) fr(b.p);
-  for (auto& v : h->d_xj) for (auto& b : v) fr(b.p);
-  for (auto& v : h->d_tmp) for (auto& b : v) fr(b.p);
-  for (Buf<char>* hb : {&h->h_pin, &h->h_pin_in, &h->h_pin_len, &h->h_pin_z, &h->h_pin_vc, &h->h_pin_cv}) if (hb->p) cudaFreeHost(hb->p);
-  for (auto& kv : h->graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-  fr(h->d_prm.p);
-  fr(h->d_pref.p);
-  fr(h->d_chunk.p);
-  fr(h->d_zp_dbg.p);
-  if (h->h_map) cudaFreeHost(h->h_map);
-  for (auto& e : h->ev) if (e) cudaEventDestroy(e);
-  for (auto& e : h->prof_ev) if (e) cudaEventDestroy(e);
-  for (auto& e : h->tc_prof_ev) if (e) cudaEventDestroy(e);
-  for (auto& b : h->pl_pool) fr(b.p);
-  for (auto& st : h->side) if (st) cudaStreamDestroy(st);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  for (auto& e : h->ev_join) if (e) cudaEventDestroy(e);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  if (h->d_tl.p) {        // a timeline this handle left armed must not point at its buffer once that is freed
+    unsigned long long* cur = nullptr;
+    if (cudaMemcpyFromSymbol(&cur, g_timeline, sizeof(cur)) == cudaSuccess && cur == h->d_tl.p) {
+      cur = nullptr;
+      cudaMemcpyToSymbol(g_timeline, &cur, sizeof(cur));
+    }
+  }
   delete h;
+}
+
+int vtts_debug_live_bytes(uint64_t* device_bytes, uint64_t* pinned_bytes) {
+  if (!device_bytes || !pinned_bytes) return VTTS_ERR_INVALID;
+  *device_bytes = g_live_device_bytes;
+  *pinned_bytes = g_live_pinned_bytes;
+  return VTTS_OK;
 }
 
 static thread_local std::string g_free_err;      // last error of the handle-free entry points (vtts_maximum_path*), per thread
@@ -3725,21 +3675,19 @@ int vtts_maximum_path(const float* neg_cent, const int32_t* t_ys, const int32_t*
       g_free_err = "vtts_maximum_path: lengths must satisfy 0 <= t_x <= t_y <= T_y, t_x <= T_x (utterance " + std::to_string(b) + ")";
       return VTTS_ERR_INVALID;
     }
-  float* dv = nullptr; int *dp = nullptr, *dl = nullptr;
+  Buf<float> dv;
+  Buf<int> dp, dl;
   const size_t n = (size_t)B * T_y * T_x;
   int rc = VTTS_OK;
   cudaError_t e = cudaSetDevice(device);
-  if (e == cudaSuccess) e = cudaMalloc(&dv, n * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&dp, n * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&dl, (size_t)2 * B * sizeof(int));
-  if (e == cudaSuccess) e = cudaMemcpy(dv, neg_cent, n * sizeof(float), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(dl, t_ys, (size_t)B * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(dl + B, t_xs, (size_t)B * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) rc = mas_launch(dv, dl, dl + B, B, T_y, T_x, dp, 0);
-  if (e == cudaSuccess && rc == VTTS_OK) e = cudaMemcpy(path, dp, n * sizeof(int), cudaMemcpyDeviceToHost);
-  if (dv) cudaFree(dv);
-  if (dp) cudaFree(dp);
-  if (dl) cudaFree(dl);
+  if (e == cudaSuccess) e = dv.alloc(n);
+  if (e == cudaSuccess) e = dp.alloc(n);
+  if (e == cudaSuccess) e = dl.alloc((size_t)2 * B);
+  if (e == cudaSuccess) e = cudaMemcpy(dv.p, neg_cent, n * sizeof(float), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(dl.p, t_ys, (size_t)B * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(dl.p + B, t_xs, (size_t)B * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) rc = mas_launch(dv.p, dl.p, dl.p + B, B, T_y, T_x, dp.p, 0);
+  if (e == cudaSuccess && rc == VTTS_OK) e = cudaMemcpy(path, dp.p, n * sizeof(int), cudaMemcpyDeviceToHost);
   if (e != cudaSuccess) { g_free_err = std::string("vtts_maximum_path: ") + cudaGetErrorString(e); return VTTS_ERR_CUDA; }
   return rc;
 }
@@ -3794,7 +3742,7 @@ int vtts_decode_chunk(vtts_handle h, int f0, int f1, float* wav, int64_t wav_cap
     const int halo = 24;
     const int lo = std::max(0, f0 - halo), hi = std::min(T, f1 + halo);
     int* dc = h->ensure(h->d_chunk, 4);
-    int* pin = reinterpret_cast<int*>(h->ensure_pinned(h->h_pin_len, 64));
+    int* pin = reinterpret_cast<int*>(h->ensure(h->h_pin_len, 64));
     pin[0] = hi - lo; pin[1] = lo; pin[2] = hi;
     CK(cudaMemcpyAsync(dc, pin, 3 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     // the launch helpers size grids and split-K from the host copies of the lengths: point them at the chunk
@@ -3946,18 +3894,17 @@ int vtts_profile_read(vtts_handle h, double* conv_ms, uint64_t* conv_launches, d
 // Timeline: enable -> every kernel's first CTA appends (source line, globaltimer) to a device buffer; read returns pairs.
 int vtts_timeline(vtts_handle h, int enable, unsigned long long* out, size_t max_pairs, size_t* n_out) {
   return guarded(h, [&] {
-    static unsigned long long* d_tl = nullptr;
     CK(cudaStreamSynchronize(h->stream));
     if (enable == 1) {
-      if (!d_tl) CK(cudaMalloc(&d_tl, (1 + 2 * 4000) * 8));
-      CK(cudaMemset(d_tl, 0, (1 + 2 * 4000) * 8));
-      CK(cudaMemcpyToSymbol(g_timeline, &d_tl, sizeof(d_tl)));
+      if (!h->d_tl.p) CK(h->d_tl.alloc(1 + 2 * 4000));
+      CK(cudaMemset(h->d_tl.p, 0, (1 + 2 * 4000) * 8));
+      CK(cudaMemcpyToSymbol(g_timeline, &h->d_tl.p, sizeof(h->d_tl.p)));
     } else if (enable == 0) {
       unsigned long long* z = nullptr;
       CK(cudaMemcpyToSymbol(g_timeline, &z, sizeof(z)));
-    } else if (d_tl && out && n_out) {
+    } else if (h->d_tl.p && out && n_out) {
       std::vector<unsigned long long> hbuf(1 + 2 * 4000);
-      CK(cudaMemcpy(hbuf.data(), d_tl, hbuf.size() * 8, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(hbuf.data(), h->d_tl.p, hbuf.size() * 8, cudaMemcpyDeviceToHost));
       size_t n = std::min<size_t>((size_t)hbuf[0], std::min<size_t>(4000, max_pairs));
       memcpy(out, hbuf.data() + 1, n * 16);
       *n_out = n;
@@ -4049,18 +3996,13 @@ int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav
                                                out_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
 }
 
-// Host copies of a debug hook's arguments on the device (freed on every exit).
-struct DebugBufs {
-  std::vector<void*> p;
-  ~DebugBufs() { for (void* q : p) cudaFree(q); }
-  void* up(const void* src, size_t bytes, cudaStream_t s) {
-    void* d = nullptr;
-    CK(cudaMalloc(&d, std::max<size_t>(bytes, 16)));
-    p.push_back(d);
-    if (src) CK(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, s));
-    return d;
-  }
-};
+// A device copy of a debug hook's host argument, held by `dev` (so freed on every exit).
+static void* upload(std::vector<Buf<char>>& dev, const void* src, size_t bytes, cudaStream_t s) {
+  Buf<char>& d = dev.emplace_back();
+  CK(d.alloc(std::max<size_t>(bytes, 16)));
+  if (src) CK(cudaMemcpyAsync(d.p, src, bytes, cudaMemcpyHostToDevice, s));
+  return d.p;
+}
 
 // Unit-test hook of the attention kernels (include/vtts.h): one launch through launch_attn_tc / launch_attn on host tensors.
 int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* lens, const int* launch_lens, const float* qkv,
@@ -4129,22 +4071,22 @@ int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* len
     }
     REQUIRE(!(use_tc && planes && p_planes != 2), VTTS_ERR_INVALID, "debug_attention: the tensor-core kernel writes 2 output planes");
     // ---- device copies
-    DebugBufs dev;
+    std::vector<Buf<char>> dev;
     cudaStream_t st = h->stream;
     CK(cudaStreamSynchronize(st));
     std::vector<int> lo(2 * B + 3);
     for (int b = 0; b < B; ++b) lo[b] = lens[b];
     for (int b = 0; b <= B; ++b) lo[B + b] = (int)off[b];
     lo[2 * B + 1] = (int)rows; lo[2 * B + 2] = 0;   // all rows as one span (input split)
-    int* dl = static_cast<int*>(dev.up(lo.data(), lo.size() * sizeof(int), st));
+    int* dl = static_cast<int*>(upload(dev, lo.data(), lo.size() * sizeof(int), st));
     const int* dlens = dl;
     const int* doffs = dl + B;
-    const float* dq = static_cast<const float*>(dev.up(qkv, rows * 3 * H * sizeof(float), st));
-    float* dout = static_cast<float*>(dev.up(out, rows * H * sizeof(float), st));   // (the FFMA kernels always write fp32)
+    const float* dq = static_cast<const float*>(upload(dev, qkv, rows * 3 * H * sizeof(float), st));
+    float* dout = static_cast<float*>(upload(dev, out, rows * H * sizeof(float), st));   // (the FFMA kernels always write fp32)
     const size_t pn = rows * H;
     Planes po;
     if (planes) {
-      __nv_bfloat16* dp = static_cast<__nv_bfloat16*>(dev.up(planes, (size_t)p_planes * pn * 2, st));
+      __nv_bfloat16* dp = static_cast<__nv_bfloat16*>(upload(dev, planes, (size_t)p_planes * pn * 2, st));
       po.hi = dp; po.mid = p_planes == 3 ? dp + pn : nullptr; po.lo = dp + (p_planes - 1) * pn; po.C = H; po.rows = (long)rows;
     }
     Planes pq;
@@ -4167,8 +4109,8 @@ int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* len
     if (planes) CK(cudaMemcpy(planes, po.hi, (size_t)p_planes * pn * 2, cudaMemcpyDeviceToHost));
     if (report) *report = h->last_attn;
     if (iters > 0 && ms_out) {
-      cudaEvent_t e0, e1;
-      CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+      Event e0, e1;
+      CK(cudaEventCreate(e0.out())); CK(cudaEventCreate(e1.out()));
       CK(cudaEventRecord(e0, st));
       for (int i = 0; i < iters; ++i) once();
       CK(cudaEventRecord(e1, st));
@@ -4176,7 +4118,6 @@ int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* len
       float ms = 0.f;
       CK(cudaEventElapsedTime(&ms, e0, e1));
       *ms_out = ms / iters;
-      cudaEventDestroy(e0); cudaEventDestroy(e1);
     }
   });
 }
@@ -4298,21 +4239,21 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
     h->h_frm_off.assign(off.begin(), off.end());
     h->v_frm_len = h->h_frm_len;                  // the heuristics see this call's lengths
     // ---- device copies (freed on every exit)
-    DebugBufs dev;
+    std::vector<Buf<char>> dev;
     cudaStream_t st = h->stream;
     CK(cudaStreamSynchronize(st));
     std::vector<int> lo(2 * B + 1);
     for (int b = 0; b < B; ++b) lo[b] = lens[b];
     for (int b = 0; b <= B; ++b) lo[B + b] = (int)off[b];
-    int* dl = static_cast<int*>(dev.up(lo.data(), lo.size() * sizeof(int), st));
+    int* dl = static_cast<int*>(upload(dev, lo.data(), lo.size() * sizeof(int), st));
     const int* dlens = dl;
     const int* doffs = dl + B;
-    float* dy = y ? static_cast<float*>(dev.up(y, y_n * sizeof(float), st)) : nullptr;
-    const float* dres = res ? static_cast<const float*>(dev.up(res, res_n * sizeof(float), st)) : nullptr;
-    __nv_bfloat16* dp = any_planes ? static_cast<__nv_bfloat16*>(dev.up(p_out, (size_t)p_planes * p_n * 2, st)) : nullptr;
+    float* dy = y ? static_cast<float*>(upload(dev, y, y_n * sizeof(float), st)) : nullptr;
+    const float* dres = res ? static_cast<const float*>(upload(dev, res, res_n * sizeof(float), st)) : nullptr;
+    __nv_bfloat16* dp = any_planes ? static_cast<__nv_bfloat16*>(upload(dev, p_out, (size_t)p_planes * p_n * 2, st)) : nullptr;
     __nv_bfloat16 *dp_hi = dp, *dp_mid = (dp && p_planes == 3) ? dp + p_n : nullptr, *dp_lo = dp ? dp + (p_planes - 1) * p_n : nullptr;
     auto cond_of = [&](const vtts_conv_problem& q) {
-      return q.cond ? static_cast<const float*>(dev.up(q.cond, (size_t)B * q.cond_ld * sizeof(float), st)) : nullptr;
+      return q.cond ? static_cast<const float*>(upload(dev, q.cond, (size_t)B * q.cond_ld * sizeof(float), st)) : nullptr;
     };
     if (use_tc) {
       const int Cin = P0.Cin;
@@ -4329,10 +4270,10 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
         const size_t wn = (size_t)q.k * q.Cout * q.Cin;
         TcSpec s;
         s.in = in;
-        s.w.hi = static_cast<const __nv_bfloat16*>(dev.up(q.w_hi, wn * 2, st));
-        s.w.lo = static_cast<const __nv_bfloat16*>(dev.up(q.w_lo, wn * 2, st));
-        if (q.w_mid) s.w.mid = static_cast<const __nv_bfloat16*>(dev.up(q.w_mid, wn * 2, st));
-        s.bias = static_cast<const float*>(dev.up(q.bias, (size_t)q.Cout * sizeof(float), st));
+        s.w.hi = static_cast<const __nv_bfloat16*>(upload(dev, q.w_hi, wn * 2, st));
+        s.w.lo = static_cast<const __nv_bfloat16*>(upload(dev, q.w_lo, wn * 2, st));
+        if (q.w_mid) s.w.mid = static_cast<const __nv_bfloat16*>(upload(dev, q.w_mid, wn * 2, st));
+        s.bias = static_cast<const float*>(upload(dev, q.bias, (size_t)q.Cout * sizeof(float), st));
         s.Cin = q.Cin; s.Cout = q.Cout; s.k = q.k; s.dil = q.dil; s.pad = q.pad;
         s.y = q.y_on ? dy : nullptr; s.ldy = q.ldy; s.yoff = q.yoff;
         s.res = q.res == 1 ? dres : (q.res == 2 ? dy : nullptr); s.ldr = q.ldr; s.roff = q.roff;
@@ -4345,14 +4286,14 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
       }
       h->launch_tc(ps, rmul, dlens, doffs, maxLen, B);
     } else {
-      const float* dx = static_cast<const float*>(dev.up(x, x_n * sizeof(float), st));
+      const float* dx = static_cast<const float*>(upload(dev, x, x_n * sizeof(float), st));
       std::vector<ConvP> ps;
       for (int i = 0; i < n_problems; ++i) {
         const vtts_conv_problem& q = problems[i];
         ConvW W;
         W.Cin = q.Cin; W.Cout = q.Cout; W.k = q.k; W.ldw = (q.Cout + 3) / 4 * 4;
-        W.w = static_cast<const float*>(dev.up(q.w, (size_t)q.k * q.Cin * W.ldw * sizeof(float), st));
-        W.b = static_cast<const float*>(dev.up(q.bias, (size_t)W.ldw * sizeof(float), st));
+        W.w = static_cast<const float*>(upload(dev, q.w, (size_t)q.k * q.Cin * W.ldw * sizeof(float), st));
+        W.b = static_cast<const float*>(upload(dev, q.bias, (size_t)W.ldw * sizeof(float), st));
         ConvP p = mk(W, dx, q.ldx, q.xoff, dy, q.ldy, q.yoff, q.dil, q.pad);
         p.cond = cond_of(q); p.cond_ld = q.cond_ld;
         p.res = q.res == 1 ? dres : (q.res == 2 ? dy : nullptr); p.ldr = q.ldr; p.roff = q.roff;
@@ -4443,79 +4384,77 @@ float vtts_microbench(vtts_handle h, const char* what, int iters) {
     const bool is_tc = strcmp(kind, "tc") == 0;
     REQUIRE(is_tc || strcmp(kind, "ffma") == 0, VTTS_ERR_INVALID, "unknown microbench kind");
     REQUIRE(!is_tc || h->tc, VTTS_ERR_INVALID, "tc microbench needs a precision-1 engine");
-    // save state that the launch helpers read
-    const int B0 = h->B; const std::vector<int> fl0 = h->h_frm_len, tl0 = h->h_tok_len, vf0 = h->v_frm_len, vt0 = h->v_tok_len;
+    struct Saved {       // state the launch helpers read, restored on every exit
+      vtts_engine* h; int B; bool prof; std::vector<int> fl, tl, vf, vt;
+      ~Saved() { h->B = B; h->profiling = prof; h->h_frm_len = fl; h->h_tok_len = tl; h->v_frm_len = vf; h->v_tok_len = vt; h->tc_dbg = nullptr; }
+    } saved{h, h->B, h->profiling, h->h_frm_len, h->h_tok_len, h->v_frm_len, h->v_tok_len};
     h->B = 1; h->h_frm_len.assign(1, rows); h->h_tok_len.assign(1, rows); h->v_frm_len = h->h_frm_len; h->v_tok_len = h->h_tok_len;
-    int* dl = nullptr; int* dof = nullptr; float *x = nullptr, *y = nullptr, *w = nullptr, *bias = nullptr;
-    __nv_bfloat16 *ph = nullptr, *pl = nullptr, *wh = nullptr, *wl = nullptr;
+    Buf<int> dl, dof;
+    Buf<float> x, y, w, bias;
+    Buf<__nv_bfloat16> ph, pl, wh, wl;
     const int ldw = (Cout + 3) / 4 * 4;
-    CK(cudaMalloc(&dl, 8)); CK(cudaMalloc(&dof, 8));
+    CK(dl.alloc(2)); CK(dof.alloc(2));
     const int hl[2] = {rows, rows}, ho[2] = {0, rows};
-    CK(cudaMemcpy(dl, hl, 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dof, ho, 8, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&y, (size_t)rows * Cout * 4)); CK(cudaMalloc(&bias, (size_t)ldw * 4)); CK(cudaMemset(bias, 0, (size_t)ldw * 4));
+    CK(cudaMemcpy(dl.p, hl, 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dof.p, ho, 8, cudaMemcpyHostToDevice));
+    CK(y.alloc((size_t)rows * Cout)); CK(bias.alloc(ldw)); CK(cudaMemset(bias.p, 0, (size_t)ldw * 4));
     if (is_tc) {
-      CK(cudaMalloc(&ph, (size_t)rows * Cin * 2)); CK(cudaMalloc(&pl, (size_t)rows * Cin * 2));
-      CK(cudaMalloc(&wh, (size_t)k * Cout * Cin * 2)); CK(cudaMalloc(&wl, (size_t)k * Cout * Cin * 2));
-      CK(cudaMemset(ph, 0, (size_t)rows * Cin * 2)); CK(cudaMemset(pl, 0, (size_t)rows * Cin * 2));
-      CK(cudaMemset(wh, 0, (size_t)k * Cout * Cin * 2)); CK(cudaMemset(wl, 0, (size_t)k * Cout * Cin * 2));
+      CK(ph.alloc((size_t)rows * Cin)); CK(pl.alloc((size_t)rows * Cin));
+      CK(wh.alloc((size_t)k * Cout * Cin)); CK(wl.alloc((size_t)k * Cout * Cin));
+      CK(cudaMemset(ph.p, 0, (size_t)rows * Cin * 2)); CK(cudaMemset(pl.p, 0, (size_t)rows * Cin * 2));
+      CK(cudaMemset(wh.p, 0, (size_t)k * Cout * Cin * 2)); CK(cudaMemset(wl.p, 0, (size_t)k * Cout * Cin * 2));
     } else {
-      CK(cudaMalloc(&x, (size_t)rows * Cin * 4)); CK(cudaMalloc(&w, (size_t)k * Cin * ldw * 4));
-      CK(cudaMemset(x, 0, (size_t)rows * Cin * 4)); CK(cudaMemset(w, 0, (size_t)k * Cin * ldw * 4));
+      CK(x.alloc((size_t)rows * Cin)); CK(w.alloc((size_t)k * Cin * ldw));
+      CK(cudaMemset(x.p, 0, (size_t)rows * Cin * 4)); CK(cudaMemset(w.p, 0, (size_t)k * Cin * ldw * 4));
     }
     auto once = [&] {
       if (is_tc) {
         TcSpec q;
-        q.in.hi = ph; q.in.lo = pl; q.in.C = Cin; q.in.rows = rows;
-        q.w.hi = wh; q.w.lo = wl; q.bias = bias; q.Cin = Cin; q.Cout = Cout; q.k = k; q.dil = dil; q.pad = dil * (k - 1) / 2;
-        q.y = y; q.ldy = Cout;
-        h->launch_tc({q}, 1, dl, dof, rows, 1);
+        q.in.hi = ph.p; q.in.lo = pl.p; q.in.C = Cin; q.in.rows = rows;
+        q.w.hi = wh.p; q.w.lo = wl.p; q.bias = bias.p; q.Cin = Cin; q.Cout = Cout; q.k = k; q.dil = dil; q.pad = dil * (k - 1) / 2;
+        q.y = y.p; q.ldy = Cout;
+        h->launch_tc({q}, 1, dl.p, dof.p, rows, 1);
       } else {
-        ConvW W; W.w = w; W.b = bias; W.Cin = Cin; W.Cout = Cout; W.k = k; W.ldw = ldw;
-        h->launch_conv({mk(W, x, Cin, 0, y, Cout, 0, dil, dil * (k - 1) / 2)}, 1, dl, dof, rows, 1);
+        ConvW W; W.w = w.p; W.b = bias.p; W.Cin = Cin; W.Cout = Cout; W.k = k; W.ldw = ldw;
+        h->launch_conv({mk(W, x.p, Cin, 0, y.p, Cout, 0, dil, dil * (k - 1) / 2)}, 1, dl.p, dof.p, rows, 1);
       }
     };
-    const bool prof0 = h->profiling; h->profiling = false;
+    h->profiling = false;
     for (int i = 0; i < 3; ++i) once();
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    Event e0, e1;
+    CK(cudaEventCreate(e0.out())); CK(cudaEventCreate(e1.out()));
     // the launches are captured into one CUDA graph so that the host launch path is not what gets timed
-    cudaGraph_t graph = nullptr; cudaGraphExec_t gexec = nullptr;
+    Graph graph;
+    GraphExec gexec;
     CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
     for (int i = 0; i < iters; ++i) once();
-    CK(cudaStreamEndCapture(h->stream, &graph));
-    CK(cudaGraphInstantiate(&gexec, graph, 0));
+    CK(cudaStreamEndCapture(h->stream, graph.out()));
+    CK(cudaGraphInstantiate(gexec.out(), graph, 0));
     CK(cudaGraphLaunch(gexec, h->stream));           // warm
     CK(cudaStreamSynchronize(h->stream));
     CK(cudaEventRecord(e0, h->stream));
     CK(cudaGraphLaunch(gexec, h->stream));
     CK(cudaEventRecord(e1, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    cudaGraphExecDestroy(gexec); cudaGraphDestroy(graph);
     if (is_tc && getenv("VTTS_TC_STAMPS")) {
-      unsigned long long* d = nullptr;
-      CK(cudaMalloc(&d, 16 * 8)); CK(cudaMemset(d, 0, 16 * 8));
-      h->tc_dbg = d;
-      cudaEvent_t a0, a1; CK(cudaEventCreate(&a0)); CK(cudaEventCreate(&a1));
+      Buf<unsigned long long> d;
+      CK(d.alloc(16)); CK(cudaMemset(d.p, 0, 16 * 8));
+      h->tc_dbg = d.p;
+      Event a0, a1; CK(cudaEventCreate(a0.out())); CK(cudaEventCreate(a1.out()));
       CK(cudaEventRecord(a0, h->stream));
       once();
       CK(cudaEventRecord(a1, h->stream));
       CK(cudaStreamSynchronize(h->stream));
       h->tc_dbg = nullptr;
       unsigned long long st[16];
-      CK(cudaMemcpy(st, d, sizeof(st), cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(st, d.p, sizeof(st), cudaMemcpyDeviceToHost));
       float one = 0.f; CK(cudaEventElapsedTime(&one, a0, a1));
       fprintf(stderr, "[tc stamps %s] event %.2f us | entry->setup %.2f | ->first TMA issued %.2f | ->all TMA issued %.2f | ->first full %.2f | ->mma issued %.2f | ->acc ready %.2f | ->epi done %.2f | ->sync %.2f (us since entry)\n",
               what, one * 1e3, (st[1] - st[0]) / 1e3, (st[2] - st[0]) / 1e3, (st[3] - st[0]) / 1e3, (st[4] - st[0]) / 1e3,
               (st[5] - st[0]) / 1e3, (st[6] - st[0]) / 1e3, (st[7] - st[0]) / 1e3, (st[8] - st[0]) / 1e3);
-      cudaFree(d); cudaEventDestroy(a0); cudaEventDestroy(a1);
     }
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, e0, e1));
     result = ms / iters;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    h->profiling = prof0;
-    for (void* p2 : {(void*)dl, (void*)dof, (void*)x, (void*)y, (void*)w, (void*)bias, (void*)ph, (void*)pl, (void*)wh, (void*)wl}) if (p2) cudaFree(p2);
-    h->B = B0; h->h_frm_len = fl0; h->h_tok_len = tl0; h->v_frm_len = vf0; h->v_tok_len = vt0;
   });
   return rc == VTTS_OK ? result : (float)rc;
 }

@@ -55,7 +55,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
-           "vtts_quickvc_convert_wav"]
+           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1}    # vtts_config.model_family
 
@@ -231,6 +231,8 @@ def load_library(build_if_missing=True):
     lib.vtts_content_units.restype = i32
     lib.vtts_quickvc_convert_wav.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_float, vp, i32, C.c_uint64, vp, C.c_int64, vp]
     lib.vtts_quickvc_convert_wav.restype = i32
+    lib.vtts_debug_live_bytes.argtypes = [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    lib.vtts_debug_live_bytes.restype = i32
     _LIB = lib
     return lib
 
@@ -250,6 +252,14 @@ def tc_split_plan(problems, lens, rmul, n_sm, cluster_cap, max_len=None, bn=0, m
     if st != 0:
         raise VttsError(st, "vtts_tc_split_plan: invalid arguments")
     return int(plan[0]), int(plan[1]), [int(s) for s in plan[2:2 + len(problems)]]
+
+
+def live_bytes():
+    """(device bytes, pinned host bytes) the library holds in this process right now, over every engine (a test hook)."""
+    dev, pin = C.c_uint64(), C.c_uint64()
+    if load_library().vtts_debug_live_bytes(C.byref(dev), C.byref(pin)) != 0:
+        raise VttsError(-1, "vtts_debug_live_bytes failed")
+    return int(dev.value), int(pin.value)
 
 
 def make_c_config(cfg, precision=0):
