@@ -399,6 +399,36 @@ int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav
                              float noise_scale, const float* noise, int noise_ld, uint64_t seed, float* out_wav, int64_t out_ld,
                              int64_t* out_frames);
 
+/* Resampling of recordings to a model's rate, and optional silence trimming: librosa.load(path, sr=...) followed, for
+ * QuickVC targets, by librosa.effects.trim(y, top_db=20), as vc/convert.py:65-66 prepares its inputs.  The resampler is
+ * scipy.signal.resample_poly(x, up, down) with its defaults (up / down = to_rate / from_rate in lowest terms; a Kaiser
+ * (beta 5) windowed-sinc low-pass of 2 * 10 * max(up, down) + 1 taps, cutoff 1 / max(up, down), gain up; zeros outside the
+ * clip), not librosa's default soxr_hq: the two differ in filter design, not in kind.  Clip b gives ceil(wav_lengths[b] * up
+ * / down) samples; equal rates copy the clip exactly.  Each clip is resampled as if alone: its output is bit-identical in any
+ * batch.
+ *   wav          float [B, wav_ld], clip b = its first wav_lengths[b] samples, 1 <= wav_lengths[b] <= wav_ld
+ *   from_rate, to_rate   in [VTTS_RESAMPLE_MIN_RATE, VTTS_RESAMPLE_MAX_RATE] Hz; the pair's filter must have at most
+ *                VTTS_RESAMPLE_MAX_TAPS taps (44 100 <-> 16 000 takes 8 821, 96 000 <-> 22 050 12 801)
+ *   trim_top_db  > 0: trim each resampled clip as librosa.effects.trim(y, top_db=trim_top_db) (librosa >= 0.10): frames of 2048
+ *                samples at hop 512, centred with zero padding; a frame is kept iff its mean square is above max(1e-10, the
+ *                loudest frame's) by more than -trim_top_db dB; the clip keeps [first * 512, min(n, (last + 1) * 512)).
+ *                <= 0: no trim.
+ *   out          out float [B, out_ld]: clip b's out_lengths[b] samples; the rest of each row is not written.  out_ld must
+ *                hold the untrimmed length ceil(wav_lengths[b] * up / down).
+ *   out_lengths  out int64 [B]
+ *   trim_bounds  out int64 [B, 2] or NULL: [start, end) of each kept part in the untrimmed resampled clip ([0, n) untrimmed)
+ * Host pointers, atomic on the handle; serves engines of every model family.  The taps of a rate pair are computed on the
+ * host in float64, rounded to fp32 once and kept on the device by the handle.  VTTS_ERR_INVALID: B < 1, a length outside
+ * [1, wav_ld], a rate out of range, a pair over the tap cap, a batch whose packed rows exceed
+ * VTTS_RESAMPLE_MAX_BATCH_SAMPLES (per clip the larger of its input and output length, plus 8), a clip of digital silence
+ * (every frame's mean square <= 1e-10) when trimming.  VTTS_ERR_CAPACITY: out_ld below an untrimmed clip's length. */
+#define VTTS_RESAMPLE_MIN_RATE 4000
+#define VTTS_RESAMPLE_MAX_RATE 384000
+#define VTTS_RESAMPLE_MAX_TAPS 64001
+#define VTTS_RESAMPLE_MAX_BATCH_SAMPLES (1LL << 30)
+int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,
+                  float trim_top_db, float* out, int64_t out_ld, int64_t* out_lengths, int64_t* trim_bounds);
+
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are
  * read with vtts_last_error(NULL) on the calling thread.

@@ -25,6 +25,8 @@ def main(argv=None):
     p.add_argument("--source-speaker", type=int, help="speaker id of the --convert-from recording")
     p.add_argument("--align", type=str, metavar="WAV",
                    help="forced alignment (extension): print the phoneme segments of --input in this mono WAV as JSON")
+    p.add_argument("--resample", default=False, action="store_true",
+                   help="--convert-from / --align: read a 16-bit WAV at any rate, mono or stereo, and resample it on the GPU")
     args = p.parse_args(argv)
     logging.getLogger().setLevel(args.log_level.upper())
     if args.list_models:
@@ -37,13 +39,15 @@ def main(argv=None):
         if args.source_speaker is None or args.speaker is None:
             p.error("--convert-from needs --source-speaker and --speaker (the target)")
         model = Model(args.model, args.model_name, args.lang, device=args.device, voice_conversion=True)
-        Synth(model).convert(args.convert_from, args.output, args.source_speaker, args.speaker)
+        extra = {"resample": True} if args.resample else {}
+        Synth(model).convert(args.convert_from, args.output, args.source_speaker, args.speaker, **extra)
         return 0
     if args.align:
         if not args.input:
             p.error("--align needs --input (the transcript of the recording)")
         model = Model(args.model, args.model_name, args.lang, device=args.device, voice_conversion=True)
-        print(json.dumps(Synth(model).align(args.align, args.input, speaker_id=args.speaker)))
+        extra = {"resample": True} if args.resample else {}
+        print(json.dumps(Synth(model).align(args.align, args.input, speaker_id=args.speaker, **extra)))
         return 0
     if not args.input:
         logging.info("Please specify input text or file")

@@ -29,6 +29,7 @@
 #include "vc.cuh"
 #include "spk.cuh"
 #include "contentvec.cuh"
+#include "resample.cuh"
 #include "owned.cuh"
 
 using namespace vtts;
@@ -662,6 +663,15 @@ struct vtts_engine {
       e->conv_max_s = ms; e->conv_min_g = ming; e->conv_big_g = bigg; e->conv_auto_g = autog;
     }
   };
+
+  // ---- resampling of recordings (vtts_resample; resample.cuh): the taps of each rate pair, uploaded on first use
+  struct RsTaps { Buf<float> taps; int up = 0, down = 0, K = 0; };
+  std::map<std::pair<int, int>, RsTaps> rs_taps;
+  Buf<int> d_rsi;                                  // [in_off B][in_len B][out_off B][out_len B][e_off B]
+  Buf<float> d_rsin, d_rsout;
+  Buf<double> d_rse;                               // frame energies of the trim
+  PinnedBuf<char> h_pin_rs, h_pin_rse;
+  const RsTaps& resample_taps(int up, int down);
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
   Buf<float> d_ncent, d_ncent_dbg, d_ascore;       // neg_cent [B][maxFrm][maxTok] (MAS accumulates in place), scores [B]
@@ -3492,6 +3502,157 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const float*
   }
 }
 
+// I0 by its power series (the Kaiser window's; np.i0 within a few ulps for the beta 5 of resample_poly)
+static double bessel_i0(double x) {
+  double sum = 1.0, term = 1.0;
+  for (int k = 1; k < 200 && term > 1e-18 * sum; ++k) {
+    const double r = x / (2.0 * k);
+    term *= r * r;
+    sum += term;
+  }
+  return sum;
+}
+
+}  // namespace
+
+// The low-pass of resample_poly for (up, down) (firwin(2 half + 1, 1 / max(up, down), window=("kaiser", 5.0)) * up, half =
+// 10 max(up, down)) in float64, rounded to fp32 once, laid out per phase [up][K]: phase p holds h[p + up q], zeros past L.
+const vtts_engine::RsTaps& vtts_engine::resample_taps(int up, int down) {
+  RsTaps& r = rs_taps[{up, down}];
+  if (r.taps.p) return r;
+  const int M = std::max(up, down), half = 10 * M, L = 2 * half + 1, K = (L + up - 1) / up;
+  std::vector<double> h(L);
+  const double pi = 3.14159265358979323846, alpha = 0.5 * (L - 1), i0b = bessel_i0(5.0);
+  double sum = 0.0;
+  for (int i = 0; i < L; ++i) {
+    const double n = (double)(i - half) / M, u = (i - alpha) / alpha;
+    const double sinc = n == 0.0 ? 1.0 : std::sin(pi * n) / (pi * n);
+    h[i] = sinc / M * (bessel_i0(5.0 * std::sqrt(std::max(0.0, 1.0 - u * u))) / i0b);
+    sum += h[i];
+  }
+  std::vector<float> poly((size_t)up * K, 0.f);
+  for (int i = 0; i < L; ++i) poly[(size_t)(i % up) * K + i / up] = (float)(h[i] / sum * up);
+  Buf<float> buf;
+  CK(buf.alloc(poly.size()));
+  // On the engine's stream, so that the kernels enqueued behind it read the taps only after the copy has landed (the stream
+  // is non-blocking: a cudaMemcpy on the legacy stream would not order them).  A pageable source is staged before the call
+  // returns, so `poly` may go when it does.
+  CK(cudaMemcpyAsync(buf.p, poly.data(), poly.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+  r.taps = std::move(buf);
+  r.up = up; r.down = down; r.K = K;
+  return r;
+}
+
+namespace {
+
+// Resampling (and trimming) through host buffers (vtts_resample): the clips are packed as rows with SEQ_GAP between them
+// into pinned staging with the row table, uploaded, resampled (equal rates: the uploaded rows are the output), the frame
+// energies of the trim computed on the device and read back, the bounds picked on the host, then the kept rows read back.
+static void impl_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,
+                          float trim_top_db, float* out, int64_t out_ld, int64_t* out_lengths, int64_t* trim_bounds) {
+  REQUIRE(wav && lengths && out && out_lengths, VTTS_ERR_INVALID, "wav, lengths, out and out_lengths are required");
+  REQUIRE(B >= 1 && B <= 16384, VTTS_ERR_INVALID, "bad batch size");
+  REQUIRE(ld >= 1, VTTS_ERR_INVALID, "bad wav_ld");
+  for (int r : {from_rate, to_rate})
+    REQUIRE(r >= VTTS_RESAMPLE_MIN_RATE && r <= VTTS_RESAMPLE_MAX_RATE, VTTS_ERR_INVALID,
+            "sample rates must lie in [" + std::to_string(VTTS_RESAMPLE_MIN_RATE) + ", " + std::to_string(VTTS_RESAMPLE_MAX_RATE) +
+            "] Hz, not " + std::to_string(r));
+  int a = from_rate, c = to_rate;
+  while (c) { const int t = a % c; a = c; c = t; }
+  const int up = to_rate / a, down = from_rate / a;
+  const int64_t ntaps = 20LL * std::max(up, down) + 1;
+  REQUIRE(ntaps <= VTTS_RESAMPLE_MAX_TAPS, VTTS_ERR_INVALID,
+          "resampling " + std::to_string(from_rate) + " -> " + std::to_string(to_rate) + " Hz needs a filter of " +
+          std::to_string(ntaps) + " taps, more than the " + std::to_string(VTTS_RESAMPLE_MAX_TAPS) + " this call supports");
+  const bool same = up == down;
+  std::vector<int> in_len(B), out_len(B), in_off, out_off, e_off(B + 1, 0);
+  int64_t total = 0;
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lengths[b] >= 1 && lengths[b] <= ld, VTTS_ERR_INVALID, "wav_lengths must be in [1, wav_ld]");
+    const int64_t n = ((int64_t)lengths[b] * up + down - 1) / down;
+    REQUIRE(n <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than a resampled clip (ceil(len * to_rate / from_rate))");
+    total += std::max<int64_t>(lengths[b], n) + SEQ_GAP;
+    REQUIRE(total <= VTTS_RESAMPLE_MAX_BATCH_SAMPLES, VTTS_ERR_INVALID, "the batch holds too many samples for one call");
+    in_len[b] = (int)lengths[b];
+    out_len[b] = (int)n;
+    e_off[b + 1] = e_off[b] + 1 + out_len[b] / RS_HOP;
+  }
+  vtts_engine::pack_rows(in_len, in_off);
+  if (same) out_off = in_off;
+  else vtts_engine::pack_rows(out_len, out_off);
+  // staging: the row table, then the packed input rows
+  const size_t head = ((size_t)5 * B * sizeof(int) + 63) / 64 * 64, nin = (size_t)in_off[B];
+  char* pin = h->ensure(h->h_pin_rs, head + nin * sizeof(float) + 64);
+  int* tab = reinterpret_cast<int*>(pin);
+  for (int b = 0; b < B; ++b) {
+    tab[b] = in_off[b]; tab[B + b] = in_len[b]; tab[2 * B + b] = out_off[b]; tab[3 * B + b] = out_len[b]; tab[4 * B + b] = e_off[b];
+    memcpy(reinterpret_cast<float*>(pin + head) + in_off[b], wav + (size_t)b * ld, (size_t)in_len[b] * sizeof(float));
+  }
+  int* di = h->ensure(h->d_rsi, (size_t)5 * B);
+  float* din = h->ensure(h->d_rsin, nin);
+  CK(cudaMemcpyAsync(di, pin, (size_t)5 * B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(din, pin + head, nin * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  const int max_out = *std::max_element(out_len.begin(), out_len.end());
+  const float* y = din;
+  if (!same) {
+    const vtts_engine::RsTaps& rt = h->resample_taps(up, down);
+    const int K = rt.K, half = 10 * std::max(up, down);
+    int tile = RS_TILE_MAX;
+    while (tile > 32 && rs_window(tile, up, down, K) > RS_WIN_MAX) tile /= 2;
+    const int taps_smem = (int64_t)up * rs_taps_pitch(K) <= RS_TAPS_SMEM ? 1 : 0;
+    const size_t smem = ((size_t)(taps_smem ? up * rs_taps_pitch(K) : 0) + rs_window(tile, up, down, K)) * sizeof(float);
+    REQUIRE(smem <= 200 * 1024, VTTS_ERR_INVALID, "resampler window does not fit shared memory");
+    CK(cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    float* dout = h->ensure(h->d_rsout, (size_t)out_off[B]);
+    h->klaunch(resample_kernel, dim3((max_out + tile - 1) / tile, B), dim3(RS_THREADS), smem, (const float*)din, (const int*)di, B,
+               (const float*)rt.taps.p, up, down, K, half, tile, taps_smem, dout);
+    CK(cudaGetLastError());
+    ++h->launches;
+    y = dout;
+  }
+  std::vector<int> keep_off(out_off.begin(), out_off.begin() + B), keep_len = out_len;
+  if (trim_top_db > 0.f) {
+    const int max_nf = 1 + max_out / RS_HOP;
+    double* de = h->ensure(h->d_rse, (size_t)e_off[B]);
+    h->klaunch(frame_energy_kernel, dim3((max_nf + RS_FRAME_WARPS - 1) / RS_FRAME_WARPS, B), dim3(RS_FRAME_WARPS * 32), (size_t)0, y,
+               (const int*)(di + 2 * B), B, de);
+    CK(cudaGetLastError());
+    ++h->launches;
+    double* pe = reinterpret_cast<double*>(h->ensure(h->h_pin_rse, (size_t)e_off[B] * sizeof(double)));
+    CK(cudaMemcpyAsync(pe, de, (size_t)e_off[B] * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    const double amin = 1e-10, thr = -(double)trim_top_db;
+    for (int b = 0; b < B; ++b) {
+      const double* e = pe + e_off[b];
+      const int nf = e_off[b + 1] - e_off[b];
+      double top = 0.0;
+      for (int f = 0; f < nf; ++f) top = std::max(top, e[f] / RS_FRAME);
+      REQUIRE(top > amin, VTTS_ERR_INVALID, "clip " + std::to_string(b) +
+              " is silent throughout (every frame's mean square is at most 1e-10): trimming leaves nothing to keep");
+      const double ref = 10.0 * std::log10(std::max(amin, top));
+      int first = -1, last = -1;
+      for (int f = 0; f < nf; ++f) {
+        if (10.0 * std::log10(std::max(amin, e[f] / RS_FRAME)) - ref > thr) {
+          if (first < 0) first = f;
+          last = f;
+        }
+      }
+      const int s0 = first * RS_HOP, s1 = std::min(out_len[b], (last + 1) * RS_HOP);
+      keep_off[b] = out_off[b] + s0;
+      keep_len[b] = s1 - s0;
+      if (trim_bounds) { trim_bounds[2 * b] = s0; trim_bounds[2 * b + 1] = s1; }
+    }
+  } else if (trim_bounds) {
+    for (int b = 0; b < B; ++b) { trim_bounds[2 * b] = 0; trim_bounds[2 * b + 1] = out_len[b]; }
+  }
+  // read back the packed span from the first kept sample to the last (with a trim: not the first clip's leading and the last
+  // clip's trailing silence)
+  const int lo = keep_off[0], hi = keep_off[B - 1] + keep_len[B - 1];
+  for (int& o : keep_off) o -= lo;
+  read_clips(h, y + lo, (size_t)(hi - lo), (size_t)(hi - lo), keep_off.data(), keep_len, 1, out, out_ld);
+  for (int b = 0; b < B; ++b) out_lengths[b] = keep_len[b];
+}
+
 static void impl_synthesize_dev(vtts_handle h, const float* d_noise_z, int z_ld, float* d_wav, int64_t wav_ld) {
   REQUIRE(h->have_durations, VTTS_ERR_STATE, "vtts_synthesize_dev called without vtts_durations_dev");
   REQUIRE((int64_t)h->real_maxFrm * h->hop <= wav_ld, VTTS_ERR_CAPACITY, "wav_ld is smaller than hop * max(y_lengths)");
@@ -3994,6 +4155,12 @@ int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav
   if (!wav || !wav_lengths || !out_wav || !out_frames) return VTTS_ERR_INVALID;
   return guarded(h, [&] { impl_quickvc_convert(h, nullptr, wav, wav_lengths, B, wav_ld, g, noise_scale, noise, noise_ld, seed, out_wav,
                                                out_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,
+                  float trim_top_db, float* out, int64_t out_ld, int64_t* out_lengths, int64_t* trim_bounds) {
+  return guarded(h, [&] { impl_resample(h, wav, lengths, B, ld, from_rate, to_rate, trim_top_db, out, out_ld, out_lengths, trim_bounds); },
+                 G_ATOMIC, ANY_FAMILY);
 }
 
 // A device copy of a debug hook's host argument, held by `dev` (so freed on every exit).

@@ -1,6 +1,7 @@
 """ctypes binding of libvtts.so (include/vtts.h).  No CPU fallback: importing works without a GPU
 (the library only needs libcudart), creating an Engine requires a CUDA device."""
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -55,7 +56,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
-           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes"]
+           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1}    # vtts_config.model_family
 
@@ -233,6 +234,8 @@ def load_library(build_if_missing=True):
     lib.vtts_quickvc_convert_wav.restype = i32
     lib.vtts_debug_live_bytes.argtypes = [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     lib.vtts_debug_live_bytes.restype = i32
+    lib.vtts_resample.argtypes = [vp, vp, vp, i32, C.c_int64, i32, i32, C.c_float, vp, C.c_int64, vp, vp]
+    lib.vtts_resample.restype = i32
     _LIB = lib
     return lib
 
@@ -658,6 +661,27 @@ class Engine:
         are the large buffers): one call of that size, so later calls within these bounds move no buffer."""
         self.content_units(np.zeros((int(batch), int(max_samples)), np.float32))
         return int(max_samples)
+
+    # ---- resampling of recordings (librosa.load(path, sr=...) and librosa.effects.trim, as vc/convert.py:65-66 uses them)
+    def resample(self, wav, from_rate, to_rate, lengths=None, trim_top_db=None, return_bounds=False):
+        """Clips at `from_rate` Hz resampled to `to_rate` Hz (vtts_resample: scipy.signal.resample_poly's filter, not soxr), and
+        with `trim_top_db` trimmed of leading and trailing silence as librosa.effects.trim(y, top_db=trim_top_db) does.  wav:
+        one clip [L], a padded batch [B, L] with `lengths`, or a list of ragged clips.  Works on engines of every model family.
+        Returns the list of float32 clips; with return_bounds also int64 [B, 2], the [start, end) kept of each resampled clip."""
+        if min(int(from_rate), int(to_rate)) <= 0:
+            raise ValueError("sample rates must be positive")
+        wav, lengths = _batch(wav, lengths, 2, ragged=True)
+        B = wav.shape[0]
+        g = math.gcd(int(from_rate), int(to_rate))
+        up, down = int(to_rate) // g, int(from_rate) // g
+        out_len = -(-lengths * up // down)
+        out = np.zeros((B, max(1, int(out_len.max()))), np.float32)
+        n = np.zeros(B, np.int64)
+        bounds = np.zeros((B, 2), np.int64)
+        self._check(self.lib.vtts_resample(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], int(from_rate), int(to_rate),
+                                           float(trim_top_db or 0.0), _ptr(out), out.shape[1], _ptr(n), _ptr(bounds)))
+        clips = [out[b, :int(n[b])].copy() for b in range(B)]
+        return (clips, bounds) if return_bounds else clips
 
     # ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
     def _align(self, from_wav, ids, lengths, sid, x, x_lengths, noise_scale, noise, seed):

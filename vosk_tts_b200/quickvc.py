@@ -12,12 +12,19 @@ With a ContentVec checkpoint (a Hugging Face directory with config.json and pyto
     wav = vc.convert(source_wav, g=g)               # 16 kHz float source in [-1, 1]
     units = vc.units(source_wav)                    # ContentVec last_hidden_state [T, 768]
 
-Unlike convert.py, the target recording is not trimmed of silence (librosa.effects.trim(top_db=20)); trim it before
-embedding for the same g.
+Recordings at another rate are resampled on the GPU when their rate is given, and the target is trimmed of leading and
+trailing silence as convert.py does (librosa.effects.trim(top_db=20)) when asked; by default neither happens:
+
+    g = vc.embed(target_44k, sampling_rate=44100, trim=True)
+    wav = vc.convert(source_48k, g=g, sampling_rate=48000)
+
+The resampler is scipy.signal.resample_poly's (a Kaiser-windowed sinc), not librosa.load's default soxr_hq: the filters
+differ in design, not in kind, so the samples differ slightly from convert.py's.
 
 CLI:  python -m vosk_tts_b200.quickvc --config quickvc.json --checkpoint G.pth --units a.npy b.npy --target tgt.wav --out-dir out
 writes out/<units file name>.wav, 16 kHz int16, clipped to the int16 range (convert.py's astype(int16) wraps instead).
-With --contentvec DIR, --source a.wav ... takes 16 kHz source recordings in place of --units.
+With --contentvec DIR, --source a.wav ... takes 16 kHz source recordings in place of --units.  --resample reads the WAV
+files at any rate, mono or stereo, and resamples them on the GPU; --trim-target trims the target as convert.py does.
 """
 import argparse
 import os
@@ -27,6 +34,7 @@ import wave
 import numpy as np
 
 from . import config as _config, weights as _weights
+from .wav import read_pcm16
 
 
 def read_wav(path, sampling_rate=16000):
@@ -65,29 +73,44 @@ class QuickVC:
         self.engine = Engine(self.cfg, blob, man, device=device, precision=precision)
         self.sampling_rate = int(self.cfg["sampling_rate"])
 
-    def embed(self, target_wav):
-        """The target voice g [256] of a recording (float [-1, 1] at the model's rate)."""
-        return self.engine.speaker_embedding(np.asarray(target_wav, np.float32))[0]
+    def resample(self, clips, sampling_rate, trim=False):
+        """A list of 1-D clips at `sampling_rate` Hz (None: the model's) -> the list at the model's rate, resampled on the GPU
+        in one ragged call (Engine.resample) and, with trim, trimmed as librosa.effects.trim(top_db=20) does; float32 copies
+        when neither applies."""
+        clips = [np.asarray(x, np.float32).reshape(-1) for x in clips]
+        rate = self.sampling_rate if sampling_rate is None else int(sampling_rate)
+        if rate == self.sampling_rate and not trim:
+            return clips
+        return self.engine.resample(clips, rate, self.sampling_rate, trim_top_db=20.0 if trim else None)
 
-    def units(self, wav):
-        """ContentVec units [T, 768] of a source recording (float [-1, 1] at 16 kHz), or a list of them for a list of sources."""
+    def embed(self, target_wav, sampling_rate=None, trim=False):
+        """The target voice g [256] of a recording (float [-1, 1] at the model's rate, or at `sampling_rate` Hz: resampled on
+        the GPU first).  trim: trim leading and trailing silence first as convert.py does (librosa.effects.trim(top_db=20))."""
+        if (sampling_rate is None or int(sampling_rate) == self.sampling_rate) and not trim:
+            return self.engine.speaker_embedding(np.asarray(target_wav, np.float32))[0]
+        return self.engine.speaker_embedding(self.resample([target_wav], sampling_rate, trim)[0])[0]
+
+    def units(self, wav, sampling_rate=None):
+        """ContentVec units [T, 768] of a source recording (float [-1, 1] at 16 kHz, or at `sampling_rate` Hz: resampled on the
+        GPU first), or a list of them for a list of sources."""
         single = not isinstance(wav, (list, tuple))
         clips = [wav] if single else list(wav)
-        u, frames = self.engine.content_units([np.asarray(x, np.float32).reshape(-1) for x in clips])
+        u, frames = self.engine.content_units(self.resample(clips, sampling_rate))
         out = [u[b, :int(frames[b])] for b in range(len(clips))]
         return out[0] if single else out
 
-    def convert(self, units, target_wav=None, g=None, noise_scale=1.0, seed=0):
+    def convert(self, units, target_wav=None, g=None, noise_scale=1.0, seed=0, sampling_rate=None):
         """Units [T, 768], or source waveforms (1-D, 16 kHz; needs contentvec), or a list of either, in the voice of g or of
-        target_wav's g: float32 waveform(s) at the model's rate."""
+        target_wav's g: float32 waveform(s) at the model's rate.  sampling_rate: the rate of the waveforms of this call (the
+        sources and target_wav), resampled to the model's on the GPU first; None: already at the model's rate."""
         if g is None:
             if target_wav is None:
                 raise ValueError("convert needs a target: target_wav or g")
-            g = self.embed(target_wav)
+            g = self.embed(target_wav, sampling_rate=sampling_rate)
         single = not isinstance(units, (list, tuple))
         clips = [units] if single else list(units)
         if all(np.ndim(c) == 1 for c in clips):
-            wav, frames = self.engine.quickvc_convert_wav([np.asarray(c, np.float32) for c in clips], g, noise_scale=noise_scale, seed=seed)
+            wav, frames = self.engine.quickvc_convert_wav(self.resample(clips, sampling_rate), g, noise_scale=noise_scale, seed=seed)
         else:
             wav, frames = self.engine.quickvc_convert(clips, g, noise_scale=noise_scale, seed=seed)
         out = [wav[b, :int(frames[b]) * self.engine.hop] for b in range(len(clips))]
@@ -106,6 +129,10 @@ def main(argv=None):
     src.add_argument("--source", nargs="+", help="source recordings, 16 kHz mono 16-bit WAV (needs --contentvec)")
     ap.add_argument("--contentvec", help="ContentVec checkpoint directory (config.json + pytorch_model.bin)")
     ap.add_argument("--target", required=True, help="recording of the target voice, 16 kHz mono 16-bit WAV")
+    ap.add_argument("--resample", action="store_true",
+                    help="read --target and --source WAV files at any rate, mono or stereo, and resample them on the GPU")
+    ap.add_argument("--trim-target", action="store_true",
+                    help="trim the target's leading and trailing silence as convert.py does (librosa.effects.trim, top_db=20)")
     ap.add_argument("--out-dir", required=True)
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--precision", type=int, default=1, choices=[0, 1])
@@ -114,16 +141,20 @@ def main(argv=None):
     if a.source and not a.contentvec:
         ap.error("--source needs --contentvec DIR (the ContentVec checkpoint that computes the units)")
     cfg = _config.from_quickvc_json(a.config)
+    sr = int(cfg["sampling_rate"])
+    read = read_pcm16 if a.resample else (lambda p: (read_wav(p, sr), sr))     # -> (samples, their rate)
     try:
-        target = read_wav(a.target, int(cfg["sampling_rate"]))
+        target, target_sr = read(a.target)
     except ValueError as ex:
         ap.error(str(ex))
-    units = []
+    units, rates = [], []
     for p in a.source or []:
         try:
-            units.append(read_wav(p, int(cfg["sampling_rate"])))
+            x, r = read(p)
         except ValueError as ex:
             ap.error(str(ex))
+        units.append(x)
+        rates.append(r)
     for p in a.units or []:
         u = np.load(p)
         if u.ndim != 2 or u.shape[1] != cfg["unit_channels"] or u.shape[0] < 1:
@@ -131,7 +162,11 @@ def main(argv=None):
         units.append(u.astype(np.float32))
     vc = QuickVC(a.config, a.checkpoint, device=a.device, precision=a.precision, contentvec=a.contentvec)
     try:
-        g = vc.embed(target)
+        g = vc.embed(target, sampling_rate=target_sr, trim=a.trim_target)
+        for r in sorted(set(rates)):                 # the sources of one rate in one ragged call
+            idx = [i for i, q in enumerate(rates) if q == r]
+            for i, x in zip(idx, vc.resample([units[i] for i in idx], r)):
+                units[i] = x
         os.makedirs(a.out_dir, exist_ok=True)
         for p, w in zip(a.source or a.units, vc.convert(units, g=g, seed=a.seed)):
             out = os.path.join(a.out_dir, os.path.splitext(os.path.basename(p))[0] + ".wav")

@@ -138,5 +138,10 @@ class VitsSession:
             self.last_wav_lengths = frames * self.engine.hop
         return dur[0], tof[0, : int(frames[0])], float(score[0])
 
+    def resample(self, wav, from_rate, to_rate):
+        """One clip float32 [L] at `from_rate` Hz resampled to `to_rate` Hz on the GPU (Engine.resample; extension)."""
+        with self._lock:
+            return self.engine.resample(np.asarray(wav, np.float32).reshape(-1), from_rate, to_rate)[0]
+
     def close(self):
         self.engine.close()

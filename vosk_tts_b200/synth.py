@@ -13,6 +13,7 @@ import wave
 import numpy as np
 
 from .g2p import convert
+from .wav import read_pcm16
 
 _PUNCT = "([,.?!;:\"() ])"
 
@@ -115,11 +116,13 @@ class Synth:
             return int(cfg["sampling_rate"])
         return int(self.model.config.get("audio", {}).get("sample_rate", self.model.config.get("data", {}).get("sampling_rate", 22050)))
 
-    def convert_audio(self, audio, src_speaker, tgt_speaker, noise_scale=None, scale=None):
+    def convert_audio(self, audio, src_speaker, tgt_speaker, noise_scale=None, scale=None, sampling_rate=None):
         """Voice conversion (extension): re-voices `audio` of speaker `src_speaker` as `tgt_speaker` of the same model
         (SynthesizerTrn.voice_conversion, models.py:1710-1718).  audio: int16 samples (divided by 32768, data_utils.py:77) or
-        float in [-1, 1], at the model's sample rate.  Returns int16 [256 * (len // 256)] for the reference configuration."""
-        wav = self._float_audio(audio, "convert_audio")
+        float in [-1, 1], at the model's sample rate, or at `sampling_rate` Hz: it is then resampled to the model's rate on
+        the GPU first (as librosa.load(path, sr=...) would, with resample_poly's filter).  Returns int16 [256 * (len // 256)]
+        of the model-rate clip for the reference configuration."""
+        wav = self._at_model_rate(self._float_audio(audio, "convert_audio"), sampling_rate)
         if src_speaker is None or tgt_speaker is None:
             raise ValueError("voice conversion needs both a source and a target speaker id")
         inf = self.model.config.get("inference", {})
@@ -132,6 +135,13 @@ class Synth:
         dur = out.shape[-1] / self._sample_rate()
         logging.info("Real-time factor: %0.2f (convert=%0.2f sec, audio=%0.2f sec)" % (sec / dur if dur > 0 else 0.0, sec, dur))
         return out
+
+    def _at_model_rate(self, wav, sampling_rate):
+        """wav at `sampling_rate` Hz (None: already at the model's rate) -> the model's rate, resampled on the GPU."""
+        sr = self._sample_rate()
+        if sampling_rate is None or int(sampling_rate) == sr:
+            return wav
+        return self.model.onnx.resample(wav, int(sampling_rate), sr)
 
     def _read_wav(self, iname):
         """A mono 16-bit WAV at the model's sample rate (no resampling) -> int16 samples."""
@@ -157,27 +167,31 @@ class Synth:
             return wav
         raise ValueError("audio must be int16 or float samples, not %s" % audio.dtype)
 
-    def convert(self, iname, oname, src_speaker, tgt_speaker, noise_scale=None, scale=None):
-        """Reads a mono 16-bit WAV at the model's sample rate (no resampling), writes the converted clip as one."""
+    def convert(self, iname, oname, src_speaker, tgt_speaker, noise_scale=None, scale=None, resample=False):
+        """Reads a mono 16-bit WAV at the model's sample rate (no resampling), writes the converted clip as one at that rate.
+        resample: read a 16-bit WAV at any rate, mono or multichannel (averaged to mono), and resample it on the GPU."""
         sr = self._sample_rate()
-        audio = self._read_wav(iname)
-        out = self.convert_audio(audio, src_speaker, tgt_speaker, noise_scale, scale)
+        if resample:
+            audio, rate = read_pcm16(iname)
+            out = self.convert_audio(audio, src_speaker, tgt_speaker, noise_scale, scale, sampling_rate=rate)
+        else:
+            out = self.convert_audio(self._read_wav(iname), src_speaker, tgt_speaker, noise_scale, scale)
         with wave.open(oname, "w") as f:
             f.setnchannels(1)
             f.setsampwidth(2)
             f.setframerate(sr)
             f.writeframes(out.tobytes())
 
-    def align_audio(self, text, audio, speaker_id=0, noise_scale=None):
+    def align_audio(self, text, audio, speaker_id=0, noise_scale=None, sampling_rate=None):
         """Forced alignment (extension): the phonemes of `text` (the g2p of synth_audio) against `audio` of speaker
         `speaker_id`, by the model's own monotonic alignment search (SynthesizerTrn.forward, models.py:1632-1660).  audio as
-        in convert_audio.  Returns one dict per g2p phoneme, "^", "$" and punctuation included -- {"phoneme", "start", "end"}
+        in convert_audio (`sampling_rate`: its rate, resampled to the model's on the GPU).  Returns one dict per g2p phoneme, "^", "$" and punctuation included -- {"phoneme", "start", "end"}
         in seconds (frames * hop / sample rate) -- with each interspersed blank as its own entry with phoneme None; the
         frames of a phoneme that maps to several ids are merged, and the entries tile [0, frames * hop / sample rate).
         The best path's log-likelihood (higher: the audio fits the text better) is kept in `last_score`."""
         if self.model.tokenizer is not None or str(self.model.config.get("model_type", "")).startswith("multistream"):
             raise ValueError("model_type %r is not a VITS2 graph: not supported by this engine" % self.model.config.get("model_type"))
-        wav = self._float_audio(audio, "align_audio")
+        wav = self._at_model_rate(self._float_audio(audio, "align_audio"), sampling_rate)
         phonemes, ids, spans = self._g2p(re.sub("—", "-", text.strip()))
         noise_scale = 1.0 if noise_scale is None else noise_scale      # the reference samples the posterior at scale 1 (:841)
         t0 = time.perf_counter()
@@ -195,8 +209,12 @@ class Synth:
         logging.info("Alignment: %d phonemes, %d frames, score %.1f (%.2f sec)" % (len(phonemes), int(cum[-1]), score, sec))
         return entries
 
-    def align(self, wav_path, text, speaker_id=0, noise_scale=None):
-        """align_audio of a mono 16-bit WAV at the model's sample rate (no resampling)."""
+    def align(self, wav_path, text, speaker_id=0, noise_scale=None, resample=False):
+        """align_audio of a mono 16-bit WAV at the model's sample rate (no resampling).  resample: a 16-bit WAV at any rate,
+        mono or multichannel (averaged to mono), resampled on the GPU; the segment times are those of the model-rate clip."""
+        if resample:
+            audio, rate = read_pcm16(wav_path)
+            return self.align_audio(text, audio, speaker_id, noise_scale, sampling_rate=rate)
         return self.align_audio(text, self._read_wav(wav_path), speaker_id, noise_scale)
 
     def _hop(self):
