@@ -70,9 +70,15 @@ typedef struct vtts_config {
   int32_t filter_length, hop_length, win_length, n_mel_channels;
   float mel_fmin, mel_fmax;        /* (the mel filter bank itself is packed into the blob) */
   /* Model family of the blob: 0 = VITS2 SynthesizerTrn (every entry point above and below except the QuickVC ones),
-   * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding* and vtts_quickvc_convert.  The entry points of one family
-   * return VTTS_ERR_INVALID on an engine of the other. */
+   * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding* and vtts_quickvc_convert,
+   * 2 = StableTTS (the flow-matching decoder; weights.pack_stabletts_cfm), which serves vtts_cfm_decode.  The entry points of
+   * one family return VTTS_ERR_INVALID on an engine of another. */
   int32_t model_family;
+  /* StableTTS flow-matching decoder (model_family 2; CFM of training/stabletts/matcha/models/components/flow_matching.py:301,
+   * weights.pack_stabletts_cfm): vtts_cfm_decode.  The other families leave these 0. */
+  int32_t st_noise, st_cond, st_hidden, st_filter;         /* mel channels 80, encoder output 256, hidden 384, FFN / prenet 768 */
+  int32_t st_layers, st_heads, st_kernel;                  /* 6 DitWrapper blocks (even: U-Net long skips), 4 heads, k = 3 */
+  int32_t st_spk_dim, st_n_spks;                           /* speaker embedding width 128, rows of spk_emb */
   /* ContentVec (HubertModel of vc/contentvec.py, transformers' HubertConfig; QuickVC engines whose blob carries cv.*):
    * vtts_content_units / vtts_quickvc_convert_wav.  cv_layers == 0: no ContentVec. */
   int32_t cv_layers, cv_hidden, cv_heads, cv_ffn;          /* transformer: 12 post-LN layers, 768 wide, 12 heads, FFN 3072 */
@@ -84,6 +90,7 @@ typedef struct vtts_config {
 
 #define VTTS_FAMILY_VITS2 0
 #define VTTS_FAMILY_QUICKVC 1
+#define VTTS_FAMILY_STABLETTS 2
 
 /* Replaces onnxruntime.InferenceSession(model.onnx) (vosk_tts/model.py:46).
  * `blob` holds the packed fp32 tensors produced by vosk_tts_b200.weights.pack(); `manifest` is a
@@ -428,6 +435,35 @@ int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav
 #define VTTS_RESAMPLE_MAX_BATCH_SAMPLES (1LL << 30)
 int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,
                   float trim_top_db, float* out, int64_t out_ld, int64_t* out_lengths, int64_t* trim_bounds);
+
+/* StableTTS flow-matching decoder (CFM.forward -> solve_euler -> Decoder, flow_matching.py:33-100,182-194, decoder.py:103-138,
+ * as MatchaTTS.synthesise calls it at matcha_tts.py:183): the encoder output expanded to frames and a speaker in, mel out.
+ * z = noise * temperature; t_span = 1 - cos(linspace(0, 1, n + 1) pi / 2); n fixed Euler steps x += dt (v_c + s (v_c - v_u))
+ * with v_c = estimator(x, mu, t, speaker) and v_u = estimator(x, fake_content, t, fake_speaker) (classifier-free guidance;
+ * the reference fixes s = 0.5).  Each utterance is decoded as if alone (the prenet's convs are zero padded at its own ends),
+ * and its mel is bit-identical in any batch.  One call is one enqueue: no host wait between the steps.
+ *   mu           float [B, mu_ld, st_cond], frame-major: utterance b = its first lengths[b] frames, 1 <= lengths[b] <= mu_ld
+ *   sid          int64 [B] rows of spk_emb, or NULL when spk_rows is given
+ *   spk_rows     float [B, st_spk_dim] speaker embeddings used instead of spk_emb[sid], or NULL
+ *   n_timesteps  in [1, VTTS_CFM_MAX_STEPS]
+ *   guidance_scale  s >= 0; 0 skips the unconditional branch
+ *   noise        float [B, noise_ld, st_noise] frame-major, standing in for torch.randn (flow_matching.py:52), or NULL for
+ *                Philox(seed); with noise given, seed is not read
+ *   mel_out      out float [B, mel_ld, st_noise] frame-major: utterance b's lengths[b] frames, the rest of each row is not written
+ *   denormalise  != 0: mel * mel_std + mel_mean (matcha_tts.py:205), else the normalised mel of the last Euler step
+ * Host pointers, atomic on the handle; graphed per (batch, frame bucket, n_timesteps, s == 0, noise / speaker input kind).
+ * Runs on the fp32 FFMA pipe in every precision mode.  VTTS_ERR_INVALID: not a StableTTS engine, B < 1, a length outside
+ * [1, mu_ld], n_timesteps out of range, a temperature or guidance scale that is not finite (or s < 0), a speaker id outside
+ * [0, st_n_spks), neither sid nor spk_rows.  VTTS_ERR_CAPACITY: mel_ld or noise_ld below the longest utterance.
+ * After a call with bit0 of vtts_debug_flags set, vtts_debug_read gives "st_film" [steps][layers][2 hidden], "st_ada"
+ * [sequences][layers][6 hidden] (the unconditional sequences after the B conditional ones), "st_cond" (the in_proj operand
+ * rows [rows][st_noise + st_hidden]: x after the last step, then cond_proj's output), "st_rope" [max frames][dk / 4] (cos, sin)
+ * pairs, and of the first estimator evaluation "st_norm1" (block 0's modulated LayerNorm) and "st_qkv" (block 0's q, k
+ * after the rotary embedding, and v), rows [rows][hidden] and [rows][3 hidden]. */
+#define VTTS_CFM_MAX_STEPS 64
+int vtts_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int B, int64_t mu_ld, const int64_t* sid,
+                    const float* spk_rows, int n_timesteps, float temperature, float guidance_scale, const float* noise,
+                    int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld, int denormalise);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

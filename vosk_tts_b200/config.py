@@ -163,6 +163,46 @@ def from_quickvc_json(path_or_dict):
     return out
 
 
+STABLETTS_CFM = {
+    # CFM.__init__ hard-codes the estimator (flow_matching.py:301); n_spks / spk_emb_dim and the mel statistics come from the
+    # experiment's yaml (MatchaTTS.__init__, matcha_tts.py:28-38,92)
+    "model_family": "stabletts",
+    "noise_channels": 80, "cond_channels": 256, "hidden_channels": 384, "filter_channels": 768,
+    "n_layers": 6, "n_heads": 4, "kernel_size": 3, "use_lsc": True,
+    "n_spks": 2, "spk_emb_dim": 128,
+    "solver": "euler",
+}
+
+
+def stabletts_cfm_config(overrides=None):
+    """Engine config of the StableTTS flow-matching decoder, model_family "stabletts": the estimator's constants
+    (flow_matching.py:301) with `overrides` (e.g. n_spks / spk_emb_dim of a checkpoint).  What is not built is refused with
+    the reason."""
+    out = copy.deepcopy(STABLETTS_CFM)
+    out.update(overrides or {})
+    H, heads, L = int(out["hidden_channels"]), int(out["n_heads"]), int(out["n_layers"])
+    if not out.get("use_lsc", True):
+        raise ValueError("use_lsc=false is not supported: the engine builds the U-Net long skips the reference always enables "
+                         "(flow_matching.py:301)")
+    if L < 2 or L % 2 or L > 8:
+        raise ValueError("n_layers must be even and in 2..8: the long skips pair block i with block n_layers - 1 - i "
+                         "(decoder.py:93-95)")
+    if H % heads or (H // heads) not in (32, 64, 96, 128):
+        raise ValueError("head width hidden_channels / n_heads must be 32, 64, 96 or 128: the attention kernels take no other")
+    if out["solver"] != "euler":
+        raise ValueError("only the fixed-step Euler solver is built (the reference's heun / midpoint / dopri5 paths are "
+                         "commented out or unreachable, flow_matching.py:57-69)")
+    if int(out["kernel_size"]) % 2 != 1:
+        raise ValueError("kernel_size must be odd (padding = kernel_size // 2 keeps the length)")
+    if H % 16 or H > 512 or int(out["filter_channels"]) % 16 or int(out["filter_channels"]) > 1024 or int(out["cond_channels"]) % 16 \
+            or (int(out["noise_channels"]) + H) % 16 or int(out["noise_channels"]) % 4:
+        raise ValueError("channel widths must be multiples of 16 (noise_channels of 4, noise + hidden of 16), hidden up to 512, "
+                         "filter up to 1024: the FFMA conv and LayerNorm kernels' tiles")
+    if int(out["n_spks"]) < 1 or not 1 <= int(out["spk_emb_dim"]) <= 1024:
+        raise ValueError("n_spks must be >= 1 and spk_emb_dim in 1..1024")
+    return out
+
+
 def convt_pad(cfg, i):
     """(padding, output_padding) of the decoder's upsampling ConvTranspose1d of stage i: (K-u)//2 and 0 in VITS2
     (training/vits2/models.py, every generator), (K-u+1-i)//2 and 1-i in QuickVC (vc/models.py:428-430).  The engine lays out

@@ -29,6 +29,7 @@
 #include "vc.cuh"
 #include "spk.cuh"
 #include "contentvec.cuh"
+#include "dit.cuh"
 #include "resample.cuh"
 #include "owned.cuh"
 
@@ -360,7 +361,7 @@ struct vtts_engine {
   // phase tag, the first element of every key
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
-    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7
+    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -663,6 +664,26 @@ struct vtts_engine {
       e->conv_max_s = ms; e->conv_min_g = ming; e->conv_big_g = bigg; e->conv_auto_g = autog;
     }
   };
+
+  // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh), fp32 FFMA in every mode
+  ConvW st_cp[3], st_in, st_final;                 // cond_proj's three convs, in_proj over (x | cond), final_proj
+  std::vector<ConvW> st_lsc;                       // the long-skip convs over (x | skip)
+  std::vector<EncLayerW> st_blk;                   // qkv / o / ffn1 / ffn2 of each block; relk / relv point at zeros
+  const float *st_tw1 = nullptr, *st_tb1 = nullptr, *st_tw2 = nullptr, *st_tb2 = nullptr, *st_fw = nullptr, *st_fb = nullptr;
+  const float *st_aw1 = nullptr, *st_ab1 = nullptr, *st_aw2 = nullptr, *st_ab2 = nullptr;
+  const float *st_emb = nullptr, *st_fake_spk = nullptr, *st_fake_content = nullptr, *st_mel_mean = nullptr, *st_mel_std = nullptr;
+  // shape of the current call: NS sequences (B, or 2B with guidance: the unconditional branches follow the conditional
+  // ones), Ttot rows over all of them, the staged inputs' kinds
+  struct StPlan { int NS = 0, steps = 0, Ttot = 0; bool guided = false, noise = false, rows = false; } stp;
+  static constexpr int ST_PRM = 16 + 2 * VTTS_CFM_MAX_STEPS;     // prm[16], t of every step, dt of every step
+  Buf<int> d_sti;                                  // [len NS][off NS][sid NS]
+  Buf<float> d_stf, d_stmu, d_stnoise, d_stfilm, d_stada, d_strope, d_stxc, d_stp0, d_stp1, d_stcat[4], d_stx, d_stx2, d_sth, d_stn,
+      d_stqkv, d_stao, d_sty, d_stff, d_stv, d_stmel, d_stzero, d_stdbg_n, d_stdbg_qkv;
+  PinnedBuf<char> h_pin_st;
+  struct StPin { int* ints; float *prm, *spk, *mu, *noise; };
+  StPin st_layout();
+  void bind_stabletts();
+  void st_enqueue();
 
   // ---- resampling of recordings (vtts_resample; resample.cuh): the taps of each rate pair, uploaded on first use
   struct RsTaps { Buf<float> taps; int up = 0, down = 0, K = 0; };
@@ -2893,6 +2914,186 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// StableTTS flow-matching decoder (flow_matching.py:33-100,182-194; decoder.py:103-138; diffusion_transformer.py:98-116)
+// ---------------------------------------------------------------------------------------------------
+void vtts_engine::bind_stabletts() {
+  const vtts_config& c = cfg;
+  const int NC = c.st_noise, MC = c.st_cond, H = c.st_hidden, F = c.st_filter, NL = c.st_layers, G = c.st_spk_dim, k = c.st_kernel;
+  REQUIRE(NL >= 2 && NL % 2 == 0 && NL <= 8, VTTS_ERR_INVALID, "unsupported StableTTS decoder: the U-Net long skips need an even number of blocks (2..8)");
+  REQUIRE(c.st_heads >= 1 && H % c.st_heads == 0 && (H / c.st_heads) % 32 == 0 && H / c.st_heads <= 128 && (H / c.st_heads) % 4 == 0,
+          VTTS_ERR_INVALID, "unsupported StableTTS decoder: the attention kernels take head widths 32, 64, 96 and 128");
+  REQUIRE(H % CV_CK == 0 && H <= 32 * DIT_LN_MAXV && F % CV_CK == 0 && F <= DIT_MAXC && MC % CV_CK == 0 && (NC + H) % CV_CK == 0 && NC % 4 == 0 &&
+              G >= 1 && G <= DIT_MAXC && k % 2 == 1 && k >= 1 && k <= 15 && c.st_n_spks >= 1,
+          VTTS_ERR_INVALID, "unsupported StableTTS decoder (widths in multiples of 16, hidden up to 512, filter up to 1024, odd kernel)");
+  st_cp[0] = conv("st.cp0", MC, F, k);
+  st_cp[1] = conv("st.cp1", F, F, k);
+  st_cp[2] = conv("st.cp2", F, H, k);
+  st_in = conv("st.in", NC + H, H, 1);
+  st_final = conv("st.final", H, NC, 1);
+  st_tw1 = vec("st.time.w1", (size_t)F * H); st_tb1 = vec("st.time.b1", F);
+  st_tw2 = vec("st.time.w2", (size_t)H * F); st_tb2 = vec("st.time.b2", H);
+  st_fw = vec("st.film.w", (size_t)NL * 2 * H * H); st_fb = vec("st.film.b", (size_t)NL * 2 * H);
+  st_aw1 = vec("st.ada.w1", (size_t)NL * H * G); st_ab1 = vec("st.ada.b1", (size_t)NL * H);
+  st_aw2 = vec("st.ada.w2", (size_t)NL * 6 * H * H); st_ab2 = vec("st.ada.b2", (size_t)NL * 6 * H);
+  st_emb = vec("st.spk_emb", (size_t)c.st_n_spks * G);
+  st_fake_spk = vec("st.fake_spk", G);
+  st_fake_content = vec("st.fake_content", MC);
+  st_mel_mean = vec("st.mel_mean", 1);
+  st_mel_std = vec("st.mel_std", 1);
+  float* zero = ensure(d_stzero, (size_t)H);       // the attention's relative tables: no window, both terms exact zeros
+  CK(cudaMemsetAsync(zero, 0, d_stzero.cap * sizeof(float), stream));
+  st_blk.clear();
+  st_lsc.clear();
+  for (int l = 0; l < NL; ++l) {
+    const std::string p = "st.l" + std::to_string(l);
+    EncLayerW L;
+    L.heads = c.st_heads;
+    L.qkv = conv(p + ".qkv", H, 3 * H, 1);
+    L.o = conv(p + ".o", H, H, 1);
+    L.ffn1 = conv(p + ".ffn1", H, F, k);
+    L.ffn2 = conv(p + ".ffn2", F, H, k);
+    L.relk = L.relv = zero;
+    st_blk.push_back(L);
+    if (l >= NL / 2) st_lsc.push_back(conv("st.lsc" + std::to_string(l - NL / 2), 2 * H, H, k));
+  }
+}
+
+// Pinned staging of a vtts_cfm_decode call: ints [len NS][off NS][sid NS], then floats prm[16] | t[64] | dt[64] | speaker rows
+// [B][G] (when given) | mu rows [Tfrm][MC] packed as the engine's rows | noise rows [Tfrm][NC] (when given).  Every offset
+// follows from the graph key (batch, frame buckets, guided, input kinds).
+vtts_engine::StPin vtts_engine::st_layout() {
+  const vtts_config& c = cfg;
+  const size_t head = ((size_t)3 * stp.NS * sizeof(int) + 63) / 64 * 64;
+  const size_t nspk = stp.rows ? (size_t)B * c.st_spk_dim : 0, nmu = (size_t)Tfrm * c.st_cond, nn = stp.noise ? (size_t)Tfrm * c.st_noise : 0;
+  char* pin = ensure(h_pin_st, head + (ST_PRM + nspk + nmu + nn) * sizeof(float) + 64);
+  StPin pp;
+  pp.ints = reinterpret_cast<int*>(pin);
+  pp.prm = reinterpret_cast<float*>(pin + head);
+  pp.spk = pp.prm + ST_PRM;
+  pp.mu = pp.spk + nspk;
+  pp.noise = pp.mu + nmu;
+  return pp;
+}
+
+// The whole call: uploads, the hoisted conditioning (FiLM rows of every step, adaLN rows of every sequence, cond_proj of both
+// branches, the rotary table), then n Euler steps of the estimator over the ragged batch of both branches.  The step loop is
+// unrolled into the enqueue (and so into the call's graph): step k's FiLM rows and dt are addresses, not values.
+void vtts_engine::st_enqueue() {
+  const vtts_config& c = cfg;
+  const int NC = c.st_noise, MC = c.st_cond, H = c.st_hidden, F = c.st_filter, NL = c.st_layers, G = c.st_spk_dim;
+  const int NS = stp.NS, Bu = B, XW = NC + H, dk = H / c.st_heads, rd = dk / 2, nlsc = NL / 2;
+  // One fixed launch shape for every conv (no split-K over a cluster or thread groups) and one attention kernel: every row is
+  // summed in the same order whatever the batch, so an utterance's mel does not depend on what it is batched with.
+  SavedLaunch saved(this);
+  struct Restore { vtts_engine* e; int B, rows; ~Restore() { e->B = B; e->attn_rows = rows; } } restore{this, B, attn_rows};
+  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
+  attn_rows = 4;
+  StPin pp = st_layout();
+  const size_t T = (size_t)stp.Ttot;
+  int* di = ensure(d_sti, 3 * NS);
+  float* df = ensure(d_stf, ST_PRM + (size_t)Bu * G);
+  float* mu = ensure(d_stmu, T * MC);
+  CK(cudaMemcpyAsync(di, pp.ints, 3 * NS * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(df, pp.prm, (ST_PRM + (stp.rows ? (size_t)Bu * G : 0)) * sizeof(float), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(mu, pp.mu, (size_t)Tfrm * MC * sizeof(float), cudaMemcpyHostToDevice, stream));
+  float* noise = nullptr;
+  if (stp.noise) {
+    noise = ensure(d_stnoise, (size_t)Tfrm * NC);
+    CK(cudaMemcpyAsync(noise, pp.noise, (size_t)Tfrm * NC * sizeof(float), cudaMemcpyHostToDevice, stream));
+  }
+  const int *lens = di, *offs = di + NS, *sid = di + 2 * NS;
+  const float *prm = df, *ts = df + 16, *dts = df + 16 + VTTS_CFM_MAX_STEPS;
+  B = NS;                                           // launch_attn and the launch heuristics read the member
+  v_frm_len.assign(NS, maxFrm);
+  {
+    std::vector<int> two(h_frm_len.begin(), h_frm_len.begin() + Bu);
+    if (stp.guided) two.insert(two.end(), h_frm_len.begin(), h_frm_len.begin() + Bu);
+    h_frm_len = two;
+  }
+  float* film = ensure(d_stfilm, (size_t)VTTS_CFM_MAX_STEPS * NL * 2 * H);
+  float* ada = ensure(d_stada, (size_t)NS * NL * 6 * H);
+  float2* rope = reinterpret_cast<float2*>(ensure(d_strope, (size_t)maxFrm * rd));
+  float *xc = ensure(d_stxc, T * XW), *p0 = ensure(d_stp0, T * F), *p1 = ensure(d_stp1, T * F);
+  float* cat[4];
+  for (int j = 0; j < nlsc; ++j) cat[j] = ensure(d_stcat[j], T * 2 * H);
+  float *X = ensure(d_stx, T * H), *X2 = ensure(d_stx2, T * H), *Hb = ensure(d_sth, T * H), *N = ensure(d_stn, T * H);
+  float *QKV = ensure(d_stqkv, T * 3 * H), *AO = ensure(d_stao, T * H), *Y = ensure(d_sty, T * H), *FF = ensure(d_stff, T * F);
+  float *V = ensure(d_stv, T * NC), *mel = ensure(d_stmel, (size_t)Tfrm * NC);
+  const dim3 gs(maxFrm, NS), gn((maxFrm + DIT_LN_WARPS - 1) / DIT_LN_WARPS, NS);
+  // ---- once per call
+  klaunch(dit_init_kernel, gs, dim3(128), (size_t)0, (const float*)noise, prm, st_fake_content, xc, XW, NC, mu, MC, lens, offs, Bu);
+  klaunch(dit_time_kernel, dim3(stp.steps), dim3(256), (size_t)0, ts, st_tw1, st_tb1, st_tw2, st_tb2, st_fw, st_fb, H, F, NL, film);
+  klaunch(dit_ada_kernel, dim3(NL, NS), dim3(256), (size_t)0, st_emb, st_fake_spk, stp.rows ? (const float*)(df + ST_PRM) : (const float*)nullptr,
+          sid, st_aw1, st_ab1, st_aw2, st_ab2, G, H, NL, c.st_n_spks, ada);
+  klaunch(dit_rope_table_kernel, dim3((maxFrm * (rd / 2) + 127) / 128), dim3(128), (size_t)0, rope, maxFrm, rd);
+  CK(cudaGetLastError());
+  launches += 4;
+  auto silu = [&](float* y, int width) {
+    klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, y, width, lens, offs);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff) {
+    launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, lens, offs, maxFrm, NS);
+  };
+  // cond_proj (decoder.py:121; not masked: zero padded at each sequence's own ends) into the cond columns of the in_proj operand
+  cv(st_cp[0], mu, MC, p0, F, 0);
+  silu(p0, F);
+  cv(st_cp[1], p0, F, p1, F, 0);
+  silu(p1, F);
+  cv(st_cp[2], p1, F, xc, XW, NC);
+  const int ald = NL * 6 * H;
+  auto norm = [&](const float* a, int lda, const float* fl, const float* y, int l, int gate, int shift, int scale) {
+    klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, (const float*)(ada + (size_t)l * 6 * H), ald, gate * H, shift * H,
+            scale * H, 1e-5f, Hb, N, lens, offs, H);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  // DitWrapper (decoder.py:15-18) of block l at step s: x rows at xin (pitch ldi) -> xout (pitch ldo)
+  auto block = [&](int l, int s, const float* xin, int ldi, float* xout, int ldo) {
+    const EncLayerW& L = st_blk[l];
+    norm(xin, ldi, film + ((size_t)s * NL + l) * 2 * H, nullptr, l, 2, 0, 1);
+    const bool tap = (debug_flags & 1) && l == 0 && s == 0;
+    if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_n, T * H), N, T * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    cv(L.qkv, N, H, QKV, 3 * H, 0);
+    klaunch(dit_rope_kernel, gs, dim3(128), (size_t)0, QKV, (const float2*)rope, c.st_heads, dk, rd, lens, offs);
+    CK(cudaGetLastError());
+    ++launches;
+    if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_qkv, T * 3 * H), QKV, T * 3 * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    launch_attn(QKV, AO, L, H, lens, offs, maxFrm, nullptr);
+    cv(L.o, AO, H, Y, H, 0);
+    norm(Hb, H, nullptr, Y, l, 2, 3, 4);
+    cv(L.ffn1, N, H, FF, F, 0);
+    silu(FF, F);
+    cv(L.ffn2, FF, F, Y, H, 0);
+    klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)Hb, (const float*)Y, (const float*)(ada + (size_t)l * 6 * H), ald, 5 * H, xout, ldo,
+            lens, offs, H);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  for (int s = 0; s < stp.steps; ++s) {
+    // in_proj over (x | cond) (decoder.py:123-124) -> the skip half of the last long-skip operand
+    cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H);
+    // blocks 0 .. NL/2-1 leave their input as a skip (decoder.py:130-131): block i reads the skip half of cat[nlsc-1-i] and
+    // writes the skip half of the next one; the last of them writes the x half of cat[0]
+    for (int i = 0; i < nlsc; ++i)
+      block(i, s, cat[nlsc - 1 - i] + H, 2 * H, i + 1 < nlsc ? cat[nlsc - 2 - i] + H : cat[0], 2 * H);
+    // blocks NL/2 ..: the long-skip conv over (x | skip) (decoder.py:133-134), then the block
+    for (int j = 0; j < nlsc; ++j) {
+      cv(st_lsc[j], cat[j], 2 * H, X, H, 0);
+      const bool last = j + 1 == nlsc;
+      block(nlsc + j, s, X, H, last ? X2 : cat[j + 1], last ? H : 2 * H);
+    }
+    cv(st_final, X2, H, V, NC, 0);
+    const bool end = s + 1 == stp.steps;
+    klaunch(dit_euler_kernel, dim3(maxFrm, Bu), dim3(128), (size_t)0, (const float*)V, xc, XW, NC, dts + s, prm, stp.guided ? 1 : 0,
+            end ? mel : (float*)nullptr, st_mel_mean, st_mel_std, lens, offs, Bu);
+    CK(cudaGetLastError());
+    ++launches;
+  }
+}
+
 // Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
 // d_sseq (host copy); max_len: the longest slice.
 void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int max_len) {
@@ -2987,8 +3188,8 @@ int guarded(vtts_handle h, Fn fn, int mode = G_ATOMIC, int family = VTTS_FAMILY_
   if (!h) return VTTS_ERR_INVALID;
   std::unique_lock<std::mutex> lk(h->mu);
   if (family != ANY_FAMILY && h->cfg.model_family != family) {
-    h->err = h->cfg.model_family == VTTS_FAMILY_QUICKVC ? "this entry point serves VITS2 models; the engine holds a QuickVC model"
-                                                        : "this entry point serves QuickVC models; the engine holds a VITS2 model";
+    static const char* const names[] = {"VITS2", "QuickVC", "StableTTS"};
+    h->err = std::string("this entry point serves ") + names[family] + " models; the engine holds a " + names[h->cfg.model_family] + " model";
     return VTTS_ERR_INVALID;
   }
   const std::thread::id me = std::this_thread::get_id();
@@ -3502,6 +3703,75 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const float*
   }
 }
 
+// StableTTS flow-matching decoder through host buffers (vtts_cfm_decode).
+static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int B, int64_t mu_ld, const int64_t* sid,
+                            const float* spk_rows, int n, float temperature, float s, const float* noise, int64_t noise_ld, uint64_t seed,
+                            float* mel_out, int64_t mel_ld, int denormalise) {
+  const vtts_config& c = h->cfg;
+  REQUIRE(B >= 1 && B <= 8192 && mu_ld >= 1 && mu_ld < (1LL << 24), VTTS_ERR_INVALID, "bad batch size / mu_ld");
+  REQUIRE(n >= 1 && n <= VTTS_CFM_MAX_STEPS, VTTS_ERR_INVALID, "n_timesteps must be in [1, " + std::to_string(VTTS_CFM_MAX_STEPS) + "]");
+  REQUIRE(std::isfinite(temperature), VTTS_ERR_INVALID, "temperature must be finite");
+  REQUIRE(std::isfinite(s) && s >= 0.f, VTTS_ERR_INVALID, "guidance_scale must be finite and >= 0");
+  REQUIRE(sid || spk_rows, VTTS_ERR_INVALID, "a speaker is required: sid or spk_rows");
+  std::vector<int> frames(B);
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lengths[b] >= 1 && lengths[b] <= mu_ld, VTTS_ERR_INVALID, "lengths must be in [1, mu_ld]");
+    REQUIRE(spk_rows || (sid[b] >= 0 && sid[b] < c.st_n_spks), VTTS_ERR_INVALID, "speaker id out of range [0, n_spks)");
+    frames[b] = (int)lengths[b];
+  }
+  const int real_max = *std::max_element(frames.begin(), frames.end());
+  REQUIRE(mel_ld >= real_max, VTTS_ERR_CAPACITY, "mel_ld is smaller than the longest utterance");
+  REQUIRE(!noise || noise_ld >= real_max, VTTS_ERR_CAPACITY, "noise has fewer frames than the longest utterance");
+  h->B = B;
+  h->have_durations = false;
+  h->have_latent = false;
+  h->pack_frames(frames);
+  vtts_engine::StPlan& P = h->stp;
+  P.guided = s > 0.f;
+  P.NS = P.guided ? 2 * B : B;
+  P.steps = n;
+  P.noise = noise != nullptr;
+  P.rows = spk_rows != nullptr;
+  P.Ttot = P.guided ? 2 * h->Tfrm + SEQ_GAP : h->Tfrm;
+  REQUIRE((int64_t)P.Ttot * 3 * c.st_filter < (int64_t)INT32_MAX, VTTS_ERR_INVALID, "the batch holds too many frames for one call");
+  const int NC = c.st_noise, MC = c.st_cond, G = c.st_spk_dim, NS = P.NS;
+  const vtts_engine::StPin pp = h->st_layout();
+  for (int q = 0; q < NS; ++q) {
+    const int b = q < B ? q : q - B;
+    pp.ints[q] = frames[b];
+    pp.ints[NS + q] = h->h_frm_off[b] + (q < B ? 0 : h->Tfrm + SEQ_GAP);
+    pp.ints[2 * NS + q] = q < B ? (sid ? (int)sid[b] : 0) : -1;
+  }
+  const float sc[3] = {temperature, s, denormalise ? 1.f : 0.f};
+  vtts_engine::put_scalars(pp.prm, vtts_engine::ST_PRM, sc, 3, seed);
+  {   // t_span = 1 - cos(linspace(0, 1, n + 1) pi / 2) and the Euler loop's t and dt, in the reference's fp32 steps
+      // (flow_matching.py:54-55,87-98: t accumulates, dt is the distance from it to the next knot)
+    std::vector<float> span(n + 1);
+    const float step = 1.f / (float)n;
+    for (int i = 0; i <= n; ++i) {
+      const float lin = i < (n + 1) / 2 ? step * (float)i : 1.f - step * (float)(n - i);
+      const float a = (lin * 0.5f) * (float)M_PI;
+      span[i] = 1.f - (float)std::cos((double)a);
+    }
+    float t = span[0], dt = span[1] - span[0];
+    for (int k = 0; k < n; ++k) {
+      pp.prm[16 + k] = t;
+      pp.prm[16 + VTTS_CFM_MAX_STEPS + k] = dt;
+      t = t + dt;
+      if (k + 1 < n) dt = span[k + 2] - t;
+    }
+  }
+  if (spk_rows) memcpy(pp.spk, spk_rows, (size_t)B * G * sizeof(float));
+  for (int b = 0; b < B; ++b) {
+    const size_t o = (size_t)h->h_frm_off[b];
+    memcpy(pp.mu + o * MC, mu + (size_t)b * mu_ld * MC, (size_t)frames[b] * MC * sizeof(float));
+    if (noise) memcpy(pp.noise + o * NC, noise + (size_t)b * noise_ld * NC, (size_t)frames[b] * NC * sizeof(float));
+  }
+  h->run_graphed({vtts_engine::TAG_CFM, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, P.rows ? 1 : 0}, [&] { h->st_enqueue(); });
+  read_clips(h, (const float*)h->d_stmel.p, (size_t)h->real_Tfrm * NC, (size_t)h->Tfrm * NC, h->h_frm_off.data(), frames, NC, mel_out,
+             mel_ld * NC);
+}
+
 // I0 by its power series (the Kaiser window's; np.i0 within a few ulps for the beta 5 of resample_poly)
 static double bessel_i0(double x) {
   double sum = 1.0, term = 1.0;
@@ -3758,8 +4028,9 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     if (const char* e = getenv("VTTS_SPEC_MARGIN")) h->spec_margin = (float)atof(e);      // (< 1 forces mispredictions: tests)
     if (const char* e = getenv("VTTS_CAPTURE_FIRST")) h->capture_on_first = atoi(e) != 0;   // 0: capture a bucket's graph on its second call          // 0: never enqueue phase 2 before the lengths are known    // 0: size everything by the exact lengths
     if (const char* e = getenv("VTTS_PREFETCH")) h->use_prefetch = atoi(e) != 0;
-    REQUIRE(cfg->model_family == VTTS_FAMILY_VITS2 || cfg->model_family == VTTS_FAMILY_QUICKVC, VTTS_ERR_INVALID, "unknown model family");
+    REQUIRE(cfg->model_family >= VTTS_FAMILY_VITS2 && cfg->model_family <= VTTS_FAMILY_STABLETTS, VTTS_ERR_INVALID, "unknown model family");
     if (cfg->model_family == VTTS_FAMILY_QUICKVC) h->bind_quickvc();
+    else if (cfg->model_family == VTTS_FAMILY_STABLETTS) h->bind_stabletts();
     else h->bind_weights();
     h->build_prefetch_list();
     CK(cudaMemsetAsync(h->ensure(h->d_done_ctr, 4), 0, 4 * sizeof(int), h->stream));     // ticket counter of duration_kernel (self-resetting)
@@ -4109,6 +4380,12 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "cv_feat") { src = h->d_cvl[(c.cv_n_conv - 1) & 1].p; n = (size_t)h->cvp.tot0 / h->cv_P * c.cv_conv_dim; }
     else if (nm == "cv_gn_sum") { src = h->d_cvps.p; n = (size_t)h->B * h->cvp.MC * c.cv_conv_dim; }
     else if (nm == "cv_gn_sq") { src = h->d_cvpq.p; n = (size_t)h->B * h->cvp.MC * c.cv_conv_dim; }
+    else if (nm == "st_film") { src = h->d_stfilm.p; n = (size_t)h->stp.steps * c.st_layers * 2 * c.st_hidden; }
+    else if (nm == "st_ada") { src = h->d_stada.p; n = (size_t)h->stp.NS * c.st_layers * 6 * c.st_hidden; }
+    else if (nm == "st_cond") { src = h->d_stxc.p; n = (size_t)h->stp.Ttot * (c.st_noise + c.st_hidden); }
+    else if (nm == "st_rope") { src = h->d_strope.p; n = (size_t)h->maxFrm * (c.st_hidden / c.st_heads / 2); }
+    else if (nm == "st_norm1") { src = h->d_stdbg_n.p; n = (size_t)h->stp.Ttot * c.st_hidden; }
+    else if (nm == "st_qkv") { src = h->d_stdbg_qkv.p; n = (size_t)h->stp.Ttot * 3 * c.st_hidden; }
     else if (nm == "cv_enc_in") { src = h->d_cvdbg.p; n = (size_t)h->cvp.tot0 / h->cv_P * c.cv_hidden; }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);
@@ -4155,6 +4432,14 @@ int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav
   if (!wav || !wav_lengths || !out_wav || !out_frames) return VTTS_ERR_INVALID;
   return guarded(h, [&] { impl_quickvc_convert(h, nullptr, wav, wav_lengths, B, wav_ld, g, noise_scale, noise, noise_ld, seed, out_wav,
                                                out_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int B, int64_t mu_ld, const int64_t* sid,
+                    const float* spk_rows, int n_timesteps, float temperature, float guidance_scale, const float* noise,
+                    int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld, int denormalise) {
+  if (!mu || !lengths || !mel_out) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_cfm_decode(h, mu, lengths, B, mu_ld, sid, spk_rows, n_timesteps, temperature, guidance_scale, noise, noise_ld,
+                                          seed, mel_out, mel_ld, denormalise); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
 }
 
 int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,

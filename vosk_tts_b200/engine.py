@@ -41,6 +41,9 @@ class VttsConfig(C.Structure):
         ("filter_length", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32), ("n_mel_channels", C.c_int32),
         ("mel_fmin", C.c_float), ("mel_fmax", C.c_float),
         ("model_family", C.c_int32),
+        ("st_noise", C.c_int32), ("st_cond", C.c_int32), ("st_hidden", C.c_int32), ("st_filter", C.c_int32),
+        ("st_layers", C.c_int32), ("st_heads", C.c_int32), ("st_kernel", C.c_int32), ("st_spk_dim", C.c_int32),
+        ("st_n_spks", C.c_int32),
         ("cv_layers", C.c_int32), ("cv_hidden", C.c_int32), ("cv_heads", C.c_int32), ("cv_ffn", C.c_int32),
         ("cv_conv_dim", C.c_int32), ("cv_n_conv", C.c_int32), ("cv_conv_kernel", C.c_int32 * 8), ("cv_conv_stride", C.c_int32 * 8),
         ("cv_pos_k", C.c_int32), ("cv_pos_groups", C.c_int32), ("cv_ln_eps", C.c_float), ("cv_gn_eps", C.c_float),
@@ -56,9 +59,10 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
-           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample"]
+           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode"]
 
-MODEL_FAMILIES = {"vits2": 0, "quickvc": 1}    # vtts_config.model_family
+MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
+CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
 
 CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
 
@@ -236,6 +240,9 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_live_bytes.restype = i32
     lib.vtts_resample.argtypes = [vp, vp, vp, i32, C.c_int64, i32, i32, C.c_float, vp, C.c_int64, vp, vp]
     lib.vtts_resample.restype = i32
+    lib.vtts_cfm_decode.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, i32, C.c_float, C.c_float, vp, C.c_int64, C.c_uint64, vp,
+                                    C.c_int64, i32]
+    lib.vtts_cfm_decode.restype = i32
     _LIB = lib
     return lib
 
@@ -267,6 +274,14 @@ def live_bytes():
 
 def make_c_config(cfg, precision=0):
     c = VttsConfig()
+    if cfg.get("model_family") == "stabletts":        # the flow-matching decoder reads none of the VITS2 fields
+        c.model_family = MODEL_FAMILIES["stabletts"]
+        c.precision = int(precision)
+        for dst, src in (("st_noise", "noise_channels"), ("st_cond", "cond_channels"), ("st_hidden", "hidden_channels"),
+                         ("st_filter", "filter_channels"), ("st_layers", "n_layers"), ("st_heads", "n_heads"),
+                         ("st_kernel", "kernel_size"), ("st_spk_dim", "spk_emb_dim"), ("st_n_spks", "n_spks")):
+            setattr(c, dst, int(cfg[src]))
+        return c
     for k in ("n_vocab", "n_speakers", "gin_channels", "inter_channels", "hidden_channels", "filter_channels",
               "n_heads", "n_layers", "kernel_size", "window_size", "cond_layer_idx", "flow_kernel_size",
               "flow_dilation_rate", "flow_wn_layers", "flow_n_flows", "dp_filter_channels", "dp_kernel_size",
@@ -663,6 +678,33 @@ class Engine:
         return int(max_samples)
 
     # ---- resampling of recordings (librosa.load(path, sr=...) and librosa.effects.trim, as vc/convert.py:65-66 uses them)
+    def cfm_decode(self, mu, sid=None, lengths=None, n_timesteps=10, temperature=1.0, guidance_scale=0.5, noise=None, seed=0,
+                   spk_rows=None, denormalise=False):
+        """StableTTS flow-matching decoder (vtts_cfm_decode): mu frame-major [T, cond], [B, T, cond] with `lengths`, or a list
+        of ragged [T_b, cond] items; sid int [B] (or one for all), or spk_rows float [B, spk_emb_dim]; noise like mu with
+        noise_channels columns, or None for Philox(seed).  Returns (mel float32 [B, max T, noise_channels] frame-major, zeros
+        past each utterance; lengths int64 [B]); denormalise: mel * mel_std + mel_mean."""
+        mu, lengths = _batch(mu, lengths, 3, t_axis=1, ragged=True)
+        B, T = mu.shape[0], mu.shape[1]
+        NC, MC, G = (int(self.cfg[k]) for k in ("noise_channels", "cond_channels", "spk_emb_dim"))
+        if mu.shape[2] != MC:
+            raise ValueError("mu must be frame-major [.., T, %d]" % MC)
+        noise_ld = 0
+        if noise is not None:
+            noise, _ = _batch(noise, None, 3, t_axis=1, ragged=True)
+            if noise.shape[0] != B or noise.shape[2] != NC:
+                raise ValueError("noise must be frame-major [B, >= T, %d]" % NC)
+            noise_ld = noise.shape[1]
+        if sid is not None:
+            sid = np.ascontiguousarray(np.broadcast_to(np.asarray(sid, np.int64).reshape(-1), (B,)))
+        if spk_rows is not None:
+            spk_rows = _per_item(spk_rows, B, G)
+        mel = np.zeros((B, T, NC), np.float32)
+        self._check(self.lib.vtts_cfm_decode(self.h, _ptr(mu), _ptr(lengths), B, T, _ptr(sid), _ptr(spk_rows), int(n_timesteps),
+                                             float(temperature), float(guidance_scale), _ptr(noise), noise_ld, int(seed),
+                                             _ptr(mel), T, int(bool(denormalise))))
+        return mel, lengths
+
     def resample(self, wav, from_rate, to_rate, lengths=None, trim_top_db=None, return_bounds=False):
         """Clips at `from_rate` Hz resampled to `to_rate` Hz (vtts_resample: scipy.signal.resample_poly's filter, not soxr), and
         with `trim_top_db` trimmed of leading and trailing silence as librosa.effects.trim(y, top_db=trim_top_db) does.  wav:

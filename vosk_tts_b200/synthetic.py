@@ -19,6 +19,7 @@ tensor name), so the values do not depend on enumeration order or torch's global
 import math
 import zlib
 
+import numpy as np
 import torch
 
 
@@ -317,4 +318,38 @@ def make_random_contentvec(seed=1234, cv=None):
     nrm = v.norm(dim=(0, 1), keepdim=True)
     sd[pos + "weight_g"] = (nrm * (1.0 + 0.15 * torch.randn(nrm.shape, generator=_gen(pos + "weight_g", seed)))).float().contiguous()
     sd[pos + "bias"] = (torch.randn((H,), generator=_gen(pos + "bias", seed)) * 0.05).float().contiguous()
+    return sd
+
+
+def make_random_stabletts_cfm(cfg, seed=1234):
+    """The tensors weights.pack_stabletts_cfm reads of a MatchaTTS state dict (decoder.estimator.*, spk_emb.weight,
+    fake_speaker, fake_content, mel_mean, mel_std), CPU fp32, deterministic for (cfg, seed); every tensor is seeded by its name.
+    Weights are drawn at 1 / sqrt(fan-in) so that activations keep their scale through the blocks.  The last adaLN linear,
+    which the reference initialises to zero (decoder.py:98-101), is random here: with zeros every gate is 0 and every block
+    the identity, and a comparison would prove nothing."""
+    NC, MC, H, F, NL, G = (int(cfg[k]) for k in ("noise_channels", "cond_channels", "hidden_channels", "filter_channels", "n_layers",
+                                                 "spk_emb_dim"))
+    k = int(cfg["kernel_size"])
+    e = "decoder.estimator."
+    shapes = [(e + "time_mlp.layer.0", (F, H)), (e + "time_mlp.layer.2", (H, F)), (e + "in_proj", (H, NC + H, 1)),
+              (e + "final_proj", (NC, H, 1)), (e + "cond_proj.0", (F, MC, k)), (e + "cond_proj.2", (F, F, k)),
+              (e + "cond_proj.4", (H, F, k))]
+    for l in range(NL):
+        b = e + "blocks.%d." % l
+        shapes += [(b + "time_fusion.film", (2 * H, H, 1)), (b + "block.adaLN_modulation.0", (H, G)),
+                   (b + "block.adaLN_modulation.2", (6 * H, H)), (b + "block.mlp.conv_1", (F, H, k)), (b + "block.mlp.conv_2", (H, F, k))]
+        shapes += [(b + "block.attn.conv_%s" % n, (H, H, 1)) for n in "qkvo"]
+    shapes += [(e + "lsc_layers.%d" % j, (H, 2 * H, k)) for j in range(NL // 2)]
+    sd = {}
+    for name, shape in shapes:
+        fan = int(np.prod(shape[1:]))
+        sd[name + ".weight"] = (torch.randn(shape, generator=_gen(name + ".weight", seed)) / math.sqrt(fan)).float().contiguous()
+        sd[name + ".bias"] = (torch.randn(shape[0], generator=_gen(name + ".bias", seed)) * 0.1).float().contiguous()
+    for l in range(NL):      # FiLM's gamma around 1 (gamma * x + beta)
+        sd[e + "blocks.%d.time_fusion.film.bias" % l][:H] += 1.0
+    for name, shape, scale in (("spk_emb.weight", (int(cfg["n_spks"]), G), 1.0), ("fake_speaker", (1, G), 0.5),
+                               ("fake_content", (1, MC, 1), 0.5)):
+        sd[name] = (torch.randn(shape, generator=_gen(name, seed)) * scale).float().contiguous()
+    sd["mel_mean"] = torch.tensor(-5.5)
+    sd["mel_std"] = torch.tensor(2.1)
     return sd

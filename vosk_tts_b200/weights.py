@@ -673,3 +673,55 @@ def pack_quickvc(w, cfg, tc=True, precision=None, contentvec=None, cv=None):
         _pack_contentvec(P, fold_contentvec_pos_conv(contentvec) if CV_POS + "weight" not in contentvec else contentvec,
                          cv or _config.contentvec_config(), tc and precision != 0)
     return P.finish()
+
+
+def pack_stabletts_cfm(sd, cfg):
+    """The flow-matching decoder of a MatchaTTS (StableTTS) state dict -> (blob, manifest) of a model_family "stabletts" engine.
+    sd: the checkpoint's `state_dict` entry (keys decoder.estimator.*, spk_emb.weight, fake_speaker, fake_content, mel_mean,
+    mel_std); cfg: config.stabletts_cfm_config.  Convs go in the FFMA layout (q, k, v stacked into one 1x1 conv), the small
+    linears of the conditioning path (time_mlp, each block's film conv and adaLN_modulation) row-major [out][in] and stacked
+    over the blocks.  Everything is fp32: the decoder runs on the FFMA pipe in every precision mode, so there are no
+    mode-dependent split planes to add yet."""
+    g = lambda k: sd[k].detach().cpu().float().numpy() if hasattr(sd[k], "detach") else np.asarray(sd[k], np.float32)
+    e = "decoder.estimator."
+    NC, MC, H, F, NL, G = (int(cfg[k]) for k in ("noise_channels", "cond_channels", "hidden_channels", "filter_channels", "n_layers",
+                                                 "spk_emb_dim"))
+    k = int(cfg["kernel_size"])
+
+    def want(name, shape):
+        a = g(name)
+        if tuple(a.shape) != tuple(shape):
+            raise ValueError("%s has shape %s, expected %s" % (name, tuple(a.shape), tuple(shape)))
+        return a
+
+    P = _Packer()
+    for i, (j, co, ci) in enumerate(((0, F, MC), (2, F, F), (4, H, F))):
+        P.conv("st.cp%d" % i, want(e + "cond_proj.%d.weight" % j, (co, ci, k)), want(e + "cond_proj.%d.bias" % j, (co,)))
+    P.conv("st.in", want(e + "in_proj.weight", (H, NC + H, 1)), g(e + "in_proj.bias"))
+    P.conv("st.final", want(e + "final_proj.weight", (NC, H, 1)), g(e + "final_proj.bias"))
+    P.add("st.time.w1", want(e + "time_mlp.layer.0.weight", (F, H)))
+    P.add("st.time.b1", g(e + "time_mlp.layer.0.bias"))
+    P.add("st.time.w2", want(e + "time_mlp.layer.2.weight", (H, F)))
+    P.add("st.time.b2", g(e + "time_mlp.layer.2.bias"))
+    b = e + "blocks.%d."
+    P.add("st.film.w", np.stack([want(b % l + "time_fusion.film.weight", (2 * H, H, 1))[:, :, 0] for l in range(NL)]))
+    P.add("st.film.b", np.stack([g(b % l + "time_fusion.film.bias") for l in range(NL)]))
+    P.add("st.ada.w1", np.stack([want(b % l + "block.adaLN_modulation.0.weight", (H, G)) for l in range(NL)]))
+    P.add("st.ada.b1", np.stack([g(b % l + "block.adaLN_modulation.0.bias") for l in range(NL)]))
+    P.add("st.ada.w2", np.stack([want(b % l + "block.adaLN_modulation.2.weight", (6 * H, H)) for l in range(NL)]))
+    P.add("st.ada.b2", np.stack([g(b % l + "block.adaLN_modulation.2.bias") for l in range(NL)]))
+    P.add("st.spk_emb", want("spk_emb.weight", (int(cfg["n_spks"]), G)))
+    P.add("st.fake_spk", want("fake_speaker", (1, G)))
+    P.add("st.fake_content", want("fake_content", (1, MC, 1)))
+    P.add("st.mel_mean", np.asarray(g("mel_mean"), np.float32).reshape(1))
+    P.add("st.mel_std", np.asarray(g("mel_std"), np.float32).reshape(1))
+    for l in range(NL):
+        a = b % l + "block.attn.conv_%s."
+        P.conv("st.l%d.qkv" % l, np.concatenate([want(a % n + "weight", (H, H, 1)) for n in "qkv"], 0),
+               np.concatenate([g(a % n + "bias") for n in "qkv"]))
+        P.conv("st.l%d.o" % l, want(a % "o" + "weight", (H, H, 1)), g(a % "o" + "bias"))
+        P.conv("st.l%d.ffn1" % l, want(b % l + "block.mlp.conv_1.weight", (F, H, k)), g(b % l + "block.mlp.conv_1.bias"))
+        P.conv("st.l%d.ffn2" % l, want(b % l + "block.mlp.conv_2.weight", (H, F, k)), g(b % l + "block.mlp.conv_2.bias"))
+    for j in range(NL // 2):
+        P.conv("st.lsc%d" % j, want(e + "lsc_layers.%d.weight" % j, (H, 2 * H, k)), g(e + "lsc_layers.%d.bias" % j))
+    return P.finish()
