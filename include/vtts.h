@@ -71,14 +71,21 @@ typedef struct vtts_config {
   float mel_fmin, mel_fmax;        /* (the mel filter bank itself is packed into the blob) */
   /* Model family of the blob: 0 = VITS2 SynthesizerTrn (every entry point above and below except the QuickVC ones),
    * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding* and vtts_quickvc_convert,
-   * 2 = StableTTS (the flow-matching decoder; weights.pack_stabletts_cfm), which serves vtts_cfm_decode.  The entry points of
-   * one family return VTTS_ERR_INVALID on an engine of another. */
+   * 2 = StableTTS (weights.pack_stabletts_cfm: the flow-matching decoder, which serves vtts_cfm_decode; weights.pack_stabletts:
+   * the text encoder as well, which also serves vtts_stabletts_synthesise).  The entry points of one family return
+   * VTTS_ERR_INVALID on an engine of another. */
   int32_t model_family;
   /* StableTTS flow-matching decoder (model_family 2; CFM of training/stabletts/matcha/models/components/flow_matching.py:301,
    * weights.pack_stabletts_cfm): vtts_cfm_decode.  The other families leave these 0. */
   int32_t st_noise, st_cond, st_hidden, st_filter;         /* mel channels 80, encoder output 256, hidden 384, FFN / prenet 768 */
   int32_t st_layers, st_heads, st_kernel;                  /* 6 DitWrapper blocks (even: U-Net long skips), 4 heads, k = 3 */
   int32_t st_spk_dim, st_n_spks;                           /* speaker embedding width 128, rows of spk_emb */
+  /* StableTTS text encoder and durations (TextEncoder of components/text_encoder.py:55-139; model_family 2 blobs of
+   * weights.pack_stabletts): vtts_stabletts_synthesise.  st_enc_layers == 0: the blob holds the decoder only. */
+  int32_t st_n_vocab, st_streams;                          /* rows of emb / punc_emb; id streams per token: 5 (1 + 4 punctuation) */
+  int32_t st_emb_dim, st_punc_dim, st_bert_dim, st_bert_proj;  /* 160, 16, 768 -> 32: 160 + 4 x 16 + 32 = st_cond */
+  int32_t st_enc_hidden, st_enc_filter, st_enc_layers, st_enc_heads, st_enc_kernel;  /* both stacks: 256, 1024, 4 blocks, 4 heads, k = 3 */
+  int32_t st_dur_channels;                                 /* dp_encoder's proj: 50 channels whose sigmoids sum to a duration */
   /* ContentVec (HubertModel of vc/contentvec.py, transformers' HubertConfig; QuickVC engines whose blob carries cv.*):
    * vtts_content_units / vtts_quickvc_convert_wav.  cv_layers == 0: no ContentVec. */
   int32_t cv_layers, cv_hidden, cv_heads, cv_ffn;          /* transformer: 12 post-LN layers, 768 wide, 12 heads, FFN 3072 */
@@ -464,6 +471,43 @@ int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B
 int vtts_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int B, int64_t mu_ld, const int64_t* sid,
                     const float* spk_rows, int n_timesteps, float temperature, float guidance_scale, const float* noise,
                     int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld, int denormalise);
+
+/* StableTTS text-to-mel (MatchaTTS.synthesise, training/stabletts/matcha/models/matcha_tts.py:93-211; the graph
+ * matcha/onnx/export.py exports without a vocoder): multistream ids, BERT features and pause durations in, durations and mel
+ * out.  x = (emb(ids[0]) sqrt(160) | punc_emb(ids[1..4]) sqrt(16) | bert_proj(bert)); dp_encoder(x, dur_spk_emb[sid]) -> 50
+ * channels; a token's duration is the sum of their sigmoids, or its pause where that is not 0, times length_scale, rounded
+ * half to even, at least 1; mu_y = x expanded by the durations; the decoder of vtts_cfm_decode refines it; every frame of a
+ * token with a pause > 0 takes the mel of the utterance's frame 0.
+ * Each utterance is processed as if alone: its own frame 0 is its silence frame (the reference, called with one utterance,
+ * takes utterance 0's), and the decoder's unmasked stages (noise, cond_proj, in_proj) run on its own frame count rounded up
+ * to a multiple of 4, as synthesise pads it (matcha_tts.py:162-165).  Durations and mel are bit-identical in any batch.
+ *   ids          int64 [B, st_streams, t_max], each in [0, st_n_vocab); utterance b = the first id_lengths[b] columns
+ *   bert         float [B, t_max, st_bert_dim], token-major
+ *   pause        float [B, t_max] (phone_duration_extra, frames before length_scale; 0: predict), or NULL for none
+ *   sid          int64 [B] rows of spk_emb and dur_spk_emb
+ *   noise        float [B, noise_ld, st_noise] frame-major, standing in for torch.randn over the padded frame axis
+ *                (flow_matching.py:54): ceil4(frames) rows per utterance are read; or NULL for Philox(seed)
+ *   mel_out      out float [B, mel_ld, st_noise] frame-major, mel_lengths[b] frames of utterance b; the rest is not written
+ *   mel_lengths  out int64 [B]
+ *   durations    out int32 [B, t_max] frames of every token (0 past id_lengths[b]), or NULL
+ *   prior_out    out float [B, mel_ld, st_noise]: the mel encoder's output expanded to frames (encoder_outputs; mel_enc with
+ *                denormalise), or NULL: the mel encoder then does not run
+ *   denormalise  != 0: mel * mel_std + mel_mean
+ * Two enqueues with one host wait between them for the frame counts: the text phase is graphed per (batch, token bucket),
+ * the mel phase per (batch, token and frame buckets, n_timesteps, s == 0, noise kind).  fp32 FFMA in every precision mode.
+ * VTTS_ERR_INVALID: not a StableTTS engine or a decoder-only blob, B < 1, t_max outside [1, VTTS_ST_MAX_TOKENS], a length
+ * outside [1, t_max], an id or speaker out of range, a pause outside [0, VTTS_ST_MAX_TOKEN_FRAMES], length_scale outside
+ * (0, 100], the sampling arguments as vtts_cfm_decode.  VTTS_ERR_CAPACITY, returned after the text phase with mel_lengths
+ * filled in: mel_ld below the longest utterance, or noise_ld below it rounded up to a multiple of 4.
+ * After a call, vtts_debug_read gives "st_tok_x" (the token rows x [tokens][st_cond]), "st_mu_dp" [tokens][st_dur_channels],
+ * "st_logw" [tokens] (durations before rounding) and "st_mu" (the decoder's mu rows [rows][st_cond], packed by padded frame
+ * count, the unconditional sequences after the conditional ones). */
+#define VTTS_ST_MAX_TOKENS 16384
+#define VTTS_ST_MAX_TOKEN_FRAMES 4096
+int vtts_stabletts_synthesise(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max, const float* bert,
+                              const float* pause, const int64_t* sid, int n_timesteps, float temperature, float length_scale,
+                              float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld,
+                              int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

@@ -203,6 +203,37 @@ def stabletts_cfm_config(overrides=None):
     return out
 
 
+STABLETTS_TEXT = {
+    # TextEncoder.__init__ hard-codes both stacks and the embedding widths (text_encoder.py:72-106); n_vocab comes from the
+    # experiment's yaml
+    "n_vocab": 178, "n_streams": 5, "emb_dim": 160, "punc_dim": 16, "bert_dim": 768, "bert_proj_dim": 32,
+    "enc_hidden_channels": 256, "enc_filter_channels": 1024, "enc_n_layers": 4, "enc_n_heads": 4, "enc_kernel_size": 3,
+    "dur_channels": 50,
+}
+
+
+def stabletts_config(overrides=None):
+    """Engine config of StableTTS text-to-mel: stabletts_cfm_config plus the text encoder's constants (STABLETTS_TEXT) with
+    `overrides` (n_vocab, n_spks, ... of a checkpoint)."""
+    out = stabletts_cfm_config(dict(STABLETTS_TEXT, **(overrides or {})))
+    H, heads = int(out["enc_hidden_channels"]), int(out["enc_n_heads"])
+    if int(out["emb_dim"]) + (int(out["n_streams"]) - 1) * int(out["punc_dim"]) + int(out["bert_proj_dim"]) != int(out["cond_channels"]) \
+            or H != int(out["cond_channels"]):
+        raise ValueError("emb_dim + (n_streams - 1) punc_dim + bert_proj_dim must equal cond_channels and enc_hidden_channels: the "
+                         "concatenated embedding is both stacks' input and the decoder's mu (text_encoder.py:131, matcha_tts.py:170)")
+    if H % heads or (H // heads) not in (32, 64, 96, 128):
+        raise ValueError("head width enc_hidden_channels / enc_n_heads must be 32, 64, 96 or 128: the attention kernels take no other")
+    if not 1 <= int(out["enc_n_layers"]) <= 8 or int(out["enc_kernel_size"]) % 2 != 1:
+        raise ValueError("enc_n_layers must be in 1..8 and enc_kernel_size odd")
+    if H % 16 or H > 512 or int(out["enc_filter_channels"]) % 16 or int(out["enc_filter_channels"]) > 1024:
+        raise ValueError("encoder widths must be multiples of 16, hidden up to 512, filter up to 1024: the FFMA conv and LayerNorm "
+                         "kernels' tiles")
+    if not 1 <= int(out["bert_dim"]) <= 1024 or not 1 <= int(out["dur_channels"]) <= 1024 or int(out["n_vocab"]) < 1 \
+            or not 1 <= int(out["n_streams"]) <= 8:
+        raise ValueError("bert_dim and dur_channels must be in 1..1024, n_streams in 1..8, n_vocab >= 1")
+    return out
+
+
 def convt_pad(cfg, i):
     """(padding, output_padding) of the decoder's upsampling ConvTranspose1d of stage i: (K-u)//2 and 0 in VITS2
     (training/vits2/models.py, every generator), (K-u+1-i)//2 and 1-i in QuickVC (vc/models.py:428-430).  The engine lays out

@@ -83,17 +83,21 @@ dit_ada_kernel(const float* __restrict__ emb, const float* __restrict__ fake, co
   dit_gemv(w2 + (long)l * 6 * H * H, b2 + (long)l * 6 * H, hid, 6 * H, H, out + ((long)s * NL + l) * 6 * H, false);
 }
 
-// Start of a call (flow_matching.py:52, 186-187): x = noise * temperature into columns [0, NC) of the in_proj operand rows
-// xc [rows][ldx] of both branches, noise from the caller ([rows of the B utterances][NC]) or Philox(seed) keyed by
-// (utterance, frame, channel); and fake_content repeated over the frames of the unconditional sequences' mu rows.
-// prm[0] temperature, prm[4..5] seed.  grid (frames, sequences).
+// Start of a call (flow_matching.py:52, 186-187) over every sequence's extent exts[s] >= lens[s] (the columns the reference
+// pads the frame axis to, matcha_tts.py:162-165; == lens[s] for a decoder called on its own): x = noise * temperature into
+// columns [0, NC) of the in_proj operand rows xc [rows][ldx] of both branches, noise from the caller ([rows of the B
+// utterances][NC]) or Philox(seed) keyed by (utterance, frame, channel); and fake_content repeated over the frames of the
+// unconditional sequences' mu rows.  Rows [lens[s], exts[s]): the conditional mu rows are zeroed, and so is the x half of
+// the last long-skip operand skx [rows][2 HC], whose skip half in_proj fills there.  prm[0] temperature, prm[4..5] seed.
+// grid (frames, sequences).
 __global__ void __launch_bounds__(128)
 dit_init_kernel(const float* __restrict__ noise, const float* __restrict__ prm, const float* __restrict__ fake_content, float* __restrict__ xc,
-                int ldx, int NC, float* __restrict__ mu, int MC, const int* __restrict__ lens, const int* __restrict__ offs, int B) {
+                int ldx, int NC, float* __restrict__ mu, int MC, float* __restrict__ skx, int HC, const int* __restrict__ lens,
+                const int* __restrict__ exts, const int* __restrict__ offs, int B) {
   PDL_LAUNCH();
   PDL_WAIT();
   const int s = blockIdx.y, t = blockIdx.x;
-  if (t >= lens[s]) return;
+  if (t >= exts[s]) return;
   const int b = s < B ? s : s - B;
   const long row = (long)offs[s] + t, nrow = (long)offs[b] + t;
   const float temp = prm[0];
@@ -104,6 +108,11 @@ dit_init_kernel(const float* __restrict__ noise, const float* __restrict__ prm, 
   }
   if (s >= B)
     for (int c = threadIdx.x; c < MC; c += blockDim.x) mu[row * MC + c] = fake_content[c];
+  if (t >= lens[s]) {
+    if (s < B)
+      for (int c = threadIdx.x; c < MC; c += blockDim.x) mu[row * MC + c] = 0.f;
+    for (int c = threadIdx.x; c < HC; c += blockDim.x) skx[row * 2 * HC + c] = 0.f;
+  }
 }
 
 // cos / sin of the rotary embedding (diffusion_transformer.py:151-166) for positions [0, n): theta_i = 1 / 10000^(2i/d) in

@@ -30,6 +30,7 @@
 #include "spk.cuh"
 #include "contentvec.cuh"
 #include "dit.cuh"
+#include "stabletts.cuh"
 #include "resample.cuh"
 #include "owned.cuh"
 
@@ -361,7 +362,7 @@ struct vtts_engine {
   // phase tag, the first element of every key
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
-    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF
+    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -673,10 +674,11 @@ struct vtts_engine {
   const float *st_aw1 = nullptr, *st_ab1 = nullptr, *st_aw2 = nullptr, *st_ab2 = nullptr;
   const float *st_emb = nullptr, *st_fake_spk = nullptr, *st_fake_content = nullptr, *st_mel_mean = nullptr, *st_mel_std = nullptr;
   // shape of the current call: NS sequences (B, or 2B with guidance: the unconditional branches follow the conditional
-  // ones), Ttot rows over all of them, the staged inputs' kinds
-  struct StPlan { int NS = 0, steps = 0, Ttot = 0; bool guided = false, noise = false, rows = false; } stp;
+  // ones), Ttot rows over all of them, the staged inputs' kinds.  text: the call is phase B of vtts_stabletts_synthesise (mu
+  // is expanded on the device from the token rows, pause frames are filled; prior: the expanded mel encoder output too)
+  struct StPlan { int NS = 0, steps = 0, Ttot = 0; bool guided = false, noise = false, rows = false, text = false, prior = false; } stp;
   static constexpr int ST_PRM = 16 + 2 * VTTS_CFM_MAX_STEPS;     // prm[16], t of every step, dt of every step
-  Buf<int> d_sti;                                  // [len NS][off NS][sid NS]
+  Buf<int> d_sti;                                  // [len NS][off NS][sid NS][extent NS]
   Buf<float> d_stf, d_stmu, d_stnoise, d_stfilm, d_stada, d_strope, d_stxc, d_stp0, d_stp1, d_stcat[4], d_stx, d_stx2, d_sth, d_stn,
       d_stqkv, d_stao, d_sty, d_stff, d_stv, d_stmel, d_stzero, d_stdbg_n, d_stdbg_qkv;
   PinnedBuf<char> h_pin_st;
@@ -684,6 +686,28 @@ struct vtts_engine {
   StPin st_layout();
   void bind_stabletts();
   void st_enqueue();
+  // One DiTConVBlock over a ragged batch (diffusion_transformer.py:98-116), shared by the decoder's blocks and the text
+  // encoder's: the rows, the conditioning and the work buffers of the caller
+  struct StBlk {
+    int H, F, heads, rd, maxLen, NS, ald;          // widths, rotary features, grid bound, sequences, pitch of a sequence's adaLN rows
+    const int *lens, *offs;
+    const float2* rope;
+    const float* ada;                              // [sequences][ald]
+    float *Hb, *N, *QKV, *AO, *Y, *FF;
+  };
+  void st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap);
+
+  // ---- StableTTS text encoder and durations (TextEncoder.forward, MatchaTTS.synthesise; stabletts.cuh): blobs of
+  // weights.pack_stabletts.  Stack 0 is the mel encoder (conditioned on spk_emb), stack 1 dp_encoder (on dur_spk_emb).
+  bool st_text = false;
+  struct StEncW { std::vector<EncLayerW> blk; ConvW proj; const float *aw1, *ab1, *aw2, *ab2, *spk; } st_enc[2];
+  const float *st_tok_emb = nullptr, *st_punc_emb = nullptr, *st_bert_w = nullptr, *st_bert_b = nullptr;
+  Buf<int> d_stti, d_sttd;                         // [tok len B][tok off B][sid B][ids streams x Ttok]; [dur Ttok][first Ttok][frames B]
+  Buf<float> d_sttf, d_stbert, d_sttx, d_stte[2], d_sttada, d_sttrope, d_stmumel, d_stmudp, d_stlogw, d_stpau;
+  PinnedBuf<char> h_pin_stt, h_pin_sttd;
+  struct SttPin { int* ints; float *prm, *pause, *bert; };
+  SttPin stt_layout();
+  void stt_enqueue(bool prior);
 
   // ---- resampling of recordings (vtts_resample; resample.cuh): the taps of each rate pair, uploaded on first use
   struct RsTaps { Buf<float> taps; int up = 0, down = 0, K = 0; };
@@ -2957,15 +2981,54 @@ void vtts_engine::bind_stabletts() {
     st_blk.push_back(L);
     if (l >= NL / 2) st_lsc.push_back(conv("st.lsc" + std::to_string(l - NL / 2), 2 * H, H, k));
   }
+  // the text encoder, when the blob carries it (weights.pack_stabletts); a decoder-only blob serves vtts_cfm_decode alone
+  st_text = c.st_enc_layers > 0;
+  if (!st_text) return;
+  const int He = c.st_enc_hidden, Fe = c.st_enc_filter, NE = c.st_enc_layers, ke = c.st_enc_kernel;
+  REQUIRE(tensors.count("st.enc.emb"), VTTS_ERR_WEIGHTS, "the config describes a StableTTS text encoder the weight blob does not carry");
+  REQUIRE(c.st_streams >= 1 && c.st_streams <= 8 && c.st_emb_dim >= 1 && c.st_punc_dim >= 1 && c.st_bert_proj >= 1 && c.st_n_vocab >= 1 &&
+              c.st_emb_dim + (c.st_streams - 1) * c.st_punc_dim + c.st_bert_proj == MC && He == MC,
+          VTTS_ERR_INVALID, "unsupported StableTTS text encoder: the embeddings and bert_proj must concatenate to cond_channels, the stacks' width");
+  REQUIRE(c.st_bert_dim >= 1 && c.st_bert_dim <= STT_MAXBERT && c.st_dur_channels >= 1 && c.st_dur_channels <= 1024, VTTS_ERR_INVALID,
+          "unsupported StableTTS text encoder: BERT rows up to 1024 wide, up to 1024 duration channels");
+  REQUIRE(NE >= 1 && NE <= 8 && c.st_enc_heads >= 1 && He % c.st_enc_heads == 0 && (He / c.st_enc_heads) % 32 == 0 && He / c.st_enc_heads <= 128 &&
+              He % CV_CK == 0 && He <= 32 * DIT_LN_MAXV && Fe % CV_CK == 0 && Fe <= DIT_MAXC && ke % 2 == 1 && ke >= 1 && ke <= 15,
+          VTTS_ERR_INVALID, "unsupported StableTTS text encoder (head widths 32..128, hidden up to 512, filter up to 1024, odd kernel)");
+  st_tok_emb = vec("st.enc.emb", (size_t)c.st_n_vocab * c.st_emb_dim);
+  st_punc_emb = vec("st.enc.punc", (size_t)c.st_n_vocab * c.st_punc_dim);
+  st_bert_w = vec("st.enc.bert.w", (size_t)c.st_bert_proj * c.st_bert_dim);
+  st_bert_b = vec("st.enc.bert.b", c.st_bert_proj);
+  for (int e = 0; e < 2; ++e) {
+    const std::string p = e == 0 ? "st.enc.mel" : "st.enc.dp";
+    StEncW& W = st_enc[e];
+    W.blk.clear();
+    for (int l = 0; l < NE; ++l) {
+      const std::string q = p + ".l" + std::to_string(l);
+      EncLayerW L;
+      L.heads = c.st_enc_heads;
+      L.qkv = conv(q + ".qkv", He, 3 * He, 1);
+      L.o = conv(q + ".o", He, He, 1);
+      L.ffn1 = conv(q + ".ffn1", He, Fe, ke);
+      L.ffn2 = conv(q + ".ffn2", Fe, He, ke);
+      L.relk = L.relv = zero;
+      W.blk.push_back(L);
+    }
+    W.proj = conv(p + ".proj", He, e == 0 ? NC : c.st_dur_channels, 1);
+    W.aw1 = vec(p + ".ada.w1", (size_t)NE * He * G); W.ab1 = vec(p + ".ada.b1", (size_t)NE * He);
+    W.aw2 = vec(p + ".ada.w2", (size_t)NE * 6 * He * He); W.ab2 = vec(p + ".ada.b2", (size_t)NE * 6 * He);
+    W.spk = e == 0 ? st_emb : vec("st.dur_spk_emb", (size_t)c.st_n_spks * G);
+  }
 }
 
-// Pinned staging of a vtts_cfm_decode call: ints [len NS][off NS][sid NS], then floats prm[16] | t[64] | dt[64] | speaker rows
-// [B][G] (when given) | mu rows [Tfrm][MC] packed as the engine's rows | noise rows [Tfrm][NC] (when given).  Every offset
-// follows from the graph key (batch, frame buckets, guided, input kinds).
+// Pinned staging of a flow-matching call: ints [len NS][off NS][sid NS][extent NS], then floats prm[16] | t[64] | dt[64] |
+// speaker rows [B][G] (when given) | mu rows [Tfrm][MC] packed as the engine's rows (vtts_cfm_decode; text-to-mel expands them
+// on the device) | noise rows [Tfrm][NC] (when given).  Every offset follows from the graph key (batch, frame buckets,
+// guided, input kinds).
 vtts_engine::StPin vtts_engine::st_layout() {
   const vtts_config& c = cfg;
-  const size_t head = ((size_t)3 * stp.NS * sizeof(int) + 63) / 64 * 64;
-  const size_t nspk = stp.rows ? (size_t)B * c.st_spk_dim : 0, nmu = (size_t)Tfrm * c.st_cond, nn = stp.noise ? (size_t)Tfrm * c.st_noise : 0;
+  const size_t head = ((size_t)4 * stp.NS * sizeof(int) + 63) / 64 * 64;
+  const size_t nspk = stp.rows ? (size_t)B * c.st_spk_dim : 0, nmu = stp.text ? 0 : (size_t)Tfrm * c.st_cond,
+               nn = stp.noise ? (size_t)Tfrm * c.st_noise : 0;
   char* pin = ensure(h_pin_st, head + (ST_PRM + nspk + nmu + nn) * sizeof(float) + 64);
   StPin pp;
   pp.ints = reinterpret_cast<int*>(pin);
@@ -2976,9 +3039,50 @@ vtts_engine::StPin vtts_engine::st_layout() {
   return pp;
 }
 
+// modulated LayerNorm -> qkv 1x1 -> rotary -> attention (zero relative tables) -> out 1x1 -> gated residual + modulated
+// LayerNorm -> conv -> SiLU -> conv -> gated residual; x rows at xin (pitch ldi) -> xout (pitch ldo).  film: the FiLM rows
+// DitWrapper applies first (decoder.py:15-18), or null for the text encoder's plain blocks.
+void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap) {
+  const int H = k.H, F = k.F, dk = H / k.heads;
+  const size_t T = (size_t)stp.Ttot;
+  const dim3 gs(k.maxLen, k.NS), gn((k.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, k.NS);
+  const float* ada = k.ada + (size_t)l * 6 * H;
+  auto norm = [&](const float* a, int lda, const float* fl, const float* y, int gate, int shift, int scale) {
+    klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f, k.Hb, k.N,
+            k.lens, k.offs, H);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy) {
+    launch_conv({mk(W, x, ldx, 0, y, ldy, 0, 1, (W.k - 1) / 2)}, 1, k.lens, k.offs, k.maxLen, k.NS);
+  };
+  norm(xin, ldi, film, nullptr, 2, 0, 1);
+  if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_n, T * H), k.N, T * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  cv(L.qkv, k.N, H, k.QKV, 3 * H);
+  klaunch(dit_rope_kernel, gs, dim3(128), (size_t)0, k.QKV, k.rope, k.heads, dk, k.rd, k.lens, k.offs);
+  CK(cudaGetLastError());
+  ++launches;
+  if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_qkv, T * 3 * H), k.QKV, T * 3 * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  launch_attn(k.QKV, k.AO, L, H, k.lens, k.offs, k.maxLen, nullptr);
+  cv(L.o, k.AO, H, k.Y, H);
+  norm(k.Hb, H, nullptr, k.Y, 2, 3, 4);
+  cv(L.ffn1, k.N, H, k.FF, F);
+  klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, k.FF, F, k.lens, k.offs);
+  CK(cudaGetLastError());
+  ++launches;
+  cv(L.ffn2, k.FF, F, k.Y, H);
+  klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, k.lens, k.offs, H);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
 // The whole call: uploads, the hoisted conditioning (FiLM rows of every step, adaLN rows of every sequence, cond_proj of both
 // branches, the rotary table), then n Euler steps of the estimator over the ragged batch of both branches.  The step loop is
 // unrolled into the enqueue (and so into the call's graph): step k's FiLM rows and dt are addresses, not values.
+//
+// Every sequence has a length and an extent >= it (rows are packed by extent).  The reference's synthesise pads the frame axis
+// to a multiple of 4 and masks only what the blocks write, so the noise, cond_proj and in_proj live on the extent and reach
+// the last valid frames through the convs' taps; everything else lives on the length.  vtts_cfm_decode passes extent == length.
 void vtts_engine::st_enqueue() {
   const vtts_config& c = cfg;
   const int NC = c.st_noise, MC = c.st_cond, H = c.st_hidden, F = c.st_filter, NL = c.st_layers, G = c.st_spk_dim;
@@ -2991,18 +3095,18 @@ void vtts_engine::st_enqueue() {
   attn_rows = 4;
   StPin pp = st_layout();
   const size_t T = (size_t)stp.Ttot;
-  int* di = ensure(d_sti, 3 * NS);
+  int* di = ensure(d_sti, 4 * NS);
   float* df = ensure(d_stf, ST_PRM + (size_t)Bu * G);
   float* mu = ensure(d_stmu, T * MC);
-  CK(cudaMemcpyAsync(di, pp.ints, 3 * NS * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(di, pp.ints, 4 * NS * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(df, pp.prm, (ST_PRM + (stp.rows ? (size_t)Bu * G : 0)) * sizeof(float), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(mu, pp.mu, (size_t)Tfrm * MC * sizeof(float), cudaMemcpyHostToDevice, stream));
+  if (!stp.text) CK(cudaMemcpyAsync(mu, pp.mu, (size_t)Tfrm * MC * sizeof(float), cudaMemcpyHostToDevice, stream));
   float* noise = nullptr;
   if (stp.noise) {
     noise = ensure(d_stnoise, (size_t)Tfrm * NC);
     CK(cudaMemcpyAsync(noise, pp.noise, (size_t)Tfrm * NC * sizeof(float), cudaMemcpyHostToDevice, stream));
   }
-  const int *lens = di, *offs = di + NS, *sid = di + 2 * NS;
+  const int *lens = di, *offs = di + NS, *sid = di + 2 * NS, *exts = di + 3 * NS;
   const float *prm = df, *ts = df + 16, *dts = df + 16 + VTTS_CFM_MAX_STEPS;
   B = NS;                                           // launch_attn and the launch heuristics read the member
   v_frm_len.assign(NS, maxFrm);
@@ -3017,12 +3121,20 @@ void vtts_engine::st_enqueue() {
   float *xc = ensure(d_stxc, T * XW), *p0 = ensure(d_stp0, T * F), *p1 = ensure(d_stp1, T * F);
   float* cat[4];
   for (int j = 0; j < nlsc; ++j) cat[j] = ensure(d_stcat[j], T * 2 * H);
-  float *X = ensure(d_stx, T * H), *X2 = ensure(d_stx2, T * H), *Hb = ensure(d_sth, T * H), *N = ensure(d_stn, T * H);
-  float *QKV = ensure(d_stqkv, T * 3 * H), *AO = ensure(d_stao, T * H), *Y = ensure(d_sty, T * H), *FF = ensure(d_stff, T * F);
-  float *V = ensure(d_stv, T * NC), *mel = ensure(d_stmel, (size_t)Tfrm * NC);
-  const dim3 gs(maxFrm, NS), gn((maxFrm + DIT_LN_WARPS - 1) / DIT_LN_WARPS, NS);
+  float *X = ensure(d_stx, T * H), *X2 = ensure(d_stx2, T * H);
+  StBlk kb{H, F, c.st_heads, rd, maxFrm, NS, NL * 6 * H, lens, offs, rope, ada,
+           ensure(d_sth, T * H), ensure(d_stn, T * H), ensure(d_stqkv, T * 3 * H), ensure(d_stao, T * H), ensure(d_sty, T * H), ensure(d_stff, T * F)};
+  float *V = ensure(d_stv, T * NC), *mel = ensure(d_stmel, (size_t)Tfrm * NC * (stp.prior ? 2 : 1));
+  const dim3 gs(maxFrm, NS);
   // ---- once per call
-  klaunch(dit_init_kernel, gs, dim3(128), (size_t)0, (const float*)noise, prm, st_fake_content, xc, XW, NC, mu, MC, lens, offs, Bu);
+  if (stp.text) {     // mu rows, pause flags and the prior from the token rows the text phase left on the device
+    const int *tl = d_stti.p, *to = tl + Bu, *dur = d_sttd.p, *first = dur + Ttok;
+    klaunch(stt_expand_kernel, dim3(maxTok, Bu), dim3(128), (size_t)0, (const float*)d_sttx.p, MC, (const float*)(d_sttf.p + 16), (const float*)d_stmumel.p, NC,
+            dur, first, mu, ensure(d_stpau, (size_t)Tfrm), stp.prior ? mel + (size_t)Tfrm * NC : (float*)nullptr, prm, st_mel_mean, st_mel_std, tl, to, offs);
+    CK(cudaGetLastError());
+    ++launches;
+  }
+  klaunch(dit_init_kernel, gs, dim3(128), (size_t)0, (const float*)noise, prm, st_fake_content, xc, XW, NC, mu, MC, cat[nlsc - 1], H, lens, exts, offs, Bu);
   klaunch(dit_time_kernel, dim3(stp.steps), dim3(256), (size_t)0, ts, st_tw1, st_tb1, st_tw2, st_tb2, st_fw, st_fb, H, F, NL, film);
   klaunch(dit_ada_kernel, dim3(NL, NS), dim3(256), (size_t)0, st_emb, st_fake_spk, stp.rows ? (const float*)(df + ST_PRM) : (const float*)nullptr,
           sid, st_aw1, st_ab1, st_aw2, st_ab2, G, H, NL, c.st_n_spks, ada);
@@ -3030,68 +3142,122 @@ void vtts_engine::st_enqueue() {
   CK(cudaGetLastError());
   launches += 4;
   auto silu = [&](float* y, int width) {
-    klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, y, width, lens, offs);
+    klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, y, width, exts, offs);
     CK(cudaGetLastError());
     ++launches;
   };
-  auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff) {
-    launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, lens, offs, maxFrm, NS);
+  auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff, const int* ln) {
+    launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, ln, offs, maxFrm, NS);
   };
-  // cond_proj (decoder.py:121; not masked: zero padded at each sequence's own ends) into the cond columns of the in_proj operand
-  cv(st_cp[0], mu, MC, p0, F, 0);
+  // cond_proj (decoder.py:121; not masked: zero padded at the ends of each sequence's extent) into the cond columns of the
+  // in_proj operand
+  cv(st_cp[0], mu, MC, p0, F, 0, exts);
   silu(p0, F);
-  cv(st_cp[1], p0, F, p1, F, 0);
+  cv(st_cp[1], p0, F, p1, F, 0, exts);
   silu(p1, F);
-  cv(st_cp[2], p1, F, xc, XW, NC);
-  const int ald = NL * 6 * H;
-  auto norm = [&](const float* a, int lda, const float* fl, const float* y, int l, int gate, int shift, int scale) {
-    klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, (const float*)(ada + (size_t)l * 6 * H), ald, gate * H, shift * H,
-            scale * H, 1e-5f, Hb, N, lens, offs, H);
-    CK(cudaGetLastError());
-    ++launches;
-  };
-  // DitWrapper (decoder.py:15-18) of block l at step s: x rows at xin (pitch ldi) -> xout (pitch ldo)
+  cv(st_cp[2], p1, F, xc, XW, NC, exts);
+  // DitWrapper (decoder.py:15-18) of block l at step s
   auto block = [&](int l, int s, const float* xin, int ldi, float* xout, int ldo) {
-    const EncLayerW& L = st_blk[l];
-    norm(xin, ldi, film + ((size_t)s * NL + l) * 2 * H, nullptr, l, 2, 0, 1);
-    const bool tap = (debug_flags & 1) && l == 0 && s == 0;
-    if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_n, T * H), N, T * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-    cv(L.qkv, N, H, QKV, 3 * H, 0);
-    klaunch(dit_rope_kernel, gs, dim3(128), (size_t)0, QKV, (const float2*)rope, c.st_heads, dk, rd, lens, offs);
-    CK(cudaGetLastError());
-    ++launches;
-    if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_qkv, T * 3 * H), QKV, T * 3 * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-    launch_attn(QKV, AO, L, H, lens, offs, maxFrm, nullptr);
-    cv(L.o, AO, H, Y, H, 0);
-    norm(Hb, H, nullptr, Y, l, 2, 3, 4);
-    cv(L.ffn1, N, H, FF, F, 0);
-    silu(FF, F);
-    cv(L.ffn2, FF, F, Y, H, 0);
-    klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)Hb, (const float*)Y, (const float*)(ada + (size_t)l * 6 * H), ald, 5 * H, xout, ldo,
-            lens, offs, H);
-    CK(cudaGetLastError());
-    ++launches;
+    st_block(kb, st_blk[l], l, film + ((size_t)s * NL + l) * 2 * H, xin, ldi, xout, ldo, (debug_flags & 1) && l == 0 && s == 0);
   };
   for (int s = 0; s < stp.steps; ++s) {
-    // in_proj over (x | cond) (decoder.py:123-124) -> the skip half of the last long-skip operand
-    cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H);
+    // in_proj over (x | cond) (decoder.py:123-124; not masked: over the extent) -> the skip half of the last long-skip operand
+    cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H, exts);
     // blocks 0 .. NL/2-1 leave their input as a skip (decoder.py:130-131): block i reads the skip half of cat[nlsc-1-i] and
     // writes the skip half of the next one; the last of them writes the x half of cat[0]
     for (int i = 0; i < nlsc; ++i)
       block(i, s, cat[nlsc - 1 - i] + H, 2 * H, i + 1 < nlsc ? cat[nlsc - 2 - i] + H : cat[0], 2 * H);
-    // blocks NL/2 ..: the long-skip conv over (x | skip) (decoder.py:133-134), then the block
+    // blocks NL/2 ..: the long-skip conv over (x | skip) (decoder.py:133-134), then the block.  The last one's skip is
+    // in_proj's output, whose rows past the length its taps read: its input rows are the extent's (the x half is zero there)
     for (int j = 0; j < nlsc; ++j) {
-      cv(st_lsc[j], cat[j], 2 * H, X, H, 0);
       const bool last = j + 1 == nlsc;
+      cv(st_lsc[j], cat[j], 2 * H, X, H, 0, last ? exts : lens);
       block(nlsc + j, s, X, H, last ? X2 : cat[j + 1], last ? H : 2 * H);
     }
-    cv(st_final, X2, H, V, NC, 0);
+    cv(st_final, X2, H, V, NC, 0, lens);
     const bool end = s + 1 == stp.steps;
     klaunch(dit_euler_kernel, dim3(maxFrm, Bu), dim3(128), (size_t)0, (const float*)V, xc, XW, NC, dts + s, prm, stp.guided ? 1 : 0,
             end ? mel : (float*)nullptr, st_mel_mean, st_mel_std, lens, offs, Bu);
     CK(cudaGetLastError());
     ++launches;
   }
+  if (stp.text) {
+    klaunch(stt_pause_fill_kernel, dim3(maxFrm, Bu), dim3(128), (size_t)0, mel, NC, (const float*)d_stpau.p, lens, offs);
+    CK(cudaGetLastError());
+    ++launches;
+  }
+}
+
+// Pinned staging of the text phase: ints [tok len B][tok off B][sid B][ids streams x Ttok], then floats prm[16] | pause [Ttok]
+// | bert rows [Ttok][bert_dim], tokens packed as the engine's rows.
+vtts_engine::SttPin vtts_engine::stt_layout() {
+  const vtts_config& c = cfg;
+  const size_t ni = (size_t)3 * B + (size_t)c.st_streams * Ttok, head = (ni * sizeof(int) + 63) / 64 * 64;
+  char* pin = ensure(h_pin_stt, head + (16 + (size_t)Ttok * (1 + c.st_bert_dim)) * sizeof(float) + 64);
+  SttPin pp;
+  pp.ints = reinterpret_cast<int*>(pin);
+  pp.prm = reinterpret_cast<float*>(pin + head);
+  pp.pause = pp.prm + 16;
+  pp.bert = pp.pause + Ttok;
+  return pp;
+}
+
+// Text phase of vtts_stabletts_synthesise: uploads, the token rows x, dp_encoder and its proj, the durations and their scan;
+// with `prior` the mel encoder and its proj as well.  Leaves x, the durations, each token's first frame, the pauses and
+// mu_mel on the device for the mel phase, and copies [dur][first][frames of every utterance] to pinned memory.
+void vtts_engine::stt_enqueue(bool prior) {
+  const vtts_config& c = cfg;
+  const int MC = c.st_cond, H = c.st_enc_hidden, F = c.st_enc_filter, NE = c.st_enc_layers, G = c.st_spk_dim, S = c.st_streams;
+  const int dk = H / c.st_enc_heads, rd = dk / 2, DC = c.st_dur_channels, NC = c.st_noise;
+  SavedLaunch saved(this);
+  struct Restore { vtts_engine* e; int rows; ~Restore() { e->attn_rows = rows; } } restore{this, attn_rows};
+  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;   // the decoder's fixed launch shape: durations do not depend on the batch
+  attn_rows = 4;
+  v_frm_len.assign(B, maxTok);
+  h_frm_len = h_tok_len;
+  SttPin pp = stt_layout();
+  const size_t T = (size_t)Ttok, ni = (size_t)3 * B + (size_t)S * T;
+  int* di = ensure(d_stti, ni);
+  float* df = ensure(d_sttf, 16 + T);
+  float* bert = ensure(d_stbert, T * c.st_bert_dim);
+  CK(cudaMemcpyAsync(di, pp.ints, ni * sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(df, pp.prm, (16 + T) * sizeof(float), cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(bert, pp.bert, T * c.st_bert_dim * sizeof(float), cudaMemcpyHostToDevice, stream));
+  const int *lens = di, *offs = di + B, *sid = di + 2 * B, *ids = di + 3 * B;
+  float* x = ensure(d_sttx, T * MC);
+  float2* rope = reinterpret_cast<float2*>(ensure(d_sttrope, (size_t)maxTok * rd));
+  float* ada = ensure(d_sttada, (size_t)B * NE * 6 * H);
+  float *e0 = ensure(d_stte[0], T * H), *e1 = ensure(d_stte[1], T * H);
+  float *mu_mel = ensure(d_stmumel, T * NC), *mu_dp = ensure(d_stmudp, T * DC), *logw = ensure(d_stlogw, T);
+  int* dd = ensure(d_sttd, 2 * T + B);
+  StBlk kb{H, F, c.st_enc_heads, rd, maxTok, B, NE * 6 * H, lens, offs, rope, ada,
+           ensure(d_sth, T * H), ensure(d_stn, T * H), ensure(d_stqkv, T * 3 * H), ensure(d_stao, T * H), ensure(d_sty, T * H), ensure(d_stff, T * F)};
+  klaunch(stt_front_kernel, dim3(maxTok, B), dim3(256), (size_t)0, ids, Ttok, (const float*)bert, st_tok_emb, (float)std::sqrt((double)c.st_emb_dim),
+          st_punc_emb, (float)std::sqrt((double)c.st_punc_dim), st_bert_w, st_bert_b, S, c.st_emb_dim, c.st_punc_dim, c.st_bert_dim, c.st_bert_proj,
+          x, lens, offs);
+  klaunch(dit_rope_table_kernel, dim3((maxTok * (rd / 2) + 127) / 128), dim3(128), (size_t)0, rope, maxTok, rd);
+  CK(cudaGetLastError());
+  launches += 2;
+  for (int e = prior ? 0 : 1; e < 2; ++e) {
+    const StEncW& W = st_enc[e];
+    klaunch(dit_ada_kernel, dim3(NE, B), dim3(256), (size_t)0, W.spk, (const float*)nullptr, (const float*)nullptr, sid, W.aw1, W.ab1, W.aw2, W.ab2, G, H,
+            NE, c.st_n_spks, ada);
+    CK(cudaGetLastError());
+    ++launches;
+    const float* in = x;
+    for (int l = 0; l < NE; ++l) {
+      float* out = l % 2 ? e1 : e0;
+      st_block(kb, W.blk[l], l, nullptr, in, H, out, H, false);
+      in = out;
+    }
+    launch_conv({mk(W.proj, in, H, 0, e == 0 ? mu_mel : mu_dp, e == 0 ? NC : DC, 0, 1, 0)}, 1, lens, offs, maxTok, B);
+  }
+  klaunch(stt_dur_kernel, dim3(B), dim3(STT_SCAN), (size_t)0, (const float*)mu_dp, DC, DC, (const float*)(df + 16), (const float*)df,
+          (float)VTTS_ST_MAX_TOKEN_FRAMES, dd, dd + Ttok, dd + 2 * Ttok, logw, lens, offs);
+  CK(cudaGetLastError());
+  ++launches;
+  int* back = reinterpret_cast<int*>(ensure(h_pin_sttd, (2 * T + B) * sizeof(int)));
+  CK(cudaMemcpyAsync(back, dd, (2 * T + B) * sizeof(int), cudaMemcpyDeviceToHost, stream));
 }
 
 // Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
@@ -3703,15 +3869,68 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const float*
   }
 }
 
+// t_span = 1 - cos(linspace(0, 1, n + 1) pi / 2) and the Euler loop's t and dt into prm[16 ..], in the reference's fp32 steps
+// (flow_matching.py:54-55,87-98: t accumulates, dt is the distance from it to the next knot)
+static void st_schedule(float* prm, int n) {
+  std::vector<float> span(n + 1);
+  const float step = 1.f / (float)n;
+  for (int i = 0; i <= n; ++i) {
+    const float lin = i < (n + 1) / 2 ? step * (float)i : 1.f - step * (float)(n - i);
+    const float a = (lin * 0.5f) * (float)M_PI;
+    span[i] = 1.f - (float)std::cos((double)a);
+  }
+  float t = span[0], dt = span[1] - span[0];
+  for (int k = 0; k < n; ++k) {
+    prm[16 + k] = t;
+    prm[16 + VTTS_CFM_MAX_STEPS + k] = dt;
+    t = t + dt;
+    if (k + 1 < n) dt = span[k + 2] - t;
+  }
+}
+
+// The flow-matching plan of a call and its staged table: sequence q < B is utterance q's conditional branch, B + q its
+// unconditional one; rows are packed by extent.
+static vtts_engine::StPin st_plan(vtts_handle h, int B, const std::vector<int>& frames, const std::vector<int>& extents, const int64_t* sid, int n,
+                                  float temperature, float s, bool noise, bool rows, bool text, bool prior, int denormalise, uint64_t seed) {
+  h->pack_frames(extents);
+  vtts_engine::StPlan& P = h->stp;
+  P.guided = s > 0.f;
+  P.NS = P.guided ? 2 * B : B;
+  P.steps = n;
+  P.noise = noise;
+  P.rows = rows;
+  P.text = text;
+  P.prior = prior;
+  P.Ttot = P.guided ? 2 * h->Tfrm + SEQ_GAP : h->Tfrm;
+  REQUIRE((int64_t)P.Ttot * 3 * h->cfg.st_filter < (int64_t)INT32_MAX, VTTS_ERR_INVALID, "the batch holds too many frames for one call");
+  const int NS = P.NS;
+  const vtts_engine::StPin pp = h->st_layout();
+  for (int q = 0; q < NS; ++q) {
+    const int b = q < B ? q : q - B;
+    pp.ints[q] = frames[b];
+    pp.ints[NS + q] = h->h_frm_off[b] + (q < B ? 0 : h->Tfrm + SEQ_GAP);
+    pp.ints[2 * NS + q] = q < B ? (sid ? (int)sid[b] : 0) : -1;
+    pp.ints[3 * NS + q] = extents[b];
+  }
+  const float sc[3] = {temperature, s, denormalise ? 1.f : 0.f};
+  vtts_engine::put_scalars(pp.prm, vtts_engine::ST_PRM, sc, 3, seed);
+  st_schedule(pp.prm, n);
+  return pp;
+}
+
+static void st_check_sampling(int n, float temperature, float s) {
+  REQUIRE(n >= 1 && n <= VTTS_CFM_MAX_STEPS, VTTS_ERR_INVALID, "n_timesteps must be in [1, " + std::to_string(VTTS_CFM_MAX_STEPS) + "]");
+  REQUIRE(std::isfinite(temperature), VTTS_ERR_INVALID, "temperature must be finite");
+  REQUIRE(std::isfinite(s) && s >= 0.f, VTTS_ERR_INVALID, "guidance_scale must be finite and >= 0");
+}
+
 // StableTTS flow-matching decoder through host buffers (vtts_cfm_decode).
 static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int B, int64_t mu_ld, const int64_t* sid,
                             const float* spk_rows, int n, float temperature, float s, const float* noise, int64_t noise_ld, uint64_t seed,
                             float* mel_out, int64_t mel_ld, int denormalise) {
   const vtts_config& c = h->cfg;
   REQUIRE(B >= 1 && B <= 8192 && mu_ld >= 1 && mu_ld < (1LL << 24), VTTS_ERR_INVALID, "bad batch size / mu_ld");
-  REQUIRE(n >= 1 && n <= VTTS_CFM_MAX_STEPS, VTTS_ERR_INVALID, "n_timesteps must be in [1, " + std::to_string(VTTS_CFM_MAX_STEPS) + "]");
-  REQUIRE(std::isfinite(temperature), VTTS_ERR_INVALID, "temperature must be finite");
-  REQUIRE(std::isfinite(s) && s >= 0.f, VTTS_ERR_INVALID, "guidance_scale must be finite and >= 0");
+  st_check_sampling(n, temperature, s);
   REQUIRE(sid || spk_rows, VTTS_ERR_INVALID, "a speaker is required: sid or spk_rows");
   std::vector<int> frames(B);
   for (int b = 0; b < B; ++b) {
@@ -3725,42 +3944,10 @@ static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengt
   h->B = B;
   h->have_durations = false;
   h->have_latent = false;
-  h->pack_frames(frames);
-  vtts_engine::StPlan& P = h->stp;
-  P.guided = s > 0.f;
-  P.NS = P.guided ? 2 * B : B;
-  P.steps = n;
-  P.noise = noise != nullptr;
-  P.rows = spk_rows != nullptr;
-  P.Ttot = P.guided ? 2 * h->Tfrm + SEQ_GAP : h->Tfrm;
-  REQUIRE((int64_t)P.Ttot * 3 * c.st_filter < (int64_t)INT32_MAX, VTTS_ERR_INVALID, "the batch holds too many frames for one call");
-  const int NC = c.st_noise, MC = c.st_cond, G = c.st_spk_dim, NS = P.NS;
-  const vtts_engine::StPin pp = h->st_layout();
-  for (int q = 0; q < NS; ++q) {
-    const int b = q < B ? q : q - B;
-    pp.ints[q] = frames[b];
-    pp.ints[NS + q] = h->h_frm_off[b] + (q < B ? 0 : h->Tfrm + SEQ_GAP);
-    pp.ints[2 * NS + q] = q < B ? (sid ? (int)sid[b] : 0) : -1;
-  }
-  const float sc[3] = {temperature, s, denormalise ? 1.f : 0.f};
-  vtts_engine::put_scalars(pp.prm, vtts_engine::ST_PRM, sc, 3, seed);
-  {   // t_span = 1 - cos(linspace(0, 1, n + 1) pi / 2) and the Euler loop's t and dt, in the reference's fp32 steps
-      // (flow_matching.py:54-55,87-98: t accumulates, dt is the distance from it to the next knot)
-    std::vector<float> span(n + 1);
-    const float step = 1.f / (float)n;
-    for (int i = 0; i <= n; ++i) {
-      const float lin = i < (n + 1) / 2 ? step * (float)i : 1.f - step * (float)(n - i);
-      const float a = (lin * 0.5f) * (float)M_PI;
-      span[i] = 1.f - (float)std::cos((double)a);
-    }
-    float t = span[0], dt = span[1] - span[0];
-    for (int k = 0; k < n; ++k) {
-      pp.prm[16 + k] = t;
-      pp.prm[16 + VTTS_CFM_MAX_STEPS + k] = dt;
-      t = t + dt;
-      if (k + 1 < n) dt = span[k + 2] - t;
-    }
-  }
+  const int NC = c.st_noise, MC = c.st_cond, G = c.st_spk_dim;
+  const vtts_engine::StPin pp = st_plan(h, B, frames, frames, sid, n, temperature, s, noise != nullptr, spk_rows != nullptr,
+                                        false, false, denormalise, seed);
+  const vtts_engine::StPlan& P = h->stp;
   if (spk_rows) memcpy(pp.spk, spk_rows, (size_t)B * G * sizeof(float));
   for (int b = 0; b < B; ++b) {
     const size_t o = (size_t)h->h_frm_off[b];
@@ -3770,6 +3957,97 @@ static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengt
   h->run_graphed({vtts_engine::TAG_CFM, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, P.rows ? 1 : 0}, [&] { h->st_enqueue(); });
   read_clips(h, (const float*)h->d_stmel.p, (size_t)h->real_Tfrm * NC, (size_t)h->Tfrm * NC, h->h_frm_off.data(), frames, NC, mel_out,
              mel_ld * NC);
+}
+
+// StableTTS text-to-mel through host buffers (vtts_stabletts_synthesise): the text phase, one wait for the frame counts, the
+// mel phase.
+static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max, const float* bert,
+                                      const float* pause, const int64_t* sid, int n, float temperature, float length_scale, float s,
+                                      const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld, int64_t* mel_lengths,
+                                      int32_t* durations, float* prior_out, int denormalise) {
+  const vtts_config& c = h->cfg;
+  REQUIRE(h->st_text, VTTS_ERR_INVALID, "the weight blob holds the flow-matching decoder only (weights.pack_stabletts_cfm): text-to-mel needs the "
+                                         "text encoder of weights.pack_stabletts");
+  REQUIRE(B >= 1 && B <= 8192 && t_max >= 1 && t_max <= VTTS_ST_MAX_TOKENS, VTTS_ERR_INVALID, "bad batch size / t_max");
+  st_check_sampling(n, temperature, s);
+  REQUIRE(std::isfinite(length_scale) && length_scale > 0.f && length_scale <= 100.f, VTTS_ERR_INVALID, "length_scale must be in (0, 100]");
+  const int S = c.st_streams, BD = c.st_bert_dim, NC = c.st_noise;
+  h->B = B;
+  h->have_durations = false;
+  h->have_latent = false;
+  h->h_tok_len.resize(B);
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(id_lengths[b] >= 1 && id_lengths[b] <= t_max, VTTS_ERR_INVALID, "id_lengths must be in [1, t_max]");
+    REQUIRE(sid[b] >= 0 && sid[b] < c.st_n_spks, VTTS_ERR_INVALID, "speaker id out of range [0, n_spks)");
+    h->h_tok_len[b] = (int)id_lengths[b];
+    for (int q = 0; q < S; ++q)
+      for (int i = 0; i < h->h_tok_len[b]; ++i) {
+        const int64_t v = ids[((size_t)b * S + q) * t_max + i];
+        REQUIRE(v >= 0 && v < c.st_n_vocab, VTTS_ERR_INVALID, "token id out of range [0, n_vocab)");
+      }
+    if (pause)
+      for (int i = 0; i < h->h_tok_len[b]; ++i) {
+        const float v = pause[(size_t)b * t_max + i];
+        REQUIRE(v >= 0.f && v <= (float)VTTS_ST_MAX_TOKEN_FRAMES, VTTS_ERR_INVALID, "pause durations must be in [0, VTTS_ST_MAX_TOKEN_FRAMES]");
+      }
+  }
+  vtts_engine::pack_rows(h->h_tok_len, h->h_tok_off);
+  h->set_token_shape();
+  const int Ttok = h->Ttok;
+  {
+    const vtts_engine::SttPin pp = h->stt_layout();
+    memset(pp.ints + 3 * B, 0, (size_t)S * Ttok * sizeof(int));
+    std::fill(pp.pause, pp.pause + Ttok, 0.f);
+    vtts_engine::put_scalars(pp.prm, 16, &length_scale, 1, seed);
+    for (int b = 0; b < B; ++b) {
+      const int len = h->h_tok_len[b], o = h->h_tok_off[b];
+      pp.ints[b] = len;
+      pp.ints[B + b] = o;
+      pp.ints[2 * B + b] = (int)sid[b];
+      for (int q = 0; q < S; ++q)
+        for (int i = 0; i < len; ++i) pp.ints[3 * B + (size_t)q * Ttok + o + i] = (int)ids[((size_t)b * S + q) * t_max + i];
+      if (pause) memcpy(pp.pause + o, pause + (size_t)b * t_max, (size_t)len * sizeof(float));
+      memcpy(pp.bert + (size_t)o * BD, bert + (size_t)b * t_max * BD, (size_t)len * BD * sizeof(float));
+    }
+  }
+  const bool prior = prior_out != nullptr;
+  h->run_graphed({vtts_engine::TAG_ST_TEXT, B, h->maxTok, Ttok, prior ? 1 : 0}, [&] { h->stt_enqueue(prior); });
+  CK(cudaStreamSynchronize(h->stream));            // the one wait of the path: the frame counts size the mel phase
+  const int* back = reinterpret_cast<const int*>(h->h_pin_sttd.p);
+  std::vector<int> frames(B), extents(B);
+  int64_t total = 0;
+  for (int b = 0; b < B; ++b) {
+    frames[b] = back[2 * (size_t)Ttok + b];
+    extents[b] = (frames[b] + 3) / 4 * 4;
+    mel_lengths[b] = frames[b];
+    total += extents[b];
+    if (durations) {
+      std::fill(durations + (size_t)b * t_max, durations + (size_t)(b + 1) * t_max, 0);
+      memcpy(durations + (size_t)b * t_max, back + h->h_tok_off[b], (size_t)h->h_tok_len[b] * sizeof(int));
+    }
+  }
+  REQUIRE(total < (1LL << 24), VTTS_ERR_INVALID, "the batch expands to too many frames for one call");
+  const int real_max = *std::max_element(frames.begin(), frames.end()), ext_max = (real_max + 3) / 4 * 4;
+  REQUIRE(mel_ld >= real_max, VTTS_ERR_CAPACITY, "mel_ld is smaller than the longest utterance (mel_lengths holds the frame counts)");
+  REQUIRE(!noise || noise_ld >= ext_max, VTTS_ERR_CAPACITY, "noise has fewer frames than the longest utterance padded to a multiple of 4 "
+                                                            "(mel_lengths holds the frame counts)");
+  const vtts_engine::StPin pp = st_plan(h, B, frames, extents, sid, n, temperature, s, noise != nullptr, false, true, prior, denormalise, seed);
+  const vtts_engine::StPlan& P = h->stp;
+  if (noise)
+    for (int b = 0; b < B; ++b)
+      memcpy(pp.noise + (size_t)h->h_frm_off[b] * NC, noise + (size_t)b * noise_ld * NC, (size_t)extents[b] * NC * sizeof(float));
+  h->run_graphed({vtts_engine::TAG_ST_MEL, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, prior ? 1 : 0, h->maxTok, Ttok},
+                 [&] { h->st_enqueue(); });
+  const size_t plane = (size_t)h->Tfrm * NC, nread = prior ? plane + (size_t)h->real_Tfrm * NC : (size_t)h->real_Tfrm * NC;
+  float* pin = reinterpret_cast<float*>(h->ensure_pinned(2 * plane * sizeof(float) + 64));
+  CK(cudaMemcpyAsync(pin, h->d_stmel.p, nread * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaEventRecord(h->ev[7], h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; ++b) {
+    const size_t o = (size_t)h->h_frm_off[b] * NC, nb = (size_t)frames[b] * NC * sizeof(float);
+    memcpy(mel_out + (size_t)b * mel_ld * NC, pin + o, nb);
+    if (prior) memcpy(prior_out + (size_t)b * mel_ld * NC, pin + plane + o, nb);
+  }
 }
 
 // I0 by its power series (the Kaiser window's; np.i0 within a few ulps for the beta 5 of resample_poly)
@@ -4386,6 +4664,10 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "st_rope") { src = h->d_strope.p; n = (size_t)h->maxFrm * (c.st_hidden / c.st_heads / 2); }
     else if (nm == "st_norm1") { src = h->d_stdbg_n.p; n = (size_t)h->stp.Ttot * c.st_hidden; }
     else if (nm == "st_qkv") { src = h->d_stdbg_qkv.p; n = (size_t)h->stp.Ttot * 3 * c.st_hidden; }
+    else if (nm == "st_mu") { src = h->d_stmu.p; n = (size_t)h->stp.Ttot * c.st_cond; }
+    else if (nm == "st_tok_x") { src = h->d_sttx.p; n = T * c.st_cond; }
+    else if (nm == "st_mu_dp") { src = h->d_stmudp.p; n = T * c.st_dur_channels; }
+    else if (nm == "st_logw") { src = h->d_stlogw.p; n = T; }
     else if (nm == "cv_enc_in") { src = h->d_cvdbg.p; n = (size_t)h->cvp.tot0 / h->cv_P * c.cv_hidden; }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);
@@ -4440,6 +4722,16 @@ int vtts_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int 
   if (!mu || !lengths || !mel_out) return VTTS_ERR_INVALID;
   return guarded(h, [&] { impl_cfm_decode(h, mu, lengths, B, mu_ld, sid, spk_rows, n_timesteps, temperature, guidance_scale, noise, noise_ld,
                                           seed, mel_out, mel_ld, denormalise); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
+}
+
+int vtts_stabletts_synthesise(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max, const float* bert,
+                              const float* pause, const int64_t* sid, int n_timesteps, float temperature, float length_scale,
+                              float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld,
+                              int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise) {
+  if (!ids || !id_lengths || !bert || !sid || !mel_out || !mel_lengths) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_stabletts_synthesise(h, ids, id_lengths, B, t_max, bert, pause, sid, n_timesteps, temperature, length_scale,
+                                                    guidance_scale, noise, noise_ld, seed, mel_out, mel_ld, mel_lengths, durations, prior_out,
+                                                    denormalise); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
 }
 
 int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,

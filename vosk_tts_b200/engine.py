@@ -44,6 +44,9 @@ class VttsConfig(C.Structure):
         ("st_noise", C.c_int32), ("st_cond", C.c_int32), ("st_hidden", C.c_int32), ("st_filter", C.c_int32),
         ("st_layers", C.c_int32), ("st_heads", C.c_int32), ("st_kernel", C.c_int32), ("st_spk_dim", C.c_int32),
         ("st_n_spks", C.c_int32),
+        ("st_n_vocab", C.c_int32), ("st_streams", C.c_int32), ("st_emb_dim", C.c_int32), ("st_punc_dim", C.c_int32),
+        ("st_bert_dim", C.c_int32), ("st_bert_proj", C.c_int32), ("st_enc_hidden", C.c_int32), ("st_enc_filter", C.c_int32),
+        ("st_enc_layers", C.c_int32), ("st_enc_heads", C.c_int32), ("st_enc_kernel", C.c_int32), ("st_dur_channels", C.c_int32),
         ("cv_layers", C.c_int32), ("cv_hidden", C.c_int32), ("cv_heads", C.c_int32), ("cv_ffn", C.c_int32),
         ("cv_conv_dim", C.c_int32), ("cv_n_conv", C.c_int32), ("cv_conv_kernel", C.c_int32 * 8), ("cv_conv_stride", C.c_int32 * 8),
         ("cv_pos_k", C.c_int32), ("cv_pos_groups", C.c_int32), ("cv_ln_eps", C.c_float), ("cv_gn_eps", C.c_float),
@@ -59,7 +62,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
-           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode"]
+           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -243,6 +246,9 @@ def load_library(build_if_missing=True):
     lib.vtts_cfm_decode.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, i32, C.c_float, C.c_float, vp, C.c_int64, C.c_uint64, vp,
                                     C.c_int64, i32]
     lib.vtts_cfm_decode.restype = i32
+    lib.vtts_stabletts_synthesise.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, vp, i32, C.c_float, C.c_float, C.c_float, vp, C.c_int64,
+                                              C.c_uint64, vp, C.c_int64, vp, vp, vp, i32]
+    lib.vtts_stabletts_synthesise.restype = i32
     _LIB = lib
     return lib
 
@@ -281,6 +287,12 @@ def make_c_config(cfg, precision=0):
                          ("st_filter", "filter_channels"), ("st_layers", "n_layers"), ("st_heads", "n_heads"),
                          ("st_kernel", "kernel_size"), ("st_spk_dim", "spk_emb_dim"), ("st_n_spks", "n_spks")):
             setattr(c, dst, int(cfg[src]))
+        if "enc_n_layers" in cfg:                      # config.stabletts_config: the text encoder of weights.pack_stabletts
+            for dst, src in (("st_n_vocab", "n_vocab"), ("st_streams", "n_streams"), ("st_emb_dim", "emb_dim"), ("st_punc_dim", "punc_dim"),
+                             ("st_bert_dim", "bert_dim"), ("st_bert_proj", "bert_proj_dim"), ("st_enc_hidden", "enc_hidden_channels"),
+                             ("st_enc_filter", "enc_filter_channels"), ("st_enc_layers", "enc_n_layers"), ("st_enc_heads", "enc_n_heads"),
+                             ("st_enc_kernel", "enc_kernel_size"), ("st_dur_channels", "dur_channels")):
+                setattr(c, dst, int(cfg[src]))
         return c
     for k in ("n_vocab", "n_speakers", "gin_channels", "inter_channels", "hidden_channels", "filter_channels",
               "n_heads", "n_layers", "kernel_size", "window_size", "cond_layer_idx", "flow_kernel_size",
@@ -704,6 +716,57 @@ class Engine:
                                              float(temperature), float(guidance_scale), _ptr(noise), noise_ld, int(seed),
                                              _ptr(mel), T, int(bool(denormalise))))
         return mel, lengths
+
+    def stabletts_synthesise(self, ids, bert, sid, lengths=None, pause=None, n_timesteps=10, temperature=1.0, length_scale=1.0,
+                             guidance_scale=0.5, noise=None, seed=0, mel_frames=None, want_prior=False, denormalise=False):
+        """StableTTS text-to-mel (vtts_stabletts_synthesise).  ids int [B, n_streams, T] (or [n_streams, T]); bert float [B, T,
+        bert_dim] token-major; lengths int [B] (None: T for all); pause float [B, T] or None; sid int [B] (or one for all);
+        noise float [B, >= ceil4(frames), noise_channels] frame-major over the padded frame axis, or None for Philox(seed).
+        mel_frames: the frame capacity of the result; None asks the engine for the frame counts first (a call with no room,
+        which ends after the text phase) and then runs the call with exactly enough.  Returns a dict: mel [B, frames,
+        noise_channels] frame-major (zeros past each utterance), mel_lengths int64 [B], durations int32 [B, T], and prior (the
+        expanded mel encoder output) when want_prior."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        if ids.ndim == 2:
+            ids = ids[None]
+        B, S, T = ids.shape
+        NC, BD = int(self.cfg["noise_channels"]), int(self.cfg.get("bert_dim", 0))
+        if S != int(self.cfg.get("n_streams", S)):
+            raise ValueError("ids must be [B, %d, T]" % int(self.cfg["n_streams"]))
+        bert = np.ascontiguousarray(bert, dtype=np.float32)
+        if bert.ndim == 2:
+            bert = bert[None]
+        if bert.shape != (B, T, BD):
+            raise ValueError("bert must be token-major [B, T, %d]" % BD)
+        lengths = np.full(B, T, np.int64) if lengths is None else np.ascontiguousarray(np.broadcast_to(np.asarray(lengths, np.int64).reshape(-1), (B,)))
+        sid = np.ascontiguousarray(np.broadcast_to(np.asarray(sid, np.int64).reshape(-1), (B,)))
+        if pause is not None:
+            pause = np.ascontiguousarray(pause, dtype=np.float32).reshape(-1, T)
+            if pause.shape != (B, T):
+                raise ValueError("pause must be [B, T]")
+        noise_ld = 0
+        if noise is not None:
+            noise, _ = _batch(noise, None, 3, t_axis=1, ragged=True)
+            if noise.shape[0] != B or noise.shape[2] != NC:
+                raise ValueError("noise must be frame-major [B, >= ceil4(frames), %d]" % NC)
+            noise_ld = noise.shape[1]
+        mel_len = np.zeros(B, np.int64)
+        dur = np.zeros((B, T), np.int32)
+        if mel_frames is None:      # a token lasts at most max(sum of dur_channels sigmoids, its pause) * length_scale frames
+            per = np.full((B, T), float(self.cfg["dur_channels"]), np.float64) if pause is None else np.maximum(pause, float(self.cfg["dur_channels"]))
+            per = np.maximum(np.ceil(per * float(length_scale)) + 1, 1) * (np.arange(T)[None, :] < lengths[:, None])
+            mel_frames = int(per.sum(1).max())
+        mel = np.zeros((B, int(mel_frames), NC), np.float32)
+        prior = np.zeros_like(mel) if want_prior else None
+        self._check(self.lib.vtts_stabletts_synthesise(self.h, _ptr(ids), _ptr(lengths), B, T, _ptr(bert), _ptr(pause), _ptr(sid), int(n_timesteps),
+                                                       float(temperature), float(length_scale), float(guidance_scale), _ptr(noise), noise_ld,
+                                                       int(seed), _ptr(mel), int(mel_frames), _ptr(mel_len), _ptr(dur), _ptr(prior),
+                                                       int(bool(denormalise))))
+        top = int(mel_len.max())
+        out = {"mel": np.ascontiguousarray(mel[:, :top]), "mel_lengths": mel_len, "durations": dur}
+        if want_prior:
+            out["prior"] = np.ascontiguousarray(prior[:, :top])
+        return out
 
     def resample(self, wav, from_rate, to_rate, lengths=None, trim_top_db=None, return_bounds=False):
         """Clips at `from_rate` Hz resampled to `to_rate` Hz (vtts_resample: scipy.signal.resample_poly's filter, not soxr), and

@@ -1,7 +1,8 @@
-"""StableTTS on the GPU, as far as it is built: the conditional-flow-matching decoder that turns the text encoder's output,
-already expanded to frames, into a mel spectrogram (CFM.forward of training/stabletts/matcha/models/components/flow_matching.py,
-called at matcha_tts.py:183).  The text encoder, the duration predictor and the vocoder are not part of this module: a caller
-supplies mu_y (matcha_tts.py:170-171) and vocodes the mel itself."""
+"""StableTTS on the GPU, as far as it is built: text-to-mel (MatchaTTS.synthesise of training/stabletts/matcha/models/
+matcha_tts.py:93-211: multistream ids, BERT features and pause durations in, durations and mel out) and its
+conditional-flow-matching decoder alone (CFM.forward of components/flow_matching.py, called at matcha_tts.py:183).  The BERT
+model and the vocoder are not part of this module: a caller supplies the BERT features, as the exported graph's `bert` feed
+does, and vocodes the mel itself."""
 import numpy as np
 
 from . import config as _config
@@ -9,17 +10,69 @@ from . import weights as _weights
 
 
 class StableTTS:
-    """A MatchaTTS (StableTTS) checkpoint's flow-matching decoder on one GPU."""
+    """A MatchaTTS (StableTTS) checkpoint on one GPU: text-to-mel when it carries the text encoder, else the flow-matching
+    decoder alone."""
 
     def __init__(self, config, checkpoint, device=0, precision=1):
-        """config: overrides of config.STABLETTS_CFM (n_spks, spk_emb_dim, ...) or None; checkpoint: a path (Lightning's
-        `state_dict` entry is taken when present) or a state dict."""
+        """config: overrides of config.STABLETTS_CFM / STABLETTS_TEXT (n_vocab, n_spks, spk_emb_dim, ...) or None; checkpoint: a
+        path (Lightning's `state_dict` entry is taken when present) or a state dict.  A state dict without encoder.* serves
+        refine() only."""
         from .engine import Engine
-        self.cfg = _config.stabletts_cfm_config(config)
         sd = _weights.load_checkpoint(checkpoint) if isinstance(checkpoint, str) else checkpoint
         sd = sd.get("state_dict", sd)
-        blob, man = _weights.pack_stabletts_cfm(sd, self.cfg)
+        self.has_text = "encoder.emb.weight" in sd
+        if self.has_text:
+            self.cfg = _config.stabletts_config(dict({"n_vocab": int(sd["encoder.emb.weight"].shape[0])}, **(config or {})))
+            blob, man = _weights.pack_stabletts(sd, self.cfg)
+        else:
+            self.cfg = _config.stabletts_cfm_config(config)
+            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg)
+        self.mel_mean, self.mel_std = np.float32(sd["mel_mean"]), np.float32(sd["mel_std"])
         self.engine = Engine(self.cfg, blob, man, device=device, precision=precision)
+
+    @staticmethod
+    def from_scales(scales):
+        """The exported graph's `scales` feed in the order its forward reads it (matcha/onnx/export.py:47-49): [temperature,
+        length_scale, dp_temperature] -> keyword arguments of synthesise.  dp_temperature is not used by the deterministic
+        duration predictor."""
+        return {"temperature": float(scales[0]), "length_scale": float(scales[1])}
+
+    def synthesise(self, x, bert, sid, phone_duration_extra=None, n_timesteps=10, temperature=1.0, length_scale=1.0,
+                   guidance_scale=0.5, noise=None, seed=0, return_prior=False):
+        """x: the ids [n_streams, T] of one utterance, or a list of them; bert [bert_dim, T] and phone_duration_extra [T] (or
+        None) alike; sid: a speaker id for all, or one per utterance; noise: [noise_channels, >= ceil4(frames)] per utterance
+        standing in for torch.randn over the padded frame axis, or None for the engine's Philox(seed).  Returns the
+        reference's names: mel and decoder_outputs [noise_channels, frames] (denormalised and as the model produces them),
+        mel_lengths, durations [T] (w_round), and with return_prior encoder_outputs / mel_enc; each a list for a list."""
+        single = not isinstance(x, (list, tuple))
+        xs = [np.asarray(u, np.int64) for u in ([x] if single else x)]
+        berts = [np.asarray(u, np.float32) for u in ([bert] if single else bert)]
+        B, T = len(xs), max(u.shape[1] for u in xs)
+        ids = np.zeros((B, xs[0].shape[0], T), np.int64)
+        feats = np.zeros((B, T, berts[0].shape[0]), np.float32)
+        pause = None if phone_duration_extra is None else np.zeros((B, T), np.float32)
+        for b, (u, f) in enumerate(zip(xs, berts)):
+            if f.shape[1] != u.shape[1]:
+                raise ValueError("bert must have one column per token")
+            ids[b, :, :u.shape[1]] = u
+            feats[b, :u.shape[1]] = f.T
+            if pause is not None:
+                pause[b, :u.shape[1]] = np.asarray(phone_duration_extra if single else phone_duration_extra[b], np.float32).reshape(-1)
+        nz = None
+        if noise is not None:
+            nz = [np.ascontiguousarray(np.asarray(n, np.float32).T) for n in ([noise] if single else list(noise))]
+        r = self.engine.stabletts_synthesise(ids, feats, sid, lengths=[u.shape[1] for u in xs], pause=pause, n_timesteps=n_timesteps,
+                                             temperature=temperature, length_scale=length_scale, guidance_scale=guidance_scale,
+                                             noise=nz, seed=seed, want_prior=return_prior)
+        den = lambda a: a * self.mel_std + self.mel_mean          # denormalize (matcha/utils/model.py), fp32 like the reference
+        cut = lambda a: [np.ascontiguousarray(a[b, :int(r["mel_lengths"][b])].T) for b in range(B)]
+        out = {"decoder_outputs": cut(r["mel"]), "mel_lengths": [int(v) for v in r["mel_lengths"]],
+               "durations": [r["durations"][b, :xs[b].shape[1]].copy() for b in range(B)]}
+        out["mel"] = [den(m) for m in out["decoder_outputs"]]
+        if return_prior:
+            out["encoder_outputs"] = cut(r["prior"])
+            out["mel_enc"] = [den(m) for m in out["encoder_outputs"]]
+        return {k: v[0] for k, v in out.items()} if single else out
 
     def refine(self, mu_y, sid, n_timesteps=10, temperature=1.0, guidance_scale=0.5, noise=None, seed=0, denormalise=False):
         """mu_y: the aligned encoder output [cond_channels, T] of one utterance, or a list of them; sid: a speaker id for all, or

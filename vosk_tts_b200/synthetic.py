@@ -353,3 +353,32 @@ def make_random_stabletts_cfm(cfg, seed=1234):
     sd["mel_mean"] = torch.tensor(-5.5)
     sd["mel_std"] = torch.tensor(2.1)
     return sd
+
+
+def make_random_stabletts(cfg, seed=1234):
+    """make_random_stabletts_cfm plus the tensors weights.pack_stabletts reads of the text side (encoder.*, dur_spk_emb.weight),
+    for cfg = config.stabletts_config.  The embeddings are drawn at the reference's 1 / sqrt(width) (text_encoder.py:99,103);
+    the last adaLN linear of every encoder block, zero in the reference (text_encoder.py:35-38), is random for the reason given
+    there.  dp_encoder's proj gets a bias of -2.8 so that the 50 sigmoids sum to a few frames per token, as a trained model's."""
+    sd = make_random_stabletts_cfm(cfg, seed)
+    V, E, PD, BD, R, H, F, NE, G, DC = (int(cfg[k]) for k in ("n_vocab", "emb_dim", "punc_dim", "bert_dim", "bert_proj_dim",
+                                                             "enc_hidden_channels", "enc_filter_channels", "enc_n_layers", "spk_emb_dim",
+                                                             "dur_channels"))
+    k = int(cfg["enc_kernel_size"])
+    shapes = [("encoder.bert_proj.1", (R, BD))]
+    for stack, co in (("encoder.encoder.", int(cfg["noise_channels"])), ("encoder.dp_encoder.", DC)):
+        shapes.append((stack + "proj", (co, H, 1)))
+        for l in range(NE):
+            b = stack + "encoder.%d." % l
+            shapes += [(b + "adaLN_modulation.0", (H, G)), (b + "adaLN_modulation.2", (6 * H, H)), (b + "mlp.conv_1", (F, H, k)),
+                       (b + "mlp.conv_2", (H, F, k))]
+            shapes += [(b + "attn.conv_%s" % n, (H, H, 1)) for n in "qkvo"]
+    for name, shape in shapes:
+        fan = int(np.prod(shape[1:]))
+        sd[name + ".weight"] = (torch.randn(shape, generator=_gen(name + ".weight", seed)) / math.sqrt(fan)).float().contiguous()
+        sd[name + ".bias"] = (torch.randn(shape[0], generator=_gen(name + ".bias", seed)) * 0.1).float().contiguous()
+    sd["encoder.dp_encoder.proj.bias"] -= 2.8
+    for name, shape, scale in (("encoder.emb.weight", (V, E), E ** -0.5), ("encoder.punc_emb.weight", (V, PD), PD ** -0.5),
+                               ("dur_spk_emb.weight", (int(cfg["n_spks"]), G), 1.0)):
+        sd[name] = (torch.randn(shape, generator=_gen(name, seed)) * scale).float().contiguous()
+    return sd

@@ -675,26 +675,32 @@ def pack_quickvc(w, cfg, tc=True, precision=None, contentvec=None, cv=None):
     return P.finish()
 
 
-def pack_stabletts_cfm(sd, cfg):
-    """The flow-matching decoder of a MatchaTTS (StableTTS) state dict -> (blob, manifest) of a model_family "stabletts" engine.
-    sd: the checkpoint's `state_dict` entry (keys decoder.estimator.*, spk_emb.weight, fake_speaker, fake_content, mel_mean,
-    mel_std); cfg: config.stabletts_cfm_config.  Convs go in the FFMA layout (q, k, v stacked into one 1x1 conv), the small
-    linears of the conditioning path (time_mlp, each block's film conv and adaLN_modulation) row-major [out][in] and stacked
-    over the blocks.  Everything is fp32: the decoder runs on the FFMA pipe in every precision mode, so there are no
-    mode-dependent split planes to add yet."""
+def _sd_getter(sd):
     g = lambda k: sd[k].detach().cpu().float().numpy() if hasattr(sd[k], "detach") else np.asarray(sd[k], np.float32)
-    e = "decoder.estimator."
-    NC, MC, H, F, NL, G = (int(cfg[k]) for k in ("noise_channels", "cond_channels", "hidden_channels", "filter_channels", "n_layers",
-                                                 "spk_emb_dim"))
-    k = int(cfg["kernel_size"])
 
     def want(name, shape):
         a = g(name)
         if tuple(a.shape) != tuple(shape):
             raise ValueError("%s has shape %s, expected %s" % (name, tuple(a.shape), tuple(shape)))
         return a
+    return g, want
 
-    P = _Packer()
+
+def _pack_dit_block(P, g, want, dst, src, H, F, k):
+    """qkv / o / ffn1 / ffn2 of one DiTConVBlock (diffusion_transformer.py:82-96) at state-dict prefix src -> tensors dst.*"""
+    a = src + "attn.conv_%s."
+    P.conv(dst + ".qkv", np.concatenate([want(a % n + "weight", (H, H, 1)) for n in "qkv"], 0), np.concatenate([g(a % n + "bias") for n in "qkv"]))
+    P.conv(dst + ".o", want(a % "o" + "weight", (H, H, 1)), g(a % "o" + "bias"))
+    P.conv(dst + ".ffn1", want(src + "mlp.conv_1.weight", (F, H, k)), g(src + "mlp.conv_1.bias"))
+    P.conv(dst + ".ffn2", want(src + "mlp.conv_2.weight", (H, F, k)), g(src + "mlp.conv_2.bias"))
+
+
+def _pack_stabletts_decoder(P, sd, cfg):
+    g, want = _sd_getter(sd)
+    e = "decoder.estimator."
+    NC, MC, H, F, NL, G = (int(cfg[k]) for k in ("noise_channels", "cond_channels", "hidden_channels", "filter_channels", "n_layers",
+                                                 "spk_emb_dim"))
+    k = int(cfg["kernel_size"])
     for i, (j, co, ci) in enumerate(((0, F, MC), (2, F, F), (4, H, F))):
         P.conv("st.cp%d" % i, want(e + "cond_proj.%d.weight" % j, (co, ci, k)), want(e + "cond_proj.%d.bias" % j, (co,)))
     P.conv("st.in", want(e + "in_proj.weight", (H, NC + H, 1)), g(e + "in_proj.bias"))
@@ -716,12 +722,49 @@ def pack_stabletts_cfm(sd, cfg):
     P.add("st.mel_mean", np.asarray(g("mel_mean"), np.float32).reshape(1))
     P.add("st.mel_std", np.asarray(g("mel_std"), np.float32).reshape(1))
     for l in range(NL):
-        a = b % l + "block.attn.conv_%s."
-        P.conv("st.l%d.qkv" % l, np.concatenate([want(a % n + "weight", (H, H, 1)) for n in "qkv"], 0),
-               np.concatenate([g(a % n + "bias") for n in "qkv"]))
-        P.conv("st.l%d.o" % l, want(a % "o" + "weight", (H, H, 1)), g(a % "o" + "bias"))
-        P.conv("st.l%d.ffn1" % l, want(b % l + "block.mlp.conv_1.weight", (F, H, k)), g(b % l + "block.mlp.conv_1.bias"))
-        P.conv("st.l%d.ffn2" % l, want(b % l + "block.mlp.conv_2.weight", (H, F, k)), g(b % l + "block.mlp.conv_2.bias"))
+        _pack_dit_block(P, g, want, "st.l%d" % l, b % l + "block.", H, F, k)
     for j in range(NL // 2):
         P.conv("st.lsc%d" % j, want(e + "lsc_layers.%d.weight" % j, (H, 2 * H, k)), g(e + "lsc_layers.%d.bias" % j))
+
+
+def pack_stabletts_cfm(sd, cfg):
+    """The flow-matching decoder of a MatchaTTS (StableTTS) state dict -> (blob, manifest) of a model_family "stabletts" engine.
+    sd: the checkpoint's `state_dict` entry (keys decoder.estimator.*, spk_emb.weight, fake_speaker, fake_content, mel_mean,
+    mel_std); cfg: config.stabletts_cfm_config.  Convs go in the FFMA layout (q, k, v stacked into one 1x1 conv), the small
+    linears of the conditioning path (time_mlp, each block's film conv and adaLN_modulation) row-major [out][in] and stacked
+    over the blocks.  Everything is fp32: the decoder runs on the FFMA pipe in every precision mode, so there are no
+    mode-dependent split planes to add yet."""
+    P = _Packer()
+    _pack_stabletts_decoder(P, sd, cfg)
+    return P.finish()
+
+
+def pack_stabletts(sd, cfg):
+    """A MatchaTTS (StableTTS) state dict without its vocoder -> (blob, manifest) of an engine that serves text-to-mel
+    (vtts_stabletts_synthesise) and the decoder alone: the decoder part of pack_stabletts_cfm, then the text encoder
+    (encoder.emb, encoder.punc_emb, encoder.bert_proj.1, both stacks encoder.encoder / encoder.dp_encoder with their proj) and
+    dur_spk_emb.  cfg: config.stabletts_config."""
+    if "enc_n_layers" not in cfg:
+        raise ValueError("pack_stabletts needs config.stabletts_config (the text encoder's constants), not stabletts_cfm_config")
+    g, want = _sd_getter(sd)
+    P = _Packer()
+    _pack_stabletts_decoder(P, sd, cfg)
+    V, E, PD, BD, R, H, F, NE, G, DC = (int(cfg[k]) for k in ("n_vocab", "emb_dim", "punc_dim", "bert_dim", "bert_proj_dim",
+                                                             "enc_hidden_channels", "enc_filter_channels", "enc_n_layers", "spk_emb_dim",
+                                                             "dur_channels"))
+    k = int(cfg["enc_kernel_size"])
+    P.add("st.enc.emb", want("encoder.emb.weight", (V, E)))
+    P.add("st.enc.punc", want("encoder.punc_emb.weight", (V, PD)))
+    P.add("st.enc.bert.w", want("encoder.bert_proj.1.weight", (R, BD)))
+    P.add("st.enc.bert.b", want("encoder.bert_proj.1.bias", (R,)))
+    P.add("st.dur_spk_emb", want("dur_spk_emb.weight", (int(cfg["n_spks"]), G)))
+    for dst, src, co in (("st.enc.mel", "encoder.encoder.", int(cfg["noise_channels"])), ("st.enc.dp", "encoder.dp_encoder.", DC)):
+        b = src + "encoder.%d."
+        for l in range(NE):
+            _pack_dit_block(P, g, want, "%s.l%d" % (dst, l), b % l, H, F, k)
+        P.add(dst + ".ada.w1", np.stack([want(b % l + "adaLN_modulation.0.weight", (H, G)) for l in range(NE)]))
+        P.add(dst + ".ada.b1", np.stack([g(b % l + "adaLN_modulation.0.bias") for l in range(NE)]))
+        P.add(dst + ".ada.w2", np.stack([want(b % l + "adaLN_modulation.2.weight", (6 * H, H)) for l in range(NE)]))
+        P.add(dst + ".ada.b2", np.stack([g(b % l + "adaLN_modulation.2.bias") for l in range(NE)]))
+        P.conv(dst + ".proj", want(src + "proj.weight", (co, H, 1)), g(src + "proj.bias"))
     return P.finish()
