@@ -509,6 +509,39 @@ int vtts_stabletts_synthesise(vtts_handle h, const int64_t* ids, const int64_t* 
                               float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld,
                               int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise);
 
+/* StableTTS vocoder: the HiFi-GAN Generator of training/stabletts/matcha/hifigan/models.py:148-206 (conv_pre, n_upsamples x
+ * (LeakyReLU 0.1, ConvTranspose1d, mean of the MRF resblocks), LeakyReLU 0.01, conv_post, tanh), as cli.py:65-71 loads it
+ * (config v1, weight norm removed) and calls it on a denormalised mel; the reference's clamp(-1, 1) after tanh changes
+ * nothing.  Engines whose blob carries dec.* (StableTTS(..., vocoder=...), weights.pack_hifigan), described by the decoder
+ * fields of vtts_config: decoder_type 1, resblock_*, upsample_*, upsample_initial_channel, inter_channels = st_noise.
+ * Each utterance is vocoded as if alone (zero padding at its own ends, as the reference at batch 1).
+ *   mel          float [B, mel_ld, st_noise], frame-major, denormalised; utterance b = its first mel_lengths[b] frames,
+ *                1 <= mel_lengths[b] <= mel_ld
+ *   wav          out float [B, wav_ld]: utterance b's wav_lengths[b] = hop * mel_lengths[b] samples (hop = the product of the
+ *                upsampling rates, 256 for v1); the rest of each row is not written
+ * Host pointers, atomic on the handle; graphed per (batch, frame bucket).  Precision 0 runs every conv on the fp32 FFMA pipe
+ * in one fixed launch shape: the waveform is bit-identical alone, in any batch, eager and replayed.  Precision >= 1 runs the
+ * upsampling convs whose input width is a multiple of 64 and the MRFs of the stages before the last such conv on the
+ * split-bf16 tensor cores (for v1: every upsampling conv and the MRFs of stages 1-3); their split-K plans follow the batch,
+ * so the waveform is bit-identical eager and replayed but may differ in the last bits between batch shapes.
+ * VTTS_ERR_INVALID: not a StableTTS engine, a blob without a vocoder, B < 1, a length outside [1, mel_ld], a batch whose
+ * largest vocoder buffer would exceed 2^31 values.  VTTS_ERR_CAPACITY: wav_ld < hop * max(mel_lengths). */
+int vtts_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* wav, int64_t wav_ld,
+                        int64_t* wav_lengths);
+
+/* StableTTS text-to-waveform: vtts_stabletts_synthesise followed by vtts_hifigan_vocode on its denormalised mel, in the same two
+ * enqueues (the vocoder runs in the mel phase's graph on the mel rows already on the device: no mel round trip, one host wait
+ * between the phases as before).  Arguments as vtts_stabletts_synthesise, plus wav [B, wav_ld] and wav_lengths int64 [B]
+ * (= hop * mel_lengths) as vtts_hifigan_vocode; mel_out may be NULL (then prior_out must be NULL too).  Each utterance is
+ * vocoded over its own frame count, not its padded extent (matcha_tts.py:184, 207).  Precision 0: wav is bit-identical to
+ * vtts_stabletts_synthesise followed by vtts_hifigan_vocode on its denormalised mel.  VTTS_ERR_INVALID also for a blob without
+ * a vocoder.  VTTS_ERR_CAPACITY, returned after the text phase with mel_lengths filled in: also wav_ld < hop * max(mel_lengths). */
+int vtts_stabletts_synthesise_wav(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max, const float* bert,
+                                  const float* pause, const int64_t* sid, int n_timesteps, float temperature, float length_scale,
+                                  float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld,
+                                  int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise, float* wav, int64_t wav_ld,
+                                  int64_t* wav_lengths);
+
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are
  * read with vtts_last_error(NULL) on the calling thread.

@@ -234,6 +234,45 @@ def stabletts_config(overrides=None):
     return out
 
 
+# The HiFi-GAN vocoder StableTTS's cli.py:65-71 loads (hifigan_T2_v1 / hifigan_univ_v1): always config v1 of
+# matcha/hifigan/config.py, its Generator reading 80 mel channels (models.py:154).
+HIFIGAN_V1 = {
+    "resblock": "1", "upsample_rates": [8, 8, 2, 2], "upsample_kernel_sizes": [16, 16, 4, 4], "upsample_initial_channel": 512,
+    "resblock_kernel_sizes": [3, 7, 11], "resblock_dilation_sizes": [[1, 3, 5], [1, 3, 5], [1, 3, 5]], "num_mels": 80,
+}
+
+
+def hifigan_config(h=None):
+    """The vocoder's shape from the reference's config-dict keys (HIFIGAN_V1 where `h` is None or leaves a key out).  Refuses,
+    with the reason, what the engine does not build."""
+    out = copy.deepcopy(HIFIGAN_V1)
+    out.update({k: copy.deepcopy(v) for k, v in (h or {}).items() if k in HIFIGAN_V1})
+    ur, uk, rk, rd = out["upsample_rates"], out["upsample_kernel_sizes"], out["resblock_kernel_sizes"], out["resblock_dilation_sizes"]
+    if str(out["resblock"]) not in ("1", "2"):
+        raise ValueError("resblock must be '1' or '2'")
+    out["resblock"] = str(out["resblock"])
+    if not 1 <= len(ur) <= 8 or len(uk) != len(ur) or any(k < u or (k - u) % 2 for u, k in zip(ur, uk)):
+        raise ValueError("1..8 upsampling stages, each kernel >= its rate with kernel - rate even (padding (k - u) / 2 emits u T samples)")
+    c0 = int(out["upsample_initial_channel"])
+    if c0 % (1 << len(ur)) or (c0 >> len(ur)) % 16:
+        raise ValueError("upsample_initial_channel must halve to a multiple of 16 at every stage (the FFMA conv's channel chunk)")
+    if not 1 <= len(rk) <= 3 or len(rd) != len(rk) or len({len(d) for d in rd}) != 1 or not 1 <= len(rd[0]) <= 8:
+        raise ValueError("1..3 resblock kernels per stage, each with the same number (1..8) of dilations")
+    if any(k % 2 == 0 for k in rk):
+        raise ValueError("resblock kernels must be odd")
+    if int(out["num_mels"]) % 16:
+        raise ValueError("num_mels must be a multiple of 16 (the FFMA conv's channel chunk)")
+    return out
+
+
+def hop_samples(h):
+    """Samples per mel frame of a vocoder config: the product of its upsampling rates (256 for v1)."""
+    n = 1
+    for u in h["upsample_rates"]:
+        n *= int(u)
+    return n
+
+
 def convt_pad(cfg, i):
     """(padding, output_padding) of the decoder's upsampling ConvTranspose1d of stage i: (K-u)//2 and 0 in VITS2
     (training/vits2/models.py, every generator), (K-u+1-i)//2 and 1-i in QuickVC (vc/models.py:428-430).  The engine lays out

@@ -31,6 +31,7 @@
 #include "contentvec.cuh"
 #include "dit.cuh"
 #include "stabletts.cuh"
+#include "hifigan.cuh"
 #include "resample.cuh"
 #include "owned.cuh"
 
@@ -362,7 +363,7 @@ struct vtts_engine {
   // phase tag, the first element of every key
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
-    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2
+    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2, TAG_HIFIGAN = 0xD3
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -539,11 +540,12 @@ struct vtts_engine {
   struct DecPl { Planes pz, cur; std::vector<Planes> px, nxt; std::vector<std::vector<Planes>> pj, pt; } dcp;
   void alloc_flow_planes();
   void alloc_decoder_planes();
-  void decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready);
+  bool decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready);
   void flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, const float* cond, int cond_ld, bool forward);
   void launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen, Planes* pl);
   void bind_weights();
   void bind_flow_decoder();
+  void bind_decoder();
   void bind_wn_encoder(const std::string& p, int cin);
   void launch_conv(const std::vector<ConvP>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
   void encoder_layer(const EncLayerW& L, float*& x, float*& xb, float* qkv, float* ao, float* y, float* ffh, int Hc, int Fc,
@@ -708,6 +710,16 @@ struct vtts_engine {
   struct SttPin { int* ints; float *prm, *pause, *bert; };
   SttPin stt_layout();
   void stt_enqueue(bool prior);
+
+  // ---- StableTTS vocoder (the HiFi-GAN Generator of matcha/hifigan/models.py; hifigan.cuh), bound into the decoder members
+  // (dec.*) when the blob carries it.  In precision modes >= 1 the first voc_nt upsampling stages and their MRFs run on the
+  // tensor cores, the upsampling conv after them too; conv_pre, the later MRFs and conv_post stay on the FFMA pipe.
+  bool has_voc = false;
+  int voc_nt = 0;
+  Buf<int> d_hgi;                                  // [len B][off B] of vtts_hifigan_vocode
+  Buf<float> d_hgmel;                              // the denormalised mel rows the vocoder reads [Tfrm][st_noise]
+  PinnedBuf<char> h_pin_hg;
+  void voc_enqueue(const float* mel, const int* fl, const int* fo);
 
   // ---- resampling of recordings (vtts_resample; resample.cuh): the taps of each rate pair, uploaded on first use
   struct RsTaps { Buf<float> taps; int up = 0, down = 0, K = 0; };
@@ -911,9 +923,28 @@ void vtts_engine::bind_flow_decoder() {
     }
     flow.push_back(F);
   }
+  bind_decoder();
+}
+
+// The decoder (dec.*): the VITS2 / QuickVC decoders behind the flow, or the StableTTS vocoder (has_voc).
+void vtts_engine::bind_decoder() {
+  const vtts_config& c = cfg;
+  const int I = c.inter_channels;
   tc = c.precision >= 1 && c.precision <= 3;
-  dec_pre = conv("dec.pre", I, c.upsample_initial_channel, 7, !tc);
-  if (tc) {
+  voc_nt = 0;
+  if (has_voc && tc) {
+    // the leading stages whose MRF width is a multiple of 64 (TC_BK) go to the tensor cores, and so does the upsampling conv
+    // after them, which hands fp32 rows to the first FFMA stage; conv_post always reads fp32 rows
+    REQUIRE(c.resblock_type == 1, VTTS_ERR_INVALID, "unsupported vocoder: in precision modes >= 1 the tensor-core stages take ResBlock1 only");
+    int w = c.upsample_initial_channel;
+    while (voc_nt < c.n_upsamples && (w / 2) % TC_BK == 0) { w /= 2; ++voc_nt; }
+    REQUIRE(voc_nt >= 1 && voc_nt < c.n_upsamples, VTTS_ERR_INVALID,
+            "unsupported vocoder for precision modes >= 1: the first stage's width must be a multiple of 64 and the last stage's not "
+            "(use precision 0)");
+  }
+  const bool pre_tc = tc && !has_voc;              // (the vocoder's conv_pre reads 80 mel channels: FFMA)
+  dec_pre = conv("dec.pre", I, c.upsample_initial_channel, 7, !pre_tc);
+  if (pre_tc) {
     REQUIRE(c.decoder_type == 0 && c.resblock_type == 1, VTTS_ERR_INVALID, "tensor-core mode supports the MB-iSTFT / ResBlock1 decoder");
     tc_pre = tcw("dec.pre", I, c.upsample_initial_channel, 7);
   }
@@ -922,6 +953,7 @@ void vtts_engine::bind_flow_decoder() {
   int ch = c.upsample_initial_channel;
   up_total = 1;
   for (int i = 0; i < c.n_upsamples; ++i) {
+    const bool up_tc = tc && (!has_voc || i <= voc_nt), mrf_tc = tc && (!has_voc || i < voc_nt);
     // ConvTranspose1d padding: (K-u)/2 in VITS2 (training/vits2/models.py:857-858, 989-990), (K-u+1-i)/2 with output_padding 1-i in
     // QuickVC (vc/models.py:428-430); both make exactly u*T output rows (config.convt_pad checks QuickVC's)
     const int u = c.upsample_rates[i], K = c.upsample_kernel_sizes[i];
@@ -931,8 +963,8 @@ void vtts_engine::bind_flow_decoder() {
       // polyphase split of ConvTranspose1d (see weights.convt_phases): taps per phase and left padding
       int d_min = -((r + p) / u);
       int d_max = (K - 1 - r - p) / u;
-      U.phase.push_back(conv("dec.up" + std::to_string(i) + ".p" + std::to_string(r), ch, ch / 2, d_max - d_min + 1, !tc));
-      if (tc) U.tphase.push_back(tcw("dec.up" + std::to_string(i) + ".p" + std::to_string(r), ch, ch / 2, d_max - d_min + 1));
+      U.phase.push_back(conv("dec.up" + std::to_string(i) + ".p" + std::to_string(r), ch, ch / 2, d_max - d_min + 1, !up_tc));
+      if (up_tc) U.tphase.push_back(tcw("dec.up" + std::to_string(i) + ".p" + std::to_string(r), ch, ch / 2, d_max - d_min + 1));
       U.pad.push_back(d_max);
     }
     ups.push_back(U);
@@ -943,9 +975,9 @@ void vtts_engine::bind_flow_decoder() {
       const std::string p2 = "dec.rb" + std::to_string(i * c.n_resblock_kernels + j);
       for (int d = 0; d < c.n_resblock_dilations; ++d) {
         if (c.resblock_type == 1) {
-          R.c1.push_back(conv(p2 + ".c1." + std::to_string(d), ch, ch, c.resblock_kernel_sizes[j], !tc));
-          R.c2.push_back(conv(p2 + ".c2." + std::to_string(d), ch, ch, c.resblock_kernel_sizes[j], !tc));
-          if (tc) {
+          R.c1.push_back(conv(p2 + ".c1." + std::to_string(d), ch, ch, c.resblock_kernel_sizes[j], !mrf_tc));
+          R.c2.push_back(conv(p2 + ".c2." + std::to_string(d), ch, ch, c.resblock_kernel_sizes[j], !mrf_tc));
+          if (mrf_tc) {
             R.t1.push_back(tcw(p2 + ".c1." + std::to_string(d), ch, ch, c.resblock_kernel_sizes[j]));
             R.t2.push_back(tcw(p2 + ".c2." + std::to_string(d), ch, ch, c.resblock_kernel_sizes[j]));
           }
@@ -969,6 +1001,15 @@ void vtts_engine::bind_flow_decoder() {
     dec_post = conv("dec.post", ch, 1, 7);
     hop = up_total;
   }
+}
+
+// The vocoder of a StableTTS engine over mel rows [rows][st_noise] (utterance b: fl[b] rows from fo[b]) -> d_wav, sample
+// offset fo[b] * hop.  The FFMA convs run in one fixed launch shape (no split-K, one thread group), so that in precision mode
+// 0 an utterance's waveform does not depend on what it is batched with.
+void vtts_engine::voc_enqueue(const float* mel, const int* fl, const int* fo) {
+  SavedLaunch saved(this);
+  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
+  decode(const_cast<float*>(mel), fl, fo);
 }
 
 CUtensorMap vtts_engine::make_map(const void* base, int C, long rows, int box_rows) {
@@ -1412,13 +1453,13 @@ void vtts_engine::alloc_flow_planes() {
 void vtts_engine::alloc_decoder_planes() {
   const vtts_config& c = cfg;
   const long F = Tfrm;
-  const int nk = c.n_resblock_kernels;
+  const int nk = c.n_resblock_kernels, nst = has_voc ? voc_nt : c.n_upsamples;
   int slot = 0;
   dcp.pz = planes(slot++, F, 1, c.inter_channels);
   dcp.cur = planes(slot++, F, 1, c.upsample_initial_channel);
   dcp.px.resize(c.n_upsamples); dcp.nxt.resize(c.n_upsamples); dcp.pj.resize(c.n_upsamples); dcp.pt.resize(c.n_upsamples);
   int rmp = 1, chp = c.upsample_initial_channel;
-  for (int i = 0; i < c.n_upsamples; ++i) {
+  for (int i = 0; i < nst; ++i) {
     rmp *= c.upsample_rates[i];
     chp /= 2;
     dcp.px[i] = planes(slot++, F, rmp, chp);
@@ -1521,23 +1562,29 @@ void vtts_engine::wn_tc(const std::vector<TcW>& t_in, const std::vector<ConvW>& 
 }
 
 // Decoder on the tensor cores (models.py:1016-1040): every conv consumes the split-bf16 planes written by its
-// producer's epilogue; fp32 copies exist only where a residual or the MRF mean needs them.
-void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready) {
+// producer's epilogue; fp32 copies exist only where a residual or the MRF mean needs them.  The StableTTS vocoder runs only
+// its first voc_nt stages here, from an FFMA conv_pre that writes the planes, and then the next upsampling conv into fp32
+// rows d_stage[voc_nt]: returns false, and decode() continues on the FFMA pipe from there.
+bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready) {
   const vtts_config& c = cfg;
   const int I = c.inter_channels;
   const long F = Tfrm;
-  const int nk = c.n_resblock_kernels, nd = c.n_resblock_dilations;
+  const int nk = c.n_resblock_kernels, nd = c.n_resblock_dilations, nst = has_voc ? voc_nt : c.n_upsamples;
   Planes pz = dcp.pz, cur = dcp.cur;
   const std::vector<Planes>&st_px = dcp.px, &st_nxt = dcp.nxt;
   const std::vector<std::vector<Planes>>&st_pj = dcp.pj, &st_pt = dcp.pt;
-  if (!pz_ready) {
+  if (!pz_ready && !has_voc) {
     dim3 g((maxFrm + EW_ROWS - 1) / EW_ROWS, B);
     klaunch(split_planes_kernel, dim3(g), dim3(EW_THREADS), (size_t)(0), z, I, pz.hi, pz.lo, I, I, 1.f, 0, 1, fl, fo);
     CK(cudaGetLastError());
     ++launches;
   }
   int ch = c.upsample_initial_channel;
-  {
+  if (has_voc) {         // conv_pre on the FFMA pipe, its output handed over as the planes of lrelu(x, 0.1)
+    ConvP p = mk(dec_pre, z, I, 0, ensure(d_d0, (size_t)F * ch), ch, 0, 1, 3);
+    p.p_hi = cur.hi; p.p_lo = cur.lo; p.ldp = ch; p.pl_slope = 0.1f;
+    launch_conv({p}, 1, fl, fo, maxFrm, B);
+  } else {
     TcSpec q;
     q.in = pz; q.w = tc_pre; q.bias = dec_pre.b; q.Cin = I; q.Cout = ch; q.k = 7; q.dil = 1; q.pad = 3;
     q.out = cur; q.pl_slope = 0.1f;
@@ -1553,7 +1600,7 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     for (int i = 0; i < c.n_upsamples; ++i) { d_xj[i].resize(nk); d_tmp[i].resize(nk); }
   }
   float* lastX = nullptr;
-  for (int i = 0; i < c.n_upsamples; ++i) {
+  for (int i = 0; i < nst; ++i) {
     const int u = c.upsample_rates[i], ch2 = ch / 2;
     const long rows = F * rm * u;
     float* X = ensure(d_stage[i], (size_t)rows * ch2);
@@ -1640,6 +1687,22 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     lastX = X;
   }
   (void)lastX;
+  if (has_voc) {
+    const int u = c.upsample_rates[nst], ch2 = ch / 2;
+    float* X = ensure(d_stage[nst], (size_t)F * rm * u * ch2);
+    for (int r0 = 0; r0 < u; r0 += TC_MAXP) {
+      std::vector<TcSpec> ps;
+      for (int r = r0; r < std::min(u, r0 + TC_MAXP); ++r) {
+        TcSpec q;
+        q.in = cur; q.w = ups[nst].tphase[r]; q.bias = ups[nst].phase[r].b; q.Cin = ch; q.Cout = ch2;
+        q.k = ups[nst].phase[r].k; q.dil = 1; q.pad = ups[nst].pad[r];
+        q.y = X; q.ldy = ch2; q.out_mul = u; q.out_add = r;
+        ps.push_back(q);
+      }
+      launch_tc(ps, rm, fl, fo, maxFrm, B);
+    }
+    return false;
+  }
   const int cps = c.istft_n_fft + 2, pc = c.subbands * cps;
   float* post = ensure(d_post, ((size_t)F * rm + B) * pc);
   {
@@ -1656,6 +1719,7 @@ void vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
   klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1, istft_w2);
   CK(cudaGetLastError());
   ++launches;
+  return true;
 }
 
 void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB) {
@@ -2263,24 +2327,27 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
   const int I = c.inter_channels;
   const size_t F = (size_t)Tfrm;
   // ---- decoder (models.py:1016-1054 / 872-891)
+  int ch = c.upsample_initial_channel, rm = 1, i0 = 0;
+  float* cur = nullptr;
   if (tc) {
     if (!planes_ready) {          // (chunked decoding: the decoder runs on its own)
       begin_planes();
       alloc_decoder_planes();
       flush_tails(fl, fo);
     }
-    decoder_tc(z, fl, fo, pz_ready);
-    if (!capturing) CK(cudaEventRecord(ev[6], stream));
-    return;
-  }
-  int ch = c.upsample_initial_channel;
-  float* cur = ensure(d_d0, F * ch);
-  {
+    if (decoder_tc(z, fl, fo, pz_ready)) {
+      if (!capturing) CK(cudaEventRecord(ev[6], stream));
+      return;
+    }
+    // the vocoder: stages voc_nt.. on the FFMA pipe, from the upsampled rows decoder_tc left in d_stage[voc_nt]
+    i0 = voc_nt;
+    for (int i = 0; i < i0; ++i) { rm *= c.upsample_rates[i]; ch /= 2; }
+  } else {
+    cur = ensure(d_d0, F * ch);
     ConvP p = mk(dec_pre, z, I, 0, cur, ch, 0, 1, 3);
     if (r_dec >= 0) { p.cond = d_condv.p + r_dec; p.cond_ld = condR; }     // x = conv_pre(z) + cond(g)
     launch_conv({p}, 1, fl, fo, maxFrm, B);
   }
-  int rm = 1;
   const int nk = c.n_resblock_kernels, nd = c.n_resblock_dilations;
   if ((int)d_stage.size() < c.n_upsamples) {
     d_stage.resize(c.n_upsamples);
@@ -2288,11 +2355,11 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     d_tmp.resize(c.n_upsamples);
     for (int i = 0; i < c.n_upsamples; ++i) { d_xj[i].resize(nk); d_tmp[i].resize(nk); }
   }
-  for (int i = 0; i < c.n_upsamples; ++i) {
+  for (int i = i0; i < c.n_upsamples; ++i) {
     const int u = c.upsample_rates[i], ch2 = ch / 2;
     const size_t rows = F * rm * u;
     float* X = ensure(d_stage[i], rows * ch2);
-    for (int r0 = 0; r0 < u; r0 += CV_MAXP) {
+    for (int r0 = 0; r0 < u && cur; r0 += CV_MAXP) {
       std::vector<ConvP> ps;
       for (int r = r0; r < std::min(u, r0 + CV_MAXP); ++r) {
         ConvP p = mk(ups[i].phase[r], cur, ch, 0, X, ch2, 0, 1, ups[i].pad[r]);
@@ -2980,6 +3047,21 @@ void vtts_engine::bind_stabletts() {
     L.relk = L.relv = zero;
     st_blk.push_back(L);
     if (l >= NL / 2) st_lsc.push_back(conv("st.lsc" + std::to_string(l - NL / 2), 2 * H, H, k));
+  }
+  // the vocoder, when the blob carries it (weights.pack_hifigan): described by the decoder fields of the config
+  has_voc = tensors.count("dec.pre.w") > 0;
+  if (has_voc) {
+    REQUIRE(c.decoder_type == 1, VTTS_ERR_INVALID, "unsupported vocoder: only the HiFi-GAN Generator (decoder_type 1) is built");
+    REQUIRE(c.inter_channels == NC, VTTS_ERR_INVALID, "unsupported vocoder: conv_pre's input (inter_channels) must equal st_noise");
+    REQUIRE(c.n_upsamples >= 1 && c.n_upsamples <= 8 && c.n_resblock_kernels >= 1 && c.n_resblock_dilations >= 1 &&
+                c.n_resblock_dilations <= 8 && (c.upsample_initial_channel >> c.n_upsamples) >= CV_CK &&
+                (c.upsample_initial_channel >> c.n_upsamples) << c.n_upsamples == c.upsample_initial_channel,
+            VTTS_ERR_INVALID, "unsupported vocoder: 1..8 upsampling stages halving upsample_initial_channel to a multiple of 16");
+    REQUIRE(c.n_resblock_kernels <= 3, VTTS_ERR_INVALID, "unsupported vocoder: at most 3 resblocks per stage");
+    for (int i = 0; i < c.n_upsamples; ++i)
+      REQUIRE(c.upsample_rates[i] >= 1 && c.upsample_kernel_sizes[i] >= c.upsample_rates[i] && (c.upsample_kernel_sizes[i] - c.upsample_rates[i]) % 2 == 0,
+              VTTS_ERR_INVALID, "unsupported vocoder: every ConvTranspose1d needs kernel - rate even and >= 0 (padding (k - u) / 2 gives u T rows)");
+    bind_decoder();       // (also refuses a receptive field wider than the conv tile)
   }
   // the text encoder, when the blob carries it (weights.pack_stabletts); a decoder-only blob serves vtts_cfm_decode alone
   st_text = c.st_enc_layers > 0;
@@ -3964,8 +4046,10 @@ static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengt
 static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max, const float* bert,
                                       const float* pause, const int64_t* sid, int n, float temperature, float length_scale, float s,
                                       const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld, int64_t* mel_lengths,
-                                      int32_t* durations, float* prior_out, int denormalise) {
+                                      int32_t* durations, float* prior_out, int denormalise, float* wav = nullptr, int64_t wav_ld = 0,
+                                      int64_t* wav_lengths = nullptr) {
   const vtts_config& c = h->cfg;
+  REQUIRE(!wav || h->has_voc, VTTS_ERR_INVALID, "the weight blob has no vocoder (StableTTS(..., vocoder=...) / weights.pack_hifigan)");
   REQUIRE(h->st_text, VTTS_ERR_INVALID, "the weight blob holds the flow-matching decoder only (weights.pack_stabletts_cfm): text-to-mel needs the "
                                          "text encoder of weights.pack_stabletts");
   REQUIRE(B >= 1 && B <= 8192 && t_max >= 1 && t_max <= VTTS_ST_MAX_TOKENS, VTTS_ERR_INVALID, "bad batch size / t_max");
@@ -4028,7 +4112,9 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
   }
   REQUIRE(total < (1LL << 24), VTTS_ERR_INVALID, "the batch expands to too many frames for one call");
   const int real_max = *std::max_element(frames.begin(), frames.end()), ext_max = (real_max + 3) / 4 * 4;
-  REQUIRE(mel_ld >= real_max, VTTS_ERR_CAPACITY, "mel_ld is smaller than the longest utterance (mel_lengths holds the frame counts)");
+  REQUIRE(!mel_out || mel_ld >= real_max, VTTS_ERR_CAPACITY, "mel_ld is smaller than the longest utterance (mel_lengths holds the frame counts)");
+  REQUIRE(!wav || wav_ld >= (int64_t)real_max * h->hop, VTTS_ERR_CAPACITY,
+          "wav_ld is smaller than the longest utterance times the hop (mel_lengths holds the frame counts)");
   REQUIRE(!noise || noise_ld >= ext_max, VTTS_ERR_CAPACITY, "noise has fewer frames than the longest utterance padded to a multiple of 4 "
                                                             "(mel_lengths holds the frame counts)");
   const vtts_engine::StPin pp = st_plan(h, B, frames, extents, sid, n, temperature, s, noise != nullptr, false, true, prior, denormalise, seed);
@@ -4036,18 +4122,91 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
   if (noise)
     for (int b = 0; b < B; ++b)
       memcpy(pp.noise + (size_t)h->h_frm_off[b] * NC, noise + (size_t)b * noise_ld * NC, (size_t)extents[b] * NC * sizeof(float));
-  h->run_graphed({vtts_engine::TAG_ST_MEL, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, prior ? 1 : 0, h->maxTok, Ttok},
-                 [&] { h->st_enqueue(); });
+  // the vocoder reads the conditional sequences' rows: lens and offsets are the first B of the phase's [len NS][off NS] table
+  h->run_graphed({vtts_engine::TAG_ST_MEL, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, prior ? 1 : 0, h->maxTok, Ttok, wav ? 1 : 0},
+                 [&] {
+                   h->st_enqueue();
+                   if (wav) {
+                     const int *lens = h->d_sti.p, *offs = lens + P.NS;
+                     float* in = h->ensure(h->d_hgmel, (size_t)h->Tfrm * NC);
+                     h->klaunch(hg_mel_in_kernel, dim3(h->maxFrm, B), dim3(128), (size_t)0, (const float*)h->d_stmel.p, NC, (const float*)h->d_stf.p,
+                                h->st_mel_mean, h->st_mel_std, in, lens, offs);
+                     CK(cudaGetLastError());
+                     ++h->launches;
+                     h->voc_enqueue(in, lens, offs);
+                   }
+                 });
   const size_t plane = (size_t)h->Tfrm * NC, nread = prior ? plane + (size_t)h->real_Tfrm * NC : (size_t)h->real_Tfrm * NC;
-  float* pin = reinterpret_cast<float*>(h->ensure_pinned(2 * plane * sizeof(float) + 64));
-  CK(cudaMemcpyAsync(pin, h->d_stmel.p, nread * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  const size_t wcap = wav ? (size_t)h->Tfrm * h->hop : 0;
+  float* pin = reinterpret_cast<float*>(h->ensure_pinned((2 * plane + wcap) * sizeof(float) + 64));
+  if (mel_out || prior) CK(cudaMemcpyAsync(pin, h->d_stmel.p, nread * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (wav) CK(cudaMemcpyAsync(pin + 2 * plane, h->d_wav.p, (size_t)h->real_Tfrm * h->hop * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaEventRecord(h->ev[7], h->stream));
   CK(cudaStreamSynchronize(h->stream));
   for (int b = 0; b < B; ++b) {
     const size_t o = (size_t)h->h_frm_off[b] * NC, nb = (size_t)frames[b] * NC * sizeof(float);
-    memcpy(mel_out + (size_t)b * mel_ld * NC, pin + o, nb);
+    if (mel_out) memcpy(mel_out + (size_t)b * mel_ld * NC, pin + o, nb);
     if (prior) memcpy(prior_out + (size_t)b * mel_ld * NC, pin + plane + o, nb);
+    if (wav) {
+      memcpy(wav + (size_t)b * wav_ld, pin + 2 * plane + (size_t)h->h_frm_off[b] * h->hop, (size_t)frames[b] * h->hop * sizeof(float));
+      wav_lengths[b] = (int64_t)frames[b] * h->hop;
+    }
   }
+}
+
+static void require_vocoder(vtts_handle h) {
+  REQUIRE(h->has_voc, VTTS_ERR_INVALID, "the weight blob has no vocoder (StableTTS(..., vocoder=...) / weights.pack_hifigan)");
+}
+
+// Rows of the largest buffer the vocoder allocates for a packed batch of `rows` frames must stay below 2^31 values.
+static void voc_check_rows(vtts_handle h, int64_t rows) {
+  const vtts_config& c = h->cfg;
+  int64_t rm = 1, ch = c.upsample_initial_channel, most = rows * ch;
+  for (int i = 0; i < c.n_upsamples; ++i) { rm *= c.upsample_rates[i]; ch /= 2; most = std::max(most, rows * rm * ch); }
+  REQUIRE(most < (int64_t)INT32_MAX, VTTS_ERR_INVALID, "the batch holds too many frames for one vocoder call");
+}
+
+// StableTTS vocoder through host buffers (vtts_hifigan_vocode): one graphed enqueue per (batch, frame bucket).
+static void impl_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* wav, int64_t wav_ld,
+                                int64_t* wav_lengths) {
+  const vtts_config& c = h->cfg;
+  require_vocoder(h);
+  REQUIRE(B >= 1 && B <= 8192 && mel_ld >= 1 && mel_ld < (1LL << 24), VTTS_ERR_INVALID, "bad batch size / mel_ld");
+  std::vector<int> frames(B);
+  int64_t total = 0;
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(mel_lengths[b] >= 1 && mel_lengths[b] <= mel_ld, VTTS_ERR_INVALID, "mel_lengths must be in [1, mel_ld]");
+    frames[b] = (int)mel_lengths[b];
+    total += frames[b] + SEQ_GAP;
+  }
+  voc_check_rows(h, total + 1024);
+  const int real_max = *std::max_element(frames.begin(), frames.end());
+  REQUIRE(wav_ld >= (int64_t)real_max * h->hop, VTTS_ERR_CAPACITY, "wav_ld is smaller than the longest utterance times the hop");
+  const int NC = c.st_noise;
+  h->B = B;
+  h->have_durations = false;
+  h->have_latent = false;
+  h->pack_frames(frames);
+  voc_check_rows(h, h->Tfrm);
+  // pinned staging: ints [len B][off B], then the mel rows [Tfrm][NC] packed as the engine's rows
+  const size_t head = ((size_t)2 * B * sizeof(int) + 63) / 64 * 64;
+  char* pin = h->ensure(h->h_pin_hg, head + (size_t)h->Tfrm * NC * sizeof(float) + 64);
+  int* pi = reinterpret_cast<int*>(pin);
+  float* pm = reinterpret_cast<float*>(pin + head);
+  for (int b = 0; b < B; ++b) {
+    pi[b] = frames[b];
+    pi[B + b] = h->h_frm_off[b];
+    memcpy(pm + (size_t)h->h_frm_off[b] * NC, mel + (size_t)b * mel_ld * NC, (size_t)frames[b] * NC * sizeof(float));
+  }
+  h->run_graphed({vtts_engine::TAG_HIFIGAN, B, h->maxFrm, h->Tfrm}, [&] {
+    int* di = h->ensure(h->d_hgi, 2 * (size_t)B);
+    float* dm = h->ensure(h->d_hgmel, (size_t)h->Tfrm * NC);
+    CK(cudaMemcpyAsync(di, pi, 2 * (size_t)B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(dm, pm, (size_t)h->Tfrm * NC * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    h->voc_enqueue(dm, di, di + B);
+  });
+  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames, h->hop, wav, wav_ld);
+  for (int b = 0; b < B; ++b) wav_lengths[b] = (int64_t)frames[b] * h->hop;
 }
 
 // I0 by its power series (the Kaiser window's; np.i0 within a few ulps for the beta 5 of resample_poly)
@@ -4732,6 +4891,23 @@ int vtts_stabletts_synthesise(vtts_handle h, const int64_t* ids, const int64_t* 
   return guarded(h, [&] { impl_stabletts_synthesise(h, ids, id_lengths, B, t_max, bert, pause, sid, n_timesteps, temperature, length_scale,
                                                     guidance_scale, noise, noise_ld, seed, mel_out, mel_ld, mel_lengths, durations, prior_out,
                                                     denormalise); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
+}
+
+int vtts_stabletts_synthesise_wav(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max, const float* bert,
+                                  const float* pause, const int64_t* sid, int n_timesteps, float temperature, float length_scale,
+                                  float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld,
+                                  int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise, float* wav, int64_t wav_ld,
+                                  int64_t* wav_lengths) {
+  if (!ids || !id_lengths || !bert || !sid || !mel_lengths || !wav || !wav_lengths || (prior_out && !mel_out)) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_stabletts_synthesise(h, ids, id_lengths, B, t_max, bert, pause, sid, n_timesteps, temperature, length_scale,
+                                                    guidance_scale, noise, noise_ld, seed, mel_out, mel_ld, mel_lengths, durations, prior_out,
+                                                    denormalise, wav, wav_ld, wav_lengths); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
+}
+
+int vtts_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* wav, int64_t wav_ld,
+                        int64_t* wav_lengths) {
+  if (!mel || !mel_lengths || !wav || !wav_lengths) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_hifigan_vocode(h, mel, mel_lengths, B, mel_ld, wav, wav_ld, wav_lengths); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
 }
 
 int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, int from_rate, int to_rate,

@@ -62,7 +62,8 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_maximum_path", "vtts_maximum_path_dev", "vtts_convert", "vtts_convert_spec", "vtts_debug_conv",
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
-           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise"]
+           "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
+           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -249,6 +250,10 @@ def load_library(build_if_missing=True):
     lib.vtts_stabletts_synthesise.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, vp, i32, C.c_float, C.c_float, C.c_float, vp, C.c_int64,
                                               C.c_uint64, vp, C.c_int64, vp, vp, vp, i32]
     lib.vtts_stabletts_synthesise.restype = i32
+    lib.vtts_stabletts_synthesise_wav.argtypes = lib.vtts_stabletts_synthesise.argtypes + [vp, C.c_int64, vp]
+    lib.vtts_stabletts_synthesise_wav.restype = i32
+    lib.vtts_hifigan_vocode.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64, vp]
+    lib.vtts_hifigan_vocode.restype = i32
     _LIB = lib
     return lib
 
@@ -278,6 +283,24 @@ def live_bytes():
     return int(dev.value), int(pin.value)
 
 
+def _set_decoder_shape(c, cfg):
+    """resblock_* and upsample_* of the decoder (VITS2 / QuickVC) or of the vocoder (config.hifigan_config)."""
+    c.resblock_type = 1 if str(cfg["resblock"]) == "1" else 2
+    rk, rd = cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]
+    c.n_resblock_kernels = len(rk)
+    c.n_resblock_dilations = len(rd[0])
+    for j, k in enumerate(rk):
+        c.resblock_kernel_sizes[j] = int(k)
+        assert len(rd[j]) == len(rd[0])
+        for d, v in enumerate(rd[j]):
+            c.resblock_dilations[j][d] = int(v)
+    c.n_upsamples = len(cfg["upsample_rates"])
+    for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
+        c.upsample_rates[i] = int(u)
+        c.upsample_kernel_sizes[i] = int(k)
+    c.upsample_initial_channel = int(cfg["upsample_initial_channel"])
+
+
 def make_c_config(cfg, precision=0):
     c = VttsConfig()
     if cfg.get("model_family") == "stabletts":        # the flow-matching decoder reads none of the VITS2 fields
@@ -293,6 +316,11 @@ def make_c_config(cfg, precision=0):
                              ("st_enc_filter", "enc_filter_channels"), ("st_enc_layers", "enc_n_layers"), ("st_enc_heads", "enc_n_heads"),
                              ("st_enc_kernel", "enc_kernel_size"), ("st_dur_channels", "dur_channels")):
                 setattr(c, dst, int(cfg[src]))
+        voc = cfg.get("vocoder")
+        if voc:                                        # config.hifigan_config: the vocoder in the decoder fields
+            c.decoder_type = 1
+            c.inter_channels = int(voc["num_mels"])
+            _set_decoder_shape(c, voc)
         return c
     for k in ("n_vocab", "n_speakers", "gin_channels", "inter_channels", "hidden_channels", "filter_channels",
               "n_heads", "n_layers", "kernel_size", "window_size", "cond_layer_idx", "flow_kernel_size",
@@ -305,19 +333,7 @@ def make_c_config(cfg, precision=0):
     # 0: conv_post -> exp / pi*sin -> inverse STFT -> 63-tap filter bank (Multiband_ / Multistream_ / plain iSTFT_Generator differ only
     #    in the bank: fixed PQMF, learned, unit impulse; models.py:901-971, 974-1063, 1066-1169); 1: HiFi-GAN Generator
     c.decoder_type = 0 if cfg["decoder"] in ("mb_istft", "ms_istft", "istft") else 1
-    c.resblock_type = 1 if str(cfg["resblock"]) == "1" else 2
-    rk, rd = cfg["resblock_kernel_sizes"], cfg["resblock_dilation_sizes"]
-    c.n_resblock_kernels = len(rk)
-    c.n_resblock_dilations = len(rd[0])
-    for j, k in enumerate(rk):
-        c.resblock_kernel_sizes[j] = int(k)
-        assert len(rd[j]) == len(rd[0])
-        for d, v in enumerate(rd[j]):
-            c.resblock_dilations[j][d] = int(v)
-    c.n_upsamples = len(cfg["upsample_rates"])
-    for i, (u, k) in enumerate(zip(cfg["upsample_rates"], cfg["upsample_kernel_sizes"])):
-        c.upsample_rates[i] = int(u)
-        c.upsample_kernel_sizes[i] = int(k)
+    _set_decoder_shape(c, cfg)
     c.istft_n_fft = int(cfg["gen_istft_n_fft"])
     c.istft_hop = int(cfg["gen_istft_hop_size"])
     c.precision = int(precision)
@@ -717,15 +733,35 @@ class Engine:
                                              _ptr(mel), T, int(bool(denormalise))))
         return mel, lengths
 
+    def hifigan_vocode(self, mel, lengths=None):
+        """StableTTS vocoder (vtts_hifigan_vocode): mel frame-major [T, num_mels], [B, T, num_mels] with `lengths`, or a list of
+        ragged [T_b, num_mels] items, denormalised.  Returns (wav float32 [B, hop * max T], zeros past each utterance;
+        wav_lengths int64 [B] = hop * lengths)."""
+        mel, lengths = _batch(mel, lengths, 3, t_axis=1, ragged=True)
+        B, T = mel.shape[0], mel.shape[1]
+        voc = self.cfg.get("vocoder")
+        if not voc:
+            raise ValueError("this engine has no vocoder")
+        if mel.shape[2] != int(voc["num_mels"]):
+            raise ValueError("mel must be frame-major [.., T, %d]" % int(voc["num_mels"]))
+        hop = _config.hop_samples(voc)
+        wav = np.zeros((B, T * hop), np.float32)
+        wl = np.zeros(B, np.int64)
+        self._check(self.lib.vtts_hifigan_vocode(self.h, _ptr(mel), _ptr(lengths), B, T, _ptr(wav), T * hop, _ptr(wl)))
+        return wav, wl
+
     def stabletts_synthesise(self, ids, bert, sid, lengths=None, pause=None, n_timesteps=10, temperature=1.0, length_scale=1.0,
-                             guidance_scale=0.5, noise=None, seed=0, mel_frames=None, want_prior=False, denormalise=False):
+                             guidance_scale=0.5, noise=None, seed=0, mel_frames=None, want_prior=False, denormalise=False,
+                             want_wav=False):
         """StableTTS text-to-mel (vtts_stabletts_synthesise).  ids int [B, n_streams, T] (or [n_streams, T]); bert float [B, T,
         bert_dim] token-major; lengths int [B] (None: T for all); pause float [B, T] or None; sid int [B] (or one for all);
         noise float [B, >= ceil4(frames), noise_channels] frame-major over the padded frame axis, or None for Philox(seed).
         mel_frames: the frame capacity of the result; None asks the engine for the frame counts first (a call with no room,
         which ends after the text phase) and then runs the call with exactly enough.  Returns a dict: mel [B, frames,
         noise_channels] frame-major (zeros past each utterance), mel_lengths int64 [B], durations int32 [B, T], and prior (the
-        expanded mel encoder output) when want_prior."""
+        expanded mel encoder output) when want_prior, and with want_wav the vocoder's wav [B, hop * frames] (zeros past each
+        utterance) and wav_lengths int64 [B] (vtts_stabletts_synthesise_wav: the vocoder reads the denormalised mel on the
+        device)."""
         ids = np.ascontiguousarray(ids, dtype=np.int64)
         if ids.ndim == 2:
             ids = ids[None]
@@ -758,12 +794,20 @@ class Engine:
             mel_frames = int(per.sum(1).max())
         mel = np.zeros((B, int(mel_frames), NC), np.float32)
         prior = np.zeros_like(mel) if want_prior else None
-        self._check(self.lib.vtts_stabletts_synthesise(self.h, _ptr(ids), _ptr(lengths), B, T, _ptr(bert), _ptr(pause), _ptr(sid), int(n_timesteps),
-                                                       float(temperature), float(length_scale), float(guidance_scale), _ptr(noise), noise_ld,
-                                                       int(seed), _ptr(mel), int(mel_frames), _ptr(mel_len), _ptr(dur), _ptr(prior),
-                                                       int(bool(denormalise))))
+        args = (self.h, _ptr(ids), _ptr(lengths), B, T, _ptr(bert), _ptr(pause), _ptr(sid), int(n_timesteps), float(temperature),
+                float(length_scale), float(guidance_scale), _ptr(noise), noise_ld, int(seed), _ptr(mel), int(mel_frames), _ptr(mel_len),
+                _ptr(dur), _ptr(prior), int(bool(denormalise)))
+        if want_wav:
+            hop = _config.hop_samples(self.cfg["vocoder"]) if self.cfg.get("vocoder") else 1
+            wav = np.zeros((B, int(mel_frames) * hop), np.float32)
+            wl = np.zeros(B, np.int64)
+            self._check(self.lib.vtts_stabletts_synthesise_wav(*args, _ptr(wav), wav.shape[1], _ptr(wl)))
+        else:
+            self._check(self.lib.vtts_stabletts_synthesise(*args))
         top = int(mel_len.max())
         out = {"mel": np.ascontiguousarray(mel[:, :top]), "mel_lengths": mel_len, "durations": dur}
+        if want_wav:
+            out["wav"], out["wav_lengths"] = np.ascontiguousarray(wav[:, :top * hop]), wl
         if want_prior:
             out["prior"] = np.ascontiguousarray(prior[:, :top])
         return out

@@ -1,8 +1,8 @@
 """StableTTS on the GPU, as far as it is built: text-to-mel (MatchaTTS.synthesise of training/stabletts/matcha/models/
 matcha_tts.py:93-211: multistream ids, BERT features and pause durations in, durations and mel out) and its
-conditional-flow-matching decoder alone (CFM.forward of components/flow_matching.py, called at matcha_tts.py:183).  The BERT
-model and the vocoder are not part of this module: a caller supplies the BERT features, as the exported graph's `bert` feed
-does, and vocodes the mel itself."""
+conditional-flow-matching decoder alone (CFM.forward of components/flow_matching.py, called at matcha_tts.py:183), and, with a
+HiFi-GAN checkpoint (matcha/hifigan, as cli.py:65-71 loads it), the vocoder: mel to waveform, and text to waveform in one call.
+The BERT model is not part of this module: a caller supplies the BERT features, as the exported graph's `bert` feed does."""
 import numpy as np
 
 from . import config as _config
@@ -13,20 +13,30 @@ class StableTTS:
     """A MatchaTTS (StableTTS) checkpoint on one GPU: text-to-mel when it carries the text encoder, else the flow-matching
     decoder alone."""
 
-    def __init__(self, config, checkpoint, device=0, precision=1):
+    def __init__(self, config, checkpoint, device=0, precision=1, vocoder=None, vocoder_config=None):
         """config: overrides of config.STABLETTS_CFM / STABLETTS_TEXT (n_vocab, n_spks, spk_emb_dim, ...) or None; checkpoint: a
         path (Lightning's `state_dict` entry is taken when present) or a state dict.  A state dict without encoder.* serves
-        refine() only."""
+        refine() only.  vocoder: a HiFi-GAN checkpoint path (weights.load_hifigan) or its folded `generator` state dict, or None;
+        vocoder_config: the reference's config-dict keys (config.hifigan_config; None: v1)."""
         from .engine import Engine
         sd = _weights.load_checkpoint(checkpoint) if isinstance(checkpoint, str) else checkpoint
         sd = sd.get("state_dict", sd)
         self.has_text = "encoder.emb.weight" in sd
+        voc = None
+        if vocoder is not None:
+            vsd = _weights.load_hifigan(vocoder) if isinstance(vocoder, str) else _weights.fold_weight_norm(vocoder)
+            voc = (vsd, _config.hifigan_config(vocoder_config))
         if self.has_text:
             self.cfg = _config.stabletts_config(dict({"n_vocab": int(sd["encoder.emb.weight"].shape[0])}, **(config or {})))
-            blob, man = _weights.pack_stabletts(sd, self.cfg)
+            blob, man = _weights.pack_stabletts(sd, self.cfg, vocoder=voc)
         else:
             self.cfg = _config.stabletts_cfm_config(config)
-            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg)
+            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg, vocoder=voc)
+        if voc is not None:
+            if int(voc[1]["num_mels"]) != int(self.cfg["noise_channels"]):
+                raise ValueError("the vocoder reads %d mel channels, the model makes %d" % (int(voc[1]["num_mels"]), int(self.cfg["noise_channels"])))
+            self.cfg["vocoder"] = voc[1]
+        self.hop = _config.hop_samples(voc[1]) if voc is not None else None
         self.mel_mean, self.mel_std = np.float32(sd["mel_mean"]), np.float32(sd["mel_std"])
         self.engine = Engine(self.cfg, blob, man, device=device, precision=precision)
 
@@ -38,12 +48,13 @@ class StableTTS:
         return {"temperature": float(scales[0]), "length_scale": float(scales[1])}
 
     def synthesise(self, x, bert, sid, phone_duration_extra=None, n_timesteps=10, temperature=1.0, length_scale=1.0,
-                   guidance_scale=0.5, noise=None, seed=0, return_prior=False):
+                   guidance_scale=0.5, noise=None, seed=0, return_prior=False, return_wav=False):
         """x: the ids [n_streams, T] of one utterance, or a list of them; bert [bert_dim, T] and phone_duration_extra [T] (or
         None) alike; sid: a speaker id for all, or one per utterance; noise: [noise_channels, >= ceil4(frames)] per utterance
         standing in for torch.randn over the padded frame axis, or None for the engine's Philox(seed).  Returns the
         reference's names: mel and decoder_outputs [noise_channels, frames] (denormalised and as the model produces them),
-        mel_lengths, durations [T] (w_round), and with return_prior encoder_outputs / mel_enc; each a list for a list."""
+        mel_lengths, durations [T] (w_round), with return_prior encoder_outputs / mel_enc, and with return_wav the vocoder's
+        wav [hop * frames] (vocoder(mel).clamp(-1, 1), run on the device behind the mel) and wav_lengths; each a list for a list."""
         single = not isinstance(x, (list, tuple))
         xs = [np.asarray(u, np.int64) for u in ([x] if single else x)]
         berts = [np.asarray(u, np.float32) for u in ([bert] if single else bert)]
@@ -63,7 +74,7 @@ class StableTTS:
             nz = [np.ascontiguousarray(np.asarray(n, np.float32).T) for n in ([noise] if single else list(noise))]
         r = self.engine.stabletts_synthesise(ids, feats, sid, lengths=[u.shape[1] for u in xs], pause=pause, n_timesteps=n_timesteps,
                                              temperature=temperature, length_scale=length_scale, guidance_scale=guidance_scale,
-                                             noise=nz, seed=seed, want_prior=return_prior)
+                                             noise=nz, seed=seed, want_prior=return_prior, want_wav=return_wav)
         den = lambda a: a * self.mel_std + self.mel_mean          # denormalize (matcha/utils/model.py), fp32 like the reference
         cut = lambda a: [np.ascontiguousarray(a[b, :int(r["mel_lengths"][b])].T) for b in range(B)]
         out = {"decoder_outputs": cut(r["mel"]), "mel_lengths": [int(v) for v in r["mel_lengths"]],
@@ -72,7 +83,19 @@ class StableTTS:
         if return_prior:
             out["encoder_outputs"] = cut(r["prior"])
             out["mel_enc"] = [den(m) for m in out["encoder_outputs"]]
+        if return_wav:
+            out["wav_lengths"] = [int(v) for v in r["wav_lengths"]]
+            out["wav"] = [r["wav"][b, :out["wav_lengths"][b]].copy() for b in range(B)]
         return {k: v[0] for k, v in out.items()} if single else out
+
+    def vocode(self, mel):
+        """mel: the denormalised mel [num_mels, T] of one utterance (synthesise's `mel`), or a list of them.  Returns the
+        waveform [hop * T] of each (a list for a list): vocoder(mel).clamp(-1, 1)."""
+        single = not isinstance(mel, (list, tuple))
+        rows = [np.ascontiguousarray(np.asarray(m, np.float32).T) for m in ([mel] if single else list(mel))]
+        wav, wl = self.engine.hifigan_vocode(rows)
+        out = [wav[b, :int(wl[b])].copy() for b in range(len(rows))]
+        return out[0] if single else out
 
     def refine(self, mu_y, sid, n_timesteps=10, temperature=1.0, guidance_scale=0.5, noise=None, seed=0, denormalise=False):
         """mu_y: the aligned encoder output [cond_channels, T] of one utterance, or a list of them; sid: a speaker id for all, or

@@ -382,3 +382,30 @@ def make_random_stabletts(cfg, seed=1234):
                                ("dur_spk_emb.weight", (int(cfg["n_spks"]), G), 1.0)):
         sd[name] = (torch.randn(shape, generator=_gen(name, seed)) * scale).float().contiguous()
     return sd
+
+
+def make_random_hifigan(seed=1234, h=None, gain=None):
+    """A HiFi-GAN Generator checkpoint's `generator` state dict (matcha/hifigan/models.py:148-206, weight-normed convs as
+    weight_g / weight_v pairs, which weights.load_hifigan folds), CPU fp32, deterministic for (h, seed); h: config.hifigan_config
+    (None: v1).  The reference's init_weights (N(0, 0.01)) leaves a random mel's waveform near |wav| 0.06; the weights here are
+    drawn at GAIN / sqrt(fan-in) instead, so that a mel of the scale synthesise produces reaches |wav| of about 0.3-0.9 without
+    saturating tanh, and an absolute tolerance on it means something."""
+    from . import config as _config
+    h = _config.hifigan_config(h)
+    gain = dict(HIFIGAN_GAIN, **(gain or {}))
+    spec = []
+    c0, ch = int(h["upsample_initial_channel"]), int(h["upsample_initial_channel"])
+    _conv(spec, "conv_pre", c0, int(h["num_mels"]), 7, wn=True, gain=gain["pre"])
+    for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
+        _conv(spec, "ups.%d" % i, ch // 2, ch, k, wn=True, gain=gain["up"] * math.sqrt(u), transposed=True)
+        ch //= 2
+        for j, (ks, dils) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
+            n = i * len(h["resblock_kernel_sizes"]) + j
+            for d in range(len(dils)):
+                for m in ((1, 2) if h["resblock"] == "1" else ("",)):
+                    _conv(spec, "resblocks.%d.convs%s.%d" % (n, m, d), ch, ch, ks, wn=True, gain=gain["rb"])
+    _conv(spec, "conv_post", 1, ch, 7, wn=True, gain=gain["post"])
+    return _draw(spec, seed)
+
+
+HIFIGAN_GAIN = {"pre": 0.25, "up": 1.0, "rb": 0.5, "post": 0.05}   # v1 on a mel of -5.5 + 2.1 N(0, 1): max |wav| 0.67, mean 0.18

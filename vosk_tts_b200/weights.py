@@ -727,23 +727,74 @@ def _pack_stabletts_decoder(P, sd, cfg):
         P.conv("st.lsc%d" % j, want(e + "lsc_layers.%d.weight" % j, (H, 2 * H, k)), g(e + "lsc_layers.%d.bias" % j))
 
 
-def pack_stabletts_cfm(sd, cfg):
+def load_hifigan(path):
+    """A HiFi-GAN checkpoint of StableTTS's vocoder (cli.py:65-71: `{"generator": state_dict}`, generator_v1 / hifigan_T2_v1)
+    -> its state dict with the weight norm folded, as remove_weight_norm leaves it.  Read with weights_only=True."""
+    ck = torch.load(path, map_location="cpu", weights_only=True)
+    return fold_weight_norm(ck["generator"] if isinstance(ck, dict) and "generator" in ck else ck)
+
+
+def _pack_hifigan(P, sd, h):
+    """The Generator (matcha/hifigan/models.py:148-206) of a folded state dict under the decoder names csrc/engine.cu binds:
+    dec.pre, dec.up<i>.p<r> (the polyphase phases of each ConvTranspose1d), dec.rb<n>.c1/c2.<d> (ResBlock1) or .c.<d>
+    (ResBlock2) and dec.post.  Every conv is packed for the FFMA pipe; those whose input width is a multiple of 64 also as
+    split-bf16 planes, which precision modes >= 1 read."""
+    g, want = _sd_getter(sd)
+    c0, nm = int(h["upsample_initial_channel"]), int(h["num_mels"])
+    tc = lambda ci: ci % 64 == 0
+
+    def conv(dst, w, b):
+        P.conv(dst, w, b)
+        if tc(w.shape[1]):
+            P.conv_tc(dst, w)
+    P.conv("dec.pre", want("conv_pre.weight", (c0, nm, 7)), g("conv_pre.bias"))
+    ch = c0
+    nk = len(h["resblock_kernel_sizes"])
+    for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
+        wt = want("ups.%d.weight" % i, (ch, ch // 2, k))               # ConvTranspose1d: [Cin, Cout, K]
+        for r, (pad, js) in enumerate(convt_phases(u, k, (k - u) // 2)):
+            conv("dec.up%d.p%d" % (i, r), np.transpose(np.stack([wt[:, :, j] for j in js], axis=-1), (1, 0, 2)), g("ups.%d.bias" % i))
+        ch //= 2
+        for j, (ks, dils) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
+            n = i * nk + j
+            for d in range(len(dils)):
+                if h["resblock"] == "1":
+                    for m in (1, 2):
+                        src = "resblocks.%d.convs%d.%d." % (n, m, d)
+                        conv("dec.rb%d.c%d.%d" % (n, m, d), want(src + "weight", (ch, ch, ks)), g(src + "bias"))
+                else:
+                    src = "resblocks.%d.convs.%d." % (n, d)
+                    P.conv("dec.rb%d.c.%d" % (n, d), want(src + "weight", (ch, ch, ks)), g(src + "bias"))
+    P.conv("dec.post", want("conv_post.weight", (1, ch, 7)), g("conv_post.bias"))
+
+
+def pack_hifigan(sd, h):
+    """The vocoder alone -> (blob, manifest) (see _pack_hifigan); h: config.hifigan_config."""
+    P = _Packer()
+    _pack_hifigan(P, sd, h)
+    return P.finish()
+
+
+def pack_stabletts_cfm(sd, cfg, vocoder=None):
     """The flow-matching decoder of a MatchaTTS (StableTTS) state dict -> (blob, manifest) of a model_family "stabletts" engine.
     sd: the checkpoint's `state_dict` entry (keys decoder.estimator.*, spk_emb.weight, fake_speaker, fake_content, mel_mean,
     mel_std); cfg: config.stabletts_cfm_config.  Convs go in the FFMA layout (q, k, v stacked into one 1x1 conv), the small
     linears of the conditioning path (time_mlp, each block's film conv and adaLN_modulation) row-major [out][in] and stacked
     over the blocks.  Everything is fp32: the decoder runs on the FFMA pipe in every precision mode, so there are no
-    mode-dependent split planes to add yet."""
+    mode-dependent split planes to add yet.  vocoder: (folded Generator state dict, config.hifigan_config) appended as
+    pack_hifigan lays it out, or None."""
     P = _Packer()
     _pack_stabletts_decoder(P, sd, cfg)
+    if vocoder is not None:
+        _pack_hifigan(P, *vocoder)
     return P.finish()
 
 
-def pack_stabletts(sd, cfg):
+def pack_stabletts(sd, cfg, vocoder=None):
     """A MatchaTTS (StableTTS) state dict without its vocoder -> (blob, manifest) of an engine that serves text-to-mel
     (vtts_stabletts_synthesise) and the decoder alone: the decoder part of pack_stabletts_cfm, then the text encoder
     (encoder.emb, encoder.punc_emb, encoder.bert_proj.1, both stacks encoder.encoder / encoder.dp_encoder with their proj) and
-    dur_spk_emb.  cfg: config.stabletts_config."""
+    dur_spk_emb.  cfg: config.stabletts_config; vocoder as in pack_stabletts_cfm."""
     if "enc_n_layers" not in cfg:
         raise ValueError("pack_stabletts needs config.stabletts_config (the text encoder's constants), not stabletts_cfm_config")
     g, want = _sd_getter(sd)
@@ -767,4 +818,6 @@ def pack_stabletts(sd, cfg):
         P.add(dst + ".ada.w2", np.stack([want(b % l + "adaLN_modulation.2.weight", (6 * H, H)) for l in range(NE)]))
         P.add(dst + ".ada.b2", np.stack([g(b % l + "adaLN_modulation.2.bias") for l in range(NE)]))
         P.conv(dst + ".proj", want(src + "proj.weight", (co, H, 1)), g(src + "proj.bias"))
+    if vocoder is not None:
+        _pack_hifigan(P, *vocoder)
     return P.finish()
