@@ -116,6 +116,98 @@ struct RbW {
   std::vector<TcW> t1, t2;
 };
 
+// Launch tuning of the conv and attention kernels.  The engine holds the defaults (from_env); a path that must not depend on
+// the batch launches with one of the named fixed shapes below, a copy of the defaults.  Fields are set here and nowhere else.
+struct Tuning {
+  // FFMA convs (launch_conv): split-K cluster cap, tile target of the split, thread groups per CTA (cap; machine-filling
+  // launches; single utterances; k-steps per rank needed to add one, 0 never)
+  int conv_max_s = 8, conv_target = 120, conv_max_g = 4, conv_big_g = 1, conv_min_g = 1, conv_auto_g = 4;
+  // tensor-core convs (launch_tc)
+  int tc_tall = 0, tc_baseoff = 0, tc_dbgskip = 0, tc_bn = 0, tc_mc = 0, tc_split = 0, tc_min_steps = 2, tc_persist = 1,
+      tc_persist_min = 1, tc_wmc = 0;
+  // attention: query rows per warp (0 auto), the split-KV kernel allowed, wgmma attention where the qkv conv runs on tensor
+  // cores (0 never, 1 when throughput bound, 2 always)
+  int attn_rows = 0, attn_split = 1, attn_tc_mode = 1;
+
+  static Tuning from_env() {
+    Tuning t;
+    if (const char* e = getenv("VTTS_CONV_MAXS")) t.conv_max_s = std::max(1, atoi(e));
+    if (const char* e = getenv("VTTS_CONV_TARGET")) t.conv_target = std::max(1, atoi(e));
+    if (const char* e = getenv("VTTS_CONV_MAXG")) t.conv_max_g = std::max(1, std::min(4, atoi(e)));
+    if (const char* e = getenv("VTTS_CONV_BIGG")) t.conv_big_g = std::max(1, std::min(4, atoi(e)));   // thread groups per CTA on machine-filling FFMA launches
+    if (const char* e = getenv("VTTS_TC_TALL")) t.tc_tall = atoi(e);
+    if (const char* e = getenv("VTTS_TC_BASEOFF")) t.tc_baseoff = atoi(e);
+    if (const char* e = getenv("VTTS_TC_BN")) t.tc_bn = atoi(e);
+    if (const char* e = getenv("VTTS_TC_MULTICAST")) t.tc_mc = atoi(e);
+    if (const char* e = getenv("VTTS_TC_SPLIT")) t.tc_split = atoi(e);
+    if (const char* e = getenv("VTTS_TC_MINSTEPS")) t.tc_min_steps = std::max(1, atoi(e));   // k-steps per CTA below which split-K stops
+    if (const char* e = getenv("VTTS_TC_PERSIST")) t.tc_persist = atoi(e);                 // 0: one tile per CTA also on machine-filling launches; 2: persistent grid on every launch without split-K (tests)
+    if (const char* e = getenv("VTTS_TC_DBGSKIP")) t.tc_dbgskip = atoi(e);                 // timing experiments only (wrong results)
+    if (const char* e = getenv("VTTS_TC_WMC")) t.tc_wmc = atoi(e);                         // 1: weight-tile multicast between CTA pairs of persistent launches (measured neutral, off)
+    if (const char* e = getenv("VTTS_TC_PERSIST_MIN")) t.tc_persist_min = std::max(1, atoi(e));   // tiles per SM from which the persistent grid is used
+    if (const char* e = getenv("VTTS_ATTN_SPLIT")) t.attn_split = atoi(e);       // 0: never use the split-KV attention
+    if (const char* e = getenv("VTTS_CONV_AUTOG")) t.conv_auto_g = std::max(0, atoi(e));   // k-steps per rank needed to add thread groups; 0 = never
+    if (const char* e = getenv("VTTS_CONV_MING")) t.conv_min_g = std::max(1, std::min(4, atoi(e)));      // 0 auto, 1 off, 2/4/8 cap
+    if (const char* e = getenv("VTTS_ATTN_ROWS")) t.attn_rows = atoi(e);
+    if (const char* e = getenv("VTTS_ATTN_TC")) t.attn_tc_mode = atoi(e);
+    return t;
+  }
+  // One FFMA conv launch shape whatever the rows (no split-K over a cluster, one thread group): every output is summed in the
+  // same order, so a sequence's result does not depend on what it is batched with.  The vocoder in precision mode 0, the
+  // QuickVC speaker encoder and both StableTTS phases.
+  Tuning fixed_ffma() const {
+    Tuning t = *this;
+    t.conv_max_s = 1; t.conv_min_g = 1; t.conv_big_g = 1; t.conv_auto_g = 0;
+    return t;
+  }
+  // One attention kernel whatever the rows: the register-blocked FFMA kernel (StableTTS).
+  Tuning fixed_attention() const {
+    Tuning t = *this;
+    t.attn_rows = 4;
+    return t;
+  }
+  // Tensor-core convs without split-K (every output summed by one CTA in one k order, whatever the launch shape) and attention
+  // on attn_tc_kernel whenever it takes the layer, unless switched off (ContentVec in precision modes >= 1).
+  Tuning fixed_tc() const {
+    Tuning t = *this;
+    t.tc_split = 1;
+    if (t.attn_tc_mode > 0) t.attn_tc_mode = 2;
+    return t;
+  }
+  // vtts_debug_conv's overrides (VTTS_CONV_KEEP: this value)
+  Tuning with(const vtts_conv_overrides& ov) const {
+    Tuning t = *this;
+    auto set = [](int& f, int v) { if (v != VTTS_CONV_KEEP) f = v; };
+    set(t.tc_bn, ov.tc_bn); set(t.tc_split, ov.tc_split); set(t.tc_tall, ov.tc_tall); set(t.tc_mc, ov.tc_mc);
+    set(t.tc_persist, ov.tc_persist); set(t.tc_wmc, ov.tc_wmc); set(t.tc_min_steps, ov.tc_min_steps); set(t.conv_max_s, ov.conv_max_s);
+    set(t.conv_min_g, ov.conv_min_g); set(t.conv_max_g, ov.conv_max_g); set(t.conv_big_g, ov.conv_big_g);
+    return t;
+  }
+  // vtts_debug_attention's kernel selection (VTTS_ATTN_*)
+  Tuning with_attention(int kernel) const {
+    Tuning t = *this;
+    switch (kernel) {
+      case VTTS_ATTN_TC: t.attn_tc_mode = 2; break;
+      case VTTS_ATTN_SPLIT: t.attn_split = 1; t.attn_rows = 1; break;
+      case VTTS_ATTN_R1: t.attn_split = 0; t.attn_rows = 1; break;
+      case VTTS_ATTN_R4: t.attn_split = 0; t.attn_rows = 4; break;
+      default: break;                               // AUTO / FFMA: the engine's choice
+    }
+    return t;
+  }
+};
+
+// The rows a launch runs over: n sequences of at most maxLen rows at the device lengths / offsets the kernels read, the host
+// lengths the launch heuristics size for (`sized`: functions of the length buckets only, so that a graph captured for a
+// bucket is valid for every call that maps to it), the true host lengths the profiler counts FLOPs with (`real`), and the
+// tuning the launches run with.
+struct Rows {
+  const int *lens, *offs;
+  int n, maxLen;
+  std::vector<int> sized, real;
+  Tuning tune;
+};
+
 struct Err {
   int code;
   std::string msg;
@@ -278,6 +370,9 @@ struct vtts_engine {
     virtual_lens(v_frm_len, B, Tfrm, maxFrm);
     if (!use_buckets) v_frm_len = h_frm_len;
   }
+  // the rows of the current call shape, at the engine's tuning
+  Rows tok_rows() const { return Rows{d_tok_len.p, d_tok_off.p, B, maxTok, v_tok_len, h_tok_len, tune}; }
+  Rows frm_rows() const { return Rows{d_frm_len.p, d_frm_off.p, B, maxFrm, v_frm_len, h_frm_len, tune}; }
   // plane buffers whose rows behind each utterance must be zeroed for this phase (see zero_tails_kernel)
   TailList tail;
   bool collecting = false;
@@ -323,7 +418,8 @@ struct vtts_engine {
   uint64_t ws_gen = 0, graph_clock = 0, graph_replays = 0;
   bool capture_on_first = true;
   bool capturing = false, use_graphs = true, last_graphed = false, use_pdl = true;    // programmatic dependent launch (VTTS_PDL=0 turns it off)
-  int conv_max_s = 8, conv_target = 120, conv_max_g = 4, conv_big_g = 1, tc_tall = 0, tc_baseoff = 0, tc_bn = 0, attn_rows = 0, tc_mc = 0, tc_split = 0, conv_min_g = 1, tc_min_steps = 2, conv_auto_g = 4, attn_split = 1, tc_persist = 1, tc_persist_min = 1, n_sm = 132, tc_dbgskip = 0, tc_wmc = 0;
+  Tuning tune;                             // the launch tuning of every path without a fixed launch shape
+  int n_sm = 132;
   // shape of the last dense conv launch (vtts_debug_conv) and, while log_conv is set, of every one (vtts_debug_conv_log)
   vtts_conv_report last_conv{};
   vtts_attn_report last_attn{};               // the last attention launch (vtts_debug_attention)
@@ -333,8 +429,7 @@ struct vtts_engine {
     last_conv = r;
     if (log_conv) conv_log.push_back(r);
   }
-  int tc_cluster_cap[2][3] = {{0, 0, 0}, {0, 0, 0}};   // co-resident clusters of 2/4/8 conv_tc CTAs, [BN 64/128][log2(S)-1]   // multicast measured slower (see DESIGN.md 4.2)   // tuning knobs (env VTTS_CONV_MAXS / _TARGET / _MAXG)
-  int attn_tc_mode = 1;                    // wgmma attention where the qkv conv runs on tensor cores: 0 never, 1 when throughput bound, 2 always
+  int tc_cluster_cap[2][3] = {{0, 0, 0}, {0, 0, 0}};   // co-resident clusters of 2/4/8 conv_tc CTAs, [BN 64/128][log2(S)-1]   // multicast measured slower (see DESIGN.md 4.2)
   int mrf_heavy_first = 1;
   int mrf_branch = 0;                      // VTTS_MRF_BRANCH=1: one stream per resblock chain (measured slower: 1.74 vs 1.62 ms)
   float stage_ms[8] = {};
@@ -529,29 +624,28 @@ struct vtts_engine {
     return p;
   }
   CUtensorMap make_map(const void* base, int C, long rows, int box_rows);
-  bool attn_tc_ok(const EncLayerW& L, int Hc) const;
-  bool attn_use_tc(const EncLayerW& L, int Hc, const int* lens, int maxLen) const;
-  bool attn_split_fits(const EncLayerW& L, int Hc, const int* lens, int maxLen) const;
-  void launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen);
-  void launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
+  bool attn_tc_ok(const EncLayerW& L, int Hc, const Tuning& t) const;
+  bool attn_use_tc(const EncLayerW& L, int Hc, const Rows& r) const;
+  bool attn_split_fits(const EncLayerW& L, int Hc, const Rows& r) const;
+  void launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const EncLayerW& L, int Hc, const Rows& r);
+  void launch_tc(const std::vector<TcSpec>& ps, int rmul, const Rows& r);
   // plane buffers of the frame-resolution stages: allocated (and their tails zeroed by ONE zero_tails launch) before the
   // first kernel of the phase
   struct FlowPl { Planes ph, pao, ph1, pff, pwx, pacts, pskip, pqkv; } flp;
   struct DecPl { Planes pz, cur; std::vector<Planes> px, nxt; std::vector<std::vector<Planes>> pj, pt; } dcp;
   void alloc_flow_planes();
   void alloc_decoder_planes();
-  bool decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready);
-  void flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, const float* cond, int cond_ld, bool forward);
-  void launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen, Planes* pl);
+  bool decoder_tc(float* z, bool pz_ready, const Rows& r);
+  void flow_tc(float* z, bool emit_pz, const float* cond, int cond_ld, bool forward, const Rows& r);
+  void launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, Planes* pl, const Rows& r);
   void bind_weights();
   void bind_flow_decoder();
   void bind_decoder();
   void bind_wn_encoder(const std::string& p, int cin);
-  void launch_conv(const std::vector<ConvP>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB);
+  void launch_conv(const std::vector<ConvP>& ps, int rmul, const Rows& r);
   void encoder_layer(const EncLayerW& L, float*& x, float*& xb, float* qkv, float* ao, float* y, float* ffh, int Hc, int Fc,
-                     int ks, const int* lens, const int* offs, int maxLen, const float* vec_after, int vec_ld,
-                     const float* cadd_after);
-  void dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const int* lens, const int* offs, int maxLen,
+                     int ks, const float* vec_after, int vec_ld, const float* cadd_after, const Rows& r);
+  void dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const Rows& r,
                  const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
   struct P1Pin { int *len, *off, *sid, *ids; float *prm, *eps; };
   P1Pin p1_layout(bool eps);
@@ -581,7 +675,7 @@ struct vtts_engine {
     float* pin = reinterpret_cast<float*>(ensure(h_pin_z, (size_t)B * cfg.inter_channels * maxFrm * sizeof(float)));
     stage_noise(pin, noise_z, z_ld, std::vector<int>(B, std::min(z_ld, maxFrm)));
   }
-  void decode(float* z, const int* fl, const int* fo, bool planes_ready = false, bool pz_ready = false);
+  void decode(float* z, const Rows& r, bool planes_ready = false, bool pz_ready = false);
   bool have_latent = false;
   Buf<int> d_chunk;                              // [len, off, off_end] of the chunk being decoded
 
@@ -589,12 +683,12 @@ struct vtts_engine {
   // cores, its planes px) is updated in place, `skip` receives the summed skip halves (planes pskip from the last layer);
   // layer i adds the cond rows cond + i*2H (row stride cond_ld) before the gate, none when cond is null.
   void wn_ffma(const std::vector<ConvW>& in, const std::vector<ConvW>& rsx, const std::vector<ConvW>& rss, int nl, int fk,
-               int dil_rate, float* x, float* acts, float* skip, const float* cond, int cond_ld, const int* fl, const int* fo);
+               int dil_rate, float* x, float* acts, float* skip, const float* cond, int cond_ld, const Rows& r);
   void wn_tc(const std::vector<TcW>& t_in, const std::vector<ConvW>& in, const std::vector<TcW>& t_rsx, const std::vector<ConvW>& rsx,
              const std::vector<TcW>& t_rss, const std::vector<ConvW>& rss, int nl, int fk, int dil_rate, float* x, float* skip, const Planes& px,
-             const Planes& pacts, const Planes& pskip, const float* cond, int cond_ld, const int* fl, const int* fo);
+             const Planes& pacts, const Planes& pskip, const float* cond, int cond_ld, const Rows& r);
   // The flow on the fp32 pipe; forward = models.py:750-753 (layers in order, x1 <- x1 + m), else the reverse of infer.
-  void flow_ffma(float* z, const int* fl, const int* fo, const float* cond, int cond_ld, bool forward);
+  void flow_ffma(float* z, const float* cond, int cond_ld, bool forward, const Rows& r);
 
   // ---- voice conversion (SynthesizerTrn.voice_conversion, models.py:1710-1718)
   bool has_encq = false, q_tc = false;
@@ -618,8 +712,8 @@ struct vtts_engine {
   float* vc_upload(ClipIn in, bool eps);
   float* cond_src(bool tgt);
   float* front_end(bool from_spec);
-  void posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld);
-  void posterior_side(bool from_spec, const float* noise, const float* csrc);
+  void posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld, const Rows& r);
+  void posterior_side(bool from_spec, const float* noise, const float* csrc, const Rows& r);
   void convert_enqueue(bool from_spec, bool eps);
 
   // ---- QuickVC speaker encoder (SpeakerEncoder.embed_utterance, vc/models.py:728-767; spk.cuh)
@@ -655,18 +749,6 @@ struct vtts_engine {
   void bind_contentvec();
   std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
   void cv_enqueue(float* out, const int* out_offs);
-  // Restores, on scope exit, the host-side frame lengths and the launch knobs an enqueue overrides for its own launches.
-  struct SavedLaunch {
-    vtts_engine* e;
-    std::vector<int> vf, hf;
-    int split, atc, ms, ming, bigg, autog;
-    explicit SavedLaunch(vtts_engine* h) : e(h), vf(h->v_frm_len), hf(h->h_frm_len), split(h->tc_split), atc(h->attn_tc_mode),
-                                           ms(h->conv_max_s), ming(h->conv_min_g), bigg(h->conv_big_g), autog(h->conv_auto_g) {}
-    ~SavedLaunch() {
-      e->v_frm_len = vf; e->h_frm_len = hf; e->tc_split = split; e->attn_tc_mode = atc;
-      e->conv_max_s = ms; e->conv_min_g = ming; e->conv_big_g = bigg; e->conv_auto_g = autog;
-    }
-  };
 
   // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh), fp32 FFMA in every mode
   ConvW st_cp[3], st_in, st_final;                 // cond_proj's three convs, in_proj over (x | cond), final_proj
@@ -689,15 +771,15 @@ struct vtts_engine {
   void bind_stabletts();
   void st_enqueue();
   // One DiTConVBlock over a ragged batch (diffusion_transformer.py:98-116), shared by the decoder's blocks and the text
-  // encoder's: the rows, the conditioning and the work buffers of the caller
+  // encoder's: the conditioning and the work buffers of the caller, over the rows r
   struct StBlk {
-    int H, F, heads, rd, maxLen, NS, ald;          // widths, rotary features, grid bound, sequences, pitch of a sequence's adaLN rows
-    const int *lens, *offs;
+    int H, F, heads, rd, ald;                      // widths, rotary features, pitch of a sequence's adaLN rows
     const float2* rope;
     const float* ada;                              // [sequences][ald]
     float *Hb, *N, *QKV, *AO, *Y, *FF;
   };
-  void st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap);
+  void st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap,
+                const Rows& r);
 
   // ---- StableTTS text encoder and durations (TextEncoder.forward, MatchaTTS.synthesise; stabletts.cuh): blobs of
   // weights.pack_stabletts.  Stack 0 is the mel encoder (conditioned on spk_emb), stack 1 dp_encoder (on dur_spk_emb).
@@ -1004,12 +1086,12 @@ void vtts_engine::bind_decoder() {
 }
 
 // The vocoder of a StableTTS engine over mel rows [rows][st_noise] (utterance b: fl[b] rows from fo[b]) -> d_wav, sample
-// offset fo[b] * hop.  The FFMA convs run in one fixed launch shape (no split-K, one thread group), so that in precision mode
-// 0 an utterance's waveform does not depend on what it is batched with.
+// offset fo[b] * hop.  The FFMA convs run in one fixed launch shape (Tuning::fixed_ffma), so that in precision mode 0 an
+// utterance's waveform does not depend on what it is batched with.
 void vtts_engine::voc_enqueue(const float* mel, const int* fl, const int* fo) {
-  SavedLaunch saved(this);
-  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
-  decode(const_cast<float*>(mel), fl, fo);
+  Rows r = frm_rows();
+  r.lens = fl; r.offs = fo; r.tune = tune.fixed_ffma();
+  decode(const_cast<float*>(mel), r);
 }
 
 CUtensorMap vtts_engine::make_map(const void* base, int C, long rows, int box_rows) {
@@ -1104,12 +1186,14 @@ static TcSplitPlan tc_split_plan(const TcSplitIn& in) {
 }
 
 // Grouped tensor-core conv launch (conv_tc.cuh).  One CTA = 128 rows x 64 output channels of one problem.
-void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB) {
+void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const Rows& r) {
+  const Tuning& t = r.tune;
+  const int nB = r.n, maxLen = r.maxLen;
+  const std::vector<int>& hl = r.sized;
   // 128-wide channel tiles halve the activation traffic and run the MMA at its smem-operand optimum, but halve the CTA
   // count: used once the launch still fills the machine (batched calls), or when forced (VTTS_TC_BN).
   int BN = 64;
   {
-    const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
     long ctas128 = 0;
     bool wide = true;
     for (const TcSpec& q : ps) {
@@ -1117,7 +1201,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
       for (int b = 0; b < nB; ++b) ctas128 += (long)((hl[b] * rmul + q.in_extra + TC_BM - 1) / TC_BM) * ((q.Cout + 127) / 128);
     }
     if (wide && ctas128 >= 2 * n_sm) BN = 128;
-    if (tc_bn == 64 || tc_bn == 128) BN = tc_bn;
+    if (t.tc_bn == 64 || t.tc_bn == 128) BN = t.tc_bn;
   }
   REQUIRE(!ps.empty() && (int)ps.size() <= TC_MAXP, VTTS_ERR_INVALID, "bad grouped tensor-core conv");
   TcBatch& tb = tc_batch;   // per-engine scratch (2.6 KB: kept off the stack frame of every caller)
@@ -1131,13 +1215,12 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   int psplit[TC_MAXP] = {1, 1, 1, 1};
   int gx = 0;                                // row tiles of the grid
   for (const TcSpec& q : ps) gx = std::max(gx, (maxLen * rmul + q.in_extra + TC_BM - 1) / TC_BM);
-  if (tc_tall <= 0 && tc_split != 1 && (tc_bn == 64 || tc_bn == 128 || BN == 64)) {
-    const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
+  if (t.tc_tall <= 0 && t.tc_split != 1 && (t.tc_bn == 64 || t.tc_bn == 128 || BN == 64)) {
     TcSplitIn in;
     in.n = (int)ps.size(); in.nb = nB; in.gx = gx;
-    in.bn = (tc_bn == 64 || tc_bn == 128) ? tc_bn : 0;
-    in.max_split = tc_split > 1 ? tc_split : 8;
-    in.min_steps = tc_min_steps;
+    in.bn = (t.tc_bn == 64 || t.tc_bn == 128) ? t.tc_bn : 0;
+    in.max_split = t.tc_split > 1 ? t.tc_split : 8;
+    in.min_steps = t.tc_min_steps;
     in.n_sm = n_sm;
     memcpy(in.cluster_cap, tc_cluster_cap, sizeof(in.cluster_cap));
     in.lens = hl.data(); in.rmul = rmul;
@@ -1164,8 +1247,8 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     if (q.w.mid && q.in.mid) np3 = true;
     grid_tiles += (long)((maxLen * rmul + q.in_extra + TC_BM - 1) / TC_BM) * ((q.Cout + BN - 1) / BN) * nB;
   }
-  const bool big = tc_persist == 2 || (tc_persist && grid_tiles > (long)tc_persist_min * n_sm);   // (2: forced, for tests)
-  bool tall = split == 1 && (tc_tall > 0 || (tc_tall == 0 && big));
+  const bool big = t.tc_persist == 2 || (t.tc_persist && grid_tiles > (long)t.tc_persist_min * n_sm);   // (2: forced, for tests)
+  bool tall = split == 1 && (t.tc_tall > 0 || (t.tc_tall == 0 && big));
   for (const TcSpec& q : ps) {
     const int nr = TC_BM + (q.k - 1) * q.dil;
     if (nr > 192) tall = false;              // shared-memory budget of the activation ring (and TMA box <= 256)
@@ -1181,7 +1264,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   // TMA multicast of the activation tile across the channel-tile CTAs of a cluster: only when every problem of the
   // launch has the same number of channel tiles (no CTA of a cluster may drop out) and the tile is not "tall"
   int cn = 1;
-  if (tc_mc && !tall) {
+  if (t.tc_mc && !tall) {
     int ny = -1;
     bool same = true;
     for (const TcSpec& q : ps) {
@@ -1189,7 +1272,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
       if (ny < 0) ny = n; else if (n != ny) same = false;
     }
     if (same) cn = (ny % 4 == 0) ? 4 : (ny % 2 == 0 ? 2 : 1);
-    if (tc_mc == 2 && same && ny % 2 == 0) cn = 2;          // VTTS_TC_MULTICAST=2: pairs only
+    if (t.tc_mc == 2 && same && ny % 2 == 0) cn = 2;          // VTTS_TC_MULTICAST=2: pairs only
   }
   if (split > 1) cn = 1;
   int np = 0;
@@ -1215,15 +1298,15 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     for (const TcSpec& q : ps) mc = std::max(mc, q.Cout);
     tiles_all = (long)gx * ((mc + BN - 1) / BN) * nB * (long)ps.size() * split;
   }
-  const bool one_wave = tiles_all <= n_sm && !(tc_persist == 2 && split == 1 && cn == 1);
+  const bool one_wave = tiles_all <= n_sm && !(t.tc_persist == 2 && split == 1 && cn == 1);
   tb.wst = np == 3 ? (BN == 128 ? 2 : 3) : (BN == 128 ? tc_wst<128>() : tc_wst<64>());
   tb.split = split;
   tb.cn = cn;
   tb.tall = tall ? 1 : 0;
   // persistent launches: CTA pairs share every weight tile through TMA multicast (conv_tc.cuh)
-  const int wmc = (big && tc_wmc && split == 1 && cn == 1 && np == 2 && n_sm % 2 == 0) ? 2 : 1;
-  tb.baseoff = tc_baseoff;
-  tb.dbgskip = tc_dbgskip;
+  const int wmc = (big && t.tc_wmc && split == 1 && cn == 1 && np == 2 && n_sm % 2 == 0) ? 2 : 1;
+  tb.baseoff = t.tc_baseoff;
+  tb.dbgskip = t.tc_dbgskip;
   tb.a_bytes = (maxNR * 128 + 1023) / 1024 * 1024;
   for (size_t i = 0; i < ps.size(); ++i) {
     const TcSpec& q = ps[i];
@@ -1264,7 +1347,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   if (mixed) grid = dim3(1, 1, (unsigned)tiles_all);
   tb.persist = 0;
   tb.wmc = 1;
-  if (split == 1 && cn == 1 && !tb.wpre && (tc_persist == 2 || (tc_persist && (long)grid.x * grid.y * grid.z > (long)tc_persist_min * n_sm))) {
+  if (split == 1 && cn == 1 && !tb.wpre && (t.tc_persist == 2 || (t.tc_persist && (long)grid.x * grid.y * grid.z > (long)t.tc_persist_min * n_sm))) {
     tb.persist = 1;
     tb.wmc = wmc;
     grid = dim3((unsigned)n_sm, 1, 1);
@@ -1273,12 +1356,12 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
   const bool single_wave_image = split > 1 || tb.wpre;
   const bool dyn_image = tb.np != 2 || tb.ast != (BN == 128 ? tc_ast<128>() : tc_ast<64>()) || tb.wst != (BN == 128 ? tc_wst<128>() : tc_wst<64>());
   {
-    vtts_conv_report r{};
-    r.use_tc = 1; r.bn = BN; r.split = split; r.tall = tb.tall; r.cn = cn; r.wmc = tb.wmc; r.persist = tb.persist; r.np = tb.np;
-    r.ast = tb.ast; r.wst = tb.wst; r.image = single_wave_image ? (dyn_image ? 1 : 0) : 2;
-    r.grid_x = (int)grid.x; r.grid_y = (int)grid.y; r.grid_z = (int)grid.z;
-    for (size_t p = 0; p < ps.size(); ++p) r.psplit[p] = psplit[p];
-    note_conv(r);
+    vtts_conv_report rep{};
+    rep.use_tc = 1; rep.bn = BN; rep.split = split; rep.tall = tb.tall; rep.cn = cn; rep.wmc = tb.wmc; rep.persist = tb.persist; rep.np = tb.np;
+    rep.ast = tb.ast; rep.wst = tb.wst; rep.image = single_wave_image ? (dyn_image ? 1 : 0) : 2;
+    rep.grid_x = (int)grid.x; rep.grid_y = (int)grid.y; rep.grid_z = (int)grid.z;
+    for (size_t p = 0; p < ps.size(); ++p) rep.psplit[p] = psplit[p];
+    note_conv(rep);
   }
   if (profiling) {
     if (tc_prof_used + 2 > tc_prof_ev.size()) {
@@ -1288,7 +1371,7 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     }
     for (const TcSpec& q : ps)
       for (int b = 0; b < nB; ++b)
-        tc_prof_flops += 2.0 * ((double)((lens == d_tok_len.p) ? h_tok_len[b] : h_frm_len[b]) * rmul + q.in_extra) * q.Cout * q.Cin * q.k;   // (true lengths)
+        tc_prof_flops += 2.0 * ((double)r.real[b] * rmul + q.in_extra) * q.Cout * q.Cin * q.k;   // (true lengths)
     ++tc_prof_launches;
     CK(cudaEventRecord(tc_prof_ev[tc_prof_used], stream));
   }
@@ -1315,18 +1398,18 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
     // images costs instruction-cache misses on every launch of a latency-bound chain
     if (single_wave_image) {
       if (dyn_image) {
-        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, true>, tb, lens, offs));
-        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, true>, tb, lens, offs));
+        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, true>, tb, r.lens, r.offs));
+        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, true>, tb, r.lens, r.offs));
       } else {                    // the default launches carry the descriptor without the third-plane tensor maps
         // (a one-slot descriptor for the single-conv launches was tried as well: alternating between two kernel images on the
         //  chain cost more than the 2 KB of parameters saved -- conv_tc 723 -> 765 us in-graph)
         const auto tl = tc_lite<TC_MAXP>(tb);
-        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, false, TC_MAXP>, tl, lens, offs));
-        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, false, TC_MAXP>, tl, lens, offs));
+        if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<128, false, TC_MAXP>, tl, r.lens, r.offs));
+        else CK(cudaLaunchKernelEx(&lc, conv_tc_kernel<64, false, TC_MAXP>, tl, r.lens, r.offs));
       }
     } else {                      // more than one wave of tiles: the persistent kernel (also runs them one per CTA when tb.persist == 0)
-      if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_persist_kernel<128>, tb, lens, offs));
-      else CK(cudaLaunchKernelEx(&lc, conv_tc_persist_kernel<64>, tb, lens, offs));
+      if (BN == 128) CK(cudaLaunchKernelEx(&lc, conv_tc_persist_kernel<128>, tb, r.lens, r.offs));
+      else CK(cudaLaunchKernelEx(&lc, conv_tc_persist_kernel<64>, tb, r.lens, r.offs));
     }
   }
   CK(cudaGetLastError());
@@ -1338,35 +1421,35 @@ void vtts_engine::launch_tc(const std::vector<TcSpec>& ps, int rmul, const int* 
 }
 
 // Attention on the tensor cores (attn_tc.cuh): q, k, v come as the split-bf16 planes the qkv conv's epilogue wrote.
-bool vtts_engine::attn_tc_ok(const EncLayerW& L, int Hc) const {
+bool vtts_engine::attn_tc_ok(const EncLayerW& L, int Hc, const Tuning& t) const {
   const int dk = Hc / L.heads;
-  return attn_tc_mode > 0 && L.rk_hi != nullptr && dk % 32 == 0 && dk <= 128 && 2 * cfg.window_size + 1 <= ATC_RS && (3 * Hc) % 8 == 0;
+  return t.attn_tc_mode > 0 && L.rk_hi != nullptr && dk % 32 == 0 && dk <= 128 && 2 * cfg.window_size + 1 <= ATC_RS && (3 * Hc) % 8 == 0;
 }
 // Which attention kernel for this launch?  The tensor-core kernel wins as soon as the launch is throughput bound (batches,
 // long utterances: 8.8x at 4765 frames, 2.8x on the flow of a 64-utterance batch).  A single short utterance is latency
 // bound -- a 128-row wgmma tile walks its 2-4 key tiles serially while the split-KV FFMA kernel spreads 4 query rows x 4
 // key segments over 16 warps of ~80 CTAs -- and keeps the FFMA kernel (measured at 162 frames: 6 vs 19 us per launch in the
 // graph).  VTTS_ATTN_TC = 0 never / 1 this rule / 2 always.
-bool vtts_engine::attn_use_tc(const EncLayerW& L, int Hc, const int* lens, int maxLen) const {
-  if (!attn_tc_ok(L, Hc)) return false;
-  if (attn_tc_mode >= 2) return true;
-  return !((attn_rows == 0 || attn_rows == 1) && attn_split_fits(L, Hc, lens, maxLen));
+bool vtts_engine::attn_use_tc(const EncLayerW& L, int Hc, const Rows& r) const {
+  const Tuning& t = r.tune;
+  if (!attn_tc_ok(L, Hc, t)) return false;
+  if (t.attn_tc_mode >= 2) return true;
+  return !((t.attn_rows == 0 || t.attn_rows == 1) && attn_split_fits(L, Hc, r));
 }
 
 // Can the split-KV FFMA kernel take this launch?  All key tiles of the longest utterance must be resident in shared memory
 // (at most ATS_MAXT tiles, and at most ATS_SMEM_MAX bytes: dk 128 at W 4 overflows from 7 tiles, i.e. 193 positions), and
 // the CTAs must fit one wave.
-bool vtts_engine::attn_split_fits(const EncLayerW& L, int Hc, const int* lens, int maxLen) const {
+bool vtts_engine::attn_split_fits(const EncLayerW& L, int Hc, const Rows& r) const {
   const int dk = Hc / L.heads, nrel = 2 * cfg.window_size + 1;
-  const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
   long ctas = 0;
-  for (int b = 0; b < B; ++b) ctas += (long)((hl[b] + ATS_ROWS - 1) / ATS_ROWS) * L.heads;
-  const int mt = (maxLen + AT_KT - 1) / AT_KT;
-  return attn_split && mt <= ATS_MAXT && ctas <= n_sm && dk % 32 == 0 && dk <= 128 &&
+  for (int b = 0; b < r.n; ++b) ctas += (long)((r.sized[b] + ATS_ROWS - 1) / ATS_ROWS) * L.heads;
+  const int mt = (r.maxLen + AT_KT - 1) / AT_KT;
+  return r.tune.attn_split && mt <= ATS_MAXT && ctas <= n_sm && dk % 32 == 0 && dk <= 128 &&
          (long)attn_split_smem_floats(dk, nrel, mt) * (long)sizeof(float) <= ATS_SMEM_MAX;
 }
 
-void vtts_engine::launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen) {
+void vtts_engine::launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const EncLayerW& L, int Hc, const Rows& r) {
   const int dk = Hc / L.heads;
   AttnTcParams ap;
   memset(&ap, 0, sizeof(ap));
@@ -1383,38 +1466,38 @@ void vtts_engine::launch_attn_tc(const Planes& qkv, float* ao, Planes* pl, const
   ap.p_hi = pl ? pl->hi : nullptr; ap.p_lo = pl ? pl->lo : nullptr; ap.ldp = pl ? pl->C : 0;
   ap.n_heads = L.heads; ap.window = cfg.window_size;
   ap.koff = Hc; ap.voff = 2 * Hc;
-  dim3 grid((maxLen + ATC_BM - 1) / ATC_BM, L.heads, B);
+  dim3 grid((r.maxLen + ATC_BM - 1) / ATC_BM, L.heads, r.n);
   if (grid.x == 0) return;
   last_attn = vtts_attn_report{VTTS_ATTN_TC, dk, 0, (int)grid.x, (int)grid.y, (int)grid.z, atc_smem_bytes(dk)};
   switch (dk / 32) {
-    case 1: klaunch(attn_tc_kernel<32>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(32), ap, lens, offs); break;
-    case 2: klaunch(attn_tc_kernel<64>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(64), ap, lens, offs); break;
-    case 3: klaunch(attn_tc_kernel<96>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(96), ap, lens, offs); break;
-    default: klaunch(attn_tc_kernel<128>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(128), ap, lens, offs); break;
+    case 1: klaunch(attn_tc_kernel<32>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(32), ap, r.lens, r.offs); break;
+    case 2: klaunch(attn_tc_kernel<64>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(64), ap, r.lens, r.offs); break;
+    case 3: klaunch(attn_tc_kernel<96>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(96), ap, r.lens, r.offs); break;
+    default: klaunch(attn_tc_kernel<128>, grid, dim3(ATC_THREADS), (size_t)atc_smem_bytes(128), ap, r.lens, r.offs); break;
   }
   CK(cudaGetLastError());
   ++launches;
 }
 
-void vtts_engine::launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, const int* lens, const int* offs, int maxLen, Planes* pl) {
+void vtts_engine::launch_attn(const float* qkv, float* ao, const EncLayerW& L, int Hc, Planes* pl, const Rows& r) {
+  const int maxLen = r.maxLen, rows_per_warp = r.tune.attn_rows;
   const int n_heads = L.heads;
   const int dk = Hc / n_heads, nrel = 2 * cfg.window_size + 1;
   __nv_bfloat16* ph = pl ? pl->hi : nullptr;
   __nv_bfloat16* plo = pl ? pl->lo : nullptr;
   __nv_bfloat16* pmi = pl ? pl->mid : nullptr;
   // register-blocked variant (4 query rows per warp) once the launch is throughput bound
-  const std::vector<int>& hl = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
   long rows = 0;
-  for (int b = 0; b < B; ++b) rows += hl[b];
-  const int R = (attn_rows == 1 || attn_rows == 4) ? attn_rows : (rows * n_heads >= 8L * 2 * n_sm * 4 ? 4 : 1);
+  for (int b = 0; b < r.n; ++b) rows += r.sized[b];
+  const int R = (rows_per_warp == 1 || rows_per_warp == 4) ? rows_per_warp : (rows * n_heads >= 8L * 2 * n_sm * 4 ? 4 : 1);
   // single short utterances: split-KV variant (all K/V tiles resident, 4 warps per query row) when it fits one wave
   {
     const int mt = (maxLen + AT_KT - 1) / AT_KT;
-    if (R == 1 && attn_split_fits(L, Hc, lens, maxLen)) {
-      dim3 grid((maxLen + ATS_ROWS - 1) / ATS_ROWS, n_heads, B);
+    if (R == 1 && attn_split_fits(L, Hc, r)) {
+      dim3 grid((maxLen + ATS_ROWS - 1) / ATS_ROWS, n_heads, r.n);
       const size_t smem = (size_t)attn_split_smem_floats(dk, nrel, mt) * sizeof(float);
       last_attn = vtts_attn_report{VTTS_ATTN_SPLIT, dk, 1, (int)grid.x, (int)grid.y, (int)grid.z, (int)smem};
-#define ATTN_SPLIT(D) klaunch(attn_split_kernel<D>, grid, dim3(ATS_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, mt, lens, offs, ph, plo, pmi)
+#define ATTN_SPLIT(D) klaunch(attn_split_kernel<D>, grid, dim3(ATS_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, mt, r.lens, r.offs, ph, plo, pmi)
       switch (dk / 32) { case 1: ATTN_SPLIT(1); break; case 2: ATTN_SPLIT(2); break; case 3: ATTN_SPLIT(3); break; default: ATTN_SPLIT(4); break; }
 #undef ATTN_SPLIT
       CK(cudaGetLastError());
@@ -1423,10 +1506,10 @@ void vtts_engine::launch_attn(const float* qkv, float* ao, const EncLayerW& L, i
     }
   }
   const int QT = 8 * R;
-  dim3 grid((maxLen + QT - 1) / QT, n_heads, B);
+  dim3 grid((maxLen + QT - 1) / QT, n_heads, r.n);
   const size_t smem = (size_t)attn_smem_floats(dk, nrel, R) * sizeof(float);
   last_attn = vtts_attn_report{R == 4 ? VTTS_ATTN_R4 : VTTS_ATTN_R1, dk, R, (int)grid.x, (int)grid.y, (int)grid.z, (int)smem};
-#define ATTN_CASE(D, RR) klaunch(attn_kernel<D, RR>, grid, dim3(AT_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, lens, offs, ph, plo, pmi)
+#define ATTN_CASE(D, RR) klaunch(attn_kernel<D, RR>, grid, dim3(AT_THREADS), smem, qkv, 3 * Hc, ao, Hc, L.relk, L.relv, n_heads, cfg.window_size, r.lens, r.offs, ph, plo, pmi)
   if (R == 4) {
     switch (dk / 32) { case 1: ATTN_CASE(1, 4); break; case 2: ATTN_CASE(2, 4); break; case 3: ATTN_CASE(3, 4); break; default: ATTN_CASE(4, 4); break; }
   } else {
@@ -1474,7 +1557,7 @@ void vtts_engine::alloc_decoder_planes() {
 // forward: the flow's forward direction (models.py:750-753, x1 <- x1 + m, layers in order) for voice conversion; the
 // Flip folding of the packed weights is valid for it when flow_n_flows is even.  cond: the [B][cond_ld] rows of the stacked
 // conditioning matrix of the speaker the flow runs for (null: unconditioned).
-void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, const float* cond, int cond_ld, bool forward) {
+void vtts_engine::flow_tc(float* z, bool emit_pz, const float* cond, int cond_ld, bool forward, const Rows& r) {
   const vtts_config& c = cfg;
   const int H = c.hidden_channels, I = c.inter_channels, half = I / 2;
   const long F = Tfrm;
@@ -1487,7 +1570,7 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, 
   float* fqkv = ensure(d_fqkv, (size_t)F * 3 * H);
   float* fao = ensure(d_fao, (size_t)F * H);
   Planes ph = flp.ph, pao = flp.pao, ph1 = flp.ph1, pff = flp.pff, pwx = flp.pwx, pacts = flp.pacts, pskip = flp.pskip, pqkv = flp.pqkv;
-  dim3 lg((maxFrm + 3) / 4, B);
+  dim3 lg((r.maxLen + 3) / 4, r.n);
   for (int s = 0; s < nf; ++s) {
     const int f = forward ? s : nf - 1 - s;
     const FlowW& W = flow[f];
@@ -1497,65 +1580,65 @@ void vtts_engine::flow_tc(float* z, const int* fl, const int* fo, bool emit_pz, 
       ConvP p = mk(W.pre, z, I, x0off, h, H, 0, 1, 0);
       Planes& dst = c.use_transformer_flows ? ph : pwx;
       p.p_hi = dst.hi; p.p_lo = dst.lo; p.ldp = H; p.pl_slope = 1.f;
-      launch_conv({p}, 1, fl, fo, maxFrm, B);
+      launch_conv({p}, 1, r);
     }
     float* wn_x = h;
     if (c.use_transformer_flows) {
-      if (attn_use_tc(W.tr, H, fl, maxFrm)) {
+      if (attn_use_tc(W.tr, H, r)) {
         // q, k, v leave the qkv conv as split-bf16 planes only; attention runs on wgmma (attn_tc.cuh)
         { TcSpec q; q.in = ph; q.w = W.t_qkv; q.bias = W.tr.qkv.b; q.Cin = H; q.Cout = 3 * H; q.out = pqkv; q.pl_slope = 1.f;
-          launch_tc({q}, 1, fl, fo, maxFrm, B); }
-        launch_attn_tc(pqkv, nullptr, &pao, W.tr, H, fl, fo, maxFrm);
+          launch_tc({q}, 1, r); }
+        launch_attn_tc(pqkv, nullptr, &pao, W.tr, H, r);
       } else {
         { TcSpec q; q.in = ph; q.w = W.t_qkv; q.bias = W.tr.qkv.b; q.Cin = H; q.Cout = 3 * H; q.y = fqkv; q.ldy = 3 * H;
-          launch_tc({q}, 1, fl, fo, maxFrm, B); }
-        launch_attn(fqkv, fao, W.tr, H, fl, fo, maxFrm, &pao);
+          launch_tc({q}, 1, r); }
+        launch_attn(fqkv, fao, W.tr, H, &pao, r);
       }
       { TcSpec q; q.in = pao; q.w = W.t_o; q.bias = W.tr.o.b; q.Cin = H; q.Cout = H; q.y = fy; q.ldy = H;
-        launch_tc({q}, 1, fl, fo, maxFrm, B); }
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), h, fy, W.tr.ln1.g, W.tr.ln1.b, nullptr, nullptr, 0, h1, fl, fo, H, ph1.hi, ph1.lo, (__nv_bfloat16*)nullptr);
+        launch_tc({q}, 1, r); }
+      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), h, fy, W.tr.ln1.g, W.tr.ln1.b, nullptr, nullptr, 0, h1, r.lens, r.offs, H, ph1.hi, ph1.lo, (__nv_bfloat16*)nullptr);
       CK(cudaGetLastError());
       ++launches;
       { TcSpec q; q.in = ph1; q.w = W.t_ffn1; q.bias = W.tr.ffn1.b; q.Cin = H; q.Cout = H; q.k = fk; q.pad = (fk - 1) / 2;
         q.epi = TCE_RELU; q.out = pff; q.pl_slope = 1.f;
-        launch_tc({q}, 1, fl, fo, maxFrm, B); }
+        launch_tc({q}, 1, r); }
       { TcSpec q; q.in = pff; q.w = W.t_ffn2; q.bias = W.tr.ffn2.b; q.Cin = H; q.Cout = H; q.k = fk; q.pad = (fk - 1) / 2;
         q.y = fy; q.ldy = H;
-        launch_tc({q}, 1, fl, fo, maxFrm, B); }
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), h1, fy, W.tr.ln2.g, W.tr.ln2.b, h, nullptr, 0, wx, fl, fo, H, pwx.hi, pwx.lo, (__nv_bfloat16*)nullptr);
+        launch_tc({q}, 1, r); }
+      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), h1, fy, W.tr.ln2.g, W.tr.ln2.b, h, nullptr, 0, wx, r.lens, r.offs, H, pwx.hi, pwx.lo, (__nv_bfloat16*)nullptr);
       CK(cudaGetLastError());
       ++launches;
       wn_x = wx;
     }
     wn_tc(W.t_in, W.in, W.t_rsx, W.rsx, W.t_rss, W.rss, nl, fk, c.flow_dilation_rate, wn_x, skip, pwx, pacts, pskip,
-          cond ? cond + r_flow + f * nl * 2 * H : nullptr, cond_ld, fl, fo);
+          cond ? cond + r_flow + f * nl * 2 * H : nullptr, cond_ld, r);
     { TcSpec q; q.in = pskip; q.w = W.t_post; q.bias = W.post.b; q.Cin = H; q.Cout = half; q.alpha = forward ? 1.f : -1.f;
       q.y = z; q.ldy = I; q.yoff = x1off; q.res = z; q.ldr = I; q.roff = x1off;
       if (emit_pz && f <= 1) { q.out = dcp.pz; q.poff = x1off; q.pl_slope = 1.f; }     // this half of z is final now
-      launch_tc({q}, 1, fl, fo, maxFrm, B); }
+      launch_tc({q}, 1, r); }
   }
 }
 
 void vtts_engine::wn_tc(const std::vector<TcW>& t_in, const std::vector<ConvW>& in, const std::vector<TcW>& t_rsx,
                         const std::vector<ConvW>& rsx, const std::vector<TcW>& t_rss, const std::vector<ConvW>& rss, int nl, int fk,
                         int dil_rate, float* x, float* skip, const Planes& px, const Planes& pacts, const Planes& pskip, const float* cond,
-                        int cond_ld, const int* fl, const int* fo) {
+                        int cond_ld, const Rows& r) {
   const int H = cfg.hidden_channels;
   int dil = 1;
   for (int i = 0; i < nl; ++i) {
     { TcSpec q; q.in = px; q.w = t_in[i]; q.bias = in[i].b; q.Cin = H; q.Cout = 2 * H; q.k = fk; q.dil = dil;
       q.pad = dil * (fk - 1) / 2; q.epi = TCE_GATE; q.out = pacts; q.pl_slope = 1.f;
       if (cond) { q.cond = cond + i * 2 * H; q.cond_ld = cond_ld; }
-      launch_tc({q}, 1, fl, fo, maxFrm, B); }
+      launch_tc({q}, 1, r); }
     TcSpec qs; qs.in = pacts; qs.w = t_rss[i]; qs.bias = rss[i].b; qs.Cin = H; qs.Cout = H; qs.y = skip; qs.ldy = H;
     if (i > 0) { qs.res = skip; qs.ldr = H; }
     if (i < nl - 1) {
       TcSpec qx; qx.in = pacts; qx.w = t_rsx[i]; qx.bias = rsx[i].b; qx.Cin = H; qx.Cout = H; qx.y = x; qx.ldy = H;
       qx.res = x; qx.ldr = H; qx.out = px; qx.pl_slope = 1.f;
-      launch_tc({qx, qs}, 1, fl, fo, maxFrm, B);
+      launch_tc({qx, qs}, 1, r);
     } else {
       qs.out = pskip; qs.pl_slope = 1.f;
-      launch_tc({qs}, 1, fl, fo, maxFrm, B);
+      launch_tc({qs}, 1, r);
     }
     dil *= dil_rate;
   }
@@ -1565,7 +1648,7 @@ void vtts_engine::wn_tc(const std::vector<TcW>& t_in, const std::vector<ConvW>& 
 // producer's epilogue; fp32 copies exist only where a residual or the MRF mean needs them.  The StableTTS vocoder runs only
 // its first voc_nt stages here, from an FFMA conv_pre that writes the planes, and then the next upsampling conv into fp32
 // rows d_stage[voc_nt]: returns false, and decode() continues on the FFMA pipe from there.
-bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_ready) {
+bool vtts_engine::decoder_tc(float* z, bool pz_ready, const Rows& r) {
   const vtts_config& c = cfg;
   const int I = c.inter_channels;
   const long F = Tfrm;
@@ -1574,8 +1657,8 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
   const std::vector<Planes>&st_px = dcp.px, &st_nxt = dcp.nxt;
   const std::vector<std::vector<Planes>>&st_pj = dcp.pj, &st_pt = dcp.pt;
   if (!pz_ready && !has_voc) {
-    dim3 g((maxFrm + EW_ROWS - 1) / EW_ROWS, B);
-    klaunch(split_planes_kernel, dim3(g), dim3(EW_THREADS), (size_t)(0), z, I, pz.hi, pz.lo, I, I, 1.f, 0, 1, fl, fo);
+    dim3 g((r.maxLen + EW_ROWS - 1) / EW_ROWS, r.n);
+    klaunch(split_planes_kernel, dim3(g), dim3(EW_THREADS), (size_t)(0), z, I, pz.hi, pz.lo, I, I, 1.f, 0, 1, r.lens, r.offs);
     CK(cudaGetLastError());
     ++launches;
   }
@@ -1583,14 +1666,14 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
   if (has_voc) {         // conv_pre on the FFMA pipe, its output handed over as the planes of lrelu(x, 0.1)
     ConvP p = mk(dec_pre, z, I, 0, ensure(d_d0, (size_t)F * ch), ch, 0, 1, 3);
     p.p_hi = cur.hi; p.p_lo = cur.lo; p.ldp = ch; p.pl_slope = 0.1f;
-    launch_conv({p}, 1, fl, fo, maxFrm, B);
+    launch_conv({p}, 1, r);
   } else {
     TcSpec q;
     q.in = pz; q.w = tc_pre; q.bias = dec_pre.b; q.Cin = I; q.Cout = ch; q.k = 7; q.dil = 1; q.pad = 3;
     q.out = cur; q.pl_slope = 0.1f;
     if (r_dec >= 0) { q.cond = d_condv.p + r_dec; q.cond_ld = condR; }     // x = conv_pre(z) + cond(g) (QuickVC, vc/models.py:465)
     if (debug_flags & 1) { q.y = ensure(d_d0, (size_t)F * ch); q.ldy = ch; }
-    launch_tc({q}, 1, fl, fo, maxFrm, B);
+    launch_tc({q}, 1, r);
   }
   int rm = 1;
   if ((int)d_stage.size() < c.n_upsamples) {
@@ -1607,14 +1690,14 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     Planes px = st_px[i];
     for (int r0 = 0; r0 < u; r0 += TC_MAXP) {
       std::vector<TcSpec> ps;
-      for (int r = r0; r < std::min(u, r0 + TC_MAXP); ++r) {
+      for (int ph = r0; ph < std::min(u, r0 + TC_MAXP); ++ph) {
         TcSpec q;
-        q.in = cur; q.w = ups[i].tphase[r]; q.bias = ups[i].phase[r].b; q.Cin = ch; q.Cout = ch2;
-        q.k = ups[i].phase[r].k; q.dil = 1; q.pad = ups[i].pad[r];
-        q.y = X; q.ldy = ch2; q.out = px; q.pl_slope = 0.1f; q.out_mul = u; q.out_add = r;
+        q.in = cur; q.w = ups[i].tphase[ph]; q.bias = ups[i].phase[ph].b; q.Cin = ch; q.Cout = ch2;
+        q.k = ups[i].phase[ph].k; q.dil = 1; q.pad = ups[i].pad[ph];
+        q.y = X; q.ldy = ch2; q.out = px; q.pl_slope = 0.1f; q.out_mul = u; q.out_add = ph;
         ps.push_back(q);
       }
-      launch_tc(ps, rm, fl, fo, maxFrm, B);
+      launch_tc(ps, rm, r);
     }
     rm *= u;
     ch = ch2;
@@ -1640,15 +1723,15 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     // the split-K width that suits its own k-loop -- correct, but the concurrent cluster launches of three streams
     // contend and the step gets slower (1.74 vs 1.62 ms).
     long group_tiles = 0;
-    for (int b = 0; b < B; ++b) group_tiles += (long)nk * ((v_frm_len[b] * rm + TC_BM - 1) / TC_BM) * ((ch + 63) / 64);
+    for (int b = 0; b < r.n; ++b) group_tiles += (long)nk * ((r.sized[b] * rm + TC_BM - 1) / TC_BM) * ((ch + 63) / 64);
     const bool branch = mrf_branch && !profiling && nk > 1 && nk - 1 <= 3 && group_tiles <= n_sm;
     if (branch) {
       auto chain = [&](int j) {
         for (int d = 0; d < nd; ++d) {
           TcSpec a, b2;
           rb_pair(j, d, a, b2);
-          launch_tc({a}, rm, fl, fo, maxFrm, B);
-          launch_tc({b2}, rm, fl, fo, maxFrm, B);
+          launch_tc({a}, rm, r);
+          launch_tc({b2}, rm, r);
         }
       };
       CK(cudaEventRecord(ev_fork, stream));
@@ -1669,17 +1752,17 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
         // longest k-loop (largest kernel size) goes first, so that the last tiles are short ones.  Single-wave launches give
         // each resblock its own split instead (tc_split_plan), where the order does not matter.
         for (int j = 0; j < nk; ++j) rb_pair(j, d, p1[mrf_heavy_first ? nk - 1 - j : j], p2[mrf_heavy_first ? nk - 1 - j : j]);
-        launch_tc(p1, rm, fl, fo, maxFrm, B);
-        launch_tc(p2, rm, fl, fo, maxFrm, B);
+        launch_tc(p1, rm, r);
+        launch_tc(p2, rm, r);
       }
     }
     const bool last = (i + 1 == c.n_upsamples);
     Planes nxt = st_nxt[i];
     {
-      dim3 g((maxFrm * rm + (last ? 1 : 0) + EW_ROWS - 1) / EW_ROWS, B);
+      dim3 g((r.maxLen * rm + (last ? 1 : 0) + EW_ROWS - 1) / EW_ROWS, r.n);
       klaunch(mrf_mean_planes_kernel, dim3(g), dim3(EW_THREADS), (size_t)(0), xj[0], nk > 1 ? xj[1] : nullptr, nk > 2 ? xj[2] : nullptr, std::min(nk, 3),
                                                    (debug_flags & 1) ? X : nullptr, nxt.hi, nxt.lo, ch, last ? 0.01f : 0.1f,
-                                                   last ? 1 : 0, rm, fl, fo);
+                                                   last ? 1 : 0, rm, r.lens, r.offs);
       CK(cudaGetLastError());
       ++launches;
     }
@@ -1692,14 +1775,14 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     float* X = ensure(d_stage[nst], (size_t)F * rm * u * ch2);
     for (int r0 = 0; r0 < u; r0 += TC_MAXP) {
       std::vector<TcSpec> ps;
-      for (int r = r0; r < std::min(u, r0 + TC_MAXP); ++r) {
+      for (int ph = r0; ph < std::min(u, r0 + TC_MAXP); ++ph) {
         TcSpec q;
-        q.in = cur; q.w = ups[nst].tphase[r]; q.bias = ups[nst].phase[r].b; q.Cin = ch; q.Cout = ch2;
-        q.k = ups[nst].phase[r].k; q.dil = 1; q.pad = ups[nst].pad[r];
-        q.y = X; q.ldy = ch2; q.out_mul = u; q.out_add = r;
+        q.in = cur; q.w = ups[nst].tphase[ph]; q.bias = ups[nst].phase[ph].b; q.Cin = ch; q.Cout = ch2;
+        q.k = ups[nst].phase[ph].k; q.dil = 1; q.pad = ups[nst].pad[ph];
+        q.y = X; q.ldy = ch2; q.out_mul = u; q.out_add = ph;
         ps.push_back(q);
       }
-      launch_tc(ps, rm, fl, fo, maxFrm, B);
+      launch_tc(ps, rm, r);
     }
     return false;
   }
@@ -1709,20 +1792,22 @@ bool vtts_engine::decoder_tc(float* z, const int* fl, const int* fo, bool pz_rea
     TcSpec q;
     q.in = cur; q.w = tc_post; q.bias = dec_post.b; q.Cin = ch; q.Cout = pc; q.k = 7; q.dil = 1; q.pad = 3;
     q.y = post; q.ldy = pc; q.in_extra = 1; q.out_seq_extra = 1;
-    launch_tc({q}, rm, fl, fo, maxFrm, B);
+    launch_tc({q}, rm, r);
   }
   float* wav = ensure(d_wav, (size_t)F * hop + 16);
-  const int M = maxFrm * rm * c.istft_hop;
-  dim3 g((M + TL_M - 1) / TL_M, B);
+  const int M = r.maxLen * rm * c.istft_hop;
+  dim3 g((M + TL_M - 1) / TL_M, r.n);
   const size_t smem = ((size_t)tl_rec_frames(63, c.subbands, c.istft_n_fft, c.istft_hop) * pc + (size_t)c.subbands * (TL_M + 2 * tl_halo(63, c.subbands))) * sizeof(float);
   REQUIRE(c.istft_hop == 4 && c.istft_n_fft == 16, VTTS_ERR_INVALID, "iSTFT tail kernel is sized for n_fft=16, hop=4");
-  klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1, istft_w2);
+  klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, r.lens, r.offs, wav, 0, 1, istft_w2);
   CK(cudaGetLastError());
   ++launches;
   return true;
 }
 
-void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int* lens, const int* offs, int maxLen, int nB) {
+void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const Rows& r) {
+  const Tuning& t = r.tune;
+  const int nB = r.n, maxLen = r.maxLen;
   ConvBatch cb;
   memset(&cb, 0, sizeof(cb));
   REQUIRE(!ps.empty() && (int)ps.size() <= CV_MAXP, VTTS_ERR_INVALID, "bad grouped conv");
@@ -1736,16 +1821,14 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
   }
   cb.n = (int)ps.size();
   cb.rmul = rmul;
-  const std::vector<int>& hl0 = (lens == d_tok_len.p) ? v_tok_len : v_frm_len;
-  const std::vector<int>& hl_true = (lens == d_tok_len.p) ? h_tok_len : h_frm_len;
   long base0 = 0;
   for (const ConvP& q : ps)
-    for (int b = 0; b < nB; ++b) base0 += (long)((hl0[b] * rmul + q.in_extra + CV_TT - 1) / CV_TT) * ((q.Cout + CV_TC - 1) / CV_TC);
+    for (int b = 0; b < nB; ++b) base0 += (long)((r.sized[b] * rmul + q.in_extra + CV_TT - 1) / CV_TT) * ((q.Cout + CV_TC - 1) / CV_TC);
   // many tiles (batched calls): one thread group per CTA (several CTAs per SM; r2, batch 64: 6.98 ms per step against 8.01 / 8.21
   // with 2 / 4 groups), no cluster.  Few tiles (batch 1): the k-steps of a tile are
   // spread over a cluster of S CTAs until the launch fills ~1 wave of SMs; ranks that still have long k-loops then get
   // 2-4 thread groups each (a lone warp per scheduler issues an FFMA only every other cycle).
-  int G = base0 >= 2 * n_sm ? conv_big_g : conv_min_g;
+  int G = base0 >= 2 * n_sm ? t.conv_big_g : t.conv_min_g;
   for (const ConvP& q : ps)
     while (G > 1 && q.Cin % (CV_CK * G) != 0) G >>= 1;
   auto min_steps = [&](int g) {
@@ -1754,14 +1837,14 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
     return ms;
   };
   int S = 1;
-  while (S < conv_max_s && base0 * S < conv_target && S * 2 <= min_steps(G)) S *= 2;
+  while (S < t.conv_max_s && base0 * S < t.conv_target && S * 2 <= min_steps(G)) S *= 2;
   const int xw = (CV_TT + maxHalo + 7) / 8 * 8 + 1;
   auto smem_floats = [&](int g) {
     const size_t pipe = (size_t)2 * CV_CK * g * xw + (size_t)CV_NS * CV_CK * g * CV_TC;
     return (std::max(pipe, (size_t)(g - 1) * 32 * CV_THREADS) + 3) / 4 * 4 + (size_t)32 * CV_THREADS;
   };
-  if (conv_auto_g && base0 < 2 * n_sm)
-    while (G * 2 <= conv_max_g && min_steps(G * 2) / S >= conv_auto_g && smem_floats(G * 2) * sizeof(float) <= (size_t)CONV_SMEM_MAX) G *= 2;
+  if (t.conv_auto_g && base0 < 2 * n_sm)
+    while (G * 2 <= t.conv_max_g && min_steps(G * 2) / S >= t.conv_auto_g && smem_floats(G * 2) * sizeof(float) <= (size_t)CONV_SMEM_MAX) G *= 2;
   REQUIRE(smem_floats(G) * sizeof(float) <= (size_t)CONV_SMEM_MAX, VTTS_ERR_INVALID, "conv tile does not fit in shared memory");
   cb.S = S;
   cb.xw = xw;
@@ -1770,14 +1853,13 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
   const size_t stage_off = (std::max(pipe_floats, red_floats) + 3) / 4 * 4;
   cb.stage_off = (int)stage_off;
   const size_t smem = (stage_off + (S > 1 ? (size_t)32 * CV_THREADS : 0)) * sizeof(float);
-  const std::vector<int>& hl = hl_true;      // (profiling FLOP count below)
   dim3 grid(((maxL + CV_TT - 1) / CV_TT) * S, (maxCout + CV_TC - 1) / CV_TC, nB * cb.n);
   if (grid.x == 0) return;
   {
-    vtts_conv_report r{};
-    r.S = S; r.G = G;
-    r.grid_x = (int)grid.x; r.grid_y = (int)grid.y; r.grid_z = (int)grid.z;
-    note_conv(r);
+    vtts_conv_report rep{};
+    rep.S = S; rep.G = G;
+    rep.grid_x = (int)grid.x; rep.grid_y = (int)grid.y; rep.grid_z = (int)grid.z;
+    note_conv(rep);
   }
   if (profiling) {
     if (prof_used + 2 > prof_ev.size()) {
@@ -1787,7 +1869,7 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
     }
     for (const ConvP& q : ps)
       for (int b = 0; b < nB; ++b)
-        prof_flops += 2.0 * ((double)hl[b] * rmul + q.in_extra) * q.Cout * q.Cin * q.k;
+        prof_flops += 2.0 * ((double)r.real[b] * rmul + q.in_extra) * q.Cout * q.Cin * q.k;
     ++prof_launches;
     CK(cudaEventRecord(prof_ev[prof_used], stream));
   }
@@ -1815,9 +1897,9 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
     lc.attrs = at;
     lc.numAttrs = na;
     switch (G) {
-      case 4: CK(cudaLaunchKernelEx(&lc, conv_kernel<4>, cb, lens, offs)); break;
-      case 2: CK(cudaLaunchKernelEx(&lc, conv_kernel<2>, cb, lens, offs)); break;
-      default: CK(cudaLaunchKernelEx(&lc, conv_kernel<1>, cb, lens, offs)); break;
+      case 4: CK(cudaLaunchKernelEx(&lc, conv_kernel<4>, cb, r.lens, r.offs)); break;
+      case 2: CK(cudaLaunchKernelEx(&lc, conv_kernel<2>, cb, r.lens, r.offs)); break;
+      default: CK(cudaLaunchKernelEx(&lc, conv_kernel<1>, cb, r.lens, r.offs)); break;
     }
   }
   CK(cudaGetLastError());
@@ -1830,28 +1912,26 @@ void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const int*
 
 // One relative-attention encoder layer (attentions.py:57-63): x <- LN2(x1 + FFN(x1)), x1 = LN1(x + MHA(x)).
 void vtts_engine::encoder_layer(const EncLayerW& L, float*& x, float*& xb, float* qkv, float* ao, float* y, float* ffh, int Hc,
-                                int Fc, int ks, const int* lens, const int* offs, int maxLen, const float* vec_after, int vec_ld,
-                                const float* cadd_after) {
-  const int nB = B;
-  launch_conv({mk(L.qkv, x, Hc, 0, qkv, 3 * Hc, 0, 1, 0)}, 1, lens, offs, maxLen, nB);
-  launch_attn(qkv, ao, L, Hc, lens, offs, maxLen, nullptr);
-  launch_conv({mk(L.o, ao, Hc, 0, y, Hc, 0, 1, 0)}, 1, lens, offs, maxLen, nB);
-  dim3 lg((maxLen + 3) / 4, nB);
-  klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), x, y, L.ln1.g, L.ln1.b, nullptr, nullptr, 0, xb, lens, offs, Hc, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
+                                int Fc, int ks, const float* vec_after, int vec_ld, const float* cadd_after, const Rows& r) {
+  launch_conv({mk(L.qkv, x, Hc, 0, qkv, 3 * Hc, 0, 1, 0)}, 1, r);
+  launch_attn(qkv, ao, L, Hc, nullptr, r);
+  launch_conv({mk(L.o, ao, Hc, 0, y, Hc, 0, 1, 0)}, 1, r);
+  dim3 lg((r.maxLen + 3) / 4, r.n);
+  klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), x, y, L.ln1.g, L.ln1.b, nullptr, nullptr, 0, xb, r.lens, r.offs, Hc, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
   CK(cudaGetLastError());
   ++launches;
   {
     ConvP p = mk(L.ffn1, xb, Hc, 0, ffh, Fc, 0, 1, (ks - 1) / 2);
     p.epi = EPI_RELU;
-    launch_conv({p}, 1, lens, offs, maxLen, nB);
+    launch_conv({p}, 1, r);
   }
-  launch_conv({mk(L.ffn2, ffh, Fc, 0, y, Hc, 0, 1, (ks - 1) / 2)}, 1, lens, offs, maxLen, nB);
-  klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xb, y, L.ln2.g, L.ln2.b, cadd_after, vec_after, vec_ld, x, lens, offs, Hc, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
+  launch_conv({mk(L.ffn2, ffh, Fc, 0, y, Hc, 0, 1, (ks - 1) / 2)}, 1, r);
+  klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xb, y, L.ln2.g, L.ln2.b, cadd_after, vec_after, vec_ld, x, r.lens, r.offs, Hc, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
   CK(cudaGetLastError());
   ++launches;
 }
 
-void vtts_engine::dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const int* lens, const int* offs, int maxLen,
+void vtts_engine::dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const Rows& r,
                             const float* x0, const float* pre_w, const float* pre_b, const float* cond) {
   int dil = 1;
   for (int i = 0; i < 3; ++i) {
@@ -1865,9 +1945,9 @@ void vtts_engine::dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, c
     P.C = C; P.k = k; P.dil = dil;
     // (16 positions per CTA were tried for batched calls -- 4x less weight streaming per position -- and measured slower:
     //  duration stage 3.20 vs 2.95 ms at batch 64)
-    dim3 grid((maxLen + DDS_TT - 1) / DDS_TT, B);
+    dim3 grid((r.maxLen + DDS_TT - 1) / DDS_TT, r.n);
     const size_t smem = ((size_t)DDS_NS * DDS_CH * C + (size_t)C * DDS_TT + 8 * DDS_TT) * sizeof(float);
-    klaunch(dds_layer_kernel<DDS_TT>, dim3(grid), dim3(C), (size_t)(smem), P, lens, offs);
+    klaunch(dds_layer_kernel<DDS_TT>, dim3(grid), dim3(C), (size_t)(smem), P, r.lens, r.offs);
     CK(cudaGetLastError());
     ++launches;
     std::swap(a, b);
@@ -1890,6 +1970,7 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   int* ids = ensure(d_ids, T);
   int* sid = ensure(d_sid, B);
   float* prm = ensure(d_prm, 8);
+  const Rows r = tok_rows();
   {
     P1Pin pp = p1_layout(noise_dp && !noise_on_device);
     CK(cudaMemcpyAsync(tl, pp.len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
@@ -1945,12 +2026,12 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   {
     ConvP p = mk(dp_pre, x, H, 0, dA, D, 0, 1, 0);
     if (has_g) { p.cond = condv + r_dp; p.cond_ld = condR; }
-    launch_conv({p}, 1, tl, to, maxTok, B);
+    launch_conv({p}, 1, r);
   }
   {
     float *a = dA, *b = dB;
-    dds_stack(dp_dds, D, c.dp_kernel_size, a, b, tl, to, maxTok);
-    launch_conv({mk(dp_proj, a, D, 0, dx, D, 0, 1, 0)}, 1, tl, to, maxTok, B);
+    dds_stack(dp_dds, D, c.dp_kernel_size, a, b, r);
+    launch_conv({mk(dp_proj, a, D, 0, dx, D, 0, 1, 0)}, 1, r);
   }
   {
     dim3 g((maxTok + 127) / 128, B);
@@ -1966,8 +2047,8 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
     const CfW& F = cf[n - 2];
     // (the ConvFlow front h = pre(x0) + cond, modules.py:366-367, is computed inside the first DDS layer)
     float *a = dA, *b = dB;
-    dds_stack(F.dds, D, c.dp_kernel_size, a, b, tl, to, maxTok, cvar, F.pre_w, F.pre_b, dx);
-    launch_conv({mk(F.proj, a, D, 0, h29, 32, 0, 1, 0)}, 1, tl, to, maxTok, B);
+    dds_stack(F.dds, D, c.dp_kernel_size, a, b, r, cvar, F.pre_w, F.pre_b, dx);
+    launch_conv({mk(F.proj, a, D, 0, h29, 32, 0, 1, 0)}, 1, r);
     {
       dim3 g((maxTok + 127) / 128, B);
       klaunch(spline_inverse_kernel, dim3(g), dim3(128), (size_t)(0), h29, 32, tvar, nbins, c.dp_tail_bound, sqrtf((float)D), tl, to);
@@ -2009,6 +2090,7 @@ void vtts_engine::text_encoder(const float* cond, int cond_ld) {
   const int* tl = d_tok_len.p;
   const int* to = d_tok_off.p;
   const int* ids = d_ids.p;
+  const Rows r = tok_rows();
   const float* spk_vec = (cond && r_spk >= 0) ? cond + r_spk : nullptr;
 
   // ---- text encoder (models.py:317-326)
@@ -2037,32 +2119,32 @@ void vtts_engine::text_encoder(const float* cond, int cond_ld) {
   for (int i = 0; i < c.n_layers; ++i) {
     const float* va = (spk_vec && c.cond_layer_idx == i + 1) ? spk_vec : nullptr;
     if (!enc_on_tc) {
-      encoder_layer(enc[i], x, xb, qkv, ao, y, ffh, H, Fc, c.kernel_size, tl, to, maxTok, va, cond_ld, nullptr);
+      encoder_layer(enc[i], x, xb, qkv, ao, y, ffh, H, Fc, c.kernel_size, va, cond_ld, nullptr, r);
       continue;
     }
     // precision mode 2: same layer with the four convs on wgmma (attentions.py:57-63)
     const EncLayerW& L = enc[i];
     const int ks = c.kernel_size;
     dim3 lg((maxTok + 3) / 4, B);
-    if (attn_use_tc(L, H, tl, maxTok)) {
+    if (attn_use_tc(L, H, r)) {
       { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.out = pqkv; q.pl_slope = 1.f;
-        launch_tc({q}, 1, tl, to, maxTok, B); }
-      launch_attn_tc(pqkv, nullptr, &pao, L, H, tl, to, maxTok);
+        launch_tc({q}, 1, r); }
+      launch_attn_tc(pqkv, nullptr, &pao, L, H, r);
     } else {
       { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.y = qkv; q.ldy = 3 * H;
-        launch_tc({q}, 1, tl, to, maxTok, B); }
-      launch_attn(qkv, ao, L, H, tl, to, maxTok, &pao);
+        launch_tc({q}, 1, r); }
+      launch_attn(qkv, ao, L, H, &pao, r);
     }
     { TcSpec q; q.in = pao; q.w = L.t_o; q.bias = L.o.b; q.Cin = H; q.Cout = H; q.y = y; q.ldy = H;
-      launch_tc({q}, 1, tl, to, maxTok, B); }
+      launch_tc({q}, 1, r); }
     klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, x, y, L.ln1.g, L.ln1.b, (const float*)nullptr, (const float*)nullptr, 0, xb, tl, to, H, px1.hi, px1.lo, px1.mid);
     ++launches;
     { TcSpec q; q.in = px1; q.w = L.t_ffn1; q.bias = L.ffn1.b; q.Cin = H; q.Cout = Fc; q.k = ks; q.pad = (ks - 1) / 2;
       q.epi = TCE_RELU; q.out = pff; q.pl_slope = 1.f;
-      launch_tc({q}, 1, tl, to, maxTok, B); }
+      launch_tc({q}, 1, r); }
     { TcSpec q; q.in = pff; q.w = L.t_ffn2; q.bias = L.ffn2.b; q.Cin = Fc; q.Cout = H; q.k = ks; q.pad = (ks - 1) / 2;
       q.y = y; q.ldy = H;
-      launch_tc({q}, 1, tl, to, maxTok, B); }
+      launch_tc({q}, 1, r); }
     klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, xb, y, L.ln2.g, L.ln2.b, (const float*)nullptr, va, cond_ld, x, tl, to, H, px.hi, px.lo, px.mid);
     ++launches;
   }
@@ -2071,14 +2153,13 @@ void vtts_engine::text_encoder(const float* cond, int cond_ld) {
 // Prior statistics m_p, logs_p (models.py:323-325): enc_p.proj of text_encoder's output -> d_stats [Ttok][2I].
 void vtts_engine::prior_stats() {
   const int H = cfg.hidden_channels, I = cfg.inter_channels;
-  const int* tl = d_tok_len.p;
-  const int* to = d_tok_off.p;
+  const Rows r = tok_rows();
   float* stats = ensure(d_stats, (size_t)Ttok * 2 * I);
   if (enc_on_tc) {
     TcSpec q; q.in = enc_px; q.w = tc_encproj; q.bias = enc_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
-    launch_tc({q}, 1, tl, to, maxTok, B);
+    launch_tc({q}, 1, r);
   } else {
-    launch_conv({mk(enc_proj, d_x.p, H, 0, stats, 2 * I, 0, 1, 0)}, 1, tl, to, maxTok, B);
+    launch_conv({mk(enc_proj, d_x.p, H, 0, stats, 2 * I, 0, 1, 0)}, 1, r);
   }
 }
 
@@ -2154,8 +2235,7 @@ void vtts_engine::finish1() {
       CK(cudaStreamSynchronize(stream));
       REQUIRE(*flag == call_seq, VTTS_ERR_CUDA, "phase 1 finished without publishing the utterance lengths");
     }
-    h_frm_len.assign(map.p + 1, map.p + 1 + B);
-    h_frm_off.assign(map.p + 1 + B, map.p + 1 + 2 * B + 1);
+    read_published_lengths();
     set_frame_shape();
     have_durations = true;
     return;
@@ -2179,6 +2259,7 @@ void vtts_engine::phase2(const float* noise_z, int z_ld, bool noise_on_device, b
   const int* to = d_tok_off.p;
   const int* fl = d_frm_len.p;
   const int* fo = d_frm_off.p;
+  const Rows r = frm_rows();
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
   if (noise_z && !noise_on_device) {
     // host noise was staged into h_pin_z by the caller (stage_noise_z) as [B][I][maxFrm]: the layout depends on the bucket only
@@ -2226,17 +2307,17 @@ void vtts_engine::phase2(const float* noise_z, int z_ld, bool noise_on_device, b
   }
   (void)h; (void)h1; (void)wx; (void)acts; (void)skip; (void)fy; (void)fqkv; (void)fao; (void)ffh2; (void)nl; (void)fk; (void)half;
   const float* cond = has_g ? d_condv.p : nullptr;
-  if (flow_on_tc) flow_tc(z, fl, fo, emit_pz, cond, condR, /*forward=*/false);
-  else flow_ffma(z, fl, fo, cond, condR, /*forward=*/false);
+  if (flow_on_tc) flow_tc(z, emit_pz, cond, condR, /*forward=*/false, r);
+  else flow_ffma(z, cond, condR, /*forward=*/false, r);
   if (!capturing) CK(cudaEventRecord(ev[5], stream));
 
   if (!run_decoder) return;
-  decode(z, fl, fo, /*planes_ready=*/dec_now, /*pz_ready=*/emit_pz);
+  decode(z, r, /*planes_ready=*/dec_now, /*pz_ready=*/emit_pz);
 }
 
 // Flow on the fp32 pipe (models.py:750-757).  Flip (modules.py:272-279) is folded into the packed pre/post weights: for a
 // "flipped" layer x0 lives in physical channels [half, 2*half), x1 in [0, half).  forward / cond: see flow_tc.
-void vtts_engine::flow_ffma(float* z, const int* fl, const int* fo, const float* cond, int cond_ld, bool forward) {
+void vtts_engine::flow_ffma(float* z, const float* cond, int cond_ld, bool forward, const Rows& r) {
   const vtts_config& c = cfg;
   const int H = c.hidden_channels, I = c.inter_channels, half = I / 2;
   const size_t F = (size_t)Tfrm;
@@ -2258,46 +2339,45 @@ void vtts_engine::flow_ffma(float* z, const int* fl, const int* fo, const float*
     const FlowW& W = flow[f];
     const bool flipped = ((nf - f) % 2) == 1;
     const int x0off = flipped ? half : 0, x1off = flipped ? 0 : half;
-    launch_conv({mk(W.pre, z, I, x0off, h, H, 0, 1, 0)}, 1, fl, fo, maxFrm, B);
+    launch_conv({mk(W.pre, z, I, x0off, h, H, 0, 1, 0)}, 1, r);
     float* wn_in = h;
     if (c.use_transformer_flows) {
       // h = h + Encoder(h)  (models.py:377): the layer's last LN adds `h` back and lands in wx
       float* xa = h; float* xb2 = h1;
       // encoder_layer writes its result into `xa` (== h) -- we need h preserved for the residual, so run the
       // layer on explicit buffers instead of the ping-pong helper:
-      launch_conv({mk(W.tr.qkv, h, H, 0, fqkv, 3 * H, 0, 1, 0)}, 1, fl, fo, maxFrm, B);
-      launch_attn(fqkv, fao, W.tr, H, fl, fo, maxFrm, nullptr);
-      launch_conv({mk(W.tr.o, fao, H, 0, fy, H, 0, 1, 0)}, 1, fl, fo, maxFrm, B);
-      dim3 lg((maxFrm + 3) / 4, B);
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xa, fy, W.tr.ln1.g, W.tr.ln1.b, nullptr, nullptr, 0, xb2, fl, fo, H, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
+      launch_conv({mk(W.tr.qkv, h, H, 0, fqkv, 3 * H, 0, 1, 0)}, 1, r);
+      launch_attn(fqkv, fao, W.tr, H, nullptr, r);
+      launch_conv({mk(W.tr.o, fao, H, 0, fy, H, 0, 1, 0)}, 1, r);
+      dim3 lg((r.maxLen + 3) / 4, r.n);
+      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xa, fy, W.tr.ln1.g, W.tr.ln1.b, nullptr, nullptr, 0, xb2, r.lens, r.offs, H, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
       CK(cudaGetLastError());
       ++launches;
       {
         ConvP p = mk(W.tr.ffn1, xb2, H, 0, ffh2, H, 0, 1, (fk - 1) / 2);
         p.epi = EPI_RELU;
-        launch_conv({p}, 1, fl, fo, maxFrm, B);
+        launch_conv({p}, 1, r);
       }
-      launch_conv({mk(W.tr.ffn2, ffh2, H, 0, fy, H, 0, 1, (fk - 1) / 2)}, 1, fl, fo, maxFrm, B);
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xb2, fy, W.tr.ln2.g, W.tr.ln2.b, h, nullptr, 0, wx, fl, fo, H, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
+      launch_conv({mk(W.tr.ffn2, ffh2, H, 0, fy, H, 0, 1, (fk - 1) / 2)}, 1, r);
+      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xb2, fy, W.tr.ln2.g, W.tr.ln2.b, h, nullptr, 0, wx, r.lens, r.offs, H, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
       CK(cudaGetLastError());
       ++launches;
       wn_in = wx;
     }
     // WN (modules.py:148-176).  The hidden state is updated in place in `wn_in`.
-    wn_ffma(W.in, W.rsx, W.rss, nl, fk, c.flow_dilation_rate, wn_in, acts, skip, cond ? cond + r_flow + f * nl * 2 * H : nullptr, cond_ld,
-            fl, fo);
+    wn_ffma(W.in, W.rsx, W.rss, nl, fk, c.flow_dilation_rate, wn_in, acts, skip, cond ? cond + r_flow + f * nl * 2 * H : nullptr, cond_ld, r);
     {
       // x1 <- x1 - post(h) (reverse) / x1 + post(h) (forward) (mean_only; models.py:381-391)
       ConvP p = mk(W.post, skip, H, 0, z, I, x1off, 1, 0);
       p.alpha = forward ? 1.f : -1.f;
       p.res = z; p.ldr = I; p.roff = x1off;
-      launch_conv({p}, 1, fl, fo, maxFrm, B);
+      launch_conv({p}, 1, r);
     }
   }
 }
 
 void vtts_engine::wn_ffma(const std::vector<ConvW>& in, const std::vector<ConvW>& rsx, const std::vector<ConvW>& rss, int nl, int fk,
-                          int dil_rate, float* x, float* acts, float* skip, const float* cond, int cond_ld, const int* fl, const int* fo) {
+                          int dil_rate, float* x, float* acts, float* skip, const float* cond, int cond_ld, const Rows& r) {
   const int H = cfg.hidden_channels;
   int dil = 1;
   for (int i = 0; i < nl; ++i) {
@@ -2305,24 +2385,24 @@ void vtts_engine::wn_ffma(const std::vector<ConvW>& in, const std::vector<ConvW>
       ConvP p = mk(in[i], x, H, 0, acts, H, 0, dil, dil * (fk - 1) / 2);
       p.epi = EPI_GATE;
       if (cond) { p.cond = cond + i * 2 * H; p.cond_ld = cond_ld; }
-      launch_conv({p}, 1, fl, fo, maxFrm, B);
+      launch_conv({p}, 1, r);
     }
     ConvP ps = mk(rss[i], acts, H, 0, skip, H, 0, 1, 0);
     if (i > 0) { ps.res = skip; ps.ldr = H; ps.roff = 0; }
     if (i < nl - 1) {
       ConvP px = mk(rsx[i], acts, H, 0, x, H, 0, 1, 0);
       px.res = x; px.ldr = H; px.roff = 0;
-      launch_conv({px, ps}, 1, fl, fo, maxFrm, B);
+      launch_conv({px, ps}, 1, r);
     } else {
-      launch_conv({ps}, 1, fl, fo, maxFrm, B);
+      launch_conv({ps}, 1, r);
     }
     dil *= dil_rate;
   }
 }
 
-// Decoder over the utterance rows described by (fl, fo) -- the whole batch, or one halo-extended chunk of a single
+// Decoder over the rows r -- the whole batch, or one halo-extended chunk of a single
 // utterance (vtts_decode_chunk).
-void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_ready, bool pz_ready) {
+void vtts_engine::decode(float* z, const Rows& r, bool planes_ready, bool pz_ready) {
   const vtts_config& c = cfg;
   const int I = c.inter_channels;
   const size_t F = (size_t)Tfrm;
@@ -2333,9 +2413,9 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     if (!planes_ready) {          // (chunked decoding: the decoder runs on its own)
       begin_planes();
       alloc_decoder_planes();
-      flush_tails(fl, fo);
+      flush_tails(r.lens, r.offs);
     }
-    if (decoder_tc(z, fl, fo, pz_ready)) {
+    if (decoder_tc(z, pz_ready, r)) {
       if (!capturing) CK(cudaEventRecord(ev[6], stream));
       return;
     }
@@ -2346,7 +2426,7 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     cur = ensure(d_d0, F * ch);
     ConvP p = mk(dec_pre, z, I, 0, cur, ch, 0, 1, 3);
     if (r_dec >= 0) { p.cond = d_condv.p + r_dec; p.cond_ld = condR; }     // x = conv_pre(z) + cond(g)
-    launch_conv({p}, 1, fl, fo, maxFrm, B);
+    launch_conv({p}, 1, r);
   }
   const int nk = c.n_resblock_kernels, nd = c.n_resblock_dilations;
   if ((int)d_stage.size() < c.n_upsamples) {
@@ -2361,13 +2441,13 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     float* X = ensure(d_stage[i], rows * ch2);
     for (int r0 = 0; r0 < u && cur; r0 += CV_MAXP) {
       std::vector<ConvP> ps;
-      for (int r = r0; r < std::min(u, r0 + CV_MAXP); ++r) {
-        ConvP p = mk(ups[i].phase[r], cur, ch, 0, X, ch2, 0, 1, ups[i].pad[r]);
+      for (int ph = r0; ph < std::min(u, r0 + CV_MAXP); ++ph) {
+        ConvP p = mk(ups[i].phase[ph], cur, ch, 0, X, ch2, 0, 1, ups[i].pad[ph]);
         p.pro = PRO_LRELU; p.slope = 0.1f;
-        p.out_mul = u; p.out_add = r;
+        p.out_mul = u; p.out_add = ph;
         ps.push_back(p);
       }
-      launch_conv(ps, rm, fl, fo, maxFrm, B);
+      launch_conv(ps, rm, r);
     }
     rm *= u;
     ch = ch2;
@@ -2397,9 +2477,9 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
           p1.push_back(a);
         }
       }
-      launch_conv(p1, rm, fl, fo, maxFrm, B);
+      launch_conv(p1, rm, r);
       if (c.resblock_type == 1) {
-        launch_conv(p2, rm, fl, fo, maxFrm, B);
+        launch_conv(p2, rm, r);
       } else if (d > 0) {
         for (int j = 0; j < nk; ++j) std::swap(xj[j], tmp[j]);   // ResBlock2 ping-pong (halo reads forbid in-place)
       }
@@ -2421,19 +2501,19 @@ void vtts_engine::decode(float* z, const int* fl, const int* fo, bool planes_rea
     ConvP p = mk(dec_post, cur, ch, 0, post, pc, 0, 1, 3);
     p.pro = PRO_LRELU; p.slope = 0.01f;
     p.reflect = 1; p.in_extra = 1; p.out_seq_extra = 1;
-    launch_conv({p}, rm, fl, fo, maxFrm, B);
-    const int M = maxFrm * rm * c.istft_hop;
-    dim3 g((M + TL_M - 1) / TL_M, B);
+    launch_conv({p}, rm, r);
+    const int M = r.maxLen * rm * c.istft_hop;
+    dim3 g((M + TL_M - 1) / TL_M, r.n);
     const size_t smem = ((size_t)tl_rec_frames(63, c.subbands, c.istft_n_fft, c.istft_hop) * pc + (size_t)c.subbands * (TL_M + 2 * tl_halo(63, c.subbands))) * sizeof(float);
     REQUIRE(c.istft_hop == 4 && c.istft_n_fft == 16, VTTS_ERR_INVALID, "iSTFT tail kernel is sized for n_fft=16, hop=4");
-    klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, fl, fo, wav, 0, 1, istft_w2);
+    klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, r.lens, r.offs, wav, 0, 1, istft_w2);
     CK(cudaGetLastError());
     ++launches;
   } else {
     ConvP p = mk(dec_post, cur, ch, 0, wav, 1, 0, 1, 3);
     p.pro = PRO_LRELU; p.slope = 0.01f;
     p.epi = EPI_TANH;
-    launch_conv({p}, rm, fl, fo, maxFrm, B);
+    launch_conv({p}, rm, r);
   }
   if (!capturing) CK(cudaEventRecord(ev[6], stream));
 }
@@ -2554,12 +2634,10 @@ float* vtts_engine::front_end(bool from_spec) {
 // Posterior encoder over feature rows [Tfrm][feat_ld] (models.py:836-842; QuickVC's enc_p, vc/models.py:264-271): pre ->
 // 16-layer WN (cond rows qcond, row stride qld; null: none) -> proj -> stats (d_vstats) -> z = m + eps * exp(logs) in d_z.
 // Opens the phase's plane collection (the flow's WN planes, also used here) for the frame shape.
-void vtts_engine::posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld) {
+void vtts_engine::posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld, const Rows& r) {
   const vtts_config& c = cfg;
   const int H = c.hidden_channels, I = c.inter_channels;
   const size_t F = (size_t)Tfrm;
-  const int* fl = d_frm_len.p;
-  const int* fo = d_frm_off.p;
   float* h = ensure(d_h, F * H);
   float* acts = ensure(d_acts, F * H);
   float* skip = ensure(d_skip, F * H);
@@ -2569,64 +2647,61 @@ void vtts_engine::posterior_encode(const float* feat, int feat_ld, const float* 
   if (flow_on_tc || q_tc) {
     begin_planes();
     alloc_flow_planes();                     // (enc_q uses the flow's WN planes before the flow runs)
-    flush_tails(fl, fo);
+    flush_tails(r.lens, r.offs);
   }
   {
     ConvP p = mk(q_pre, feat, feat_ld, 0, h, H, 0, 1, 0);
     if (q_tc) { p.p_hi = flp.pwx.hi; p.p_lo = flp.pwx.lo; p.ldp = H; p.pl_slope = 1.f; }
-    launch_conv({p}, 1, fl, fo, maxFrm, B);
+    launch_conv({p}, 1, r);
   }
   if (q_tc) {
-    wn_tc(qt_in, q_in, qt_rsx, q_rsx, qt_rss, q_rss, Q_LAYERS, Q_KERNEL, 1, h, skip, flp.pwx, flp.pacts, flp.pskip, qcond, qld, fl, fo);
+    wn_tc(qt_in, q_in, qt_rsx, q_rsx, qt_rss, q_rss, Q_LAYERS, Q_KERNEL, 1, h, skip, flp.pwx, flp.pacts, flp.pskip, qcond, qld, r);
     TcSpec q; q.in = flp.pskip; q.w = qt_proj; q.bias = q_proj.b; q.Cin = H; q.Cout = 2 * I; q.y = stats; q.ldy = 2 * I;
-    launch_tc({q}, 1, fl, fo, maxFrm, B);
+    launch_tc({q}, 1, r);
   } else {
-    wn_ffma(q_in, q_rsx, q_rss, Q_LAYERS, Q_KERNEL, 1, h, acts, skip, qcond, qld, fl, fo);
-    launch_conv({mk(q_proj, skip, H, 0, stats, 2 * I, 0, 1, 0)}, 1, fl, fo, maxFrm, B);
+    wn_ffma(q_in, q_rsx, q_rss, Q_LAYERS, Q_KERNEL, 1, h, acts, skip, qcond, qld, r);
+    launch_conv({mk(q_proj, skip, H, 0, stats, 2 * I, 0, 1, 0)}, 1, r);
   }
-  klaunch(posterior_sample_kernel, dim3(maxFrm, B), dim3(64), (size_t)0, (const float*)stats, I, noise, maxFrm,
-          (const float*)d_vprm.p, fl, fo, z);
+  klaunch(posterior_sample_kernel, dim3(r.maxLen, r.n), dim3(64), (size_t)0, (const float*)stats, I, noise, maxFrm,
+          (const float*)d_vprm.p, r.lens, r.offs, z);
   CK(cudaGetLastError());
   ++launches;
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vz_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
 }
 
-void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc) {
+void vtts_engine::posterior_side(bool from_spec, const float* noise, const float* csrc, const Rows& r) {
   const int I = cfg.inter_channels;
   const size_t F = (size_t)Tfrm;
   const int qld = condR + q_R;
-  const int* fl = d_frm_len.p;
-  const int* fo = d_frm_off.p;
   // ---- enc_q input rows [F][spec_pad]
   float* feat = front_end(from_spec);
   // ---- posterior encoder (models.py:836-842): pre -> 16-layer WN (g_src) -> proj -> sample
-  posterior_encode(feat, spec_pad, noise, csrc ? csrc + condR : nullptr, qld);
+  posterior_encode(feat, spec_pad, noise, csrc ? csrc + condR : nullptr, qld, r);
   float* z = d_z.p;
   // ---- z_p = flow(z, g_src)   (models.py:1715, 1640)
   const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
-  if (flow_on_tc) flow_tc(z, fl, fo, false, csrc, qld, /*forward=*/true);
-  else flow_ffma(z, fl, fo, csrc, qld, /*forward=*/true);
+  if (flow_on_tc) flow_tc(z, false, csrc, qld, /*forward=*/true, r);
+  else flow_ffma(z, csrc, qld, /*forward=*/true, r);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vzp_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
 }
 
 void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
   const float* noise = vc_upload(from_spec ? IN_SPEC : IN_WAV, eps);
+  const Rows r = frm_rows();
   // ---- g_src / g_tgt (models.py:1712-1713) and every cond row of both, one launch: src -> d_vcsrc [B][condR + q_R]
   //      (the TTS rows, then enc_q's), tgt -> d_condv [B][condR] (where the reverse flow and the decoder read them)
   const float* csrc = cond_src(/*tgt=*/true);
   const float* ctgt = d_condv.p;
-  posterior_side(from_spec, noise, csrc);
+  posterior_side(from_spec, noise, csrc, r);
   // ---- z_hat = flow^-1(z_p, g_tgt)   (models.py:1716)
-  const int* fl = d_frm_len.p;
-  const int* fo = d_frm_off.p;
   float* z = d_z.p;
   const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
-  if (flow_on_tc) flow_tc(z, fl, fo, false, ctgt, condR, /*forward=*/false);
-  else flow_ffma(z, fl, fo, ctgt, condR, /*forward=*/false);
+  if (flow_on_tc) flow_tc(z, false, ctgt, condR, /*forward=*/false, r);
+  else flow_ffma(z, ctgt, condR, /*forward=*/false, r);
   if (!capturing) CK(cudaEventRecord(ev[5], stream));
   // ---- o_hat = dec(z_hat * y_mask, g=g_tgt)   (models.py:1717)
-  decode(z, fl, fo);
+  decode(z, r);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -2656,7 +2731,7 @@ void vtts_engine::align_enqueue(bool from_spec, bool eps) {
   prior_stats();
   if (!capturing) CK(cudaEventRecord(ev[2], stream));
   // ---- z_p = flow(enc_q(y, g), g)   (models.py:1639-1640)
-  posterior_side(from_spec, noise, csrc);
+  posterior_side(from_spec, noise, csrc, frm_rows());
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
   // ---- neg_cent [B][T_y][T_x] over the frame and token buckets (models.py:1645-1651), then MAS (:1656-1660)
   const int Ty = maxFrm, Tx = maxTok;
@@ -2880,13 +2955,9 @@ std::vector<int> vtts_engine::cv_stage(const float* wav, const int64_t* lengths,
 void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   const vtts_config& c = cfg;
   const int NL = c.cv_n_conv, C = c.cv_conv_dim, H = c.cv_hidden, Fh = c.cv_ffn, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
-  // The tensor-core GEMMs run without split-K (every output summed by one CTA in one k order, whatever its launch shape) and
-  // attention on attn_tc_kernel whenever it takes the layer: a clip's units are then the same alone and in any batch.
-  SavedLaunch saved(this);
-  if (cv_tc) {
-    tc_split = 1;
-    if (attn_tc_mode > 0) attn_tc_mode = 2;
-  }
+  // Tensor-core GEMMs without split-K and attention on attn_tc_kernel (Tuning::fixed_tc): a clip's units are then the same
+  // alone and in any batch.
+  const Tuning tn = cv_tc ? tune.fixed_tc() : tune;
   const size_t head = ((size_t)cvp.nint * sizeof(int) + 63) / 64 * 64;
   const size_t nsamp = (size_t)cvp.tot0 * s0 + K0;
   int* di = ensure(d_cvi, cvp.nint);
@@ -2897,6 +2968,8 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   auto Os = [&](int l) -> const int* { return di + (NL + l) * B; };
   const int* woff = di + 2 * NL * B;
   const float* mu = reinterpret_cast<const float*>(di + (2 * NL + 1) * B);
+  // the rows of level l; the launch heuristics and the profiler see each clip at the level's bucket
+  auto level = [&](int l) { return Rows{Ls(l), Os(l), B, cvp.maxL[l], std::vector<int>(B, cvp.maxL[l]), std::vector<int>(B, cvp.maxL[l]), tn}; };
   const size_t np = (size_t)B * cvp.MC * C;
   float* ps = ensure(d_cvps, np);
   float* pq = ensure(d_cvpq, np);
@@ -2919,15 +2992,14 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   float* x = lv[0];
   for (int i = 1; i < NL; ++i) {
     float* y = lv[i & 1];
-    v_frm_len.assign(B, cvp.maxL[i]);
-    h_frm_len = v_frm_len;
-    launch_conv({mk(cv_conv[i], x, c.cv_conv_stride[i] * C, 0, y, C, 0, 1, 0)}, 1, Ls(i), Os(i), cvp.maxL[i], B);
+    launch_conv({mk(cv_conv[i], x, c.cv_conv_stride[i] * C, 0, y, C, 0, 1, 0)}, 1, level(i));
     gelu(y, C, Ls(i), Os(i), cvp.maxL[i], nullptr);
     x = y;
   }
   const int* Lf = Ls(NL - 1);
   const int* Of = Os(NL - 1);
   const int maxF = cvp.maxL[NL - 1];
+  const Rows rf = level(NL - 1);
   const size_t Tf = (size_t)cvp.tot0 / cv_P;
   float *X = ensure(d_cvx, Tf * H), *X1 = ensure(d_cvx1, Tf * H), *Y = ensure(d_cvy, Tf * H), *QKV = ensure(d_cvqkv, Tf * 3 * H);
   float *AO = ensure(d_cvao, Tf * std::max(H, C)), *FF = ensure(d_cvff, Tf * Fh);
@@ -2951,11 +3023,11 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
     s.in = in; s.w = w; s.bias = cw.b; s.Cin = cw.Cin; s.Cout = cw.Cout;
     s.y = y; s.ldy = cw.Cout; s.res = res; s.ldr = res ? cw.Cout : 0; s.epi = epi;
     if (out) s.out = *out;
-    launch_tc({s}, 1, Lf, Of, maxF, B);
+    launch_tc({s}, 1, rf);
   };
   ln(x, nullptr, cv_fp_g, cv_fp_b, AO, Of, C, cv_tc ? &P512 : nullptr);
   if (cv_tc) gemm(P512, cv_tfp, cv_fp, X, nullptr, nullptr, 0);
-  else launch_conv({mk(cv_fp, AO, C, 0, X, H, 0, 1, 0)}, 1, Lf, Of, maxF, B);
+  else launch_conv({mk(cv_fp, AO, C, 0, X, H, 0, 1, 0)}, 1, rf);
   const int G = c.cv_pos_groups, Cg = H / G, kh = c.cv_pos_k / 2;
   for (int half = 0; half < 2; ++half)
     for (int g0 = 0; g0 < G; g0 += CV_MAXP) {
@@ -2969,7 +3041,7 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
         if (half) { p.res = Y; p.ldr = H; p.roff = g * Cg; }
         pp.push_back(p);
       }
-      launch_conv(pp, 1, Lf, Of, maxF, B);
+      launch_conv(pp, 1, rf);
     }
   ln(X, Y, cv_enc_g, cv_enc_b, X1, Of, H, cv_tc ? &PX : nullptr);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_cvdbg, Tf * H), X1, Tf * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -2977,8 +3049,8 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   for (size_t l = 0; l < cv_enc.size() && cv_tc; ++l) {
     const EncLayerW& Lw = cv_enc[l];
     gemm(PX, Lw.t_qkv, Lw.qkv, QKV, nullptr, &PQKV, 0);
-    if (attn_use_tc(Lw, H, Lf, maxF)) launch_attn_tc(PQKV, AO, &PAO, Lw, H, Lf, Of, maxF);
-    else launch_attn(QKV, AO, Lw, H, Lf, Of, maxF, &PAO);
+    if (attn_use_tc(Lw, H, rf)) launch_attn_tc(PQKV, AO, &PAO, Lw, H, rf);
+    else launch_attn(QKV, AO, Lw, H, &PAO, rf);
     gemm(PAO, Lw.t_o, Lw.o, Y, xa, nullptr, 0);
     ln(Y, nullptr, Lw.ln1.g, Lw.ln1.b, xb, Of, H, &PX1);
     gemm(PX1, Lw.t_ffn1, Lw.ffn1, FF, nullptr, nullptr, 0);
@@ -2989,17 +3061,17 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   }
   for (size_t l = 0; l < cv_enc.size() && !cv_tc; ++l) {
     const EncLayerW& Lw = cv_enc[l];
-    launch_conv({mk(Lw.qkv, xa, H, 0, QKV, 3 * H, 0, 1, 0)}, 1, Lf, Of, maxF, B);
-    launch_attn(QKV, AO, Lw, H, Lf, Of, maxF, nullptr);
+    launch_conv({mk(Lw.qkv, xa, H, 0, QKV, 3 * H, 0, 1, 0)}, 1, rf);
+    launch_attn(QKV, AO, Lw, H, nullptr, rf);
     ConvP po = mk(Lw.o, AO, H, 0, Y, H, 0, 1, 0);
     po.res = xa; po.ldr = H;
-    launch_conv({po}, 1, Lf, Of, maxF, B);
+    launch_conv({po}, 1, rf);
     ln(Y, nullptr, Lw.ln1.g, Lw.ln1.b, xb, Of, H, nullptr);
-    launch_conv({mk(Lw.ffn1, xb, H, 0, FF, Fh, 0, 1, 0)}, 1, Lf, Of, maxF, B);
+    launch_conv({mk(Lw.ffn1, xb, H, 0, FF, Fh, 0, 1, 0)}, 1, rf);
     gelu(FF, Fh, Lf, Of, maxF, nullptr);
     ConvP p2 = mk(Lw.ffn2, FF, Fh, 0, Y, H, 0, 1, 0);
     p2.res = xb; p2.ldr = H;
-    launch_conv({p2}, 1, Lf, Of, maxF, B);
+    launch_conv({p2}, 1, rf);
     if (l + 1 == cv_enc.size()) ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, out, out_offs ? out_offs : Of, H, nullptr);
     else ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, xa, Of, H, nullptr);
   }
@@ -3124,36 +3196,37 @@ vtts_engine::StPin vtts_engine::st_layout() {
 // modulated LayerNorm -> qkv 1x1 -> rotary -> attention (zero relative tables) -> out 1x1 -> gated residual + modulated
 // LayerNorm -> conv -> SiLU -> conv -> gated residual; x rows at xin (pitch ldi) -> xout (pitch ldo).  film: the FiLM rows
 // DitWrapper applies first (decoder.py:15-18), or null for the text encoder's plain blocks.
-void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap) {
+void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap,
+                           const Rows& r) {
   const int H = k.H, F = k.F, dk = H / k.heads;
   const size_t T = (size_t)stp.Ttot;
-  const dim3 gs(k.maxLen, k.NS), gn((k.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, k.NS);
+  const dim3 gs(r.maxLen, r.n), gn((r.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, r.n);
   const float* ada = k.ada + (size_t)l * 6 * H;
   auto norm = [&](const float* a, int lda, const float* fl, const float* y, int gate, int shift, int scale) {
     klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f, k.Hb, k.N,
-            k.lens, k.offs, H);
+            r.lens, r.offs, H);
     CK(cudaGetLastError());
     ++launches;
   };
   auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy) {
-    launch_conv({mk(W, x, ldx, 0, y, ldy, 0, 1, (W.k - 1) / 2)}, 1, k.lens, k.offs, k.maxLen, k.NS);
+    launch_conv({mk(W, x, ldx, 0, y, ldy, 0, 1, (W.k - 1) / 2)}, 1, r);
   };
   norm(xin, ldi, film, nullptr, 2, 0, 1);
   if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_n, T * H), k.N, T * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   cv(L.qkv, k.N, H, k.QKV, 3 * H);
-  klaunch(dit_rope_kernel, gs, dim3(128), (size_t)0, k.QKV, k.rope, k.heads, dk, k.rd, k.lens, k.offs);
+  klaunch(dit_rope_kernel, gs, dim3(128), (size_t)0, k.QKV, k.rope, k.heads, dk, k.rd, r.lens, r.offs);
   CK(cudaGetLastError());
   ++launches;
   if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_qkv, T * 3 * H), k.QKV, T * 3 * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  launch_attn(k.QKV, k.AO, L, H, k.lens, k.offs, k.maxLen, nullptr);
+  launch_attn(k.QKV, k.AO, L, H, nullptr, r);
   cv(L.o, k.AO, H, k.Y, H);
   norm(k.Hb, H, nullptr, k.Y, 2, 3, 4);
   cv(L.ffn1, k.N, H, k.FF, F);
-  klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, k.FF, F, k.lens, k.offs);
+  klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, k.FF, F, r.lens, r.offs);
   CK(cudaGetLastError());
   ++launches;
   cv(L.ffn2, k.FF, F, k.Y, H);
-  klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, k.lens, k.offs, H);
+  klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, r.lens, r.offs, H);
   CK(cudaGetLastError());
   ++launches;
 }
@@ -3169,12 +3242,6 @@ void vtts_engine::st_enqueue() {
   const vtts_config& c = cfg;
   const int NC = c.st_noise, MC = c.st_cond, H = c.st_hidden, F = c.st_filter, NL = c.st_layers, G = c.st_spk_dim;
   const int NS = stp.NS, Bu = B, XW = NC + H, dk = H / c.st_heads, rd = dk / 2, nlsc = NL / 2;
-  // One fixed launch shape for every conv (no split-K over a cluster or thread groups) and one attention kernel: every row is
-  // summed in the same order whatever the batch, so an utterance's mel does not depend on what it is batched with.
-  SavedLaunch saved(this);
-  struct Restore { vtts_engine* e; int B, rows; ~Restore() { e->B = B; e->attn_rows = rows; } } restore{this, B, attn_rows};
-  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
-  attn_rows = 4;
   StPin pp = st_layout();
   const size_t T = (size_t)stp.Ttot;
   int* di = ensure(d_sti, 4 * NS);
@@ -3190,13 +3257,14 @@ void vtts_engine::st_enqueue() {
   }
   const int *lens = di, *offs = di + NS, *sid = di + 2 * NS, *exts = di + 3 * NS;
   const float *prm = df, *ts = df + 16, *dts = df + 16 + VTTS_CFM_MAX_STEPS;
-  B = NS;                                           // launch_attn and the launch heuristics read the member
-  v_frm_len.assign(NS, maxFrm);
-  {
-    std::vector<int> two(h_frm_len.begin(), h_frm_len.begin() + Bu);
-    if (stp.guided) two.insert(two.end(), h_frm_len.begin(), h_frm_len.begin() + Bu);
-    h_frm_len = two;
-  }
+  // The NS sequences in one fixed launch shape for every conv and one attention kernel (Tuning::fixed_ffma, fixed_attention):
+  // every row is summed in the same order whatever the batch, so an utterance's mel does not depend on what it is batched with.
+  // The heuristics see every sequence at the bucket, the profiler the unconditional branches at their conditional twins' lengths.
+  Rows rl{lens, offs, NS, maxFrm, std::vector<int>(NS, maxFrm), std::vector<int>(h_frm_len.begin(), h_frm_len.begin() + Bu),
+          tune.fixed_ffma().fixed_attention()};
+  if (stp.guided) rl.real.insert(rl.real.end(), h_frm_len.begin(), h_frm_len.begin() + Bu);
+  Rows re = rl;                                     // the same rows over the extents
+  re.lens = exts;
   float* film = ensure(d_stfilm, (size_t)VTTS_CFM_MAX_STEPS * NL * 2 * H);
   float* ada = ensure(d_stada, (size_t)NS * NL * 6 * H);
   float2* rope = reinterpret_cast<float2*>(ensure(d_strope, (size_t)maxFrm * rd));
@@ -3204,7 +3272,7 @@ void vtts_engine::st_enqueue() {
   float* cat[4];
   for (int j = 0; j < nlsc; ++j) cat[j] = ensure(d_stcat[j], T * 2 * H);
   float *X = ensure(d_stx, T * H), *X2 = ensure(d_stx2, T * H);
-  StBlk kb{H, F, c.st_heads, rd, maxFrm, NS, NL * 6 * H, lens, offs, rope, ada,
+  StBlk kb{H, F, c.st_heads, rd, NL * 6 * H, rope, ada,
            ensure(d_sth, T * H), ensure(d_stn, T * H), ensure(d_stqkv, T * 3 * H), ensure(d_stao, T * H), ensure(d_sty, T * H), ensure(d_stff, T * F)};
   float *V = ensure(d_stv, T * NC), *mel = ensure(d_stmel, (size_t)Tfrm * NC * (stp.prior ? 2 : 1));
   const dim3 gs(maxFrm, NS);
@@ -3228,23 +3296,23 @@ void vtts_engine::st_enqueue() {
     CK(cudaGetLastError());
     ++launches;
   };
-  auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff, const int* ln) {
-    launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, ln, offs, maxFrm, NS);
+  auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff, const Rows& r) {
+    launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, r);
   };
   // cond_proj (decoder.py:121; not masked: zero padded at the ends of each sequence's extent) into the cond columns of the
   // in_proj operand
-  cv(st_cp[0], mu, MC, p0, F, 0, exts);
+  cv(st_cp[0], mu, MC, p0, F, 0, re);
   silu(p0, F);
-  cv(st_cp[1], p0, F, p1, F, 0, exts);
+  cv(st_cp[1], p0, F, p1, F, 0, re);
   silu(p1, F);
-  cv(st_cp[2], p1, F, xc, XW, NC, exts);
+  cv(st_cp[2], p1, F, xc, XW, NC, re);
   // DitWrapper (decoder.py:15-18) of block l at step s
   auto block = [&](int l, int s, const float* xin, int ldi, float* xout, int ldo) {
-    st_block(kb, st_blk[l], l, film + ((size_t)s * NL + l) * 2 * H, xin, ldi, xout, ldo, (debug_flags & 1) && l == 0 && s == 0);
+    st_block(kb, st_blk[l], l, film + ((size_t)s * NL + l) * 2 * H, xin, ldi, xout, ldo, (debug_flags & 1) && l == 0 && s == 0, rl);
   };
   for (int s = 0; s < stp.steps; ++s) {
     // in_proj over (x | cond) (decoder.py:123-124; not masked: over the extent) -> the skip half of the last long-skip operand
-    cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H, exts);
+    cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H, re);
     // blocks 0 .. NL/2-1 leave their input as a skip (decoder.py:130-131): block i reads the skip half of cat[nlsc-1-i] and
     // writes the skip half of the next one; the last of them writes the x half of cat[0]
     for (int i = 0; i < nlsc; ++i)
@@ -3253,10 +3321,10 @@ void vtts_engine::st_enqueue() {
     // in_proj's output, whose rows past the length its taps read: its input rows are the extent's (the x half is zero there)
     for (int j = 0; j < nlsc; ++j) {
       const bool last = j + 1 == nlsc;
-      cv(st_lsc[j], cat[j], 2 * H, X, H, 0, last ? exts : lens);
+      cv(st_lsc[j], cat[j], 2 * H, X, H, 0, last ? re : rl);
       block(nlsc + j, s, X, H, last ? X2 : cat[j + 1], last ? H : 2 * H);
     }
-    cv(st_final, X2, H, V, NC, 0, lens);
+    cv(st_final, X2, H, V, NC, 0, rl);
     const bool end = s + 1 == stp.steps;
     klaunch(dit_euler_kernel, dim3(maxFrm, Bu), dim3(128), (size_t)0, (const float*)V, xc, XW, NC, dts + s, prm, stp.guided ? 1 : 0,
             end ? mel : (float*)nullptr, st_mel_mean, st_mel_std, lens, offs, Bu);
@@ -3291,12 +3359,6 @@ void vtts_engine::stt_enqueue(bool prior) {
   const vtts_config& c = cfg;
   const int MC = c.st_cond, H = c.st_enc_hidden, F = c.st_enc_filter, NE = c.st_enc_layers, G = c.st_spk_dim, S = c.st_streams;
   const int dk = H / c.st_enc_heads, rd = dk / 2, DC = c.st_dur_channels, NC = c.st_noise;
-  SavedLaunch saved(this);
-  struct Restore { vtts_engine* e; int rows; ~Restore() { e->attn_rows = rows; } } restore{this, attn_rows};
-  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;   // the decoder's fixed launch shape: durations do not depend on the batch
-  attn_rows = 4;
-  v_frm_len.assign(B, maxTok);
-  h_frm_len = h_tok_len;
   SttPin pp = stt_layout();
   const size_t T = (size_t)Ttok, ni = (size_t)3 * B + (size_t)S * T;
   int* di = ensure(d_stti, ni);
@@ -3306,13 +3368,15 @@ void vtts_engine::stt_enqueue(bool prior) {
   CK(cudaMemcpyAsync(df, pp.prm, (16 + T) * sizeof(float), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(bert, pp.bert, T * c.st_bert_dim * sizeof(float), cudaMemcpyHostToDevice, stream));
   const int *lens = di, *offs = di + B, *sid = di + 2 * B, *ids = di + 3 * B;
+  // the decoder's fixed launch shape, every token row sized at the bucket: durations do not depend on the batch
+  const Rows r{lens, offs, B, maxTok, std::vector<int>(B, maxTok), h_tok_len, tune.fixed_ffma().fixed_attention()};
   float* x = ensure(d_sttx, T * MC);
   float2* rope = reinterpret_cast<float2*>(ensure(d_sttrope, (size_t)maxTok * rd));
   float* ada = ensure(d_sttada, (size_t)B * NE * 6 * H);
   float *e0 = ensure(d_stte[0], T * H), *e1 = ensure(d_stte[1], T * H);
   float *mu_mel = ensure(d_stmumel, T * NC), *mu_dp = ensure(d_stmudp, T * DC), *logw = ensure(d_stlogw, T);
   int* dd = ensure(d_sttd, 2 * T + B);
-  StBlk kb{H, F, c.st_enc_heads, rd, maxTok, B, NE * 6 * H, lens, offs, rope, ada,
+  StBlk kb{H, F, c.st_enc_heads, rd, NE * 6 * H, rope, ada,
            ensure(d_sth, T * H), ensure(d_stn, T * H), ensure(d_stqkv, T * 3 * H), ensure(d_stao, T * H), ensure(d_sty, T * H), ensure(d_stff, T * F)};
   klaunch(stt_front_kernel, dim3(maxTok, B), dim3(256), (size_t)0, ids, Ttok, (const float*)bert, st_tok_emb, (float)std::sqrt((double)c.st_emb_dim),
           st_punc_emb, (float)std::sqrt((double)c.st_punc_dim), st_bert_w, st_bert_b, S, c.st_emb_dim, c.st_punc_dim, c.st_bert_dim, c.st_bert_proj,
@@ -3329,10 +3393,10 @@ void vtts_engine::stt_enqueue(bool prior) {
     const float* in = x;
     for (int l = 0; l < NE; ++l) {
       float* out = l % 2 ? e1 : e0;
-      st_block(kb, W.blk[l], l, nullptr, in, H, out, H, false);
+      st_block(kb, W.blk[l], l, nullptr, in, H, out, H, false, r);
       in = out;
     }
-    launch_conv({mk(W.proj, in, H, 0, e == 0 ? mu_mel : mu_dp, e == 0 ? NC : DC, 0, 1, 0)}, 1, lens, offs, maxTok, B);
+    launch_conv({mk(W.proj, in, H, 0, e == 0 ? mu_mel : mu_dp, e == 0 ? NC : DC, 0, 1, 0)}, 1, r);
   }
   klaunch(stt_dur_kernel, dim3(B), dim3(STT_SCAN), (size_t)0, (const float*)mu_dp, DC, DC, (const float*)(df + 16), (const float*)df,
           (float)VTTS_ST_MAX_TOKEN_FRAMES, dd, dd + Ttok, dd + 2 * Ttok, logw, lens, offs);
@@ -3356,19 +3420,19 @@ void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int ma
   int NS = 1, li = 0;
   while (NS < 8 && (ns + NS - 1) / NS > spk_clusters[li]) { NS *= 2; ++li; }
   const int groups = (ns + NS - 1) / NS;
-  // The projections run with one fixed launch shape (no split-K across CTAs or thread groups), so every row is summed in the
-  // same order whatever the batch: a clip's g does not depend on the clips it is batched with.  Layers 1 and 2 launch over
-  // the slices, so the host-side lengths the launch heuristics read are the slices' for those launches.
-  SavedLaunch saved(this);
-  conv_max_s = 1; conv_min_g = 1; conv_big_g = 1; conv_auto_g = 0;
+  // The projections run with one fixed launch shape (Tuning::fixed_ffma), so every row is summed in the same order whatever
+  // the batch: a clip's g does not depend on the clips it is batched with.  Layer 0 runs over the frames, layers 1 and 2 over
+  // the slices.
+  Rows rf = frm_rows();
+  rf.tune = tune.fixed_ffma();
   const std::vector<int> slen_h(seq.begin() + ns, seq.begin() + 2 * ns);
+  const Rows rs{slen, soff, ns, max_len, slen_h, slen_h, rf.tune};
   const float* x = feat;
   for (int l = 0; l < 3; ++l) {
-    if (l == 1) { v_frm_len = slen_h; h_frm_len = slen_h; }
     float* xp = ensure(d_sx[l], (size_t)(l == 0 ? Tfrm : spk_rows) * SPK_GATES);
     float* hs = ensure(d_sh[l], (size_t)spk_rows * SPK_H);
-    if (l == 0) launch_conv({mk(spk_ih[0], x, spec_pad, 0, xp, SPK_GATES, 0, 1, 0)}, 1, d_frm_len.p, d_frm_off.p, maxFrm, B);
-    else launch_conv({mk(spk_ih[l], x, SPK_H, 0, xp, SPK_GATES, 0, 1, 0)}, 1, slen, soff, max_len, ns);
+    if (l == 0) launch_conv({mk(spk_ih[0], x, spec_pad, 0, xp, SPK_GATES, 0, 1, 0)}, 1, rf);
+    else launch_conv({mk(spk_ih[l], x, SPK_H, 0, xp, SPK_GATES, 0, 1, 0)}, 1, rs);
     const int* xr = l == 0 ? xrow : soff;
     const dim3 grid(groups * SPK_CTAS), blk(SPK_THREADS);
     switch (NS) {
@@ -3395,8 +3459,8 @@ void vtts_engine::quickvc_enqueue(bool eps, bool from_wav) {
   const int G = cfg.gin_channels;
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
   const float* noise = vc_upload(from_wav ? IN_NONE : IN_UNITS, eps);
-  const int* fl = d_frm_len.p;
   const int* fo = d_frm_off.p;
+  const Rows r = frm_rows();
   float* units = ensure(d_vin, (size_t)Tfrm * QV_UNITS);       // unit rows, packed as the engine's rows
   if (from_wav) {      // ContentVec writes the unit rows; the gaps between clips and the bucket's tail stay zero
     CK(cudaMemsetAsync(units, 0, (size_t)Tfrm * QV_UNITS * sizeof(float), stream));
@@ -3410,15 +3474,15 @@ void vtts_engine::quickvc_enqueue(bool eps, bool from_wav) {
   CK(cudaGetLastError());
   ++launches;
   // ---- z_p, m_p, logs_p = enc_p(c)   (models.py:868)
-  posterior_encode(units, QV_UNITS, noise, nullptr, 0);
+  posterior_encode(units, QV_UNITS, noise, nullptr, 0, r);
   // ---- z = flow(z_p, g, reverse=True)   (models.py:869)
   float* z = d_z.p;
   const bool flow_on_tc = tc && !flow.empty() && !flow[0].t_in.empty();
-  if (flow_on_tc) flow_tc(z, fl, fo, false, cond, condR, /*forward=*/false);
-  else flow_ffma(z, fl, fo, cond, condR, /*forward=*/false);
+  if (flow_on_tc) flow_tc(z, false, cond, condR, /*forward=*/false, r);
+  else flow_ffma(z, cond, condR, /*forward=*/false, r);
   if (!capturing) CK(cudaEventRecord(ev[5], stream));
   // ---- o = dec(z * c_mask, g)   (models.py:870)
-  decode(z, fl, fo);
+  decode(z, r);
 }
 
 // ===================================================================================================
@@ -4056,27 +4120,21 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
   st_check_sampling(n, temperature, s);
   REQUIRE(std::isfinite(length_scale) && length_scale > 0.f && length_scale <= 100.f, VTTS_ERR_INVALID, "length_scale must be in (0, 100]");
   const int S = c.st_streams, BD = c.st_bert_dim, NC = c.st_noise;
-  h->B = B;
-  h->have_durations = false;
-  h->have_latent = false;
-  h->h_tok_len.resize(B);
   for (int b = 0; b < B; ++b) {
     REQUIRE(id_lengths[b] >= 1 && id_lengths[b] <= t_max, VTTS_ERR_INVALID, "id_lengths must be in [1, t_max]");
     REQUIRE(sid[b] >= 0 && sid[b] < c.st_n_spks, VTTS_ERR_INVALID, "speaker id out of range [0, n_spks)");
-    h->h_tok_len[b] = (int)id_lengths[b];
     for (int q = 0; q < S; ++q)
-      for (int i = 0; i < h->h_tok_len[b]; ++i) {
+      for (int64_t i = 0; i < id_lengths[b]; ++i) {
         const int64_t v = ids[((size_t)b * S + q) * t_max + i];
         REQUIRE(v >= 0 && v < c.st_n_vocab, VTTS_ERR_INVALID, "token id out of range [0, n_vocab)");
       }
     if (pause)
-      for (int i = 0; i < h->h_tok_len[b]; ++i) {
+      for (int64_t i = 0; i < id_lengths[b]; ++i) {
         const float v = pause[(size_t)b * t_max + i];
         REQUIRE(v >= 0.f && v <= (float)VTTS_ST_MAX_TOKEN_FRAMES, VTTS_ERR_INVALID, "pause durations must be in [0, VTTS_ST_MAX_TOKEN_FRAMES]");
       }
   }
-  vtts_engine::pack_rows(h->h_tok_len, h->h_tok_off);
-  h->set_token_shape();
+  setup_lengths(h, id_lengths, B, (int)t_max);
   const int Ttok = h->Ttok;
   {
     const vtts_engine::SttPin pp = h->stt_layout();
@@ -4436,27 +4494,9 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
       REQUIRE(off + n <= blob_floats, VTTS_ERR_WEIGHTS, "manifest entry exceeds the blob");
       h->tensors[name] = Tensor{h->d_blob.p + off, (size_t)n};
     }
-    if (const char* e = getenv("VTTS_CONV_MAXS")) h->conv_max_s = std::max(1, atoi(e));
-    if (const char* e = getenv("VTTS_CONV_TARGET")) h->conv_target = std::max(1, atoi(e));
-    if (const char* e = getenv("VTTS_CONV_MAXG")) h->conv_max_g = std::max(1, std::min(4, atoi(e)));
-    if (const char* e = getenv("VTTS_CONV_BIGG")) h->conv_big_g = std::max(1, std::min(4, atoi(e)));   // thread groups per CTA on machine-filling FFMA launches
-    if (const char* e = getenv("VTTS_TC_TALL")) h->tc_tall = atoi(e);
-    if (const char* e = getenv("VTTS_TC_BASEOFF")) h->tc_baseoff = atoi(e);
-    if (const char* e = getenv("VTTS_TC_BN")) h->tc_bn = atoi(e);
-    if (const char* e = getenv("VTTS_TC_MULTICAST")) h->tc_mc = atoi(e);
-    if (const char* e = getenv("VTTS_TC_SPLIT")) h->tc_split = atoi(e);
-    if (const char* e = getenv("VTTS_TC_MINSTEPS")) h->tc_min_steps = std::max(1, atoi(e));   // k-steps per CTA below which split-K stops
-    if (const char* e = getenv("VTTS_TC_PERSIST")) h->tc_persist = atoi(e);                 // 0: one tile per CTA also on machine-filling launches; 2: persistent grid on every launch without split-K (tests)
-    if (const char* e = getenv("VTTS_TC_DBGSKIP")) h->tc_dbgskip = atoi(e);                 // timing experiments only (wrong results)
-    if (const char* e = getenv("VTTS_TC_WMC")) h->tc_wmc = atoi(e);                         // 1: weight-tile multicast between CTA pairs of persistent launches (measured neutral, off)
-    if (const char* e = getenv("VTTS_TC_PERSIST_MIN")) h->tc_persist_min = std::max(1, atoi(e));   // tiles per SM from which the persistent grid is used
+    h->tune = Tuning::from_env();
     if (const char* e = getenv("VTTS_MRF_BRANCH")) h->mrf_branch = atoi(e);
     if (const char* e = getenv("VTTS_MRF_HEAVY_FIRST")) h->mrf_heavy_first = atoi(e);
-    if (const char* e = getenv("VTTS_ATTN_SPLIT")) h->attn_split = atoi(e);       // 0: never use the split-KV attention
-    if (const char* e = getenv("VTTS_CONV_AUTOG")) h->conv_auto_g = std::max(0, atoi(e));   // k-steps per rank needed to add thread groups; 0 = never
-    if (const char* e = getenv("VTTS_CONV_MING")) h->conv_min_g = std::max(1, std::min(4, atoi(e)));      // 0 auto, 1 off, 2/4/8 cap
-    if (const char* e = getenv("VTTS_ATTN_ROWS")) h->attn_rows = atoi(e);
-    if (const char* e = getenv("VTTS_ATTN_TC")) h->attn_tc_mode = atoi(e);
     if (const char* e = getenv("VTTS_PDL")) h->use_pdl = atoi(e) != 0;
     if (const char* e = getenv("VTTS_NO_POLL")) h->use_poll = atoi(e) == 0;
     if (const char* e = getenv("VTTS_NO_GRAPHS")) h->use_graphs = atoi(e) == 0;
@@ -4614,22 +4654,11 @@ int vtts_decode_chunk(vtts_handle h, int f0, int f1, float* wav, int64_t wav_cap
     int* pin = reinterpret_cast<int*>(h->ensure(h->h_pin_len, 64));
     pin[0] = hi - lo; pin[1] = lo; pin[2] = hi;
     CK(cudaMemcpyAsync(dc, pin, 3 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    // the launch helpers size grids and split-K from the host copies of the lengths: point them at the chunk
-    // (the planes keep the full utterance's row count, Tfrm: the chunk is addressed by its absolute rows)
-    const std::vector<int> len0 = h->h_frm_len, off0 = h->h_frm_off, v0 = h->v_frm_len;
-    const int max0 = h->maxFrm;
-    h->h_frm_len.assign(1, hi - lo);
-    h->h_frm_off = {lo, hi};
-    h->v_frm_len = h->h_frm_len;
-    h->maxFrm = hi - lo;
-    try {
-      h->last_graphed = false;
-      h->decode(h->d_z.p, dc, dc + 1);
-    } catch (...) {
-      h->h_frm_len = len0; h->h_frm_off = off0; h->maxFrm = max0; h->v_frm_len = v0;
-      throw;
-    }
-    h->h_frm_len = len0; h->h_frm_off = off0; h->maxFrm = max0; h->v_frm_len = v0;
+    // the launches size grids and split-K for the chunk (the planes keep the full utterance's row count, Tfrm: the chunk is
+    // addressed by its absolute rows)
+    const Rows r{dc, dc + 1, 1, hi - lo, {hi - lo}, {hi - lo}, h->tune};
+    h->last_graphed = false;
+    h->decode(h->d_z.p, r);
     const size_t n = (size_t)(f1 - f0) * h->hop;
     float* pw = reinterpret_cast<float*>(h->ensure_pinned(n * sizeof(float)));
     CK(cudaMemcpyAsync(pw, h->d_wav.p + (size_t)f0 * h->hop, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
@@ -4957,37 +4986,23 @@ int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* len
       maxLen = std::max(maxLen, ll[b]);
     }
     REQUIRE((long)rows >= off[B], VTTS_ERR_INVALID, "debug_attention: qkv has fewer rows than the packed utterances");
-    // ---- per-call engine state the launch code reads, restored on every exit
-    struct Saved {
-      vtts_engine* h;
-      int B, maxFrm, maxTok, tc_mode, split, arows;
-      std::vector<int> fl, tl, vf, vt;
-      explicit Saved(vtts_engine* e) : h(e), B(e->B), maxFrm(e->maxFrm), maxTok(e->maxTok), tc_mode(e->attn_tc_mode),
-          split(e->attn_split), arows(e->attn_rows), fl(e->h_frm_len), tl(e->h_tok_len), vf(e->v_frm_len), vt(e->v_tok_len) {}
-      ~Saved() {
-        h->B = B; h->maxFrm = maxFrm; h->maxTok = maxTok; h->attn_tc_mode = tc_mode; h->attn_split = split; h->attn_rows = arows;
-        h->h_frm_len = fl; h->h_tok_len = tl; h->v_frm_len = vf; h->v_tok_len = vt;
-      }
-    } saved(h);
-    h->B = B; h->maxFrm = maxLen; h->maxTok = maxLen;
-    h->h_frm_len.assign(lens, lens + B); h->h_tok_len = h->h_frm_len;
-    h->v_frm_len = ll; h->v_tok_len = ll;           // the heuristics see the launch lengths
+    // planes() and flush_tails() read the member B: restored on every exit
+    struct KeepB { vtts_engine* h; int B; ~KeepB() { h->B = B; } } keep{h, h->B};
+    h->B = B;
+    // the heuristics see the launch lengths; the device lengths are set below
+    Rows r{nullptr, nullptr, B, maxLen, ll, std::vector<int>(lens, lens + B), h->tune.with_attention(kernel)};
     // ---- kernel selection (refused before anything is launched)
     bool use_tc = false;
     switch (kernel) {
-      case VTTS_ATTN_AUTO: use_tc = h->attn_use_tc(*L, H, nullptr, maxLen); break;
+      case VTTS_ATTN_AUTO: use_tc = h->attn_use_tc(*L, H, r); break;
       case VTTS_ATTN_TC:
-        h->attn_tc_mode = 2;
-        REQUIRE(h->attn_tc_ok(*L, H), VTTS_ERR_INVALID, "debug_attention: tensor-core attention is not available for this layer (relative tables / window)");
+        REQUIRE(h->attn_tc_ok(*L, H, r.tune), VTTS_ERR_INVALID, "debug_attention: tensor-core attention is not available for this layer (relative tables / window)");
         use_tc = true;
         break;
       case VTTS_ATTN_SPLIT:
-        h->attn_split = 1; h->attn_rows = 1;
-        REQUIRE(h->attn_split_fits(*L, H, nullptr, maxLen), VTTS_ERR_INVALID, "debug_attention: the split-KV kernel does not fit this launch");
+        REQUIRE(h->attn_split_fits(*L, H, r), VTTS_ERR_INVALID, "debug_attention: the split-KV kernel does not fit this launch");
         break;
-      case VTTS_ATTN_R1: h->attn_split = 0; h->attn_rows = 1; break;
-      case VTTS_ATTN_R4: h->attn_split = 0; h->attn_rows = 4; break;
-      default: break;                               // VTTS_ATTN_FFMA: launch_attn's own choice
+      default: break;                               // R1 / R4 / FFMA: launch_attn's choice under that tuning
     }
     REQUIRE(!(use_tc && planes && p_planes != 2), VTTS_ERR_INVALID, "debug_attention: the tensor-core kernel writes 2 output planes");
     // ---- device copies
@@ -5001,6 +5016,7 @@ int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* len
     int* dl = static_cast<int*>(upload(dev, lo.data(), lo.size() * sizeof(int), st));
     const int* dlens = dl;
     const int* doffs = dl + B;
+    r.lens = dlens; r.offs = doffs;
     const float* dq = static_cast<const float*>(upload(dev, qkv, rows * 3 * H * sizeof(float), st));
     float* dout = static_cast<float*>(upload(dev, out, rows * H * sizeof(float), st));   // (the FFMA kernels always write fp32)
     const size_t pn = rows * H;
@@ -5020,8 +5036,8 @@ int vtts_debug_attention(vtts_handle h, const char* layer, int B, const int* len
       h->flush_tails(dlens, doffs);
     }
     auto once = [&] {
-      if (use_tc) h->launch_attn_tc(pq, out ? dout : nullptr, planes ? &po : nullptr, *L, H, dlens, doffs, maxLen);
-      else h->launch_attn(dq, dout, *L, H, dlens, doffs, maxLen, planes ? &po : nullptr);
+      if (use_tc) h->launch_attn_tc(pq, out ? dout : nullptr, planes ? &po : nullptr, *L, H, r);
+      else h->launch_attn(dq, dout, *L, H, planes ? &po : nullptr, r);
     };
     once();
     CK(cudaStreamSynchronize(st));
@@ -5133,31 +5149,9 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
         REQUIRE(right <= ZT_ROWS || rows_cap <= end_last + ZT_ROWS, VTTS_ERR_INVALID, "debug_conv: conv halo reaches rows behind the zeroed tail");
       }
     }
-    // ---- per-call engine state the launch code reads, restored on every exit
-    struct Saved {
-      vtts_engine* h;
-      int B, maxFrm, knobs[11];
-      std::vector<int> fl, fo, vf;
-      int* kp[11];
-      explicit Saved(vtts_engine* e) : h(e), B(e->B), maxFrm(e->maxFrm), fl(e->h_frm_len), fo(e->h_frm_off), vf(e->v_frm_len),
-          kp{&e->tc_bn, &e->tc_split, &e->tc_tall, &e->tc_mc, &e->tc_persist, &e->tc_wmc, &e->tc_min_steps, &e->conv_max_s,
-             &e->conv_min_g, &e->conv_max_g, &e->conv_big_g} {
-        for (int i = 0; i < 11; ++i) knobs[i] = *kp[i];
-      }
-      ~Saved() {
-        h->B = B; h->maxFrm = maxFrm; h->h_frm_len = fl; h->h_frm_off = fo; h->v_frm_len = vf;
-        for (int i = 0; i < 11; ++i) *kp[i] = knobs[i];
-      }
-    } saved(h);
-    if (ov) {
-      const int v[11] = {ov->tc_bn, ov->tc_split, ov->tc_tall, ov->tc_mc, ov->tc_persist, ov->tc_wmc, ov->tc_min_steps, ov->conv_max_s,
-                         ov->conv_min_g, ov->conv_max_g, ov->conv_big_g};
-      for (int i = 0; i < 11; ++i) if (v[i] != VTTS_CONV_KEEP) *saved.kp[i] = v[i];
-    }
-    h->B = B; h->maxFrm = maxLen;
-    h->h_frm_len.assign(lens, lens + B);
-    h->h_frm_off.assign(off.begin(), off.end());
-    h->v_frm_len = h->h_frm_len;                  // the heuristics see this call's lengths
+    // planes() and flush_tails() read the member B: restored on every exit
+    struct KeepB { vtts_engine* h; int B; ~KeepB() { h->B = B; } } keep{h, h->B};
+    h->B = B;
     // ---- device copies (freed on every exit)
     std::vector<Buf<char>> dev;
     cudaStream_t st = h->stream;
@@ -5168,6 +5162,8 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
     int* dl = static_cast<int*>(upload(dev, lo.data(), lo.size() * sizeof(int), st));
     const int* dlens = dl;
     const int* doffs = dl + B;
+    const std::vector<int> hl(lens, lens + B);     // the heuristics see this call's lengths
+    const Rows r{dlens, doffs, B, maxLen, hl, hl, ov ? h->tune.with(*ov) : h->tune};
     float* dy = y ? static_cast<float*>(upload(dev, y, y_n * sizeof(float), st)) : nullptr;
     const float* dres = res ? static_cast<const float*>(upload(dev, res, res_n * sizeof(float), st)) : nullptr;
     __nv_bfloat16* dp = any_planes ? static_cast<__nv_bfloat16*>(upload(dev, p_out, (size_t)p_planes * p_n * 2, st)) : nullptr;
@@ -5204,7 +5200,7 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
         s.cond = cond_of(q); s.cond_ld = q.cond_ld;
         ps.push_back(s);
       }
-      h->launch_tc(ps, rmul, dlens, doffs, maxLen, B);
+      h->launch_tc(ps, rmul, r);
     } else {
       const float* dx = static_cast<const float*>(upload(dev, x, x_n * sizeof(float), st));
       std::vector<ConvP> ps;
@@ -5223,7 +5219,7 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
         p.pl_slope = q.pl_slope;
         ps.push_back(p);
       }
-      h->launch_conv(ps, rmul, dlens, doffs, maxLen, B);
+      h->launch_conv(ps, rmul, r);
     }
     CK(cudaStreamSynchronize(st));
     if (y) CK(cudaMemcpy(y, dy, y_n * sizeof(float), cudaMemcpyDeviceToHost));
@@ -5304,11 +5300,10 @@ float vtts_microbench(vtts_handle h, const char* what, int iters) {
     const bool is_tc = strcmp(kind, "tc") == 0;
     REQUIRE(is_tc || strcmp(kind, "ffma") == 0, VTTS_ERR_INVALID, "unknown microbench kind");
     REQUIRE(!is_tc || h->tc, VTTS_ERR_INVALID, "tc microbench needs a precision-1 engine");
-    struct Saved {       // state the launch helpers read, restored on every exit
-      vtts_engine* h; int B; bool prof; std::vector<int> fl, tl, vf, vt;
-      ~Saved() { h->B = B; h->profiling = prof; h->h_frm_len = fl; h->h_tok_len = tl; h->v_frm_len = vf; h->v_tok_len = vt; h->tc_dbg = nullptr; }
-    } saved{h, h->B, h->profiling, h->h_frm_len, h->h_tok_len, h->v_frm_len, h->v_tok_len};
-    h->B = 1; h->h_frm_len.assign(1, rows); h->h_tok_len.assign(1, rows); h->v_frm_len = h->h_frm_len; h->v_tok_len = h->h_tok_len;
+    struct KeepProfiling {       // the profiler switch and the stamps buffer, restored on every exit
+      vtts_engine* h; bool prof;
+      ~KeepProfiling() { h->profiling = prof; h->tc_dbg = nullptr; }
+    } keep{h, h->profiling};
     Buf<int> dl, dof;
     Buf<float> x, y, w, bias;
     Buf<__nv_bfloat16> ph, pl, wh, wl;
@@ -5316,6 +5311,7 @@ float vtts_microbench(vtts_handle h, const char* what, int iters) {
     CK(dl.alloc(2)); CK(dof.alloc(2));
     const int hl[2] = {rows, rows}, ho[2] = {0, rows};
     CK(cudaMemcpy(dl.p, hl, 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dof.p, ho, 8, cudaMemcpyHostToDevice));
+    const Rows r{dl.p, dof.p, 1, rows, {rows}, {rows}, h->tune};
     CK(y.alloc((size_t)rows * Cout)); CK(bias.alloc(ldw)); CK(cudaMemset(bias.p, 0, (size_t)ldw * 4));
     if (is_tc) {
       CK(ph.alloc((size_t)rows * Cin)); CK(pl.alloc((size_t)rows * Cin));
@@ -5332,10 +5328,10 @@ float vtts_microbench(vtts_handle h, const char* what, int iters) {
         q.in.hi = ph.p; q.in.lo = pl.p; q.in.C = Cin; q.in.rows = rows;
         q.w.hi = wh.p; q.w.lo = wl.p; q.bias = bias.p; q.Cin = Cin; q.Cout = Cout; q.k = k; q.dil = dil; q.pad = dil * (k - 1) / 2;
         q.y = y.p; q.ldy = Cout;
-        h->launch_tc({q}, 1, dl.p, dof.p, rows, 1);
+        h->launch_tc({q}, 1, r);
       } else {
         ConvW W; W.w = w.p; W.b = bias.p; W.Cin = Cin; W.Cout = Cout; W.k = k; W.ldw = ldw;
-        h->launch_conv({mk(W, x.p, Cin, 0, y.p, Cout, 0, dil, dil * (k - 1) / 2)}, 1, dl.p, dof.p, rows, 1);
+        h->launch_conv({mk(W, x.p, Cin, 0, y.p, Cout, 0, dil, dil * (k - 1) / 2)}, 1, r);
       }
     };
     h->profiling = false;
