@@ -93,6 +93,10 @@ typedef struct vtts_config {
   int32_t cv_conv_kernel[8], cv_conv_stride[8];            /* (10,3,3,3,3,2,2) / (5,2,2,2,2,2,2) */
   int32_t cv_pos_k, cv_pos_groups;                         /* positional conv: 128 taps, 16 groups */
   float cv_ln_eps, cv_gn_eps;                              /* LayerNorm eps (layer_norm_eps), layer 0's GroupNorm eps */
+  /* In StableTTS engines whose blob carries bt.* (BERT: vtts_bert_features) the cv_* fields above describe BERT's transformer:
+   * cv_layers the layers that run (the exported graph returns hidden_states[-3], so n_layers - 2 of a checkpoint), cv_hidden,
+   * cv_heads, cv_ffn and cv_ln_eps (1e-12).  The rows of the word, position and token-type tables are those of the blob's
+   * bt.emb.word / .pos / .type. */
 } vtts_config;
 
 #define VTTS_FAMILY_VITS2 0
@@ -541,6 +545,20 @@ int vtts_stabletts_synthesise_wav(vtts_handle h, const int64_t* ids, const int64
                                   float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld,
                                   int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise, float* wav, int64_t wav_ld,
                                   int64_t* wav_lengths);
+
+/* BERT features (the logits of training/stabletts/matcha/onnx/bert-export.py: BertModel(input_ids, attention_mask = 1,
+ * token_type_ids = 0).hidden_states[-3], as vosk_tts/synth.py:25-44 runs it on one sentence's word pieces): word + token-type 0
+ * + position embeddings and their LayerNorm, then cv_layers post-LN layers.  Each sentence is processed as if alone (its
+ * positions count from 0; the reference's all-ones attention mask of one sentence); its rows are bit-identical alone, in any
+ * batch, eager and replayed.
+ *   ids        int64 [B, ids_ld] WordPiece ids ([CLS] ... [SEP] as the tokenizer gives them); sentence b = its first lengths[b]
+ *   out        out float [B, out_ld, cv_hidden]: the last layer's rows of sentence b, zeros after them
+ * Host pointers, atomic on the handle; graphed per (batch, longest-sentence bucket, row bucket).  Precision 0 runs on the fp32
+ * FFMA pipe in one fixed launch shape; modes >= 1 run the GEMMs on the split-bf16 tensor cores without split-K and the
+ * attention on attn_tc_kernel (the ContentVec path).  VTTS_ERR_INVALID: not a StableTTS engine, a blob without bt.*, B < 1, a
+ * length outside [1, ids_ld] or above the position table's rows (the reference's lookup fails there too), an id
+ * outside the word table.  VTTS_ERR_CAPACITY: out_ld below a sentence's length. */
+int vtts_bert_features(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, float* out, int64_t out_ld);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

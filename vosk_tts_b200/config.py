@@ -358,3 +358,44 @@ def contentvec_frames(n_samples, cv=None):
         n = n_samples if L is None else L
         L = (n - k) // s + 1 if n >= k else 0
     return max(L, 0)
+
+
+# BERT as training/stabletts/matcha/onnx/bert-export.py exports it (transformers' BertModel returning hidden_states[-3]): the
+# defaults of BertConfig, which are rubert-base's shape.
+BERT_DEFAULTS = {
+    "hidden_size": 768, "num_hidden_layers": 12, "num_attention_heads": 12, "intermediate_size": 3072, "hidden_act": "gelu",
+    "layer_norm_eps": 1e-12, "vocab_size": 30522, "max_position_embeddings": 512, "type_vocab_size": 2,
+    "position_embedding_type": "absolute",
+}
+BERT_DROPPED_LAYERS = 2   # hidden_states[-3] is the output of layer n_layers - 2: the last two layers never run
+
+
+def bert_config(path_or_dict=None, layers=None):
+    """The engine's BERT shape (cv_* keys for the transformer, bt_* for the embeddings) from a Hugging Face BertConfig
+    config.json (None: the defaults).  cv_layers is the number of layers that run: `layers` when given (what an exported graph
+    holds), else num_hidden_layers - 2.  Refuses, with the reason, what the engine does not compute."""
+    cfg = dict(BERT_DEFAULTS)
+    if path_or_dict is not None:
+        src = path_or_dict
+        if not isinstance(src, dict):
+            with open(path_or_dict) as f:
+                src = json.load(f)
+        cfg.update({k: src[k] for k in BERT_DEFAULTS if k in src and src[k] is not None})
+    if cfg["hidden_act"] != "gelu":
+        raise ValueError("hidden_act %r: only 'gelu' (erf) is supported" % cfg["hidden_act"])
+    if cfg["position_embedding_type"] != "absolute":
+        raise ValueError("position_embedding_type %r: only 'absolute' is supported" % cfg["position_embedding_type"])
+    H, nh, F = int(cfg["hidden_size"]), int(cfg["num_attention_heads"]), int(cfg["intermediate_size"])
+    if H % nh or (H // nh) % 32 or H // nh > 128 or H % 16 or H > 1024:
+        raise ValueError("hidden_size %d / %d heads: the attention kernels take head widths that are multiples of 32 up to 128, "
+                         "and the LayerNorm kernel widths up to 1024" % (H, nh))
+    if F % 16 or F < 16:
+        raise ValueError("intermediate_size must be a positive multiple of 16")
+    n = int(cfg["num_hidden_layers"]) - BERT_DROPPED_LAYERS if layers is None else int(layers)
+    if n < 1:
+        raise ValueError("no BERT layer would run (num_hidden_layers must be at least 3: hidden_states[-3] is layer n - 2)")
+    if int(cfg["vocab_size"]) < 1 or int(cfg["max_position_embeddings"]) < 1 or int(cfg["type_vocab_size"]) < 1:
+        raise ValueError("vocab_size, max_position_embeddings and type_vocab_size must be positive")
+    return {"cv_layers": n, "cv_hidden": H, "cv_heads": nh, "cv_ffn": F, "cv_ln_eps": float(cfg["layer_norm_eps"]),
+            "bt_vocab": int(cfg["vocab_size"]), "bt_max_pos": int(cfg["max_position_embeddings"]),
+            "bt_type_rows": int(cfg["type_vocab_size"])}

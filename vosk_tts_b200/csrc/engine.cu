@@ -29,6 +29,7 @@
 #include "vc.cuh"
 #include "spk.cuh"
 #include "contentvec.cuh"
+#include "bert.cuh"
 #include "dit.cuh"
 #include "stabletts.cuh"
 #include "hifigan.cuh"
@@ -458,7 +459,8 @@ struct vtts_engine {
   // phase tag, the first element of every key
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
-    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2, TAG_HIFIGAN = 0xD3
+    TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2, TAG_HIFIGAN = 0xD3,
+    TAG_BERT = 0xD4
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -749,6 +751,31 @@ struct vtts_engine {
   void bind_contentvec();
   std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
   void cv_enqueue(float* out, const int* out_offs);
+  // The post-LN transformer layers ContentVec and BERT share, and the launches they are made of: work buffers xa (the input
+  // rows, whose planes are PX), xb, Y, QKV, AO, FF and, on the tensor cores, the planes of every GEMM operand
+  struct PostLnWs { float *xa, *xb, *Y, *QKV, *AO, *FF; Planes PX, PQKV, PAO, PX1, PFF; };
+  void post_ln_layers(const std::vector<EncLayerW>& layers, bool on_tc, int H, int Fh, float eps, PostLnWs w, float* out,
+                      const int* out_offs, const Rows& r);
+  void ln_rows(const float* a, const float* y, const LnW& w, float eps, float* out, const int* out_offs, int C, const Planes* pl,
+               const Rows& r);
+  void gelu_rows(float* y, int C, const Planes* pl, const Rows& r);
+  void gemm_rows(const Planes& in, const TcW& w, const ConvW& cw, float* y, const float* res, const Planes* out, const Rows& r);
+
+  // ---- BERT (transformers' BertModel as bert-export.py exports it; bert.cuh): word pieces -> the hidden rows of the last
+  //      layer that runs, in StableTTS engines whose blob carries bt.*.  Described by the cv_* fields of vtts_config.
+  bool has_bert = false, bt_tc = false;
+  int bt_vocab = 0, bt_max_pos = 0;                // rows of the word and position tables
+  const float *bt_word = nullptr, *bt_pos = nullptr, *bt_type = nullptr;
+  LnW bt_ln;
+  std::vector<EncLayerW> bt_enc;
+  // shape of the current call: maxL the longest sentence's bucket, tot the rows of the packed sentences (bucketed)
+  struct BtPlan { int maxL = 0, tot = 0; std::vector<int> len, off; } btp;
+  Buf<int> d_bti;                                  // [len B][off B][ids tot]
+  Buf<float> d_btzero, d_btx, d_btx1, d_bty, d_btqkv, d_btao, d_btff, d_btout;
+  PinnedBuf<char> h_pin_bt;
+  void bind_bert();
+  void bt_stage(const int64_t* ids, const int64_t* lengths, int64_t ld);
+  void bt_enqueue(float* out);
 
   // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh), fp32 FFMA in every mode
   ConvW st_cp[3], st_in, st_final;                 // cond_proj's three convs, in_proj over (x | cond), final_proj
@@ -2983,50 +3010,29 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   klaunch(cv_gn_kernel<2>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
   CK(cudaGetLastError());
   launches += 3;
-  auto gelu = [&](float* y, int width, const int* lens, const int* offs, int maxLen, const Planes* pl) {
-    klaunch(cv_gelu_kernel, dim3(maxLen, B), dim3(256), (size_t)0, y, width, lens, offs, pl ? pl->hi : (__nv_bfloat16*)nullptr,
-            pl ? pl->lo : (__nv_bfloat16*)nullptr);
-    CK(cudaGetLastError());
-    ++launches;
-  };
   float* x = lv[0];
   for (int i = 1; i < NL; ++i) {
     float* y = lv[i & 1];
     launch_conv({mk(cv_conv[i], x, c.cv_conv_stride[i] * C, 0, y, C, 0, 1, 0)}, 1, level(i));
-    gelu(y, C, Ls(i), Os(i), cvp.maxL[i], nullptr);
+    gelu_rows(y, C, nullptr, level(i));
     x = y;
   }
-  const int* Lf = Ls(NL - 1);
   const int* Of = Os(NL - 1);
-  const int maxF = cvp.maxL[NL - 1];
   const Rows rf = level(NL - 1);
   const size_t Tf = (size_t)cvp.tot0 / cv_P;
   float *X = ensure(d_cvx, Tf * H), *X1 = ensure(d_cvx1, Tf * H), *Y = ensure(d_cvy, Tf * H), *QKV = ensure(d_cvqkv, Tf * 3 * H);
   float *AO = ensure(d_cvao, Tf * std::max(H, C)), *FF = ensure(d_cvff, Tf * Fh);
-  const dim3 lg((maxF + CVL_WARPS - 1) / CVL_WARPS, B), lb(32 * CVL_WARPS);
   // precision modes >= 1: the projection and the transformer's qkv / out / FFN convs on conv_tc_kernel, attention on
   // attn_tc_kernel; every producer of a GEMM operand also writes its split-bf16 planes.  All of
   // them are 1x1, and the attention masks keys past a clip, so no plane row behind a clip is read (no tail zeroing).
-  Planes PX, P512, PQKV, PAO, PX1, PFF;
+  PostLnWs w{X1, X, Y, QKV, AO, FF};
+  Planes P512;
   if (cv_tc) {
-    P512 = planes(50, (long)Tf, 1, C); PX = planes(51, (long)Tf, 1, H); PQKV = planes(52, (long)Tf, 1, 3 * H);
-    PAO = planes(53, (long)Tf, 1, H); PX1 = planes(54, (long)Tf, 1, H); PFF = planes(55, (long)Tf, 1, Fh);
+    P512 = planes(50, (long)Tf, 1, C); w.PX = planes(51, (long)Tf, 1, H); w.PQKV = planes(52, (long)Tf, 1, 3 * H);
+    w.PAO = planes(53, (long)Tf, 1, H); w.PX1 = planes(54, (long)Tf, 1, H); w.PFF = planes(55, (long)Tf, 1, Fh);
   }
-  auto ln = [&](const float* a, const float* yy, const float* g, const float* bt, float* o, const int* oo, int width, const Planes* pl) {
-    klaunch(cv_ln_kernel, lg, lb, (size_t)0, a, yy, g, bt, c.cv_ln_eps, o, Lf, Of, oo, width, pl ? pl->hi : (__nv_bfloat16*)nullptr,
-            pl ? pl->lo : (__nv_bfloat16*)nullptr);
-    CK(cudaGetLastError());
-    ++launches;
-  };
-  auto gemm = [&](const Planes& in, const TcW& w, const ConvW& cw, float* y, const float* res, const Planes* out, int epi) {
-    TcSpec s;
-    s.in = in; s.w = w; s.bias = cw.b; s.Cin = cw.Cin; s.Cout = cw.Cout;
-    s.y = y; s.ldy = cw.Cout; s.res = res; s.ldr = res ? cw.Cout : 0; s.epi = epi;
-    if (out) s.out = *out;
-    launch_tc({s}, 1, rf);
-  };
-  ln(x, nullptr, cv_fp_g, cv_fp_b, AO, Of, C, cv_tc ? &P512 : nullptr);
-  if (cv_tc) gemm(P512, cv_tfp, cv_fp, X, nullptr, nullptr, 0);
+  ln_rows(x, nullptr, LnW{cv_fp_g, cv_fp_b}, c.cv_ln_eps, AO, Of, C, cv_tc ? &P512 : nullptr, rf);
+  if (cv_tc) gemm_rows(P512, cv_tfp, cv_fp, X, nullptr, nullptr, rf);
   else launch_conv({mk(cv_fp, AO, C, 0, X, H, 0, 1, 0)}, 1, rf);
   const int G = c.cv_pos_groups, Cg = H / G, kh = c.cv_pos_k / 2;
   for (int half = 0; half < 2; ++half)
@@ -3043,38 +3049,190 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
       }
       launch_conv(pp, 1, rf);
     }
-  ln(X, Y, cv_enc_g, cv_enc_b, X1, Of, H, cv_tc ? &PX : nullptr);
+  ln_rows(X, Y, LnW{cv_enc_g, cv_enc_b}, c.cv_ln_eps, X1, Of, H, cv_tc ? &w.PX : nullptr, rf);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_cvdbg, Tf * H), X1, Tf * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  float *xa = X1, *xb = X;
-  for (size_t l = 0; l < cv_enc.size() && cv_tc; ++l) {
-    const EncLayerW& Lw = cv_enc[l];
-    gemm(PX, Lw.t_qkv, Lw.qkv, QKV, nullptr, &PQKV, 0);
-    if (attn_use_tc(Lw, H, rf)) launch_attn_tc(PQKV, AO, &PAO, Lw, H, rf);
-    else launch_attn(QKV, AO, Lw, H, &PAO, rf);
-    gemm(PAO, Lw.t_o, Lw.o, Y, xa, nullptr, 0);
-    ln(Y, nullptr, Lw.ln1.g, Lw.ln1.b, xb, Of, H, &PX1);
-    gemm(PX1, Lw.t_ffn1, Lw.ffn1, FF, nullptr, nullptr, 0);
-    gelu(FF, Fh, Lf, Of, maxF, &PFF);
-    gemm(PFF, Lw.t_ffn2, Lw.ffn2, Y, xb, nullptr, 0);
-    if (l + 1 == cv_enc.size()) ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, out, out_offs ? out_offs : Of, H, nullptr);
-    else ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, xa, Of, H, &PX);
+  post_ln_layers(cv_enc, cv_tc, H, Fh, c.cv_ln_eps, w, out, out_offs ? out_offs : Of, rf);
+}
+
+// LayerNorm of the rows r (cv_ln_kernel): out = LN(a + gelu(y)) (y null: LN(a)), rows read at r.offs, written at out_offs.
+void vtts_engine::ln_rows(const float* a, const float* y, const LnW& w, float eps, float* out, const int* out_offs, int C,
+                          const Planes* pl, const Rows& r) {
+  klaunch(cv_ln_kernel, dim3((r.maxLen + CVL_WARPS - 1) / CVL_WARPS, r.n), dim3(32 * CVL_WARPS), (size_t)0, a, y, w.g, w.b, eps, out,
+          r.lens, r.offs, out_offs, C, pl ? pl->hi : (__nv_bfloat16*)nullptr, pl ? pl->lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+// GELU of the rows r (cv_gelu_kernel): in place, or into the planes pl.
+void vtts_engine::gelu_rows(float* y, int C, const Planes* pl, const Rows& r) {
+  klaunch(cv_gelu_kernel, dim3(r.maxLen, r.n), dim3(256), (size_t)0, y, C, r.lens, r.offs, pl ? pl->hi : (__nv_bfloat16*)nullptr,
+          pl ? pl->lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+// One 1x1 conv of the rows r on the tensor cores: y = in W^T + bias (+ res), and the planes of y when out is given.
+void vtts_engine::gemm_rows(const Planes& in, const TcW& w, const ConvW& cw, float* y, const float* res, const Planes* out, const Rows& r) {
+  TcSpec s;
+  s.in = in; s.w = w; s.bias = cw.b; s.Cin = cw.Cin; s.Cout = cw.Cout;
+  s.y = y; s.ldy = cw.Cout; s.res = res; s.ldr = res ? cw.Cout : 0; s.epi = 0;
+  if (out) s.out = *out;
+  launch_tc({s}, 1, r);
+}
+
+// The post-LN transformer layers of ContentVec (HubertEncoderLayer) and BERT (BertLayer): x = LN(x + o(attention(qkv(x)))),
+// x = LN(x + ffn2(gelu(ffn1(x)))), with no relative positions (relk / relv of every layer point at zeros).  The input rows are
+// w.xa (on_tc: and their planes w.PX); the last LayerNorm writes row t of sequence b to out row out_offs[b] + t.  on_tc: the
+// convs on conv_tc_kernel and the attention on attn_tc_kernel where r.tune takes it, else everything on the FFMA pipe.
+void vtts_engine::post_ln_layers(const std::vector<EncLayerW>& layers, bool on_tc, int H, int Fh, float eps, PostLnWs w,
+                                 float* out, const int* out_offs, const Rows& r) {
+  float *xa = w.xa, *xb = w.xb;
+  for (size_t l = 0; l < layers.size() && on_tc; ++l) {
+    const EncLayerW& Lw = layers[l];
+    gemm_rows(w.PX, Lw.t_qkv, Lw.qkv, w.QKV, nullptr, &w.PQKV, r);
+    if (attn_use_tc(Lw, H, r)) launch_attn_tc(w.PQKV, w.AO, &w.PAO, Lw, H, r);
+    else launch_attn(w.QKV, w.AO, Lw, H, &w.PAO, r);
+    gemm_rows(w.PAO, Lw.t_o, Lw.o, w.Y, xa, nullptr, r);
+    ln_rows(w.Y, nullptr, Lw.ln1, eps, xb, r.offs, H, &w.PX1, r);
+    gemm_rows(w.PX1, Lw.t_ffn1, Lw.ffn1, w.FF, nullptr, nullptr, r);
+    gelu_rows(w.FF, Fh, &w.PFF, r);
+    gemm_rows(w.PFF, Lw.t_ffn2, Lw.ffn2, w.Y, xb, nullptr, r);
+    if (l + 1 == layers.size()) ln_rows(w.Y, nullptr, Lw.ln2, eps, out, out_offs, H, nullptr, r);
+    else ln_rows(w.Y, nullptr, Lw.ln2, eps, xa, r.offs, H, &w.PX, r);
   }
-  for (size_t l = 0; l < cv_enc.size() && !cv_tc; ++l) {
-    const EncLayerW& Lw = cv_enc[l];
-    launch_conv({mk(Lw.qkv, xa, H, 0, QKV, 3 * H, 0, 1, 0)}, 1, rf);
-    launch_attn(QKV, AO, Lw, H, nullptr, rf);
-    ConvP po = mk(Lw.o, AO, H, 0, Y, H, 0, 1, 0);
+  for (size_t l = 0; l < layers.size() && !on_tc; ++l) {
+    const EncLayerW& Lw = layers[l];
+    launch_conv({mk(Lw.qkv, xa, H, 0, w.QKV, 3 * H, 0, 1, 0)}, 1, r);
+    launch_attn(w.QKV, w.AO, Lw, H, nullptr, r);
+    ConvP po = mk(Lw.o, w.AO, H, 0, w.Y, H, 0, 1, 0);
     po.res = xa; po.ldr = H;
-    launch_conv({po}, 1, rf);
-    ln(Y, nullptr, Lw.ln1.g, Lw.ln1.b, xb, Of, H, nullptr);
-    launch_conv({mk(Lw.ffn1, xb, H, 0, FF, Fh, 0, 1, 0)}, 1, rf);
-    gelu(FF, Fh, Lf, Of, maxF, nullptr);
-    ConvP p2 = mk(Lw.ffn2, FF, Fh, 0, Y, H, 0, 1, 0);
+    launch_conv({po}, 1, r);
+    ln_rows(w.Y, nullptr, Lw.ln1, eps, xb, r.offs, H, nullptr, r);
+    launch_conv({mk(Lw.ffn1, xb, H, 0, w.FF, Fh, 0, 1, 0)}, 1, r);
+    gelu_rows(w.FF, Fh, nullptr, r);
+    ConvP p2 = mk(Lw.ffn2, w.FF, Fh, 0, w.Y, H, 0, 1, 0);
     p2.res = xb; p2.ldr = H;
-    launch_conv({p2}, 1, rf);
-    if (l + 1 == cv_enc.size()) ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, out, out_offs ? out_offs : Of, H, nullptr);
-    else ln(Y, nullptr, Lw.ln2.g, Lw.ln2.b, xa, Of, H, nullptr);
+    launch_conv({p2}, 1, r);
+    if (l + 1 == layers.size()) ln_rows(w.Y, nullptr, Lw.ln2, eps, out, out_offs, H, nullptr, r);
+    else ln_rows(w.Y, nullptr, Lw.ln2, eps, xa, r.offs, H, nullptr, r);
   }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// BERT (transformers' BertModel as training/stabletts/matcha/onnx/bert-export.py exports it: hidden_states[-3], i.e. the output
+// of the last layer the blob holds; bert.cuh)
+// ---------------------------------------------------------------------------------------------------
+void vtts_engine::bind_bert() {
+  const vtts_config& c = cfg;
+  has_bert = tensors.count("bt.emb.word") > 0;
+  if (!has_bert) return;
+  const int H = c.cv_hidden, Fh = c.cv_ffn, nh = c.cv_heads;
+  REQUIRE(c.cv_layers >= 1 && nh >= 1 && H % nh == 0 && (H / nh) % 32 == 0 && H / nh <= 128 && H % CV_CK == 0 && H <= 32 * CVL_MAXV &&
+              Fh >= CV_CK && Fh % CV_CK == 0,
+          VTTS_ERR_INVALID, "unsupported BERT shape (at least one layer, head width a multiple of 32 up to 128, width a multiple of 16 "
+          "up to 1024, FFN a multiple of 16)");
+  REQUIRE(c.cv_ln_eps > 0.f, VTTS_ERR_INVALID, "BERT needs a positive LayerNorm eps");
+  // the tables' rows are the blob's: vocabulary, positions (the longest sentence) and token types
+  auto rows = [&](const char* name) {
+    const size_t n = tensor(name).n;
+    REQUIRE(n >= (size_t)H && n % H == 0 && n / H <= (size_t)INT32_MAX, VTTS_ERR_WEIGHTS, std::string("bad BERT table ") + name);
+    return (int)(n / H);
+  };
+  bt_vocab = rows("bt.emb.word");
+  bt_max_pos = rows("bt.emb.pos");
+  bt_tc = c.precision >= 1 && c.precision <= 3;
+  if (bt_tc) {
+    REQUIRE(H % TC_BK == 0 && Fh % TC_BK == 0, VTTS_ERR_INVALID, "BERT on the tensor cores needs widths in multiples of 64");
+    REQUIRE(tensors.count("bt.l0.qkv.th") > 0, VTTS_ERR_WEIGHTS, "the blob lacks BERT's tensor-core weights");
+  }
+  bt_word = vec("bt.emb.word", (size_t)bt_vocab * H);
+  bt_pos = vec("bt.emb.pos", (size_t)bt_max_pos * H);
+  bt_type = vec("bt.emb.type", (size_t)rows("bt.emb.type") * H);
+  bt_ln = ln("bt.emb.ln", H);
+  // zeros: the relative tables of the attention (fp32, and the [16][128] bf16 tiles of the tensor-core attention).  BERT has
+  // absolute positions only; the attention kernels always add a relative term, which these zeros make vanish exactly.  A
+  // StableTTS engine leaves window_size 0 (make_c_config does not set it), so that term is one offset per query row.
+  const size_t nz = std::max<size_t>({(size_t)H, (size_t)(2 * c.window_size + 1) * (H / nh), (size_t)ATC_RELP * 128});
+  float* zero = ensure(d_btzero, nz);
+  CK(cudaMemsetAsync(zero, 0, d_btzero.cap * sizeof(float), stream));
+  bt_enc.clear();
+  for (int l = 0; l < c.cv_layers; ++l) {
+    const std::string p = "bt.l" + std::to_string(l);
+    EncLayerW L;
+    L.heads = nh;
+    L.qkv = conv(p + ".qkv", H, 3 * H, 1);
+    L.o = conv(p + ".o", H, H, 1);
+    L.ln1 = ln(p + ".ln1", H);
+    L.ffn1 = conv(p + ".ffn1", H, Fh, 1);
+    L.ffn2 = conv(p + ".ffn2", Fh, H, 1);
+    L.ln2 = ln(p + ".ln2", H);
+    L.relk = L.relv = zero;
+    if (bt_tc) {
+      L.t_qkv = tcw(p + ".qkv", H, 3 * H, 1);
+      L.t_o = tcw(p + ".o", H, H, 1);
+      L.t_ffn1 = tcw(p + ".ffn1", H, Fh, 1);
+      L.t_ffn2 = tcw(p + ".ffn2", Fh, H, 1);
+      const __nv_bfloat16* zb = reinterpret_cast<const __nv_bfloat16*>(zero);
+      L.rk_hi = L.rk_lo = L.rv_hi = L.rv_lo = zb;
+    }
+    bt_enc.push_back(L);
+  }
+}
+
+// Host side of a BERT call: validates the word pieces and packs the sentences' rows back to back (each starting at a multiple
+// of 8), then stages [len B][off B][ids] in pinned memory.  The longest sentence and the row total are bucketed (32 rows; 1024
+// rows for batches), so a captured graph serves every call of the bucket.
+void vtts_engine::bt_stage(const int64_t* ids, const int64_t* lengths, int64_t ld) {
+  const vtts_config& c = cfg;
+  btp.len.assign(B, 0);
+  btp.off.assign(B, 0);
+  int mx = 0, tot = 0;
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lengths[b] >= 1 && lengths[b] <= ld, VTTS_ERR_INVALID, "lengths must be in [1, ids_ld]");
+    REQUIRE(lengths[b] <= bt_max_pos, VTTS_ERR_INVALID, "a sentence is longer than BERT's position table (max_position_embeddings)");
+    for (int64_t t = 0; t < lengths[b]; ++t) {
+      const int64_t v = ids[(size_t)b * ld + t];
+      REQUIRE(v >= 0 && v < bt_vocab, VTTS_ERR_INVALID, "a word-piece id is outside BERT's vocabulary");
+    }
+    btp.len[b] = (int)lengths[b];
+    btp.off[b] = tot;
+    tot += (btp.len[b] + 7) / 8 * 8;
+    REQUIRE(tot <= (1 << 24), VTTS_ERR_INVALID, "the batch holds too many word pieces for one call");
+    mx = std::max(mx, btp.len[b]);
+  }
+  btp.maxL = use_buckets ? (mx + 31) / 32 * 32 : mx;
+  btp.tot = !use_buckets ? tot : B == 1 ? btp.maxL : (tot + 1023) / 1024 * 1024;
+  int* pin = reinterpret_cast<int*>(ensure(h_pin_bt, ((size_t)2 * B + btp.tot) * sizeof(int) + 64));
+  memcpy(pin, btp.len.data(), B * sizeof(int));
+  memcpy(pin + B, btp.off.data(), B * sizeof(int));
+  std::fill(pin + 2 * B, pin + 2 * B + btp.tot, 0);
+  for (int b = 0; b < B; ++b)
+    for (int t = 0; t < btp.len[b]; ++t) pin[2 * B + btp.off[b] + t] = (int)ids[(size_t)b * ld + t];
+}
+
+// BERT of the staged sentences (bt_stage): the embeddings, then the post-LN layers; the last LayerNorm writes the packed rows
+// to out.  Every launch has one shape whatever the batch (Tuning::fixed_ffma and fixed_attention in mode 0, fixed_tc in modes
+// >= 1), so a sentence's rows are the same alone and in any batch.
+void vtts_engine::bt_enqueue(float* out) {
+  const vtts_config& c = cfg;
+  const int H = c.cv_hidden, Fh = c.cv_ffn;
+  const Tuning tn = bt_tc ? tune.fixed_tc() : tune.fixed_ffma().fixed_attention();
+  const size_t T = btp.tot, nint = 2 * (size_t)B + T;
+  int* di = ensure(d_bti, nint);
+  CK(cudaMemcpyAsync(di, h_pin_bt.p, nint * sizeof(int), cudaMemcpyHostToDevice, stream));
+  const Rows r{di, di + B, B, btp.maxL, std::vector<int>(B, btp.maxL), btp.len, tn};
+  PostLnWs w{ensure(d_btx, T * H), ensure(d_btx1, T * H), ensure(d_bty, T * H), ensure(d_btqkv, T * 3 * H), ensure(d_btao, T * H),
+             ensure(d_btff, T * Fh)};
+  if (bt_tc) {
+    w.PX = planes(51, (long)T, 1, H); w.PQKV = planes(52, (long)T, 1, 3 * H);
+    w.PAO = planes(53, (long)T, 1, H); w.PX1 = planes(54, (long)T, 1, H); w.PFF = planes(55, (long)T, 1, Fh);
+  }
+  klaunch(bert_embed_kernel, dim3((btp.maxL + CVL_WARPS - 1) / CVL_WARPS, B), dim3(32 * CVL_WARPS), (size_t)0, (const int*)(di + 2 * B),
+          bt_word, bt_pos, bt_type, bt_ln.g, bt_ln.b, c.cv_ln_eps, w.xa, r.lens, r.offs, H, bt_tc ? w.PX.hi : (__nv_bfloat16*)nullptr,
+          bt_tc ? w.PX.lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++launches;
+  post_ln_layers(bt_enc, bt_tc, H, Fh, c.cv_ln_eps, w, out, r.offs, r);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -3952,6 +4110,22 @@ static void impl_content_units(vtts_handle h, const float* wav, const int64_t* l
   }
 }
 
+// BERT features through host buffers (vtts_bert_features).
+static void impl_bert_features(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, float* out, int64_t out_ld) {
+  REQUIRE(h->has_bert, VTTS_ERR_INVALID, "the weight blob has no BERT (bt.*): build the engine with StableTTS(..., bert=...)");
+  REQUIRE(B >= 1 && B <= 16384, VTTS_ERR_INVALID, "bad batch size");
+  REQUIRE(ids_ld >= 1, VTTS_ERR_INVALID, "bad ids_ld");
+  h->B = B;
+  h->bt_stage(ids, lengths, ids_ld);
+  for (int b = 0; b < B; ++b) REQUIRE(h->btp.len[b] <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than a sentence's length");
+  const int H = h->cfg.cv_hidden;
+  const size_t n = (size_t)h->btp.tot * H;
+  h->ensure_pinned(n * sizeof(float) + 64);     // the readback's staging, grown before the graph captures (growth retires it)
+  h->run_graphed({vtts_engine::TAG_BERT, B, h->btp.maxL, h->btp.tot}, [&] { h->bt_enqueue(h->ensure(h->d_btout, n)); });
+  read_clips(h, (const float*)h->d_btout.p, n, n, h->btp.off.data(), h->btp.len, H, out, out_ld * H);
+  for (int b = 0; b < B; ++b) std::fill(out + ((size_t)b * out_ld + h->btp.len[b]) * H, out + (size_t)(b + 1) * out_ld * H, 0.f);
+}
+
 // QuickVC conversion through host buffers: from content units (vtts_quickvc_convert, wav null) or from source waveforms through
 // ContentVec (vtts_quickvc_convert_wav, units null; in_ld is then wav_ld).
 static void impl_quickvc_convert(vtts_handle h, const float* units, const float* wav, const int64_t* lengths, int B, int64_t in_ld,
@@ -4507,7 +4681,10 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     if (const char* e = getenv("VTTS_PREFETCH")) h->use_prefetch = atoi(e) != 0;
     REQUIRE(cfg->model_family >= VTTS_FAMILY_VITS2 && cfg->model_family <= VTTS_FAMILY_STABLETTS, VTTS_ERR_INVALID, "unknown model family");
     if (cfg->model_family == VTTS_FAMILY_QUICKVC) h->bind_quickvc();
-    else if (cfg->model_family == VTTS_FAMILY_STABLETTS) h->bind_stabletts();
+    else if (cfg->model_family == VTTS_FAMILY_STABLETTS) {
+      h->bind_stabletts();
+      h->bind_bert();
+    }
     else h->bind_weights();
     h->build_prefetch_list();
     CK(cudaMemsetAsync(h->ensure(h->d_done_ctr, 4), 0, 4 * sizeof(int), h->stream));     // ticket counter of duration_kernel (self-resetting)
@@ -4894,6 +5071,11 @@ int vtts_content_units(vtts_handle h, const float* wav, const int64_t* wav_lengt
                        int64_t units_ld, int64_t* out_frames) {
   if (!wav || !wav_lengths || !units || !out_frames) return VTTS_ERR_INVALID;
   return guarded(h, [&] { impl_content_units(h, wav, wav_lengths, B, wav_ld, units, units_ld, out_frames); }, G_ATOMIC, VTTS_FAMILY_QUICKVC);
+}
+
+int vtts_bert_features(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, float* out, int64_t out_ld) {
+  if (!ids || !lengths || !out) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_bert_features(h, ids, lengths, B, ids_ld, out, out_ld); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
 }
 
 int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const float* g,

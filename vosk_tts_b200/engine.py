@@ -63,7 +63,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
-           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav"]
+           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -254,6 +254,8 @@ def load_library(build_if_missing=True):
     lib.vtts_stabletts_synthesise_wav.restype = i32
     lib.vtts_hifigan_vocode.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64, vp]
     lib.vtts_hifigan_vocode.restype = i32
+    lib.vtts_bert_features.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64]
+    lib.vtts_bert_features.restype = i32
     _LIB = lib
     return lib
 
@@ -321,6 +323,11 @@ def make_c_config(cfg, precision=0):
             c.decoder_type = 1
             c.inter_channels = int(voc["num_mels"])
             _set_decoder_shape(c, voc)
+        bt = cfg.get("bert")
+        if bt:                                         # config.bert_config: BERT's transformer in the cv_* fields
+            for k in ("cv_layers", "cv_hidden", "cv_heads", "cv_ffn"):
+                setattr(c, k, int(bt[k]))
+            c.cv_ln_eps = float(bt["cv_ln_eps"])
         return c
     for k in ("n_vocab", "n_speakers", "gin_channels", "inter_channels", "hidden_channels", "filter_channels",
               "n_heads", "n_layers", "kernel_size", "window_size", "cond_layer_idx", "flow_kernel_size",
@@ -811,6 +818,29 @@ class Engine:
         if want_prior:
             out["prior"] = np.ascontiguousarray(prior[:, :top])
         return out
+
+    def bert_features(self, ids, lengths=None):
+        """BERT's last-layer rows of word-piece sentences (vtts_bert_features): ids int64 [B, L] with lengths, or a list of
+        sequences.  Returns float32 [B, max length, hidden] (zeros after each sentence) and the lengths."""
+        if isinstance(ids, (list, tuple)):
+            if not ids:
+                raise ValueError("bert_features needs at least one sentence")
+            seqs = [np.asarray(u, np.int64).reshape(-1) for u in ids]
+            lengths = np.array([u.size for u in seqs], np.int64)
+            ids = np.zeros((len(seqs), max(1, int(lengths.max()))), np.int64)
+            for b, u in enumerate(seqs):
+                ids[b, :u.size] = u
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        if ids.ndim == 1:
+            ids = ids[None]
+        B, L = ids.shape
+        if B == 0 or L == 0:
+            raise ValueError("bert_features needs at least one sentence of at least one word piece")
+        lengths = np.full(B, L, np.int64) if lengths is None else np.ascontiguousarray(np.broadcast_to(np.asarray(lengths, np.int64).reshape(-1), (B,)))
+        H = int(self.cfg["bert"]["cv_hidden"]) if self.cfg.get("bert") else 1
+        out = np.zeros((B, max(1, int(lengths.max())), H), np.float32)
+        self._check(self.lib.vtts_bert_features(self.h, _ptr(ids), _ptr(lengths), B, L, _ptr(out), out.shape[1]))
+        return out, lengths
 
     def resample(self, wav, from_rate, to_rate, lengths=None, trim_top_db=None, return_bounds=False):
         """Clips at `from_rate` Hz resampled to `to_rate` Hz (vtts_resample: scipy.signal.resample_poly's filter, not soxr), and

@@ -2,7 +2,8 @@
 matcha_tts.py:93-211: multistream ids, BERT features and pause durations in, durations and mel out) and its
 conditional-flow-matching decoder alone (CFM.forward of components/flow_matching.py, called at matcha_tts.py:183), and, with a
 HiFi-GAN checkpoint (matcha/hifigan, as cli.py:65-71 loads it), the vocoder: mel to waveform, and text to waveform in one call.
-The BERT model is not part of this module: a caller supplies the BERT features, as the exported graph's `bert` feed does."""
+With a BERT checkpoint (the model vosk_tts/synth.py's get_word_bert runs) the engine also computes BERT's features of word-piece
+ids on the GPU (bert_features); synthesise still takes the features per token, as the exported graph's `bert` feed does."""
 import numpy as np
 
 from . import config as _config
@@ -13,11 +14,13 @@ class StableTTS:
     """A MatchaTTS (StableTTS) checkpoint on one GPU: text-to-mel when it carries the text encoder, else the flow-matching
     decoder alone."""
 
-    def __init__(self, config, checkpoint, device=0, precision=1, vocoder=None, vocoder_config=None):
+    def __init__(self, config, checkpoint, device=0, precision=1, vocoder=None, vocoder_config=None, bert=None):
         """config: overrides of config.STABLETTS_CFM / STABLETTS_TEXT (n_vocab, n_spks, spk_emb_dim, ...) or None; checkpoint: a
         path (Lightning's `state_dict` entry is taken when present) or a state dict.  A state dict without encoder.* serves
         refine() only.  vocoder: a HiFi-GAN checkpoint path (weights.load_hifigan) or its folded `generator` state dict, or None;
-        vocoder_config: the reference's config-dict keys (config.hifigan_config; None: v1)."""
+        vocoder_config: the reference's config-dict keys (config.hifigan_config; None: v1).  bert: bert-export.py's graph (a multistream
+        model's bert/ directory or its model.onnx) or a Hugging Face BERT checkpoint directory (weights.load_bert), or a
+        (BertModel state dict, config.bert_config) pair, or None."""
         from .engine import Engine
         sd = _weights.load_checkpoint(checkpoint) if isinstance(checkpoint, str) else checkpoint
         sd = sd.get("state_dict", sd)
@@ -26,12 +29,18 @@ class StableTTS:
         if vocoder is not None:
             vsd = _weights.load_hifigan(vocoder) if isinstance(vocoder, str) else _weights.fold_weight_norm(vocoder)
             voc = (vsd, _config.hifigan_config(vocoder_config))
+        bt = None
+        if bert is not None:
+            bsd, bcfg = _weights.load_bert(bert) if isinstance(bert, str) else bert
+            bt = (bsd, bcfg, precision != 0)
         if self.has_text:
             self.cfg = _config.stabletts_config(dict({"n_vocab": int(sd["encoder.emb.weight"].shape[0])}, **(config or {})))
-            blob, man = _weights.pack_stabletts(sd, self.cfg, vocoder=voc)
+            blob, man = _weights.pack_stabletts(sd, self.cfg, vocoder=voc, bert=bt)
         else:
             self.cfg = _config.stabletts_cfm_config(config)
-            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg, vocoder=voc)
+            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg, vocoder=voc, bert=bt)
+        if bt is not None:
+            self.cfg["bert"] = bt[1]
         if voc is not None:
             if int(voc[1]["num_mels"]) != int(self.cfg["noise_channels"]):
                 raise ValueError("the vocoder reads %d mel channels, the model makes %d" % (int(voc[1]["num_mels"]), int(self.cfg["noise_channels"])))
@@ -87,6 +96,15 @@ class StableTTS:
             out["wav_lengths"] = [int(v) for v in r["wav_lengths"]]
             out["wav"] = [r["wav"][b, :out["wav_lengths"][b]].copy() for b in range(B)]
         return {k: v[0] for k, v in out.items()} if single else out
+
+    def bert_features(self, ids):
+        """ids: the WordPiece ids of one sentence ([CLS] ... [SEP], as the reference's tokenizer encodes it), or a list of them.
+        Returns BERT's rows [length, hidden] of each (a list for a list): bert-export.py's logits, hidden_states[-3]."""
+        single = not isinstance(ids, (list, tuple)) or (len(ids) > 0 and np.isscalar(ids[0]))
+        seqs = [ids] if single else list(ids)
+        feats, lengths = self.engine.bert_features(seqs)
+        out = [feats[b, :int(lengths[b])].copy() for b in range(len(seqs))]
+        return out[0] if single else out
 
     def vocode(self, mel):
         """mel: the denormalised mel [num_mels, T] of one utterance (synthesise's `mel`), or a list of them.  Returns the

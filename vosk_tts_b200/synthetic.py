@@ -409,3 +409,32 @@ def make_random_hifigan(seed=1234, h=None, gain=None):
 
 
 HIFIGAN_GAIN = {"pre": 0.25, "up": 1.0, "rb": 0.5, "post": 0.05}   # v1 on a mel of -5.5 + 2.1 N(0, 1): max |wav| 0.67, mean 0.18
+
+
+def make_random_bert(bt=None, seed=1234):
+    """A BertModel state dict (CPU fp32) in transformers' names and shapes for the shape bt (config.bert_config; default
+    rubert-base's), holding all num_hidden_layers = cv_layers + 2 layers as a checkpoint does, every tensor seeded by its name.
+    Weights are drawn at 1 / sqrt(fan-in), embeddings at 0.5, LayerNorm affines around (1, 0)."""
+    from . import config as _config
+    bt = bt or _config.bert_config()
+    H, F = bt["cv_hidden"], bt["cv_ffn"]
+    out = []
+    ln = lambda name, c: out.extend([(name + ".weight", (c,), "gamma", 0.1), (name + ".bias", (c,), "normal", 0.1)])
+    e = "embeddings."
+    for n, rows in (("word", bt["bt_vocab"]), ("position", bt["bt_max_pos"]), ("token_type", bt["bt_type_rows"])):
+        out.append((e + n + "_embeddings.weight", (rows, H), "normal", 0.5))
+    ln(e + "LayerNorm", H)
+    for l in range(bt["cv_layers"] + _config.BERT_DROPPED_LAYERS):
+        p = "encoder.layer.%d." % l
+        for n in ("query", "key", "value"):
+            _conv(out, p + "attention.self." + n, H, H, 1, gain=1.5 if n != "value" else 1.0)
+        _conv(out, p + "attention.output.dense", H, H, 1)
+        ln(p + "attention.output.LayerNorm", H)
+        _conv(out, p + "intermediate.dense", F, H, 1)
+        _conv(out, p + "output.dense", H, F, 1)
+        ln(p + "output.LayerNorm", H)
+    sd = _draw(out, seed)
+    for name, shape, _, _ in out:
+        if len(shape) == 3 and shape[2] == 1:
+            sd[name] = sd[name][:, :, 0].contiguous()          # the Linear layers: [out, in]
+    return sd

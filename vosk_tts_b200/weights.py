@@ -6,6 +6,8 @@ stored as ``weight_g`` / ``weight_v``; the exporter loads it and removes weight 
 ``flow`` before tracing.  ``fold_weight_norm`` performs the same fold; ``pack`` (below) lays every
 tensor out the way the CUDA kernels consume it.
 """
+import json
+
 import numpy as np
 import torch
 
@@ -775,26 +777,122 @@ def pack_hifigan(sd, h):
     return P.finish()
 
 
-def pack_stabletts_cfm(sd, cfg, vocoder=None):
+def _bert_from_onnx(path, heads, layer_norm_eps):
+    """The BERT graph bert-export.py writes (bert/model.onnx of a multistream model) -> (state dict, config.bert_config).
+    Named initializers are taken as they are; each Linear's weight is recovered from the MatMul whose output the Add of its
+    `<module>.bias` consumes (onnx_weights.state_dict_from_onnx).  The graph holds only the layers hidden_states[-3] depends on,
+    and that count is the number that runs.  Widths and table rows follow from the tensors; the head count and the LayerNorm
+    eps are not in the graph's weights, so they come from a config.json beside it or from the arguments (rubert-base's)."""
+    import os
+    import re
+    from . import onnx_weights
+    sd = onnx_weights.state_dict_from_onnx(path)
+    layers = sorted({int(m.group(1)) for m in (re.match(r"encoder\.layer\.(\d+)\.", k) for k in sd) if m})
+    if "embeddings.word_embeddings.weight" not in sd or not layers or layers != list(range(len(layers))):
+        raise ValueError("%s is not a BERT graph of bert-export.py (no embeddings / encoder.layer.<i> tensors)" % path)
+    cfg = {"num_attention_heads": heads, "layer_norm_eps": layer_norm_eps}
+    side = os.path.join(os.path.dirname(os.path.abspath(path)), "config.json")
+    if os.path.exists(side):
+        with open(side) as f:
+            cfg.update({k: v for k, v in json.load(f).items() if k in ("num_attention_heads", "layer_norm_eps", "hidden_act")})
+    word, pos, typ = (sd["embeddings.%s_embeddings.weight" % n] for n in ("word", "position", "token_type"))
+    cfg.update({"hidden_size": word.shape[1], "vocab_size": word.shape[0], "max_position_embeddings": pos.shape[0],
+                "type_vocab_size": typ.shape[0], "intermediate_size": sd["encoder.layer.0.intermediate.dense.weight"].shape[0]})
+    for l in layers:
+        if "encoder.layer.%d.output.dense.weight" % l not in sd:
+            raise ValueError("%s: the Linear weights of layer %d were not recovered from the graph" % (path, l))
+    return sd, _config.bert_config(cfg, layers=len(layers))
+
+
+def load_bert(path, heads=12, layer_norm_eps=1e-12):
+    """A BERT checkpoint -> (state dict in BertModel's names, config.bert_config).  `path` is either
+    - bert-export.py's ONNX graph (a .onnx file, or a directory holding model.onnx, as a multistream model's bert/ does): the
+      layers that run are the ones the graph holds; heads and layer_norm_eps come from a config.json beside it, else from the
+      arguments (rubert-base's 12 and 1e-12); or
+    - a Hugging Face checkpoint directory (config.json and pytorch_model.bin, read with weights_only=True, or
+      model.safetensors): the layers that run are num_hidden_layers - 2, as bert-export.py's hidden_states[-3] leaves them.
+      A BertForMaskedLM / BertForPreTraining checkpoint's `bert.` prefix is dropped; its heads are not read."""
+    import os
+    if os.path.isfile(path) and path.endswith(".onnx"):
+        return _bert_from_onnx(path, heads, layer_norm_eps)
+    if not os.path.isdir(path):
+        raise ValueError("%s: a BERT checkpoint is bert-export.py's .onnx graph or a directory holding model.onnx, or config.json "
+                         "and pytorch_model.bin or model.safetensors" % path)
+    st, pt = os.path.join(path, "model.safetensors"), os.path.join(path, "pytorch_model.bin")
+    if not os.path.exists(st) and not os.path.exists(pt) and os.path.exists(os.path.join(path, "model.onnx")):
+        return _bert_from_onnx(os.path.join(path, "model.onnx"), heads, layer_norm_eps)
+    bt = _config.bert_config(os.path.join(path, "config.json") if os.path.exists(os.path.join(path, "config.json")) else None)
+    if os.path.exists(st):
+        from safetensors.torch import load_file
+        sd = load_file(st)
+    elif os.path.exists(pt):
+        sd = torch.load(pt, map_location="cpu", weights_only=True)
+    else:
+        raise ValueError("%s holds none of model.onnx, model.safetensors and pytorch_model.bin" % path)
+    sd = {k[len("bert."):] if k.startswith("bert.") else k: v for k, v in sd.items()}
+    return sd, bt
+
+
+def _pack_bert(P, sd, bt, tc):
+    """bt.* tensors of the engine's BERT (csrc/bert.cuh, engine.cu bt_enqueue): the three embedding tables row-major and their
+    LayerNorm, then per layer that runs (bt["cv_layers"]) the fused q | k | v 1x1 conv, the attention's output conv, the FFN's
+    two convs and both LayerNorms, laid out as ContentVec's.  tc: also the split-bf16 copies (.th / .tl) that precision modes
+    >= 1 run on the tensor cores."""
+    g, want = _sd_getter(sd)
+    H, F, V, NP, NT = (int(bt[k]) for k in ("cv_hidden", "cv_ffn", "bt_vocab", "bt_max_pos", "bt_type_rows"))
+    e = "embeddings."
+    P.add("bt.emb.word", want(e + "word_embeddings.weight", (V, H)))
+    P.add("bt.emb.pos", want(e + "position_embeddings.weight", (NP, H)))
+    P.add("bt.emb.type", want(e + "token_type_embeddings.weight", (NT, H)))
+    P.add("bt.emb.ln.g", want(e + "LayerNorm.weight", (H,)))
+    P.add("bt.emb.ln.b", want(e + "LayerNorm.bias", (H,)))
+    conv = lambda name, w, b: (P.conv(name, w[:, :, None], b), tc and P.conv_tc(name, w[:, :, None]))
+    for l in range(int(bt["cv_layers"])):
+        p = "encoder.layer.%d." % l
+        a = p + "attention.self.%s."
+        conv("bt.l%d.qkv" % l, np.concatenate([want(a % n + "weight", (H, H)) for n in ("query", "key", "value")], 0),
+             np.concatenate([want(a % n + "bias", (H,)) for n in ("query", "key", "value")]))
+        conv("bt.l%d.o" % l, want(p + "attention.output.dense.weight", (H, H)), want(p + "attention.output.dense.bias", (H,)))
+        P.add("bt.l%d.ln1.g" % l, want(p + "attention.output.LayerNorm.weight", (H,)))
+        P.add("bt.l%d.ln1.b" % l, want(p + "attention.output.LayerNorm.bias", (H,)))
+        conv("bt.l%d.ffn1" % l, want(p + "intermediate.dense.weight", (F, H)), want(p + "intermediate.dense.bias", (F,)))
+        conv("bt.l%d.ffn2" % l, want(p + "output.dense.weight", (H, F)), want(p + "output.dense.bias", (H,)))
+        P.add("bt.l%d.ln2.g" % l, want(p + "output.LayerNorm.weight", (H,)))
+        P.add("bt.l%d.ln2.b" % l, want(p + "output.LayerNorm.bias", (H,)))
+
+
+def pack_bert(sd, bt, tc=True):
+    """BERT alone -> (blob, manifest) (see _pack_bert); bt: config.bert_config.  StableTTS(..., bert=...) appends the same
+    tensors to its blob through pack_stabletts(..., bert=...)."""
+    P = _Packer()
+    _pack_bert(P, sd, bt, tc)
+    return P.finish()
+
+
+def pack_stabletts_cfm(sd, cfg, vocoder=None, bert=None):
     """The flow-matching decoder of a MatchaTTS (StableTTS) state dict -> (blob, manifest) of a model_family "stabletts" engine.
     sd: the checkpoint's `state_dict` entry (keys decoder.estimator.*, spk_emb.weight, fake_speaker, fake_content, mel_mean,
     mel_std); cfg: config.stabletts_cfm_config.  Convs go in the FFMA layout (q, k, v stacked into one 1x1 conv), the small
     linears of the conditioning path (time_mlp, each block's film conv and adaLN_modulation) row-major [out][in] and stacked
     over the blocks.  Everything is fp32: the decoder runs on the FFMA pipe in every precision mode, so there are no
     mode-dependent split planes to add yet.  vocoder: (folded Generator state dict, config.hifigan_config) appended as
-    pack_hifigan lays it out, or None."""
+    pack_hifigan lays it out, or None; bert: (BertModel state dict, config.bert_config, tc) appended as pack_bert lays it out,
+    or None."""
     P = _Packer()
     _pack_stabletts_decoder(P, sd, cfg)
     if vocoder is not None:
         _pack_hifigan(P, *vocoder)
+    if bert is not None:
+        _pack_bert(P, *bert)
     return P.finish()
 
 
-def pack_stabletts(sd, cfg, vocoder=None):
+def pack_stabletts(sd, cfg, vocoder=None, bert=None):
     """A MatchaTTS (StableTTS) state dict without its vocoder -> (blob, manifest) of an engine that serves text-to-mel
     (vtts_stabletts_synthesise) and the decoder alone: the decoder part of pack_stabletts_cfm, then the text encoder
     (encoder.emb, encoder.punc_emb, encoder.bert_proj.1, both stacks encoder.encoder / encoder.dp_encoder with their proj) and
-    dur_spk_emb.  cfg: config.stabletts_config; vocoder as in pack_stabletts_cfm."""
+    dur_spk_emb.  cfg: config.stabletts_config; vocoder as in pack_stabletts_cfm; bert: (BertModel state dict, config.bert_config,
+    tc) appended as pack_bert lays it out, or None."""
     if "enc_n_layers" not in cfg:
         raise ValueError("pack_stabletts needs config.stabletts_config (the text encoder's constants), not stabletts_cfm_config")
     g, want = _sd_getter(sd)
@@ -820,4 +918,6 @@ def pack_stabletts(sd, cfg, vocoder=None):
         P.conv(dst + ".proj", want(src + "proj.weight", (co, H, 1)), g(src + "proj.bias"))
     if vocoder is not None:
         _pack_hifigan(P, *vocoder)
+    if bert is not None:
+        _pack_bert(P, *bert)
     return P.finish()
