@@ -304,6 +304,50 @@ int vtts_debug_conv(vtts_handle h, int use_tc, int B, const int* lens, int rmul,
 /* Launch-shape log of the dense conv launches: mode 1 clears and starts it, 0 stops it, 2 copies up to max_n entries (one
  * per launch the host enqueued since it was started; graph replays enqueue none) and sets *n_out. */
 int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_n, int* n_out);
+/* Unit-test hooks for the duration path: each runs the kernels of one stage through the engine's own launch code, on host
+ * tensors.  B, lens: utterances packed as the engine packs them (utterance b starts at row offs[b], SEQ_GAP (8) rows between
+ * consecutive utterances); every row buffer has `rows` rows (>= the packed utterances), and rows outside the utterances keep
+ * what the caller wrote in every in/out buffer.  Malformed arguments return VTTS_ERR_INVALID before anything is launched.
+ *
+ * vtts_debug_dds: the three DDSConv layers (dilations 1, k, k^2; dds_layer_kernel) of `stack` of the loaded model, launched
+ * as dds_stack launches them:
+ *   "dp.convs"              x fp32 [rows][dp_filter_channels]; x0 and cond NULL
+ *   "dp.flows.<i>.convs"    the ConvFlow at the reference's module index i = 2n - 1 (n = 2 .. dp_n_flows), its front
+ *                           pre(x0) + cond fused into layer 0: x0 fp32 [rows], cond fp32 [rows][dp_filter_channels]; x NULL
+ *   y                       out (in/out) fp32 [3][rows][dp_filter_channels]: the output of each layer (layer i > 0 reads
+ *                           layer i - 1's); y[2] is the stack's result */
+int vtts_debug_dds(vtts_handle h, const char* stack, int B, const int* lens, size_t rows, const float* x, const float* x0,
+                   const float* cond, float* y);
+/* vtts_debug_spline: spline_inverse_kernel on params fp32 [rows][ldh] (widths | heights | interior derivatives, 3 * nb - 1
+ * used, unscaled as the ConvFlow's proj writes them) and x1 fp32 [rows] (in place), with the engine's dp_num_bins (nb),
+ * dp_tail_bound and sqrt(dp_filter_channels). */
+int vtts_debug_spline(vtts_handle h, int B, const int* lens, size_t rows, const float* params, int ldh, float* x1);
+/* vtts_debug_durations: duration_kernel, then sample_prior_kernel, as phase 1 and phase 2 run them.
+ *   z [rows]                    the flows' output x1 channel; logw = (z - m) * exp(-logs) with the model's ElementwiseAffine
+ *   length_scale, frame_cap     frame_cap > 0: the frame count a speculative second phase is sized for (0: none)
+ *   stats [rows][2I], eps [B][I][eps_ld], noise_scale    the prior: z_p = m + eps * exp(logs) * noise_scale (I = inter_channels)
+ *   wceil, cum [rows]           out (in/out) int: ceil durations and their inclusive scan
+ *   ylen, ylen_real [B]         out: the device frame lengths (capped at frame_cap) and the true ones
+ *   frm_off [B + 1]             out: the device frame offsets (capped layout)
+ *   published [2B + 1]          out: the lengths and offsets the host reads (uncapped)
+ *   z_p [frame_rows][I], frame_token [frame_rows]    out (in/out): the prior sample and token of every frame
+ * Durations summing past INT32_MAX frames (an utterance, or the batch's frame rows) return VTTS_ERR_INVALID after the
+ * duration kernel, as vtts_durations does; frame_rows or eps_ld too small return VTTS_ERR_CAPACITY. */
+int vtts_debug_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* z, float length_scale, int frame_cap,
+                         const float* stats, const float* eps, int64_t eps_ld, float noise_scale, int32_t* wceil, int32_t* cum,
+                         int32_t* ylen, int32_t* ylen_real, int32_t* frm_off, int32_t* published, size_t frame_rows, float* z_p,
+                         int32_t* frame_token);
+/* vtts_debug_stt_durations (StableTTS engines with a text encoder): stt_dur_kernel, stt_expand_kernel, stt_pause_fill_kernel.
+ *   mu_dp [rows][dur_channels], pause [rows], length_scale      the duration rule's inputs (pauses as given, unchecked)
+ *   x [rows][cond_channels], mu_mel [rows][noise_channels]      token rows expanded to frames (mu_mel may be NULL without prior)
+ *   denormalise                 prior rows times mel_std plus mel_mean
+ *   dur, first [rows] int, logw [rows], ylen [B]     out (dur, first, logw in/out): durations, first frames, pre-rounding values
+ *   mu [frame_rows][cond_channels], pau [frame_rows], prior [frame_rows][noise_channels] or NULL    out (in/out): the expansion
+ *   mel [frame_rows][noise_channels]    in/out: the pause fill runs on it
+ * Frame rows are packed from ylen as the mel phase packs them; frame_rows too small returns VTTS_ERR_CAPACITY. */
+int vtts_debug_stt_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* mu_dp, const float* pause,
+                             float length_scale, const float* x, const float* mu_mel, int denormalise, int32_t* dur, int32_t* first,
+                             int32_t* ylen, float* logw, size_t frame_rows, float* mu, float* pau, float* prior, float* mel);
 /* The split-K plan the engine makes for one grouped tensor-core conv launch, computed on the host alone (no device, no
  * engine).  Problems p < n (1..4): cin[p] (a multiple of 64), cout[p], k[p], in_extra[p]; B utterances of lens[b] <= max_len
  * rows / rmul; bn 64 / 128 pins the tile width (0: either); max_split caps the cluster size (8: none); min_steps = k-steps

@@ -338,7 +338,14 @@ struct vtts_engine {
     if (!map.p || map.p[0] != call_seq) return false;
     h_frm_len.assign(map.p + 1, map.p + 1 + B);
     h_frm_off.assign(map.p + 1 + B, map.p + 1 + 2 * B + 1);
+    check_frame_lengths(h_frm_len.data(), h_frm_off[B], B);
     return true;
+  }
+  // The frame lengths duration_kernel leaves: -1 for an utterance whose durations sum past INT32_MAX frames, and a total
+  // offset of -1 for a batch whose frame rows do not fit an int (the engine indexes frame rows with int).
+  static void check_frame_lengths(const int* len, int total, int n) {
+    for (int b = 0; b < n; ++b) REQUIRE(len[b] >= 1, VTTS_ERR_INVALID, "an utterance's durations sum past INT32_MAX frames");
+    REQUIRE(total >= 0, VTTS_ERR_INVALID, "the batch's durations sum past INT32_MAX frames");
   }
   int eps_dp_ld = 0;                 // row pitch of the duration-predictor noise the phase-1 kernels read
   static int bucket_tok(int n) { return n <= 256 ? (n + 15) / 16 * 16 : (n + 63) / 64 * 64; }
@@ -392,7 +399,7 @@ struct vtts_engine {
 
   // ---- workspace
   Buf<int> d_ids, d_tok_len, d_tok_off, d_sid, d_wceil, d_cum, d_frm_len, d_frm_off, d_ftok, d_done_ctr, d_frm_len_real;
-  Buf<float> d_condv, d_x, d_xb, d_qkv, d_ao, d_y, d_ffh, d_stats, d_dA, d_dB, d_dx, d_h29, d_za, d_zb, d_eps_dp;
+  Buf<float> d_condv, d_x, d_xb, d_qkv, d_ao, d_y, d_ffh, d_stats, d_dA, d_dB, d_dx, d_spl, d_za, d_zb, d_eps_dp;
   Buf<float> d_z, d_h, d_h1, d_wx, d_acts, d_skip, d_fqkv, d_fao, d_fy, d_ffh2, d_eps_z, d_d0, d_post, d_wav;
   std::vector<Buf<float>> d_stage;               // X_i
   std::vector<std::vector<Buf<float>>> d_xj, d_tmp;
@@ -649,6 +656,8 @@ struct vtts_engine {
                      int ks, const float* vec_after, int vec_ld, const float* cadd_after, const Rows& r);
   void dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const Rows& r,
                  const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
+  void dds_layer(const DdsW& d, int C, int k, int dil, const float* x, float* y, const Rows& r,
+                 const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
   struct P1Pin { int *len, *off, *sid, *ids; float *prm, *eps; };
   P1Pin p1_layout(bool eps);
   P1Pin stage_tokens(const int64_t* ids, int t_max, bool eps);
@@ -898,7 +907,7 @@ void vtts_engine::bind_weights() {
   const int fheads = c.flow_n_heads > 0 ? c.flow_n_heads : 2;      // models.py:355: the flow's pre_transformer always has 2 heads
   REQUIRE(!c.use_transformer_flows || ((H / fheads) % 32 == 0 && H / fheads <= 128 && H % fheads == 0), VTTS_ERR_INVALID,
           "flow head dim must be 32/64/96/128");
-  REQUIRE(c.dp_num_bins <= SPL_MAXB, VTTS_ERR_INVALID, "too many spline bins");
+  REQUIRE(c.dp_num_bins >= 1 && c.dp_num_bins <= SPL_MAXB, VTTS_ERR_INVALID, "dp_num_bins must be in [1, 16]");
   REQUIRE(c.dp_kernel_size % 2 == 1 && c.flow_kernel_size % 2 == 1, VTTS_ERR_INVALID, "odd kernels expected");
   REQUIRE(c.n_resblock_kernels <= CV_MAXP, VTTS_ERR_INVALID, "at most 4 resblocks per stage");
   has_g = c.n_speakers > 0 && G > 0;
@@ -1962,24 +1971,30 @@ void vtts_engine::dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, c
                             const float* x0, const float* pre_w, const float* pre_b, const float* cond) {
   int dil = 1;
   for (int i = 0; i < 3; ++i) {
-    DdsP P;
-    P.x = a; P.y = b;
-    P.x0 = (i == 0) ? x0 : nullptr; P.pre_w = pre_w; P.pre_b = pre_b; P.cond = cond;
-    P.sep_w = d[i].sep_w; P.sep_b = d[i].sep_b;
-    P.ln1g = d[i].ln1.g; P.ln1b = d[i].ln1.b;
-    P.pw_w = d[i].pw.w; P.pw_b = d[i].pw.b; P.ldw = d[i].pw.ldw;
-    P.ln2g = d[i].ln2.g; P.ln2b = d[i].ln2.b;
-    P.C = C; P.k = k; P.dil = dil;
-    // (16 positions per CTA were tried for batched calls -- 4x less weight streaming per position -- and measured slower:
-    //  duration stage 3.20 vs 2.95 ms at batch 64)
-    dim3 grid((r.maxLen + DDS_TT - 1) / DDS_TT, r.n);
-    const size_t smem = ((size_t)DDS_NS * DDS_CH * C + (size_t)C * DDS_TT + 8 * DDS_TT) * sizeof(float);
-    klaunch(dds_layer_kernel<DDS_TT>, dim3(grid), dim3(C), (size_t)(smem), P, r.lens, r.offs);
-    CK(cudaGetLastError());
-    ++launches;
+    dds_layer(d[i], C, k, dil, a, b, r, i == 0 ? x0 : nullptr, pre_w, pre_b, cond);
     std::swap(a, b);
     dil *= k;
   }
+}
+
+// One DDSConv layer x -> y; with x0 set the layer's input is the ConvFlow front pre_w * x0 + pre_b + cond instead of x.
+void vtts_engine::dds_layer(const DdsW& d, int C, int k, int dil, const float* x, float* y, const Rows& r,
+                            const float* x0, const float* pre_w, const float* pre_b, const float* cond) {
+  DdsP P;
+  P.x = x; P.y = y;
+  P.x0 = x0; P.pre_w = pre_w; P.pre_b = pre_b; P.cond = cond;
+  P.sep_w = d.sep_w; P.sep_b = d.sep_b;
+  P.ln1g = d.ln1.g; P.ln1b = d.ln1.b;
+  P.pw_w = d.pw.w; P.pw_b = d.pw.b; P.ldw = d.pw.ldw;
+  P.ln2g = d.ln2.g; P.ln2b = d.ln2.b;
+  P.C = C; P.k = k; P.dil = dil;
+  // (16 positions per CTA were tried for batched calls -- 4x less weight streaming per position -- and measured slower:
+  //  duration stage 3.20 vs 2.95 ms at batch 64)
+  dim3 grid((r.maxLen + DDS_TT - 1) / DDS_TT, r.n);
+  const size_t smem = ((size_t)DDS_NS * DDS_CH * C + (size_t)C * DDS_TT + 8 * DDS_TT) * sizeof(float);
+  klaunch(dds_layer_kernel<DDS_TT>, dim3(grid), dim3(C), (size_t)(smem), P, r.lens, r.offs);
+  CK(cudaGetLastError());
+  ++launches;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -2047,7 +2062,9 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   float* dA = ensure(d_dA, T * D);
   float* dB = ensure(d_dB, T * D);
   float* dx = ensure(d_dx, T * D);
-  float* h29 = ensure(d_h29, T * 32);
+  // spline parameters of a ConvFlow (3 * nbins - 1 per token; rows padded to float4)
+  const int nbins = c.dp_num_bins, ldh = spline_pitch(nbins);
+  float* spl = ensure(d_spl, T * ldh);
   float* za = ensure(d_za, T);
   float* zb = ensure(d_zb, T);
   {
@@ -2068,17 +2085,15 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   }
   float* cvar = zb;   // conditioning half (x0 after the Flip)
   float* tvar = za;   // transformed half (x1)
-  const int nbins = c.dp_num_bins;
-  REQUIRE(3 * nbins - 1 <= 32, VTTS_ERR_INVALID, "spline parameter row too wide");
   for (int n = c.dp_n_flows; n >= 2; --n) {
     const CfW& F = cf[n - 2];
     // (the ConvFlow front h = pre(x0) + cond, modules.py:366-367, is computed inside the first DDS layer)
     float *a = dA, *b = dB;
     dds_stack(F.dds, D, c.dp_kernel_size, a, b, r, cvar, F.pre_w, F.pre_b, dx);
-    launch_conv({mk(F.proj, a, D, 0, h29, 32, 0, 1, 0)}, 1, r);
+    launch_conv({mk(F.proj, a, D, 0, spl, ldh, 0, 1, 0)}, 1, r);
     {
       dim3 g((maxTok + 127) / 128, B);
-      klaunch(spline_inverse_kernel, dim3(g), dim3(128), (size_t)(0), h29, 32, tvar, nbins, c.dp_tail_bound, sqrtf((float)D), tl, to);
+      klaunch(spline_inverse_kernel, dim3(g), dim3(128), (size_t)(0), spl, ldh, tvar, nbins, c.dp_tail_bound, sqrtf((float)D), tl, to);
       CK(cudaGetLastError());
       ++launches;
     }
@@ -2271,6 +2286,7 @@ void vtts_engine::finish1() {
   const int* p_len = reinterpret_cast<const int*>(h_pin_len.p);
   h_frm_len.assign(p_len, p_len + B);
   h_frm_off.assign(p_len + B, p_len + 2 * B + 1);
+  check_frame_lengths(h_frm_len.data(), h_frm_off[B], B);
   set_frame_shape();
   have_durations = true;
 }
@@ -5422,6 +5438,221 @@ int vtts_debug_conv_log(vtts_handle h, int mode, vtts_conv_report* out, int max_
       *n_out = n;
     }
   }, G_ATOMIC, ANY_FAMILY);
+}
+
+// ---- Unit-test hooks of the duration path (include/vtts.h): the kernels' own launches on host tensors.
+namespace {
+
+// Utterances of the duration hooks packed as the engine packs them (pack_rows), checked against the caller's row count;
+// `dev` receives their device copy [lens B][offs B + 1].
+struct HookRows {
+  std::vector<int> len, off;
+  int maxLen = 0;
+  int* d = nullptr;
+  const int* lens() const { return d; }
+  const int* offs() const { return d + len.size(); }
+};
+HookRows hook_rows(const char* who, int B, const int* lens, size_t rows) {
+  REQUIRE(lens && B >= 1 && B <= 16384, VTTS_ERR_INVALID, std::string(who) + ": bad batch size or missing lengths");
+  HookRows hr;
+  hr.len.assign(lens, lens + B);
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lens[b] >= 1, VTTS_ERR_INVALID, std::string(who) + ": lengths must be >= 1");
+    hr.maxLen = std::max(hr.maxLen, lens[b]);
+  }
+  vtts_engine::pack_rows(hr.len, hr.off);
+  REQUIRE(rows >= (size_t)hr.off[B], VTTS_ERR_INVALID, std::string(who) + ": fewer rows than the packed utterances");
+  return hr;
+}
+void upload_rows(HookRows& hr, std::vector<Buf<char>>& dev, cudaStream_t st) {
+  std::vector<int> lo(hr.len);
+  lo.insert(lo.end(), hr.off.begin(), hr.off.end());
+  hr.d = static_cast<int*>(upload(dev, lo.data(), lo.size() * sizeof(int), st));
+}
+
+}  // namespace
+
+int vtts_debug_dds(vtts_handle h, const char* stack, int B, const int* lens, size_t rows, const float* x, const float* x0,
+                   const float* cond, float* y) {
+  return guarded(h, [&] {
+    REQUIRE(stack && y, VTTS_ERR_INVALID, "debug_dds: missing stack or output");
+    const vtts_config& c = h->cfg;
+    const int D = c.dp_filter_channels;
+    const std::string nm(stack);
+    const DdsW* d = nullptr;
+    const CfW* F = nullptr;
+    if (nm == "dp.convs") {
+      d = h->dp_dds;
+    } else if (nm.rfind("dp.flows.", 0) == 0 && nm.size() > 15 && nm.compare(nm.size() - 6, 6, ".convs") == 0) {
+      // the reference's module index: the ConvFlow n (2 .. dp_n_flows) is dp.flows.<2n - 1>
+      const std::string idx = nm.substr(9, nm.size() - 15);
+      REQUIRE(idx.size() <= 3 && idx.find_first_not_of("0123456789") == std::string::npos, VTTS_ERR_INVALID,
+              "debug_dds: stack must be dp.convs or dp.flows.<2n-1>.convs");
+      const int i = atoi(idx.c_str()), n = (i + 1) / 2;
+      REQUIRE(i % 2 == 1 && n >= 2 && n <= c.dp_n_flows, VTTS_ERR_INVALID, "debug_dds: no such ConvFlow");
+      F = &h->cf[n - 2];
+      d = F->dds;
+    }
+    REQUIRE(d != nullptr, VTTS_ERR_INVALID, "debug_dds: stack must be dp.convs or dp.flows.<2n-1>.convs");
+    REQUIRE(F ? (x0 && cond && !x) : (x && !x0 && !cond), VTTS_ERR_INVALID,
+            "debug_dds: dp.convs takes x, a ConvFlow stack takes x0 and cond");
+    HookRows hr = hook_rows("debug_dds", B, lens, rows);
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * D;
+    // the layers of dds_stack, each into its own buffer holding the caller's rows, so that every layer can be checked on
+    // the kernel's own input
+    const float* in = static_cast<const float*>(upload(dev, x, n * sizeof(float), st));
+    float* out = static_cast<float*>(upload(dev, y, 3 * n * sizeof(float), st));
+    const float* dx0 = F ? static_cast<const float*>(upload(dev, x0, rows * sizeof(float), st)) : nullptr;
+    const float* dc = F ? static_cast<const float*>(upload(dev, cond, n * sizeof(float), st)) : nullptr;
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    for (int i = 0, dil = 1; i < 3; ++i, dil *= c.dp_kernel_size) {
+      h->dds_layer(d[i], D, c.dp_kernel_size, dil, in, out + i * n, r, i == 0 ? dx0 : nullptr, F ? F->pre_w : nullptr,
+                   F ? F->pre_b : nullptr, dc);
+      in = out + i * n;
+    }
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(y, out, 3 * n * sizeof(float), cudaMemcpyDeviceToHost));
+  });
+}
+
+int vtts_debug_spline(vtts_handle h, int B, const int* lens, size_t rows, const float* params, int ldh, float* x1) {
+  return guarded(h, [&] {
+    const vtts_config& c = h->cfg;
+    REQUIRE(params && x1, VTTS_ERR_INVALID, "debug_spline: missing parameters or x1");
+    REQUIRE(ldh >= 3 * c.dp_num_bins - 1, VTTS_ERR_INVALID, "debug_spline: parameter rows narrower than 3 * dp_num_bins - 1");
+    HookRows hr = hook_rows("debug_spline", B, lens, rows);
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const float* dp = static_cast<const float*>(upload(dev, params, rows * ldh * sizeof(float), st));
+    float* dx = static_cast<float*>(upload(dev, x1, rows * sizeof(float), st));
+    h->klaunch(spline_inverse_kernel, dim3((hr.maxLen + 127) / 128, B), dim3(128), (size_t)0, dp, ldh, dx, c.dp_num_bins, c.dp_tail_bound,
+               sqrtf((float)c.dp_filter_channels), hr.lens(), hr.offs());
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(x1, dx, rows * sizeof(float), cudaMemcpyDeviceToHost));
+  });
+}
+
+int vtts_debug_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* z, float length_scale, int frame_cap,
+                         const float* stats, const float* eps, int64_t eps_ld, float noise_scale, int32_t* wceil, int32_t* cum,
+                         int32_t* ylen, int32_t* ylen_real, int32_t* frm_off, int32_t* published, size_t frame_rows, float* z_p,
+                         int32_t* frame_token) {
+  return guarded(h, [&] {
+    REQUIRE(z && stats && eps && wceil && cum && ylen && ylen_real && frm_off && published && z_p && frame_token, VTTS_ERR_INVALID,
+            "debug_durations: missing input or output");
+    REQUIRE(frame_cap >= 0 && eps_ld >= 1, VTTS_ERR_INVALID, "debug_durations: frame_cap must be >= 0 and eps_ld >= 1");
+    HookRows hr = hook_rows("debug_durations", B, lens, rows);
+    const int I = h->cfg.inter_channels;
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    float prm[8] = {noise_scale, length_scale, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const int seq = 1;
+    memcpy(&prm[6], &seq, 4);
+    memcpy(&prm[7], &frame_cap, 4);
+    const float* dprm = static_cast<const float*>(upload(dev, prm, sizeof(prm), st));
+    const float* dz = static_cast<const float*>(upload(dev, z, rows * sizeof(float), st));
+    int* dwc = static_cast<int*>(upload(dev, wceil, rows * sizeof(int), st));
+    int* dcum = static_cast<int*>(upload(dev, cum, rows * sizeof(int), st));
+    int* dlen = static_cast<int*>(upload(dev, nullptr, (3 * (size_t)B + 1) * sizeof(int), st));   // ylen | ylen_real | offsets
+    MappedBuf<int> pub;
+    CK(pub.alloc(2 * (size_t)B + 2));
+    pub.p[0] = 0;
+    // the engine's own ticket counter: it must be back at 0 after every launch
+    unsigned int* dctr = reinterpret_cast<unsigned int*>(h->ensure(h->d_done_ctr, 4));
+    h->klaunch(duration_kernel, dim3(B), dim3(256), (size_t)0, dz, h->dp_ea, 0, 2, dprm, dwc, dcum, dlen, hr.lens(), hr.offs(),
+               dlen + 2 * B, B, (volatile int*)pub.d, dctr, dlen + B);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    REQUIRE(pub.p[0] == seq, VTTS_ERR_CUDA, "debug_durations: the lengths were not published");
+    CK(cudaMemcpy(wceil, dwc, rows * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(cum, dcum, rows * sizeof(int), cudaMemcpyDeviceToHost));
+    std::vector<int> lo(3 * B + 1);
+    CK(cudaMemcpy(lo.data(), dlen, lo.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    std::copy(lo.begin(), lo.begin() + B, ylen);
+    std::copy(lo.begin() + B, lo.begin() + 2 * B, ylen_real);
+    std::copy(lo.begin() + 2 * B, lo.end(), frm_off);
+    std::copy(pub.p + 1, pub.p + 2 * B + 2, published);
+    // what the host reads, refused as the engine refuses it; then the prior over the device lengths, as phase 2 runs it
+    vtts_engine::check_frame_lengths(pub.p + 1, pub.p[2 * B + 1], B);
+    int maxFrm = 0;
+    for (int b = 0; b < B; ++b) maxFrm = std::max(maxFrm, lo[b]);
+    REQUIRE((size_t)lo[3 * B] <= frame_rows, VTTS_ERR_CAPACITY, "debug_durations: fewer frame rows than the packed frames");
+    REQUIRE(eps_ld >= maxFrm, VTTS_ERR_CAPACITY, "debug_durations: eps_ld is smaller than the longest utterance's frames");
+    const float* dst = static_cast<const float*>(upload(dev, stats, (size_t)hr.off[B] * 2 * I * sizeof(float), st));
+    const float* deps = static_cast<const float*>(upload(dev, eps, (size_t)B * I * eps_ld * sizeof(float), st));
+    float* dzp = static_cast<float*>(upload(dev, z_p, frame_rows * I * sizeof(float), st));
+    int* dft = static_cast<int*>(upload(dev, frame_token, frame_rows * sizeof(int), st));
+    h->klaunch(sample_prior_kernel, dim3(maxFrm, B), dim3(64), (size_t)0, dst, I, (const int*)dcum, hr.lens(), hr.offs(),
+               (const int*)dlen, (const int*)(dlen + 2 * B), deps, (int)eps_ld, dprm, dzp, dft);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(z_p, dzp, frame_rows * I * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(frame_token, dft, frame_rows * sizeof(int), cudaMemcpyDeviceToHost));
+  });
+}
+
+int vtts_debug_stt_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* mu_dp, const float* pause,
+                             float length_scale, const float* x, const float* mu_mel, int denormalise, int32_t* dur, int32_t* first,
+                             int32_t* ylen, float* logw, size_t frame_rows, float* mu, float* pau, float* prior, float* mel) {
+  return guarded(h, [&] {
+    const vtts_config& c = h->cfg;
+    REQUIRE(h->st_text, VTTS_ERR_INVALID, "debug_stt_durations: the engine has no text encoder");
+    REQUIRE(mu_dp && pause && x && dur && first && ylen && logw && mu && pau && mel, VTTS_ERR_INVALID,
+            "debug_stt_durations: missing input or output");
+    REQUIRE(!prior || mu_mel, VTTS_ERR_INVALID, "debug_stt_durations: the prior rows need mu_mel");
+    HookRows hr = hook_rows("debug_stt_durations", B, lens, rows);
+    const int DC = c.st_dur_channels, MC = c.st_cond, NC = c.st_noise;
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    float prm[16] = {length_scale, 0.f, denormalise ? 1.f : 0.f};
+    const float* dprm = static_cast<const float*>(upload(dev, prm, sizeof(prm), st));
+    const float* dmu = static_cast<const float*>(upload(dev, mu_dp, rows * DC * sizeof(float), st));
+    const float* dpause = static_cast<const float*>(upload(dev, pause, rows * sizeof(float), st));
+    int* ddur = static_cast<int*>(upload(dev, dur, rows * sizeof(int), st));
+    int* dfirst = static_cast<int*>(upload(dev, first, rows * sizeof(int), st));
+    float* dlogw = static_cast<float*>(upload(dev, logw, rows * sizeof(float), st));
+    int* dylen = static_cast<int*>(upload(dev, nullptr, (size_t)B * sizeof(int), st));
+    h->klaunch(stt_dur_kernel, dim3(B), dim3(STT_SCAN), (size_t)0, dmu, DC, DC, dpause, dprm, (float)VTTS_ST_MAX_TOKEN_FRAMES, ddur, dfirst,
+               dylen, dlogw, hr.lens(), hr.offs());
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(dur, ddur, rows * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(first, dfirst, rows * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(logw, dlogw, rows * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(ylen, dylen, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost));
+    // frame rows of the utterances, packed as the mel phase packs them
+    HookRows fr;
+    fr.len.assign(ylen, ylen + B);
+    for (int b = 0; b < B; ++b) fr.maxLen = std::max(fr.maxLen, ylen[b]);
+    vtts_engine::pack_rows(fr.len, fr.off);
+    REQUIRE((size_t)fr.off[B] <= frame_rows, VTTS_ERR_CAPACITY, "debug_stt_durations: fewer frame rows than the packed frames");
+    upload_rows(fr, dev, st);
+    const float* dx = static_cast<const float*>(upload(dev, x, rows * MC * sizeof(float), st));
+    const float* dmm = mu_mel ? static_cast<const float*>(upload(dev, mu_mel, rows * NC * sizeof(float), st)) : nullptr;
+    float* dmuf = static_cast<float*>(upload(dev, mu, frame_rows * MC * sizeof(float), st));
+    float* dpau = static_cast<float*>(upload(dev, pau, frame_rows * sizeof(float), st));
+    float* dprior = prior ? static_cast<float*>(upload(dev, prior, frame_rows * NC * sizeof(float), st)) : nullptr;
+    float* dmel = static_cast<float*>(upload(dev, mel, frame_rows * NC * sizeof(float), st));
+    h->klaunch(stt_expand_kernel, dim3(hr.maxLen, B), dim3(128), (size_t)0, dx, MC, dpause, dmm, NC, (const int*)ddur, (const int*)dfirst,
+               dmuf, dpau, dprior, dprm, h->st_mel_mean, h->st_mel_std, hr.lens(), hr.offs(), fr.offs());
+    h->klaunch(stt_pause_fill_kernel, dim3(fr.maxLen, B), dim3(128), (size_t)0, dmel, NC, (const float*)dpau, fr.lens(), fr.offs());
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(mu, dmuf, frame_rows * MC * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(pau, dpau, frame_rows * sizeof(float), cudaMemcpyDeviceToHost));
+    if (prior) CK(cudaMemcpy(prior, dprior, frame_rows * NC * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(mel, dmel, frame_rows * NC * sizeof(float), cudaMemcpyDeviceToHost));
+  }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
 }
 
 // Host-only restatement of launch_tc's split-K plan (tc_split_plan) for tests: no device, no engine.

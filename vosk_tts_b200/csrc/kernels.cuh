@@ -1252,6 +1252,8 @@ __global__ void dp_noise_kernel(const float* __restrict__ eps, int eps_ld, const
 // (no FMA contraction) because ceil() of the resulting duration must be bit-stable.
 // ------------------------------------------------------------------------------------------------
 constexpr int SPL_MAXB = 16;
+// row pitch of the parameter rows: 3 * nb - 1 floats (widths, heights, interior derivatives) padded to a float4
+constexpr int spline_pitch(int nb) { return (3 * nb - 1 + 3) / 4 * 4; }
 
 __global__ void spline_inverse_kernel(const float* __restrict__ h, int ldh, float* __restrict__ x1, int nb, float bound,
                                       float sqrt_filter, const int* __restrict__ lens, const int* __restrict__ offs) {
@@ -1319,7 +1321,9 @@ constexpr int SEQ_GAP = 8;
 // ------------------------------------------------------------------------------------------------
 // Durations (models.py:1689-1691; modules.py:296 for the ElementwiseAffine inverse):
 //   logw = (z - m) * exp(-logs);  w = exp(logw) * length_scale;  w_ceil = ceil(w);  cum = cumsum(w_ceil)
-// One CTA per utterance; y_len = max(sum, 1).
+// One CTA per utterance; y_len = max(sum, 1).  A token has at most 1e6 frames, so one 256-token pass sums to well inside
+// an int, but a long utterance or batch can pass INT32_MAX frames: the running sums are 64-bit, and an utterance whose frames
+// do not fit an int gets y_len -1, a batch whose frame layout does not fit gets the total offset -1 (the host refuses both).
 // ------------------------------------------------------------------------------------------------
 __global__ void duration_kernel(const float* __restrict__ z, const float* __restrict__ ea, int ea_ch, int ea_n, const float* __restrict__ prm,
                                 int* __restrict__ wceil, int* __restrict__ cum, int* __restrict__ ylen,
@@ -1332,7 +1336,7 @@ __global__ void duration_kernel(const float* __restrict__ z, const float* __rest
   const int len = lens[b];
   const long base = offs[b];
   __shared__ int part[1024];
-  __shared__ int carry;
+  __shared__ long long carry;
   const float length_scale = prm[1];
   const float m = ea[ea_ch], nlogs = -ea[ea_n + ea_ch];
   const float es = expf(nlogs);
@@ -1357,13 +1361,13 @@ __global__ void duration_kernel(const float* __restrict__ z, const float* __rest
       part[threadIdx.x] += add;
       __syncthreads();
     }
-    if (t < len) cum[base + t] = carry + part[threadIdx.x];
+    if (t < len) cum[base + t] = (int)(carry + part[threadIdx.x]);
     __syncthreads();
     if (threadIdx.x == blockDim.x - 1) carry += part[threadIdx.x];
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    ylen[b] = carry < 1 ? 1 : carry;
+    ylen[b] = carry > (long long)INT_MAX ? -1 : (carry < 1 ? 1 : (int)carry);
     // the block that finishes last lays the utterances out at frame resolution and publishes lengths + offsets to the host
     // (what frame_offsets_kernel does as a separate launch)
     __threadfence();
@@ -1374,21 +1378,23 @@ __global__ void duration_kernel(const float* __restrict__ z, const float* __rest
       // (speculative phase 2).  Its buffers, tensor maps and grids are sized for the bucket, so the device-side lengths it
       // reads are clamped to it; the host gets the true lengths, sees that the prediction was too small and repeats the
       // phase after restoring them from ylen_real (restore_lengths_kernel).
+      // (an utterance refused for its length, y_len -1, runs as `cap` frames in an already enqueued second phase)
       const int cap = __float_as_int(prm[7]);
-      int o = 0, o_real = 0;
+      long long o = 0, o_real = 0;
       for (int b2 = 0; b2 < B; ++b2) {
         const int yl = *((volatile int*)&ylen[b2]);
         ylen_real[b2] = yl;
-        const int ylc = (cap > 0 && yl > cap) ? cap : yl;
+        const int ylc = (cap > 0 && (yl > cap || yl < 1)) ? cap : yl;
         if (ylc != yl) ylen[b2] = ylc;
-        yoff[b2] = o;
-        if (host_out) { host_out[1 + b2] = yl; host_out[1 + B + b2] = o_real; }
+        yoff[b2] = (int)o;
+        if (host_out) { host_out[1 + b2] = yl; host_out[1 + B + b2] = (int)o_real; }
         o += ylc + (b2 + 1 < B ? SEQ_GAP : 0);
-        o_real += yl + (b2 + 1 < B ? SEQ_GAP : 0);
+        o_real += (long long)yl + (b2 + 1 < B ? SEQ_GAP : 0);
       }
-      yoff[B] = o;
+      const bool too_long = o_real > (long long)INT_MAX;
+      yoff[B] = too_long ? -1 : (int)o;
       if (host_out) {
-        host_out[1 + 2 * B] = o_real;
+        host_out[1 + 2 * B] = too_long ? -1 : (int)o_real;
         __threadfence_system();
         host_out[0] = __float_as_int(prm[6]);
       }

@@ -63,7 +63,8 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
-           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features"]
+           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features",
+           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -210,6 +211,16 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_conv.argtypes = [vp, i32, i32, vp, i32, i32, C.POINTER(ConvProblem), vp, C.c_size_t, i32, vp, C.c_size_t, vp,
                                     C.c_size_t, vp, C.c_size_t, i32, C.POINTER(ConvOverrides), C.POINTER(ConvReport)]
     lib.vtts_debug_conv.restype = i32
+    lib.vtts_debug_dds.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t, vp, vp, vp, vp]
+    lib.vtts_debug_dds.restype = i32
+    lib.vtts_debug_spline.argtypes = [vp, i32, vp, C.c_size_t, vp, i32, vp]
+    lib.vtts_debug_spline.restype = i32
+    lib.vtts_debug_durations.argtypes = [vp, i32, vp, C.c_size_t, vp, C.c_float, i32, vp, vp, C.c_int64, C.c_float, vp, vp, vp, vp,
+                                         vp, vp, C.c_size_t, vp, vp]
+    lib.vtts_debug_durations.restype = i32
+    lib.vtts_debug_stt_durations.argtypes = [vp, i32, vp, C.c_size_t, vp, vp, C.c_float, vp, vp, i32, vp, vp, vp, vp, C.c_size_t,
+                                             vp, vp, vp, vp]
+    lib.vtts_debug_stt_durations.restype = i32
     lib.vtts_debug_conv_log.argtypes = [vp, i32, C.POINTER(ConvReport), i32, C.POINTER(C.c_int)]
     lib.vtts_debug_conv_log.restype = i32
     lib.vtts_tc_split_plan.argtypes = [i32, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp]
@@ -1081,6 +1092,97 @@ class Engine:
             _ptr(planes), 0 if planes is None else planes.shape[1], 0 if planes is None else planes.shape[0],
             None if ov is None else C.byref(ov), C.byref(rep)))
         return y, planes, rep.as_dict()
+
+    def _hook_arrays(self, spec):
+        """Contiguous copies of a debug hook's arrays, each checked against its shape: spec is a list of (name, array or None,
+        dtype, shape); a shape entry None takes any extent.  Raises ValueError before anything reaches the library."""
+        out = []
+        for name, a, dt, shape in spec:
+            if a is None:
+                out.append(None)
+                continue
+            a = np.ascontiguousarray(a, dtype=dt).copy()
+            if a.ndim != len(shape) or any(n is not None and a.shape[i] != n for i, n in enumerate(shape)):
+                raise ValueError("%s: shape %s, expected %s" % (name, a.shape, tuple("*" if n is None else n for n in shape)))
+            out.append(a)
+        return out
+
+    def debug_dds(self, stack, lens, y, x=None, x0=None, cond=None):
+        """The three DDSConv layers of `stack` ("dp.convs" with x, or "dp.flows.<i>.convs" with x0 and cond), launched as
+        dds_stack launches them (vtts_debug_dds).  Rows packed as cr.offsets(lens); y: float32 [3, rows, D], rows outside the
+        utterances keep it.  Returns the new y: the output of every layer, each computed from the previous one."""
+        D = int(self.cfg["dp_filter_channels"])
+        y = np.ascontiguousarray(y, dtype=np.float32)
+        rows = y.shape[1] if y.ndim == 3 else -1
+        y, x, x0, cond = self._hook_arrays([("y", y, np.float32, (3, rows, D)), ("x", x, np.float32, (rows, D)),
+                                            ("x0", x0, np.float32, (rows,)), ("cond", cond, np.float32, (rows, D))])
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        self._check(self.lib.vtts_debug_dds(self.h, stack.encode(), lens.size, _ptr(lens), rows, _ptr(x), _ptr(x0), _ptr(cond),
+                                            _ptr(y)))
+        return y
+
+    def debug_spline(self, lens, params, x1):
+        """spline_inverse_kernel on params float32 [rows, ldh] and x1 float32 [rows] (vtts_debug_spline).  Returns the new x1."""
+        params = np.ascontiguousarray(params, dtype=np.float32)
+        if params.ndim != 2:
+            raise ValueError("params: shape %s, expected (rows, ldh)" % (params.shape,))
+        x1, = self._hook_arrays([("x1", x1, np.float32, (params.shape[0],))])
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        self._check(self.lib.vtts_debug_spline(self.h, lens.size, _ptr(lens), x1.shape[0], _ptr(params), params.shape[1], _ptr(x1)))
+        return x1
+
+    def debug_durations(self, lens, z, length_scale, stats, eps, noise_scale, frame_rows, frame_cap=0, wceil=None, cum=None, z_p=None,
+                        frame_token=None):
+        """duration_kernel then sample_prior_kernel (vtts_debug_durations).  z float32 [rows]; stats float32 [rows, 2I]; eps
+        float32 [B, I, eps_ld]; wceil / cum int32 [rows], z_p float32 [frame_rows, I], frame_token int32 [frame_rows]: initial
+        contents (default zeros) that rows outside the utterances keep.  Returns a dict of wceil, cum, ylen, ylen_real, frm_off,
+        published (host-read lengths [B] then offsets [B + 1]), z_p, frame_token."""
+        z = np.ascontiguousarray(z, dtype=np.float32)
+        rows, B, I, F = z.shape[0], len(lens), int(self.cfg["inter_channels"]), int(frame_rows)
+        if z.ndim != 1:
+            raise ValueError("z: shape %s, expected (rows,)" % (z.shape,))
+        zeros = lambda a, shape, dt: np.zeros(shape, dt) if a is None else a
+        stats, eps, wceil, cum, z_p, frame_token = self._hook_arrays([
+            ("stats", stats, np.float32, (rows, 2 * I)), ("eps", eps, np.float32, (B, I, None)),
+            ("wceil", zeros(wceil, rows, np.int32), np.int32, (rows,)), ("cum", zeros(cum, rows, np.int32), np.int32, (rows,)),
+            ("z_p", zeros(z_p, (F, I), np.float32), np.float32, (F, I)),
+            ("frame_token", zeros(frame_token, F, np.int32), np.int32, (F,))])
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        o = dict(wceil=wceil, cum=cum, ylen=np.zeros(B, np.int32), ylen_real=np.zeros(B, np.int32), frm_off=np.zeros(B + 1, np.int32),
+                 published=np.zeros(2 * B + 1, np.int32), z_p=z_p, frame_token=frame_token)
+        self._check(self.lib.vtts_debug_durations(
+            self.h, B, _ptr(lens), rows, _ptr(z), float(length_scale), int(frame_cap), _ptr(stats), _ptr(eps), eps.shape[-1],
+            float(noise_scale), _ptr(o["wceil"]), _ptr(o["cum"]), _ptr(o["ylen"]), _ptr(o["ylen_real"]), _ptr(o["frm_off"]),
+            _ptr(o["published"]), F, _ptr(o["z_p"]), _ptr(o["frame_token"])))
+        return o
+
+    def debug_stt_durations(self, lens, mu_dp, pause, length_scale, x, frame_rows, mu_mel=None, denormalise=False, prior=True,
+                            init=None):
+        """stt_dur_kernel, stt_expand_kernel and stt_pause_fill_kernel (vtts_debug_stt_durations).  mu_dp float32 [rows, DC],
+        pause [rows], x [rows, MC], mu_mel [rows, NC].  init: dict of initial dur / first / logw / mu / pau / prior / mel
+        buffers (default zeros), which rows outside the utterances keep.  Returns a dict of those and ylen."""
+        c = self.cfg
+        if "dur_channels" not in c:
+            raise ValueError("debug_stt_durations needs a StableTTS engine with a text encoder")
+        DC, MC, NC = int(c["dur_channels"]), int(c["cond_channels"]), int(c["noise_channels"])
+        mu_dp = np.ascontiguousarray(mu_dp, dtype=np.float32)
+        rows, B, F = mu_dp.shape[0], len(lens), int(frame_rows)
+        init = init or {}
+        buf = lambda k, shape, dt: init[k] if k in init else np.zeros(shape, dt)
+        (mu_dp, pause, x, mu_mel, dur, first, logw, mu, pau, pr, mel) = self._hook_arrays([
+            ("mu_dp", mu_dp, np.float32, (rows, DC)), ("pause", pause, np.float32, (rows,)), ("x", x, np.float32, (rows, MC)),
+            ("mu_mel", mu_mel, np.float32, (rows, NC)), ("dur", buf("dur", rows, np.int32), np.int32, (rows,)),
+            ("first", buf("first", rows, np.int32), np.int32, (rows,)), ("logw", buf("logw", rows, np.float32), np.float32, (rows,)),
+            ("mu", buf("mu", (F, MC), np.float32), np.float32, (F, MC)), ("pau", buf("pau", F, np.float32), np.float32, (F,)),
+            ("prior", buf("prior", (F, NC), np.float32) if prior else None, np.float32, (F, NC)),
+            ("mel", buf("mel", (F, NC), np.float32), np.float32, (F, NC))])
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        o = dict(dur=dur, first=first, ylen=np.zeros(B, np.int32), logw=logw, mu=mu, pau=pau, prior=pr, mel=mel)
+        self._check(self.lib.vtts_debug_stt_durations(
+            self.h, B, _ptr(lens), rows, _ptr(mu_dp), _ptr(pause), float(length_scale), _ptr(x), _ptr(mu_mel), int(bool(denormalise)),
+            _ptr(o["dur"]), _ptr(o["first"]), _ptr(o["ylen"]), _ptr(o["logw"]), F, _ptr(o["mu"]), _ptr(o["pau"]),
+            _ptr(o["prior"]), _ptr(o["mel"])))
+        return o
 
     def conv_log(self, mode):
         """Launch-shape log of the dense conv launches (vtts_debug_conv_log): 1 clears and starts it, 0 stops it, 2 returns the
