@@ -604,6 +604,24 @@ int vtts_stabletts_synthesise_wav(vtts_handle h, const int64_t* ids, const int64
  * outside the word table.  VTTS_ERR_CAPACITY: out_ld below a sentence's length. */
 int vtts_bert_features(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, float* out, int64_t out_ld);
 
+/* StableTTS text-to-waveform from word pieces: vtts_stabletts_synthesise_wav with each token's BERT row computed and gathered on
+ * the device (what vosk_tts/synth.py:25-87 does on the host with get_word_bert and the word index of g2p_multistream*): the
+ * text phase's graph runs BERT on every sentence's word pieces (as vtts_bert_features), then copies row bert_rows[b][t] of
+ * sentence b's rows to token t.  The [T, bert_dim] features never reach the host.  Arguments as
+ * vtts_stabletts_synthesise_wav, with `bert` replaced by
+ *   pieces        int64 [B, pieces_ld] WordPiece ids of sentence b ([CLS] ... [SEP]), its first piece_lengths[b]
+ *   bert_rows     int32 [B, t_max] the row among sentence b's pieces that token t reads, for t < id_lengths[b]
+ * Graphed per (batch, token bucket, BERT's longest-sentence and row buckets).  In every precision mode the outputs are
+ * bit-identical to vtts_bert_features, the same gather on the host and vtts_stabletts_synthesise_wav.  VTTS_ERR_INVALID, with
+ * nothing launched: also a blob without bt.*, st_bert_dim != cv_hidden, a row outside [0, piece_lengths[b]), and what
+ * vtts_bert_features refuses of the pieces. */
+int vtts_stabletts_synthesise_pieces_wav(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max,
+                                         const int64_t* pieces, const int64_t* piece_lengths, int64_t pieces_ld, const int32_t* bert_rows,
+                                         const float* pause, const int64_t* sid, int n_timesteps, float temperature, float length_scale,
+                                         float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out,
+                                         int64_t mel_ld, int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise, float* wav,
+                                         int64_t wav_ld, int64_t* wav_lengths);
+
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are
  * read with vtts_last_error(NULL) on the calling thread.

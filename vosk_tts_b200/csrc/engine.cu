@@ -467,7 +467,7 @@ struct vtts_engine {
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
     TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2, TAG_HIFIGAN = 0xD3,
-    TAG_BERT = 0xD4
+    TAG_BERT = 0xD4, TAG_ST_TEXT_PIECES = 0xD5
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -827,7 +827,12 @@ struct vtts_engine {
   PinnedBuf<char> h_pin_stt, h_pin_sttd;
   struct SttPin { int* ints; float *prm, *pause, *bert; };
   SttPin stt_layout();
-  void stt_enqueue(bool prior);
+  void stt_enqueue(bool prior, bool bert_on_device = false);
+  // vtts_stabletts_synthesise_pieces_wav: BERT of the staged sentences (bt_stage), then each token's row gathered into d_stbert.
+  // h_pin_stg stages the token rows' lengths and offsets and each one's source, BERT's packed row btp.off[b] + bert_rows[b][t].
+  Buf<int> d_stg;
+  PinnedBuf<char> h_pin_stg;
+  void stt_bert_enqueue();
 
   // ---- StableTTS vocoder (the HiFi-GAN Generator of matcha/hifigan/models.py; hifigan.cuh), bound into the decoder members
   // (dec.*) when the blob carries it.  In precision modes >= 1 the first voc_nt upsampling stages and their MRFs run on the
@@ -3529,7 +3534,7 @@ vtts_engine::SttPin vtts_engine::stt_layout() {
 // Text phase of vtts_stabletts_synthesise: uploads, the token rows x, dp_encoder and its proj, the durations and their scan;
 // with `prior` the mel encoder and its proj as well.  Leaves x, the durations, each token's first frame, the pauses and
 // mu_mel on the device for the mel phase, and copies [dur][first][frames of every utterance] to pinned memory.
-void vtts_engine::stt_enqueue(bool prior) {
+void vtts_engine::stt_enqueue(bool prior, bool bert_on_device) {
   const vtts_config& c = cfg;
   const int MC = c.st_cond, H = c.st_enc_hidden, F = c.st_enc_filter, NE = c.st_enc_layers, G = c.st_spk_dim, S = c.st_streams;
   const int dk = H / c.st_enc_heads, rd = dk / 2, DC = c.st_dur_channels, NC = c.st_noise;
@@ -3540,7 +3545,7 @@ void vtts_engine::stt_enqueue(bool prior) {
   float* bert = ensure(d_stbert, T * c.st_bert_dim);
   CK(cudaMemcpyAsync(di, pp.ints, ni * sizeof(int), cudaMemcpyHostToDevice, stream));
   CK(cudaMemcpyAsync(df, pp.prm, (16 + T) * sizeof(float), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(bert, pp.bert, T * c.st_bert_dim * sizeof(float), cudaMemcpyHostToDevice, stream));
+  if (!bert_on_device) CK(cudaMemcpyAsync(bert, pp.bert, T * c.st_bert_dim * sizeof(float), cudaMemcpyHostToDevice, stream));
   const int *lens = di, *offs = di + B, *sid = di + 2 * B, *ids = di + 3 * B;
   // the decoder's fixed launch shape, every token row sized at the bucket: durations do not depend on the batch
   const Rows r{lens, offs, B, maxTok, std::vector<int>(B, maxTok), h_tok_len, tune.fixed_ffma().fixed_attention()};
@@ -3578,6 +3583,23 @@ void vtts_engine::stt_enqueue(bool prior) {
   ++launches;
   int* back = reinterpret_cast<int*>(ensure(h_pin_sttd, (2 * T + B) * sizeof(int)));
   CK(cudaMemcpyAsync(back, dd, (2 * T + B) * sizeof(int), cudaMemcpyDeviceToHost, stream));
+}
+
+// BERT rows of the text phase from word pieces: BERT of the sentences bt_stage staged, into its packed rows d_btout, then
+// st_bert_gather_kernel copies each token's row into d_stbert, where stt_enqueue(prior, true) reads it.  h_pin_stg holds
+// [tok len B][tok off B][source row of every token row Ttok].
+void vtts_engine::stt_bert_enqueue() {
+  const vtts_config& c = cfg;
+  const size_t T = (size_t)Ttok, ni = 2 * (size_t)B + T;
+  float* feat = ensure(d_btout, (size_t)btp.tot * c.cv_hidden);
+  bt_enqueue(feat);
+  int* di = ensure(d_stg, ni);
+  float* bert = ensure(d_stbert, T * c.st_bert_dim);
+  CK(cudaMemcpyAsync(di, h_pin_stg.p, ni * sizeof(int), cudaMemcpyHostToDevice, stream));
+  klaunch(st_bert_gather_kernel, dim3(maxTok, B), dim3(128), (size_t)0, (const float*)feat, (const int*)(di + 2 * B), c.st_bert_dim, bert,
+          (const int*)di, (const int*)(di + B));
+  CK(cudaGetLastError());
+  ++launches;
 }
 
 // Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
@@ -4301,7 +4323,8 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
                                       const float* pause, const int64_t* sid, int n, float temperature, float length_scale, float s,
                                       const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out, int64_t mel_ld, int64_t* mel_lengths,
                                       int32_t* durations, float* prior_out, int denormalise, float* wav = nullptr, int64_t wav_ld = 0,
-                                      int64_t* wav_lengths = nullptr) {
+                                      int64_t* wav_lengths = nullptr, const int64_t* pieces = nullptr, const int64_t* piece_lengths = nullptr,
+                                      int64_t pieces_ld = 0, const int32_t* bert_rows = nullptr) {
   const vtts_config& c = h->cfg;
   REQUIRE(!wav || h->has_voc, VTTS_ERR_INVALID, "the weight blob has no vocoder (StableTTS(..., vocoder=...) / weights.pack_hifigan)");
   REQUIRE(h->st_text, VTTS_ERR_INVALID, "the weight blob holds the flow-matching decoder only (weights.pack_stabletts_cfm): text-to-mel needs the "
@@ -4324,7 +4347,18 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
         REQUIRE(v >= 0.f && v <= (float)VTTS_ST_MAX_TOKEN_FRAMES, VTTS_ERR_INVALID, "pause durations must be in [0, VTTS_ST_MAX_TOKEN_FRAMES]");
       }
   }
+  if (pieces) {
+    REQUIRE(h->has_bert, VTTS_ERR_INVALID, "the weight blob has no BERT (bt.*): build the engine with StableTTS(..., bert=...)");
+    REQUIRE(BD == c.cv_hidden, VTTS_ERR_INVALID, "bert_dim differs from BERT's hidden width");
+    REQUIRE(pieces_ld >= 1, VTTS_ERR_INVALID, "bad pieces_ld");
+    for (int b = 0; b < B; ++b)
+      for (int64_t i = 0; i < id_lengths[b]; ++i) {
+        const int32_t v = bert_rows[(size_t)b * t_max + i];
+        REQUIRE(v >= 0 && v < piece_lengths[b], VTTS_ERR_INVALID, "a BERT row is outside its sentence's word pieces [0, piece_lengths)");
+      }
+  }
   setup_lengths(h, id_lengths, B, (int)t_max);
+  if (pieces) h->bt_stage(pieces, piece_lengths, pieces_ld);
   const int Ttok = h->Ttok;
   {
     const vtts_engine::SttPin pp = h->stt_layout();
@@ -4339,11 +4373,24 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
       for (int q = 0; q < S; ++q)
         for (int i = 0; i < len; ++i) pp.ints[3 * B + (size_t)q * Ttok + o + i] = (int)ids[((size_t)b * S + q) * t_max + i];
       if (pause) memcpy(pp.pause + o, pause + (size_t)b * t_max, (size_t)len * sizeof(float));
-      memcpy(pp.bert + (size_t)o * BD, bert + (size_t)b * t_max * BD, (size_t)len * BD * sizeof(float));
+      if (bert) memcpy(pp.bert + (size_t)o * BD, bert + (size_t)b * t_max * BD, (size_t)len * BD * sizeof(float));
     }
   }
   const bool prior = prior_out != nullptr;
-  h->run_graphed({vtts_engine::TAG_ST_TEXT, B, h->maxTok, Ttok, prior ? 1 : 0}, [&] { h->stt_enqueue(prior); });
+  if (pieces) {
+    int* g = reinterpret_cast<int*>(h->ensure(h->h_pin_stg, (2 * (size_t)B + Ttok) * sizeof(int) + 64));
+    memcpy(g, h->h_tok_len.data(), B * sizeof(int));
+    memcpy(g + B, h->h_tok_off.data(), B * sizeof(int));
+    std::fill(g + 2 * B, g + 2 * B + Ttok, 0);
+    for (int b = 0; b < B; ++b)
+      for (int i = 0; i < h->h_tok_len[b]; ++i) g[2 * B + h->h_tok_off[b] + i] = h->btp.off[b] + bert_rows[(size_t)b * t_max + i];
+    h->run_graphed({vtts_engine::TAG_ST_TEXT_PIECES, B, h->maxTok, Ttok, prior ? 1 : 0, h->btp.maxL, h->btp.tot}, [&] {
+      h->stt_bert_enqueue();
+      h->stt_enqueue(prior, true);
+    });
+  } else {
+    h->run_graphed({vtts_engine::TAG_ST_TEXT, B, h->maxTok, Ttok, prior ? 1 : 0}, [&] { h->stt_enqueue(prior); });
+  }
   CK(cudaStreamSynchronize(h->stream));            // the one wait of the path: the frame counts size the mel phase
   const int* back = reinterpret_cast<const int*>(h->h_pin_sttd.p);
   std::vector<int> frames(B), extents(B);
@@ -5129,6 +5176,20 @@ int vtts_stabletts_synthesise_wav(vtts_handle h, const int64_t* ids, const int64
   return guarded(h, [&] { impl_stabletts_synthesise(h, ids, id_lengths, B, t_max, bert, pause, sid, n_timesteps, temperature, length_scale,
                                                     guidance_scale, noise, noise_ld, seed, mel_out, mel_ld, mel_lengths, durations, prior_out,
                                                     denormalise, wav, wav_ld, wav_lengths); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
+}
+
+int vtts_stabletts_synthesise_pieces_wav(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int B, int64_t t_max,
+                                         const int64_t* pieces, const int64_t* piece_lengths, int64_t pieces_ld, const int32_t* bert_rows,
+                                         const float* pause, const int64_t* sid, int n_timesteps, float temperature, float length_scale,
+                                         float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out,
+                                         int64_t mel_ld, int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise, float* wav,
+                                         int64_t wav_ld, int64_t* wav_lengths) {
+  if (!ids || !id_lengths || !pieces || !piece_lengths || !bert_rows || !sid || !mel_lengths || !wav || !wav_lengths || (prior_out && !mel_out))
+    return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_stabletts_synthesise(h, ids, id_lengths, B, t_max, nullptr, pause, sid, n_timesteps, temperature, length_scale,
+                                                    guidance_scale, noise, noise_ld, seed, mel_out, mel_ld, mel_lengths, durations, prior_out,
+                                                    denormalise, wav, wav_ld, wav_lengths, pieces, piece_lengths, pieces_ld, bert_rows); },
+                 G_ATOMIC, VTTS_FAMILY_STABLETTS);
 }
 
 int vtts_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* mel_lengths, int B, int64_t mel_ld, float* wav, int64_t wav_ld,

@@ -124,4 +124,10 @@ stt_pause_fill_kernel(float* __restrict__ mel, int NC, const float* __restrict__
   for (int c = threadIdx.x; c < NC; c += blockDim.x) mel[r * NC + c] = mel[r0 * NC + c];
 }
 
+// Each token's BERT row (vosk_tts/synth.py:25-44 and the word index of g2p_multistream*, :273-454): bert [token rows][BD] <-
+// feat [src[token row]][BD], BERT's packed rows of the utterance's own sentence.  grid (tokens, utterances).  Defined in
+// st_gather.cu, a translation unit of its own: see there.
+__global__ void st_bert_gather_kernel(const float* __restrict__ feat, const int* __restrict__ src, int BD, float* __restrict__ bert,
+                                      const int* __restrict__ lens, const int* __restrict__ offs);
+
 }  // namespace vtts

@@ -63,7 +63,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_debug_conv_log", "vtts_tc_split_plan", "vtts_align", "vtts_align_spec", "vtts_speaker_embedding",
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
-           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features",
+           "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
            "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
@@ -267,6 +267,9 @@ def load_library(build_if_missing=True):
     lib.vtts_hifigan_vocode.restype = i32
     lib.vtts_bert_features.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64]
     lib.vtts_bert_features.restype = i32
+    st = lib.vtts_stabletts_synthesise_wav.argtypes
+    lib.vtts_stabletts_synthesise_pieces_wav.argtypes = st[:5] + [vp, vp, C.c_int64, vp] + st[6:]
+    lib.vtts_stabletts_synthesise_pieces_wav.restype = i32
     _LIB = lib
     return lib
 
@@ -770,7 +773,7 @@ class Engine:
 
     def stabletts_synthesise(self, ids, bert, sid, lengths=None, pause=None, n_timesteps=10, temperature=1.0, length_scale=1.0,
                              guidance_scale=0.5, noise=None, seed=0, mel_frames=None, want_prior=False, denormalise=False,
-                             want_wav=False):
+                             want_wav=False, pieces=None, bert_rows=None, piece_lengths=None):
         """StableTTS text-to-mel (vtts_stabletts_synthesise).  ids int [B, n_streams, T] (or [n_streams, T]); bert float [B, T,
         bert_dim] token-major; lengths int [B] (None: T for all); pause float [B, T] or None; sid int [B] (or one for all);
         noise float [B, >= ceil4(frames), noise_channels] frame-major over the padded frame axis, or None for Philox(seed).
@@ -779,7 +782,11 @@ class Engine:
         noise_channels] frame-major (zeros past each utterance), mel_lengths int64 [B], durations int32 [B, T], and prior (the
         expanded mel encoder output) when want_prior, and with want_wav the vocoder's wav [B, hop * frames] (zeros past each
         utterance) and wav_lengths int64 [B] (vtts_stabletts_synthesise_wav: the vocoder reads the denormalised mel on the
-        device)."""
+        device).
+        pieces / bert_rows (with bert=None): each utterance's sentence of word pieces, a list of B sequences or int [B, L] with
+        piece_lengths int [B] (None: every row is a whole sentence of L pieces), and int [B, T] the row among its own pieces that
+        each token reads; BERT then runs on the device and its rows are gathered there (vtts_stabletts_synthesise_pieces_wav,
+        which always vocodes: want_wav is implied)."""
         ids = np.ascontiguousarray(ids, dtype=np.int64)
         if ids.ndim == 2:
             ids = ids[None]
@@ -787,11 +794,35 @@ class Engine:
         NC, BD = int(self.cfg["noise_channels"]), int(self.cfg.get("bert_dim", 0))
         if S != int(self.cfg.get("n_streams", S)):
             raise ValueError("ids must be [B, %d, T]" % int(self.cfg["n_streams"]))
-        bert = np.ascontiguousarray(bert, dtype=np.float32)
-        if bert.ndim == 2:
-            bert = bert[None]
-        if bert.shape != (B, T, BD):
-            raise ValueError("bert must be token-major [B, T, %d]" % BD)
+        if (bert is None) == (pieces is None) or (pieces is None) != (bert_rows is None):
+            raise ValueError("give either bert, or pieces with bert_rows")
+        if pieces is None:
+            bert = np.ascontiguousarray(bert, dtype=np.float32)
+            if bert.ndim == 2:
+                bert = bert[None]
+            if bert.shape != (B, T, BD):
+                raise ValueError("bert must be token-major [B, T, %d]" % BD)
+        else:
+            if not self.cfg.get("bert"):
+                raise ValueError("this engine has no BERT")
+            if isinstance(pieces, (list, tuple)):
+                seqs = [np.asarray(u, np.int64).reshape(-1) for u in pieces] or [np.zeros(0, np.int64)]
+                piece_len = np.array([u.size for u in seqs], np.int64)
+                pieces = np.zeros((len(seqs), max(1, int(piece_len.max()))), np.int64)
+                for b, u in enumerate(seqs):
+                    pieces[b, :u.size] = u
+            else:
+                pieces = np.ascontiguousarray(pieces, dtype=np.int64)
+                pieces = pieces[None] if pieces.ndim == 1 else pieces
+                piece_len = np.full(pieces.shape[0], pieces.shape[-1], np.int64) if piece_lengths is None else \
+                    np.ascontiguousarray(np.broadcast_to(np.asarray(piece_lengths, np.int64).reshape(-1), (pieces.shape[0],)))
+            bert_rows = np.ascontiguousarray(bert_rows, dtype=np.int32)
+            bert_rows = bert_rows[None] if bert_rows.ndim == 1 else bert_rows
+            if pieces.ndim != 2 or pieces.shape[0] != B or pieces.shape[1] < 1 or (piece_len < 1).any() or (piece_len > pieces.shape[1]).any():
+                raise ValueError("pieces must hold one sentence of at least one word piece per utterance")
+            if bert_rows.shape != (B, T):
+                raise ValueError("bert_rows must be [B, T]")
+            want_wav = True
         lengths = np.full(B, T, np.int64) if lengths is None else np.ascontiguousarray(np.broadcast_to(np.asarray(lengths, np.int64).reshape(-1), (B,)))
         sid = np.ascontiguousarray(np.broadcast_to(np.asarray(sid, np.int64).reshape(-1), (B,)))
         if pause is not None:
@@ -819,7 +850,11 @@ class Engine:
             hop = _config.hop_samples(self.cfg["vocoder"]) if self.cfg.get("vocoder") else 1
             wav = np.zeros((B, int(mel_frames) * hop), np.float32)
             wl = np.zeros(B, np.int64)
-            self._check(self.lib.vtts_stabletts_synthesise_wav(*args, _ptr(wav), wav.shape[1], _ptr(wl)))
+            if pieces is not None:
+                args = args[:5] + (_ptr(pieces), _ptr(piece_len), pieces.shape[1], _ptr(bert_rows)) + args[6:]
+                self._check(self.lib.vtts_stabletts_synthesise_pieces_wav(*args, _ptr(wav), wav.shape[1], _ptr(wl)))
+            else:
+                self._check(self.lib.vtts_stabletts_synthesise_wav(*args, _ptr(wav), wav.shape[1], _ptr(wl)))
         else:
             self._check(self.lib.vtts_stabletts_synthesise(*args))
         top = int(mel_len.max())

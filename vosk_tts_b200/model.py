@@ -6,6 +6,11 @@ training/vits2/onnx_export.py:55) and, optionally, the training json (`vits_conf
 `model` block.  A directory that holds only what vosk-tts ships (`model.onnx`, `config.json`, `dictionary`) works too: the
 weights AND the architecture are read from the graph's initializers (`onnx_weights.py`, no `onnx` package needed).
 Downloading models needs a network and is out of scope -- a missing model is an error, never a silent fallback.
+
+A multistream StableTTS voice (`model_type` multistream_v1 / v2 / v3) holds what the reference ships (`config.json`,
+`dictionary`, and `bert/vocab.txt` with BERT's `bert/model.onnx` for the models with a tokenizer) plus the checkpoints that
+matcha/onnx/export.py reads: the Matcha checkpoint (`model.ckpt`, else the newest `*.ckpt`) and the HiFi-GAN generator
+(`generator_v1`, `hifigan_T2_v1` or `hifigan_univ_v1`, config v1).  Its `.onnx` is a StableTTSSession.
 """
 import glob
 import json
@@ -16,7 +21,11 @@ from pathlib import Path
 
 from . import config as _config
 from . import weights as _weights
-from .session import VitsSession
+from .session import StableTTSSession, VitsSession
+from .wordpiece import BertWordPieceTokenizer
+
+MULTISTREAM_TYPES = ("multistream_v1", "multistream_v2", "multistream_v3")
+VOCODER_NAMES = ("generator_v1", "hifigan_T2_v1", "hifigan_univ_v1")      # matcha/cli.py's vocoders
 
 MODEL_DIRS = [os.getenv("VOSK_MODEL_PATH"), Path("/usr/share/vosk"), Path.home() / "AppData/Local/vosk",
               Path.home() / ".cache/vosk"]
@@ -55,9 +64,11 @@ def _reserve_from_env():
 
 
 class Model:
-    def __init__(self, model_path=None, model_name=None, lang=None, device=0, precision=1, session=None, voice_conversion=False):
+    def __init__(self, model_path=None, model_name=None, lang=None, device=0, precision=1, session=None, voice_conversion=False,
+                 n_timesteps=5):
         """voice_conversion: also load the posterior encoder (Synth.convert_audio); needs the training checkpoint (G_*.pth)
-        -- model.onnx is a trace of SynthesizerTrn.infer and holds no enc_q."""
+        -- model.onnx is a trace of SynthesizerTrn.infer and holds no enc_q.  n_timesteps: the flow-matching steps of a
+        multistream voice (export.py's default; a deployed graph bakes its own count, which a checkpoint does not record)."""
         if model_path is None:
             model_path = self.get_model_path(model_name, lang)
         model_path = Path(model_path)
@@ -65,7 +76,11 @@ class Model:
         self.config = json.load(open(model_path / "config.json"))
         self.dic = load_dictionary(model_path / "dictionary") if (model_path / "dictionary").exists() else {}
         self.tokenizer = None
-        if (model_path / "bert" / "vocab.txt").exists() or str(self.config.get("model_type", "")).startswith("multistream"):
+        model_type = str(self.config.get("model_type", ""))
+        if model_type in MULTISTREAM_TYPES:
+            self._load_multistream(model_path, device, precision, session, n_timesteps)
+            return
+        if (model_path / "bert" / "vocab.txt").exists() or model_type.startswith("multistream"):
             raise ValueError("bert-conditioned / multistream models are not VITS2 graphs: not supported by this engine")
         if session is not None:
             self.onnx = session
@@ -98,6 +113,37 @@ class Model:
         folded = _weights.load_checkpoint(cks[-1])
         self.onnx = VitsSession(state_dict=folded, cfg=cfg, device=device, precision=precision, reserve=_reserve_from_env(),
                                 voice_conversion=voice_conversion)
+
+    def _load_multistream(self, model_path, device, precision, session, n_timesteps):
+        has_bert = (model_path / "bert" / "vocab.txt").exists()
+        if has_bert:
+            self.tokenizer = BertWordPieceTokenizer(vocab=str(model_path / "bert" / "vocab.txt"), unk_token="[UNK]", lowercase=True)
+        if session is not None:
+            if not getattr(session, "multistream", False):
+                raise ValueError("a multistream model needs a multistream session (StableTTSSession), not %s" % type(session).__name__)
+            self.onnx = session
+            return
+        ckpt = model_path / "model.ckpt"
+        if not ckpt.exists():
+            cks = sorted(model_path.glob("*.ckpt"), key=lambda p: p.stat().st_mtime)
+            ckpt = cks[-1] if cks else None
+        voc = next((model_path / n for n in VOCODER_NAMES if (model_path / n).exists()), None)
+        if ckpt is None or voc is None:
+            if (model_path / "model.onnx").exists():
+                raise ValueError("%s holds the exported multistream graph model.onnx: reading StableTTS weights from the exported "
+                                 "graph is not built; put the Matcha checkpoint (*.ckpt) and the HiFi-GAN generator (%s) beside it"
+                                 % (model_path, " / ".join(VOCODER_NAMES)))
+            raise FileNotFoundError("no weights in %s: a multistream model needs the Matcha checkpoint (model.ckpt or *.ckpt) and "
+                                    "the HiFi-GAN generator (%s)" % (model_path, " / ".join(VOCODER_NAMES)))
+        from .stabletts import StableTTS
+        sd = _weights.load_lightning_state_dict(str(ckpt))
+        if "spk_emb.weight" not in sd:
+            raise ValueError("%s has no spk_emb: a single-speaker Matcha checkpoint (n_spks = 1) is not supported by this engine, "
+                             "whose StableTTS encoder and decoder are conditioned on a speaker embedding" % ckpt)
+        n_spks, spk_dim = (int(v) for v in sd["spk_emb.weight"].shape)
+        bert = _weights.load_bert(str(model_path / "bert")) if has_bert else None
+        tts = StableTTS({"n_spks": n_spks, "spk_emb_dim": spk_dim}, sd, device=device, precision=precision, vocoder=str(voc), bert=bert)
+        self.onnx = StableTTSSession(tts, n_timesteps=n_timesteps)
 
     def get_model_path(self, model_name, lang):
         for directory in MODEL_DIRS:

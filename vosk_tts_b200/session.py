@@ -145,3 +145,88 @@ class VitsSession:
 
     def close(self):
         self.engine.close()
+
+
+class StableTTSSession:
+    """`Model.onnx` of a multistream StableTTS voice: an onnxruntime-shaped facade over the graph matcha/onnx/export.py writes
+    (MatchaWithVocoder: text to waveform, n_timesteps baked in, guidance 0.5 as flow_matching.py:61 fixes it), plus the
+    word-piece call that Synth uses so that BERT's rows are computed and gathered on the GPU."""
+    multistream = True
+
+    def __init__(self, tts, n_timesteps=5, seed=0):
+        """tts: a stabletts.StableTTS with the text encoder and a vocoder (and BERT, for models with a tokenizer)."""
+        if not tts.has_text or tts.hop is None:
+            raise ValueError("a multistream session needs the StableTTS text encoder and a vocoder")
+        self.tts = tts
+        self.n_timesteps = int(n_timesteps)
+        self.cfg = {"sampling_rate": 22050, "hop_length": int(tts.hop)}
+        self._lock = threading.Lock()
+        self._seed = int(seed)
+        self._calls = 0
+        self.last_wav_lengths = None
+
+    def get_providers(self):
+        return ["B200VttsExecutionProvider"]
+
+    def _next_seed(self):
+        self._calls += 1
+        return (self._seed * 0x9E3779B97F4A7C15 + self._calls) & 0xFFFFFFFFFFFFFFFF
+
+    @staticmethod
+    def _feeds(feeds):
+        ids = np.asarray(feeds["input"], np.int64)
+        if ids.ndim != 3:
+            raise ValueError("input must be the multistream ids [B, n_streams, T]")
+        B = ids.shape[0]
+        lengths = np.asarray(feeds["input_lengths"], np.int64).reshape(-1)
+        if lengths.shape != (B,) or (lengths < 1).any() or (lengths > ids.shape[2]).any():
+            raise ValueError("input_lengths must hold one length in [1, T] per utterance")
+        sid = feeds.get("sid")
+        sid = np.zeros(B, np.int64) if sid is None else np.broadcast_to(np.asarray(sid, np.int64).reshape(-1), (B,))
+        extra = feeds.get("phone_duration_extra")
+        if extra is not None:
+            extra = np.broadcast_to(np.asarray(extra, np.float32).reshape(-1, ids.shape[2]), (B, ids.shape[2]))
+        scales = np.asarray(feeds["scales"], np.float32).reshape(3)
+        return ids, lengths, sid, extra, scales
+
+    def _synthesise(self, ids, lengths, sid, extra, scales, **kw):
+        xs = [ids[b, :, :lengths[b]] for b in range(ids.shape[0])]
+        pause = None if extra is None else [extra[b, :lengths[b]] for b in range(ids.shape[0])]
+        with self._lock:
+            r = self.tts.synthesise(xs, kw.pop("bert", None), list(sid), phone_duration_extra=pause, n_timesteps=self.n_timesteps, guidance_scale=0.5,
+                                    seed=self._next_seed(), return_wav=True, **kw, **self.tts.from_scales(scales))
+        wl = np.array(r["wav_lengths"], np.int64)
+        wav = np.zeros((len(xs), int(wl.max())), np.float32)
+        for b, w in enumerate(r["wav"]):
+            wav[b, :w.size] = w
+        self.last_wav_lengths = wl
+        return [wav, wl]
+
+    def run(self, output_names, feeds):
+        """feeds of export.py's graph: input int64 [B, n_streams, T], input_lengths [B], scales [temperature, length_scale,
+        dp_temperature], sid [B] or None, bert float [B, bert_dim, T], phone_duration_extra [B, T] or None.  Returns [wav float32
+        [B, max samples] (zeros after each utterance), wav_lengths int64 [B] = hop * mel_lengths]."""
+        ids, lengths, sid, extra, scales = self._feeds(feeds)
+        bert = np.asarray(feeds["bert"], np.float32)
+        if bert.ndim != 3 or bert.shape[0] != ids.shape[0] or bert.shape[2] != ids.shape[2]:
+            raise ValueError("bert must be [B, bert_dim, T]")
+        return self._synthesise(ids, lengths, sid, extra, scales, bert=[bert[b, :, :lengths[b]] for b in range(ids.shape[0])])
+
+    def run_pieces(self, feeds, pieces, bert_rows):
+        """run() with the `bert` feed replaced by each utterance's word pieces (a list of int sequences, [CLS] ... [SEP]) and
+        bert_rows int [B, T], the row among its own pieces that each token reads: BERT runs and its rows are gathered on the
+        GPU (vtts_stabletts_synthesise_pieces_wav)."""
+        ids, lengths, sid, extra, scales = self._feeds(feeds)
+        rows = np.asarray(bert_rows, np.int64)
+        if rows.ndim != 2 or rows.shape != (ids.shape[0], ids.shape[2]) or len(pieces) != ids.shape[0]:
+            raise ValueError("bert_rows must be [B, T] and pieces hold one sentence per utterance")
+        return self._synthesise(ids, lengths, sid, extra, scales, pieces=list(pieces),
+                                bert_rows=[rows[b, :lengths[b]] for b in range(ids.shape[0])])
+
+    def bert_features(self, ids):
+        """BERT's rows [L, hidden] of one sentence's word pieces, as the reference's bert/model.onnx returns them."""
+        with self._lock:
+            return self.tts.bert_features(np.asarray(ids, np.int64).reshape(-1))
+
+    def close(self):
+        self.tts.close()

@@ -3,7 +3,8 @@ matcha_tts.py:93-211: multistream ids, BERT features and pause durations in, dur
 conditional-flow-matching decoder alone (CFM.forward of components/flow_matching.py, called at matcha_tts.py:183), and, with a
 HiFi-GAN checkpoint (matcha/hifigan, as cli.py:65-71 loads it), the vocoder: mel to waveform, and text to waveform in one call.
 With a BERT checkpoint (the model vosk_tts/synth.py's get_word_bert runs) the engine also computes BERT's features of word-piece
-ids on the GPU (bert_features); synthesise still takes the features per token, as the exported graph's `bert` feed does."""
+ids on the GPU (bert_features), and synthesise takes either the features per token, as the exported graph's `bert` feed does,
+or each sentence's word pieces and the row each token reads, gathering BERT's rows on the device."""
 import numpy as np
 
 from . import config as _config
@@ -57,33 +58,51 @@ class StableTTS:
         return {"temperature": float(scales[0]), "length_scale": float(scales[1])}
 
     def synthesise(self, x, bert, sid, phone_duration_extra=None, n_timesteps=10, temperature=1.0, length_scale=1.0,
-                   guidance_scale=0.5, noise=None, seed=0, return_prior=False, return_wav=False):
+                   guidance_scale=0.5, noise=None, seed=0, return_prior=False, return_wav=False, pieces=None, bert_rows=None):
         """x: the ids [n_streams, T] of one utterance, or a list of them; bert [bert_dim, T] and phone_duration_extra [T] (or
         None) alike; sid: a speaker id for all, or one per utterance; noise: [noise_channels, >= ceil4(frames)] per utterance
         standing in for torch.randn over the padded frame axis, or None for the engine's Philox(seed).  Returns the
         reference's names: mel and decoder_outputs [noise_channels, frames] (denormalised and as the model produces them),
         mel_lengths, durations [T] (w_round), with return_prior encoder_outputs / mel_enc, and with return_wav the vocoder's
-        wav [hop * frames] (vocoder(mel).clamp(-1, 1), run on the device behind the mel) and wav_lengths; each a list for a list."""
+        wav [hop * frames] (vocoder(mel).clamp(-1, 1), run on the device behind the mel) and wav_lengths; each a list for a list.
+        pieces / bert_rows, with bert=None: the word pieces of each utterance's sentence ([CLS] ... [SEP]) and the row among them
+        that each token reads [T] (an engine with BERT and a vocoder; return_wav is implied)."""
         single = not isinstance(x, (list, tuple))
         xs = [np.asarray(u, np.int64) for u in ([x] if single else x)]
-        berts = [np.asarray(u, np.float32) for u in ([bert] if single else bert)]
         B, T = len(xs), max(u.shape[1] for u in xs)
         ids = np.zeros((B, xs[0].shape[0], T), np.int64)
-        feats = np.zeros((B, T, berts[0].shape[0]), np.float32)
+        feats = rows = None
+        if (bert is None) == (pieces is None) or (pieces is None) != (bert_rows is None):
+            raise ValueError("give either bert, or pieces with bert_rows")
+        if bert is not None:
+            berts = [np.asarray(u, np.float32) for u in ([bert] if single else bert)]
+            feats = np.zeros((B, T, berts[0].shape[0]), np.float32)
+        if bert_rows is not None:
+            rs = [np.asarray(u, np.int32).reshape(-1) for u in ([bert_rows] if single else bert_rows)]
+            if len(rs) != B or any(r.size != u.shape[1] for r, u in zip(rs, xs)):
+                raise ValueError("bert_rows must hold one row index per token")
+            rows = np.zeros((B, T), np.int32)
+            for b, r in enumerate(rs):
+                rows[b, :r.size] = r
+            pieces = [pieces] if single else pieces
         pause = None if phone_duration_extra is None else np.zeros((B, T), np.float32)
-        for b, (u, f) in enumerate(zip(xs, berts)):
-            if f.shape[1] != u.shape[1]:
-                raise ValueError("bert must have one column per token")
+        for b, u in enumerate(xs):
             ids[b, :, :u.shape[1]] = u
-            feats[b, :u.shape[1]] = f.T
+            if feats is not None:
+                if berts[b].shape[1] != u.shape[1]:
+                    raise ValueError("bert must have one column per token")
+                feats[b, :u.shape[1]] = berts[b].T
             if pause is not None:
                 pause[b, :u.shape[1]] = np.asarray(phone_duration_extra if single else phone_duration_extra[b], np.float32).reshape(-1)
         nz = None
         if noise is not None:
             nz = [np.ascontiguousarray(np.asarray(n, np.float32).T) for n in ([noise] if single else list(noise))]
+        return_wav = return_wav or rows is not None
         r = self.engine.stabletts_synthesise(ids, feats, sid, lengths=[u.shape[1] for u in xs], pause=pause, n_timesteps=n_timesteps,
                                              temperature=temperature, length_scale=length_scale, guidance_scale=guidance_scale,
-                                             noise=nz, seed=seed, want_prior=return_prior, want_wav=return_wav)
+                                             noise=nz, seed=seed, want_prior=return_prior, want_wav=return_wav,
+                                             pieces=None if rows is None else [np.asarray(p, np.int64).reshape(-1) for p in pieces],
+                                             bert_rows=rows)
         den = lambda a: a * self.mel_std + self.mel_mean          # denormalize (matcha/utils/model.py), fp32 like the reference
         cut = lambda a: [np.ascontiguousarray(a[b, :int(r["mel_lengths"][b])].T) for b in range(B)]
         out = {"decoder_outputs": cut(r["mel"]), "mel_lengths": [int(v) for v in r["mel_lengths"]],

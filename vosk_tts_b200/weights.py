@@ -729,6 +729,75 @@ def _pack_stabletts_decoder(P, sd, cfg):
         P.conv("st.lsc%d" % j, want(e + "lsc_layers.%d.weight" % j, (H, 2 * H, k)), g(e + "lsc_layers.%d.bias" % j))
 
 
+class _Inert:
+    """What a global outside _STATE_DICT_GLOBALS unpickles to: it accepts any arguments and state and does nothing, so a
+    checkpoint's hyper-parameters (Hydra configs, functools.partial of an optimizer) load as placeholders and nothing named
+    in the file is imported or called."""
+
+    def __init__(self, *args, **kwargs):
+        pass
+
+    def __call__(self, *args, **kwargs):
+        return _Inert()
+
+    def __setstate__(self, state):
+        pass
+
+    def __setitem__(self, key, value):
+        pass
+
+    def append(self, value):
+        pass
+
+    def extend(self, values):
+        pass
+
+
+# the globals a state dict of tensors needs; storages are resolved by torch.load itself
+_STATE_DICT_GLOBALS = {
+    ("collections", "OrderedDict"): "collections.OrderedDict",
+    ("torch", "Size"): "torch.Size",
+    ("torch._utils", "_rebuild_tensor"): "torch._utils._rebuild_tensor",
+    ("torch._utils", "_rebuild_tensor_v2"): "torch._utils._rebuild_tensor_v2",
+    ("torch._utils", "_rebuild_parameter"): "torch._utils._rebuild_parameter",
+    ("torch._utils", "_rebuild_parameter_with_state"): "torch._utils._rebuild_parameter_with_state",
+    ("torch._tensor", "_rebuild_from_type_v2"): "torch._tensor._rebuild_from_type_v2",
+    ("torch._tensor", "Tensor"): "torch.Tensor",
+    ("torch.nn.parameter", "Parameter"): "torch.nn.Parameter",
+}
+
+
+def _state_dict_pickle_module():
+    import importlib
+    import pickle
+    import types
+
+    class Unpickler(pickle.Unpickler):
+        def find_class(self, module, name):
+            if (module, name) not in _STATE_DICT_GLOBALS:
+                return _Inert
+            mod, _, attr = _STATE_DICT_GLOBALS[(module, name)].rpartition(".")
+            return getattr(importlib.import_module(mod), attr)
+
+    m = types.ModuleType("vtts_state_dict_pickle")
+    m.Unpickler, m.load = Unpickler, pickle.load
+    m.__dict__.update({k: getattr(pickle, k) for k in ("UnpicklingError", "HIGHEST_PROTOCOL")})
+    return m
+
+
+def load_lightning_state_dict(path):
+    """The state dict of a PyTorch Lightning checkpoint (`{"state_dict": ..., "hyper_parameters": ..., ...}`, as the
+    reference's training/stabletts writes `*.ckpt`), or of a file holding the state dict alone, with the weight norm folded.
+    torch.load(weights_only=True) refuses such a checkpoint: its hyper_parameters hold Hydra configs and a functools.partial of
+    the optimizer.  The file is read with an unpickler that resolves only the globals a state dict of tensors needs and turns
+    every other one into an inert placeholder, so loading imports and runs nothing the file names."""
+    ck = torch.load(path, map_location="cpu", weights_only=False, pickle_module=_state_dict_pickle_module())
+    sd = ck["state_dict"] if isinstance(ck, dict) and "state_dict" in ck else ck
+    if not isinstance(sd, dict) or not all(isinstance(v, torch.Tensor) for v in sd.values()):
+        raise ValueError("%s holds no state dict of tensors" % path)
+    return fold_weight_norm(sd)
+
+
 def load_hifigan(path):
     """A HiFi-GAN checkpoint of StableTTS's vocoder (cli.py:65-71: `{"generator": state_dict}`, generator_v1 / hifigan_T2_v1)
     -> its state dict with the weight norm folded, as remove_weight_norm leaves it.  Read with weights_only=True."""
