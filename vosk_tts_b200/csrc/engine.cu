@@ -819,7 +819,7 @@ struct vtts_engine {
 
   // ---- StableTTS text encoder and durations (TextEncoder.forward, MatchaTTS.synthesise; stabletts.cuh): blobs of
   // weights.pack_stabletts.  Stack 0 is the mel encoder (conditioned on spk_emb), stack 1 dp_encoder (on dur_spk_emb).
-  bool st_text = false;
+  bool st_text = false, st_prior = false;
   struct StEncW { std::vector<EncLayerW> blk; ConvW proj; const float *aw1, *ab1, *aw2, *ab2, *spk; } st_enc[2];
   const float *st_tok_emb = nullptr, *st_punc_emb = nullptr, *st_bert_w = nullptr, *st_bert_b = nullptr;
   Buf<int> d_stti, d_sttd;                         // [tok len B][tok off B][sid B][ids streams x Ttok]; [dur Ttok][first Ttok][frames B]
@@ -3331,7 +3331,10 @@ void vtts_engine::bind_stabletts() {
   st_punc_emb = vec("st.enc.punc", (size_t)c.st_n_vocab * c.st_punc_dim);
   st_bert_w = vec("st.enc.bert.w", (size_t)c.st_bert_proj * c.st_bert_dim);
   st_bert_b = vec("st.enc.bert.b", c.st_bert_proj);
-  for (int e = 0; e < 2; ++e) {
+  // the mel encoder feeds only the prior (encoder_outputs); an exported graph (matcha/onnx/export.py) does not output it and
+  // so does not carry its weights
+  st_prior = tensors.count("st.enc.mel.proj.w") > 0;
+  for (int e = st_prior ? 0 : 1; e < 2; ++e) {
     const std::string p = e == 0 ? "st.enc.mel" : "st.enc.dp";
     StEncW& W = st_enc[e];
     W.blk.clear();
@@ -4329,6 +4332,8 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
   REQUIRE(!wav || h->has_voc, VTTS_ERR_INVALID, "the weight blob has no vocoder (StableTTS(..., vocoder=...) / weights.pack_hifigan)");
   REQUIRE(h->st_text, VTTS_ERR_INVALID, "the weight blob holds the flow-matching decoder only (weights.pack_stabletts_cfm): text-to-mel needs the "
                                          "text encoder of weights.pack_stabletts");
+  REQUIRE(!prior_out || h->st_prior, VTTS_ERR_INVALID, "the weight blob has no mel encoder (encoder.encoder.*, which an exported graph "
+                                                          "drops): the prior (encoder_outputs) cannot be computed");
   REQUIRE(B >= 1 && B <= 8192 && t_max >= 1 && t_max <= VTTS_ST_MAX_TOKENS, VTTS_ERR_INVALID, "bad batch size / t_max");
   st_check_sampling(n, temperature, s);
   REQUIRE(std::isfinite(length_scale) && length_scale > 0.f && length_scale <= 100.f, VTTS_ERR_INVALID, "length_scale must be in (0, 100]");

@@ -10,7 +10,9 @@ Downloading models needs a network and is out of scope -- a missing model is an 
 A multistream StableTTS voice (`model_type` multistream_v1 / v2 / v3) holds what the reference ships (`config.json`,
 `dictionary`, and `bert/vocab.txt` with BERT's `bert/model.onnx` for the models with a tokenizer) plus the checkpoints that
 matcha/onnx/export.py reads: the Matcha checkpoint (`model.ckpt`, else the newest `*.ckpt`) and the HiFi-GAN generator
-(`generator_v1`, `hifigan_T2_v1` or `hifigan_univ_v1`, config v1).  Its `.onnx` is a StableTTSSession.
+(`generator_v1`, `hifigan_T2_v1` or `hifigan_univ_v1`, config v1).  Without those, the exported `model.onnx` the reference
+loads (matcha/onnx/export.py's graph, vocoder included) is read instead (onnx_weights.stabletts_from_onnx).  Its `.onnx` is a
+StableTTSSession.
 """
 import glob
 import json
@@ -65,10 +67,11 @@ def _reserve_from_env():
 
 class Model:
     def __init__(self, model_path=None, model_name=None, lang=None, device=0, precision=1, session=None, voice_conversion=False,
-                 n_timesteps=5):
+                 n_timesteps=None):
         """voice_conversion: also load the posterior encoder (Synth.convert_audio); needs the training checkpoint (G_*.pth)
         -- model.onnx is a trace of SynthesizerTrn.infer and holds no enc_q.  n_timesteps: the flow-matching steps of a
-        multistream voice (export.py's default; a deployed graph bakes its own count, which a checkpoint does not record)."""
+        multistream voice.  A checkpoint does not record them: None means export.py's default, 5.  An exported model.onnx
+        unrolls its own count: None means that count, and any other is refused."""
         if model_path is None:
             model_path = self.get_model_path(model_name, lang)
         model_path = Path(model_path)
@@ -128,14 +131,20 @@ class Model:
             cks = sorted(model_path.glob("*.ckpt"), key=lambda p: p.stat().st_mtime)
             ckpt = cks[-1] if cks else None
         voc = next((model_path / n for n in VOCODER_NAMES if (model_path / n).exists()), None)
+        from .stabletts import StableTTS
         if ckpt is None or voc is None:
             if (model_path / "model.onnx").exists():
-                raise ValueError("%s holds the exported multistream graph model.onnx: reading StableTTS weights from the exported "
-                                 "graph is not built; put the Matcha checkpoint (*.ckpt) and the HiFi-GAN generator (%s) beside it"
-                                 % (model_path, " / ".join(VOCODER_NAMES)))
+                # the deployed layout (vosk_tts/model.py:46): weights, shapes and the step count come out of the graph
+                tts = StableTTS.from_onnx(str(model_path / "model.onnx"), device=device, precision=precision,
+                                          bert=str(model_path / "bert") if has_bert else None)
+                if n_timesteps is not None and int(n_timesteps) != tts.n_timesteps:
+                    tts.close()
+                    raise ValueError("%s unrolls %d flow-matching steps; n_timesteps=%d would not compute what the graph computes"
+                                     % (model_path / "model.onnx", tts.n_timesteps, int(n_timesteps)))
+                self.onnx = StableTTSSession(tts, n_timesteps=tts.n_timesteps)
+                return
             raise FileNotFoundError("no weights in %s: a multistream model needs the Matcha checkpoint (model.ckpt or *.ckpt) and "
                                     "the HiFi-GAN generator (%s)" % (model_path, " / ".join(VOCODER_NAMES)))
-        from .stabletts import StableTTS
         sd = _weights.load_lightning_state_dict(str(ckpt))
         if "spk_emb.weight" not in sd:
             raise ValueError("%s has no spk_emb: a single-speaker Matcha checkpoint (n_spks = 1) is not supported by this engine, "
@@ -143,7 +152,7 @@ class Model:
         n_spks, spk_dim = (int(v) for v in sd["spk_emb.weight"].shape)
         bert = _weights.load_bert(str(model_path / "bert")) if has_bert else None
         tts = StableTTS({"n_spks": n_spks, "spk_emb_dim": spk_dim}, sd, device=device, precision=precision, vocoder=str(voc), bert=bert)
-        self.onnx = StableTTSSession(tts, n_timesteps=n_timesteps)
+        self.onnx = StableTTSSession(tts, n_timesteps=5 if n_timesteps is None else n_timesteps)
 
     def get_model_path(self, model_name, lang):
         for directory in MODEL_DIRS:

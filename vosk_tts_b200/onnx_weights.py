@@ -10,8 +10,12 @@ Add that consumes ``<module>.bias``.
 The ``onnx`` package is not a dependency: ModelProto / GraphProto / TensorProto are read with the ~60-line protobuf
 wire-format reader below (only the fields needed: graph=7; node=1, initializer=5; TensorProto dims=1, data_type=2,
 float_data=4, int64_data=7, name=8, raw_data=9; NodeProto input=1, output=2, op_type=4, attribute=5 with
-AttributeProto name=1, i=3, ints=8).
+AttributeProto name=1, i=3, t=5, ints=8).
+
+``stabletts_from_onnx`` reads a multistream (StableTTS) voice's model.onnx, the MatchaWithVocoder graph of
+matcha/onnx/export.py, the same way (DESIGN.md section 4.q).
 """
+import re
 import struct
 
 import numpy as np
@@ -22,6 +26,8 @@ _DTYPES = {1: np.float32, 6: np.int32, 7: np.int64, 10: np.float16, 11: np.float
 def _varint(buf, pos):
     out, shift = 0, 0
     while True:
+        if pos >= len(buf):
+            raise ValueError("truncated protobuf varint")
         b = buf[pos]
         pos += 1
         out |= (b & 0x7F) << shift
@@ -47,6 +53,8 @@ def _fields(buf):
             v = bytes(buf[pos:pos + 4]); pos += 4
         else:
             raise ValueError("unsupported protobuf wire type %d" % wt)
+        if pos > n:
+            raise ValueError("truncated protobuf message")
         yield fno, wt, v
 
 
@@ -90,8 +98,9 @@ def _tensor(buf):
 
 
 def _attributes(buf):
-    """{name: int or [ints]} of one NodeProto.attribute entry (only integer attributes are needed: strides, dilations)."""
-    name, ints, i = "", [], None
+    """(name, int or [ints] or ndarray) of one NodeProto.attribute entry: the integer attributes (strides, dilations) and the
+    tensor-valued ones (a Constant node's value)."""
+    name, ints, i, t = "", [], None, None
     for fno, wt, v in _fields(buf):
         if fno == 1:
             name = bytes(v).decode()
@@ -99,7 +108,9 @@ def _attributes(buf):
             ints += _packed_varints(v) if wt == 2 else [v]
         elif fno == 3 and wt == 0:
             i = v
-    return name, (ints if ints else i)
+        elif fno == 5 and wt == 2:
+            t = _tensor(v)[1]
+    return name, (t if t is not None else ints if ints else i)
 
 
 def read_graph(path, with_attributes=False):
@@ -166,9 +177,28 @@ def state_dict_from_onnx(path):
 
 
 def _count(sd, pattern):
-    import re
     rx = re.compile(pattern)
     return len({m.group(1) for k in sd for m in [rx.match(k)] if m})
+
+
+def _hifigan_shape(sd, attr_of, p):
+    """The HiFi-GAN Generator's shape (config keys upsample_* and resblock*) of the weights under prefix p: widths and kernels
+    from the tensors, upsampling rates and dilations from the strides / dilations of the (Conv)Transpose nodes."""
+    q = re.escape(p)
+    n_ups = _count(sd, q + r"ups\.(\d+)\.weight")
+    one = p + "resblocks.0.convs1.0.weight" in sd
+    stem = "convs1" if one else "convs"
+    nk = _count(sd, q + r"resblocks\.(\d+)\.convs1?\.0\.weight") // max(n_ups, 1)
+    dil = []
+    for j in range(nk):
+        n_conv = _count(sd, q + r"resblocks\.%d\.%s\.(\d+)\.weight" % (j, stem))
+        dil.append([int((attr_of[p + "resblocks.%d.%s.%d.weight" % (j, stem, m)][1].get("dilations") or [1])[0]) for m in range(n_conv)])
+    return {"upsample_initial_channel": int(sd[p + "conv_pre.weight"].shape[0]),
+            "upsample_kernel_sizes": [int(sd[p + "ups.%d.weight" % i].shape[2]) for i in range(n_ups)],
+            "upsample_rates": [int(attr_of[p + "ups.%d.weight" % i][1]["strides"][0]) for i in range(n_ups)],
+            "resblock": "1" if one else "2",
+            "resblock_kernel_sizes": [int(sd[p + "resblocks.%d.%s.0.weight" % (j, stem)].shape[2]) for j in range(nk)],
+            "resblock_dilation_sizes": dil}
 
 
 def config_from_onnx(path, sampling_rate=22050):
@@ -227,21 +257,7 @@ def config_from_onnx(path, sampling_rate=22050):
         cfg["decoder"] = "istft"
     else:
         cfg["decoder"] = "hifigan"
-    cfg["upsample_initial_channel"] = int(sd["dec.conv_pre.weight"].shape[0])
-    n_ups = _count(sd, r"dec\.ups\.(\d+)\.weight")
-    cfg["upsample_kernel_sizes"] = [int(sd["dec.ups.%d.weight" % i].shape[2]) for i in range(n_ups)]
-    cfg["upsample_rates"] = [int(attr_of["dec.ups.%d.weight" % i][1]["strides"][0]) for i in range(n_ups)]
-    n_rb = _count(sd, r"dec\.resblocks\.(\d+)\.convs1?\.0\.weight")
-    nk = n_rb // max(n_ups, 1)
-    one = "dec.resblocks.0.convs1.0.weight" in sd
-    cfg["resblock"] = "1" if one else "2"
-    stem = "convs1" if one else "convs"
-    cfg["resblock_kernel_sizes"] = [int(sd["dec.resblocks.%d.%s.0.weight" % (j, stem)].shape[2]) for j in range(nk)]
-    dil = []
-    for j in range(nk):
-        n_conv = _count(sd, r"dec\.resblocks\.%d\.%s\.(\d+)\.weight" % (j, stem))
-        dil.append([int((attr_of["dec.resblocks.%d.%s.%d.weight" % (j, stem, m)][1].get("dilations") or [1])[0]) for m in range(n_conv)])
-    cfg["resblock_dilation_sizes"] = dil
+    cfg.update(_hifigan_shape(sd, attr_of, "dec."))
     if cfg["decoder"] != "hifigan":
         if len(basis) != 1:
             raise ValueError("cannot locate the inverse-STFT basis of the decoder in the graph")
@@ -253,3 +269,104 @@ def config_from_onnx(path, sampling_rate=22050):
     if not cfg["use_transformer_flows"]:
         raise ValueError("plain coupling flows are unreachable through the reference exporter; unexpected graph")
     return cfg
+
+
+NOT_EXPORT = "the exported graph is not built as matcha/onnx/export.py builds it"
+
+
+def stabletts_from_onnx(path):
+    """A multistream voice's model.onnx -- matcha/onnx/export.py's MatchaWithVocoder: MatchaTTS.synthesise with n_timesteps
+    unrolled, then the HiFi-GAN -- read back into what StableTTS takes.  Returns a dict:
+      state_dict     MatchaTTS's tensors in the checkpoint's names (the "matcha." prefix dropped), weight_norm-free;
+      vocoder        the Generator's tensors (the "vocoder." prefix dropped), as remove_weight_norm left them;
+      config         config.stabletts_config of the graph's shapes (widths, layer and head counts, streams, speakers);
+      vocoder_config config.hifigan_config of the Generator's shapes and its (Conv)Transpose nodes' strides and dilations;
+      n_timesteps    the Euler steps the graph unrolls.
+    The exporter keeps every parameter under its module name, and that includes the time conditioning (time_mlp, each
+    block's film), fake_speaker and fake_content: it folds nothing that needs them.  nn.Linear layers on 3-D input
+    (encoder.bert_proj.1) become a MatMul with the transposed weight as an anonymous initializer, recovered through the Add
+    of its bias.  mel_mean and mel_std become anonymous scalars: the Mul and Add that denormalise the mel the vocoder reads.
+    The graph has no mel encoder (encoder.encoder.*): it feeds only encoder_outputs, which the graph does not return.
+    Anything else is refused with a ValueError that names the reason."""
+    def refuse(reason):
+        raise ValueError("%s: %s: %s" % (path, NOT_EXPORT, reason))
+    try:
+        inits, nodes = read_graph(path, with_attributes=True)
+    except (ValueError, UnicodeDecodeError, struct.error) as e:
+        refuse("not a readable self-contained ONNX model (%s)" % e)
+    sd = state_dict_from_onnx((inits, nodes))
+    if any(k.startswith(("enc_p.", "dec.")) for k in sd):
+        refuse("it holds a VITS model (enc_p.*, dec.*), not MatchaWithVocoder")
+    if "encoder.emb.weight" in sd:
+        refuse("it is a mel-only export without the vocoder (MatchaTTS at the top level); the engine needs the graph with the "
+               "HiFi-GAN embedded")
+    mt = {k[len("matcha."):]: v for k, v in sd.items() if k.startswith("matcha.")}
+    voc = {k[len("vocoder."):]: v for k, v in sd.items() if k.startswith("vocoder.")}
+    if "encoder.emb.weight" not in mt or "conv_pre.weight" not in voc:
+        refuse("it has no matcha.encoder.emb.weight or no vocoder.conv_pre.weight")
+    if "spk_emb.weight" not in mt:
+        refuse("a single-speaker model (no spk_emb): the engine's StableTTS is conditioned on a speaker embedding")
+    e = "decoder.estimator."
+    for k in (e + "time_mlp.layer.0.weight", e + "blocks.0.time_fusion.film.weight", "fake_speaker", "fake_content",
+              "encoder.bert_proj.1.weight", "encoder.dp_encoder.proj.weight"):
+        if k not in mt:
+            refuse("matcha.%s is missing (folded into constants or not exported)" % k)
+    producer, consumers, const = {}, {}, {}
+    for i, (op, ins, outs, attrs) in enumerate(nodes):
+        for o in outs:
+            producer[o] = i
+        for x in ins:
+            consumers.setdefault(x, []).append(i)
+        if op == "Constant" and isinstance(attrs.get("value"), np.ndarray):
+            const[outs[0]] = attrs["value"]
+    const.update(inits)
+    attr_of = {ins[1]: (op, attrs) for op, ins, outs, attrs in nodes if op in ("Conv", "ConvTranspose") and len(ins) >= 2}
+
+    def uses(name, op):
+        return [i for i in consumers.get(name, []) if nodes[i][0] == op]
+
+    def heads(w_name, width):
+        # MultiHeadAttention views conv_q's output as [b, n_heads, k_channels, t]: a Reshape whose shape is a Concat of
+        # the dynamic b, the constants n_heads and k_channels, and the dynamic t
+        convs = uses(w_name, "Conv")
+        for r in (uses(nodes[convs[0]][2][0], "Reshape") if convs else []):
+            cat = nodes[producer[nodes[r][1][1]]] if nodes[r][1][1] in producer else None
+            if cat and cat[0] == "Concat" and len(cat[1]) == 4 and all(x in const for x in cat[1][1:3]):
+                h, dk = (int(np.asarray(const[x]).reshape(-1)[0]) for x in cat[1][1:3])
+                if h * dk == width:
+                    return h
+        refuse("cannot read the head count of %s from its Reshape" % w_name)
+
+    # mel = decoder_outputs * mel_std + mel_mean (matcha/utils/model.py denormalize) is what the vocoder's conv_pre reads
+    add = nodes[producer.get(nodes[uses("vocoder.conv_pre.weight", "Conv")[0]][1][0], 0)]
+    scal = lambda x: x in inits and inits[x].size == 1 and inits[x].dtype == np.float32
+    mul = nodes[producer[add[1][0]]] if add[0] == "Add" and add[1][0] in producer else None
+    if not (mul and mul[0] == "Mul" and scal(add[1][1]) and scal(mul[1][1])):
+        refuse("the vocoder's input is not the denormalised mel (x * mel_std + mel_mean)")
+    mt["mel_std"], mt["mel_mean"] = inits[mul[1][1]].reshape(()), inits[add[1][1]].reshape(())
+    # the estimator runs twice per Euler step (the conditional and the guidance branch, flow_matching.py:179-194)
+    passes = len(uses("matcha." + e + "in_proj.weight", "Conv"))
+    if passes < 2 or passes % 2:
+        refuse("%d estimator passes, not two per Euler step" % passes)
+    dp, f1 = "encoder.dp_encoder.encoder.", mt[e + "blocks.0.block.mlp.conv_1.weight"]
+    ef1 = mt[dp + "0.mlp.conv_1.weight"]
+    n_blocks = _count(mt, re.escape(e) + r"blocks\.(\d+)\.block\.attn\.conv_q\.weight")
+    n_enc = _count(mt, re.escape(dp) + r"(\d+)\.attn\.conv_q\.weight")
+    cfg = {"noise_channels": int(mt[e + "final_proj.weight"].shape[0]), "cond_channels": int(mt[e + "cond_proj.0.weight"].shape[1]),
+           "hidden_channels": int(mt[e + "in_proj.weight"].shape[0]), "filter_channels": int(f1.shape[0]),
+           "kernel_size": int(f1.shape[2]), "n_layers": n_blocks,
+           "n_heads": heads("matcha." + e + "blocks.0.block.attn.conv_q.weight", int(mt[e + "in_proj.weight"].shape[0])),
+           "n_spks": int(mt["spk_emb.weight"].shape[0]), "spk_emb_dim": int(mt["spk_emb.weight"].shape[1]),
+           "n_vocab": int(mt["encoder.emb.weight"].shape[0]), "emb_dim": int(mt["encoder.emb.weight"].shape[1]),
+           "punc_dim": int(mt["encoder.punc_emb.weight"].shape[1]),
+           "n_streams": 1 + len(uses("matcha.encoder.punc_emb.weight", "Gather")),
+           "bert_dim": int(mt["encoder.bert_proj.1.weight"].shape[1]), "bert_proj_dim": int(mt["encoder.bert_proj.1.weight"].shape[0]),
+           "enc_hidden_channels": int(mt[dp + "0.attn.conv_q.weight"].shape[0]), "enc_filter_channels": int(ef1.shape[0]),
+           "enc_kernel_size": int(ef1.shape[2]), "enc_n_layers": n_enc,
+           "enc_n_heads": heads("matcha." + dp + "0.attn.conv_q.weight", int(mt[dp + "0.attn.conv_q.weight"].shape[0])),
+           "dur_channels": int(mt["encoder.dp_encoder.proj.weight"].shape[0])}
+    h = _hifigan_shape({"vocoder." + k: v for k, v in voc.items()}, attr_of, "vocoder.")
+    h["num_mels"] = int(voc["conv_pre.weight"].shape[1])
+    from . import config as _config
+    return {"state_dict": mt, "vocoder": voc, "config": _config.stabletts_config(cfg), "vocoder_config": _config.hifigan_config(h),
+            "n_timesteps": passes // 2}

@@ -50,6 +50,18 @@ class StableTTS:
         self.mel_mean, self.mel_std = np.float32(sd["mel_mean"]), np.float32(sd["mel_std"])
         self.engine = Engine(self.cfg, blob, man, device=device, precision=precision)
 
+    @classmethod
+    def from_onnx(cls, path, device=0, precision=1, bert=None):
+        """A multistream voice's model.onnx (matcha/onnx/export.py's graph, read by onnx_weights.stabletts_from_onnx) on one GPU,
+        with its vocoder; bert as in __init__.  n_timesteps: the Euler steps the graph unrolls, which StableTTSSession runs.
+        The graph carries no mel encoder, so synthesise(..., return_prior=True) is refused."""
+        from . import onnx_weights
+        g = onnx_weights.stabletts_from_onnx(path)
+        tts = cls(g["config"], g["state_dict"], device=device, precision=precision, vocoder=g["vocoder"],
+                  vocoder_config=g["vocoder_config"], bert=bert)
+        tts.n_timesteps = g["n_timesteps"]
+        return tts
+
     @staticmethod
     def from_scales(scales):
         """The exported graph's `scales` feed in the order its forward reads it (matcha/onnx/export.py:47-49): [temperature,

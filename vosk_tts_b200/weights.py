@@ -960,7 +960,8 @@ def pack_stabletts(sd, cfg, vocoder=None, bert=None):
     """A MatchaTTS (StableTTS) state dict without its vocoder -> (blob, manifest) of an engine that serves text-to-mel
     (vtts_stabletts_synthesise) and the decoder alone: the decoder part of pack_stabletts_cfm, then the text encoder
     (encoder.emb, encoder.punc_emb, encoder.bert_proj.1, both stacks encoder.encoder / encoder.dp_encoder with their proj) and
-    dur_spk_emb.  cfg: config.stabletts_config; vocoder as in pack_stabletts_cfm; bert: (BertModel state dict, config.bert_config,
+    dur_spk_emb.  Without encoder.encoder.* (a state dict read from an exported graph, onnx_weights.stabletts_from_onnx) the
+    engine serves everything but the prior.  cfg: config.stabletts_config; vocoder as in pack_stabletts_cfm; bert: (BertModel state dict, config.bert_config,
     tc) appended as pack_bert lays it out, or None."""
     if "enc_n_layers" not in cfg:
         raise ValueError("pack_stabletts needs config.stabletts_config (the text encoder's constants), not stabletts_cfm_config")
@@ -977,6 +978,8 @@ def pack_stabletts(sd, cfg, vocoder=None, bert=None):
     P.add("st.enc.bert.b", want("encoder.bert_proj.1.bias", (R,)))
     P.add("st.dur_spk_emb", want("dur_spk_emb.weight", (int(cfg["n_spks"]), G)))
     for dst, src, co in (("st.enc.mel", "encoder.encoder.", int(cfg["noise_channels"])), ("st.enc.dp", "encoder.dp_encoder.", DC)):
+        if dst == "st.enc.mel" and src + "proj.weight" not in sd:
+            continue            # the mel encoder feeds only the prior; an exported graph does not carry it
         b = src + "encoder.%d."
         for l in range(NE):
             _pack_dit_block(P, g, want, "%s.l%d" % (dst, l), b % l, H, F, k)
