@@ -61,7 +61,10 @@ typedef struct vtts_config {
   int32_t upsample_initial_channel;
   int32_t subbands, istft_n_fft, istft_hop;
   int32_t precision;               /* 0 = fp32 FFMA everywhere; 1 = split-bf16 wgmma for the flow + decoder (dense convs and
-                                      attention); 2 = text encoder on wgmma as well */
+                                      attention); 2 = text encoder on wgmma as well.  StableTTS: 1 = vocoder and BERT on
+                                      wgmma; 2 = also the flow-matching decoder's convs (where their widths are multiples
+                                      of 64) and attention, from the split-bf16 weights weights.pack_stabletts*(...,
+                                      precision=2) adds; its text phase stays fp32 FFMA in every mode */
   int32_t flow_n_heads;            /* heads of the flow's pre_transformer: the reference hard-codes 2 (models.py:355) */
   /* Voice conversion (vtts_convert): input features of the posterior encoder enc_q (models.py:1616, mel_processing.py).
    * Only read when the blob carries enc_q (weights.pack(..., posterior=True)). */
@@ -507,14 +510,20 @@ int vtts_resample(vtts_handle h, const float* wav, const int64_t* lengths, int B
  *   mel_out      out float [B, mel_ld, st_noise] frame-major: utterance b's lengths[b] frames, the rest of each row is not written
  *   denormalise  != 0: mel * mel_std + mel_mean (matcha_tts.py:205), else the normalised mel of the last Euler step
  * Host pointers, atomic on the handle; graphed per (batch, frame bucket, n_timesteps, s == 0, noise / speaker input kind).
- * Runs on the fp32 FFMA pipe in every precision mode.  VTTS_ERR_INVALID: not a StableTTS engine, B < 1, a length outside
+ * Runs on the fp32 FFMA pipe in precision modes 0, 1 and 3; in mode 2 the estimator's convs whose widths are multiples of 64
+ * and its attention run on split-bf16 wgmma (in_proj, final_proj and the Euler update stay fp32), an utterance's mel still the
+ * same alone and in any batch.  VTTS_ERR_INVALID: not a StableTTS engine, B < 1, a length outside
  * [1, mu_ld], n_timesteps out of range, a temperature or guidance scale that is not finite (or s < 0), a speaker id outside
  * [0, st_n_spks), neither sid nor spk_rows.  VTTS_ERR_CAPACITY: mel_ld or noise_ld below the longest utterance.
  * After a call with bit0 of vtts_debug_flags set, vtts_debug_read gives "st_film" [steps][layers][2 hidden], "st_ada"
  * [sequences][layers][6 hidden] (the unconditional sequences after the B conditional ones), "st_cond" (the in_proj operand
  * rows [rows][st_noise + st_hidden]: x after the last step, then cond_proj's output), "st_rope" [max frames][dk / 4] (cos, sin)
  * pairs, and of the first estimator evaluation "st_norm1" (block 0's modulated LayerNorm) and "st_qkv" (block 0's q, k
- * after the rotary embedding, and v), rows [rows][hidden] and [rows][3 hidden]. */
+ * after the rotary embedding, and v), rows [rows][hidden] and [rows][3 hidden].  In precision mode 2 also, of block 0 at step
+ * 0, each plane-writing kernel's input and output rows: "tc_norm_in", "tc_qkv_in" (before the rotary embedding),
+ * "tc_silu_in", "tc_silu", "tc_gate_x", "tc_gate_y", "tc_gate" (fp32 rows), and the planes of "tc_norm", "tc_qkv",
+ * "tc_silu" and "tc_gate" as "<name>_hi" / "<name>_lo" (bf16 bit patterns, two per float), for the kernels whose consumer
+ * runs on the tensor cores. */
 #define VTTS_CFM_MAX_STEPS 64
 int vtts_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int B, int64_t mu_ld, const int64_t* sid,
                     const float* spk_rows, int n_timesteps, float temperature, float guidance_scale, const float* noise,
@@ -542,7 +551,9 @@ int vtts_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengths, int 
  *                denormalise), or NULL: the mel encoder then does not run
  *   denormalise  != 0: mel * mel_std + mel_mean
  * Two enqueues with one host wait between them for the frame counts: the text phase is graphed per (batch, token bucket),
- * the mel phase per (batch, token and frame buckets, n_timesteps, s == 0, noise kind).  fp32 FFMA in every precision mode.
+ * the mel phase per (batch, token and frame buckets, n_timesteps, s == 0, noise kind).  The text phase is fp32 FFMA in every
+ * precision mode, so durations and frame counts do not depend on it; the mel phase is as in vtts_cfm_decode (mode 2: on
+ * the tensor cores).
  * VTTS_ERR_INVALID: not a StableTTS engine or a decoder-only blob, B < 1, t_max outside [1, VTTS_ST_MAX_TOKENS], a length
  * outside [1, t_max], an id or speaker out of range, a pause outside [0, VTTS_ST_MAX_TOKEN_FRAMES], length_scale outside
  * (0, 100], the sampling arguments as vtts_cfm_decode.  VTTS_ERR_CAPACITY, returned after the text phase with mel_lengths

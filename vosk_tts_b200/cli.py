@@ -21,6 +21,10 @@ def main(argv=None):
     p.add_argument("--output", "-o", default="out.wav", type=str, help="optional output filename path")
     p.add_argument("--log-level", default="INFO", help="logging level")
     p.add_argument("--device", type=int, default=0, help="CUDA device index (extension)")
+    p.add_argument("--precision", type=int, default=1, choices=(0, 1, 2, 3),
+                   help="engine precision mode (extension).  VITS voices: 0 fp32 FFMA, 1 flow and decoder on the tensor cores, "
+                        "2 the text encoder as well, 3 as 2 with exact durations.  Multistream voices: 0 fp32 FFMA, 1 vocoder and "
+                        "BERT on the tensor cores, 2 the flow-matching decoder as well, 3 as 1")
     p.add_argument("--convert-from", type=str, help="voice conversion (extension): re-voice this mono WAV as --speaker")
     p.add_argument("--source-speaker", type=int, help="speaker id of the --convert-from recording")
     p.add_argument("--align", type=str, metavar="WAV",
@@ -52,7 +56,7 @@ def main(argv=None):
     if not args.input:
         logging.info("Please specify input text or file")
         return 1
-    model = Model(args.model, args.model_name, args.lang, device=args.device)
+    model = Model(args.model, args.model_name, args.lang, device=args.device, precision=args.precision)
     Synth(model).synth(args.input, args.output, speaker_id=args.speaker, speech_rate=args.speech_rate)
     return 0
 

@@ -256,4 +256,20 @@ dit_euler_kernel(const float* __restrict__ v, float* __restrict__ xc, int ldx, i
   }
 }
 
+// Precision mode 2 (the mel phase's convs and attention on the tensor cores): the kernels above that feed a wgmma operand,
+// writing the same fp32 rows and also the split-bf16 planes of their output.  Defined in st_tc.cu, a translation unit of
+// its own: see there.
+__global__ void dit_norm_planes_kernel(const float* __restrict__ a, int lda, const float* __restrict__ film, const float* __restrict__ y,
+                                       const float* __restrict__ ada, int ada_ld, int gate_off, int shift_off, int scale_off, float eps,
+                                       float* __restrict__ xo, float* __restrict__ no, __nv_bfloat16* __restrict__ p_hi,
+                                       __nv_bfloat16* __restrict__ p_lo, const int* __restrict__ lens, const int* __restrict__ offs, int C);
+__global__ void dit_rope_planes_kernel(float* __restrict__ qkv, const float2* __restrict__ tab, int heads, int dk, int d,
+                                       __nv_bfloat16* __restrict__ p_hi, __nv_bfloat16* __restrict__ p_lo, const int* __restrict__ lens,
+                                       const int* __restrict__ offs);
+__global__ void dit_silu_planes_kernel(float* __restrict__ y, int C, __nv_bfloat16* __restrict__ p_hi, __nv_bfloat16* __restrict__ p_lo,
+                                       const int* __restrict__ lens, const int* __restrict__ offs);
+__global__ void dit_gate_planes_kernel(const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ ada, int ada_ld,
+                                       int gate_off, float* __restrict__ out, int ldo, __nv_bfloat16* __restrict__ p_hi,
+                                       __nv_bfloat16* __restrict__ p_lo, const int* __restrict__ lens, const int* __restrict__ offs, int C);
+
 }  // namespace vtts

@@ -786,9 +786,33 @@ struct vtts_engine {
   void bt_stage(const int64_t* ids, const int64_t* lengths, int64_t ld);
   void bt_enqueue(float* out);
 
-  // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh), fp32 FFMA in every mode
+  // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh): fp32 FFMA in modes 0, 1 and 3; in
+  //      mode 2 the convs in stp_tc and the attention on the tensor cores (DESIGN.md 4.r)
   ConvW st_cp[3], st_in, st_final;                 // cond_proj's three convs, in_proj over (x | cond), final_proj
   std::vector<ConvW> st_lsc;                       // the long-skip convs over (x | skip)
+  // the pipe of each mel-phase stage in precision mode 2 (all false otherwise): a conv runs on conv_tc_kernel when its input
+  // and output widths are multiples of TC_BK (st_tc_fits); in_proj (x | cond) and final_proj stay on the FFMA pipe
+  struct StPipe { bool on = false, cp[3] = {false, false, false}, qkv = false, o = false, ffn1 = false, ffn2 = false, lsc = false, attn = false; } stp_tc;
+  static bool st_tc_fits(int cin, int cout) { return cin % TC_BK == 0 && cout % TC_BK == 0; }
+  TcW st_tcp[3];                                   // split-bf16 weights of cond_proj's convs, of the long skips
+  std::vector<TcW> st_tlsc;
+  // planes of the mel phase's tensor-core operands: mu, cond_proj's two SiLU outputs, the modulated LayerNorm, q | k | v,
+  // the attention output, SiLU(ffn1) and the long-skip operands (null where the consumer runs on the FFMA pipe)
+  struct StPl { Planes mu, p0, p1, N, QKV, AO, FF, cat[4]; } stpl;
+  // debug_flags & 1 in mode 2: copies of what block 0's plane-writing kernels read and wrote at step 0 (vtts_debug_read
+  // "tc_*"): Ttot rows of row_bytes each, taken from rows of pitch_bytes (fp32 rows, or bf16 planes two per float)
+  struct Tap { Buf<float> buf; size_t n = 0; };
+  std::map<std::string, Tap> st_taps;
+  void st_tap(const char* name, const void* src, size_t row_bytes, size_t pitch_bytes) {
+    const size_t T = (size_t)stp.Ttot;
+    Tap& t = st_taps[name];
+    t.n = (T * row_bytes + 3) / 4;
+    CK(cudaMemcpy2DAsync(ensure(t.buf, t.n), row_bytes, src, pitch_bytes, row_bytes, T, cudaMemcpyDeviceToDevice, stream));
+  }
+  void st_tap_planes(const char* hi, const char* lo, const Planes& p, int C, int ld) {
+    st_tap(hi, p.hi, (size_t)C * 2, (size_t)ld * 2);
+    st_tap(lo, p.lo, (size_t)C * 2, (size_t)ld * 2);
+  }
   std::vector<EncLayerW> st_blk;                   // qkv / o / ffn1 / ffn2 of each block; relk / relv point at zeros
   const float *st_tw1 = nullptr, *st_tb1 = nullptr, *st_tw2 = nullptr, *st_tb2 = nullptr, *st_fw = nullptr, *st_fb = nullptr;
   const float *st_aw1 = nullptr, *st_ab1 = nullptr, *st_aw2 = nullptr, *st_ab2 = nullptr;
@@ -816,6 +840,9 @@ struct vtts_engine {
   };
   void st_block(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo, bool tap,
                 const Rows& r);
+  // the same block in precision mode 2 (stp_tc, stpl); xout_pl: the planes of xout's column block, or null
+  void st_block_tc(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo,
+                   const Planes* xout_pl, bool tap, const Rows& r);
 
   // ---- StableTTS text encoder and durations (TextEncoder.forward, MatchaTTS.synthesise; stabletts.cuh): blobs of
   // weights.pack_stabletts.  Stack 0 is the mel encoder (conditioned on spk_emb), stack 1 dp_encoder (on dur_spk_emb).
@@ -3299,6 +3326,39 @@ void vtts_engine::bind_stabletts() {
     st_blk.push_back(L);
     if (l >= NL / 2) st_lsc.push_back(conv("st.lsc" + std::to_string(l - NL / 2), 2 * H, H, k));
   }
+  // precision mode 2: each conv's pipe (st_tc_fits), its split-bf16 weights (weights.pack_stabletts*(..., precision=2)), and
+  // the attention on attn_tc_kernel with zero relative tiles, as BERT runs it (bind_bert)
+  stp_tc = StPipe{};
+  st_tlsc.clear();
+  if (c.precision == 2) {
+    StPipe& p = stp_tc;
+    p.on = true;
+    p.cp[0] = st_tc_fits(MC, F); p.cp[1] = st_tc_fits(F, F); p.cp[2] = st_tc_fits(F, H);
+    p.qkv = st_tc_fits(H, 3 * H); p.o = st_tc_fits(H, H); p.ffn1 = st_tc_fits(H, F); p.ffn2 = st_tc_fits(F, H); p.lsc = st_tc_fits(2 * H, H);
+    const char* first = p.qkv ? "st.l0.qkv" : p.o ? "st.l0.o" : p.ffn1 ? "st.l0.ffn1" : p.ffn2 ? "st.l0.ffn2" : p.lsc ? "st.lsc0"
+                      : p.cp[0] ? "st.cp0" : p.cp[1] ? "st.cp1" : p.cp[2] ? "st.cp2" : nullptr;
+    REQUIRE(!first || tensors.count(std::string(first) + ".th"), VTTS_ERR_WEIGHTS,
+            "the blob lacks the StableTTS decoder's tensor-core weights (pack it with precision=2)");
+    for (int i = 0; i < 3; ++i)
+      if (p.cp[i]) st_tcp[i] = tcw("st.cp" + std::to_string(i), st_cp[i].Cin, st_cp[i].Cout, k);
+    for (int j = 0; j < NL / 2 && p.lsc; ++j) st_tlsc.push_back(tcw("st.lsc" + std::to_string(j), 2 * H, H, k));
+    const int dk = H / c.st_heads;
+    p.attn = dk % 32 == 0 && dk <= 128 && c.window_size == 0;
+    float* z = ensure(d_stzero, std::max<size_t>((size_t)H, (size_t)ATC_RELP * 128));     // (the [16][128] bf16 tiles as well)
+    CK(cudaMemsetAsync(z, 0, d_stzero.cap * sizeof(float), stream));
+    zero = z;                                        // (the text encoder's tables below point here too)
+    const __nv_bfloat16* zb = reinterpret_cast<const __nv_bfloat16*>(z);
+    for (int l = 0; l < NL; ++l) {
+      EncLayerW& L = st_blk[l];
+      const std::string q = "st.l" + std::to_string(l);
+      L.relk = L.relv = z;
+      if (p.qkv) L.t_qkv = tcw(q + ".qkv", H, 3 * H, 1);
+      if (p.o) L.t_o = tcw(q + ".o", H, H, 1);
+      if (p.ffn1) L.t_ffn1 = tcw(q + ".ffn1", H, F, k);
+      if (p.ffn2) L.t_ffn2 = tcw(q + ".ffn2", F, H, k);
+      if (p.attn) L.rk_hi = L.rk_lo = L.rv_hi = L.rv_lo = zb;
+    }
+  }
   // the vocoder, when the blob carries it (weights.pack_hifigan): described by the decoder fields of the config
   has_voc = tensors.count("dec.pre.w") > 0;
   if (has_voc) {
@@ -3413,6 +3473,84 @@ void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const floa
   ++launches;
 }
 
+// st_block with the convs stp_tc takes on conv_tc_kernel and the attention on attn_tc_kernel (precision mode 2, the mel phase
+// only).  Every producer still writes its fp32 rows; those that feed a tensor-core operand also write its planes (stpl).
+void vtts_engine::st_block_tc(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo,
+                              const Planes* xout_pl, bool tap, const Rows& r) {
+  const StPipe& p = stp_tc;
+  const StPl& pl = stpl;
+  const int H = k.H, F = k.F, dk = H / k.heads;
+  const size_t T = (size_t)stp.Ttot;
+  const dim3 gs(r.maxLen, r.n), gn((r.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, r.n);
+  const float* ada = k.ada + (size_t)l * 6 * H;
+  const bool attn_tc = p.attn && attn_use_tc(L, H, r);
+  auto norm = [&](const float* a, int lda, const float* fl, const float* y, int gate, int shift, int scale, bool planes) {
+    if (planes)
+      klaunch(dit_norm_planes_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f,
+              k.Hb, k.N, pl.N.hi, pl.N.lo, r.lens, r.offs, H);
+    else
+      klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f, k.Hb, k.N,
+              r.lens, r.offs, H);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  // one conv of the block: on the tensor cores from the planes `in` when `tc`, else on the FFMA pipe from the fp32 rows x;
+  // `out`: the planes of y its consumer reads (or null)
+  auto cv = [&](bool tc, const ConvW& W, const TcW& tw, const Planes& in, const float* x, float* y, const Planes* out) {
+    if (tc) {
+      TcSpec q;
+      q.in = in; q.w = tw; q.bias = W.b; q.Cin = W.Cin; q.Cout = W.Cout; q.k = W.k; q.pad = (W.k - 1) / 2;
+      q.y = y; q.ldy = W.Cout;
+      if (out) q.out = *out;
+      launch_tc({q}, 1, r);
+    } else {
+      ConvP c = mk(W, x, W.Cin, 0, y, W.Cout, 0, 1, (W.k - 1) / 2);
+      if (out) { c.p_hi = out->hi; c.p_lo = out->lo; c.ldp = out->C; c.pl_slope = 1.f; }
+      launch_conv({c}, 1, r);
+    }
+  };
+  if (tap) st_tap("tc_norm_in", xin, (size_t)H * 4, (size_t)ldi * 4);
+  norm(xin, ldi, film, nullptr, 2, 0, 1, p.qkv || p.ffn1);
+  if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_n, T * H), k.N, T * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  if (tap && (p.qkv || p.ffn1)) st_tap_planes("tc_norm_hi", "tc_norm_lo", pl.N, H, H);
+  cv(p.qkv, L.qkv, L.t_qkv, pl.N, k.N, k.QKV, attn_tc ? &pl.QKV : nullptr);
+  if (tap) st_tap("tc_qkv_in", k.QKV, (size_t)3 * H * 4, (size_t)3 * H * 4);
+  if (attn_tc)
+    klaunch(dit_rope_planes_kernel, gs, dim3(128), (size_t)0, k.QKV, k.rope, k.heads, dk, k.rd, pl.QKV.hi, pl.QKV.lo, r.lens, r.offs);
+  else
+    klaunch(dit_rope_kernel, gs, dim3(128), (size_t)0, k.QKV, k.rope, k.heads, dk, k.rd, r.lens, r.offs);
+  CK(cudaGetLastError());
+  ++launches;
+  if (tap) CK(cudaMemcpyAsync(ensure(d_stdbg_qkv, T * 3 * H), k.QKV, T * 3 * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  if (tap && attn_tc) st_tap_planes("tc_qkv_hi", "tc_qkv_lo", pl.QKV, 3 * H, 3 * H);
+  Planes* pao = p.o ? const_cast<Planes*>(&pl.AO) : nullptr;
+  if (attn_tc) launch_attn_tc(pl.QKV, k.AO, pao, L, H, r);
+  else launch_attn(k.QKV, k.AO, L, H, pao, r);
+  cv(p.o, L.o, L.t_o, pl.AO, k.AO, k.Y, nullptr);
+  norm(k.Hb, H, nullptr, k.Y, 2, 3, 4, p.ffn1);
+  cv(p.ffn1, L.ffn1, L.t_ffn1, pl.N, k.N, k.FF, nullptr);
+  if (tap) st_tap("tc_silu_in", k.FF, (size_t)F * 4, (size_t)F * 4);
+  if (p.ffn2)
+    klaunch(dit_silu_planes_kernel, gs, dim3(256), (size_t)0, k.FF, F, pl.FF.hi, pl.FF.lo, r.lens, r.offs);
+  else
+    klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, k.FF, F, r.lens, r.offs);
+  CK(cudaGetLastError());
+  ++launches;
+  if (tap) st_tap("tc_silu", k.FF, (size_t)F * 4, (size_t)F * 4);
+  if (tap && p.ffn2) st_tap_planes("tc_silu_hi", "tc_silu_lo", pl.FF, F, F);
+  cv(p.ffn2, L.ffn2, L.t_ffn2, pl.FF, k.FF, k.Y, nullptr);
+  if (tap) { st_tap("tc_gate_x", k.Hb, (size_t)H * 4, (size_t)H * 4); st_tap("tc_gate_y", k.Y, (size_t)H * 4, (size_t)H * 4); }
+  if (xout_pl)
+    klaunch(dit_gate_planes_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, xout_pl->hi,
+            xout_pl->lo, r.lens, r.offs, H);
+  else
+    klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, r.lens, r.offs, H);
+  CK(cudaGetLastError());
+  ++launches;
+  if (tap) st_tap("tc_gate", xout, (size_t)H * 4, (size_t)ldo * 4);
+  if (tap && xout_pl) st_tap_planes("tc_gate_hi", "tc_gate_lo", *xout_pl, H, ldo);
+}
+
 // The whole call: uploads, the hoisted conditioning (FiLM rows of every step, adaLN rows of every sequence, cond_proj of both
 // branches, the rotary table), then n Euler steps of the estimator over the ragged batch of both branches.  The step loop is
 // unrolled into the enqueue (and so into the call's graph): step k's FiLM rows and dt are addresses, not values.
@@ -3442,8 +3580,11 @@ void vtts_engine::st_enqueue() {
   // The NS sequences in one fixed launch shape for every conv and one attention kernel (Tuning::fixed_ffma, fixed_attention):
   // every row is summed in the same order whatever the batch, so an utterance's mel does not depend on what it is batched with.
   // The heuristics see every sequence at the bucket, the profiler the unconditional branches at their conditional twins' lengths.
+  // In precision mode 2 the tensor-core convs run without split-K and the attention on attn_tc_kernel (Tuning::fixed_tc), which
+  // keeps that property: each output is summed by one CTA in one k order whatever the launch shape.
+  const StPipe& pp_tc = stp_tc;
   Rows rl{lens, offs, NS, maxFrm, std::vector<int>(NS, maxFrm), std::vector<int>(h_frm_len.begin(), h_frm_len.begin() + Bu),
-          tune.fixed_ffma().fixed_attention()};
+          pp_tc.on ? tune.fixed_ffma().fixed_attention().fixed_tc() : tune.fixed_ffma().fixed_attention()};
   if (stp.guided) rl.real.insert(rl.real.end(), h_frm_len.begin(), h_frm_len.begin() + Bu);
   Rows re = rl;                                     // the same rows over the extents
   re.lens = exts;
@@ -3481,30 +3622,102 @@ void vtts_engine::st_enqueue() {
   auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff, const Rows& r) {
     launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, r);
   };
+  // precision mode 2: the planes of every tensor-core operand (stpl), whose rows behind each sequence's length one
+  // zero_tails launch over the NS sequences clears (producers over the extent then write their rows up to it), and a conv
+  // on the tensor cores where stp_tc puts it
+  const StPipe& pt = pp_tc;
+  stpl = StPl{};
+  if (pt.on) {
+    begin_planes();
+    const long R = (long)T;
+    int slot = 40;    // plane slots 40.. (the flow's in a VITS2 engine; the vocoder uses 0.., BERT 51..)
+    if (pt.cp[0]) stpl.mu = planes(slot++, R, 1, MC);
+    if (pt.cp[1]) stpl.p0 = planes(slot++, R, 1, F);
+    if (pt.cp[2]) stpl.p1 = planes(slot++, R, 1, F);
+    if (pt.qkv || pt.ffn1) stpl.N = planes(slot++, R, 1, H);
+    if (pt.attn) stpl.QKV = planes(slot++, R, 1, 3 * H);
+    if (pt.o) stpl.AO = planes(slot++, R, 1, H);
+    if (pt.ffn2) stpl.FF = planes(slot++, R, 1, F);
+    for (int j = 0; j < nlsc && pt.lsc; ++j) stpl.cat[j] = planes(slot++, R, 1, 2 * H);
+    collecting = false;
+    if (tail.n) {
+      klaunch(zero_tails_kernel, dim3(tail.n, NS), dim3(128), (size_t)0, tail, lens, offs, NS);
+      CK(cudaGetLastError());
+      ++launches;
+    }
+  }
+  auto cvt = [&](bool tc, const ConvW& W, const TcW& tw, const Planes& in, const float* x, int ldx, float* y, int ldy, int yoff, const Planes* out,
+                 int poff, const Rows& r) {
+    if (!tc) {
+      ConvP p = mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2);
+      if (out) { p.p_hi = out->hi + poff; p.p_lo = out->lo + poff; p.ldp = out->C; p.pl_slope = 1.f; }
+      launch_conv({p}, 1, r);
+      return;
+    }
+    TcSpec q;
+    q.in = in; q.w = tw; q.bias = W.b; q.Cin = W.Cin; q.Cout = W.Cout; q.k = W.k; q.pad = (W.k - 1) / 2;
+    q.y = y; q.ldy = ldy; q.yoff = yoff;
+    if (out) { q.out = *out; q.poff = poff; }
+    launch_tc({q}, 1, r);
+  };
+  auto silu_pl = [&](float* y, int width, const Planes& pl) {
+    klaunch(dit_silu_planes_kernel, gs, dim3(256), (size_t)0, y, width, pl.hi, pl.lo, exts, offs);
+    CK(cudaGetLastError());
+    ++launches;
+  };
   // cond_proj (decoder.py:121; not masked: zero padded at the ends of each sequence's extent) into the cond columns of the
   // in_proj operand
-  cv(st_cp[0], mu, MC, p0, F, 0, re);
-  silu(p0, F);
-  cv(st_cp[1], p0, F, p1, F, 0, re);
-  silu(p1, F);
-  cv(st_cp[2], p1, F, xc, XW, NC, re);
-  // DitWrapper (decoder.py:15-18) of block l at step s
-  auto block = [&](int l, int s, const float* xin, int ldi, float* xout, int ldo) {
-    st_block(kb, st_blk[l], l, film + ((size_t)s * NL + l) * 2 * H, xin, ldi, xout, ldo, (debug_flags & 1) && l == 0 && s == 0, rl);
+  if (!pt.on) {
+    cv(st_cp[0], mu, MC, p0, F, 0, re);
+    silu(p0, F);
+    cv(st_cp[1], p0, F, p1, F, 0, re);
+    silu(p1, F);
+    cv(st_cp[2], p1, F, xc, XW, NC, re);
+  } else {
+    if (pt.cp[0]) {     // mu's planes over the extents (dit_init_kernel wrote the padding rows)
+      klaunch(split_planes_kernel, dim3((maxFrm + EW_ROWS - 1) / EW_ROWS, NS), dim3(EW_THREADS), (size_t)0, (const float*)mu, MC, stpl.mu.hi,
+              stpl.mu.lo, MC, MC, 1.f, 0, 1, exts, offs);
+      CK(cudaGetLastError());
+      ++launches;
+    }
+    cvt(pt.cp[0], st_cp[0], st_tcp[0], stpl.mu, mu, MC, p0, F, 0, nullptr, 0, re);
+    if (pt.cp[1]) silu_pl(p0, F, stpl.p0);
+    else silu(p0, F);
+    cvt(pt.cp[1], st_cp[1], st_tcp[1], stpl.p0, p0, F, p1, F, 0, nullptr, 0, re);
+    if (pt.cp[2]) silu_pl(p1, F, stpl.p1);
+    else silu(p1, F);
+    cvt(pt.cp[2], st_cp[2], st_tcp[2], stpl.p1, p1, F, xc, XW, NC, nullptr, 0, re);
+  }
+  // DitWrapper (decoder.py:15-18) of block l at step s; pl: the planes of xout's column block (mode 2), or null
+  auto block = [&](int l, int s, const float* xin, int ldi, float* xout, int ldo, const Planes* pl) {
+    const bool tap = (debug_flags & 1) && l == 0 && s == 0;
+    if (pt.on) st_block_tc(kb, st_blk[l], l, film + ((size_t)s * NL + l) * 2 * H, xin, ldi, xout, ldo, pl, tap, rl);
+    else st_block(kb, st_blk[l], l, film + ((size_t)s * NL + l) * 2 * H, xin, ldi, xout, ldo, tap, rl);
   };
+  // the planes of column block `half` (0: x, 1: skip) of long-skip operand j, or null on the FFMA pipe
+  Planes half_pl[4][2];
+  for (int j = 0; j < nlsc && pt.lsc; ++j)
+    for (int h = 0; h < 2; ++h) {
+      half_pl[j][h] = stpl.cat[j];
+      half_pl[j][h].hi += h * H; half_pl[j][h].lo += h * H;
+    }
+  auto cat_pl = [&](int j, int h) { return pt.lsc ? &half_pl[j][h] : (const Planes*)nullptr; };
   for (int s = 0; s < stp.steps; ++s) {
     // in_proj over (x | cond) (decoder.py:123-124; not masked: over the extent) -> the skip half of the last long-skip operand
-    cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H, re);
+    if (pt.lsc) cvt(false, st_in, TcW{}, Planes{}, xc, XW, cat[nlsc - 1], 2 * H, H, &stpl.cat[nlsc - 1], H, re);
+    else cv(st_in, xc, XW, cat[nlsc - 1], 2 * H, H, re);
     // blocks 0 .. NL/2-1 leave their input as a skip (decoder.py:130-131): block i reads the skip half of cat[nlsc-1-i] and
     // writes the skip half of the next one; the last of them writes the x half of cat[0]
     for (int i = 0; i < nlsc; ++i)
-      block(i, s, cat[nlsc - 1 - i] + H, 2 * H, i + 1 < nlsc ? cat[nlsc - 2 - i] + H : cat[0], 2 * H);
+      block(i, s, cat[nlsc - 1 - i] + H, 2 * H, i + 1 < nlsc ? cat[nlsc - 2 - i] + H : cat[0], 2 * H,
+            i + 1 < nlsc ? cat_pl(nlsc - 2 - i, 1) : cat_pl(0, 0));
     // blocks NL/2 ..: the long-skip conv over (x | skip) (decoder.py:133-134), then the block.  The last one's skip is
     // in_proj's output, whose rows past the length its taps read: its input rows are the extent's (the x half is zero there)
     for (int j = 0; j < nlsc; ++j) {
       const bool last = j + 1 == nlsc;
-      cv(st_lsc[j], cat[j], 2 * H, X, H, 0, last ? re : rl);
-      block(nlsc + j, s, X, H, last ? X2 : cat[j + 1], last ? H : 2 * H);
+      if (pt.on) cvt(pt.lsc, st_lsc[j], pt.lsc ? st_tlsc[j] : TcW{}, stpl.cat[j], cat[j], 2 * H, X, H, 0, nullptr, 0, last ? re : rl);
+      else cv(st_lsc[j], cat[j], 2 * H, X, H, 0, last ? re : rl);
+      block(nlsc + j, s, X, H, last ? X2 : cat[j + 1], last ? H : 2 * H, last ? nullptr : cat_pl(j + 1, 0));
     }
     cv(st_final, X2, H, V, NC, 0, rl);
     const bool end = s + 1 == stp.steps;
@@ -5109,6 +5322,7 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
       for (int j = 0; j <= i; ++j) { rm *= c.upsample_rates[j]; ch /= 2; }
       src = h->d_stage[i].p; n = F * rm * ch;
     }
+    else if (h->st_taps.count(nm)) { src = h->st_taps[nm].buf.p; n = h->st_taps[nm].n; }
     REQUIRE(src != nullptr, VTTS_ERR_INVALID, "unknown or unallocated debug tensor");
     REQUIRE(n <= max_floats, VTTS_ERR_CAPACITY, "debug buffer too small");
     CK(cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));

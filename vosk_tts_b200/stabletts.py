@@ -36,10 +36,10 @@ class StableTTS:
             bt = (bsd, bcfg, precision != 0)
         if self.has_text:
             self.cfg = _config.stabletts_config(dict({"n_vocab": int(sd["encoder.emb.weight"].shape[0])}, **(config or {})))
-            blob, man = _weights.pack_stabletts(sd, self.cfg, vocoder=voc, bert=bt)
+            blob, man = _weights.pack_stabletts(sd, self.cfg, vocoder=voc, bert=bt, precision=precision)
         else:
             self.cfg = _config.stabletts_cfm_config(config)
-            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg, vocoder=voc, bert=bt)
+            blob, man = _weights.pack_stabletts_cfm(sd, self.cfg, vocoder=voc, bert=bt, precision=precision)
         if bt is not None:
             self.cfg["bert"] = bt[1]
         if voc is not None:

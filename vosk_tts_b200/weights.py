@@ -688,23 +688,47 @@ def _sd_getter(sd):
     return g, want
 
 
-def _pack_dit_block(P, g, want, dst, src, H, F, k):
-    """qkv / o / ffn1 / ffn2 of one DiTConVBlock (diffusion_transformer.py:82-96) at state-dict prefix src -> tensors dst.*"""
+def _pack_dit_block(P, g, want, dst, src, H, F, k, convs=None):
+    """qkv / o / ffn1 / ffn2 of one DiTConVBlock (diffusion_transformer.py:82-96) at state-dict prefix src -> tensors dst.*;
+    convs: a dict that also receives each conv's weight [Co, Ci, k] under its tensor name, or None"""
     a = src + "attn.conv_%s."
-    P.conv(dst + ".qkv", np.concatenate([want(a % n + "weight", (H, H, 1)) for n in "qkv"], 0), np.concatenate([g(a % n + "bias") for n in "qkv"]))
-    P.conv(dst + ".o", want(a % "o" + "weight", (H, H, 1)), g(a % "o" + "bias"))
-    P.conv(dst + ".ffn1", want(src + "mlp.conv_1.weight", (F, H, k)), g(src + "mlp.conv_1.bias"))
-    P.conv(dst + ".ffn2", want(src + "mlp.conv_2.weight", (H, F, k)), g(src + "mlp.conv_2.bias"))
+    ws = {".qkv": (np.concatenate([want(a % n + "weight", (H, H, 1)) for n in "qkv"], 0), np.concatenate([g(a % n + "bias") for n in "qkv"])),
+          ".o": (want(a % "o" + "weight", (H, H, 1)), g(a % "o" + "bias")),
+          ".ffn1": (want(src + "mlp.conv_1.weight", (F, H, k)), g(src + "mlp.conv_1.bias")),
+          ".ffn2": (want(src + "mlp.conv_2.weight", (H, F, k)), g(src + "mlp.conv_2.bias"))}
+    for n, (w, b) in ws.items():
+        P.conv(dst + n, w, b)
+        if convs is not None:
+            convs[dst + n] = w
 
 
-def _pack_stabletts_decoder(P, sd, cfg):
+def stabletts_tc_convs(cfg):
+    """Names of the StableTTS decoder convs that precision mode 2 runs on the tensor cores (engine.cu bind_stabletts, the
+    same rule): those whose input and output widths are both multiples of 64 (TC_BK, one 128-byte swizzle atom of bf16).
+    in_proj (x | cond) and final_proj stay on the FFMA pipe: x, the Euler state, and the velocity stay fp32 rows."""
+    NC, MC, H, F, NL = (int(cfg[k]) for k in ("noise_channels", "cond_channels", "hidden_channels", "filter_channels", "n_layers"))
+    fits = lambda ci, co: ci % 64 == 0 and co % 64 == 0
+    names = ["st.cp%d" % i for i, (ci, co) in enumerate(((MC, F), (F, F), (F, H))) if fits(ci, co)]
+    for l in range(NL):
+        names += ["st.l%d%s" % (l, n) for n, ci, co in ((".qkv", H, 3 * H), (".o", H, H), (".ffn1", H, F), (".ffn2", F, H)) if fits(ci, co)]
+    names += ["st.lsc%d" % j for j in range(NL // 2) if fits(2 * H, H)]
+    return names
+
+
+def _pack_stabletts_decoder(P, sd, cfg, precision=1):
+    """st.* tensors of the flow-matching decoder; precision 2 appends the split-bf16 copies (.th / .tl) of the convs in
+    stabletts_tc_convs(cfg), which that mode runs on the tensor cores."""
+    if precision not in (0, 1, 2, 3):
+        raise ValueError("precision must be 0, 1, 2 or 3")
     g, want = _sd_getter(sd)
     e = "decoder.estimator."
     NC, MC, H, F, NL, G = (int(cfg[k]) for k in ("noise_channels", "cond_channels", "hidden_channels", "filter_channels", "n_layers",
                                                  "spk_emb_dim"))
     k = int(cfg["kernel_size"])
+    convs = {}
     for i, (j, co, ci) in enumerate(((0, F, MC), (2, F, F), (4, H, F))):
-        P.conv("st.cp%d" % i, want(e + "cond_proj.%d.weight" % j, (co, ci, k)), want(e + "cond_proj.%d.bias" % j, (co,)))
+        convs["st.cp%d" % i] = want(e + "cond_proj.%d.weight" % j, (co, ci, k))
+        P.conv("st.cp%d" % i, convs["st.cp%d" % i], want(e + "cond_proj.%d.bias" % j, (co,)))
     P.conv("st.in", want(e + "in_proj.weight", (H, NC + H, 1)), g(e + "in_proj.bias"))
     P.conv("st.final", want(e + "final_proj.weight", (NC, H, 1)), g(e + "final_proj.bias"))
     P.add("st.time.w1", want(e + "time_mlp.layer.0.weight", (F, H)))
@@ -724,9 +748,13 @@ def _pack_stabletts_decoder(P, sd, cfg):
     P.add("st.mel_mean", np.asarray(g("mel_mean"), np.float32).reshape(1))
     P.add("st.mel_std", np.asarray(g("mel_std"), np.float32).reshape(1))
     for l in range(NL):
-        _pack_dit_block(P, g, want, "st.l%d" % l, b % l + "block.", H, F, k)
+        _pack_dit_block(P, g, want, "st.l%d" % l, b % l + "block.", H, F, k, convs)
     for j in range(NL // 2):
-        P.conv("st.lsc%d" % j, want(e + "lsc_layers.%d.weight" % j, (H, 2 * H, k)), g(e + "lsc_layers.%d.bias" % j))
+        convs["st.lsc%d" % j] = want(e + "lsc_layers.%d.weight" % j, (H, 2 * H, k))
+        P.conv("st.lsc%d" % j, convs["st.lsc%d" % j], g(e + "lsc_layers.%d.bias" % j))
+    if precision == 2:
+        for name in stabletts_tc_convs(cfg):
+            P.conv_tc(name, convs[name])
 
 
 class _Inert:
@@ -938,17 +966,17 @@ def pack_bert(sd, bt, tc=True):
     return P.finish()
 
 
-def pack_stabletts_cfm(sd, cfg, vocoder=None, bert=None):
+def pack_stabletts_cfm(sd, cfg, vocoder=None, bert=None, precision=1):
     """The flow-matching decoder of a MatchaTTS (StableTTS) state dict -> (blob, manifest) of a model_family "stabletts" engine.
     sd: the checkpoint's `state_dict` entry (keys decoder.estimator.*, spk_emb.weight, fake_speaker, fake_content, mel_mean,
     mel_std); cfg: config.stabletts_cfm_config.  Convs go in the FFMA layout (q, k, v stacked into one 1x1 conv), the small
     linears of the conditioning path (time_mlp, each block's film conv and adaLN_modulation) row-major [out][in] and stacked
-    over the blocks.  Everything is fp32: the decoder runs on the FFMA pipe in every precision mode, so there are no
-    mode-dependent split planes to add yet.  vocoder: (folded Generator state dict, config.hifigan_config) appended as
-    pack_hifigan lays it out, or None; bert: (BertModel state dict, config.bert_config, tc) appended as pack_bert lays it out,
-    or None."""
+    over the blocks, all fp32.  precision: the engine's precision mode; 2 also packs the split-bf16 copies (.th / .tl) of the
+    convs that mode runs on the tensor cores (stabletts_tc_convs), the other modes the same blob as each other.  vocoder:
+    (folded Generator state dict, config.hifigan_config) appended as pack_hifigan lays it out, or None; bert: (BertModel
+    state dict, config.bert_config, tc) appended as pack_bert lays it out, or None."""
     P = _Packer()
-    _pack_stabletts_decoder(P, sd, cfg)
+    _pack_stabletts_decoder(P, sd, cfg, precision)
     if vocoder is not None:
         _pack_hifigan(P, *vocoder)
     if bert is not None:
@@ -956,18 +984,19 @@ def pack_stabletts_cfm(sd, cfg, vocoder=None, bert=None):
     return P.finish()
 
 
-def pack_stabletts(sd, cfg, vocoder=None, bert=None):
+def pack_stabletts(sd, cfg, vocoder=None, bert=None, precision=1):
     """A MatchaTTS (StableTTS) state dict without its vocoder -> (blob, manifest) of an engine that serves text-to-mel
     (vtts_stabletts_synthesise) and the decoder alone: the decoder part of pack_stabletts_cfm, then the text encoder
     (encoder.emb, encoder.punc_emb, encoder.bert_proj.1, both stacks encoder.encoder / encoder.dp_encoder with their proj) and
     dur_spk_emb.  Without encoder.encoder.* (a state dict read from an exported graph, onnx_weights.stabletts_from_onnx) the
-    engine serves everything but the prior.  cfg: config.stabletts_config; vocoder as in pack_stabletts_cfm; bert: (BertModel state dict, config.bert_config,
-    tc) appended as pack_bert lays it out, or None."""
+    engine serves everything but the prior.  cfg: config.stabletts_config; vocoder and precision as in pack_stabletts_cfm (the
+    text encoder is fp32 in every mode); bert: (BertModel state dict, config.bert_config, tc) appended as pack_bert lays it
+    out, or None."""
     if "enc_n_layers" not in cfg:
         raise ValueError("pack_stabletts needs config.stabletts_config (the text encoder's constants), not stabletts_cfm_config")
     g, want = _sd_getter(sd)
     P = _Packer()
-    _pack_stabletts_decoder(P, sd, cfg)
+    _pack_stabletts_decoder(P, sd, cfg, precision)
     V, E, PD, BD, R, H, F, NE, G, DC = (int(cfg[k]) for k in ("n_vocab", "emb_dim", "punc_dim", "bert_dim", "bert_proj_dim",
                                                              "enc_hidden_channels", "enc_filter_channels", "enc_n_layers", "spk_emb_dim",
                                                              "dur_channels"))
