@@ -76,7 +76,8 @@ typedef struct vtts_config {
    * 1 = QuickVC (vc/models.py; weights.pack_quickvc), which serves vtts_speaker_embedding* and vtts_quickvc_convert,
    * 2 = StableTTS (weights.pack_stabletts_cfm: the flow-matching decoder, which serves vtts_cfm_decode; weights.pack_stabletts:
    * the text encoder as well, which also serves vtts_stabletts_synthesise).  The entry points of one family return
-   * VTTS_ERR_INVALID on an engine of another. */
+   * VTTS_ERR_INVALID on an engine of another.  3 = GPT-SoVITS text-to-semantic decoder (weights.pack_t2s), which serves
+   * vtts_t2s_decode. */
   int32_t model_family;
   /* StableTTS flow-matching decoder (model_family 2; CFM of training/stabletts/matcha/models/components/flow_matching.py:301,
    * weights.pack_stabletts_cfm): vtts_cfm_decode.  The other families leave these 0. */
@@ -99,12 +100,16 @@ typedef struct vtts_config {
   /* In StableTTS engines whose blob carries bt.* (BERT: vtts_bert_features) the cv_* fields above describe BERT's transformer:
    * cv_layers the layers that run (the exported graph returns hidden_states[-3], so n_layers - 2 of a checkpoint), cv_hidden,
    * cv_heads, cv_ffn and cv_ln_eps (1e-12).  The rows of the word, position and token-type tables are those of the blob's
-   * bt.emb.word / .pos / .type. */
+   * bt.emb.word / .pos / .type.
+   * In GPT-SoVITS text-to-semantic engines (model_family 3) they describe the GPT's post-LN layers: cv_layers (n_layer),
+   * cv_hidden (hidden_dim = embedding_dim), cv_heads (head), cv_ffn (4 hidden_dim) and cv_ln_eps (1e-5); the phone and semantic
+   * vocabularies and the positions are the rows of the blob's t2s.temb / t2s.aemb / t2s.pe. */
 } vtts_config;
 
 #define VTTS_FAMILY_VITS2 0
 #define VTTS_FAMILY_QUICKVC 1
 #define VTTS_FAMILY_STABLETTS 2
+#define VTTS_FAMILY_T2S 3
 
 /* Replaces onnxruntime.InferenceSession(model.onnx) (vosk_tts/model.py:46).
  * `blob` holds the packed fp32 tensors produced by vosk_tts_b200.weights.pack(); `manifest` is a
@@ -632,6 +637,38 @@ int vtts_stabletts_synthesise_pieces_wav(vtts_handle h, const int64_t* ids, cons
                                          float guidance_scale, const float* noise, int64_t noise_ld, uint64_t seed, float* mel_out,
                                          int64_t mel_ld, int64_t* mel_lengths, int32_t* durations, float* prior_out, int denormalise, float* wav,
                                          int64_t wav_ld, int64_t* wav_lengths);
+
+/* GPT-SoVITS text-to-semantic decoding (Text2SemanticDecoder.infer_panel, training/gpt-sovits/ar/models/t2s_model.py:324-448,
+ * with the sampler of ar/models/utils.py:110-161), for a ragged batch of sentences, each decoded as if alone.
+ *   ids            int64 [B, ids_ld] phone ids; sentence b = its first lengths[b] (1 <= lengths[b] <= ids_ld, at most the
+ *                  position table's rows), every id in [0, rows of t2s.temb)
+ *   bert           float [B, ids_ld, 1024] token-major BERT features, or NULL for zeros (bert_proj's bias alone, as the Russian
+ *                  voice's get_phones_and_bert gives)
+ *   prompts        int64 [B, prompts_ld] semantic tokens of the reference audio with prompt_lengths[b] in [0, prompts_ld], each
+ *                  in [0, EOS), or both NULL (no prompt)
+ *   top_k >= 1, top_p (applied when < 1), temperature (max(temperature, 1e-5) divides), repetition_penalty > 0 (the reference
+ *                  hard-codes 1.35), early_stop_num (-1: none), step_cap (the reference's 1500): an utterance samples at most
+ *                  min(step_cap, early_stop_num + 1) tokens (the step limit)
+ *   seeds          uint64 [B]: q ~ Exp(1) of entry v at sampling step i drawn by Philox keyed by (seeds[b], i, v); or NULL with
+ *   q              float [B, q_ld, V] the reference's q of each sampling step (V = EOS + 1 entries; step 0 reads the first V - 1),
+ *                  q_ld >= the step limit; NULL: seeds
+ *   tokens         out int64 [B, tokens_ld] (tokens_ld >= prompt length + step limit): y[:, :-1] of each utterance, its prompt
+ *                  then the sampled tokens without the last one, n_tokens[b] of them (out int64 [B])
+ *   idx            out int64 [B]: the reference's second return value (0 without a prompt, else the sampled count minus 2)
+ *   logits         out float [B, logits_ld, V] or NULL: the raw logits of every sampling step below logits_ld (step 0's EOS entry
+ *                  included)
+ * The [text; prompt] rows are prefilled under infer_panel's prefix mask; then each step samples one token per utterance and
+ * runs the layers on it.  An utterance stops, frozen, when its count exceeds early_stop_num, when the argmax of its
+ * penalised logits or its sample is EOS, or at step_cap.  The prefill is post_ln_layers: fp32 FFMA in precision
+ * mode 0, split-bf16 tensor cores in modes >= 1; the decode steps are fp32 FFMA in every mode.  Each utterance's tokens are
+ * the same alone and in any batch.  Host pointers, atomic on the handle.  VTTS_ERR_INVALID, before any launch: not a
+ * text-to-semantic engine, B outside [1, 4096], an id or prompt token out of range, a length out of range, a prompt plus the
+ * step limit beyond the position table, top_k < 1, a non-finite or non-positive sampling argument, early_stop_num < -1,
+ * step_cap outside [1, 2^20], neither seeds nor q, q_ld below the step limit.  VTTS_ERR_CAPACITY: tokens_ld too small. */
+int vtts_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, const float* bert,
+                    const int64_t* prompts, const int64_t* prompt_lengths, int64_t prompts_ld, int top_k, float top_p, float temperature,
+                    float repetition_penalty, int early_stop_num, int step_cap, const uint64_t* seeds, const float* q, int64_t q_ld,
+                    int64_t* tokens, int64_t tokens_ld, int64_t* n_tokens, int64_t* idx, float* logits, int64_t logits_ld);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

@@ -6,8 +6,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvtts.so")
-SOURCES = ["engine.cu", "st_gather.cu", "st_tc.cu"]
-DEPS = ["engine.cu", "st_gather.cu", "st_tc.cu", "kernels.cuh", "conv_tc.cuh", "attn_tc.cuh", "wgmma.cuh", "mas.cuh", "vc.cuh", "spk.cuh", "contentvec.cuh", "bert.cuh", "dit.cuh", "stabletts.cuh", "hifigan.cuh", "resample.cuh", "owned.cuh", os.path.join("..", "..", "include", "vtts.h")]
+SOURCES = ["engine.cu", "st_gather.cu", "st_tc.cu", "t2s.cu"]
+DEPS = ["engine.cu", "st_gather.cu", "st_tc.cu", "t2s.cu", "t2s.cuh", "kernels.cuh", "conv_tc.cuh", "attn_tc.cuh", "wgmma.cuh", "mas.cuh", "vc.cuh", "spk.cuh", "contentvec.cuh", "bert.cuh", "dit.cuh", "stabletts.cuh", "hifigan.cuh", "resample.cuh", "owned.cuh", os.path.join("..", "..", "include", "vtts.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

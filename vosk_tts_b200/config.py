@@ -399,3 +399,42 @@ def bert_config(path_or_dict=None, layers=None):
     return {"cv_layers": n, "cv_hidden": H, "cv_heads": nh, "cv_ffn": F, "cv_ln_eps": float(cfg["layer_norm_eps"]),
             "bt_vocab": int(cfg["vocab_size"]), "bt_max_pos": int(cfg["max_position_embeddings"]),
             "bt_type_rows": int(cfg["type_vocab_size"])}
+
+
+T2S_MAX_POSITIONS = 4000     # rows of the sine table SinePositionalEmbedding builds at construction (embedding.py:48)
+
+
+def t2s_config(model, sd=None):
+    """The engine's GPT-SoVITS text-to-semantic shape (cv_* keys for the layers, t2s_* for the tables) from the `model` block
+    of a checkpoint's config (Text2SemanticDecoder.__init__, ar/models/t2s_model.py:39-80), checked against the state dict's
+    tensors when given.  Refuses, with the reason, what the engine does not compute."""
+    H, E, nh, L = (int(model[k]) for k in ("hidden_dim", "embedding_dim", "head", "n_layer"))
+    V, PV, EOS = int(model["vocab_size"]), int(model["phoneme_vocab_size"]), int(model["EOS"])
+    if E != H:
+        raise ValueError("embedding_dim %d != hidden_dim %d: the layers read the embeddings directly" % (E, H))
+    if EOS != V - 1:
+        raise ValueError("EOS %d != vocab_size - 1 (%d): the sampler takes EOS as the last logit" % (EOS, V - 1))
+    if L < 1 or nh < 1 or H % nh or (H // nh) % 32 or H // nh > 128 or H % 16 or H > 1024:
+        raise ValueError("hidden_dim %d / %d heads: the attention kernels take head widths that are multiples of 32 up to 128, "
+                         "and the LayerNorm kernels widths up to 1024" % (H, nh))
+    if 4 * H > 4096:
+        raise ValueError("the FFN width 4 hidden_dim must be at most 4096")
+    if V < 2 or V > 4096:
+        raise ValueError("vocab_size %d: the sampler's block sort takes 2 to 4096 entries" % V)
+    if PV < 1:
+        raise ValueError("phoneme_vocab_size must be positive")
+    if sd is not None:
+        shapes = {"ar_text_embedding.word_embeddings.weight": (PV, H), "ar_audio_embedding.word_embeddings.weight": (V, H),
+                  "ar_predict_layer.weight": (V, H), "bert_proj.weight": (H, 1024)}
+        for k, shp in shapes.items():
+            if k not in sd or tuple(sd[k].shape) != shp:
+                raise ValueError("%s: expected shape %s, found %s" % (k, shp, None if k not in sd else tuple(sd[k].shape)))
+        n = 0
+        while "h.layers.%d.self_attn.in_proj_weight" % n in sd:
+            n += 1
+        if n != L:
+            raise ValueError("the state dict holds %d layers, the config n_layer %d" % (n, L))
+        if tuple(sd["h.layers.0.linear1.weight"].shape) != (4 * H, H):
+            raise ValueError("linear1 must be [4 hidden_dim, hidden_dim] (dim_feedforward = 4 hidden_dim)")
+    return {"model_family": "t2s", "cv_layers": L, "cv_hidden": H, "cv_heads": nh, "cv_ffn": 4 * H, "cv_ln_eps": 1e-5,
+            "t2s_vocab": V, "t2s_phone_vocab": PV, "t2s_positions": T2S_MAX_POSITIONS}

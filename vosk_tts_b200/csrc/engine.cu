@@ -12,6 +12,7 @@
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
+#include <functional>
 #include <thread>
 #include <initializer_list>
 #include <map>
@@ -35,6 +36,7 @@
 #include "hifigan.cuh"
 #include "resample.cuh"
 #include "owned.cuh"
+#include "t2s.cuh"
 
 using namespace vtts;
 
@@ -467,7 +469,7 @@ struct vtts_engine {
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
     TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2, TAG_HIFIGAN = 0xD3,
-    TAG_BERT = 0xD4, TAG_ST_TEXT_PIECES = 0xD5
+    TAG_BERT = 0xD4, TAG_ST_TEXT_PIECES = 0xD5, TAG_T2S = 0xE1
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -764,7 +766,8 @@ struct vtts_engine {
   // rows, whose planes are PX), xb, Y, QKV, AO, FF and, on the tensor cores, the planes of every GEMM operand
   struct PostLnWs { float *xa, *xb, *Y, *QKV, *AO, *FF; Planes PX, PQKV, PAO, PX1, PFF; };
   void post_ln_layers(const std::vector<EncLayerW>& layers, bool on_tc, int H, int Fh, float eps, PostLnWs w, float* out,
-                      const int* out_offs, const Rows& r);
+                      const int* out_offs, const Rows& r, bool relu = false, const std::function<void(int)>* after_qkv = nullptr,
+                      const int* prefix = nullptr);
   void ln_rows(const float* a, const float* y, const LnW& w, float eps, float* out, const int* out_offs, int C, const Planes* pl,
                const Rows& r);
   void gelu_rows(float* y, int C, const Planes* pl, const Rows& r);
@@ -785,6 +788,25 @@ struct vtts_engine {
   void bind_bert();
   void bt_stage(const int64_t* ids, const int64_t* lengths, int64_t ld);
   void bt_enqueue(float* out);
+
+  // ---- GPT-SoVITS text-to-semantic decoder (Text2SemanticDecoder.infer_panel; t2s.cuh, DESIGN.md 4.s): the text rows'
+  //      prefill on post_ln_layers, then one-token decode steps on the t2s_* kernels, graphed T2S_CHUNK steps at a time
+  static constexpr int T2S_CHUNK = 16;
+  static constexpr int T2S_BERT = 1024;             // bert_proj's input width (t2s_model.py:54)
+  int t2s_text_vocab = 0, t2s_vocab = 0, t2s_npos = 0;
+  bool t2s_tc = false;
+  float t2s_alpha[2] = {1.f, 1.f};                 // ar_text_position.alpha, ar_audio_position.alpha
+  const float *t2s_temb = nullptr, *t2s_aemb = nullptr, *t2s_pe = nullptr;
+  ConvW t2s_bp, t2s_pred;
+  std::vector<EncLayerW> t2s_enc;
+  Buf<float> d_t2s_zero, d_t2s_x, d_t2s_x1, d_t2s_y, d_t2s_qkv, d_t2s_ao, d_t2s_ff, d_t2s_pre, d_t2s_bert, d_t2s_bp;
+  Buf<float> d_t2s_k, d_t2s_v, d_t2s_dec, d_t2s_part, d_t2s_q, d_t2s_raw;
+  Buf<int> d_t2s_i, d_t2s_st, d_t2s_tok;
+  Buf<unsigned> d_t2s_seen;
+  Buf<T2sPrm> d_t2s_prm;
+  Buf<unsigned long long> d_t2s_seed;
+  PinnedBuf<char> h_pin_t2s;
+  void bind_t2s();
 
   // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh): fp32 FFMA in modes 0, 1 and 3; in
   //      mode 2 the convs in stp_tc and the attention on the tensor cores (DESIGN.md 4.r)
@@ -3128,22 +3150,43 @@ void vtts_engine::gemm_rows(const Planes& in, const TcW& w, const ConvW& cw, flo
   launch_tc({s}, 1, r);
 }
 
-// The post-LN transformer layers of ContentVec (HubertEncoderLayer) and BERT (BertLayer): x = LN(x + o(attention(qkv(x)))),
-// x = LN(x + ffn2(gelu(ffn1(x)))), with no relative positions (relk / relv of every layer point at zeros).  The input rows are
+// The post-LN transformer layers of ContentVec (HubertEncoderLayer), BERT (BertLayer) and GPT-SoVITS's text prefill
+// (TransformerEncoderLayer; relu): x = LN(x + o(attention(qkv(x)))), x = LN(x + ffn2(act(ffn1(x)))), act GELU or ReLU, with no relative positions (relk / relv of every layer point at zeros).  The input rows are
 // w.xa (on_tc: and their planes w.PX); the last LayerNorm writes row t of sequence b to out row out_offs[b] + t.  on_tc: the
 // convs on conv_tc_kernel and the attention on attn_tc_kernel where r.tune takes it, else everything on the FFMA pipe.
+// after_qkv (or null) is called with the layer index right behind each layer's qkv GEMM, whose rows w.QKV then holds.
+// prefix (or null): [B][4] ints whose first is the text length T of each sequence; the attention then runs under
+// GPT-SoVITS's prefix mask (t2s_prefix_attn_kernel: row t sees key k iff k < T or k <= t) on the fp32 qkv rows.
 void vtts_engine::post_ln_layers(const std::vector<EncLayerW>& layers, bool on_tc, int H, int Fh, float eps, PostLnWs w,
-                                 float* out, const int* out_offs, const Rows& r) {
+                                 float* out, const int* out_offs, const Rows& r, bool relu, const std::function<void(int)>* after_qkv,
+                                 const int* prefix) {
   float *xa = w.xa, *xb = w.xb;
+  auto prefix_attn = [&](const EncLayerW& Lw, const Planes* pl) {
+    const int dk = H / Lw.heads;
+    klaunch(t2s_prefix_attn_kernel, dim3(r.maxLen, Lw.heads, r.n), dim3(32), (size_t)0, (const float*)w.QKV, H, dk,
+            (float)std::sqrt(1.0 / dk), w.AO, r.lens, r.offs, prefix, pl ? pl->hi : (__nv_bfloat16*)nullptr,
+            pl ? pl->lo : (__nv_bfloat16*)nullptr);
+    CK(cudaGetLastError());
+    ++launches;
+  };
+  auto act = [&](const Planes* pl) {
+    if (!relu) { gelu_rows(w.FF, Fh, pl, r); return; }
+    klaunch(t2s_relu_kernel, dim3(r.maxLen, r.n), dim3(256), (size_t)0, w.FF, Fh, r.lens, r.offs, pl ? pl->hi : (__nv_bfloat16*)nullptr,
+            pl ? pl->lo : (__nv_bfloat16*)nullptr);
+    CK(cudaGetLastError());
+    ++launches;
+  };
   for (size_t l = 0; l < layers.size() && on_tc; ++l) {
     const EncLayerW& Lw = layers[l];
     gemm_rows(w.PX, Lw.t_qkv, Lw.qkv, w.QKV, nullptr, &w.PQKV, r);
-    if (attn_use_tc(Lw, H, r)) launch_attn_tc(w.PQKV, w.AO, &w.PAO, Lw, H, r);
+    if (after_qkv) (*after_qkv)((int)l);
+    if (prefix) prefix_attn(Lw, &w.PAO);
+    else if (attn_use_tc(Lw, H, r)) launch_attn_tc(w.PQKV, w.AO, &w.PAO, Lw, H, r);
     else launch_attn(w.QKV, w.AO, Lw, H, &w.PAO, r);
     gemm_rows(w.PAO, Lw.t_o, Lw.o, w.Y, xa, nullptr, r);
     ln_rows(w.Y, nullptr, Lw.ln1, eps, xb, r.offs, H, &w.PX1, r);
     gemm_rows(w.PX1, Lw.t_ffn1, Lw.ffn1, w.FF, nullptr, nullptr, r);
-    gelu_rows(w.FF, Fh, &w.PFF, r);
+    act(&w.PFF);
     gemm_rows(w.PFF, Lw.t_ffn2, Lw.ffn2, w.Y, xb, nullptr, r);
     if (l + 1 == layers.size()) ln_rows(w.Y, nullptr, Lw.ln2, eps, out, out_offs, H, nullptr, r);
     else ln_rows(w.Y, nullptr, Lw.ln2, eps, xa, r.offs, H, &w.PX, r);
@@ -3151,13 +3194,15 @@ void vtts_engine::post_ln_layers(const std::vector<EncLayerW>& layers, bool on_t
   for (size_t l = 0; l < layers.size() && !on_tc; ++l) {
     const EncLayerW& Lw = layers[l];
     launch_conv({mk(Lw.qkv, xa, H, 0, w.QKV, 3 * H, 0, 1, 0)}, 1, r);
-    launch_attn(w.QKV, w.AO, Lw, H, nullptr, r);
+    if (after_qkv) (*after_qkv)((int)l);
+    if (prefix) prefix_attn(Lw, nullptr);
+    else launch_attn(w.QKV, w.AO, Lw, H, nullptr, r);
     ConvP po = mk(Lw.o, w.AO, H, 0, w.Y, H, 0, 1, 0);
     po.res = xa; po.ldr = H;
     launch_conv({po}, 1, r);
     ln_rows(w.Y, nullptr, Lw.ln1, eps, xb, r.offs, H, nullptr, r);
     launch_conv({mk(Lw.ffn1, xb, H, 0, w.FF, Fh, 0, 1, 0)}, 1, r);
-    gelu_rows(w.FF, Fh, nullptr, r);
+    act(nullptr);
     ConvP p2 = mk(Lw.ffn2, w.FF, Fh, 0, w.Y, H, 0, 1, 0);
     p2.res = xb; p2.ldr = H;
     launch_conv({p2}, 1, r);
@@ -3281,6 +3326,66 @@ void vtts_engine::bt_enqueue(float* out) {
   CK(cudaGetLastError());
   ++launches;
   post_ln_layers(bt_enc, bt_tc, H, Fh, c.cv_ln_eps, w, out, r.offs, r);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// GPT-SoVITS text-to-semantic decoder (Text2SemanticDecoder, training/gpt-sovits/ar/models/t2s_model.py:324-448; t2s.cuh)
+// ---------------------------------------------------------------------------------------------------
+void vtts_engine::bind_t2s() {
+  const vtts_config& c = cfg;
+  const int H = c.cv_hidden, F = c.cv_ffn, nh = c.cv_heads;
+  REQUIRE(c.cv_layers >= 1 && nh >= 1 && H % nh == 0 && (H / nh) % 32 == 0 && H / nh <= 128 && H % CV_CK == 0 && H <= 32 * CVL_MAXV &&
+              F >= CV_CK && F % T2S_WARPS == 0 && F <= T2S_MAX_V,
+          VTTS_ERR_INVALID, "unsupported text-to-semantic shape (at least one layer, head width a multiple of 32 up to 128, width a "
+          "multiple of 32 up to 1024, FFN a multiple of 32 up to 4096)");
+  REQUIRE(c.cv_ln_eps > 0.f, VTTS_ERR_INVALID, "the text-to-semantic decoder needs a positive LayerNorm eps");
+  auto rows = [&](const char* name) {
+    const size_t n = tensor(name).n;
+    REQUIRE(n >= (size_t)H && n % H == 0 && n / H <= (size_t)INT32_MAX, VTTS_ERR_WEIGHTS, std::string("bad text-to-semantic table ") + name);
+    return (int)(n / H);
+  };
+  t2s_text_vocab = rows("t2s.temb");
+  t2s_vocab = rows("t2s.aemb");
+  t2s_npos = rows("t2s.pe");
+  REQUIRE(t2s_vocab >= 2 && t2s_vocab <= T2S_MAX_V, VTTS_ERR_INVALID, "the semantic vocabulary (EOS included) must have 2 to 4096 entries");
+  t2s_temb = vec("t2s.temb", (size_t)t2s_text_vocab * H);
+  t2s_aemb = vec("t2s.aemb", (size_t)t2s_vocab * H);
+  t2s_pe = vec("t2s.pe", (size_t)t2s_npos * H);
+  CK(cudaMemcpy(t2s_alpha, vec("t2s.alpha", 2), 2 * sizeof(float), cudaMemcpyDeviceToHost));
+  t2s_bp = conv("t2s.bert_proj", T2S_BERT, H, 1);
+  t2s_pred = conv("t2s.pred", H, t2s_vocab, 1);
+  t2s_tc = c.precision >= 1 && c.precision <= 3;
+  if (t2s_tc) {
+    REQUIRE(H % TC_BK == 0 && F % TC_BK == 0, VTTS_ERR_INVALID, "the text prefill on the tensor cores needs widths in multiples of 64");
+    REQUIRE(tensors.count("t2s.l0.qkv.th") > 0, VTTS_ERR_WEIGHTS, "the blob lacks the text prefill's tensor-core weights");
+  }
+  // zeros for the attention's relative terms, which post_ln_layers' kernels always add (as bind_bert)
+  const size_t nz = std::max<size_t>({(size_t)H, (size_t)(2 * c.window_size + 1) * (H / nh), (size_t)ATC_RELP * 128});
+  float* zero = ensure(d_t2s_zero, nz);
+  CK(cudaMemsetAsync(zero, 0, d_t2s_zero.cap * sizeof(float), stream));
+  t2s_enc.clear();
+  for (int l = 0; l < c.cv_layers; ++l) {
+    const std::string p = "t2s.l" + std::to_string(l);
+    EncLayerW L;
+    L.heads = nh;
+    L.qkv = conv(p + ".qkv", H, 3 * H, 1);
+    L.o = conv(p + ".o", H, H, 1);
+    L.ln1 = ln(p + ".ln1", H);
+    L.ffn1 = conv(p + ".ffn1", H, F, 1);
+    L.ffn2 = conv(p + ".ffn2", F, H, 1);
+    L.ln2 = ln(p + ".ln2", H);
+    L.relk = L.relv = zero;
+    if (t2s_tc) {
+      L.t_qkv = tcw(p + ".qkv", H, 3 * H, 1);
+      L.t_o = tcw(p + ".o", H, H, 1);
+      L.t_ffn1 = tcw(p + ".ffn1", H, F, 1);
+      L.t_ffn2 = tcw(p + ".ffn2", F, H, 1);
+      const __nv_bfloat16* zb = reinterpret_cast<const __nv_bfloat16*>(zero);
+      L.rk_hi = L.rk_lo = L.rv_hi = L.rv_lo = zb;
+    }
+    t2s_enc.push_back(L);
+  }
+  CK(cudaFuncSetAttribute(t2s_ffn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T2S_GEMV_SMEM(F)));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -3912,7 +4017,7 @@ int guarded(vtts_handle h, Fn fn, int mode = G_ATOMIC, int family = VTTS_FAMILY_
   if (!h) return VTTS_ERR_INVALID;
   std::unique_lock<std::mutex> lk(h->mu);
   if (family != ANY_FAMILY && h->cfg.model_family != family) {
-    static const char* const names[] = {"VITS2", "QuickVC", "StableTTS"};
+    static const char* const names[] = {"VITS2", "QuickVC", "StableTTS", "GPT-SoVITS text-to-semantic"};
     h->err = std::string("this entry point serves ") + names[family] + " models; the engine holds a " + names[h->cfg.model_family] + " model";
     return VTTS_ERR_INVALID;
   }
@@ -4378,6 +4483,217 @@ static void impl_bert_features(vtts_handle h, const int64_t* ids, const int64_t*
   h->run_graphed({vtts_engine::TAG_BERT, B, h->btp.maxL, h->btp.tot}, [&] { h->bt_enqueue(h->ensure(h->d_btout, n)); });
   read_clips(h, (const float*)h->d_btout.p, n, n, h->btp.off.data(), h->btp.len, H, out, out_ld * H);
   for (int b = 0; b < B; ++b) std::fill(out + ((size_t)b * out_ld + h->btp.len[b]) * H, out + (size_t)(b + 1) * out_ld * H, 0.f);
+}
+
+// Text-to-semantic decoding through host buffers (vtts_t2s_decode).  The text rows run through post_ln_layers once (each
+// layer's k, v rows copied into the cache behind its qkv GEMM); then every step runs the layers on one audio token per
+// utterance (a prompt token, or the token sampled the step before) and samples the next token once the prompt is read.
+// Steps are enqueued T2S_CHUNK at a time as one graph; between chunks the host reads how many utterances have stopped, one
+// chunk behind, so the device never waits for it.
+static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, const float* bert,
+                            const int64_t* prompts, const int64_t* prompt_lengths, int64_t prompts_ld, int top_k, float top_p,
+                            float temperature, float penalty, int early_stop, int step_cap, const uint64_t* seeds, const float* q,
+                            int64_t q_ld, int64_t* tokens, int64_t tokens_ld, int64_t* n_tokens, int64_t* idx, float* logits,
+                            int64_t logits_ld) {
+  const vtts_config& c = h->cfg;
+  const int H = c.cv_hidden, F = c.cv_ffn, nh = c.cv_heads, dk = H / nh, NL = c.cv_layers, V = h->t2s_vocab;
+  REQUIRE(B >= 1 && B <= 4096, VTTS_ERR_INVALID, "bad batch size");
+  REQUIRE(ids && lengths && ids_ld >= 1, VTTS_ERR_INVALID, "ids, lengths and ids_ld >= 1 are required");
+  REQUIRE(top_k >= 1, VTTS_ERR_INVALID, "top_k must be at least 1");
+  REQUIRE(std::isfinite(top_p) && std::isfinite(temperature) && std::isfinite(penalty) && penalty > 0.f, VTTS_ERR_INVALID,
+          "top_p, temperature and a positive repetition penalty must be finite");
+  REQUIRE(early_stop >= -1, VTTS_ERR_INVALID, "early_stop_num must be -1 (none) or >= 0");
+  REQUIRE(step_cap >= 1 && step_cap <= (1 << 20), VTTS_ERR_INVALID, "the step cap must be in [1, 2^20]");
+  REQUIRE(q || seeds, VTTS_ERR_INVALID, "give per-utterance seeds or q");
+  REQUIRE(!prompts == !prompt_lengths, VTTS_ERR_INVALID, "prompts and prompt_lengths go together");
+  const int gen_max = early_stop < 0 ? step_cap : std::min(step_cap, early_stop + 1);
+  REQUIRE(!q || q_ld >= gen_max, VTTS_ERR_INVALID, "q must hold a row for every step that can sample (q_ld >= the step limit)");
+  REQUIRE(!logits || logits_ld >= 1, VTTS_ERR_INVALID, "logits_ld must be >= 1");
+  std::vector<int> T(B), P(B, 0), Lr(B), off(B), init(4 * (size_t)B), poff(B);
+  long tot = 0, kvn = 0, ytot = 0, ptot = 0;
+  int maxT = 0, maxKv = 0;
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(lengths[b] >= 1 && lengths[b] <= ids_ld, VTTS_ERR_INVALID, "lengths must be in [1, ids_ld]");
+    REQUIRE(lengths[b] <= h->t2s_npos, VTTS_ERR_INVALID, "a text is longer than the position table");
+    T[b] = (int)lengths[b];
+    for (int t = 0; t < T[b]; ++t) {
+      const int64_t v = ids[(size_t)b * ids_ld + t];
+      REQUIRE(v >= 0 && v < h->t2s_text_vocab, VTTS_ERR_INVALID, "a phone id is outside the text embedding table");
+    }
+    if (prompts) {
+      REQUIRE(prompt_lengths[b] >= 0 && prompt_lengths[b] <= prompts_ld, VTTS_ERR_INVALID, "prompt_lengths must be in [0, prompts_ld]");
+      P[b] = (int)prompt_lengths[b];
+      for (int t = 0; t < P[b]; ++t) {
+        const int64_t v = prompts[(size_t)b * prompts_ld + t];
+        REQUIRE(v >= 0 && v < V - 1, VTTS_ERR_INVALID, "a prompt token is outside [0, EOS)");
+      }
+    }
+    REQUIRE((long)P[b] + gen_max <= h->t2s_npos, VTTS_ERR_INVALID, "prompt plus the step limit is longer than the position table");
+    REQUIRE(!tokens || tokens_ld >= (long)P[b] + gen_max, VTTS_ERR_CAPACITY, "tokens_ld is below a prompt length plus the step limit");
+    off[b] = (int)tot;
+    Lr[b] = T[b] + P[b];                             // prefill rows: the text, then the prompt
+    tot += (Lr[b] + 7) / 8 * 8;
+    const int kv = T[b] + P[b] + gen_max;
+    init[4 * b] = T[b]; init[4 * b + 1] = P[b]; init[4 * b + 2] = (int)kvn; init[4 * b + 3] = (int)ytot;
+    poff[b] = (int)ptot;
+    kvn += kv; ytot += P[b] + gen_max; ptot += P[b];
+    REQUIRE(tot < (1L << 24) && kvn < (1L << 28), VTTS_ERR_INVALID, "the batch holds too many rows for one call");
+    maxT = std::max(maxT, Lr[b]); maxKv = std::max(maxKv, kv);
+  }
+  h->B = B;
+  // pinned staging: [T + P B][off B][init 4B][poff B][prefill ids tot][prompts ptot], then the sampling scalars, the seeds and the stop flags
+  const size_t nint = 7 * (size_t)B + tot + ptot;
+  char* pin = h->ensure(h->h_pin_t2s, (nint * sizeof(int) + 15) / 16 * 16 + 64 + 8 * (size_t)B + 16);
+  int* pi = reinterpret_cast<int*>(pin);
+  memcpy(pi, Lr.data(), B * sizeof(int));
+  memcpy(pi + B, off.data(), B * sizeof(int));
+  memcpy(pi + 2 * B, init.data(), 4 * (size_t)B * sizeof(int));
+  memcpy(pi + 6 * B, poff.data(), B * sizeof(int));
+  std::fill(pi + 7 * B, pi + 7 * B + tot, 0);
+  for (int b = 0; b < B; ++b) {
+    for (int t = 0; t < T[b]; ++t) pi[7 * B + off[b] + t] = (int)ids[(size_t)b * ids_ld + t];
+    for (int t = 0; t < P[b]; ++t)
+      pi[7 * B + off[b] + T[b] + t] = pi[7 * B + tot + poff[b] + t] = (int)prompts[(size_t)b * prompts_ld + t];
+  }
+  T2sPrm prm{top_p, temperature, penalty, top_k, early_stop, step_cap, q ? (int)q_ld : 0, logits ? (int)logits_ld : 0};
+  char* pprm = pin + ((nint * sizeof(int) + 15) / 16 * 16);
+  memcpy(pprm, &prm, sizeof(prm));
+  unsigned long long* psd = reinterpret_cast<unsigned long long*>(pprm + 64);
+  for (int b = 0; b < B; ++b) psd[b] = seeds ? (unsigned long long)seeds[b] : 0ull;
+  cudaStream_t s = h->stream;
+  int* di = h->ensure(h->d_t2s_i, nint);
+  CK(cudaMemcpyAsync(di, pi, nint * sizeof(int), cudaMemcpyHostToDevice, s));
+  T2sPrm* dprm = h->ensure(h->d_t2s_prm, 1);
+  CK(cudaMemcpyAsync(dprm, pprm, sizeof(T2sPrm), cudaMemcpyHostToDevice, s));
+  unsigned long long* dseed = h->ensure(h->d_t2s_seed, (size_t)B);
+  CK(cudaMemcpyAsync(dseed, psd, (size_t)B * 8, cudaMemcpyHostToDevice, s));
+  float* dq = nullptr;
+  if (q) {
+    dq = h->ensure(h->d_t2s_q, (size_t)B * q_ld * V);
+    CK(cudaMemcpyAsync(dq, q, (size_t)B * q_ld * V * sizeof(float), cudaMemcpyHostToDevice, s));
+  }
+  float* draw = logits ? h->ensure(h->d_t2s_raw, (size_t)B * logits_ld * V) : nullptr;
+  if (draw) CK(cudaMemsetAsync(draw, 0, (size_t)B * logits_ld * V * sizeof(float), s));
+  const int* dlen = di;
+  const int* doff = di + B;
+  const int* dinit = di + 2 * B;
+
+  // ---- prefill of the [text; prompt] rows under the prefix mask: one fixed launch shape per precision mode, so an
+  //      utterance's rows do not depend on the batch
+  const Tuning tn = h->t2s_tc ? h->tune.fixed_tc() : h->tune.fixed_ffma().fixed_attention();
+  const Rows r{dlen, doff, B, maxT, std::vector<int>(B, maxT), Lr, tn};
+  vtts_engine::PostLnWs w{h->ensure(h->d_t2s_x, tot * H), h->ensure(h->d_t2s_x1, tot * H), h->ensure(h->d_t2s_y, tot * H),
+                          h->ensure(h->d_t2s_qkv, tot * 3 * H), h->ensure(h->d_t2s_ao, tot * H), h->ensure(h->d_t2s_ff, tot * F)};
+  if (h->t2s_tc) {
+    w.PX = h->planes(51, tot, 1, H); w.PQKV = h->planes(52, tot, 1, 3 * H);
+    w.PAO = h->planes(53, tot, 1, H); w.PX1 = h->planes(54, tot, 1, H); w.PFF = h->planes(55, tot, 1, F);
+  }
+  float* kc = h->ensure(h->d_t2s_k, (size_t)NL * kvn * H);
+  float* vc = h->ensure(h->d_t2s_v, (size_t)NL * kvn * H);
+  const float* bp = nullptr;
+  if (bert) {
+    const size_t nb = (size_t)tot * vtts_engine::T2S_BERT;
+    float* hb = reinterpret_cast<float*>(h->ensure(h->h_pin_bt, nb * sizeof(float) + 64));
+    std::fill(hb, hb + nb, 0.f);
+    for (int b = 0; b < B; ++b)
+      memcpy(hb + (size_t)off[b] * vtts_engine::T2S_BERT, bert + (size_t)b * ids_ld * vtts_engine::T2S_BERT,
+             (size_t)T[b] * vtts_engine::T2S_BERT * sizeof(float));
+    float* db = h->ensure(h->d_t2s_bert, nb);
+    CK(cudaMemcpyAsync(db, hb, nb * sizeof(float), cudaMemcpyHostToDevice, s));
+    float* dbp = h->ensure(h->d_t2s_bp, (size_t)tot * H);
+    h->launch_conv({mk(h->t2s_bp, db, vtts_engine::T2S_BERT, 0, dbp, H, 0, 1, 0)}, 1, r);
+    bp = dbp;
+  }
+  h->klaunch(t2s_prefill_embed_kernel, dim3(maxT, B), dim3(128), (size_t)0, (const int*)(di + 7 * B), h->t2s_temb, h->t2s_aemb, bp,
+             h->t2s_bp.b, h->t2s_pe, h->t2s_alpha[0], h->t2s_alpha[1], H, w.xa, dlen, doff, dinit,
+             h->t2s_tc ? w.PX.hi : (__nv_bfloat16*)nullptr, h->t2s_tc ? w.PX.lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++h->launches;
+  const std::function<void(int)> store = [&](int l) {
+    h->klaunch(t2s_kv_store_kernel, dim3(maxT, B), dim3(128), (size_t)0, (const float*)w.QKV, H, kc + (size_t)l * kvn * H,
+               vc + (size_t)l * kvn * H, dlen, doff, dinit);
+    CK(cudaGetLastError());
+    ++h->launches;
+  };
+  float* pre = h->ensure(h->d_t2s_pre, (size_t)tot * H);
+  h->post_ln_layers(h->t2s_enc, h->t2s_tc, H, F, c.cv_ln_eps, w, pre, doff, r, true, &store, dinit);
+
+  // ---- decode state
+  const int rt = (B + T2S_RB - 1) / T2S_RB, nw = (V + 31) / 32;
+  const int nsplit = ((maxKv + T2S_KS - 1) / T2S_KS + 7) / 8 * 8;
+  int* dst = h->ensure(h->d_t2s_st, (size_t)B * T2S_ST + 1);
+  int* nstop = dst + (size_t)B * T2S_ST;
+  int* dy = h->ensure(h->d_t2s_tok, (size_t)ytot);
+  unsigned* seen = h->ensure(h->d_t2s_seen, (size_t)B * nw);
+  float* dec = h->ensure(h->d_t2s_dec, (size_t)B * (6 * H + F + V));
+  float *dx = dec, *dqv = dx + (size_t)B * H, *y1 = dqv + (size_t)B * H, *xm = y1 + (size_t)B * H, *y2 = xm + (size_t)B * H,
+        *hx = y2 + (size_t)B * H, *ff = hx + (size_t)B * H, *lg = ff + (size_t)B * F;
+  float* part = h->ensure(h->d_t2s_part, (size_t)B * nh * nsplit * (dk + 2));
+  CK(cudaMemsetAsync(nstop, 0, sizeof(int), s));
+  h->klaunch(t2s_init_kernel, dim3(B), dim3(256), (size_t)0, dinit, (const int*)(di + 7 * B + tot), (const int*)(di + 6 * B), (const float*)pre,
+             doff, H, V, dst, dy, seen, hx);
+  CK(cudaGetLastError());
+  ++h->launches;
+  std::vector<T2sLayer> Ls(NL);
+  for (int l = 0; l < NL; ++l) {
+    const EncLayerW& E = h->t2s_enc[l];
+    Ls[l] = T2sLayer{E.qkv.w, E.qkv.b, E.o.w, E.o.b, E.ffn1.w, E.ffn1.b, E.ffn2.w, E.ffn2.b, E.ln1.g, E.ln1.b, E.ln2.g, E.ln2.b,
+                     E.qkv.ldw, E.o.ldw, E.ffn1.ldw, E.ffn2.ldw, c.cv_ln_eps, kc + (size_t)l * kvn * H, vc + (size_t)l * kvn * H};
+  }
+  const float scale = (float)std::sqrt(1.0 / dk);
+  auto step = [&] {
+    for (int l = 0; l < NL; ++l) {
+      const T2sLayer& L = Ls[l];
+      h->klaunch(t2s_qkv_kernel, dim3((3 * H + T2S_COLS - 1) / T2S_COLS, rt), dim3(32 * T2S_WARPS), T2S_GEMV_SMEM(H), L,
+                 l ? Ls[l - 1].ln2g : (const float*)nullptr, l ? Ls[l - 1].ln2b : (const float*)nullptr, h->t2s_aemb, h->t2s_pe,
+                 h->t2s_alpha[1], (const int*)dy, (const float*)y2, dx, dqv, (const int*)dst, B, H);
+      h->klaunch(t2s_attn_kernel, dim3(nsplit, nh, B), dim3(32), (size_t)0, (const float*)dqv, (const float*)L.kc, (const float*)L.vc, part,
+                 (const int*)dst, H, dk, scale, nsplit);
+      h->klaunch(t2s_o_kernel, dim3((H + T2S_COLS - 1) / T2S_COLS, rt), dim3(32 * T2S_WARPS), T2S_GEMV_SMEM(H), L, (const float*)part,
+                 (const float*)dx, y1, (const int*)dst, B, H, dk, nsplit);
+      h->klaunch(t2s_ffn1_kernel, dim3((F + T2S_COLS - 1) / T2S_COLS, rt), dim3(32 * T2S_WARPS), T2S_GEMV_SMEM(H), L, (const float*)y1, xm,
+                 ff, (const int*)dst, B, H, F);
+      h->klaunch(t2s_ffn2_kernel, dim3((H + T2S_COLS - 1) / T2S_COLS, rt), dim3(32 * T2S_WARPS), T2S_GEMV_SMEM(F), L, (const float*)ff,
+                 (const float*)xm, y2, (const int*)dst, B, H, F);
+    }
+    h->klaunch(t2s_logits_kernel, dim3((V + T2S_COLS - 1) / T2S_COLS, rt), dim3(32 * T2S_WARPS), T2S_GEMV_SMEM(H), h->t2s_pred.w,
+               h->t2s_pred.ldw, Ls[NL - 1].ln2g, Ls[NL - 1].ln2b, c.cv_ln_eps, (const float*)y2, (const float*)hx, lg, (const int*)dst, B,
+               H, V);
+    h->klaunch(t2s_sample_kernel, dim3(B), dim3(T2S_SAMPLE_THREADS), (size_t)0, (const float*)lg, (const T2sPrm*)dprm,
+               (const unsigned long long*)dseed, (const float*)dq, draw, dst, dy, seen, nstop, V);
+    CK(cudaGetLastError());
+    h->launches += 5 * (uint64_t)NL + 2;
+  };
+  // ---- decode loop: every utterance has stopped after gen_max steps at the latest
+  int* flag = reinterpret_cast<int*>(psd + B);      // two slots, one per chunk in flight
+  const long bound = gen_max;
+  for (long it = 0, chunk = 0;; ++chunk) {
+    h->run_graphed({vtts_engine::TAG_T2S, B, nsplit, kvn, ytot, q ? q_ld : -1, logits ? logits_ld : -1},
+                   [&] { for (int k = 0; k < vtts_engine::T2S_CHUNK; ++k) step(); });
+    CK(cudaMemcpyAsync(flag + (chunk & 1), nstop, sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaEventRecord(h->ev[chunk & 1], s));
+    it += vtts_engine::T2S_CHUNK;
+    if (it >= bound) break;
+    if (chunk >= 1) {
+      CK(cudaEventSynchronize(h->ev[(chunk - 1) & 1]));
+      if (flag[(chunk - 1) & 1] >= B) break;
+    }
+  }
+  // ---- read back
+  std::vector<int> sth((size_t)B * T2S_ST), yh((size_t)ytot);
+  CK(cudaMemcpyAsync(sth.data(), dst, sth.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(yh.data(), dy, yh.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (logits) CK(cudaMemcpyAsync(logits, draw, (size_t)B * logits_ld * V * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (int b = 0; b < B; ++b) {
+    const int* sb = sth.data() + (size_t)b * T2S_ST;
+    REQUIRE(sb[ST_STOP] == 1, VTTS_ERR_STATE, "an utterance did not stop within its step limit");
+    const int gen = sb[ST_GEN], n = P[b] + gen - 1;          // y[:, :-1]: the last appended token is dropped
+    if (n_tokens) n_tokens[b] = n;
+    if (idx) idx[b] = P[b] > 0 ? gen - 2 : 0;
+    if (tokens)
+      for (int i = 0; i < n; ++i) tokens[(size_t)b * tokens_ld + i] = yh[(size_t)init[4 * b + 3] + i];
+  }
 }
 
 // QuickVC conversion through host buffers: from content units (vtts_quickvc_convert, wav null) or from source waveforms through
@@ -4960,8 +5276,9 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     if (const char* e = getenv("VTTS_SPEC_MARGIN")) h->spec_margin = (float)atof(e);      // (< 1 forces mispredictions: tests)
     if (const char* e = getenv("VTTS_CAPTURE_FIRST")) h->capture_on_first = atoi(e) != 0;   // 0: capture a bucket's graph on its second call          // 0: never enqueue phase 2 before the lengths are known    // 0: size everything by the exact lengths
     if (const char* e = getenv("VTTS_PREFETCH")) h->use_prefetch = atoi(e) != 0;
-    REQUIRE(cfg->model_family >= VTTS_FAMILY_VITS2 && cfg->model_family <= VTTS_FAMILY_STABLETTS, VTTS_ERR_INVALID, "unknown model family");
+    REQUIRE(cfg->model_family >= VTTS_FAMILY_VITS2 && cfg->model_family <= VTTS_FAMILY_T2S, VTTS_ERR_INVALID, "unknown model family");
     if (cfg->model_family == VTTS_FAMILY_QUICKVC) h->bind_quickvc();
+    else if (cfg->model_family == VTTS_FAMILY_T2S) h->bind_t2s();
     else if (cfg->model_family == VTTS_FAMILY_STABLETTS) {
       h->bind_stabletts();
       h->bind_bert();
@@ -5358,6 +5675,15 @@ int vtts_content_units(vtts_handle h, const float* wav, const int64_t* wav_lengt
 int vtts_bert_features(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, float* out, int64_t out_ld) {
   if (!ids || !lengths || !out) return VTTS_ERR_INVALID;
   return guarded(h, [&] { impl_bert_features(h, ids, lengths, B, ids_ld, out, out_ld); }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
+}
+
+int vtts_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* lengths, int B, int64_t ids_ld, const float* bert,
+                    const int64_t* prompts, const int64_t* prompt_lengths, int64_t prompts_ld, int top_k, float top_p, float temperature,
+                    float repetition_penalty, int early_stop_num, int step_cap, const uint64_t* seeds, const float* q, int64_t q_ld,
+                    int64_t* tokens, int64_t tokens_ld, int64_t* n_tokens, int64_t* idx, float* logits, int64_t logits_ld) {
+  return guarded(h, [&] { impl_t2s_decode(h, ids, lengths, B, ids_ld, bert, prompts, prompt_lengths, prompts_ld, top_k, top_p, temperature,
+                                          repetition_penalty, early_stop_num, step_cap, seeds, q, q_ld, tokens, tokens_ld, n_tokens, idx,
+                                          logits, logits_ld); }, G_ATOMIC, VTTS_FAMILY_T2S);
 }
 
 int vtts_quickvc_convert_wav(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const float* g,

@@ -64,9 +64,9 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
            "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
-           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations"]
+           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode"]
 
-MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2}    # vtts_config.model_family
+MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
 
 CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
@@ -270,6 +270,9 @@ def load_library(build_if_missing=True):
     st = lib.vtts_stabletts_synthesise_wav.argtypes
     lib.vtts_stabletts_synthesise_pieces_wav.argtypes = st[:5] + [vp, vp, C.c_int64, vp] + st[6:]
     lib.vtts_stabletts_synthesise_pieces_wav.restype = i32
+    lib.vtts_t2s_decode.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, vp, C.c_int64, i32, C.c_float, C.c_float, C.c_float, i32, i32,
+                                    vp, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, C.c_int64]
+    lib.vtts_t2s_decode.restype = i32
     _LIB = lib
     return lib
 
@@ -319,6 +322,13 @@ def _set_decoder_shape(c, cfg):
 
 def make_c_config(cfg, precision=0):
     c = VttsConfig()
+    if cfg.get("model_family") == "t2s":               # config.t2s_config: the GPT's layers in the cv_* fields
+        c.model_family = MODEL_FAMILIES["t2s"]
+        c.precision = int(precision)
+        for k in ("cv_layers", "cv_hidden", "cv_heads", "cv_ffn"):
+            setattr(c, k, int(cfg[k]))
+        c.cv_ln_eps = float(cfg["cv_ln_eps"])
+        return c
     if cfg.get("model_family") == "stabletts":        # the flow-matching decoder reads none of the VITS2 fields
         c.model_family = MODEL_FAMILIES["stabletts"]
         c.precision = int(precision)
@@ -887,6 +897,68 @@ class Engine:
         out = np.zeros((B, max(1, int(lengths.max())), H), np.float32)
         self._check(self.lib.vtts_bert_features(self.h, _ptr(ids), _ptr(lengths), B, L, _ptr(out), out.shape[1]))
         return out, lengths
+
+    def t2s_decode(self, phones, prompts=None, bert=None, top_k=20, top_p=0.6, temperature=0.6, repetition_penalty=1.35,
+                   early_stop_num=-1, step_cap=1500, seeds=0, q=None, logits_steps=0):
+        """GPT-SoVITS text-to-semantic decoding (vtts_t2s_decode) of a ragged batch.  phones: a list of B phone-id sequences;
+        prompts: None or a list of B semantic-token sequences (empty for none); bert: None or a list of B float [T_b, 1024]
+        token-major features; seeds: B ints, or one int s giving sentence b the seed s + b (so that no two sentences of a call
+        share a Philox stream; a sentence keeps its tokens in another batch when it keeps its seed); q: float [B, steps, V] replacing the Philox draws; logits_steps > 0 also
+        returns the raw logits of the first that many sampling steps, float [B, logits_steps, V].
+        Returns (tokens: list of B int64 arrays = y[:, :-1] with the prompt, idx: int64 [B][, logits])."""
+        B = len(phones)
+        if B < 1:
+            raise ValueError("t2s_decode needs at least one sentence")
+        lens = np.array([len(p) for p in phones], np.int64)
+        L = max(1, int(lens.max()))
+        ids = np.zeros((B, L), np.int64)
+        for b, p in enumerate(phones):
+            ids[b, :len(p)] = np.asarray(p, np.int64)
+        pr = pl = None
+        Pld = 0
+        if prompts is not None:
+            if len(prompts) != B:
+                raise ValueError("one prompt per sentence")
+            pl = np.array([len(p) for p in prompts], np.int64)
+            Pld = max(1, int(pl.max()))
+            pr = np.zeros((B, Pld), np.int64)
+            for b, p in enumerate(prompts):
+                pr[b, :len(p)] = np.asarray(p, np.int64)
+        bt = None
+        if bert is not None:
+            bt = np.zeros((B, L, 1024), np.float32)
+            for b, f in enumerate(bert):
+                f = np.asarray(f, np.float32)
+                if f.shape != (lens[b], 1024):
+                    raise ValueError("bert[%d] must be [T, 1024] token-major" % b)
+                bt[b, :lens[b]] = f
+        V = int(self.cfg["t2s_vocab"])
+        gen_max = step_cap if early_stop_num < 0 else min(step_cap, early_stop_num + 1)
+        tok_ld = Pld + max(gen_max, 1)
+        sd = None
+        q_ld = 0
+        if q is not None:
+            q = np.ascontiguousarray(q, np.float32)
+            if q.ndim != 3 or q.shape[0] != B or q.shape[2] != V:
+                raise ValueError("q must be float32 [B, steps, V]")
+            q_ld = q.shape[1]
+        else:
+            sd = np.asarray(seeds, np.uint64).reshape(-1)
+            if sd.size == 1:
+                sd = sd[0] + np.arange(B, dtype=np.uint64)
+            if sd.size != B:
+                raise ValueError("seeds: one int or one per sentence")
+            sd = np.ascontiguousarray(sd)
+        tokens = np.zeros((B, tok_ld), np.int64)
+        n = np.zeros(B, np.int64)
+        idx = np.zeros(B, np.int64)
+        lg = np.zeros((B, logits_steps, V), np.float32) if logits_steps > 0 else None
+        self._check(self.lib.vtts_t2s_decode(self.h, _ptr(ids), _ptr(lens), B, L, _ptr(bt), _ptr(pr), _ptr(pl), Pld, int(top_k),
+                                             float(top_p), float(temperature), float(repetition_penalty), int(early_stop_num),
+                                             int(step_cap), _ptr(sd), _ptr(q), q_ld, _ptr(tokens), tok_ld, _ptr(n), _ptr(idx),
+                                             _ptr(lg), logits_steps))
+        out = [tokens[b, :n[b]].copy() for b in range(B)]
+        return (out, idx, lg) if lg is not None else (out, idx)
 
     def resample(self, wav, from_rate, to_rate, lengths=None, trim_top_db=None, return_bounds=False):
         """Clips at `from_rate` Hz resampled to `to_rate` Hz (vtts_resample: scipy.signal.resample_poly's filter, not soxr), and

@@ -438,3 +438,35 @@ def make_random_bert(bt=None, seed=1234):
         if len(shape) == 3 and shape[2] == 1:
             sd[name] = sd[name][:, :, 0].contiguous()          # the Linear layers: [out, in]
     return sd
+
+
+def make_random_t2s(cfg, seed=1234, eos_scale=1.0):
+    """A Text2SemanticDecoder state dict (CPU fp32) in the reference's names for the shape cfg (config.t2s_config), every tensor
+    seeded by its name.  Weights are drawn at 1 / sqrt(fan-in), embeddings at 0.5, LayerNorm affines around (1, 0), alphas
+    around 1.  eos_scale multiplies the EOS row of ar_predict_layer: above 1 a seeded model stops sooner (its EOS logit
+    spreads further), 0 never lets EOS win."""
+    H, F, V, PV = cfg["cv_hidden"], cfg["cv_ffn"], cfg["t2s_vocab"], cfg["t2s_phone_vocab"]
+    out = [("ar_text_embedding.word_embeddings.weight", (PV, H), "normal", 0.5),
+           ("ar_audio_embedding.word_embeddings.weight", (V, H), "normal", 0.5),
+           ("ar_text_position.alpha", (1,), "gamma", 0.1), ("ar_audio_position.alpha", (1,), "gamma", 0.1)]
+    _conv(out, "bert_proj", H, 1024, 1)
+    _conv(out, "ar_predict_layer", V, H, 1, bias=False, gain=2.0)
+    ln = lambda name: out.extend([(name + ".weight", (H,), "gamma", 0.1), (name + ".bias", (H,), "normal", 0.1)])
+    for l in range(cfg["cv_layers"]):
+        p = "h.layers.%d." % l
+        _conv(out, p + "self_attn.in_proj", 3 * H, H, 1, gain=1.5)
+        _conv(out, p + "self_attn.out_proj", H, H, 1)
+        _conv(out, p + "linear1", F, H, 1)
+        _conv(out, p + "linear2", H, F, 1)
+        ln(p + "norm1")
+        ln(p + "norm2")
+    sd = _draw(out, seed)
+    for name, shape, _, _ in out:
+        if len(shape) == 3 and shape[2] == 1:
+            sd[name] = sd[name][:, :, 0].contiguous()
+    for p in ("in_proj", ):
+        for l in range(cfg["cv_layers"]):
+            w = "h.layers.%d.self_attn.%s" % (l, p)
+            sd[w + "_weight"], sd[w + "_bias"] = sd.pop(w + ".weight"), sd.pop(w + ".bias")
+    sd["ar_predict_layer.weight"][V - 1] *= eos_scale
+    return sd

@@ -7,6 +7,7 @@ stored as ``weight_g`` / ``weight_v``; the exporter loads it and removes weight 
 tensor out the way the CUDA kernels consume it.
 """
 import json
+import math
 
 import numpy as np
 import torch
@@ -1021,4 +1022,68 @@ def pack_stabletts(sd, cfg, vocoder=None, bert=None, precision=1):
         _pack_hifigan(P, *vocoder)
     if bert is not None:
         _pack_bert(P, *bert)
+    return P.finish()
+
+
+def load_t2s(path):
+    """A GPT-SoVITS text-to-semantic checkpoint -> (fp32 state dict in Text2SemanticDecoder's names, config.t2s_config).  Both
+    layouts the reference writes are read:
+    - PyTorch Lightning's (`state_dict` with `model.*` keys, `hyper_parameters.config`), as inference_cli.py:85-97 loads it;
+    - the half-weight export of s1_train.py:73-90 (`weight` in fp16, `config`), as onnx_export.py:89-92 loads it.
+    The file is read with the restricted unpickler of load_lightning_state_dict: nothing it names is imported or called."""
+    ck = torch.load(path, map_location="cpu", weights_only=False, pickle_module=_state_dict_pickle_module())
+    if not isinstance(ck, dict):
+        raise ValueError("%s is not a GPT-SoVITS text-to-semantic checkpoint" % path)
+    if "state_dict" in ck:
+        hp = ck.get("hyper_parameters")
+        conf = hp.get("config") if isinstance(hp, dict) else None
+        sd = {k[len("model."):]: v for k, v in ck["state_dict"].items() if k.startswith("model.")}
+    elif "weight" in ck:
+        conf, sd = ck.get("config"), ck["weight"]
+    else:
+        raise ValueError("%s holds neither `state_dict` (Lightning) nor `weight` (half-weight export)" % path)
+    if not isinstance(conf, dict) or not isinstance(conf.get("model"), dict):
+        raise ValueError("%s carries no config with a `model` block" % path)
+    if not isinstance(sd, dict) or not sd or not all(isinstance(v, torch.Tensor) for v in sd.values()):
+        raise ValueError("%s holds no state dict of tensors" % path)
+    sd = {k: v.float() for k, v in sd.items()}
+    return sd, _config.t2s_config(conf["model"], sd)
+
+
+def t2s_sine_table(n, dim):
+    """SinePositionalEmbedding.extend_pe (ar/modules/embedding.py:53-76) in fp32 on the host, with the reference's formula."""
+    position = torch.arange(0, n, dtype=torch.float32).unsqueeze(1)
+    div_term = torch.exp(torch.arange(0, dim, 2, dtype=torch.float32) * -(math.log(10000.0) / dim))
+    pe = torch.zeros(n, dim)
+    pe[:, 0::2] = torch.sin(position * div_term)
+    pe[:, 1::2] = torch.cos(position * div_term)
+    return pe.numpy()
+
+
+def pack_t2s(sd, cfg, tc=True):
+    """Text2SemanticDecoder (config.t2s_config) -> (blob, manifest) of a model_family "t2s" engine: t2s.temb / t2s.aemb (the
+    phone and semantic embedding tables), t2s.pe (the sine table, computed here), t2s.alpha (text, audio), t2s.bert_proj and
+    t2s.pred (ar_predict_layer, zero bias) as 1x1 convs, then per layer the in_proj q | k | v conv, out_proj, norm1, linear1,
+    linear2 and norm2.  tc: also the split-bf16 copies (.th / .tl) of the layer convs, which the prefill reads in precision
+    modes >= 1."""
+    g, want = _sd_getter(sd)
+    H, F, V, PV, L = (int(cfg[k]) for k in ("cv_hidden", "cv_ffn", "t2s_vocab", "t2s_phone_vocab", "cv_layers"))
+    P = _Packer()
+    P.add("t2s.temb", want("ar_text_embedding.word_embeddings.weight", (PV, H)))
+    P.add("t2s.aemb", want("ar_audio_embedding.word_embeddings.weight", (V, H)))
+    P.add("t2s.pe", t2s_sine_table(int(cfg["t2s_positions"]), H))
+    P.add("t2s.alpha", np.array([float(want("ar_text_position.alpha", (1,))[0]), float(want("ar_audio_position.alpha", (1,))[0])]))
+    P.conv("t2s.bert_proj", want("bert_proj.weight", (H, 1024))[:, :, None], want("bert_proj.bias", (H,)))
+    P.conv("t2s.pred", want("ar_predict_layer.weight", (V, H))[:, :, None], np.zeros(V, np.float32))
+    conv = lambda name, w, b: (P.conv(name, w[:, :, None], b), tc and P.conv_tc(name, w[:, :, None]))
+    for l in range(L):
+        p = "h.layers.%d." % l
+        conv("t2s.l%d.qkv" % l, want(p + "self_attn.in_proj_weight", (3 * H, H)), want(p + "self_attn.in_proj_bias", (3 * H,)))
+        conv("t2s.l%d.o" % l, want(p + "self_attn.out_proj.weight", (H, H)), want(p + "self_attn.out_proj.bias", (H,)))
+        P.add("t2s.l%d.ln1.g" % l, want(p + "norm1.weight", (H,)))
+        P.add("t2s.l%d.ln1.b" % l, want(p + "norm1.bias", (H,)))
+        conv("t2s.l%d.ffn1" % l, want(p + "linear1.weight", (F, H)), want(p + "linear1.bias", (F,)))
+        conv("t2s.l%d.ffn2" % l, want(p + "linear2.weight", (H, F)), want(p + "linear2.bias", (H,)))
+        P.add("t2s.l%d.ln2.g" % l, want(p + "norm2.weight", (H,)))
+        P.add("t2s.l%d.ln2.b" % l, want(p + "norm2.bias", (H,)))
     return P.finish()
