@@ -669,6 +669,21 @@ int vtts_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* lengths, i
                     const int64_t* prompts, const int64_t* prompt_lengths, int64_t prompts_ld, int top_k, float top_p, float temperature,
                     float repetition_penalty, int early_stop_num, int step_cap, const uint64_t* seeds, const float* q, int64_t q_ld,
                     int64_t* tokens, int64_t tokens_ld, int64_t* n_tokens, int64_t* idx, float* logits, int64_t logits_ld);
+/* Unit-test hook of the text-to-semantic sampler: one t2s_sample_kernel launch, as a decode step launches it, on host rows.
+ *   logits [B][V]             one step's logits per row (V = the engine's vocabulary, EOS last)
+ *   state (in/out) [B][8]     each row's decode state as the kernel reads it (t2s.cuh T2sSt: P, NY, GEN, STOP, YOFF); YOFF is
+ *                             set to b * y_ld
+ *   y (in/out) [B][y_ld]      each row's tokens: y[b][0, P + GEN) are its previous tokens (prompt, then sampled), which also
+ *                             make its seen bitmap; the sampled token lands at y[b][P + GEN]
+ *   top_k .. step_cap         the sampling scalars of vtts_t2s_decode
+ *   seeds [B] or q [B][q_ld][V]   the Philox streams, or the caller's Exp(1) draws (row GEN of each)
+ *   seen (out) [B][(V + 31) / 32], n_stopped (out): the bitmap after the launch and the rows that stopped in it
+ *   raw (in/out) [B][raw_ld][V] or NULL: the raw-logit rows the kernel writes (row GEN, when GEN < raw_ld)
+ * VTTS_ERR_INVALID before the launch: not a text-to-semantic engine, B outside [1, 4096], a token outside [0, V), a state out
+ * of range, y_ld <= P + GEN, q_ld <= GEN, both or neither of seeds and q, a sampling argument vtts_t2s_decode refuses. */
+int vtts_debug_t2s_sample(vtts_handle h, int B, const float* logits, int32_t* state, int32_t* y, int y_ld, int top_k, float top_p,
+                          float temperature, float repetition_penalty, int early_stop_num, int step_cap, const uint64_t* seeds,
+                          const float* q, int q_ld, uint32_t* seen, int32_t* n_stopped, float* raw, int raw_ld);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

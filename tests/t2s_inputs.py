@@ -11,6 +11,20 @@ WIDE = {"hidden_dim": 128, "embedding_dim": 128, "head": 4, "n_layer": 3, "vocab
         "dropout": 0.0, "EOS": 256}
 
 
+def _block(hidden, heads, vocab, layers=2):
+    return {"hidden_dim": hidden, "embedding_dim": hidden, "head": heads, "n_layer": layers, "vocab_size": vocab,
+            "phoneme_vocab_size": 60, "dropout": 0.0, "EOS": vocab - 1}
+
+
+# the head widths above 32 (dk = hidden / heads), the vocabularies whose padded sort size is the vocabulary itself or above
+# 2048, and the widest shape the engine takes (FFN 4096: t2s_ffn2_kernel's 80 KiB of shared memory)
+D64 = _block(128, 2, 1024)
+D96 = _block(192, 2, 2049)
+D96_1 = _block(96, 1, 65)          # width 96: the tensor-core prefill (precision mode >= 1) refuses it
+D128 = _block(256, 2, 4096)
+MAX = _block(1024, 8, 4096)
+
+
 def model(block=SMALL, seed=5, eos_scale=1.0, eos_logit=None):
     """eos_logit: the last layer's norm2 weight scaled by 0.3 and the EOS row of ar_predict_layer set so that the hidden rows'
     common part (norm2's bias) gives EOS that logit: EOS then competes with the top tokens at every step, and the repetition

@@ -6145,6 +6145,62 @@ int vtts_debug_spline(vtts_handle h, int B, const int* lens, size_t rows, const 
   });
 }
 
+int vtts_debug_t2s_sample(vtts_handle h, int B, const float* logits, int32_t* state, int32_t* y, int y_ld, int top_k, float top_p,
+                          float temperature, float penalty, int early_stop, int step_cap, const uint64_t* seeds, const float* q, int q_ld,
+                          uint32_t* seen, int32_t* n_stopped, float* raw, int raw_ld) {
+  return guarded(h, [&] {
+    const int V = h->t2s_vocab, nw = (V + 31) / 32;
+    REQUIRE(B >= 1 && B <= 4096, VTTS_ERR_INVALID, "debug_t2s_sample: bad batch size");
+    REQUIRE(logits && state && y && seen && n_stopped, VTTS_ERR_INVALID, "debug_t2s_sample: missing input or output");
+    REQUIRE(!q != !seeds, VTTS_ERR_INVALID, "debug_t2s_sample: give per-row seeds or q, not both");
+    REQUIRE(top_k >= 1 && std::isfinite(top_p) && std::isfinite(temperature) && std::isfinite(penalty) && penalty > 0.f &&
+                early_stop >= -1 && step_cap >= 1,
+            VTTS_ERR_INVALID, "debug_t2s_sample: bad sampling arguments");
+    REQUIRE(!raw || raw_ld >= 1, VTTS_ERR_INVALID, "debug_t2s_sample: raw_ld must be >= 1");
+    REQUIRE(y_ld >= 1 && (size_t)B * y_ld < (1u << 31), VTTS_ERR_INVALID, "debug_t2s_sample: y_ld must be >= 1 and y below 2^31 slots");
+    // each row's tokens sit at y[b][0 ..): its state's YOFF is b * y_ld, and its previous tokens y[b][0, P + GEN) mark the
+    // seen bitmap, as t2s_init_kernel and the earlier steps leave it
+    std::vector<int32_t> sh(state, state + (size_t)B * T2S_ST);
+    std::vector<uint32_t> sn((size_t)B * nw, 0u);
+    for (int b = 0; b < B; ++b) {
+      int32_t* s = sh.data() + (size_t)b * T2S_ST;
+      const int P = s[ST_P], gen = s[ST_GEN], ny = s[ST_NY];
+      REQUIRE(P >= 0 && gen >= 0 && ny >= 0 && ny <= P + gen && (s[ST_STOP] == 0 || s[ST_STOP] == 1), VTTS_ERR_INVALID,
+              "debug_t2s_sample: a row's state is out of range (P, GEN >= 0, 0 <= NY <= P + GEN, STOP 0 or 1)");
+      REQUIRE(y_ld > P + gen, VTTS_ERR_INVALID, "debug_t2s_sample: y_ld must exceed P + GEN, the slot of the next token");
+      REQUIRE(!q || q_ld > gen, VTTS_ERR_INVALID, "debug_t2s_sample: q_ld must exceed GEN, the row of this step's draws");
+      s[ST_YOFF] = b * y_ld;
+      for (int i = 0; i < P + gen; ++i) {
+        const int tok = y[(size_t)b * y_ld + i];
+        REQUIRE(tok >= 0 && tok < V, VTTS_ERR_INVALID, "debug_t2s_sample: a previous token is outside the vocabulary");
+        sn[(size_t)b * nw + (tok >> 5)] |= 1u << (tok & 31);
+      }
+    }
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    const T2sPrm prm{top_p, temperature, penalty, top_k, early_stop, step_cap, q ? q_ld : 0, raw ? raw_ld : 0};
+    const float* dlg = static_cast<const float*>(upload(dev, logits, (size_t)B * V * sizeof(float), st));
+    const T2sPrm* dprm = static_cast<const T2sPrm*>(upload(dev, &prm, sizeof(prm), st));
+    const unsigned long long* dsd = seeds ? static_cast<const unsigned long long*>(upload(dev, seeds, (size_t)B * 8, st)) : nullptr;
+    const float* dq = q ? static_cast<const float*>(upload(dev, q, (size_t)B * q_ld * V * sizeof(float), st)) : nullptr;
+    float* draw = raw ? static_cast<float*>(upload(dev, raw, (size_t)B * raw_ld * V * sizeof(float), st)) : nullptr;
+    int* dst = static_cast<int*>(upload(dev, sh.data(), sh.size() * sizeof(int), st));
+    int* dy = static_cast<int*>(upload(dev, y, (size_t)B * y_ld * sizeof(int), st));
+    unsigned* dsn = static_cast<unsigned*>(upload(dev, sn.data(), sn.size() * sizeof(unsigned), st));
+    const int zero = 0;
+    int* dns = static_cast<int*>(upload(dev, &zero, sizeof(int), st));
+    h->klaunch(t2s_sample_kernel, dim3(B), dim3(T2S_SAMPLE_THREADS), (size_t)0, dlg, dprm, dsd, dq, draw, dst, dy, dsn, dns, V);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(state, dst, (size_t)B * T2S_ST * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(y, dy, (size_t)B * y_ld * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(seen, dsn, sn.size() * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(n_stopped, dns, sizeof(int), cudaMemcpyDeviceToHost));
+    if (raw) CK(cudaMemcpy(raw, draw, (size_t)B * raw_ld * V * sizeof(float), cudaMemcpyDeviceToHost));
+  }, G_ATOMIC, VTTS_FAMILY_T2S);
+}
+
 int vtts_debug_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* z, float length_scale, int frame_cap,
                          const float* stats, const float* eps, int64_t eps_ld, float noise_scale, int32_t* wceil, int32_t* cum,
                          int32_t* ylen, int32_t* ylen_real, int32_t* frm_off, int32_t* published, size_t frame_rows, float* z_p,

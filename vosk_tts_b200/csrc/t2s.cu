@@ -659,6 +659,7 @@ t2s_sample_kernel(const float* __restrict__ lg, const T2sPrm* __restrict__ prm, 
   const float temp = fmaxf(pr.temperature, 1e-5f);
   const int kk = min(pr.top_k, Vv);
   const float pivot = kk - 1 < K ? __fdiv_rn(kv[kk - 1], temp) : -INFINITY;
+  __syncthreads();                                 // every warp has read kv[kk - 1] before the loop below overwrites it
   // final logits in sorted order, softmax, then argmax(probs / q) (first index on ties)
   float mx = -INFINITY;
   for (int i = tid; i < NS; i += blockDim.x) {

@@ -64,7 +64,8 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
            "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
-           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode"]
+           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode",
+           "vtts_debug_t2s_sample"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -273,6 +274,9 @@ def load_library(build_if_missing=True):
     lib.vtts_t2s_decode.argtypes = [vp, vp, vp, i32, C.c_int64, vp, vp, vp, C.c_int64, i32, C.c_float, C.c_float, C.c_float, i32, i32,
                                     vp, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, C.c_int64]
     lib.vtts_t2s_decode.restype = i32
+    lib.vtts_debug_t2s_sample.argtypes = [vp, i32, vp, vp, vp, i32, i32, C.c_float, C.c_float, C.c_float, i32, i32, vp, vp, i32, vp, vp,
+                                          vp, i32]
+    lib.vtts_debug_t2s_sample.restype = i32
     _LIB = lib
     return lib
 
@@ -1237,6 +1241,30 @@ class Engine:
         lens = np.ascontiguousarray(lens, dtype=np.int32)
         self._check(self.lib.vtts_debug_spline(self.h, lens.size, _ptr(lens), x1.shape[0], _ptr(params), params.shape[1], _ptr(x1)))
         return x1
+
+    def debug_t2s_sample(self, logits, state, y, top_k=20, top_p=0.6, temperature=0.6, repetition_penalty=1.35, early_stop_num=-1,
+                         step_cap=1500, seeds=None, q=None, raw=None):
+        """One t2s_sample_kernel launch (vtts_debug_t2s_sample) on logits float32 [B, V], state int32 [B, 8] (P, NY, GEN, STOP,
+        YOFF at the indices of t2s.cuh T2sSt; YOFF becomes b * y_ld) and y int32 [B, y_ld], whose first P + GEN entries of a
+        row are its previous tokens.  Exactly one of seeds (uint64 [B]) and q (float32 [B, q_ld, V]); raw: float32
+        [B, raw_ld, V] raw-logit rows to fill, or None.  Returns a dict of state, y, seen (uint32 [B, (V + 31) // 32]),
+        n_stopped and raw."""
+        V = int(self.cfg["t2s_vocab"])
+        logits = np.ascontiguousarray(logits, dtype=np.float32)
+        if logits.ndim != 2 or logits.shape[1] != V:
+            raise ValueError("logits: shape %s, expected (B, %d)" % (logits.shape, V))
+        B = logits.shape[0]
+        y = np.ascontiguousarray(y, dtype=np.int32)
+        state, y, seeds, q, raw = self._hook_arrays([("state", state, np.int32, (B, 8)), ("y", y, np.int32, (B, None)),
+                                                     ("seeds", seeds, np.uint64, (B,)), ("q", q, np.float32, (B, None, V)),
+                                                     ("raw", raw, np.float32, (B, None, V))])
+        seen = np.zeros((B, (V + 31) // 32), np.uint32)
+        ns = np.zeros(1, np.int32)
+        self._check(self.lib.vtts_debug_t2s_sample(self.h, B, _ptr(logits), _ptr(state), _ptr(y), y.shape[1], int(top_k), float(top_p),
+                                                   float(temperature), float(repetition_penalty), int(early_stop_num), int(step_cap),
+                                                   _ptr(seeds), _ptr(q), 0 if q is None else q.shape[1], _ptr(seen), _ptr(ns),
+                                                   _ptr(raw), 0 if raw is None else raw.shape[1]))
+        return dict(state=state, y=y, seen=seen, n_stopped=int(ns[0]), raw=raw)
 
     def debug_durations(self, lens, z, length_scale, stats, eps, noise_scale, frame_rows, frame_cap=0, wceil=None, cum=None, z_p=None,
                         frame_token=None):
