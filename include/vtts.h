@@ -356,6 +356,23 @@ int vtts_debug_durations(vtts_handle h, int B, const int* lens, size_t rows, con
 int vtts_debug_stt_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* mu_dp, const float* pause,
                              float length_scale, const float* x, const float* mu_mel, int denormalise, int32_t* dur, int32_t* first,
                              int32_t* ylen, float* logw, size_t frame_rows, float* mu, float* pau, float* prior, float* mel);
+/* Unit-test hooks of the spectral kernels, with the packing and in/out rules of the duration hooks above.
+ * vtts_debug_front_end: the front end of vtts_convert / vtts_align / vtts_speaker_embedding (clip lengths checked and framed
+ * as they are, staged with NaN behind every clip) on wav [B][ld] (from_spec 0) or features [B][spec_channels][ld] (1):
+ * frames [B] out, mag [rows][filter_length/2+1] (in/out, mel engines' waveform input only, else NULL) and feat [rows][spec_pad
+ * (spec_channels rounded up to 16, n_mel_channels for QuickVC)] (in/out), rows packed from the frame counts. */
+int vtts_debug_front_end(vtts_handle h, int from_spec, const float* in, const int64_t* lengths, int B, int64_t ld, int32_t* frames,
+                         size_t rows, float* mag, float* feat);
+/* vtts_debug_istft: istft_pqmf_kernel as the decoders launch it, on conv_post rows post [rows][subbands * (istft_n_fft + 2)]
+ * of B utterances of lens[b] frames, packed from row `first` (utterance b: up_total * lens[b] + 1 rows from up_total * offs[b]
+ * + b) -> wav [n_wav] (in/out; utterance b: hop * lens[b] samples from hop * offs[b]). */
+int vtts_debug_istft(vtts_handle h, int B, const int* lens, int first, size_t rows, const float* post, size_t n_wav, float* wav);
+/* vtts_debug_mrf_mean: the MRF mean of n (1..3) resblock outputs x [n][rows][C] (utterance b: rmul * lens[b] rows from rmul *
+ * offs[b]).  use_tc 0: mrf_mean_kernel over all rows -> out [rows][C]; hi / lo NULL.  use_tc 1: mrf_mean_planes_kernel ->
+ * split-bf16 planes hi / lo [plane_rows][C] (in/out) of lrelu(mean, last ? 0.01 : 0.1), with `last` the reflect row at
+ * row rmul * offs[b] + b, and the mean into out [rows][C] (in/out) unless NULL. */
+int vtts_debug_mrf_mean(vtts_handle h, int use_tc, int B, const int* lens, int rmul, int C, int n, size_t rows, const float* x,
+                        int last, float* out, size_t plane_rows, uint16_t* hi, uint16_t* lo);
 /* The split-K plan the engine makes for one grouped tensor-core conv launch, computed on the host alone (no device, no
  * engine).  Problems p < n (1..4): cin[p] (a multiple of 64), cout[p], k[p], in_extra[p]; B utterances of lens[b] <= max_len
  * rows / rmul; bn 64 / 128 pins the tile width (0: either); max_split caps the cluster size (8: none); min_steps = k-steps
@@ -370,14 +387,14 @@ int vtts_tc_split_plan(int n, const int* cin, const int* cout, const int* k, con
  * from the input lengths: frames = (len + 2*pad - filter_length) / hop_length + 1, pad = (filter_length - hop_length) / 2,
  * i.e. len / 256 for the reference configuration).
  *   wav          float [B, wav_ld] in [-1, 1], clip b = wav[b*wav_ld .. + wav_lengths[b]); every clip is padded and framed
- *                on its own samples; needs wav_lengths[b] > pad (385 samples for the reference configuration)
+ *                on its own samples; needs wav_lengths[b] >= max(pad + 1, hop_length) (385 samples for the reference configuration)
  *   noise_scale  scales the posterior's eps (the reference uses 1); 0 gives z = m
  *   noise_q      float [B, inter_channels, q_ld] replaces torch.randn_like at models.py:841 (columns < frames[b] read), or
  *                NULL -> Philox(seed)
  *   out_wav      out float [B, out_ld]: clip b gets hop * out_frames[b] samples
  *   out_frames   out int64 [B]
  * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: the blob has no enc_q, n_speakers <= 1, a speaker id out of range,
- * a clip too short for the reflect padding, or an odd flow_n_flows (the Flip folding of the packed flow is only valid for
+ * a clip too short for the reflect padding and one frame, or an odd flow_n_flows (the Flip folding of the packed flow is only valid for
  * both directions with an even count).  VTTS_ERR_CAPACITY: out_ld < hop * max(frames). */
 int vtts_convert(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, const int64_t* sid_src,
                  const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed, float* out_wav,
@@ -401,7 +418,7 @@ int vtts_convert_spec(vtts_handle h, const float* spec, const int64_t* spec_leng
  *   out_frames   out int64 [B]
  * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: the blob has no enc_q (model.onnx never has it: pack with
  * posterior=True), an odd flow_n_flows, a phoneme id out of [0, n_vocab), a speaker id out of range for a multi-speaker
- * model, a clip too short for the reflect padding, t_x < 1, t_x > frames (no monotonic path exists) or t_x > 2048.
+ * model, a clip too short for the reflect padding and one frame, t_x < 1, t_x > frames (no monotonic path exists) or t_x > 2048.
  * VTTS_ERR_CAPACITY: tof_ld < max(frames) or q_ld < max(frames). */
 int vtts_align(vtts_handle h, const int64_t* ids, const int64_t* id_lengths, int t_max, const int64_t* sid, const float* wav,
                const int64_t* wav_lengths, int B, int64_t wav_ld, float noise_scale, const float* noise_q, int q_ld, uint64_t seed,
@@ -418,10 +435,10 @@ int vtts_align_spec(vtts_handle h, const int64_t* ids, const int64_t* id_lengths
  * and L2 normalisation, and g is the mean over the clip's slices.  One call, no host synchronisation inside.
  *   wav          float [B, wav_ld] in [-1, 1] at the model's sampling rate (16 kHz), clip b = wav[b*wav_ld .. +
  *                wav_lengths[b]); each clip is framed on its own samples (frames = (len + 2*pad - filter_length) / hop_length
- *                + 1, pad = (filter_length - hop_length) / 2), and needs wav_lengths[b] > pad (480 samples at the published
- *                configuration)
+ *                + 1, pad = (filter_length - hop_length) / 2), and needs wav_lengths[b] >= max(pad + 1, hop_length) (481 samples at
+ *                the published configuration)
  *   g_out        out float [B, gin_channels]
- * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: not a QuickVC engine, a clip too short for the reflect padding. */
+ * Host pointers, atomic on the handle.  VTTS_ERR_INVALID: not a QuickVC engine, a clip too short for the reflect padding and one frame. */
 int vtts_speaker_embedding(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, float* g_out);
 /* Same from log-mel rows: mel float [B, n_mel_channels, mel_ld] (the reference's mel_spectrogram_torch output),
  * mel_lengths[b] frames valid (1 <= mel_lengths[b] <= mel_ld). */

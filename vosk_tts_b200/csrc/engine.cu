@@ -689,6 +689,10 @@ struct vtts_engine {
     stage_noise(pin, noise_z, z_ld, std::vector<int>(B, std::min(z_ld, maxFrm)));
   }
   void decode(float* z, const Rows& r, bool planes_ready = false, bool pz_ready = false);
+  // The decoder's element-wise launches, shared by both decoders and the unit-test hooks (vtts_debug_mrf_mean / _istft)
+  void mrf_mean(const std::vector<float*>& xj, float* X, long total4);
+  void mrf_mean_planes(const std::vector<float*>& xj, float* out, const Planes& nxt, int ch, bool last, int rm, const Rows& r);
+  void istft_tail(const float* post, int rm, const Rows& r, float* wav);
   bool have_latent = false;
   Buf<int> d_chunk;                              // [len, off, off_end] of the chunk being decoded
 
@@ -1018,6 +1022,8 @@ void vtts_engine::bind_weights() {
                 c.filter_length > c.hop_length && (c.filter_length - c.hop_length) % 2 == 0,
             VTTS_ERR_INVALID, "bad spectrogram configuration (filter_length must be a multiple of 64, above hop_length)");
     REQUIRE(c.win_length == c.filter_length, VTTS_ERR_INVALID, "win_length != filter_length is not supported by the spectrogram front end");
+    REQUIRE(!c.use_mel_posterior_encoder || mel_smem_bytes(c.filter_length) <= (size_t)MEL_SMEM_MAX, VTTS_ERR_INVALID,
+            "filter_length too large for the mel projection (its spectrum rows must fit in shared memory)");
     REQUIRE(c.use_mel_posterior_encoder ? c.spec_channels == c.n_mel_channels : c.spec_channels == c.filter_length / 2 + 1,
             VTTS_ERR_INVALID, "spec_channels does not match the posterior encoder's input (n_mel_channels / filter_length/2+1)");
     spec_pad = (c.spec_channels + CV_CK - 1) / CV_CK * CV_CK;     // enc_q.pre runs on the FFMA conv: input zero-padded to 16 channels
@@ -1848,14 +1854,7 @@ bool vtts_engine::decoder_tc(float* z, bool pz_ready, const Rows& r) {
     }
     const bool last = (i + 1 == c.n_upsamples);
     Planes nxt = st_nxt[i];
-    {
-      dim3 g((r.maxLen * rm + (last ? 1 : 0) + EW_ROWS - 1) / EW_ROWS, r.n);
-      klaunch(mrf_mean_planes_kernel, dim3(g), dim3(EW_THREADS), (size_t)(0), xj[0], nk > 1 ? xj[1] : nullptr, nk > 2 ? xj[2] : nullptr, std::min(nk, 3),
-                                                   (debug_flags & 1) ? X : nullptr, nxt.hi, nxt.lo, ch, last ? 0.01f : 0.1f,
-                                                   last ? 1 : 0, rm, r.lens, r.offs);
-      CK(cudaGetLastError());
-      ++launches;
-    }
+    mrf_mean_planes(xj, (debug_flags & 1) ? X : nullptr, nxt, ch, last, rm, r);
     cur = nxt;
     lastX = X;
   }
@@ -1884,7 +1883,36 @@ bool vtts_engine::decoder_tc(float* z, bool pz_ready, const Rows& r) {
     q.y = post; q.ldy = pc; q.in_extra = 1; q.out_seq_extra = 1;
     launch_tc({q}, rm, r);
   }
-  float* wav = ensure(d_wav, (size_t)F * hop + 16);
+  istft_tail(post, rm, r, ensure(d_wav, (size_t)F * hop + 16));
+  return true;
+}
+
+// MRF mean of the FFMA decoder over whole stage buffers (total4 float4 units: rows outside the utterances too).
+void vtts_engine::mrf_mean(const std::vector<float*>& xj, float* X, long total4) {
+  const int nk = (int)xj.size();
+  REQUIRE(nk <= 3, VTTS_ERR_INVALID, "more than 3 resblocks per stage not supported");
+  klaunch(mrf_mean_kernel, dim3((unsigned)((total4 + 255) / 256)), dim3(256), (size_t)(0), xj[0], nk > 1 ? xj[1] : nullptr, nk > 2 ? xj[2] : nullptr,
+          std::min(nk, 3), X, total4);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+// MRF mean of the tensor-core decoder over the utterances' rows -> planes of lrelu(mean) (the last stage: slope 0.01 and the
+// ReflectionPad1d((1,0)) row, models.py:1038-1039), and the fp32 mean into `out` when it is not null.
+void vtts_engine::mrf_mean_planes(const std::vector<float*>& xj, float* out, const Planes& nxt, int ch, bool last, int rm, const Rows& r) {
+  const int nk = (int)xj.size();
+  dim3 g((r.maxLen * rm + (last ? 1 : 0) + EW_ROWS - 1) / EW_ROWS, r.n);
+  klaunch(mrf_mean_planes_kernel, dim3(g), dim3(EW_THREADS), (size_t)(0), xj[0], nk > 1 ? xj[1] : nullptr, nk > 2 ? xj[2] : nullptr, std::min(nk, 3),
+          out, nxt.hi, nxt.lo, ch, last ? 0.01f : 0.1f, last ? 1 : 0, rm, r.lens, r.offs);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+// iSTFT + synthesis filter (istft_pqmf_kernel) over the conv_post rows `post` (utterance b: frames rm * len + 1 from row
+// offs[b] * rm + b) -> packed waveform rows (utterance b from sample offs[b] * hop).
+void vtts_engine::istft_tail(const float* post, int rm, const Rows& r, float* wav) {
+  const vtts_config& c = cfg;
+  const int pc = c.subbands * (c.istft_n_fft + 2);
   const int M = r.maxLen * rm * c.istft_hop;
   dim3 g((M + TL_M - 1) / TL_M, r.n);
   const size_t smem = ((size_t)tl_rec_frames(63, c.subbands, c.istft_n_fft, c.istft_hop) * pc + (size_t)c.subbands * (TL_M + 2 * tl_halo(63, c.subbands))) * sizeof(float);
@@ -1892,7 +1920,6 @@ bool vtts_engine::decoder_tc(float* z, bool pz_ready, const Rows& r) {
   klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, r.lens, r.offs, wav, 0, 1, istft_w2);
   CK(cudaGetLastError());
   ++launches;
-  return true;
 }
 
 void vtts_engine::launch_conv(const std::vector<ConvP>& ps, int rmul, const Rows& r) {
@@ -2581,14 +2608,7 @@ void vtts_engine::decode(float* z, const Rows& r, bool planes_ready, bool pz_rea
         for (int j = 0; j < nk; ++j) std::swap(xj[j], tmp[j]);   // ResBlock2 ping-pong (halo reads forbid in-place)
       }
     }
-    {
-      REQUIRE(nk <= 3, VTTS_ERR_INVALID, "more than 3 resblocks per stage not supported");
-      const long total4 = (long)(rows * ch / 4);
-      klaunch(mrf_mean_kernel, dim3((unsigned)((total4 + 255) / 256)), dim3(256), (size_t)(0), xj[0], nk > 1 ? xj[1] : nullptr, nk > 2 ? xj[2] : nullptr,
-                                                                           std::min(nk, 3), X, total4);
-      CK(cudaGetLastError());
-      ++launches;
-    }
+    mrf_mean(xj, X, (long)(rows * ch / 4));
     cur = X;
   }
   float* wav = ensure(d_wav, F * hop + 16);
@@ -2599,13 +2619,7 @@ void vtts_engine::decode(float* z, const Rows& r, bool planes_ready, bool pz_rea
     p.pro = PRO_LRELU; p.slope = 0.01f;
     p.reflect = 1; p.in_extra = 1; p.out_seq_extra = 1;
     launch_conv({p}, rm, r);
-    const int M = r.maxLen * rm * c.istft_hop;
-    dim3 g((M + TL_M - 1) / TL_M, r.n);
-    const size_t smem = ((size_t)tl_rec_frames(63, c.subbands, c.istft_n_fft, c.istft_hop) * pc + (size_t)c.subbands * (TL_M + 2 * tl_halo(63, c.subbands))) * sizeof(float);
-    REQUIRE(c.istft_hop == 4 && c.istft_n_fft == 16, VTTS_ERR_INVALID, "iSTFT tail kernel is sized for n_fft=16, hop=4");
-    klaunch(istft_pqmf_kernel, dim3(g), dim3(TL_THREADS), (size_t)(smem), post, pc, istft_basis, pqmf, c.subbands, c.istft_n_fft, c.istft_hop, 63, rm, r.lens, r.offs, wav, 0, 1, istft_w2);
-    CK(cudaGetLastError());
-    ++launches;
+    istft_tail(post, rm, r, wav);
   } else {
     ConvP p = mk(dec_post, cur, ch, 0, wav, 1, 0, 1, 3);
     p.pro = PRO_LRELU; p.slope = 0.01f;
@@ -2866,6 +2880,8 @@ void vtts_engine::bind_quickvc() {
   REQUIRE(c.filter_length > 0 && c.hop_length > 0 && c.filter_length % ST_TN == 0 && c.filter_length > c.hop_length &&
               (c.filter_length - c.hop_length) % 2 == 0 && c.win_length == c.filter_length,
           VTTS_ERR_INVALID, "bad spectrogram configuration (filter_length must be a multiple of 64, above hop_length, == win_length)");
+  REQUIRE(mel_smem_bytes(c.filter_length) <= (size_t)MEL_SMEM_MAX, VTTS_ERR_INVALID,
+          "filter_length too large for the mel projection (its spectrum rows must fit in shared memory)");
   spec_pad = c.n_mel_channels;
   vc_pad = (c.filter_length - c.hop_length) / 2;
   for (int l = 0; l < 3; ++l) {
@@ -4290,8 +4306,10 @@ static std::vector<int> clip_frames(vtts_handle h, bool from_spec, const int64_t
       frames[b] = (int)L;
     } else {
       REQUIRE(L <= ld, VTTS_ERR_INVALID, "wav_lengths must not exceed wav_ld");
-      REQUIRE(L > h->vc_pad, VTTS_ERR_INVALID, "clip too short: the reflect padding of the spectrogram needs more than " +
-              std::to_string(h->vc_pad) + " samples");
+      // the reflect padding needs L > pad, and one frame needs L + 2 * pad >= filter_length, i.e. L >= hop_length
+      const int64_t min_len = std::max<int64_t>(h->vc_pad + 1, c.hop_length);
+      REQUIRE(L >= min_len, VTTS_ERR_INVALID, "clip too short: the spectrogram needs at least " + std::to_string(min_len) +
+              " samples (more than the reflect padding of " + std::to_string(h->vc_pad) + ", and one frame)");
       REQUIRE(L < (1LL << 30), VTTS_ERR_INVALID, "clip too long");
       frames[b] = (int)((L + 2 * h->vc_pad - c.filter_length) / c.hop_length + 1);
     }
@@ -5306,6 +5324,7 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     CK(cudaFuncSetAttribute(conv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONV_SMEM_MAX));
     CK(cudaFuncSetAttribute(conv_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONV_SMEM_MAX));
     CK(cudaFuncSetAttribute(conv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, CONV_SMEM_MAX));
+    CK(cudaFuncSetAttribute(mel_log_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MEL_SMEM_MAX));
     CK(cudaStreamSynchronize(h->stream));
   }, G_ATOMIC, ANY_FAMILY);
 }
@@ -6315,6 +6334,113 @@ int vtts_debug_stt_durations(vtts_handle h, int B, const int* lens, size_t rows,
     if (prior) CK(cudaMemcpy(prior, dprior, frame_rows * NC * sizeof(float), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(mel, dmel, frame_rows * NC * sizeof(float), cudaMemcpyDeviceToHost));
   }, G_ATOMIC, VTTS_FAMILY_STABLETTS);
+}
+
+// ---- Unit-test hooks of the spectral kernels (include/vtts.h): the front end and the decoder tail on host tensors.
+int vtts_debug_front_end(vtts_handle h, int from_spec, const float* in, const int64_t* lengths, int B, int64_t ld, int32_t* frames,
+                         size_t rows, float* mag, float* feat) {
+  return guarded(h, [&] {
+    const vtts_config& c = h->cfg;
+    REQUIRE(h->stft_basis, VTTS_ERR_INVALID, "debug_front_end: the engine has no spectrogram front end");
+    REQUIRE(in && lengths && frames && feat, VTTS_ERR_INVALID, "debug_front_end: missing input or output");
+    const bool mel = !from_spec && c.use_mel_posterior_encoder;
+    REQUIRE(mel == (mag != nullptr), VTTS_ERR_INVALID, "debug_front_end: mag is the magnitude rows of a mel engine's waveform input "
+            "(NULL otherwise: a linear engine's magnitude rows are the features)");
+    const std::vector<int> fr = clip_frames(h, from_spec != 0, lengths, B, ld);
+    std::vector<int> off;
+    vtts_engine::pack_rows(fr, off);
+    REQUIRE(rows >= (size_t)off[B], VTTS_ERR_INVALID, "debug_front_end: fewer rows than the packed frames");
+    const size_t nbins = c.filter_length / 2 + 1, n = off[B];
+    h->B = B;
+    h->have_durations = false;
+    h->have_latent = false;
+    stage_clips(h, from_spec != 0, in, lengths, ld, fr, nullptr, nullptr, 0.f, nullptr, 0, 0);
+    if (!from_spec) {     // NaN behind every clip in the staging, so that a read outside a clip shows in its rows
+      const vtts_engine::VcPin pp = h->vc_layout(vtts_engine::IN_WAV, false);
+      for (int b = 0; b < B; ++b)
+        std::fill(pp.in + (size_t)b * h->vc_wld + lengths[b], pp.in + (size_t)(b + 1) * h->vc_wld, std::nanf(""));
+    }
+    cudaStream_t st = h->stream;
+    h->vc_upload(from_spec ? vtts_engine::IN_SPEC : vtts_engine::IN_WAV, false);
+    float* dfeat = h->ensure(h->d_vfeat, (size_t)h->Tfrm * h->spec_pad);
+    float* dmag = mel ? h->ensure(h->d_vlin, (size_t)h->Tfrm * nbins) : nullptr;
+    CK(cudaMemcpyAsync(dfeat, feat, n * h->spec_pad * sizeof(float), cudaMemcpyHostToDevice, st));
+    if (mel) CK(cudaMemcpyAsync(dmag, mag, n * nbins * sizeof(float), cudaMemcpyHostToDevice, st));
+    REQUIRE(h->front_end(from_spec != 0) == dfeat, VTTS_ERR_CUDA, "debug_front_end: the front end wrote another buffer");
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(feat, dfeat, n * h->spec_pad * sizeof(float), cudaMemcpyDeviceToHost));
+    if (mel) CK(cudaMemcpy(mag, dmag, n * nbins * sizeof(float), cudaMemcpyDeviceToHost));
+    std::copy(fr.begin(), fr.end(), frames);
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_istft(vtts_handle h, int B, const int* lens, int first, size_t rows, const float* post, size_t n_wav, float* wav) {
+  return guarded(h, [&] {
+    const vtts_config& c = h->cfg;
+    REQUIRE(h->istft_basis && h->pqmf, VTTS_ERR_INVALID, "debug_istft: the engine has no inverse-STFT decoder");
+    REQUIRE(post && wav, VTTS_ERR_INVALID, "debug_istft: missing input or output");
+    REQUIRE(first >= 0, VTTS_ERR_INVALID, "debug_istft: first must be >= 0");
+    HookRows hr = hook_rows("debug_istft", B, lens, (size_t)-1);
+    for (int& o : hr.off) {
+      REQUIRE((int64_t)o + first < (1LL << 30), VTTS_ERR_INVALID, "debug_istft: first row too large");
+      o += first;
+    }
+    const int rm = h->up_total, pc = c.subbands * (c.istft_n_fft + 2);
+    REQUIRE(rows >= (size_t)hr.off[B] * rm + B, VTTS_ERR_INVALID, "debug_istft: fewer post rows than the packed utterances' frames");
+    REQUIRE(n_wav >= (size_t)hr.off[B] * h->hop, VTTS_ERR_INVALID, "debug_istft: fewer samples than the packed utterances'");
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const float* dpost = static_cast<const float*>(upload(dev, post, rows * pc * sizeof(float), st));
+    float* dwav = static_cast<float*>(upload(dev, wav, n_wav * sizeof(float), st));
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->istft_tail(dpost, rm, r, dwav);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(wav, dwav, n_wav * sizeof(float), cudaMemcpyDeviceToHost));
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_mrf_mean(vtts_handle h, int use_tc, int B, const int* lens, int rmul, int C, int n, size_t rows, const float* x,
+                        int last, float* out, size_t plane_rows, uint16_t* hi, uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(x && (use_tc ? (hi && lo) : (out && !hi && !lo)), VTTS_ERR_INVALID,
+            "debug_mrf_mean: x and out (FFMA), or x, hi and lo (tensor cores) are required");
+    REQUIRE(n >= 1 && n <= 3 && C >= 4 && C % 4 == 0 && rmul >= 1, VTTS_ERR_INVALID,
+            "debug_mrf_mean: needs 1 to 3 inputs, C a multiple of 4 and rmul >= 1");
+    HookRows hr = hook_rows("debug_mrf_mean", B, lens, (size_t)-1);
+    REQUIRE(rows >= (size_t)hr.off[B] * rmul, VTTS_ERR_INVALID, "debug_mrf_mean: fewer rows than the packed utterances'");
+    if (use_tc) {
+      REQUIRE(plane_rows >= (size_t)hr.off[B] * rmul + (last ? B : 0), VTTS_ERR_INVALID,
+              "debug_mrf_mean: fewer plane rows than the packed utterances' (and their reflect rows)");
+      for (int b = 0; b < B; ++b)
+        REQUIRE(!last || (int64_t)lens[b] * rmul >= 2, VTTS_ERR_INVALID, "debug_mrf_mean: the reflect row needs 2 rows per utterance");
+    }
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t nx = rows * C;
+    const float* dx = static_cast<const float*>(upload(dev, x, n * nx * sizeof(float), st));
+    std::vector<float*> xj;
+    for (int j = 0; j < n; ++j) xj.push_back(const_cast<float*>(dx) + j * nx);
+    float* dout = out ? static_cast<float*>(upload(dev, out, nx * sizeof(float), st)) : nullptr;
+    Planes pl;
+    if (use_tc) {
+      pl.hi = static_cast<__nv_bfloat16*>(upload(dev, hi, plane_rows * C * 2, st));
+      pl.lo = static_cast<__nv_bfloat16*>(upload(dev, lo, plane_rows * C * 2, st));
+      const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+      h->mrf_mean_planes(xj, dout, pl, C, last != 0, rmul, r);
+    } else {
+      h->mrf_mean(xj, dout, (long)(nx / 4));
+    }
+    CK(cudaStreamSynchronize(st));
+    if (out) CK(cudaMemcpy(out, dout, nx * sizeof(float), cudaMemcpyDeviceToHost));
+    if (use_tc) {
+      CK(cudaMemcpy(hi, pl.hi, plane_rows * C * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, plane_rows * C * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 // Host-only restatement of launch_tc's split-K plan (tc_split_plan) for tests: no device, no engine.

@@ -134,6 +134,9 @@ stft_mag_kernel(const float* __restrict__ wav, long wav_ld, const int* __restric
 // One CTA = MEL_ROWS frames of one clip; the spectrum rows are staged in shared memory.
 // ------------------------------------------------------------------------------------------------
 constexpr int MEL_ROWS = 8, MEL_THREADS = 256;
+// dynamic shared memory of a launch for n_fft; the engine opts the kernel in to MEL_SMEM_MAX and refuses an n_fft above it
+constexpr int MEL_SMEM_MAX = 227 * 1024;
+constexpr size_t mel_smem_bytes(int nfft) { return (size_t)MEL_ROWS * (nfft / 2 + 1) * sizeof(float); }
 
 __global__ void __launch_bounds__(MEL_THREADS)
 mel_log_kernel(const float* __restrict__ spec, int lds, const float* __restrict__ mel, int nbins, int nmel,

@@ -65,7 +65,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
            "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
            "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode",
-           "vtts_debug_t2s_sample"]
+           "vtts_debug_t2s_sample", "vtts_debug_front_end", "vtts_debug_istft", "vtts_debug_mrf_mean"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -222,6 +222,12 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_stt_durations.argtypes = [vp, i32, vp, C.c_size_t, vp, vp, C.c_float, vp, vp, i32, vp, vp, vp, vp, C.c_size_t,
                                              vp, vp, vp, vp]
     lib.vtts_debug_stt_durations.restype = i32
+    lib.vtts_debug_front_end.argtypes = [vp, i32, vp, vp, i32, C.c_int64, vp, C.c_size_t, vp, vp]
+    lib.vtts_debug_front_end.restype = i32
+    lib.vtts_debug_istft.argtypes = [vp, i32, vp, i32, C.c_size_t, vp, C.c_size_t, vp]
+    lib.vtts_debug_istft.restype = i32
+    lib.vtts_debug_mrf_mean.argtypes = [vp, i32, i32, vp, i32, i32, i32, C.c_size_t, vp, i32, vp, C.c_size_t, vp, vp]
+    lib.vtts_debug_mrf_mean.restype = i32
     lib.vtts_debug_conv_log.argtypes = [vp, i32, C.POINTER(ConvReport), i32, C.POINTER(C.c_int)]
     lib.vtts_debug_conv_log.restype = i32
     lib.vtts_tc_split_plan.argtypes = [i32, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp]
@@ -628,12 +634,19 @@ class Engine:
 
     def convert_frames(self, wav_lengths):
         """Frames of the spectrogram of clips of `wav_lengths` samples (center=False after reflect padding by
-        (filter_length - hop_length) / 2 on both sides, mel_processing.py:67-71): len // 256 for the reference configuration."""
+        (filter_length - hop_length) / 2 on both sides, mel_processing.py:67-71): len // 256 for the reference configuration.
+        0 for a clip shorter than min_clip_samples(), which the engine refuses."""
         c = self.cfg
         n_fft, hop = int(c.get("filter_length", 1024)), int(c.get("hop_length", 256))
         pad = (n_fft - hop) // 2
         L = np.asarray(wav_lengths, np.int64)
-        return np.maximum((L + 2 * pad - n_fft) // hop + 1, 0)
+        return np.where(L >= self.min_clip_samples(), (L + 2 * pad - n_fft) // hop + 1, 0)
+
+    def min_clip_samples(self):
+        """The shortest clip the spectrogram front end takes: more samples than the reflect padding (filter_length -
+        hop_length) / 2, and at least one frame (hop_length samples)."""
+        n_fft, hop = int(self.cfg.get("filter_length", 1024)), int(self.cfg.get("hop_length", 256))
+        return max((n_fft - hop) // 2 + 1, hop)
 
     def convert(self, wav, sid_src, sid_tgt, lengths=None, noise_scale=1.0, noise=None, seed=0):
         """Re-voices clips of speaker `sid_src` as speaker `sid_tgt` (vtts_convert).  wav: float32 [B, L] (or [L]) in [-1, 1],
@@ -1241,6 +1254,49 @@ class Engine:
         lens = np.ascontiguousarray(lens, dtype=np.int32)
         self._check(self.lib.vtts_debug_spline(self.h, lens.size, _ptr(lens), x1.shape[0], _ptr(params), params.shape[1], _ptr(x1)))
         return x1
+
+    def debug_front_end(self, x, lengths, feat, mag=None, from_spec=False):
+        """The spectrogram front end of conversion, alignment and the speaker encoder (vtts_debug_front_end) on waveforms x
+        float32 [B, ld] (or caller features [B, spec_channels, ld] with from_spec).  feat float32 [rows, spec_pad] and, for a
+        mel engine's waveform input, mag float32 [rows, filter_length // 2 + 1]: initial contents that rows outside the clips
+        keep.  Returns (frames int32 [B], mag, feat), rows packed from the frame counts."""
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        lengths = np.ascontiguousarray(lengths, dtype=np.int64)
+        feat = np.ascontiguousarray(feat, dtype=np.float32).copy()
+        if feat.ndim != 2:
+            raise ValueError("feat: shape %s, expected (rows, spec_pad)" % (feat.shape,))
+        mag, = self._hook_arrays([("mag", mag, np.float32, (feat.shape[0], None))])
+        frames = np.zeros(lengths.size, np.int32)
+        self._check(self.lib.vtts_debug_front_end(self.h, int(bool(from_spec)), _ptr(x), _ptr(lengths), lengths.size, x.shape[-1],
+                                                  _ptr(frames), feat.shape[0], _ptr(mag), _ptr(feat)))
+        return frames, mag, feat
+
+    def debug_istft(self, lens, post, wav, first=0):
+        """The decoder tail istft_pqmf_kernel (vtts_debug_istft) on conv_post rows post float32 [rows, subbands * (n_fft + 2)]
+        of utterances of lens frames packed from row `first`.  wav float32 [n]: initial contents that samples outside the
+        utterances keep.  Returns the new wav."""
+        post = np.ascontiguousarray(post, dtype=np.float32)
+        if post.ndim != 2:
+            raise ValueError("post: shape %s, expected (rows, channels)" % (post.shape,))
+        wav, = self._hook_arrays([("wav", wav, np.float32, (None,))])
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        self._check(self.lib.vtts_debug_istft(self.h, lens.size, _ptr(lens), int(first), post.shape[0], _ptr(post), wav.size, _ptr(wav)))
+        return wav
+
+    def debug_mrf_mean(self, lens, rmul, x, out=None, hi=None, lo=None, use_tc=False, last=False):
+        """The MRF mean (vtts_debug_mrf_mean) of x float32 [n, rows, C]: mrf_mean_kernel into out float32 [rows, C], or with
+        use_tc mrf_mean_planes_kernel into the planes hi / lo uint16 [plane_rows, C] (and out, if given).  Initial contents
+        are kept where the kernel does not write.  Returns (out, hi, lo)."""
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        if x.ndim != 3:
+            raise ValueError("x: shape %s, expected (n, rows, C)" % (x.shape,))
+        n, rows, Cc = x.shape
+        out, hi, lo = self._hook_arrays([("out", out, np.float32, (rows, Cc)), ("hi", hi, np.uint16, (None, Cc)),
+                                         ("lo", lo, np.uint16, (None, Cc))])
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        self._check(self.lib.vtts_debug_mrf_mean(self.h, int(bool(use_tc)), lens.size, _ptr(lens), int(rmul), Cc, n, rows, _ptr(x),
+                                                 int(bool(last)), _ptr(out), 0 if hi is None else hi.shape[0], _ptr(hi), _ptr(lo)))
+        return out, hi, lo
 
     def debug_t2s_sample(self, logits, state, y, top_k=20, top_p=0.6, temperature=0.6, repetition_penalty=1.35, early_stop_num=-1,
                          step_cap=1500, seeds=None, q=None, raw=None):
