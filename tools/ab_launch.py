@@ -1,7 +1,9 @@
 """A/B of the launch shapes of two builds of libvtts.so: every entry point of every model family (seeded synthetic weights), at
-B = 1 and on a ragged batch, in precision modes 0, 1 and 2, graphs off.  One process per library (VTTS_LIB) prints, per call,
-the conv-launch log, the profiler's FLOPs and launch counts and a SHA-256 of every output; the two transcripts must be equal
-line for line.  usage: python tools/ab_launch.py libA.so libB.so [out_dir]"""
+B = 1 and on a ragged batch, in precision modes 0, 1 and 2.  One process per library (VTTS_LIB) prints, per call, the
+conv-launch log, the launch counts and a SHA-256 of every output; the two transcripts must be equal line for line.  Two
+passes: graphs off with the profiler on (its FLOPs too), then graphs on with the profiler off (which bypasses graphs), each
+call made twice so that the second replays the graph the first captured.
+usage: python tools/ab_launch.py libA.so libB.so [out_dir]"""
 import difflib
 import os
 import subprocess
@@ -18,8 +20,11 @@ import numpy as np
 from vosk_tts_b200 import config as C, synthetic, weights
 from vosk_tts_b200.engine import Engine
 from vosk_tts_b200.stabletts import StableTTS
-import contentvec_inputs as CI, hifigan_inputs as HI, quickvc_convert_inputs as QC, quickvc_inputs as QI
-import stabletts_cfm_inputs as SI, stabletts_inputs as TI
+import bert_inputs as BI, contentvec_inputs as CI, hifigan_inputs as HI, quickvc_convert_inputs as QC, quickvc_inputs as QI
+import stabletts_cfm_inputs as SI, stabletts_inputs as TI, t2s_inputs as T2
+from vosk_tts_b200.gpt_sovits import Text2Semantic
+
+GRAPHED = False                            # the pass: graphs off and the profiler on, or graphs on and the profiler off
 
 
 def digest(x):
@@ -35,16 +40,18 @@ def digest(x):
 
 def run(eng, name, fn):
     eng.conv_log(1)
-    eng.profile(True)
+    eng.profile(not GRAPHED)
     try:
-        out = digest(fn())
+        out = digest([fn(), fn()] if GRAPHED else fn())
     except Exception as e:                 # (a refusal is part of the transcript too)
         out = "error: %s" % e
     log = eng.conv_log(2)
     eng.conv_log(0)
-    p = eng.profile_read()
-    print(json.dumps({"call": name, "out": out, "conv_launches": p["conv_launches"], "conv_flops": p["conv_flops"],
-                      "tc_launches": p["tc_launches"], "tc_flops": p["tc_flops"], "kernel_launches": eng.kernel_launches()}))
+    rec = {"call": name, "out": out, "kernel_launches": eng.kernel_launches()}
+    if not GRAPHED:
+        p = eng.profile_read()
+        rec.update(conv_launches=p["conv_launches"], conv_flops=p["conv_flops"], tc_launches=p["tc_launches"], tc_flops=p["tc_flops"])
+    print(json.dumps(rec))
     for r in log:
         print("  " + json.dumps(r, sort_keys=True))
     sys.stdout.flush()
@@ -52,7 +59,7 @@ def run(eng, name, fn):
 
 def engine(cfg, blob, man, p):
     e = Engine(cfg, blob, man, device=0, precision=p)
-    e.set_graphs(False)
+    e.set_graphs(GRAPHED)
     return e
 
 
@@ -82,6 +89,9 @@ def vits2(p, batch, tag):
     run(e, tag + " flow+decode_chunk", lambda: list(e.synthesize_stream(ids[:1, :T[0]], 1, sc, chunk_frames=40, seed=3)))
     run(e, tag + " convert", lambda: e.convert(wav(batch), sid, sid[::-1], lengths=wl(batch), seed=4))
     run(e, tag + " align", lambda: e.align(ids, T, sid, wav(batch), wl(batch), seed=5))
+    clips = [c[:n] for c, n in zip(wav(batch), wl(batch))]
+    for fr, to in ((16000, 22050), (22050, 22050)):
+        run(e, tag + " resample %d->%d" % (fr, to), lambda: e.resample(clips, fr, to, trim_top_db=20, return_bounds=True))
     e.close()
 
 
@@ -107,7 +117,7 @@ def stabletts(p, batch, tag):
     e.close()
     tts = StableTTS({"n_vocab": tcfg["n_vocab"]}, TI.model(tcfg), device=0, precision=p, vocoder=HI.checkpoint())
     e = tts.engine
-    e.set_graphs(False)
+    e.set_graphs(GRAPHED)
     r = np.random.RandomState(9)
     L = [7 * k + 4 for k in batch]
     xs = [r.randint(0, tcfg["n_vocab"], (tcfg["n_streams"], t)) for t in L]
@@ -119,6 +129,39 @@ def stabletts(p, batch, tag):
     tts.close()
 
 
+def multistream(p, batch, tag):
+    bt = BI.tiny()
+    mc = {"n_vocab": 120, "bert_dim": bt["cv_hidden"]}
+    tts = StableTTS(mc, synthetic.make_random_stabletts(C.stabletts_config(mc), 8642), device=0, precision=p, vocoder=HI.checkpoint(),
+                    bert=(BI.model(bt), bt))
+    e = tts.engine
+    e.set_graphs(GRAPHED)
+    r = np.random.default_rng(10)
+    sents = [BI.sentence(bt, 5 * k + 3, salt=k) for k in batch]
+    run(e, tag + " bert_features", lambda: tts.bert_features(sents))
+    T = [6 * k + 2 for k in batch]
+    ids = [r.integers(0, 120, (5, t)).astype(np.int64) for t in T]
+    rows = [np.sort(r.integers(0, len(s), t)).astype(np.int32) for s, t in zip(sents, T)]
+    pause = [np.where(r.random(t) < 0.1, 3.0, 0.0).astype(np.float32) for t in T]
+    run(e, tag + " stabletts_synthesise pieces", lambda: tts.synthesise(ids, None, [b % 2 for b in range(len(T))], pause, n_timesteps=3,
+                                                                        seed=11, return_wav=True, pieces=sents, bert_rows=rows))
+    tts.close()
+
+
+def t2s(p, batch, tag):
+    sd, c = T2.model(T2.SMALL)
+    m = Text2Semantic((sd, c), precision=p)
+    e = m.engine
+    e.set_graphs(GRAPHED)
+    phs = [T2.phones(c, 6 * k + 4, 20 + b) for b, k in enumerate(batch)]
+    prs = [T2.prompt(c, 3 * k, 30 + b) for b, k in enumerate(batch)]
+    berts = [np.random.default_rng(40 + b).standard_normal((len(x), 1024)).astype(np.float32) * 0.3 for b, x in enumerate(phs)]
+    run(e, tag + " t2s_decode", lambda: e.t2s_decode(phs, prs, berts, step_cap=40, seeds=12))
+    q = np.stack([T2.q_draws(c, 40, 50 + b) for b in range(len(batch))])
+    run(e, tag + " t2s_decode q", lambda: e.t2s_decode(phs, None, None, step_cap=40, q=q, logits_steps=8))
+    m.close()
+
+
 def wl(batch):
     return [4000 * k + 1234 for k in batch]
 
@@ -127,14 +170,16 @@ def wav(batch):
     return (np.random.RandomState(len(batch)).rand(len(batch), max(wl(batch))).astype(np.float32) - 0.5) * 0.4
 
 
-for p in (0, 1, 2):
-    for batch in ((1,), (3, 1, 2)):
-        for fam in (vits2, quickvc, stabletts):
-            tag = "p%d B%d" % (p, len(batch))
-            try:
-                fam(p, batch, tag)
-            except Exception as ex:            # an engine the family refuses in this mode
-                print(json.dumps({"family": fam.__name__, "tag": tag, "error": str(ex)}))
+for GRAPHED in (False, True):
+    print(json.dumps({"pass": "graphs on, profiler off" if GRAPHED else "graphs off, profiler on"}))
+    for p in (0, 1, 2):
+        for batch in ((1,), (3, 1, 2)):
+            for fam in (vits2, quickvc, stabletts, multistream, t2s):
+                tag = "p%d B%d" % (p, len(batch))
+                try:
+                    fam(p, batch, tag)
+                except Exception as ex:            # an engine the family refuses in this mode
+                    print(json.dumps({"family": fam.__name__, "tag": tag, "error": str(ex)}))
 '''
 
 

@@ -414,7 +414,7 @@ struct vtts_engine {
   Buf<unsigned long long> d_tl;                  // vtts_timeline's counter and (source line, ns) pairs
   Buf<float> d_zp_dbg;                           // copy of z_p kept when debug_flags & 1
   int debug_flags = 0;
-  PinnedBuf<char> h_pin, h_pin_in, h_pin_len, h_pin_z;  // pinned staging (host): outputs, phase-1 inputs, lengths, noise_z
+  PinnedBuf<char> h_pin, h_pin_len;              // pinned readback (host): outputs; phase-1 lengths and T2S stop counts
   Buf<float> d_prm;                              // per-call scalars (see kernels.cuh prm_seed)
   MappedBuf<int> map;                            // mapped pinned host memory: [0] sequence flag, lengths, offsets
   int call_seq = 0;
@@ -457,6 +457,52 @@ struct vtts_engine {
     return b.p;
   }
   char* ensure_pinned(size_t n) { return ensure(h_pin, n); }
+
+  // Pinned staging of one kind of call input: a pinned block and the ordered fields the call copies from it, each to one
+  // engine buffer.  A call lists its fields (begin, add), sizes the block and the destinations once (commit), fills the
+  // fields on the host (host: a field is named by the buffer it is copied to), and enqueues the copies where its enqueue
+  // runs them (upload), one cudaMemcpyAsync per field in field order, to the destination as it is at that moment.
+  // A replayed graph copies from the pinned addresses it captured, so the layout of a call must follow from its graph key
+  // alone.  It does by construction: each field starts at the first 64-byte boundary behind the one before, so the layout is
+  // a function of the field sizes, and those are the sizes of the copies the graph holds.
+  struct Staging {
+    struct Field { void* dst; size_t off, n, bytes; void* (*ensure)(vtts_engine&, void* dst, size_t n); };
+    vtts_engine* e = nullptr;
+    PinnedBuf<char> pin;
+    std::vector<Field> fields;
+    size_t end() const { return fields.empty() ? 0 : fields.back().off + fields.back().bytes; }
+    void begin() { fields.clear(); }
+    template <typename T>
+    void add(Buf<T>& dst, size_t n) {
+      fields.push_back({&dst, (end() + 63) / 64 * 64, n, n * sizeof(T),
+                        [](vtts_engine& h, void* b, size_t k) -> void* { return h.ensure(*static_cast<Buf<T>*>(b), k); }});
+    }
+    void commit() {
+      e->ensure(pin, end());
+      for (const Field& f : fields) f.ensure(*e, f.dst, f.n);
+    }
+    template <typename T>
+    T* host(const Buf<T>& dst) {
+      for (const Field& f : fields)
+        if (f.dst == &dst) return reinterpret_cast<T*>(pin.p + f.off);
+      throw Err{VTTS_ERR_STATE, "a staged input was filled that the call does not copy"};
+    }
+    void upload() {
+      for (const Field& f : fields)
+        CK(cudaMemcpyAsync(f.ensure(*e, f.dst, f.n), pin.p + f.off, f.bytes, cudaMemcpyHostToDevice, e->stream));
+    }
+  };
+  // One staging per input kind; inputs that one call holds at the same time are in different kinds.
+  enum StagingKind {
+    STG_TOKENS,       // token lengths, offsets and ids, and phase 1's scalars, speaker ids and noise (TTS phase 1, alignment)
+    STG_NOISE_Z,      // phase 2's noise_z
+    STG_CLIPS,        // calls on recordings (conversion, alignment, speaker embedding, QuickVC conversion)
+    STG_CONTENTVEC, STG_BERT, STG_ST_TEXT, STG_ST_PIECES, STG_ST_MEL, STG_VOCODER, STG_RESAMPLE, STG_T2S,
+    STG_SPK_SLICES,   // the speaker encoder's slice table
+    STG_CHUNK,        // the rows of vtts_decode_chunk
+    STG_KINDS
+  };
+  Staging stg[STG_KINDS];                        // (vtts_create points each at its engine)
 
   // Runs `enqueue` (which only enqueues work on `stream`) eagerly the first time a shape key is seen -- that run also
   // performs every workspace growth -- and right behind it records the same work into a CUDA graph (capture only, no second
@@ -660,10 +706,8 @@ struct vtts_engine {
                  const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
   void dds_layer(const DdsW& d, int C, int k, int dil, const float* x, float* y, const Rows& r,
                  const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
-  struct P1Pin { int *len, *off, *sid, *ids; float *prm, *eps; };
-  P1Pin p1_layout(bool eps);
-  P1Pin stage_tokens(const int64_t* ids, int t_max, bool eps);
-  void stage1(const P1Pin& pp, int t_max, const float* noise_dp_host);
+  void stage_tokens(const int64_t* ids, int t_max, bool phase1, bool eps);
+  void stage1(int t_max, const float* noise_dp_host);
   void finish1();
   Planes enc_px;                               // the text encoder's output planes (precision modes 2 / 3), read by prior_stats
   void text_encoder(const float* cond, int cond_ld);
@@ -685,8 +729,11 @@ struct vtts_engine {
         memcpy(pin + ((size_t)b * I + ch) * maxFrm, noise + ((size_t)b * I + ch) * ld, (size_t)cols[b] * sizeof(float));
   }
   void stage_noise_z(const float* noise_z, int z_ld) {
-    float* pin = reinterpret_cast<float*>(ensure(h_pin_z, (size_t)B * cfg.inter_channels * maxFrm * sizeof(float)));
-    stage_noise(pin, noise_z, z_ld, std::vector<int>(B, std::min(z_ld, maxFrm)));
+    Staging& s = stg[STG_NOISE_Z];
+    s.begin();
+    s.add(d_eps_z, (size_t)B * cfg.inter_channels * maxFrm);
+    s.commit();
+    stage_noise(s.host(d_eps_z), noise_z, z_ld, std::vector<int>(B, std::min(z_ld, maxFrm)));
   }
   void decode(float* z, const Rows& r, bool planes_ready = false, bool pz_ready = false);
   // The decoder's element-wise launches, shared by both decoders and the unit-test hooks (vtts_debug_mrf_mean / _istft)
@@ -719,14 +766,11 @@ struct vtts_engine {
   int q_R = 0, spec_pad = 0, vc_pad = 0, vc_wld = 0;
   Buf<int> d_vint;                                 // [clip_len B][sid 2B]
   Buf<float> d_vprm, d_vin, d_vlin, d_vfeat, d_vstats, d_vcsrc, d_vnoise, d_vz_dbg, d_vzp_dbg, d_qg;
-  PinnedBuf<char> h_pin_vc;
   // what a call on recordings stages as its input: waveforms, spectrogram (or log-mel) rows, QuickVC's content-unit rows, or
   // nothing (ContentVec writes the unit rows on the device); the last two also stage QuickVC's target voice g
   enum ClipIn { IN_WAV, IN_SPEC, IN_UNITS, IN_NONE };
-  struct VcPin { int *frm_len, *frm_off, *clip_len, *sid; float *prm, *in, *g, *eps; };
-  size_t vc_in_floats(ClipIn in) const;
-  VcPin vc_layout(ClipIn in, bool eps);
-  float* vc_upload(ClipIn in, bool eps);
+  void stage_clip_fields(ClipIn in, bool eps);
+  float* vc_upload(bool eps);
   float* cond_src(bool tgt);
   float* front_end(bool from_spec);
   void posterior_encode(const float* feat, int feat_ld, const float* noise, const float* qcond, int qld, const Rows& r);
@@ -762,7 +806,6 @@ struct vtts_engine {
   struct CvPlan { int maxS = 0, tot0 = 0, MC = 0, nint = 0; std::vector<int> maxL; std::vector<int> h; } cvp;
   Buf<int> d_cvi;
   Buf<float> d_cvzero, d_cvwav, d_cvps, d_cvpq, d_cvl[2], d_cvx, d_cvx1, d_cvy, d_cvqkv, d_cvao, d_cvff, d_cvu, d_cvdbg;
-  PinnedBuf<char> h_pin_cv;
   void bind_contentvec();
   std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
   void cv_enqueue(float* out, const int* out_offs);
@@ -788,7 +831,6 @@ struct vtts_engine {
   struct BtPlan { int maxL = 0, tot = 0; std::vector<int> len, off; } btp;
   Buf<int> d_bti;                                  // [len B][off B][ids tot]
   Buf<float> d_btzero, d_btx, d_btx1, d_bty, d_btqkv, d_btao, d_btff, d_btout;
-  PinnedBuf<char> h_pin_bt;
   void bind_bert();
   void bt_stage(const int64_t* ids, const int64_t* lengths, int64_t ld);
   void bt_enqueue(float* out);
@@ -809,7 +851,6 @@ struct vtts_engine {
   Buf<unsigned> d_t2s_seen;
   Buf<T2sPrm> d_t2s_prm;
   Buf<unsigned long long> d_t2s_seed;
-  PinnedBuf<char> h_pin_t2s;
   void bind_t2s();
 
   // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh): fp32 FFMA in modes 0, 1 and 3; in
@@ -851,9 +892,6 @@ struct vtts_engine {
   Buf<int> d_sti;                                  // [len NS][off NS][sid NS][extent NS]
   Buf<float> d_stf, d_stmu, d_stnoise, d_stfilm, d_stada, d_strope, d_stxc, d_stp0, d_stp1, d_stcat[4], d_stx, d_stx2, d_sth, d_stn,
       d_stqkv, d_stao, d_sty, d_stff, d_stv, d_stmel, d_stzero, d_stdbg_n, d_stdbg_qkv;
-  PinnedBuf<char> h_pin_st;
-  struct StPin { int* ints; float *prm, *spk, *mu, *noise; };
-  StPin st_layout();
   void bind_stabletts();
   void st_enqueue();
   // One DiTConVBlock over a ragged batch (diffusion_transformer.py:98-116), shared by the decoder's blocks and the text
@@ -877,14 +915,11 @@ struct vtts_engine {
   const float *st_tok_emb = nullptr, *st_punc_emb = nullptr, *st_bert_w = nullptr, *st_bert_b = nullptr;
   Buf<int> d_stti, d_sttd;                         // [tok len B][tok off B][sid B][ids streams x Ttok]; [dur Ttok][first Ttok][frames B]
   Buf<float> d_sttf, d_stbert, d_sttx, d_stte[2], d_sttada, d_sttrope, d_stmumel, d_stmudp, d_stlogw, d_stpau;
-  PinnedBuf<char> h_pin_stt, h_pin_sttd;
-  struct SttPin { int* ints; float *prm, *pause, *bert; };
-  SttPin stt_layout();
-  void stt_enqueue(bool prior, bool bert_on_device = false);
+  PinnedBuf<char> h_pin_sttd;                      // readback of d_sttd
+  void stt_enqueue(bool prior);
   // vtts_stabletts_synthesise_pieces_wav: BERT of the staged sentences (bt_stage), then each token's row gathered into d_stbert.
-  // h_pin_stg stages the token rows' lengths and offsets and each one's source, BERT's packed row btp.off[b] + bert_rows[b][t].
+  // d_stg holds the token rows' lengths and offsets and each one's source, BERT's packed row btp.off[b] + bert_rows[b][t].
   Buf<int> d_stg;
-  PinnedBuf<char> h_pin_stg;
   void stt_bert_enqueue();
 
   // ---- StableTTS vocoder (the HiFi-GAN Generator of matcha/hifigan/models.py; hifigan.cuh), bound into the decoder members
@@ -894,7 +929,6 @@ struct vtts_engine {
   int voc_nt = 0;
   Buf<int> d_hgi;                                  // [len B][off B] of vtts_hifigan_vocode
   Buf<float> d_hgmel;                              // the denormalised mel rows the vocoder reads [Tfrm][st_noise]
-  PinnedBuf<char> h_pin_hg;
   void voc_enqueue(const float* mel, const int* fl, const int* fo);
 
   // ---- resampling of recordings (vtts_resample; resample.cuh): the taps of each rate pair, uploaded on first use
@@ -903,7 +937,7 @@ struct vtts_engine {
   Buf<int> d_rsi;                                  // [in_off B][in_len B][out_off B][out_len B][e_off B]
   Buf<float> d_rsin, d_rsout;
   Buf<double> d_rse;                               // frame energies of the trim
-  PinnedBuf<char> h_pin_rs, h_pin_rse;
+  PinnedBuf<char> h_pin_rse;                       // readback of d_rse
   const RsTaps& resample_taps(int up, int down);
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
@@ -2086,7 +2120,7 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   const int H = c.hidden_channels, D = c.dp_filter_channels;
   const size_t T = (size_t)Ttok;
   if (!capturing) CK(cudaEventRecord(ev[0], stream));
-  // ---- inputs (host data was staged into h_pin_in by stage_tokens() and stage1(); only device work is enqueued here;
+  // ---- inputs (host data was staged by stage_tokens() and stage1(); only device work is enqueued here;
   //      d_ids64 null: the ids and speaker ids were staged by the host too)
   int* tl = ensure(d_tok_len, B);
   int* to = ensure(d_tok_off, B + 1);
@@ -2094,28 +2128,16 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   int* sid = ensure(d_sid, B);
   float* prm = ensure(d_prm, 8);
   const Rows r = tok_rows();
-  {
-    P1Pin pp = p1_layout(noise_dp && !noise_on_device);
-    CK(cudaMemcpyAsync(tl, pp.len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(to, pp.off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(prm, pp.prm, 8 * sizeof(float), cudaMemcpyHostToDevice, stream));
-    if (!d_ids64) {
-      CK(cudaMemcpyAsync(ids, pp.ids, T * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CK(cudaMemcpyAsync(sid, pp.sid, B * sizeof(int), cudaMemcpyHostToDevice, stream));
-    } else {
-      dim3 g((maxTok + 127) / 128, B);
-      klaunch(pack_ids_kernel, dim3(g), dim3(128), (size_t)(0), d_ids64, t_max, ids, tl, to);
-      CK(cudaGetLastError());
-      klaunch(cast_sid_kernel, dim3((B + 127) / 128), dim3(128), (size_t)(0), d_sid64, sid, B);
-      CK(cudaGetLastError());
-      launches += 2;
-    }
-    if (noise_dp && !noise_on_device) {      // staged as [B][2][maxTok] (stage1)
-      float* de = ensure(d_eps_dp, (size_t)B * 2 * maxTok);
-      CK(cudaMemcpyAsync(de, pp.eps, (size_t)B * 2 * maxTok * sizeof(float), cudaMemcpyHostToDevice, stream));
-      noise_dp = de;
-    }
+  stg[STG_TOKENS].upload();
+  if (d_ids64) {
+    dim3 g((maxTok + 127) / 128, B);
+    klaunch(pack_ids_kernel, dim3(g), dim3(128), (size_t)(0), d_ids64, t_max, ids, tl, to);
+    CK(cudaGetLastError());
+    klaunch(cast_sid_kernel, dim3((B + 127) / 128), dim3(128), (size_t)(0), d_sid64, sid, B);
+    CK(cudaGetLastError());
+    launches += 2;
   }
+  if (noise_dp && !noise_on_device) noise_dp = d_eps_dp.p;     // staged as [B][2][maxTok] (stage1)
   if (!capturing) CK(cudaEventRecord(ev[1], stream));
 
   if (use_prefetch && n_pref > 0) {
@@ -2286,45 +2308,38 @@ void vtts_engine::prior_stats() {
   }
 }
 
-// Host side of phase 1: stage the call's inputs in pinned memory (fixed layout, so a captured graph can re-read it).
-vtts_engine::P1Pin vtts_engine::p1_layout(bool eps) {
-  const size_t T = (size_t)Ttok;
-  const size_t bytes = (size_t)(3 * B + 1) * sizeof(int) + T * sizeof(int) + 8 * sizeof(float) +
-                       (eps ? (size_t)B * 2 * maxTok * sizeof(float) : 0) + 64;
-  char* pin = ensure(h_pin_in, bytes);
-  P1Pin pp;
-  pp.len = reinterpret_cast<int*>(pin);
-  pp.off = pp.len + B;
-  pp.sid = pp.off + B + 1;
-  pp.ids = pp.sid + B;
-  pp.prm = reinterpret_cast<float*>(pp.ids + T);
-  pp.eps = pp.prm + 8;
-  return pp;
-}
-
 // Token rows of a call (TTS phase 1, alignment): lengths and offsets of the token shape and, from host ids [B][t_max], the
 // packed ids (zero between and behind the utterances), each checked against n_vocab.  ids null: packed on the device.
-// eps: room for phase 1's staged noise (stage1).
-vtts_engine::P1Pin vtts_engine::stage_tokens(const int64_t* ids, int t_max, bool eps) {
-  P1Pin pp = p1_layout(eps);
-  memcpy(pp.len, h_tok_len.data(), B * sizeof(int));
-  memcpy(pp.off, h_tok_off.data(), (B + 1) * sizeof(int));
+// phase1: room for phase 1's scalars, and speaker ids with host ids (filled by the caller); eps: for its noise (stage1).
+void vtts_engine::stage_tokens(const int64_t* ids, int t_max, bool phase1, bool eps) {
+  Staging& s = stg[STG_TOKENS];
+  s.begin();
+  s.add(d_tok_len, B);
+  s.add(d_tok_off, B + 1);
+  if (phase1) s.add(d_prm, 8);
+  if (ids) s.add(d_ids, Ttok);
+  if (ids && phase1) s.add(d_sid, B);
+  if (eps) s.add(d_eps_dp, (size_t)B * 2 * maxTok);
+  s.commit();
+  memcpy(s.host(d_tok_len), h_tok_len.data(), B * sizeof(int));
+  memcpy(s.host(d_tok_off), h_tok_off.data(), (B + 1) * sizeof(int));
   if (ids) {
-    memset(pp.ids, 0, (size_t)Ttok * sizeof(int));
+    int* pi = s.host(d_ids);
+    memset(pi, 0, (size_t)Ttok * sizeof(int));
     for (int b = 0; b < B; ++b)
       for (int t = 0; t < h_tok_len[b]; ++t) {
         const int64_t id = ids[(size_t)b * t_max + t];
         REQUIRE(id >= 0 && id < cfg.n_vocab, VTTS_ERR_INVALID, "phoneme id out of range [0, n_vocab)");
-        pp.ids[h_tok_off[b] + t] = (int)id;
+        pi[h_tok_off[b] + t] = (int)id;
       }
   }
-  return pp;
 }
 
-// The phase-1 rest of the staging (pp from stage_tokens): scales and seed, the poll sequence, the speculation's frame cap
-// and the duration predictor's noise.
-void vtts_engine::stage1(const P1Pin& pp, int t_max, const float* noise_dp_host) {
-  put_scalars(pp.prm, 8, scales, 3, seed);
+// The phase-1 rest of the staging (after stage_tokens): scales and seed, the poll sequence, the speculation's frame cap and
+// the duration predictor's noise.
+void vtts_engine::stage1(int t_max, const float* noise_dp_host) {
+  float* prm = stg[STG_TOKENS].host(d_prm);
+  put_scalars(prm, 8, scales, 3, seed);
   if (use_poll) {
     const size_t need = (size_t)(2 * B + 4);
     if (need > map.cap) {
@@ -2335,12 +2350,13 @@ void vtts_engine::stage1(const P1Pin& pp, int t_max, const float* noise_dp_host)
       ++ws_gen;
     }
     call_seq = (call_seq % 1000000) + 1;
-    memcpy(&pp.prm[6], &call_seq, 4);       // (0 without polling)
+    memcpy(&prm[6], &call_seq, 4);          // (0 without polling)
   }
-  memcpy(&pp.prm[7], &spec_cap, 4);        // frames the speculative second phase is sized for (0: none), see duration_kernel
+  memcpy(&prm[7], &spec_cap, 4);           // frames the speculative second phase is sized for (0: none), see duration_kernel
   if (noise_dp_host) {        // [B][2][t_max] -> [B][2][maxTok]: the device layout depends on the length bucket only
+    float* eps = stg[STG_TOKENS].host(d_eps_dp);
     for (int r = 0; r < 2 * B; ++r)
-      memcpy(pp.eps + (size_t)r * maxTok, noise_dp_host + (size_t)r * t_max, (size_t)std::min(t_max, maxTok) * sizeof(float));
+      memcpy(eps + (size_t)r * maxTok, noise_dp_host + (size_t)r * t_max, (size_t)std::min(t_max, maxTok) * sizeof(float));
     eps_dp_ld = maxTok;
   }
 }
@@ -2386,11 +2402,9 @@ void vtts_engine::phase2(const float* noise_z, int z_ld, bool noise_on_device, b
   const Rows r = frm_rows();
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
   if (noise_z && !noise_on_device) {
-    // host noise was staged into h_pin_z by the caller (stage_noise_z) as [B][I][maxFrm]: the layout depends on the bucket only
-    const size_t n = (size_t)B * I * maxFrm;
-    float* de = ensure(d_eps_z, n);
-    CK(cudaMemcpyAsync(de, h_pin_z.p, n * sizeof(float), cudaMemcpyHostToDevice, stream));
-    noise_z = de;
+    // host noise was staged by the caller (stage_noise_z) as [B][I][maxFrm]: the layout depends on the bucket only
+    stg[STG_NOISE_Z].upload();
+    noise_z = d_eps_z.p;
     z_ld = maxFrm;
   }
   float* z = ensure(d_z, F * I);
@@ -2633,64 +2647,30 @@ void vtts_engine::decode(float* z, const Rows& r, bool planes_ready, bool pz_rea
 // Voice conversion (models.py:1710-1718): spectrogram front end, enc_q with g_src, flow forward with g_src, flow reverse
 // with g_tgt, decoder.  The frame counts follow from the input lengths, so the whole call is ONE graphed phase.
 // ---------------------------------------------------------------------------------------------------
-// Pinned staging of a call on recordings (voice conversion, alignment, speaker embedding, QuickVC conversion): ints
-// [frm_len B][frm_off B+1][clip_len B][sid_src B][sid_tgt B], prm[16], the input (wav [B][vc_wld], spec [B][C][maxFrm],
-// unit rows [Tfrm][QV_UNITS] packed as the engine's rows, or none), g [B][gin] (QuickVC conversion only), eps [B][inter][maxFrm].
-// A captured graph copies from these fixed pinned addresses on replay, so every offset here must follow from the graph key
-// alone (batch, length buckets, input kind, noise on / off): the callers key their graphs on all of them.
-size_t vtts_engine::vc_in_floats(ClipIn in) const {
-  switch (in) {
-    case IN_WAV: return (size_t)B * vc_wld;
-    case IN_SPEC: return (size_t)B * cfg.spec_channels * maxFrm;
-    case IN_UNITS: return (size_t)Tfrm * QV_UNITS;
-    default: return 0;
-  }
-}
-
-vtts_engine::VcPin vtts_engine::vc_layout(ClipIn in, bool eps) {
+// Staged inputs of a call on recordings (voice conversion, alignment, speaker embedding, QuickVC conversion): frame lengths
+// and offsets, d_vint [clip_len B][sid_src B][sid_tgt B], the per-call scalars, the input (wav [B][vc_wld], spec
+// [B][C][maxFrm], unit rows [Tfrm][QV_UNITS] packed as the engine's rows, or none), g [B][gin] (QuickVC conversion only) and
+// the posterior eps [B][inter][maxFrm].
+void vtts_engine::stage_clip_fields(ClipIn in, bool eps) {
   const vtts_config& c = cfg;
-  const size_t nin = vc_in_floats(in), ng = in >= IN_UNITS ? (size_t)B * c.gin_channels : 0;
-  const size_t ne = eps ? (size_t)B * c.inter_channels * maxFrm : 0;
-  const size_t ints = (size_t)(5 * B + 1) * sizeof(int);
-  const size_t head = (ints + 63) / 64 * 64;
-  char* pin = ensure(h_pin_vc, head + (16 + nin + ng + ne) * sizeof(float) + 64);
-  VcPin pp;
-  pp.frm_len = reinterpret_cast<int*>(pin);
-  pp.frm_off = pp.frm_len + B;
-  pp.clip_len = pp.frm_off + B + 1;
-  pp.sid = pp.clip_len + B;
-  pp.prm = reinterpret_cast<float*>(pin + head);
-  pp.in = pp.prm + 16;
-  pp.g = pp.in + nin;
-  pp.eps = pp.g + ng;
-  return pp;
+  Staging& s = stg[STG_CLIPS];
+  s.begin();
+  s.add(d_frm_len, B);
+  s.add(d_frm_off, B + 1);
+  s.add(d_vint, 3 * B);
+  s.add(d_vprm, 16);
+  if (in == IN_WAV) s.add(d_vin, (size_t)B * vc_wld);
+  if (in == IN_SPEC) s.add(d_vin, (size_t)B * c.spec_channels * maxFrm);
+  if (in == IN_UNITS) s.add(d_vin, (size_t)Tfrm * QV_UNITS);
+  if (in >= IN_UNITS) s.add(d_qg, (size_t)B * c.gin_channels);
+  if (eps) s.add(d_vnoise, (size_t)B * c.inter_channels * maxFrm);
+  s.commit();
 }
 
-// Inputs of a call on recordings, from the pinned staging (vc_layout) to the device: frame lengths / offsets, clip lengths
-// and speaker ids (d_vint), the per-call scalars, the input (d_vin), g (d_qg), and the posterior eps (returned; null: Philox).
-float* vtts_engine::vc_upload(ClipIn in, bool eps) {
-  const int I = cfg.inter_channels;
-  VcPin pp = vc_layout(in, eps);
-  int* fl = ensure(d_frm_len, B);
-  int* fo = ensure(d_frm_off, B + 1);
-  int* vi = ensure(d_vint, 3 * B);                       // [clip_len B][sid_src B][sid_tgt B]
-  float* prm = ensure(d_vprm, 16);
-  CK(cudaMemcpyAsync(fl, pp.frm_len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(fo, pp.frm_off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(vi, pp.clip_len, 3 * B * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(prm, pp.prm, 16 * sizeof(float), cudaMemcpyHostToDevice, stream));
-  if (const size_t nin = vc_in_floats(in))
-    CK(cudaMemcpyAsync(ensure(d_vin, nin), pp.in, nin * sizeof(float), cudaMemcpyHostToDevice, stream));
-  if (in >= IN_UNITS) {
-    const size_t ng = (size_t)B * cfg.gin_channels;
-    CK(cudaMemcpyAsync(ensure(d_qg, ng), pp.g, ng * sizeof(float), cudaMemcpyHostToDevice, stream));
-  }
-  float* noise = nullptr;
-  if (eps) {
-    noise = ensure(d_vnoise, (size_t)B * I * maxFrm);
-    CK(cudaMemcpyAsync(noise, pp.eps, (size_t)B * I * maxFrm * sizeof(float), cudaMemcpyHostToDevice, stream));
-  }
-  return noise;
+// Uploads the staged inputs of a call on recordings (stage_clip_fields); returns the posterior eps (null: Philox).
+float* vtts_engine::vc_upload(bool eps) {
+  stg[STG_CLIPS].upload();
+  return eps ? d_vnoise.p : nullptr;
 }
 
 // Conditioning rows of g_src (rows [0, condR) of the stacked TTS matrix, then enc_q's q_R rows) -> d_vcsrc [B][condR + q_R];
@@ -2798,7 +2778,7 @@ void vtts_engine::posterior_side(bool from_spec, const float* noise, const float
 
 void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
-  const float* noise = vc_upload(from_spec ? IN_SPEC : IN_WAV, eps);
+  const float* noise = vc_upload(eps);
   const Rows r = frm_rows();
   // ---- g_src / g_tgt (models.py:1712-1713) and every cond row of both, one launch: src -> d_vcsrc [B][condR + q_R]
   //      (the TTS rows, then enc_q's), tgt -> d_condv [B][condR] (where the reverse flow and the decoder read them)
@@ -2824,16 +2804,10 @@ void vtts_engine::convert_enqueue(bool from_spec, bool eps) {
 void vtts_engine::align_enqueue(bool from_spec, bool eps) {
   const int I = cfg.inter_channels;
   if (!capturing) CK(cudaEventRecord(ev[0], stream));
-  const float* noise = vc_upload(from_spec ? IN_SPEC : IN_WAV, eps);
-  int* tl = ensure(d_tok_len, B);
-  int* to = ensure(d_tok_off, B + 1);
-  int* ids = ensure(d_ids, Ttok);
-  {
-    P1Pin pp = p1_layout(false);                    // (staged by the host: lengths, offsets, packed ids)
-    CK(cudaMemcpyAsync(tl, pp.len, B * sizeof(int), cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(to, pp.off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
-    CK(cudaMemcpyAsync(ids, pp.ids, (size_t)Ttok * sizeof(int), cudaMemcpyHostToDevice, stream));
-  }
+  const float* noise = vc_upload(eps);
+  stg[STG_TOKENS].upload();                         // (staged by the host: lengths, offsets, packed ids)
+  const int* tl = d_tok_len.p;
+  const int* to = d_tok_off.p;
   const int* fl = d_frm_len.p;
   const int* fo = d_frm_off.p;
   const float* csrc = has_g ? cond_src(/*tgt=*/false) : nullptr;
@@ -2849,7 +2823,7 @@ void vtts_engine::align_enqueue(bool from_spec, bool eps) {
   float* nc = ensure(d_ncent, (size_t)B * Ty * Tx);
   if (debug_flags & 1) CK(cudaMemsetAsync(nc, 0xFF, (size_t)B * Ty * Tx * sizeof(float), stream));   // NaN outside the utterances
   klaunch(neg_cent_kernel, dim3((Tx + NC_T - 1) / NC_T, (Ty + NC_T - 1) / NC_T, B), dim3(NC_THREADS), (size_t)0, (const float*)d_z.p,
-          (const float*)d_stats.p, I, fl, fo, (const int*)tl, (const int*)to, nc, Ty, Tx);
+          (const float*)d_stats.p, I, fl, fo, tl, to, nc, Ty, Tx);
   CK(cudaGetLastError());
   ++launches;
   if (debug_flags & 1) {       // [B][max t_y][max t_x] (debug runs are eager: the real shape is known here)
@@ -2861,8 +2835,8 @@ void vtts_engine::align_enqueue(bool from_spec, bool eps) {
   int* dur = ensure(d_adur, Ttok);
   int* tof = ensure(d_atof, Tfrm);
   float* score = ensure(d_ascore, B);
-  klaunch(mas_kernel, dim3(B), dim3(MAS_THREADS), (size_t)2 * Tx * sizeof(float), nc, (int*)nullptr, fl, (const int*)tl, Ty, Tx, tof, fo,
-          dur, (const int*)to, score);
+  klaunch(mas_kernel, dim3(B), dim3(MAS_THREADS), (size_t)2 * Tx * sizeof(float), nc, (int*)nullptr, fl, tl, Ty, Tx, tof, fo, dur, to,
+          score);
   CK(cudaGetLastError());
   ++launches;
   if (!capturing) CK(cudaEventRecord(ev[5], stream));
@@ -3043,11 +3017,14 @@ std::vector<int> vtts_engine::cv_stage(const float* wav, const int64_t* lengths,
     off0 += padded(L[0]);
   }
   cvp.tot0 = (B == 1 || !use_buckets) ? std::max(off0, use_buckets ? padded(cvp.maxL[0]) : 0) : (off0 + 65535) / 65536 * 65536;
-  const size_t head = ((size_t)cvp.nint * sizeof(int) + 63) / 64 * 64;
-  const size_t nsamp = (size_t)cvp.tot0 * s0 + K0;
-  char* pin = ensure(h_pin_cv, head + nsamp * sizeof(float) + 64);
-  memcpy(pin, h.data(), (size_t)(2 * NL + 1) * B * sizeof(int));
-  float* ps = reinterpret_cast<float*>(pin + head);
+  Staging& s = stg[STG_CONTENTVEC];
+  s.begin();
+  s.add(d_cvi, cvp.nint);
+  s.add(d_cvwav, (size_t)cvp.tot0 * s0 + K0);
+  s.commit();
+  int* pi = s.host(d_cvi);
+  memcpy(pi, h.data(), (size_t)(2 * NL + 1) * B * sizeof(int));
+  float* ps = s.host(d_cvwav);
   for (int b = 0; b < B; ++b) {
     const int L0 = h[b];
     const int64_t need = std::min<int64_t>(lengths[b], (int64_t)(L0 - 1) * s0 + K0);
@@ -3056,7 +3033,7 @@ std::vector<int> vtts_engine::cv_stage(const float* wav, const int64_t* lengths,
     double sum = 0.0;                                  // the clip's mean, in one fixed order (layer 0 runs centred on it)
     for (int64_t i = 0; i < lengths[b]; ++i) sum += src[i];
     const float mu = (float)(sum / (double)lengths[b]);
-    memcpy(pin + ((2 * NL + 1) * B + b) * sizeof(int), &mu, sizeof(float));
+    memcpy(pi + (2 * NL + 1) * B + b, &mu, sizeof(float));
   }
   return frames;
 }
@@ -3071,12 +3048,9 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   // Tensor-core GEMMs without split-K and attention on attn_tc_kernel (Tuning::fixed_tc): a clip's units are then the same
   // alone and in any batch.
   const Tuning tn = cv_tc ? tune.fixed_tc() : tune;
-  const size_t head = ((size_t)cvp.nint * sizeof(int) + 63) / 64 * 64;
-  const size_t nsamp = (size_t)cvp.tot0 * s0 + K0;
   int* di = ensure(d_cvi, cvp.nint);
-  float* dw = ensure(d_cvwav, nsamp);
-  CK(cudaMemcpyAsync(di, h_pin_cv.p, cvp.nint * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(dw, h_pin_cv.p + head, nsamp * sizeof(float), cudaMemcpyHostToDevice, stream));
+  float* dw = ensure(d_cvwav, (size_t)cvp.tot0 * s0 + K0);
+  stg[STG_CONTENTVEC].upload();
   auto Ls = [&](int l) -> const int* { return di + l * B; };
   auto Os = [&](int l) -> const int* { return di + (NL + l) * B; };
   const int* woff = di + 2 * NL * B;
@@ -3311,7 +3285,11 @@ void vtts_engine::bt_stage(const int64_t* ids, const int64_t* lengths, int64_t l
   }
   btp.maxL = use_buckets ? (mx + 31) / 32 * 32 : mx;
   btp.tot = !use_buckets ? tot : B == 1 ? btp.maxL : (tot + 1023) / 1024 * 1024;
-  int* pin = reinterpret_cast<int*>(ensure(h_pin_bt, ((size_t)2 * B + btp.tot) * sizeof(int) + 64));
+  Staging& s = stg[STG_BERT];
+  s.begin();
+  s.add(d_bti, 2 * (size_t)B + btp.tot);
+  s.commit();
+  int* pin = s.host(d_bti);
   memcpy(pin, btp.len.data(), B * sizeof(int));
   memcpy(pin + B, btp.off.data(), B * sizeof(int));
   std::fill(pin + 2 * B, pin + 2 * B + btp.tot, 0);
@@ -3328,7 +3306,7 @@ void vtts_engine::bt_enqueue(float* out) {
   const Tuning tn = bt_tc ? tune.fixed_tc() : tune.fixed_ffma().fixed_attention();
   const size_t T = btp.tot, nint = 2 * (size_t)B + T;
   int* di = ensure(d_bti, nint);
-  CK(cudaMemcpyAsync(di, h_pin_bt.p, nint * sizeof(int), cudaMemcpyHostToDevice, stream));
+  stg[STG_BERT].upload();
   const Rows r{di, di + B, B, btp.maxL, std::vector<int>(B, btp.maxL), btp.len, tn};
   PostLnWs w{ensure(d_btx, T * H), ensure(d_btx1, T * H), ensure(d_bty, T * H), ensure(d_btqkv, T * 3 * H), ensure(d_btao, T * H),
              ensure(d_btff, T * Fh)};
@@ -3537,25 +3515,6 @@ void vtts_engine::bind_stabletts() {
   }
 }
 
-// Pinned staging of a flow-matching call: ints [len NS][off NS][sid NS][extent NS], then floats prm[16] | t[64] | dt[64] |
-// speaker rows [B][G] (when given) | mu rows [Tfrm][MC] packed as the engine's rows (vtts_cfm_decode; text-to-mel expands them
-// on the device) | noise rows [Tfrm][NC] (when given).  Every offset follows from the graph key (batch, frame buckets,
-// guided, input kinds).
-vtts_engine::StPin vtts_engine::st_layout() {
-  const vtts_config& c = cfg;
-  const size_t head = ((size_t)4 * stp.NS * sizeof(int) + 63) / 64 * 64;
-  const size_t nspk = stp.rows ? (size_t)B * c.st_spk_dim : 0, nmu = stp.text ? 0 : (size_t)Tfrm * c.st_cond,
-               nn = stp.noise ? (size_t)Tfrm * c.st_noise : 0;
-  char* pin = ensure(h_pin_st, head + (ST_PRM + nspk + nmu + nn) * sizeof(float) + 64);
-  StPin pp;
-  pp.ints = reinterpret_cast<int*>(pin);
-  pp.prm = reinterpret_cast<float*>(pin + head);
-  pp.spk = pp.prm + ST_PRM;
-  pp.mu = pp.spk + nspk;
-  pp.noise = pp.mu + nmu;
-  return pp;
-}
-
 // modulated LayerNorm -> qkv 1x1 -> rotary -> attention (zero relative tables) -> out 1x1 -> gated residual + modulated
 // LayerNorm -> conv -> SiLU -> conv -> gated residual; x rows at xin (pitch ldi) -> xout (pitch ldo).  film: the FiLM rows
 // DitWrapper applies first (decoder.py:15-18), or null for the text encoder's plain blocks.
@@ -3683,19 +3642,12 @@ void vtts_engine::st_enqueue() {
   const vtts_config& c = cfg;
   const int NC = c.st_noise, MC = c.st_cond, H = c.st_hidden, F = c.st_filter, NL = c.st_layers, G = c.st_spk_dim;
   const int NS = stp.NS, Bu = B, XW = NC + H, dk = H / c.st_heads, rd = dk / 2, nlsc = NL / 2;
-  StPin pp = st_layout();
   const size_t T = (size_t)stp.Ttot;
   int* di = ensure(d_sti, 4 * NS);
   float* df = ensure(d_stf, ST_PRM + (size_t)Bu * G);
   float* mu = ensure(d_stmu, T * MC);
-  CK(cudaMemcpyAsync(di, pp.ints, 4 * NS * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(df, pp.prm, (ST_PRM + (stp.rows ? (size_t)Bu * G : 0)) * sizeof(float), cudaMemcpyHostToDevice, stream));
-  if (!stp.text) CK(cudaMemcpyAsync(mu, pp.mu, (size_t)Tfrm * MC * sizeof(float), cudaMemcpyHostToDevice, stream));
-  float* noise = nullptr;
-  if (stp.noise) {
-    noise = ensure(d_stnoise, (size_t)Tfrm * NC);
-    CK(cudaMemcpyAsync(noise, pp.noise, (size_t)Tfrm * NC * sizeof(float), cudaMemcpyHostToDevice, stream));
-  }
+  float* noise = stp.noise ? ensure(d_stnoise, (size_t)Tfrm * NC) : nullptr;
+  stg[STG_ST_MEL].upload();
   const int *lens = di, *offs = di + NS, *sid = di + 2 * NS, *exts = di + 3 * NS;
   const float *prm = df, *ts = df + 16, *dts = df + 16 + VTTS_CFM_MAX_STEPS;
   // The NS sequences in one fixed launch shape for every conv and one attention kernel (Tuning::fixed_ffma, fixed_attention):
@@ -3854,35 +3806,19 @@ void vtts_engine::st_enqueue() {
   }
 }
 
-// Pinned staging of the text phase: ints [tok len B][tok off B][sid B][ids streams x Ttok], then floats prm[16] | pause [Ttok]
-// | bert rows [Ttok][bert_dim], tokens packed as the engine's rows.
-vtts_engine::SttPin vtts_engine::stt_layout() {
-  const vtts_config& c = cfg;
-  const size_t ni = (size_t)3 * B + (size_t)c.st_streams * Ttok, head = (ni * sizeof(int) + 63) / 64 * 64;
-  char* pin = ensure(h_pin_stt, head + (16 + (size_t)Ttok * (1 + c.st_bert_dim)) * sizeof(float) + 64);
-  SttPin pp;
-  pp.ints = reinterpret_cast<int*>(pin);
-  pp.prm = reinterpret_cast<float*>(pin + head);
-  pp.pause = pp.prm + 16;
-  pp.bert = pp.pause + Ttok;
-  return pp;
-}
-
 // Text phase of vtts_stabletts_synthesise: uploads, the token rows x, dp_encoder and its proj, the durations and their scan;
 // with `prior` the mel encoder and its proj as well.  Leaves x, the durations, each token's first frame, the pauses and
-// mu_mel on the device for the mel phase, and copies [dur][first][frames of every utterance] to pinned memory.
-void vtts_engine::stt_enqueue(bool prior, bool bert_on_device) {
+// mu_mel on the device for the mel phase, and copies [dur][first][frames of every utterance] to pinned memory.  The BERT rows
+// are in d_stbert: uploaded with the staged inputs, or gathered there by stt_bert_enqueue.
+void vtts_engine::stt_enqueue(bool prior) {
   const vtts_config& c = cfg;
   const int MC = c.st_cond, H = c.st_enc_hidden, F = c.st_enc_filter, NE = c.st_enc_layers, G = c.st_spk_dim, S = c.st_streams;
   const int dk = H / c.st_enc_heads, rd = dk / 2, DC = c.st_dur_channels, NC = c.st_noise;
-  SttPin pp = stt_layout();
   const size_t T = (size_t)Ttok, ni = (size_t)3 * B + (size_t)S * T;
   int* di = ensure(d_stti, ni);
   float* df = ensure(d_sttf, 16 + T);
   float* bert = ensure(d_stbert, T * c.st_bert_dim);
-  CK(cudaMemcpyAsync(di, pp.ints, ni * sizeof(int), cudaMemcpyHostToDevice, stream));
-  CK(cudaMemcpyAsync(df, pp.prm, (16 + T) * sizeof(float), cudaMemcpyHostToDevice, stream));
-  if (!bert_on_device) CK(cudaMemcpyAsync(bert, pp.bert, T * c.st_bert_dim * sizeof(float), cudaMemcpyHostToDevice, stream));
+  stg[STG_ST_TEXT].upload();
   const int *lens = di, *offs = di + B, *sid = di + 2 * B, *ids = di + 3 * B;
   // the decoder's fixed launch shape, every token row sized at the bucket: durations do not depend on the batch
   const Rows r{lens, offs, B, maxTok, std::vector<int>(B, maxTok), h_tok_len, tune.fixed_ffma().fixed_attention()};
@@ -3923,8 +3859,8 @@ void vtts_engine::stt_enqueue(bool prior, bool bert_on_device) {
 }
 
 // BERT rows of the text phase from word pieces: BERT of the sentences bt_stage staged, into its packed rows d_btout, then
-// st_bert_gather_kernel copies each token's row into d_stbert, where stt_enqueue(prior, true) reads it.  h_pin_stg holds
-// [tok len B][tok off B][source row of every token row Ttok].
+// st_bert_gather_kernel copies each token's row into d_stbert, where stt_enqueue reads it.  d_stg holds [tok len B][tok off B]
+// [source row of every token row Ttok].
 void vtts_engine::stt_bert_enqueue() {
   const vtts_config& c = cfg;
   const size_t T = (size_t)Ttok, ni = 2 * (size_t)B + T;
@@ -3932,7 +3868,7 @@ void vtts_engine::stt_bert_enqueue() {
   bt_enqueue(feat);
   int* di = ensure(d_stg, ni);
   float* bert = ensure(d_stbert, T * c.st_bert_dim);
-  CK(cudaMemcpyAsync(di, h_pin_stg.p, ni * sizeof(int), cudaMemcpyHostToDevice, stream));
+  stg[STG_ST_PIECES].upload();
   klaunch(st_bert_gather_kernel, dim3(maxTok, B), dim3(128), (size_t)0, (const float*)feat, (const int*)(di + 2 * B), c.st_bert_dim, bert,
           (const int*)di, (const int*)(di + B));
   CK(cudaGetLastError());
@@ -3940,13 +3876,18 @@ void vtts_engine::stt_bert_enqueue() {
 }
 
 // Front end (or the caller's log-mel), the three LSTM layers over every slice, and the embedding.  seq: the slice table of
-// d_sseq (host copy); max_len: the longest slice.
+// d_sseq (host copy); max_len: the longest slice.  Not graphed: the slice table is staged here.
 void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int max_len) {
   const int ns = spk_nseq;
-  int* ds = ensure(d_sseq, seq.size());
-  CK(cudaMemcpyAsync(ds, seq.data(), seq.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+  Staging& s = stg[STG_SPK_SLICES];
+  s.begin();
+  s.add(d_sseq, seq.size());
+  s.commit();
+  std::copy(seq.begin(), seq.end(), s.host(d_sseq));
+  s.upload();
+  const int* ds = d_sseq.p;
   const int *xrow = ds, *slen = ds + ns, *soff = ds + 2 * ns, *last = ds + 3 * ns + 1, *of_clip = ds + 4 * ns + 1;
-  vc_upload(from_mel ? IN_SPEC : IN_WAV, false);
+  vc_upload(false);
   const float* feat = front_end(from_mel);
   // Sequences per cluster: the fewest that keep every cluster co-resident; more sequences per cluster lengthen each step,
   // more clusters than fit run in waves.
@@ -3991,7 +3932,7 @@ void vtts_engine::spk_enqueue(bool from_mel, const std::vector<int>& seq, int ma
 void vtts_engine::quickvc_enqueue(bool eps, bool from_wav) {
   const int G = cfg.gin_channels;
   if (!capturing) CK(cudaEventRecord(ev[4], stream));
-  const float* noise = vc_upload(from_wav ? IN_NONE : IN_UNITS, eps);
+  const float* noise = vc_upload(eps);
   const int* fo = d_frm_off.p;
   const Rows r = frm_rows();
   float* units = ensure(d_vin, (size_t)Tfrm * QV_UNITS);       // unit rows, packed as the engine's rows
@@ -4125,12 +4066,13 @@ static void enqueue_phase1_host(vtts_handle h, const int64_t* ids, const int64_t
   memcpy(h->scales, scales, 3 * sizeof(float));
   h->seed = seed;
   h->spec_cap = (may_speculate && spec_ok(h, B)) ? vtts_engine::bucket_frm(h->spec_predict()) : 0;
-  const vtts_engine::P1Pin pp = h->stage_tokens(ids, t_max, noise_dp != nullptr);
+  h->stage_tokens(ids, t_max, true, noise_dp != nullptr);
+  int* ps = h->stg[vtts_engine::STG_TOKENS].host(h->d_sid);
   for (int b = 0; b < B; ++b) {
     REQUIRE(!h->has_g || (sid[b] >= 0 && sid[b] < h->cfg.n_speakers), VTTS_ERR_INVALID, "speaker id out of range [0, n_speakers)");
-    pp.sid[b] = (int)sid[b];
+    ps[b] = (int)sid[b];
   }
-  h->stage1(pp, t_max, noise_dp);
+  h->stage1(t_max, noise_dp);
   h->run_graphed({vtts_engine::TAG_PHASE1, B, h->maxTok, h->Ttok, noise_dp ? 1 : 0},
                  [&] { h->phase1(nullptr, t_max, nullptr, noise_dp, false); });
 }
@@ -4174,7 +4116,8 @@ static void enqueue_phase1_dev(vtts_handle h, const int64_t* d_ids, const int64_
   memcpy(h->scales, scales, 3 * sizeof(float));
   h->seed = seed;
   h->spec_cap = (may_speculate && spec_ok(h, B)) ? vtts_engine::bucket_frm(h->spec_predict()) : 0;
-  h->stage1(h->stage_tokens(nullptr, t_max, false), t_max, nullptr);
+  h->stage_tokens(nullptr, t_max, true, false);
+  h->stage1(t_max, nullptr);
   h->eps_dp_ld = t_max;      // device noise is read in the caller's [B][2][t_max] layout
   h->run_graphed({vtts_engine::TAG_PHASE1_DEV, B, h->maxTok, h->Ttok, t_max, (long long)(uintptr_t)d_ids, (long long)(uintptr_t)d_sid,
                   (long long)(uintptr_t)d_noise_dp},
@@ -4317,7 +4260,7 @@ static std::vector<int> clip_frames(vtts_handle h, bool from_spec, const int64_t
   return frames;
 }
 
-// Sets the frame shape and stages the recordings, speaker ids (sid_tgt may be null), noise and scalars in vc_layout.
+// Sets the frame shape and stages the recordings, speaker ids (sid_tgt may be null), noise and scalars (stage_clip_fields).
 static void stage_clips(vtts_handle h, bool from_spec, const float* in, const int64_t* lengths, int64_t ld, const std::vector<int>& frames,
                         const int64_t* sid_src, const int64_t* sid_tgt, float noise_scale, const float* noise_q, int q_ld, uint64_t seed) {
   const vtts_config& c = h->cfg;
@@ -4325,22 +4268,25 @@ static void stage_clips(vtts_handle h, bool from_spec, const float* in, const in
   h->pack_frames(frames);
   h->vc_wld = (h->maxFrm + 2) * c.hop_length + c.filter_length;
   const int maxF = h->maxFrm, C = c.spec_channels;
-  const vtts_engine::VcPin pp = h->vc_layout(from_spec ? vtts_engine::IN_SPEC : vtts_engine::IN_WAV, noise_q != nullptr);
-  memcpy(pp.frm_len, frames.data(), B * sizeof(int));
-  memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
+  h->stage_clip_fields(from_spec ? vtts_engine::IN_SPEC : vtts_engine::IN_WAV, noise_q != nullptr);
+  vtts_engine::Staging& s = h->stg[vtts_engine::STG_CLIPS];
+  memcpy(s.host(h->d_frm_len), frames.data(), B * sizeof(int));
+  memcpy(s.host(h->d_frm_off), h->h_frm_off.data(), (B + 1) * sizeof(int));
+  int* vi = s.host(h->d_vint);
+  float* pin = s.host(h->d_vin);
   for (int b = 0; b < B; ++b) {
-    pp.clip_len[b] = (int)lengths[b];
-    pp.sid[b] = sid_src ? (int)sid_src[b] : 0;
-    pp.sid[B + b] = sid_tgt ? (int)sid_tgt[b] : 0;
+    vi[b] = (int)lengths[b];
+    vi[B + b] = sid_src ? (int)sid_src[b] : 0;
+    vi[2 * B + b] = sid_tgt ? (int)sid_tgt[b] : 0;
     if (from_spec) {
       for (int ch = 0; ch < C; ++ch)
-        memcpy(pp.in + ((size_t)b * C + ch) * maxF, in + ((size_t)b * C + ch) * ld, (size_t)frames[b] * sizeof(float));
+        memcpy(pin + ((size_t)b * C + ch) * maxF, in + ((size_t)b * C + ch) * ld, (size_t)frames[b] * sizeof(float));
     } else {
-      memcpy(pp.in + (size_t)b * h->vc_wld, in + (size_t)b * ld, (size_t)lengths[b] * sizeof(float));
+      memcpy(pin + (size_t)b * h->vc_wld, in + (size_t)b * ld, (size_t)lengths[b] * sizeof(float));
     }
   }
-  if (noise_q) h->stage_noise(pp.eps, noise_q, q_ld, frames);
-  vtts_engine::put_scalars(pp.prm, 16, &noise_scale, 1, seed);
+  if (noise_q) h->stage_noise(s.host(h->d_vnoise), noise_q, q_ld, frames);
+  vtts_engine::put_scalars(s.host(h->d_vprm), 16, &noise_scale, 1, seed);
 }
 
 // Voice conversion through host buffers (vtts_convert / vtts_convert_spec).
@@ -4437,7 +4383,7 @@ static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const 
   REQUIRE(!token_of_frame || tof_ld >= real_max, VTTS_ERR_CAPACITY, "tof_ld is smaller than max(frames)");
   REQUIRE(!noise_q || q_ld >= real_max, VTTS_ERR_CAPACITY, "noise_q has fewer columns than max(frames)");
   setup_lengths(h, id_lengths, B, t_max);
-  h->stage_tokens(ids, t_max, false);               // (the alignment does not advance phase 1's poll sequence)
+  h->stage_tokens(ids, t_max, false, false);        // (the alignment does not advance phase 1's poll sequence)
   stage_clips(h, from_spec, in, lengths, ld, frames, h->has_g ? sid : nullptr, nullptr, noise_scale, noise_q, q_ld, seed);
   h->run_graphed({vtts_engine::TAG_ALIGN, B, h->maxTok, h->Ttok, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
                  [&] { h->align_enqueue(from_spec, noise_q != nullptr); });
@@ -4559,10 +4505,16 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
     maxT = std::max(maxT, Lr[b]); maxKv = std::max(maxKv, kv);
   }
   h->B = B;
-  // pinned staging: [T + P B][off B][init 4B][poff B][prefill ids tot][prompts ptot], then the sampling scalars, the seeds and the stop flags
-  const size_t nint = 7 * (size_t)B + tot + ptot;
-  char* pin = h->ensure(h->h_pin_t2s, (nint * sizeof(int) + 15) / 16 * 16 + 64 + 8 * (size_t)B + 16);
-  int* pi = reinterpret_cast<int*>(pin);
+  // staged: [T + P B][off B][init 4B][poff B][prefill ids tot][prompts ptot], the sampling scalars, the seeds and the BERT rows
+  const size_t nint = 7 * (size_t)B + tot + ptot, nb = (size_t)tot * vtts_engine::T2S_BERT;
+  vtts_engine::Staging& st = h->stg[vtts_engine::STG_T2S];
+  st.begin();
+  st.add(h->d_t2s_i, nint);
+  st.add(h->d_t2s_prm, 1);
+  st.add(h->d_t2s_seed, (size_t)B);
+  if (bert) st.add(h->d_t2s_bert, nb);
+  st.commit();
+  int* pi = st.host(h->d_t2s_i);
   memcpy(pi, Lr.data(), B * sizeof(int));
   memcpy(pi + B, off.data(), B * sizeof(int));
   memcpy(pi + 2 * B, init.data(), 4 * (size_t)B * sizeof(int));
@@ -4573,18 +4525,21 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
     for (int t = 0; t < P[b]; ++t)
       pi[7 * B + off[b] + T[b] + t] = pi[7 * B + tot + poff[b] + t] = (int)prompts[(size_t)b * prompts_ld + t];
   }
-  T2sPrm prm{top_p, temperature, penalty, top_k, early_stop, step_cap, q ? (int)q_ld : 0, logits ? (int)logits_ld : 0};
-  char* pprm = pin + ((nint * sizeof(int) + 15) / 16 * 16);
-  memcpy(pprm, &prm, sizeof(prm));
-  unsigned long long* psd = reinterpret_cast<unsigned long long*>(pprm + 64);
+  *st.host(h->d_t2s_prm) = T2sPrm{top_p, temperature, penalty, top_k, early_stop, step_cap, q ? (int)q_ld : 0, logits ? (int)logits_ld : 0};
+  unsigned long long* psd = st.host(h->d_t2s_seed);
   for (int b = 0; b < B; ++b) psd[b] = seeds ? (unsigned long long)seeds[b] : 0ull;
+  if (bert) {
+    float* hb = st.host(h->d_t2s_bert);
+    std::fill(hb, hb + nb, 0.f);
+    for (int b = 0; b < B; ++b)
+      memcpy(hb + (size_t)off[b] * vtts_engine::T2S_BERT, bert + (size_t)b * ids_ld * vtts_engine::T2S_BERT,
+             (size_t)T[b] * vtts_engine::T2S_BERT * sizeof(float));
+  }
   cudaStream_t s = h->stream;
-  int* di = h->ensure(h->d_t2s_i, nint);
-  CK(cudaMemcpyAsync(di, pi, nint * sizeof(int), cudaMemcpyHostToDevice, s));
-  T2sPrm* dprm = h->ensure(h->d_t2s_prm, 1);
-  CK(cudaMemcpyAsync(dprm, pprm, sizeof(T2sPrm), cudaMemcpyHostToDevice, s));
-  unsigned long long* dseed = h->ensure(h->d_t2s_seed, (size_t)B);
-  CK(cudaMemcpyAsync(dseed, psd, (size_t)B * 8, cudaMemcpyHostToDevice, s));
+  st.upload();
+  const int* di = h->d_t2s_i.p;
+  const T2sPrm* dprm = h->d_t2s_prm.p;
+  const unsigned long long* dseed = h->d_t2s_seed.p;
   float* dq = nullptr;
   if (q) {
     dq = h->ensure(h->d_t2s_q, (size_t)B * q_ld * V);
@@ -4610,16 +4565,8 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
   float* vc = h->ensure(h->d_t2s_v, (size_t)NL * kvn * H);
   const float* bp = nullptr;
   if (bert) {
-    const size_t nb = (size_t)tot * vtts_engine::T2S_BERT;
-    float* hb = reinterpret_cast<float*>(h->ensure(h->h_pin_bt, nb * sizeof(float) + 64));
-    std::fill(hb, hb + nb, 0.f);
-    for (int b = 0; b < B; ++b)
-      memcpy(hb + (size_t)off[b] * vtts_engine::T2S_BERT, bert + (size_t)b * ids_ld * vtts_engine::T2S_BERT,
-             (size_t)T[b] * vtts_engine::T2S_BERT * sizeof(float));
-    float* db = h->ensure(h->d_t2s_bert, nb);
-    CK(cudaMemcpyAsync(db, hb, nb * sizeof(float), cudaMemcpyHostToDevice, s));
     float* dbp = h->ensure(h->d_t2s_bp, (size_t)tot * H);
-    h->launch_conv({mk(h->t2s_bp, db, vtts_engine::T2S_BERT, 0, dbp, H, 0, 1, 0)}, 1, r);
+    h->launch_conv({mk(h->t2s_bp, h->d_t2s_bert.p, vtts_engine::T2S_BERT, 0, dbp, H, 0, 1, 0)}, 1, r);
     bp = dbp;
   }
   h->klaunch(t2s_prefill_embed_kernel, dim3(maxT, B), dim3(128), (size_t)0, (const int*)(di + 7 * B), h->t2s_temb, h->t2s_aemb, bp,
@@ -4683,7 +4630,7 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
     h->launches += 5 * (uint64_t)NL + 2;
   };
   // ---- decode loop: every utterance has stopped after gen_max steps at the latest
-  int* flag = reinterpret_cast<int*>(psd + B);      // two slots, one per chunk in flight
+  int* flag = reinterpret_cast<int*>(h->ensure(h->h_pin_len, 2 * sizeof(int)));      // two slots, one per chunk in flight
   const long bound = gen_max;
   for (long it = 0, chunk = 0;; ++chunk) {
     h->run_graphed({vtts_engine::TAG_T2S, B, nsplit, kvn, ytot, q ? q_ld : -1, logits ? logits_ld : -1},
@@ -4747,23 +4694,26 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const float*
   h->pack_frames(frames);
   constexpr int U = vtts_engine::QV_UNITS;
   const int G = c.gin_channels;
-  const vtts_engine::VcPin pp = h->vc_layout(units ? vtts_engine::IN_UNITS : vtts_engine::IN_NONE, noise != nullptr);
-  memcpy(pp.frm_len, frames.data(), B * sizeof(int));
-  memcpy(pp.frm_off, h->h_frm_off.data(), (B + 1) * sizeof(int));
+  h->stage_clip_fields(units ? vtts_engine::IN_UNITS : vtts_engine::IN_NONE, noise != nullptr);
+  vtts_engine::Staging& s = h->stg[vtts_engine::STG_CLIPS];
+  memcpy(s.host(h->d_frm_len), frames.data(), B * sizeof(int));
+  memcpy(s.host(h->d_frm_off), h->h_frm_off.data(), (B + 1) * sizeof(int));
+  int* vi = s.host(h->d_vint);
+  float* pin = units ? s.host(h->d_vin) : nullptr;
   for (int b = 0; b < B; ++b) {
-    pp.clip_len[b] = frames[b];
-    pp.sid[b] = b;                                      // cond_vc_kernel's row of g
-    pp.sid[B + b] = 0;
+    vi[b] = frames[b];
+    vi[B + b] = b;                                      // cond_vc_kernel's row of g
+    vi[2 * B + b] = 0;
     const int o = h->h_frm_off[b];
     if (units) {
-      memcpy(pp.in + (size_t)o * U, units + (size_t)b * units_ld * U, (size_t)frames[b] * U * sizeof(float));
+      memcpy(pin + (size_t)o * U, units + (size_t)b * units_ld * U, (size_t)frames[b] * U * sizeof(float));
       const int gap_end = b + 1 < B ? h->h_frm_off[b + 1] : h->Tfrm;       // rows behind the clip: the gap, or the bucket's tail
-      memset(pp.in + (size_t)(o + frames[b]) * U, 0, (size_t)(gap_end - o - frames[b]) * U * sizeof(float));
+      memset(pin + (size_t)(o + frames[b]) * U, 0, (size_t)(gap_end - o - frames[b]) * U * sizeof(float));
     }
   }
-  memcpy(pp.g, g, (size_t)B * G * sizeof(float));
-  if (noise) h->stage_noise(pp.eps, noise, noise_ld, frames);
-  vtts_engine::put_scalars(pp.prm, 16, &noise_scale, 1, seed);
+  memcpy(s.host(h->d_qg), g, (size_t)B * G * sizeof(float));
+  if (noise) h->stage_noise(s.host(h->d_vnoise), noise, noise_ld, frames);
+  vtts_engine::put_scalars(s.host(h->d_vprm), 16, &noise_scale, 1, seed);
   if (wav)
     h->run_graphed({vtts_engine::TAG_QUICKVC_WAV, B, h->maxFrm, h->Tfrm, noise ? 1 : 0, h->cvp.maxS, h->cvp.tot0},
                    [&] { h->quickvc_enqueue(noise != nullptr, true); });
@@ -4796,10 +4746,12 @@ static void st_schedule(float* prm, int n) {
   }
 }
 
-// The flow-matching plan of a call and its staged table: sequence q < B is utterance q's conditional branch, B + q its
-// unconditional one; rows are packed by extent.
-static vtts_engine::StPin st_plan(vtts_handle h, int B, const std::vector<int>& frames, const std::vector<int>& extents, const int64_t* sid, int n,
-                                  float temperature, float s, bool noise, bool rows, bool text, bool prior, int denormalise, uint64_t seed) {
+// The flow-matching plan of a call and its staged inputs: d_sti [len NS][off NS][sid NS][extent NS], where sequence q < B is
+// utterance q's conditional branch and B + q its unconditional one (rows packed by extent); d_stf prm[16] | t[64] | dt[64] |
+// speaker rows [B][G] (rows); the mu rows [Tfrm][MC] packed as the engine's rows (vtts_cfm_decode; text-to-mel expands them
+// on the device); the noise rows [Tfrm][NC] (noise).  The caller fills the speaker, mu and noise rows.
+static void st_plan(vtts_handle h, int B, const std::vector<int>& frames, const std::vector<int>& extents, const int64_t* sid, int n,
+                    float temperature, float s, bool noise, bool rows, bool text, bool prior, int denormalise, uint64_t seed) {
   h->pack_frames(extents);
   vtts_engine::StPlan& P = h->stp;
   P.guided = s > 0.f;
@@ -4812,18 +4764,26 @@ static vtts_engine::StPin st_plan(vtts_handle h, int B, const std::vector<int>& 
   P.Ttot = P.guided ? 2 * h->Tfrm + SEQ_GAP : h->Tfrm;
   REQUIRE((int64_t)P.Ttot * 3 * h->cfg.st_filter < (int64_t)INT32_MAX, VTTS_ERR_INVALID, "the batch holds too many frames for one call");
   const int NS = P.NS;
-  const vtts_engine::StPin pp = h->st_layout();
+  const vtts_config& c = h->cfg;
+  vtts_engine::Staging& st = h->stg[vtts_engine::STG_ST_MEL];
+  st.begin();
+  st.add(h->d_sti, 4 * (size_t)NS);
+  st.add(h->d_stf, vtts_engine::ST_PRM + (rows ? (size_t)B * c.st_spk_dim : 0));
+  if (!text) st.add(h->d_stmu, (size_t)h->Tfrm * c.st_cond);
+  if (noise) st.add(h->d_stnoise, (size_t)h->Tfrm * c.st_noise);
+  st.commit();
+  int* pi = st.host(h->d_sti);
   for (int q = 0; q < NS; ++q) {
     const int b = q < B ? q : q - B;
-    pp.ints[q] = frames[b];
-    pp.ints[NS + q] = h->h_frm_off[b] + (q < B ? 0 : h->Tfrm + SEQ_GAP);
-    pp.ints[2 * NS + q] = q < B ? (sid ? (int)sid[b] : 0) : -1;
-    pp.ints[3 * NS + q] = extents[b];
+    pi[q] = frames[b];
+    pi[NS + q] = h->h_frm_off[b] + (q < B ? 0 : h->Tfrm + SEQ_GAP);
+    pi[2 * NS + q] = q < B ? (sid ? (int)sid[b] : 0) : -1;
+    pi[3 * NS + q] = extents[b];
   }
   const float sc[3] = {temperature, s, denormalise ? 1.f : 0.f};
-  vtts_engine::put_scalars(pp.prm, vtts_engine::ST_PRM, sc, 3, seed);
-  st_schedule(pp.prm, n);
-  return pp;
+  float* prm = st.host(h->d_stf);
+  vtts_engine::put_scalars(prm, vtts_engine::ST_PRM, sc, 3, seed);
+  st_schedule(prm, n);
 }
 
 static void st_check_sampling(int n, float temperature, float s) {
@@ -4853,14 +4813,16 @@ static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengt
   h->have_durations = false;
   h->have_latent = false;
   const int NC = c.st_noise, MC = c.st_cond, G = c.st_spk_dim;
-  const vtts_engine::StPin pp = st_plan(h, B, frames, frames, sid, n, temperature, s, noise != nullptr, spk_rows != nullptr,
-                                        false, false, denormalise, seed);
+  st_plan(h, B, frames, frames, sid, n, temperature, s, noise != nullptr, spk_rows != nullptr, false, false, denormalise, seed);
   const vtts_engine::StPlan& P = h->stp;
-  if (spk_rows) memcpy(pp.spk, spk_rows, (size_t)B * G * sizeof(float));
+  vtts_engine::Staging& st = h->stg[vtts_engine::STG_ST_MEL];
+  if (spk_rows) memcpy(st.host(h->d_stf) + vtts_engine::ST_PRM, spk_rows, (size_t)B * G * sizeof(float));
+  float* pmu = st.host(h->d_stmu);
+  float* pn = noise ? st.host(h->d_stnoise) : nullptr;
   for (int b = 0; b < B; ++b) {
     const size_t o = (size_t)h->h_frm_off[b];
-    memcpy(pp.mu + o * MC, mu + (size_t)b * mu_ld * MC, (size_t)frames[b] * MC * sizeof(float));
-    if (noise) memcpy(pp.noise + o * NC, noise + (size_t)b * noise_ld * NC, (size_t)frames[b] * NC * sizeof(float));
+    memcpy(pmu + o * MC, mu + (size_t)b * mu_ld * MC, (size_t)frames[b] * MC * sizeof(float));
+    if (noise) memcpy(pn + o * NC, noise + (size_t)b * noise_ld * NC, (size_t)frames[b] * NC * sizeof(float));
   }
   h->run_graphed({vtts_engine::TAG_CFM, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, P.rows ? 1 : 0}, [&] { h->st_enqueue(); });
   read_clips(h, (const float*)h->d_stmel.p, (size_t)h->real_Tfrm * NC, (size_t)h->Tfrm * NC, h->h_frm_off.data(), frames, NC, mel_out,
@@ -4913,24 +4875,38 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
   if (pieces) h->bt_stage(pieces, piece_lengths, pieces_ld);
   const int Ttok = h->Ttok;
   {
-    const vtts_engine::SttPin pp = h->stt_layout();
-    memset(pp.ints + 3 * B, 0, (size_t)S * Ttok * sizeof(int));
-    std::fill(pp.pause, pp.pause + Ttok, 0.f);
-    vtts_engine::put_scalars(pp.prm, 16, &length_scale, 1, seed);
+    // [tok len B][tok off B][sid B][ids streams x Ttok]; prm[16] | pause [Ttok]; the BERT rows [Ttok][bert_dim] (without
+    // pieces), tokens packed as the engine's rows
+    vtts_engine::Staging& st = h->stg[vtts_engine::STG_ST_TEXT];
+    st.begin();
+    st.add(h->d_stti, (size_t)3 * B + (size_t)S * Ttok);
+    st.add(h->d_sttf, 16 + (size_t)Ttok);
+    if (!pieces) st.add(h->d_stbert, (size_t)Ttok * BD);
+    st.commit();
+    int* pi = st.host(h->d_stti);
+    float* prm = st.host(h->d_sttf);
+    float* pp = prm + 16;
+    memset(pi + 3 * B, 0, (size_t)S * Ttok * sizeof(int));
+    std::fill(pp, pp + Ttok, 0.f);
+    vtts_engine::put_scalars(prm, 16, &length_scale, 1, seed);
     for (int b = 0; b < B; ++b) {
       const int len = h->h_tok_len[b], o = h->h_tok_off[b];
-      pp.ints[b] = len;
-      pp.ints[B + b] = o;
-      pp.ints[2 * B + b] = (int)sid[b];
+      pi[b] = len;
+      pi[B + b] = o;
+      pi[2 * B + b] = (int)sid[b];
       for (int q = 0; q < S; ++q)
-        for (int i = 0; i < len; ++i) pp.ints[3 * B + (size_t)q * Ttok + o + i] = (int)ids[((size_t)b * S + q) * t_max + i];
-      if (pause) memcpy(pp.pause + o, pause + (size_t)b * t_max, (size_t)len * sizeof(float));
-      if (bert) memcpy(pp.bert + (size_t)o * BD, bert + (size_t)b * t_max * BD, (size_t)len * BD * sizeof(float));
+        for (int i = 0; i < len; ++i) pi[3 * B + (size_t)q * Ttok + o + i] = (int)ids[((size_t)b * S + q) * t_max + i];
+      if (pause) memcpy(pp + o, pause + (size_t)b * t_max, (size_t)len * sizeof(float));
+      if (bert) memcpy(st.host(h->d_stbert) + (size_t)o * BD, bert + (size_t)b * t_max * BD, (size_t)len * BD * sizeof(float));
     }
   }
   const bool prior = prior_out != nullptr;
   if (pieces) {
-    int* g = reinterpret_cast<int*>(h->ensure(h->h_pin_stg, (2 * (size_t)B + Ttok) * sizeof(int) + 64));
+    vtts_engine::Staging& sg = h->stg[vtts_engine::STG_ST_PIECES];
+    sg.begin();
+    sg.add(h->d_stg, 2 * (size_t)B + Ttok);
+    sg.commit();
+    int* g = sg.host(h->d_stg);
     memcpy(g, h->h_tok_len.data(), B * sizeof(int));
     memcpy(g + B, h->h_tok_off.data(), B * sizeof(int));
     std::fill(g + 2 * B, g + 2 * B + Ttok, 0);
@@ -4938,7 +4914,7 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
       for (int i = 0; i < h->h_tok_len[b]; ++i) g[2 * B + h->h_tok_off[b] + i] = h->btp.off[b] + bert_rows[(size_t)b * t_max + i];
     h->run_graphed({vtts_engine::TAG_ST_TEXT_PIECES, B, h->maxTok, Ttok, prior ? 1 : 0, h->btp.maxL, h->btp.tot}, [&] {
       h->stt_bert_enqueue();
-      h->stt_enqueue(prior, true);
+      h->stt_enqueue(prior);
     });
   } else {
     h->run_graphed({vtts_engine::TAG_ST_TEXT, B, h->maxTok, Ttok, prior ? 1 : 0}, [&] { h->stt_enqueue(prior); });
@@ -4964,11 +4940,12 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
           "wav_ld is smaller than the longest utterance times the hop (mel_lengths holds the frame counts)");
   REQUIRE(!noise || noise_ld >= ext_max, VTTS_ERR_CAPACITY, "noise has fewer frames than the longest utterance padded to a multiple of 4 "
                                                             "(mel_lengths holds the frame counts)");
-  const vtts_engine::StPin pp = st_plan(h, B, frames, extents, sid, n, temperature, s, noise != nullptr, false, true, prior, denormalise, seed);
+  st_plan(h, B, frames, extents, sid, n, temperature, s, noise != nullptr, false, true, prior, denormalise, seed);
   const vtts_engine::StPlan& P = h->stp;
   if (noise)
     for (int b = 0; b < B; ++b)
-      memcpy(pp.noise + (size_t)h->h_frm_off[b] * NC, noise + (size_t)b * noise_ld * NC, (size_t)extents[b] * NC * sizeof(float));
+      memcpy(h->stg[vtts_engine::STG_ST_MEL].host(h->d_stnoise) + (size_t)h->h_frm_off[b] * NC, noise + (size_t)b * noise_ld * NC,
+             (size_t)extents[b] * NC * sizeof(float));
   // the vocoder reads the conditional sequences' rows: lens and offsets are the first B of the phase's [len NS][off NS] table
   h->run_graphed({vtts_engine::TAG_ST_MEL, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, prior ? 1 : 0, h->maxTok, Ttok, wav ? 1 : 0},
                  [&] {
@@ -5035,11 +5012,14 @@ static void impl_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* 
   h->have_latent = false;
   h->pack_frames(frames);
   voc_check_rows(h, h->Tfrm);
-  // pinned staging: ints [len B][off B], then the mel rows [Tfrm][NC] packed as the engine's rows
-  const size_t head = ((size_t)2 * B * sizeof(int) + 63) / 64 * 64;
-  char* pin = h->ensure(h->h_pin_hg, head + (size_t)h->Tfrm * NC * sizeof(float) + 64);
-  int* pi = reinterpret_cast<int*>(pin);
-  float* pm = reinterpret_cast<float*>(pin + head);
+  // staged: [len B][off B], then the mel rows [Tfrm][NC] packed as the engine's rows
+  vtts_engine::Staging& st = h->stg[vtts_engine::STG_VOCODER];
+  st.begin();
+  st.add(h->d_hgi, 2 * (size_t)B);
+  st.add(h->d_hgmel, (size_t)h->Tfrm * NC);
+  st.commit();
+  int* pi = st.host(h->d_hgi);
+  float* pm = st.host(h->d_hgmel);
   for (int b = 0; b < B; ++b) {
     pi[b] = frames[b];
     pi[B + b] = h->h_frm_off[b];
@@ -5048,8 +5028,7 @@ static void impl_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* 
   h->run_graphed({vtts_engine::TAG_HIFIGAN, B, h->maxFrm, h->Tfrm}, [&] {
     int* di = h->ensure(h->d_hgi, 2 * (size_t)B);
     float* dm = h->ensure(h->d_hgmel, (size_t)h->Tfrm * NC);
-    CK(cudaMemcpyAsync(di, pi, 2 * (size_t)B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(dm, pm, (size_t)h->Tfrm * NC * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    st.upload();
     h->voc_enqueue(dm, di, di + B);
   });
   read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames, h->hop, wav, wav_ld);
@@ -5135,17 +5114,20 @@ static void impl_resample(vtts_handle h, const float* wav, const int64_t* length
   if (same) out_off = in_off;
   else vtts_engine::pack_rows(out_len, out_off);
   // staging: the row table, then the packed input rows
-  const size_t head = ((size_t)5 * B * sizeof(int) + 63) / 64 * 64, nin = (size_t)in_off[B];
-  char* pin = h->ensure(h->h_pin_rs, head + nin * sizeof(float) + 64);
-  int* tab = reinterpret_cast<int*>(pin);
+  vtts_engine::Staging& st = h->stg[vtts_engine::STG_RESAMPLE];
+  st.begin();
+  st.add(h->d_rsi, (size_t)5 * B);
+  st.add(h->d_rsin, (size_t)in_off[B]);
+  st.commit();
+  int* tab = st.host(h->d_rsi);
+  float* pin = st.host(h->d_rsin);
   for (int b = 0; b < B; ++b) {
     tab[b] = in_off[b]; tab[B + b] = in_len[b]; tab[2 * B + b] = out_off[b]; tab[3 * B + b] = out_len[b]; tab[4 * B + b] = e_off[b];
-    memcpy(reinterpret_cast<float*>(pin + head) + in_off[b], wav + (size_t)b * ld, (size_t)in_len[b] * sizeof(float));
+    memcpy(pin + in_off[b], wav + (size_t)b * ld, (size_t)in_len[b] * sizeof(float));
   }
-  int* di = h->ensure(h->d_rsi, (size_t)5 * B);
-  float* din = h->ensure(h->d_rsin, nin);
-  CK(cudaMemcpyAsync(di, pin, (size_t)5 * B * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaMemcpyAsync(din, pin + head, nin * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  st.upload();
+  const int* di = h->d_rsi.p;
+  const float* din = h->d_rsin.p;
   const int max_out = *std::max_element(out_len.begin(), out_len.end());
   const float* y = din;
   if (!same) {
@@ -5230,6 +5212,7 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
   if (!cfg || !blob || !manifest || !out) return VTTS_ERR_INVALID;
   *out = nullptr;
   vtts_engine* h = new vtts_engine();
+  for (vtts_engine::Staging& s : h->stg) s.e = h;
   h->cfg = *cfg;
   h->device = device;
   *out = h;   // returned even on failure so that vtts_last_error() is readable; caller destroys it
@@ -5445,9 +5428,13 @@ int vtts_decode_chunk(vtts_handle h, int f0, int f1, float* wav, int64_t wav_cap
     const int halo = 24;
     const int lo = std::max(0, f0 - halo), hi = std::min(T, f1 + halo);
     int* dc = h->ensure(h->d_chunk, 4);
-    int* pin = reinterpret_cast<int*>(h->ensure(h->h_pin_len, 64));
+    vtts_engine::Staging& st = h->stg[vtts_engine::STG_CHUNK];
+    st.begin();
+    st.add(h->d_chunk, 3);
+    st.commit();
+    int* pin = st.host(h->d_chunk);
     pin[0] = hi - lo; pin[1] = lo; pin[2] = hi;
-    CK(cudaMemcpyAsync(dc, pin, 3 * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    st.upload();
     // the launches size grids and split-K for the chunk (the planes keep the full utterance's row count, Tfrm: the chunk is
     // addressed by its absolute rows)
     const Rows r{dc, dc + 1, 1, hi - lo, {hi - lo}, {hi - lo}, h->tune};
@@ -6356,12 +6343,12 @@ int vtts_debug_front_end(vtts_handle h, int from_spec, const float* in, const in
     h->have_latent = false;
     stage_clips(h, from_spec != 0, in, lengths, ld, fr, nullptr, nullptr, 0.f, nullptr, 0, 0);
     if (!from_spec) {     // NaN behind every clip in the staging, so that a read outside a clip shows in its rows
-      const vtts_engine::VcPin pp = h->vc_layout(vtts_engine::IN_WAV, false);
+      float* pin = h->stg[vtts_engine::STG_CLIPS].host(h->d_vin);
       for (int b = 0; b < B; ++b)
-        std::fill(pp.in + (size_t)b * h->vc_wld + lengths[b], pp.in + (size_t)(b + 1) * h->vc_wld, std::nanf(""));
+        std::fill(pin + (size_t)b * h->vc_wld + lengths[b], pin + (size_t)(b + 1) * h->vc_wld, std::nanf(""));
     }
     cudaStream_t st = h->stream;
-    h->vc_upload(from_spec ? vtts_engine::IN_SPEC : vtts_engine::IN_WAV, false);
+    h->vc_upload(false);
     float* dfeat = h->ensure(h->d_vfeat, (size_t)h->Tfrm * h->spec_pad);
     float* dmag = mel ? h->ensure(h->d_vlin, (size_t)h->Tfrm * nbins) : nullptr;
     CK(cudaMemcpyAsync(dfeat, feat, n * h->spec_pad * sizeof(float), cudaMemcpyHostToDevice, st));
