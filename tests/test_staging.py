@@ -1,6 +1,7 @@
-"""Every host input of a call reaches the device through the engine's pinned staging (struct Staging in csrc/engine.cu): the
-layout of a call's pinned block is decided in one place, so a replayed graph, which copies from the pinned addresses it
-captured, reads every field at the offset the host filled."""
+"""Every host input of a call reaches the device, and every output of a call reaches the host, through the engine's pinned
+staging (struct Staging in csrc/engine.cu): the layout of a call's pinned block is decided in one place, so a replayed graph,
+which copies to or from the pinned addresses it captured, finds every field at the offset where the host filled it or
+reads it."""
 import os
 import re
 
@@ -8,7 +9,10 @@ ENGINE = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))
 # Host-to-device copies that stay direct: the weight blob, the resampler's taps, the prefetch list, the handle-free
 # maximum path, and the microbenchmark and unit-test hooks; "upload" is Staging::upload and the hooks' upload helper
 DIRECT = ("vtts_create", "resample_taps", "build_prefetch_list", "vtts_maximum_path", "vtts_microbench", "upload")
-READBACK = {"h_pin", "h_pin_len", "h_pin_sttd", "h_pin_rse", "map"}
+# Device-to-host copies that stay direct: the T2S weights' alpha read at load, the handle-free maximum path, the timeline,
+# and the microbenchmark and unit-test hooks; "download" is Staging::download
+DIRECT_READ = ("bind_t2s", "vtts_maximum_path", "vtts_timeline", "vtts_microbench", "download")
+MAPPED = {"map"}                # the mapped buffer phase 1 publishes the frame lengths into
 ROUND64 = re.compile(r"\+ 63\) / 64 \* 64")
 
 
@@ -46,24 +50,42 @@ def _line(src, pos):
     return src.count("\n", 0, pos) + 1
 
 
-def test_host_to_device_copies_go_through_the_staging():
-    src = _source()
-    allowed = [s for name in DIRECT for s in _definitions(src, name)]
+def _copies_outside(src, kind, direct, caller_arg):
+    """Lines of every `kind` copy outside the definitions in `direct`, the unit-test hooks (vtts_debug_*) and, in
+    impl_t2s_decode, the copy of the caller's array `caller_arg`."""
+    allowed = [s for name in direct for s in _definitions(src, name)]
     allowed += [s for s in (_block(src, m.start()) for m in re.finditer(r"^\w.*\bvtts_debug_\w+\s*\([^;{]*\)\s*\{", src, re.M))]
     t2s = _definitions(src, "impl_t2s_decode")
     offenders = []
-    for m in re.finditer(r"cudaMemcpyHostToDevice", src):
+    for m in re.finditer(kind, src):
         if any(lo <= m.start() < hi for lo, hi in allowed):
             continue
         if any(lo <= m.start() < hi for lo, hi in t2s):
             call = src[src.rindex("cudaMemcpy", 0, m.start()):m.start()]
-            if re.search(r",\s*q\s*,", call):        # the caller's sampling draws, up to B * q_ld * V floats, copied once
+            if re.search(r"[(,]\s*%s\s*," % caller_arg, call):
                 continue
         offenders.append("line %d" % _line(src, m.start()))
+    return offenders
+
+
+def test_host_to_device_copies_go_through_the_staging():
+    # (the caller's sampling draws q, up to B * q_ld * V floats, are copied once straight from its memory)
+    offenders = _copies_outside(_source(), "cudaMemcpyHostToDevice", DIRECT, "q")
     assert not offenders, "host-to-device copies outside Staging::upload:\n" + "\n".join(offenders)
 
 
-def test_pinned_members_are_the_staging_and_the_readback_buffers():
+def test_device_to_host_copies_go_through_the_staging():
+    # (the caller's logits, up to B * logits_ld * V floats, are copied once straight to its memory)
+    offenders = _copies_outside(_source(), "cudaMemcpyDeviceToHost", DIRECT_READ, "logits")
+    assert not offenders, "device-to-host copies outside Staging::download:\n" + "\n".join(offenders)
+
+
+def test_readback_helpers_are_gone():
+    src = _source()
+    assert not re.search(r"\bensure_pinned\b", src), "engine.cu still has ensure_pinned"
+
+
+def test_pinned_members_are_the_staging_and_the_mapped_buffer():
     src = _source()
     eng = _struct(src, "vtts_engine")
     staging = _struct(src, "Staging", eng)
@@ -71,7 +93,7 @@ def test_pinned_members_are_the_staging_and_the_readback_buffers():
     members = set()
     for decl in re.findall(r"\b(?:PinnedBuf|MappedBuf)<[^>]*>\s+([^;]+);", body):
         members.update(n.strip() for n in decl.split(","))
-    assert members == READBACK, "pinned members of vtts_engine besides its staging: %s" % sorted(members - READBACK)
+    assert members == MAPPED, "pinned members of vtts_engine besides its staging: %s" % sorted(members - MAPPED)
     assert re.findall(r"\b(?:PinnedBuf|MappedBuf)<[^>]*>\s+([^;]+);", src[staging[0]:staging[1]]) == ["pin"]
     assert re.search(r"\bStaging\s+stg\s*\[\s*STG_KINDS\s*\]\s*;", body), "vtts_engine has no staging array"
 

@@ -86,6 +86,7 @@ def vits2(p, batch, tag):
     run(e, tag + " infer", lambda: e.infer(ids, T, sid, sc, seed=1))
     run(e, tag + " durations", lambda: e.durations(ids, T, sid, sc, seed=2, want_durations=True))
     run(e, tag + " synthesize", lambda: e.synthesize(e.durations(ids, T, sid, sc, seed=2)))
+    run(e, tag + " synthesize alignment", lambda: e.synthesize(e.durations(ids, T, sid, sc, seed=2), want_alignment=True))
     run(e, tag + " flow+decode_chunk", lambda: list(e.synthesize_stream(ids[:1, :T[0]], 1, sc, chunk_frames=40, seed=3)))
     run(e, tag + " convert", lambda: e.convert(wav(batch), sid, sid[::-1], lengths=wl(batch), seed=4))
     run(e, tag + " align", lambda: e.align(ids, T, sid, wav(batch), wl(batch), seed=5))
@@ -98,6 +99,9 @@ def vits2(p, batch, tag):
 def quickvc(p, batch, tag):
     e = engine(qcfg, sblob, sman, p)
     run(e, tag + " speaker_embedding", lambda: e.speaker_embedding(wav(batch), wl(batch)))
+    F = [60 * k + 71 for k in batch]
+    mel = np.random.RandomState(12).normal(-4.0, 2.0, (len(F), qcfg["n_mel_channels"], max(F))).astype(np.float32)
+    run(e, tag + " speaker_embedding_mel", lambda: e.speaker_embedding_mel(mel, F))
     e.close()
     e = engine(ccfg, cblob, cman, p)
     U = [13 * k + 4 for k in batch]
@@ -124,6 +128,7 @@ def stabletts(p, batch, tag):
     berts = [r.randn(tcfg["bert_dim"], t).astype(np.float32) for t in L]
     for w in (False, True):
         run(e, tag + " stabletts_synthesise wav=%d" % w, lambda: tts.synthesise(xs, berts, 0, n_timesteps=3, seed=9, return_wav=w))
+    run(e, tag + " stabletts_synthesise prior", lambda: tts.synthesise(xs, berts, 0, n_timesteps=3, seed=9, return_prior=True))
     mels = [m.T for m in HI.case_mels(("ab", [11 * k + 6 for k in batch]))]
     run(e, tag + " hifigan_vocode", lambda: e.hifigan_vocode(mels if len(mels) > 1 else mels[0]))
     tts.close()

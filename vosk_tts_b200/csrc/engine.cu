@@ -414,7 +414,6 @@ struct vtts_engine {
   Buf<unsigned long long> d_tl;                  // vtts_timeline's counter and (source line, ns) pairs
   Buf<float> d_zp_dbg;                           // copy of z_p kept when debug_flags & 1
   int debug_flags = 0;
-  PinnedBuf<char> h_pin, h_pin_len;              // pinned readback (host): outputs; phase-1 lengths and T2S stop counts
   Buf<float> d_prm;                              // per-call scalars (see kernels.cuh prm_seed)
   MappedBuf<int> map;                            // mapped pinned host memory: [0] sequence flag, lengths, offsets
   int call_seq = 0;
@@ -456,43 +455,61 @@ struct vtts_engine {
     }
     return b.p;
   }
-  char* ensure_pinned(size_t n) { return ensure(h_pin, n); }
 
-  // Pinned staging of one kind of call input: a pinned block and the ordered fields the call copies from it, each to one
-  // engine buffer.  A call lists its fields (begin, add), sizes the block and the destinations once (commit), fills the
-  // fields on the host (host: a field is named by the buffer it is copied to), and enqueues the copies where its enqueue
-  // runs them (upload), one cudaMemcpyAsync per field in field order, to the destination as it is at that moment.
-  // A replayed graph copies from the pinned addresses it captured, so the layout of a call must follow from its graph key
-  // alone.  It does by construction: each field starts at the first 64-byte boundary behind the one before, so the layout is
-  // a function of the field sizes, and those are the sizes of the copies the graph holds.
+  // Pinned staging of one kind of call input or output: a pinned block and the ordered fields a call copies to or from it,
+  // each from or to one engine buffer (n elements of the buffer from element `at`).  A call lists its fields (begin, add),
+  // sizes the block once (commit; for an input kind the destinations as well, while a readback never grows its sources), and
+  // enqueues the copies where its enqueue runs them, one cudaMemcpyAsync per field in field order, to or from the buffer as
+  // it is at that moment: upload after the host has filled the fields, download before the host reads them.  The host
+  // names a field by its buffer (host).  A field may reserve room for more elements than it copies, so that a block sized
+  // for a length bucket does not grow with every new length.
+  // A replayed graph copies to or from the pinned addresses it captured, so the layout of a call must follow from its graph
+  // key alone.  It does by construction: each field starts at the first 64-byte boundary behind the one before, so the
+  // layout is a function of the field sizes, and those are the sizes of the copies the graph holds.
   struct Staging {
-    struct Field { void* dst; size_t off, n, bytes; void* (*ensure)(vtts_engine&, void* dst, size_t n); };
+    struct Field { void* buf; size_t off, at, n, bytes, room; void* (*dev)(vtts_engine&, void* buf, size_t at, size_t n, bool grow); };
     vtts_engine* e = nullptr;
+    bool readback = false;                       // copied from its buffers (vtts_create sets it: a kind goes one way)
     PinnedBuf<char> pin;
     std::vector<Field> fields;
-    size_t end() const { return fields.empty() ? 0 : fields.back().off + fields.back().bytes; }
+    size_t end() const { return fields.empty() ? 0 : fields.back().off + fields.back().room; }
     void begin() { fields.clear(); }
     template <typename T>
-    void add(Buf<T>& dst, size_t n) {
-      fields.push_back({&dst, (end() + 63) / 64 * 64, n, n * sizeof(T),
-                        [](vtts_engine& h, void* b, size_t k) -> void* { return h.ensure(*static_cast<Buf<T>*>(b), k); }});
+    void add(Buf<T>& buf, size_t n, size_t at = 0, size_t room = 0) {
+      fields.push_back({&buf, (end() + 63) / 64 * 64, at, n, n * sizeof(T), std::max(n, room) * sizeof(T),
+                        [](vtts_engine& h, void* b, size_t at, size_t k, bool grow) -> void* {
+                          Buf<T>& d = *static_cast<Buf<T>*>(b);
+                          REQUIRE(grow || d.cap >= at + k, VTTS_ERR_STATE, "a readback reads past the end of its source buffer");
+                          return (grow ? h.ensure(d, at + k) : d.p) + at;
+                        }});
     }
     void commit() {
       e->ensure(pin, end());
-      for (const Field& f : fields) f.ensure(*e, f.dst, f.n);
+      if (!readback)
+        for (const Field& f : fields) f.dev(*e, f.buf, f.at, f.n, true);
     }
     template <typename T>
-    T* host(const Buf<T>& dst) {
+    T* host(const Buf<T>& buf) {
       for (const Field& f : fields)
-        if (f.dst == &dst) return reinterpret_cast<T*>(pin.p + f.off);
-      throw Err{VTTS_ERR_STATE, "a staged input was filled that the call does not copy"};
+        if (f.buf == &buf) return reinterpret_cast<T*>(pin.p + f.off);
+      throw Err{VTTS_ERR_STATE, "a staged field was named that the call does not copy"};
     }
     void upload() {
       for (const Field& f : fields)
-        CK(cudaMemcpyAsync(f.ensure(*e, f.dst, f.n), pin.p + f.off, f.bytes, cudaMemcpyHostToDevice, e->stream));
+        CK(cudaMemcpyAsync(f.dev(*e, f.buf, f.at, f.n, true), pin.p + f.off, f.bytes, cudaMemcpyHostToDevice, e->stream));
+    }
+    void download() {
+      for (const Field& f : fields)
+        CK(cudaMemcpyAsync(pin.p + f.off, f.dev(*e, f.buf, f.at, f.n, false), f.bytes, cudaMemcpyDeviceToHost, e->stream));
+    }
+    // outside a graph: download, mark the end of the call's device work (ev[7], read by collect_timings) and wait for it
+    void download_and_wait() {
+      download();
+      CK(cudaEventRecord(e->ev[7], e->stream));
+      CK(cudaStreamSynchronize(e->stream));
     }
   };
-  // One staging per input kind; inputs that one call holds at the same time are in different kinds.
+  // One staging per kind of input or output; what one call holds at the same time is in different kinds.
   enum StagingKind {
     STG_TOKENS,       // token lengths, offsets and ids, and phase 1's scalars, speaker ids and noise (TTS phase 1, alignment)
     STG_NOISE_Z,      // phase 2's noise_z
@@ -500,6 +517,11 @@ struct vtts_engine {
     STG_CONTENTVEC, STG_BERT, STG_ST_TEXT, STG_ST_PIECES, STG_ST_MEL, STG_VOCODER, STG_RESAMPLE, STG_T2S,
     STG_SPK_SLICES,   // the speaker encoder's slice table
     STG_CHUNK,        // the rows of vtts_decode_chunk
+    STG_OUT,          // readbacks from here on: a call's outputs
+    STG_LENGTHS,      // phase 1's frame lengths and offsets without polling (copied inside its graph)
+    STG_T2S_STOP0, STG_T2S_STOP1,   // T2S's count of stopped utterances after an even / odd chunk (two chunks in flight)
+    STG_ST_DURATIONS, // the StableTTS text phase's d_sttd (copied inside its graph)
+    STG_TRIM,         // the resampler's frame energies
     STG_KINDS
   };
   Staging stg[STG_KINDS];                        // (vtts_create points each at its engine)
@@ -915,7 +937,6 @@ struct vtts_engine {
   const float *st_tok_emb = nullptr, *st_punc_emb = nullptr, *st_bert_w = nullptr, *st_bert_b = nullptr;
   Buf<int> d_stti, d_sttd;                         // [tok len B][tok off B][sid B][ids streams x Ttok]; [dur Ttok][first Ttok][frames B]
   Buf<float> d_sttf, d_stbert, d_sttx, d_stte[2], d_sttada, d_sttrope, d_stmumel, d_stmudp, d_stlogw, d_stpau;
-  PinnedBuf<char> h_pin_sttd;                      // readback of d_sttd
   void stt_enqueue(bool prior);
   // vtts_stabletts_synthesise_pieces_wav: BERT of the staged sentences (bt_stage), then each token's row gathered into d_stbert.
   // d_stg holds the token rows' lengths and offsets and each one's source, BERT's packed row btp.off[b] + bert_rows[b][t].
@@ -937,7 +958,6 @@ struct vtts_engine {
   Buf<int> d_rsi;                                  // [in_off B][in_len B][out_off B][out_len B][e_off B]
   Buf<float> d_rsin, d_rsout;
   Buf<double> d_rse;                               // frame energies of the trim
-  PinnedBuf<char> h_pin_rse;                       // readback of d_rse
   const RsTaps& resample_taps(int up, int down);
 
   // ---- forced alignment (the alignment of SynthesizerTrn.forward, models.py:1632-1660)
@@ -2215,11 +2235,7 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
   CK(cudaGetLastError());
   ++launches;
   if (!capturing) CK(cudaEventRecord(ev[3], stream));
-  if (!use_poll) {
-    int* p_len = reinterpret_cast<int*>(ensure(h_pin_len, (size_t)(2 * B + 2) * sizeof(int)));
-    CK(cudaMemcpyAsync(p_len, fl, B * sizeof(int), cudaMemcpyDeviceToHost, stream));
-    CK(cudaMemcpyAsync(p_len + B, fo, (B + 1) * sizeof(int), cudaMemcpyDeviceToHost, stream));
-  }
+  if (!use_poll) stg[STG_LENGTHS].download();
   // prior statistics m_p, logs_p (models.py:323-325): overlaps the host's round trip between the two phases
   prior_stats();
 }
@@ -2335,12 +2351,18 @@ void vtts_engine::stage_tokens(const int64_t* ids, int t_max, bool phase1, bool 
   }
 }
 
-// The phase-1 rest of the staging (after stage_tokens): scales and seed, the poll sequence, the speculation's frame cap and
-// the duration predictor's noise.
+// The phase-1 rest of the staging (after stage_tokens): scales and seed, the poll sequence (or without polling the frame
+// lengths' readback), the speculation's frame cap and the duration predictor's noise.
 void vtts_engine::stage1(int t_max, const float* noise_dp_host) {
   float* prm = stg[STG_TOKENS].host(d_prm);
   put_scalars(prm, 8, scales, 3, seed);
-  if (use_poll) {
+  if (!use_poll) {
+    Staging& s = stg[STG_LENGTHS];
+    s.begin();
+    s.add(d_frm_len, B);
+    s.add(d_frm_off, B + 1);
+    s.commit();
+  } else {
     const size_t need = (size_t)(2 * B + 4);
     if (need > map.cap) {
       REQUIRE(!capturing, VTTS_ERR_STATE, "mapped buffer growth during capture");
@@ -2380,9 +2402,9 @@ void vtts_engine::finish1() {
     return;
   }
   CK(cudaStreamSynchronize(stream));
-  const int* p_len = reinterpret_cast<const int*>(h_pin_len.p);
-  h_frm_len.assign(p_len, p_len + B);
-  h_frm_off.assign(p_len + B, p_len + 2 * B + 1);
+  const int *len = stg[STG_LENGTHS].host(d_frm_len), *off = stg[STG_LENGTHS].host(d_frm_off);
+  h_frm_len.assign(len, len + B);
+  h_frm_off.assign(off, off + B + 1);
   check_frame_lengths(h_frm_len.data(), h_frm_off[B], B);
   set_frame_shape();
   have_durations = true;
@@ -3808,7 +3830,7 @@ void vtts_engine::st_enqueue() {
 
 // Text phase of vtts_stabletts_synthesise: uploads, the token rows x, dp_encoder and its proj, the durations and their scan;
 // with `prior` the mel encoder and its proj as well.  Leaves x, the durations, each token's first frame, the pauses and
-// mu_mel on the device for the mel phase, and copies [dur][first][frames of every utterance] to pinned memory.  The BERT rows
+// mu_mel on the device for the mel phase, and downloads d_sttd, [dur][first][frames of every utterance] (STG_ST_DURATIONS).  The BERT rows
 // are in d_stbert: uploaded with the staged inputs, or gathered there by stt_bert_enqueue.
 void vtts_engine::stt_enqueue(bool prior) {
   const vtts_config& c = cfg;
@@ -3854,8 +3876,7 @@ void vtts_engine::stt_enqueue(bool prior) {
           (float)VTTS_ST_MAX_TOKEN_FRAMES, dd, dd + Ttok, dd + 2 * Ttok, logw, lens, offs);
   CK(cudaGetLastError());
   ++launches;
-  int* back = reinterpret_cast<int*>(ensure(h_pin_sttd, (2 * T + B) * sizeof(int)));
-  CK(cudaMemcpyAsync(back, dd, (2 * T + B) * sizeof(int), cudaMemcpyDeviceToHost, stream));
+  stg[STG_ST_DURATIONS].download();
 }
 
 // BERT rows of the text phase from word pieces: BERT of the sentences bt_stage staged, into its packed rows d_btout, then
@@ -4027,18 +4048,24 @@ void collect_timings(vtts_handle h) {
   cudaEventElapsedTime(&t, h->ev[6], h->ev[7]); h->stage_ms[5] = t;
 }
 
-// Readback of a call's packed output rows: D2H of the first n values of src into pinned staging sized for `cap` values (the
-// bucket's, so that it does not grow with every new length), ev[7], a sync, then clip b's lens[b] rows of `width` values
-// from packed row offs[b] to out + b * out_ld.  The rest of each output row is left as it is.
+// Readback of one output field of a call (STG_OUT): the n values of src from element `at`, in a field with room for `room`
+// values (a bucket's, so that the block does not grow with every new length).  Returns the values.
 template <typename T>
-void read_clips(vtts_handle h, const T* src, size_t n, size_t cap, const int* offs, const std::vector<int>& lens, int width,
-                T* out, int64_t out_ld) {
-  T* pin = reinterpret_cast<T*>(h->ensure_pinned(cap * sizeof(T) + 64));
-  CK(cudaMemcpyAsync(pin, src, n * sizeof(T), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaEventRecord(h->ev[7], h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+const T* read_back(vtts_handle h, Buf<T>& src, size_t n, size_t room = 0, size_t at = 0) {
+  vtts_engine::Staging& s = h->stg[vtts_engine::STG_OUT];
+  s.begin();
+  s.add(src, n, at, room);
+  s.commit();
+  s.download_and_wait();
+  return s.host(src);
+}
+
+// Clip b's lens[b] rows of `width` values from packed row offs[b] of a call's read-back rows to out + b * out_ld.  The rest
+// of each output row is left as it is.
+template <typename T>
+void read_clips(const T* rows, const int* offs, const std::vector<int>& lens, int width, T* out, int64_t out_ld) {
   for (size_t b = 0; b < lens.size(); ++b)
-    memcpy(out + b * out_ld, pin + (size_t)offs[b] * width, (size_t)lens[b] * width * sizeof(T));
+    memcpy(out + b * out_ld, rows + (size_t)offs[b] * width, (size_t)lens[b] * width * sizeof(T));
 }
 
 void setup_lengths(vtts_handle h, const int64_t* lengths, int B, int t_max) {
@@ -4084,9 +4111,7 @@ static void impl_durations(vtts_handle h, const int64_t* ids, const int64_t* len
   if (B == 1) h->spec_learn();
   for (int b = 0; b < B; ++b) y_lengths[b] = h->h_frm_len[b];
   if (durations) {
-    std::vector<int> wc(h->Ttok);
-    CK(cudaMemcpyAsync(wc.data(), h->d_wceil.p, h->Ttok * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    const int* wc = read_back(h, h->d_wceil, h->Ttok);
     for (int b = 0; b < B; ++b) {
       for (int t = 0; t < t_max; ++t)
         durations[(size_t)b * t_max + t] = t < h->h_tok_len[b] ? wc[h->h_tok_off[b] + t] : 0;
@@ -4102,10 +4127,14 @@ static void impl_synthesize(vtts_handle h, const float* noise_z, int z_ld, float
   if (noise_z) h->stage_noise_z(noise_z, z_ld);
   // graph key = the length BUCKETS (token rows, frame rows), not the lengths: kernels read the true lengths on the device
   h->run_graphed({vtts_engine::TAG_PHASE2, h->B, h->maxFrm, h->Tfrm, noise_z ? 1 : 0}, [&] { h->phase2(noise_z, z_ld, false); });
-  if (frame_token)
-    read_clips(h, (const int*)h->d_ftok.p, h->real_Tfrm, h->Tfrm, h->h_frm_off.data(), h->h_frm_len, 1, frame_token, idx_ld);
-  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), h->h_frm_len,
-             h->hop, wav, wav_ld);
+  vtts_engine::Staging& s = h->stg[vtts_engine::STG_OUT];
+  s.begin();
+  if (frame_token) s.add(h->d_ftok, h->real_Tfrm, 0, h->Tfrm);
+  s.add(h->d_wav, (size_t)h->real_Tfrm * h->hop, 0, (size_t)h->Tfrm * h->hop);
+  s.commit();
+  s.download_and_wait();
+  if (frame_token) read_clips(s.host(h->d_ftok), h->h_frm_off.data(), h->h_frm_len, 1, frame_token, idx_ld);
+  read_clips(s.host(h->d_wav), h->h_frm_off.data(), h->h_frm_len, h->hop, wav, wav_ld);
   collect_timings(h);
   h->have_durations = false;
 }
@@ -4154,12 +4183,12 @@ static void impl_infer(vtts_handle h, const int64_t* ids, const int64_t* lengths
     if (noise_z) h->stage_noise_z(noise_z, z_ld);
     h->run_graphed({vtts_engine::TAG_PHASE2, h->B, h->maxFrm, h->Tfrm, noise_z ? 1 : 0}, [&] { h->phase2(noise_z, z_ld, false); });
     // the true length is not known on the host yet: the bucket's worth of samples comes back
-    const size_t ncap = (size_t)cap * h->hop;
-    char* pin = h->ensure_pinned(ncap * sizeof(float) + (size_t)cap * sizeof(int) + 64);
-    float* pw = reinterpret_cast<float*>(pin);
-    int* pi = reinterpret_cast<int*>(pw + ncap);
-    CK(cudaMemcpyAsync(pw, h->d_wav.p, ncap * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-    if (frame_token) CK(cudaMemcpyAsync(pi, h->d_ftok.p, (size_t)cap * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    vtts_engine::Staging& s = h->stg[vtts_engine::STG_OUT];
+    s.begin();
+    s.add(h->d_wav, (size_t)cap * h->hop);
+    if (frame_token) s.add(h->d_ftok, cap);
+    s.commit();
+    s.download();
     const double t_2 = now_us();
     CK(cudaStreamSynchronize(h->stream));
     const double t_3 = now_us();
@@ -4178,8 +4207,8 @@ static void impl_infer(vtts_handle h, const int64_t* ids, const int64_t* lengths
       REQUIRE((int64_t)real * h->hop <= wav_ld, VTTS_ERR_CAPACITY, "wav_ld is smaller than hop * max(y_lengths)");
       REQUIRE(!noise_z || z_ld >= real, VTTS_ERR_CAPACITY, "noise_z has fewer columns than max(y_lengths)");
       REQUIRE(!frame_token || idx_ld >= real, VTTS_ERR_CAPACITY, "frame_token has fewer columns than max(y_lengths)");
-      memcpy(wav, pw, (size_t)real * h->hop * sizeof(float));
-      if (frame_token) memcpy(frame_token, pi, (size_t)real * sizeof(int));
+      memcpy(wav, s.host(h->d_wav), (size_t)real * h->hop * sizeof(float));
+      if (frame_token) memcpy(frame_token, s.host(h->d_ftok), (size_t)real * sizeof(int));
       h->have_durations = false;
       h->host_us[3] = now_us() - t_3; h->host_us[4] = now_us() - t_0;
       return;
@@ -4312,8 +4341,8 @@ static void impl_convert(vtts_handle h, bool from_spec, const float* in, const i
   stage_clips(h, from_spec, in, lengths, ld, frames, sid_src, sid_tgt, noise_scale, noise_q, q_ld, seed);
   h->run_graphed({vtts_engine::TAG_CONVERT, B, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
                  [&] { h->convert_enqueue(from_spec, noise_q != nullptr); });
-  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames,
-             h->hop, out_wav, out_ld);
+  read_clips(read_back(h, h->d_wav, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop), h->h_frm_off.data(), frames, h->hop,
+             out_wav, out_ld);
   std::copy(frames.begin(), frames.end(), out_frames);
 }
 
@@ -4352,10 +4381,7 @@ static void impl_speaker_embedding(vtts_handle h, bool from_mel, const float* in
   std::vector<int> seq;
   for (auto* v : {&xrow, &slen, &soff, &last, &of_clip}) seq.insert(seq.end(), v->begin(), v->end());
   h->spk_enqueue(from_mel, seq, max_len);
-  float* pg = reinterpret_cast<float*>(h->ensure_pinned((size_t)B * SPK_H * sizeof(float) + 64));
-  CK(cudaMemcpyAsync(pg, h->d_sg.p, (size_t)B * SPK_H * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  memcpy(g_out, pg, (size_t)B * SPK_H * sizeof(float));
+  memcpy(g_out, read_back(h, h->d_sg, (size_t)B * SPK_H), (size_t)B * SPK_H * sizeof(float));
 }
 
 // Forced alignment through host buffers (vtts_align / vtts_align_spec).
@@ -4387,24 +4413,24 @@ static void impl_align(vtts_handle h, bool from_spec, const int64_t* ids, const 
   stage_clips(h, from_spec, in, lengths, ld, frames, h->has_g ? sid : nullptr, nullptr, noise_scale, noise_q, q_ld, seed);
   h->run_graphed({vtts_engine::TAG_ALIGN, B, h->maxTok, h->Ttok, h->maxFrm, h->Tfrm, from_spec ? 1 : 0, noise_q ? 1 : 0},
                  [&] { h->align_enqueue(from_spec, noise_q != nullptr); });
-  const size_t nt = (size_t)h->real_Ttok, nf = (size_t)h->real_Tfrm;
-  int* pin = reinterpret_cast<int*>(h->ensure_pinned((nt + nf + (size_t)B) * sizeof(int) + 64));
-  CK(cudaMemcpyAsync(pin, h->d_adur.p, nt * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(pin + nt, h->d_atof.p, nf * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(pin + nt + nf, h->d_ascore.p, (size_t)B * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaEventRecord(h->ev[7], h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  vtts_engine::Staging& s = h->stg[vtts_engine::STG_OUT];
+  s.begin();
+  s.add(h->d_adur, h->real_Ttok);
+  s.add(h->d_atof, h->real_Tfrm);
+  s.add(h->d_ascore, B);
+  s.commit();
+  s.download_and_wait();
   for (int b = 0; b < B; ++b) {
     const int tx = h->h_tok_len[b], ty = frames[b];
     int32_t* d = durations + (size_t)b * t_max;
-    memcpy(d, pin + h->h_tok_off[b], (size_t)tx * sizeof(int));
+    memcpy(d, s.host(h->d_adur) + h->h_tok_off[b], (size_t)tx * sizeof(int));
     std::fill(d + tx, d + t_max, 0);
     if (token_of_frame) {
       int32_t* f = token_of_frame + (size_t)b * tof_ld;
-      memcpy(f, pin + nt + h->h_frm_off[b], (size_t)ty * sizeof(int));
+      memcpy(f, s.host(h->d_atof) + h->h_frm_off[b], (size_t)ty * sizeof(int));
       std::fill(f + ty, f + tof_ld, -1);
     }
-    if (score) memcpy(score + b, pin + nt + nf + b, sizeof(float));
+    if (score) score[b] = s.host(h->d_ascore)[b];
     out_frames[b] = ty;
   }
 }
@@ -4426,7 +4452,7 @@ static void impl_content_units(vtts_handle h, const float* wav, const int64_t* l
   const int H = h->cfg.cv_hidden, NL = h->cfg.cv_n_conv;
   const size_t Tf = (size_t)h->cvp.tot0 / h->cv_P;
   h->run_graphed({vtts_engine::TAG_CONTENTVEC, B, h->cvp.maxS, h->cvp.tot0}, [&] { h->cv_enqueue(h->ensure(h->d_cvu, Tf * H), nullptr); });
-  read_clips(h, (const float*)h->d_cvu.p, Tf * H, Tf * H, h->cvp.h.data() + (NL + NL - 1) * B, frames, H, units, units_ld * H);
+  read_clips(read_back(h, h->d_cvu, Tf * H), h->cvp.h.data() + (NL + NL - 1) * B, frames, H, units, units_ld * H);
   for (int b = 0; b < B; ++b) {
     std::fill(units + ((size_t)b * units_ld + frames[b]) * H, units + (size_t)(b + 1) * units_ld * H, 0.f);
     out_frames[b] = frames[b];
@@ -4443,9 +4469,13 @@ static void impl_bert_features(vtts_handle h, const int64_t* ids, const int64_t*
   for (int b = 0; b < B; ++b) REQUIRE(h->btp.len[b] <= out_ld, VTTS_ERR_CAPACITY, "out_ld is smaller than a sentence's length");
   const int H = h->cfg.cv_hidden;
   const size_t n = (size_t)h->btp.tot * H;
-  h->ensure_pinned(n * sizeof(float) + 64);     // the readback's staging, grown before the graph captures (growth retires it)
+  vtts_engine::Staging& s = h->stg[vtts_engine::STG_OUT];      // listed before the graph captures (growth retires it)
+  s.begin();
+  s.add(h->d_btout, n);
+  s.commit();
   h->run_graphed({vtts_engine::TAG_BERT, B, h->btp.maxL, h->btp.tot}, [&] { h->bt_enqueue(h->ensure(h->d_btout, n)); });
-  read_clips(h, (const float*)h->d_btout.p, n, n, h->btp.off.data(), h->btp.len, H, out, out_ld * H);
+  s.download_and_wait();
+  read_clips(s.host(h->d_btout), h->btp.off.data(), h->btp.len, H, out, out_ld * H);
   for (int b = 0; b < B; ++b) std::fill(out + ((size_t)b * out_ld + h->btp.len[b]) * H, out + (size_t)(b + 1) * out_ld * H, 0.f);
 }
 
@@ -4629,29 +4659,39 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
     CK(cudaGetLastError());
     h->launches += 5 * (uint64_t)NL + 2;
   };
+  // ---- readbacks, sized before the chunks' graphs capture (growth retires them): the stop count behind the state rows, one
+  //      staging per chunk in flight; then the state rows and the tokens
+  vtts_engine::Staging* stop = &h->stg[vtts_engine::STG_T2S_STOP0];
+  for (int k = 0; k < 2; ++k) {
+    stop[k].begin();
+    stop[k].add(h->d_t2s_st, 1, (size_t)B * T2S_ST);
+    stop[k].commit();
+  }
+  vtts_engine::Staging& out = h->stg[vtts_engine::STG_OUT];
+  out.begin();
+  out.add(h->d_t2s_st, (size_t)B * T2S_ST);
+  out.add(h->d_t2s_tok, (size_t)ytot);
+  out.commit();
   // ---- decode loop: every utterance has stopped after gen_max steps at the latest
-  int* flag = reinterpret_cast<int*>(h->ensure(h->h_pin_len, 2 * sizeof(int)));      // two slots, one per chunk in flight
   const long bound = gen_max;
   for (long it = 0, chunk = 0;; ++chunk) {
     h->run_graphed({vtts_engine::TAG_T2S, B, nsplit, kvn, ytot, q ? q_ld : -1, logits ? logits_ld : -1},
                    [&] { for (int k = 0; k < vtts_engine::T2S_CHUNK; ++k) step(); });
-    CK(cudaMemcpyAsync(flag + (chunk & 1), nstop, sizeof(int), cudaMemcpyDeviceToHost, s));
+    stop[chunk & 1].download();
     CK(cudaEventRecord(h->ev[chunk & 1], s));
     it += vtts_engine::T2S_CHUNK;
     if (it >= bound) break;
     if (chunk >= 1) {
       CK(cudaEventSynchronize(h->ev[(chunk - 1) & 1]));
-      if (flag[(chunk - 1) & 1] >= B) break;
+      if (*stop[(chunk - 1) & 1].host(h->d_t2s_st) >= B) break;
     }
   }
-  // ---- read back
-  std::vector<int> sth((size_t)B * T2S_ST), yh((size_t)ytot);
-  CK(cudaMemcpyAsync(sth.data(), dst, sth.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(yh.data(), dy, yh.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  // ---- read back (the caller's logits, up to B * logits_ld * V floats, straight to its memory, as q comes from it)
   if (logits) CK(cudaMemcpyAsync(logits, draw, (size_t)B * logits_ld * V * sizeof(float), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
+  out.download_and_wait();
+  const int *sth = out.host(h->d_t2s_st), *yh = out.host(h->d_t2s_tok);
   for (int b = 0; b < B; ++b) {
-    const int* sb = sth.data() + (size_t)b * T2S_ST;
+    const int* sb = sth + (size_t)b * T2S_ST;
     REQUIRE(sb[ST_STOP] == 1, VTTS_ERR_STATE, "an utterance did not stop within its step limit");
     const int gen = sb[ST_GEN], n = P[b] + gen - 1;          // y[:, :-1]: the last appended token is dropped
     if (n_tokens) n_tokens[b] = n;
@@ -4719,8 +4759,8 @@ static void impl_quickvc_convert(vtts_handle h, const float* units, const float*
                    [&] { h->quickvc_enqueue(noise != nullptr, true); });
   else
     h->run_graphed({vtts_engine::TAG_QUICKVC, B, h->maxFrm, h->Tfrm, noise ? 1 : 0}, [&] { h->quickvc_enqueue(noise != nullptr); });
-  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames,
-             h->hop, out_wav, out_ld);
+  read_clips(read_back(h, h->d_wav, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop), h->h_frm_off.data(), frames, h->hop,
+             out_wav, out_ld);
   for (int b = 0; b < B; ++b) {
     std::fill(out_wav + (size_t)b * out_ld + (size_t)frames[b] * h->hop, out_wav + (size_t)(b + 1) * out_ld, 0.f);
     out_frames[b] = frames[b];
@@ -4825,7 +4865,7 @@ static void impl_cfm_decode(vtts_handle h, const float* mu, const int64_t* lengt
     if (noise) memcpy(pn + o * NC, noise + (size_t)b * noise_ld * NC, (size_t)frames[b] * NC * sizeof(float));
   }
   h->run_graphed({vtts_engine::TAG_CFM, B, h->maxFrm, h->Tfrm, n, P.guided ? 1 : 0, P.noise ? 1 : 0, P.rows ? 1 : 0}, [&] { h->st_enqueue(); });
-  read_clips(h, (const float*)h->d_stmel.p, (size_t)h->real_Tfrm * NC, (size_t)h->Tfrm * NC, h->h_frm_off.data(), frames, NC, mel_out,
+  read_clips(read_back(h, h->d_stmel, (size_t)h->real_Tfrm * NC, (size_t)h->Tfrm * NC), h->h_frm_off.data(), frames, NC, mel_out,
              mel_ld * NC);
 }
 
@@ -4901,6 +4941,10 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
     }
   }
   const bool prior = prior_out != nullptr;
+  vtts_engine::Staging& sd = h->stg[vtts_engine::STG_ST_DURATIONS];     // (downloaded inside the text phase's graph)
+  sd.begin();
+  sd.add(h->d_sttd, 2 * (size_t)Ttok + B);
+  sd.commit();
   if (pieces) {
     vtts_engine::Staging& sg = h->stg[vtts_engine::STG_ST_PIECES];
     sg.begin();
@@ -4920,17 +4964,17 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
     h->run_graphed({vtts_engine::TAG_ST_TEXT, B, h->maxTok, Ttok, prior ? 1 : 0}, [&] { h->stt_enqueue(prior); });
   }
   CK(cudaStreamSynchronize(h->stream));            // the one wait of the path: the frame counts size the mel phase
-  const int* back = reinterpret_cast<const int*>(h->h_pin_sttd.p);
+  const int* sttd = sd.host(h->d_sttd);
   std::vector<int> frames(B), extents(B);
   int64_t total = 0;
   for (int b = 0; b < B; ++b) {
-    frames[b] = back[2 * (size_t)Ttok + b];
+    frames[b] = sttd[2 * (size_t)Ttok + b];
     extents[b] = (frames[b] + 3) / 4 * 4;
     mel_lengths[b] = frames[b];
     total += extents[b];
     if (durations) {
       std::fill(durations + (size_t)b * t_max, durations + (size_t)(b + 1) * t_max, 0);
-      memcpy(durations + (size_t)b * t_max, back + h->h_tok_off[b], (size_t)h->h_tok_len[b] * sizeof(int));
+      memcpy(durations + (size_t)b * t_max, sttd + h->h_tok_off[b], (size_t)h->h_tok_len[b] * sizeof(int));
     }
   }
   REQUIRE(total < (1LL << 24), VTTS_ERR_INVALID, "the batch expands to too many frames for one call");
@@ -4960,19 +5004,20 @@ static void impl_stabletts_synthesise(vtts_handle h, const int64_t* ids, const i
                      h->voc_enqueue(in, lens, offs);
                    }
                  });
-  const size_t plane = (size_t)h->Tfrm * NC, nread = prior ? plane + (size_t)h->real_Tfrm * NC : (size_t)h->real_Tfrm * NC;
-  const size_t wcap = wav ? (size_t)h->Tfrm * h->hop : 0;
-  float* pin = reinterpret_cast<float*>(h->ensure_pinned((2 * plane + wcap) * sizeof(float) + 64));
-  if (mel_out || prior) CK(cudaMemcpyAsync(pin, h->d_stmel.p, nread * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (wav) CK(cudaMemcpyAsync(pin + 2 * plane, h->d_wav.p, (size_t)h->real_Tfrm * h->hop * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaEventRecord(h->ev[7], h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  // d_stmel holds the mel plane [Tfrm][NC], then with `prior` the prior's
+  const size_t plane = (size_t)h->Tfrm * NC;
+  vtts_engine::Staging& so = h->stg[vtts_engine::STG_OUT];
+  so.begin();
+  if (mel_out || prior) so.add(h->d_stmel, (prior ? plane : 0) + (size_t)h->real_Tfrm * NC, 0, 2 * plane);
+  if (wav) so.add(h->d_wav, (size_t)h->real_Tfrm * h->hop, 0, (size_t)h->Tfrm * h->hop);
+  so.commit();
+  so.download_and_wait();
   for (int b = 0; b < B; ++b) {
     const size_t o = (size_t)h->h_frm_off[b] * NC, nb = (size_t)frames[b] * NC * sizeof(float);
-    if (mel_out) memcpy(mel_out + (size_t)b * mel_ld * NC, pin + o, nb);
-    if (prior) memcpy(prior_out + (size_t)b * mel_ld * NC, pin + plane + o, nb);
+    if (mel_out) memcpy(mel_out + (size_t)b * mel_ld * NC, so.host(h->d_stmel) + o, nb);
+    if (prior) memcpy(prior_out + (size_t)b * mel_ld * NC, so.host(h->d_stmel) + plane + o, nb);
     if (wav) {
-      memcpy(wav + (size_t)b * wav_ld, pin + 2 * plane + (size_t)h->h_frm_off[b] * h->hop, (size_t)frames[b] * h->hop * sizeof(float));
+      memcpy(wav + (size_t)b * wav_ld, so.host(h->d_wav) + (size_t)h->h_frm_off[b] * h->hop, (size_t)frames[b] * h->hop * sizeof(float));
       wav_lengths[b] = (int64_t)frames[b] * h->hop;
     }
   }
@@ -5031,7 +5076,8 @@ static void impl_hifigan_vocode(vtts_handle h, const float* mel, const int64_t* 
     st.upload();
     h->voc_enqueue(dm, di, di + B);
   });
-  read_clips(h, (const float*)h->d_wav.p, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop, h->h_frm_off.data(), frames, h->hop, wav, wav_ld);
+  read_clips(read_back(h, h->d_wav, (size_t)h->real_Tfrm * h->hop, (size_t)h->Tfrm * h->hop), h->h_frm_off.data(), frames, h->hop, wav,
+             wav_ld);
   for (int b = 0; b < B; ++b) wav_lengths[b] = (int64_t)frames[b] * h->hop;
 }
 
@@ -5154,9 +5200,12 @@ static void impl_resample(vtts_handle h, const float* wav, const int64_t* length
                (const int*)(di + 2 * B), B, de);
     CK(cudaGetLastError());
     ++h->launches;
-    double* pe = reinterpret_cast<double*>(h->ensure(h->h_pin_rse, (size_t)e_off[B] * sizeof(double)));
-    CK(cudaMemcpyAsync(pe, de, (size_t)e_off[B] * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    vtts_engine::Staging& se = h->stg[vtts_engine::STG_TRIM];
+    se.begin();
+    se.add(h->d_rse, (size_t)e_off[B]);
+    se.commit();
+    se.download_and_wait();
+    const double* pe = se.host(h->d_rse);
     const double amin = 1e-10, thr = -(double)trim_top_db;
     for (int b = 0; b < B; ++b) {
       const double* e = pe + e_off[b];
@@ -5185,7 +5234,7 @@ static void impl_resample(vtts_handle h, const float* wav, const int64_t* length
   // clip's trailing silence)
   const int lo = keep_off[0], hi = keep_off[B - 1] + keep_len[B - 1];
   for (int& o : keep_off) o -= lo;
-  read_clips(h, y + lo, (size_t)(hi - lo), (size_t)(hi - lo), keep_off.data(), keep_len, 1, out, out_ld);
+  read_clips(read_back(h, same ? h->d_rsin : h->d_rsout, (size_t)(hi - lo), 0, (size_t)lo), keep_off.data(), keep_len, 1, out, out_ld);
   for (int b = 0; b < B; ++b) out_lengths[b] = keep_len[b];
 }
 
@@ -5212,7 +5261,7 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
   if (!cfg || !blob || !manifest || !out) return VTTS_ERR_INVALID;
   *out = nullptr;
   vtts_engine* h = new vtts_engine();
-  for (vtts_engine::Staging& s : h->stg) s.e = h;
+  for (int k = 0; k < vtts_engine::STG_KINDS; ++k) { h->stg[k].e = h; h->stg[k].readback = k >= vtts_engine::STG_OUT; }
   h->cfg = *cfg;
   h->device = device;
   *out = h;   // returned even on failure so that vtts_last_error() is readable; caller destroys it
@@ -5441,10 +5490,7 @@ int vtts_decode_chunk(vtts_handle h, int f0, int f1, float* wav, int64_t wav_cap
     h->last_graphed = false;
     h->decode(h->d_z.p, r);
     const size_t n = (size_t)(f1 - f0) * h->hop;
-    float* pw = reinterpret_cast<float*>(h->ensure_pinned(n * sizeof(float)));
-    CK(cudaMemcpyAsync(pw, h->d_wav.p + (size_t)f0 * h->hop, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(wav, pw, n * sizeof(float));
+    memcpy(wav, read_back(h, h->d_wav, n, 0, (size_t)f0 * h->hop), n * sizeof(float));
   });
 }
 
