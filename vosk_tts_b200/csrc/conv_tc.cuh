@@ -565,19 +565,18 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
           }
         }
         cluster_sync_all();                                  // (2) all partials have landed; nobody writes into a CTA after this point
-#pragma unroll
-        for (int jn = 0; jn < BN / 8; ++jn) {
-          const int cc = jn * 8 + 2 * q4;
-          if (cc / W != sp) continue;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float v0 = 0.f, v1 = 0.f;
-            for (int src = 0; src < T.s; ++src) {
-              const float2 p2 = *reinterpret_cast<const float2*>(stage + ((size_t)src * TC_BM + rbase + 8 * h) * W + (cc - sp * W));
-              v0 += p2.x; v1 += p2.y;
-            }
-            if (rowok[h]) tc_epi_pair(P, b, orow[h], co0 + cc, v0, v1, tb.dbgskip);
+        // The owner's column pairs (cw, cw + 1) of rows rbase and rbase + 8, summed in rank order.  A loop that is not unrolled,
+        // so the epilogue is one copy of its code: unrolled over the tile's BN/8 x 2 pairs it ran once per CTA from a cold
+        // instruction cache and cost 6-12 us of every split-K launch (CTA 0 stamps, tools/decoder_phases.py).
+#pragma unroll 1
+        for (int u = 0; u < W / 4; ++u) {
+          const int cw = 2 * q4 + 8 * (u >> 1), row = rbase + 8 * (u & 1), t = T.t0 + row;
+          float v0 = 0.f, v1 = 0.f;
+          for (int src = 0; src < T.s; ++src) {
+            const float2 p2 = *reinterpret_cast<const float2*>(stage + ((size_t)src * TC_BM + row) * W + cw);
+            v0 += p2.x; v1 += p2.y;
           }
+          if (t < L) tc_epi_pair(P, b, out_base + (long)t * P.out_mul + P.out_add, co0 + sp * W + cw, v0, v1, tb.dbgskip);
         }
       }
     }
