@@ -77,7 +77,8 @@ typedef struct vtts_config {
    * 2 = StableTTS (weights.pack_stabletts_cfm: the flow-matching decoder, which serves vtts_cfm_decode; weights.pack_stabletts:
    * the text encoder as well, which also serves vtts_stabletts_synthesise).  The entry points of one family return
    * VTTS_ERR_INVALID on an engine of another.  3 = GPT-SoVITS text-to-semantic decoder (weights.pack_t2s), which serves
-   * vtts_t2s_decode. */
+   * vtts_t2s_decode.  4 = GPT-SoVITS SoVITS (weights.pack_sovits: HuBERT, ssl_proj and the quantizer's codebook), which
+   * serves vtts_sovits_semantic and vtts_sovits_latent. */
   int32_t model_family;
   /* StableTTS flow-matching decoder (model_family 2; CFM of training/stabletts/matcha/models/components/flow_matching.py:301,
    * weights.pack_stabletts_cfm): vtts_cfm_decode.  The other families leave these 0. */
@@ -103,13 +104,16 @@ typedef struct vtts_config {
    * bt.emb.word / .pos / .type.
    * In GPT-SoVITS text-to-semantic engines (model_family 3) they describe the GPT's post-LN layers: cv_layers (n_layer),
    * cv_hidden (hidden_dim = embedding_dim), cv_heads (head), cv_ffn (4 hidden_dim) and cv_ln_eps (1e-5); the phone and semantic
-   * vocabularies and the positions are the rows of the blob's t2s.temb / t2s.aemb / t2s.pe. */
+   * vocabularies and the positions are the rows of the blob's t2s.temb / t2s.aemb / t2s.pe.
+   * In GPT-SoVITS SoVITS engines (model_family 4) they describe chinese-hubert-base (a HubertModel of ContentVec's shape), and
+   * n_vocab is the entry count of the quantizer's codebook (1024): the semantic tokens' vocabulary. */
 } vtts_config;
 
 #define VTTS_FAMILY_VITS2 0
 #define VTTS_FAMILY_QUICKVC 1
 #define VTTS_FAMILY_STABLETTS 2
 #define VTTS_FAMILY_T2S 3
+#define VTTS_FAMILY_SOVITS 4
 
 /* Replaces onnxruntime.InferenceSession(model.onnx) (vosk_tts/model.py:46).
  * `blob` holds the packed fp32 tensors produced by vosk_tts_b200.weights.pack(); `manifest` is a
@@ -701,6 +705,28 @@ int vtts_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* lengths, i
 int vtts_debug_t2s_sample(vtts_handle h, int B, const float* logits, int32_t* state, int32_t* y, int y_ld, int top_k, float top_p,
                           float temperature, float repetition_penalty, int early_stop_num, int step_cap, const uint64_t* seeds,
                           const float* q, int q_ld, uint32_t* seen, int32_t* n_stopped, float* raw, int raw_ld);
+
+/* GPT-SoVITS prompt tokens (model_family 4): a reference recording's semantic codes, as inference_cli.py:176-200 computes
+ * them with chinese-hubert-base and SynthesizerTrn.extract_latent (module/models.py:990-993).
+ *   wav        float [B, wav_ld] at 16 kHz, clip b = its first wav_lengths[b] samples, already padded by the caller (the
+ *              reference appends int(0.3 * the s2 config's sampling_rate) zeros); no normalisation
+ *   codes      out int64 [B, codes_ld]: clip b's frames / 2 codes (frames: HuBERT's frames of the clip), -1 after them
+ *   out_frames out int64 [B]: the code counts
+ * HuBERT runs as vtts_content_units runs ContentVec (fp32 FFMA in mode 0, split-bf16 tensor cores in modes >= 1), with every
+ * launch in one shape whatever the batch; ssl_proj (Conv1d(768, 768, 2, stride 2): an odd last frame is dropped), the
+ * codebook scores 2 x.E - |E|^2 and their argmax (lowest index on ties) are fp32 FFMA in every mode.  A clip's codes are
+ * bit-identical alone and in any batch.  Host pointers, atomic on the handle; one graphed call keyed by batch and
+ * sample-length bucket.  VTTS_ERR_INVALID: not a SoVITS engine, B < 1, a clip too short for one HuBERT frame or longer than
+ * wav_ld.  VTTS_ERR_CAPACITY: codes_ld below a clip's code count.
+ * After a call, vtts_debug_read "sv_proj" is ssl_proj's output rows [pairs][cv_hidden]: clip 0's codes' rows from row 0,
+ * clip b's from sum over earlier clips of ceil(frames / 2). */
+int vtts_sovits_semantic(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, int64_t* codes,
+                         int64_t codes_ld, int64_t* out_frames);
+/* The same tail on the caller's HuBERT rows (extract_latent of a stored last_hidden_state, as
+ * prepare_datasets/3-get-semantic-vosk.py runs it): feats float [B, feats_ld, cv_hidden] frame-major, clip b = its first
+ * frames[b] rows (0 allowed).  codes / out_frames as vtts_sovits_semantic. */
+int vtts_sovits_latent(vtts_handle h, const float* feats, const int64_t* frames, int B, int64_t feats_ld, int64_t* codes,
+                       int64_t codes_ld, int64_t* out_frames);
 
 /* Monotonic Alignment Search on the GPU -- replaces monotonic_align.maximum_path (training/vits2/monotonic_align/__init__.py:6-22,
  * core.pyx:7-43; called from SynthesizerTrn.forward, models.py:1658).  Handle-free (no engine state); errors of these two are

@@ -438,3 +438,36 @@ def t2s_config(model, sd=None):
             raise ValueError("linear1 must be [4 hidden_dim, hidden_dim] (dim_feedforward = 4 hidden_dim)")
     return {"model_family": "t2s", "cv_layers": L, "cv_hidden": H, "cv_heads": nh, "cv_ffn": 4 * H, "cv_ln_eps": 1e-5,
             "t2s_vocab": V, "t2s_phone_vocab": PV, "t2s_positions": T2S_MAX_POSITIONS}
+
+
+# GPT-SoVITS SoVITS (SynthesizerTrn of training/gpt-sovits/module/models.py): what inference_cli.py:164-200 runs on a reference
+# recording before text-to-semantic decoding.  The prompt's length limits are at 16 kHz (inference_cli.py:182).
+SOVITS_PROMPT_MIN, SOVITS_PROMPT_MAX = 48000, 320000
+SOVITS_PROMPT_MESSAGE = "Prompt audio length must be longer than 3 seconds and shorter than 20 seconds!"
+
+
+def sovits_pad(sampling_rate):
+    """Zeros appended to a 16 kHz prompt: int(hps.data.sampling_rate * 0.3) (inference_cli.py:176-192), counted at the s2
+    model's rate although the samples they follow are at 16 kHz."""
+    return int(sampling_rate * 0.3)
+
+
+def sovits_config(s2_config, hubert_config=None, codebook=1024):
+    """The engine's GPT-SoVITS SoVITS shape, model_family "sovits": the cv_* fields of the HuBERT (contentvec_config of its
+    config.json, with its refusals; None: chinese-hubert-base's shape, HubertConfig's defaults), the quantizer's codebook
+    entries (sv_codebook), and from the s2 config.json (path or dict) its data.sampling_rate and the prompt pad it implies."""
+    src = s2_config
+    if not isinstance(src, dict):
+        with open(s2_config) as f:
+            src = json.load(f)
+    data = src.get("data") if isinstance(src, dict) else None
+    if not isinstance(data, dict) or "sampling_rate" not in data:
+        raise ValueError("the s2 config has no data.sampling_rate")
+    sr = int(data["sampling_rate"])
+    if sr <= 0:
+        raise ValueError("data.sampling_rate must be positive (got %d)" % sr)
+    if int(codebook) < 1 or int(codebook) > 65536:
+        raise ValueError("the codebook must hold 1 to 65536 entries (got %d)" % int(codebook))
+    out = {"model_family": "sovits", "sampling_rate": sr, "sovits_pad": sovits_pad(sr), "sv_codebook": int(codebook)}
+    out.update(contentvec_config(hubert_config))
+    return out

@@ -30,6 +30,7 @@
 #include "vc.cuh"
 #include "spk.cuh"
 #include "contentvec.cuh"
+#include "sovits.cuh"
 #include "bert.cuh"
 #include "dit.cuh"
 #include "stabletts.cuh"
@@ -517,6 +518,7 @@ struct vtts_engine {
     STG_CONTENTVEC, STG_BERT, STG_ST_TEXT, STG_ST_PIECES, STG_ST_MEL, STG_VOCODER, STG_RESAMPLE, STG_T2S,
     STG_SPK_SLICES,   // the speaker encoder's slice table
     STG_CHUNK,        // the rows of vtts_decode_chunk
+    STG_SOVITS,       // the SoVITS tail's row tables, and the caller's HuBERT rows (vtts_sovits_latent)
     STG_OUT,          // readbacks from here on: a call's outputs
     STG_LENGTHS,      // phase 1's frame lengths and offsets without polling (copied inside its graph)
     STG_T2S_STOP0, STG_T2S_STOP1,   // T2S's count of stopped utterances after an even / odd chunk (two chunks in flight)
@@ -537,7 +539,7 @@ struct vtts_engine {
   enum GraphTag : long long {
     TAG_PHASE1 = 0x11, TAG_PHASE2 = 0x22, TAG_PHASE1_DEV = 0x33, TAG_PHASE2_DEV = 0x44, TAG_CONVERT = 0x55, TAG_ALIGN = 0x66,
     TAG_QUICKVC = 0x77, TAG_QUICKVC_WAV = 0x78, TAG_CONTENTVEC = 0xC7, TAG_CFM = 0xCF, TAG_ST_TEXT = 0xD1, TAG_ST_MEL = 0xD2, TAG_HIFIGAN = 0xD3,
-    TAG_BERT = 0xD4, TAG_ST_TEXT_PIECES = 0xD5, TAG_T2S = 0xE1
+    TAG_BERT = 0xD4, TAG_ST_TEXT_PIECES = 0xD5, TAG_T2S = 0xE1, TAG_SOVITS = 0xE2, TAG_SOVITS_LATENT = 0xE3
   };
   template <typename Fn>
   void run_graphed(std::initializer_list<long long> key_il, Fn&& enqueue) {
@@ -830,7 +832,7 @@ struct vtts_engine {
   Buf<float> d_cvzero, d_cvwav, d_cvps, d_cvpq, d_cvl[2], d_cvx, d_cvx1, d_cvy, d_cvqkv, d_cvao, d_cvff, d_cvu, d_cvdbg;
   void bind_contentvec();
   std::vector<int> cv_stage(const float* wav, const int64_t* lengths, int64_t ld);
-  void cv_enqueue(float* out, const int* out_offs);
+  void cv_enqueue(float* out, const int* out_offs, bool fixed = false);
   // The post-LN transformer layers ContentVec and BERT share, and the launches they are made of: work buffers xa (the input
   // rows, whose planes are PX), xb, Y, QKV, AO, FF and, on the tensor cores, the planes of every GEMM operand
   struct PostLnWs { float *xa, *xb, *Y, *QKV, *AO, *FF; Planes PX, PQKV, PAO, PX1, PFF; };
@@ -841,6 +843,21 @@ struct vtts_engine {
                const Rows& r);
   void gelu_rows(float* y, int C, const Planes* pl, const Rows& r);
   void gemm_rows(const Planes& in, const TcW& w, const ConvW& cw, float* y, const float* res, const Planes* out, const Rows& r);
+
+  // ---- SoVITS (SynthesizerTrn of GPT-SoVITS module/models.py; sovits.cuh): HuBERT rows -> 25 Hz semantic codes.  HuBERT is
+  //      the ContentVec above (cv.*); ssl_proj (k = 2, stride 2) is a 1x1 conv over pair rows, the codebook scores a 1x1 conv
+  //      (weight 2E, bias -|E|^2), both fp32 FFMA in every mode, then sv_argmax_kernel.
+  ConvW sv_proj, sv_score;
+  int sv_K = 0;                                    // codebook entries
+  // shape of the current call: B clips, pairs_cap the pair rows the buffers hold (a function of the graph key), maxP the
+  // launch's pair rows per clip, h the int table [HuBERT row offsets][pair counts][pair offsets] x B.  Clip b's HuBERT rows
+  // start at row 2 q_b, q_b = sum over earlier clips of ceil(frames / 2), so its pair rows (2 frames each) start at q_b.
+  struct SvPlan { int pairs_cap = 0, maxP = 0; std::vector<int> h, frames; } svp;
+  Buf<int> d_svi, d_svcodes;
+  Buf<float> d_svfeat, d_svproj, d_svscore;
+  void bind_sovits();
+  void sv_stage(const std::vector<int>& frames, int pairs_cap, int maxP, const float* feats = nullptr, int64_t feats_ld = 0);
+  void sv_enqueue(bool from_wav);
 
   // ---- BERT (transformers' BertModel as bert-export.py exports it; bert.cuh): word pieces -> the hidden rows of the last
   //      layer that runs, in StableTTS engines whose blob carries bt.*.  Described by the cv_* fields of vtts_config.
@@ -3064,12 +3081,15 @@ std::vector<int> vtts_engine::cv_stage(const float* wav, const int64_t* lengths,
 // GELU epilogue), LayerNorm + projection, the grouped positional conv (two launches of half the taps each: the tile halo of
 // conv_kernel), LayerNorm(x + gelu(pos)), then the post-LN transformer layers.  The last LayerNorm writes frame t of clip b
 // to out row out_offs[b] + t (out_offs null: the frame level's own offsets).
-void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
+void vtts_engine::cv_enqueue(float* out, const int* out_offs, bool fixed) {
   const vtts_config& c = cfg;
   const int NL = c.cv_n_conv, C = c.cv_conv_dim, H = c.cv_hidden, Fh = c.cv_ffn, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
   // Tensor-core GEMMs without split-K and attention on attn_tc_kernel (Tuning::fixed_tc): a clip's units are then the same
   // alone and in any batch.
-  const Tuning tn = cv_tc ? tune.fixed_tc() : tune;
+  // fixed: every launch in one shape whatever the batch (FFMA convs without split-K, one attention kernel), so that a clip's
+  // rows are bit-identical alone and in any batch (SoVITS, whose codes are an argmax of them).
+  const Tuning tn = fixed ? (cv_tc ? tune.fixed_ffma().fixed_attention().fixed_tc() : tune.fixed_ffma().fixed_attention())
+                          : (cv_tc ? tune.fixed_tc() : tune);
   int* di = ensure(d_cvi, cvp.nint);
   float* dw = ensure(d_cvwav, (size_t)cvp.tot0 * s0 + K0);
   stg[STG_CONTENTVEC].upload();
@@ -3134,6 +3154,73 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs) {
   ln_rows(X, Y, LnW{cv_enc_g, cv_enc_b}, c.cv_ln_eps, X1, Of, H, cv_tc ? &w.PX : nullptr, rf);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_cvdbg, Tf * H), X1, Tf * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   post_ln_layers(cv_enc, cv_tc, H, Fh, c.cv_ln_eps, w, out, out_offs ? out_offs : Of, rf);
+}
+
+// SoVITS: ContentVec's tensors (shared binding), then ssl_proj and the codebook scores.
+void vtts_engine::bind_sovits() {
+  const vtts_config& c = cfg;
+  bind_contentvec();
+  REQUIRE(has_cv, VTTS_ERR_WEIGHTS, "the weight blob has no HuBERT (cv.*): pack it with weights.pack_sovits");
+  const int H = c.cv_hidden;
+  sv_K = c.n_vocab;                                // (the codebook's entries: the semantic tokens' vocabulary)
+  REQUIRE(sv_K >= 1 && sv_K <= (1 << 16), VTTS_ERR_INVALID, "the codebook (n_vocab) must hold 1 to 65536 entries");
+  sv_proj = conv("sv.proj", 2 * H, H, 1);
+  sv_score = conv("sv.score", H, sv_K, 1);
+}
+
+// Host side of the SoVITS tail: clip b's frames[b] HuBERT rows at row 2 q_b, its frames[b] / 2 pair rows at q_b (an odd last
+// frame is dropped, as ssl_proj's stride-2 conv drops it).  feats (vtts_sovits_latent): the caller's rows [B][feats_ld][H],
+// staged into those rows; without it ContentVec writes them.
+void vtts_engine::sv_stage(const std::vector<int>& frames, int pairs_cap, int maxP, const float* feats, int64_t feats_ld) {
+  const int H = cfg.cv_hidden;
+  svp.pairs_cap = pairs_cap;
+  svp.maxP = maxP;
+  svp.frames = frames;
+  std::vector<int>& h = svp.h;
+  h.assign(3 * B, 0);
+  int q = 0;
+  for (int b = 0; b < B; ++b) {
+    h[b] = 2 * q;
+    h[B + b] = frames[b] / 2;
+    h[2 * B + b] = q;
+    q += (frames[b] + 1) / 2;
+  }
+  REQUIRE(q <= pairs_cap, VTTS_ERR_STATE, "SoVITS pair rows exceed their buffers");
+  Staging& s = stg[STG_SOVITS];
+  s.begin();
+  s.add(d_svi, 3 * B);
+  if (feats) s.add(d_svfeat, (size_t)2 * pairs_cap * H);
+  s.commit();
+  memcpy(s.host(d_svi), h.data(), h.size() * sizeof(int));
+  if (feats) {
+    float* pf = s.host(d_svfeat);
+    for (int b = 0; b < B; ++b)
+      memcpy(pf + (size_t)h[b] * H, feats + (size_t)b * feats_ld * H, (size_t)frames[b] * H * sizeof(float));
+  }
+}
+
+// The SoVITS tail of the staged clips (sv_stage), after ContentVec of the clips staged by cv_stage when from_wav:
+// proj = ssl_proj(pairs), scores = 2 proj.E - |E|^2, codes = the row argmax.  Each output is summed in one order whatever the
+// batch (Tuning::fixed_ffma), so a clip's codes are the same alone and in any batch.
+void vtts_engine::sv_enqueue(bool from_wav) {
+  const int H = cfg.cv_hidden, K = sv_K;
+  const size_t P = (size_t)svp.pairs_cap;
+  int* di = ensure(d_svi, (size_t)3 * B);
+  float* feat = ensure(d_svfeat, 2 * P * H);
+  stg[STG_SOVITS].upload();
+  if (from_wav) cv_enqueue(feat, di, true);
+  float* proj = ensure(d_svproj, P * H);
+  float* score = ensure(d_svscore, P * K);
+  int* codes = ensure(d_svcodes, P);
+  std::vector<int> real(B);
+  for (int b = 0; b < B; ++b) real[b] = svp.h[B + b];
+  const Rows r{di + B, di + 2 * B, B, svp.maxP, std::vector<int>(B, svp.maxP), real, tune.fixed_ffma()};
+  launch_conv({mk(sv_proj, feat, 2 * H, 0, proj, H, 0, 1, 0)}, 1, r);
+  launch_conv({mk(sv_score, proj, H, 0, score, K, 0, 1, 0)}, 1, r);
+  klaunch(sv_argmax_kernel, dim3((std::max(svp.maxP, 1) + SVA_WARPS - 1) / SVA_WARPS, B), dim3(32 * SVA_WARPS), (size_t)0,
+          (const float*)score, K, (const int*)(di + B), (const int*)(di + 2 * B), codes);
+  CK(cudaGetLastError());
+  ++launches;
 }
 
 // LayerNorm of the rows r (cv_ln_kernel): out = LN(a + gelu(y)) (y null: LN(a)), rows read at r.offs, written at out_offs.
@@ -3995,7 +4082,7 @@ int guarded(vtts_handle h, Fn fn, int mode = G_ATOMIC, int family = VTTS_FAMILY_
   if (!h) return VTTS_ERR_INVALID;
   std::unique_lock<std::mutex> lk(h->mu);
   if (family != ANY_FAMILY && h->cfg.model_family != family) {
-    static const char* const names[] = {"VITS2", "QuickVC", "StableTTS", "GPT-SoVITS text-to-semantic"};
+    static const char* const names[] = {"VITS2", "QuickVC", "StableTTS", "GPT-SoVITS text-to-semantic", "GPT-SoVITS SoVITS"};
     h->err = std::string("this entry point serves ") + names[family] + " models; the engine holds a " + names[h->cfg.model_family] + " model";
     return VTTS_ERR_INVALID;
   }
@@ -4456,6 +4543,46 @@ static void impl_content_units(vtts_handle h, const float* wav, const int64_t* l
   for (int b = 0; b < B; ++b) {
     std::fill(units + ((size_t)b * units_ld + frames[b]) * H, units + (size_t)(b + 1) * units_ld * H, 0.f);
     out_frames[b] = frames[b];
+  }
+}
+
+// SoVITS semantic codes through host buffers (vtts_sovits_semantic / vtts_sovits_latent): stages the tail, runs it (after
+// ContentVec of wav when given) as one graphed phase, and reads each clip's frames / 2 codes back, -1 after them.
+static void impl_sovits(vtts_handle h, const float* wav, const float* feats, const int64_t* lengths, int B, int64_t ld,
+                        int64_t* codes, int64_t codes_ld, int64_t* out_frames) {
+  REQUIRE(B >= 1 && B <= 16384, VTTS_ERR_INVALID, "bad batch size");
+  REQUIRE(ld >= 1 && codes_ld >= 0, VTTS_ERR_INVALID, "bad wav_ld / feats_ld / codes_ld");
+  h->B = B;
+  std::vector<int> frames(B);
+  std::vector<long long> key;
+  int pairs_cap = 0, maxP = 0;
+  if (wav) {
+    frames = h->cv_stage(wav, lengths, ld);
+    const int NL = h->cfg.cv_n_conv;
+    // HuBERT's frame rows of the key's layer-0 rows bound every clip's pair rows (frames + 1 <= its padded rows / cv_P)
+    pairs_cap = (h->cvp.tot0 / h->cv_P + 1) / 2;
+    maxP = h->cvp.maxL[NL - 1] / 2;
+    key = {vtts_engine::TAG_SOVITS, B, h->cvp.maxS, h->cvp.tot0};
+  } else {
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(lengths[b] >= 0 && lengths[b] <= ld, VTTS_ERR_INVALID, "frames must be in [0, feats_ld]");
+      frames[b] = (int)lengths[b];
+      pairs_cap += (frames[b] + 1) / 2;
+      maxP = std::max(maxP, frames[b] / 2);
+    }
+    pairs_cap = std::max(pairs_cap, 1);
+    key = {vtts_engine::TAG_SOVITS_LATENT, B, maxP, pairs_cap};
+  }
+  for (int b = 0; b < B; ++b) REQUIRE(frames[b] / 2 <= codes_ld, VTTS_ERR_CAPACITY, "codes_ld is smaller than a clip's code count");
+  h->sv_stage(frames, pairs_cap, maxP, feats, ld);
+  const bool from_wav = wav != nullptr;
+  h->run_graphed({key[0], key[1], key[2], key[3]}, [&] { h->sv_enqueue(from_wav); });
+  const int* rows = read_back(h, h->d_svcodes, (size_t)pairs_cap);
+  for (int b = 0; b < B; ++b) {
+    const int n = frames[b] / 2, off = h->svp.h[2 * B + b];
+    for (int t = 0; t < n; ++t) codes[(size_t)b * codes_ld + t] = rows[off + t];
+    for (int64_t t = n; t < codes_ld; ++t) codes[(size_t)b * codes_ld + t] = -1;
+    out_frames[b] = n;
   }
 }
 
@@ -5326,9 +5453,10 @@ int vtts_create(const vtts_config* cfg, const float* blob, size_t blob_floats, c
     if (const char* e = getenv("VTTS_SPEC_MARGIN")) h->spec_margin = (float)atof(e);      // (< 1 forces mispredictions: tests)
     if (const char* e = getenv("VTTS_CAPTURE_FIRST")) h->capture_on_first = atoi(e) != 0;   // 0: capture a bucket's graph on its second call          // 0: never enqueue phase 2 before the lengths are known    // 0: size everything by the exact lengths
     if (const char* e = getenv("VTTS_PREFETCH")) h->use_prefetch = atoi(e) != 0;
-    REQUIRE(cfg->model_family >= VTTS_FAMILY_VITS2 && cfg->model_family <= VTTS_FAMILY_T2S, VTTS_ERR_INVALID, "unknown model family");
+    REQUIRE(cfg->model_family >= VTTS_FAMILY_VITS2 && cfg->model_family <= VTTS_FAMILY_SOVITS, VTTS_ERR_INVALID, "unknown model family");
     if (cfg->model_family == VTTS_FAMILY_QUICKVC) h->bind_quickvc();
     else if (cfg->model_family == VTTS_FAMILY_T2S) h->bind_t2s();
+    else if (cfg->model_family == VTTS_FAMILY_SOVITS) h->bind_sovits();
     else if (cfg->model_family == VTTS_FAMILY_STABLETTS) {
       h->bind_stabletts();
       h->bind_bert();
@@ -5684,6 +5812,7 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     else if (nm == "st_mu_dp") { src = h->d_stmudp.p; n = T * c.st_dur_channels; }
     else if (nm == "st_logw") { src = h->d_stlogw.p; n = T; }
     else if (nm == "cv_enc_in") { src = h->d_cvdbg.p; n = (size_t)h->cvp.tot0 / h->cv_P * c.cv_hidden; }
+    else if (nm == "sv_proj") { src = h->d_svproj.p; n = (size_t)h->svp.pairs_cap * c.cv_hidden; }
     else if (nm.rfind("stage", 0) == 0) {
       const int i = atoi(nm.c_str() + 5);
       REQUIRE(i >= 0 && i < (int)h->d_stage.size(), VTTS_ERR_INVALID, "no such stage");
@@ -5698,6 +5827,20 @@ int vtts_debug_read(vtts_handle h, const char* name, float* out, size_t max_floa
     CK(cudaStreamSynchronize(h->stream));
     *n_out = n;
   }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_sovits_semantic(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, int64_t* codes,
+                         int64_t codes_ld, int64_t* out_frames) {
+  if (!wav || !wav_lengths || !codes || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_sovits(h, wav, nullptr, wav_lengths, B, wav_ld, codes, codes_ld, out_frames); }, G_ATOMIC,
+                 VTTS_FAMILY_SOVITS);
+}
+
+int vtts_sovits_latent(vtts_handle h, const float* feats, const int64_t* frames, int B, int64_t feats_ld, int64_t* codes,
+                       int64_t codes_ld, int64_t* out_frames) {
+  if (!feats || !frames || !codes || !out_frames) return VTTS_ERR_INVALID;
+  return guarded(h, [&] { impl_sovits(h, nullptr, feats, frames, B, feats_ld, codes, codes_ld, out_frames); }, G_ATOMIC,
+                 VTTS_FAMILY_SOVITS);
 }
 
 int vtts_speaker_embedding(vtts_handle h, const float* wav, const int64_t* wav_lengths, int B, int64_t wav_ld, float* g_out) {

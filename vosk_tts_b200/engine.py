@@ -65,9 +65,10 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
            "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
            "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode",
-           "vtts_debug_t2s_sample", "vtts_debug_front_end", "vtts_debug_istft", "vtts_debug_mrf_mean"]
+           "vtts_debug_t2s_sample", "vtts_debug_front_end", "vtts_debug_istft", "vtts_debug_mrf_mean",
+           "vtts_sovits_semantic", "vtts_sovits_latent"]
 
-MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3}    # vtts_config.model_family
+MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3, "sovits": 4}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
 
 CONV_KEEP = -1000000     # VTTS_CONV_KEEP: leave a launch-shape setting at the engine's value
@@ -283,6 +284,9 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_t2s_sample.argtypes = [vp, i32, vp, vp, vp, i32, i32, C.c_float, C.c_float, C.c_float, i32, i32, vp, vp, i32, vp, vp,
                                           vp, i32]
     lib.vtts_debug_t2s_sample.restype = i32
+    for fn in (lib.vtts_sovits_semantic, lib.vtts_sovits_latent):
+        fn.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64, vp]
+        fn.restype = i32
     _LIB = lib
     return lib
 
@@ -339,6 +343,12 @@ def make_c_config(cfg, precision=0):
             setattr(c, k, int(cfg[k]))
         c.cv_ln_eps = float(cfg["cv_ln_eps"])
         return c
+    if cfg.get("model_family") == "sovits":            # config.sovits_config: the HuBERT in the cv_* fields, the codebook in n_vocab
+        c.model_family = MODEL_FAMILIES["sovits"]
+        c.precision = int(precision)
+        _set_contentvec_shape(c, cfg)
+        c.n_vocab = int(cfg["sv_codebook"])
+        return c
     if cfg.get("model_family") == "stabletts":        # the flow-matching decoder reads none of the VITS2 fields
         c.model_family = MODEL_FAMILIES["stabletts"]
         c.precision = int(precision)
@@ -390,13 +400,18 @@ def make_c_config(cfg, precision=0):
     c.model_family = MODEL_FAMILIES[cfg.get("model_family", "vits2")]
     cv = cfg.get("contentvec")
     if cv:
-        for k in ("cv_layers", "cv_hidden", "cv_heads", "cv_ffn", "cv_conv_dim", "cv_pos_k", "cv_pos_groups"):
-            setattr(c, k, int(cv[k]))
-        c.cv_n_conv = len(cv["cv_conv_kernel"])
-        for i, (k, s) in enumerate(zip(cv["cv_conv_kernel"], cv["cv_conv_stride"])):
-            c.cv_conv_kernel[i], c.cv_conv_stride[i] = int(k), int(s)
-        c.cv_ln_eps, c.cv_gn_eps = float(cv["cv_ln_eps"]), float(cv["cv_gn_eps"])
+        _set_contentvec_shape(c, cv)
     return c
+
+
+def _set_contentvec_shape(c, cv):
+    """The cv_* fields of a HuBERT / ContentVec shape (config.contentvec_config)."""
+    for k in ("cv_layers", "cv_hidden", "cv_heads", "cv_ffn", "cv_conv_dim", "cv_pos_k", "cv_pos_groups"):
+        setattr(c, k, int(cv[k]))
+    c.cv_n_conv = len(cv["cv_conv_kernel"])
+    for i, (k, s) in enumerate(zip(cv["cv_conv_kernel"], cv["cv_conv_stride"])):
+        c.cv_conv_kernel[i], c.cv_conv_stride[i] = int(k), int(s)
+    c.cv_ln_eps, c.cv_gn_eps = float(cv["cv_ln_eps"]), float(cv["cv_gn_eps"])
 
 
 def _ptr(a):
@@ -976,6 +991,44 @@ class Engine:
                                              _ptr(lg), logits_steps))
         out = [tokens[b, :n[b]].copy() for b in range(B)]
         return (out, idx, lg) if lg is not None else (out, idx)
+
+    # ---- GPT-SoVITS prompt tokens (HuBERT and SynthesizerTrn.extract_latent); cfg is config.sovits_config
+    def sovits_semantic(self, wav, lengths=None):
+        """Semantic codes of 16 kHz recordings, already padded (vtts_sovits_semantic): wav [L], [B, L] with `lengths`, or a list
+        of ragged clips.  Returns (codes int64 [B, max n], -1 after each clip's codes; n int64 [B], HuBERT's frames // 2)."""
+        wav, lengths = _batch(wav, lengths, 2, ragged=True)
+        B = wav.shape[0]
+        T = max(1, max(_config.contentvec_frames(int(n), self.cfg) // 2 for n in lengths))
+        codes = np.zeros((B, T), np.int64)
+        n = np.zeros(B, np.int64)
+        self._check(self.lib.vtts_sovits_semantic(self.h, _ptr(wav), _ptr(lengths), B, wav.shape[1], _ptr(codes), T, _ptr(n)))
+        return codes, n
+
+    def sovits_latent(self, feats, frames=None):
+        """Semantic codes of HuBERT rows (vtts_sovits_latent): feats frame-major [T, hidden], [B, T, hidden] with `frames`, or a
+        list of ragged [T_b, hidden] clips.  Returns (codes int64 [B, max T // 2], -1 after each clip's codes; n int64 [B])."""
+        H = int(self.cfg["cv_hidden"])
+        if isinstance(feats, (list, tuple)):
+            items = [np.asarray(f, np.float32).reshape(-1, H) for f in feats]
+            frames = np.array([f.shape[0] for f in items], np.int64)
+            x = np.zeros((len(items), max(1, int(frames.max())), H), np.float32)
+            for b, f in enumerate(items):
+                x[b, :f.shape[0]] = f
+        else:
+            x = np.ascontiguousarray(feats, dtype=np.float32)
+            if x.ndim == 2:
+                x = x[None]
+            if x.ndim != 3 or x.shape[2] != H:
+                raise ValueError("feats must be [T, %d], [B, T, %d] or a list of [T_b, %d]" % (H, H, H))
+            B = x.shape[0]
+            frames = np.full(B, x.shape[1], np.int64) if frames is None else \
+                np.ascontiguousarray(np.broadcast_to(np.asarray(frames, np.int64).reshape(-1), (B,)))
+        B = x.shape[0]
+        T = max(1, int(frames.max()) // 2)
+        codes = np.zeros((B, T), np.int64)
+        n = np.zeros(B, np.int64)
+        self._check(self.lib.vtts_sovits_latent(self.h, _ptr(x), _ptr(frames), B, x.shape[1], _ptr(codes), T, _ptr(n)))
+        return codes, n
 
     def resample(self, wav, from_rate, to_rate, lengths=None, trim_top_db=None, return_bounds=False):
         """Clips at `from_rate` Hz resampled to `to_rate` Hz (vtts_resample: scipy.signal.resample_poly's filter, not soxr), and

@@ -1,5 +1,6 @@
-"""GPT-SoVITS text-to-semantic decoding on the GPU: the reference's Text2SemanticDecoder.infer_panel
-(training/gpt-sovits/ar/models/t2s_model.py:324-448) behind its own signature, and a ragged batch of sentences in one call."""
+"""GPT-SoVITS on the GPU.  Text-to-semantic decoding: the reference's Text2SemanticDecoder.infer_panel
+(training/gpt-sovits/ar/models/t2s_model.py:324-448) behind its own signature, and a ragged batch of sentences in one call (Text2Semantic).  The prompt's tokens of a reference
+recording: HuBERT and SynthesizerTrn.extract_latent (SemanticEncoder)."""
 import numpy as np
 
 from . import config as _config
@@ -45,3 +46,54 @@ class Text2Semantic:
         return self.engine.t2s_decode(phones_list, prompts, bert, top_k=top_k, top_p=top_p, temperature=temperature,
                                       repetition_penalty=repetition_penalty, early_stop_num=early_stop_num, step_cap=step_cap,
                                       seeds=seeds, q=q)
+
+
+class SemanticEncoder:
+    """The prompt's semantic tokens of GPT-SoVITS on the GPU: chinese-hubert-base over a reference recording, then the s2
+    model's SynthesizerTrn.extract_latent (inference_cli.py:176-200, module/models.py:990-993), whose codes prompt
+    Text2Semantic.decode.  sovits_checkpoint: an s2 G_*.pth (either layout weights.load_sovits reads, with its config.json as
+    `config`) or (state dict, config.sovits_config).  hubert: a chinese-hubert-base directory (weights.load_contentvec) or
+    (state dict, config.contentvec_config).  precision 0 runs HuBERT on the fp32 FFMA pipe; >= 1 its GEMMs and attention on
+    the split-bf16 tensor cores.  ssl_proj, the codebook scores and their argmax are fp32 in every mode."""
+
+    def __init__(self, sovits_checkpoint, hubert, config=None, device=0, precision=1):
+        hsd, hcv = _weights.load_contentvec(hubert) if isinstance(hubert, str) else hubert
+        if isinstance(sovits_checkpoint, str):
+            if config is None:
+                raise ValueError("an s2 checkpoint path needs its config.json (config=...): the prompt pad comes from its sampling_rate")
+            sd, cfg = _weights.load_sovits(sovits_checkpoint, config)
+        else:
+            sd, cfg = sovits_checkpoint
+        cfg = dict(cfg)
+        cfg.update(hcv)
+        self.cfg = cfg
+        blob, manifest = _weights.pack_sovits(sd, cfg, hsd, tc=precision >= 1)
+        self.engine = Engine(cfg, blob, manifest, device=device, precision=precision)
+
+    def close(self):
+        self.engine.close()
+
+    def extract_latent(self, ssl_content):
+        """SynthesizerTrn.extract_latent: HuBERT's last_hidden_state float [B, 768, T] -> int64 codes [B, 1, T // 2]."""
+        x = np.asarray(ssl_content, np.float32)
+        if x.ndim != 3:
+            raise ValueError("ssl_content must be [B, %d, T]" % int(self.cfg["cv_hidden"]))
+        codes, _ = self.engine.sovits_latent(np.ascontiguousarray(x.transpose(0, 2, 1)))
+        return codes[:, None, : x.shape[2] // 2]
+
+    def prompts(self, wavs, sampling_rate=None):
+        """Recordings -> their prompt tokens, one int64 array each, ready for Text2Semantic.decode(prompts=...).  wavs: a list of
+        1-D float recordings at `sampling_rate` Hz (None: 16 kHz), resampled to 16 kHz on the GPU (Engine.resample) when
+        another rate is given.  As inference_cli.py:180-192: a recording of fewer than 48000 or more than 320000 samples at
+        16 kHz is refused, then int(0.3 * the s2 config's sampling_rate) zeros are appended.  One engine call per batch."""
+        wavs = [np.asarray(w, np.float32).reshape(-1) for w in wavs]
+        if not wavs:
+            return []
+        if sampling_rate is not None and int(sampling_rate) != 16000:
+            wavs = self.engine.resample(wavs, int(sampling_rate), 16000)
+        for w in wavs:
+            if w.size > _config.SOVITS_PROMPT_MAX or w.size < _config.SOVITS_PROMPT_MIN:
+                raise ValueError(_config.SOVITS_PROMPT_MESSAGE)
+        pad = np.zeros(int(self.cfg["sovits_pad"]), np.float32)
+        codes, n = self.engine.sovits_semantic([np.concatenate([w, pad]) for w in wavs])
+        return [codes[b, : n[b]].copy() for b in range(len(wavs))]

@@ -470,3 +470,37 @@ def make_random_t2s(cfg, seed=1234, eos_scale=1.0):
             sd[w + "_weight"], sd[w + "_bias"] = sd.pop(w + ".weight"), sd.pop(w + ".bias")
     sd["ar_predict_layer.weight"][V - 1] *= eos_scale
     return sd
+
+
+def make_random_sovits(hubert, rows=None, seed=2525, codebook=1024, spacing=12):
+    """The tensors of a GPT-SoVITS s2 checkpoint that the prompt's codes read (weights.load_sovits's state dict), seeded, for a
+    HuBERT state dict `hubert` (make_random_contentvec): ssl_proj = Conv1d(768, 768, 2, stride 2) with PyTorch's default
+    init scale and a bias on a 1/8 grid (a zero feature row then projects to exactly representable values), and a codebook
+    drawn where projected speech lies, so that speech uses many codes (a codebook drawn without regard to it picks the few
+    codewords of smallest norm).  rows [N, 768], HuBERT's rows of some recordings: codeword k < (N - 1) // spacing is ssl_proj
+    of the rows (k spacing, k spacing + 1) plus noise of 1e-3 of the codewords' spread (rows `spacing` apart, so that
+    neighbouring codewords are told apart by more than the rounding of an fp32 HuBERT).  The other codewords (all of them
+    without rows) are ssl_proj of rows gamma * n + beta, n zero-mean unit-variance over the channels and gamma / beta the
+    encoder's last LayerNorm affine.  inited = 1: the codebook is trained."""
+    H = int(np.asarray(hubert["encoder.layer_norm.weight"]).shape[0])
+    r = np.random.default_rng(seed)
+    w = r.uniform(-1, 1, (H, H, 2)) / math.sqrt(2 * H)
+    b = np.round(r.normal(0, 0.1, H) * 8) / 8
+    last = "encoder.layers.%d.final_layer_norm." % (sum(1 for k in hubert if k.endswith(".final_layer_norm.weight")) - 1)
+    gamma = np.asarray(hubert[last + "weight"], np.float64)
+    beta = np.asarray(hubert[last + "bias"], np.float64)
+    z = r.standard_normal((2, codebook, H))
+    z = (z - z.mean(2, keepdims=True)) / z.std(2, keepdims=True)
+    x0, x1 = gamma * z[0] + beta, gamma * z[1] + beta
+    n = 0
+    if rows is not None:
+        rows = np.asarray(rows, np.float64)
+        n = min(codebook, (rows.shape[0] - 1) // spacing)
+        i = np.arange(n) * spacing
+        x0[:n], x1[:n] = rows[i], rows[i + 1]
+    E = x0 @ w[:, :, 0].T + x1 @ w[:, :, 1].T + b
+    if n:
+        E[:n] += 1e-3 * E[:n].std(0) * r.standard_normal((n, H))
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float32))
+    return {"ssl_proj.weight": t(w), "ssl_proj.bias": t(b), "quantizer.vq.layers.0._codebook.embed": t(E),
+            "quantizer.vq.layers.0._codebook.inited": torch.ones(1)}

@@ -1087,3 +1087,67 @@ def pack_t2s(sd, cfg, tc=True):
         P.add("t2s.l%d.ln2.g" % l, want(p + "norm2.weight", (H,)))
         P.add("t2s.l%d.ln2.b" % l, want(p + "norm2.bias", (H,)))
     return P.finish()
+
+
+SV_PROJ = "ssl_proj."
+SV_CODEBOOK = "quantizer.vq.layers.0._codebook."
+
+
+def load_sovits(path, config_json, hubert_config=None):
+    """The tensors of a GPT-SoVITS s2 checkpoint (SynthesizerTrn, module/models.py) that the prompt's semantic codes need ->
+    (fp32 state dict of ssl_proj.* and the codebook's embed / inited, config.sovits_config).  Both layouts the reference writes
+    are read: `{"model": ...}` (utils.save_checkpoint, as inference_cli.py:65-81 loads it) and `{"weight": ...}` (the
+    pretrained s2G488k.pth, as s2_train.py:239 loads it).  The file is read with the restricted unpickler of
+    load_lightning_state_dict: a hyper-parameter object stored beside the weights loads as an inert placeholder, and
+    nothing the file names is imported or called.  The sampling rate comes from the s2 config.json; hubert_config: the
+    HuBERT's config.json (None: chinese-hubert-base's shape)."""
+    ck = torch.load(path, map_location="cpu", weights_only=False, pickle_module=_state_dict_pickle_module())
+    sd = None
+    if isinstance(ck, dict):
+        sd = ck.get("model") if isinstance(ck.get("model"), dict) else ck.get("weight")
+    if not isinstance(sd, dict):
+        raise ValueError("%s holds neither `model` (utils.save_checkpoint) nor `weight` (s2G488k.pth) state dict" % path)
+    keep = (SV_PROJ + "weight", SV_PROJ + "bias", SV_CODEBOOK + "embed", SV_CODEBOOK + "inited")
+    for k in keep:
+        if not isinstance(sd.get(k), torch.Tensor):
+            raise ValueError("%s has no tensor %s" % (path, k))
+    sd = {k: sd[k].float() for k in keep}
+    return sd, _config.sovits_config(config_json, hubert_config, int(sd[SV_CODEBOOK + "embed"].shape[0]))
+
+
+def check_sovits(sd, cfg):
+    """Refuses, with the reason, an s2 state dict the engine does not compute: a 50 Hz ssl_proj ([768, 768, 1]), a codebook
+    that is not [K, hidden], a codebook EuclideanCodebook never initialised (inited 0: the reference's first forward would
+    overwrite it with a k-means of its input)."""
+    g = lambda k: sd[k].detach().cpu().float().numpy() if hasattr(sd[k], "detach") else np.asarray(sd[k], np.float32)
+    H = int(cfg["cv_hidden"])
+    w = g(SV_PROJ + "weight")
+    if w.shape == (H, H, 1):
+        raise ValueError("ssl_proj is Conv1d(%d, %d, 1): a 50 Hz model (semantic_frame_rate \"50hz\"); only 25 Hz models "
+                         "(Conv1d(%d, %d, 2, stride=2), which inference_cli.py loads) are supported" % (H, H, H, H))
+    if w.shape != (H, H, 2) or g(SV_PROJ + "bias").shape != (H,):
+        raise ValueError("ssl_proj.weight has shape %s, expected %s" % (w.shape, (H, H, 2)))
+    E = g(SV_CODEBOOK + "embed")
+    if E.ndim != 2 or E.shape[1] != H or E.shape[0] < 1:
+        raise ValueError("the codebook %sembed has shape %s, expected [K, %d]" % (SV_CODEBOOK, E.shape, H))
+    if E.shape[0] != int(cfg["sv_codebook"]):
+        raise ValueError("the codebook holds %d entries, the config sv_codebook %d" % (E.shape[0], cfg["sv_codebook"]))
+    if not np.all(g(SV_CODEBOOK + "inited") != 0):
+        raise ValueError("the codebook was never initialised (%sinited is 0): the checkpoint's codebook is untrained" % SV_CODEBOOK)
+    return w, g(SV_PROJ + "bias"), E
+
+
+def pack_sovits(sd, cfg, hubert, tc=True):
+    """s2 tensors (load_sovits) and the HuBERT state dict (load_contentvec; config.sovits_config's cv_* fields describe it) ->
+    (blob, manifest) of a model_family "sovits" engine: the cv.* tensors of _pack_contentvec, then sv.proj (ssl_proj's two taps
+    as a 1x1 conv over pair rows [frame 2t | frame 2t + 1], tap-major, as _pack_contentvec lays out the feature encoder) and
+    sv.score (weight 2E, bias -|E|^2: argmax_k of x.2E_k - |E_k|^2 is EuclideanCodebook.quantize's argmax of -|x - E_k|^2).
+    tc: also HuBERT's split-bf16 copies, which precision modes >= 1 read."""
+    w, b, E = check_sovits(sd, cfg)
+    P = _Packer()
+    _pack_contentvec(P, fold_contentvec_pos_conv(hubert) if CV_POS + "weight" not in hubert else hubert, cfg, tc)
+    H = w.shape[0]
+    P.conv("sv.proj", np.transpose(w, (0, 2, 1)).reshape(H, 2 * H)[:, :, None], b)
+    E64 = E.astype(np.float64)
+    P.conv("sv.score", (2.0 * E)[:, :, None], -(E64 * E64).sum(1))
+    return P.finish()
