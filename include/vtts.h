@@ -377,6 +377,46 @@ int vtts_debug_istft(vtts_handle h, int B, const int* lens, int first, size_t ro
  * row rmul * offs[b] + b, and the mean into out [rows][C] (in/out) unless NULL. */
 int vtts_debug_mrf_mean(vtts_handle h, int use_tc, int B, const int* lens, int rmul, int C, int n, size_t rows, const float* x,
                         int last, float* out, size_t plane_rows, uint16_t* hi, uint16_t* lo);
+/* Unit-test hooks of the normalisation kernels: each runs the launch helper the model families run, on caller rows packed as
+ * the duration hooks pack them (utterance b: lens[b] rows from the sum of the earlier lengths).  Outputs are in/out: rows
+ * outside the utterances keep what the caller passed.  Planes hi / mid / lo are split-bf16 bit patterns at the pitch of the
+ * fp32 rows they split, given together (mid only with hi and lo) or NULL; where a kernel writes no planes they are unused.
+ * vtts_debug_add_ln: add_ln_kernel, out [rows][C] = LayerNorm(a + b) * g + beta (+ cadd) (+ vec row b [B][vec_ld]), eps 1e-5,
+ * rows a, b, cadd [rows][C]; b, cadd and vec may be NULL.  mid given: the exact 3-way split.  32 <= C <= 256, C % 32 == 0. */
+int vtts_debug_add_ln(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* a, const float* b, const float* g,
+                      const float* beta, const float* cadd, const float* vec, int vec_ld, float* out, uint16_t* hi, uint16_t* mid,
+                      uint16_t* lo);
+/* vtts_debug_ln: cv_ln_kernel (ln_rows), out row out_offs[b] + t [out_rows][C] = LayerNorm(a + gelu(y)) * g + beta (y NULL:
+ * LayerNorm(a)) of input row t of utterance b, a and y [rows][C].  1 <= C <= 1024. */
+int vtts_debug_ln(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* a, const float* y, const float* g, const float* beta,
+                  float eps, const int* out_offs, size_t out_rows, float* out, uint16_t* hi, uint16_t* lo);
+/* vtts_debug_bert_embed: bert_embed_kernel, out [rows][C] = LayerNorm((word[ids[row]] + type0) + pos[t]) * g + beta, t counted
+ * from the sentence's first row; tables word [V][C], pos [P][C], type0 [C].  Refuses ids outside [0, V), sentences longer
+ * than P and C outside 1..1024. */
+int vtts_debug_bert_embed(vtts_handle h, int B, const int* lens, size_t rows, int C, const int* ids, int V, const float* word, int P,
+                          const float* pos, const float* type0, const float* g, const float* beta, float eps, float* out, uint16_t* hi,
+                          uint16_t* lo);
+/* vtts_debug_dit_norm: dit_norm_kernel (hi, lo NULL) or dit_norm_planes_kernel (the planes of no).  v = a (rows of pitch lda >=
+ * C), FiLM'd (film [2C] = gamma | beta: gamma v + beta) unless film is NULL, plus gate * y (y [rows][C]) unless y is NULL ->
+ * xo [rows][C]; no [rows][C] = LayerNorm(v) * (1 + scale) + shift, eps 1e-5.  gate / shift / scale: C columns from gate_off
+ * / shift_off / scale_off of utterance b's row of ada [B][ada_ld].  1 <= C <= 512. */
+int vtts_debug_dit_norm(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* a, int lda, const float* film, const float* y,
+                        const float* ada, int ada_ld, int gate_off, int shift_off, int scale_off, float* xo, float* no, uint16_t* hi,
+                        uint16_t* lo);
+/* vtts_debug_act: the activation passes on y [rows][C].  act 0: cv_gelu_kernel (erf GELU), in place, or only into the planes
+ * when hi / lo are given (y unchanged).  act 1: dit_silu_kernel in place, or dit_silu_planes_kernel, in place and into the
+ * planes. */
+int vtts_debug_act(vtts_handle h, int act, int B, const int* lens, size_t rows, int C, float* y, uint16_t* hi, uint16_t* lo);
+/* vtts_debug_gate: dit_gate_kernel (hi, lo NULL) or dit_gate_planes_kernel: out rows of pitch ldo >= C [rows][ldo] (and their
+ * planes, same pitch) = x + gate * y, x and y [rows][C], gate: C columns from gate_off of utterance b's row of ada [B][ada_ld]. */
+int vtts_debug_gate(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* x, const float* y, const float* ada, int ada_ld,
+                    int gate_off, float* out, int ldo, uint16_t* hi, uint16_t* lo);
+/* vtts_debug_groupnorm (engines holding ContentVec / HuBERT): the clips wav [B][ld] of lengths[b] samples, staged as
+ * vtts_content_units stages them with NaN behind every clip, then the feature encoder's layer 0 + GroupNorm + GELU (the three
+ * cv_gn_kernel passes) with the loaded weights -> out [rows][cv_conv_dim] (in/out): clip b's len0[b] rows from row off0[b].
+ * rows must hold the staged layer-0 rows. */
+int vtts_debug_groupnorm(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, size_t rows, float* out, int32_t* len0,
+                         int32_t* off0);
 /* The split-K plan the engine makes for one grouped tensor-core conv launch, computed on the host alone (no device, no
  * engine).  Problems p < n (1..4): cin[p] (a multiple of 64), cout[p], k[p], in_extra[p]; B utterances of lens[b] <= max_len
  * rows / rmul; bn 64 / 128 pins the tile width (0: either); max_split caps the cluster size (8: none); min_steps = k-steps

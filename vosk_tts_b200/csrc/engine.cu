@@ -726,6 +726,10 @@ struct vtts_engine {
   void launch_conv(const std::vector<ConvP>& ps, int rmul, const Rows& r);
   void encoder_layer(const EncLayerW& L, float*& x, float*& xb, float* qkv, float* ao, float* y, float* ffh, int Hc, int Fc,
                      int ks, const float* vec_after, int vec_ld, const float* cadd_after, const Rows& r);
+  // out = LN(a + b) * w.g + w.b (+ cadd) (+ the utterance's vec row) of the rows r (add_ln_kernel); pl (or null): also the planes
+  // of out, hi / lo, and mid when pl->mid is set
+  void add_ln(const float* a, const float* b, const LnW& w, const float* cadd, const float* vec, int vec_ld, float* out, int C,
+              const Planes* pl, const Rows& r);
   void dds_stack(const DdsW* d, int C, int k, float*& a, float*& b, const Rows& r,
                  const float* x0 = nullptr, const float* pre_w = nullptr, const float* pre_b = nullptr, const float* cond = nullptr);
   void dds_layer(const DdsW& d, int C, int k, int dil, const float* x, float* y, const Rows& r,
@@ -842,6 +846,9 @@ struct vtts_engine {
   void ln_rows(const float* a, const float* y, const LnW& w, float eps, float* out, const int* out_offs, int C, const Planes* pl,
                const Rows& r);
   void gelu_rows(float* y, int C, const Planes* pl, const Rows& r);
+  // Layer 0 + GroupNorm + GELU of the clips cv_stage staged (wav, and the int table di) into their layer-0 rows out: the three
+  // cv_gn_kernel passes, with the chunk sums in ps and pq
+  void cv_layer0(const float* wav, const int* di, float* ps, float* pq, float* out);
   void gemm_rows(const Planes& in, const TcW& w, const ConvW& cw, float* y, const float* res, const Planes* out, const Rows& r);
 
   // ---- SoVITS (SynthesizerTrn of GPT-SoVITS module/models.py; sovits.cuh): HuBERT rows -> 25 Hz semantic codes.  HuBERT is
@@ -873,6 +880,10 @@ struct vtts_engine {
   void bind_bert();
   void bt_stage(const int64_t* ids, const int64_t* lengths, int64_t ld);
   void bt_enqueue(float* out);
+  // LN((word[id] + type0) + pos[t]) of the word pieces ids, one per row of r, t counted from each sentence's start, into out
+  // (bert_embed_kernel); pl (or null): also their planes
+  void bt_embed(const int* ids, const float* word, const float* pos, const float* type0, const LnW& ln, float eps, float* out, int C,
+                const Planes* pl, const Rows& r);
 
   // ---- GPT-SoVITS text-to-semantic decoder (Text2SemanticDecoder.infer_panel; t2s.cuh, DESIGN.md 4.s): the text rows'
   //      prefill on post_ln_layers, then one-token decode steps on the t2s_* kernels, graphed T2S_CHUNK steps at a time
@@ -946,6 +957,15 @@ struct vtts_engine {
   // the same block in precision mode 2 (stp_tc, stpl); xout_pl: the planes of xout's column block, or null
   void st_block_tc(const StBlk& k, const EncLayerW& L, int l, const float* film, const float* xin, int ldi, float* xout, int ldo,
                    const Planes* xout_pl, bool tap, const Rows& r);
+  // The blocks' row launches over the rows r.  dit_norm: v = FiLM(a rows of pitch lda) (+ gate * y) -> xo, no = LN(v) *
+  // (1 + scale) + shift, gate / shift / scale at those offsets of the sequence's ada row (dit_norm_kernel; pl: also the
+  // planes of no, dit_norm_planes_kernel).  silu_rows: y = silu(y) in place (and its planes).  gate_rows: out = x + gate * y,
+  // out rows (and their planes) of pitch ldo.
+  void dit_norm(const float* a, int lda, const float* film, const float* y, const float* ada, int ada_ld, int gate_off, int shift_off,
+                int scale_off, float* xo, float* no, const Planes* pl, int C, const Rows& r);
+  void silu_rows(float* y, int C, const Planes* pl, const Rows& r);
+  void gate_rows(const float* x, const float* y, const float* ada, int ada_ld, int gate_off, float* out, int ldo, const Planes* pl, int C,
+                 const Rows& r);
 
   // ---- StableTTS text encoder and durations (TextEncoder.forward, MatchaTTS.synthesise; stabletts.cuh): blobs of
   // weights.pack_stabletts.  Stack 0 is the mel encoder (conditioned on spk_emb), stack 1 dp_encoder (on dur_spk_emb).
@@ -1737,7 +1757,6 @@ void vtts_engine::flow_tc(float* z, bool emit_pz, const float* cond, int cond_ld
   float* fqkv = ensure(d_fqkv, (size_t)F * 3 * H);
   float* fao = ensure(d_fao, (size_t)F * H);
   Planes ph = flp.ph, pao = flp.pao, ph1 = flp.ph1, pff = flp.pff, pwx = flp.pwx, pacts = flp.pacts, pskip = flp.pskip, pqkv = flp.pqkv;
-  dim3 lg((r.maxLen + 3) / 4, r.n);
   for (int s = 0; s < nf; ++s) {
     const int f = forward ? s : nf - 1 - s;
     const FlowW& W = flow[f];
@@ -1763,18 +1782,14 @@ void vtts_engine::flow_tc(float* z, bool emit_pz, const float* cond, int cond_ld
       }
       { TcSpec q; q.in = pao; q.w = W.t_o; q.bias = W.tr.o.b; q.Cin = H; q.Cout = H; q.y = fy; q.ldy = H;
         launch_tc({q}, 1, r); }
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), h, fy, W.tr.ln1.g, W.tr.ln1.b, nullptr, nullptr, 0, h1, r.lens, r.offs, H, ph1.hi, ph1.lo, (__nv_bfloat16*)nullptr);
-      CK(cudaGetLastError());
-      ++launches;
+      add_ln(h, fy, W.tr.ln1, nullptr, nullptr, 0, h1, H, &ph1, r);
       { TcSpec q; q.in = ph1; q.w = W.t_ffn1; q.bias = W.tr.ffn1.b; q.Cin = H; q.Cout = H; q.k = fk; q.pad = (fk - 1) / 2;
         q.epi = TCE_RELU; q.out = pff; q.pl_slope = 1.f;
         launch_tc({q}, 1, r); }
       { TcSpec q; q.in = pff; q.w = W.t_ffn2; q.bias = W.tr.ffn2.b; q.Cin = H; q.Cout = H; q.k = fk; q.pad = (fk - 1) / 2;
         q.y = fy; q.ldy = H;
         launch_tc({q}, 1, r); }
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), h1, fy, W.tr.ln2.g, W.tr.ln2.b, h, nullptr, 0, wx, r.lens, r.offs, H, pwx.hi, pwx.lo, (__nv_bfloat16*)nullptr);
-      CK(cudaGetLastError());
-      ++launches;
+      add_ln(h1, fy, W.tr.ln2, h, nullptr, 0, wx, H, &pwx, r);
       wn_x = wx;
     }
     wn_tc(W.t_in, W.in, W.t_rsx, W.rsx, W.t_rss, W.rss, nl, fk, c.flow_dilation_rate, wn_x, skip, pwx, pacts, pskip,
@@ -2104,17 +2119,20 @@ void vtts_engine::encoder_layer(const EncLayerW& L, float*& x, float*& xb, float
   launch_conv({mk(L.qkv, x, Hc, 0, qkv, 3 * Hc, 0, 1, 0)}, 1, r);
   launch_attn(qkv, ao, L, Hc, nullptr, r);
   launch_conv({mk(L.o, ao, Hc, 0, y, Hc, 0, 1, 0)}, 1, r);
-  dim3 lg((r.maxLen + 3) / 4, r.n);
-  klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), x, y, L.ln1.g, L.ln1.b, nullptr, nullptr, 0, xb, r.lens, r.offs, Hc, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
-  CK(cudaGetLastError());
-  ++launches;
+  add_ln(x, y, L.ln1, nullptr, nullptr, 0, xb, Hc, nullptr, r);
   {
     ConvP p = mk(L.ffn1, xb, Hc, 0, ffh, Fc, 0, 1, (ks - 1) / 2);
     p.epi = EPI_RELU;
     launch_conv({p}, 1, r);
   }
   launch_conv({mk(L.ffn2, ffh, Fc, 0, y, Hc, 0, 1, (ks - 1) / 2)}, 1, r);
-  klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xb, y, L.ln2.g, L.ln2.b, cadd_after, vec_after, vec_ld, x, r.lens, r.offs, Hc, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
+  add_ln(xb, y, L.ln2, cadd_after, vec_after, vec_ld, x, Hc, nullptr, r);
+}
+
+void vtts_engine::add_ln(const float* a, const float* b, const LnW& w, const float* cadd, const float* vec, int vec_ld, float* out, int C,
+                         const Planes* pl, const Rows& r) {
+  klaunch(add_ln_kernel, dim3((r.maxLen + 3) / 4, r.n), dim3(128), (size_t)0, a, b, w.g, w.b, cadd, vec, vec_ld, out, r.lens, r.offs, C,
+          pl ? pl->hi : (__nv_bfloat16*)nullptr, pl ? pl->lo : (__nv_bfloat16*)nullptr, pl ? pl->mid : (__nv_bfloat16*)nullptr);
   CK(cudaGetLastError());
   ++launches;
 }
@@ -2303,7 +2321,6 @@ void vtts_engine::text_encoder(const float* cond, int cond_ld) {
     // precision mode 2: same layer with the four convs on wgmma (attentions.py:57-63)
     const EncLayerW& L = enc[i];
     const int ks = c.kernel_size;
-    dim3 lg((maxTok + 3) / 4, B);
     if (attn_use_tc(L, H, r)) {
       { TcSpec q; q.in = px; q.w = L.t_qkv; q.bias = L.qkv.b; q.Cin = H; q.Cout = 3 * H; q.out = pqkv; q.pl_slope = 1.f;
         launch_tc({q}, 1, r); }
@@ -2315,16 +2332,14 @@ void vtts_engine::text_encoder(const float* cond, int cond_ld) {
     }
     { TcSpec q; q.in = pao; q.w = L.t_o; q.bias = L.o.b; q.Cin = H; q.Cout = H; q.y = y; q.ldy = H;
       launch_tc({q}, 1, r); }
-    klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, x, y, L.ln1.g, L.ln1.b, (const float*)nullptr, (const float*)nullptr, 0, xb, tl, to, H, px1.hi, px1.lo, px1.mid);
-    ++launches;
+    add_ln(x, y, L.ln1, nullptr, nullptr, 0, xb, H, &px1, r);
     { TcSpec q; q.in = px1; q.w = L.t_ffn1; q.bias = L.ffn1.b; q.Cin = H; q.Cout = Fc; q.k = ks; q.pad = (ks - 1) / 2;
       q.epi = TCE_RELU; q.out = pff; q.pl_slope = 1.f;
       launch_tc({q}, 1, r); }
     { TcSpec q; q.in = pff; q.w = L.t_ffn2; q.bias = L.ffn2.b; q.Cin = Fc; q.Cout = H; q.k = ks; q.pad = (ks - 1) / 2;
       q.y = y; q.ldy = H;
       launch_tc({q}, 1, r); }
-    klaunch(add_ln_kernel, lg, dim3(128), (size_t)0, xb, y, L.ln2.g, L.ln2.b, (const float*)nullptr, va, cond_ld, x, tl, to, H, px.hi, px.lo, px.mid);
-    ++launches;
+    add_ln(xb, y, L.ln2, nullptr, va, cond_ld, x, H, &px, r);
   }
 }
 
@@ -2526,19 +2541,14 @@ void vtts_engine::flow_ffma(float* z, const float* cond, int cond_ld, bool forwa
       launch_conv({mk(W.tr.qkv, h, H, 0, fqkv, 3 * H, 0, 1, 0)}, 1, r);
       launch_attn(fqkv, fao, W.tr, H, nullptr, r);
       launch_conv({mk(W.tr.o, fao, H, 0, fy, H, 0, 1, 0)}, 1, r);
-      dim3 lg((r.maxLen + 3) / 4, r.n);
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xa, fy, W.tr.ln1.g, W.tr.ln1.b, nullptr, nullptr, 0, xb2, r.lens, r.offs, H, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
-      CK(cudaGetLastError());
-      ++launches;
+      add_ln(xa, fy, W.tr.ln1, nullptr, nullptr, 0, xb2, H, nullptr, r);
       {
         ConvP p = mk(W.tr.ffn1, xb2, H, 0, ffh2, H, 0, 1, (fk - 1) / 2);
         p.epi = EPI_RELU;
         launch_conv({p}, 1, r);
       }
       launch_conv({mk(W.tr.ffn2, ffh2, H, 0, fy, H, 0, 1, (fk - 1) / 2)}, 1, r);
-      klaunch(add_ln_kernel, dim3(lg), dim3(128), (size_t)(0), xb2, fy, W.tr.ln2.g, W.tr.ln2.b, h, nullptr, 0, wx, r.lens, r.offs, H, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
-      CK(cudaGetLastError());
-      ++launches;
+      add_ln(xb2, fy, W.tr.ln2, h, nullptr, 0, wx, H, nullptr, r);
       wn_in = wx;
     }
     // WN (modules.py:148-176).  The hidden state is updated in place in `wn_in`.
@@ -3095,23 +3105,13 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs, bool fixed) {
   stg[STG_CONTENTVEC].upload();
   auto Ls = [&](int l) -> const int* { return di + l * B; };
   auto Os = [&](int l) -> const int* { return di + (NL + l) * B; };
-  const int* woff = di + 2 * NL * B;
-  const float* mu = reinterpret_cast<const float*>(di + (2 * NL + 1) * B);
   // the rows of level l; the launch heuristics and the profiler see each clip at the level's bucket
   auto level = [&](int l) { return Rows{Ls(l), Os(l), B, cvp.maxL[l], std::vector<int>(B, cvp.maxL[l]), std::vector<int>(B, cvp.maxL[l]), tn}; };
   const size_t np = (size_t)B * cvp.MC * C;
   float* ps = ensure(d_cvps, np);
   float* pq = ensure(d_cvpq, np);
   float* lv[2] = {ensure(d_cvl[0], (size_t)cvp.tot0 * C), ensure(d_cvl[1], (size_t)cvp.tot0 / c.cv_conv_stride[1] * C)};
-  const dim3 gg(cvp.MC, B), gb(CVG_THREADS);
-  const size_t gsm = (size_t)((CVG_CH - 1) * s0 + K0) * sizeof(float);
-  klaunch(cv_gn_kernel<0>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
-  CK(cudaGetLastError());
-  klaunch(cv_gn_kernel<1>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
-  CK(cudaGetLastError());
-  klaunch(cv_gn_kernel<2>, gg, gb, gsm, (const float*)dw, mu, woff, Ls(0), Os(0), cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, lv[0]);
-  CK(cudaGetLastError());
-  launches += 3;
+  cv_layer0(dw, di, ps, pq, lv[0]);
   float* x = lv[0];
   for (int i = 1; i < NL; ++i) {
     float* y = lv[i & 1];
@@ -3154,6 +3154,22 @@ void vtts_engine::cv_enqueue(float* out, const int* out_offs, bool fixed) {
   ln_rows(X, Y, LnW{cv_enc_g, cv_enc_b}, c.cv_ln_eps, X1, Of, H, cv_tc ? &w.PX : nullptr, rf);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_cvdbg, Tf * H), X1, Tf * H * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   post_ln_layers(cv_enc, cv_tc, H, Fh, c.cv_ln_eps, w, out, out_offs ? out_offs : Of, rf);
+}
+
+void vtts_engine::cv_layer0(const float* wav, const int* di, float* ps, float* pq, float* out) {
+  const vtts_config& c = cfg;
+  const int NL = c.cv_n_conv, C = c.cv_conv_dim, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
+  const int *L0 = di, *O0 = di + NL * B, *woff = di + 2 * NL * B;
+  const float* mu = reinterpret_cast<const float*>(di + (2 * NL + 1) * B);
+  const dim3 gg(cvp.MC, B), gb(CVG_THREADS);
+  const size_t gsm = (size_t)((CVG_CH - 1) * s0 + K0) * sizeof(float);
+  klaunch(cv_gn_kernel<0>, gg, gb, gsm, wav, mu, woff, L0, O0, cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, out);
+  CK(cudaGetLastError());
+  klaunch(cv_gn_kernel<1>, gg, gb, gsm, wav, mu, woff, L0, O0, cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, out);
+  CK(cudaGetLastError());
+  klaunch(cv_gn_kernel<2>, gg, gb, gsm, wav, mu, woff, L0, O0, cv_w0, C, K0, s0, ps, pq, cvp.MC, cv_gn_g, cv_gn_b, c.cv_gn_eps, out);
+  CK(cudaGetLastError());
+  launches += 3;
 }
 
 // SoVITS: ContentVec's tensors (shared binding), then ssl_proj and the codebook scores.
@@ -3423,12 +3439,16 @@ void vtts_engine::bt_enqueue(float* out) {
     w.PX = planes(51, (long)T, 1, H); w.PQKV = planes(52, (long)T, 1, 3 * H);
     w.PAO = planes(53, (long)T, 1, H); w.PX1 = planes(54, (long)T, 1, H); w.PFF = planes(55, (long)T, 1, Fh);
   }
-  klaunch(bert_embed_kernel, dim3((btp.maxL + CVL_WARPS - 1) / CVL_WARPS, B), dim3(32 * CVL_WARPS), (size_t)0, (const int*)(di + 2 * B),
-          bt_word, bt_pos, bt_type, bt_ln.g, bt_ln.b, c.cv_ln_eps, w.xa, r.lens, r.offs, H, bt_tc ? w.PX.hi : (__nv_bfloat16*)nullptr,
-          bt_tc ? w.PX.lo : (__nv_bfloat16*)nullptr);
+  bt_embed(di + 2 * B, bt_word, bt_pos, bt_type, bt_ln, c.cv_ln_eps, w.xa, H, bt_tc ? &w.PX : nullptr, r);
+  post_ln_layers(bt_enc, bt_tc, H, Fh, c.cv_ln_eps, w, out, r.offs, r);
+}
+
+void vtts_engine::bt_embed(const int* ids, const float* word, const float* pos, const float* type0, const LnW& ln, float eps, float* out,
+                           int C, const Planes* pl, const Rows& r) {
+  klaunch(bert_embed_kernel, dim3((r.maxLen + CVL_WARPS - 1) / CVL_WARPS, r.n), dim3(32 * CVL_WARPS), (size_t)0, ids, word, pos, type0, ln.g,
+          ln.b, eps, out, r.lens, r.offs, C, pl ? pl->hi : (__nv_bfloat16*)nullptr, pl ? pl->lo : (__nv_bfloat16*)nullptr);
   CK(cudaGetLastError());
   ++launches;
-  post_ln_layers(bt_enc, bt_tc, H, Fh, c.cv_ln_eps, w, out, r.offs, r);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -3631,13 +3651,10 @@ void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const floa
                            const Rows& r) {
   const int H = k.H, F = k.F, dk = H / k.heads;
   const size_t T = (size_t)stp.Ttot;
-  const dim3 gs(r.maxLen, r.n), gn((r.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, r.n);
+  const dim3 gs(r.maxLen, r.n);
   const float* ada = k.ada + (size_t)l * 6 * H;
   auto norm = [&](const float* a, int lda, const float* fl, const float* y, int gate, int shift, int scale) {
-    klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f, k.Hb, k.N,
-            r.lens, r.offs, H);
-    CK(cudaGetLastError());
-    ++launches;
+    dit_norm(a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, k.Hb, k.N, nullptr, H, r);
   };
   auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy) {
     launch_conv({mk(W, x, ldx, 0, y, ldy, 0, 1, (W.k - 1) / 2)}, 1, r);
@@ -3653,11 +3670,39 @@ void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const floa
   cv(L.o, k.AO, H, k.Y, H);
   norm(k.Hb, H, nullptr, k.Y, 2, 3, 4);
   cv(L.ffn1, k.N, H, k.FF, F);
-  klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, k.FF, F, r.lens, r.offs);
+  silu_rows(k.FF, F, nullptr, r);
+  cv(L.ffn2, k.FF, F, k.Y, H);
+  gate_rows(k.Hb, k.Y, ada, k.ald, 5 * H, xout, ldo, nullptr, H, r);
+}
+
+void vtts_engine::dit_norm(const float* a, int lda, const float* film, const float* y, const float* ada, int ada_ld, int gate_off, int shift_off,
+                           int scale_off, float* xo, float* no, const Planes* pl, int C, const Rows& r) {
+  const dim3 gn((r.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, r.n);
+  if (pl)
+    klaunch(dit_norm_planes_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, film, y, ada, ada_ld, gate_off, shift_off, scale_off, 1e-5f,
+            xo, no, pl->hi, pl->lo, r.lens, r.offs, C);
+  else
+    klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, film, y, ada, ada_ld, gate_off, shift_off, scale_off, 1e-5f, xo, no,
+            r.lens, r.offs, C);
   CK(cudaGetLastError());
   ++launches;
-  cv(L.ffn2, k.FF, F, k.Y, H);
-  klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, r.lens, r.offs, H);
+}
+
+void vtts_engine::silu_rows(float* y, int C, const Planes* pl, const Rows& r) {
+  const dim3 gs(r.maxLen, r.n);
+  if (pl) klaunch(dit_silu_planes_kernel, gs, dim3(256), (size_t)0, y, C, pl->hi, pl->lo, r.lens, r.offs);
+  else klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, y, C, r.lens, r.offs);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::gate_rows(const float* x, const float* y, const float* ada, int ada_ld, int gate_off, float* out, int ldo, const Planes* pl, int C,
+                            const Rows& r) {
+  const dim3 gs(r.maxLen, r.n);
+  if (pl)
+    klaunch(dit_gate_planes_kernel, gs, dim3(128), (size_t)0, x, y, ada, ada_ld, gate_off, out, ldo, pl->hi, pl->lo, r.lens, r.offs, C);
+  else
+    klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, x, y, ada, ada_ld, gate_off, out, ldo, r.lens, r.offs, C);
   CK(cudaGetLastError());
   ++launches;
 }
@@ -3670,18 +3715,11 @@ void vtts_engine::st_block_tc(const StBlk& k, const EncLayerW& L, int l, const f
   const StPl& pl = stpl;
   const int H = k.H, F = k.F, dk = H / k.heads;
   const size_t T = (size_t)stp.Ttot;
-  const dim3 gs(r.maxLen, r.n), gn((r.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, r.n);
+  const dim3 gs(r.maxLen, r.n);
   const float* ada = k.ada + (size_t)l * 6 * H;
   const bool attn_tc = p.attn && attn_use_tc(L, H, r);
   auto norm = [&](const float* a, int lda, const float* fl, const float* y, int gate, int shift, int scale, bool planes) {
-    if (planes)
-      klaunch(dit_norm_planes_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f,
-              k.Hb, k.N, pl.N.hi, pl.N.lo, r.lens, r.offs, H);
-    else
-      klaunch(dit_norm_kernel, gn, dim3(32 * DIT_LN_WARPS), (size_t)0, a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, 1e-5f, k.Hb, k.N,
-              r.lens, r.offs, H);
-    CK(cudaGetLastError());
-    ++launches;
+    dit_norm(a, lda, fl, y, ada, k.ald, gate * H, shift * H, scale * H, k.Hb, k.N, planes ? &pl.N : nullptr, H, r);
   };
   // one conv of the block: on the tensor cores from the planes `in` when `tc`, else on the FFMA pipe from the fp32 rows x;
   // `out`: the planes of y its consumer reads (or null)
@@ -3719,23 +3757,12 @@ void vtts_engine::st_block_tc(const StBlk& k, const EncLayerW& L, int l, const f
   norm(k.Hb, H, nullptr, k.Y, 2, 3, 4, p.ffn1);
   cv(p.ffn1, L.ffn1, L.t_ffn1, pl.N, k.N, k.FF, nullptr);
   if (tap) st_tap("tc_silu_in", k.FF, (size_t)F * 4, (size_t)F * 4);
-  if (p.ffn2)
-    klaunch(dit_silu_planes_kernel, gs, dim3(256), (size_t)0, k.FF, F, pl.FF.hi, pl.FF.lo, r.lens, r.offs);
-  else
-    klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, k.FF, F, r.lens, r.offs);
-  CK(cudaGetLastError());
-  ++launches;
+  silu_rows(k.FF, F, p.ffn2 ? &pl.FF : nullptr, r);
   if (tap) st_tap("tc_silu", k.FF, (size_t)F * 4, (size_t)F * 4);
   if (tap && p.ffn2) st_tap_planes("tc_silu_hi", "tc_silu_lo", pl.FF, F, F);
   cv(p.ffn2, L.ffn2, L.t_ffn2, pl.FF, k.FF, k.Y, nullptr);
   if (tap) { st_tap("tc_gate_x", k.Hb, (size_t)H * 4, (size_t)H * 4); st_tap("tc_gate_y", k.Y, (size_t)H * 4, (size_t)H * 4); }
-  if (xout_pl)
-    klaunch(dit_gate_planes_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, xout_pl->hi,
-            xout_pl->lo, r.lens, r.offs, H);
-  else
-    klaunch(dit_gate_kernel, gs, dim3(128), (size_t)0, (const float*)k.Hb, (const float*)k.Y, ada, k.ald, 5 * H, xout, ldo, r.lens, r.offs, H);
-  CK(cudaGetLastError());
-  ++launches;
+  gate_rows(k.Hb, k.Y, ada, k.ald, 5 * H, xout, ldo, xout_pl, H, r);
   if (tap) st_tap("tc_gate", xout, (size_t)H * 4, (size_t)ldo * 4);
   if (tap && xout_pl) st_tap_planes("tc_gate_hi", "tc_gate_lo", *xout_pl, H, ldo);
 }
@@ -3796,11 +3823,7 @@ void vtts_engine::st_enqueue() {
   klaunch(dit_rope_table_kernel, dim3((maxFrm * (rd / 2) + 127) / 128), dim3(128), (size_t)0, rope, maxFrm, rd);
   CK(cudaGetLastError());
   launches += 4;
-  auto silu = [&](float* y, int width) {
-    klaunch(dit_silu_kernel, gs, dim3(256), (size_t)0, y, width, exts, offs);
-    CK(cudaGetLastError());
-    ++launches;
-  };
+  auto silu = [&](float* y, int width) { silu_rows(y, width, nullptr, re); };
   auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff, const Rows& r) {
     launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, r);
   };
@@ -3842,11 +3865,7 @@ void vtts_engine::st_enqueue() {
     if (out) { q.out = *out; q.poff = poff; }
     launch_tc({q}, 1, r);
   };
-  auto silu_pl = [&](float* y, int width, const Planes& pl) {
-    klaunch(dit_silu_planes_kernel, gs, dim3(256), (size_t)0, y, width, pl.hi, pl.lo, exts, offs);
-    CK(cudaGetLastError());
-    ++launches;
-  };
+  auto silu_pl = [&](float* y, int width, const Planes& pl) { silu_rows(y, width, &pl, re); };
   // cond_proj (decoder.py:121; not masked: zero padded at the ends of each sequence's extent) into the cond columns of the
   // in_proj operand
   if (!pt.on) {
@@ -6616,6 +6635,254 @@ int vtts_debug_mrf_mean(vtts_handle h, int use_tc, int B, const int* lens, int r
       CK(cudaMemcpy(hi, pl.hi, plane_rows * C * 2, cudaMemcpyDeviceToHost));
       CK(cudaMemcpy(lo, pl.lo, plane_rows * C * 2, cudaMemcpyDeviceToHost));
     }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+// ---- Unit-test hooks of the normalisation kernels (include/vtts.h): the engine's launch helpers on host rows.
+namespace {
+
+// The planes hi / lo (and mid) of a normalisation hook: both or neither of hi and lo, mid only with them.
+bool hook_planes(const char* who, uint16_t* hi, uint16_t* mid, uint16_t* lo) {
+  REQUIRE(!hi == !lo && (!mid || hi), VTTS_ERR_INVALID, std::string(who) + ": give hi and lo together (and mid only with them)");
+  return hi != nullptr;
+}
+
+// Device copies of the planes (n values each) of a hook; pl.hi stays null without them.
+Planes upload_planes(std::vector<Buf<char>>& dev, uint16_t* hi, uint16_t* mid, uint16_t* lo, size_t n, cudaStream_t st) {
+  Planes pl;
+  if (!hi) return pl;
+  pl.hi = static_cast<__nv_bfloat16*>(upload(dev, hi, n * 2, st));
+  pl.lo = static_cast<__nv_bfloat16*>(upload(dev, lo, n * 2, st));
+  if (mid) pl.mid = static_cast<__nv_bfloat16*>(upload(dev, mid, n * 2, st));
+  return pl;
+}
+
+}  // namespace
+
+int vtts_debug_add_ln(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* a, const float* b, const float* g,
+                      const float* beta, const float* cadd, const float* vec, int vec_ld, float* out, uint16_t* hi, uint16_t* mid,
+                      uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(a && g && beta && out, VTTS_ERR_INVALID, "debug_add_ln: missing input or output");
+    REQUIRE(C >= 32 && C <= 256 && C % 32 == 0, VTTS_ERR_INVALID, "debug_add_ln: add_ln_kernel needs C a multiple of 32, at most 256");
+    REQUIRE(!vec || vec_ld >= C, VTTS_ERR_INVALID, "debug_add_ln: vec_ld must be >= C");
+    const bool planes = hook_planes("debug_add_ln", hi, mid, lo);
+    HookRows hr = hook_rows("debug_add_ln", B, lens, rows);
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * C;
+    const float* da = static_cast<const float*>(upload(dev, a, n * 4, st));
+    const float* db = b ? static_cast<const float*>(upload(dev, b, n * 4, st)) : nullptr;
+    const float* dc = cadd ? static_cast<const float*>(upload(dev, cadd, n * 4, st)) : nullptr;
+    const float* dv = vec ? static_cast<const float*>(upload(dev, vec, (size_t)B * vec_ld * 4, st)) : nullptr;
+    const LnW w{static_cast<const float*>(upload(dev, g, C * 4, st)), static_cast<const float*>(upload(dev, beta, C * 4, st))};
+    float* dout = static_cast<float*>(upload(dev, out, n * 4, st));
+    const Planes pl = upload_planes(dev, hi, mid, lo, n, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->add_ln(da, db, w, dc, dv, vec_ld, dout, C, planes ? &pl : nullptr, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, n * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, n * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
+      if (mid) CK(cudaMemcpy(mid, pl.mid, n * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_ln(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* a, const float* y, const float* g, const float* beta,
+                  float eps, const int* out_offs, size_t out_rows, float* out, uint16_t* hi, uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(a && g && beta && out_offs && out, VTTS_ERR_INVALID, "debug_ln: missing input or output");
+    REQUIRE(C >= 1 && C <= 32 * CVL_MAXV, VTTS_ERR_INVALID, "debug_ln: cv_ln_kernel needs 1 <= C <= 1024");
+    REQUIRE(std::isfinite(eps) && eps > 0.f, VTTS_ERR_INVALID, "debug_ln: eps must be > 0");
+    const bool planes = hook_planes("debug_ln", hi, nullptr, lo);
+    HookRows hr = hook_rows("debug_ln", B, lens, rows);
+    for (int b = 0; b < B; ++b)
+      REQUIRE(out_offs[b] >= 0 && (size_t)out_offs[b] + lens[b] <= out_rows, VTTS_ERR_INVALID, "debug_ln: an utterance's output rows pass out_rows");
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * C, no = out_rows * C;
+    const float* da = static_cast<const float*>(upload(dev, a, n * 4, st));
+    const float* dy = y ? static_cast<const float*>(upload(dev, y, n * 4, st)) : nullptr;
+    const LnW w{static_cast<const float*>(upload(dev, g, C * 4, st)), static_cast<const float*>(upload(dev, beta, C * 4, st))};
+    const int* doffs = static_cast<const int*>(upload(dev, out_offs, (size_t)B * 4, st));
+    float* dout = static_cast<float*>(upload(dev, out, no * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, no, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->ln_rows(da, dy, w, eps, dout, doffs, C, planes ? &pl : nullptr, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, no * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, no * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, no * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_bert_embed(vtts_handle h, int B, const int* lens, size_t rows, int C, const int* ids, int V, const float* word, int P,
+                          const float* pos, const float* type0, const float* g, const float* beta, float eps, float* out, uint16_t* hi,
+                          uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(ids && word && pos && type0 && g && beta && out, VTTS_ERR_INVALID, "debug_bert_embed: missing input or output");
+    REQUIRE(C >= 1 && C <= 32 * CVL_MAXV, VTTS_ERR_INVALID, "debug_bert_embed: bert_embed_kernel needs 1 <= C <= 1024");
+    REQUIRE(V >= 1 && P >= 1 && std::isfinite(eps) && eps > 0.f, VTTS_ERR_INVALID, "debug_bert_embed: bad table sizes or eps");
+    const bool planes = hook_planes("debug_bert_embed", hi, nullptr, lo);
+    HookRows hr = hook_rows("debug_bert_embed", B, lens, rows);
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(lens[b] <= P, VTTS_ERR_INVALID, "debug_bert_embed: a sentence is longer than the position table");
+      for (int t = 0; t < lens[b]; ++t)
+        REQUIRE(ids[hr.off[b] + t] >= 0 && ids[hr.off[b] + t] < V, VTTS_ERR_INVALID, "debug_bert_embed: a word-piece id is outside the table");
+    }
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * C;
+    const int* did = static_cast<const int*>(upload(dev, ids, rows * 4, st));
+    const float* dw = static_cast<const float*>(upload(dev, word, (size_t)V * C * 4, st));
+    const float* dp = static_cast<const float*>(upload(dev, pos, (size_t)P * C * 4, st));
+    const float* dt = static_cast<const float*>(upload(dev, type0, C * 4, st));
+    const LnW w{static_cast<const float*>(upload(dev, g, C * 4, st)), static_cast<const float*>(upload(dev, beta, C * 4, st))};
+    float* dout = static_cast<float*>(upload(dev, out, n * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, n, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->bt_embed(did, dw, dp, dt, w, eps, dout, C, planes ? &pl : nullptr, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, n * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, n * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_dit_norm(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* a, int lda, const float* film, const float* y,
+                        const float* ada, int ada_ld, int gate_off, int shift_off, int scale_off, float* xo, float* no, uint16_t* hi,
+                        uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(a && ada && xo && no, VTTS_ERR_INVALID, "debug_dit_norm: missing input or output");
+    REQUIRE(C >= 1 && C <= 32 * DIT_LN_MAXV, VTTS_ERR_INVALID, "debug_dit_norm: dit_norm_kernel needs 1 <= C <= 512");
+    REQUIRE(lda >= C, VTTS_ERR_INVALID, "debug_dit_norm: lda must be >= C");
+    REQUIRE(shift_off >= 0 && scale_off >= 0 && shift_off + C <= ada_ld && scale_off + C <= ada_ld && (!y || (gate_off >= 0 && gate_off + C <= ada_ld)),
+            VTTS_ERR_INVALID, "debug_dit_norm: the gate / shift / scale columns pass ada_ld");
+    const bool planes = hook_planes("debug_dit_norm", hi, nullptr, lo);
+    HookRows hr = hook_rows("debug_dit_norm", B, lens, rows);
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * C;
+    const float* da = static_cast<const float*>(upload(dev, a, rows * lda * 4, st));
+    const float* df = film ? static_cast<const float*>(upload(dev, film, 2 * (size_t)C * 4, st)) : nullptr;
+    const float* dy = y ? static_cast<const float*>(upload(dev, y, n * 4, st)) : nullptr;
+    const float* dada = static_cast<const float*>(upload(dev, ada, (size_t)B * ada_ld * 4, st));
+    float* dxo = static_cast<float*>(upload(dev, xo, n * 4, st));
+    float* dno = static_cast<float*>(upload(dev, no, n * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, n, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->dit_norm(da, lda, df, dy, dada, ada_ld, gate_off, shift_off, scale_off, dxo, dno, planes ? &pl : nullptr, C, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(xo, dxo, n * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(no, dno, n * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, n * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_act(vtts_handle h, int act, int B, const int* lens, size_t rows, int C, float* y, uint16_t* hi, uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(y, VTTS_ERR_INVALID, "debug_act: missing rows");
+    REQUIRE(act == 0 || act == 1, VTTS_ERR_INVALID, "debug_act: act must be 0 (GELU) or 1 (SiLU)");
+    REQUIRE(C >= 1, VTTS_ERR_INVALID, "debug_act: C must be >= 1");
+    const bool planes = hook_planes("debug_act", hi, nullptr, lo);
+    HookRows hr = hook_rows("debug_act", B, lens, rows);
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * C;
+    float* dy = static_cast<float*>(upload(dev, y, n * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, n, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    if (act == 0) h->gelu_rows(dy, C, planes ? &pl : nullptr, r);
+    else h->silu_rows(dy, C, planes ? &pl : nullptr, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(y, dy, n * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, n * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_gate(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* x, const float* y, const float* ada, int ada_ld,
+                    int gate_off, float* out, int ldo, uint16_t* hi, uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(x && y && ada && out, VTTS_ERR_INVALID, "debug_gate: missing input or output");
+    REQUIRE(C >= 1 && ldo >= C && gate_off >= 0 && gate_off + C <= ada_ld, VTTS_ERR_INVALID,
+            "debug_gate: needs C >= 1, ldo >= C and the gate columns inside ada_ld");
+    const bool planes = hook_planes("debug_gate", hi, nullptr, lo);
+    HookRows hr = hook_rows("debug_gate", B, lens, rows);
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * C, nout = rows * ldo;
+    const float* dx = static_cast<const float*>(upload(dev, x, n * 4, st));
+    const float* dy = static_cast<const float*>(upload(dev, y, n * 4, st));
+    const float* dada = static_cast<const float*>(upload(dev, ada, (size_t)B * ada_ld * 4, st));
+    float* dout = static_cast<float*>(upload(dev, out, nout * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, nout, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->gate_rows(dx, dy, dada, ada_ld, gate_off, dout, ldo, planes ? &pl : nullptr, C, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, nout * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, nout * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, nout * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_groupnorm(vtts_handle h, const float* wav, const int64_t* lengths, int B, int64_t ld, size_t rows, float* out, int32_t* len0,
+                         int32_t* off0) {
+  return guarded(h, [&] {
+    require_contentvec(h, B);
+    REQUIRE(wav && lengths && out && len0 && off0 && ld >= 1, VTTS_ERR_INVALID, "debug_groupnorm: missing input or output, or bad ld");
+    const vtts_config& c = h->cfg;
+    const int NL = c.cv_n_conv, C = c.cv_conv_dim, K0 = c.cv_conv_kernel[0], s0 = c.cv_conv_stride[0];
+    h->B = B;
+    h->cv_stage(wav, lengths, ld);
+    const std::vector<int>& t = h->cvp.h;
+    REQUIRE(rows >= (size_t)h->cvp.tot0, VTTS_ERR_INVALID, "debug_groupnorm: fewer rows than the staged layer-0 rows");
+    // NaN behind every clip's samples in the staging, so that a read past the last window shows in the clip's rows
+    const size_t nw = (size_t)h->cvp.tot0 * s0 + K0;
+    float* pin = h->stg[vtts_engine::STG_CONTENTVEC].host(h->d_cvwav);
+    for (int b = 0; b < B; ++b) {
+      const size_t beg = (size_t)t[2 * NL * B + b] + (size_t)(t[b] - 1) * s0 + K0;
+      const size_t end = b + 1 < B ? (size_t)t[2 * NL * B + b + 1] : nw;
+      std::fill(pin + beg, pin + end, std::nanf(""));
+    }
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    int* di = h->ensure(h->d_cvi, h->cvp.nint);
+    float* dw = h->ensure(h->d_cvwav, nw);
+    h->stg[vtts_engine::STG_CONTENTVEC].upload();
+    const size_t np = (size_t)B * h->cvp.MC * C;
+    std::vector<Buf<char>> dev;
+    float* dout = static_cast<float*>(upload(dev, out, rows * C * 4, st));
+    h->cv_layer0(dw, di, h->ensure(h->d_cvps, np), h->ensure(h->d_cvpq, np), dout);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, rows * C * 4, cudaMemcpyDeviceToHost));
+    std::copy(t.begin(), t.begin() + B, len0);
+    std::copy(t.begin() + NL * B, t.begin() + (NL + 1) * B, off0);
   }, G_ATOMIC, ANY_FAMILY);
 }
 

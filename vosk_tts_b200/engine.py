@@ -66,7 +66,8 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
            "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode",
            "vtts_debug_t2s_sample", "vtts_debug_front_end", "vtts_debug_istft", "vtts_debug_mrf_mean",
-           "vtts_sovits_semantic", "vtts_sovits_latent"]
+           "vtts_sovits_semantic", "vtts_sovits_latent", "vtts_debug_add_ln", "vtts_debug_ln", "vtts_debug_bert_embed",
+           "vtts_debug_dit_norm", "vtts_debug_act", "vtts_debug_gate", "vtts_debug_groupnorm"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3, "sovits": 4}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -229,6 +230,21 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_istft.restype = i32
     lib.vtts_debug_mrf_mean.argtypes = [vp, i32, i32, vp, i32, i32, i32, C.c_size_t, vp, i32, vp, C.c_size_t, vp, vp]
     lib.vtts_debug_mrf_mean.restype = i32
+    sz, f32 = C.c_size_t, C.c_float
+    lib.vtts_debug_add_ln.argtypes = [vp, i32, vp, sz, i32, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp]
+    lib.vtts_debug_add_ln.restype = i32
+    lib.vtts_debug_ln.argtypes = [vp, i32, vp, sz, i32, vp, vp, vp, vp, f32, vp, sz, vp, vp, vp]
+    lib.vtts_debug_ln.restype = i32
+    lib.vtts_debug_bert_embed.argtypes = [vp, i32, vp, sz, i32, vp, i32, vp, i32, vp, vp, vp, vp, f32, vp, vp, vp]
+    lib.vtts_debug_bert_embed.restype = i32
+    lib.vtts_debug_dit_norm.argtypes = [vp, i32, vp, sz, i32, vp, i32, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp]
+    lib.vtts_debug_dit_norm.restype = i32
+    lib.vtts_debug_act.argtypes = [vp, i32, i32, vp, sz, i32, vp, vp, vp]
+    lib.vtts_debug_act.restype = i32
+    lib.vtts_debug_gate.argtypes = [vp, i32, vp, sz, i32, vp, vp, vp, i32, i32, vp, i32, vp, vp]
+    lib.vtts_debug_gate.restype = i32
+    lib.vtts_debug_groupnorm.argtypes = [vp, vp, vp, i32, C.c_int64, sz, vp, vp, vp]
+    lib.vtts_debug_groupnorm.restype = i32
     lib.vtts_debug_conv_log.argtypes = [vp, i32, C.POINTER(ConvReport), i32, C.POINTER(C.c_int)]
     lib.vtts_debug_conv_log.restype = i32
     lib.vtts_tc_split_plan.argtypes = [i32, vp, vp, vp, vp, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp]
@@ -1350,6 +1366,119 @@ class Engine:
         self._check(self.lib.vtts_debug_mrf_mean(self.h, int(bool(use_tc)), lens.size, _ptr(lens), int(rmul), Cc, n, rows, _ptr(x),
                                                  int(bool(last)), _ptr(out), 0 if hi is None else hi.shape[0], _ptr(hi), _ptr(lo)))
         return out, hi, lo
+
+    # ---- the normalisation kernels (include/vtts.h): rows packed as cr.offsets(lens); every output array is an initial
+    #      content that rows outside the utterances keep, and planes are uint16 bf16 bit patterns (None: not written)
+
+    def _rows(self, lens, a, name="a"):
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.ndim != 2:
+            raise ValueError("%s: shape %s, expected (rows, C)" % (name, a.shape))
+        return np.ascontiguousarray(lens, dtype=np.int32), a
+
+    def debug_add_ln(self, lens, a, g, beta, out, b=None, cadd=None, vec=None, hi=None, mid=None, lo=None):
+        """add_ln_kernel (vtts_debug_add_ln): out = LayerNorm(a + b) * g + beta (+ cadd) (+ vec[utterance]), a float32
+        [rows, C]; mid with hi and lo: the 3-way split.  Returns (out, hi, mid, lo)."""
+        lens, a = self._rows(lens, a)
+        rows, Cc = a.shape
+        out, b, cadd, vec, g, beta, hi, mid, lo = self._hook_arrays([
+            ("out", out, np.float32, (rows, Cc)), ("b", b, np.float32, (rows, Cc)), ("cadd", cadd, np.float32, (rows, Cc)),
+            ("vec", vec, np.float32, (lens.size, None)), ("g", g, np.float32, (Cc,)), ("beta", beta, np.float32, (Cc,)),
+            ("hi", hi, np.uint16, (rows, Cc)), ("mid", mid, np.uint16, (rows, Cc)), ("lo", lo, np.uint16, (rows, Cc))])
+        self._check(self.lib.vtts_debug_add_ln(self.h, lens.size, _ptr(lens), rows, Cc, _ptr(a), _ptr(b), _ptr(g), _ptr(beta), _ptr(cadd),
+                                               _ptr(vec), 0 if vec is None else vec.shape[1], _ptr(out), _ptr(hi), _ptr(mid), _ptr(lo)))
+        return out, hi, mid, lo
+
+    def debug_ln(self, lens, a, g, beta, eps, out_offs, out, y=None, hi=None, lo=None):
+        """cv_ln_kernel through ln_rows (vtts_debug_ln): out row out_offs[b] + t = LayerNorm(a + gelu(y)) * g + beta (y None:
+        LayerNorm(a)) of input row t of utterance b; out float32 [out_rows, C].  Returns (out, hi, lo)."""
+        lens, a = self._rows(lens, a)
+        rows, Cc = a.shape
+        out = np.ascontiguousarray(out, dtype=np.float32)
+        out, y, g, beta, hi, lo = self._hook_arrays([
+            ("out", out, np.float32, (None, Cc)), ("y", y, np.float32, (rows, Cc)), ("g", g, np.float32, (Cc,)),
+            ("beta", beta, np.float32, (Cc,)), ("hi", hi, np.uint16, (out.shape[0], Cc)), ("lo", lo, np.uint16, (out.shape[0], Cc))])
+        offs = np.ascontiguousarray(out_offs, dtype=np.int32)
+        if offs.shape != lens.shape:
+            raise ValueError("out_offs: one offset per utterance")
+        self._check(self.lib.vtts_debug_ln(self.h, lens.size, _ptr(lens), rows, Cc, _ptr(a), _ptr(y), _ptr(g), _ptr(beta), float(eps),
+                                           _ptr(offs), out.shape[0], _ptr(out), _ptr(hi), _ptr(lo)))
+        return out, hi, lo
+
+    def debug_bert_embed(self, lens, ids, word, pos, type0, g, beta, eps, out, hi=None, lo=None):
+        """bert_embed_kernel (vtts_debug_bert_embed): out row = LayerNorm((word[ids[row]] + type0) + pos[t]) * g + beta, t the
+        row's place in its sentence; ids int32 [rows], tables word [V, C], pos [P, C].  Returns (out, hi, lo)."""
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        word = np.ascontiguousarray(word, dtype=np.float32)
+        pos = np.ascontiguousarray(pos, dtype=np.float32)
+        Cc = word.shape[1]
+        out, type0, g, beta, hi, lo = self._hook_arrays([
+            ("out", out, np.float32, (ids.size, Cc)), ("type0", type0, np.float32, (Cc,)), ("g", g, np.float32, (Cc,)),
+            ("beta", beta, np.float32, (Cc,)), ("hi", hi, np.uint16, (ids.size, Cc)), ("lo", lo, np.uint16, (ids.size, Cc))])
+        if pos.ndim != 2 or pos.shape[1] != Cc:
+            raise ValueError("pos: shape %s, expected (P, %d)" % (pos.shape, Cc))
+        self._check(self.lib.vtts_debug_bert_embed(self.h, lens.size, _ptr(lens), ids.size, Cc, _ptr(ids), word.shape[0], _ptr(word),
+                                                   pos.shape[0], _ptr(pos), _ptr(type0), _ptr(g), _ptr(beta), float(eps), _ptr(out),
+                                                   _ptr(hi), _ptr(lo)))
+        return out, hi, lo
+
+    def debug_dit_norm(self, lens, a, width, ada, shift_off, scale_off, xo, no, film=None, y=None, gate_off=0, hi=None, lo=None):
+        """dit_norm_kernel, or dit_norm_planes_kernel with hi / lo (vtts_debug_dit_norm): a float32 [rows, lda >= width], ada
+        float32 [B, ada_ld]; xo, no float32 [rows, width].  Returns (xo, no, hi, lo)."""
+        lens, a = self._rows(lens, a)
+        rows = a.shape[0]
+        ada = np.ascontiguousarray(ada, dtype=np.float32)
+        xo, no, film, y, hi, lo = self._hook_arrays([
+            ("xo", xo, np.float32, (rows, width)), ("no", no, np.float32, (rows, width)), ("film", film, np.float32, (2 * width,)),
+            ("y", y, np.float32, (rows, width)), ("hi", hi, np.uint16, (rows, width)), ("lo", lo, np.uint16, (rows, width))])
+        if ada.ndim != 2 or ada.shape[0] != lens.size:
+            raise ValueError("ada: shape %s, expected (B, ada_ld)" % (ada.shape,))
+        self._check(self.lib.vtts_debug_dit_norm(self.h, lens.size, _ptr(lens), rows, int(width), _ptr(a), a.shape[1], _ptr(film), _ptr(y),
+                                                 _ptr(ada), ada.shape[1], int(gate_off), int(shift_off), int(scale_off), _ptr(xo),
+                                                 _ptr(no), _ptr(hi), _ptr(lo)))
+        return xo, no, hi, lo
+
+    def debug_act(self, act, lens, y, hi=None, lo=None):
+        """An activation pass (vtts_debug_act) on y float32 [rows, C]: act "gelu" (cv_gelu_kernel: in place, or into hi / lo
+        only) or "silu" (dit_silu_kernel, or dit_silu_planes_kernel with hi / lo).  Returns (y, hi, lo)."""
+        lens, y = self._rows(lens, y, "y")
+        y = y.copy()
+        hi, lo = self._hook_arrays([("hi", hi, np.uint16, y.shape), ("lo", lo, np.uint16, y.shape)])
+        self._check(self.lib.vtts_debug_act(self.h, {"gelu": 0, "silu": 1}[act], lens.size, _ptr(lens), y.shape[0], y.shape[1], _ptr(y),
+                                            _ptr(hi), _ptr(lo)))
+        return y, hi, lo
+
+    def debug_gate(self, lens, x, y, ada, gate_off, out, hi=None, lo=None):
+        """dit_gate_kernel, or dit_gate_planes_kernel with hi / lo (vtts_debug_gate): out rows [rows, ldo] = x + gate * y,
+        x and y float32 [rows, C].  Returns (out, hi, lo)."""
+        lens, x = self._rows(lens, x, "x")
+        rows, Cc = x.shape
+        ada = np.ascontiguousarray(ada, dtype=np.float32)
+        out = np.ascontiguousarray(out, dtype=np.float32)
+        out, y, hi, lo = self._hook_arrays([("out", out, np.float32, (rows, None)), ("y", y, np.float32, (rows, Cc)),
+                                            ("hi", hi, np.uint16, out.shape), ("lo", lo, np.uint16, out.shape)])
+        if ada.ndim != 2 or ada.shape[0] != lens.size:
+            raise ValueError("ada: shape %s, expected (B, ada_ld)" % (ada.shape,))
+        self._check(self.lib.vtts_debug_gate(self.h, lens.size, _ptr(lens), rows, Cc, _ptr(x), _ptr(y), _ptr(ada), ada.shape[1],
+                                             int(gate_off), _ptr(out), out.shape[1], _ptr(hi), _ptr(lo)))
+        return out, hi, lo
+
+    def debug_groupnorm(self, wav, lengths, out):
+        """ContentVec's layer 0 + GroupNorm + GELU (vtts_debug_groupnorm) of the clips wav float32 [B, ld], staged with NaN
+        behind every clip; out float32 [rows, cv_conv_dim].  Returns (out, len0 int32 [B], off0 int32 [B]): clip b's layer-0
+        rows are out[off0[b] : off0[b] + len0[b]]."""
+        wav = np.ascontiguousarray(wav, dtype=np.float32)
+        if wav.ndim != 2:
+            raise ValueError("wav: shape %s, expected (B, ld)" % (wav.shape,))
+        lengths = np.ascontiguousarray(lengths, dtype=np.int64)
+        cv = self.cfg.get("contentvec") or (self.cfg if "cv_conv_dim" in self.cfg else _config.contentvec_config())
+        out, = self._hook_arrays([("out", out, np.float32, (None, int(cv["cv_conv_dim"])))])
+        len0 = np.zeros(wav.shape[0], np.int32)
+        off0 = np.zeros(wav.shape[0], np.int32)
+        self._check(self.lib.vtts_debug_groupnorm(self.h, _ptr(wav), _ptr(lengths), wav.shape[0], wav.shape[1], out.shape[0], _ptr(out),
+                                                  _ptr(len0), _ptr(off0)))
+        return out, len0, off0
 
     def debug_t2s_sample(self, logits, state, y, top_k=20, top_p=0.6, temperature=0.6, repetition_penalty=1.35, early_stop_num=-1,
                          step_cap=1500, seeds=None, q=None, raw=None):
