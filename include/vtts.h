@@ -360,6 +360,26 @@ int vtts_debug_durations(vtts_handle h, int B, const int* lens, size_t rows, con
 int vtts_debug_stt_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* mu_dp, const float* pause,
                              float length_scale, const float* x, const float* mu_mel, int denormalise, int32_t* dur, int32_t* first,
                              int32_t* ylen, float* logw, size_t frame_rows, float* mu, float* pau, float* prior, float* mel);
+/* vtts_debug_noise (any engine): one launch of a kernel that draws the engine's Gaussian noise (Philox4x32-10 under `seed`,
+ * then Box-Muller) because the caller gave none, through the launch helper production uses; the seed travels in the
+ * call's scalar block as production's does.  Rows are packed as the duration hooks pack them; every output is in/out, and
+ * what the kernel does not write keeps its initial contents.
+ *   VTTS_NOISE_DP         dp_noise_kernel over B utterances of lens tokens: out [2][rows] = (za, zb) = (e0, e1) * scale
+ *                         (scale: noise_scale_w); C = 1
+ *   VTTS_NOISE_PRIOR      sample_prior_kernel with one token per frame (cum 1, 2, ..): frame t of utterance b reads stats
+ *                         row t; out [rows][C] = m + e * exp(logs) * scale (scale: noise_scale, C: inter_channels)
+ *   VTTS_NOISE_POSTERIOR  posterior_sample_kernel: out [rows][C] = m + e * exp(logs) * scale, stats [rows][2C] = [m | logs]
+ *   VTTS_NOISE_DIT        dit_init_kernel over 2B sequences, utterance b's conditional one (b) and its unconditional twin
+ *                         (B + b), of lens frames over extents exts (lens <= exts; rows packed by exts, the twins' rows
+ *                         from row `rows` on): out = xc [2 rows][C + HC] (columns [0, C) = e * scale, scale: temperature,
+ *                         C: noise_channels), mu [2 rows][MC], skx [2 rows][2 HC]; fake_content [MC]
+ * stats, exts, fake_content, mu and skx are given exactly where the kernel takes them; others must be NULL. */
+#define VTTS_NOISE_DP 0
+#define VTTS_NOISE_PRIOR 1
+#define VTTS_NOISE_POSTERIOR 2
+#define VTTS_NOISE_DIT 3
+int vtts_debug_noise(vtts_handle h, int kernel, uint64_t seed, int B, const int* lens, const int* exts, size_t rows, int C, float scale,
+                     const float* stats, const float* fake_content, int MC, int HC, float* out, float* mu, float* skx);
 /* Unit-test hooks of the spectral kernels, with the packing and in/out rules of the duration hooks above.
  * vtts_debug_front_end: the front end of vtts_convert / vtts_align / vtts_speaker_embedding (clip lengths checked and framed
  * as they are, staged with NaN behind every clip) on wav [B][ld] (from_spec 0) or features [B][spec_channels][ld] (1):

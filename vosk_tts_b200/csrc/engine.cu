@@ -749,6 +749,19 @@ struct vtts_engine {
     const uint32_t half[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
     memcpy(prm + 4, half, sizeof(half));
   }
+  // The launches of the four kernels that draw philox_normal when the caller gives no noise (eps / noise null), shared by
+  // production and vtts_debug_noise; prm is the call's scalar block (seed at [4..5]).  dp_noise: za, zb of n utterances of
+  // lens tokens (dp_noise_kernel, grid (ceil(maxLen / 128), n)).  sample_prior: frames of n utterances over their tokens' stats
+  // rows (sample_prior_kernel, grid (maxFrm, n)).  posterior_sample: z over stats rows (posterior_sample_kernel, grid (maxLen,
+  // n)).  dit_init: the start of a flow-matching call over NS sequences, B of them conditional (dit_init_kernel, grid (maxLen,
+  // NS)).
+  void dp_noise(const float* eps, int eps_ld, const float* prm, float* za, float* zb, const int* lens, const int* offs, int maxLen, int n);
+  void sample_prior(const float* stats, int I, const int* cum, const int* tok_len, const int* tok_off, const int* frm_len,
+                    const int* frm_off, int maxFrm, int n, const float* eps, int eps_ld, const float* prm, float* zp, int* ftok);
+  void posterior_sample(const float* stats, int I, const float* eps, int eps_ld, const float* prm, float* z, const int* lens,
+                        const int* offs, int maxLen, int n);
+  void dit_init(const float* noise, const float* prm, const float* fake, float* xc, int ldx, int NC, float* mu, int MC, float* skx,
+                int HC, const int* lens, const int* exts, const int* offs, int maxLen, int NS, int B);
   // Caller noise rows [B][I][ld] (memory maybe pageable) -> pinned [B][I][maxFrm]: the first cols[b] columns of item b
   void stage_noise(float* pin, const float* noise, int64_t ld, const std::vector<int>& cols) {
     const int I = cfg.inter_channels;
@@ -2235,12 +2248,7 @@ void vtts_engine::phase1(const int64_t* d_ids64, int t_max, const int64_t* d_sid
     dds_stack(dp_dds, D, c.dp_kernel_size, a, b, r);
     launch_conv({mk(dp_proj, a, D, 0, dx, D, 0, 1, 0)}, 1, r);
   }
-  {
-    dim3 g((maxTok + 127) / 128, B);
-    klaunch(dp_noise_kernel, dim3(g), dim3(128), (size_t)(0), noise_dp, eps_dp_ld, prm, za, zb, tl, to);
-    CK(cudaGetLastError());
-    ++launches;
-  }
+  dp_noise(noise_dp, eps_dp_ld, prm, za, zb, tl, to, maxTok, B);
   float* cvar = zb;   // conditioning half (x0 after the Flip)
   float* tvar = za;   // transformed half (x1)
   for (int n = c.dp_n_flows; n >= 2; --n) {
@@ -2463,12 +2471,7 @@ void vtts_engine::phase2(const float* noise_z, int z_ld, bool noise_on_device, b
   }
   float* z = ensure(d_z, F * I);
   int* ftok = ensure(d_ftok, F);
-  {
-    dim3 g(maxFrm, B);
-    klaunch(sample_prior_kernel, dim3(g), dim3(64), (size_t)(0), d_stats.p, I, d_cum.p, tl, to, fl, fo, noise_z, z_ld, d_prm.p, z, ftok);
-    CK(cudaGetLastError());
-    ++launches;
-  }
+  sample_prior(d_stats.p, I, d_cum.p, tl, to, fl, fo, maxFrm, B, noise_z, z_ld, d_prm.p, z, ftok);
   if (debug_flags & 1) {
     float* zp = ensure(d_zp_dbg, F * I);
     CK(cudaMemcpyAsync(zp, z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
@@ -2802,10 +2805,7 @@ void vtts_engine::posterior_encode(const float* feat, int feat_ld, const float* 
     wn_ffma(q_in, q_rsx, q_rss, Q_LAYERS, Q_KERNEL, 1, h, acts, skip, qcond, qld, r);
     launch_conv({mk(q_proj, skip, H, 0, stats, 2 * I, 0, 1, 0)}, 1, r);
   }
-  klaunch(posterior_sample_kernel, dim3(r.maxLen, r.n), dim3(64), (size_t)0, (const float*)stats, I, noise, maxFrm,
-          (const float*)d_vprm.p, r.lens, r.offs, z);
-  CK(cudaGetLastError());
-  ++launches;
+  posterior_sample(stats, I, noise, maxFrm, d_vprm.p, z, r.lens, r.offs, r.maxLen, r.n);
   if (debug_flags & 1) CK(cudaMemcpyAsync(ensure(d_vz_dbg, F * I), z, F * I * sizeof(float), cudaMemcpyDeviceToDevice, stream));
 }
 
@@ -3675,6 +3675,34 @@ void vtts_engine::st_block(const StBlk& k, const EncLayerW& L, int l, const floa
   gate_rows(k.Hb, k.Y, ada, k.ald, 5 * H, xout, ldo, nullptr, H, r);
 }
 
+void vtts_engine::dp_noise(const float* eps, int eps_ld, const float* prm, float* za, float* zb, const int* lens, const int* offs, int maxLen,
+                           int n) {
+  klaunch(dp_noise_kernel, dim3((maxLen + 127) / 128, n), dim3(128), (size_t)0, eps, eps_ld, prm, za, zb, lens, offs);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::sample_prior(const float* stats, int I, const int* cum, const int* tok_len, const int* tok_off, const int* frm_len,
+                               const int* frm_off, int maxFrm, int n, const float* eps, int eps_ld, const float* prm, float* zp, int* ftok) {
+  klaunch(sample_prior_kernel, dim3(maxFrm, n), dim3(64), (size_t)0, stats, I, cum, tok_len, tok_off, frm_len, frm_off, eps, eps_ld, prm, zp, ftok);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::posterior_sample(const float* stats, int I, const float* eps, int eps_ld, const float* prm, float* z, const int* lens,
+                                   const int* offs, int maxLen, int n) {
+  klaunch(posterior_sample_kernel, dim3(maxLen, n), dim3(64), (size_t)0, stats, I, eps, eps_ld, prm, lens, offs, z);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::dit_init(const float* noise, const float* prm, const float* fake, float* xc, int ldx, int NC, float* mu, int MC, float* skx,
+                           int HC, const int* lens, const int* exts, const int* offs, int maxLen, int NS, int B) {
+  klaunch(dit_init_kernel, dim3(maxLen, NS), dim3(128), (size_t)0, noise, prm, fake, xc, ldx, NC, mu, MC, skx, HC, lens, exts, offs, B);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
 void vtts_engine::dit_norm(const float* a, int lda, const float* film, const float* y, const float* ada, int ada_ld, int gate_off, int shift_off,
                            int scale_off, float* xo, float* no, const Planes* pl, int C, const Rows& r) {
   const dim3 gn((r.maxLen + DIT_LN_WARPS - 1) / DIT_LN_WARPS, r.n);
@@ -3816,13 +3844,13 @@ void vtts_engine::st_enqueue() {
     CK(cudaGetLastError());
     ++launches;
   }
-  klaunch(dit_init_kernel, gs, dim3(128), (size_t)0, (const float*)noise, prm, st_fake_content, xc, XW, NC, mu, MC, cat[nlsc - 1], H, lens, exts, offs, Bu);
+  dit_init(noise, prm, st_fake_content, xc, XW, NC, mu, MC, cat[nlsc - 1], H, lens, exts, offs, maxFrm, NS, Bu);
   klaunch(dit_time_kernel, dim3(stp.steps), dim3(256), (size_t)0, ts, st_tw1, st_tb1, st_tw2, st_tb2, st_fw, st_fb, H, F, NL, film);
   klaunch(dit_ada_kernel, dim3(NL, NS), dim3(256), (size_t)0, st_emb, st_fake_spk, stp.rows ? (const float*)(df + ST_PRM) : (const float*)nullptr,
           sid, st_aw1, st_ab1, st_aw2, st_ab2, G, H, NL, c.st_n_spks, ada);
   klaunch(dit_rope_table_kernel, dim3((maxFrm * (rd / 2) + 127) / 128), dim3(128), (size_t)0, rope, maxFrm, rd);
   CK(cudaGetLastError());
-  launches += 4;
+  launches += 3;
   auto silu = [&](float* y, int width) { silu_rows(y, width, nullptr, re); };
   auto cv = [&](const ConvW& W, const float* x, int ldx, float* y, int ldy, int yoff, const Rows& r) {
     launch_conv({mk(W, x, ldx, 0, y, ldy, yoff, 1, (W.k - 1) / 2)}, 1, r);
@@ -6466,13 +6494,74 @@ int vtts_debug_durations(vtts_handle h, int B, const int* lens, size_t rows, con
     const float* deps = static_cast<const float*>(upload(dev, eps, (size_t)B * I * eps_ld * sizeof(float), st));
     float* dzp = static_cast<float*>(upload(dev, z_p, frame_rows * I * sizeof(float), st));
     int* dft = static_cast<int*>(upload(dev, frame_token, frame_rows * sizeof(int), st));
-    h->klaunch(sample_prior_kernel, dim3(maxFrm, B), dim3(64), (size_t)0, dst, I, (const int*)dcum, hr.lens(), hr.offs(),
-               (const int*)dlen, (const int*)(dlen + 2 * B), deps, (int)eps_ld, dprm, dzp, dft);
-    CK(cudaGetLastError());
+    h->sample_prior(dst, I, dcum, hr.lens(), hr.offs(), dlen, dlen + 2 * B, maxFrm, B, deps, (int)eps_ld, dprm, dzp, dft);
     CK(cudaStreamSynchronize(st));
     CK(cudaMemcpy(z_p, dzp, frame_rows * I * sizeof(float), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(frame_token, dft, frame_rows * sizeof(int), cudaMemcpyDeviceToHost));
   });
+}
+
+int vtts_debug_noise(vtts_handle h, int kernel, uint64_t seed, int B, const int* lens, const int* exts, size_t rows, int C, float scale,
+                     const float* stats, const float* fake_content, int MC, int HC, float* out, float* mu, float* skx) {
+  return guarded(h, [&] {
+    REQUIRE(kernel >= VTTS_NOISE_DP && kernel <= VTTS_NOISE_DIT, VTTS_ERR_INVALID, "debug_noise: unknown kernel");
+    REQUIRE(out, VTTS_ERR_INVALID, "debug_noise: missing output");
+    REQUIRE(C >= 1 && (kernel != VTTS_NOISE_DP || C == 1), VTTS_ERR_INVALID, "debug_noise: C must be >= 1 (1 for dp_noise_kernel)");
+    REQUIRE((kernel == VTTS_NOISE_PRIOR || kernel == VTTS_NOISE_POSTERIOR) == (stats != nullptr), VTTS_ERR_INVALID,
+            "debug_noise: the samplers take stats, the other kernels none");
+    const bool dit = kernel == VTTS_NOISE_DIT;
+    REQUIRE(dit == (exts != nullptr) && dit == (fake_content != nullptr) && dit == (mu != nullptr) && dit == (skx != nullptr), VTTS_ERR_INVALID,
+            "debug_noise: dit_init_kernel takes exts, fake_content, mu and skx, the other kernels none");
+    REQUIRE(!dit || (MC >= 1 && HC >= 1), VTTS_ERR_INVALID, "debug_noise: dit_init_kernel needs MC >= 1 and HC >= 1");
+    REQUIRE((int64_t)B * C < (int64_t)INT32_MAX, VTTS_ERR_INVALID, "debug_noise: B * C must stay below 2^31 (the counter's bidx)");
+    // dit_init_kernel's rows are packed by extent, the unconditional sequences' behind the conditional ones at row `rows`
+    HookRows hr = hook_rows("debug_noise", B, dit ? exts : lens, rows);
+    if (dit)
+      for (int b = 0; b < B; ++b)
+        REQUIRE(lens && lens[b] >= 1 && lens[b] <= exts[b], VTTS_ERR_INVALID, "debug_noise: lengths must be in [1, exts]");
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    float prm[8];
+    const float sc[3] = {scale, 0.f, scale};       // the samplers' noise_scale / DiT's temperature, and dp's noise_scale_w
+    vtts_engine::put_scalars(prm, 8, sc, 3, seed);
+    const float* dprm = static_cast<const float*>(upload(dev, prm, sizeof(prm), st));
+    const size_t nout = kernel == VTTS_NOISE_DP ? 2 * rows : dit ? 2 * rows * (C + HC) : rows * C;
+    float* dout = static_cast<float*>(upload(dev, out, nout * 4, st));
+    if (kernel == VTTS_NOISE_DP) {
+      h->dp_noise(nullptr, 0, dprm, dout, dout + rows, hr.lens(), hr.offs(), hr.maxLen, B);
+    } else if (!dit) {
+      const float* ds = static_cast<const float*>(upload(dev, stats, rows * 2 * C * 4, st));
+      if (kernel == VTTS_NOISE_PRIOR) {   // one token per frame: cum = 1, 2, .. so that frame j reads stats row j
+        std::vector<int> cum(rows, 0);
+        for (int b = 0; b < B; ++b)
+          for (int i = 0; i < lens[b]; ++i) cum[hr.off[b] + i] = i + 1;
+        const int* dcum = static_cast<const int*>(upload(dev, cum.data(), rows * 4, st));
+        h->sample_prior(ds, C, dcum, hr.lens(), hr.offs(), hr.lens(), hr.offs(), hr.maxLen, B, nullptr, 0, dprm, dout, nullptr);
+      } else {
+        h->posterior_sample(ds, C, nullptr, 0, dprm, dout, hr.lens(), hr.offs(), hr.maxLen, B);
+      }
+    } else {
+      std::vector<int> si(6 * (size_t)B);              // lens | exts | offs of the 2B sequences
+      for (int q = 0; q < 2 * B; ++q) {
+        const int b = q < B ? q : q - B;
+        si[q] = lens[b];
+        si[2 * B + q] = exts[b];
+        si[4 * B + q] = hr.off[b] + (q < B ? 0 : (int)rows);
+      }
+      const int* dsi = static_cast<const int*>(upload(dev, si.data(), si.size() * 4, st));
+      const float* dfake = static_cast<const float*>(upload(dev, fake_content, (size_t)MC * 4, st));
+      float* dmu = static_cast<float*>(upload(dev, mu, 2 * rows * MC * 4, st));
+      float* dskx = static_cast<float*>(upload(dev, skx, 2 * rows * 2 * HC * 4, st));
+      h->dit_init(nullptr, dprm, dfake, dout, C + HC, C, dmu, MC, dskx, HC, dsi, dsi + 2 * B, dsi + 4 * B, hr.maxLen, 2 * B, B);
+      CK(cudaStreamSynchronize(st));
+      CK(cudaMemcpy(mu, dmu, 2 * rows * MC * 4, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(skx, dskx, 2 * rows * 2 * HC * 4, cudaMemcpyDeviceToHost));
+    }
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, nout * 4, cudaMemcpyDeviceToHost));
+  }, G_ATOMIC, ANY_FAMILY);
 }
 
 int vtts_debug_stt_durations(vtts_handle h, int B, const int* lens, size_t rows, const float* mu_dp, const float* pause,

@@ -64,7 +64,7 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_speaker_embedding_mel", "vtts_quickvc_convert", "vtts_content_units",
            "vtts_quickvc_convert_wav", "vtts_debug_live_bytes", "vtts_resample", "vtts_cfm_decode", "vtts_stabletts_synthesise",
            "vtts_hifigan_vocode", "vtts_stabletts_synthesise_wav", "vtts_bert_features", "vtts_stabletts_synthesise_pieces_wav",
-           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_t2s_decode",
+           "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_debug_noise", "vtts_t2s_decode",
            "vtts_debug_t2s_sample", "vtts_debug_front_end", "vtts_debug_istft", "vtts_debug_mrf_mean",
            "vtts_sovits_semantic", "vtts_sovits_latent", "vtts_debug_add_ln", "vtts_debug_ln", "vtts_debug_bert_embed",
            "vtts_debug_dit_norm", "vtts_debug_act", "vtts_debug_gate", "vtts_debug_groupnorm"]
@@ -224,6 +224,8 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_stt_durations.argtypes = [vp, i32, vp, C.c_size_t, vp, vp, C.c_float, vp, vp, i32, vp, vp, vp, vp, C.c_size_t,
                                              vp, vp, vp, vp]
     lib.vtts_debug_stt_durations.restype = i32
+    lib.vtts_debug_noise.argtypes = [vp, i32, C.c_uint64, i32, vp, vp, C.c_size_t, i32, C.c_float, vp, vp, i32, i32, vp, vp, vp]
+    lib.vtts_debug_noise.restype = i32
     lib.vtts_debug_front_end.argtypes = [vp, i32, vp, vp, i32, C.c_int64, vp, C.c_size_t, vp, vp]
     lib.vtts_debug_front_end.restype = i32
     lib.vtts_debug_istft.argtypes = [vp, i32, vp, i32, C.c_size_t, vp, C.c_size_t, vp]
@@ -1556,6 +1558,41 @@ class Engine:
             _ptr(o["dur"]), _ptr(o["first"]), _ptr(o["ylen"]), _ptr(o["logw"]), F, _ptr(o["mu"]), _ptr(o["pau"]),
             _ptr(o["prior"]), _ptr(o["mel"])))
         return o
+
+    NOISE_KERNELS = {"dp": 0, "prior": 1, "posterior": 2, "dit": 3}
+
+    def debug_noise(self, kernel, seed, lens, out, scale=1.0, stats=None, exts=None, fake_content=None, mu=None, skx=None):
+        """One launch of a noise kernel drawing its own Philox noise under the 64-bit `seed` (vtts_debug_noise); `out` and the
+        other in/out buffers hold initial contents that what the kernel does not write keeps.  kernel:
+          "dp"         dp_noise_kernel: out float32 [2, rows] (za, zb) over utterances of lens tokens; scale = noise_scale_w
+          "prior"      sample_prior_kernel, one token per frame: stats float32 [rows, 2C], out [rows, C]; scale = noise_scale
+          "posterior"  posterior_sample_kernel: stats float32 [rows, 2C], out [rows, C]; scale = noise_scale
+          "dit"        dit_init_kernel over each utterance's conditional sequence and its unconditional twin, rows packed by
+                       exts (the twins' from row rows on): out = xc float32 [2 rows, C + HC], mu [2 rows, MC], skx [2 rows,
+                       2 HC], fake_content [MC]; scale = temperature
+        Returns out (and for "dit" (out, mu, skx))."""
+        k = self.NOISE_KERNELS[kernel]
+        lens = np.ascontiguousarray(lens, dtype=np.int32)
+        out = np.ascontiguousarray(out, dtype=np.float32).copy()
+        if out.ndim != 2:
+            raise ValueError("out: shape %s, expected 2-d" % (out.shape,))
+        dit = kernel == "dit"
+        rows = out.shape[1] if kernel == "dp" else out.shape[0] // 2 if dit else out.shape[0]
+        MC = 0 if fake_content is None else np.asarray(fake_content).size
+        HC = 0 if skx is None else np.asarray(skx).shape[-1] // 2
+        C_ = 1 if kernel == "dp" else out.shape[1] - HC if dit else out.shape[1]
+        stats, fake_content, mu, skx = self._hook_arrays([
+            ("stats", stats, np.float32, (rows, 2 * C_)), ("fake_content", fake_content, np.float32, (MC,)),
+            ("mu", mu, np.float32, (2 * rows, MC)), ("skx", skx, np.float32, (2 * rows, 2 * HC))])
+        if (kernel == "dp" and out.shape[0] != 2) or (dit and out.shape[0] != 2 * rows):
+            raise ValueError("out: shape %s, expected (2, rows) for dp, (2 rows, C + HC) for dit" % (out.shape,))
+        if exts is not None:
+            exts = np.ascontiguousarray(exts, dtype=np.int32)
+            if exts.shape != lens.shape:
+                raise ValueError("exts: one extent per utterance")
+        self._check(self.lib.vtts_debug_noise(self.h, k, int(seed), lens.size, _ptr(lens), _ptr(exts), rows, C_,
+                                              float(scale), _ptr(stats), _ptr(fake_content), MC, HC, _ptr(out), _ptr(mu), _ptr(skx)))
+        return (out, mu, skx) if dit else out
 
     def conv_log(self, mode):
         """Launch-shape log of the dense conv launches (vtts_debug_conv_log): 1 clears and starts it, 0 stops it, 2 returns the
