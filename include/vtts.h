@@ -425,7 +425,7 @@ int vtts_debug_dit_norm(vtts_handle h, int B, const int* lens, size_t rows, int 
                         uint16_t* lo);
 /* vtts_debug_act: the activation passes on y [rows][C].  act 0: cv_gelu_kernel (erf GELU), in place, or only into the planes
  * when hi / lo are given (y unchanged).  act 1: dit_silu_kernel in place, or dit_silu_planes_kernel, in place and into the
- * planes. */
+ * planes.  act 2: t2s_relu_kernel (the GPT-SoVITS prefill's FFN ReLU) as act 0: in place, or only into the planes. */
 int vtts_debug_act(vtts_handle h, int act, int B, const int* lens, size_t rows, int C, float* y, uint16_t* hi, uint16_t* lo);
 /* vtts_debug_gate: dit_gate_kernel (hi, lo NULL) or dit_gate_planes_kernel: out rows of pitch ldo >= C [rows][ldo] (and their
  * planes, same pitch) = x + gate * y, x and y [rows][C], gate: C columns from gate_off of utterance b's row of ada [B][ada_ld]. */
@@ -765,6 +765,35 @@ int vtts_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* lengths, i
 int vtts_debug_t2s_sample(vtts_handle h, int B, const float* logits, int32_t* state, int32_t* y, int y_ld, int top_k, float top_p,
                           float temperature, float repetition_penalty, int early_stop_num, int step_cap, const uint64_t* seeds,
                           const float* q, int q_ld, uint32_t* seen, int32_t* n_stopped, float* raw, int raw_ld);
+/* Unit-test hooks of the text prefill of vtts_t2s_decode, each through the launch helper production uses.  Rows are packed as
+ * vtts_t2s_decode packs them: utterance b's T[b] text rows and then its P[b] prompt rows start at a multiple of 8, with no gap
+ * between utterances, so adjacent utterances can touch; `rows` is the caller's row count, at least the packed total.  Every
+ * output is in/out: what the kernel does not write keeps the caller's contents.  hi / lo: uint16 bf16 planes of the fp32
+ * output (hi = rne(v), lo = rne(v - hi)), given together or not at all.  VTTS_ERR_INVALID before any launch for what the
+ * kernels cannot take: B outside [1, 4096], T < 1, P < 0, too few rows.
+ * vtts_debug_t2s_prefix_attn (any engine; no weights): t2s_prefix_attn_kernel on qkv [rows][3H] (q, k, v of head h at
+ *   columns h dk, H + h dk, 2H + h dk): row t of an utterance attends to its key k iff k < T or k <= t, softmax(q k / sqrt(dk)),
+ *   into out [rows][H] (and hi / lo).  launch_rows: the grid's row count (production sizes it by the batch's longest T + P);
+ *   0 takes the longest, else it must be at least that.  Refuses dk = H / heads not a multiple of 32 or above 128.
+ * vtts_debug_t2s_embed (text-to-semantic engines): t2s_prefill_embed_kernel with the engine's t2s.temb, t2s.aemb, t2s.pe and
+ *   alphas: text row t = (temb[ids] + bert_proj) + alpha_t pe[t], prompt row t = aemb[ids] + alpha_a pe[t - T], into x
+ *   [rows][H] (and hi / lo).  ids [rows]: phone ids on text rows, semantic tokens on prompt rows.  bert_proj [rows][H] is
+ *   bert_proj's output on the text rows, or NULL for its bias alone (no BERT features).  Refuses an id outside its table and T
+ *   or P beyond the position table.
+ * vtts_debug_t2s_state (text-to-semantic engines): t2s_kv_store_kernel, then t2s_init_kernel, as the prefill's last steps run
+ *   them.  Row t of utterance b's qkv [rows][3H] k and v go to cache row kv_off[b] + t of kc, vc [kv_rows][H].  Then state
+ *   [B][8] = (T, P, kv_off, NY = P, GEN 0, STOP 0, y_off, 0), the prompt tokens (prompts: the B prompts back to back, P[b]
+ *   each) at y[y_off[b] ..] of y [y_len], the bitmap of the prompt's tokens in row b of the first B rows of (V + 31) / 32
+ *   words of seen [seen_len] (every word of those rows rewritten, the words behind them kept), and hx [B][H] = pre row
+ *   T + P - 1 of pre [rows][H].  Refuses prompt tokens outside [0, V - 1), seen_len below B (V + 31) / 32, and cache or
+ *   token regions that pass kv_rows or y_len or overlap one another. */
+int vtts_debug_t2s_prefix_attn(vtts_handle h, int H, int heads, int B, const int* T, const int* P, int launch_rows, size_t rows,
+                               const float* qkv, float* out, uint16_t* hi, uint16_t* lo);
+int vtts_debug_t2s_embed(vtts_handle h, int B, const int* T, const int* P, size_t rows, const int* ids, const float* bert_proj, float* x,
+                         uint16_t* hi, uint16_t* lo);
+int vtts_debug_t2s_state(vtts_handle h, int B, const int* T, const int* P, size_t rows, const float* qkv, const float* pre, const int* prompts,
+                         const int* kv_off, size_t kv_rows, float* kc, float* vc, const int* y_off, size_t y_len, int32_t* state, int32_t* y,
+                         uint32_t* seen, size_t seen_len, float* hx);
 
 /* GPT-SoVITS prompt tokens (model_family 4): a reference recording's semantic codes, as inference_cli.py:176-200 computes
  * them with chinese-hubert-base and SynthesizerTrn.extract_latent (module/models.py:990-993).

@@ -18,33 +18,45 @@ def sine_table(n, dim, dtype):
     return pe.to(dtype)
 
 
-def step_logits(sd, cfg, phones, y, bert=None, dtype=torch.float64, P=0):
-    """Logits [len(y) - P + 1, V] of every sampling step along the token sequence y (its first P tokens the prompt, then the
-    sampled tokens): step i reads row T + P + i - 1 of [text; y]."""
-    w = {k: v.to(dtype) for k, v in sd.items()}
-    H, nh, L = cfg["cv_hidden"], cfg["cv_heads"], cfg["cv_layers"]
+def embed(w, cfg, phones, y, bert=None, dtype=torch.float64):
+    """The rows [text; y] infer_panel feeds its layers (w: the state dict in dtype)."""
     x = torch.as_tensor(np.asarray(phones, np.int64))
     T = x.numel()
     y = torch.as_tensor(np.asarray(y, np.int64)).reshape(-1)
-    pe = sine_table(max(T, y.numel()) + 1, H, dtype)
+    pe = sine_table(max(T, y.numel()) + 1, cfg["cv_hidden"], dtype)
     xt = w["ar_text_embedding.word_embeddings.weight"][x]
     bp = torch.zeros(T, 1024, dtype=dtype) if bert is None else torch.as_tensor(np.asarray(bert)).to(dtype)
     xt = xt + (bp @ w["bert_proj.weight"].T + w["bert_proj.bias"])
     xt = xt + w["ar_text_position.alpha"] * pe[:T]
     ya = w["ar_audio_embedding.word_embeddings.weight"][y] + w["ar_audio_position.alpha"] * pe[:y.numel()]
-    h = torch.cat([xt, ya], 0)
-    n = h.shape[0]
+    return torch.cat([xt, ya], 0)
+
+
+def prefix_attention(qkv, T, nh):
+    """The attention core of one layer on its qkv rows [n, 3H]: softmax(q k^T sqrt(1 / dk)) v per head under infer_panel's
+    prefix mask (key k is visible to query q iff k < T or k <= q), [n, H]."""
+    n, H = qkv.shape[0], qkv.shape[1] // 3
+    dk = H // nh
     qi = torch.arange(n)[:, None]
     ki = torch.arange(n)[None, :]
     visible = (ki < T) | (ki <= qi)
-    dk = H // nh
+    q, k, v = (qkv[:, i * H:(i + 1) * H].reshape(n, nh, dk).transpose(0, 1) for i in range(3))
+    a = (q * math.sqrt(1.0 / dk)) @ k.transpose(1, 2)
+    a = torch.softmax(a.masked_fill(~visible, float("-inf")), -1) @ v
+    return a.transpose(0, 1).reshape(n, H)
+
+
+def step_logits(sd, cfg, phones, y, bert=None, dtype=torch.float64, P=0):
+    """Logits [len(y) - P + 1, V] of every sampling step along the token sequence y (its first P tokens the prompt, then the
+    sampled tokens): step i reads row T + P + i - 1 of [text; y]."""
+    w = {k: v.to(dtype) for k, v in sd.items()}
+    H, nh, L = cfg["cv_hidden"], cfg["cv_heads"], cfg["cv_layers"]
+    T = len(phones)
+    h = embed(w, cfg, phones, y, bert, dtype)
     for l in range(L):
         p = "h.layers.%d." % l
         qkv = h @ w[p + "self_attn.in_proj_weight"].T + w[p + "self_attn.in_proj_bias"]
-        q, k, v = (qkv[:, i * H:(i + 1) * H].reshape(n, nh, dk).transpose(0, 1) for i in range(3))
-        a = (q * math.sqrt(1.0 / dk)) @ k.transpose(1, 2)
-        a = torch.softmax(a.masked_fill(~visible, float("-inf")), -1) @ v
-        a = a.transpose(0, 1).reshape(n, H) @ w[p + "self_attn.out_proj.weight"].T + w[p + "self_attn.out_proj.bias"]
+        a = prefix_attention(qkv, T, nh) @ w[p + "self_attn.out_proj.weight"].T + w[p + "self_attn.out_proj.bias"]
         h = torch.nn.functional.layer_norm(h + a, (H,), w[p + "norm1.weight"], w[p + "norm1.bias"], 1e-5)
         f = torch.relu(h @ w[p + "linear1.weight"].T + w[p + "linear1.bias"]) @ w[p + "linear2.weight"].T + w[p + "linear2.bias"]
         h = torch.nn.functional.layer_norm(h + f, (H,), w[p + "norm2.weight"], w[p + "norm2.bias"], 1e-5)

@@ -32,7 +32,14 @@ Bound.  What the emulation cannot restate exactly is bounded per output element:
                    n_v u sum_j p_ij |v~_j|.
   l and 1/l        the row sum of n_keys positive terms in fp32, the reciprocal and the product: (n_keys + 8) u |o_i|.
 Lazy running max.  The tensor-core kernel refreshes its running max only when a tile exceeds it by more than ATC_LAZY = 6
-(p up to e^6 before the division): the products and sums scale with l, so every relative bound above holds unchanged."""
+(p up to e^6 before the division): the products and sums scale with l, so every relative bound above holds unchanged.
+
+Prefix mask (T given; csrc/t2s.cu t2s_prefix_attn_kernel, GPT-SoVITS's text prefill).  No band (W = 0, no tables); row i of
+an utterance whose first T rows are its text sees key j iff j < T or j <= i, so each row has its own key count n_i (T for a
+text row, i + 1 for a prompt row), and every term above that counts keys (n_t tiles of 32, n_v, the n_keys + 8 of l) takes
+n_i.  The kernel is an FFMA kernel (fp32 fmaf dot products, n_s = dk) with an online softmax that rescales once per 32-key
+tile, and it scales q by the fp32 sqrtf(1 / dk) (the reference's q * sqrt(1 / dk)) instead of dividing by sqrtf(dk): the
+operands here are those.  `/` is correctly rounded (the build has no fast-math flags), covered by the l term."""
 import numpy as np
 
 from conv_ref import SEQ_GAP, U23, U24, bf16_value, offsets, split_bf16  # noqa: F401  (SEQ_GAP: the packing)
@@ -81,20 +88,32 @@ def _head(qkv, r0, n, h, dk, H, col_shift=0):
     return np.asarray(q, np.float32), np.asarray(k, np.float32), np.asarray(v, np.float32)
 
 
-def reference(qkv, lens, heads, W, tables, kind, corrupt=None):
+def _prefix_keys(n, T):
+    """Keys row i of a T-text-row utterance of n rows sees: T for a text row, i + 1 for a prompt row ([n, 1])."""
+    i = np.arange(n)
+    return np.where(i < T, T, i + 1)[:, None]
+
+
+def reference(qkv, lens, heads, W, tables, kind, corrupt=None, T=None, offs=None):
     """Float64 reference of every utterance.  Returns a list of (rows [n], out [n, H], bound [n, H]): the qkv / output rows
     of the utterance and the value a correct kernel is within `bound` of.
       kind      "tc" (operand-exact emulation of attn_tc_kernel) or "ffma" (exact attention of the FFMA kernels' operands)
       corrupt   deliberate errors for the rejection studies: drop_slot (band term dropped at that relative slot), shift
                 (band slots shifted by that many keys), no_ev, mask_last (last valid key masked), unmask_next (the first
                 row beyond the utterance read as a key), rel_scale2 (1/sqrt(dk) twice on the relative logits), head_shift
-                (head 0 reads q 32 channels further), drop_qlkh (tensor cores: no ql.kh product)"""
+                (head 0 reads q 32 channels further), drop_qlkh (tensor cores: no ql.kh product)
+      T         the prefix mask (see above) with utterance b's first T[b] rows its text; W = 0, tables None, kind "ffma"
+      offs      the utterances' first rows (default: offsets(lens))"""
     corrupt = corrupt or {}
     qkv = np.asarray(qkv, np.float32)
     H = qkv.shape[1] // 3
     dk = H // heads
     nrel = 2 * W + 1
-    offs = offsets(lens)
+    offs = offsets(lens) if offs is None else offs
+    prefix = T is not None
+    if prefix:
+        assert W == 0 and tables is None and kind == "ffma"
+        tables = dict(relk=np.zeros((1, dk), np.float32), relv=np.zeros((1, dk), np.float32))
     tc = kind == "tc"
     if tc:
         ekh, ekl = tables["rk"]
@@ -131,14 +150,18 @@ def reference(qkv, lens, heads, W, tables, kind, corrupt=None):
                 n_t = -(-nk // TC_KT)
                 n_v = 3 * (n_t * TC_KT + 3 * 16) + n_t
             else:
-                qs = (q / sq).astype(np.float64)            # the kernels' fp32 pre-scaled q
+                if prefix:                                   # t2s_prefix_attn_kernel: q * (float)sqrt(1.0 / dk)
+                    qs = (q * np.float32(np.sqrt(1.0 / dk))).astype(np.float64)
+                else:
+                    qs = (q / sq).astype(np.float64)        # the kernels' fp32 pre-scaled q
                 S, Sa = qs @ k.T.astype(np.float64), np.abs(qs) @ np.abs(k.T.astype(np.float64))
                 Sr, Sra = qs @ ek.T, np.abs(qs) @ np.abs(ek.T)
                 if "rel_scale2" in corrupt:
                     Sr = Sr / float(sq)
                 vt = v.astype(np.float64)
-                n_t = -(-nk // FFMA_KT)
-                n_v = nk + nrel + 4 + n_t
+                nkr = _prefix_keys(nq, T[b]) if prefix else nk
+                n_t = -(-nkr // FFMA_KT)
+                n_v = nkr + nrel + 4 + n_t
             for i0 in range(0, nq, QBLK):
                 i1 = min(nq, i0 + QBLK)
                 i = np.arange(i0, i1)[:, None]
@@ -150,11 +173,14 @@ def reference(qkv, lens, heads, W, tables, kind, corrupt=None):
                     inband = inband & (slot != corrupt["drop_slot"])
                 s = S[i0:i1] + np.where(inband, np.take_along_axis(Sr[i0:i1], slot, 1), 0.0)
                 A = Sa[i0:i1] + np.where(inband, np.take_along_axis(Sra[i0:i1], slot, 1), 0.0)
-                m = s.max(1, keepdims=True)
-                p = np.exp(s - m)
+                vis = (j < T[b]) | (j <= i) if prefix else np.ones(s.shape, bool)
+                s = np.where(vis, s, 0.0)
+                m = np.where(vis, s, -np.inf).max(1, keepdims=True)
+                p = np.where(vis, np.exp(s - m), 0.0)
                 p /= p.sum(1, keepdims=True)
                 M = np.abs(s).max(1, keepdims=True)
-                D = (n_s + 4) * U23 * A + 4 * U23 * (np.abs(s) + M) + (n_t + 2) * 2.0 ** -21
+                rt = n_t[i0:i1] if prefix else n_t
+                D = (n_s + 4) * U23 * A + 4 * U23 * (np.abs(s) + M) + (rt + 2) * 2.0 ** -21
 
                 def band_scatter(w):               # [nq, nk] -> [nq, nrel]: weight of each relative slot
                     r = np.zeros((i1 - i0, nrel))
@@ -166,8 +192,9 @@ def reference(qkv, lens, heads, W, tables, kind, corrupt=None):
                 pv_abs = p @ np.abs(vt) + pb @ np.abs(evt)
                 Dbar = (p * D).sum(1, keepdims=True)
                 soft = 1.05 * ((p * D) @ np.abs(vt) + band_scatter(p * D) @ np.abs(evt) + Dbar * pv_abs)
-                acc = n_v * U23 * pv_abs * (1.0 + 2.0 ** -7 if tc else 1.0)
-                e = soft + acc + (SPLIT_ERR * pv_abs if tc else 0.0) + (nk + 8) * U23 * np.abs(o)
+                rv, rk = (n_v[i0:i1], nkr[i0:i1]) if prefix else (n_v, nk)
+                acc = rv * U23 * pv_abs * (1.0 + 2.0 ** -7 if tc else 1.0)
+                e = soft + acc + (SPLIT_ERR * pv_abs if tc else 0.0) + (rk + 8) * U23 * np.abs(o)
                 out[i0:i1, h * dk:(h + 1) * dk] = o
                 bnd[i0:i1, h * dk:(h + 1) * dk] = e
         res.append((r0 + np.arange(nq), out, bnd))
@@ -180,20 +207,28 @@ def within(out, ref, bound):
 
 
 def worst(out, results):
-    """Largest |out - ref| / bound over all utterances of one launch (out: [rows, H])."""
+    """Largest |out - ref| / bound over all utterances of one launch (out: [rows, H]); inf when any output is not finite."""
     w = 0.0
     for rows, ref, bnd in results:
-        err = np.abs(np.asarray(out, np.float64)[rows] - ref)
-        w = max(w, float(np.max(err / bnd)))
+        o = np.asarray(out, np.float64)[rows]
+        if not np.all(np.isfinite(o)):
+            return float("inf")
+        w = max(w, float(np.max(np.abs(o - ref) / bnd)))
     return w
 
 
 # ------------------------------------------------------------------------------------------------ float32 restatements
-def f32_attention(qkv, lens, heads, W, relk, relv, lazy=None, no_rescale=False, tile=TC_KT):
+def f32_attention(qkv, lens, heads, W, relk, relv, lazy=None, no_rescale=False, tile=TC_KT, T=None, offs=None, corrupt=()):
     """The attention in float32 arithmetic on the FFMA kernels' operands.  lazy=None: one softmax over all keys, products
     and sums taken in reverse key order; lazy=threshold: online softmax over key tiles with the running max refreshed only
     when a tile exceeds it by more than `threshold` (as attn_tc_kernel), no_rescale: such a refresh leaves O and l as they
-    are (a corruption).  Returns (out [rows, H] float32, number of refreshes)."""
+    are (a corruption).  Returns (out [rows, H] float32, number of refreshes).
+    T: the prefix mask as t2s_prefix_attn_kernel computes it (W = 0, relk / relv unused): key order, 32-key chunks, the
+    running max raised by every chunk that exceeds it, l and the accumulators rescaled each chunk, then acc / l; rows at
+    offs.  corrupt (deliberate errors): "self" (a prompt row does not see itself), "text_sees_prompt" (text rows see every
+    row), "no_rescale" (acc is not rescaled; l is), "no_max" (no running max: p = expf(s), nothing rescaled)."""
+    if T is not None:
+        return _f32_prefix(qkv, lens, heads, T, offs, corrupt), 0
     qkv = np.asarray(qkv, np.float32)
     H = qkv.shape[1] // 3
     dk = H // heads
@@ -246,3 +281,44 @@ def f32_attention(qkv, lens, heads, W, relk, relv, lazy=None, no_rescale=False, 
                         o = (o + p[:, jj:jj + 1] * vj).astype(np.float32)
             out[r0:r0 + n, h * dk:(h + 1) * dk] = (o / l).astype(np.float32)
     return out, refreshes
+
+
+def _f32_prefix(qkv, lens, heads, T, offs, corrupt):
+    qkv = np.asarray(qkv, np.float32)
+    H = qkv.shape[1] // 3
+    dk = H // heads
+    out = np.zeros((qkv.shape[0], H), np.float32)
+    scale = np.float32(np.sqrt(1.0 / dk))
+    f32 = np.float32
+    for b, n in enumerate(lens):
+        r0, Tb = offs[b], T[b]
+        i = np.arange(n)
+        nk = _prefix_keys(n, Tb)[:, 0]
+        if "self" in corrupt:
+            nk = np.where(i < Tb, Tb, i)                  # n = t < T ? T : t
+        if "text_sees_prompt" in corrupt:
+            nk = np.where(i < Tb, n, i + 1)
+        for h in range(heads):
+            q, k, v = _head(qkv, r0, n, h, dk, H)
+            S = ((q * scale).astype(f32) @ k.T).astype(f32)
+            m = np.full(n, -np.inf, f32)
+            l = np.zeros(n, f32)
+            acc = np.zeros((n, dk), f32)
+            for k0 in range(0, int(nk.max()), FFMA_KT):
+                cols = np.arange(k0, min(k0 + FFMA_KT, n))
+                vis = cols[None, :] < nk[:, None]
+                sc = np.where(vis, S[:, cols], -np.inf).astype(f32)
+                mn = np.maximum(m, sc.max(1)) if "no_max" not in corrupt else np.zeros(n, f32)
+                with np.errstate(invalid="ignore"):
+                    corr = np.where(vis.any(1), np.exp(m - mn), f32(1)).astype(f32)
+                with np.errstate(over="ignore", invalid="ignore"):
+                    p = np.where(vis, np.exp(sc - mn[:, None]), 0).astype(f32)
+                with np.errstate(over="ignore", invalid="ignore"):
+                    l = (l * corr + p.sum(1, dtype=f32)).astype(f32)
+                    if "no_rescale" not in corrupt:
+                        acc = (acc * corr[:, None]).astype(f32)
+                    acc = (acc + p @ v[cols]).astype(f32)
+                m = mn
+            with np.errstate(over="ignore", invalid="ignore"):
+                out[r0:r0 + n, h * dk:(h + 1) * dk] = (acc / l[:, None]).astype(f32)
+    return out

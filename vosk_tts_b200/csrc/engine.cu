@@ -915,6 +915,19 @@ struct vtts_engine {
   Buf<T2sPrm> d_t2s_prm;
   Buf<unsigned long long> d_t2s_seed;
   void bind_t2s();
+  // The launches of the text prefill's own kernels, shared by impl_t2s_decode / post_ln_layers and the vtts_debug_t2s_*
+  // hooks.  r holds each utterance's T + P prefill rows; init [n][4] is T, P, the first cache row and the first token slot of
+  // each.  t2s_embed: the [text; prompt] embedding rows of ids into x (bp: bert_proj's output rows, or null for its bias
+  // alone).  t2s_prefix_attn: the attention of the qkv rows under the prefix mask into out.  t2s_relu: ReLU of y in place,
+  // or only into pl.  t2s_kv_store: each qkv row's k, v into cache row init[b][2] + t.  t2s_init: the decode state st, the
+  // prompt tokens in y, the seen bitmap and hx = the pre row T + P - 1 of each of n utterances.  pl (or null): the planes
+  // of what is written.
+  void t2s_embed(const int* ids, const float* bp, float* x, const Planes* pl, const int* init, const Rows& r);
+  void t2s_prefix_attn(const float* qkv, int H, int heads, const int* init, float* out, const Planes* pl, const Rows& r);
+  void t2s_relu(float* y, int C, const Planes* pl, const Rows& r);
+  void t2s_kv_store(const float* qkv, int H, float* kc, float* vc, const int* init, const Rows& r);
+  void t2s_init(const int* init, const int* prompt, const int* poffs, const float* pre, const int* offs, int H, int n, int* st, int* y,
+                unsigned* seen, float* hx);
 
   // ---- StableTTS flow-matching decoder (CFM.forward / solve_euler / Decoder; dit.cuh): fp32 FFMA in modes 0, 1 and 3; in
   //      mode 2 the convs in stp_tc and the attention on the tensor cores (DESIGN.md 4.r)
@@ -3276,20 +3289,10 @@ void vtts_engine::post_ln_layers(const std::vector<EncLayerW>& layers, bool on_t
                                  float* out, const int* out_offs, const Rows& r, bool relu, const std::function<void(int)>* after_qkv,
                                  const int* prefix) {
   float *xa = w.xa, *xb = w.xb;
-  auto prefix_attn = [&](const EncLayerW& Lw, const Planes* pl) {
-    const int dk = H / Lw.heads;
-    klaunch(t2s_prefix_attn_kernel, dim3(r.maxLen, Lw.heads, r.n), dim3(32), (size_t)0, (const float*)w.QKV, H, dk,
-            (float)std::sqrt(1.0 / dk), w.AO, r.lens, r.offs, prefix, pl ? pl->hi : (__nv_bfloat16*)nullptr,
-            pl ? pl->lo : (__nv_bfloat16*)nullptr);
-    CK(cudaGetLastError());
-    ++launches;
-  };
+  auto prefix_attn = [&](const EncLayerW& Lw, const Planes* pl) { t2s_prefix_attn(w.QKV, H, Lw.heads, prefix, w.AO, pl, r); };
   auto act = [&](const Planes* pl) {
     if (!relu) { gelu_rows(w.FF, Fh, pl, r); return; }
-    klaunch(t2s_relu_kernel, dim3(r.maxLen, r.n), dim3(256), (size_t)0, w.FF, Fh, r.lens, r.offs, pl ? pl->hi : (__nv_bfloat16*)nullptr,
-            pl ? pl->lo : (__nv_bfloat16*)nullptr);
-    CK(cudaGetLastError());
-    ++launches;
+    t2s_relu(w.FF, Fh, pl, r);
   };
   for (size_t l = 0; l < layers.size() && on_tc; ++l) {
     const EncLayerW& Lw = layers[l];
@@ -3324,6 +3327,41 @@ void vtts_engine::post_ln_layers(const std::vector<EncLayerW>& layers, bool on_t
     if (l + 1 == layers.size()) ln_rows(w.Y, nullptr, Lw.ln2, eps, out, out_offs, H, nullptr, r);
     else ln_rows(w.Y, nullptr, Lw.ln2, eps, xa, r.offs, H, nullptr, r);
   }
+}
+
+void vtts_engine::t2s_embed(const int* ids, const float* bp, float* x, const Planes* pl, const int* init, const Rows& r) {
+  klaunch(t2s_prefill_embed_kernel, dim3(r.maxLen, r.n), dim3(128), (size_t)0, ids, t2s_temb, t2s_aemb, bp, t2s_bp.b, t2s_pe, t2s_alpha[0],
+          t2s_alpha[1], cfg.cv_hidden, x, r.lens, r.offs, init, pl ? pl->hi : (__nv_bfloat16*)nullptr, pl ? pl->lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::t2s_prefix_attn(const float* qkv, int H, int heads, const int* init, float* out, const Planes* pl, const Rows& r) {
+  const int dk = H / heads;
+  klaunch(t2s_prefix_attn_kernel, dim3(r.maxLen, heads, r.n), dim3(32), (size_t)0, qkv, H, dk, (float)std::sqrt(1.0 / dk), out, r.lens,
+          r.offs, init, pl ? pl->hi : (__nv_bfloat16*)nullptr, pl ? pl->lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::t2s_relu(float* y, int C, const Planes* pl, const Rows& r) {
+  klaunch(t2s_relu_kernel, dim3(r.maxLen, r.n), dim3(256), (size_t)0, y, C, r.lens, r.offs, pl ? pl->hi : (__nv_bfloat16*)nullptr,
+          pl ? pl->lo : (__nv_bfloat16*)nullptr);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::t2s_kv_store(const float* qkv, int H, float* kc, float* vc, const int* init, const Rows& r) {
+  klaunch(t2s_kv_store_kernel, dim3(r.maxLen, r.n), dim3(128), (size_t)0, qkv, H, kc, vc, r.lens, r.offs, init);
+  CK(cudaGetLastError());
+  ++launches;
+}
+
+void vtts_engine::t2s_init(const int* init, const int* prompt, const int* poffs, const float* pre, const int* offs, int H, int n, int* st,
+                           int* y, unsigned* seen, float* hx) {
+  klaunch(t2s_init_kernel, dim3(n), dim3(256), (size_t)0, init, prompt, poffs, pre, offs, H, t2s_vocab, st, y, seen, hx);
+  CK(cudaGetLastError());
+  ++launches;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -3508,7 +3546,9 @@ void vtts_engine::bind_t2s() {
     }
     t2s_enc.push_back(L);
   }
-  CK(cudaFuncSetAttribute(t2s_ffn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T2S_GEMV_SMEM(F)));
+  // The attribute belongs to the kernel, not to this engine: sized for the widest FFN any engine takes, so that binding an
+  // engine with a narrower FFN cannot lower it under another engine of the process.
+  CK(cudaFuncSetAttribute(t2s_ffn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T2S_GEMV_SMEM(T2S_MAX_V)));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -4773,16 +4813,9 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
     h->launch_conv({mk(h->t2s_bp, h->d_t2s_bert.p, vtts_engine::T2S_BERT, 0, dbp, H, 0, 1, 0)}, 1, r);
     bp = dbp;
   }
-  h->klaunch(t2s_prefill_embed_kernel, dim3(maxT, B), dim3(128), (size_t)0, (const int*)(di + 7 * B), h->t2s_temb, h->t2s_aemb, bp,
-             h->t2s_bp.b, h->t2s_pe, h->t2s_alpha[0], h->t2s_alpha[1], H, w.xa, dlen, doff, dinit,
-             h->t2s_tc ? w.PX.hi : (__nv_bfloat16*)nullptr, h->t2s_tc ? w.PX.lo : (__nv_bfloat16*)nullptr);
-  CK(cudaGetLastError());
-  ++h->launches;
+  h->t2s_embed(di + 7 * B, bp, w.xa, h->t2s_tc ? &w.PX : nullptr, dinit, r);
   const std::function<void(int)> store = [&](int l) {
-    h->klaunch(t2s_kv_store_kernel, dim3(maxT, B), dim3(128), (size_t)0, (const float*)w.QKV, H, kc + (size_t)l * kvn * H,
-               vc + (size_t)l * kvn * H, dlen, doff, dinit);
-    CK(cudaGetLastError());
-    ++h->launches;
+    h->t2s_kv_store(w.QKV, H, kc + (size_t)l * kvn * H, vc + (size_t)l * kvn * H, dinit, r);
   };
   float* pre = h->ensure(h->d_t2s_pre, (size_t)tot * H);
   h->post_ln_layers(h->t2s_enc, h->t2s_tc, H, F, c.cv_ln_eps, w, pre, doff, r, true, &store, dinit);
@@ -4799,10 +4832,7 @@ static void impl_t2s_decode(vtts_handle h, const int64_t* ids, const int64_t* le
         *hx = y2 + (size_t)B * H, *ff = hx + (size_t)B * H, *lg = ff + (size_t)B * F;
   float* part = h->ensure(h->d_t2s_part, (size_t)B * nh * nsplit * (dk + 2));
   CK(cudaMemsetAsync(nstop, 0, sizeof(int), s));
-  h->klaunch(t2s_init_kernel, dim3(B), dim3(256), (size_t)0, dinit, (const int*)(di + 7 * B + tot), (const int*)(di + 6 * B), (const float*)pre,
-             doff, H, V, dst, dy, seen, hx);
-  CK(cudaGetLastError());
-  ++h->launches;
+  h->t2s_init(dinit, di + 7 * B + tot, di + 6 * B, pre, doff, H, B, dst, dy, seen, hx);
   std::vector<T2sLayer> Ls(NL);
   for (int l = 0; l < NL; ++l) {
     const EncLayerW& E = h->t2s_enc[l];
@@ -6888,7 +6918,7 @@ int vtts_debug_dit_norm(vtts_handle h, int B, const int* lens, size_t rows, int 
 int vtts_debug_act(vtts_handle h, int act, int B, const int* lens, size_t rows, int C, float* y, uint16_t* hi, uint16_t* lo) {
   return guarded(h, [&] {
     REQUIRE(y, VTTS_ERR_INVALID, "debug_act: missing rows");
-    REQUIRE(act == 0 || act == 1, VTTS_ERR_INVALID, "debug_act: act must be 0 (GELU) or 1 (SiLU)");
+    REQUIRE(act >= 0 && act <= 2, VTTS_ERR_INVALID, "debug_act: act must be 0 (GELU), 1 (SiLU) or 2 (ReLU)");
     REQUIRE(C >= 1, VTTS_ERR_INVALID, "debug_act: C must be >= 1");
     const bool planes = hook_planes("debug_act", hi, nullptr, lo);
     HookRows hr = hook_rows("debug_act", B, lens, rows);
@@ -6901,7 +6931,8 @@ int vtts_debug_act(vtts_handle h, int act, int B, const int* lens, size_t rows, 
     const Planes pl = upload_planes(dev, hi, nullptr, lo, n, st);
     const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
     if (act == 0) h->gelu_rows(dy, C, planes ? &pl : nullptr, r);
-    else h->silu_rows(dy, C, planes ? &pl : nullptr, r);
+    else if (act == 1) h->silu_rows(dy, C, planes ? &pl : nullptr, r);
+    else h->t2s_relu(dy, C, planes ? &pl : nullptr, r);
     CK(cudaStreamSynchronize(st));
     CK(cudaMemcpy(y, dy, n * 4, cudaMemcpyDeviceToHost));
     if (planes) {
@@ -6909,6 +6940,169 @@ int vtts_debug_act(vtts_handle h, int act, int B, const int* lens, size_t rows, 
       CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
     }
   }, G_ATOMIC, ANY_FAMILY);
+}
+
+namespace {
+
+// Utterances of the text-prefill hooks packed as impl_t2s_decode packs them: T[b] + P[b] rows from a multiple of 8, with no
+// gap, checked against the caller's row count; init [B][4] = T, P, 0, 0 (t2s_init_kernel's first cache row and token slot
+// are set by the caller).
+HookRows t2s_hook_rows(const char* who, int B, const int* T, const int* P, size_t rows, std::vector<int>& init) {
+  REQUIRE(T && P && B >= 1 && B <= 4096, VTTS_ERR_INVALID, std::string(who) + ": bad batch size or missing lengths");
+  HookRows hr;
+  hr.len.assign(B, 0);
+  hr.off.assign(B + 1, 0);
+  init.assign(4 * (size_t)B, 0);
+  int64_t tot = 0;
+  for (int b = 0; b < B; ++b) {
+    REQUIRE(T[b] >= 1 && P[b] >= 0 && (int64_t)T[b] + P[b] < (1 << 24), VTTS_ERR_INVALID,
+            std::string(who) + ": T must be >= 1 and P >= 0");
+    hr.len[b] = T[b] + P[b];
+    hr.off[b] = (int)tot;
+    tot += (hr.len[b] + 7) / 8 * 8;
+    REQUIRE(tot < (1 << 24), VTTS_ERR_INVALID, std::string(who) + ": the batch holds too many rows");
+    hr.maxLen = std::max(hr.maxLen, hr.len[b]);
+    init[4 * b] = T[b];
+    init[4 * b + 1] = P[b];
+  }
+  hr.off[B] = (int)tot;
+  REQUIRE(rows >= (size_t)tot, VTTS_ERR_INVALID, std::string(who) + ": fewer rows than the packed utterances");
+  return hr;
+}
+
+}  // namespace
+
+int vtts_debug_t2s_prefix_attn(vtts_handle h, int H, int heads, int B, const int* T, const int* P, int launch_rows, size_t rows,
+                               const float* qkv, float* out, uint16_t* hi, uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(qkv && out, VTTS_ERR_INVALID, "debug_t2s_prefix_attn: missing input or output");
+    REQUIRE(heads >= 1 && heads <= 65535 && H >= 1 && H % heads == 0 && (H / heads) % 32 == 0 && H / heads <= 128, VTTS_ERR_INVALID,
+            "debug_t2s_prefix_attn: t2s_prefix_attn_kernel needs H = heads * dk, dk a multiple of 32 up to 128");
+    const bool planes = hook_planes("debug_t2s_prefix_attn", hi, nullptr, lo);
+    std::vector<int> init;
+    HookRows hr = t2s_hook_rows("debug_t2s_prefix_attn", B, T, P, rows, init);
+    REQUIRE(launch_rows == 0 || (launch_rows >= hr.maxLen && launch_rows < (1 << 24)), VTTS_ERR_INVALID,
+            "debug_t2s_prefix_attn: launch_rows must be 0 or at least the longest T + P");
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * H;
+    const int* dinit = static_cast<const int*>(upload(dev, init.data(), init.size() * 4, st));
+    const float* dqkv = static_cast<const float*>(upload(dev, qkv, 3 * n * 4, st));
+    float* dout = static_cast<float*>(upload(dev, out, n * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, n, st);
+    const Rows r{hr.lens(), hr.offs(), B, launch_rows ? launch_rows : hr.maxLen, hr.len, hr.len, h->tune};
+    h->t2s_prefix_attn(dqkv, H, heads, dinit, dout, planes ? &pl : nullptr, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(out, dout, n * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, n * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, ANY_FAMILY);
+}
+
+int vtts_debug_t2s_embed(vtts_handle h, int B, const int* T, const int* P, size_t rows, const int* ids, const float* bert_proj, float* x,
+                         uint16_t* hi, uint16_t* lo) {
+  return guarded(h, [&] {
+    REQUIRE(ids && x, VTTS_ERR_INVALID, "debug_t2s_embed: missing ids or output");
+    const int H = h->cfg.cv_hidden;
+    const bool planes = hook_planes("debug_t2s_embed", hi, nullptr, lo);
+    std::vector<int> init;
+    HookRows hr = t2s_hook_rows("debug_t2s_embed", B, T, P, rows, init);
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(T[b] <= h->t2s_npos && P[b] <= h->t2s_npos, VTTS_ERR_INVALID, "debug_t2s_embed: T or P is longer than the position table");
+      for (int t = 0; t < hr.len[b]; ++t) {
+        const int v = ids[hr.off[b] + t];
+        REQUIRE(v >= 0 && v < (t < T[b] ? h->t2s_text_vocab : h->t2s_vocab), VTTS_ERR_INVALID,
+                "debug_t2s_embed: an id is outside its embedding table");
+      }
+    }
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const size_t n = rows * H;
+    const int* dinit = static_cast<const int*>(upload(dev, init.data(), init.size() * 4, st));
+    const int* did = static_cast<const int*>(upload(dev, ids, rows * 4, st));
+    const float* dbp = bert_proj ? static_cast<const float*>(upload(dev, bert_proj, n * 4, st)) : nullptr;
+    float* dx = static_cast<float*>(upload(dev, x, n * 4, st));
+    const Planes pl = upload_planes(dev, hi, nullptr, lo, n, st);
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->t2s_embed(did, dbp, dx, planes ? &pl : nullptr, dinit, r);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(x, dx, n * 4, cudaMemcpyDeviceToHost));
+    if (planes) {
+      CK(cudaMemcpy(hi, pl.hi, n * 2, cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(lo, pl.lo, n * 2, cudaMemcpyDeviceToHost));
+    }
+  }, G_ATOMIC, VTTS_FAMILY_T2S);
+}
+
+int vtts_debug_t2s_state(vtts_handle h, int B, const int* T, const int* P, size_t rows, const float* qkv, const float* pre, const int* prompts,
+                         const int* kv_off, size_t kv_rows, float* kc, float* vc, const int* y_off, size_t y_len, int32_t* state, int32_t* y,
+                         uint32_t* seen, size_t seen_len, float* hx) {
+  return guarded(h, [&] {
+    REQUIRE(qkv && pre && kv_off && kc && vc && y_off && y && state && seen && hx, VTTS_ERR_INVALID,
+            "debug_t2s_state: missing input or output");
+    const int H = h->cfg.cv_hidden, V = h->t2s_vocab, nw = (V + 31) / 32;
+    std::vector<int> init;
+    HookRows hr = t2s_hook_rows("debug_t2s_state", B, T, P, rows, init);
+    REQUIRE(kv_rows < (1u << 28) && y_len < (1u << 28), VTTS_ERR_INVALID, "debug_t2s_state: caches or y too large");
+    REQUIRE(seen_len >= (size_t)B * nw && seen_len < (1u << 28), VTTS_ERR_INVALID, "debug_t2s_state: seen holds fewer than B rows of (V + 31) / 32 words");
+    std::vector<int> poff(B, 0);
+    int ptot = 0;
+    for (int b = 0; b < B; ++b) {
+      REQUIRE(kv_off[b] >= 0 && (size_t)kv_off[b] + hr.len[b] <= kv_rows, VTTS_ERR_INVALID,
+              "debug_t2s_state: an utterance's cache rows pass kv_rows");
+      REQUIRE(y_off[b] >= 0 && (size_t)y_off[b] + P[b] <= y_len, VTTS_ERR_INVALID, "debug_t2s_state: an utterance's token slots pass y_len");
+      init[4 * b + 2] = kv_off[b];
+      init[4 * b + 3] = y_off[b];
+      poff[b] = ptot;
+      for (int i = 0; i < P[b]; ++i)
+        REQUIRE(prompts && prompts[ptot + i] >= 0 && prompts[ptot + i] < V - 1, VTTS_ERR_INVALID,
+                "debug_t2s_state: a prompt token is outside [0, EOS)");
+      ptot += P[b];
+    }
+    // the utterances' cache regions [kv_off, + T + P) and token regions [y_off, + P) must not overlap: t2s_kv_store_kernel
+    // and t2s_init_kernel write them from different CTAs
+    auto disjoint = [&](const int* off, bool tokens) {
+      std::vector<std::pair<int, int>> reg;
+      for (int b = 0; b < B; ++b)
+        if (tokens ? P[b] > 0 : true) reg.push_back({off[b], off[b] + (tokens ? P[b] : hr.len[b])});
+      std::sort(reg.begin(), reg.end());
+      for (size_t i = 1; i < reg.size(); ++i)
+        if (reg[i].first < reg[i - 1].second) return false;
+      return true;
+    };
+    REQUIRE(disjoint(kv_off, false) && disjoint(y_off, true), VTTS_ERR_INVALID, "debug_t2s_state: two utterances' cache or token regions overlap");
+    std::vector<Buf<char>> dev;
+    cudaStream_t st = h->stream;
+    CK(cudaStreamSynchronize(st));
+    upload_rows(hr, dev, st);
+    const int* dinit = static_cast<const int*>(upload(dev, init.data(), init.size() * 4, st));
+    const int* dpoff = static_cast<const int*>(upload(dev, poff.data(), poff.size() * 4, st));
+    const int* dpr = static_cast<const int*>(upload(dev, prompts, (size_t)ptot * 4, st));
+    const float* dqkv = static_cast<const float*>(upload(dev, qkv, rows * 3 * H * 4, st));
+    const float* dpre = static_cast<const float*>(upload(dev, pre, rows * H * 4, st));
+    float* dkc = static_cast<float*>(upload(dev, kc, kv_rows * H * 4, st));
+    float* dvc = static_cast<float*>(upload(dev, vc, kv_rows * H * 4, st));
+    int* dst = static_cast<int*>(upload(dev, state, (size_t)B * T2S_ST * 4, st));
+    int* dy = static_cast<int*>(upload(dev, y, y_len * 4, st));
+    unsigned* dsn = static_cast<unsigned*>(upload(dev, seen, seen_len * 4, st));
+    float* dhx = static_cast<float*>(upload(dev, hx, (size_t)B * H * 4, st));
+    const Rows r{hr.lens(), hr.offs(), B, hr.maxLen, hr.len, hr.len, h->tune};
+    h->t2s_kv_store(dqkv, H, dkc, dvc, dinit, r);
+    h->t2s_init(dinit, dpr, dpoff, dpre, hr.offs(), H, B, dst, dy, dsn, dhx);
+    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpy(kc, dkc, kv_rows * H * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(vc, dvc, kv_rows * H * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(state, dst, (size_t)B * T2S_ST * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(y, dy, y_len * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(seen, dsn, seen_len * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(hx, dhx, (size_t)B * H * 4, cudaMemcpyDeviceToHost));
+  }, G_ATOMIC, VTTS_FAMILY_T2S);
 }
 
 int vtts_debug_gate(vtts_handle h, int B, const int* lens, size_t rows, int C, const float* x, const float* y, const float* ada, int ada_ld,

@@ -67,7 +67,8 @@ EXPORTS = ["vtts_create", "vtts_destroy", "vtts_last_error", "vtts_durations", "
            "vtts_debug_dds", "vtts_debug_spline", "vtts_debug_durations", "vtts_debug_stt_durations", "vtts_debug_noise", "vtts_t2s_decode",
            "vtts_debug_t2s_sample", "vtts_debug_front_end", "vtts_debug_istft", "vtts_debug_mrf_mean",
            "vtts_sovits_semantic", "vtts_sovits_latent", "vtts_debug_add_ln", "vtts_debug_ln", "vtts_debug_bert_embed",
-           "vtts_debug_dit_norm", "vtts_debug_act", "vtts_debug_gate", "vtts_debug_groupnorm"]
+           "vtts_debug_dit_norm", "vtts_debug_act", "vtts_debug_gate", "vtts_debug_groupnorm", "vtts_debug_t2s_prefix_attn",
+           "vtts_debug_t2s_embed", "vtts_debug_t2s_state"]
 
 MODEL_FAMILIES = {"vits2": 0, "quickvc": 1, "stabletts": 2, "t2s": 3, "sovits": 4}    # vtts_config.model_family
 CFM_MAX_STEPS = 64       # VTTS_CFM_MAX_STEPS
@@ -302,6 +303,12 @@ def load_library(build_if_missing=True):
     lib.vtts_debug_t2s_sample.argtypes = [vp, i32, vp, vp, vp, i32, i32, C.c_float, C.c_float, C.c_float, i32, i32, vp, vp, i32, vp, vp,
                                           vp, i32]
     lib.vtts_debug_t2s_sample.restype = i32
+    lib.vtts_debug_t2s_prefix_attn.argtypes = [vp, i32, i32, i32, vp, vp, i32, sz, vp, vp, vp, vp]
+    lib.vtts_debug_t2s_prefix_attn.restype = i32
+    lib.vtts_debug_t2s_embed.argtypes = [vp, i32, vp, vp, sz, vp, vp, vp, vp, vp]
+    lib.vtts_debug_t2s_embed.restype = i32
+    lib.vtts_debug_t2s_state.argtypes = [vp, i32, vp, vp, sz, vp, vp, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp, sz, vp]
+    lib.vtts_debug_t2s_state.restype = i32
     for fn in (lib.vtts_sovits_semantic, lib.vtts_sovits_latent):
         fn.argtypes = [vp, vp, vp, i32, C.c_int64, vp, C.c_int64, vp]
         fn.restype = i32
@@ -1443,11 +1450,12 @@ class Engine:
 
     def debug_act(self, act, lens, y, hi=None, lo=None):
         """An activation pass (vtts_debug_act) on y float32 [rows, C]: act "gelu" (cv_gelu_kernel: in place, or into hi / lo
-        only) or "silu" (dit_silu_kernel, or dit_silu_planes_kernel with hi / lo).  Returns (y, hi, lo)."""
+        only), "silu" (dit_silu_kernel, or dit_silu_planes_kernel with hi / lo) or "relu" (t2s_relu_kernel: in place, or into
+        hi / lo only).  Returns (y, hi, lo)."""
         lens, y = self._rows(lens, y, "y")
         y = y.copy()
         hi, lo = self._hook_arrays([("hi", hi, np.uint16, y.shape), ("lo", lo, np.uint16, y.shape)])
-        self._check(self.lib.vtts_debug_act(self.h, {"gelu": 0, "silu": 1}[act], lens.size, _ptr(lens), y.shape[0], y.shape[1], _ptr(y),
+        self._check(self.lib.vtts_debug_act(self.h, {"gelu": 0, "silu": 1, "relu": 2}[act], lens.size, _ptr(lens), y.shape[0], y.shape[1], _ptr(y),
                                             _ptr(hi), _ptr(lo)))
         return y, hi, lo
 
@@ -1505,6 +1513,70 @@ class Engine:
                                                    _ptr(seeds), _ptr(q), 0 if q is None else q.shape[1], _ptr(seen), _ptr(ns),
                                                    _ptr(raw), 0 if raw is None else raw.shape[1]))
         return dict(state=state, y=y, seen=seen, n_stopped=int(ns[0]), raw=raw)
+
+    # ---- the text prefill's kernels (include/vtts.h): utterance b's T[b] + P[b] rows packed from a multiple of 8 with no gap
+    #      (t2s_prefill_ref.offsets); every output array is an initial content that what the kernel does not write keeps
+
+    def _tp(self, T, P):
+        T = np.ascontiguousarray(T, dtype=np.int32).reshape(-1)
+        P = np.ascontiguousarray(P, dtype=np.int32).reshape(-1)
+        if T.shape != P.shape:
+            raise ValueError("T and P: one length each per utterance")
+        return T, P
+
+    def debug_t2s_prefix_attn(self, T, P, heads, qkv, out, hi=None, lo=None, launch_rows=0):
+        """t2s_prefix_attn_kernel (vtts_debug_t2s_prefix_attn) on qkv float32 [rows, 3H]: row t of an utterance attends to key
+        k iff k < T or k <= t; out float32 [rows, H], hi / lo uint16 [rows, H].  launch_rows: the grid's rows (0: the longest
+        T + P).  Returns (out, hi, lo)."""
+        T, P = self._tp(T, P)
+        qkv = np.ascontiguousarray(qkv, dtype=np.float32)
+        if qkv.ndim != 2 or qkv.shape[1] % 3:
+            raise ValueError("qkv: shape %s, expected (rows, 3H)" % (qkv.shape,))
+        rows, H = qkv.shape[0], qkv.shape[1] // 3
+        out, hi, lo = self._hook_arrays([("out", out, np.float32, (rows, H)), ("hi", hi, np.uint16, (rows, H)),
+                                         ("lo", lo, np.uint16, (rows, H))])
+        self._check(self.lib.vtts_debug_t2s_prefix_attn(self.h, H, int(heads), T.size, _ptr(T), _ptr(P), int(launch_rows), rows,
+                                                        _ptr(qkv), _ptr(out), _ptr(hi), _ptr(lo)))
+        return out, hi, lo
+
+    def debug_t2s_embed(self, T, P, ids, x, bert_proj=None, hi=None, lo=None):
+        """t2s_prefill_embed_kernel (vtts_debug_t2s_embed) with the engine's tables: ids int32 [rows] (phone ids on text rows,
+        semantic tokens on prompt rows), bert_proj float32 [rows, H] or None (bert_proj's bias alone); x float32 [rows, H], hi /
+        lo uint16 [rows, H].  Returns (x, hi, lo)."""
+        T, P = self._tp(T, P)
+        H = int(self.cfg["cv_hidden"])
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        if ids.ndim != 1:
+            raise ValueError("ids: shape %s, expected (rows,)" % (ids.shape,))
+        rows = ids.size
+        x, bert_proj, hi, lo = self._hook_arrays([("x", x, np.float32, (rows, H)), ("bert_proj", bert_proj, np.float32, (rows, H)),
+                                                  ("hi", hi, np.uint16, (rows, H)), ("lo", lo, np.uint16, (rows, H))])
+        self._check(self.lib.vtts_debug_t2s_embed(self.h, T.size, _ptr(T), _ptr(P), rows, _ptr(ids), _ptr(bert_proj), _ptr(x), _ptr(hi),
+                                                  _ptr(lo)))
+        return x, hi, lo
+
+    def debug_t2s_state(self, T, P, qkv, pre, prompts, kv_off, kc, vc, y_off, y, state, seen, hx):
+        """t2s_kv_store_kernel then t2s_init_kernel (vtts_debug_t2s_state): qkv float32 [rows, 3H], pre float32 [rows, H],
+        prompts int32 [sum P] (the prompts back to back); kv_off, y_off int32 [B]: each utterance's first cache row and token
+        slot.  In/out: kc, vc float32 [kv_rows, H], y int32 [y_len], state int32 [B, 8], seen uint32 [seen_len >= B nw] (row b
+        of the bitmap at words [b nw, (b + 1) nw), nw = (V + 31) // 32; words behind the B rows are kept), hx float32 [B, H].
+        Returns a dict of kc, vc, y, state, seen, hx."""
+        T, P = self._tp(T, P)
+        B, H, V = T.size, int(self.cfg["cv_hidden"]), int(self.cfg["t2s_vocab"])
+        qkv = np.ascontiguousarray(qkv, dtype=np.float32)
+        if qkv.ndim != 2 or qkv.shape[1] != 3 * H:
+            raise ValueError("qkv: shape %s, expected (rows, %d)" % (qkv.shape, 3 * H))
+        rows = qkv.shape[0]
+        kc = np.ascontiguousarray(kc, dtype=np.float32)
+        pre, prompts, kv_off, kc, vc, y_off, y, state, seen, hx = self._hook_arrays([
+            ("pre", pre, np.float32, (rows, H)), ("prompts", prompts, np.int32, (int(P.sum()),)), ("kv_off", kv_off, np.int32, (B,)),
+            ("kc", kc, np.float32, (None, H)), ("vc", vc, np.float32, kc.shape), ("y_off", y_off, np.int32, (B,)),
+            ("y", y, np.int32, (None,)), ("state", state, np.int32, (B, 8)), ("seen", seen, np.uint32, (None,)),
+            ("hx", hx, np.float32, (B, H))])
+        self._check(self.lib.vtts_debug_t2s_state(self.h, B, _ptr(T), _ptr(P), rows, _ptr(qkv), _ptr(pre), _ptr(prompts), _ptr(kv_off),
+                                                  kc.shape[0], _ptr(kc), _ptr(vc), _ptr(y_off), y.size, _ptr(state), _ptr(y), _ptr(seen),
+                                                  seen.size, _ptr(hx)))
+        return dict(kc=kc, vc=vc, y=y, state=state, seen=seen, hx=hx)
 
     def debug_durations(self, lens, z, length_scale, stats, eps, noise_scale, frame_rows, frame_cap=0, wceil=None, cum=None, z_p=None,
                         frame_token=None):
