@@ -152,70 +152,143 @@ __device__ __forceinline__ void tc_release(uint64_t* bar, int n) {
   }
 }
 
-// ---- epilogue of one accumulator pair: columns (c, c+1) of output row `orow`; v0/v1 are the accumulator (or the split-K sum)
-__device__ __forceinline__ float tc_bias(const TcProblemBase& P, int b, int c) {
-  float bv = P.bias[c];
-  if (P.cond) bv += P.cond[(long)b * P.cond_ld + c];
-  return bv;
+// ---- epilogue: acc (+ split partials) + bias (+ cond) -> gate / ReLU -> x alpha -> + residual -> fp32 rows and/or the
+// split-bf16 planes of lrelu(., pl_slope) for the next conv.  A consumer thread finishes its tile share one column pair at a
+// time, in both of its rows: every global load of a column pair (bias, cond, the residual of both rows) is issued before any
+// of its stores, and the next column pair's loads before the current one's stores.  (y and res may alias -- the in-place
+// residuals of the WN stacks and the flow's post conv -- so the compiler keeps loads and stores in source order: one
+// (row, column pair) at a time made every pair a serial global round trip.)  Loading later pairs ahead of earlier pairs'
+// stores is safe under that aliasing: each element is read and written by the one thread that finishes it, and read first.
+
+// The epilogue operands of one problem, read out of the launch descriptor once per tile.
+struct TcEpi {
+  const float* bias;
+  const float* cond;          // this utterance's conditioning row (or null)
+  const float* res;           // (null with dbgskip & 4)
+  float* y;
+  __nv_bfloat16 *p_hi, *p_lo, *p_mid;
+  int ldr, roff, ldy, yoff, ldp, poff;
+  int ncol;                   // output channels: Cout, or Cout / 2 behind the gate
+  float alpha, pl_slope;
+  bool gate, relu, store;     // store: false with dbgskip & 1
+};
+template <class PT>
+__device__ __forceinline__ TcEpi tc_epi(const PT& P, int b, int dbgskip) {
+  TcEpi E;
+  E.bias = P.bias;
+  E.cond = P.cond ? P.cond + (long)b * P.cond_ld : nullptr;
+  E.res = (dbgskip & 4) ? nullptr : P.res;
+  E.y = P.y;
+  E.p_hi = P.p_hi; E.p_lo = P.p_lo; E.p_mid = P.p_mid;
+  E.ldr = P.ldr; E.roff = P.roff; E.ldy = P.ldy; E.yoff = P.yoff; E.ldp = P.ldp; E.poff = P.poff;
+  E.gate = (P.epi & TCE_GATE) != 0;
+  E.relu = (P.epi & TCE_RELU) != 0;
+  E.ncol = E.gate ? P.Cout >> 1 : P.Cout;
+  E.alpha = P.alpha; E.pl_slope = P.pl_slope;
+  E.store = !(dbgskip & 1);
+  return E;
 }
-__device__ __forceinline__ void tc_epi_pair(const TcProblemBase& P, int b, long orow, int c, float v0, float v1, int dbgskip) {
-  const bool gate = (P.epi & TCE_GATE) != 0;
+// One column pair of a consumer thread: accumulator columns (c, c + 1), in each of the thread's two rows.  Gate: the pair
+// makes output channel oc = c / 2.
+struct TcEpiCol {
+  int c, oc, nout;
+  bool ok;                    // the pair exists in this thread's share of the tile and has an output channel
+};
+__device__ __forceinline__ TcEpiCol tc_epi_col(const TcEpi& E, int c, bool in_tile) {
+  TcEpiCol k;
+  k.c = c;
+  k.oc = E.gate ? c >> 1 : c;
+  k.ok = in_tile && k.oc < E.ncol;
+  k.nout = E.gate ? 1 : min(2, E.ncol - k.oc);
+  return k;
+}
+// The global loads of one column pair: bias and cond of its columns, the residual of each row (rowok: the row lies in the
+// utterance).
+struct TcEpiIn {
+  float b0, b1, c0, c1, r[2][2];
+};
+__device__ __forceinline__ TcEpiIn tc_epi_load(const TcEpi& E, const TcEpiCol& k, const long (&orow)[2], const bool (&rowok)[2]) {
+  TcEpiIn in = {};
+  if (!(k.ok && (rowok[0] || rowok[1]))) return in;
+  const bool two = E.gate || k.nout > 1;       // columns c and c + 1 are both used
+  in.b0 = E.bias[k.c];
+  if (two) in.b1 = E.bias[k.c + 1];
+  if (E.cond) {
+    in.c0 = E.cond[k.c];
+    if (two) in.c1 = E.cond[k.c + 1];
+  }
+  if (E.res) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!rowok[h]) continue;
+      const float* rp = E.res + orow[h] * (long)E.ldr + E.roff + k.oc;
+      if (k.nout == 2 && ((E.ldr | E.roff | k.oc) & 1) == 0) {
+        const float2 q2 = *reinterpret_cast<const float2*>(rp);
+        in.r[h][0] = q2.x; in.r[h][1] = q2.y;
+      } else {
+        in.r[h][0] = rp[0];
+        if (k.nout > 1) in.r[h][1] = rp[1];
+      }
+    }
+  }
+  return in;
+}
+// The arithmetic and the stores of column pair `k` in output row `orow`, whose loads have landed: bias b, cond c, residual
+// r; v0 / v1 = the accumulator (or the split-K sum).  (alpha and the residual are an explicit multiply and add, never one
+// fused multiply-add.)
+__device__ __forceinline__ void tc_epi_store(const TcEpi& E, const TcEpiCol& k, long orow, float b0, float b1, float c0, float c1,
+                                             float r0, float r1, float v0, float v1) {
+  const float bv0 = E.cond ? b0 + c0 : b0, bv1 = E.cond ? b1 + c1 : b1;
   float u[2];
-  int oc, nout;
-  if (gate) {                                   // channel pair (2i, 2i+1) makes output channel i
-    oc = c >> 1;
-    if (oc >= (P.Cout >> 1)) return;
-    nout = 1;
-    const float a = v0 + tc_bias(P, b, c), s = v1 + tc_bias(P, b, c + 1);
+  if (E.gate) {
+    const float a = v0 + bv0, s = v1 + bv1;
     u[0] = tanhf(a) * (1.f / (1.f + expf(-s)));
     u[1] = 0.f;
   } else {
-    oc = c;
-    if (oc >= P.Cout) return;
-    nout = min(2, P.Cout - oc);
-    u[0] = v0 + tc_bias(P, b, c);
-    u[1] = nout > 1 ? v1 + tc_bias(P, b, c + 1) : 0.f;
+    u[0] = v0 + bv0;
+    u[1] = k.nout > 1 ? v1 + bv1 : 0.f;
   }
-  const bool relu = (P.epi & TCE_RELU) != 0;
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     float q = u[e];
-    if (relu) q = fmaxf(q, 0.f);
-    u[e] = q * P.alpha;
+    if (E.relu) q = fmaxf(q, 0.f);
+    u[e] = __fmul_rn(q, E.alpha);
   }
-  if (P.res && !(dbgskip & 4)) {
-    const float* rp = P.res + orow * (long)P.ldr + P.roff + oc;
-    if (nout == 2 && ((P.ldr | P.roff | oc) & 1) == 0) {
-      const float2 q2 = *reinterpret_cast<const float2*>(rp);
-      u[0] += q2.x; u[1] += q2.y;
+  if (E.res) {
+    u[0] = __fadd_rn(u[0], r0);
+    if (k.nout > 1) u[1] = __fadd_rn(u[1], r1);
+  }
+  if (!E.store) return;
+  const int oc = k.oc, nout = k.nout;
+  if (E.y) {
+    float* yr = E.y + orow * (long)E.ldy + E.yoff + oc;
+    if (nout == 2 && ((E.ldy | E.yoff | oc) & 1) == 0) {
+      *reinterpret_cast<float2*>(yr) = make_float2(u[0], u[1]);
     } else {
-      for (int e = 0; e < nout; ++e) u[e] += rp[e];
+      yr[0] = u[0];
+      if (nout > 1) yr[1] = u[1];
     }
   }
-  if (dbgskip & 1) return;
-  if (P.y) {
-    float* yr = P.y + orow * (long)P.ldy + P.yoff + oc;
-    if (nout == 2 && ((P.ldy | P.yoff | oc) & 1) == 0) *reinterpret_cast<float2*>(yr) = make_float2(u[0], u[1]);
-    else for (int e = 0; e < nout; ++e) yr[e] = u[e];
-  }
-  if (P.p_hi) {
-    const long po = orow * (long)P.ldp + P.poff + oc;
-    __align__(4) __nv_bfloat16 hb[2], mb[2], lb[2];
+  if (E.p_hi) {
+    const long po = orow * (long)E.ldp + E.poff + oc;
+    __nv_bfloat16 hb[2], mb[2], lb[2];
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
       float q = u[e];
-      q = q > 0.f ? q : q * P.pl_slope;
-      if (P.p_mid) split_bf16_3(q, hb[e], mb[e], lb[e]);
+      q = q > 0.f ? q : q * E.pl_slope;
+      if (E.p_mid) split_bf16_3(q, hb[e], mb[e], lb[e]);
       else split_bf16(q, hb[e], lb[e]);
     }
-    if (nout == 2 && ((P.ldp | P.poff | oc) & 1) == 0) {
-      *reinterpret_cast<uint32_t*>(P.p_hi + po) = *reinterpret_cast<const uint32_t*>(hb);
-      *reinterpret_cast<uint32_t*>(P.p_lo + po) = *reinterpret_cast<const uint32_t*>(lb);
-      if (P.p_mid) *reinterpret_cast<uint32_t*>(P.p_mid + po) = *reinterpret_cast<const uint32_t*>(mb);
+    if (nout == 2 && ((E.ldp | E.poff | oc) & 1) == 0) {
+      *reinterpret_cast<__nv_bfloat162*>(E.p_hi + po) = __halves2bfloat162(hb[0], hb[1]);
+      *reinterpret_cast<__nv_bfloat162*>(E.p_lo + po) = __halves2bfloat162(lb[0], lb[1]);
+      if (E.p_mid) *reinterpret_cast<__nv_bfloat162*>(E.p_mid + po) = __halves2bfloat162(mb[0], mb[1]);
     } else {
-      for (int e = 0; e < nout; ++e) {
-        P.p_hi[po + e] = hb[e]; P.p_lo[po + e] = lb[e];
-        if (P.p_mid) P.p_mid[po + e] = mb[e];
+      E.p_hi[po] = hb[0]; E.p_lo[po] = lb[0];
+      if (E.p_mid) E.p_mid[po] = mb[0];
+      if (nout > 1) {
+        E.p_hi[po + 1] = hb[1]; E.p_lo[po + 1] = lb[1];
+        if (E.p_mid) E.p_mid[po + 1] = mb[1];
       }
     }
   }
@@ -521,6 +594,28 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
         }
         if (++j == P.k) j = 0;
       }
+      // ---- epilogue.  This thread finishes the column pairs j = 0 .. W/8 - 1 of the tile's columns [co0 + sp W, + W) that
+      // its CTA owns (W = BN unsplit): columns 8 j + 2 q4 of rows rbase and rbase + 8.  Unsplit, pair j of row h is the
+      // accumulator pair (acc[4j + 2h], acc[4j + 2h + 1]).  The loops are not unrolled, so the epilogue is one copy of its
+      // code: unrolled over a tile's pairs it ran once per CTA from a cold instruction cache and cost 6-12 us of every
+      // split-K launch (CTA 0 stamps, tools/decoder_phases.py).
+      const int W = BN / T.s, ncp = W / 8;
+      const TcEpi E = tc_epi(P, T.b, tb.dbgskip);
+      const int cbase = T.co0 + T.sp * W + 2 * q4;
+      long orow[2];
+      bool rowok[2];
+      {
+        const long out_base = (long)offs[T.b] * tb.rmul * P.out_mul + (long)T.b * P.out_seq_extra;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int t = T.t0 + rbase + 8 * h;
+          rowok[h] = t < L;
+          orow[h] = out_base + (long)t * P.out_mul + P.out_add;
+        }
+      }
+      auto col = [&](int j) { return tc_epi_col(E, cbase + 8 * j, j < ncp); };
+      // the first pair's loads go out before the last MMAs retire (and before the split-K cluster barriers)
+      TcEpiIn in = tc_epi_load(E, col(0), orow, rowok);
       wgmma_wait<0>();
       wgmma_touch<NACC>(acc);
       if (leader) {
@@ -528,30 +623,11 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
         if (prev_a >= 0) tc_release(&a_empty[prev_a], cn);
       }
       if (threadIdx.x == 0) TC_STAMP(5);
-      // ---- epilogue
-      const int b = T.b, co0 = T.co0;
-      const long out_base = (long)offs[b] * tb.rmul * P.out_mul + (long)b * P.out_seq_extra;
-      long orow[2];
-      bool rowok[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int t = T.t0 + rbase + 8 * h;
-        rowok[h] = t < L;
-        orow[h] = out_base + (long)t * P.out_mul + P.out_add;
-      }
-      if (T.s == 1) {
-#pragma unroll
-        for (int jn = 0; jn < BN / 8; ++jn) {
-          const int c = co0 + jn * 8 + 2 * q4;
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            if (rowok[h]) tc_epi_pair(P, b, orow[h], c, acc[4 * jn + 2 * h], acc[4 * jn + 2 * h + 1], tb.dbgskip);
-        }
-      } else {
+      float* stage = reinterpret_cast<float*>(smem);         // split-K: [T.s][128][W] fp32 (BN/2 KB), aliases the operand rings
+      if (T.s > 1) {
         // split-K reduce-scatter among the T.s ranks g0 .. g0 + T.s - 1 of the tile: rank g0 + q finishes columns [q W, q W + W).
         // Every CTA sends each partial pair to the owner's staging buffer [src][row][W]; the owner adds the partials in rank order.
-        const int W = BN / T.s, sp = T.sp, g0 = MIXED ? (int)blockIdx.z % S - sp : 0;
-        float* stage = reinterpret_cast<float*>(smem);       // [T.s][128][W] fp32 (BN/2 KB), aliases the operand rings
+        const int sp = T.sp, g0 = MIXED ? (int)blockIdx.z % S - sp : 0;
         cluster_sync_all();                                  // (1) every CTA of the cluster is done with its operand rings
 #pragma unroll
         for (int jn = 0; jn < BN / 8; ++jn) {
@@ -565,19 +641,33 @@ __device__ __forceinline__ void conv_tc_body(const TcBatchT<PT, MP>& tb, const i
           }
         }
         cluster_sync_all();                                  // (2) all partials have landed; nobody writes into a CTA after this point
-        // The owner's column pairs (cw, cw + 1) of rows rbase and rbase + 8, summed in rank order.  A loop that is not unrolled,
-        // so the epilogue is one copy of its code: unrolled over the tile's BN/8 x 2 pairs it ran once per CTA from a cold
-        // instruction cache and cost 6-12 us of every split-K launch (CTA 0 stamps, tools/decoder_phases.py).
+      }
 #pragma unroll 1
-        for (int u = 0; u < W / 4; ++u) {
-          const int cw = 2 * q4 + 8 * (u >> 1), row = rbase + 8 * (u & 1), t = T.t0 + row;
-          float v0 = 0.f, v1 = 0.f;
-          for (int src = 0; src < T.s; ++src) {
-            const float2 p2 = *reinterpret_cast<const float2*>(stage + ((size_t)src * TC_BM + row) * W + cw);
-            v0 += p2.x; v1 += p2.y;
+      for (int j = 0; j < ncp; ++j) {
+        const TcEpiIn nx = tc_epi_load(E, col(j + 1), orow, rowok);   // the next pair's loads, ahead of this pair's stores
+        const TcEpiCol k = col(j);
+        // one row at a time, so the code of a (row, column pair) exists once: with both rows inlined the 128-wide images
+        // spill at their register limit (168 = 64K / (3 warps per SM sub-partition x 32 x 4))
+#pragma unroll 1
+        for (int h = 0; h < 2; ++h) {
+          if (!k.ok || !(h ? rowok[1] : rowok[0])) continue;
+          float v0 = h ? acc[2] : acc[0], v1 = h ? acc[3] : acc[1];
+          if (T.s > 1) {                                     // the owner's sum of the partials, in rank order
+            const float* st = stage + (size_t)(rbase + 8 * h) * W + 8 * j + 2 * q4;
+            v0 = 0.f; v1 = 0.f;
+#pragma unroll 1
+            for (int src = 0; src < T.s; ++src) {
+              const float2 p2 = *reinterpret_cast<const float2*>(st + (size_t)src * TC_BM * W);
+              v0 += p2.x; v1 += p2.y;
+            }
           }
-          if (t < L) tc_epi_pair(P, b, out_base + (long)t * P.out_mul + P.out_add, co0 + sp * W + cw, v0, v1, tb.dbgskip);
+          tc_epi_store(E, k, h ? orow[1] : orow[0], in.b0, in.b1, in.c0, in.c1, h ? in.r[1][0] : in.r[0][0],
+                       h ? in.r[1][1] : in.r[0][1], v0, v1);
         }
+        // the next pair's accumulators move to the front (static register indices in a loop that is not unrolled)
+#pragma unroll
+        for (int i = 0; i + 4 < NACC; ++i) acc[i] = acc[i + 4];
+        in = nx;
       }
     }
   }
